@@ -53,7 +53,38 @@ def parse():
     ap.add_argument("--cols", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the output layers of the last timed step as DIR/<layer>.npy and "
+                         "DIR/<layer>_invalid.npy (float32)")
     return ap.parse_args()
+
+
+LAYERS = ("slope", "step", "roughness", "traversability")
+DUMP_CELLS = 1 << 20  # cells kept per output layer: four layers, their masks and the index stay under 64 MB
+
+
+def dump_outputs(path, arrays, suffix=""):
+    """--dump-outputs: every output layer in float32 as two finite arrays: <path>/<name><suffix>.npy holds its values with the
+    invalid cells (NaN, as the reference leaves a cell whose window has no valid data) set to 0, and <name><suffix>_invalid.npy
+    is 1.0 exactly where the layer is not finite.  Layers of more than DUMP_CELLS cells are reduced to one fixed, seeded sample of
+    cells (the same for every layer and every run of the same size); sample_index.npy holds the sampled flat indices
+    (column-major: j * rows + i, map after map) as float64."""
+    import torch
+    os.makedirs(path, exist_ok=True)
+    flat = {k: (v if isinstance(v, torch.Tensor) else torch.from_numpy(np.asarray(v).reshape(-1, order="F"))).reshape(-1)
+            for k, v in arrays.items()}
+    n = {t.numel() for t in flat.values()}
+    assert len(n) == 1, n
+    n = n.pop()
+    if n > DUMP_CELLS:
+        idx = np.unique(np.random.default_rng(0).integers(0, n, DUMP_CELLS))
+        np.save(os.path.join(path, f"sample_index{suffix}.npy"), idx.astype(np.float64))
+        flat = {k: t[torch.from_numpy(idx).to(t.device)] for k, t in flat.items()}
+    for k, t in flat.items():
+        v = t.float().cpu().numpy()
+        bad = ~np.isfinite(v)
+        np.save(os.path.join(path, f"{k}{suffix}.npy"), np.where(bad, np.float32(0.0), v))
+        np.save(os.path.join(path, f"{k}{suffix}_invalid.npy"), bad.astype(np.float32))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -116,7 +147,7 @@ def terrain_torch(torch, rows, col0, ncols, cols_total, seed, holes, device):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -202,16 +233,7 @@ def measured_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def profile_traffic():
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture, if any."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline_latest.json")) as f:
-            return json.load(f)
-    except Exception:
-        return None
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def run_reference(args):
@@ -226,16 +248,16 @@ def run_reference(args):
     g = ob.Geometry.make(n, n, RES)
     p = ob.ChainParams.yaml_defaults(0)
     threads = len(os.sched_getaffinity(0))  # all host threads, also under torchrun (which exports OMP_NUM_THREADS=1)
-    # each step is one pass over the bounded sample; the step count is capped so the whole run ends within minutes
-    steps, warmup = min(args.steps, 20), min(args.warmup, 2)
-    for _ in range(warmup):
+    # each step is one pass over the bounded sample
+    for _ in range(args.warmup):
         ob.chain(g, p, z, nthreads=threads)
     t0 = time.perf_counter()
-    for _ in range(steps):
-        ob.chain(g, p, z, nthreads=threads)
+    for _ in range(args.steps):
+        r = ob.chain(g, p, z, nthreads=threads)
     dt = time.perf_counter() - t0
-    val = n * n * steps / dt / 1e6
-    args.steps, args.warmup = steps, warmup
+    val = n * n * args.steps / dt / 1e6
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {k: r[k] for k in LAYERS})
     out = {"impl": "reference", "metric": "Mcells/s full filter chain, synthetic elevation", "value": val, "unit": "Mcells/s",
            "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": dt / args.steps * 1e3,
            "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None, "dtype": "f64 compute / f32 layers",
@@ -258,6 +280,8 @@ def run_plugin_chain(args, torch, dev):
     with the cross-plugin fusion registry (one te_chain launch per map) and with TE_B200_FUSE_CHAIN=0 (three stand-alone literal
     kernels, the round-1 behaviour)."""
     import tempfile
+    if args.dump_outputs:
+        raise SystemExit("--dump-outputs: the plugin_chain layers stay inside the plugin harness")
     plugin = os.path.join(ROOT, "traversability_estimation_b200", "plugin")
     subprocess.check_call(["make", "-C", plugin, "-s"])
     rows = cols = args.rows or 4096
@@ -266,7 +290,7 @@ def run_plugin_chain(args, torch, dev):
     with tempfile.TemporaryDirectory() as tmp:
         src = os.path.join(tmp, "elev.bin")
         z.cpu().numpy().tofile(src)
-        passes = max(2, min(args.steps, 5))
+        passes = args.steps
         for name, fuse in (("fused_registry", "1"), ("standalone_literal", "0")):
             env = dict(os.environ, TE_B200_FUSE_CHAIN=fuse)
             r = subprocess.run([os.path.join(plugin, "test_plugins"), "bench", str(rows), str(cols), repr(RES), src, str(passes)],
@@ -305,6 +329,7 @@ def run_other(args, torch, dist, te, world, rank, local, dev):
         outs = [torch.empty((n, cols, rows), dtype=torch.float32, device=dev) for _ in range(4)]
         cells = n_total * rows * cols
         name = f"{n_total} independent {rows}x{cols} maps, full fused chain, {n} maps per GPU"
+        dump = dict(zip(LAYERS, outs))
 
         def step():
             ctx.chain_batched(g, prm, n, z, *outs, te.MEM_DEVICE)
@@ -316,6 +341,7 @@ def run_other(args, torch, dist, te, world, rank, local, dev):
         out = torch.empty_like(nz)
         cells = rows * cols
         name = f"SlopeFilter only (te_slope) over a {rows}x{cols} surface_normal_z layer, 8 B/cell"
+        dump = {"slope": out}
 
         def step():
             ctx.slope(g, 1.0, nz, out, te.MEM_DEVICE)
@@ -332,6 +358,7 @@ def run_other(args, torch, dist, te, world, rank, local, dev):
         out = torch.empty((cols, rows), dtype=torch.float32, device=dev)
         cells = rows * cols
         name = f"footprint sweep r=0.30 m offset={fp.offset:.2f} m over {rows}x{cols} traversability/slope/step/elevation"
+        dump = {"traversability_footprint": out}
 
         def step():
             ctx.footprint(g, fp, lay[3], lay[0], lay[1], z, out, te.MEM_DEVICE)
@@ -340,6 +367,7 @@ def run_other(args, torch, dist, te, world, rank, local, dev):
             poly = [[0.45, 0.30], [0.45, -0.30], [-0.45, -0.30], [-0.45, 0.30]]
             out2 = torch.empty((cols, rows), dtype=torch.float32, device=dev)
             name = f"polygon footprint sweep (0.9 m x 0.6 m, yaw 0.7854: traversability_x + traversability_rot) over {rows}x{cols}"
+            dump = {"traversability_x": out, "traversability_rot": out2}
 
             def step():  # noqa: F811
                 ctx.footprint_polygon(g, fp, poly, 0.7854, lay[3], lay[0], lay[1], z, out, out2, te.MEM_DEVICE)
@@ -364,6 +392,8 @@ def run_other(args, torch, dist, te, world, rank, local, dev):
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms = float(ms)
     l1, _ = ctx.stats()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dump, "" if world == 1 else f"_rank{rank}")
     if rank == 0:
         peak, src = measured_peak()
         bpc = 8 if args.workload == "slope8192" else (24 if args.workload == "footprint_polygon4096" else ALG_BYTES_PER_CELL)
@@ -429,7 +459,7 @@ def main():
     own = terrain_torch(torch, rows, col0, my_cols, cols_total, 3, args.holes, dev)  # (my_cols, rows): column-major layer
     elev = torch.full((hl + my_cols + hr, rows), float("nan"), dtype=torch.float32, device=dev)
     elev[hl:hl + my_cols].copy_(own)
-    # a pass touches 20 B/cell; when that fits the 126 MB L2, rotate through enough buffer sets that every timed pass
+    # a pass touches 20 B/cell; when that could stay in the 50 MB L2, rotate through enough buffer sets that every timed pass
     # streams from HBM ("inputs larger than L2" by rotation instead of an explicit flush)
     pass_bytes = 20 * rows * my_cols
     nsets = 1 if pass_bytes > 3e8 else int(np.ceil(6e8 / pass_bytes))
@@ -530,6 +560,8 @@ def main():
     barrier()
     timed[0] = False
     ms_total = ev0.elapsed_time(ev1)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dict(zip(LAYERS, outsets[(rot[0] - 1) % nsets])), "" if world == 1 else f"_rank{rank}")
     halo_ms = (sum(a.elapsed_time(b) for a, b in hev[:timed[1]]) / max(timed[1], 1)) if world > 1 else 0.0
     clocks = sampler.stop() if rank == 0 else None
     launches1, slow_cells = ctx.stats()
@@ -605,9 +637,6 @@ def main():
     peak, peak_src = measured_peak()
     cells_per_launch = rows * my_cols
     achieved = ALG_BYTES_PER_CELL * cells_per_launch / (main_avg * 1e-3) / 1e9 if main_avg > 0 else None
-    prof = profile_traffic()
-    # the committed ncu capture is of one launch over an 8192 x 8192 slab with the fused kernel: quote it only there
-    traffic = (prof or {}).get("dram_bytes_per_launch") if (rows == 8192 and my_cols == 8192 and args.kernel != "generic") else None
     out = {
         "metric": "Mcells/s full filter chain, synthetic elevation", "value": value, "unit": "Mcells/s",
         "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_total / args.steps,
@@ -618,12 +647,12 @@ def main():
                              ((" + 4-column halo, " + (("peer-mapped pull over NVLink (te_halo_pull, CUDA IPC)" + (", the next buffer set's pull overlapped on a side stream" if overlap else "")) if args.halo == "ipc" else "NCCL send/recv"))
                               if world > 1 else ""),
                    "holes": args.holes, "kernel": args.kernel,
-                   "l2": ("working set %.2f GB/GPU per pass > 126 MB L2, no flush needed" % (pass_bytes / 1e9)) if nsets == 1 else
+                   "l2": ("working set %.2f GB/GPU per pass > 50 MB L2, no flush needed" % (pass_bytes / 1e9)) if nsets == 1 else
                          ("%d buffer sets rotated (%.0f MB total) so every pass streams from HBM" % (nsets, nsets * pass_bytes / 1e6)),
                    "slow_path_cells_per_launch": int(slow_cells)},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                      "frac": (achieved / peak) if achieved else None,
-                     "traffic": traffic, "peak_source": peak_src,
+                     "traffic": None, "peak_source": peak_src,
                      "kernel": "k_chain_fused" if args.kernel != "generic" else "k_chain_generic",
                      "kernel_ms": main_avg, "fixup_kernel_ms": fix_avg,
                      "algorithmic_bytes_per_launch": ALG_BYTES_PER_CELL * cells_per_launch,

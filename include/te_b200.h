@@ -1,5 +1,5 @@
 /*
- * te_b200.h — C ABI of the B200-native traversability filter chain and footprint sweep.
+ * te_b200.h — C ABI of the H100-native (sm_90a) traversability filter chain and footprint sweep.
  *
  * This is the drop-in boundary: plain pointers and sizes, no C++/torch types.  Each entry point
  * names the reference interface it replaces (path:line relative to the reference repository

@@ -60,17 +60,17 @@ def test_fused_work_units_tile_every_map_exactly_once(te, rows, cols, nmaps, sms
 
 
 def test_fused_plan_shapes_of_the_bench_configurations(te):
-    """What plan_levels decides for the sizes the bench lines are quoted on (profiles/README.md, round 2): one long unit per warp
-    first for the big single map, one round of one segment length for small launches, the tapering plan in between."""
-    big = te.capi.fused_plan(8192, 8192, 1, 148)["levels"]
-    assert (big[0]["seg_len"], big[0]["nseg"]) == (512, 12) and big[1]["seg_len"] == 24 and big[2]["seg_len"] == 16
-    assert 137 * 12 <= 148 * 12                                    # at most one long unit per warp
-    slab = te.capi.fused_plan(8192, 1024, 1, 148)
-    assert slab["levels"][0]["seg_len"] == 88 and slab["units"] == 137 * 12 <= 148 * 12   # one round
-    small = te.capi.fused_plan(2048, 2048, 1, 148)
-    assert small["levels"][0]["seg_len"] == 44 and small["units"] <= 148 * 12
-    batch = te.capi.fused_plan(512, 512, 256, 148)["levels"]
-    assert batch[0]["seg_len"] == 80 and batch[1]["seg_len"] == 24  # many rounds: long segments first, short ones last
+    """What plan_levels decides on an H100 (132 SMs x 12 warps) for the sizes the bench lines are quoted on: one long unit per
+    warp first for the big single map, one round of one segment length for small launches, the tapering plan in between."""
+    big = te.capi.fused_plan(8192, 8192, 1, 132)["levels"]
+    assert (big[0]["seg_len"], big[0]["nseg"]) == (552, 11) and big[1]["seg_len"] == 24 and big[2]["seg_len"] == 16
+    assert 137 * 11 <= 132 * 12                                    # at most one long unit per warp
+    slab = te.capi.fused_plan(8192, 1024, 1, 132)
+    assert slab["levels"][0]["seg_len"] == 96 and slab["units"] == 137 * 11 <= 132 * 12   # one round
+    small = te.capi.fused_plan(2048, 2048, 1, 132)
+    assert small["levels"][0]["seg_len"] == 48 and small["units"] <= 132 * 12
+    batch = te.capi.fused_plan(512, 512, 256, 132)["levels"]
+    assert batch[0]["seg_len"] == 96 and batch[1]["seg_len"] == 32  # many rounds: long segments first, short ones last
 
 
 def test_fused_plan_rejects_bad_sizes(te):

@@ -1,11 +1,13 @@
-"""Extract the reference's golden vector into tests/golden/ (run in the build container only).
+"""Extract the reference's golden vector into tests/golden/.
 
-Source: /root/reference/traversability_estimation/maps/elevation_map.bag — the reference's
-only known-answer material (SURVEY.md Appendix B).  /root/reference does not exist on the
-GPU box, so the decoded layers are committed as a small .npz next to this script's output
-manifest (crc32 per layer, so a reader can re-derive them from the bag and compare).
+    python tools/make_golden.py <reference checkout>/traversability_estimation/maps/elevation_map.bag
+
+The bag is the reference's only known-answer material (SURVEY.md Appendix B).  The decoded layers
+are stored as a small .npz with a manifest (crc32 per layer), and the bag itself xz-compressed, so
+the tests re-derive the layers from the bag without the reference checkout.
 """
 import json
+import lzma
 import os
 import sys
 import zlib
@@ -15,7 +17,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from bag import read_gridmap_bag  # noqa: E402
 
-SRC = "/root/reference/traversability_estimation/maps/elevation_map.bag"
+SRC = sys.argv[1] if len(sys.argv) > 1 else "traversability_estimation/maps/elevation_map.bag"
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 KEEP = ["elevation", "traversability_slope", "traversability_step", "traversability_roughness",
         "traversability", "traversability_footprint", "slope_footprint", "step_footprint"]
@@ -26,6 +28,8 @@ def main():
     os.makedirs(OUT, exist_ok=True)
     arrays = {k: m.data[k] for k in KEEP}
     np.savez_compressed(os.path.join(OUT, "fixture_gridmap.npz"), **arrays)
+    with open(SRC, "rb") as f, lzma.open(os.path.join(OUT, "elevation_map.bag.xz"), "wb", preset=9 | lzma.PRESET_EXTREME) as g:
+        g.write(f.read())
     manifest = {
         "source": "traversability_estimation/maps/elevation_map.bag",
         "sha256": "02cba247d0526fb9aaa84b19dffd87e31abb3e8b3bdaa11e0a50f14c18e38448",

@@ -1,4 +1,4 @@
-"""B200-native traversability filter chain + footprint sweep (sm_100a CUDA behind a C ABI).
+"""H100-native traversability filter chain + footprint sweep (sm_90a CUDA behind a C ABI).
 
 The product is `libte_b200.so` (include/te_b200.h); its reference-facing host side are the C++
 filter plugin shells in `plugin/`.  This Python module is only a ctypes view of the same C ABI for

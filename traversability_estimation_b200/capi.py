@@ -83,7 +83,7 @@ def library_path() -> str:
 
 
 def build_library(force: bool = False) -> str:
-    """nvcc-compile csrc/ for sm_100a into libte_b200.so (in-tree, travels to the GPU box)."""
+    """nvcc-compile csrc/ for sm_90a into libte_b200.so, next to this file."""
     args = ["make", "-C", os.path.join(_HERE, "csrc"), "-s"]
     if force:
         args.append("-B")
@@ -133,7 +133,7 @@ def load_library():
     return _lib
 
 
-def fused_plan(rows: int, out_ncols: int, nmaps: int = 1, sms: int = 148) -> dict:
+def fused_plan(rows: int, out_ncols: int, nmaps: int = 1, sms: int = 132) -> dict:
     """te_fused_plan: the (level, map, segment, strip) work units of the fused launch; host arithmetic, no GPU needed."""
     L = load_library()
     out = (C.c_int32 * 19)()

@@ -78,7 +78,7 @@ inline int reach_true(double radius, double res) { return (int)std::floor(radius
 
 struct te_ctx {
   int device = 0;
-  int sms = 148;
+  int sms = 132;
   cudaStream_t own_stream = nullptr;
   cudaStream_t stream = nullptr;
   std::mutex mu;

@@ -437,8 +437,10 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
     const bool active = i < A.rows;
     const size_t c = (size_t)blockIdx.y * A.rows + (active ? i : 0);
     const double cx = A.X[active ? i : 0], cy = A.Y[j];
-    // disk columns that exist in the map and in this slab's buffer
-    const int l_lo = max(-A.L, max(-j, A.in_col0 - j)), l_hi = min(A.L, min(A.cols_total - 1 - j, A.in_col0 + A.in_ncols - 1 - j));
+    // disk columns that exist in the map and in this slab's buffer.  l_lo is written as a negated minimum: ptxas of CUDA 12.9 for
+    // sm_90a fuses max(-L, max(-j, in_col0 - j)) into one three-input VIMNMX3 that reads +L, and the loops bounded by l_hi then ran
+    // past it whenever the disk is clipped on the right
+    const int l_lo = -min(A.L, min(j, j - A.in_col0)), l_hi = min(A.L, min(A.cols_total - 1 - j, A.in_col0 + A.in_ncols - 1 - j));
     // ---- warp-wide early out: is any cell blocked in the box of rows [i0 - L, i0 + 31 + L] x disk columns?  (packed flags,
     //      a few words per column, shared by the 32 centres)  Mostly not: then no lane has anything to look for.
     bool warp_any;
@@ -679,7 +681,7 @@ __global__ void __launch_bounds__(256) k_sweep_tile(FpArgs A, Layers L, const un
     if (j >= A.out_col0 + A.out_ncols) break;
     const size_t c = (size_t)(j - A.out_col0) * A.rows + (active ? i : 0);
     const double cy = A.Y[j];
-    const int l_lo = max(-Lr, max(-j, A.in_col0 - j)), l_hi = min(Lr, min(A.cols_total - 1 - j, A.in_col0 + A.in_ncols - 1 - j));
+    const int l_lo = -min(Lr, min(j, j - A.in_col0)), l_hi = min(Lr, min(A.cols_total - 1 - j, A.in_col0 + A.in_ncols - 1 - j));  // see k_sweep_fast
     bool warp_any = false;
     if (tile_any) {
       const int s0 = j + l_lo - ca, cnt = l_hi - l_lo + 1;  // cnt <= 63, bits [s0, s0 + cnt) of the 128-bit mask

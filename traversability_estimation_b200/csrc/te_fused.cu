@@ -1,4 +1,4 @@
-// te_fused.cu — the fused chain stencil for sm_100a.
+// te_fused.cu — the fused chain stencil for sm_90a (H100).
 //
 // One launch computes, for every cell of a column slab, what the reference's six-filter chain
 // (robot_filter_parameter.yaml:2-37) computes — normals -> slope, step (both passes), roughness,
@@ -7,7 +7,7 @@
 //
 // Execution model (DESIGN.md §"fused stencil"):
 //   * The layer is column-major, row index contiguous.  A WARP owns a strip of 64 rows (two adjacent
-//     rows per lane, so all arithmetic is issued as packed f32x2 FFMA2/FADD2) and marches along the
+//     rows per lane, so all arithmetic is issued on row pairs) and marches along the
 //     column index.  Warps are autonomous: each has its own TMA ring (4 stages x 5 columns x 68 rows,
 //     NaN out-of-bounds fill so map borders look like invalid cells), its own mbarriers and a tiny
 //     step_height exchange buffer; there is no __syncthreads in the kernel.  Work units are (60-row strip,
@@ -135,10 +135,11 @@ struct FusedArgs {
 };
 
 // ---------------------------------------------------------------------------------------------
-// packed f32x2 arithmetic (Blackwell FFMA2/FADD2/FMUL2): .x = row i, .y = row i+1 of the lane
+// paired f32 arithmetic: .x = row i, .y = row i+1 of the lane
 // ---------------------------------------------------------------------------------------------
-// An f2 lives in ONE aligned 64-bit register pair for its whole life, so FFMA2/FADD2/FMUL2 take it
-// without any repacking; lo()/hi() only name the halves.
+// An f2 lives in one 64-bit register pair; lo()/hi() only name the halves.  sm_90 has no packed
+// f32x2 instructions, so every pair operation is two scalar round-to-nearest instructions (never
+// contracted), which round each half exactly as a packed instruction would.
 __device__ __forceinline__ f2 mk(float x, float y) {
   f2 r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(x), "f"(y));
@@ -154,30 +155,14 @@ __device__ __forceinline__ float hi(f2 v) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
   return b;
 }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) {
-  f2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f2 sub2(f2 a, f2 b) {
-  f2 r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) {
-  f2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
-  f2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return mk(__fadd_rn(lo(a), lo(b)), __fadd_rn(hi(a), hi(b))); }
+__device__ __forceinline__ f2 sub2(f2 a, f2 b) { return mk(__fsub_rn(lo(a), lo(b)), __fsub_rn(hi(a), hi(b))); }
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return mk(__fmul_rn(lo(a), lo(b)), __fmul_rn(hi(a), hi(b))); }
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return mk(__fmaf_rn(lo(a), lo(b), lo(c)), __fmaf_rn(hi(a), hi(b), hi(c))); }
 __device__ __forceinline__ f2 bc(float v) { return mk(v, v); }
 __device__ __forceinline__ f2 neg2(f2 a) { return a ^ 0x8000000080000000ull; }
-// -a for both rows, written as two scalar negations: ptxas folds the pair into the operand modifier of the consuming
-// FFMA2/FADD2/FMUL2 (`FFMA2 R4, -R4.F32x2.HI_LO, ...`), so the negation costs no instruction (an integer XOR would cost two).
+// -a for both rows, written as two scalar negations: ptxas folds each into the operand modifier of the consuming
+// FFMA/FADD/FMUL, so the negation costs no instruction (an integer XOR would cost two).
 __device__ __forceinline__ f2 negf2(f2 a) { return mk(-lo(a), -hi(a)); }
 // TE_NOCORR: bit mask of the Newton corrections that are dropped (bit0 D = sqrt(hh): MUFU.SQRT, rel. error 2^-23; bit1 g2/dph and
 // bit2 g2/m^2: MUFU.RCP, 2^-23).  What they feed tolerates it: lambda0 is certified against 1e-5 cmag, s = 1 - n_z against a
@@ -192,17 +177,18 @@ __device__ __forceinline__ f2 negf2(f2 a) { return mk(-lo(a), -hi(a)); }
 #define TE_MATH2 1
 #endif
 
-// Three-input min/max (FMNMX3) with IEEE minNum/maxNum semantics: NaN operands are skipped, which is
+// Three-input min/max with IEEE minNum/maxNum semantics: NaN operands are skipped, which is
 // exactly how the reference's step filter treats invalid cells (StepFilter.cpp:126,159); the result is
-// NaN only when every operand is.  Excluded on-circle tips are passed as NaN.
+// NaN only when every operand is.  Excluded on-circle tips are passed as NaN.  Two chained FMNMX (sm_90
+// has no three-input form).
 __device__ __forceinline__ float max3n(float a, float b, float c) {
   float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
+  asm("{ .reg .f32 t; max.f32 t, %1, %2; max.f32 %0, t, %3; }" : "=f"(r) : "f"(a), "f"(b), "f"(c));
   return r;
 }
 __device__ __forceinline__ float min3n(float a, float b, float c) {
   float r;
-  asm("min.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
+  asm("{ .reg .f32 t; min.f32 t, %1, %2; min.f32 %0, t, %3; }" : "=f"(r) : "f"(a), "f"(b), "f"(c));
   return r;
 }
 // 1.0f / 0.0f comparison result in one instruction (FSET.BF)
@@ -961,8 +947,7 @@ PFN_encodeTiled get_encode() {
 // Splits the output columns of every map into up to NLVL runs of segments, longest segments first.  A warp
 // pops (segment, strip) units in that order, so the last units handed out are short and the warps finish
 // within one short unit of each other.  Each unit pays 8 warm-up columns (cheap: the later stages are
-// skipped), so the bulk of the map stays in longer segments; about eight long units per warp measured best
-// from 2048^2 to 8192^2 and for batches of 512^2 maps (profiles/README.md).
+// skipped), so the bulk of the map stays in longer segments (about eight long units per warp).
 void plan_levels(FusedArgs& a, int out_ncols, int nmaps, int total_warps) {
   const double share = (double)a.nstrips * out_ncols * nmaps / (double)total_warps;  // strip-columns per warp
   const int len0 = std::min(128, std::max(16, (int)std::lround(share / 8.0 / 8.0) * 8));
@@ -972,8 +957,8 @@ void plan_levels(FusedArgs& a, int out_ncols, int nmaps, int total_warps) {
   if (share >= 400.0 && (long long)a.nstrips * nmaps <= total_warps / 4) {
     // Large single maps: ONE long unit per warp first — as many segments per strip as give every warp (at most) one unit, over
     // three quarters of the columns, so that a warp pays its 8 warm-up columns once for most of its work — then the tapering
-    // tail (24- and 16-column segments) that evens out the warps' different speeds.  8192^2: 12 segments of 512 columns per
-    // strip (1 644 units on 1 776 warps), measured 0.553 ms against 0.564 ms with 80-column segments (profiles/README.md).
+    // tail (24- and 16-column segments) that evens out the warps' different speeds.  8192^2 on an H100 (132 SMs): 11 segments
+    // of 552 columns per strip (1 507 units on 1 584 warps).
     const int nseg0 = (int)(total_warps / ((long long)a.nstrips * nmaps));
     const int l0 = (int)(0.75 * out_ncols / nseg0) / 8 * 8;
     if (l0 >= 128) {
