@@ -230,6 +230,37 @@ int te_check_footprint_paths2(te_ctx* ctx, const te_geometry* g, const float* tr
                               const float* robot_slope_or_null, double traversability_default, int32_t npaths,
                               const int32_t* path_begin, const double* poses_xy, uint8_t* is_safe, double* traversability, int memory);
 
+/* checkCircularFootprintPath (TraversabilityMap.cpp:345-462) as the reference's check_footprint_path service answers it on a
+ * freshly computed map (TraversabilityEstimation.cpp:278-295): computeTraversability leaves traversability_footprint empty (NaN,
+ * TraversabilityMap.cpp:225-228), so every isTraversable(center, radius + offset, ...) walks the SpiralIterator over the chain
+ * layers (:679-736) instead of reading a swept layer.  That branch differs from te_check_footprint_paths2:
+ *   - a blocked cell between radius and radius + offset (the first one in visit order) makes the circle untraversable (:714-717);
+ *   - a circle's mean reaches the path sum in double, not rounded to float32 (:733);
+ *   - a single pose is evaluated at the pose itself: the circle test of the outer two rings is against the pose position;
+ *   - compute_untraversable_polygon[q] != 0 (FootprintPath.compute_untraversable_polygon; NULL = all 0) keeps the walk going: a
+ *     first blocker in that annulus leaves the circle traversable with its mean divided by the cell count twice (:707, :733);
+ *   - a centre that an earlier segment of the same path checked reads the float32 value the first check stored (:673-675):
+ *     traversable iff it is != 0.
+ * Cache across paths — a deliberate choice: every path is answered as the first check after computeTraversability, on an empty
+ * cache; within a path the cache is reproduced exactly.  The reference keeps the cache across the paths of a request and across
+ * requests until the next map update, so its answers depend on a call history no caller controls.
+ * Layers: the chain outputs traversability, traversability_slope, traversability_step (traversability_roughness when
+ * p->verify_roughness is set) and elevation; robot_slope_or_null switches checkRobotInclination_ on, as in
+ * te_check_footprint_paths2.  From `p` only offset (radiusMax = radius + offset; the reference hard-codes 0.15, :348),
+ * traversability_default, max_gap_width, critical_step_height, radius_is_integer_norm and verify_roughness are used; p->radius
+ * is ignored — radius[q] is FootprintPath.radius of path q.  Paths, outputs and conventions (empty path, poses outside the map,
+ * lengthPath) as te_check_footprint_paths2.  Whole maps only.
+ * Errors: TE_ERR_MISSING_LAYER for a missing layer; TE_ERR_BAD_ARG for null or negative arguments and, in TE_MEM_HOST, a radius
+ * that is NaN or negative; TE_ERR_UNSUPPORTED in TE_MEM_HOST when ceil((radius + offset) / resolution) exceeds 127 rings, and
+ * in TE_MEM_DEVICE for a non-zero start index.  TE_MEM_DEVICE is asynchronous on the context stream and cannot read the radii:
+ * a path with such a radius gets is_safe = 0 and traversability = NaN (a checked path never yields NaN).  TE_MEM_HOST takes a
+ * circular-buffer start index (the layers are unwrapped on upload; poses are map-frame positions and need no change). */
+int te_check_footprint_paths_fresh(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, const float* traversability,
+                                   const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                                   const float* robot_slope_or_null, int32_t npaths, const int32_t* path_begin, const double* poses_xy,
+                                   const double* radius, const uint8_t* compute_untraversable_polygon_or_null, uint8_t* is_safe,
+                                   double* traversability_out, int memory);
+
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the
  * neighbours' boundary columns of the INPUT layer(s) into this rank's halo.  The reference has no counterpart (it is a

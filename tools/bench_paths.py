@@ -1,0 +1,126 @@
+"""Circular footprint path checks on a 4096^2 map: the fresh-cache entry against the sweep + memoised check.
+
+  (a) te_check_footprint_paths_fresh (TE_MEM_DEVICE): the paths straight from the chain layers;
+  (b) te_footprint(0.3, 0.15) over the whole map, then te_check_footprint_paths2 (TE_MEM_DEVICE) on the swept layer.
+
+The two answer different questions (see include/te_b200.h): (a) is what the reference's service returns on a freshly computed
+map, (b) what it returns once the footprint layer has been swept.  Paths are planner-like: 2-8 poses 0.1-0.5 m apart, radius
+0.3 m.  Batches of 1, 100 and 1000 paths are timed with CUDA events after warm-up; the result is one JSON line per batch size,
+with the GPU name and its power limit.
+
+    python tools/bench_paths.py [--size 4096] [--reps 20]
+"""
+from __future__ import annotations
+
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in (ROOT, os.path.join(ROOT, "tools")):
+    if p not in sys.path:
+        sys.path.insert(0, p)
+
+
+def planner_paths(rng, n, npaths, res):
+    half = 0.45 * n * res
+    begin, poses = [0], []
+    for _ in range(npaths):
+        k = int(rng.integers(2, 9))
+        p = [rng.uniform(-half, half, size=2)]
+        for _ in range(k - 1):
+            ang, d = rng.uniform(0, 2 * np.pi), rng.uniform(0.1, 0.5)
+            p.append(p[-1] + d * np.array([np.cos(ang), np.sin(ang)]))
+        poses.extend(np.asarray(p).tolist())
+        begin.append(len(poses))
+    return np.asarray(begin, np.int32), np.asarray(poses, np.float64).reshape(-1, 2)
+
+
+def gpu_info(torch):
+    name = torch.cuda.get_device_name(0)
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        power = float(out.splitlines()[0])
+    except Exception:
+        power = None
+    return name, power
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--size", type=int, default=4096)
+    ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    args = ap.parse_args()
+    import torch
+    import synth
+    import traversability_estimation_b200 as te
+
+    n, res = args.size, 0.02
+    g = te.Geometry.make(n, n, res)
+    fp = te.FootprintParams.yaml_defaults()            # radius 0.3, offset 0.15 (robot_footprint_parameter.yaml)
+    ctx = te.Context(0)
+    z = synth.terrain(n, n, res, 4096, "mixed")
+    layers = ctx.chain_host(g, te.ChainParams.yaml_defaults(0), z)
+    dev = lambda a: torch.from_numpy(np.ascontiguousarray(np.asarray(a, np.float32).T)).cuda()  # noqa: E731
+    trav, slope, step, elev = (dev(a) for a in (layers["traversability"], layers["slope"], layers["step"], z))
+    swept = torch.empty_like(trav)
+    stream = torch.cuda.Stream()
+    ctx.set_stream(stream.cuda_stream)
+    L = te.load_library()
+    L.te_check_footprint_paths2.argtypes = [C.c_void_p, C.POINTER(te.Geometry), C.c_void_p, C.c_void_p, C.c_double, C.c_int32] + \
+        [C.c_void_p] * 4 + [C.c_int]
+    name, power = gpu_info(torch)
+    rng = np.random.default_rng(1)
+    for batch in (1, 100, 1000):
+        begin, poses = planner_paths(rng, n, batch, res)
+        db = torch.from_numpy(begin).cuda()
+        dp = torch.from_numpy(poses).cuda()
+        dr = torch.full((batch,), 0.3, dtype=torch.float64, device="cuda")
+        safe_a = torch.empty(batch, dtype=torch.uint8, device="cuda")
+        t_a = torch.empty(batch, dtype=torch.float64, device="cuda")
+        safe_b, t_b = torch.empty_like(safe_a), torch.empty_like(t_a)
+        torch.cuda.synchronize()
+
+        def run_a():
+            ctx.check_footprint_paths_fresh(g, fp, trav, slope, step, elev, db, dp, dr, memory=te.MEM_DEVICE, is_safe=safe_a,
+                                            traversability_out=t_a)
+
+        def run_b():
+            ctx.footprint(g, fp, trav, slope, step, elev, swept, te.MEM_DEVICE)
+            rc = L.te_check_footprint_paths2(ctx._h, C.byref(g), swept.data_ptr(), None, fp.traversability_default, batch,
+                                             db.data_ptr(), dp.data_ptr(), safe_b.data_ptr(), t_b.data_ptr(), te.MEM_DEVICE)
+            assert rc == 0, rc
+
+        res_ms = {}
+        for key, fn in (("fresh", run_a), ("sweep_then_check", run_b)):
+            for _ in range(args.warmup):
+                fn()
+            stream.synchronize()
+            ts = []
+            for _ in range(args.reps):
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                fn()
+                e1.record(stream)
+                e1.synchronize()
+                ts.append(e0.elapsed_time(e1))
+            res_ms[key] = {"median_ms": float(np.median(ts)), "min_ms": float(np.min(ts))}
+        stream.synchronize()
+        differ = int((safe_a != safe_b).sum().item())
+        print(json.dumps({"gpu": name, "power_limit_w": power, "map": f"{n}x{n}", "resolution": res, "radius": 0.3,
+                          "offset": fp.offset, "paths": batch, "poses": int(begin[-1]), **res_ms,
+                          "safe_fresh": int(safe_a.sum().item()), "safe_swept": int(safe_b.sum().item()), "is_safe_differs": differ}),
+              flush=True)
+    ctx.set_stream(None)
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()

@@ -18,7 +18,7 @@ KERNEL_AUTO, KERNEL_GENERIC, KERNEL_FUSED = 0, 1, 2
 
 EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set_stream", "te_synchronize",
            "te_set_kernel", "te_get_stats", "te_enable_timing", "te_get_timing", "te_get_flag_counters", "te_get_escalation_stats", "te_fused_plan", "te_slope", "te_normals", "te_step", "te_roughness", "te_chain",
-           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_check_footprint_paths", "te_check_footprint_paths2", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
+           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
            "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free"]
 
 
@@ -293,6 +293,41 @@ class Context:
         self._check(self._L.te_check_footprint_paths2(self._h, C.byref(g), f.ctypes.data, rs.ctypes.data if rs is not None else None,
                                                       traversability_default, n, pb.ctypes.data, xy.ctypes.data, safe.ctypes.data,
                                                       trav.ctypes.data, MEM_HOST))
+        return safe, trav
+
+    def check_footprint_paths_fresh(self, g, fp, traversability, slope, step, elevation, path_begin, poses_xy, radius, robot_slope=None,
+                                    roughness=None, compute_untraversable_polygon=None, memory=MEM_HOST, is_safe=None,
+                                    traversability_out=None):
+        """te_check_footprint_paths_fresh: checkCircularFootprintPath on the chain layers as the reference's service answers it on a
+        freshly computed map (empty traversability_footprint cache per path).  radius: FootprintPath.radius per path (float64);
+        fp supplies offset, traversability_default, max_gap_width, critical_step_height, radius_is_integer_norm and
+        verify_roughness.  MEM_HOST: numpy arguments, returns (is_safe uint8[npaths], traversability float64[npaths]).
+        MEM_DEVICE: every argument is a device tensor (path_begin int32, poses_xy / radius float64,
+        compute_untraversable_polygon uint8) and the results go to the caller's is_safe / traversability_out tensors."""
+        sig = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + [C.c_int32] + [C.c_void_p] * 6 + [C.c_int]
+        self._L.te_check_footprint_paths_fresh.argtypes = sig
+        if memory == MEM_DEVICE:
+            self._order_after_torch(memory)
+            n = int(path_begin.numel()) - 1
+            self._check(self._L.te_check_footprint_paths_fresh(
+                self._h, C.byref(g), C.byref(fp), _addr(traversability), _addr(slope), _addr(step), _addr(roughness), _addr(elevation),
+                _addr(robot_slope), n, _addr(path_begin), _addr(poses_xy), _addr(radius), _addr(compute_untraversable_polygon),
+                _addr(is_safe), _addr(traversability_out), MEM_DEVICE))
+            return is_safe, traversability_out
+        lay = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)  # noqa: E731
+        t, s, st, e, rs, r = (lay(a) for a in (traversability, slope, step, elevation, robot_slope, roughness))
+        pb = np.ascontiguousarray(path_begin, dtype=np.int32)
+        xy = np.ascontiguousarray(poses_xy, dtype=np.float64)
+        rad = np.ascontiguousarray(radius, dtype=np.float64)
+        cup = None if compute_untraversable_polygon is None else np.ascontiguousarray(compute_untraversable_polygon, dtype=np.uint8)
+        n = len(pb) - 1
+        if len(rad) != n or (cup is not None and len(cup) != n):
+            raise ValueError("radius / compute_untraversable_polygon need one entry per path")
+        safe = np.zeros(n, dtype=np.uint8) if is_safe is None else is_safe
+        trav = np.zeros(n, dtype=np.float64) if traversability_out is None else traversability_out
+        self._check(self._L.te_check_footprint_paths_fresh(
+            self._h, C.byref(g), C.byref(fp), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), n, pb.ctypes.data,
+            xy.ctypes.data, rad.ctypes.data, _addr(cup), safe.ctypes.data, trav.ctypes.data, MEM_HOST))
         return safe, trav
 
     # ---- multi-GPU halo (te_halo_pull and the IPC helpers around it)

@@ -33,6 +33,9 @@ struct FootprintState {
   void* d_poly[2] = {nullptr, nullptr};  // run / uncertain-offset tables of the unrotated and the rotated footprint polygon
   size_t poly_cap[2] = {0, 0};
   bool poly_attr = false;
+  void* d_rings = nullptr;   // fresh path checks: ring starts + SpiralIterator visit order of rings 0..127 (built once)
+  void* d_memo = nullptr;    // fresh path checks: per-cell isTraversableForFilters memo of one call
+  size_t memo_cap = 0;
   void invalidate() { valid = false; tables_valid = false; }
   void release();
 };
@@ -53,5 +56,12 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
 // TraversabilityMap::checkCircularFootprintPath for a batch of paths on a complete traversability_footprint layer (device pointers).
 void launch_check_paths(const SlabView& v, const te_geometry* g, double traversability_default, const float* footprint, const float* robot_slope, int npaths,
                         const int* path_begin, const double* xy, unsigned char* is_safe, double* trav, cudaStream_t s);
+
+// The same on the chain layers with an empty traversability_footprint cache per path (te_check_footprint_paths_fresh); whole map,
+// device pointers, radius / compute_untraversable_polygon per path.  Asynchronous on `s`.
+int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                             const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                             int npaths, const int* path_begin, const double* xy, const double* radius, const unsigned char* cup,
+                             unsigned char* is_safe, double* trav_out, cudaStream_t s);
 
 }  // namespace te
