@@ -261,6 +261,46 @@ int te_check_footprint_paths_fresh(te_ctx* ctx, const te_geometry* g, const te_f
                                    const double* radius, const uint8_t* compute_untraversable_polygon_or_null, uint8_t* is_safe,
                                    double* traversability_out, int memory);
 
+/* checkPolygonalFootprintPath (TraversabilityMap.cpp:464-584), the half of the check_footprint_path service that runs when
+ * FootprintPath.footprint has vertices (checkFootprintPath :320-343), for a batch of paths on the chain layers.  Per pose k of a
+ * path the footprint is placed with the pose's full 3-D orientation: vertex = R(q_k) * v + t_k, x and y kept (:488-508), R being
+ * Eigen's Quaternion::toRotationMatrix of (qx, qy, qz, qw) AS GIVEN (not normalised), v the float32 vertex widened to double.  A
+ * single-pose path checks that polygon (:522-543); a longer path checks the convex hull of consecutive footprints per segment
+ * (:545-579) and combines the segment means weighted by hull area: area += getArea(hull) - getArea(polygon1).  With
+ * conservative[q] set (FootprintPath.conservative; NULL = all 0) each footprint also gets the previous one shifted forward and vice
+ * versa (:510-520); the lists accumulate along the path, and getArea is taken of the concatenated (non-simple) polygon1 list, as
+ * the reference does.  isTraversable(polygon) (:592-645): PolygonIterator over the hull's bounding box bound to the map, unsafe at
+ * the first cell failing isTraversableForFilters, else the mean of traversability (traversability_default for invalid cells; the
+ * default when no cell centre is inside, traversable iff it is != 0).  robot_slope_or_null switches checkRobotInclination_ on
+ * (checkInclination, :748-762) as in te_check_footprint_paths2.
+ * RECALLED, not in the reference checkout: grid_map 1.6.x Polygon::convexHull (monotone chain of polygon1 ++ polygon2, lexicographic
+ * sort, cross <= 0 pops; 3 points or fewer kept as given), Polygon::getArea (shoelace from j = n-1, abs(area / 2.0)),
+ * Polygon::isInside, PolygonIterator, and Eigen's toRotationMatrix operand order (oracle/README.md).
+ * Arguments: footprint_xyz = nfootprint (1..16) vertices x, y, z as float32 (geometry_msgs/Point32), a HOST array in both modes,
+ * shared by every path; poses = 7 doubles per pose, x y z qx qy qz qw (geometry_msgs/Pose order); path q = poses
+ * path_begin[q] .. path_begin[q+1]-1, nposes = path_begin[npaths].  From `p` only traversability_default, max_gap_width,
+ * critical_step_height and verify_roughness are used.  compute_untraversable_polygon is not an argument: in isTraversable it only
+ * changes the published polygon, never is_safe, traversability or area.  Outputs: TraversabilityResult.is_safe, .traversability,
+ * .area.  Poses outside the map are legal (PolygonIterator bounds the hull to the map); with robot_slope a pose outside the map
+ * makes the path unsafe.  An empty path is unsafe with 0.
+ * Deviation: an unsafe path reports 0 in traversability and area; the reference returns early (:536-538, :564-567) and leaves the
+ * values of earlier segments in its result.  A footprint of zero area (1 or 2 vertices, collinear) can give a combined area of 0
+ * and traversability 0/0 = NaN, as in the reference.
+ * Limits: a conservative path may not need more than 1024 vertices in polygon2 (nfootprint * poses <= 1024).  Whole maps only.
+ * Errors: TE_ERR_MISSING_LAYER for a missing layer; TE_ERR_BAD_ARG for null pointers, a negative count, nfootprint outside 1..16,
+ * a non-finite footprint vertex, and in TE_MEM_HOST for nposes != path_begin[npaths], a decreasing path_begin or a non-finite
+ * pose; TE_ERR_UNSUPPORTED in TE_MEM_HOST for a conservative path past the vertex cap, and in TE_MEM_DEVICE for a non-zero start
+ * index.  TE_MEM_DEVICE is asynchronous on the context stream and cannot read the paths: a path it cannot check (non-finite
+ * pose, past the conservative cap, a range outside 0..nposes) gets is_safe = 0 and NaN in traversability and area.  A conservative
+ * flag array in TE_MEM_DEVICE sizes the kernel's shared memory for the cap (slower); TE_MEM_HOST sizes it from the paths and
+ * takes a circular-buffer start index (the layers are unwrapped on upload). */
+int te_check_footprint_paths_polygon(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, const float* traversability,
+                                     const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                                     const float* robot_slope_or_null, int32_t nfootprint, const float* footprint_xyz, int32_t npaths,
+                                     int32_t nposes, const int32_t* path_begin, const double* poses,
+                                     const uint8_t* conservative_or_null, uint8_t* is_safe, double* traversability_out,
+                                     double* area_out, int memory);
+
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the
  * neighbours' boundary columns of the INPUT layer(s) into this rank's halo.  The reference has no counterpart (it is a

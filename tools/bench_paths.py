@@ -9,6 +9,11 @@ map, (b) what it returns once the footprint layer has been swept.  Paths are pla
 with the GPU name and its power limit.
 
     python tools/bench_paths.py [--size 4096] [--reps 20]
+
+--footprint polygon times te_check_footprint_paths_polygon (TE_MEM_DEVICE) instead, with the YAML footprint polygon
+(robot_footprint_parameter.yaml:3) and planner-like paths with a random yaw per pose, conservative off and on, and the CPU oracle
+of the same call (tests/polygon_paths_oracle.cpp, all host threads, one run; it includes the oracle's whole-map
+isTraversableForFilters pass, which the GPU evaluates only where a polygon looks).
 """
 from __future__ import annotations
 
@@ -57,7 +62,10 @@ def main():
     ap.add_argument("--size", type=int, default=4096)
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--footprint", choices=("circle", "polygon"), default="circle")
     args = ap.parse_args()
+    if args.footprint == "polygon":
+        return main_polygon(args)
     import torch
     import synth
     import traversability_estimation_b200 as te
@@ -118,6 +126,75 @@ def main():
                           "offset": fp.offset, "paths": batch, "poses": int(begin[-1]), **res_ms,
                           "safe_fresh": int(safe_a.sum().item()), "safe_swept": int(safe_b.sum().item()), "is_safe_differs": differ}),
               flush=True)
+    ctx.set_stream(None)
+    ctx.close()
+
+
+YAML_FOOTPRINT = [(0.45, 0.30, 0.0), (0.45, -0.30, 0.0), (-0.45, -0.30, 0.0), (-0.45, 0.30, 0.0)]  # robot_footprint_parameter.yaml:3
+
+
+def main_polygon(args):
+    import time
+    import torch
+    import synth
+    import traversability_estimation_b200 as te
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import polygon_paths_oracle as ppo
+    from oracle import binding as ob
+
+    n, res = args.size, 0.02
+    g, og = te.Geometry.make(n, n, res), ob.Geometry.make(n, n, res)
+    fp, ofp = te.FootprintParams.yaml_defaults(), ob.FootprintParams.yaml_defaults()
+    fxyz = np.asarray(YAML_FOOTPRINT, np.float32)
+    ctx = te.Context(0)
+    z = synth.terrain(n, n, res, 4096, "mixed")
+    layers = ctx.chain_host(g, te.ChainParams.yaml_defaults(0), z)
+    dev = lambda a: torch.from_numpy(np.ascontiguousarray(np.asarray(a, np.float32).T)).cuda()  # noqa: E731
+    trav, slope, step, elev = (dev(a) for a in (layers["traversability"], layers["slope"], layers["step"], z))
+    stream = torch.cuda.Stream()
+    ctx.set_stream(stream.cuda_stream)
+    name, power = gpu_info(torch)
+    rng = np.random.default_rng(1)
+    for batch in (1, 100, 1000):
+        begin, xy = planner_paths(rng, n, batch, res)
+        yaw = rng.uniform(0, 2 * np.pi, len(xy))
+        poses = np.stack([xy[:, 0], xy[:, 1], np.zeros(len(xy)), np.zeros(len(xy)), np.zeros(len(xy)), np.sin(yaw / 2),
+                          np.cos(yaw / 2)], axis=1)
+        db, dp = torch.from_numpy(begin).cuda(), torch.from_numpy(poses).cuda()
+        for conservative in (0, 1):
+            cons = np.full(batch, conservative, np.uint8)
+            dc = torch.from_numpy(cons).cuda()
+            safe = torch.empty(batch, dtype=torch.uint8, device="cuda")
+            tout = torch.empty(batch, dtype=torch.float64, device="cuda")
+            aout = torch.empty(batch, dtype=torch.float64, device="cuda")
+            torch.cuda.synchronize()
+
+            def run():
+                ctx.check_footprint_paths_polygon(g, fp, trav, slope, step, elev, fxyz, db, dp, conservative=dc if conservative else None,
+                                                  memory=te.MEM_DEVICE, is_safe=safe, traversability_out=tout, area_out=aout)
+
+            for _ in range(args.warmup):
+                run()
+            stream.synchronize()
+            ts = []
+            for _ in range(args.reps):
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                run()
+                e1.record(stream)
+                e1.synchronize()
+                ts.append(e0.elapsed_time(e1))
+            t0 = time.perf_counter()
+            want = ppo.check_polygonal_paths(og, ofp, layers["traversability"], layers["slope"], layers["step"], z, fxyz, begin, poses,
+                                             conservative=cons if conservative else None)
+            cpu_ms = (time.perf_counter() - t0) * 1e3
+            got = (safe.cpu().numpy(), tout.cpu().numpy(), aout.cpu().numpy())
+            same = all(np.array_equal(a.view(np.uint8), b.view(np.uint8)) for a, b in zip(got, want))
+            print(json.dumps({"gpu": name, "power_limit_w": power, "map": f"{n}x{n}", "resolution": res, "footprint": "yaml_polygon",
+                              "paths": batch, "poses": int(begin[-1]), "conservative": conservative,
+                              "gpu_median_ms": float(np.median(ts)), "gpu_min_ms": float(np.min(ts)),
+                              "cpu_oracle_ms": cpu_ms, "cpu_threads": os.cpu_count(), "safe": int(got[0].sum()),
+                              "matches_oracle": bool(same)}), flush=True)
     ctx.set_stream(None)
     ctx.close()
 

@@ -18,7 +18,7 @@ KERNEL_AUTO, KERNEL_GENERIC, KERNEL_FUSED = 0, 1, 2
 
 EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set_stream", "te_synchronize",
            "te_set_kernel", "te_get_stats", "te_enable_timing", "te_get_timing", "te_get_flag_counters", "te_get_escalation_stats", "te_fused_plan", "te_slope", "te_normals", "te_step", "te_roughness", "te_chain",
-           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
+           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
            "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free"]
 
 
@@ -329,6 +329,44 @@ class Context:
             self._h, C.byref(g), C.byref(fp), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), n, pb.ctypes.data,
             xy.ctypes.data, rad.ctypes.data, _addr(cup), safe.ctypes.data, trav.ctypes.data, MEM_HOST))
         return safe, trav
+
+    def check_footprint_paths_polygon(self, g, fp, traversability, slope, step, elevation, footprint_xyz, path_begin, poses,
+                                      robot_slope=None, roughness=None, conservative=None, memory=MEM_HOST, is_safe=None,
+                                      traversability_out=None, area_out=None):
+        """te_check_footprint_paths_polygon: checkPolygonalFootprintPath on the chain layers.  footprint_xyz: (n, 3) vertices
+        (float32, host in both modes); poses: (nposes, 7) x y z qx qy qz qw; conservative: FootprintPath.conservative per path.
+        fp supplies traversability_default, max_gap_width, critical_step_height and verify_roughness.  MEM_HOST: numpy arguments,
+        returns (is_safe uint8, traversability float64, area float64) per path.  MEM_DEVICE: every other argument is a device
+        tensor (path_begin int32, poses float64, conservative uint8) and the results go to the caller's is_safe /
+        traversability_out / area_out tensors."""
+        sig = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + [C.c_int32, C.c_void_p, C.c_int32,
+                                                                                                 C.c_int32] + [C.c_void_p] * 6 + [C.c_int]
+        self._L.te_check_footprint_paths_polygon.argtypes = sig
+        fxyz = np.ascontiguousarray(footprint_xyz, dtype=np.float32).reshape(-1, 3)
+        if memory == MEM_DEVICE:
+            self._order_after_torch(memory)
+            n = int(path_begin.numel()) - 1
+            nposes = int(poses.numel()) // 7
+            self._check(self._L.te_check_footprint_paths_polygon(
+                self._h, C.byref(g), C.byref(fp), _addr(traversability), _addr(slope), _addr(step), _addr(roughness), _addr(elevation),
+                _addr(robot_slope), len(fxyz), fxyz.ctypes.data, n, nposes, _addr(path_begin), _addr(poses), _addr(conservative),
+                _addr(is_safe), _addr(traversability_out), _addr(area_out), MEM_DEVICE))
+            return is_safe, traversability_out, area_out
+        lay = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)  # noqa: E731
+        t, s, st, e, rs, r = (lay(a) for a in (traversability, slope, step, elevation, robot_slope, roughness))
+        pb = np.ascontiguousarray(path_begin, dtype=np.int32)
+        ps = np.ascontiguousarray(poses, dtype=np.float64).reshape(-1, 7)
+        cons = None if conservative is None else np.ascontiguousarray(conservative, dtype=np.uint8)
+        n = len(pb) - 1
+        if cons is not None and len(cons) != n:
+            raise ValueError("conservative needs one entry per path")
+        safe = np.zeros(n, dtype=np.uint8) if is_safe is None else is_safe
+        trav = np.zeros(n, dtype=np.float64) if traversability_out is None else traversability_out
+        area = np.zeros(n, dtype=np.float64) if area_out is None else area_out
+        self._check(self._L.te_check_footprint_paths_polygon(
+            self._h, C.byref(g), C.byref(fp), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), len(fxyz), fxyz.ctypes.data,
+            n, len(ps), pb.ctypes.data, ps.ctypes.data, _addr(cons), safe.ctypes.data, trav.ctypes.data, area.ctypes.data, MEM_HOST))
+        return safe, trav, area
 
     # ---- multi-GPU halo (te_halo_pull and the IPC helpers around it)
     def ipc_export(self, device_ptr) -> bytes:

@@ -1067,6 +1067,101 @@ int te_check_footprint_paths_fresh(te_ctx* c, const te_geometry* g_in, const te_
   return TE_OK;
 }
 
+int te_check_footprint_paths_polygon(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
+                                     const float* step, const float* rough, const float* elev, const float* robot_slope, int32_t nfootprint,
+                                     const float* footprint_xyz, int32_t npaths, int32_t nposes, const int32_t* path_begin,
+                                     const double* poses, const uint8_t* conservative, uint8_t* is_safe, double* traversability,
+                                     double* area, int memory) {
+  TE_ENTER(c);
+  if (int rc = check_geometry(g_in, true)) return rc;
+  const int sr = g_in->start_row, sc = g_in->start_col;  // circular-buffer maps: host memory only, like te_footprint2
+  const bool wrapped = sr != 0 || sc != 0;
+  if (wrapped && memory == TE_MEM_DEVICE)
+    return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0) is supported for maps in host memory only", sr, sc);
+  te_geometry g0 = *g_in;
+  g0.start_row = g0.start_col = 0;
+  const te_geometry* g = &g0;
+  if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
+  if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
+  if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
+  if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
+  if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
+  if (p->verify_roughness && !rough) return fail(TE_ERR_MISSING_LAYER, "layer traversability_roughness is missing (verify_roughness is set)");
+  if (npaths < 0 || nposes < 0 || !path_begin || !poses || !footprint_xyz || !is_safe || !traversability || !area)
+    return fail(TE_ERR_BAD_ARG, "null argument or negative count");
+  if (nfootprint < 1 || nfootprint > te::kPolyMaxVerts) return fail(TE_ERR_BAD_ARG, "footprint needs 1..%d vertices, got %d", te::kPolyMaxVerts, nfootprint);
+  for (int k = 0; k < 3 * nfootprint; ++k)
+    if (!std::isfinite(footprint_xyz[k])) return fail(TE_ERR_BAD_ARG, "footprint vertex %d is not finite", k / 3);
+  if (npaths == 0) return TE_OK;
+  const bool use_rough = p->verify_roughness != 0;
+  if (int rc = ensure_geometry(c, g)) return rc;
+  const te_slab s{0, g->cols, 0, 0};
+  const te::SlabView v = make_view(c, g, s);
+  int nl = 0;
+  if (memory == TE_MEM_DEVICE) {  // nothing is read back: a path that cannot be checked gets is_safe 0, traversability and area NaN
+    const int mp = conservative ? 2 * te::kPolyConsCap : 2 * nfootprint;
+    int rc = te::launch_check_paths_polygon(c->fp, v, g, p, trav, slope, step, use_rough ? rough : nullptr, elev, robot_slope, nfootprint,
+                                            footprint_xyz, npaths, nposes, path_begin, poses, conservative, mp, is_safe, traversability,
+                                            area, c->stream, &nl);
+    if (rc != 0) return fail(rc, "polygonal path check failed: %s", c->fp.why.c_str());
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(TE_ERR_CUDA, "polygonal path check launch failed: %s", cudaGetErrorString(e));
+    c->launches += nl;
+    return TE_OK;
+  }
+  if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
+  if (path_begin[npaths] != nposes) return fail(TE_ERR_BAD_ARG, "path_begin[npaths] = %d != nposes = %d", path_begin[npaths], nposes);
+  int mp = 2 * nfootprint;
+  for (int32_t q = 0; q < npaths; ++q) {
+    const int32_t n = path_begin[q + 1] - path_begin[q];
+    if (n < 0) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
+    if (conservative && conservative[q] && n > 1) {
+      if ((long long)nfootprint * n > te::kPolyConsCap)
+        return fail(TE_ERR_UNSUPPORTED, "conservative path %d needs %lld polygon vertices, more than %d", q, (long long)nfootprint * n,
+                    te::kPolyConsCap);
+      mp = std::max(mp, 2 * nfootprint * n);
+    }
+  }
+  for (size_t k = 0; k < 7 * (size_t)nposes; ++k)
+    if (!std::isfinite(poses[k])) return fail(TE_ERR_BAD_ARG, "pose %zu is not finite", k / 7);
+  const size_t lbytes = sizeof(float) * (size_t)g->rows * g->cols;
+  // staging: layers 0..3 (+ roughness 11, robot_slope 4), paths 5, 6, 8, results 9, 10, 7
+  const float* in[6] = {trav, slope, step, elev, use_rough ? rough : nullptr, robot_slope};
+  const int slot_in[6] = {0, 1, 2, 3, 11, 4};
+  for (int k = 0; k < 6; ++k) {
+    if (!in[k]) continue;
+    TE_CUDA(c->stage[slot_in[k]].reserve(lbytes));
+    if (wrapped) TE_CUDA(copy_wrapped((float*)c->stage[slot_in[k]].p, 0, const_cast<float*>(in[k]), g->rows, g->cols, sr, sc, 0, g->cols, true, c->stream));
+    else TE_CUDA(cudaMemcpyAsync(c->stage[slot_in[k]].p, in[k], lbytes, cudaMemcpyHostToDevice, c->stream));
+    in[k] = (const float*)c->stage[slot_in[k]].p;
+  }
+  TE_CUDA(c->stage[5].reserve(sizeof(int32_t) * (size_t)(npaths + 1)));
+  TE_CUDA(c->stage[6].reserve(sizeof(double) * 7 * (size_t)std::max(nposes, 1)));
+  TE_CUDA(c->stage[7].reserve(sizeof(double) * (size_t)npaths));
+  TE_CUDA(c->stage[9].reserve((size_t)npaths));
+  TE_CUDA(c->stage[10].reserve(sizeof(double) * (size_t)npaths));
+  TE_CUDA(cudaMemcpyAsync(c->stage[5].p, path_begin, sizeof(int32_t) * (size_t)(npaths + 1), cudaMemcpyHostToDevice, c->stream));
+  if (nposes > 0) TE_CUDA(cudaMemcpyAsync(c->stage[6].p, poses, sizeof(double) * 7 * (size_t)nposes, cudaMemcpyHostToDevice, c->stream));
+  const unsigned char* dcons = nullptr;
+  if (conservative) {
+    TE_CUDA(c->stage[8].reserve((size_t)npaths));
+    TE_CUDA(cudaMemcpyAsync(c->stage[8].p, conservative, (size_t)npaths, cudaMemcpyHostToDevice, c->stream));
+    dcons = (const unsigned char*)c->stage[8].p;
+  }
+  int rc = te::launch_check_paths_polygon(c->fp, v, g, p, in[0], in[1], in[2], in[4], in[3], in[5], nfootprint, footprint_xyz, npaths, nposes,
+                                          (const int*)c->stage[5].p, (const double*)c->stage[6].p, dcons, mp, (unsigned char*)c->stage[9].p,
+                                          (double*)c->stage[10].p, (double*)c->stage[7].p, c->stream, &nl);
+  if (rc != 0) return fail(rc, "polygonal path check failed: %s", c->fp.why.c_str());
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(TE_ERR_CUDA, "polygonal path check launch failed: %s", cudaGetErrorString(e));
+  c->launches += nl;
+  TE_CUDA(cudaMemcpyAsync(is_safe, c->stage[9].p, (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
+  TE_CUDA(cudaMemcpyAsync(traversability, c->stage[10].p, sizeof(double) * (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
+  TE_CUDA(cudaMemcpyAsync(area, c->stage[7].p, sizeof(double) * (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
+  TE_CUDA(cudaStreamSynchronize(c->stream));
+  return TE_OK;
+}
+
 // A te IPC handle is the CUDA handle of the ALLOCATION that contains the pointer (cudaIpcGetMemHandle always describes the whole
 // allocation; sub-allocating pools such as torch's caching allocator hand out interior pointers) plus the offset into it.
 struct TeIpcHandle {

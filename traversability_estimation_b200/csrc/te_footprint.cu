@@ -1293,6 +1293,289 @@ __global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, P
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// TraversabilityMap::checkPolygonalFootprintPath (TraversabilityMap.cpp:464-584) for a batch of paths that share one footprint
+// polygon.  A work item is one polygon the reference evaluates: the footprint at the pose of a single-pose path, or the convex hull
+// of segment (k-1, k) of a longer path.  Items are independent (the polygonal check keeps no traversability_footprint cache), so
+// k_check_polygon_items runs one warp per pose index and k_check_polygon_combine folds the items of a path in order (:569-579).
+struct PolyItem {
+  int q;             // path of the item; -1: the pose is not an item
+  int flag;          // 0: unsafe (checkInclination or isTraversable failed), 1: traversable, 2: not checkable
+  double mean;       // isTraversable's `traversability`
+  double hull_area;  // getArea of the checked polygon (the hull, or polygon2 for a single pose)
+  double poly1_area; // getArea of the (possibly augmented) polygon1 list
+};
+
+struct PolyPathArgs {
+  const float* rslope;           // robot_slope, nullptr: checkRobotInclination_ off
+  int npaths, nposes, nfp;
+  int mcap;                      // hull input points one warp's shared memory holds (2 * mcap + mcap double2)
+  const int* path_begin;
+  const double* poses;           // 7 per pose: x y z qx qy qz qw
+  const unsigned char* cons;     // FootprintPath.conservative per path, nullptr: all 0
+  unsigned char* memo;           // per map cell isTraversableForFilters memo (see blocked_memo_d)
+  PolyItem* items;               // [nposes]
+  unsigned char* is_safe;
+  double* trav_out;
+  double* area_out;
+  float fx[kPolyMaxVerts], fy[kPolyMaxVerts], fz[kPolyMaxVerts];  // footprint vertices (geometry_msgs/Point32)
+};
+
+// Translation * Quaternion of a pose: Eigen::QuaternionBase::toRotationMatrix of the quaternion as given (not normalised), rows 0
+// and 1 (the z of a transformed vertex is dropped, :505-507).
+struct PoseRT {
+  double tx, ty, r00, r01, r02, r10, r11, r12;
+};
+__device__ __forceinline__ PoseRT pose_rt_d(const double* p) {
+  const double qx = p[3], qy = p[4], qz = p[5], qw = p[6];
+  const double tx = 2.0 * qx, ty = 2.0 * qy, tz = 2.0 * qz;
+  const double twx = tx * qw, twy = ty * qw, twz = tz * qw;
+  const double txx = tx * qx, txy = ty * qx, txz = tz * qx;
+  const double tyy = ty * qy, tyz = tz * qy, tzz = tz * qz;
+  PoseRT T;
+  T.tx = p[0]; T.ty = p[1];
+  T.r00 = 1.0 - (tyy + tzz); T.r01 = txy - twz; T.r02 = txz + twy;
+  T.r10 = txy + twz; T.r11 = 1.0 - (txx + tzz); T.r12 = tyz - twx;
+  return T;
+}
+
+// `toPosition * orientation * positionToVertex` (:496-500) for footprint vertex v, in the operand order of Eigen's Transform * vector.
+__device__ __forceinline__ double2 footprint_vertex_d(const PolyPathArgs& P, const PoseRT& T, int v) {
+  const double vx = (double)P.fx[v], vy = (double)P.fy[v], vz = (double)P.fz[v];
+  return make_double2(((T.r00 * vx + T.r01 * vy) + T.r02 * vz) + T.tx, ((T.r10 * vx + T.r11 * vy) + T.r12 * vz) + T.ty);
+}
+
+// grid_map::Polygon::getArea (recalled, see the oracle): the shoelace sum in vertex order, one thread.
+__device__ double polygon_area_d(const double2* v, int n) {
+  double area = 0.0;
+  int j = n - 1;
+  for (int i = 0; i < n; i++) {
+    area += (v[j].x + v[i].x) * (v[j].y - v[i].y);
+    j = i;
+  }
+  return fabs(area / 2.0);
+}
+
+// grid_map::Polygon::isInside (crossing-number test over (v[i], v[i-1]), as poly_inside_d) on a vertex list in shared memory.
+__device__ __forceinline__ bool polygon_inside_d(const double2* v, int n, double px, double py) {
+  int cross = 0;
+  for (int i = 0, j = n - 1; i < n; j = i++) {
+    if (((v[i].y > py) != (v[j].y > py)) && (px < (v[j].x - v[i].x) * (py - v[i].y) / (v[j].y - v[i].y) + v[i].x)) ++cross;
+  }
+  return (cross & 1) != 0;
+}
+
+__device__ __forceinline__ bool lex_less_d(double2 a, double2 b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
+
+// grid_map::Polygon::monotoneChainConvexHullOfPoints (recalled) of the m > 3 points `sorted` (already in lexicographic order) into
+// `hull` (2m entries, the reference's own allocation); returns the vertex count.  One thread.
+__device__ int monotone_chain_d(const double2* sorted, int m, double2* hull) {
+  auto clockwise = [](double2 o, double2 a, double2 b) {
+    const double ux = a.x - o.x, uy = a.y - o.y, wx = b.x - o.x, wy = b.y - o.y;
+    return (ux * wy - uy * wx) <= 0;
+  };
+  int k = 0;
+  for (int i = 0; i < m; ++i) {
+    while (k >= 2 && clockwise(hull[k - 2], hull[k - 1], sorted[i])) k--;
+    hull[k++] = sorted[i];
+  }
+  for (int i = m - 2, t = k + 1; i >= 0; i--) {
+    while (k >= t && clockwise(hull[k - 2], hull[k - 1], sorted[i])) k--;
+    hull[k++] = sorted[i];
+  }
+  return k - 1;
+}
+
+// One warp per pose index p.  Shared memory per warp: sA (2 mcap points: the hull input polygon1 ++ polygon2, then the hull) and
+// sB (mcap points: a conservative path's earlier polygon2, then the sorted hull input).
+__global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L, PolyPathArgs P) {
+  extern __shared__ double2 sPoly[];
+  const int lane = threadIdx.x & 31;
+  const int p = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (p >= P.nposes) return;  // whole warp
+  double2* sA = sPoly + (size_t)(threadIdx.x >> 5) * 3 * P.mcap;
+  double2* sB = sA + 2 * P.mcap;
+  PolyItem it{-1, 2, 0.0, 0.0, 0.0};
+  // the path of pose p: the last q with path_begin[q] <= p
+  int lo = 0, hi = P.npaths - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (P.path_begin[mid] <= p) lo = mid; else hi = mid - 1;
+  }
+  const int q = lo, b = P.path_begin[q], e = P.path_begin[q + 1], n = e - b, k = p - b;
+  if (!(b >= 0 && b <= p && p < e && e <= P.nposes && (n == 1 || k >= 1))) {
+    if (lane == 0) P.items[p] = it;
+    return;
+  }
+  it.q = q;
+  const int nfp = P.nfp;
+  const bool cons = n > 1 && P.cons != nullptr && P.cons[q] != 0;
+  const int m = n == 1 ? nfp : cons ? 2 * nfp * (k + 1) : 2 * nfp;  // points of polygon1 ++ polygon2
+  bool finite = true;
+  for (int s = (cons ? 0 : max(k - 1, 0)) + lane; s <= k; s += 32)
+    for (int c = 0; c < 7; ++c) finite = finite && isfinite(P.poses[7 * (size_t)(b + s) + c]);
+  if (!__all_sync(0xffffffffu, finite) || m > P.mcap || (cons && nfp * (k + 1) > kPolyConsCap)) {
+    if (lane == 0) P.items[p] = it;  // flag 2
+    return;
+  }
+  const double* pk = P.poses + 7 * (size_t)(b + k);
+  const double ex = pk[0], ey = pk[1];
+  const double sx = n == 1 ? ex : pk[-7], sy = n == 1 ? ey : pk[-6];
+  const int h = m / 2;  // polygon1 = sA[0, h), polygon2 = sA[h, m) for n > 1
+  if (n == 1) {  // polygon2 of the pose
+    const PoseRT T = pose_rt_d(pk);
+    if (lane < nfp) sA[lane] = footprint_vertex_d(P, T, lane);
+  } else if (!cons) {  // polygon1 = T_{k-1}(footprint), polygon2 = T_k(footprint)
+    const PoseRT T = pose_rt_d(lane < nfp ? pk - 7 : pk);
+    if (lane < 2 * nfp) sA[lane] = footprint_vertex_d(P, T, lane < nfp ? lane : lane - nfp);
+  } else {
+    // polygon2 of pose k-1 by footprint slot s = 0..k-1 (list order: slot k-1 first): slot s holds T_s(footprint) plus the
+    // start-to-end vectors d_{s+1}, ..., d_{k-1} added in that order (:510-520).  Entry i is always lane i % 32's.
+    for (int j = 0; j < k; ++j) {
+      const double* pj = P.poses + 7 * (size_t)(b + j);
+      const PoseRT T = pose_rt_d(pj);
+      const double dx = j > 0 ? pj[0] - pj[-7] : 0.0, dy = j > 0 ? pj[1] - pj[-6] : 0.0;
+      for (int i = lane; i < nfp * (j + 1); i += 32) {
+        if (i >= nfp * j) sB[i] = footprint_vertex_d(P, T, i - nfp * j);
+        else sB[i] = make_double2(sB[i].x + dx, sB[i].y + dy);
+      }
+    }
+    __syncwarp();
+    // polygon1 = polygon2(k-1) ++ (T_k(footprint) - d_k); polygon2 = T_k(footprint) ++ (polygon2(k-1) + d_k)
+    const PoseRT T = pose_rt_d(pk);
+    const double dx = ex - sx, dy = ey - sy;
+    const int ns = nfp * k;
+    for (int l = lane; l < h; l += 32) {
+      if (l < ns) {
+        const double2 w = sB[(k - 1 - l / nfp) * nfp + l % nfp];
+        sA[l] = w;
+        sA[h + nfp + l] = make_double2(w.x + dx, w.y + dy);
+      } else {
+        const double2 w = footprint_vertex_d(P, T, l - ns);
+        sA[l] = make_double2(w.x - dx, w.y - dy);
+        sA[h + l - ns] = w;
+      }
+    }
+  }
+  __syncwarp();
+  if (lane == 0 && n > 1 && k > 1) it.poly1_area = polygon_area_d(sA, h);
+  int nh = m;  // Polygon(points) as given: a single pose's polygon2, or a hull input of at most 3 points
+  if (n > 1 && m > 3) {
+    // lexicographic order by rank (ties between equal points by position; they change no later result)
+    for (int i = lane; i < m; i += 32) {
+      const double2 a = sA[i];
+      int r = 0;
+      for (int j = 0; j < m; ++j) {
+        const double2 c = sA[j];
+        r += (lex_less_d(c, a) || (c.x == a.x && c.y == a.y && j < i)) ? 1 : 0;
+      }
+      sB[r] = a;
+    }
+    __syncwarp();
+    if (lane == 0) nh = monotone_chain_d(sB, m, sA);
+    nh = __shfl_sync(0xffffffffu, nh, 0);
+    __syncwarp();
+  }
+  if (lane == 0) it.hull_area = polygon_area_d(sA, nh);
+  // checkInclination (:524-526, :550-554), then isTraversable(polygon) (:592-645)
+  bool ok = inclination_ok_d(A, P.rslope, sx, sy, ex, ey);
+  double t = 0.0;
+  if (ok) {
+    double tlx = sA[0].x, tly = sA[0].y, brx = tlx, bry = tly;  // PolygonIterator::findSubmapParameters
+    for (int i = 1; i < nh; ++i) {
+      const double2 w = sA[i];
+      tlx = fmax(tlx, w.x); tly = fmax(tly, w.y);
+      brx = fmin(brx, w.x); bry = fmin(bry, w.y);
+    }
+    bound_position_d(A, tlx, tly);
+    bound_position_d(A, brx, bry);
+    int si, sj, ei, ej;
+    get_index_d(A, tlx, tly, si, sj);
+    get_index_d(A, brx, bry, ei, ej);
+    const int nr = ei - si + 1, nc = ej - sj + 1;
+    const long long total = (nr > 0 && nc > 0) ? (long long)nr * nc : 0;
+    unsigned cnt = 0;
+    for (long long base = 0; base < total; base += 32) {  // SubmapIterator order, 32 cells per pass; the sum in visit order
+      const long long c = base + lane;
+      bool member = false, blk = false;
+      double v = 0.0;
+      if (c < total) {
+        const int a = si + (int)(c / nc), bb = sj + (int)(c % nc);
+        if (a >= 0 && bb >= 0 && a < A.rows && bb < A.cols_total && polygon_inside_d(sA, nh, A.X[a], A.Y[bb])) {
+          member = true;
+          blk = blocked_memo_d(A, L, P.memo, a, bb);
+          if (!blk) {
+            const float f = __ldg(L.trav + (size_t)bb * A.rows + a);
+            v = finitef(f) ? (double)f : A.tdefault;  // :613-619
+          }
+        }
+      }
+      if (__any_sync(0xffffffffu, blk)) { ok = false; break; }  // :602-611
+      const unsigned take = __ballot_sync(0xffffffffu, member);
+      cnt += __popc(take);
+#pragma unroll
+      for (int l = 0; l < 32; ++l) {
+        const double o = __shfl_sync(0xffffffffu, v, l);
+        if ((take >> l) & 1u) t += o;
+      }
+    }
+    if (ok) {
+      if (cnt == 0) {  // :623-628
+        t = A.tdefault;
+        ok = A.tdefault != 0.0;
+      } else {
+        t /= (double)cnt;  // :630
+      }
+    }
+  }
+  if (lane == 0) {
+    it.flag = ok ? 1 : 0;
+    it.mean = t;
+    P.items[p] = it;
+  }
+}
+
+// One thread per path: the area-weighted combination of the segment results in path order (:522-579).  An unsafe path reports 0;
+// a path the items could not check (bad range, non-finite pose, conservative list past the cap) is_safe 0 and NaN.
+__global__ void __launch_bounds__(128) k_check_polygon_combine(PolyPathArgs P) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= P.npaths) return;
+  const int b = P.path_begin[q], e = P.path_begin[q + 1], n = e - b;
+  bool checkable = b >= 0 && e >= b && e <= P.nposes;
+  unsigned char safe = 0;
+  double trav = 0.0, area = 0.0;
+  if (checkable && n > 0) {
+    const bool cons = n > 1 && P.cons != nullptr && P.cons[q] != 0;
+    if (cons && (long long)P.nfp * n > kPolyConsCap) checkable = false;
+    for (long long c = 7LL * b; c < 7LL * e && checkable; ++c) checkable = isfinite(P.poses[c]);
+    const int k0 = n == 1 ? 0 : 1;
+    for (int k = k0; k < n && checkable; ++k) checkable = P.items[b + k].q == q && P.items[b + k].flag != 2;
+    if (checkable) {
+      bool ok = true;
+      for (int k = k0; k < n && ok; ++k) {
+        const PolyItem it = P.items[b + k];
+        ok = it.flag == 1;
+        if (!ok) break;  // :536-538, :564-567
+        if (n == 1 || k == 1) {  // :541-542, :576-578
+          area = it.hull_area;
+          trav = it.mean;
+        } else {  // :570-575
+          const double areaPrevious = area;
+          const double areaPolygon = it.hull_area - it.poly1_area;
+          area += areaPolygon;
+          trav = (areaPolygon * it.mean + areaPrevious * trav) / area;
+        }
+      }
+      if (ok) safe = 1;
+      else trav = area = 0.0;
+    }
+  }
+  if (!checkable) trav = area = nan("");
+  P.is_safe[q] = safe;
+  P.trav_out[q] = trav;
+  P.area_out[q] = area;
+}
+
 inline int signum(int v) { return (0 < v) - (v < 0); }
 
 // grid_map::SpiralIterator::generateRing, executed literally (SURVEY.md A.3): rings 0 .. nRings in visit order, packed
@@ -1338,8 +1621,9 @@ void FootprintState::release() {
   if (d_list) cudaFree(d_list);
   if (d_rings) cudaFree(d_rings);
   if (d_memo) cudaFree(d_memo);
-  d_rings = d_memo = nullptr;
-  memo_cap = 0;
+  if (d_items) cudaFree(d_items);
+  d_rings = d_memo = d_items = nullptr;
+  memo_cap = items_cap = 0;
   for (int k = 0; k < 2; ++k) {
     if (d_poly[k]) cudaFree(d_poly[k]);
     d_poly[k] = nullptr;
@@ -1385,6 +1669,19 @@ FpArgs filter_args(const SlabView& v, const te_geometry* g, const te_footprint_p
   a.step_R = (int)std::floor(2.5 * g->resolution / g->resolution) + 1;
   return a;
 }
+
+// The per-call isTraversableForFilters memo of the path checks (blocked_memo_d): one byte per map cell, cleared on `s`.
+int reset_filter_memo(FootprintState& st, const SlabView& v, cudaStream_t s) {
+  const size_t ncell = (size_t)v.rows * v.cols_total;
+  if (st.memo_cap < ncell) {
+    if (st.d_memo) cudaFree(st.d_memo);
+    st.d_memo = nullptr; st.memo_cap = 0;
+    if (cudaMalloc(&st.d_memo, ncell) != cudaSuccess) { st.why = "cudaMalloc(predicate memo) failed"; return TE_ERR_CUDA; }
+    st.memo_cap = ncell;
+  }
+  if (cudaMemsetAsync(st.d_memo, 0, ncell, s) != cudaSuccess) { st.why = "cudaMemsetAsync(predicate memo) failed"; return TE_ERR_CUDA; }
+  return 0;
+}
 }  // namespace
 
 int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
@@ -1405,14 +1702,7 @@ int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geo
       return TE_ERR_CUDA;
     }
   }
-  const size_t ncell = (size_t)v.rows * v.cols_total;
-  if (st.memo_cap < ncell) {
-    if (st.d_memo) cudaFree(st.d_memo);
-    st.d_memo = nullptr; st.memo_cap = 0;
-    if (cudaMalloc(&st.d_memo, ncell) != cudaSuccess) { st.why = "cudaMalloc(predicate memo) failed"; return TE_ERR_CUDA; }
-    st.memo_cap = ncell;
-  }
-  if (cudaMemsetAsync(st.d_memo, 0, ncell, s) != cudaSuccess) { st.why = "cudaMemsetAsync(predicate memo) failed"; return TE_ERR_CUDA; }
+  if (int rc = reset_filter_memo(st, v, s)) return rc;
   const FpArgs a = filter_args(v, g, p, rough);
   const Layers L{trav, slope, step, elev, rough};
   PathArgs P{};
@@ -1424,6 +1714,51 @@ int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geo
   P.is_safe = is_safe; P.trav_out = trav_out;
   const long long threads = 32LL * npaths;
   k_check_paths_fresh<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P);
+  return 0;
+}
+
+int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                               const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                               int nfp, const float* footprint_xyz, int npaths, int nposes, const int* path_begin, const double* poses,
+                               const unsigned char* conservative, int max_points, unsigned char* is_safe, double* trav_out,
+                               double* area_out, cudaStream_t s, int* launches) {
+  *launches = 0;
+  if (nfp < 1 || nfp > kPolyMaxVerts || max_points < 2 * nfp || max_points > 2 * kPolyConsCap) { st.why = "bad footprint size"; return TE_ERR_BAD_ARG; }
+  if (int rc = reset_filter_memo(st, v, s)) return rc;
+  const size_t nitems = (size_t)std::max(nposes, 1);
+  if (st.items_cap < nitems) {
+    if (st.d_items) cudaFree(st.d_items);
+    st.d_items = nullptr; st.items_cap = 0;
+    if (cudaMalloc(&st.d_items, sizeof(PolyItem) * nitems) != cudaSuccess) { st.why = "cudaMalloc(polygon items) failed"; return TE_ERR_CUDA; }
+    st.items_cap = nitems;
+  }
+  const FpArgs a = filter_args(v, g, p, rough);
+  const Layers L{trav, slope, step, elev, rough};
+  PolyPathArgs P{};
+  P.rslope = robot_slope; P.npaths = npaths; P.nposes = nposes; P.nfp = nfp; P.mcap = max_points;
+  P.path_begin = path_begin; P.poses = poses; P.cons = conservative;
+  P.memo = (unsigned char*)st.d_memo;
+  P.items = (PolyItem*)st.d_items;
+  P.is_safe = is_safe; P.trav_out = trav_out; P.area_out = area_out;
+  for (int k = 0; k < nfp; ++k) {
+    P.fx[k] = footprint_xyz[3 * k]; P.fy[k] = footprint_xyz[3 * k + 1]; P.fz[k] = footprint_xyz[3 * k + 2];
+  }
+  if (nposes > 0) {
+    // four warps per block while their shared memory stays small; one warp per block for long conservative paths
+    const size_t per_warp = sizeof(double2) * 3 * (size_t)max_points;
+    const int wpb = per_warp * 4 <= 48 * 1024 ? 4 : 1;
+    const size_t smem = per_warp * wpb;
+    if (smem > 48 * 1024 &&
+        cudaFuncSetAttribute(k_check_polygon_items, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+      st.why = "cudaFuncSetAttribute(k_check_polygon_items) failed";
+      return TE_ERR_CUDA;
+    }
+    const long long blocks = ((long long)nposes + wpb - 1) / wpb;
+    k_check_polygon_items<<<(unsigned)blocks, 32 * wpb, smem, s>>>(a, L, P);
+    ++*launches;
+  }
+  k_check_polygon_combine<<<(unsigned)((npaths + 127) / 128), 128, 0, s>>>(P);
+  ++*launches;
   return 0;
 }
 

@@ -34,8 +34,10 @@ struct FootprintState {
   size_t poly_cap[2] = {0, 0};
   bool poly_attr = false;
   void* d_rings = nullptr;   // fresh path checks: ring starts + SpiralIterator visit order of rings 0..127 (built once)
-  void* d_memo = nullptr;    // fresh path checks: per-cell isTraversableForFilters memo of one call
+  void* d_memo = nullptr;    // fresh and polygonal path checks: per-cell isTraversableForFilters memo of one call
   size_t memo_cap = 0;
+  void* d_items = nullptr;   // polygonal path checks: one result record per pose index
+  size_t items_cap = 0;
   void invalidate() { valid = false; tables_valid = false; }
   void release();
 };
@@ -63,5 +65,16 @@ int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geo
                              const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
                              int npaths, const int* path_begin, const double* xy, const double* radius, const unsigned char* cup,
                              unsigned char* is_safe, double* trav_out, cudaStream_t s);
+
+// TraversabilityMap::checkPolygonalFootprintPath for a batch of paths sharing one footprint (te_check_footprint_paths_polygon);
+// whole map, device pointers except `footprint_xyz` (host, nfp x 3 floats).  `max_points` bounds the hull input of one item
+// (polygon1 ++ polygon2): 2 * nfp without conservative paths, 2 * nfp * (poses of the longest conservative path) otherwise.
+constexpr int kPolyMaxVerts = 16;   // footprint vertices
+constexpr int kPolyConsCap = 1024;  // vertices of a conservative path's polygon2 (nfp * poses up to the segment)
+int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                               const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                               int nfp, const float* footprint_xyz, int npaths, int nposes, const int* path_begin, const double* poses,
+                               const unsigned char* conservative, int max_points, unsigned char* is_safe, double* trav_out,
+                               double* area_out, cudaStream_t s, int* launches);
 
 }  // namespace te
