@@ -38,24 +38,7 @@ int fail(int code, const char* fmt, ...) {
     if (e__ != cudaSuccess) return fail(TE_ERR_CUDA, "%s failed: %s", #expr, cudaGetErrorString(e__)); \
   } while (0)
 
-struct DevBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  cudaError_t reserve(size_t bytes) {
-    if (bytes <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    cudaError_t e = cudaMalloc(&p, bytes);
-    if (e == cudaSuccess) cap = bytes;
-    return e;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-  }
-};
+using te::DevBuf;
 
 // grid_map::getPositionFromIndex operand order (SURVEY.md A.1).
 inline double cell_coord(double map_pos, double length, double res, int idx) {
@@ -91,7 +74,7 @@ struct te_ctx {
   DevBuf dX, dY;
   std::vector<double> hX, hY;
 
-  DevBuf stage[12];          // TE_MEM_HOST staging: 0..3 inputs, 4..11 outputs
+  DevBuf stage[12];          // TE_MEM_HOST staging (handed out in order by Staging)
   DevBuf worklist, worklist3, counter;  // fused-kernel fix-up lists (tier 2, tier 3) and their counters
   // The counters are two 512-byte blocks used alternately: the last kernel of a chain call (k_fixup_cells) zeroes the block of the
   // NEXT call, so a call needs no cudaMemsetAsync of its own (one stream operation and one launch gap less per map).
@@ -239,12 +222,144 @@ struct Guard {
   Guard guard__(ctx);                                                   \
   if (!guard__.ok) return fail(TE_ERR_CUDA, "cudaSetDevice(%d) failed", (ctx)->device)
 
-int launch_check(te_ctx* c, const char* what) {
+// Checks the launches just enqueued and counts them (te_get_stats).
+int launch_check(te_ctx* c, const char* what, int n = 1) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(TE_ERR_CUDA, "%s launch failed: %s", what, cudaGetErrorString(e));
-  ++c->launches;
+  c->launches += n;
   return TE_OK;
 }
+
+// Validates the geometry of an entry that honours a circular-buffer start index where `supported` (whole maps in host memory:
+// the staging copies unwrap and re-wrap the layers) and returns it with the start index cleared.  The kernels always see the
+// default order: positions depend on the unwrapped index only.
+int unwrap_geometry(const te_geometry* g, bool supported, te_geometry* out) {
+  if (int rc = check_geometry(g, true)) return rc;
+  if ((g->start_row != 0 || g->start_col != 0) && !supported)
+    return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0) is supported for whole maps in host memory only",
+                g->start_row, g->start_col);
+  *out = *g;
+  out->start_row = out->start_col = 0;
+  return TE_OK;
+}
+
+// The layers isTraversableForFilters reads, in the order every footprint entry reports them.
+int check_filter_layers(const te_footprint_params* p, const float* trav, const float* slope, const float* step, const float* elev,
+                        const float* rough) {
+  if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
+  if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
+  if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
+  if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
+  if (p->verify_roughness && !rough) return fail(TE_ERR_MISSING_LAYER, "layer traversability_roughness is missing (verify_roughness is set)");
+  return TE_OK;
+}
+
+// Columns [c0, c0 + n) between a device buffer in default order (column c at dev + c * rows) and a host layer.  With a start
+// index (sr, sc) != (0, 0) the host layer is a whole map of `cols` columns stored as a grid_map circular buffer: cell (i, j) of
+// the map lives at stored[((j + sc) % cols) * rows + (i + sr) % rows] (GridMap::getIndex... / convertToDefaultStartIndex,
+// SURVEY.md A.1) and moves in up to four 2-D copies.  Otherwise the host layer is in default order too: one plain copy.  This
+// is what lets the TE_MEM_HOST entries take the message / GridMap buffers of a moving (robot-centric) map as they are, without
+// an unwrapped host copy (SURVEY.md §8f-1).  upload_cols and download_cols are the only code that knows this layout.
+template <class F>
+cudaError_t for_wrapped_pieces(int rows, int cols, int sr, int sc, int c0, int n, F&& copy) {
+  for (int done = 0; done < n;) {
+    const int c = c0 + done, js = (c + sc) % cols;  // stored column of map column c
+    const int m = std::min(n - done, cols - js);     // columns until the stored index wraps
+    const size_t d = (size_t)c * rows, h = (size_t)js * rows;
+    // rows [0, rows - sr) of the map are stored rows [sr, rows); rows [rows - sr, rows) are stored rows [0, sr)
+    cudaError_t e = copy(d, h + sr, rows - sr, m);
+    if (e == cudaSuccess && sr > 0) e = copy(d + (rows - sr), h, sr, m);
+    if (e != cudaSuccess) return e;
+    done += m;
+  }
+  return cudaSuccess;
+}
+
+cudaError_t upload_cols(float* dev, const float* host, int rows, int cols, int sr, int sc, int c0, int n, cudaStream_t s) {
+  const size_t pitch = sizeof(float) * (size_t)rows;
+  if (sr == 0 && sc == 0) return cudaMemcpyAsync(dev + (size_t)c0 * rows, host + (size_t)c0 * rows, pitch * n, cudaMemcpyHostToDevice, s);
+  return for_wrapped_pieces(rows, cols, sr, sc, c0, n, [&](size_t d, size_t h, int r, int m) {
+    return cudaMemcpy2DAsync(dev + d, pitch, host + h, pitch, sizeof(float) * r, m, cudaMemcpyHostToDevice, s);
+  });
+}
+
+cudaError_t download_cols(float* host, const float* dev, int rows, int cols, int sr, int sc, int c0, int n, cudaStream_t s) {
+  const size_t pitch = sizeof(float) * (size_t)rows;
+  if (sr == 0 && sc == 0) return cudaMemcpyAsync(host + (size_t)c0 * rows, dev + (size_t)c0 * rows, pitch * n, cudaMemcpyDeviceToHost, s);
+  return for_wrapped_pieces(rows, cols, sr, sc, c0, n, [&](size_t d, size_t h, int r, int m) {
+    return cudaMemcpy2DAsync(host + h, pitch, dev + d, pitch, sizeof(float) * r, m, cudaMemcpyDeviceToHost, s);
+  });
+}
+
+// The staging of one call.  In host memory it hands out the context's staging buffers in order, uploads the inputs on the
+// context stream and records the outputs; finish() copies those back and returns once they are on the host.  In device memory
+// every pointer passes through and finish() enqueues nothing.  Host layers are `rows` x ncols in default order or, with the start
+// index of `g`, whole maps in circular-buffer order (upload_cols).  The first failure is kept in `rc`: later steps do nothing.
+struct Staging {
+  te_ctx* c;
+  bool host;
+  int rows, cols, sr, sc;
+  int rc = TE_OK;
+  int used = 0;
+  struct Out { void* host; const void* dev; size_t bytes; int ncols; };  // ncols > 0: a layer of that many columns
+  Out outs[sizeof(te_ctx::stage) / sizeof(DevBuf)];
+  int nout = 0;
+
+  Staging(te_ctx* ctx, bool host_memory, const te_geometry* g)
+      : c(ctx), host(host_memory), rows(g->rows), cols(g->cols), sr(g->start_row), sc(g->start_col) {}
+
+  void check(cudaError_t e, const char* what) {
+    if (rc == TE_OK && e != cudaSuccess) rc = fail(TE_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(e));
+  }
+  // The next staging buffer, at least `bytes` long (grow-only: once every slot has reached its largest size, nothing is allocated).
+  void* slot(size_t bytes) {
+    if (rc != TE_OK) return nullptr;
+    if (used == (int)(sizeof(outs) / sizeof(outs[0]))) {
+      rc = fail(TE_ERR_CUDA, "out of staging buffers");
+      return nullptr;
+    }
+    DevBuf& b = c->stage[used++];
+    check(b.reserve(std::max<size_t>(bytes, 1)), "staging allocation");
+    return rc == TE_OK ? b.p : nullptr;
+  }
+  size_t layer_bytes(int ncols) const { return sizeof(float) * (size_t)rows * ncols; }
+  // An input layer of `ncols` columns; null stays null.
+  const float* in_layer(const float* h, int ncols) {
+    if (!host || !h) return h;
+    float* d = (float*)slot(layer_bytes(ncols));
+    if (d) check(upload_cols(d, h, rows, cols, sr, sc, 0, ncols, c->stream), "layer upload");
+    return d;
+  }
+  // An input array of `n` elements; null stays null.
+  template <class T>
+  const T* in(const T* h, size_t n) {
+    if (!host || !h) return h;
+    T* d = (T*)slot(sizeof(T) * n);
+    if (d && n) check(cudaMemcpyAsync(d, h, sizeof(T) * n, cudaMemcpyHostToDevice, c->stream), "upload");
+    return d;
+  }
+  // An output layer of `ncols` columns / an output array of `n` elements; null stays null.
+  float* out_layer(float* h, int ncols) { return (float*)record(h, layer_bytes(ncols), ncols); }
+  template <class T>
+  T* out(T* h, size_t n) { return (T*)record(h, sizeof(T) * n, 0); }
+  void* record(void* h, size_t bytes, int ncols) {
+    if (!host || !h) return h;
+    void* d = slot(bytes);
+    if (d) outs[nout++] = Out{h, d, bytes, ncols};
+    return d;
+  }
+  int finish() {
+    if (!host || rc != TE_OK) return rc;
+    for (int k = 0; k < nout; ++k) {
+      const Out& o = outs[k];
+      check(o.ncols ? download_cols((float*)o.host, (const float*)o.dev, rows, cols, sr, sc, 0, o.ncols, c->stream)
+                    : cudaMemcpyAsync(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost, c->stream),
+            "download");
+    }
+    check(cudaStreamSynchronize(c->stream), "cudaStreamSynchronize");
+    return rc;
+  }
+};
 
 // The next triple of timing events; the pool grows on demand and is reused after te_get_timing.
 int next_timing_slot(te_ctx* c, te_ctx::Ev3** out) {
@@ -520,24 +635,13 @@ int te_slope(te_ctx* c, const te_geometry* g, double crit, const float* nz, floa
   if (crit > M_PI_2 || crit < 0.0 || std::isnan(crit)) return fail(TE_ERR_BAD_ARG, "Critical slope must be in the interval [0, PI/2]");
   if (!nz) return fail(TE_ERR_MISSING_LAYER, "layer surface_normal_z is missing");
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
-  const long long n = (long long)g->rows * g->cols;
-  const size_t bytes = sizeof(float) * (size_t)n;
-  const float* din = nz;
-  float* dout = out;
-  if (memory == TE_MEM_HOST) {
-    TE_CUDA(c->stage[0].reserve(bytes));
-    TE_CUDA(c->stage[4].reserve(bytes));
-    TE_CUDA(cudaMemcpyAsync(c->stage[0].p, nz, bytes, cudaMemcpyHostToDevice, c->stream));
-    din = (const float*)c->stage[0].p;
-    dout = (float*)c->stage[4].p;
-  }
-  te::launch_slope(n, crit, din, dout, c->sms, c->stream);
+  Staging st(c, memory == TE_MEM_HOST, g);
+  const float* din = st.in_layer(nz, g->cols);
+  float* dout = st.out_layer(out, g->cols);
+  if (st.rc) return st.rc;
+  te::launch_slope((long long)g->rows * g->cols, crit, din, dout, c->sms, c->stream);
   if (int rc = launch_check(c, "k_slope")) return rc;
-  if (memory == TE_MEM_HOST) {
-    TE_CUDA(cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, c->stream));
-    TE_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return TE_OK;
+  return st.finish();
 }
 
 int te_normals(te_ctx* c, const te_geometry* g, const te_chain_params* p, const float* elev, float* nx, float* ny, float* nz, int memory) {
@@ -547,27 +651,14 @@ int te_normals(te_ctx* c, const te_geometry* g, const te_chain_params* p, const 
   if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
   if (!nx || !ny || !nz) return fail(TE_ERR_BAD_ARG, "output layer is null");
   if (int rc = ensure_geometry(c, g)) return rc;
-  const size_t bytes = sizeof(float) * (size_t)g->rows * g->cols;
-  const float* din = elev;
-  float* o[3] = {nx, ny, nz};
-  if (memory == TE_MEM_HOST) {
-    TE_CUDA(c->stage[0].reserve(bytes));
-    TE_CUDA(cudaMemcpyAsync(c->stage[0].p, elev, bytes, cudaMemcpyHostToDevice, c->stream));
-    din = (const float*)c->stage[0].p;
-    for (int k = 0; k < 3; ++k) {
-      TE_CUDA(c->stage[4 + k].reserve(bytes));
-      o[k] = (float*)c->stage[4 + k].p;
-    }
-  }
+  Staging st(c, memory == TE_MEM_HOST, g);
+  const float* din = st.in_layer(elev, g->cols);
+  float* o[3] = {st.out_layer(nx, g->cols), st.out_layer(ny, g->cols), st.out_layer(nz, g->cols)};
+  if (st.rc) return st.rc;
   te_slab s{0, g->cols, 0, 0};
   te::launch_normals(make_view(c, g, s), make_chain_dev(g, p), din, o[0], o[1], o[2], c->sms, c->stream);
   if (int rc = launch_check(c, "k_normals")) return rc;
-  if (memory == TE_MEM_HOST) {
-    float* h[3] = {nx, ny, nz};
-    for (int k = 0; k < 3; ++k) TE_CUDA(cudaMemcpyAsync(h[k], o[k], bytes, cudaMemcpyDeviceToHost, c->stream));
-    TE_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return TE_OK;
+  return st.finish();
 }
 
 int te_step(te_ctx* c, const te_geometry* g, const te_chain_params* p, const float* elev, float* out, int memory) {
@@ -577,24 +668,14 @@ int te_step(te_ctx* c, const te_geometry* g, const te_chain_params* p, const flo
   if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
   if (int rc = ensure_geometry(c, g)) return rc;
-  const size_t bytes = sizeof(float) * (size_t)g->rows * g->cols;
-  const float* din = elev;
-  float* dout = out;
-  if (memory == TE_MEM_HOST) {
-    TE_CUDA(c->stage[0].reserve(bytes));
-    TE_CUDA(c->stage[4].reserve(bytes));
-    TE_CUDA(cudaMemcpyAsync(c->stage[0].p, elev, bytes, cudaMemcpyHostToDevice, c->stream));
-    din = (const float*)c->stage[0].p;
-    dout = (float*)c->stage[4].p;
-  }
+  Staging st(c, memory == TE_MEM_HOST, g);
+  const float* din = st.in_layer(elev, g->cols);
+  float* dout = st.out_layer(out, g->cols);
+  if (st.rc) return st.rc;
   te_slab s{0, g->cols, 0, 0};
   te::launch_step(make_view(c, g, s), make_chain_dev(g, p), din, dout, c->sms, c->stream);
   if (int rc = launch_check(c, "k_step")) return rc;
-  if (memory == TE_MEM_HOST) {
-    TE_CUDA(cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, c->stream));
-    TE_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return TE_OK;
+  return st.finish();
 }
 
 int te_roughness(te_ctx* c, const te_geometry* g, const te_chain_params* p, const float* elev, const float* nx, const float* ny,
@@ -606,73 +687,27 @@ int te_roughness(te_ctx* c, const te_geometry* g, const te_chain_params* p, cons
   if (!nx || !ny || !nz) return fail(TE_ERR_MISSING_LAYER, "layer surface_normal_{x,y,z} is missing");
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
   if (int rc = ensure_geometry(c, g)) return rc;
-  const size_t bytes = sizeof(float) * (size_t)g->rows * g->cols;
-  const float* in[4] = {elev, nx, ny, nz};
-  float* dout = out;
-  if (memory == TE_MEM_HOST) {
-    for (int k = 0; k < 4; ++k) {
-      TE_CUDA(c->stage[k].reserve(bytes));
-      TE_CUDA(cudaMemcpyAsync(c->stage[k].p, in[k], bytes, cudaMemcpyHostToDevice, c->stream));
-      in[k] = (const float*)c->stage[k].p;
-    }
-    TE_CUDA(c->stage[4].reserve(bytes));
-    dout = (float*)c->stage[4].p;
-  }
+  Staging st(c, memory == TE_MEM_HOST, g);
+  const float* in[4] = {st.in_layer(elev, g->cols), st.in_layer(nx, g->cols), st.in_layer(ny, g->cols), st.in_layer(nz, g->cols)};
+  float* dout = st.out_layer(out, g->cols);
+  if (st.rc) return st.rc;
   te_slab s{0, g->cols, 0, 0};
   te::launch_roughness(make_view(c, g, s), make_chain_dev(g, p), in[0], in[1], in[2], in[3], dout, c->sms, c->stream);
   if (int rc = launch_check(c, "k_roughness")) return rc;
-  if (memory == TE_MEM_HOST) {
-    TE_CUDA(cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, c->stream));
-    TE_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return TE_OK;
+  return st.finish();
 }
 
 // Host-memory chain on a large map: column chunks flow H2D -> kernels -> D2H on three streams so that the two PCIe
 // directions and the compute overlap (the transfers dominate: 20 B/cell over PCIe against 20 B/cell over HBM).
-// Columns [c0, c0 + n) of the map in DEFAULT order <-> a host layer stored as a grid_map circular buffer with start index
-// (sr, sc): cell (i, j) of the map lives at stored[((j + sc) % cols) * rows + (i + sr) % rows] (GridMap::getIndex... /
-// convertToDefaultStartIndex, SURVEY.md A.1).  `dev` holds map column c at dev + (c - dev_col0) * rows.  Up to four 2-D copies;
-// one plain copy when nothing wraps.  This is what lets te_chain(TE_MEM_HOST) take the message / GridMap buffers of a moving
-// (robot-centric) map as they are, without an unwrapped host copy (SURVEY.md §8f-1).
-static cudaError_t copy_wrapped(float* dev, int dev_col0, float* host, int rows, int cols, int sr, int sc, int c0, int n, bool to_device,
-                                cudaStream_t s) {
-  const size_t pitch = sizeof(float) * (size_t)rows;
-  int done = 0;
-  while (done < n) {
-    const int c = c0 + done, js = (c + sc) % cols;     // stored column of map column c
-    const int m = std::min(n - done, cols - js);       // columns until the stored index wraps
-    float* d = dev + (size_t)(c - dev_col0) * rows;
-    float* h = host + (size_t)js * rows;
-    // rows [0, rows - sr) of the map are stored rows [sr, rows); rows [rows - sr, rows) are stored rows [0, sr)
-    const int r1 = rows - sr;
-    cudaError_t e;
-    if (to_device) e = cudaMemcpy2DAsync(d, pitch, h + sr, pitch, sizeof(float) * (size_t)r1, m, cudaMemcpyHostToDevice, s);
-    else e = cudaMemcpy2DAsync(h + sr, pitch, d, pitch, sizeof(float) * (size_t)r1, m, cudaMemcpyDeviceToHost, s);
-    if (e != cudaSuccess) return e;
-    if (sr > 0) {
-      if (to_device) e = cudaMemcpy2DAsync(d + r1, pitch, h, pitch, sizeof(float) * (size_t)sr, m, cudaMemcpyHostToDevice, s);
-      else e = cudaMemcpy2DAsync(h, pitch, d + r1, pitch, sizeof(float) * (size_t)sr, m, cudaMemcpyDeviceToHost, s);
-      if (e != cudaSuccess) return e;
-    }
-    done += m;
-  }
-  return cudaSuccess;
-}
-
-static int chain_host_pipelined(te_ctx* c, const te_geometry* g, const te_slab& s, const te_chain_params* p, const float* elev,
-                                float* const host_out[7], int sr = 0, int sc = 0) {
+static int chain_host_pipelined(te_ctx* c, Staging& st, const te_geometry* g, const te_slab& s, const te_chain_params* p, const float* elev,
+                                float* const host_out[7]) {
   const int rows = g->rows, need = chain_halo(g, p);
-  const bool wrapped = sr != 0 || sc != 0;  // only with the whole map (no slab): buffer column == map column
   const int in_cols = s.halo_left + s.col_count + s.halo_right;
-  const size_t col_bytes = sizeof(float) * (size_t)rows;
-  TE_CUDA(c->stage[0].reserve(col_bytes * in_cols));
+  float* const din = (float*)st.slot(st.layer_bytes(in_cols));
   float* dev_out[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   for (int k = 0; k < 7; ++k)
-    if (host_out[k]) {
-      TE_CUDA(c->stage[4 + k].reserve(col_bytes * s.col_count));
-      dev_out[k] = (float*)c->stage[4 + k].p;
-    }
+    if (host_out[k]) dev_out[k] = (float*)st.slot(st.layer_bytes(s.col_count));
+  if (st.rc) return st.rc;
   if (!c->s_h2d) TE_CUDA(cudaStreamCreateWithFlags(&c->s_h2d, cudaStreamNonBlocking));
   if (!c->s_d2h) TE_CUDA(cudaStreamCreateWithFlags(&c->s_d2h, cudaStreamNonBlocking));
   const int nchunk = std::min(16, std::max(2, s.col_count / 512));
@@ -703,7 +738,6 @@ static int chain_host_pipelined(te_ctx* c, const te_geometry* g, const te_slab& 
   TE_CUDA(cudaEventRecord(start, c->stream));  // order after whatever the caller queued on the context stream
   TE_CUDA(cudaStreamWaitEvent(c->s_h2d, start, 0));
   TE_CUDA(cudaStreamWaitEvent(c->s_d2h, start, 0));
-  const float* din = (const float*)c->stage[0].p;
   te::SlabView v = make_view(c, g, s);
   int uploaded = 0;  // input-buffer columns already queued for upload
   int rc = TE_OK;
@@ -713,10 +747,7 @@ static int chain_host_pipelined(te_ctx* c, const te_geometry* g, const te_slab& 
     // chunk k reads input-buffer columns [halo_left + off - need, halo_left + off + cnt + need)
     const int upto = std::min(in_cols, s.halo_left + off + cnt + need);
     if (upto > uploaded) {
-      cudaError_t e = wrapped ? copy_wrapped((float*)c->stage[0].p, 0, const_cast<float*>(elev), rows, g->cols, sr, sc, uploaded,
-                                             upto - uploaded, true, c->s_h2d)
-                              : cudaMemcpyAsync((char*)c->stage[0].p + col_bytes * uploaded, (const char*)elev + col_bytes * uploaded,
-                                                col_bytes * (upto - uploaded), cudaMemcpyHostToDevice, c->s_h2d);
+      cudaError_t e = upload_cols(din, elev, rows, st.cols, st.sr, st.sc, uploaded, upto - uploaded, c->s_h2d);
       if (e != cudaSuccess) { rc = fail(TE_ERR_CUDA, "H2D chunk copy failed: %s", cudaGetErrorString(e)); break; }
       uploaded = upto;
     }
@@ -734,9 +765,7 @@ static int chain_host_pipelined(te_ctx* c, const te_geometry* g, const te_slab& 
     cudaStreamWaitEvent(c->s_d2h, done[k], 0);
     for (int l = 0; l < 7; ++l)
       if (host_out[l]) {
-        cudaError_t e = wrapped ? copy_wrapped(dev_out[l], 0, host_out[l], rows, g->cols, sr, sc, off, cnt, false, c->s_d2h)
-                                : cudaMemcpyAsync(host_out[l] + (size_t)off * rows, dev_out[l] + (size_t)off * rows, col_bytes * cnt,
-                                                  cudaMemcpyDeviceToHost, c->s_d2h);
+        cudaError_t e = download_cols(host_out[l], dev_out[l], rows, st.cols, st.sr, st.sc, off, cnt, c->s_d2h);
         if (e != cudaSuccess) { rc = fail(TE_ERR_CUDA, "D2H chunk copy failed: %s", cudaGetErrorString(e)); break; }
       }
   }
@@ -749,15 +778,8 @@ static int chain_host_pipelined(te_ctx* c, const te_geometry* g, const te_slab& 
 
 static int chain_common(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const te_chain_params* p, int nmaps, const float* elev,
                         float* slope, float* step, float* rough, float* trav, float* nx, float* ny, float* nz, int memory) {
-  if (int rc = check_geometry(g_in, true)) return rc;
-  // A circular-buffer start index is honoured for whole host maps: the copies to and from the device unwrap / re-wrap the
-  // layers, the kernels always see the default order (positions depend on the unwrapped index only).
-  const int sr = g_in->start_row, sc = g_in->start_col;
-  const bool wrapped = sr != 0 || sc != 0;
-  if (wrapped && (memory != TE_MEM_HOST || slab != nullptr || nmaps != 1))
-    return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0) is supported for whole maps in host memory only", sr, sc);
-  te_geometry g0 = *g_in;
-  g0.start_row = g0.start_col = 0;
+  te_geometry g0;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && slab == nullptr && nmaps == 1, &g0)) return rc;
   const te_geometry* g = &g0;
   if (int rc = check_params(p)) return rc;
   if (nmaps <= 0) return fail(TE_ERR_BAD_ARG, "number of maps must be positive");
@@ -766,36 +788,16 @@ static int chain_common(te_ctx* c, const te_geometry* g_in, const te_slab* slab,
   te_slab s;
   if (int rc = resolve_slab(g, slab, chain_halo(g, p), &s)) return rc;
   if (int rc = ensure_geometry(c, g)) return rc;
-  const size_t in_bytes = sizeof(float) * (size_t)g->rows * (s.halo_left + s.col_count + s.halo_right) * nmaps;
-  const size_t out_bytes = sizeof(float) * (size_t)g->rows * s.col_count * nmaps;
-  te::ChainOut o{slope, step, rough, trav, nx, ny, nz};
-  const float* din = elev;
+  Staging st(c, memory == TE_MEM_HOST, g_in);
   float* host_out[7] = {slope, step, rough, trav, nx, ny, nz};
   if (memory == TE_MEM_HOST && nmaps == 1 && s.col_count >= 1024 && (size_t)g->rows * s.col_count >= ((size_t)1 << 22))
-    return chain_host_pipelined(c, g, s, p, elev, host_out, sr, sc);
-  if (memory == TE_MEM_HOST) {
-    TE_CUDA(c->stage[0].reserve(in_bytes));
-    if (wrapped) TE_CUDA(copy_wrapped((float*)c->stage[0].p, 0, const_cast<float*>(elev), g->rows, g->cols, sr, sc, 0, g->cols, true, c->stream));
-    else TE_CUDA(cudaMemcpyAsync(c->stage[0].p, elev, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    din = (const float*)c->stage[0].p;
-    float** dev_out[7] = {&o.slope, &o.step, &o.rough, &o.trav, &o.nx, &o.ny, &o.nz};
-    for (int k = 0; k < 7; ++k) {
-      if (!host_out[k]) continue;
-      TE_CUDA(c->stage[4 + k].reserve(out_bytes));
-      *dev_out[k] = (float*)c->stage[4 + k].p;
-    }
-  }
-  if (int rc = run_chain_device(c, g, make_view(c, g, s), p, din, o, nmaps)) return rc;
-  if (memory == TE_MEM_HOST) {
-    float* dev_out[7] = {o.slope, o.step, o.rough, o.trav, o.nx, o.ny, o.nz};
-    for (int k = 0; k < 7; ++k)
-      if (host_out[k]) {
-        if (wrapped) TE_CUDA(copy_wrapped(dev_out[k], 0, host_out[k], g->rows, g->cols, sr, sc, 0, g->cols, false, c->stream));
-        else TE_CUDA(cudaMemcpyAsync(host_out[k], dev_out[k], out_bytes, cudaMemcpyDeviceToHost, c->stream));
-      }
-    TE_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return TE_OK;
+    return chain_host_pipelined(c, st, g, s, p, elev, host_out);
+  const float* din = st.in_layer(elev, (s.halo_left + s.col_count + s.halo_right) * nmaps);
+  float* o[7];
+  for (int k = 0; k < 7; ++k) o[k] = st.out_layer(host_out[k], s.col_count * nmaps);
+  if (st.rc) return st.rc;
+  if (int rc = run_chain_device(c, g, make_view(c, g, s), p, din, te::ChainOut{o[0], o[1], o[2], o[3], o[4], o[5], o[6]}, nmaps)) return rc;
+  return st.finish();
 }
 
 int te_chain(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_chain_params* p, const float* elev, float* slope,
@@ -814,130 +816,62 @@ int te_footprint2(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const
                   const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
                   float* step_fp, float* rough_fp, int memory) {
   TE_ENTER(c);
-  if (int rc = check_geometry(g_in, true)) return rc;
-  const int sr = g_in->start_row, sc = g_in->start_col;  // circular-buffer maps: whole host maps only, like te_chain
-  const bool wrapped = sr != 0 || sc != 0;
-  if (wrapped && (memory != TE_MEM_HOST || slab != nullptr))
-    return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0) is supported for whole maps in host memory only", sr, sc);
-  te_geometry g0 = *g_in;
-  g0.start_row = g0.start_col = 0;
+  te_geometry g0;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && slab == nullptr, &g0)) return rc;
   const te_geometry* g = &g0;
   if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
   if (!(p->radius >= 0.0) || !(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint radius/offset must be >= 0");
-  if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
-  if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
-  if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
-  if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
-  if (p->verify_roughness && !rough) return fail(TE_ERR_MISSING_LAYER, "layer traversability_roughness is missing (verify_roughness is set)");
+  if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
   const bool use_rough = p->verify_roughness != 0;
   te_slab s;
-  const int need = te::footprint_halo(g, p);
-  if (int rc = resolve_slab(g, slab, need, &s)) return rc;
+  if (int rc = resolve_slab(g, slab, te::footprint_halo(g, p), &s)) return rc;
   if (int rc = ensure_geometry(c, g)) return rc;
-  const size_t in_bytes = sizeof(float) * (size_t)g->rows * (s.halo_left + s.col_count + s.halo_right);
-  const size_t out_bytes = sizeof(float) * (size_t)g->rows * s.col_count;
-  const float* in[5] = {trav, slope, step, elev, use_rough ? rough : nullptr};
-  float* o[4] = {out, slope_fp, step_fp, use_rough ? rough_fp : nullptr};
-  float* host_o[4] = {out, slope_fp, step_fp, use_rough ? rough_fp : nullptr};
-  if (memory == TE_MEM_HOST) {
-    // staging: inputs 0..3 (+ roughness in slot 11), outputs 4..7
-    const int slot_in[5] = {0, 1, 2, 3, 11};
-    for (int k = 0; k < 5; ++k) {
-      if (!in[k]) continue;
-      TE_CUDA(c->stage[slot_in[k]].reserve(in_bytes));
-      if (wrapped) TE_CUDA(copy_wrapped((float*)c->stage[slot_in[k]].p, 0, const_cast<float*>(in[k]), g->rows, g->cols, sr, sc, 0, g->cols, true, c->stream));
-      else TE_CUDA(cudaMemcpyAsync(c->stage[slot_in[k]].p, in[k], in_bytes, cudaMemcpyHostToDevice, c->stream));
-      in[k] = (const float*)c->stage[slot_in[k]].p;
-    }
-    for (int k = 0; k < 4; ++k) {
-      if (!host_o[k]) continue;
-      TE_CUDA(c->stage[4 + k].reserve(out_bytes));
-      o[k] = (float*)c->stage[4 + k].p;
-    }
-  }
-  const te::SlabView v = make_view(c, g, s);
+  Staging st(c, memory == TE_MEM_HOST, g_in);
+  const int in_cols = s.halo_left + s.col_count + s.halo_right;
+  const float* in[5] = {st.in_layer(trav, in_cols), st.in_layer(slope, in_cols), st.in_layer(step, in_cols), st.in_layer(elev, in_cols),
+                        st.in_layer(use_rough ? rough : nullptr, in_cols)};
+  float* o[4] = {st.out_layer(out, s.col_count), st.out_layer(slope_fp, s.col_count), st.out_layer(step_fp, s.col_count),
+                 st.out_layer(use_rough ? rough_fp : nullptr, s.col_count)};
+  if (st.rc) return st.rc;
   int nl = 0;
-  int rc = te::launch_footprint(c->fp, v, g, p, c->hX, c->hY, in[0], in[1], in[2], in[4], in[3], o[0], o[1], o[2], o[3], c->sms,
+  int rc = te::launch_footprint(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], o[0], o[1], o[2], o[3], c->sms,
                                 c->stream, &nl);
   if (rc != 0) return fail(rc, "footprint sweep failed: %s", c->fp.why.c_str());
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(TE_ERR_CUDA, "footprint launch failed: %s", cudaGetErrorString(e));
-  c->launches += nl;
-  if (memory == TE_MEM_HOST) {
-    for (int k = 0; k < 4; ++k)
-      if (host_o[k]) {
-        if (wrapped) TE_CUDA(copy_wrapped(o[k], 0, host_o[k], g->rows, g->cols, sr, sc, 0, g->cols, false, c->stream));
-        else TE_CUDA(cudaMemcpyAsync(host_o[k], o[k], out_bytes, cudaMemcpyDeviceToHost, c->stream));
-      }
-    TE_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return TE_OK;
+  if (int r2 = launch_check(c, "footprint", nl)) return r2;
+  return st.finish();
 }
 
-int te_footprint_polygon(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, int32_t npts,
+int te_footprint_polygon(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const te_footprint_params* p, int32_t npts,
                          const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step, const float* rough,
                          const float* elev, float* out_x, float* out_rot, int memory) {
   TE_ENTER(c);
-  if (int rc = check_geometry(g, true)) return rc;
-  const int sr = g->start_row, sc = g->start_col;  // circular-buffer maps: whole host maps only, like te_chain
-  const bool wrapped = sr != 0 || sc != 0;
-  if (wrapped && (memory != TE_MEM_HOST || slab != nullptr))
-    return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0) is supported for whole maps in host memory only", sr, sc);
-  te_geometry g0 = *g;
-  g0.start_row = g0.start_col = 0;
-  g = &g0;
+  te_geometry g0;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && slab == nullptr, &g0)) return rc;
+  const te_geometry* g = &g0;
   if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
   if (npts < 3 || npts > 16 || !pts_xy) return fail(TE_ERR_BAD_ARG, "footprint polygon needs 3 to 16 vertices");
   if (!std::isfinite(yaw)) return fail(TE_ERR_BAD_ARG, "footprint yaw is not finite");
   for (int k = 0; k < 2 * npts; ++k)
     if (!std::isfinite(pts_xy[k])) return fail(TE_ERR_BAD_ARG, "footprint polygon vertex is not finite");
-  if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
-  if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
-  if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
-  if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
-  if (p->verify_roughness && !rough) return fail(TE_ERR_MISSING_LAYER, "layer traversability_roughness is missing (verify_roughness is set)");
+  if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
   if (!out_x || !out_rot) return fail(TE_ERR_BAD_ARG, "output layer is null");
   const bool use_rough = p->verify_roughness != 0;
   te_slab s;
   if (int rc = resolve_slab(g, slab, te::footprint_polygon_halo(g, p, npts, pts_xy), &s)) return rc;
   if (int rc = ensure_geometry(c, g)) return rc;
-  const size_t in_bytes = sizeof(float) * (size_t)g->rows * (s.halo_left + s.col_count + s.halo_right);
-  const size_t out_bytes = sizeof(float) * (size_t)g->rows * s.col_count;
-  const float* in[5] = {trav, slope, step, elev, use_rough ? rough : nullptr};
-  float* o[2] = {out_x, out_rot};
-  if (memory == TE_MEM_HOST) {
-    const int slot_in[5] = {0, 1, 2, 3, 11};
-    for (int k = 0; k < 5; ++k) {
-      if (!in[k]) continue;
-      TE_CUDA(c->stage[slot_in[k]].reserve(in_bytes));
-      if (wrapped) TE_CUDA(copy_wrapped((float*)c->stage[slot_in[k]].p, 0, const_cast<float*>(in[k]), g->rows, g->cols, sr, sc, 0, g->cols, true, c->stream));
-      else TE_CUDA(cudaMemcpyAsync(c->stage[slot_in[k]].p, in[k], in_bytes, cudaMemcpyHostToDevice, c->stream));
-      in[k] = (const float*)c->stage[slot_in[k]].p;
-    }
-    for (int k = 0; k < 2; ++k) {
-      TE_CUDA(c->stage[4 + k].reserve(out_bytes));
-      o[k] = (float*)c->stage[4 + k].p;
-    }
-  }
-  const te::SlabView v = make_view(c, g, s);
+  Staging st(c, memory == TE_MEM_HOST, g_in);
+  const int in_cols = s.halo_left + s.col_count + s.halo_right;
+  const float* in[5] = {st.in_layer(trav, in_cols), st.in_layer(slope, in_cols), st.in_layer(step, in_cols), st.in_layer(elev, in_cols),
+                        st.in_layer(use_rough ? rough : nullptr, in_cols)};
+  float* o[2] = {st.out_layer(out_x, s.col_count), st.out_layer(out_rot, s.col_count)};
+  if (st.rc) return st.rc;
   int nl = 0;
-  int rc = te::launch_footprint_polygon(c->fp, v, g, p, npts, pts_xy, yaw, in[0], in[1], in[2], in[4], in[3], o[0], o[1], c->sms, c->stream, &nl);
+  int rc = te::launch_footprint_polygon(c->fp, make_view(c, g, s), g, p, npts, pts_xy, yaw, in[0], in[1], in[2], in[4], in[3], o[0], o[1],
+                                        c->sms, c->stream, &nl);
   if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", c->fp.why.c_str());
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(TE_ERR_CUDA, "polygon footprint launch failed: %s", cudaGetErrorString(e));
-  c->launches += nl;
-  if (memory == TE_MEM_HOST) {
-    if (wrapped) {
-      TE_CUDA(copy_wrapped(o[0], 0, out_x, g->rows, g->cols, sr, sc, 0, g->cols, false, c->stream));
-      TE_CUDA(copy_wrapped(o[1], 0, out_rot, g->rows, g->cols, sr, sc, 0, g->cols, false, c->stream));
-    } else {
-      TE_CUDA(cudaMemcpyAsync(out_x, o[0], out_bytes, cudaMemcpyDeviceToHost, c->stream));
-      TE_CUDA(cudaMemcpyAsync(out_rot, o[1], out_bytes, cudaMemcpyDeviceToHost, c->stream));
-    }
-    TE_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return TE_OK;
+  if (int r2 = launch_check(c, "polygon footprint", nl)) return r2;
+  return st.finish();
 }
 
 int te_footprint(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, const float* trav,
@@ -960,35 +894,24 @@ int te_check_footprint_paths2(te_ctx* c, const te_geometry* g, const float* foot
   if (npaths < 0 || !path_begin || !poses_xy || !is_safe || !traversability) return fail(TE_ERR_BAD_ARG, "null argument or negative path count");
   if (npaths == 0) return TE_OK;
   if (int rc = ensure_geometry(c, g)) return rc;
+  const bool host = memory != TE_MEM_DEVICE;
+  int32_t nposes = 0;
+  if (host) {  // path_begin is readable here, so the pose count is known
+    nposes = path_begin[npaths];
+    if (nposes < 0) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
+  }
+  Staging st(c, host, g);
+  const float* dfp = st.in_layer(footprint, g->cols);
+  const float* drs = st.in_layer(robot_slope, g->cols);
+  const int32_t* dpb = st.in(path_begin, (size_t)npaths + 1);
+  const double* dxy = st.in(poses_xy, 2 * (size_t)nposes);
+  uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
+  double* dtrav = st.out(traversability, (size_t)npaths);
+  if (st.rc) return st.rc;
   const te_slab s{0, g->cols, 0, 0};
-  const te::SlabView v = make_view(c, g, s);
-  if (memory == TE_MEM_DEVICE) {
-    te::launch_check_paths(v, g, traversability_default, footprint, robot_slope, npaths, path_begin, poses_xy, is_safe, traversability, c->stream);
-    return launch_check(c, "k_check_paths");
-  }
-  // host arguments: path_begin is readable here, so the pose count is known
-  const int32_t nposes = path_begin[npaths];
-  if (nposes < 0) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
-  const size_t lbytes = sizeof(float) * (size_t)g->rows * g->cols;
-  TE_CUDA(c->stage[0].reserve(lbytes));
-  TE_CUDA(c->stage[1].reserve(sizeof(int32_t) * (size_t)(npaths + 1)));
-  TE_CUDA(c->stage[2].reserve(sizeof(double) * 2 * (size_t)std::max(nposes, 1)));
-  TE_CUDA(c->stage[4].reserve((size_t)npaths));
-  TE_CUDA(c->stage[5].reserve(sizeof(double) * (size_t)npaths));
-  TE_CUDA(cudaMemcpyAsync(c->stage[0].p, footprint, lbytes, cudaMemcpyHostToDevice, c->stream));
-  if (robot_slope) {
-    TE_CUDA(c->stage[3].reserve(lbytes));
-    TE_CUDA(cudaMemcpyAsync(c->stage[3].p, robot_slope, lbytes, cudaMemcpyHostToDevice, c->stream));
-  }
-  TE_CUDA(cudaMemcpyAsync(c->stage[1].p, path_begin, sizeof(int32_t) * (size_t)(npaths + 1), cudaMemcpyHostToDevice, c->stream));
-  TE_CUDA(cudaMemcpyAsync(c->stage[2].p, poses_xy, sizeof(double) * 2 * (size_t)nposes, cudaMemcpyHostToDevice, c->stream));
-  te::launch_check_paths(v, g, traversability_default, (const float*)c->stage[0].p, robot_slope ? (const float*)c->stage[3].p : nullptr, npaths, (const int*)c->stage[1].p,
-                         (const double*)c->stage[2].p, (unsigned char*)c->stage[4].p, (double*)c->stage[5].p, c->stream);
+  te::launch_check_paths(make_view(c, g, s), g, traversability_default, dfp, drs, npaths, dpb, dxy, dsafe, dtrav, c->stream);
   if (int rc = launch_check(c, "k_check_paths")) return rc;
-  TE_CUDA(cudaMemcpyAsync(is_safe, c->stage[4].p, (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
-  TE_CUDA(cudaMemcpyAsync(traversability, c->stage[5].p, sizeof(double) * (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
-  TE_CUDA(cudaStreamSynchronize(c->stream));
-  return TE_OK;
+  return st.finish();
 }
 
 int te_check_footprint_paths_fresh(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
@@ -996,75 +919,45 @@ int te_check_footprint_paths_fresh(te_ctx* c, const te_geometry* g_in, const te_
                                    const int32_t* path_begin, const double* poses_xy, const double* radius, const uint8_t* cup,
                                    uint8_t* is_safe, double* traversability, int memory) {
   TE_ENTER(c);
-  if (int rc = check_geometry(g_in, true)) return rc;
-  const int sr = g_in->start_row, sc = g_in->start_col;  // circular-buffer maps: host memory only, like te_footprint2
-  const bool wrapped = sr != 0 || sc != 0;
-  if (wrapped && memory == TE_MEM_DEVICE)
-    return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0) is supported for maps in host memory only", sr, sc);
-  te_geometry g0 = *g_in;
-  g0.start_row = g0.start_col = 0;
+  te_geometry g0;
+  if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
   const te_geometry* g = &g0;
   if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
   if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
-  if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
-  if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
-  if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
-  if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
-  if (p->verify_roughness && !rough) return fail(TE_ERR_MISSING_LAYER, "layer traversability_roughness is missing (verify_roughness is set)");
+  if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
   if (npaths < 0 || !path_begin || !poses_xy || !radius || !is_safe || !traversability) return fail(TE_ERR_BAD_ARG, "null argument or negative path count");
   if (npaths == 0) return TE_OK;
   const bool use_rough = p->verify_roughness != 0;
   if (int rc = ensure_geometry(c, g)) return rc;
+  // Device memory reads nothing back: a path whose radius cannot be checked gets is_safe 0, traversability NaN.
+  const bool host = memory != TE_MEM_DEVICE;
+  int32_t nposes = 0;
+  if (host) {
+    if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
+    for (int32_t q = 0; q < npaths; ++q) {
+      if (path_begin[q + 1] < path_begin[q]) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
+      if (!(radius[q] >= 0.0)) return fail(TE_ERR_BAD_ARG, "radius of path %d is negative or NaN", q);
+      if (!(std::ceil((radius[q] + p->offset) / g->resolution) <= 127.0))
+        return fail(TE_ERR_UNSUPPORTED, "radius of path %d + offset spans more than 127 cells", q);
+    }
+    nposes = path_begin[npaths];
+  }
+  Staging st(c, host, g_in);
+  const float* in[6] = {st.in_layer(trav, g->cols), st.in_layer(slope, g->cols), st.in_layer(step, g->cols), st.in_layer(elev, g->cols),
+                        st.in_layer(use_rough ? rough : nullptr, g->cols), st.in_layer(robot_slope, g->cols)};
+  const int32_t* dpb = st.in(path_begin, (size_t)npaths + 1);
+  const double* dxy = st.in(poses_xy, 2 * (size_t)nposes);
+  const double* drad = st.in(radius, (size_t)npaths);
+  const uint8_t* dcup = st.in(cup, (size_t)npaths);
+  uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
+  double* dtrav = st.out(traversability, (size_t)npaths);
+  if (st.rc) return st.rc;
   const te_slab s{0, g->cols, 0, 0};
-  const te::SlabView v = make_view(c, g, s);
-  if (memory == TE_MEM_DEVICE) {  // nothing is read back: a path whose radius cannot be checked gets is_safe 0, traversability NaN
-    int rc = te::launch_check_paths_fresh(c->fp, v, g, p, trav, slope, step, use_rough ? rough : nullptr, elev, robot_slope, npaths,
-                                          path_begin, poses_xy, radius, cup, is_safe, traversability, c->stream);
-    if (rc != 0) return fail(rc, "fresh path check failed: %s", c->fp.why.c_str());
-    return launch_check(c, "k_check_paths_fresh");
-  }
-  if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
-  for (int32_t q = 0; q < npaths; ++q) {
-    if (path_begin[q + 1] < path_begin[q]) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
-    if (!(radius[q] >= 0.0)) return fail(TE_ERR_BAD_ARG, "radius of path %d is negative or NaN", q);
-    if (!(std::ceil((radius[q] + p->offset) / g->resolution) <= 127.0))
-      return fail(TE_ERR_UNSUPPORTED, "radius of path %d + offset spans more than 127 cells", q);
-  }
-  const int32_t nposes = path_begin[npaths];
-  const size_t lbytes = sizeof(float) * (size_t)g->rows * g->cols;
-  // staging: layers 0..3 (+ roughness 11, robot_slope 4), paths 5..8, results 9..10
-  const float* in[6] = {trav, slope, step, elev, use_rough ? rough : nullptr, robot_slope};
-  const int slot_in[6] = {0, 1, 2, 3, 11, 4};
-  for (int k = 0; k < 6; ++k) {
-    if (!in[k]) continue;
-    TE_CUDA(c->stage[slot_in[k]].reserve(lbytes));
-    if (wrapped) TE_CUDA(copy_wrapped((float*)c->stage[slot_in[k]].p, 0, const_cast<float*>(in[k]), g->rows, g->cols, sr, sc, 0, g->cols, true, c->stream));
-    else TE_CUDA(cudaMemcpyAsync(c->stage[slot_in[k]].p, in[k], lbytes, cudaMemcpyHostToDevice, c->stream));
-    in[k] = (const float*)c->stage[slot_in[k]].p;
-  }
-  TE_CUDA(c->stage[5].reserve(sizeof(int32_t) * (size_t)(npaths + 1)));
-  TE_CUDA(c->stage[6].reserve(sizeof(double) * 2 * (size_t)std::max(nposes, 1)));
-  TE_CUDA(c->stage[7].reserve(sizeof(double) * (size_t)npaths));
-  TE_CUDA(c->stage[9].reserve((size_t)npaths));
-  TE_CUDA(c->stage[10].reserve(sizeof(double) * (size_t)npaths));
-  TE_CUDA(cudaMemcpyAsync(c->stage[5].p, path_begin, sizeof(int32_t) * (size_t)(npaths + 1), cudaMemcpyHostToDevice, c->stream));
-  if (nposes > 0) TE_CUDA(cudaMemcpyAsync(c->stage[6].p, poses_xy, sizeof(double) * 2 * (size_t)nposes, cudaMemcpyHostToDevice, c->stream));
-  TE_CUDA(cudaMemcpyAsync(c->stage[7].p, radius, sizeof(double) * (size_t)npaths, cudaMemcpyHostToDevice, c->stream));
-  const unsigned char* dcup = nullptr;
-  if (cup) {
-    TE_CUDA(c->stage[8].reserve((size_t)npaths));
-    TE_CUDA(cudaMemcpyAsync(c->stage[8].p, cup, (size_t)npaths, cudaMemcpyHostToDevice, c->stream));
-    dcup = (const unsigned char*)c->stage[8].p;
-  }
-  int rc = te::launch_check_paths_fresh(c->fp, v, g, p, in[0], in[1], in[2], in[4], in[3], in[5], npaths, (const int*)c->stage[5].p,
-                                        (const double*)c->stage[6].p, (const double*)c->stage[7].p, dcup, (unsigned char*)c->stage[9].p,
-                                        (double*)c->stage[10].p, c->stream);
+  int rc = te::launch_check_paths_fresh(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], in[5], npaths, dpb, dxy, drad,
+                                        dcup, dsafe, dtrav, c->stream);
   if (rc != 0) return fail(rc, "fresh path check failed: %s", c->fp.why.c_str());
-  if (int rc2 = launch_check(c, "k_check_paths_fresh")) return rc2;
-  TE_CUDA(cudaMemcpyAsync(is_safe, c->stage[9].p, (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
-  TE_CUDA(cudaMemcpyAsync(traversability, c->stage[10].p, sizeof(double) * (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
-  TE_CUDA(cudaStreamSynchronize(c->stream));
-  return TE_OK;
+  if (int r2 = launch_check(c, "k_check_paths_fresh")) return r2;
+  return st.finish();
 }
 
 int te_check_footprint_paths_polygon(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
@@ -1073,20 +966,11 @@ int te_check_footprint_paths_polygon(te_ctx* c, const te_geometry* g_in, const t
                                      const double* poses, const uint8_t* conservative, uint8_t* is_safe, double* traversability,
                                      double* area, int memory) {
   TE_ENTER(c);
-  if (int rc = check_geometry(g_in, true)) return rc;
-  const int sr = g_in->start_row, sc = g_in->start_col;  // circular-buffer maps: host memory only, like te_footprint2
-  const bool wrapped = sr != 0 || sc != 0;
-  if (wrapped && memory == TE_MEM_DEVICE)
-    return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0) is supported for maps in host memory only", sr, sc);
-  te_geometry g0 = *g_in;
-  g0.start_row = g0.start_col = 0;
+  te_geometry g0;
+  if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
   const te_geometry* g = &g0;
   if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
-  if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
-  if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
-  if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
-  if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
-  if (p->verify_roughness && !rough) return fail(TE_ERR_MISSING_LAYER, "layer traversability_roughness is missing (verify_roughness is set)");
+  if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
   if (npaths < 0 || nposes < 0 || !path_begin || !poses || !footprint_xyz || !is_safe || !traversability || !area)
     return fail(TE_ERR_BAD_ARG, "null argument or negative count");
   if (nfootprint < 1 || nfootprint > te::kPolyMaxVerts) return fail(TE_ERR_BAD_ARG, "footprint needs 1..%d vertices, got %d", te::kPolyMaxVerts, nfootprint);
@@ -1095,71 +979,43 @@ int te_check_footprint_paths_polygon(te_ctx* c, const te_geometry* g_in, const t
   if (npaths == 0) return TE_OK;
   const bool use_rough = p->verify_roughness != 0;
   if (int rc = ensure_geometry(c, g)) return rc;
-  const te_slab s{0, g->cols, 0, 0};
-  const te::SlabView v = make_view(c, g, s);
-  int nl = 0;
-  if (memory == TE_MEM_DEVICE) {  // nothing is read back: a path that cannot be checked gets is_safe 0, traversability and area NaN
-    const int mp = conservative ? 2 * te::kPolyConsCap : 2 * nfootprint;
-    int rc = te::launch_check_paths_polygon(c->fp, v, g, p, trav, slope, step, use_rough ? rough : nullptr, elev, robot_slope, nfootprint,
-                                            footprint_xyz, npaths, nposes, path_begin, poses, conservative, mp, is_safe, traversability,
-                                            area, c->stream, &nl);
-    if (rc != 0) return fail(rc, "polygonal path check failed: %s", c->fp.why.c_str());
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(TE_ERR_CUDA, "polygonal path check launch failed: %s", cudaGetErrorString(e));
-    c->launches += nl;
-    return TE_OK;
-  }
-  if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
-  if (path_begin[npaths] != nposes) return fail(TE_ERR_BAD_ARG, "path_begin[npaths] = %d != nposes = %d", path_begin[npaths], nposes);
-  int mp = 2 * nfootprint;
-  for (int32_t q = 0; q < npaths; ++q) {
-    const int32_t n = path_begin[q + 1] - path_begin[q];
-    if (n < 0) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
-    if (conservative && conservative[q] && n > 1) {
-      if ((long long)nfootprint * n > te::kPolyConsCap)
-        return fail(TE_ERR_UNSUPPORTED, "conservative path %d needs %lld polygon vertices, more than %d", q, (long long)nfootprint * n,
-                    te::kPolyConsCap);
-      mp = std::max(mp, 2 * nfootprint * n);
+  // Device memory reads nothing back: a path that cannot be checked gets is_safe 0, traversability and area NaN.
+  const bool host = memory != TE_MEM_DEVICE;
+  int mp = conservative ? 2 * te::kPolyConsCap : 2 * nfootprint;  // hull input bound of one item; host memory sizes it from the paths
+  if (host) {
+    if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
+    if (path_begin[npaths] != nposes) return fail(TE_ERR_BAD_ARG, "path_begin[npaths] = %d != nposes = %d", path_begin[npaths], nposes);
+    mp = 2 * nfootprint;
+    for (int32_t q = 0; q < npaths; ++q) {
+      const int32_t n = path_begin[q + 1] - path_begin[q];
+      if (n < 0) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
+      if (conservative && conservative[q] && n > 1) {
+        if ((long long)nfootprint * n > te::kPolyConsCap)
+          return fail(TE_ERR_UNSUPPORTED, "conservative path %d needs %lld polygon vertices, more than %d", q, (long long)nfootprint * n,
+                      te::kPolyConsCap);
+        mp = std::max(mp, 2 * nfootprint * n);
+      }
     }
+    for (size_t k = 0; k < 7 * (size_t)nposes; ++k)
+      if (!std::isfinite(poses[k])) return fail(TE_ERR_BAD_ARG, "pose %zu is not finite", k / 7);
   }
-  for (size_t k = 0; k < 7 * (size_t)nposes; ++k)
-    if (!std::isfinite(poses[k])) return fail(TE_ERR_BAD_ARG, "pose %zu is not finite", k / 7);
-  const size_t lbytes = sizeof(float) * (size_t)g->rows * g->cols;
-  // staging: layers 0..3 (+ roughness 11, robot_slope 4), paths 5, 6, 8, results 9, 10, 7
-  const float* in[6] = {trav, slope, step, elev, use_rough ? rough : nullptr, robot_slope};
-  const int slot_in[6] = {0, 1, 2, 3, 11, 4};
-  for (int k = 0; k < 6; ++k) {
-    if (!in[k]) continue;
-    TE_CUDA(c->stage[slot_in[k]].reserve(lbytes));
-    if (wrapped) TE_CUDA(copy_wrapped((float*)c->stage[slot_in[k]].p, 0, const_cast<float*>(in[k]), g->rows, g->cols, sr, sc, 0, g->cols, true, c->stream));
-    else TE_CUDA(cudaMemcpyAsync(c->stage[slot_in[k]].p, in[k], lbytes, cudaMemcpyHostToDevice, c->stream));
-    in[k] = (const float*)c->stage[slot_in[k]].p;
-  }
-  TE_CUDA(c->stage[5].reserve(sizeof(int32_t) * (size_t)(npaths + 1)));
-  TE_CUDA(c->stage[6].reserve(sizeof(double) * 7 * (size_t)std::max(nposes, 1)));
-  TE_CUDA(c->stage[7].reserve(sizeof(double) * (size_t)npaths));
-  TE_CUDA(c->stage[9].reserve((size_t)npaths));
-  TE_CUDA(c->stage[10].reserve(sizeof(double) * (size_t)npaths));
-  TE_CUDA(cudaMemcpyAsync(c->stage[5].p, path_begin, sizeof(int32_t) * (size_t)(npaths + 1), cudaMemcpyHostToDevice, c->stream));
-  if (nposes > 0) TE_CUDA(cudaMemcpyAsync(c->stage[6].p, poses, sizeof(double) * 7 * (size_t)nposes, cudaMemcpyHostToDevice, c->stream));
-  const unsigned char* dcons = nullptr;
-  if (conservative) {
-    TE_CUDA(c->stage[8].reserve((size_t)npaths));
-    TE_CUDA(cudaMemcpyAsync(c->stage[8].p, conservative, (size_t)npaths, cudaMemcpyHostToDevice, c->stream));
-    dcons = (const unsigned char*)c->stage[8].p;
-  }
-  int rc = te::launch_check_paths_polygon(c->fp, v, g, p, in[0], in[1], in[2], in[4], in[3], in[5], nfootprint, footprint_xyz, npaths, nposes,
-                                          (const int*)c->stage[5].p, (const double*)c->stage[6].p, dcons, mp, (unsigned char*)c->stage[9].p,
-                                          (double*)c->stage[10].p, (double*)c->stage[7].p, c->stream, &nl);
+  Staging st(c, host, g_in);
+  const float* in[6] = {st.in_layer(trav, g->cols), st.in_layer(slope, g->cols), st.in_layer(step, g->cols), st.in_layer(elev, g->cols),
+                        st.in_layer(use_rough ? rough : nullptr, g->cols), st.in_layer(robot_slope, g->cols)};
+  const int32_t* dpb = st.in(path_begin, (size_t)npaths + 1);
+  const double* dposes = st.in(poses, 7 * (size_t)nposes);
+  const uint8_t* dcons = st.in(conservative, (size_t)npaths);
+  uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
+  double* dtrav = st.out(traversability, (size_t)npaths);
+  double* darea = st.out(area, (size_t)npaths);
+  if (st.rc) return st.rc;
+  const te_slab s{0, g->cols, 0, 0};
+  int nl = 0;
+  int rc = te::launch_check_paths_polygon(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], in[5], nfootprint, footprint_xyz,
+                                          npaths, nposes, dpb, dposes, dcons, mp, dsafe, dtrav, darea, c->stream, &nl);
   if (rc != 0) return fail(rc, "polygonal path check failed: %s", c->fp.why.c_str());
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(TE_ERR_CUDA, "polygonal path check launch failed: %s", cudaGetErrorString(e));
-  c->launches += nl;
-  TE_CUDA(cudaMemcpyAsync(is_safe, c->stage[9].p, (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
-  TE_CUDA(cudaMemcpyAsync(traversability, c->stage[10].p, sizeof(double) * (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
-  TE_CUDA(cudaMemcpyAsync(area, c->stage[7].p, sizeof(double) * (size_t)npaths, cudaMemcpyDeviceToHost, c->stream));
-  TE_CUDA(cudaStreamSynchronize(c->stream));
-  return TE_OK;
+  if (int r2 = launch_check(c, "polygonal path check", nl)) return r2;
+  return st.finish();
 }
 
 // A te IPC handle is the CUDA handle of the ALLOCATION that contains the pointer (cudaIpcGetMemHandle always describes the whole

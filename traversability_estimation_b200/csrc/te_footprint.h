@@ -5,6 +5,7 @@
 #include <vector>
 #include "../../include/te_b200.h"
 #include "te_device.cuh"
+#include "te_kernels.h"
 
 namespace te {
 
@@ -13,41 +14,31 @@ struct FootprintState {
   bool valid = false;
   te_geometry key_geo{};
   te_footprint_params key_par{};
-  void* d_spiral = nullptr;  // packed (di,dj) of the SpiralIterator visit order
-  size_t spiral_cap = 0;
+  DevBuf spiral;  // packed (di,dj) of the SpiralIterator visit order
   int n_spiral = 0;
-  void* d_block = nullptr;   // per-cell predicate bytes for the slab + halo
-  size_t block_cap = 0;
+  DevBuf block;   // per-cell predicate bytes for the slab + halo
   // prefix-sum sweep: half-width / ring tables (depend on radius and resolution) and per-call prefix sums + bit columns
-  void* d_tables = nullptr;
-  size_t tables_cap = 0;
+  DevBuf tables;
   bool tables_valid = false;
   size_t off_ring = 0, off_fuzzy = 0, off_halfw = 0, off_inner = 0;
   int n_fuzzy = 0, L = 0, nrings = 0;
   signed char h_halfw[64] = {0};
-  void* d_prefix = nullptr;   // packed blocked flags + nearest-blocked bytes (the prefix sums live in k_sweep_tile's shared memory)
-  size_t prefix_cap = 0;
-  bool tile_attr = false;     // k_sweep_tile's dynamic shared-memory limit has been raised (a per-device function attribute)
-  void* d_list = nullptr;    // work list of the cells whose predicates need the window / gap-walk code (word 0: length)
-  size_t list_cap = 0;
-  void* d_poly[2] = {nullptr, nullptr};  // run / uncertain-offset tables of the unrotated and the rotated footprint polygon
-  size_t poly_cap[2] = {0, 0};
+  DevBuf prefix;  // per input-buffer column: prefix sums of t', packed blocked flags, nearest-blocked bytes (k_sweep_fast)
+  DevBuf list;    // work list of the cells whose predicates need the window / gap-walk code (word 0: length)
+  DevBuf poly[2];  // run / uncertain-offset tables of the unrotated and the rotated footprint polygon
   bool poly_attr = false;
-  void* d_rings = nullptr;   // fresh path checks: ring starts + SpiralIterator visit order of rings 0..127 (built once)
-  void* d_memo = nullptr;    // fresh and polygonal path checks: per-cell isTraversableForFilters memo of one call
-  size_t memo_cap = 0;
-  void* d_items = nullptr;   // polygonal path checks: one result record per pose index
-  size_t items_cap = 0;
+  DevBuf rings;   // fresh path checks: ring starts + SpiralIterator visit order of rings 0..127 (built once)
+  DevBuf memo;    // fresh and polygonal path checks: per-cell isTraversableForFilters memo of one call
+  DevBuf items;   // polygonal path checks: one result record per pose index
   void invalidate() { valid = false; tables_valid = false; }
   void release();
 };
 
 int footprint_halo(const te_geometry* g, const te_footprint_params* p);
 
-int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p,
-                     const std::vector<double>& X, const std::vector<double>& Y, const float* trav, const float* slope,
-                     const float* step, const float* rough, const float* elev, float* out, float* slope_fp, float* step_fp,
-                     float* rough_fp, int sms, cudaStream_t s, int* launches);
+int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                     const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
+                     float* step_fp, float* rough_fp, int sms, cudaStream_t s, int* launches);
 
 // TraversabilityMap::traversabilityFootprint(double footprintYaw) (TraversabilityMap.cpp:239-305): layers traversability_x / _rot.
 int footprint_polygon_halo(const te_geometry* g, const te_footprint_params* p, int npts, const double* pts_xy);

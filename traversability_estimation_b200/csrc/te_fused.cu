@@ -1064,10 +1064,8 @@ void fused_plan(int rows, int out_ncols, int nmaps, int sms, int out[19]) {
 }
 
 void FusedState::release() {
-  if (d_rowmask) cudaFree(d_rowmask);
-  if (d_colmask) cudaFree(d_colmask);
-  d_rowmask = d_colmask = nullptr;
-  rowmask_cap = colmask_cap = 0;
+  rowmask.release();
+  colmask.release();
   valid = false;
 }
 
@@ -1117,20 +1115,12 @@ bool fused_eligible(FusedState& st, const std::vector<double>& X, const std::vec
   for (int j = 0; j < g->cols; ++j) cm[j] = bits(Y, j, g->cols);
   // Kernels of an earlier asynchronous call may still read the tables: the overwrite is ordered after them on the context
   // stream (a reallocation waits for the stream first).
-  auto upload = [&](void*& d, size_t& cap, const std::vector<unsigned char>& h) {
-    if (cap < h.size()) {
-      if (d) {
-        if (cudaStreamSynchronize(stream) != cudaSuccess) return false;
-        cudaFree(d);
-      }
-      d = nullptr;
-      cap = 0;
-      if (cudaMalloc(&d, h.size()) != cudaSuccess) return false;
-      cap = h.size();
-    }
-    return cudaMemcpyAsync(d, h.data(), h.size(), cudaMemcpyHostToDevice, stream) == cudaSuccess;
+  auto upload = [&](DevBuf& d, const std::vector<unsigned char>& h) {
+    if (d.p && d.cap < h.size() && cudaStreamSynchronize(stream) != cudaSuccess) return false;
+    return d.reserve(h.size()) == cudaSuccess &&
+           cudaMemcpyAsync(d.p, h.data(), h.size(), cudaMemcpyHostToDevice, stream) == cudaSuccess;
   };
-  if (!upload(st.d_rowmask, st.rowmask_cap, rm) || !upload(st.d_colmask, st.colmask_cap, cm)) return no("mask table upload failed");
+  if (!upload(st.rowmask, rm) || !upload(st.colmask, cm)) return no("mask table upload failed");
   if (cudaStreamSynchronize(stream) != cudaSuccess) return no("mask table upload failed");  // the host copies are reused
   st.shape_id = id;
   st.valid = true;
@@ -1158,8 +1148,8 @@ void make_fixup_args(const FusedState& st, const SlabView& v, const ChainDev& p,
   // tier 2's own error on centred coordinates an order below).  The band is 100 times that, at least 1e-6 ulp.
   a.nz_guard = std::max(1e-6, 100.0 * 6e-12 * v.coord_max / v.res);
   a.fuse_w = p.fuse_w;
-  a.rowmask = (const unsigned char*)st.d_rowmask;
-  a.colmask = (const unsigned char*)st.d_colmask;
+  a.rowmask = (const unsigned char*)st.rowmask.p;
+  a.colmask = (const unsigned char*)st.colmask.p;
   *out = a;
 }
 
@@ -1240,8 +1230,8 @@ int launch_chain_fused(FusedState& st, const SlabView& v, const ChainDev& p, int
   a.k_p0 = B2(1.570796251296997); a.k_p1 = B2(-0.21459604799747467); a.k_p2 = B2(0.08894557505846024);
   a.k_p3 = B2(-0.05000271648168564); a.k_p4 = B2(0.03044925443828106); a.k_p5 = B2(-0.016484638676047325);
   a.k_p6 = B2(0.006254698149859905); a.k_p7 = B2(-0.0011488182935863733);
-  a.rowmask = (const unsigned char*)st.d_rowmask;
-  a.colmask = (const unsigned char*)st.d_colmask;
+  a.rowmask = (const unsigned char*)st.rowmask.p;
+  a.colmask = (const unsigned char*)st.colmask.p;
   a.slope = o.slope; a.step = o.step; a.rough = o.rough; a.trav = o.trav;
   a.nx = (o.nx && o.ny && o.nz) ? o.nx : nullptr; a.ny = o.ny; a.nz = o.nz;
   a.list = list; a.count = count; a.cap = cap;

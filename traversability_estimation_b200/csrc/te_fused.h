@@ -15,9 +15,7 @@ struct FusedState {
   te_chain_params key_par{};
   int shape_id = -1;
   std::vector<unsigned char> h_rowmask, h_colmask;  // host copies of the tables below
-  void* d_rowmask = nullptr;  // per-row on-circle membership bits
-  void* d_colmask = nullptr;
-  size_t rowmask_cap = 0, colmask_cap = 0;
+  DevBuf rowmask, colmask;  // per-row / per-column on-circle membership bits
   bool smem_attr[4] = {false, false, false, false};  // dynamic shared memory limit raised for instantiation [shape*2 + normals]
                                                      // (a per-device function attribute; a context lives on one device)
   void invalidate() { valid = false; }

@@ -5,6 +5,25 @@
 
 namespace te {
 
+// A grow-only device allocation: reserve() reallocates (without keeping the contents) only when `bytes` exceeds the capacity.
+struct DevBuf {
+  void* p = nullptr;
+  size_t cap = 0;
+  cudaError_t reserve(size_t bytes) {
+    if (bytes <= cap) return cudaSuccess;
+    release();
+    cudaError_t e = cudaMalloc(&p, bytes);
+    if (e == cudaSuccess) cap = bytes;
+    else p = nullptr;
+    return e;
+  }
+  void release() {
+    if (p) cudaFree(p);
+    p = nullptr;
+    cap = 0;
+  }
+};
+
 struct ChainOut {
   float* slope;
   float* step;
