@@ -301,6 +301,53 @@ int te_check_footprint_paths_polygon(te_ctx* ctx, const te_geometry* g, const te
                                      const uint8_t* conservative_or_null, uint8_t* is_safe, double* traversability_out,
                                      double* area_out, int memory);
 
+/* The untraversable polygon of the two path checks above: what the check_footprint_path service publishes on its
+ * untraversable_polygon topic for a path with compute_untraversable_polygon set (it always checks with publishPolygons = true,
+ * TraversabilityEstimation.cpp:290).  te_check_footprint_paths_fresh2 / _polygon2 take the arguments of te_check_footprint_paths_fresh
+ * / _polygon plus the polygon outputs, and compute is_safe, traversability and area exactly as those do; with
+ * untraversable_count_or_null == NULL (and untraversable_xy_or_null == NULL) each IS its predecessor.
+ * Output per path q: the LAST NON-EMPTY polygon the service publishes for the path (publishUntraversablePolygon skips empty ones,
+ * :934), or none.  untraversable_count[q] = its vertex count (0: none; always 0 when compute_untraversable_polygon[q] is 0), and
+ * untraversable_xy[2 * max_vertices * q ...] = its first min(count, max_vertices) (x, y) vertices in the reference's order (the rest
+ * of the slot is unspecified).  A count above max_vertices means the polygon was cut to that prefix: call again with more room.  The z of the published polygon
+ * (computeMeanHeightFromPoses, TraversabilityMap.hpp:311) is left to the caller.
+ *   Circular paths (checkCircularFootprintPath :345-462, isTraversable :654-746): a circle whose spiral walk finds a first blocked
+ *   cell within radius walks on to the end of the spiral and collects every blocked cell with getCurrentRadius() <= radius (every
+ *   blocked cell for radius 0); the polygon is monotoneChainConvexHullOfPoints of their cell centres: 3 points or fewer as visited,
+ *   more as the convex hull from the lexicographically smallest vertex, counter-clockwise.  A single pose outside the map with
+ *   traversability_default 0, and a centre an earlier segment of the path cached as 0, give Polygon::fromCircle(centre,
+ *   radius + offset).  A single pose publishes its circle's polygon; a longer path publishes, for its failing segment,
+ *   convexHull(path polygon, failing circle's polygon) taken once per checked line cell from the failing one on (:407-412), which
+ *   is that polygon's hull except for 1 to 3 collected cells: 2 or 3 cells give their hull; 1 cell gives the point 2 times for an
+ *   even number of hulls and 3 times for an odd one.  checkInclination failures publish nothing.
+ *   Polygonal paths (checkPolygonalFootprintPath :464-584, isTraversable(polygon) :592-645): compute_untraversable_polygon_or_null
+ *   (FootprintPath.compute_untraversable_polygon per path; NULL = all 0) lets the PolygonIterator walk go on past blocked cells; the
+ *   polygon is monotoneChainConvexHullOfPoints of all blocked cell centres of the failing segment (or single pose).
+ * RECALLED, not in the reference checkout (grid_map 1.6.x): Polygon::fromCircle(center, radius, nVertices = 20): vertex j =
+ * center + Rotation2D(j * 2 * M_PI / 19) * (radius, 0), so the last vertex repeats the first up to the rounding of sin(2 pi); the
+ * cosines and sines come from the host's libm.  Polygon::convexHull(P1, P2) = monotoneChainConvexHullOfPoints(P1 ++ P2).
+ * Bound: a polygonal segment's (or pose's) footprint hull may span at most 1024 map rows when its polygon is requested.  Circular
+ * paths have no bound beyond the 127-ring radius limit.
+ * Errors, beyond those of the predecessors: TE_ERR_BAD_ARG for max_vertices < 0, a count pointer without an xy pointer while
+ * max_vertices > 0, and an xy pointer without a count pointer; TE_ERR_UNSUPPORTED in TE_MEM_HOST when a requested polygonal
+ * polygon passes the 1024-row bound (the other outputs are written).  TE_MEM_DEVICE cannot read the paths: a path whose polygon
+ * was requested but could not be computed (past the bound, or a path the check marks with NaN) gets count -1; its is_safe,
+ * traversability and area are those of the predecessor.  TE_MEM_HOST accepts a circular-buffer start index as the
+ * predecessors do. */
+int te_check_footprint_paths_fresh2(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, const float* traversability,
+                                    const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                                    const float* robot_slope_or_null, int32_t npaths, const int32_t* path_begin, const double* poses_xy,
+                                    const double* radius, const uint8_t* compute_untraversable_polygon_or_null, uint8_t* is_safe,
+                                    double* traversability_out, int32_t max_vertices, int32_t* untraversable_count_or_null,
+                                    double* untraversable_xy_or_null, int memory);
+int te_check_footprint_paths_polygon2(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, const float* traversability,
+                                      const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                                      const float* robot_slope_or_null, int32_t nfootprint, const float* footprint_xyz, int32_t npaths,
+                                      int32_t nposes, const int32_t* path_begin, const double* poses,
+                                      const uint8_t* conservative_or_null, uint8_t* is_safe, double* traversability_out,
+                                      double* area_out, const uint8_t* compute_untraversable_polygon_or_null, int32_t max_vertices,
+                                      int32_t* untraversable_count_or_null, double* untraversable_xy_or_null, int memory);
+
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the
  * neighbours' boundary columns of the INPUT layer(s) into this rank's halo.  The reference has no counterpart (it is a

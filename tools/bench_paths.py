@@ -14,6 +14,10 @@ with the GPU name and its power limit.
 (robot_footprint_parameter.yaml:3) and planner-like paths with a random yaw per pose, conservative off and on, and the CPU oracle
 of the same call (tests/polygon_paths_oracle.cpp, all host threads, one run; it includes the oracle's whole-map
 isTraversableForFilters pass, which the GPU evaluates only where a polygon looks).
+
+--untraversable times te_check_footprint_paths_fresh2 (radius 0.3 m) and te_check_footprint_paths_polygon2 (YAML footprint) in
+TE_MEM_DEVICE with compute_untraversable_polygon off and on for every path (room for 256 vertices per path), next to the CPU
+oracle of the same calls (tests/untraversable_oracle.cpp; all host threads, one run).
 """
 from __future__ import annotations
 
@@ -63,7 +67,10 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--footprint", choices=("circle", "polygon"), default="circle")
+    ap.add_argument("--untraversable", action="store_true")
     args = ap.parse_args()
+    if args.untraversable:
+        return main_untraversable(args)
     if args.footprint == "polygon":
         return main_polygon(args)
     import torch
@@ -195,6 +202,91 @@ def main_polygon(args):
                               "gpu_median_ms": float(np.median(ts)), "gpu_min_ms": float(np.min(ts)),
                               "cpu_oracle_ms": cpu_ms, "cpu_threads": os.cpu_count(), "safe": int(got[0].sum()),
                               "matches_oracle": bool(same)}), flush=True)
+    ctx.set_stream(None)
+    ctx.close()
+
+
+def main_untraversable(args):
+    import time
+    import torch
+    import synth
+    import traversability_estimation_b200 as te
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import untraversable_oracle as uo
+    from oracle import binding as ob
+
+    n, res, cap = args.size, 0.02, 256
+    g, og = te.Geometry.make(n, n, res), ob.Geometry.make(n, n, res)
+    fp, ofp = te.FootprintParams.yaml_defaults(), ob.FootprintParams.yaml_defaults()
+    fxyz = np.asarray(YAML_FOOTPRINT, np.float32)
+    ctx = te.Context(0)
+    z = synth.terrain(n, n, res, 4096, "mixed")
+    layers = ctx.chain_host(g, te.ChainParams.yaml_defaults(0), z)
+    dev = lambda a: torch.from_numpy(np.ascontiguousarray(np.asarray(a, np.float32).T)).cuda()  # noqa: E731
+    trav, slope, step, elev = (dev(a) for a in (layers["traversability"], layers["slope"], layers["step"], z))
+    stream = torch.cuda.Stream()
+    ctx.set_stream(stream.cuda_stream)
+    name, power = gpu_info(torch)
+    rng = np.random.default_rng(1)
+
+    def timed(run):
+        for _ in range(args.warmup):
+            run()
+        stream.synchronize()
+        ts = []
+        for _ in range(args.reps):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            run()
+            e1.record(stream)
+            e1.synchronize()
+            ts.append(e0.elapsed_time(e1))
+        return float(np.median(ts)), float(np.min(ts))
+
+    for batch in (1, 100, 1000):
+        begin, xy = planner_paths(rng, n, batch, res)
+        yaw = rng.uniform(0, 2 * np.pi, len(xy))
+        poses = np.stack([xy[:, 0], xy[:, 1], np.zeros(len(xy)), np.zeros(len(xy)), np.zeros(len(xy)), np.sin(yaw / 2),
+                          np.cos(yaw / 2)], axis=1)
+        db, dxy, dp = (torch.from_numpy(a).cuda() for a in (begin, xy, poses))
+        dr = torch.full((batch,), 0.3, dtype=torch.float64, device="cuda")
+        safe = torch.empty(batch, dtype=torch.uint8, device="cuda")
+        tout = torch.empty(batch, dtype=torch.float64, device="cuda")
+        aout = torch.empty(batch, dtype=torch.float64, device="cuda")
+        cnt = torch.empty(batch, dtype=torch.int32, device="cuda")
+        uxy = torch.empty((batch, cap, 2), dtype=torch.float64, device="cuda")
+        for cup_on in (0, 1):
+            cup = np.full(batch, cup_on, np.uint8)
+            dcup = torch.from_numpy(cup).cuda()
+            torch.cuda.synchronize()
+            kw = dict(memory=te.MEM_DEVICE, is_safe=safe, traversability_out=tout, untraversable_capacity=cap, untraversable_count=cnt,
+                      untraversable_xy=uxy)
+            for kind in ("circle", "polygon"):
+                if kind == "circle":
+                    def run():
+                        ctx.check_footprint_paths_fresh(g, fp, trav, slope, step, elev, db, dxy, dr, compute_untraversable_polygon=dcup,
+                                                        **kw)
+                else:
+                    def run():
+                        ctx.check_footprint_paths_polygon(g, fp, trav, slope, step, elev, fxyz, db, dp, compute_untraversable_polygon=dcup,
+                                                          area_out=aout, **kw)
+                med, mn = timed(run)
+                t0 = time.perf_counter()
+                if kind == "circle":
+                    want = uo.check_circular_paths_fresh2(og, ofp, layers["traversability"], layers["slope"], layers["step"], z, begin,
+                                                           xy, np.full(batch, 0.3), compute_untraversable_polygon=cup, capacity=cap)
+                    want_counts = want[2]
+                else:
+                    want = uo.check_polygonal_paths2(og, ofp, layers["traversability"], layers["slope"], layers["step"], z, fxyz, begin,
+                                                      poses, compute_untraversable_polygon=cup, capacity=cap)
+                    want_counts = want[3]
+                cpu_ms = (time.perf_counter() - t0) * 1e3
+                got = cnt.cpu().numpy()
+                print(json.dumps({"gpu": name, "power_limit_w": power, "map": f"{n}x{n}", "resolution": res, "footprint": kind,
+                                  "paths": batch, "poses": int(begin[-1]), "compute_untraversable_polygon": cup_on,
+                                  "gpu_median_ms": med, "gpu_min_ms": mn, "cpu_oracle_ms": cpu_ms, "cpu_threads": os.cpu_count(),
+                                  "safe": int(safe.sum().item()), "polygons": int((got > 0).sum()),
+                                  "counts_match_oracle": bool(np.array_equal(got, want_counts))}), flush=True)
     ctx.set_stream(None)
     ctx.close()
 

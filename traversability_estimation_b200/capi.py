@@ -18,7 +18,7 @@ KERNEL_AUTO, KERNEL_GENERIC, KERNEL_FUSED = 0, 1, 2
 
 EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set_stream", "te_synchronize",
            "te_set_kernel", "te_get_stats", "te_enable_timing", "te_get_timing", "te_get_flag_counters", "te_get_escalation_stats", "te_fused_plan", "te_slope", "te_normals", "te_step", "te_roughness", "te_chain",
-           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
+           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_check_footprint_paths_fresh2", "te_check_footprint_paths_polygon2", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
            "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free"]
 
 
@@ -159,6 +159,13 @@ def _addr(a):
     raise TypeError(type(a))
 
 
+def _untraversable_outputs(npaths, capacity):
+    """Host outputs of the untraversable polygons: counts int32[npaths], xy float64[npaths, capacity, 2]."""
+    if int(capacity) < 0:
+        raise ValueError("untraversable_capacity must be >= 0")
+    return np.zeros(npaths, dtype=np.int32), np.zeros((npaths, int(capacity), 2), dtype=np.float64)
+
+
 class Context:
     """One te_ctx (one per rank / plugin instance)."""
 
@@ -297,23 +304,38 @@ class Context:
 
     def check_footprint_paths_fresh(self, g, fp, traversability, slope, step, elevation, path_begin, poses_xy, radius, robot_slope=None,
                                     roughness=None, compute_untraversable_polygon=None, memory=MEM_HOST, is_safe=None,
-                                    traversability_out=None):
+                                    traversability_out=None, untraversable_capacity=None, untraversable_count=None,
+                                    untraversable_xy=None):
         """te_check_footprint_paths_fresh: checkCircularFootprintPath on the chain layers as the reference's service answers it on a
         freshly computed map (empty traversability_footprint cache per path).  radius: FootprintPath.radius per path (float64);
         fp supplies offset, traversability_default, max_gap_width, critical_step_height, radius_is_integer_norm and
         verify_roughness.  MEM_HOST: numpy arguments, returns (is_safe uint8[npaths], traversability float64[npaths]).
         MEM_DEVICE: every argument is a device tensor (path_begin int32, poses_xy / radius float64,
-        compute_untraversable_polygon uint8) and the results go to the caller's is_safe / traversability_out tensors."""
-        sig = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + [C.c_int32] + [C.c_void_p] * 6 + [C.c_int]
-        self._L.te_check_footprint_paths_fresh.argtypes = sig
+        compute_untraversable_polygon uint8) and the results go to the caller's is_safe / traversability_out tensors.
+        untraversable_capacity=V (te_check_footprint_paths_fresh2): the tuple gains the untraversable polygons, counts
+        (int32[npaths]: vertex count, 0 none, -1 not computed) and xy (float64[npaths, V, 2]: the first min(count, V) vertices);
+        in MEM_DEVICE they are the caller's untraversable_count / untraversable_xy tensors."""
+        if untraversable_capacity is None:
+            sig = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + [C.c_int32] + [C.c_void_p] * 6 + [C.c_int]
+            fn = self._L.te_check_footprint_paths_fresh
+            extra = ()
+        else:
+            sig = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + [C.c_int32] + [C.c_void_p] * 6 + \
+                [C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
+            fn = self._L.te_check_footprint_paths_fresh2
+        fn.argtypes = sig
         if memory == MEM_DEVICE:
             self._order_after_torch(memory)
             n = int(path_begin.numel()) - 1
-            self._check(self._L.te_check_footprint_paths_fresh(
+            if untraversable_capacity is not None:
+                extra = (int(untraversable_capacity), _addr(untraversable_count), _addr(untraversable_xy))
+            self._check(fn(
                 self._h, C.byref(g), C.byref(fp), _addr(traversability), _addr(slope), _addr(step), _addr(roughness), _addr(elevation),
                 _addr(robot_slope), n, _addr(path_begin), _addr(poses_xy), _addr(radius), _addr(compute_untraversable_polygon),
-                _addr(is_safe), _addr(traversability_out), MEM_DEVICE))
-            return is_safe, traversability_out
+                _addr(is_safe), _addr(traversability_out), *extra, MEM_DEVICE))
+            if untraversable_capacity is None:
+                return is_safe, traversability_out
+            return is_safe, traversability_out, untraversable_count, untraversable_xy
         lay = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)  # noqa: E731
         t, s, st, e, rs, r = (lay(a) for a in (traversability, slope, step, elevation, robot_slope, roughness))
         pb = np.ascontiguousarray(path_begin, dtype=np.int32)
@@ -325,33 +347,52 @@ class Context:
             raise ValueError("radius / compute_untraversable_polygon need one entry per path")
         safe = np.zeros(n, dtype=np.uint8) if is_safe is None else is_safe
         trav = np.zeros(n, dtype=np.float64) if traversability_out is None else traversability_out
-        self._check(self._L.te_check_footprint_paths_fresh(
+        if untraversable_capacity is not None:
+            counts, uxy = _untraversable_outputs(n, untraversable_capacity)
+            extra = (int(untraversable_capacity), counts.ctypes.data, uxy.ctypes.data)
+        self._check(fn(
             self._h, C.byref(g), C.byref(fp), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), n, pb.ctypes.data,
-            xy.ctypes.data, rad.ctypes.data, _addr(cup), safe.ctypes.data, trav.ctypes.data, MEM_HOST))
-        return safe, trav
+            xy.ctypes.data, rad.ctypes.data, _addr(cup), safe.ctypes.data, trav.ctypes.data, *extra, MEM_HOST))
+        if untraversable_capacity is None:
+            return safe, trav
+        return safe, trav, counts, uxy
 
     def check_footprint_paths_polygon(self, g, fp, traversability, slope, step, elevation, footprint_xyz, path_begin, poses,
                                       robot_slope=None, roughness=None, conservative=None, memory=MEM_HOST, is_safe=None,
-                                      traversability_out=None, area_out=None):
+                                      traversability_out=None, area_out=None, compute_untraversable_polygon=None,
+                                      untraversable_capacity=None, untraversable_count=None, untraversable_xy=None):
         """te_check_footprint_paths_polygon: checkPolygonalFootprintPath on the chain layers.  footprint_xyz: (n, 3) vertices
         (float32, host in both modes); poses: (nposes, 7) x y z qx qy qz qw; conservative: FootprintPath.conservative per path.
         fp supplies traversability_default, max_gap_width, critical_step_height and verify_roughness.  MEM_HOST: numpy arguments,
         returns (is_safe uint8, traversability float64, area float64) per path.  MEM_DEVICE: every other argument is a device
         tensor (path_begin int32, poses float64, conservative uint8) and the results go to the caller's is_safe /
-        traversability_out / area_out tensors."""
-        sig = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + [C.c_int32, C.c_void_p, C.c_int32,
-                                                                                                 C.c_int32] + [C.c_void_p] * 6 + [C.c_int]
-        self._L.te_check_footprint_paths_polygon.argtypes = sig
+        traversability_out / area_out tensors.  untraversable_capacity=V (te_check_footprint_paths_polygon2, with
+        compute_untraversable_polygon uint8 per path): the tuple gains counts (int32[npaths]) and xy (float64[npaths, V, 2]) as
+        in check_footprint_paths_fresh."""
+        if untraversable_capacity is None:
+            fn = self._L.te_check_footprint_paths_polygon
+            tail = []
+            extra = ()
+        else:
+            fn = self._L.te_check_footprint_paths_polygon2
+            tail = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + \
+            [C.c_int32, C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 6 + tail + [C.c_int]
         fxyz = np.ascontiguousarray(footprint_xyz, dtype=np.float32).reshape(-1, 3)
         if memory == MEM_DEVICE:
             self._order_after_torch(memory)
             n = int(path_begin.numel()) - 1
             nposes = int(poses.numel()) // 7
-            self._check(self._L.te_check_footprint_paths_polygon(
+            if untraversable_capacity is not None:
+                extra = (_addr(compute_untraversable_polygon), int(untraversable_capacity), _addr(untraversable_count),
+                         _addr(untraversable_xy))
+            self._check(fn(
                 self._h, C.byref(g), C.byref(fp), _addr(traversability), _addr(slope), _addr(step), _addr(roughness), _addr(elevation),
                 _addr(robot_slope), len(fxyz), fxyz.ctypes.data, n, nposes, _addr(path_begin), _addr(poses), _addr(conservative),
-                _addr(is_safe), _addr(traversability_out), _addr(area_out), MEM_DEVICE))
-            return is_safe, traversability_out, area_out
+                _addr(is_safe), _addr(traversability_out), _addr(area_out), *extra, MEM_DEVICE))
+            if untraversable_capacity is None:
+                return is_safe, traversability_out, area_out
+            return is_safe, traversability_out, area_out, untraversable_count, untraversable_xy
         lay = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)  # noqa: E731
         t, s, st, e, rs, r = (lay(a) for a in (traversability, slope, step, elevation, robot_slope, roughness))
         pb = np.ascontiguousarray(path_begin, dtype=np.int32)
@@ -363,10 +404,19 @@ class Context:
         safe = np.zeros(n, dtype=np.uint8) if is_safe is None else is_safe
         trav = np.zeros(n, dtype=np.float64) if traversability_out is None else traversability_out
         area = np.zeros(n, dtype=np.float64) if area_out is None else area_out
-        self._check(self._L.te_check_footprint_paths_polygon(
+        if untraversable_capacity is not None:
+            cup = None if compute_untraversable_polygon is None else np.ascontiguousarray(compute_untraversable_polygon, dtype=np.uint8)
+            if cup is not None and len(cup) != n:
+                raise ValueError("compute_untraversable_polygon needs one entry per path")
+            counts, uxy = _untraversable_outputs(n, untraversable_capacity)
+            extra = (_addr(cup), int(untraversable_capacity), counts.ctypes.data, uxy.ctypes.data)
+        self._check(fn(
             self._h, C.byref(g), C.byref(fp), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), len(fxyz), fxyz.ctypes.data,
-            n, len(ps), pb.ctypes.data, ps.ctypes.data, _addr(cons), safe.ctypes.data, trav.ctypes.data, area.ctypes.data, MEM_HOST))
-        return safe, trav, area
+            n, len(ps), pb.ctypes.data, ps.ctypes.data, _addr(cons), safe.ctypes.data, trav.ctypes.data, area.ctypes.data, *extra,
+            MEM_HOST))
+        if untraversable_capacity is None:
+            return safe, trav, area
+        return safe, trav, area, counts, uxy
 
     # ---- multi-GPU halo (te_halo_pull and the IPC helpers around it)
     def ipc_export(self, device_ptr) -> bytes:

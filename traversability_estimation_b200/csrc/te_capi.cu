@@ -74,7 +74,7 @@ struct te_ctx {
   DevBuf dX, dY;
   std::vector<double> hX, hY;
 
-  DevBuf stage[12];          // TE_MEM_HOST staging (handed out in order by Staging)
+  DevBuf stage[16];          // TE_MEM_HOST staging (handed out in order by Staging)
   DevBuf worklist, worklist3, counter;  // fused-kernel fix-up lists (tier 2, tier 3) and their counters
   // The counters are two 512-byte blocks used alternately: the last kernel of a chain call (k_fixup_cells) zeroes the block of the
   // NEXT call, so a call needs no cudaMemsetAsync of its own (one stream operation and one launch gap less per map).
@@ -880,6 +880,15 @@ int te_footprint(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_
   return te_footprint2(c, g, slab, p, trav, slope, step, nullptr, elev, out, slope_fp, step_fp, nullptr, memory);
 }
 
+// The untraversable-polygon outputs of te_check_footprint_paths_fresh2 / _polygon2: both null (no polygon), or counts with room
+// for max_vertices >= 0 points per path (xy may be null only when max_vertices is 0).
+static int check_polygon_outputs(int32_t max_vertices, const int32_t* ucount, const double* uxy) {
+  if (max_vertices < 0) return fail(TE_ERR_BAD_ARG, "max_vertices must be >= 0, got %d", max_vertices);
+  if (ucount && !uxy && max_vertices > 0) return fail(TE_ERR_BAD_ARG, "untraversable_count given without untraversable_xy");
+  if (!ucount && uxy) return fail(TE_ERR_BAD_ARG, "untraversable_xy given without untraversable_count");
+  return TE_OK;
+}
+
 int te_check_footprint_paths(te_ctx* c, const te_geometry* g, const float* footprint, double traversability_default, int32_t npaths,
                              const int32_t* path_begin, const double* poses_xy, uint8_t* is_safe, double* traversability, int memory) {
   return te_check_footprint_paths2(c, g, footprint, nullptr, traversability_default, npaths, path_begin, poses_xy, is_safe, traversability, memory);
@@ -918,6 +927,15 @@ int te_check_footprint_paths_fresh(te_ctx* c, const te_geometry* g_in, const te_
                                    const float* step, const float* rough, const float* elev, const float* robot_slope, int32_t npaths,
                                    const int32_t* path_begin, const double* poses_xy, const double* radius, const uint8_t* cup,
                                    uint8_t* is_safe, double* traversability, int memory) {
+  return te_check_footprint_paths_fresh2(c, g_in, p, trav, slope, step, rough, elev, robot_slope, npaths, path_begin, poses_xy, radius, cup,
+                                         is_safe, traversability, 0, nullptr, nullptr, memory);
+}
+
+int te_check_footprint_paths_fresh2(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
+                                    const float* step, const float* rough, const float* elev, const float* robot_slope, int32_t npaths,
+                                    const int32_t* path_begin, const double* poses_xy, const double* radius, const uint8_t* cup,
+                                    uint8_t* is_safe, double* traversability, int32_t max_vertices, int32_t* ucount, double* uxy,
+                                    int memory) {
   TE_ENTER(c);
   te_geometry g0;
   if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
@@ -926,6 +944,7 @@ int te_check_footprint_paths_fresh(te_ctx* c, const te_geometry* g_in, const te_
   if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
   if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
   if (npaths < 0 || !path_begin || !poses_xy || !radius || !is_safe || !traversability) return fail(TE_ERR_BAD_ARG, "null argument or negative path count");
+  if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
   if (npaths == 0) return TE_OK;
   const bool use_rough = p->verify_roughness != 0;
   if (int rc = ensure_geometry(c, g)) return rc;
@@ -951,12 +970,14 @@ int te_check_footprint_paths_fresh(te_ctx* c, const te_geometry* g_in, const te_
   const uint8_t* dcup = st.in(cup, (size_t)npaths);
   uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
   double* dtrav = st.out(traversability, (size_t)npaths);
+  int32_t* dcount = st.out(ucount, (size_t)npaths);
+  double* duxy = st.out(uxy, 2 * (size_t)max_vertices * npaths);
   if (st.rc) return st.rc;
   const te_slab s{0, g->cols, 0, 0};
   int rc = te::launch_check_paths_fresh(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], in[5], npaths, dpb, dxy, drad,
-                                        dcup, dsafe, dtrav, c->stream);
+                                        dcup, dsafe, dtrav, max_vertices, dcount, duxy, c->stream);
   if (rc != 0) return fail(rc, "fresh path check failed: %s", c->fp.why.c_str());
-  if (int r2 = launch_check(c, "k_check_paths_fresh")) return r2;
+  if (int r2 = launch_check(c, dcount ? "k_check_paths_fresh_poly" : "k_check_paths_fresh")) return r2;
   return st.finish();
 }
 
@@ -965,6 +986,16 @@ int te_check_footprint_paths_polygon(te_ctx* c, const te_geometry* g_in, const t
                                      const float* footprint_xyz, int32_t npaths, int32_t nposes, const int32_t* path_begin,
                                      const double* poses, const uint8_t* conservative, uint8_t* is_safe, double* traversability,
                                      double* area, int memory) {
+  return te_check_footprint_paths_polygon2(c, g_in, p, trav, slope, step, rough, elev, robot_slope, nfootprint, footprint_xyz, npaths, nposes,
+                                           path_begin, poses, conservative, is_safe, traversability, area, nullptr, 0, nullptr, nullptr,
+                                           memory);
+}
+
+int te_check_footprint_paths_polygon2(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
+                                      const float* step, const float* rough, const float* elev, const float* robot_slope, int32_t nfootprint,
+                                      const float* footprint_xyz, int32_t npaths, int32_t nposes, const int32_t* path_begin,
+                                      const double* poses, const uint8_t* conservative, uint8_t* is_safe, double* traversability,
+                                      double* area, const uint8_t* cup, int32_t max_vertices, int32_t* ucount, double* uxy, int memory) {
   TE_ENTER(c);
   te_geometry g0;
   if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
@@ -976,6 +1007,7 @@ int te_check_footprint_paths_polygon(te_ctx* c, const te_geometry* g_in, const t
   if (nfootprint < 1 || nfootprint > te::kPolyMaxVerts) return fail(TE_ERR_BAD_ARG, "footprint needs 1..%d vertices, got %d", te::kPolyMaxVerts, nfootprint);
   for (int k = 0; k < 3 * nfootprint; ++k)
     if (!std::isfinite(footprint_xyz[k])) return fail(TE_ERR_BAD_ARG, "footprint vertex %d is not finite", k / 3);
+  if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
   if (npaths == 0) return TE_OK;
   const bool use_rough = p->verify_roughness != 0;
   if (int rc = ensure_geometry(c, g)) return rc;
@@ -1008,14 +1040,23 @@ int te_check_footprint_paths_polygon(te_ctx* c, const te_geometry* g_in, const t
   uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
   double* dtrav = st.out(traversability, (size_t)npaths);
   double* darea = st.out(area, (size_t)npaths);
+  const uint8_t* dcup = ucount ? st.in(cup, (size_t)npaths) : nullptr;
+  int32_t* dcount = st.out(ucount, (size_t)npaths);
+  double* duxy = st.out(uxy, 2 * (size_t)max_vertices * npaths);
   if (st.rc) return st.rc;
   const te_slab s{0, g->cols, 0, 0};
   int nl = 0;
   int rc = te::launch_check_paths_polygon(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], in[5], nfootprint, footprint_xyz,
-                                          npaths, nposes, dpb, dposes, dcons, mp, dsafe, dtrav, darea, c->stream, &nl);
+                                          npaths, nposes, dpb, dposes, dcons, mp, dsafe, dtrav, darea, dcup, max_vertices, dcount, duxy,
+                                          c->stream, &nl);
   if (rc != 0) return fail(rc, "polygonal path check failed: %s", c->fp.why.c_str());
   if (int r2 = launch_check(c, "polygonal path check", nl)) return r2;
-  return st.finish();
+  if (int r2 = st.finish()) return r2;
+  if (host && ucount)  // the row bound of the polygon's table (kUntravRows) is only known once the hulls are
+    for (int32_t q = 0; q < npaths; ++q)
+      if (ucount[q] < 0)
+        return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);
+  return TE_OK;
 }
 
 // A te IPC handle is the CUDA handle of the ALLOCATION that contains the pointer (cudaIpcGetMemHandle always describes the whole

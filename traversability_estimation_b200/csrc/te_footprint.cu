@@ -993,7 +993,202 @@ __device__ FreshCircle fresh_circle_d(const FpArgs& A, const Layers& L, const Pa
   return FreshCircle{true, t, (float)t};
 }
 
-__global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, PathArgs P) {
+__device__ __forceinline__ bool lex_less_d(double2 a, double2 b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
+
+// grid_map::Polygon::monotoneChainConvexHullOfPoints (recalled) of the m > 3 points `sorted` (already in lexicographic order) into
+// `hull` (2m entries, the reference's own allocation); returns the vertex count.  One thread.
+__device__ int monotone_chain_d(const double2* sorted, int m, double2* hull) {
+  auto clockwise = [](double2 o, double2 a, double2 b) {
+    const double ux = a.x - o.x, uy = a.y - o.y, wx = b.x - o.x, wy = b.y - o.y;
+    return (ux * wy - uy * wx) <= 0;
+  };
+  int k = 0;
+  for (int i = 0; i < m; ++i) {
+    while (k >= 2 && clockwise(hull[k - 2], hull[k - 1], sorted[i])) k--;
+    hull[k++] = sorted[i];
+  }
+  for (int i = m - 2, t = k + 1; i >= 0; i--) {
+    while (k >= t && clockwise(hull[k - 2], hull[k - 1], sorted[i])) k--;
+    hull[k++] = sorted[i];
+  }
+  return k - 1;
+}
+
+// ---- untraversable polygon (isTraversable with computeUntraversablePolygon, :599-645 and :679-736) -------------------------
+// The reference pushes the cell centre of every collected blocked cell and returns monotoneChainConvexHullOfPoints of that list
+// (recalled, see monotone_chain_d): 3 points or fewer as given, in visit order; otherwise the sorted monotone chain.  The kernels
+// do not keep the list.  A warp records, per map row of the walk, the smallest and largest column index of its collected cells
+// (shared atomics), the number of cells and the first three in visit order.  That is exact:
+//   - X[a] falls as the row index a grows and Y[b] as the column index b grows, so reading the table by descending row and, within
+//     a row, by descending column yields the lexicographic order of std::sort (x, then y) without sorting;
+//   - all cells of one row share the double X[a].  Between its two extremes, a row's cells only ever meet the chain as the third
+//     point of a vertical triple, whose cross product is exactly 0 (both x differences are 0.0): the point is popped.  Before that
+//     the row's second point is tested against the chain from an earlier row, and that cross product is (X[a] - x') times the
+//     difference of two column positions: at least res^2 in magnitude, far from rounding for any map whose coordinates stay
+//     below res * 2^40, so it never pops.  The chain therefore goes through the same states with the extremes alone, and its
+//     stack holds at most one point per row and pass plus two (2 * rows + 2 entries).
+// A map row without collected cells has max < min in the table.
+constexpr int kFromCircleVertices = 20;    // grid_map::Polygon::fromCircle's default nVertices
+
+struct UntravOut {
+  int maxv;     // vertices the caller has room for per path
+  int* count;   // per path: vertex count (0: no polygon, -1: not computed); nullptr: polygon not requested
+  double* xy;   // per path: maxv (x, y) pairs
+};
+
+// The monotone chain of monotone_chain_d over the points of a row table (rows 0 .. nrows-1, row r at map row a0 + r, column
+// extremes tmin / tmax), pruned to the row extremes as argued above; `st` receives the hull as (row, column) and has room for
+// 2 * nrows + 4 entries.  Returns the vertex count.  One thread.  Used for more than 3 points (or 2 or 3 points hulled twice).
+__device__ int table_chain_d(const FpArgs& A, const int* tmin, const int* tmax, int nrows, int a0, int2* st) {
+  auto cw = [&](int2 o, int2 p, int2 w) {
+    const double ox = A.X[a0 + o.x], oy = A.Y[o.y];
+    const double ux = A.X[a0 + p.x] - ox, uy = A.Y[p.y] - oy, wx = A.X[a0 + w.x] - ox, wy = A.Y[w.y] - oy;
+    return (ux * wy - uy * wx) <= 0;
+  };
+  int k = 0;
+  for (int r = nrows - 1; r >= 0; --r) {  // lower hull: x ascending = row index descending; y ascending = column descending
+    const int lo = tmin[r], hi = tmax[r];
+    if (hi < lo) continue;
+    for (int e = 0; e < 2 && (e == 0 || lo != hi); ++e) {
+      const int2 p = make_int2(r, e ? lo : hi);
+      while (k >= 2 && cw(st[k - 2], st[k - 1], p)) k--;
+      st[k++] = p;
+    }
+  }
+  const int t = k + 1;
+  bool last = true;  // the upper hull starts at the second largest point
+  for (int r = 0; r < nrows; ++r) {
+    const int lo = tmin[r], hi = tmax[r];
+    if (hi < lo) continue;
+    for (int e = 0; e < 2 && (e == 0 || lo != hi); ++e) {
+      const int2 p = make_int2(r, e ? hi : lo);
+      if (last) { last = false; continue; }
+      while (k >= t && cw(st[k - 2], st[k - 1], p)) k--;
+      st[k++] = p;
+    }
+  }
+  return k - 1;
+}
+
+// A warp's polygon scratch in shared memory.
+struct UntravScratch {
+  int* tmin;
+  int* tmax;
+  int2* stack;    // 2 * rows + 4 entries; also holds the 20 + 40 points of a fromCircle hull (as double2)
+  int2* first;    // the first three collected cells (map row, map column) in visit order
+};
+
+// Records the cells whose lanes have `take` set (map row a, map column b; table row a - a0) in visit order = lane order.
+__device__ __forceinline__ void collect_cells_d(const UntravScratch& S, bool take, int a, int b, int a0, int& cnt) {
+  const int lane = threadIdx.x & 31;
+  const unsigned m = __ballot_sync(0xffffffffu, take);
+  if (take) {
+    const int rank = cnt + __popc(m & ((1u << lane) - 1u));
+    if (rank < 3) S.first[rank] = make_int2(a, b);
+    atomicMin(S.tmin + (a - a0), b);
+    atomicMax(S.tmax + (a - a0), b);
+  }
+  cnt += __popc(m);
+}
+
+__device__ __forceinline__ void clear_table_d(const UntravScratch& S, int nrows) {
+  for (int r = threadIdx.x & 31; r < nrows; r += 32) { S.tmin[r] = 0x7fffffff; S.tmax[r] = -0x7fffffff - 1; }
+  __syncwarp();
+}
+
+// Writes the polygon of `cnt` collected cells, hulled `reps` times (Polygon::convexHull(U, P) = monotone chain of U ++ P, see
+// k_check_paths_fresh_poly), to slot q of O.  One thread.
+//   reps == 1: monotoneChainConvexHullOfPoints(P): P as given for 3 points or fewer, else the chain.
+//   reps >= 2: with 2 or more distinct points, every later hull has more than 3 input points drawn from P's own points, and the
+//     chain of a point list depends only on the set of its points (a repeated point is popped by a cross product of exactly 0
+//     and pushed again onto the same stack), so it is the chain of P whatever `reps` is.  A single point p grows instead:
+//     [p] -> [p, p] -> [p, p, p] -> chain of [p, p, p, p] = [p, p] -> [p, p, p] ...: 2 vertices for even reps, 3 for odd.
+__device__ void write_cells_polygon_d(const FpArgs& A, const UntravScratch& S, int nrows, int a0, int cnt, int reps, const UntravOut& O,
+                                      int q) {
+  int* cout = O.count + q;
+  double* xy = O.xy + 2 * (size_t)O.maxv * q;
+  if (cnt >= 4 || (cnt >= 2 && reps >= 2)) {
+    const int nv = table_chain_d(A, S.tmin, S.tmax, nrows, a0, S.stack);
+    *cout = nv;
+    for (int v = 0; v < min(nv, O.maxv); ++v) {
+      xy[2 * v] = A.X[a0 + S.stack[v].x];
+      xy[2 * v + 1] = A.Y[S.stack[v].y];
+    }
+    return;
+  }
+  const int nv = (cnt == 1 && reps >= 2) ? 2 + (reps & 1) : cnt;
+  *cout = nv;
+  for (int v = 0; v < min(nv, O.maxv); ++v) {
+    const int2 c = S.first[cnt == 1 ? 0 : v];
+    xy[2 * v] = A.X[c.x];
+    xy[2 * v + 1] = A.Y[c.y];
+  }
+}
+
+// isTraversable's spiral walk with computeUntraversablePolygon on an untraversable circle (:687-729): the first blocked cell lies
+// within rmin, so the walk goes to the end of the spiral and collects every blocked cell with uR <= rmin (every blocked cell when
+// rmin == 0); later blocked cells of the annulus are skipped (:705).  Membership as in fresh_circle_d.  Table row r = map row
+// ci - nr + r.  Returns the number of collected cells.  Warp-uniform.
+__device__ int spiral_blockers_d(const FpArgs& A, const Layers& L, const PathArgs& P, const UntravScratch& S, double cx, double cy,
+                                 int ci, int cj, double rmin, double rmax, int nr) {
+  const int lane = threadIdx.x & 31;
+  const double r2 = rmax * rmax;
+  const int end = __ldg(P.ring_start + nr + 1), edge0 = __ldg(P.ring_start + max(nr - 1, 1));
+  clear_table_d(S, 2 * nr + 1);
+  int cnt = 0;
+  for (int base = 0; base < end; base += 32) {
+    const int k = base + lane;
+    bool take = false;
+    int a = 0, b = 0;
+    if (k < end) {
+      const int w = __ldg(P.rings + k);
+      const int di = (int)(signed char)(w & 0xff), dj = (int)(signed char)((w >> 8) & 0xff);
+      a = ci + di;
+      b = cj + dj;
+      bool member = false;
+      if (a >= 0 && b >= 0 && a < A.rows && b < A.cols_total) {
+        member = true;
+        if (k >= edge0) {
+          const double dx = A.X[a] - cx, dy = A.Y[b] - cy;
+          member = dx * dx + dy * dy <= r2;
+        }
+      }
+      take = member && blocked_memo_d(A, L, P.memo, a, b) && (rmin == 0.0 || current_radius_d(A, di, dj) <= rmin);
+    }
+    collect_cells_d(S, take, a, b, ci - nr, cnt);
+  }
+  __syncwarp();
+  return cnt;
+}
+
+// grid_map::Polygon::fromCircle(center, radius) (recalled): vertex j = center + Rotation2D(j * 2 * M_PI / 19) * (radius, 0); the
+// 20 cosines and sines come from the host's libm (launch_check_paths_fresh).  A single pose publishes it as it is; a segment
+// hulls it: 20 points, so every later convexHull with it is the same chain (see write_cells_polygon_d).  One thread.
+__device__ void write_circle_polygon_d(const double* cs, const double* sn, double cx, double cy, double radius, bool hulled,
+                                       double2* pts, const UntravOut& O, int q) {
+  const int nc = kFromCircleVertices;
+  double2* hull = pts + nc;
+  for (int j = 0; j < nc; ++j) {  // insertion sort into lexicographic order (equal points are equal values: order is irrelevant)
+    const double2 v = make_double2(cx + cs[j] * radius, cy + sn[j] * radius);
+    int i = j;
+    while (hulled && i > 0 && lex_less_d(v, pts[i - 1])) { pts[i] = pts[i - 1]; --i; }
+    pts[i] = v;
+  }
+  const int nv = hulled ? monotone_chain_d(pts, nc, hull) : nc;
+  const double2* out = hulled ? hull : pts;
+  O.count[q] = nv;
+  double* xy = O.xy + 2 * (size_t)O.maxv * q;
+  for (int v = 0; v < min(nv, O.maxv); ++v) { xy[2 * v] = out[v].x; xy[2 * v + 1] = out[v].y; }
+}
+
+struct CircleTable {
+  double cs[kFromCircleVertices], sn[kFromCircleVertices];
+};
+
+// The body of k_check_paths_fresh; POLY also produces the untraversable polygon (k_check_paths_fresh_poly).
+template <bool POLY>
+__device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layers& L, const PathArgs& P, const UntravOut& O,
+                                                    const CircleTable& C, const UntravScratch& S) {
   const int lane = threadIdx.x & 31;
   const int q = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   if (q >= P.npaths) return;  // whole warp
@@ -1002,13 +1197,20 @@ __global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, P
   const bool cup = P.cup != nullptr && P.cup[q] != 0;
   const double rings = ceil(rmax / A.res);  // SpiralIterator nRings
   if (!(rmin >= 0.0) || !(rings <= (double)kPathMaxRings)) {  // not checkable here: marked so that no checked result looks alike
-    if (lane == 0) { P.is_safe[q] = 0; P.trav_out[q] = nan(""); }
+    if (lane == 0) {
+      P.is_safe[q] = 0; P.trav_out[q] = nan("");
+      if (POLY) O.count[q] = cup ? -1 : 0;
+    }
     return;
   }
   const int nr = (int)rings;
   double result = 0.0, lengthPath = 0.0;
   double sx = 0.0, sy = 0.0, ex = 0.0, ey = 0.0;
   bool ok = n > 0;  // :330-334
+  // POLY: the circle that made the path fail and how often its polygon is hulled into the published one
+  int fkind = 0;  // 0: nothing published, 1: fromCircle(centre, rmax), 2: hull of the spiral's blocked cells
+  double fx = 0.0, fy = 0.0;
+  int fi = 0, fj = 0, freps = 1;
   for (int k = 0; k < n && ok; ++k) {
     sx = ex; sy = ey;
     ex = P.xy[2 * (b + k)]; ey = P.xy[2 * (b + k) + 1];
@@ -1018,10 +1220,12 @@ __global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, P
       if (!is_inside_d(A, ex, ey) || !get_index_d(A, ex, ey, i, j)) {  // :662-667
         result = A.tdefault;
         ok = A.tdefault != 0.0;
+        if (POLY && !ok) { fkind = 1; fx = ex; fy = ey; }
       } else {
         const FreshCircle f = fresh_circle_d(A, L, P, ex, ey, i, j, rmin, rmax, nr, cup);
         ok = f.ok;
         result = f.t;
+        if (POLY && !ok) { fkind = 2; fx = ex; fy = ey; fi = i; fj = j; }
       }
     }
     if (n > 1 && k > 0) {  // :389-457
@@ -1044,13 +1248,18 @@ __global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, P
           get_index_d(A, P.xy[2 * (b + s)], P.xy[2 * (b + s) + 1], pi1, pj1);
           seen = seen || line_checks_d(pi1, pj1, pi0, pj0, a, bb);
         }
-        if (__any_sync(0xffffffffu, seen)) {
+        const bool cached = __any_sync(0xffffffffu, seen);
+        if (cached) {
           ok = f.cache != 0.0f;
           sum += (double)f.cache;
         } else {
           ok = f.ok;
           sum += f.t;
         }
+        // POLY: a cached 0 publishes fromCircle of the cell centre (:673-678), a walked circle the hull of its blocked cells.  The
+        // failing circle's polygon is hulled into the path's once for itself and once per later checked cell of the line
+        // (:407-412: the && skips isTraversable, the auxiliary polygon stays).
+        if (POLY && !ok) { fkind = cached ? 1 : 2; fx = A.X[a]; fy = A.Y[bb]; fi = a; fj = bb; freps = (line.n - 1) / 4 - c / 4 + 1; }
         ++nLine;
       }
       if (!ok) break;  // :414-417, :453-456
@@ -1061,6 +1270,33 @@ __global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, P
     P.is_safe[q] = ok ? 1 : 0;
     P.trav_out[q] = ok ? result : 0.0;
   }
+  if (POLY) {
+    // the last non-empty polygon published for the path: only an untraversable circle has one (inclination failures return first)
+    if (!cup || ok || fkind == 0) {
+      if (lane == 0) O.count[q] = 0;
+    } else if (fkind == 1) {
+      if (lane == 0) write_circle_polygon_d(C.cs, C.sn, fx, fy, rmax, n > 1, reinterpret_cast<double2*>(S.stack), O, q);
+    } else {
+      const int cnt = spiral_blockers_d(A, L, P, S, fx, fy, fi, fj, rmin, rmax, nr);
+      if (lane == 0) write_cells_polygon_d(A, S, 2 * nr + 1, fi - nr, cnt, freps, O, q);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, PathArgs P) {
+  check_paths_fresh_d<false>(A, L, P, UntravOut{}, CircleTable{}, UntravScratch{});
+}
+
+// k_check_paths_fresh that also returns the untraversable polygon of every path (te_check_footprint_paths_fresh2).  Per warp:
+// a row table for the 2 * 127 + 1 rows of the largest spiral and the chain stack.
+constexpr int kFreshTableRows = 2 * kPathMaxRings + 1;
+__global__ void __launch_bounds__(128) k_check_paths_fresh_poly(FpArgs A, Layers L, PathArgs P, UntravOut O, CircleTable C) {
+  __shared__ int s_min[4][kFreshTableRows + 1], s_max[4][kFreshTableRows + 1];
+  __shared__ int2 s_stack[4][2 * kFreshTableRows + 4];
+  __shared__ int2 s_first[4][3];
+  static_assert(sizeof(s_stack[0]) >= 3 * kFromCircleVertices * sizeof(double2), "fromCircle points and hull fit the stack");
+  const int w = threadIdx.x >> 5;
+  check_paths_fresh_d<true>(A, L, P, O, C, UntravScratch{s_min[w], s_max[w], s_stack[w], s_first[w]});
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -1135,36 +1371,40 @@ __device__ __forceinline__ bool polygon_inside_d(const double2* v, int n, double
   return (cross & 1) != 0;
 }
 
-__device__ __forceinline__ bool lex_less_d(double2 a, double2 b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
+// The untraversable polygons of the polygonal path check (k_check_polygon_items_poly / k_check_polygon_combine_poly).
+struct PolyUntravArgs {
+  const unsigned char* cup;  // FootprintPath.compute_untraversable_polygon per path, nullptr: all 0
+  int* item_count;           // [nposes]: the item's vertex count (-1: its bounding box spans more than kUntravRows rows)
+  double* item_xy;           // [nposes][maxv] (x, y)
+  UntravOut out;             // per path
+};
 
-// grid_map::Polygon::monotoneChainConvexHullOfPoints (recalled) of the m > 3 points `sorted` (already in lexicographic order) into
-// `hull` (2m entries, the reference's own allocation); returns the vertex count.  One thread.
-__device__ int monotone_chain_d(const double2* sorted, int m, double2* hull) {
-  auto clockwise = [](double2 o, double2 a, double2 b) {
-    const double ux = a.x - o.x, uy = a.y - o.y, wx = b.x - o.x, wy = b.y - o.y;
-    return (ux * wy - uy * wx) <= 0;
-  };
-  int k = 0;
-  for (int i = 0; i < m; ++i) {
-    while (k >= 2 && clockwise(hull[k - 2], hull[k - 1], sorted[i])) k--;
-    hull[k++] = sorted[i];
-  }
-  for (int i = m - 2, t = k + 1; i >= 0; i--) {
-    while (k >= t && clockwise(hull[k - 2], hull[k - 1], sorted[i])) k--;
-    hull[k++] = sorted[i];
-  }
-  return k - 1;
+// Dynamic shared memory of one warp of k_check_polygon_items: sA, sB (3 mcap points); with the polygon also its UntravScratch.
+__host__ __device__ inline size_t poly_warp_smem(int mcap, bool poly) {
+  size_t s = sizeof(double2) * 3 * (size_t)mcap;
+  if (poly) s += sizeof(int2) * (2 * kUntravRows + 4 + 4) + sizeof(int) * 2 * kUntravRows;
+  return s;
 }
 
 // One warp per pose index p.  Shared memory per warp: sA (2 mcap points: the hull input polygon1 ++ polygon2, then the hull) and
-// sB (mcap points: a conservative path's earlier polygon2, then the sorted hull input).
-__global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L, PolyPathArgs P) {
+// sB (mcap points: a conservative path's earlier polygon2, then the sorted hull input).  POLY: with compute_untraversable_polygon
+// set for the item's path, the walk goes on past blocked cells and collects them (:602-608, :634-638).
+template <bool POLY>
+__device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Layers& L, const PolyPathArgs& P, const PolyUntravArgs& U) {
   extern __shared__ double2 sPoly[];
   const int lane = threadIdx.x & 31;
   const int p = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   if (p >= P.nposes) return;  // whole warp
-  double2* sA = sPoly + (size_t)(threadIdx.x >> 5) * 3 * P.mcap;
+  double2* sA = POLY ? reinterpret_cast<double2*>(reinterpret_cast<char*>(sPoly) + (threadIdx.x >> 5) * poly_warp_smem(P.mcap, true))
+                     : sPoly + (size_t)(threadIdx.x >> 5) * 3 * P.mcap;
   double2* sB = sA + 2 * P.mcap;
+  UntravScratch S{};
+  if (POLY) {
+    S.stack = reinterpret_cast<int2*>(sB + P.mcap);
+    S.first = S.stack + 2 * kUntravRows + 4;
+    S.tmin = reinterpret_cast<int*>(S.first + 4);
+    S.tmax = S.tmin + kUntravRows;
+  }
   PolyItem it{-1, 2, 0.0, 0.0, 0.0};
   // the path of pose p: the last q with path_begin[q] <= p
   int lo = 0, hi = P.npaths - 1;
@@ -1178,6 +1418,10 @@ __global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L,
     return;
   }
   it.q = q;
+  const bool cup = POLY && U.cup != nullptr && U.cup[q] != 0;
+  int ncollected = 0;  // POLY: blocked cells collected by the walk
+  bool hit = false;    // POLY: the walk stopped at a blocked cell without collecting
+  int nr_walk = 0, si_walk = 0;
   const int nfp = P.nfp;
   const bool cons = n > 1 && P.cons != nullptr && P.cons[q] != 0;
   const int m = n == 1 ? nfp : cons ? 2 * nfp * (k + 1) : 2 * nfp;  // points of polygon1 ++ polygon2
@@ -1265,12 +1509,17 @@ __global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L,
     const int nr = ei - si + 1, nc = ej - sj + 1;
     const long long total = (nr > 0 && nc > 0) ? (long long)nr * nc : 0;
     unsigned cnt = 0;
+    // POLY: collect the blocked cells (table row = map row - si) unless the bounding box has more rows than the table
+    const bool collect = POLY && cup && nr <= kUntravRows;
+    if (POLY && collect) { clear_table_d(S, nr); nr_walk = nr; si_walk = si; }
     for (long long base = 0; base < total; base += 32) {  // SubmapIterator order, 32 cells per pass; the sum in visit order
       const long long c = base + lane;
       bool member = false, blk = false;
       double v = 0.0;
+      int a = 0, bb = 0;
       if (c < total) {
-        const int a = si + (int)(c / nc), bb = sj + (int)(c % nc);
+        a = si + (int)(c / nc);
+        bb = sj + (int)(c % nc);
         if (a >= 0 && bb >= 0 && a < A.rows && bb < A.cols_total && polygon_inside_d(sA, nh, A.X[a], A.Y[bb])) {
           member = true;
           blk = blocked_memo_d(A, L, P.memo, a, bb);
@@ -1280,7 +1529,11 @@ __global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L,
           }
         }
       }
-      if (__any_sync(0xffffffffu, blk)) { ok = false; break; }  // :602-611
+      if (POLY && collect) {
+        collect_cells_d(S, blk, a, bb, si, ncollected);
+        if (ncollected > 0) { ok = false; continue; }  // no sum is read after the first blocked cell
+      }
+      if (__any_sync(0xffffffffu, blk)) { ok = false; if (POLY) hit = true; break; }  // :602-611
       const unsigned take = __ballot_sync(0xffffffffu, member);
       cnt += __popc(take);
 #pragma unroll
@@ -1303,13 +1556,35 @@ __global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L,
     it.mean = t;
     P.items[p] = it;
   }
+  if (POLY && cup) {
+    // isTraversable's polygon (:634-642): empty when traversable or when nothing was collected (checkInclination failed first, or
+    // no cell centre is inside and traversability_default is 0); 3 cells or fewer in visit order; else the chain
+    __syncwarp();
+    if (lane == 0) {
+      const UntravOut O{U.out.maxv, U.item_count, U.item_xy};
+      if (hit) *(O.count + p) = -1;  // more bounding-box rows than the table holds
+      else write_cells_polygon_d(A, S, nr_walk, si_walk, ncollected, 1, O, p);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L, PolyPathArgs P) {
+  check_polygon_item_d<false>(A, L, P, PolyUntravArgs{});
+}
+
+__global__ void __launch_bounds__(128) k_check_polygon_items_poly(FpArgs A, Layers L, PolyPathArgs P, PolyUntravArgs U) {
+  check_polygon_item_d<true>(A, L, P, U);
 }
 
 // One thread per path: the area-weighted combination of the segment results in path order (:522-579).  An unsafe path reports 0;
-// a path the items could not check (bad range, non-finite pose, conservative list past the cap) is_safe 0 and NaN.
-__global__ void __launch_bounds__(128) k_check_polygon_combine(PolyPathArgs P) {
+// a path the items could not check (bad range, non-finite pose, conservative list past the cap) is_safe 0 and NaN.  POLY: the
+// polygon of the item that failed (the reference publishes every segment's polygon and returns after the first failing one,
+// :555-567; traversable segments publish nothing); -1 for a path the items could not check.
+template <bool POLY>
+__device__ __forceinline__ void check_polygon_combine_d(const PolyPathArgs& P, const PolyUntravArgs& U) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= P.npaths) return;
+  int failed = -1;  // POLY: pose index of the failing item
   const int b = P.path_begin[q], e = P.path_begin[q + 1], n = e - b;
   bool checkable = b >= 0 && e >= b && e <= P.nposes;
   unsigned char safe = 0;
@@ -1325,7 +1600,7 @@ __global__ void __launch_bounds__(128) k_check_polygon_combine(PolyPathArgs P) {
       for (int k = k0; k < n && ok; ++k) {
         const PolyItem it = P.items[b + k];
         ok = it.flag == 1;
-        if (!ok) break;  // :536-538, :564-567
+        if (!ok) { if (POLY) failed = b + k; break; }  // :536-538, :564-567
         if (n == 1 || k == 1) {  // :541-542, :576-578
           area = it.hull_area;
           trav = it.mean;
@@ -1344,7 +1619,19 @@ __global__ void __launch_bounds__(128) k_check_polygon_combine(PolyPathArgs P) {
   P.is_safe[q] = safe;
   P.trav_out[q] = trav;
   P.area_out[q] = area;
+  if (POLY) {
+    const bool cup = U.cup != nullptr && U.cup[q] != 0;
+    const int nv = !cup ? 0 : !checkable ? -1 : failed >= 0 ? U.item_count[failed] : 0;
+    U.out.count[q] = nv;
+    const double* src = U.item_xy + 2 * (size_t)U.out.maxv * (failed >= 0 ? failed : 0);
+    double* dst = U.out.xy + 2 * (size_t)U.out.maxv * q;
+    for (int v = 0; v < 2 * min(nv, U.out.maxv); ++v) dst[v] = src[v];
+  }
 }
+
+__global__ void __launch_bounds__(128) k_check_polygon_combine(PolyPathArgs P) { check_polygon_combine_d<false>(P, PolyUntravArgs{}); }
+
+__global__ void __launch_bounds__(128) k_check_polygon_combine_poly(PolyPathArgs P, PolyUntravArgs U) { check_polygon_combine_d<true>(P, U); }
 
 inline int signum(int v) { return (0 < v) - (v < 0); }
 
@@ -1384,7 +1671,7 @@ std::vector<int> build_spiral(double radius, double res) {
 }  // namespace
 
 void FootprintState::release() {
-  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly[0], &poly[1], &rings, &memo, &items}) b->release();
+  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly[0], &poly[1], &rings, &memo, &items, &upoly}) b->release();
   tables_valid = false;
   valid = false;
 }
@@ -1440,7 +1727,7 @@ int reset_filter_memo(FootprintState& st, const SlabView& v, cudaStream_t s) {
 int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
                              const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
                              int npaths, const int* path_begin, const double* xy, const double* radius, const unsigned char* cup,
-                             unsigned char* is_safe, double* trav_out, cudaStream_t s) {
+                             unsigned char* is_safe, double* trav_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s) {
   if (!st.rings.p) {  // rings 0 .. kPathMaxRings once per context: the visit order inside a ring does not depend on the radius
     std::vector<int> ring_start;
     const std::vector<int> sp = spiral_rings(kPathMaxRings, ring_start);
@@ -1465,7 +1752,17 @@ int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geo
   P.memo = (unsigned char*)st.memo.p;
   P.is_safe = is_safe; P.trav_out = trav_out;
   const long long threads = 32LL * npaths;
-  k_check_paths_fresh<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P);
+  if (!ucount) {
+    k_check_paths_fresh<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P);
+    return 0;
+  }
+  CircleTable C{};
+  for (int j = 0; j < kFromCircleVertices; ++j) {  // Polygon::fromCircle: theta = j * 2 * M_PI / (nVertices - 1)
+    volatile double theta = j * 2 * M_PI / (kFromCircleVertices - 1);  // volatile: libm at run time, never a folded constant
+    C.cs[j] = std::cos(theta);
+    C.sn[j] = std::sin(theta);
+  }
+  k_check_paths_fresh_poly<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P, UntravOut{max_vertices, ucount, uxy}, C);
   return 0;
 }
 
@@ -1473,7 +1770,8 @@ int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_g
                                const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
                                int nfp, const float* footprint_xyz, int npaths, int nposes, const int* path_begin, const double* poses,
                                const unsigned char* conservative, int max_points, unsigned char* is_safe, double* trav_out,
-                               double* area_out, cudaStream_t s, int* launches) {
+                               double* area_out, const unsigned char* cup, int max_vertices, int* ucount, double* uxy,
+                               cudaStream_t s, int* launches) {
   *launches = 0;
   if (nfp < 1 || nfp > kPolyMaxVerts || max_points < 2 * nfp || max_points > 2 * kPolyConsCap) { st.why = "bad footprint size"; return TE_ERR_BAD_ARG; }
   if (int rc = reset_filter_memo(st, v, s)) return rc;
@@ -1489,6 +1787,35 @@ int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_g
   P.is_safe = is_safe; P.trav_out = trav_out; P.area_out = area_out;
   for (int k = 0; k < nfp; ++k) {
     P.fx[k] = footprint_xyz[3 * k]; P.fy[k] = footprint_xyz[3 * k + 1]; P.fz[k] = footprint_xyz[3 * k + 2];
+  }
+  if (ucount) {  // the untraversable polygons: per item a count and max_vertices points, copied to the paths by the combine kernel
+    PolyUntravArgs U{};
+    U.cup = cup;
+    U.out = UntravOut{max_vertices, ucount, uxy};
+    const size_t cbytes = (sizeof(int) * nitems + 15) / 16 * 16;
+    if (st.upoly.reserve(cbytes + sizeof(double2) * nitems * (size_t)std::max(max_vertices, 1)) != cudaSuccess) {
+      st.why = "allocating the untraversable polygons failed";
+      return TE_ERR_CUDA;
+    }
+    U.item_count = (int*)st.upoly.p;
+    U.item_xy = (double*)((char*)st.upoly.p + cbytes);
+    if (nposes > 0) {
+      // four warps per block while their shared memory stays below 100 KB; one warp per block for long conservative paths
+      const size_t per_warp = poly_warp_smem(max_points, true);
+      const int wpb = per_warp * 4 <= 100 * 1024 ? 4 : 1;
+      const size_t smem = per_warp * wpb;
+      if (smem > 48 * 1024 &&
+          cudaFuncSetAttribute(k_check_polygon_items_poly, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+        st.why = "cudaFuncSetAttribute(k_check_polygon_items_poly) failed";
+        return TE_ERR_CUDA;
+      }
+      const long long blocks = ((long long)nposes + wpb - 1) / wpb;
+      k_check_polygon_items_poly<<<(unsigned)blocks, 32 * wpb, smem, s>>>(a, L, P, U);
+      ++*launches;
+    }
+    k_check_polygon_combine_poly<<<(unsigned)((npaths + 127) / 128), 128, 0, s>>>(P, U);
+    ++*launches;
+    return 0;
   }
   if (nposes > 0) {
     // four warps per block while their shared memory stays small; one warp per block for long conservative paths

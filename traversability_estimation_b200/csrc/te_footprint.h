@@ -30,6 +30,7 @@ struct FootprintState {
   DevBuf rings;   // fresh path checks: ring starts + SpiralIterator visit order of rings 0..127 (built once)
   DevBuf memo;    // fresh and polygonal path checks: per-cell isTraversableForFilters memo of one call
   DevBuf items;   // polygonal path checks: one result record per pose index
+  DevBuf upoly;   // polygonal path checks with untraversable polygons: per pose index a vertex count and max_vertices points
   void invalidate() { valid = false; tables_valid = false; }
   void release();
 };
@@ -51,21 +52,26 @@ void launch_check_paths(const SlabView& v, const te_geometry* g, double traversa
                         const int* path_begin, const double* xy, unsigned char* is_safe, double* trav, cudaStream_t s);
 
 // The same on the chain layers with an empty traversability_footprint cache per path (te_check_footprint_paths_fresh); whole map,
-// device pointers, radius / compute_untraversable_polygon per path.  Asynchronous on `s`.
+// device pointers, radius / compute_untraversable_polygon per path.  Asynchronous on `s`.  `ucount` != nullptr: also the
+// untraversable polygon of every path (vertex count, up to `max_vertices` points in `uxy`; te_check_footprint_paths_fresh2).
 int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
                              const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
                              int npaths, const int* path_begin, const double* xy, const double* radius, const unsigned char* cup,
-                             unsigned char* is_safe, double* trav_out, cudaStream_t s);
+                             unsigned char* is_safe, double* trav_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s);
 
 // TraversabilityMap::checkPolygonalFootprintPath for a batch of paths sharing one footprint (te_check_footprint_paths_polygon);
 // whole map, device pointers except `footprint_xyz` (host, nfp x 3 floats).  `max_points` bounds the hull input of one item
 // (polygon1 ++ polygon2): 2 * nfp without conservative paths, 2 * nfp * (poses of the longest conservative path) otherwise.
 constexpr int kPolyMaxVerts = 16;   // footprint vertices
 constexpr int kPolyConsCap = 1024;  // vertices of a conservative path's polygon2 (nfp * poses up to the segment)
+// `ucount` != nullptr: also the untraversable polygon of every path with cup[q] set (te_check_footprint_paths_polygon2); an item
+// whose bounding box spans more than kUntravRows map rows cannot build it (shared-memory row table): its path gets count -1.
+constexpr int kUntravRows = 1024;
 int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
                                const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
                                int nfp, const float* footprint_xyz, int npaths, int nposes, const int* path_begin, const double* poses,
                                const unsigned char* conservative, int max_points, unsigned char* is_safe, double* trav_out,
-                               double* area_out, cudaStream_t s, int* launches);
+                               double* area_out, const unsigned char* cup, int max_vertices, int* ucount, double* uxy,
+                               cudaStream_t s, int* launches);
 
 }  // namespace te
