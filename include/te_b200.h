@@ -348,6 +348,40 @@ int te_check_footprint_paths_polygon2(te_ctx* ctx, const te_geometry* g, const t
                                       double* area_out, const uint8_t* compute_untraversable_polygon_or_null, int32_t max_vertices,
                                       int32_t* untraversable_count_or_null, double* untraversable_xy_or_null, int memory);
 
+/* A whole CheckFootprintPath request (TraversabilityEstimation.cpp:278-295) in one call: FootprintPath[] with circular and
+ * polygonal paths mixed, each with its own footprint, results in request order.  Path q is circular when its footprint has no
+ * vertices (checkFootprintPath, TraversabilityMap.cpp:320-343: any non-empty polygon takes the polygonal branch) and gets, bit for
+ * bit, what te_check_footprint_paths_fresh2 gives for it alone with radius[q] and compute_untraversable_polygon[q]; its area is 0,
+ * as in the reference's result.  Otherwise it gets what te_check_footprint_paths_polygon2 gives for it alone with its own
+ * footprint, conservative[q] and compute_untraversable_polygon[q]; radius[q] is then ignored, as FootprintPath.radius is.
+ * Everything those two entries document carries over per kind of path: layers and `p`, empty paths, poses outside the map,
+ * robot_slope, the empty traversability_footprint cache per path, the deviation that an unsafe path reports 0, the 127-ring,
+ * conservative-cap and 1024-row limits, the untraversable polygon outputs (max_vertices, count, xy slots) and, in TE_MEM_HOST, a
+ * circular-buffer start index.  New here:
+ *   - poses = 7 doubles per pose (x y z qx qy qz qw) for both kinds; a circular path reads x and y only.  Path q = poses
+ *     path_begin[q] .. path_begin[q+1]-1, nposes = path_begin[npaths];
+ *   - footprint_xyz = nvertices vertices x, y, z as float32; path q's footprint = vertices footprint_begin[q] ..
+ *     footprint_begin[q+1]-1 (0: circular, 1..16: polygonal).  Unlike te_check_footprint_paths_polygon2's footprint these arrays
+ *     follow `memory`;
+ *   - max_footprint_vertices (0..16) bounds every footprint and sizes the polygonal kernel's shared memory;
+ *   - one call uploads the layers once (TE_MEM_HOST) and clears one isTraversableForFilters memo, which both kinds of path share
+ *     (it depends on the layers only, so sharing it changes no result).
+ * Errors: those of the two entries, applied to each kind of path (TE_ERR_BAD_ARG for p->offset < 0 always); TE_ERR_BAD_ARG for
+ * max_footprint_vertices outside 0..16, null or negative arguments (footprint_xyz may be null when nvertices is 0), and in
+ * TE_MEM_HOST for a footprint_begin that does not start at 0, decreases or does not end at nvertices, a footprint with more
+ * vertices than max_footprint_vertices, and a non-finite vertex.  TE_MEM_DEVICE is asynchronous on the context stream and
+ * cannot read the paths: a path whose footprint cannot be checked (over max_footprint_vertices, outside the vertex array, a
+ * non-finite vertex), or that its own entry could not check, gets is_safe = 0, NaN in traversability and area, and count -1
+ * where its polygon was requested; the other paths are unaffected. */
+int te_check_footprint_request(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, const float* traversability,
+                               const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                               const float* robot_slope_or_null, int32_t npaths, int32_t nposes, const int32_t* path_begin,
+                               const double* poses, const double* radius, int32_t nvertices, const int32_t* footprint_begin,
+                               const float* footprint_xyz, int32_t max_footprint_vertices, const uint8_t* conservative_or_null,
+                               const uint8_t* compute_untraversable_polygon_or_null, uint8_t* is_safe, double* traversability_out,
+                               double* area_out, int32_t max_vertices, int32_t* untraversable_count_or_null,
+                               double* untraversable_xy_or_null, int memory);
+
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the
  * neighbours' boundary columns of the INPUT layer(s) into this rank's halo.  The reference has no counterpart (it is a

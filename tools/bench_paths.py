@@ -18,6 +18,12 @@ isTraversableForFilters pass, which the GPU evaluates only where a polygon looks
 --untraversable times te_check_footprint_paths_fresh2 (radius 0.3 m) and te_check_footprint_paths_polygon2 (YAML footprint) in
 TE_MEM_DEVICE with compute_untraversable_polygon off and on for every path (room for 256 vertices per path), next to the CPU
 oracle of the same calls (tests/untraversable_oracle.cpp; all host threads, one run).
+
+--request times te_check_footprint_request against the calls a node makes without it: te_check_footprint_paths_fresh on the
+circular paths and te_check_footprint_paths_polygon once per distinct footprint.  Every other path is circular (radius 0.3 m,
+offset 0.15 m), the rest polygonal over 1 or 4 distinct footprints, with a random yaw per pose.  Both in TE_MEM_DEVICE (CUDA
+events; the split calls write one output set each and nothing is scattered back) and in TE_MEM_HOST (host clock around the
+call, which ends in a synchronise; the split calls upload the layers once per call).  Outputs of the two are compared bit for bit.
 """
 from __future__ import annotations
 
@@ -68,7 +74,10 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--footprint", choices=("circle", "polygon"), default="circle")
     ap.add_argument("--untraversable", action="store_true")
+    ap.add_argument("--request", action="store_true")
     args = ap.parse_args()
+    if args.request:
+        return main_request(args)
     if args.untraversable:
         return main_untraversable(args)
     if args.footprint == "polygon":
@@ -287,6 +296,134 @@ def main_untraversable(args):
                                   "gpu_median_ms": med, "gpu_min_ms": mn, "cpu_oracle_ms": cpu_ms, "cpu_threads": os.cpu_count(),
                                   "safe": int(safe.sum().item()), "polygons": int((got > 0).sum()),
                                   "counts_match_oracle": bool(np.array_equal(got, want_counts))}), flush=True)
+    ctx.set_stream(None)
+    ctx.close()
+
+
+def request_footprints(k):
+    """k distinct footprints (1 or 4): the YAML rectangle, then a smaller rectangle, a hexagon and an octagon."""
+    ring = lambda m, r: [(r * np.cos(2 * np.pi * i / m), r * np.sin(2 * np.pi * i / m), 0.0) for i in range(m)]  # noqa: E731
+    fps = [YAML_FOOTPRINT, [(0.35, 0.25, 0.0), (0.35, -0.25, 0.0), (-0.35, -0.25, 0.0), (-0.35, 0.25, 0.0)], ring(6, 0.4), ring(8, 0.45)]
+    return [np.asarray(f, np.float32) for f in fps[:k]]
+
+
+def main_request(args):
+    import time
+    import torch
+    import synth
+    import traversability_estimation_b200 as te
+
+    n, res = args.size, 0.02
+    g = te.Geometry.make(n, n, res)
+    fp = te.FootprintParams.yaml_defaults()            # offset 0.15
+    ctx = te.Context(0)
+    z = synth.terrain(n, n, res, 4096, "mixed")
+    layers = ctx.chain_host(g, te.ChainParams.yaml_defaults(0), z)
+    host = {k: np.asfortranarray(a, np.float32) for k, a in (("trav", layers["traversability"]), ("slope", layers["slope"]),
+                                                             ("step", layers["step"]), ("elev", z))}
+    dev = lambda a: torch.from_numpy(np.ascontiguousarray(a.T)).cuda()  # noqa: E731
+    dl = {k: dev(a) for k, a in host.items()}
+    stream = torch.cuda.Stream()
+    ctx.set_stream(stream.cuda_stream)
+    name, power = gpu_info(torch)
+    rng = np.random.default_rng(1)
+
+    def timed(run, device):
+        for _ in range(args.warmup):
+            run()
+        stream.synchronize()
+        ts = []
+        for _ in range(args.reps):
+            if device:
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                run()
+                e1.record(stream)
+                e1.synchronize()
+                ts.append(e0.elapsed_time(e1))
+            else:   # host memory: every call ends in a synchronise of the context stream
+                t0 = time.perf_counter()
+                run()
+                ts.append((time.perf_counter() - t0) * 1e3)
+        return float(np.median(ts)), float(np.min(ts))
+
+    for batch in (1, 100, 1000):
+        begin, xy = planner_paths(rng, n, batch, res)
+        yaw = rng.uniform(0, 2 * np.pi, len(xy))
+        poses = np.stack([xy[:, 0], xy[:, 1], np.zeros(len(xy)), np.zeros(len(xy)), np.zeros(len(xy)), np.sin(yaw / 2),
+                          np.cos(yaw / 2)], axis=1)
+        for nfps in (1, 4):
+            fps = request_footprints(nfps)
+            kind = np.where(np.arange(batch) % 2 == 1, -1, (np.arange(batch) // 2) % nfps)   # odd paths circular
+            fbeg = np.concatenate([[0], np.cumsum([0 if k < 0 else len(fps[k]) for k in kind])]).astype(np.int32)
+            fxyz = np.concatenate([fps[k] for k in kind if k >= 0] + [np.zeros((0, 3), np.float32)])
+            radius = np.full(batch, 0.3)
+            groups = []   # (path indices, path_begin, poses) of the calls a node makes today: circular first, then per footprint
+            for k in range(-1, nfps):
+                idx = np.nonzero(kind == k)[0]
+                if len(idx):
+                    b = np.concatenate([[0], np.cumsum(begin[idx + 1] - begin[idx])]).astype(np.int32)
+                    groups.append((k, idx, b, np.concatenate([poses[begin[q]:begin[q + 1]] for q in idx])))
+            row = {"gpu": name, "power_limit_w": power, "map": f"{n}x{n}", "resolution": res, "paths": batch,
+                   "poses": int(begin[-1]), "circular": int((kind < 0).sum()), "distinct_footprints": nfps, "calls_split": len(groups)}
+
+            # host memory: numpy in, numpy out
+            def req_host():
+                return ctx.check_footprint_request(g, fp, host["trav"], host["slope"], host["step"], host["elev"], begin, poses,
+                                                   radius, fbeg, fxyz)
+
+            def split_host():
+                out = [np.zeros(batch, np.uint8), np.zeros(batch), np.zeros(batch)]
+                for k, idx, b, p in groups:
+                    if k < 0:
+                        r = ctx.check_footprint_paths_fresh(g, fp, host["trav"], host["slope"], host["step"], host["elev"], b,
+                                                            p[:, :2].copy(), radius[idx])
+                        r = (r[0], r[1], np.zeros(len(idx)))
+                    else:
+                        r = ctx.check_footprint_paths_polygon(g, fp, host["trav"], host["slope"], host["step"], host["elev"], fps[k], b, p)
+                    for o, v in zip(out, r):
+                        o[idx] = v
+                return out
+
+            got, want = req_host(), split_host()
+            row["identical"] = all(np.array_equal(a.view(np.uint8), b.view(np.uint8)) for a, b in zip(got, want))
+            row["host_request_ms"], row["host_request_min_ms"] = timed(req_host, False)
+            row["host_split_ms"], row["host_split_min_ms"] = timed(split_host, False)
+
+            # device memory: tensors in, preallocated tensors out; the split writes one output set per call (no scatter timed)
+            d = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
+            db, dp, dr, dfb, dfx = d(begin), d(poses), d(radius), d(fbeg), d(fxyz)
+            outs = lambda m: dict(is_safe=torch.empty(m, dtype=torch.uint8, device="cuda"),  # noqa: E731
+                                  traversability_out=torch.empty(m, dtype=torch.float64, device="cuda"))
+            rout = dict(outs(batch), area_out=torch.empty(batch, dtype=torch.float64, device="cuda"))
+            dgroups = []
+            for k, idx, b, p in groups:
+                o = outs(len(idx))
+                if k >= 0:
+                    o["area_out"] = torch.empty(len(idx), dtype=torch.float64, device="cuda")
+                dgroups.append((k, d(b), d(p[:, :2]) if k < 0 else d(p), d(radius[idx]), o))
+            mfv = max([len(f) for f in fps])
+            torch.cuda.synchronize()
+
+            def req_dev():
+                ctx.check_footprint_request(g, fp, dl["trav"], dl["slope"], dl["step"], dl["elev"], db, dp, dr, dfb, dfx,
+                                            max_footprint_vertices=mfv, memory=te.MEM_DEVICE, **rout)
+
+            def split_dev():
+                for k, b, p, r, o in dgroups:
+                    if k < 0:
+                        ctx.check_footprint_paths_fresh(g, fp, dl["trav"], dl["slope"], dl["step"], dl["elev"], b, p, r,
+                                                        memory=te.MEM_DEVICE, **o)
+                    else:
+                        ctx.check_footprint_paths_polygon(g, fp, dl["trav"], dl["slope"], dl["step"], dl["elev"], fps[k], b, p,
+                                                          memory=te.MEM_DEVICE, **o)
+
+            row["device_request_ms"], row["device_request_min_ms"] = timed(req_dev, True)
+            row["device_split_ms"], row["device_split_min_ms"] = timed(split_dev, True)
+            stream.synchronize()
+            dev_got = [rout[k].cpu().numpy() for k in ("is_safe", "traversability_out", "area_out")]
+            row["device_identical"] = all(np.array_equal(a.view(np.uint8), b.view(np.uint8)) for a, b in zip(dev_got, want))
+            print(json.dumps(row), flush=True)
     ctx.set_stream(None)
     ctx.close()
 

@@ -74,7 +74,7 @@ struct te_ctx {
   DevBuf dX, dY;
   std::vector<double> hX, hY;
 
-  DevBuf stage[16];          // TE_MEM_HOST staging (handed out in order by Staging)
+  DevBuf stage[20];          // TE_MEM_HOST staging (handed out in order by Staging; te_check_footprint_request takes 18)
   DevBuf worklist, worklist3, counter;  // fused-kernel fix-up lists (tier 2, tier 3) and their counters
   // The counters are two 512-byte blocks used alternately: the last kernel of a chain call (k_fixup_cells) zeroes the block of the
   // NEXT call, so a call needs no cudaMemsetAsync of its own (one stream operation and one launch gap less per map).
@@ -889,6 +889,14 @@ static int check_polygon_outputs(int32_t max_vertices, const int32_t* ucount, co
   return TE_OK;
 }
 
+// The radius of circular path q in host memory: the fresh check walks rings 0 .. 127 of the spiral.
+static int check_circular_radius(const te_geometry* g, const te_footprint_params* p, int32_t q, double radius) {
+  if (!(radius >= 0.0)) return fail(TE_ERR_BAD_ARG, "radius of path %d is negative or NaN", q);
+  if (!(std::ceil((radius + p->offset) / g->resolution) <= 127.0))
+    return fail(TE_ERR_UNSUPPORTED, "radius of path %d + offset spans more than 127 cells", q);
+  return TE_OK;
+}
+
 int te_check_footprint_paths(te_ctx* c, const te_geometry* g, const float* footprint, double traversability_default, int32_t npaths,
                              const int32_t* path_begin, const double* poses_xy, uint8_t* is_safe, double* traversability, int memory) {
   return te_check_footprint_paths2(c, g, footprint, nullptr, traversability_default, npaths, path_begin, poses_xy, is_safe, traversability, memory);
@@ -955,9 +963,7 @@ int te_check_footprint_paths_fresh2(te_ctx* c, const te_geometry* g_in, const te
     if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
     for (int32_t q = 0; q < npaths; ++q) {
       if (path_begin[q + 1] < path_begin[q]) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
-      if (!(radius[q] >= 0.0)) return fail(TE_ERR_BAD_ARG, "radius of path %d is negative or NaN", q);
-      if (!(std::ceil((radius[q] + p->offset) / g->resolution) <= 127.0))
-        return fail(TE_ERR_UNSUPPORTED, "radius of path %d + offset spans more than 127 cells", q);
+      if (int rc = check_circular_radius(g, p, q, radius[q])) return rc;
     }
     nposes = path_begin[npaths];
   }
@@ -1053,6 +1059,98 @@ int te_check_footprint_paths_polygon2(te_ctx* c, const te_geometry* g_in, const 
   if (int r2 = launch_check(c, "polygonal path check", nl)) return r2;
   if (int r2 = st.finish()) return r2;
   if (host && ucount)  // the row bound of the polygon's table (kUntravRows) is only known once the hulls are
+    for (int32_t q = 0; q < npaths; ++q)
+      if (ucount[q] < 0)
+        return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);
+  return TE_OK;
+}
+
+int te_check_footprint_request(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
+                               const float* step, const float* rough, const float* elev, const float* robot_slope, int32_t npaths,
+                               int32_t nposes, const int32_t* path_begin, const double* poses, const double* radius, int32_t nvertices,
+                               const int32_t* footprint_begin, const float* footprint_xyz, int32_t max_footprint_vertices,
+                               const uint8_t* conservative, const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area,
+                               int32_t max_vertices, int32_t* ucount, double* uxy, int memory) {
+  TE_ENTER(c);
+  te_geometry g0;
+  if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
+  const te_geometry* g = &g0;
+  if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
+  if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
+  if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
+  if (npaths < 0 || nposes < 0 || nvertices < 0 || !path_begin || !poses || !radius || !footprint_begin ||
+      (nvertices > 0 && !footprint_xyz) || !is_safe || !traversability || !area)
+    return fail(TE_ERR_BAD_ARG, "null argument or negative count");
+  if (max_footprint_vertices < 0 || max_footprint_vertices > te::kPolyMaxVerts)
+    return fail(TE_ERR_BAD_ARG, "max_footprint_vertices must be 0..%d, got %d", te::kPolyMaxVerts, max_footprint_vertices);
+  if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
+  if (npaths == 0) return TE_OK;
+  const bool use_rough = p->verify_roughness != 0;
+  if (int rc = ensure_geometry(c, g)) return rc;
+  // Device memory reads nothing back: a path that cannot be checked gets is_safe 0, traversability and area NaN.  The hull input
+  // bound of a polygonal item: as te_check_footprint_paths_polygon2 for the largest footprint; host memory sizes it from the paths.
+  const bool host = memory != TE_MEM_DEVICE;
+  int mp = 2 * std::max(max_footprint_vertices, 1);
+  if (conservative && max_footprint_vertices > 0) mp = 2 * te::kPolyConsCap;
+  if (host) {
+    if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
+    if (path_begin[npaths] != nposes) return fail(TE_ERR_BAD_ARG, "path_begin[npaths] = %d != nposes = %d", path_begin[npaths], nposes);
+    if (footprint_begin[0] != 0) return fail(TE_ERR_BAD_ARG, "footprint_begin[0] must be 0, got %d", footprint_begin[0]);
+    if (footprint_begin[npaths] != nvertices)
+      return fail(TE_ERR_BAD_ARG, "footprint_begin[npaths] = %d != nvertices = %d", footprint_begin[npaths], nvertices);
+    for (int32_t q = 0; q < npaths; ++q) {
+      if (path_begin[q + 1] < path_begin[q]) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
+      if (footprint_begin[q + 1] < footprint_begin[q]) return fail(TE_ERR_BAD_ARG, "footprint_begin must be non-decreasing");
+    }
+    mp = 2;
+    for (int32_t q = 0; q < npaths; ++q) {
+      const int32_t n = path_begin[q + 1] - path_begin[q], nfp = footprint_begin[q + 1] - footprint_begin[q];
+      if (nfp == 0) {  // circular: te_check_footprint_paths_fresh2
+        if (int rc = check_circular_radius(g, p, q, radius[q])) return rc;
+        continue;
+      }
+      // polygonal: te_check_footprint_paths_polygon2
+      if (nfp > max_footprint_vertices)
+        return fail(TE_ERR_BAD_ARG, "footprint of path %d has %d vertices, more than max_footprint_vertices = %d", q, nfp,
+                    max_footprint_vertices);
+      mp = std::max(mp, 2 * nfp);
+      if (conservative && conservative[q] && n > 1) {
+        if ((long long)nfp * n > te::kPolyConsCap)
+          return fail(TE_ERR_UNSUPPORTED, "conservative path %d needs %lld polygon vertices, more than %d", q, (long long)nfp * n,
+                      te::kPolyConsCap);
+        mp = std::max(mp, 2 * nfp * n);
+      }
+      for (size_t k = 7 * (size_t)path_begin[q]; k < 7 * (size_t)path_begin[q + 1]; ++k)
+        if (!std::isfinite(poses[k])) return fail(TE_ERR_BAD_ARG, "pose %zu is not finite", k / 7);
+    }
+    for (int k = 0; k < 3 * nvertices; ++k)
+      if (!std::isfinite(footprint_xyz[k])) return fail(TE_ERR_BAD_ARG, "footprint vertex %d is not finite", k / 3);
+  }
+  Staging st(c, host, g_in);
+  const float* in[6] = {st.in_layer(trav, g->cols), st.in_layer(slope, g->cols), st.in_layer(step, g->cols), st.in_layer(elev, g->cols),
+                        st.in_layer(use_rough ? rough : nullptr, g->cols), st.in_layer(robot_slope, g->cols)};
+  const int32_t* dpb = st.in(path_begin, (size_t)npaths + 1);
+  const double* dposes = st.in(poses, 7 * (size_t)nposes);
+  const double* drad = st.in(radius, (size_t)npaths);
+  const int32_t* dfb = st.in(footprint_begin, (size_t)npaths + 1);
+  const float* dfxyz = st.in(footprint_xyz, 3 * (size_t)nvertices);
+  const uint8_t* dcons = st.in(conservative, (size_t)npaths);
+  const uint8_t* dcup = st.in(cup, (size_t)npaths);
+  uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
+  double* dtrav = st.out(traversability, (size_t)npaths);
+  double* darea = st.out(area, (size_t)npaths);
+  int32_t* dcount = st.out(ucount, (size_t)npaths);
+  double* duxy = st.out(uxy, 2 * (size_t)max_vertices * npaths);
+  if (st.rc) return st.rc;
+  const te_slab s{0, g->cols, 0, 0};
+  int nl = 0;
+  int rc = te::launch_check_request(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], in[5], npaths, nposes, dpb, dposes,
+                                    drad, nvertices, dfb, dfxyz, max_footprint_vertices, dcons, dcup, mp, dsafe, dtrav, darea,
+                                    max_vertices, dcount, duxy, c->stream, &nl);
+  if (rc != 0) return fail(rc, "footprint path request failed: %s", c->fp.why.c_str());
+  if (int r2 = launch_check(c, "footprint path request", nl)) return r2;
+  if (int r2 = st.finish()) return r2;
+  if (host && ucount)  // the row bound of a polygonal path's polygon table (kUntravRows) is only known once the hulls are
     for (int32_t q = 0; q < npaths; ++q)
       if (ucount[q] < 0)
         return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);

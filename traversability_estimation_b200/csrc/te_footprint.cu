@@ -1185,20 +1185,47 @@ struct CircleTable {
   double cs[kFromCircleVertices], sn[kFromCircleVertices];
 };
 
-// The body of k_check_paths_fresh; POLY also produces the untraversable polygon (k_check_paths_fresh_poly).
-template <bool POLY>
+// A whole check_footprint_path request (te_check_footprint_request): circular and polygonal paths mixed, each with its own
+// footprint, poses 7 doubles wide for both kinds.  Path q's footprint is vertices fp_begin[q] .. fp_begin[q+1]-1 of fp_xyz: none
+// makes the path circular (the _req variants of k_check_paths_fresh), any other count polygonal (those of k_check_polygon_*).
+// Device memory cannot validate the arrays on the host, so the kernels do (request_footprint_ok_d, the pose range).
+struct RequestArgs {
+  const int* fp_begin;   // [npaths + 1]
+  const float* fp_xyz;   // 3 floats (x, y, z) per vertex
+  int nvertices;         // vertices in fp_xyz
+  int maxfp;             // max_footprint_vertices: a longer footprint is not checked
+  int nposes;
+  double* area_out;      // the area of the circular paths: 0, NaN for a path that is not checked
+};
+
+// Whether path q's footprint can be checked: 1..maxfp vertices inside fp_xyz, all finite (host memory rejects the rest).  The
+// vertex components are read from `first` in steps of `step` (a warp: lane, 32; one thread: 0, 1).
+__device__ __forceinline__ bool request_footprint_ok_d(const RequestArgs& R, int q, int first, int step) {
+  const int fb = R.fp_begin[q], nfp = R.fp_begin[q + 1] - fb;
+  bool ok = nfp >= 1 && nfp <= R.maxfp && fb >= 0 && (long long)fb + nfp <= R.nvertices;
+  for (int c = first; c < 3 * nfp && ok; c += step) ok = isfinite(R.fp_xyz[3 * (size_t)fb + c]);
+  return ok;
+}
+
+// The body of k_check_paths_fresh; POLY also produces the untraversable polygon (k_check_paths_fresh_poly); REQ checks the
+// circular paths of a request (RequestArgs) and leaves its polygonal paths to k_check_polygon_*_req.
+template <bool POLY, bool REQ>
 __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layers& L, const PathArgs& P, const UntravOut& O,
-                                                    const CircleTable& C, const UntravScratch& S) {
+                                                    const CircleTable& C, const UntravScratch& S, const RequestArgs& R) {
+  constexpr int PS = REQ ? 7 : 2;  // doubles per pose; x and y come first
   const int lane = threadIdx.x & 31;
   const int q = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   if (q >= P.npaths) return;  // whole warp
+  if (REQ && R.fp_begin[q + 1] != R.fp_begin[q]) return;  // a polygonal path
   const int b = P.path_begin[q], n = P.path_begin[q + 1] - b;
   const double rmin = P.radius[q], rmax = rmin + P.offset;
   const bool cup = P.cup != nullptr && P.cup[q] != 0;
   const double rings = ceil(rmax / A.res);  // SpiralIterator nRings
-  if (!(rmin >= 0.0) || !(rings <= (double)kPathMaxRings)) {  // not checkable here: marked so that no checked result looks alike
+  // not checkable here: marked so that no checked result looks alike (REQ: also a pose range outside the request)
+  if (!(rmin >= 0.0) || !(rings <= (double)kPathMaxRings) || (REQ && !(b >= 0 && n >= 0 && (long long)b + n <= R.nposes))) {
     if (lane == 0) {
       P.is_safe[q] = 0; P.trav_out[q] = nan("");
+      if (REQ) R.area_out[q] = nan("");
       if (POLY) O.count[q] = cup ? -1 : 0;
     }
     return;
@@ -1213,7 +1240,7 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
   int fi = 0, fj = 0, freps = 1;
   for (int k = 0; k < n && ok; ++k) {
     sx = ex; sy = ey;
-    ex = P.xy[2 * (b + k)]; ey = P.xy[2 * (b + k) + 1];
+    ex = P.xy[PS * (b + k)]; ey = P.xy[PS * (b + k) + 1];
     if (n == 1) {  // :365-387
       if (!inclination_ok_d(A, P.rslope, ex, ey, ex, ey)) { ok = false; break; }
       int i, j;
@@ -1244,8 +1271,8 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
         bool seen = false;
         for (int s = 1 + lane; s < k; s += 32) {
           int pi0, pj0, pi1, pj1;
-          get_index_d(A, P.xy[2 * (b + s - 1)], P.xy[2 * (b + s - 1) + 1], pi0, pj0);
-          get_index_d(A, P.xy[2 * (b + s)], P.xy[2 * (b + s) + 1], pi1, pj1);
+          get_index_d(A, P.xy[PS * (b + s - 1)], P.xy[PS * (b + s - 1) + 1], pi0, pj0);
+          get_index_d(A, P.xy[PS * (b + s)], P.xy[PS * (b + s) + 1], pi1, pj1);
           seen = seen || line_checks_d(pi1, pj1, pi0, pj0, a, bb);
         }
         const bool cached = __any_sync(0xffffffffu, seen);
@@ -1269,6 +1296,7 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
   if (lane == 0) {
     P.is_safe[q] = ok ? 1 : 0;
     P.trav_out[q] = ok ? result : 0.0;
+    if (REQ) R.area_out[q] = 0.0;  // TraversabilityResult.area stays 0 for a circular path
   }
   if (POLY) {
     // the last non-empty polygon published for the path: only an untraversable circle has one (inclination failures return first)
@@ -1284,7 +1312,7 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
 }
 
 __global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, PathArgs P) {
-  check_paths_fresh_d<false>(A, L, P, UntravOut{}, CircleTable{}, UntravScratch{});
+  check_paths_fresh_d<false, false>(A, L, P, UntravOut{}, CircleTable{}, UntravScratch{}, RequestArgs{});
 }
 
 // k_check_paths_fresh that also returns the untraversable polygon of every path (te_check_footprint_paths_fresh2).  Per warp:
@@ -1296,7 +1324,21 @@ __global__ void __launch_bounds__(128) k_check_paths_fresh_poly(FpArgs A, Layers
   __shared__ int2 s_first[4][3];
   static_assert(sizeof(s_stack[0]) >= 3 * kFromCircleVertices * sizeof(double2), "fromCircle points and hull fit the stack");
   const int w = threadIdx.x >> 5;
-  check_paths_fresh_d<true>(A, L, P, O, C, UntravScratch{s_min[w], s_max[w], s_stack[w], s_first[w]});
+  check_paths_fresh_d<true, false>(A, L, P, O, C, UntravScratch{s_min[w], s_max[w], s_stack[w], s_first[w]}, RequestArgs{});
+}
+
+// The two above on the circular paths of a request (te_check_footprint_request); P.xy points at the 7-wide poses.
+__global__ void __launch_bounds__(128) k_check_paths_fresh_req(FpArgs A, Layers L, PathArgs P, RequestArgs R) {
+  check_paths_fresh_d<false, true>(A, L, P, UntravOut{}, CircleTable{}, UntravScratch{}, R);
+}
+
+__global__ void __launch_bounds__(128) k_check_paths_fresh_poly_req(FpArgs A, Layers L, PathArgs P, UntravOut O, CircleTable C,
+                                                                    RequestArgs R) {
+  __shared__ int s_min[4][kFreshTableRows + 1], s_max[4][kFreshTableRows + 1];
+  __shared__ int2 s_stack[4][2 * kFreshTableRows + 4];
+  __shared__ int2 s_first[4][3];
+  const int w = threadIdx.x >> 5;
+  check_paths_fresh_d<true, true>(A, L, P, O, C, UntravScratch{s_min[w], s_max[w], s_stack[w], s_first[w]}, R);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -1346,8 +1388,15 @@ __device__ __forceinline__ PoseRT pose_rt_d(const double* p) {
 }
 
 // `toPosition * orientation * positionToVertex` (:496-500) for footprint vertex v, in the operand order of Eigen's Transform * vector.
-__device__ __forceinline__ double2 footprint_vertex_d(const PolyPathArgs& P, const PoseRT& T, int v) {
-  const double vx = (double)P.fx[v], vy = (double)P.fy[v], vz = (double)P.fz[v];
+// The vertex comes from the kernel parameters, or with REQ from the path's own footprint `fxyz` in global memory.
+template <bool REQ>
+__device__ __forceinline__ double2 footprint_vertex_d(const PolyPathArgs& P, const float* fxyz, const PoseRT& T, int v) {
+  double vx, vy, vz;
+  if (REQ) {
+    vx = (double)fxyz[3 * v]; vy = (double)fxyz[3 * v + 1]; vz = (double)fxyz[3 * v + 2];
+  } else {
+    vx = (double)P.fx[v]; vy = (double)P.fy[v]; vz = (double)P.fz[v];
+  }
   return make_double2(((T.r00 * vx + T.r01 * vy) + T.r02 * vz) + T.tx, ((T.r10 * vx + T.r11 * vy) + T.r12 * vz) + T.ty);
 }
 
@@ -1388,9 +1437,11 @@ __host__ __device__ inline size_t poly_warp_smem(int mcap, bool poly) {
 
 // One warp per pose index p.  Shared memory per warp: sA (2 mcap points: the hull input polygon1 ++ polygon2, then the hull) and
 // sB (mcap points: a conservative path's earlier polygon2, then the sorted hull input).  POLY: with compute_untraversable_polygon
-// set for the item's path, the walk goes on past blocked cells and collects them (:602-608, :634-638).
-template <bool POLY>
-__device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Layers& L, const PolyPathArgs& P, const PolyUntravArgs& U) {
+// set for the item's path, the walk goes on past blocked cells and collects them (:602-608, :634-638).  REQ: the items of the
+// polygonal paths of a request, each with its own footprint (RequestArgs); the poses of circular paths are no items.
+template <bool POLY, bool REQ>
+__device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Layers& L, const PolyPathArgs& P, const PolyUntravArgs& U,
+                                                     const RequestArgs& R) {
   extern __shared__ double2 sPoly[];
   const int lane = threadIdx.x & 31;
   const int p = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
@@ -1413,6 +1464,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
     if (P.path_begin[mid] <= p) lo = mid; else hi = mid - 1;
   }
   const int q = lo, b = P.path_begin[q], e = P.path_begin[q + 1], n = e - b, k = p - b;
+  if (REQ && R.fp_begin[q + 1] == R.fp_begin[q]) return;  // a pose of a circular path
   if (!(b >= 0 && b <= p && p < e && e <= P.nposes && (n == 1 || k >= 1))) {
     if (lane == 0) P.items[p] = it;
     return;
@@ -1422,7 +1474,17 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
   int ncollected = 0;  // POLY: blocked cells collected by the walk
   bool hit = false;    // POLY: the walk stopped at a blocked cell without collecting
   int nr_walk = 0, si_walk = 0;
-  const int nfp = P.nfp;
+  int nfp = P.nfp;
+  const float* fxyz = nullptr;  // REQ: the path's footprint
+  if (REQ) {
+    if (!__all_sync(0xffffffffu, request_footprint_ok_d(R, q, lane, 32))) {
+      if (lane == 0) P.items[p] = it;  // flag 2
+      return;
+    }
+    const int fb = R.fp_begin[q];
+    nfp = R.fp_begin[q + 1] - fb;
+    fxyz = R.fp_xyz + 3 * (size_t)fb;
+  }
   const bool cons = n > 1 && P.cons != nullptr && P.cons[q] != 0;
   const int m = n == 1 ? nfp : cons ? 2 * nfp * (k + 1) : 2 * nfp;  // points of polygon1 ++ polygon2
   bool finite = true;
@@ -1438,10 +1500,10 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
   const int h = m / 2;  // polygon1 = sA[0, h), polygon2 = sA[h, m) for n > 1
   if (n == 1) {  // polygon2 of the pose
     const PoseRT T = pose_rt_d(pk);
-    if (lane < nfp) sA[lane] = footprint_vertex_d(P, T, lane);
+    if (lane < nfp) sA[lane] = footprint_vertex_d<REQ>(P, fxyz, T, lane);
   } else if (!cons) {  // polygon1 = T_{k-1}(footprint), polygon2 = T_k(footprint)
     const PoseRT T = pose_rt_d(lane < nfp ? pk - 7 : pk);
-    if (lane < 2 * nfp) sA[lane] = footprint_vertex_d(P, T, lane < nfp ? lane : lane - nfp);
+    if (lane < 2 * nfp) sA[lane] = footprint_vertex_d<REQ>(P, fxyz, T, lane < nfp ? lane : lane - nfp);
   } else {
     // polygon2 of pose k-1 by footprint slot s = 0..k-1 (list order: slot k-1 first): slot s holds T_s(footprint) plus the
     // start-to-end vectors d_{s+1}, ..., d_{k-1} added in that order (:510-520).  Entry i is always lane i % 32's.
@@ -1450,7 +1512,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
       const PoseRT T = pose_rt_d(pj);
       const double dx = j > 0 ? pj[0] - pj[-7] : 0.0, dy = j > 0 ? pj[1] - pj[-6] : 0.0;
       for (int i = lane; i < nfp * (j + 1); i += 32) {
-        if (i >= nfp * j) sB[i] = footprint_vertex_d(P, T, i - nfp * j);
+        if (i >= nfp * j) sB[i] = footprint_vertex_d<REQ>(P, fxyz, T, i - nfp * j);
         else sB[i] = make_double2(sB[i].x + dx, sB[i].y + dy);
       }
     }
@@ -1465,7 +1527,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
         sA[l] = w;
         sA[h + nfp + l] = make_double2(w.x + dx, w.y + dy);
       } else {
-        const double2 w = footprint_vertex_d(P, T, l - ns);
+        const double2 w = footprint_vertex_d<REQ>(P, fxyz, T, l - ns);
         sA[l] = make_double2(w.x - dx, w.y - dy);
         sA[h + l - ns] = w;
       }
@@ -1569,29 +1631,45 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
 }
 
 __global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L, PolyPathArgs P) {
-  check_polygon_item_d<false>(A, L, P, PolyUntravArgs{});
+  check_polygon_item_d<false, false>(A, L, P, PolyUntravArgs{}, RequestArgs{});
 }
 
 __global__ void __launch_bounds__(128) k_check_polygon_items_poly(FpArgs A, Layers L, PolyPathArgs P, PolyUntravArgs U) {
-  check_polygon_item_d<true>(A, L, P, U);
+  check_polygon_item_d<true, false>(A, L, P, U, RequestArgs{});
+}
+
+__global__ void __launch_bounds__(128) k_check_polygon_items_req(FpArgs A, Layers L, PolyPathArgs P, RequestArgs R) {
+  check_polygon_item_d<false, true>(A, L, P, PolyUntravArgs{}, R);
+}
+
+__global__ void __launch_bounds__(128) k_check_polygon_items_poly_req(FpArgs A, Layers L, PolyPathArgs P, PolyUntravArgs U, RequestArgs R) {
+  check_polygon_item_d<true, true>(A, L, P, U, R);
 }
 
 // One thread per path: the area-weighted combination of the segment results in path order (:522-579).  An unsafe path reports 0;
 // a path the items could not check (bad range, non-finite pose, conservative list past the cap) is_safe 0 and NaN.  POLY: the
 // polygon of the item that failed (the reference publishes every segment's polygon and returns after the first failing one,
-// :555-567; traversable segments publish nothing); -1 for a path the items could not check.
-template <bool POLY>
-__device__ __forceinline__ void check_polygon_combine_d(const PolyPathArgs& P, const PolyUntravArgs& U) {
+// :555-567; traversable segments publish nothing); -1 for a path the items could not check.  REQ: the polygonal paths of a request
+// only, each with its own footprint; a footprint that cannot be checked makes its path not checkable.
+template <bool POLY, bool REQ>
+__device__ __forceinline__ void check_polygon_combine_d(const PolyPathArgs& P, const PolyUntravArgs& U, const RequestArgs& R) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= P.npaths) return;
+  int nfp = 0;  // REQ: the path's footprint vertices
+  bool fp_ok = true;
+  if (REQ) {
+    if (R.fp_begin[q + 1] == R.fp_begin[q]) return;  // a circular path: k_check_paths_fresh*_req writes its outputs
+    fp_ok = request_footprint_ok_d(R, q, 0, 1);
+    nfp = R.fp_begin[q + 1] - R.fp_begin[q];
+  }
   int failed = -1;  // POLY: pose index of the failing item
   const int b = P.path_begin[q], e = P.path_begin[q + 1], n = e - b;
-  bool checkable = b >= 0 && e >= b && e <= P.nposes;
+  bool checkable = fp_ok && b >= 0 && e >= b && e <= P.nposes;
   unsigned char safe = 0;
   double trav = 0.0, area = 0.0;
   if (checkable && n > 0) {
     const bool cons = n > 1 && P.cons != nullptr && P.cons[q] != 0;
-    if (cons && (long long)P.nfp * n > kPolyConsCap) checkable = false;
+    if (cons && (long long)(REQ ? nfp : P.nfp) * n > kPolyConsCap) checkable = false;
     for (long long c = 7LL * b; c < 7LL * e && checkable; ++c) checkable = isfinite(P.poses[c]);
     const int k0 = n == 1 ? 0 : 1;
     for (int k = k0; k < n && checkable; ++k) checkable = P.items[b + k].q == q && P.items[b + k].flag != 2;
@@ -1629,9 +1707,21 @@ __device__ __forceinline__ void check_polygon_combine_d(const PolyPathArgs& P, c
   }
 }
 
-__global__ void __launch_bounds__(128) k_check_polygon_combine(PolyPathArgs P) { check_polygon_combine_d<false>(P, PolyUntravArgs{}); }
+__global__ void __launch_bounds__(128) k_check_polygon_combine(PolyPathArgs P) {
+  check_polygon_combine_d<false, false>(P, PolyUntravArgs{}, RequestArgs{});
+}
 
-__global__ void __launch_bounds__(128) k_check_polygon_combine_poly(PolyPathArgs P, PolyUntravArgs U) { check_polygon_combine_d<true>(P, U); }
+__global__ void __launch_bounds__(128) k_check_polygon_combine_poly(PolyPathArgs P, PolyUntravArgs U) {
+  check_polygon_combine_d<true, false>(P, U, RequestArgs{});
+}
+
+__global__ void __launch_bounds__(128) k_check_polygon_combine_req(PolyPathArgs P, RequestArgs R) {
+  check_polygon_combine_d<false, true>(P, PolyUntravArgs{}, R);
+}
+
+__global__ void __launch_bounds__(128) k_check_polygon_combine_poly_req(PolyPathArgs P, PolyUntravArgs U, RequestArgs R) {
+  check_polygon_combine_d<true, true>(P, U, R);
+}
 
 inline int signum(int v) { return (0 < v) - (v < 0); }
 
@@ -1722,28 +1812,28 @@ int reset_filter_memo(FootprintState& st, const SlabView& v, cudaStream_t s) {
   if (cudaMemsetAsync(st.memo.p, 0, ncell, s) != cudaSuccess) { st.why = "cudaMemsetAsync(predicate memo) failed"; return TE_ERR_CUDA; }
   return 0;
 }
-}  // namespace
 
-int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                             const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                             int npaths, const int* path_begin, const double* xy, const double* radius, const unsigned char* cup,
-                             unsigned char* is_safe, double* trav_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s) {
-  if (!st.rings.p) {  // rings 0 .. kPathMaxRings once per context: the visit order inside a ring does not depend on the radius
-    std::vector<int> ring_start;
-    const std::vector<int> sp = spiral_rings(kPathMaxRings, ring_start);
-    std::vector<int> table(ring_start);
-    table.insert(table.end(), sp.begin(), sp.end());
-    if (st.rings.reserve(sizeof(int) * table.size()) != cudaSuccess) { st.why = "allocating the ring table failed"; return TE_ERR_CUDA; }
-    if (cudaMemcpyAsync(st.rings.p, table.data(), sizeof(int) * table.size(), cudaMemcpyHostToDevice, s) != cudaSuccess ||
-        cudaStreamSynchronize(s) != cudaSuccess) {
-      st.rings.release();
-      st.why = "ring table upload failed";
-      return TE_ERR_CUDA;
-    }
+// The ring table of the fresh path checks, rings 0 .. kPathMaxRings, uploaded once per context: the visit order inside a ring does
+// not depend on the radius.
+int ensure_ring_table(FootprintState& st, cudaStream_t s) {
+  if (st.rings.p) return 0;
+  std::vector<int> ring_start;
+  const std::vector<int> sp = spiral_rings(kPathMaxRings, ring_start);
+  std::vector<int> table(ring_start);
+  table.insert(table.end(), sp.begin(), sp.end());
+  if (st.rings.reserve(sizeof(int) * table.size()) != cudaSuccess) { st.why = "allocating the ring table failed"; return TE_ERR_CUDA; }
+  if (cudaMemcpyAsync(st.rings.p, table.data(), sizeof(int) * table.size(), cudaMemcpyHostToDevice, s) != cudaSuccess ||
+      cudaStreamSynchronize(s) != cudaSuccess) {
+    st.rings.release();
+    st.why = "ring table upload failed";
+    return TE_ERR_CUDA;
   }
-  if (int rc = reset_filter_memo(st, v, s)) return rc;
-  const FpArgs a = filter_args(v, g, p, rough);
-  const Layers L{trav, slope, step, elev, rough};
+  return 0;
+}
+
+// The path arguments of the fresh circular check (after ensure_ring_table and reset_filter_memo).
+PathArgs fresh_args(const FootprintState& st, const te_footprint_params* p, const float* robot_slope, int npaths, const int* path_begin,
+                    const double* xy, const double* radius, const unsigned char* cup, unsigned char* is_safe, double* trav_out) {
   PathArgs P{};
   P.rslope = robot_slope; P.npaths = npaths; P.path_begin = path_begin; P.xy = xy; P.radius = radius; P.cup = cup;
   P.offset = p->offset;
@@ -1751,18 +1841,95 @@ int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geo
   P.rings = P.ring_start + kPathMaxRings + 2;
   P.memo = (unsigned char*)st.memo.p;
   P.is_safe = is_safe; P.trav_out = trav_out;
-  const long long threads = 32LL * npaths;
-  if (!ucount) {
-    k_check_paths_fresh<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P);
-    return 0;
-  }
+  return P;
+}
+
+CircleTable circle_table() {
   CircleTable C{};
   for (int j = 0; j < kFromCircleVertices; ++j) {  // Polygon::fromCircle: theta = j * 2 * M_PI / (nVertices - 1)
     volatile double theta = j * 2 * M_PI / (kFromCircleVertices - 1);  // volatile: libm at run time, never a folded constant
     C.cs[j] = std::cos(theta);
     C.sn[j] = std::sin(theta);
   }
-  k_check_paths_fresh_poly<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P, UntravOut{max_vertices, ucount, uxy}, C);
+  return C;
+}
+
+// The path arguments of the polygonal check, with the per-call item records reserved (after reset_filter_memo).
+int polygon_args(FootprintState& st, const te_footprint_params* p, const float* robot_slope, int npaths, int nposes, int max_points,
+                 const int* path_begin, const double* poses, const unsigned char* conservative, unsigned char* is_safe, double* trav_out,
+                 double* area_out, PolyPathArgs* out) {
+  if (st.items.reserve(sizeof(PolyItem) * (size_t)std::max(nposes, 1)) != cudaSuccess) {
+    st.why = "allocating the polygon items failed";
+    return TE_ERR_CUDA;
+  }
+  PolyPathArgs& P = *out;
+  P = PolyPathArgs{};
+  P.rslope = robot_slope; P.npaths = npaths; P.nposes = nposes; P.mcap = max_points;
+  P.path_begin = path_begin; P.poses = poses; P.cons = conservative;
+  P.memo = (unsigned char*)st.memo.p;
+  P.items = (PolyItem*)st.items.p;
+  P.is_safe = is_safe; P.trav_out = trav_out; P.area_out = area_out;
+  return 0;
+}
+
+// The untraversable polygons of the polygonal check: per item a count and max_vertices points, copied to the paths by the combine
+// kernel.
+int polygon_untrav_args(FootprintState& st, int nposes, const unsigned char* cup, int max_vertices, int* ucount, double* uxy,
+                        PolyUntravArgs* out) {
+  const size_t nitems = (size_t)std::max(nposes, 1);
+  const size_t cbytes = (sizeof(int) * nitems + 15) / 16 * 16;
+  if (st.upoly.reserve(cbytes + sizeof(double2) * nitems * (size_t)std::max(max_vertices, 1)) != cudaSuccess) {
+    st.why = "allocating the untraversable polygons failed";
+    return TE_ERR_CUDA;
+  }
+  *out = PolyUntravArgs{};
+  out->cup = cup;
+  out->out = UntravOut{max_vertices, ucount, uxy};
+  out->item_count = (int*)st.upoly.p;
+  out->item_xy = (double*)((char*)st.upoly.p + cbytes);
+  return 0;
+}
+
+// The item kernel (one warp per pose index, skipped without poses) and then the combine kernel of a polygonal check.  Four warps
+// per block while their shared memory stays small (below 48 KB, or 100 KB with the polygon tables); one warp per block for long
+// conservative paths.  `extra` are the arguments both kernels take after the PolyPathArgs.
+template <class KItems, class KCombine, class... Extra>
+int launch_polygon_kernels(FootprintState& st, KItems items, KCombine combine, const char* items_name, bool poly, const FpArgs& a,
+                           const Layers& L, const PolyPathArgs& P, cudaStream_t s, int* launches, const Extra&... extra) {
+  if (P.nposes > 0) {
+    const size_t per_warp = poly_warp_smem(P.mcap, poly);
+    const int wpb = per_warp * 4 <= (poly ? 100 : 48) * 1024 ? 4 : 1;
+    const size_t smem = per_warp * wpb;
+    if (smem > 48 * 1024 && cudaFuncSetAttribute(items, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+      st.why = std::string("cudaFuncSetAttribute(") + items_name + ") failed";
+      return TE_ERR_CUDA;
+    }
+    const long long blocks = ((long long)P.nposes + wpb - 1) / wpb;
+    items<<<(unsigned)blocks, 32 * wpb, smem, s>>>(a, L, P, extra...);
+    ++*launches;
+  }
+  combine<<<(unsigned)((P.npaths + 127) / 128), 128, 0, s>>>(P, extra...);
+  ++*launches;
+  return 0;
+}
+}  // namespace
+
+int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                             const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                             int npaths, const int* path_begin, const double* xy, const double* radius, const unsigned char* cup,
+                             unsigned char* is_safe, double* trav_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s) {
+  if (int rc = ensure_ring_table(st, s)) return rc;
+  if (int rc = reset_filter_memo(st, v, s)) return rc;
+  const FpArgs a = filter_args(v, g, p, rough);
+  const Layers L{trav, slope, step, elev, rough};
+  const PathArgs P = fresh_args(st, p, robot_slope, npaths, path_begin, xy, radius, cup, is_safe, trav_out);
+  const long long threads = 32LL * npaths;
+  if (!ucount) {
+    k_check_paths_fresh<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P);
+    return 0;
+  }
+  k_check_paths_fresh_poly<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P, UntravOut{max_vertices, ucount, uxy},
+                                                                              circle_table());
   return 0;
 }
 
@@ -1775,65 +1942,58 @@ int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_g
   *launches = 0;
   if (nfp < 1 || nfp > kPolyMaxVerts || max_points < 2 * nfp || max_points > 2 * kPolyConsCap) { st.why = "bad footprint size"; return TE_ERR_BAD_ARG; }
   if (int rc = reset_filter_memo(st, v, s)) return rc;
-  const size_t nitems = (size_t)std::max(nposes, 1);
-  if (st.items.reserve(sizeof(PolyItem) * nitems) != cudaSuccess) { st.why = "allocating the polygon items failed"; return TE_ERR_CUDA; }
   const FpArgs a = filter_args(v, g, p, rough);
   const Layers L{trav, slope, step, elev, rough};
-  PolyPathArgs P{};
-  P.rslope = robot_slope; P.npaths = npaths; P.nposes = nposes; P.nfp = nfp; P.mcap = max_points;
-  P.path_begin = path_begin; P.poses = poses; P.cons = conservative;
-  P.memo = (unsigned char*)st.memo.p;
-  P.items = (PolyItem*)st.items.p;
-  P.is_safe = is_safe; P.trav_out = trav_out; P.area_out = area_out;
+  PolyPathArgs P;
+  if (int rc = polygon_args(st, p, robot_slope, npaths, nposes, max_points, path_begin, poses, conservative, is_safe, trav_out, area_out, &P))
+    return rc;
+  P.nfp = nfp;
   for (int k = 0; k < nfp; ++k) {
     P.fx[k] = footprint_xyz[3 * k]; P.fy[k] = footprint_xyz[3 * k + 1]; P.fz[k] = footprint_xyz[3 * k + 2];
   }
-  if (ucount) {  // the untraversable polygons: per item a count and max_vertices points, copied to the paths by the combine kernel
-    PolyUntravArgs U{};
-    U.cup = cup;
-    U.out = UntravOut{max_vertices, ucount, uxy};
-    const size_t cbytes = (sizeof(int) * nitems + 15) / 16 * 16;
-    if (st.upoly.reserve(cbytes + sizeof(double2) * nitems * (size_t)std::max(max_vertices, 1)) != cudaSuccess) {
-      st.why = "allocating the untraversable polygons failed";
-      return TE_ERR_CUDA;
-    }
-    U.item_count = (int*)st.upoly.p;
-    U.item_xy = (double*)((char*)st.upoly.p + cbytes);
-    if (nposes > 0) {
-      // four warps per block while their shared memory stays below 100 KB; one warp per block for long conservative paths
-      const size_t per_warp = poly_warp_smem(max_points, true);
-      const int wpb = per_warp * 4 <= 100 * 1024 ? 4 : 1;
-      const size_t smem = per_warp * wpb;
-      if (smem > 48 * 1024 &&
-          cudaFuncSetAttribute(k_check_polygon_items_poly, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-        st.why = "cudaFuncSetAttribute(k_check_polygon_items_poly) failed";
-        return TE_ERR_CUDA;
-      }
-      const long long blocks = ((long long)nposes + wpb - 1) / wpb;
-      k_check_polygon_items_poly<<<(unsigned)blocks, 32 * wpb, smem, s>>>(a, L, P, U);
-      ++*launches;
-    }
-    k_check_polygon_combine_poly<<<(unsigned)((npaths + 127) / 128), 128, 0, s>>>(P, U);
-    ++*launches;
-    return 0;
+  if (!ucount)
+    return launch_polygon_kernels(st, k_check_polygon_items, k_check_polygon_combine, "k_check_polygon_items", false, a, L, P, s, launches);
+  PolyUntravArgs U;
+  if (int rc = polygon_untrav_args(st, nposes, cup, max_vertices, ucount, uxy, &U)) return rc;
+  return launch_polygon_kernels(st, k_check_polygon_items_poly, k_check_polygon_combine_poly, "k_check_polygon_items_poly", true, a, L, P, s,
+                                launches, U);
+}
+
+int launch_check_request(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                         const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                         int npaths, int nposes, const int* path_begin, const double* poses, const double* radius, int nvertices,
+                         const int* footprint_begin, const float* footprint_xyz, int max_footprint_vertices,
+                         const unsigned char* conservative, const unsigned char* cup, int max_points, unsigned char* is_safe,
+                         double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s,
+                         int* launches) {
+  *launches = 0;
+  if (max_footprint_vertices < 0 || max_footprint_vertices > kPolyMaxVerts || max_points < 2 || max_points > 2 * kPolyConsCap) {
+    st.why = "bad footprint size";
+    return TE_ERR_BAD_ARG;
   }
-  if (nposes > 0) {
-    // four warps per block while their shared memory stays small; one warp per block for long conservative paths
-    const size_t per_warp = sizeof(double2) * 3 * (size_t)max_points;
-    const int wpb = per_warp * 4 <= 48 * 1024 ? 4 : 1;
-    const size_t smem = per_warp * wpb;
-    if (smem > 48 * 1024 &&
-        cudaFuncSetAttribute(k_check_polygon_items, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-      st.why = "cudaFuncSetAttribute(k_check_polygon_items) failed";
-      return TE_ERR_CUDA;
-    }
-    const long long blocks = ((long long)nposes + wpb - 1) / wpb;
-    k_check_polygon_items<<<(unsigned)blocks, 32 * wpb, smem, s>>>(a, L, P);
+  if (int rc = ensure_ring_table(st, s)) return rc;
+  if (int rc = reset_filter_memo(st, v, s)) return rc;  // one memo for both kinds of path: it depends on the layers only
+  const FpArgs a = filter_args(v, g, p, rough);
+  const Layers L{trav, slope, step, elev, rough};
+  const RequestArgs R{footprint_begin, footprint_xyz, nvertices, max_footprint_vertices, nposes, area_out};
+  PolyPathArgs P;
+  if (int rc = polygon_args(st, p, robot_slope, npaths, nposes, max_points, path_begin, poses, conservative, is_safe, trav_out, area_out, &P))
+    return rc;
+  PolyUntravArgs U;
+  if (ucount)
+    if (int rc = polygon_untrav_args(st, nposes, cup, max_vertices, ucount, uxy, &U)) return rc;
+  const PathArgs C = fresh_args(st, p, robot_slope, npaths, path_begin, poses, radius, cup, is_safe, trav_out);
+  const unsigned blocks = (unsigned)((32LL * npaths + 127) / 128);
+  if (!ucount) {
+    k_check_paths_fresh_req<<<blocks, 128, 0, s>>>(a, L, C, R);
     ++*launches;
+    return launch_polygon_kernels(st, k_check_polygon_items_req, k_check_polygon_combine_req, "k_check_polygon_items_req", false, a, L, P,
+                                  s, launches, R);
   }
-  k_check_polygon_combine<<<(unsigned)((npaths + 127) / 128), 128, 0, s>>>(P);
+  k_check_paths_fresh_poly_req<<<blocks, 128, 0, s>>>(a, L, C, UntravOut{max_vertices, ucount, uxy}, circle_table(), R);
   ++*launches;
-  return 0;
+  return launch_polygon_kernels(st, k_check_polygon_items_poly_req, k_check_polygon_combine_poly_req, "k_check_polygon_items_poly_req", true,
+                                a, L, P, s, launches, U, R);
 }
 
 // isTraversableForFilters for every cell of the slab + halo into st.block (k_pred_classify + k_pred_heavy); fills the geometry /

@@ -74,4 +74,16 @@ int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_g
                                double* area_out, const unsigned char* cup, int max_vertices, int* ucount, double* uxy,
                                cudaStream_t s, int* launches);
 
+// A whole check_footprint_path request (te_check_footprint_request): the two checks above on one predicate memo, each path with its
+// own footprint (footprint_begin / footprint_xyz, device pointers): none is circular (radius[q]), 1..max_footprint_vertices vertices
+// polygonal.  Poses are 7 doubles for both kinds.  `max_points` bounds the hull input of a polygonal item as in
+// launch_check_paths_polygon, for the largest footprint.  Three launches (two without poses), whatever the footprints.
+int launch_check_request(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                         const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                         int npaths, int nposes, const int* path_begin, const double* poses, const double* radius, int nvertices,
+                         const int* footprint_begin, const float* footprint_xyz, int max_footprint_vertices,
+                         const unsigned char* conservative, const unsigned char* cup, int max_points, unsigned char* is_safe,
+                         double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s,
+                         int* launches);
+
 }  // namespace te
