@@ -241,9 +241,9 @@ int te_check_footprint_paths2(te_ctx* ctx, const te_geometry* g, const float* tr
  *     first blocker in that annulus leaves the circle traversable with its mean divided by the cell count twice (:707, :733);
  *   - a centre that an earlier segment of the same path checked reads the float32 value the first check stored (:673-675):
  *     traversable iff it is != 0.
- * Cache across paths — a deliberate choice: every path is answered as the first check after computeTraversability, on an empty
- * cache; within a path the cache is reproduced exactly.  The reference keeps the cache across the paths of a request and across
- * requests until the next map update, so its answers depend on a call history no caller controls.
+ * Cache across paths: every path is answered as the first check after computeTraversability, on an empty cache; within a path
+ * the cache is reproduced exactly.  The reference keeps the cache across the paths of a request and across requests until the
+ * next map update; te_map_check_footprint_request on a te_map (below) answers as it does.
  * Layers: the chain outputs traversability, traversability_slope, traversability_step (traversability_roughness when
  * p->verify_roughness is set) and elevation; robot_slope_or_null switches checkRobotInclination_ on, as in
  * te_check_footprint_paths2.  From `p` only offset (radiusMax = radius + offset; the reference hard-codes 0.15, :348),
@@ -349,7 +349,8 @@ int te_check_footprint_paths_polygon2(te_ctx* ctx, const te_geometry* g, const t
                                       int32_t* untraversable_count_or_null, double* untraversable_xy_or_null, int memory);
 
 /* A whole CheckFootprintPath request (TraversabilityEstimation.cpp:278-295) in one call: FootprintPath[] with circular and
- * polygonal paths mixed, each with its own footprint, results in request order.  Path q is circular when its footprint has no
+ * polygonal paths mixed, each with its own footprint, results in request order.  Every circular path sees an empty
+ * traversability_footprint cache; for the reference node's answers over a sequence of requests use te_map_check_footprint_request.  Path q is circular when its footprint has no
  * vertices (checkFootprintPath, TraversabilityMap.cpp:320-343: any non-empty polygon takes the polygonal branch) and gets, bit for
  * bit, what te_check_footprint_paths_fresh2 gives for it alone with radius[q] and compute_untraversable_polygon[q]; its area is 0,
  * as in the reference's result.  Otherwise it gets what te_check_footprint_paths_polygon2 gives for it alone with its own
@@ -381,6 +382,73 @@ int te_check_footprint_request(te_ctx* ctx, const te_geometry* g, const te_footp
                                const uint8_t* compute_untraversable_polygon_or_null, uint8_t* is_safe, double* traversability_out,
                                double* area_out, int32_t max_vertices, int32_t* untraversable_count_or_null,
                                double* untraversable_xy_or_null, int memory);
+
+/* ---- te_map: a traversability map that stays on the device between calls -------------------------------------------------------
+ * The reference keeps its layers, the traversability_footprint cache and the isTraversableForFilters memo in one TraversabilityMap;
+ * computeTraversability (TraversabilityMap.cpp:202-237) resets them and nothing else does (resetTraversabilityFootprintLayers,
+ * :195-200, has no caller).  So the answers of its check_footprint_path service depend on the checks before them: a circle
+ * whose first blocked cell lies between radius and radius + offset is untraversable the first time (:714-717) but stores a
+ * positive value (:708) that every later check of that cell reads back as traversable (:673-675).  A te_map holds that state on
+ * the device, so a node that keeps one te_map answers as the reference node does, and uploads its layers once per map update
+ * instead of once per call.  The stateless entries above keep answering every call on an empty cache.
+ *
+ * A te_map belongs to one te_ctx: it runs on that context's stream under its lock and must be destroyed before the context.  It
+ * owns, on the device, the layers traversability, traversability_slope, traversability_step, traversability_roughness (optional),
+ * elevation and robot_slope (optional); the traversability_footprint cache (float32, NaN = empty); and the isTraversableForFilters
+ * memo, which is kept until the layers or one of max_gap_width, critical_step_height and verify_roughness change.  Whole maps only.
+ * Host layers may carry a circular-buffer start index: they are unwrapped on upload and outputs are re-wrapped to the start index
+ * of the last te_map_chain / te_map_set_layers.  Every entry but te_map_create / te_map_destroy fails with TE_ERR_BAD_ARG before
+ * layers were set.  Host-memory entries return synchronised; device-memory ones are asynchronous on the context stream. */
+typedef struct te_map te_map;
+int te_map_create(te_ctx* ctx, te_map** out);
+int te_map_destroy(te_map* map);
+
+/* computeTraversability (:202-237): te_chain on `elevation` into the map's layers, each optionally copied out (NULL: kept on the
+ * device only).  Empties the cache and the memo and leaves the map without robot_slope. */
+int te_map_chain(te_map* map, const te_geometry* g, const te_chain_params* p, const float* elevation, float* slope_or_null,
+                 float* step_or_null, float* roughness_or_null, float* traversability_or_null, int memory);
+
+/* setTraversabilityMap: the layers as given (a map received or loaded from a bag).  Empties the cache and the memo.
+ * TE_ERR_MISSING_LAYER for a missing required layer. */
+int te_map_set_layers(te_map* map, const te_geometry* g, const float* traversability, const float* slope, const float* step,
+                      const float* roughness_or_null, const float* elevation, const float* robot_slope_or_null, int memory);
+
+/* traversabilityFootprint(radius, offset) (:307-318) on the cache: a cached cell keeps its value (the memoised branch, :673-675),
+ * every other cell gets te_footprint2's value for `p`; traversability_footprint_or_null receives the cache afterwards.  The
+ * prefix-sum sweep may differ from the visit-by-visit one in the last float32 bit of a few cells (DESIGN.md §4.3); those values
+ * then stay in the cache.  Errors as te_footprint2 (TE_ERR_MISSING_LAYER: verify_roughness without a roughness layer). */
+int te_map_footprint(te_map* map, const te_footprint_params* p, float* traversability_footprint_or_null, int memory);
+
+/* traversabilityFootprint(yaw) (:239-305): te_footprint_polygon on the map's layers.  Reads and changes no cache. */
+int te_map_footprint_polygon(te_map* map, const te_footprint_params* p, int32_t npts, const double* polygon_xy, double footprint_yaw,
+                             float* traversability_x, float* traversability_rot, int memory);
+
+/* A CheckFootprintPath request on the map, as the reference service loop answers it (TraversabilityEstimation.cpp:278-295, with
+ * publishPolygons = true).  Arguments, outputs, conventions, limits and errors are those of te_check_footprint_request, with the
+ * layers and the memory mode taken from the map: every array is in HOST memory (requests come from a ROS message, and which checks
+ * run depends on values earlier checks cached, which the host resolves); the call returns synchronised.  Planners whose requests
+ * live on the device use te_check_footprint_request.  Paths run in request order.  A circular path's isTraversable calls
+ * (:654-746) read and fill the cache exactly as the reference's do: a centre outside the map gives the default and stores
+ * nothing; a cached cell gives its float32 value and is traversable iff it is != 0 (with compute_untraversable_polygon, a cached 0
+ * publishes Polygon::fromCircle); any other cell walks the spiral with this check's radius, offset and flag, returns the double
+ * mean to the path sum and stores (float) of what the reference stores.  Checks after the first failure of a segment, and the
+ * checks of a segment or pose whose checkInclination fails, do not run and store nothing.  Polygonal paths neither read nor
+ * change the cache. */
+int te_map_check_footprint_request(te_map* map, const te_footprint_params* p, int32_t npaths, int32_t nposes, const int32_t* path_begin,
+                                   const double* poses, const double* radius, int32_t nvertices, const int32_t* footprint_begin,
+                                   const float* footprint_xyz, int32_t max_footprint_vertices, const uint8_t* conservative_or_null,
+                                   const uint8_t* compute_untraversable_polygon_or_null, uint8_t* is_safe, double* traversability_out,
+                                   double* area_out, int32_t max_vertices, int32_t* untraversable_count_or_null,
+                                   double* untraversable_xy_or_null);
+
+/* The cache as publishTraversabilityMap publishes its traversability_footprint layer (in host memory: in the map's buffer
+ * order; device memory needs a map without a start index), and resetTraversabilityFootprintLayers (:195-200). */
+int te_map_get_footprint(te_map* map, float* traversability_footprint, int memory);
+int te_map_clear_footprint(te_map* map);
+
+/* Counters of the last te_map_check_footprint_request: out[0] isTraversable calls its circular paths could make, out[1] distinct
+ * circles among them (each is walked once on the device), out[2] cache cells the request stored.  No reference counterpart. */
+int te_map_request_stats(te_map* map, int64_t out[3]);
 
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the

@@ -75,7 +75,10 @@ def main():
     ap.add_argument("--footprint", choices=("circle", "polygon"), default="circle")
     ap.add_argument("--untraversable", action="store_true")
     ap.add_argument("--request", action="store_true")
+    ap.add_argument("--map", action="store_true")
     args = ap.parse_args()
+    if args.map:
+        return main_map(args)
     if args.request:
         return main_request(args)
     if args.untraversable:
@@ -425,6 +428,90 @@ def main_request(args):
             row["device_identical"] = all(np.array_equal(a.view(np.uint8), b.view(np.uint8)) for a, b in zip(dev_got, want))
             print(json.dumps(row), flush=True)
     ctx.set_stream(None)
+    ctx.close()
+
+
+def main_map(args):
+    """te_map_check_footprint_request against te_check_footprint_request, both in host memory, on planner-like batches with every
+    other path circular (radius 0.3) and the YAML footprint on the others.  `map_cleared_ms`: the map request on an empty cache
+    (te_map_clear_footprint before each call, not timed); `map_repeat_ms`: the same request again on the cache it left.  The
+    device time is the sum of the map request's kernels (torch.profiler, CUDA activities) per call."""
+    import time
+    import torch
+    import synth
+    import traversability_estimation_b200 as te
+
+    n, res = args.size, 0.02
+    g = te.Geometry.make(n, n, res)
+    fp = te.FootprintParams.yaml_defaults()
+    ctx = te.Context(0)
+    z = synth.terrain(n, n, res, 4096, "mixed")
+    layers = ctx.chain_host(g, te.ChainParams.yaml_defaults(0), z)
+    host = {k: np.asfortranarray(a, np.float32) for k, a in (("trav", layers["traversability"]), ("slope", layers["slope"]),
+                                                             ("step", layers["step"]), ("elev", z))}
+    m = ctx.map()
+    t0 = time.perf_counter()
+    m.set_layers(g, host["trav"], host["slope"], host["step"], host["elev"])
+    set_ms = (time.perf_counter() - t0) * 1e3
+    name, power = gpu_info(torch)
+    rng = np.random.default_rng(1)
+
+    def timed(run, before=None):
+        for _ in range(args.warmup):
+            if before:
+                before()
+            run()
+        ts = []
+        for _ in range(args.reps):
+            if before:
+                before()
+            t = time.perf_counter()
+            run()
+            ts.append((time.perf_counter() - t) * 1e3)
+        return float(np.median(ts)), float(np.min(ts))
+
+    for batch in (1, 100, 1000):
+        begin, xy = planner_paths(rng, n, batch, res)
+        yaw = rng.uniform(0, 2 * np.pi, len(xy))
+        poses = np.stack([xy[:, 0], xy[:, 1], np.zeros(len(xy)), np.zeros(len(xy)), np.zeros(len(xy)), np.sin(yaw / 2),
+                          np.cos(yaw / 2)], axis=1)
+        fps = request_footprints(1)
+        kind = np.where(np.arange(batch) % 2 == 1, -1, 0)
+        fbeg = np.concatenate([[0], np.cumsum([0 if k < 0 else len(fps[0]) for k in kind])]).astype(np.int32)
+        fxyz = np.concatenate([fps[0] for k in kind if k >= 0] + [np.zeros((0, 3), np.float32)])
+        radius = np.full(batch, 0.3)
+
+        def stateless():
+            return ctx.check_footprint_request(g, fp, host["trav"], host["slope"], host["step"], host["elev"], begin, poses, radius,
+                                               fbeg, fxyz)
+
+        def on_map():
+            return m.check_footprint_request(fp, begin, poses, radius, fbeg, fxyz)
+
+        m.clear_footprint()
+        first = on_map()
+        cand, keys, stored = m.request_stats()
+        row = {"gpu": name, "power_limit_w": power, "map": f"{n}x{n}", "resolution": res, "paths": batch, "poses": int(begin[-1]),
+               "circular": int((kind < 0).sum()), "candidate_checks": cand, "distinct_keys": keys, "cells_stored": stored,
+               "set_layers_ms": round(set_ms, 2)}
+        want = stateless()
+        # equal unless paths of the batch check the same cells: the map then answers as the reference does, the stateless entry
+        # on an empty cache per path
+        row["equal_to_stateless"] = all(np.array_equal(a.view(np.uint8), b.view(np.uint8)) for a, b in zip(first, want))
+        row["stateless_ms"], row["stateless_min_ms"] = timed(stateless)
+        row["map_cleared_ms"], row["map_cleared_min_ms"] = timed(on_map, m.clear_footprint)
+        row["map_repeat_ms"], row["map_repeat_min_ms"] = timed(on_map)
+        for label, before in (("cleared", m.clear_footprint), ("repeat", None)):
+            reps = 5
+            with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+                for _ in range(reps):
+                    if before:
+                        before()
+                    on_map()
+            ev = [e for e in prof.key_averages() if "k_map_" in e.key or "k_check_polygon" in e.key]
+            row[f"map_{label}_kernels_ms"] = round(sum(e.self_device_time_total for e in ev) / 1e3 / reps, 4)
+        print(json.dumps(row), flush=True)
+    m.close()
     ctx.close()
 
 

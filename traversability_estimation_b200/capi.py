@@ -19,7 +19,9 @@ KERNEL_AUTO, KERNEL_GENERIC, KERNEL_FUSED = 0, 1, 2
 EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set_stream", "te_synchronize",
            "te_set_kernel", "te_get_stats", "te_enable_timing", "te_get_timing", "te_get_flag_counters", "te_get_escalation_stats", "te_fused_plan", "te_slope", "te_normals", "te_step", "te_roughness", "te_chain",
            "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_check_footprint_paths_fresh2", "te_check_footprint_paths_polygon2", "te_check_footprint_request", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
-           "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free"]
+           "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free", "te_map_create", "te_map_destroy",
+           "te_map_chain", "te_map_set_layers", "te_map_footprint", "te_map_footprint_polygon", "te_map_check_footprint_request",
+           "te_map_get_footprint", "te_map_clear_footprint", "te_map_request_stats"]
 
 
 IPC_HANDLE_BYTES = 80  # TE_IPC_HANDLE_BYTES
@@ -475,6 +477,10 @@ class Context:
             return safe, trav, area
         return safe, trav, area, counts, uxy
 
+    def map(self):
+        """A Map (te_map) owned by this context."""
+        return Map(self)
+
     # ---- multi-GPU halo (te_halo_pull and the IPC helpers around it)
     def ipc_export(self, device_ptr) -> bytes:
         h = C.create_string_buffer(IPC_HANDLE_BYTES)
@@ -520,3 +526,123 @@ class Context:
         self.chain(g, p, e, o["slope"], o["step"], o["roughness"], o["traversability"], MEM_HOST, **n)
         o.update(n)
         return o
+
+
+class Map:
+    """te_map: the traversability layers, the traversability_footprint cache and the isTraversableForFilters memo kept on the
+    device between calls, so that check_footprint_request answers as the reference's check_footprint_path service does over a
+    sequence of requests.  Layers are numpy arrays in host memory (rows x cols, any order; copied column-major); the geometry's
+    start index, if any, applies to them and to the layers read back."""
+
+    def __init__(self, ctx: Context):
+        self._ctx = ctx
+        self._L = ctx._L
+        h = C.c_void_p()
+        self._L.te_map_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+        self._check(self._L.te_map_create(ctx._h, C.byref(h)))
+        self._h = h
+        self._g = None
+
+    def _check(self, rc):
+        self._ctx._check(rc)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.te_map_destroy.argtypes = [C.c_void_p]
+            self._L.te_map_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _shape(self):
+        return (self._g.rows, self._g.cols)
+
+    def chain(self, g, p, elevation, outputs=False):
+        """te_map_chain (computeTraversability): empties the cache.  outputs=True also returns the four layers as a dict."""
+        fn = self._L.te_map_chain
+        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(ChainParams)] + [C.c_void_p] * 5 + [C.c_int]
+        e = np.asfortranarray(elevation, dtype=np.float32)
+        out = {k: np.empty((g.rows, g.cols), dtype=np.float32, order="F") for k in ("slope", "step", "roughness", "traversability")} \
+            if outputs else {}
+        self._check(fn(self._h, C.byref(g), C.byref(p), _addr(e), *(_addr(out.get(k)) for k in ("slope", "step", "roughness",
+                                                                                                 "traversability")), MEM_HOST))
+        self._g = g
+        return out if outputs else None
+
+    def set_layers(self, g, traversability, slope, step, elevation, roughness=None, robot_slope=None):
+        """te_map_set_layers (setTraversabilityMap): empties the cache and the memo."""
+        fn = self._L.te_map_set_layers
+        fn.argtypes = [C.c_void_p, C.POINTER(Geometry)] + [C.c_void_p] * 6 + [C.c_int]
+        lay = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)  # noqa: E731
+        t, s, st, r, e, rs = (lay(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
+        self._check(fn(self._h, C.byref(g), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST))
+        self._g = g
+
+    def footprint(self, fp):
+        """te_map_footprint (traversabilityFootprint(radius, offset) on the cache); returns the cache afterwards."""
+        fn = self._L.te_map_footprint
+        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_void_p, C.c_int]
+        out = np.empty(self._shape() if self._g else (0, 0), dtype=np.float32, order="F")
+        self._check(fn(self._h, C.byref(fp), _addr(out) if self._g else None, MEM_HOST))
+        return out
+
+    def footprint_polygon(self, fp, polygon_xy, yaw):
+        """te_map_footprint_polygon: (traversability_x, traversability_rot) of the map's layers."""
+        fn = self._L.te_map_footprint_polygon
+        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_int]
+        pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
+        ox = np.empty(self._shape(), dtype=np.float32, order="F")
+        orot = np.empty(self._shape(), dtype=np.float32, order="F")
+        self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, float(yaw), _addr(ox), _addr(orot), MEM_HOST))
+        return ox, orot
+
+    def check_footprint_request(self, fp, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices=None,
+                                conservative=None, compute_untraversable_polygon=None, untraversable_capacity=None):
+        """te_map_check_footprint_request: Context.check_footprint_request in host memory on the map's layers and cache.
+        Returns (is_safe, traversability, area) and, with untraversable_capacity=V, (counts, xy) too."""
+        fn = self._L.te_map_check_footprint_request
+        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                       C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p, C.c_void_p]
+        pb = np.ascontiguousarray(path_begin, dtype=np.int32)
+        ps = np.ascontiguousarray(poses, dtype=np.float64).reshape(-1, 7)
+        rad = np.ascontiguousarray(radius, dtype=np.float64)
+        fb = np.ascontiguousarray(footprint_begin, dtype=np.int32)
+        fxyz = np.ascontiguousarray(footprint_xyz, dtype=np.float32).reshape(-1, 3)
+        n = len(pb) - 1
+        per_path = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.uint8)  # noqa: E731
+        cons, cup = per_path(conservative), per_path(compute_untraversable_polygon)
+        if max_footprint_vertices is None:
+            max_footprint_vertices = int(np.diff(fb).max()) if n > 0 else 0
+        maxv = 0 if untraversable_capacity is None else int(untraversable_capacity)
+        safe, trav, area = np.zeros(n, dtype=np.uint8), np.zeros(n, dtype=np.float64), np.zeros(n, dtype=np.float64)
+        counts, uxy = (None, None) if untraversable_capacity is None else _untraversable_outputs(n, maxv)
+        self._check(fn(self._h, C.byref(fp), n, len(ps), pb.ctypes.data, ps.ctypes.data, rad.ctypes.data, len(fxyz), fb.ctypes.data,
+                       fxyz.ctypes.data, int(max_footprint_vertices), _addr(cons), _addr(cup), safe.ctypes.data, trav.ctypes.data,
+                       area.ctypes.data, maxv, _addr(counts), _addr(uxy)))
+        if untraversable_capacity is None:
+            return safe, trav, area
+        return safe, trav, area, counts, uxy
+
+    def get_footprint(self):
+        """te_map_get_footprint: the traversability_footprint cache (NaN = empty)."""
+        fn = self._L.te_map_get_footprint
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        out = np.empty(self._shape() if self._g else (0, 0), dtype=np.float32, order="F")
+        self._check(fn(self._h, _addr(out) if self._g else None, MEM_HOST))
+        return out
+
+    def clear_footprint(self):
+        """te_map_clear_footprint (resetTraversabilityFootprintLayers)."""
+        self._L.te_map_clear_footprint.argtypes = [C.c_void_p]
+        self._check(self._L.te_map_clear_footprint(self._h))
+
+    def request_stats(self):
+        """(candidate checks, distinct circles walked, cache cells stored) of the last request."""
+        out = (C.c_int64 * 3)()
+        self._L.te_map_request_stats.argtypes = [C.c_void_p, C.c_int64 * 3]
+        self._check(self._L.te_map_request_stats(self._h, out))
+        return tuple(int(v) for v in out)

@@ -39,12 +39,7 @@ int fail(int code, const char* fmt, ...) {
   } while (0)
 
 using te::DevBuf;
-
-// grid_map::getPositionFromIndex operand order (SURVEY.md A.1).
-inline double cell_coord(double map_pos, double length, double res, int idx) {
-  const double offset = 0.5 * length - 0.5 * res;
-  return (map_pos + offset) + res * (-(double)idx);
-}
+using te::cell_coord;
 
 // Largest index offset that can satisfy the circle test.  A cell at offset R + 1 lies (R + 1) * res from the centre up to a few
 // ulps of the absolute coordinates (~1e-14 m); it can pass `d^2 <= r^2` only if radius / res is within rounding of R + 1, and
@@ -1065,6 +1060,47 @@ int te_check_footprint_paths_polygon2(te_ctx* c, const te_geometry* g_in, const 
   return TE_OK;
 }
 
+// The host-side validation of a te_check_footprint_request request (paths, footprints, radii, conservative caps, finite poses and
+// vertices); sets *mp to the hull input bound of a polygonal item.
+static int check_request_host(const te_geometry* g, const te_footprint_params* p, int32_t npaths, int32_t nposes, const int32_t* path_begin,
+                              const double* poses, const double* radius, int32_t nvertices, const int32_t* footprint_begin,
+                              const float* footprint_xyz, int32_t max_footprint_vertices, const uint8_t* conservative, int* mp_out) {
+  if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
+  if (path_begin[npaths] != nposes) return fail(TE_ERR_BAD_ARG, "path_begin[npaths] = %d != nposes = %d", path_begin[npaths], nposes);
+  if (footprint_begin[0] != 0) return fail(TE_ERR_BAD_ARG, "footprint_begin[0] must be 0, got %d", footprint_begin[0]);
+  if (footprint_begin[npaths] != nvertices)
+    return fail(TE_ERR_BAD_ARG, "footprint_begin[npaths] = %d != nvertices = %d", footprint_begin[npaths], nvertices);
+  for (int32_t q = 0; q < npaths; ++q) {
+    if (path_begin[q + 1] < path_begin[q]) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
+    if (footprint_begin[q + 1] < footprint_begin[q]) return fail(TE_ERR_BAD_ARG, "footprint_begin must be non-decreasing");
+  }
+  int mp = 2;
+  for (int32_t q = 0; q < npaths; ++q) {
+    const int32_t n = path_begin[q + 1] - path_begin[q], nfp = footprint_begin[q + 1] - footprint_begin[q];
+    if (nfp == 0) {  // circular: te_check_footprint_paths_fresh2
+      if (int rc = check_circular_radius(g, p, q, radius[q])) return rc;
+      continue;
+    }
+    // polygonal: te_check_footprint_paths_polygon2
+    if (nfp > max_footprint_vertices)
+      return fail(TE_ERR_BAD_ARG, "footprint of path %d has %d vertices, more than max_footprint_vertices = %d", q, nfp,
+                  max_footprint_vertices);
+    mp = std::max(mp, 2 * nfp);
+    if (conservative && conservative[q] && n > 1) {
+      if ((long long)nfp * n > te::kPolyConsCap)
+        return fail(TE_ERR_UNSUPPORTED, "conservative path %d needs %lld polygon vertices, more than %d", q, (long long)nfp * n,
+                    te::kPolyConsCap);
+      mp = std::max(mp, 2 * nfp * n);
+    }
+    for (size_t k = 7 * (size_t)path_begin[q]; k < 7 * (size_t)path_begin[q + 1]; ++k)
+      if (!std::isfinite(poses[k])) return fail(TE_ERR_BAD_ARG, "pose %zu is not finite", k / 7);
+  }
+  for (int k = 0; k < 3 * nvertices; ++k)
+    if (!std::isfinite(footprint_xyz[k])) return fail(TE_ERR_BAD_ARG, "footprint vertex %d is not finite", k / 3);
+  *mp_out = mp;
+  return TE_OK;
+}
+
 int te_check_footprint_request(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
                                const float* step, const float* rough, const float* elev, const float* robot_slope, int32_t npaths,
                                int32_t nposes, const int32_t* path_begin, const double* poses, const double* radius, int32_t nvertices,
@@ -1092,40 +1128,10 @@ int te_check_footprint_request(te_ctx* c, const te_geometry* g_in, const te_foot
   const bool host = memory != TE_MEM_DEVICE;
   int mp = 2 * std::max(max_footprint_vertices, 1);
   if (conservative && max_footprint_vertices > 0) mp = 2 * te::kPolyConsCap;
-  if (host) {
-    if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
-    if (path_begin[npaths] != nposes) return fail(TE_ERR_BAD_ARG, "path_begin[npaths] = %d != nposes = %d", path_begin[npaths], nposes);
-    if (footprint_begin[0] != 0) return fail(TE_ERR_BAD_ARG, "footprint_begin[0] must be 0, got %d", footprint_begin[0]);
-    if (footprint_begin[npaths] != nvertices)
-      return fail(TE_ERR_BAD_ARG, "footprint_begin[npaths] = %d != nvertices = %d", footprint_begin[npaths], nvertices);
-    for (int32_t q = 0; q < npaths; ++q) {
-      if (path_begin[q + 1] < path_begin[q]) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
-      if (footprint_begin[q + 1] < footprint_begin[q]) return fail(TE_ERR_BAD_ARG, "footprint_begin must be non-decreasing");
-    }
-    mp = 2;
-    for (int32_t q = 0; q < npaths; ++q) {
-      const int32_t n = path_begin[q + 1] - path_begin[q], nfp = footprint_begin[q + 1] - footprint_begin[q];
-      if (nfp == 0) {  // circular: te_check_footprint_paths_fresh2
-        if (int rc = check_circular_radius(g, p, q, radius[q])) return rc;
-        continue;
-      }
-      // polygonal: te_check_footprint_paths_polygon2
-      if (nfp > max_footprint_vertices)
-        return fail(TE_ERR_BAD_ARG, "footprint of path %d has %d vertices, more than max_footprint_vertices = %d", q, nfp,
-                    max_footprint_vertices);
-      mp = std::max(mp, 2 * nfp);
-      if (conservative && conservative[q] && n > 1) {
-        if ((long long)nfp * n > te::kPolyConsCap)
-          return fail(TE_ERR_UNSUPPORTED, "conservative path %d needs %lld polygon vertices, more than %d", q, (long long)nfp * n,
-                      te::kPolyConsCap);
-        mp = std::max(mp, 2 * nfp * n);
-      }
-      for (size_t k = 7 * (size_t)path_begin[q]; k < 7 * (size_t)path_begin[q + 1]; ++k)
-        if (!std::isfinite(poses[k])) return fail(TE_ERR_BAD_ARG, "pose %zu is not finite", k / 7);
-    }
-    for (int k = 0; k < 3 * nvertices; ++k)
-      if (!std::isfinite(footprint_xyz[k])) return fail(TE_ERR_BAD_ARG, "footprint vertex %d is not finite", k / 3);
-  }
+  if (host)
+    if (int rc = check_request_host(g, p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+                                    max_footprint_vertices, conservative, &mp))
+      return rc;
   Staging st(c, host, g_in);
   const float* in[6] = {st.in_layer(trav, g->cols), st.in_layer(slope, g->cols), st.in_layer(step, g->cols), st.in_layer(elev, g->cols),
                         st.in_layer(use_rough ? rough : nullptr, g->cols), st.in_layer(robot_slope, g->cols)};
@@ -1154,6 +1160,302 @@ int te_check_footprint_request(te_ctx* c, const te_geometry* g_in, const te_foot
     for (int32_t q = 0; q < npaths; ++q)
       if (ucount[q] < 0)
         return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);
+  return TE_OK;
+}
+
+// ---- te_map: the layers, the traversability_footprint cache and the isTraversableForFilters memo, resident on the device -------
+struct te_map {
+  te_ctx* ctx = nullptr;
+  bool have_layers = false;
+  te_geometry geo_in{};  // as the layers came (host memory: with their circular-buffer start index)
+  te_geometry geo{};     // the same with the start index cleared: the device layers are in default order
+  DevBuf trav, slope, step, rough, elev, rslope, cache, fresh;
+  bool have_rough = false, have_rslope = false;
+  te::FootprintState fp;  // the map's own scratch; fp.memo is the resident memo
+  bool memo_valid = false;
+  double memo_gap = 0.0, memo_crit = 0.0;
+  int memo_rough = 0;
+  te::MapRequestStats last{};
+};
+
+namespace {
+
+size_t map_cells(const te_map* m) { return (size_t)m->geo.rows * m->geo.cols; }
+
+int map_ready(const te_map* m) {
+  if (!m->have_layers) return fail(TE_ERR_BAD_ARG, "the map has no layers yet: call te_map_chain or te_map_set_layers first");
+  return TE_OK;
+}
+
+// New layers: the geometry, an empty cache and a memo to be rebuilt.
+int map_reset(te_map* m, const te_geometry* g_in, const te_geometry* g) {
+  te_ctx* c = m->ctx;
+  const size_t bytes = sizeof(float) * (size_t)g->rows * g->cols;
+  for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->elev, &m->cache}) TE_CUDA(b->reserve(bytes));
+  TE_CUDA(cudaMemsetAsync(m->cache.p, 0xff, bytes, c->stream));  // all-ones bits: NaN, the empty cache of computeTraversability (:225-228)
+  m->geo_in = *g_in;
+  m->geo = *g;
+  m->memo_valid = false;
+  m->have_layers = false;
+  return TE_OK;
+}
+
+// One layer into the map: host layers are unwrapped from their start index; device layers are copied.
+int map_put_layer(te_map* m, DevBuf& dst, const float* src, int memory) {
+  te_ctx* c = m->ctx;
+  const te_geometry& g = m->geo_in;
+  TE_CUDA(dst.reserve(sizeof(float) * map_cells(m)));
+  if (memory == TE_MEM_HOST) TE_CUDA(upload_cols((float*)dst.p, src, g.rows, g.cols, g.start_row, g.start_col, 0, g.cols, c->stream));
+  else TE_CUDA(cudaMemcpyAsync(dst.p, src, sizeof(float) * map_cells(m), cudaMemcpyDeviceToDevice, c->stream));
+  return TE_OK;
+}
+
+// A map layer out: host layers are re-wrapped to the map's start index (the caller synchronises); device layers are copied.
+int map_get_layer(te_map* m, float* dst, const void* src, int memory) {
+  te_ctx* c = m->ctx;
+  const te_geometry& g = m->geo_in;
+  if (memory == TE_MEM_HOST) TE_CUDA(download_cols(dst, (const float*)src, g.rows, g.cols, g.start_row, g.start_col, 0, g.cols, c->stream));
+  else TE_CUDA(cudaMemcpyAsync(dst, src, sizeof(float) * map_cells(m), cudaMemcpyDeviceToDevice, c->stream));
+  return TE_OK;
+}
+
+// The resident isTraversableForFilters memo for these parameters: kept while the layers and max_gap_width, critical_step_height
+// and verify_roughness (all that checkForStep / checkForSlope / checkForRoughness read) stay the same, cleared otherwise.
+int map_memo(te_map* m, const te_footprint_params* p) {
+  const int rough = p->verify_roughness != 0;
+  if (m->memo_valid && m->memo_gap == p->max_gap_width && m->memo_crit == p->critical_step_height && m->memo_rough == rough) return TE_OK;
+  TE_CUDA(m->fp.memo.reserve(map_cells(m)));
+  TE_CUDA(cudaMemsetAsync(m->fp.memo.p, 0, map_cells(m), m->ctx->stream));
+  m->memo_valid = true;
+  m->memo_gap = p->max_gap_width;
+  m->memo_crit = p->critical_step_height;
+  m->memo_rough = rough;
+  return TE_OK;
+}
+
+int map_footprint_params(const te_map* m, const te_footprint_params* p) {
+  if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
+  if (p->verify_roughness && !m->have_rough)
+    return fail(TE_ERR_MISSING_LAYER, "layer traversability_roughness is missing (verify_roughness is set)");
+  return TE_OK;
+}
+
+#define TE_MAP_ENTER(map)                                   \
+  if (!(map)) return fail(TE_ERR_BAD_ARG, "map is null");   \
+  te_ctx* c = (map)->ctx;                                   \
+  TE_ENTER(c)
+
+}  // namespace
+
+int te_map_create(te_ctx* c, te_map** out) {
+  if (!out) return fail(TE_ERR_BAD_ARG, "out pointer is null");
+  *out = nullptr;
+  TE_ENTER(c);
+  te_map* m = new te_map();
+  m->ctx = c;
+  *out = m;
+  return TE_OK;
+}
+
+int te_map_destroy(te_map* m) {
+  if (!m) return TE_OK;
+  {
+    Guard g(m->ctx);
+    if (g.ok) {
+      cudaStreamSynchronize(m->ctx->stream);
+      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh}) b->release();
+      m->fp.release();
+    }
+  }
+  delete m;
+  return TE_OK;
+}
+
+int te_map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, const float* elev, float* slope, float* step, float* rough,
+                 float* trav, int memory) {
+  TE_MAP_ENTER(m);
+  te_geometry g0;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST, &g0)) return rc;
+  if (int rc = check_params(p)) return rc;
+  if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
+  if (int rc = map_reset(m, g_in, &g0)) return rc;
+  TE_CUDA(m->rough.reserve(sizeof(float) * map_cells(m)));
+  if (int rc = map_put_layer(m, m->elev, elev, memory)) return rc;
+  if (int rc = chain_common(c, &g0, nullptr, p, 1, (const float*)m->elev.p, (float*)m->slope.p, (float*)m->step.p, (float*)m->rough.p,
+                            (float*)m->trav.p, nullptr, nullptr, nullptr, TE_MEM_DEVICE))
+    return rc;
+  m->have_rough = true;
+  m->have_rslope = false;  // computeTraversability leaves robot_slope to a later setTraversabilityMap
+  m->have_layers = true;
+  const std::pair<float*, DevBuf*> outs[4] = {{slope, &m->slope}, {step, &m->step}, {rough, &m->rough}, {trav, &m->trav}};
+  for (const auto& o : outs)
+    if (o.first)
+      if (int rc = map_get_layer(m, o.first, o.second->p, memory)) return rc;
+  if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));
+  return TE_OK;
+}
+
+int te_map_set_layers(te_map* m, const te_geometry* g_in, const float* trav, const float* slope, const float* step, const float* rough,
+                      const float* elev, const float* robot_slope, int memory) {
+  TE_MAP_ENTER(m);
+  te_geometry g0;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST, &g0)) return rc;
+  if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
+  if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
+  if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
+  if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
+  if (int rc = map_reset(m, g_in, &g0)) return rc;
+  if (int rc = map_put_layer(m, m->trav, trav, memory)) return rc;
+  if (int rc = map_put_layer(m, m->slope, slope, memory)) return rc;
+  if (int rc = map_put_layer(m, m->step, step, memory)) return rc;
+  if (int rc = map_put_layer(m, m->elev, elev, memory)) return rc;
+  if (rough)
+    if (int rc = map_put_layer(m, m->rough, rough, memory)) return rc;
+  if (robot_slope)
+    if (int rc = map_put_layer(m, m->rslope, robot_slope, memory)) return rc;
+  m->have_rough = rough != nullptr;
+  m->have_rslope = robot_slope != nullptr;
+  if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));  // the caller may reuse its layers on return
+  m->have_layers = true;
+  return TE_OK;
+}
+
+int te_map_footprint(te_map* m, const te_footprint_params* p, float* out, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (int rc = map_footprint_params(m, p)) return rc;
+  if (!(p->radius >= 0.0) || !(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint radius/offset must be >= 0");
+  const te_geometry* g = &m->geo;
+  if (int rc = ensure_geometry(c, g)) return rc;
+  TE_CUDA(m->fresh.reserve(sizeof(float) * map_cells(m)));
+  const te_slab s{0, g->cols, 0, 0};
+  const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
+  int nl = 0;
+  int rc = te::launch_footprint(m->fp, make_view(c, g, s), g, p, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p,
+                                rough, (const float*)m->elev.p, (float*)m->fresh.p, nullptr, nullptr, nullptr, c->sms, c->stream, &nl);
+  if (rc != 0) return fail(rc, "footprint sweep failed: %s", m->fp.why.c_str());
+  te::launch_map_merge((const float*)m->fresh.p, (float*)m->cache.p, (out && memory == TE_MEM_DEVICE) ? out : nullptr, map_cells(m), c->sms,
+                       c->stream);
+  if (int r2 = launch_check(c, "map footprint", nl + 1)) return r2;
+  if (out && memory == TE_MEM_HOST) {
+    if (int r2 = map_get_layer(m, out, m->cache.p, memory)) return r2;
+    TE_CUDA(cudaStreamSynchronize(c->stream));
+  }
+  return TE_OK;
+}
+
+int te_map_footprint_polygon(te_map* m, const te_footprint_params* p, int32_t npts, const double* pts_xy, double yaw, float* out_x,
+                             float* out_rot, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (int rc = map_footprint_params(m, p)) return rc;
+  if (npts < 3 || npts > 16 || !pts_xy) return fail(TE_ERR_BAD_ARG, "footprint polygon needs 3 to 16 vertices");
+  if (!std::isfinite(yaw)) return fail(TE_ERR_BAD_ARG, "footprint yaw is not finite");
+  for (int k = 0; k < 2 * npts; ++k)
+    if (!std::isfinite(pts_xy[k])) return fail(TE_ERR_BAD_ARG, "footprint polygon vertex is not finite");
+  if (!out_x || !out_rot) return fail(TE_ERR_BAD_ARG, "output layer is null");
+  const te_geometry* g = &m->geo;
+  if (int rc = ensure_geometry(c, g)) return rc;
+  Staging st(c, memory == TE_MEM_HOST, &m->geo_in);
+  float* o[2] = {st.out_layer(out_x, g->cols), st.out_layer(out_rot, g->cols)};
+  if (st.rc) return st.rc;
+  const te_slab s{0, g->cols, 0, 0};
+  const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
+  int nl = 0;
+  int rc = te::launch_footprint_polygon(m->fp, make_view(c, g, s), g, p, npts, pts_xy, yaw, (const float*)m->trav.p, (const float*)m->slope.p,
+                                        (const float*)m->step.p, rough, (const float*)m->elev.p, o[0], o[1], c->sms, c->stream, &nl);
+  if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", m->fp.why.c_str());
+  if (int r2 = launch_check(c, "map polygon footprint", nl)) return r2;
+  return st.finish();
+}
+
+int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int32_t npaths, int32_t nposes, const int32_t* path_begin,
+                                   const double* poses, const double* radius, int32_t nvertices, const int32_t* footprint_begin,
+                                   const float* footprint_xyz, int32_t max_footprint_vertices, const uint8_t* conservative,
+                                   const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area, int32_t max_vertices,
+                                   int32_t* ucount, double* uxy) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (int rc = map_footprint_params(m, p)) return rc;
+  if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
+  if (npaths < 0 || nposes < 0 || nvertices < 0 || !path_begin || !poses || !radius || !footprint_begin ||
+      (nvertices > 0 && !footprint_xyz) || !is_safe || !traversability || !area)
+    return fail(TE_ERR_BAD_ARG, "null argument or negative count");
+  if (max_footprint_vertices < 0 || max_footprint_vertices > te::kPolyMaxVerts)
+    return fail(TE_ERR_BAD_ARG, "max_footprint_vertices must be 0..%d, got %d", te::kPolyMaxVerts, max_footprint_vertices);
+  if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
+  m->last = te::MapRequestStats{};
+  if (npaths == 0) return TE_OK;
+  const te_geometry* g = &m->geo;
+  int mp = 2;
+  if (int rc = check_request_host(g, p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+                                  max_footprint_vertices, conservative, &mp))
+    return rc;
+  if (int rc = ensure_geometry(c, g)) return rc;
+  if (int rc = map_memo(m, p)) return rc;
+  const te::SlabView v = make_view(c, g, te_slab{0, g->cols, 0, 0});
+  const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
+  const float* rslope = m->have_rslope ? (const float*)m->rslope.p : nullptr;
+  int nl = 0;
+  if (nvertices > 0) {  // the polygonal paths (TraversabilityMap.cpp:464-584) read the memo and leave the cache alone
+    Staging st(c, true, g);
+    const int32_t* dpb = st.in(path_begin, (size_t)npaths + 1);
+    const double* dposes = st.in(poses, 7 * (size_t)nposes);
+    const int32_t* dfb = st.in(footprint_begin, (size_t)npaths + 1);
+    const float* dfxyz = st.in(footprint_xyz, 3 * (size_t)nvertices);
+    const uint8_t* dcons = st.in(conservative, (size_t)npaths);
+    const uint8_t* dcup = st.in(cup, (size_t)npaths);
+    uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
+    double* dtrav = st.out(traversability, (size_t)npaths);
+    double* darea = st.out(area, (size_t)npaths);
+    int32_t* dcount = st.out(ucount, (size_t)npaths);
+    double* duxy = st.out(uxy, 2 * (size_t)max_vertices * npaths);
+    if (st.rc) return st.rc;
+    int rc = te::launch_map_polygons(m->fp, v, g, p, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p, rough,
+                                     (const float*)m->elev.p, rslope, npaths, nposes, dpb, dposes, nvertices, dfb, dfxyz,
+                                     max_footprint_vertices, dcons, dcup, mp, dsafe, dtrav, darea, max_vertices, dcount, duxy, c->stream, &nl);
+    if (rc != 0) return fail(rc, "map request (polygonal paths) failed: %s", m->fp.why.c_str());
+    if (int r2 = launch_check(c, "map request (polygonal paths)", nl)) return r2;
+    if (int r2 = st.finish()) return r2;
+  }
+  // the circular paths (TraversabilityMap.cpp:345-462) in request order on the cache; they write their own outputs on the host
+  int rc = te::launch_map_circles(m->fp, v, g, p, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p, rough,
+                                  (const float*)m->elev.p, rslope, (float*)m->cache.p, c->hX.data(), c->hY.data(), npaths, path_begin,
+                                  poses, radius, footprint_begin, cup, is_safe, traversability, area, max_vertices, ucount, uxy, c->stream,
+                                  &nl, &m->last);
+  if (rc != 0) return fail(rc, "map request (circular paths) failed: %s", m->fp.why.c_str());
+  if (int r2 = launch_check(c, "map request (circular paths)", nl)) return r2;
+  if (ucount)  // the row bound of a polygonal path's polygon table (kUntravRows) is only known once the hulls are
+    for (int32_t q = 0; q < npaths; ++q)
+      if (ucount[q] < 0)
+        return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);
+  return TE_OK;
+}
+
+int te_map_get_footprint(te_map* m, float* dst, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (!dst) return fail(TE_ERR_BAD_ARG, "output layer is null");
+  if (memory != TE_MEM_HOST && (m->geo_in.start_row != 0 || m->geo_in.start_col != 0))
+    return fail(TE_ERR_UNSUPPORTED, "the map's layers came with a circular-buffer start index: read its cache into host memory");
+  if (int rc = map_get_layer(m, dst, m->cache.p, memory)) return rc;
+  if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));
+  return TE_OK;
+}
+
+int te_map_clear_footprint(te_map* m) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  TE_CUDA(cudaMemsetAsync(m->cache.p, 0xff, sizeof(float) * map_cells(m), c->stream));
+  return TE_OK;
+}
+
+int te_map_request_stats(te_map* m, int64_t out[3]) {
+  TE_MAP_ENTER(m);
+  if (!out) return fail(TE_ERR_BAD_ARG, "null argument");
+  out[0] = m->last.candidates;
+  out[1] = m->last.keys;
+  out[2] = m->last.stored;
   return TE_OK;
 }
 

@@ -18,6 +18,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <unordered_map>
 
 namespace te {
 namespace {
@@ -69,23 +70,12 @@ __device__ __forceinline__ float lay(const FpArgs& A, const float* l, int i, int
   return __ldg(l + (size_t)lb * A.rows + i);
 }
 
-__device__ __forceinline__ double cell_coord_d(double map_pos, double length, double res, int idx) {
-  const double offset = 0.5 * length - 0.5 * res;
-  return (map_pos + offset) + res * (-(double)idx);
-}
-
 __device__ __forceinline__ bool is_inside_d(const FpArgs& A, double px, double py) {
-  const double tx = -((px - A.posx) - 0.5 * A.lenx);
-  const double ty = -((py - A.posy) - 0.5 * A.leny);
-  return tx >= 0.0 && ty >= 0.0 && tx < A.lenx && ty < A.leny;
+  return grid_is_inside(A, px, py);
 }
 
 __device__ __forceinline__ bool get_index_d(const FpArgs& A, double px, double py, int& i, int& j) {
-  const double vx = ((px - 0.5 * A.lenx) - A.posx) / A.res;
-  const double vy = ((py - 0.5 * A.leny) - A.posy) / A.res;
-  i = (int)(-vx);
-  j = (int)(-vy);
-  return is_inside_d(A, px, py) && i >= 0 && j >= 0 && i < A.rows && j < A.cols_total;
+  return grid_get_index(A, px, py, i, j);
 }
 
 __device__ __forceinline__ void bound_position_d(const FpArgs& A, double& px, double& py) {
@@ -186,7 +176,7 @@ __device__ bool check_step_d(const FpArgs& A, const Layers& L, int i, int j) {
       const int si = k % srows, sj = k / srows;
       const int pi = ti + si, pj = tj + sj;
       if (!(lay(A, L.step, pi, pj) == 0.0f && (double)lay(A, L.elev, pi, pj) < height - crit)) continue;
-      double px = cell_coord_d(spx, slx, A.res, si), py = cell_coord_d(spy, sly, A.res, sj);
+      double px = cell_coord(spx, slx, A.res, si), py = cell_coord(spy, sly, A.res, sj);
       const double vx = px - sx, vy = py - sy;
       if (sqrt(vx * vx + vy * vy) < 0.025) continue;
       if (sqrt(tcx * tcx + tcy * tcy) > 0.025) {
@@ -774,23 +764,6 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
   }
 }
 
-// grid_map::LineIterator (Bresenham) from index (i0, j0) to (i1, j1): `n` cells, (li, lj) the current one.
-struct LineD {
-  int li, lj, i1x, i2x, i1y, i2y, den, num, numAdd, n;
-  __device__ __forceinline__ LineD(int i0, int j0, int i1, int j1) {
-    const int dx = abs(i1 - i0), dy = abs(j1 - j0);
-    i1x = (i1 >= i0) ? 1 : -1; i2x = i1x; i1y = (j1 >= j0) ? 1 : -1; i2y = i1y;
-    if (dx >= dy) { i1x = 0; i2y = 0; den = dx; num = dx / 2; numAdd = dy; n = dx + 1; }
-    else { i2x = 0; i1y = 0; den = dy; num = dy / 2; numAdd = dx; n = dy + 1; }
-    li = i0; lj = j0;
-  }
-  __device__ __forceinline__ void next() {
-    num += numAdd;
-    if (num >= den) { num -= den; li += i1x; lj += i1y; }
-    li += i2x; lj += i2y;
-  }
-};
-
 // Is (a, b) one of the cells checkCircularFootprintPath checks on LineD(i0, j0, i1, j1), i.e. its cell c with c % 4 == 0
 // (nSkip = 3, TraversabilityMap.cpp:401, :421-425)?  Closed form of the walk: after c steps the minor coordinate has moved
 // floor((den / 2 + c * numAdd) / den) cells.
@@ -827,7 +800,7 @@ __device__ bool inclination_ok_d(const FpArgs& A, const float* rslope, double ax
 
 // The running, length-weighted mean of the segment means (TraversabilityMap.cpp:440-452); `lengthPath` (an uninitialised local
 // in the reference) is the running path length.
-__device__ __forceinline__ void add_segment_d(double t, double lx, double ly, int k, double& lengthPath, double& result) {
+__host__ __device__ __forceinline__ void add_segment_d(double t, double lx, double ly, int k, double& lengthPath, double& result) {
   const double lengthSegment = sqrt(lx * lx + ly * ly);
   if (k > 1) {
     const double lengthPreviousPath = lengthPath;
@@ -993,11 +966,11 @@ __device__ FreshCircle fresh_circle_d(const FpArgs& A, const Layers& L, const Pa
   return FreshCircle{true, t, (float)t};
 }
 
-__device__ __forceinline__ bool lex_less_d(double2 a, double2 b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
+__host__ __device__ __forceinline__ bool lex_less_d(double2 a, double2 b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
 
 // grid_map::Polygon::monotoneChainConvexHullOfPoints (recalled) of the m > 3 points `sorted` (already in lexicographic order) into
 // `hull` (2m entries, the reference's own allocation); returns the vertex count.  One thread.
-__device__ int monotone_chain_d(const double2* sorted, int m, double2* hull) {
+__host__ __device__ int monotone_chain_d(const double2* sorted, int m, double2* hull) {
   auto clockwise = [](double2 o, double2 a, double2 b) {
     const double ux = a.x - o.x, uy = a.y - o.y, wx = b.x - o.x, wy = b.y - o.y;
     return (ux * wy - uy * wx) <= 0;
@@ -1164,7 +1137,7 @@ __device__ int spiral_blockers_d(const FpArgs& A, const Layers& L, const PathArg
 // grid_map::Polygon::fromCircle(center, radius) (recalled): vertex j = center + Rotation2D(j * 2 * M_PI / 19) * (radius, 0); the
 // 20 cosines and sines come from the host's libm (launch_check_paths_fresh).  A single pose publishes it as it is; a segment
 // hulls it: 20 points, so every later convexHull with it is the same chain (see write_cells_polygon_d).  One thread.
-__device__ void write_circle_polygon_d(const double* cs, const double* sn, double cx, double cy, double radius, bool hulled,
+__host__ __device__ void write_circle_polygon_d(const double* cs, const double* sn, double cx, double cy, double radius, bool hulled,
                                        double2* pts, const UntravOut& O, int q) {
   const int nc = kFromCircleVertices;
   double2* hull = pts + nc;
@@ -1339,6 +1312,92 @@ __global__ void __launch_bounds__(128) k_check_paths_fresh_poly_req(FpArgs A, La
   __shared__ int2 s_first[4][3];
   const int w = threadIdx.x >> 5;
   check_paths_fresh_d<true, true>(A, L, P, O, C, UntravScratch{s_min[w], s_max[w], s_stack[w], s_first[w]}, R);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// The circular paths of a request on a te_map (launch_map_circles).  The traversability_footprint cache there persists across the
+// paths of a request and across requests, so which isTraversable calls run, and what they read, depends on what earlier calls
+// stored.  The host lists every circle the paths could check (a MapKey per distinct centre, cell, radius and polygon flag);
+// k_map_eval_circles evaluates every key on the cache as the request found it, one warp per key; the host then replays the
+// service loop in order over these records and writes the cells it stored back with k_map_scatter.
+struct MapKey {
+  double cx, cy, rmin;  // isTraversable(center, rmin + offset, cup, ..., rmin)
+  int ci, cj;           // getIndex(center)
+  int cup;              // computeUntraversablePolygon
+  int slot;             // row of the hull table for a cup key, -1: no polygon wanted
+};
+struct MapRecord {
+  double t;       // the walk's traversability output (double), or the cached value
+  float cache;    // what the walk stores at (ci, cj), or the cached value
+  int state;      // 0: walked, traversable; 1: walked, untraversable; 2: the cell was cached when the request began
+  int cnt;        // an untraversable cup walk: the blocked cells it collects (spiral_blockers_d)
+  int nv;         // ... the vertex count of their monotone chain (cnt >= 2; the first min(nv, maxv) vertices are in the hull table)
+  int2 first[3];  // ... the first three of them (map row, map column) in visit order
+};
+
+__global__ void __launch_bounds__(128) k_map_eval_circles(FpArgs A, Layers L, PathArgs P, const MapKey* __restrict__ keys, int nkeys,
+                                                          const float* __restrict__ cache, MapRecord* __restrict__ recs, int maxv,
+                                                          double* __restrict__ hulls) {
+  __shared__ int s_min[4][kFreshTableRows + 1], s_max[4][kFreshTableRows + 1];
+  __shared__ int2 s_stack[4][2 * kFreshTableRows + 4];
+  __shared__ int2 s_first[4][3];
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int k = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (k >= nkeys) return;  // whole warp
+  const MapKey K = keys[k];
+  MapRecord& R = recs[k];
+  const float c0 = __ldg(cache + (size_t)K.cj * A.rows + K.ci);
+  if (finitef(c0)) {  // :673-675
+    if (lane == 0) { R.t = (double)c0; R.cache = c0; R.state = 2; R.cnt = 0; R.nv = 0; }
+    return;
+  }
+  const double rmax = K.rmin + P.offset;
+  const int nr = (int)ceil(rmax / A.res);
+  const FreshCircle f = fresh_circle_d(A, L, P, K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, nr, K.cup != 0);
+  int cnt = 0, nv = 0;
+  if (K.cup && !f.ok && K.slot >= 0) {  // a cup walk fails only within rmin: it collects the blocked cells (:687-730)
+    const UntravScratch S{s_min[w], s_max[w], s_stack[w], s_first[w]};
+    cnt = spiral_blockers_d(A, L, P, S, K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, nr);
+    if (lane == 0) {
+      for (int v = 0; v < min(cnt, 3); ++v) R.first[v] = S.first[v];
+      if (cnt >= 2) {
+        const int a0 = K.ci - nr;
+        nv = table_chain_d(A, S.tmin, S.tmax, 2 * nr + 1, a0, S.stack);
+        double* xy = hulls + 2 * (size_t)maxv * K.slot;
+        for (int v = 0; v < min(nv, maxv); ++v) {
+          xy[2 * v] = A.X[a0 + S.stack[v].x];
+          xy[2 * v + 1] = A.Y[S.stack[v].y];
+        }
+      }
+    }
+  }
+  if (lane == 0) { R.t = f.t; R.cache = f.cache; R.state = f.ok ? 0 : 1; R.cnt = cnt; R.nv = nv; }
+}
+
+// checkInclination of every pose (x, y, x, y) or segment (start, end) the host lists, one thread each.
+__global__ void __launch_bounds__(128) k_map_inclination(FpArgs A, const float* __restrict__ rslope, const double4* __restrict__ seg,
+                                                         int nseg, unsigned char* __restrict__ ok) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= nseg) return;
+  const double4 s = seg[k];
+  ok[k] = inclination_ok_d(A, rslope, s.x, s.y, s.z, s.w) ? 1 : 0;
+}
+
+// The cells the replay stored, written into the cache.
+__global__ void __launch_bounds__(256) k_map_scatter(float* __restrict__ cache, const unsigned long long* __restrict__ cell,
+                                                     const float* __restrict__ value, int n) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) cache[cell[k]] = value[k];
+}
+
+// traversabilityFootprint(radius, offset) on a cache: a cached cell takes the memoised branch and keeps its value, every other cell
+// gets the sweep's.  `out` (may be null or `cache` itself) receives the cache afterwards.
+__global__ void __launch_bounds__(256) k_map_merge(float* cache, const float* __restrict__ fresh, float* out, size_t n) {
+  for (size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x; c < n; c += (size_t)gridDim.x * blockDim.x) {
+    const float v = finitef(cache[c]) ? cache[c] : fresh[c];
+    cache[c] = v;
+    if (out) out[c] = v;
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -1761,7 +1820,7 @@ std::vector<int> build_spiral(double radius, double res) {
 }  // namespace
 
 void FootprintState::release() {
-  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly[0], &poly[1], &rings, &memo, &items, &upoly}) b->release();
+  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly[0], &poly[1], &rings, &memo, &items, &upoly, &mapbuf}) b->release();
   tables_valid = false;
   valid = false;
 }
@@ -1959,6 +2018,26 @@ int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_g
                                 launches, U);
 }
 
+namespace {
+// The polygonal paths of a request: k_check_polygon_items(_poly)_req and the combine kernel, on the predicate memo in st.memo.
+int launch_request_polygons(FootprintState& st, const FpArgs& a, const Layers& L, const te_footprint_params* p, const float* robot_slope,
+                            int npaths, int nposes, const int* path_begin, const double* poses, const RequestArgs& R,
+                            const unsigned char* conservative, const unsigned char* cup, int max_points, unsigned char* is_safe,
+                            double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s,
+                            int* launches) {
+  PolyPathArgs P;
+  if (int rc = polygon_args(st, p, robot_slope, npaths, nposes, max_points, path_begin, poses, conservative, is_safe, trav_out, area_out, &P))
+    return rc;
+  if (!ucount)
+    return launch_polygon_kernels(st, k_check_polygon_items_req, k_check_polygon_combine_req, "k_check_polygon_items_req", false, a, L, P,
+                                  s, launches, R);
+  PolyUntravArgs U;
+  if (int rc = polygon_untrav_args(st, nposes, cup, max_vertices, ucount, uxy, &U)) return rc;
+  return launch_polygon_kernels(st, k_check_polygon_items_poly_req, k_check_polygon_combine_poly_req, "k_check_polygon_items_poly_req", true,
+                                a, L, P, s, launches, U, R);
+}
+}  // namespace
+
 int launch_check_request(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
                          const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
                          int npaths, int nposes, const int* path_begin, const double* poses, const double* radius, int nvertices,
@@ -1976,24 +2055,275 @@ int launch_check_request(FootprintState& st, const SlabView& v, const te_geometr
   const FpArgs a = filter_args(v, g, p, rough);
   const Layers L{trav, slope, step, elev, rough};
   const RequestArgs R{footprint_begin, footprint_xyz, nvertices, max_footprint_vertices, nposes, area_out};
-  PolyPathArgs P;
-  if (int rc = polygon_args(st, p, robot_slope, npaths, nposes, max_points, path_begin, poses, conservative, is_safe, trav_out, area_out, &P))
-    return rc;
-  PolyUntravArgs U;
-  if (ucount)
-    if (int rc = polygon_untrav_args(st, nposes, cup, max_vertices, ucount, uxy, &U)) return rc;
   const PathArgs C = fresh_args(st, p, robot_slope, npaths, path_begin, poses, radius, cup, is_safe, trav_out);
   const unsigned blocks = (unsigned)((32LL * npaths + 127) / 128);
-  if (!ucount) {
-    k_check_paths_fresh_req<<<blocks, 128, 0, s>>>(a, L, C, R);
-    ++*launches;
-    return launch_polygon_kernels(st, k_check_polygon_items_req, k_check_polygon_combine_req, "k_check_polygon_items_req", false, a, L, P,
-                                  s, launches, R);
-  }
-  k_check_paths_fresh_poly_req<<<blocks, 128, 0, s>>>(a, L, C, UntravOut{max_vertices, ucount, uxy}, circle_table(), R);
+  if (!ucount) k_check_paths_fresh_req<<<blocks, 128, 0, s>>>(a, L, C, R);
+  else k_check_paths_fresh_poly_req<<<blocks, 128, 0, s>>>(a, L, C, UntravOut{max_vertices, ucount, uxy}, circle_table(), R);
   ++*launches;
-  return launch_polygon_kernels(st, k_check_polygon_items_poly_req, k_check_polygon_combine_poly_req, "k_check_polygon_items_poly_req", true,
-                                a, L, P, s, launches, U, R);
+  return launch_request_polygons(st, a, L, p, robot_slope, npaths, nposes, path_begin, poses, R, conservative, cup, max_points, is_safe,
+                                 trav_out, area_out, max_vertices, ucount, uxy, s, launches);
+}
+
+int launch_map_polygons(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                        const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                        int npaths, int nposes, const int* path_begin, const double* poses, int nvertices, const int* footprint_begin,
+                        const float* footprint_xyz, int max_footprint_vertices, const unsigned char* conservative,
+                        const unsigned char* cup, int max_points, unsigned char* is_safe, double* trav_out, double* area_out,
+                        int max_vertices, int* ucount, double* uxy, cudaStream_t s, int* launches) {
+  *launches = 0;
+  if (max_footprint_vertices < 1 || max_footprint_vertices > kPolyMaxVerts || max_points < 2 || max_points > 2 * kPolyConsCap) {
+    st.why = "bad footprint size";
+    return TE_ERR_BAD_ARG;
+  }
+  const FpArgs a = filter_args(v, g, p, rough);
+  const Layers L{trav, slope, step, elev, rough};
+  const RequestArgs R{footprint_begin, footprint_xyz, nvertices, max_footprint_vertices, nposes, area_out};
+  return launch_request_polygons(st, a, L, p, robot_slope, npaths, nposes, path_begin, poses, R, conservative, cup, max_points, is_safe,
+                                 trav_out, area_out, max_vertices, ucount, uxy, s, launches);
+}
+
+namespace {
+// The identity of an isTraversable call on an empty cell: its centre, cell, radius and polygon flag, bit for bit.
+struct MapKeyBits {
+  unsigned long long cx, cy, r;
+  int ci, cj, cup;
+  bool operator==(const MapKeyBits& o) const { return cx == o.cx && cy == o.cy && r == o.r && ci == o.ci && cj == o.cj && cup == o.cup; }
+};
+struct MapKeyHash {
+  size_t operator()(const MapKeyBits& k) const {
+    unsigned long long h = k.cx * 0x9E3779B97F4A7C15ULL;
+    h = (h ^ (h >> 29)) + k.cy * 0xBF58476D1CE4E5B9ULL;
+    h = (h ^ (h >> 31)) + k.r * 0x94D049BB133111EBULL;
+    h ^= ((unsigned long long)(unsigned)k.ci << 33) ^ ((unsigned long long)(unsigned)k.cj << 1) ^ (unsigned long long)k.cup;
+    return (size_t)(h ^ (h >> 32));
+  }
+};
+unsigned long long dbits(double d) {
+  unsigned long long u;
+  std::memcpy(&u, &d, sizeof(u));
+  return u;
+}
+size_t align16(size_t b) { return (b + 15) / 16 * 16; }
+}  // namespace
+
+int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                       const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                       float* cache, const double* hX, const double* hY, int npaths, const int* path_begin, const double* poses,
+                       const double* radius, const int* footprint_begin, const unsigned char* cup, unsigned char* is_safe,
+                       double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s, int* launches,
+                       MapRequestStats* stats) {
+  *launches = 0;
+  *stats = MapRequestStats{};
+  const GridGeo G{g->rows, g->cols, g->resolution, g->length_x, g->length_y, g->position_x, g->position_y};
+  const bool want_poly = ucount != nullptr;
+  const int maxv = std::max(max_vertices, 1);
+  auto circular = [&](int q) { return footprint_begin[q + 1] == footprint_begin[q]; };
+  auto pose = [&](int k) { return poses + 7 * (size_t)k; };
+
+  // 1. every circle the circular paths could check, deduplicated, and every pose / segment checkInclination could read
+  std::unordered_map<MapKeyBits, int, MapKeyHash> index;
+  std::vector<MapKey> keys;
+  std::vector<double4> segs;
+  std::vector<int> seg_of_pose(robot_slope ? (size_t)path_begin[npaths] : 0, -1);
+  int nslots = 0;
+  auto key_of = [&](double cx, double cy, int ci, int cj, double rmin, bool c, bool insert) -> int {
+    const MapKeyBits kb{dbits(cx), dbits(cy), dbits(rmin), ci, cj, c ? 1 : 0};
+    auto it = index.find(kb);
+    if (it != index.end()) return it->second;
+    if (!insert) return -1;
+    keys.push_back(MapKey{cx, cy, rmin, ci, cj, c ? 1 : 0, (c && want_poly) ? nslots++ : -1});
+    index.emplace(kb, (int)keys.size() - 1);
+    return (int)keys.size() - 1;
+  };
+  for (int q = 0; q < npaths; ++q) {
+    if (!circular(q)) continue;
+    const int b = path_begin[q], n = path_begin[q + 1] - b;
+    const bool c = cup && cup[q];
+    for (int k = 0; k < n; ++k) {
+      const double ex = pose(b + k)[0], ey = pose(b + k)[1];
+      if (n == 1) {
+        if (robot_slope) { seg_of_pose[b] = (int)segs.size(); segs.push_back(make_double4(ex, ey, ex, ey)); }
+        int i, j;
+        if (grid_get_index(G, ex, ey, i, j)) { key_of(ex, ey, i, j, radius[q], c, true); ++stats->candidates; }
+        continue;
+      }
+      if (k == 0) continue;
+      const double sx = pose(b + k - 1)[0], sy = pose(b + k - 1)[1];
+      if (robot_slope) { seg_of_pose[b + k] = (int)segs.size(); segs.push_back(make_double4(sx, sy, ex, ey)); }
+      int si, sj, ei, ej;
+      if (!grid_get_index(G, sx, sy, si, sj) || !grid_get_index(G, ex, ey, ei, ej)) continue;
+      LineD line(ei, ej, si, sj);
+      for (int cc = 0; cc < line.n; ++cc, line.next())
+        if ((cc & 3) == 0) { key_of(hX[line.li], hY[line.lj], line.li, line.lj, radius[q], c, true); ++stats->candidates; }
+    }
+  }
+  stats->keys = (long long)keys.size();
+
+  // 2. one launch walks every key on the cache as the request found it; a second checks the inclinations
+  const int nkeys = (int)keys.size(), nseg = (int)segs.size();
+  std::vector<MapRecord> recs(nkeys);
+  std::vector<unsigned char> incl(nseg);
+  std::vector<double> hulls(want_poly ? 2 * (size_t)maxv * nslots : 0);
+  if (nkeys > 0 || nseg > 0) {
+    if (int rc = ensure_ring_table(st, s)) return rc;
+    const size_t o_keys = 0, o_segs = align16(o_keys + sizeof(MapKey) * nkeys), o_recs = align16(o_segs + sizeof(double4) * nseg);
+    const size_t o_incl = align16(o_recs + sizeof(MapRecord) * nkeys), o_hull = align16(o_incl + nseg);
+    const size_t bytes = o_hull + sizeof(double) * hulls.size();
+    if (st.mapbuf.reserve(std::max<size_t>(bytes, 16)) != cudaSuccess) { st.why = "allocating the map request records failed"; return TE_ERR_CUDA; }
+    char* base = (char*)st.mapbuf.p;
+    if (cudaMemcpyAsync(base + o_keys, keys.data(), sizeof(MapKey) * nkeys, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+        cudaMemcpyAsync(base + o_segs, segs.data(), sizeof(double4) * nseg, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+      st.why = "map request upload failed";
+      return TE_ERR_CUDA;
+    }
+    FpArgs a = filter_args(v, g, p, rough);
+    const Layers L{trav, slope, step, elev, rough};
+    const PathArgs P = fresh_args(st, p, robot_slope, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+    if (nkeys > 0) {
+      k_map_eval_circles<<<(unsigned)((32LL * nkeys + 127) / 128), 128, 0, s>>>(a, L, P, (const MapKey*)(base + o_keys), nkeys, cache,
+                                                                               (MapRecord*)(base + o_recs), maxv, (double*)(base + o_hull));
+      ++*launches;
+    }
+    if (nseg > 0) {
+      k_map_inclination<<<(unsigned)((nseg + 127) / 128), 128, 0, s>>>(a, robot_slope, (const double4*)(base + o_segs), nseg,
+                                                                      (unsigned char*)(base + o_incl));
+      ++*launches;
+    }
+    if (cudaMemcpyAsync(recs.data(), base + o_recs, sizeof(MapRecord) * nkeys, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaMemcpyAsync(incl.data(), base + o_incl, nseg, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaMemcpyAsync(hulls.data(), base + o_hull, sizeof(double) * hulls.size(), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaStreamSynchronize(s) != cudaSuccess) {
+      st.why = "map request records failed";
+      return TE_ERR_CUDA;
+    }
+  }
+
+  // 3. the service loop in request order (checkCircularFootprintPath, TraversabilityMap.cpp:345-462, with publishPolygons = true)
+  // over the records: a cell this request stored reads the overlay, any other cell its own key's record
+  std::unordered_map<unsigned long long, float> overlay;
+  std::vector<unsigned long long> order;  // overlay cells in the order they were stored
+  const CircleTable CT = circle_table();
+  const double tdefault = p->traversability_default, offset = p->offset;
+  for (int q = 0; q < npaths; ++q) {
+    if (!circular(q)) continue;
+    const int b = path_begin[q], n = path_begin[q + 1] - b;
+    const double rmin = radius[q], rmax = rmin + offset;
+    const bool c = cup && cup[q];
+    // isTraversable(center, rmax, c, t, ..., rmin) (:654-746); `cell` < 0: the centre is outside the map
+    int fkind = 0, fkey = -1, freps = 1;  // the failing circle: 0 none, 1 fromCircle(fx, fy), 2 the blocked cells of key fkey
+    double fx = 0.0, fy = 0.0;
+    auto check = [&](double cx, double cy, int ci, int cj, bool inside, double& t) -> bool {
+      if (!inside) {  // :662-667
+        t = tdefault;
+        if (tdefault == 0.0) { fkind = 1; fx = cx; fy = cy; }
+        return tdefault != 0.0;
+      }
+      const unsigned long long cell = (unsigned long long)cj * g->rows + ci;
+      float cached;
+      bool have = false;
+      auto ov = overlay.find(cell);
+      const int k = key_of(cx, cy, ci, cj, rmin, c, false);
+      if (ov != overlay.end()) { cached = ov->second; have = true; }
+      else if (recs[k].state == 2) { cached = recs[k].cache; have = true; }
+      if (have) {  // :673-678
+        t = (double)cached;
+        if (cached == 0.0f) { fkind = 1; fx = cx; fy = cy; }
+        return cached != 0.0f;
+      }
+      const MapRecord& r = recs[k];  // the first check of the cell: the walk (:679-736) stores its value
+      overlay.emplace(cell, r.cache);
+      order.push_back(cell);
+      t = r.t;
+      if (r.state == 1) { fkind = 2; fkey = k; fx = cx; fy = cy; }
+      return r.state == 0;
+    };
+    double result = 0.0, lengthPath = 0.0;
+    double sx = 0.0, sy = 0.0, ex = 0.0, ey = 0.0;
+    bool ok = n > 0;
+    for (int k = 0; k < n && ok; ++k) {
+      sx = ex; sy = ey;
+      ex = pose(b + k)[0]; ey = pose(b + k)[1];
+      if (n == 1) {  // :365-387
+        if (robot_slope && !incl[seg_of_pose[b]]) { ok = false; break; }
+        int i, j;
+        const bool inside = grid_get_index(G, ex, ey, i, j);
+        ok = check(ex, ey, i, j, inside, result);
+      }
+      if (n > 1 && k > 0) {  // :389-457
+        if (robot_slope && !incl[seg_of_pose[b + k]]) { ok = false; break; }
+        int si, sj, ei, ej;
+        if (!grid_get_index(G, sx, sy, si, sj) || !grid_get_index(G, ex, ey, ei, ej)) { ok = false; break; }
+        LineD line(ei, ej, si, sj);
+        int nLine = 0;
+        double sum = 0.0;
+        for (int cc = 0; cc < line.n && ok; ++cc, line.next()) {
+          if (cc & 3) continue;
+          double t;
+          ok = check(hX[line.li], hY[line.lj], line.li, line.lj, true, t);
+          // the failing circle's polygon is hulled into the path's once for itself and once per later checked cell (:407-412)
+          if (!ok) freps = (line.n - 1) / 4 - cc / 4 + 1;
+          sum += t;
+          ++nLine;
+        }
+        if (!ok) break;  // :414-417, :453-456
+        add_segment_d(sum / (double)nLine, ex - sx, ey - sy, k, lengthPath, result);
+      }
+    }
+    is_safe[q] = ok ? 1 : 0;
+    trav_out[q] = ok ? result : 0.0;
+    area_out[q] = 0.0;
+    if (!want_poly) continue;
+    // the last non-empty polygon published for the path: only an untraversable circle has one (inclination failures return first)
+    if (!c || ok || fkind == 0) {
+      ucount[q] = 0;
+    } else if (fkind == 1) {
+      double2 pts[3 * kFromCircleVertices];
+      write_circle_polygon_d(CT.cs, CT.sn, fx, fy, rmax, n > 1, pts, UntravOut{max_vertices, ucount, uxy}, q);
+    } else {  // as write_cells_polygon_d, from the record
+      const MapRecord& r = recs[fkey];
+      double* xy = uxy + 2 * (size_t)max_vertices * q;
+      if (r.cnt >= 4 || (r.cnt >= 2 && freps >= 2)) {
+        ucount[q] = r.nv;
+        const double* h = hulls.data() + 2 * (size_t)maxv * keys[fkey].slot;
+        for (int u = 0; u < std::min(r.nv, max_vertices); ++u) { xy[2 * u] = h[2 * u]; xy[2 * u + 1] = h[2 * u + 1]; }
+      } else {
+        const int nv = (r.cnt == 1 && freps >= 2) ? 2 + (freps & 1) : r.cnt;
+        ucount[q] = nv;
+        for (int u = 0; u < std::min(nv, max_vertices); ++u) {
+          const int2 cl = r.first[r.cnt == 1 ? 0 : u];
+          xy[2 * u] = hX[cl.x];
+          xy[2 * u + 1] = hY[cl.y];
+        }
+      }
+    }
+  }
+
+  // 4. the cells the replay stored go into the device cache
+  const int nw = (int)order.size();
+  stats->stored = nw;
+  if (nw > 0) {
+    std::vector<unsigned long long> cells(order);
+    std::vector<float> vals(nw);
+    for (int k = 0; k < nw; ++k) vals[k] = overlay.at(order[k]);
+    const size_t o_vals = align16(sizeof(unsigned long long) * nw);
+    if (st.mapbuf.reserve(o_vals + sizeof(float) * nw) != cudaSuccess) { st.why = "allocating the cache update failed"; return TE_ERR_CUDA; }
+    char* base = (char*)st.mapbuf.p;
+    if (cudaMemcpyAsync(base, cells.data(), sizeof(unsigned long long) * nw, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+        cudaMemcpyAsync(base + o_vals, vals.data(), sizeof(float) * nw, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+      st.why = "cache update upload failed";
+      return TE_ERR_CUDA;
+    }
+    k_map_scatter<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(cache, (const unsigned long long*)base, (const float*)(base + o_vals), nw);
+    ++*launches;
+    if (cudaStreamSynchronize(s) != cudaSuccess) { st.why = "cache update failed"; return TE_ERR_CUDA; }  // cells / vals are freed
+  }
+  return 0;
+}
+
+int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, int sms, cudaStream_t s) {
+  const long long blocks = std::min<long long>((long long)((n + 255) / 256), (long long)sms * 8);
+  k_map_merge<<<(unsigned)std::max(blocks, 1LL), 256, 0, s>>>(cache, fresh, out, n);
+  return 0;
 }
 
 // isTraversableForFilters for every cell of the slab + halo into st.block (k_pred_classify + k_pred_heavy); fills the geometry /

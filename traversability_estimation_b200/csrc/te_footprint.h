@@ -5,6 +5,7 @@
 #include <vector>
 #include "../../include/te_b200.h"
 #include "te_device.cuh"
+#include "te_grid.cuh"
 #include "te_kernels.h"
 
 namespace te {
@@ -31,6 +32,7 @@ struct FootprintState {
   DevBuf memo;    // fresh and polygonal path checks: per-cell isTraversableForFilters memo of one call
   DevBuf items;   // polygonal path checks: one result record per pose index
   DevBuf upoly;   // polygonal path checks with untraversable polygons: per pose index a vertex count and max_vertices points
+  DevBuf mapbuf;  // map requests: circle keys, inclination segments, their records and hulls; then the cache cells to store
   void invalidate() { valid = false; tables_valid = false; }
   void release();
 };
@@ -85,5 +87,30 @@ int launch_check_request(FootprintState& st, const SlabView& v, const te_geometr
                          const unsigned char* conservative, const unsigned char* cup, int max_points, unsigned char* is_safe,
                          double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s,
                          int* launches);
+
+// A request on a te_map (te_map_check_footprint_request).  Its polygonal paths: the polygonal half of launch_check_request on the
+// memo in st.memo, which the caller keeps (device pointers).  Its circular paths: launch_map_circles reads and fills the
+// traversability_footprint cache `cache` (device, NaN = empty) in the reference's order; every path array and output is in HOST
+// memory, hX / hY are the host copies of the cell-centre tables, and the call returns synchronised.
+int launch_map_polygons(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                        const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                        int npaths, int nposes, const int* path_begin, const double* poses, int nvertices, const int* footprint_begin,
+                        const float* footprint_xyz, int max_footprint_vertices, const unsigned char* conservative,
+                        const unsigned char* cup, int max_points, unsigned char* is_safe, double* trav_out, double* area_out,
+                        int max_vertices, int* ucount, double* uxy, cudaStream_t s, int* launches);
+struct MapRequestStats {
+  long long candidates = 0;  // isTraversable calls the circular paths could make
+  long long keys = 0;        // distinct circles among them (what k_map_eval_circles evaluates)
+  long long stored = 0;      // cache cells the request stored
+};
+int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+                       const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                       float* cache, const double* hX, const double* hY, int npaths, const int* path_begin, const double* poses,
+                       const double* radius, const int* footprint_begin, const unsigned char* cup, unsigned char* is_safe,
+                       double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s, int* launches,
+                       MapRequestStats* stats);
+// traversabilityFootprint(radius, offset) on a cache: cache = finite(cache) ? cache : fresh over n cells; `out` (device, may be
+// null) receives the result too.
+int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, int sms, cudaStream_t s);
 
 }  // namespace te
