@@ -115,11 +115,12 @@ struct FusedArgs {
   float rough_crit, inv_rough_crit, minv_rough_crit;
   float fuse_w;
   float cond_k;     // eigen-gap / scale ratio below which the fp32 eigenvector is not trusted
-  // constants pre-broadcast to both halves of a register pair (one LDC.64 each)
-  f2 k_invN, k_minvN, k_kp, k_half_a, k_nnm1, k_rough_thr, k_minv_slope, k_minv_rough, k_m0, k_m1;
-  f2 k_inv_ncrit, k_minv_step, k_fuse_w;
-  f2 k_1em5, k_1em10a, k_mcond, k_2p24, k_7p1em6, k_2em6, k_1em3;
-  f2 k_one, k_mone, k_two, k_half, k_mhalf, k_1p5, k_0375, k_m03125, k_p0, k_p1, k_p2, k_p3, k_p4, k_p5, k_p6, k_p7;
+  // constants of the row-pair arithmetic, one float each: both halves of a pair operation take the same constant-bank word
+  // as a direct FFMA/FADD/FMUL operand, so a constant costs no load and no register
+  float k_invN, k_kp, k_half_a, k_nnm1, k_rough_thr, k_m0, k_m1;
+  float k_inv_ncrit, k_fuse_w;
+  float k_1em5, k_1em10a, k_mcond, k_2p24, k_7p1em6, k_2em6, k_bmargin;
+  float k_one, k_two, k_half, k_1p5, k_0375, k_m03125, k_p0, k_p1, k_p2, k_p3, k_p4, k_p5, k_p6, k_p7;
   const unsigned char* rowmask;  // per global row: bit0/1 pass-1 tips (-2,0)/(+2,0); bit2/3 pass-2 tips
   const unsigned char* colmask;  // per global column, same bits for (0,-2)/(0,+2)
   float* slope;
@@ -159,6 +160,16 @@ __device__ __forceinline__ f2 add2(f2 a, f2 b) { return mk(__fadd_rn(lo(a), lo(b
 __device__ __forceinline__ f2 sub2(f2 a, f2 b) { return mk(__fsub_rn(lo(a), lo(b)), __fsub_rn(hi(a), hi(b))); }
 __device__ __forceinline__ f2 mul2(f2 a, f2 b) { return mk(__fmul_rn(lo(a), lo(b)), __fmul_rn(hi(a), hi(b))); }
 __device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return mk(__fmaf_rn(lo(a), lo(b), lo(c)), __fmaf_rn(hi(a), hi(b), hi(c))); }
+// a scalar constant k (a FusedArgs member) as one operand of both halves; the operand order of each scalar instruction is
+// the one the pair form with a broadcast constant had, so the results are the same bits
+__device__ __forceinline__ f2 mul2c(f2 a, float k) { return mk(__fmul_rn(lo(a), k), __fmul_rn(hi(a), k)); }
+__device__ __forceinline__ f2 sub2c(f2 a, float k) { return mk(__fsub_rn(lo(a), k), __fsub_rn(hi(a), k)); }
+__device__ __forceinline__ f2 csub2(float k, f2 a) { return mk(__fsub_rn(k, lo(a)), __fsub_rn(k, hi(a))); }
+__device__ __forceinline__ f2 fma2c(f2 a, f2 b, float k) { return mk(__fmaf_rn(lo(a), lo(b), k), __fmaf_rn(hi(a), hi(b), k)); }
+__device__ __forceinline__ f2 fma2k(f2 a, float k, f2 c) { return mk(__fmaf_rn(lo(a), k, lo(c)), __fmaf_rn(hi(a), k, hi(c))); }
+__device__ __forceinline__ f2 kfma2(float k, f2 b, f2 c) { return mk(__fmaf_rn(k, lo(b), lo(c)), __fmaf_rn(k, hi(b), hi(c))); }
+__device__ __forceinline__ f2 fma2kc(f2 a, float k, float c) { return mk(__fmaf_rn(lo(a), k, c), __fmaf_rn(hi(a), k, c)); }
+__device__ __forceinline__ f2 kmul2(float k, f2 b) { return mk(__fmul_rn(k, lo(b)), __fmul_rn(k, hi(b))); }
 __device__ __forceinline__ f2 bc(float v) { return mk(v, v); }
 __device__ __forceinline__ f2 neg2(f2 a) { return a ^ 0x8000000080000000ull; }
 // -a for both rows, written as two scalar negations: ptxas folds each into the operand modifier of the consuming
@@ -350,18 +361,25 @@ struct Normal2 {
 // acos on [0,1] for both rows: sqrt(1-x) * P7(x) (Abramowitz-Stegun 4.4.46 form, coefficients refitted for
 // relative error; float32 evaluation: max abs error 2.2e-7, max rel. error 1.7e-7).  Branch-free.
 __device__ __forceinline__ f2 acos2(const FusedArgs& A, f2 x) {
-  const f2 u = sub2(A.k_one, x);
+  const f2 u = csub2(A.k_one, x);
   const f2 sq = mk(sqrt_a(lo(u)), sqrt_a(hi(u)));
-  f2 p = fma2(x, A.k_p7, A.k_p6);
-  p = fma2(p, x, A.k_p5);
-  p = fma2(p, x, A.k_p4);
-  p = fma2(p, x, A.k_p3);
-  p = fma2(p, x, A.k_p2);
-  p = fma2(p, x, A.k_p1);
-  p = fma2(p, x, A.k_p0);
+  f2 p = fma2kc(x, A.k_p7, A.k_p6);
+  p = fma2c(p, x, A.k_p5);
+  p = fma2c(p, x, A.k_p4);
+  p = fma2c(p, x, A.k_p3);
+  p = fma2c(p, x, A.k_p2);
+  p = fma2c(p, x, A.k_p1);
+  p = fma2c(p, x, A.k_p0);
   return mul2(sq, p);
 }
 
+// h >= 0 ? a : b as one FSEL on a comparison ptxas shares between the selects of a row (a C conditional becomes a MOV and a
+// predicated MOV)
+__device__ __forceinline__ float sel_ge0(float h, float a, float b) {
+  float r;
+  asm("{ .reg .pred p; setp.ge.f32 p, %1, 0f00000000; selp.f32 %0, %2, %3, p; }" : "=f"(r) : "f"(h), "f"(a), "f"(b));
+  return r;
+}
 // NaN-propagating min (a NaN margin must fail the certification)
 __device__ __forceinline__ float min2n(float a, float b) {
   float r;
@@ -372,18 +390,18 @@ __device__ __forceinline__ float min2n(float a, float b) {
 // window for both rows of the lane, slope and roughness layers, and the certification of all of it.
 __device__ __forceinline__ Normal2 finish_normal2(const FusedArgs& A, f2 Sw, f2 Sk, f2 Sl, f2 Sww, f2 ec) {
   Normal2 o;
-  const f2 mw = mul2(Sw, A.k_invN);
-  const f2 c = fma2(negf2(mw), mw, mul2(Sww, A.k_invN));  // Czz = Sww/N - (Sw/N)^2
-  const f2 p = mul2(Sk, A.k_kp), q = mul2(Sl, A.k_kp);               // Cxz, Cyz
+  const f2 mw = mul2c(Sw, A.k_invN);
+  const f2 c = fma2(negf2(mw), mw, mul2c(Sww, A.k_invN));  // Czz = Sww/N - (Sw/N)^2
+  const f2 p = mul2c(Sk, A.k_kp), q = mul2c(Sl, A.k_kp);               // Cxz, Cyz
   const f2 g2 = fma2(p, p, mul2(q, q));
-  const f2 h = fma2(negf2(c), A.k_half, A.k_half_a);                  // (a - c)/2
+  const f2 h = fma2kc(negf2(c), A.k_half, A.k_half_a);                  // (a - c)/2
   const f2 hh = fma2(h, h, g2);
 #if TE_NOCORR & 1
   const f2 D = mk(sqrt_a(lo(hh)), sqrt_a(hi(hh)));
 #else
   const f2 rD = mk(rsq_a(lo(hh)), rsq_a(hi(hh)));
   const f2 D0 = mul2(hh, rD);
-  const f2 D = fma2(fma2(negf2(D0), D0, hh), mul2(rD, A.k_half), D0);  // sqrt(hh), one correction
+  const f2 D = fma2(fma2(negf2(D0), D0, hh), mul2c(rD, A.k_half), D0);  // sqrt(hh), one correction
 #endif
   const float h0 = lo(h), h1 = hi(h);
   const f2 dph = add2(D, mk(fabsf(h0), fabsf(h1)));
@@ -395,8 +413,8 @@ __device__ __forceinline__ Normal2 finish_normal2(const FusedArgs& A, f2 Sw, f2 
   const f2 qq = fma2(fma2(negf2(q0), dph, g2), rq, q0);  // g2 / dph, one correction
 #endif
   const bool hx = h0 >= 0.f, hy = h1 >= 0.f;
-  const f2 m = mk(hx ? lo(dph) : lo(qq), hy ? hi(dph) : hi(qq));  // a - lambda0
-  const f2 cmag = mk(hx ? lo(c) : A.a_cov, hy ? hi(c) : A.a_cov);
+  const f2 m = mk(sel_ge0(h0, lo(dph), lo(qq)), sel_ge0(h1, hi(dph), hi(qq)));  // a - lambda0
+  const f2 cmag = mk(sel_ge0(h0, lo(c), A.a_cov), sel_ge0(h1, hi(c), A.a_cov));
   const f2 lam0 = sub2(cmag, qq);                                  // smallest eigenvalue
   const f2 m2 = mul2(m, m);
   const f2 nn = add2(m2, g2);
@@ -405,7 +423,7 @@ __device__ __forceinline__ Normal2 finish_normal2(const FusedArgs& A, f2 Sw, f2 
   const f2 den = mul2(Nn, add2(m, Nn));
   const f2 rden = mk(rcp_a(lo(den)), rcp_a(hi(den)));
   const f2 s = mul2(g2, rden);
-  const f2 nz = sub2(A.k_one, s);  // s >= 0: n_z <= 1; the subtraction rounds n_z to float32 exactly like the reference's layer
+  const f2 nz = csub2(A.k_one, s);  // s >= 0: n_z <= 1; the subtraction rounds n_z to float32 exactly like the reference's layer
   {
     const f2 rn = mk(rcp_a(lo(Nn)), rcp_a(hi(Nn)));  // only the instantiation that stores the normals keeps this
     o.nx = mul2(negf2(p), rn);
@@ -414,15 +432,15 @@ __device__ __forceinline__ Normal2 finish_normal2(const FusedArgs& A, f2 Sw, f2 
   const bool smx = true, smy = true;
 #else
   const f2 r0 = mk(rsq_a(lo(nn)), rsq_a(hi(nn)));
-  const f2 rn = mul2(r0, fma2(negf2(mul2(mul2(nn, A.k_half), r0)), r0, A.k_1p5));  // rsqrt(nn), one Newton step
+  const f2 rn = mul2(r0, fma2c(negf2(mul2(mul2c(nn, A.k_half), r0)), r0, A.k_1p5));  // rsqrt(nn), one Newton step
   o.nx = mul2(negf2(p), rn);
   o.ny = mul2(negf2(q), rn);
   const f2 nzg = mul2(m, rn);
 #endif
   // roughness = sqrt(lambda0 * N/(N-1)); lambda0 is a difference of two terms of size cmag
-  const f2 rr2 = mul2(lam0, A.k_nnm1);
+  const f2 rr2 = mul2c(lam0, A.k_nnm1);
   const f2 r = mk(sqrt_a(fmaxf(lo(rr2), 0.f)), sqrt_a(fmaxf(hi(rr2), 0.f)));
-  const f2 thr = mul2(mul2(cmag, cmag), A.k_rough_thr);
+  const f2 thr = mul2c(mul2(cmag, cmag), A.k_rough_thr);
 #if !TE_MATH2
   // small inclination: n_z = 1 - s with s from t = tan^2(theta) (series; exact rounding of 1 - s)
 #if TE_NOCORR & 4
@@ -433,8 +451,8 @@ __device__ __forceinline__ Normal2 finish_normal2(const FusedArgs& A, f2 Sw, f2 
   const f2 t0 = mul2(g2, rm);
   const f2 t = fma2(fma2(negf2(t0), m2, g2), rm, t0);
 #endif
-  const f2 s = mul2(t, fma2(negf2(t), fma2(t, A.k_m03125, A.k_0375), A.k_half));
-  const f2 nzs = sub2(A.k_one, s);
+  const f2 s = mul2(t, fma2c(negf2(t), fma2kc(t, A.k_m03125, A.k_0375), A.k_half));
+  const f2 nzs = csub2(A.k_one, s);
   const bool smx = hx && lo(t) < 2.5e-3f, smy = hy && hi(t) < 2.5e-3f;
   const f2 nz = mk(fminf(smx ? lo(nzs) : lo(nzg), 1.0f), fminf(smy ? hi(nzs) : hi(nzg), 1.0f));
 #endif
@@ -443,29 +461,28 @@ __device__ __forceinline__ Normal2 finish_normal2(const FusedArgs& A, f2 Sw, f2 
   // region (1e-10 a) and of what the roughness tolerance allows (thr); conditioning: the eigen-gap min(2D, m) against
   // the matrix scale.  Invalid windows (NaN/Inf moments) fail through NaN; exactly flat windows (Sww == 0) are exact;
   // holes (invalid centre) need no second opinion.
-  const f2 lbase = fma2(cmag, A.k_1em5, A.k_1em10a);
+  const f2 lbase = fma2kc(cmag, A.k_1em5, A.k_1em10a);
   const f2 t1 = sub2(lam0, mk(fmaxf(lo(lbase), lo(thr)), fmaxf(hi(lbase), hi(thr))));
   // the eigen-gap is min(2D, a - lambda0) = a - lambda0 = m: m = D + h <= 2D because D = sqrt(h^2 + g^2) >= |h|
-  const f2 t2 = fma2(mk(fmaxf(A.a_cov, lo(c)), fmaxf(A.a_cov, hi(c))), A.k_mcond, m);
+  const f2 t2 = fma2k(mk(fmaxf(A.a_cov, lo(c)), fmaxf(A.a_cov, hi(c))), A.k_mcond, m);
   const f2 inval = sub2(ec, ec);
-  unsigned flag = 0;
-  {
-    const bool ok0 = (min2n(lo(t1), lo(t2)) > 0.f) || (lo(Sww) == 0.f);
-    const bool ok1 = (min2n(hi(t1), hi(t2)) > 0.f) || (hi(Sww) == 0.f);
-    flag = ((!ok0 && lo(inval) == 0.f) ? 1u : 0u) | ((!ok1 && hi(inval) == 0.f) ? 2u : 0u);
-  }
+  // a row fails unless its margin is positive or its window is exactly flat, and a hole is never flagged; the comparisons
+  // are combined with non-short-circuit & so that they stay predicate logic (no branch, no bytes of bools to repack)
+  const bool fail0 = !(min2n(lo(t1), lo(t2)) > 0.f) & (lo(Sww) != 0.f) & (lo(inval) == 0.f);
+  const bool fail1 = !(min2n(hi(t1), hi(t2)) > 0.f) & (hi(Sww) != 0.f) & (hi(inval) == 0.f);
+  unsigned flag = (unsigned)fail0 | ((unsigned)fail1 << 1);
   // where acos amplifies one ulp of n_z beyond the tolerance (theta < ~0.012 rad) certify its float32 rounding
   // n_z = 1 - s is rounded to float32 with spacing 2^-24: flag when s, known to relative error eps, may sit on the other
   // side of a rounding boundary (eps: the first moments carry <= 2.5e-6*sqrt(Sww) absolute error).  Both rows at once.
   const bool cx = smx && lo(s) < 7.2e-5f && lo(Sww) > 0.f, cy = smy && hi(s) < 7.2e-5f && hi(Sww) > 0.f;
   if (cx || cy) {
-    const f2 qv = mul2(s, A.k_2p24);
+    const f2 qv = mul2c(s, A.k_2p24);
     const f2 fr = sub2(qv, mk(floorf(lo(qv)), floorf(hi(qv))));
     const f2 gm2 = fma2(Sk, Sk, mul2(Sl, Sl));
     const f2 ratio = mul2(Sww, mk(rcp_a(fmaxf(lo(gm2), 1e-36f)), rcp_a(fmaxf(hi(gm2), 1e-36f))));
-    const f2 eps = fma2(mk(sqrt_a(lo(ratio)), sqrt_a(hi(ratio))), A.k_7p1em6, A.k_2em6);
-    const f2 bound = fma2(qv, eps, A.k_1em3);
-    const f2 dist = sub2(fr, A.k_half);
+    const f2 eps = fma2kc(mk(sqrt_a(lo(ratio)), sqrt_a(hi(ratio))), A.k_7p1em6, A.k_2em6);
+    const f2 bound = fma2c(qv, eps, A.k_bmargin);
+    const f2 dist = sub2c(fr, A.k_half);
     if (cx && fabsf(lo(dist)) <= lo(bound)) flag |= 1u;
     if (cy && fabsf(hi(dist)) <= hi(bound)) flag |= 2u;
   }
@@ -557,10 +574,10 @@ struct StepCtx {
   f2 cntU2, cntD2;    // pass-2 row tips as count weights: 1.0 where the offset belongs to the window, 0.0 where not
   f2* rg;             // SMEM_RINGS: the lane's element of ring 0 / slot 0 in shared memory (rings are 32 lanes x 8 bytes apart)
   unsigned lstate;    // shared address of the warp's work-list cursor {chunk base, entries used}
-  bool out_ok;        // lane produces output rows (lanes 1..30 and inside the map)
   unsigned oc;        // running output element offset (column jo, lane's first row); a launch covers < 2^30 cells.  It runs
                       // 8 columns ahead of the first store of a unit (wraps below zero; never dereferenced then)
-  int len;            // output columns of the unit (q1 - q0)
+  unsigned out_len;   // output columns of the unit (q1 - q0) the lane stores: 0 unless it produces output rows (lanes 1..30
+                      // inside the map), so that one unsigned compare per step decides a store
 };
 
 // One march step: column ce = q0 - 4 + t arrives.  PH = t % 5.
@@ -590,7 +607,7 @@ __device__ __forceinline__ void march_step(StepCtx<S>& C, Lane<S>& L, int t, uns
     if constexpr (S::NEED_N2) {
       const f2 D2 = sub2(ZP2, Z0), Dm2 = sub2(ZM2, Z0);
       ring_put<R_A2, S0>(C, L.a2, add2(A1, add2(D2, Dm2)));
-      ring_put<R_B2, S0>(C, L.b2, fma2(sub2(ZP2, ZM2), A.k_two, B1));
+      ring_put<R_B2, S0>(C, L.b2, fma2k(sub2(ZP2, ZM2), A.k_two, B1));
       ring_put<R_Q2, S0>(C, L.q2, fma2(D2, D2, fma2(Dm2, Dm2, Q1)));
     }
   }
@@ -599,9 +616,13 @@ __device__ __forceinline__ void march_step(StepCtx<S>& C, Lane<S>& L, int t, uns
     // excluded on-circle tips become NaN (x + NaN), included ones pass through (x + 0): both rows in one FADD2
     f2 TU = 0ull, TD = 0ull;
     if constexpr (S::TIP1) { TU = add2(ZM2, C.tipU1); TD = add2(ZP2, C.tipD1); }
+    // the three-row windows of the two rows, {z1,z2,z3} and {z2,z3,z4}, share min/max(z2, z3): one FMNMX each instead of
+    // two (minNum/maxNum are associative and commutative: a total order in which -0 < +0, NaN operands skipped)
+    const float mn23 = fminf(z[2], z[3]), mx23 = fmaxf(z[2], z[3]);
+    const float lo3r[2] = {fminf(z[1], mn23), fminf(mn23, z[4])}, hi3r[2] = {fmaxf(z[1], mx23), fmaxf(mx23, z[4])};
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const float lo3 = min3n(z[r + 1], z[r + 2], z[r + 3]), hi3 = max3n(z[r + 1], z[r + 2], z[r + 3]);
+      const float lo3 = lo3r[r], hi3 = hi3r[r];
       if constexpr (S::W11 == 1) { cmn[r] = lo3; cmx[r] = hi3; }
       else if constexpr (S::W11 >= 0) { cmn[r] = colmin_w<(S::W11 < 0 ? 0 : S::W11)>(z, r); cmx[r] = colmax_w<(S::W11 < 0 ? 0 : S::W11)>(z, r); }
       else { cmn[r] = cmx[r] = 0.f; }
@@ -678,9 +699,11 @@ __device__ __forceinline__ void march_step(StepCtx<S>& C, Lane<S>& L, int t, uns
     const float fmid = f[2] + f[3];
     const float c3[2] = {f[1] + fmid, fmid + f[4]};  // counts are small integers: any association is exact
     f2 PC = mk(c3[0], c3[1]);
+    const float vx23 = fmaxf(v[2], v[3]);  // shared by the windows of both rows, as in stage A
+    const float hi3r[2] = {fmaxf(v[1], vx23), fmaxf(vx23, v[4])};
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      const float hi3 = max3n(v[r + 1], v[r + 2], v[r + 3]);
+      const float hi3 = hi3r[r];
       if constexpr (S::W21 == 1) { smx[r] = hi3; sc[r] = c3[r]; }
       else if constexpr (S::W21 >= 0) { smx[r] = colmax_w<(S::W21 < 0 ? 0 : S::W21)>(v, r); sc[r] = colcnt_w<(S::W21 < 0 ? 0 : S::W21)>(f, r); }
       else { smx[r] = 0.f; sc[r] = 0.f; }
@@ -711,7 +734,7 @@ __device__ __forceinline__ void march_step(StepCtx<S>& C, Lane<S>& L, int t, uns
     if constexpr (S::WN1 >= 0) {
       const f2 dR = sub2(L.e[S1], ec), dL = sub2(L.e[S3], ec);
       const f2 aR = runA<S::WN1, S1, S0>(C, L), aL = runA<S::WN1, S3, S0>(C, L);
-      const f2 tR = fma2(A.k_m1, dR, aR), tL = fma2(A.k_m1, dL, aL);
+      const f2 tR = kfma2(A.k_m1, dR, aR), tL = kfma2(A.k_m1, dL, aL);
       Sw = add2(Sw, add2(tR, tL));
       Sl = sub2(tR, tL);
       Sk = add2(Sk, add2(runB<S::WN1, S1, S0>(C, L), runB<S::WN1, S3, S0>(C, L)));
@@ -721,9 +744,9 @@ __device__ __forceinline__ void march_step(StepCtx<S>& C, Lane<S>& L, int t, uns
     if constexpr (S::WN2 >= 0) {
       const f2 dR = sub2(L.e[S0], ec), dL = sub2(L.e[S4], ec);
       const f2 aR = runA<S::WN2, S0, S0>(C, L), aL = runA<S::WN2, S4, S0>(C, L);
-      const f2 tR = fma2(A.k_m0, dR, aR), tL = fma2(A.k_m0, dL, aL);
+      const f2 tR = kfma2(A.k_m0, dR, aR), tL = kfma2(A.k_m0, dL, aL);
       Sw = add2(Sw, add2(tR, tL));
-      Sl = fma2(A.k_two, sub2(tR, tL), Sl);
+      Sl = kfma2(A.k_two, sub2(tR, tL), Sl);
       Sk = add2(Sk, add2(runB<S::WN2, S0, S0>(C, L), runB<S::WN2, S4, S0>(C, L)));
       Sww = add2(Sww, fma2(dR, add2(aR, tR), runQ<S::WN2, S0, S0>(C, L)));
       Sww = add2(Sww, fma2(dL, add2(aL, tL), runQ<S::WN2, S4, S0>(C, L)));
@@ -734,7 +757,7 @@ __device__ __forceinline__ void march_step(StepCtx<S>& C, Lane<S>& L, int t, uns
     L.drough[S0] = n.rough;
     L.dflag[S0] = n.flag;
     if constexpr (KN)  // column jn is two columns ahead of the column the step layer is stored for
-      store_normals(A.nx, A.ny, A.nz, C.out_ok && (unsigned)(t - 6) < (unsigned)C.len, oc + 2u * (unsigned)A.rows, n.nx, n.ny, n.nz);
+      store_normals(A.nx, A.ny, A.nz, (unsigned)(t - 6) < C.out_len, oc + 2u * (unsigned)A.rows, n.nx, n.ny, n.nz);
   }
   if constexpr (!STRAIGHT) {
     if (t < 8) return;
@@ -743,7 +766,7 @@ __device__ __forceinline__ void march_step(StepCtx<S>& C, Lane<S>& L, int t, uns
   if constexpr (!STRAIGHT) {
     if (ce - 4 >= C.q1) return;
   }
-  const bool st_ok = C.out_ok && (unsigned)(t - 8) < (unsigned)C.len;  // column jo = ce - 4 = q0 + t - 8 belongs to the unit
+  const bool st_ok = (unsigned)(t - 8) < C.out_len;  // column jo = ce - 4 = q0 + t - 8 belongs to the unit
   {
     float mx2[2];
     f2 TL2 = L.sh[S4], TR2 = L.sh[S0];
@@ -767,13 +790,13 @@ __device__ __forceinline__ void march_step(StepCtx<S>& C, Lane<S>& L, int t, uns
     }
     const f2 MX = mk(mx2[0], mx2[1]);
     const f2 stepMax = mk(fmaxf(mx2[0], 0.0f), fmaxf(mx2[1], 0.0f));
-    const f2 prod = mul2(mul2(CNT, A.k_inv_ncrit), stepMax);
+    const f2 prod = mul2(mul2c(CNT, A.k_inv_ncrit), stepMax);
     const f2 st = mk(fminf(lo(stepMax), lo(prod)), fminf(hi(stepMax), hi(prod)));
     // st < crit ? 1 - st/crit : 0 ; no finite step_height in the window (mx is NaN) -> layer stays NaN (StepFilter.cpp:169)
     const f2 outv = add2(mk(fma_sat1(lo(st), A.minv_step_crit), fma_sat1(hi(st), A.minv_step_crit)), sub2(MX, MX));  // mx NaN (or Inf - Inf) keeps the layer NaN
     const f2 sl = L.dslope[S2], ro = L.drough[S2];
     const unsigned nf = L.dflag[S2];
-    const f2 tr = mul2(A.k_fuse_w, add2(add2(sl, outv), ro));
+    const f2 tr = kmul2(A.k_fuse_w, add2(add2(sl, outv), ro));
     if (st_ok) {
       *reinterpret_cast<f2*>(A.slope + oc) = sl;
       *reinterpret_cast<f2*>(A.rough + oc) = ro;
@@ -814,7 +837,7 @@ __global__ void TE_KERNEL_ATTR k_chain_fused(const __grid_constant__ CUtensorMap
   Lane<S> L{};  // the warm-up steps of a unit read ring slots before they are written (results discarded)
   StepCtx<S> C{A, ering, ering + lane * 8u, shbuf + lane * 8u, lane, 0, 0, 0, 0ull, 0ull, 0ull, 0ull, 0ull, 0ull,
                reinterpret_cast<f2*>(smem_raw + warp * WARP_SMEM_BYTES + WARP_RING_OFF) + lane,
-               bar0 + 8 * NST, false, 0u, 0};
+               bar0 + 8 * NST, 0u, 0u};
   if (lane == 0) asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(C.lstate), "r"(0u), "r"(LIST_CHUNK) : "memory");  // no chunk yet
   __syncwarp();
 
@@ -835,8 +858,7 @@ __global__ void TE_KERNEL_ATTR k_chain_fused(const __grid_constant__ CUtensorMap
     const int nsteps = (C.q1 - C.q0) + 8;
     const int nchunks = (nsteps + CH - 1) / CH;
     const int row0 = C.s0 + 2 * lane;
-    C.out_ok = lane >= 1 && lane <= 30 && row0 < A.rows;
-    C.len = C.q1 - C.q0;
+    C.out_len = (lane >= 1 && lane <= 30 && row0 < A.rows) ? (unsigned)(C.q1 - C.q0) : 0u;
     C.oc = (unsigned)mapi * A.map_cells + (unsigned)(C.q0 - A.out_col0 - 8) * (unsigned)A.rows + (unsigned)row0;
     if constexpr (S::MASKS) {
       const unsigned rm0 = (row0 >= 0 && row0 < A.rows) ? A.rowmask[row0] : 0u;
@@ -1212,20 +1234,20 @@ int launch_chain_fused(FusedState& st, const SlabView& v, const ChainDev& p, int
   a.inv_ncrit = (float)(1.0 / (double)p.ncrit);
   a.rough_crit = (float)p.rough_crit; a.inv_rough_crit = (float)(1.0 / p.rough_crit);
   a.fuse_w = p.fuse_w;
-  auto B2 = [](double v) {
-    const float f = (float)v;
-    unsigned u;
-    std::memcpy(&u, &f, 4);
-    return ((unsigned long long)u << 32) | (unsigned long long)u;
-  };
-  a.k_invN = B2(1.0 / N); a.k_minvN = B2(-1.0 / N); a.k_kp = B2(-res / N); a.k_half_a = B2(0.5 * (double)a.a_cov);
+  auto B2 = [](double v) { return (float)v; };  // a kernel constant: the double value rounded to float32 once, here
+  a.k_invN = B2(1.0 / N); a.k_kp = B2(-res / N); a.k_half_a = B2(0.5 * (double)a.a_cov);
   a.k_nnm1 = B2(N / (N - 1.0)); a.k_rough_thr = B2((double)a.rough_thr);
-  a.k_minv_slope = B2(-1.0 / p.slope_crit); a.k_minv_rough = B2(-1.0 / p.rough_crit);
-  a.k_inv_ncrit = B2((double)a.inv_ncrit); a.k_minv_step = B2(-(double)a.inv_step_crit); a.k_fuse_w = B2((double)a.fuse_w);
+  a.k_inv_ncrit = B2((double)a.inv_ncrit); a.k_fuse_w = B2((double)a.fuse_w);
   a.k_m0 = B2(wn.w[2] >= 0 ? 2 * wn.w[2] + 1 : 0); a.k_m1 = B2(wn.w[1] >= 0 ? 2 * wn.w[1] + 1 : 0);
   a.k_1em5 = B2(1e-5); a.k_1em10a = B2(1e-10 * (double)a.a_cov); a.k_mcond = B2(-cond_k);
-  a.k_2p24 = B2(16777216.0); a.k_7p1em6 = B2(7.1e-6); a.k_2em6 = B2(TE_MATH2 ? 2.5e-6 : 2e-6);  // relative error budget of s = 1 - n_z besides the moments' (MATH2: two more MUFU results in s) a.k_1em3 = B2(1e-3);
-  a.k_one = B2(1.0); a.k_mone = B2(-1.0); a.k_two = B2(2.0); a.k_half = B2(0.5); a.k_mhalf = B2(-0.5); a.k_1p5 = B2(1.5);
+  a.k_2p24 = B2(16777216.0); a.k_7p1em6 = B2(7.1e-6);
+  a.k_2em6 = B2(TE_MATH2 ? 2.5e-6 : 2e-6);  // relative error budget of s = 1 - n_z besides the moments' (MATH2: two more MUFU results in s)
+  // Absolute term of the rounding-boundary bound (qv * eps + k_bmargin, in float32 spacings of n_z).  It was meant to be 1e-3,
+  // but that assignment was lost by accident (it ended up inside a trailing comment) and the kernel has run with 0 since.  It
+  // stays 0 here so that the outputs stay bit-identical; restoring the 1e-3 floor is an open certification question (it would
+  // send more cells near a rounding boundary to the fp64 fix-up and can change their float32 rounding).
+  a.k_bmargin = B2(0.0);
+  a.k_one = B2(1.0); a.k_two = B2(2.0); a.k_half = B2(0.5); a.k_1p5 = B2(1.5);
   a.k_0375 = B2(0.375); a.k_m03125 = B2(-0.3125);
   a.k_p0 = B2(1.570796251296997); a.k_p1 = B2(-0.21459604799747467); a.k_p2 = B2(0.08894557505846024);
   a.k_p3 = B2(-0.05000271648168564); a.k_p4 = B2(0.03044925443828106); a.k_p5 = B2(-0.016484638676047325);
