@@ -176,10 +176,18 @@ def _run_device(ctx, g, ft, Ld, rsd, D, cap, mfv=16):
     return tuple(out[k].cpu().numpy() for k in keys)
 
 
-@pytest.fixture(scope="module", params=CASES, ids=lambda c: f"{c['rows']}x{c['cols']}@{c['res']}" + ("+off" if "position" in c else ""))
+def _case_id(c):
+    return f"{c['rows']}x{c['cols']}@{c['res']}" + ("+off" if "position" in c else "")
+
+
+@pytest.fixture(scope="module", params=CASES, ids=_case_id)
 def mixed_case(request, te, oracle):
-    """A map case with its chain layers, a robot_slope layer and a mixed request of about 200 paths over four footprints."""
-    case = request.param
+    return _mixed(te, oracle, request.param)
+
+
+def _mixed(te, oracle, case):
+    """A map case with its chain layers, a robot_slope layer and a mixed request of about 200 paths over four footprints (the
+    last one the conservative 256-pose path whose polygon2 reaches the vertex cap)."""
     res, pos = case["res"], case.get("position", (0.0, 0.0))
     z = synth.terrain(case["rows"], case["cols"], res, case["seed"], "mixed", pos)
     og, g = oracle.Geometry.make(case["rows"], case["cols"], res, pos), te.Geometry.make(case["rows"], case["cols"], res, pos)
@@ -210,29 +218,46 @@ def test_mixed_requests_equal_the_split_calls(te, ctx, oracle, mixed_case):
     assert want[0].any() and not want[0].all()
 
 
-def test_request_matches_the_cpu_oracles(te, ctx, oracle):
-    rows, cols = 200, 180
-    z = synth.terrain(rows, cols, 0.02, 51, "mixed")
-    og, g = oracle.Geometry.make(rows, cols, 0.02), te.Geometry.make(rows, cols, 0.02)
-    L, rs = _layers(oracle, og, z, 51)
-    rng = np.random.default_rng(51)
-    fps = _footprints(rng)
-    R = _request(rng, og, 200, fps, cap_path=False)
-    ft, fo = _fps(te, oracle, 1)
-    got = _run(ctx, g, ft, L, R, fps, rs, CAP)
+def _oracle(og, fo, L, R, fps, rs):
+    """The CPU oracles' answer to a request, path by path in request order: check_circular_paths_fresh2 for its circular paths
+    (area 0), check_polygonal_paths2 once per footprint for its polygonal paths."""
+    m = len(R["kind"])
+    out = (np.zeros(m, np.uint8), np.zeros(m), np.zeros(m), np.zeros(m, np.int32), np.zeros((m, CAP, 2)))
+    rough = L["roughness"] if fo.verify_roughness else None
     for k in range(-1, len(fps)):
         idx = np.nonzero(R["kind"] == k)[0]
+        if not len(idx):
+            continue
         b, p = _subset(R, idx)
         if k < 0:
             w = uo.check_circular_paths_fresh2(og, fo, L["traversability"], L["slope"], L["step"], L["elevation"], b, p[:, :2].copy(),
-                                               R["radius"][idx], robot_slope=rs, roughness=L["roughness"],
+                                               R["radius"][idx], robot_slope=rs, roughness=rough,
                                                compute_untraversable_polygon=R["cup"][idx], capacity=CAP)
-            want = (w[0], w[1], np.zeros(len(idx)), w[2], w[3])
+            w = (w[0], w[1], np.zeros(len(idx)), w[2], w[3])
         else:
-            want = uo.check_polygonal_paths2(og, fo, L["traversability"], L["slope"], L["step"], L["elevation"], fps[k], b, p,
-                                             robot_slope=rs, roughness=L["roughness"], conservative=R["cons"][idx],
-                                             compute_untraversable_polygon=R["cup"][idx], capacity=CAP)
-        _assert_equal(tuple(a[idx] for a in got), want, ("oracle", k))
+            w = uo.check_polygonal_paths2(og, fo, L["traversability"], L["slope"], L["step"], L["elevation"], fps[k], b, p,
+                                          robot_slope=rs, roughness=rough, conservative=R["cons"][idx],
+                                          compute_untraversable_polygon=R["cup"][idx], capacity=CAP)
+        for a, v in zip(out, w):
+            a[idx] = v
+    return out
+
+
+def test_request_matches_the_cpu_oracles(te, ctx, oracle):
+    """Every output of a mixed request against the CPU oracles, bit for bit, on the three small maps: with and without
+    verify_roughness, robot_slope and polygon outputs."""
+    for case in CASES[:3]:
+        M = _mixed(te, oracle, case)
+        og, g, L, fps, R = (M[k] for k in ("og", "g", "L", "fps", "R"))
+        assert R["cons"][-1] and R["cup"][-1] and R["begin"][-1] - R["begin"][-2] == 256
+        for verify in (0, 1):
+            ft, fo = _fps(te, oracle, verify)
+            for rs in (None, M["rs"]):
+                want = _oracle(og, fo, L, R, fps, rs)
+                for cap in (None, CAP):
+                    got = _run(ctx, g, ft, L, R, fps, rs, cap)
+                    _assert_equal(got, want if cap else want[:3], ("oracle", _case_id(case), verify, rs is None, cap))
+                assert want[0].any() and not want[0].all() and (want[3] > 0).any()
 
 
 def test_degenerate_requests(te, ctx, oracle):

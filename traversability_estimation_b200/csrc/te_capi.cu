@@ -8,6 +8,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <string>
@@ -934,52 +935,87 @@ int te_check_footprint_paths_fresh(te_ctx* c, const te_geometry* g_in, const te_
                                          is_safe, traversability, 0, nullptr, nullptr, memory);
 }
 
+// Stages the path arrays of `r` and points `r` at the device copies (host memory; null stays null).
+static void stage_paths(Staging& st, te::PathChecks& r) {
+  const size_t np = (size_t)r.npaths;
+  r.path_begin = st.in(r.path_begin, np + 1);
+  r.poses = st.in(r.poses, (size_t)r.pose_stride * r.nposes);
+  r.radius = st.in(r.radius, np);
+  r.footprint_begin = st.in(r.footprint_begin, np + 1);
+  r.footprint_xyz = st.in(r.footprint_xyz, 3 * (size_t)r.nvertices);
+  r.conservative = st.in(r.conservative, np);
+  r.cup = st.in(r.cup, np);
+  r.is_safe = st.out(r.is_safe, np);
+  r.trav_out = st.out(r.trav_out, np);
+  r.area_out = st.out(r.area_out, np);
+  r.ucount = st.out(r.ucount, np);
+  r.uxy = st.out(r.uxy, 2 * (size_t)r.max_vertices * np);
+}
+
+// The body of te_check_footprint_paths_fresh2, te_check_footprint_paths_polygon2 and te_check_footprint_request once the entry has
+// put its arguments into `r` (the caller's pointers): the checks the three share, then in host memory `host_checks(g, r)` (the
+// entry's validation of the path arrays; it sets r.nposes where the entry has none, and r.max_points), the staging, the launches
+// and the download.  Device memory reads nothing back: a path that cannot be checked gets is_safe 0 and NaN (te_b200.h).
+static int run_path_checks(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, te::PathChecks r, int memory, const char* what,
+                           const std::function<int(const te_geometry*, te::PathChecks&)>& host_checks) {
+  te_geometry g0;
+  if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
+  const te_geometry* g = &g0;
+  if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
+  const bool circular = r.footprint_begin || !r.footprint, polygonal = r.footprint_begin || r.footprint;
+  if (circular && !(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
+  if (int rc = check_filter_layers(p, r.trav, r.slope, r.step, r.elev, r.rough)) return rc;
+  if (r.npaths < 0 || !r.path_begin || !r.poses || (circular && !r.radius) || !r.is_safe || !r.trav_out ||
+      (polygonal && (r.nposes < 0 || !r.area_out)))
+    return fail(TE_ERR_BAD_ARG, "null argument or negative count");
+  if (int rc = check_polygon_outputs(r.max_vertices, r.ucount, r.uxy)) return rc;
+  if (r.npaths == 0) return TE_OK;
+  if (int rc = ensure_geometry(c, g)) return rc;
+  const bool host = memory != TE_MEM_DEVICE;
+  if (host)
+    if (int rc = host_checks(g, r)) return rc;
+  int32_t* const ucount = r.ucount;
+  Staging st(c, host, g_in);
+  r.trav = st.in_layer(r.trav, g->cols);
+  r.slope = st.in_layer(r.slope, g->cols);
+  r.step = st.in_layer(r.step, g->cols);
+  r.elev = st.in_layer(r.elev, g->cols);
+  r.rough = st.in_layer(p->verify_roughness ? r.rough : nullptr, g->cols);
+  r.robot_slope = st.in_layer(r.robot_slope, g->cols);
+  stage_paths(st, r);
+  if (st.rc) return st.rc;
+  const te_slab s{0, g->cols, 0, 0};
+  int nl = 0;
+  int rc = te::launch_path_checks(c->fp, make_view(c, g, s), g, p, r, true, true, c->stream, &nl);
+  if (rc != 0) return fail(rc, "%s failed: %s", what, c->fp.why.c_str());
+  if (int r2 = launch_check(c, what, nl)) return r2;
+  if (int r2 = st.finish()) return r2;
+  if (host && ucount)  // the row bound of a polygonal path's polygon table (kUntravRows) is only known once the hulls are
+    for (int32_t q = 0; q < r.npaths; ++q)
+      if (ucount[q] < 0)
+        return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);
+  return TE_OK;
+}
+
 int te_check_footprint_paths_fresh2(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
                                     const float* step, const float* rough, const float* elev, const float* robot_slope, int32_t npaths,
                                     const int32_t* path_begin, const double* poses_xy, const double* radius, const uint8_t* cup,
                                     uint8_t* is_safe, double* traversability, int32_t max_vertices, int32_t* ucount, double* uxy,
                                     int memory) {
   TE_ENTER(c);
-  te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
-  const te_geometry* g = &g0;
-  if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
-  if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
-  if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
-  if (npaths < 0 || !path_begin || !poses_xy || !radius || !is_safe || !traversability) return fail(TE_ERR_BAD_ARG, "null argument or negative path count");
-  if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
-  if (npaths == 0) return TE_OK;
-  const bool use_rough = p->verify_roughness != 0;
-  if (int rc = ensure_geometry(c, g)) return rc;
-  // Device memory reads nothing back: a path whose radius cannot be checked gets is_safe 0, traversability NaN.
-  const bool host = memory != TE_MEM_DEVICE;
-  int32_t nposes = 0;
-  if (host) {
+  te::PathChecks r{};
+  r.trav = trav; r.slope = slope; r.step = step; r.rough = rough; r.elev = elev; r.robot_slope = robot_slope;
+  r.npaths = npaths; r.nposes = -1; r.path_begin = path_begin; r.poses = poses_xy; r.pose_stride = 2; r.radius = radius; r.cup = cup;
+  r.is_safe = is_safe; r.trav_out = traversability; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
+  return run_path_checks(c, g_in, p, r, memory, "fresh path check", [&](const te_geometry* g, te::PathChecks& h) -> int {
     if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
     for (int32_t q = 0; q < npaths; ++q) {
       if (path_begin[q + 1] < path_begin[q]) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
       if (int rc = check_circular_radius(g, p, q, radius[q])) return rc;
     }
-    nposes = path_begin[npaths];
-  }
-  Staging st(c, host, g_in);
-  const float* in[6] = {st.in_layer(trav, g->cols), st.in_layer(slope, g->cols), st.in_layer(step, g->cols), st.in_layer(elev, g->cols),
-                        st.in_layer(use_rough ? rough : nullptr, g->cols), st.in_layer(robot_slope, g->cols)};
-  const int32_t* dpb = st.in(path_begin, (size_t)npaths + 1);
-  const double* dxy = st.in(poses_xy, 2 * (size_t)nposes);
-  const double* drad = st.in(radius, (size_t)npaths);
-  const uint8_t* dcup = st.in(cup, (size_t)npaths);
-  uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
-  double* dtrav = st.out(traversability, (size_t)npaths);
-  int32_t* dcount = st.out(ucount, (size_t)npaths);
-  double* duxy = st.out(uxy, 2 * (size_t)max_vertices * npaths);
-  if (st.rc) return st.rc;
-  const te_slab s{0, g->cols, 0, 0};
-  int rc = te::launch_check_paths_fresh(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], in[5], npaths, dpb, dxy, drad,
-                                        dcup, dsafe, dtrav, max_vertices, dcount, duxy, c->stream);
-  if (rc != 0) return fail(rc, "fresh path check failed: %s", c->fp.why.c_str());
-  if (int r2 = launch_check(c, dcount ? "k_check_paths_fresh_poly" : "k_check_paths_fresh")) return r2;
-  return st.finish();
+    h.nposes = path_begin[npaths];
+    return TE_OK;
+  });
 }
 
 int te_check_footprint_paths_polygon(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
@@ -998,27 +1034,21 @@ int te_check_footprint_paths_polygon2(te_ctx* c, const te_geometry* g_in, const 
                                       const double* poses, const uint8_t* conservative, uint8_t* is_safe, double* traversability,
                                       double* area, const uint8_t* cup, int32_t max_vertices, int32_t* ucount, double* uxy, int memory) {
   TE_ENTER(c);
-  te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
-  const te_geometry* g = &g0;
-  if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
-  if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
-  if (npaths < 0 || nposes < 0 || !path_begin || !poses || !footprint_xyz || !is_safe || !traversability || !area)
-    return fail(TE_ERR_BAD_ARG, "null argument or negative count");
+  if (!footprint_xyz) return fail(TE_ERR_BAD_ARG, "null argument or negative count");
   if (nfootprint < 1 || nfootprint > te::kPolyMaxVerts) return fail(TE_ERR_BAD_ARG, "footprint needs 1..%d vertices, got %d", te::kPolyMaxVerts, nfootprint);
   for (int k = 0; k < 3 * nfootprint; ++k)
     if (!std::isfinite(footprint_xyz[k])) return fail(TE_ERR_BAD_ARG, "footprint vertex %d is not finite", k / 3);
-  if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
-  if (npaths == 0) return TE_OK;
-  const bool use_rough = p->verify_roughness != 0;
-  if (int rc = ensure_geometry(c, g)) return rc;
-  // Device memory reads nothing back: a path that cannot be checked gets is_safe 0, traversability and area NaN.
-  const bool host = memory != TE_MEM_DEVICE;
-  int mp = conservative ? 2 * te::kPolyConsCap : 2 * nfootprint;  // hull input bound of one item; host memory sizes it from the paths
-  if (host) {
+  te::PathChecks r{};
+  r.trav = trav; r.slope = slope; r.step = step; r.rough = rough; r.elev = elev; r.robot_slope = robot_slope;
+  r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7;
+  r.nfp = nfootprint; r.footprint = footprint_xyz; r.conservative = conservative; r.cup = ucount ? cup : nullptr;
+  // the hull input bound of one item; host memory sizes it from the paths
+  r.max_points = conservative ? 2 * te::kPolyConsCap : 2 * nfootprint;
+  r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
+  return run_path_checks(c, g_in, p, r, memory, "polygonal path check", [&](const te_geometry*, te::PathChecks& h) -> int {
     if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
     if (path_begin[npaths] != nposes) return fail(TE_ERR_BAD_ARG, "path_begin[npaths] = %d != nposes = %d", path_begin[npaths], nposes);
-    mp = 2 * nfootprint;
+    h.max_points = 2 * nfootprint;
     for (int32_t q = 0; q < npaths; ++q) {
       const int32_t n = path_begin[q + 1] - path_begin[q];
       if (n < 0) return fail(TE_ERR_BAD_ARG, "path_begin must be non-decreasing");
@@ -1026,38 +1056,13 @@ int te_check_footprint_paths_polygon2(te_ctx* c, const te_geometry* g_in, const 
         if ((long long)nfootprint * n > te::kPolyConsCap)
           return fail(TE_ERR_UNSUPPORTED, "conservative path %d needs %lld polygon vertices, more than %d", q, (long long)nfootprint * n,
                       te::kPolyConsCap);
-        mp = std::max(mp, 2 * nfootprint * n);
+        h.max_points = std::max(h.max_points, 2 * nfootprint * n);
       }
     }
     for (size_t k = 0; k < 7 * (size_t)nposes; ++k)
       if (!std::isfinite(poses[k])) return fail(TE_ERR_BAD_ARG, "pose %zu is not finite", k / 7);
-  }
-  Staging st(c, host, g_in);
-  const float* in[6] = {st.in_layer(trav, g->cols), st.in_layer(slope, g->cols), st.in_layer(step, g->cols), st.in_layer(elev, g->cols),
-                        st.in_layer(use_rough ? rough : nullptr, g->cols), st.in_layer(robot_slope, g->cols)};
-  const int32_t* dpb = st.in(path_begin, (size_t)npaths + 1);
-  const double* dposes = st.in(poses, 7 * (size_t)nposes);
-  const uint8_t* dcons = st.in(conservative, (size_t)npaths);
-  uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
-  double* dtrav = st.out(traversability, (size_t)npaths);
-  double* darea = st.out(area, (size_t)npaths);
-  const uint8_t* dcup = ucount ? st.in(cup, (size_t)npaths) : nullptr;
-  int32_t* dcount = st.out(ucount, (size_t)npaths);
-  double* duxy = st.out(uxy, 2 * (size_t)max_vertices * npaths);
-  if (st.rc) return st.rc;
-  const te_slab s{0, g->cols, 0, 0};
-  int nl = 0;
-  int rc = te::launch_check_paths_polygon(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], in[5], nfootprint, footprint_xyz,
-                                          npaths, nposes, dpb, dposes, dcons, mp, dsafe, dtrav, darea, dcup, max_vertices, dcount, duxy,
-                                          c->stream, &nl);
-  if (rc != 0) return fail(rc, "polygonal path check failed: %s", c->fp.why.c_str());
-  if (int r2 = launch_check(c, "polygonal path check", nl)) return r2;
-  if (int r2 = st.finish()) return r2;
-  if (host && ucount)  // the row bound of the polygon's table (kUntravRows) is only known once the hulls are
-    for (int32_t q = 0; q < npaths; ++q)
-      if (ucount[q] < 0)
-        return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);
-  return TE_OK;
+    return TE_OK;
+  });
 }
 
 // The host-side validation of a te_check_footprint_request request (paths, footprints, radii, conservative caps, finite poses and
@@ -1108,59 +1113,22 @@ int te_check_footprint_request(te_ctx* c, const te_geometry* g_in, const te_foot
                                const uint8_t* conservative, const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area,
                                int32_t max_vertices, int32_t* ucount, double* uxy, int memory) {
   TE_ENTER(c);
-  te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
-  const te_geometry* g = &g0;
-  if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
-  if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
-  if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
-  if (npaths < 0 || nposes < 0 || nvertices < 0 || !path_begin || !poses || !radius || !footprint_begin ||
-      (nvertices > 0 && !footprint_xyz) || !is_safe || !traversability || !area)
-    return fail(TE_ERR_BAD_ARG, "null argument or negative count");
+  if (nvertices < 0 || !footprint_begin || (nvertices > 0 && !footprint_xyz)) return fail(TE_ERR_BAD_ARG, "null argument or negative count");
   if (max_footprint_vertices < 0 || max_footprint_vertices > te::kPolyMaxVerts)
     return fail(TE_ERR_BAD_ARG, "max_footprint_vertices must be 0..%d, got %d", te::kPolyMaxVerts, max_footprint_vertices);
-  if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
-  if (npaths == 0) return TE_OK;
-  const bool use_rough = p->verify_roughness != 0;
-  if (int rc = ensure_geometry(c, g)) return rc;
-  // Device memory reads nothing back: a path that cannot be checked gets is_safe 0, traversability and area NaN.  The hull input
-  // bound of a polygonal item: as te_check_footprint_paths_polygon2 for the largest footprint; host memory sizes it from the paths.
-  const bool host = memory != TE_MEM_DEVICE;
-  int mp = 2 * std::max(max_footprint_vertices, 1);
-  if (conservative && max_footprint_vertices > 0) mp = 2 * te::kPolyConsCap;
-  if (host)
-    if (int rc = check_request_host(g, p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
-                                    max_footprint_vertices, conservative, &mp))
-      return rc;
-  Staging st(c, host, g_in);
-  const float* in[6] = {st.in_layer(trav, g->cols), st.in_layer(slope, g->cols), st.in_layer(step, g->cols), st.in_layer(elev, g->cols),
-                        st.in_layer(use_rough ? rough : nullptr, g->cols), st.in_layer(robot_slope, g->cols)};
-  const int32_t* dpb = st.in(path_begin, (size_t)npaths + 1);
-  const double* dposes = st.in(poses, 7 * (size_t)nposes);
-  const double* drad = st.in(radius, (size_t)npaths);
-  const int32_t* dfb = st.in(footprint_begin, (size_t)npaths + 1);
-  const float* dfxyz = st.in(footprint_xyz, 3 * (size_t)nvertices);
-  const uint8_t* dcons = st.in(conservative, (size_t)npaths);
-  const uint8_t* dcup = st.in(cup, (size_t)npaths);
-  uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
-  double* dtrav = st.out(traversability, (size_t)npaths);
-  double* darea = st.out(area, (size_t)npaths);
-  int32_t* dcount = st.out(ucount, (size_t)npaths);
-  double* duxy = st.out(uxy, 2 * (size_t)max_vertices * npaths);
-  if (st.rc) return st.rc;
-  const te_slab s{0, g->cols, 0, 0};
-  int nl = 0;
-  int rc = te::launch_check_request(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], in[5], npaths, nposes, dpb, dposes,
-                                    drad, nvertices, dfb, dfxyz, max_footprint_vertices, dcons, dcup, mp, dsafe, dtrav, darea,
-                                    max_vertices, dcount, duxy, c->stream, &nl);
-  if (rc != 0) return fail(rc, "footprint path request failed: %s", c->fp.why.c_str());
-  if (int r2 = launch_check(c, "footprint path request", nl)) return r2;
-  if (int r2 = st.finish()) return r2;
-  if (host && ucount)  // the row bound of a polygonal path's polygon table (kUntravRows) is only known once the hulls are
-    for (int32_t q = 0; q < npaths; ++q)
-      if (ucount[q] < 0)
-        return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);
-  return TE_OK;
+  // The hull input bound of a polygonal item: as te_check_footprint_paths_polygon2 for the largest footprint; host memory sizes it
+  // from the paths.
+  te::PathChecks r{};
+  r.trav = trav; r.slope = slope; r.step = step; r.rough = rough; r.elev = elev; r.robot_slope = robot_slope;
+  r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7; r.radius = radius;
+  r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
+  r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup;
+  r.max_points = conservative && max_footprint_vertices > 0 ? 2 * te::kPolyConsCap : 2 * std::max(max_footprint_vertices, 1);
+  r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
+  return run_path_checks(c, g_in, p, r, memory, "footprint path request", [&](const te_geometry* g, te::PathChecks& h) {
+    return check_request_host(g, p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+                              max_footprint_vertices, conservative, &h.max_points);
+  });
 }
 
 // ---- te_map: the layers, the traversability_footprint cache and the isTraversableForFilters memo, resident on the device -------
@@ -1398,22 +1366,17 @@ int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int3
   const float* rslope = m->have_rslope ? (const float*)m->rslope.p : nullptr;
   int nl = 0;
   if (nvertices > 0) {  // the polygonal paths (TraversabilityMap.cpp:464-584) read the memo and leave the cache alone
+    te::PathChecks r{};
+    r.trav = (const float*)m->trav.p; r.slope = (const float*)m->slope.p; r.step = (const float*)m->step.p; r.rough = rough;
+    r.elev = (const float*)m->elev.p; r.robot_slope = rslope;
+    r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7;
+    r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
+    r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup; r.max_points = mp;
+    r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
     Staging st(c, true, g);
-    const int32_t* dpb = st.in(path_begin, (size_t)npaths + 1);
-    const double* dposes = st.in(poses, 7 * (size_t)nposes);
-    const int32_t* dfb = st.in(footprint_begin, (size_t)npaths + 1);
-    const float* dfxyz = st.in(footprint_xyz, 3 * (size_t)nvertices);
-    const uint8_t* dcons = st.in(conservative, (size_t)npaths);
-    const uint8_t* dcup = st.in(cup, (size_t)npaths);
-    uint8_t* dsafe = st.out(is_safe, (size_t)npaths);
-    double* dtrav = st.out(traversability, (size_t)npaths);
-    double* darea = st.out(area, (size_t)npaths);
-    int32_t* dcount = st.out(ucount, (size_t)npaths);
-    double* duxy = st.out(uxy, 2 * (size_t)max_vertices * npaths);
+    stage_paths(st, r);
     if (st.rc) return st.rc;
-    int rc = te::launch_map_polygons(m->fp, v, g, p, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p, rough,
-                                     (const float*)m->elev.p, rslope, npaths, nposes, dpb, dposes, nvertices, dfb, dfxyz,
-                                     max_footprint_vertices, dcons, dcup, mp, dsafe, dtrav, darea, max_vertices, dcount, duxy, c->stream, &nl);
+    int rc = te::launch_path_checks(m->fp, v, g, p, r, false, false, c->stream, &nl);
     if (rc != 0) return fail(rc, "map request (polygonal paths) failed: %s", m->fp.why.c_str());
     if (int r2 = launch_check(c, "map request (polygonal paths)", nl)) return r2;
     if (int r2 = st.finish()) return r2;

@@ -877,8 +877,9 @@ constexpr int kPathMaxRings = 127;  // the signed-byte packing of the ring table
 struct PathArgs {
   const float* rslope;           // robot_slope, nullptr: checkRobotInclination_ off
   int npaths;
+  int pose_stride;               // doubles per pose in `poses`: 2 (x y) or 7 (x y z qx qy qz qw)
   const int* path_begin;
-  const double* xy;
+  const double* poses;
   const double* radius;          // FootprintPath.radius per path
   const unsigned char* cup;      // FootprintPath.compute_untraversable_polygon per path, nullptr: all 0
   double offset;                 // radiusMax = radius + offset (:348)
@@ -1135,7 +1136,7 @@ __device__ int spiral_blockers_d(const FpArgs& A, const Layers& L, const PathArg
 }
 
 // grid_map::Polygon::fromCircle(center, radius) (recalled): vertex j = center + Rotation2D(j * 2 * M_PI / 19) * (radius, 0); the
-// 20 cosines and sines come from the host's libm (launch_check_paths_fresh).  A single pose publishes it as it is; a segment
+// 20 cosines and sines come from the host's libm (circle_table).  A single pose publishes it as it is; a segment
 // hulls it: 20 points, so every later convexHull with it is the same chain (see write_cells_polygon_d).  One thread.
 __host__ __device__ void write_circle_polygon_d(const double* cs, const double* sn, double cx, double cy, double radius, bool hulled,
                                        double2* pts, const UntravOut& O, int q) {
@@ -1158,17 +1159,18 @@ struct CircleTable {
   double cs[kFromCircleVertices], sn[kFromCircleVertices];
 };
 
-// A whole check_footprint_path request (te_check_footprint_request): circular and polygonal paths mixed, each with its own
-// footprint, poses 7 doubles wide for both kinds.  Path q's footprint is vertices fp_begin[q] .. fp_begin[q+1]-1 of fp_xyz: none
-// makes the path circular (the _req variants of k_check_paths_fresh), any other count polygonal (those of k_check_polygon_*).
-// Device memory cannot validate the arrays on the host, so the kernels do (request_footprint_ok_d, the pose range).
+// Per-path footprints and the pose count of a batch.  With fp_begin, path q's footprint is vertices fp_begin[q] .. fp_begin[q+1]-1
+// of fp_xyz, as in a whole check_footprint_path request (te_check_footprint_request): none makes the path circular (checked by
+// k_check_paths_fresh*), any other count polygonal (checked by k_check_polygon_*).  Without fp_begin every path is circular for
+// k_check_paths_fresh* and uses the one footprint of PolyPathArgs for k_check_polygon_*.  Device memory cannot validate the arrays
+// on the host, so the kernels do (request_footprint_ok_d, the pose range).
 struct RequestArgs {
-  const int* fp_begin;   // [npaths + 1]
+  const int* fp_begin;   // [npaths + 1], nullptr: no per-path footprints
   const float* fp_xyz;   // 3 floats (x, y, z) per vertex
   int nvertices;         // vertices in fp_xyz
   int maxfp;             // max_footprint_vertices: a longer footprint is not checked
-  int nposes;
-  double* area_out;      // the area of the circular paths: 0, NaN for a path that is not checked
+  int nposes;            // < 0: not known, the circular check does not test pose ranges
+  double* area_out;      // the area of the circular paths: 0, NaN for a path that is not checked; nullptr: not wanted
 };
 
 // Whether path q's footprint can be checked: 1..maxfp vertices inside fp_xyz, all finite (host memory rejects the rest).  The
@@ -1180,25 +1182,26 @@ __device__ __forceinline__ bool request_footprint_ok_d(const RequestArgs& R, int
   return ok;
 }
 
-// The body of k_check_paths_fresh; POLY also produces the untraversable polygon (k_check_paths_fresh_poly); REQ checks the
-// circular paths of a request (RequestArgs) and leaves its polygonal paths to k_check_polygon_*_req.
-template <bool POLY, bool REQ>
+// The body of k_check_paths_fresh; POLY also produces the untraversable polygon (k_check_paths_fresh_poly).  With per-path
+// footprints (R.fp_begin) it checks the circular paths of a request and leaves its polygonal paths to k_check_polygon_*.
+template <bool POLY>
 __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layers& L, const PathArgs& P, const UntravOut& O,
                                                     const CircleTable& C, const UntravScratch& S, const RequestArgs& R) {
-  constexpr int PS = REQ ? 7 : 2;  // doubles per pose; x and y come first
+  const int PS = P.pose_stride;  // x and y come first
   const int lane = threadIdx.x & 31;
   const int q = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   if (q >= P.npaths) return;  // whole warp
-  if (REQ && R.fp_begin[q + 1] != R.fp_begin[q]) return;  // a polygonal path
+  if (R.fp_begin && R.fp_begin[q + 1] != R.fp_begin[q]) return;  // a polygonal path
   const int b = P.path_begin[q], n = P.path_begin[q + 1] - b;
   const double rmin = P.radius[q], rmax = rmin + P.offset;
   const bool cup = P.cup != nullptr && P.cup[q] != 0;
   const double rings = ceil(rmax / A.res);  // SpiralIterator nRings
-  // not checkable here: marked so that no checked result looks alike (REQ: also a pose range outside the request)
-  if (!(rmin >= 0.0) || !(rings <= (double)kPathMaxRings) || (REQ && !(b >= 0 && n >= 0 && (long long)b + n <= R.nposes))) {
+  // not checkable here: marked so that no checked result looks alike (with a pose count: also a pose range outside it; written
+  // b <= nposes - n, which ptxas compiles to fewer registers in the _poly kernel than a 64-bit b + n, see DESIGN.md)
+  if (!(rmin >= 0.0) || !(rings <= (double)kPathMaxRings) || (R.nposes >= 0 && !(b >= 0 && n >= 0 && b <= R.nposes - n))) {
     if (lane == 0) {
       P.is_safe[q] = 0; P.trav_out[q] = nan("");
-      if (REQ) R.area_out[q] = nan("");
+      if (R.area_out) R.area_out[q] = nan("");
       if (POLY) O.count[q] = cup ? -1 : 0;
     }
     return;
@@ -1213,7 +1216,7 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
   int fi = 0, fj = 0, freps = 1;
   for (int k = 0; k < n && ok; ++k) {
     sx = ex; sy = ey;
-    ex = P.xy[PS * (b + k)]; ey = P.xy[PS * (b + k) + 1];
+    ex = P.poses[PS * (b + k)]; ey = P.poses[PS * (b + k) + 1];
     if (n == 1) {  // :365-387
       if (!inclination_ok_d(A, P.rslope, ex, ey, ex, ey)) { ok = false; break; }
       int i, j;
@@ -1244,8 +1247,8 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
         bool seen = false;
         for (int s = 1 + lane; s < k; s += 32) {
           int pi0, pj0, pi1, pj1;
-          get_index_d(A, P.xy[PS * (b + s - 1)], P.xy[PS * (b + s - 1) + 1], pi0, pj0);
-          get_index_d(A, P.xy[PS * (b + s)], P.xy[PS * (b + s) + 1], pi1, pj1);
+          get_index_d(A, P.poses[PS * (b + s - 1)], P.poses[PS * (b + s - 1) + 1], pi0, pj0);
+          get_index_d(A, P.poses[PS * (b + s)], P.poses[PS * (b + s) + 1], pi1, pj1);
           seen = seen || line_checks_d(pi1, pj1, pi0, pj0, a, bb);
         }
         const bool cached = __any_sync(0xffffffffu, seen);
@@ -1269,7 +1272,7 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
   if (lane == 0) {
     P.is_safe[q] = ok ? 1 : 0;
     P.trav_out[q] = ok ? result : 0.0;
-    if (REQ) R.area_out[q] = 0.0;  // TraversabilityResult.area stays 0 for a circular path
+    if (R.area_out) R.area_out[q] = 0.0;  // TraversabilityResult.area stays 0 for a circular path
   }
   if (POLY) {
     // the last non-empty polygon published for the path: only an untraversable circle has one (inclination failures return first)
@@ -1284,34 +1287,22 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
   }
 }
 
-__global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, PathArgs P) {
-  check_paths_fresh_d<false, false>(A, L, P, UntravOut{}, CircleTable{}, UntravScratch{}, RequestArgs{});
+__global__ void __launch_bounds__(128) k_check_paths_fresh(FpArgs A, Layers L, PathArgs P, RequestArgs R) {
+  check_paths_fresh_d<false>(A, L, P, UntravOut{}, CircleTable{}, UntravScratch{}, R);
 }
 
 // k_check_paths_fresh that also returns the untraversable polygon of every path (te_check_footprint_paths_fresh2).  Per warp:
-// a row table for the 2 * 127 + 1 rows of the largest spiral and the chain stack.
+// a row table for the 2 * 127 + 1 rows of the largest spiral and the chain stack.  At its 128 registers four blocks fit an SM
+// anyway; saying so makes ptxas lay the kernel out about 6 % faster on H100 (DESIGN.md).
 constexpr int kFreshTableRows = 2 * kPathMaxRings + 1;
-__global__ void __launch_bounds__(128) k_check_paths_fresh_poly(FpArgs A, Layers L, PathArgs P, UntravOut O, CircleTable C) {
+__global__ void __launch_bounds__(128, 4) k_check_paths_fresh_poly(FpArgs A, Layers L, PathArgs P, UntravOut O, CircleTable C,
+                                                                RequestArgs R) {
   __shared__ int s_min[4][kFreshTableRows + 1], s_max[4][kFreshTableRows + 1];
   __shared__ int2 s_stack[4][2 * kFreshTableRows + 4];
   __shared__ int2 s_first[4][3];
   static_assert(sizeof(s_stack[0]) >= 3 * kFromCircleVertices * sizeof(double2), "fromCircle points and hull fit the stack");
   const int w = threadIdx.x >> 5;
-  check_paths_fresh_d<true, false>(A, L, P, O, C, UntravScratch{s_min[w], s_max[w], s_stack[w], s_first[w]}, RequestArgs{});
-}
-
-// The two above on the circular paths of a request (te_check_footprint_request); P.xy points at the 7-wide poses.
-__global__ void __launch_bounds__(128) k_check_paths_fresh_req(FpArgs A, Layers L, PathArgs P, RequestArgs R) {
-  check_paths_fresh_d<false, true>(A, L, P, UntravOut{}, CircleTable{}, UntravScratch{}, R);
-}
-
-__global__ void __launch_bounds__(128) k_check_paths_fresh_poly_req(FpArgs A, Layers L, PathArgs P, UntravOut O, CircleTable C,
-                                                                    RequestArgs R) {
-  __shared__ int s_min[4][kFreshTableRows + 1], s_max[4][kFreshTableRows + 1];
-  __shared__ int2 s_stack[4][2 * kFreshTableRows + 4];
-  __shared__ int2 s_first[4][3];
-  const int w = threadIdx.x >> 5;
-  check_paths_fresh_d<true, true>(A, L, P, O, C, UntravScratch{s_min[w], s_max[w], s_stack[w], s_first[w]}, R);
+  check_paths_fresh_d<true>(A, L, P, O, C, UntravScratch{s_min[w], s_max[w], s_stack[w], s_first[w]}, R);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -1447,11 +1438,10 @@ __device__ __forceinline__ PoseRT pose_rt_d(const double* p) {
 }
 
 // `toPosition * orientation * positionToVertex` (:496-500) for footprint vertex v, in the operand order of Eigen's Transform * vector.
-// The vertex comes from the kernel parameters, or with REQ from the path's own footprint `fxyz` in global memory.
-template <bool REQ>
+// The vertex comes from the path's own footprint `fxyz` in global memory, or without one from the kernel parameters.
 __device__ __forceinline__ double2 footprint_vertex_d(const PolyPathArgs& P, const float* fxyz, const PoseRT& T, int v) {
   double vx, vy, vz;
-  if (REQ) {
+  if (fxyz) {
     vx = (double)fxyz[3 * v]; vy = (double)fxyz[3 * v + 1]; vz = (double)fxyz[3 * v + 2];
   } else {
     vx = (double)P.fx[v]; vy = (double)P.fy[v]; vz = (double)P.fz[v];
@@ -1496,9 +1486,9 @@ __host__ __device__ inline size_t poly_warp_smem(int mcap, bool poly) {
 
 // One warp per pose index p.  Shared memory per warp: sA (2 mcap points: the hull input polygon1 ++ polygon2, then the hull) and
 // sB (mcap points: a conservative path's earlier polygon2, then the sorted hull input).  POLY: with compute_untraversable_polygon
-// set for the item's path, the walk goes on past blocked cells and collects them (:602-608, :634-638).  REQ: the items of the
-// polygonal paths of a request, each with its own footprint (RequestArgs); the poses of circular paths are no items.
-template <bool POLY, bool REQ>
+// set for the item's path, the walk goes on past blocked cells and collects them (:602-608, :634-638).  With per-path footprints
+// (R.fp_begin) each polygonal path uses its own, and the poses of circular paths are no items.
+template <bool POLY>
 __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Layers& L, const PolyPathArgs& P, const PolyUntravArgs& U,
                                                      const RequestArgs& R) {
   extern __shared__ double2 sPoly[];
@@ -1523,7 +1513,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
     if (P.path_begin[mid] <= p) lo = mid; else hi = mid - 1;
   }
   const int q = lo, b = P.path_begin[q], e = P.path_begin[q + 1], n = e - b, k = p - b;
-  if (REQ && R.fp_begin[q + 1] == R.fp_begin[q]) return;  // a pose of a circular path
+  if (R.fp_begin && R.fp_begin[q + 1] == R.fp_begin[q]) return;  // a pose of a circular path
   if (!(b >= 0 && b <= p && p < e && e <= P.nposes && (n == 1 || k >= 1))) {
     if (lane == 0) P.items[p] = it;
     return;
@@ -1534,8 +1524,8 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
   bool hit = false;    // POLY: the walk stopped at a blocked cell without collecting
   int nr_walk = 0, si_walk = 0;
   int nfp = P.nfp;
-  const float* fxyz = nullptr;  // REQ: the path's footprint
-  if (REQ) {
+  const float* fxyz = nullptr;  // the path's own footprint
+  if (R.fp_begin) {
     if (!__all_sync(0xffffffffu, request_footprint_ok_d(R, q, lane, 32))) {
       if (lane == 0) P.items[p] = it;  // flag 2
       return;
@@ -1559,10 +1549,10 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
   const int h = m / 2;  // polygon1 = sA[0, h), polygon2 = sA[h, m) for n > 1
   if (n == 1) {  // polygon2 of the pose
     const PoseRT T = pose_rt_d(pk);
-    if (lane < nfp) sA[lane] = footprint_vertex_d<REQ>(P, fxyz, T, lane);
+    if (lane < nfp) sA[lane] = footprint_vertex_d(P, fxyz, T, lane);
   } else if (!cons) {  // polygon1 = T_{k-1}(footprint), polygon2 = T_k(footprint)
     const PoseRT T = pose_rt_d(lane < nfp ? pk - 7 : pk);
-    if (lane < 2 * nfp) sA[lane] = footprint_vertex_d<REQ>(P, fxyz, T, lane < nfp ? lane : lane - nfp);
+    if (lane < 2 * nfp) sA[lane] = footprint_vertex_d(P, fxyz, T, lane < nfp ? lane : lane - nfp);
   } else {
     // polygon2 of pose k-1 by footprint slot s = 0..k-1 (list order: slot k-1 first): slot s holds T_s(footprint) plus the
     // start-to-end vectors d_{s+1}, ..., d_{k-1} added in that order (:510-520).  Entry i is always lane i % 32's.
@@ -1571,7 +1561,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
       const PoseRT T = pose_rt_d(pj);
       const double dx = j > 0 ? pj[0] - pj[-7] : 0.0, dy = j > 0 ? pj[1] - pj[-6] : 0.0;
       for (int i = lane; i < nfp * (j + 1); i += 32) {
-        if (i >= nfp * j) sB[i] = footprint_vertex_d<REQ>(P, fxyz, T, i - nfp * j);
+        if (i >= nfp * j) sB[i] = footprint_vertex_d(P, fxyz, T, i - nfp * j);
         else sB[i] = make_double2(sB[i].x + dx, sB[i].y + dy);
       }
     }
@@ -1586,7 +1576,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
         sA[l] = w;
         sA[h + nfp + l] = make_double2(w.x + dx, w.y + dy);
       } else {
-        const double2 w = footprint_vertex_d<REQ>(P, fxyz, T, l - ns);
+        const double2 w = footprint_vertex_d(P, fxyz, T, l - ns);
         sA[l] = make_double2(w.x - dx, w.y - dy);
         sA[h + l - ns] = w;
       }
@@ -1689,35 +1679,27 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
   }
 }
 
-__global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L, PolyPathArgs P) {
-  check_polygon_item_d<false, false>(A, L, P, PolyUntravArgs{}, RequestArgs{});
+__global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L, PolyPathArgs P, RequestArgs R) {
+  check_polygon_item_d<false>(A, L, P, PolyUntravArgs{}, R);
 }
 
-__global__ void __launch_bounds__(128) k_check_polygon_items_poly(FpArgs A, Layers L, PolyPathArgs P, PolyUntravArgs U) {
-  check_polygon_item_d<true, false>(A, L, P, U, RequestArgs{});
-}
-
-__global__ void __launch_bounds__(128) k_check_polygon_items_req(FpArgs A, Layers L, PolyPathArgs P, RequestArgs R) {
-  check_polygon_item_d<false, true>(A, L, P, PolyUntravArgs{}, R);
-}
-
-__global__ void __launch_bounds__(128) k_check_polygon_items_poly_req(FpArgs A, Layers L, PolyPathArgs P, PolyUntravArgs U, RequestArgs R) {
-  check_polygon_item_d<true, true>(A, L, P, U, R);
+__global__ void __launch_bounds__(128) k_check_polygon_items_poly(FpArgs A, Layers L, PolyPathArgs P, PolyUntravArgs U, RequestArgs R) {
+  check_polygon_item_d<true>(A, L, P, U, R);
 }
 
 // One thread per path: the area-weighted combination of the segment results in path order (:522-579).  An unsafe path reports 0;
 // a path the items could not check (bad range, non-finite pose, conservative list past the cap) is_safe 0 and NaN.  POLY: the
 // polygon of the item that failed (the reference publishes every segment's polygon and returns after the first failing one,
-// :555-567; traversable segments publish nothing); -1 for a path the items could not check.  REQ: the polygonal paths of a request
-// only, each with its own footprint; a footprint that cannot be checked makes its path not checkable.
-template <bool POLY, bool REQ>
+// :555-567; traversable segments publish nothing); -1 for a path the items could not check.  With per-path footprints (R.fp_begin)
+// the polygonal paths only; a footprint that cannot be checked makes its path not checkable.
+template <bool POLY>
 __device__ __forceinline__ void check_polygon_combine_d(const PolyPathArgs& P, const PolyUntravArgs& U, const RequestArgs& R) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= P.npaths) return;
-  int nfp = 0;  // REQ: the path's footprint vertices
+  int nfp = P.nfp;  // the path's footprint vertices
   bool fp_ok = true;
-  if (REQ) {
-    if (R.fp_begin[q + 1] == R.fp_begin[q]) return;  // a circular path: k_check_paths_fresh*_req writes its outputs
+  if (R.fp_begin) {
+    if (R.fp_begin[q + 1] == R.fp_begin[q]) return;  // a circular path: k_check_paths_fresh* writes its outputs
     fp_ok = request_footprint_ok_d(R, q, 0, 1);
     nfp = R.fp_begin[q + 1] - R.fp_begin[q];
   }
@@ -1728,7 +1710,7 @@ __device__ __forceinline__ void check_polygon_combine_d(const PolyPathArgs& P, c
   double trav = 0.0, area = 0.0;
   if (checkable && n > 0) {
     const bool cons = n > 1 && P.cons != nullptr && P.cons[q] != 0;
-    if (cons && (long long)(REQ ? nfp : P.nfp) * n > kPolyConsCap) checkable = false;
+    if (cons && (long long)nfp * n > kPolyConsCap) checkable = false;
     for (long long c = 7LL * b; c < 7LL * e && checkable; ++c) checkable = isfinite(P.poses[c]);
     const int k0 = n == 1 ? 0 : 1;
     for (int k = k0; k < n && checkable; ++k) checkable = P.items[b + k].q == q && P.items[b + k].flag != 2;
@@ -1766,20 +1748,12 @@ __device__ __forceinline__ void check_polygon_combine_d(const PolyPathArgs& P, c
   }
 }
 
-__global__ void __launch_bounds__(128) k_check_polygon_combine(PolyPathArgs P) {
-  check_polygon_combine_d<false, false>(P, PolyUntravArgs{}, RequestArgs{});
+__global__ void __launch_bounds__(128) k_check_polygon_combine(PolyPathArgs P, RequestArgs R) {
+  check_polygon_combine_d<false>(P, PolyUntravArgs{}, R);
 }
 
-__global__ void __launch_bounds__(128) k_check_polygon_combine_poly(PolyPathArgs P, PolyUntravArgs U) {
-  check_polygon_combine_d<true, false>(P, U, RequestArgs{});
-}
-
-__global__ void __launch_bounds__(128) k_check_polygon_combine_req(PolyPathArgs P, RequestArgs R) {
-  check_polygon_combine_d<false, true>(P, PolyUntravArgs{}, R);
-}
-
-__global__ void __launch_bounds__(128) k_check_polygon_combine_poly_req(PolyPathArgs P, PolyUntravArgs U, RequestArgs R) {
-  check_polygon_combine_d<true, true>(P, U, R);
+__global__ void __launch_bounds__(128) k_check_polygon_combine_poly(PolyPathArgs P, PolyUntravArgs U, RequestArgs R) {
+  check_polygon_combine_d<true>(P, U, R);
 }
 
 inline int signum(int v) { return (0 < v) - (v < 0); }
@@ -1890,16 +1864,14 @@ int ensure_ring_table(FootprintState& st, cudaStream_t s) {
   return 0;
 }
 
-// The path arguments of the fresh circular check (after ensure_ring_table and reset_filter_memo).
-PathArgs fresh_args(const FootprintState& st, const te_footprint_params* p, const float* robot_slope, int npaths, const int* path_begin,
-                    const double* xy, const double* radius, const unsigned char* cup, unsigned char* is_safe, double* trav_out) {
+// The path arguments every circular kernel takes: the ring table (after ensure_ring_table) and the memo.
+PathArgs path_args(const FootprintState& st, const te_footprint_params* p, const float* robot_slope) {
   PathArgs P{};
-  P.rslope = robot_slope; P.npaths = npaths; P.path_begin = path_begin; P.xy = xy; P.radius = radius; P.cup = cup;
+  P.rslope = robot_slope;
   P.offset = p->offset;
   P.ring_start = (const int*)st.rings.p;
   P.rings = P.ring_start + kPathMaxRings + 2;
   P.memo = (unsigned char*)st.memo.p;
-  P.is_safe = is_safe; P.trav_out = trav_out;
   return P;
 }
 
@@ -1911,42 +1883,6 @@ CircleTable circle_table() {
     C.sn[j] = std::sin(theta);
   }
   return C;
-}
-
-// The path arguments of the polygonal check, with the per-call item records reserved (after reset_filter_memo).
-int polygon_args(FootprintState& st, const te_footprint_params* p, const float* robot_slope, int npaths, int nposes, int max_points,
-                 const int* path_begin, const double* poses, const unsigned char* conservative, unsigned char* is_safe, double* trav_out,
-                 double* area_out, PolyPathArgs* out) {
-  if (st.items.reserve(sizeof(PolyItem) * (size_t)std::max(nposes, 1)) != cudaSuccess) {
-    st.why = "allocating the polygon items failed";
-    return TE_ERR_CUDA;
-  }
-  PolyPathArgs& P = *out;
-  P = PolyPathArgs{};
-  P.rslope = robot_slope; P.npaths = npaths; P.nposes = nposes; P.mcap = max_points;
-  P.path_begin = path_begin; P.poses = poses; P.cons = conservative;
-  P.memo = (unsigned char*)st.memo.p;
-  P.items = (PolyItem*)st.items.p;
-  P.is_safe = is_safe; P.trav_out = trav_out; P.area_out = area_out;
-  return 0;
-}
-
-// The untraversable polygons of the polygonal check: per item a count and max_vertices points, copied to the paths by the combine
-// kernel.
-int polygon_untrav_args(FootprintState& st, int nposes, const unsigned char* cup, int max_vertices, int* ucount, double* uxy,
-                        PolyUntravArgs* out) {
-  const size_t nitems = (size_t)std::max(nposes, 1);
-  const size_t cbytes = (sizeof(int) * nitems + 15) / 16 * 16;
-  if (st.upoly.reserve(cbytes + sizeof(double2) * nitems * (size_t)std::max(max_vertices, 1)) != cudaSuccess) {
-    st.why = "allocating the untraversable polygons failed";
-    return TE_ERR_CUDA;
-  }
-  *out = PolyUntravArgs{};
-  out->cup = cup;
-  out->out = UntravOut{max_vertices, ucount, uxy};
-  out->item_count = (int*)st.upoly.p;
-  out->item_xy = (double*)((char*)st.upoly.p + cbytes);
-  return 0;
 }
 
 // The item kernel (one warp per pose index, skipped without poses) and then the combine kernel of a polygonal check.  Four warps
@@ -1973,113 +1909,56 @@ int launch_polygon_kernels(FootprintState& st, KItems items, KCombine combine, c
 }
 }  // namespace
 
-int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                             const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                             int npaths, const int* path_begin, const double* xy, const double* radius, const unsigned char* cup,
-                             unsigned char* is_safe, double* trav_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s) {
-  if (int rc = ensure_ring_table(st, s)) return rc;
-  if (int rc = reset_filter_memo(st, v, s)) return rc;
-  const FpArgs a = filter_args(v, g, p, rough);
-  const Layers L{trav, slope, step, elev, rough};
-  const PathArgs P = fresh_args(st, p, robot_slope, npaths, path_begin, xy, radius, cup, is_safe, trav_out);
-  const long long threads = 32LL * npaths;
-  if (!ucount) {
-    k_check_paths_fresh<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P);
-    return 0;
-  }
-  k_check_paths_fresh_poly<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(a, L, P, UntravOut{max_vertices, ucount, uxy},
-                                                                              circle_table());
-  return 0;
-}
-
-int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                               const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                               int nfp, const float* footprint_xyz, int npaths, int nposes, const int* path_begin, const double* poses,
-                               const unsigned char* conservative, int max_points, unsigned char* is_safe, double* trav_out,
-                               double* area_out, const unsigned char* cup, int max_vertices, int* ucount, double* uxy,
-                               cudaStream_t s, int* launches) {
+int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const PathChecks& r,
+                       bool circular, bool clear_memo, cudaStream_t s, int* launches) {
   *launches = 0;
-  if (nfp < 1 || nfp > kPolyMaxVerts || max_points < 2 * nfp || max_points > 2 * kPolyConsCap) { st.why = "bad footprint size"; return TE_ERR_BAD_ARG; }
-  if (int rc = reset_filter_memo(st, v, s)) return rc;
-  const FpArgs a = filter_args(v, g, p, rough);
-  const Layers L{trav, slope, step, elev, rough};
-  PolyPathArgs P;
-  if (int rc = polygon_args(st, p, robot_slope, npaths, nposes, max_points, path_begin, poses, conservative, is_safe, trav_out, area_out, &P))
-    return rc;
-  P.nfp = nfp;
-  for (int k = 0; k < nfp; ++k) {
-    P.fx[k] = footprint_xyz[3 * k]; P.fy[k] = footprint_xyz[3 * k + 1]; P.fz[k] = footprint_xyz[3 * k + 2];
+  const bool circles = circular && (r.footprint_begin || !r.footprint);
+  const bool polygons = r.footprint_begin || r.footprint;
+  const int maxfp = r.footprint_begin ? r.max_footprint_vertices : r.nfp;
+  if (polygons && (maxfp < 0 || maxfp > kPolyMaxVerts || r.max_points < 2 || r.max_points > 2 * kPolyConsCap)) {
+    st.why = "bad footprint size";
+    return TE_ERR_BAD_ARG;
   }
-  if (!ucount)
-    return launch_polygon_kernels(st, k_check_polygon_items, k_check_polygon_combine, "k_check_polygon_items", false, a, L, P, s, launches);
-  PolyUntravArgs U;
-  if (int rc = polygon_untrav_args(st, nposes, cup, max_vertices, ucount, uxy, &U)) return rc;
+  if (circles)
+    if (int rc = ensure_ring_table(st, s)) return rc;
+  if (clear_memo)  // one memo for both kinds of path: it depends on the layers only
+    if (int rc = reset_filter_memo(st, v, s)) return rc;
+  const FpArgs a = filter_args(v, g, p, r.rough);
+  const Layers L{r.trav, r.slope, r.step, r.elev, r.rough};
+  const RequestArgs R{r.footprint_begin, r.footprint_xyz, r.nvertices, r.max_footprint_vertices, r.nposes, r.area_out};
+  if (circles) {
+    PathArgs C = path_args(st, p, r.robot_slope);
+    C.npaths = r.npaths; C.pose_stride = r.pose_stride; C.path_begin = r.path_begin; C.poses = r.poses; C.radius = r.radius;
+    C.cup = r.cup; C.is_safe = r.is_safe; C.trav_out = r.trav_out;
+    const unsigned blocks = (unsigned)((32LL * r.npaths + 127) / 128);
+    if (!r.ucount) k_check_paths_fresh<<<blocks, 128, 0, s>>>(a, L, C, R);
+    else k_check_paths_fresh_poly<<<blocks, 128, 0, s>>>(a, L, C, UntravOut{r.max_vertices, r.ucount, r.uxy}, circle_table(), R);
+    ++*launches;
+  }
+  if (!polygons) return 0;
+  // the polygonal paths: per pose index one item record and, with polygons, a count and max_vertices points copied to the paths
+  // by the combine kernel
+  const size_t nitems = (size_t)std::max(r.nposes, 1);
+  if (st.items.reserve(sizeof(PolyItem) * nitems) != cudaSuccess) { st.why = "allocating the polygon items failed"; return TE_ERR_CUDA; }
+  PolyPathArgs P{};
+  P.rslope = r.robot_slope; P.npaths = r.npaths; P.nposes = r.nposes; P.nfp = r.nfp; P.mcap = r.max_points;
+  P.path_begin = r.path_begin; P.poses = r.poses; P.cons = r.conservative;
+  P.memo = (unsigned char*)st.memo.p;
+  P.items = (PolyItem*)st.items.p;
+  P.is_safe = r.is_safe; P.trav_out = r.trav_out; P.area_out = r.area_out;
+  for (int k = 0; r.footprint && k < r.nfp; ++k) {
+    P.fx[k] = r.footprint[3 * k]; P.fy[k] = r.footprint[3 * k + 1]; P.fz[k] = r.footprint[3 * k + 2];
+  }
+  if (!r.ucount) return launch_polygon_kernels(st, k_check_polygon_items, k_check_polygon_combine, "k_check_polygon_items", false, a, L, P, s,
+                                               launches, R);
+  const size_t cbytes = (sizeof(int) * nitems + 15) / 16 * 16;
+  if (st.upoly.reserve(cbytes + sizeof(double2) * nitems * (size_t)std::max(r.max_vertices, 1)) != cudaSuccess) {
+    st.why = "allocating the untraversable polygons failed";
+    return TE_ERR_CUDA;
+  }
+  const PolyUntravArgs U{r.cup, (int*)st.upoly.p, (double*)((char*)st.upoly.p + cbytes), UntravOut{r.max_vertices, r.ucount, r.uxy}};
   return launch_polygon_kernels(st, k_check_polygon_items_poly, k_check_polygon_combine_poly, "k_check_polygon_items_poly", true, a, L, P, s,
-                                launches, U);
-}
-
-namespace {
-// The polygonal paths of a request: k_check_polygon_items(_poly)_req and the combine kernel, on the predicate memo in st.memo.
-int launch_request_polygons(FootprintState& st, const FpArgs& a, const Layers& L, const te_footprint_params* p, const float* robot_slope,
-                            int npaths, int nposes, const int* path_begin, const double* poses, const RequestArgs& R,
-                            const unsigned char* conservative, const unsigned char* cup, int max_points, unsigned char* is_safe,
-                            double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s,
-                            int* launches) {
-  PolyPathArgs P;
-  if (int rc = polygon_args(st, p, robot_slope, npaths, nposes, max_points, path_begin, poses, conservative, is_safe, trav_out, area_out, &P))
-    return rc;
-  if (!ucount)
-    return launch_polygon_kernels(st, k_check_polygon_items_req, k_check_polygon_combine_req, "k_check_polygon_items_req", false, a, L, P,
-                                  s, launches, R);
-  PolyUntravArgs U;
-  if (int rc = polygon_untrav_args(st, nposes, cup, max_vertices, ucount, uxy, &U)) return rc;
-  return launch_polygon_kernels(st, k_check_polygon_items_poly_req, k_check_polygon_combine_poly_req, "k_check_polygon_items_poly_req", true,
-                                a, L, P, s, launches, U, R);
-}
-}  // namespace
-
-int launch_check_request(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                         const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                         int npaths, int nposes, const int* path_begin, const double* poses, const double* radius, int nvertices,
-                         const int* footprint_begin, const float* footprint_xyz, int max_footprint_vertices,
-                         const unsigned char* conservative, const unsigned char* cup, int max_points, unsigned char* is_safe,
-                         double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s,
-                         int* launches) {
-  *launches = 0;
-  if (max_footprint_vertices < 0 || max_footprint_vertices > kPolyMaxVerts || max_points < 2 || max_points > 2 * kPolyConsCap) {
-    st.why = "bad footprint size";
-    return TE_ERR_BAD_ARG;
-  }
-  if (int rc = ensure_ring_table(st, s)) return rc;
-  if (int rc = reset_filter_memo(st, v, s)) return rc;  // one memo for both kinds of path: it depends on the layers only
-  const FpArgs a = filter_args(v, g, p, rough);
-  const Layers L{trav, slope, step, elev, rough};
-  const RequestArgs R{footprint_begin, footprint_xyz, nvertices, max_footprint_vertices, nposes, area_out};
-  const PathArgs C = fresh_args(st, p, robot_slope, npaths, path_begin, poses, radius, cup, is_safe, trav_out);
-  const unsigned blocks = (unsigned)((32LL * npaths + 127) / 128);
-  if (!ucount) k_check_paths_fresh_req<<<blocks, 128, 0, s>>>(a, L, C, R);
-  else k_check_paths_fresh_poly_req<<<blocks, 128, 0, s>>>(a, L, C, UntravOut{max_vertices, ucount, uxy}, circle_table(), R);
-  ++*launches;
-  return launch_request_polygons(st, a, L, p, robot_slope, npaths, nposes, path_begin, poses, R, conservative, cup, max_points, is_safe,
-                                 trav_out, area_out, max_vertices, ucount, uxy, s, launches);
-}
-
-int launch_map_polygons(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                        const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                        int npaths, int nposes, const int* path_begin, const double* poses, int nvertices, const int* footprint_begin,
-                        const float* footprint_xyz, int max_footprint_vertices, const unsigned char* conservative,
-                        const unsigned char* cup, int max_points, unsigned char* is_safe, double* trav_out, double* area_out,
-                        int max_vertices, int* ucount, double* uxy, cudaStream_t s, int* launches) {
-  *launches = 0;
-  if (max_footprint_vertices < 1 || max_footprint_vertices > kPolyMaxVerts || max_points < 2 || max_points > 2 * kPolyConsCap) {
-    st.why = "bad footprint size";
-    return TE_ERR_BAD_ARG;
-  }
-  const FpArgs a = filter_args(v, g, p, rough);
-  const Layers L{trav, slope, step, elev, rough};
-  const RequestArgs R{footprint_begin, footprint_xyz, nvertices, max_footprint_vertices, nposes, area_out};
-  return launch_request_polygons(st, a, L, p, robot_slope, npaths, nposes, path_begin, poses, R, conservative, cup, max_points, is_safe,
-                                 trav_out, area_out, max_vertices, ucount, uxy, s, launches);
+                                launches, U, R);
 }
 
 namespace {
@@ -2178,7 +2057,7 @@ int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry*
     }
     FpArgs a = filter_args(v, g, p, rough);
     const Layers L{trav, slope, step, elev, rough};
-    const PathArgs P = fresh_args(st, p, robot_slope, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+    const PathArgs P = path_args(st, p, robot_slope);
     if (nkeys > 0) {
       k_map_eval_circles<<<(unsigned)((32LL * nkeys + 127) / 128), 128, 0, s>>>(a, L, P, (const MapKey*)(base + o_keys), nkeys, cache,
                                                                                (MapRecord*)(base + o_recs), maxv, (double*)(base + o_hull));

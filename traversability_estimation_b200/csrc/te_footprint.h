@@ -53,51 +53,55 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
 void launch_check_paths(const SlabView& v, const te_geometry* g, double traversability_default, const float* footprint, const float* robot_slope, int npaths,
                         const int* path_begin, const double* xy, unsigned char* is_safe, double* trav, cudaStream_t s);
 
-// The same on the chain layers with an empty traversability_footprint cache per path (te_check_footprint_paths_fresh); whole map,
-// device pointers, radius / compute_untraversable_polygon per path.  Asynchronous on `s`.  `ucount` != nullptr: also the
-// untraversable polygon of every path (vertex count, up to `max_vertices` points in `uxy`; te_check_footprint_paths_fresh2).
-int launch_check_paths_fresh(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                             const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                             int npaths, const int* path_begin, const double* xy, const double* radius, const unsigned char* cup,
-                             unsigned char* is_safe, double* trav_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s);
-
-// TraversabilityMap::checkPolygonalFootprintPath for a batch of paths sharing one footprint (te_check_footprint_paths_polygon);
-// whole map, device pointers except `footprint_xyz` (host, nfp x 3 floats).  `max_points` bounds the hull input of one item
-// (polygon1 ++ polygon2): 2 * nfp without conservative paths, 2 * nfp * (poses of the longest conservative path) otherwise.
+// Checks of footprint paths on the chain layers with an empty traversability_footprint cache per path: circular paths as
+// TraversabilityMap::checkCircularFootprintPath (te_check_footprint_paths_fresh2), polygonal paths as checkPolygonalFootprintPath
+// (te_check_footprint_paths_polygon2), or both mixed in one request (te_check_footprint_request).  Whole map; device pointers
+// except `footprint`.
 constexpr int kPolyMaxVerts = 16;   // footprint vertices
 constexpr int kPolyConsCap = 1024;  // vertices of a conservative path's polygon2 (nfp * poses up to the segment)
-// `ucount` != nullptr: also the untraversable polygon of every path with cup[q] set (te_check_footprint_paths_polygon2); an item
-// whose bounding box spans more than kUntravRows map rows cannot build it (shared-memory row table): its path gets count -1.
+// An item of a polygonal path whose bounding box spans more than kUntravRows map rows cannot build its untraversable polygon
+// (shared-memory row table): its path gets count -1.
 constexpr int kUntravRows = 1024;
-int launch_check_paths_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                               const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                               int nfp, const float* footprint_xyz, int npaths, int nposes, const int* path_begin, const double* poses,
-                               const unsigned char* conservative, int max_points, unsigned char* is_safe, double* trav_out,
-                               double* area_out, const unsigned char* cup, int max_vertices, int* ucount, double* uxy,
-                               cudaStream_t s, int* launches);
+struct PathChecks {
+  const float *trav, *slope, *step, *rough, *elev;  // isTraversableForFilters' layers; rough null unless verify_roughness
+  const float* robot_slope;                          // null: no checkRobotInclination
+  int npaths;
+  int nposes;                     // poses in `poses`; < 0: not known (circular paths then need no pose range check)
+  const int* path_begin;          // [npaths + 1]
+  const double* poses;            // pose_stride doubles per pose: x y, or x y z qx qy qz qw (polygonal paths need 7)
+  int pose_stride;
+  const double* radius;           // per path; read for circular paths only
+  // Per-path footprints: path q has vertices footprint_begin[q] .. footprint_begin[q+1]-1 of footprint_xyz (3 floats each), none
+  // for a circular path, 1..max_footprint_vertices for a polygonal one.  Without footprint_begin every path is circular, unless
+  // `footprint` (HOST memory, nfp x 3 floats) is the one footprint all paths share.
+  const int* footprint_begin;
+  const float* footprint_xyz;
+  int nvertices, max_footprint_vertices;
+  int nfp;
+  const float* footprint;
+  const unsigned char* conservative;  // per path, may be null
+  const unsigned char* cup;           // compute_untraversable_polygon per path, may be null
+  // Hull input points of one polygonal item (polygon1 ++ polygon2): 2 * nfp without conservative paths, 2 * nfp * (poses of the
+  // longest conservative path) otherwise, for the largest footprint.
+  int max_points;
+  unsigned char* is_safe;
+  double* trav_out;
+  double* area_out;                   // may be null when every path is circular
+  int max_vertices;
+  int* ucount;                        // null: no untraversable polygons; else per path a vertex count and max_vertices points in uxy
+  double* uxy;
+};
+// Asynchronous on `s`.  Launches one kernel for the circular paths (when `r` can have any and `circular` is set; a te_map checks
+// them on its cache instead), then for the polygonal paths an items kernel when there are poses and a combine kernel, whatever the
+// footprints.  `clear_memo`: start from an empty isTraversableForFilters memo (st.memo); otherwise the caller keeps st.memo valid
+// for these layers (a te_map).
+int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const PathChecks& r,
+                       bool circular, bool clear_memo, cudaStream_t s, int* launches);
 
-// A whole check_footprint_path request (te_check_footprint_request): the two checks above on one predicate memo, each path with its
-// own footprint (footprint_begin / footprint_xyz, device pointers): none is circular (radius[q]), 1..max_footprint_vertices vertices
-// polygonal.  Poses are 7 doubles for both kinds.  `max_points` bounds the hull input of a polygonal item as in
-// launch_check_paths_polygon, for the largest footprint.  Three launches (two without poses), whatever the footprints.
-int launch_check_request(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                         const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                         int npaths, int nposes, const int* path_begin, const double* poses, const double* radius, int nvertices,
-                         const int* footprint_begin, const float* footprint_xyz, int max_footprint_vertices,
-                         const unsigned char* conservative, const unsigned char* cup, int max_points, unsigned char* is_safe,
-                         double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s,
-                         int* launches);
-
-// A request on a te_map (te_map_check_footprint_request).  Its polygonal paths: the polygonal half of launch_check_request on the
-// memo in st.memo, which the caller keeps (device pointers).  Its circular paths: launch_map_circles reads and fills the
-// traversability_footprint cache `cache` (device, NaN = empty) in the reference's order; every path array and output is in HOST
-// memory, hX / hY are the host copies of the cell-centre tables, and the call returns synchronised.
-int launch_map_polygons(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                        const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                        int npaths, int nposes, const int* path_begin, const double* poses, int nvertices, const int* footprint_begin,
-                        const float* footprint_xyz, int max_footprint_vertices, const unsigned char* conservative,
-                        const unsigned char* cup, int max_points, unsigned char* is_safe, double* trav_out, double* area_out,
-                        int max_vertices, int* ucount, double* uxy, cudaStream_t s, int* launches);
+// A request on a te_map (te_map_check_footprint_request): its polygonal paths run launch_path_checks on the memo the map keeps.
+// Its circular paths: launch_map_circles reads and fills the traversability_footprint cache `cache` (device, NaN = empty) in the
+// reference's order; every path array and output is in HOST memory, hX / hY are the host copies of the cell-centre tables, and
+// the call returns synchronised.
 struct MapRequestStats {
   long long candidates = 0;  // isTraversable calls the circular paths could make
   long long keys = 0;        // distinct circles among them (what k_map_eval_circles evaluates)
