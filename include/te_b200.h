@@ -206,6 +206,26 @@ int te_footprint_polygon(te_ctx* ctx, const te_geometry* g, const te_slab* slab,
                          const float* step, const float* roughness_or_null, const float* elevation, float* traversability_x,
                          float* traversability_rot, int memory);
 
+/* TraversabilityMap::traversabilityFootprint(const double& radius, const double& offset) — TraversabilityMap.cpp:307-318, as
+ * te_footprint2 — for nmaps independent whole maps of identical geometry in one call (multi-robot and MPC roll-out batches; the
+ * layout of te_chain_batched: map m at offset m*rows*cols in every layer, input and output).  Map m's outputs equal, bit for bit,
+ * what te_footprint2 returns for that map alone; a map never reads the cells of another.  1 <= nmaps <= 65535 (TE_ERR_BAD_ARG
+ * below 1), nmaps*rows*cols < 2^32 and nmaps*cols < 2^31 (TE_ERR_UNSUPPORTED otherwise); a circular-buffer start index is
+ * TE_ERR_UNSUPPORTED.  TE_MEM_HOST stages the nmaps*cols columns of every layer; TE_MEM_DEVICE is asynchronous on the context
+ * stream. */
+int te_footprint_batched(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, int32_t nmaps,
+                         const float* traversability, const float* slope, const float* step, const float* roughness_or_null,
+                         const float* elevation, float* traversability_footprint, float* slope_footprint_or_null,
+                         float* step_footprint_or_null, float* roughness_footprint_or_null, int memory);
+
+/* TraversabilityMap::traversabilityFootprint(double footprintYaw) — TraversabilityMap.cpp:239-305, as te_footprint_polygon — for
+ * nmaps whole maps in the layout and with the limits of te_footprint_batched: map m's traversability_x / traversability_rot equal,
+ * bit for bit, what te_footprint_polygon returns for that map alone. */
+int te_footprint_polygon_batched(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, int32_t npts,
+                                 const double* polygon_xy, double footprint_yaw, const float* traversability, const float* slope,
+                                 const float* step, const float* roughness_or_null, const float* elevation, float* traversability_x,
+                                 float* traversability_rot, int memory);
+
 /* TraversabilityMap::checkFootprintPath for circular footprints — checkCircularFootprintPath, TraversabilityMap.cpp:345-462 —
  * for a BATCH of paths in one launch (one thread per path: the service callback of the reference checks one path per call;
  * planners and MPC roll-outs ask for hundreds).  It is evaluated on a complete traversability_footprint layer, i.e. the output

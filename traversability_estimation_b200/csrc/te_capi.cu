@@ -808,15 +808,27 @@ int te_chain_batched(te_ctx* c, const te_geometry* g, const te_chain_params* p, 
   return chain_common(c, g, nullptr, p, nmaps, elev, slope, step, rough, trav, nullptr, nullptr, nullptr, memory);
 }
 
-int te_footprint2(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const te_footprint_params* p, const float* trav,
-                  const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
-                  float* step_fp, float* rough_fp, int memory) {
-  TE_ENTER(c);
+// The batch of a footprint entry: nmaps whole maps of one geometry back to back (te_footprint_batched, te_footprint_polygon_batched),
+// or one map or slab (nmaps = 1).  nmaps is a grid dimension of the sweep kernels, and their predicate work list stores 32-bit cell
+// indices of the batch.
+static int check_footprint_batch(const te_geometry* g, int nmaps) {
+  if (nmaps <= 0) return fail(TE_ERR_BAD_ARG, "number of maps must be positive");
+  if (nmaps > 65535) return fail(TE_ERR_UNSUPPORTED, "batch of %d maps: at most 65535", nmaps);
+  if ((unsigned long long)nmaps * g->rows * g->cols >= (1ULL << 32)) return fail(TE_ERR_UNSUPPORTED, "batch of 2^32 or more cells");
+  if ((unsigned long long)nmaps * g->cols >= (1ULL << 31)) return fail(TE_ERR_UNSUPPORTED, "batch of 2^31 or more columns");
+  return TE_OK;
+}
+
+// te_footprint2 (one map or slab) and te_footprint_batched (nmaps whole maps).
+static int footprint_common(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const te_footprint_params* p, int nmaps,
+                            const float* trav, const float* slope, const float* step, const float* rough, const float* elev, float* out,
+                            float* slope_fp, float* step_fp, float* rough_fp, int memory) {
   te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && slab == nullptr, &g0)) return rc;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && slab == nullptr && nmaps == 1, &g0)) return rc;
   const te_geometry* g = &g0;
   if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
   if (!(p->radius >= 0.0) || !(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint radius/offset must be >= 0");
+  if (int rc = check_footprint_batch(g, nmaps)) return rc;
   if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
   const bool use_rough = p->verify_roughness != 0;
@@ -824,32 +836,47 @@ int te_footprint2(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const
   if (int rc = resolve_slab(g, slab, te::footprint_halo(g, p), &s)) return rc;
   if (int rc = ensure_geometry(c, g)) return rc;
   Staging st(c, memory == TE_MEM_HOST, g_in);
-  const int in_cols = s.halo_left + s.col_count + s.halo_right;
+  const int in_cols = (s.halo_left + s.col_count + s.halo_right) * nmaps, out_cols = s.col_count * nmaps;
   const float* in[5] = {st.in_layer(trav, in_cols), st.in_layer(slope, in_cols), st.in_layer(step, in_cols), st.in_layer(elev, in_cols),
                         st.in_layer(use_rough ? rough : nullptr, in_cols)};
-  float* o[4] = {st.out_layer(out, s.col_count), st.out_layer(slope_fp, s.col_count), st.out_layer(step_fp, s.col_count),
-                 st.out_layer(use_rough ? rough_fp : nullptr, s.col_count)};
+  float* o[4] = {st.out_layer(out, out_cols), st.out_layer(slope_fp, out_cols), st.out_layer(step_fp, out_cols),
+                 st.out_layer(use_rough ? rough_fp : nullptr, out_cols)};
   if (st.rc) return st.rc;
   int nl = 0;
-  int rc = te::launch_footprint(c->fp, make_view(c, g, s), g, p, in[0], in[1], in[2], in[4], in[3], o[0], o[1], o[2], o[3], c->sms,
+  int rc = te::launch_footprint(c->fp, make_view(c, g, s), g, p, nmaps, in[0], in[1], in[2], in[4], in[3], o[0], o[1], o[2], o[3], c->sms,
                                 c->stream, &nl);
   if (rc != 0) return fail(rc, "footprint sweep failed: %s", c->fp.why.c_str());
   if (int r2 = launch_check(c, "footprint", nl)) return r2;
   return st.finish();
 }
 
-int te_footprint_polygon(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const te_footprint_params* p, int32_t npts,
-                         const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step, const float* rough,
-                         const float* elev, float* out_x, float* out_rot, int memory) {
+int te_footprint2(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, const float* trav,
+                  const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
+                  float* step_fp, float* rough_fp, int memory) {
   TE_ENTER(c);
+  return footprint_common(c, g, slab, p, 1, trav, slope, step, rough, elev, out, slope_fp, step_fp, rough_fp, memory);
+}
+
+int te_footprint_batched(te_ctx* c, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, const float* trav,
+                         const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
+                         float* step_fp, float* rough_fp, int memory) {
+  TE_ENTER(c);
+  return footprint_common(c, g, nullptr, p, nmaps, trav, slope, step, rough, elev, out, slope_fp, step_fp, rough_fp, memory);
+}
+
+// te_footprint_polygon (one map or slab) and te_footprint_polygon_batched (nmaps whole maps).
+static int footprint_polygon_common(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const te_footprint_params* p, int nmaps,
+                                    int32_t npts, const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step,
+                                    const float* rough, const float* elev, float* out_x, float* out_rot, int memory) {
   te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && slab == nullptr, &g0)) return rc;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && slab == nullptr && nmaps == 1, &g0)) return rc;
   const te_geometry* g = &g0;
   if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
   if (npts < 3 || npts > 16 || !pts_xy) return fail(TE_ERR_BAD_ARG, "footprint polygon needs 3 to 16 vertices");
   if (!std::isfinite(yaw)) return fail(TE_ERR_BAD_ARG, "footprint yaw is not finite");
   for (int k = 0; k < 2 * npts; ++k)
     if (!std::isfinite(pts_xy[k])) return fail(TE_ERR_BAD_ARG, "footprint polygon vertex is not finite");
+  if (int rc = check_footprint_batch(g, nmaps)) return rc;
   if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
   if (!out_x || !out_rot) return fail(TE_ERR_BAD_ARG, "output layer is null");
   const bool use_rough = p->verify_roughness != 0;
@@ -857,17 +884,31 @@ int te_footprint_polygon(te_ctx* c, const te_geometry* g_in, const te_slab* slab
   if (int rc = resolve_slab(g, slab, te::footprint_polygon_halo(g, p, npts, pts_xy), &s)) return rc;
   if (int rc = ensure_geometry(c, g)) return rc;
   Staging st(c, memory == TE_MEM_HOST, g_in);
-  const int in_cols = s.halo_left + s.col_count + s.halo_right;
+  const int in_cols = (s.halo_left + s.col_count + s.halo_right) * nmaps, out_cols = s.col_count * nmaps;
   const float* in[5] = {st.in_layer(trav, in_cols), st.in_layer(slope, in_cols), st.in_layer(step, in_cols), st.in_layer(elev, in_cols),
                         st.in_layer(use_rough ? rough : nullptr, in_cols)};
-  float* o[2] = {st.out_layer(out_x, s.col_count), st.out_layer(out_rot, s.col_count)};
+  float* o[2] = {st.out_layer(out_x, out_cols), st.out_layer(out_rot, out_cols)};
   if (st.rc) return st.rc;
   int nl = 0;
   int rc = te::launch_footprint_polygon(c->fp, make_view(c, g, s), g, p, npts, pts_xy, yaw, in[0], in[1], in[2], in[4], in[3], o[0], o[1],
-                                        c->sms, c->stream, &nl);
+                                        nmaps, c->sms, c->stream, &nl);
   if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", c->fp.why.c_str());
   if (int r2 = launch_check(c, "polygon footprint", nl)) return r2;
   return st.finish();
+}
+
+int te_footprint_polygon(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, int32_t npts,
+                         const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step, const float* rough,
+                         const float* elev, float* out_x, float* out_rot, int memory) {
+  TE_ENTER(c);
+  return footprint_polygon_common(c, g, slab, p, 1, npts, pts_xy, yaw, trav, slope, step, rough, elev, out_x, out_rot, memory);
+}
+
+int te_footprint_polygon_batched(te_ctx* c, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, int32_t npts,
+                                 const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step,
+                                 const float* rough, const float* elev, float* out_x, float* out_rot, int memory) {
+  TE_ENTER(c);
+  return footprint_polygon_common(c, g, nullptr, p, nmaps, npts, pts_xy, yaw, trav, slope, step, rough, elev, out_x, out_rot, memory);
 }
 
 int te_footprint(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, const float* trav,
@@ -1299,7 +1340,7 @@ int te_map_footprint(te_map* m, const te_footprint_params* p, float* out, int me
   const te_slab s{0, g->cols, 0, 0};
   const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
   int nl = 0;
-  int rc = te::launch_footprint(m->fp, make_view(c, g, s), g, p, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p,
+  int rc = te::launch_footprint(m->fp, make_view(c, g, s), g, p, 1, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p,
                                 rough, (const float*)m->elev.p, (float*)m->fresh.p, nullptr, nullptr, nullptr, c->sms, c->stream, &nl);
   if (rc != 0) return fail(rc, "footprint sweep failed: %s", m->fp.why.c_str());
   te::launch_map_merge((const float*)m->fresh.p, (float*)m->cache.p, (out && memory == TE_MEM_DEVICE) ? out : nullptr, map_cells(m), c->sms,
@@ -1331,7 +1372,7 @@ int te_map_footprint_polygon(te_map* m, const te_footprint_params* p, int32_t np
   const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
   int nl = 0;
   int rc = te::launch_footprint_polygon(m->fp, make_view(c, g, s), g, p, npts, pts_xy, yaw, (const float*)m->trav.p, (const float*)m->slope.p,
-                                        (const float*)m->step.p, rough, (const float*)m->elev.p, o[0], o[1], c->sms, c->stream, &nl);
+                                        (const float*)m->step.p, rough, (const float*)m->elev.p, o[0], o[1], 1, c->sms, c->stream, &nl);
   if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", m->fp.why.c_str());
   if (int r2 = launch_check(c, "map polygon footprint", nl)) return r2;
   return st.finish();

@@ -62,6 +62,10 @@ struct FpArgs {
   // the same for k_sweep_fast as non-negative BYTE offsets from the prefix entry L columns and L rows before the centre's own
   // (one 32-bit add to a 64-bit base per load instead of a sign-extended 64-bit index computation)
   unsigned off8_hi[64], off8_lo[64];
+  // maps of a batch (te_footprint_batched): map m's input buffer, predicate bytes, prefix sums, bit and nearest columns start
+  // m * in_ncols columns into theirs, its outputs m * out_ncols columns into theirs.  The sweep kernels take m from blockIdx.z or
+  // decode it from their flat index.  Kept last so that the path-check kernels, which do not read it, keep their parameter layout.
+  int nmaps;
 };
 
 __device__ __forceinline__ float lay(const FpArgs& A, const float* l, int i, int j) {  // caller guarantees (i,j) is in the map
@@ -266,13 +270,13 @@ __global__ void __launch_bounds__(256) k_pred_classify(FpArgs A, Layers L, unsig
   bool heavy = false;
   size_t c = 0;
   if (in) {
-    c = (size_t)lb * A.rows + i;
+    c = ((unsigned)blockIdx.z * A.in_ncols + lb) * (unsigned)A.rows + i;  // cell of the batch, < 2^32: the work list stores it
     heavy = __ldg(L.slope + c) == 0.0f || __ldg(L.step + c) == 0.0f || (A.verify_rough && __ldg(L.rough + c) == 0.0f);
     if (!heavy) {
       blocked[c] = 0;
       const int oj = lb + A.in_col0 - A.out_col0;
       if (oj >= 0 && oj < A.out_ncols) {
-        const size_t oc = (size_t)oj * A.rows + i;
+        const size_t oc = ((unsigned)blockIdx.z * A.out_ncols + oj) * (unsigned)A.rows + i;
         if (slope_fp) slope_fp[oc] = nanf_();
         if (step_fp) step_fp[oc] = nanf_();
         if (rough_fp) rough_fp[oc] = nanf_();
@@ -295,12 +299,16 @@ __global__ void __launch_bounds__(128) k_pred_heavy(FpArgs A, Layers L, unsigned
   for (unsigned k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
     const unsigned c = list[k];
     const int i = (int)(c % (unsigned)A.rows);
-    const int j = A.in_col0 + (int)(c / (unsigned)A.rows);
-    const FilterVerdict v = filters_d(A, L, i, j);
+    const unsigned col = c / (unsigned)A.rows;            // input-buffer column of the batch
+    const unsigned m = col / (unsigned)A.in_ncols;        // its map
+    const int j = A.in_col0 + (int)(col - m * (unsigned)A.in_ncols);
+    const size_t mc = (size_t)m * A.in_ncols * A.rows;    // the map's first cell: filters_d reads its layers only
+    const Layers Lm{L.trav + mc, L.slope + mc, L.step + mc, L.elev + mc, L.rough ? L.rough + mc : nullptr};
+    const FilterVerdict v = filters_d(A, Lm, i, j);
     blocked[c] = v.ok ? 0 : 1;
     const int oj = j - A.out_col0;
     if (oj >= 0 && oj < A.out_ncols) {
-      const size_t oc = (size_t)oj * A.rows + i;
+      const size_t oc = ((size_t)m * A.out_ncols + oj) * A.rows + i;
       if (slope_fp) slope_fp[oc] = v.sfp;
       if (step_fp) step_fp[oc] = v.tfp;
       if (rough_fp) rough_fp[oc] = v.rfp;
@@ -309,10 +317,13 @@ __global__ void __launch_bounds__(128) k_pred_heavy(FpArgs A, Layers L, unsigned
 }
 
 __global__ void __launch_bounds__(256) k_sweep(FpArgs A, Layers L, const unsigned char* __restrict__ blocked, float* __restrict__ out) {
-  const long long total = (long long)A.rows * A.out_ncols;
+  const long long total = (long long)A.rows * A.out_ncols * A.nmaps;
   for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < total; c += (long long)gridDim.x * blockDim.x) {
     const int i = (int)(c % A.rows);
-    const int j = A.out_col0 + (int)(c / A.rows);
+    const unsigned col = (unsigned)(c / A.rows);  // output column of the batch
+    const unsigned m = col / (unsigned)A.out_ncols;
+    const int j = A.out_col0 + (int)(col - m * (unsigned)A.out_ncols);
+    const size_t mc = (size_t)m * A.in_ncols * A.rows;  // the map's first input cell
     const double cx = A.X[i], cy = A.Y[j];
     int n = 0;
     double t = 0.0;
@@ -329,7 +340,7 @@ __global__ void __launch_bounds__(256) k_sweep(FpArgs A, Layers L, const unsigne
       }
       const int lb = b - A.in_col0;
       if (lb < 0 || lb >= A.in_ncols) continue;  // cannot happen with the halo te_footprint demands
-      const size_t cc = (size_t)lb * A.rows + a;
+      const size_t cc = mc + (size_t)lb * A.rows + a;
       if (blocked[cc]) {
         const int d2 = di * di + dj * dj;
         const double nr = A.int_norm ? (double)(int)sqrt((double)d2) : sqrt((double)d2);
@@ -359,11 +370,10 @@ __global__ void __launch_bounds__(256) k_sweep(FpArgs A, Layers L, const unsigne
 // Distance along the row index from every cell to the nearest blocked cell of its own column (from the packed flags):
 // the sweep then needs ONE byte per disk column to know the nearest blocked cell of that column.
 __global__ void __launch_bounds__(256) k_fp_nearest(FpArgs A, unsigned char* __restrict__ near) {
-  const long long total = (long long)A.rows * A.in_ncols;
+  const long long total = (long long)A.rows * A.in_ncols * A.nmaps;  // every column of the batch: they are independent
   for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < total; c += (long long)gridDim.x * blockDim.x) {
     const int i = (int)(c % A.rows);
-    const int lb = (int)(c / A.rows);
-    const unsigned* wcol = A.bits + (size_t)lb * A.words;
+    const unsigned* wcol = A.bits + (size_t)(c / A.rows) * A.words;
     const int r0 = i - 31, w0 = r0 >> 5, sh = r0 & 31;
     const unsigned a0 = (w0 >= 0 && w0 < A.words) ? __ldg(wcol + w0) : 0u;
     const unsigned a1 = (w0 + 1 >= 0 && w0 + 1 < A.words) ? __ldg(wcol + w0 + 1) : 0u;
@@ -385,7 +395,8 @@ __global__ void __launch_bounds__(256) k_fp_prepare_p(FpArgs A, Layers L, const 
                                                     unsigned* __restrict__ bits) {
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (int lb = warp; lb < A.in_ncols; lb += nwarps) {
+  const int ncols = A.in_ncols * A.nmaps;  // every column of the batch: they are independent
+  for (int lb = warp; lb < ncols; lb += nwarps) {
     const float* tcol = L.trav + (size_t)lb * A.rows;
     const unsigned char* bcol = blocked + (size_t)lb * A.rows;
     double* pcol = P + (size_t)lb * (A.rows + 1);
@@ -423,11 +434,14 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
   // depends only on the column — which disk columns exist, whether any blocked cell lies near the warp at all — is warp-uniform
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int j = A.out_col0 + (int)blockIdx.y;
+  // map blockIdx.z of the batch: its predicate bytes, prefix sums, bit and nearest columns start mb columns into the batch's
+  // (mb + any input-buffer column < 2^31, which run_predicates checks); column b of the map is batch column b - c0
+  const int mb = (int)blockIdx.z * A.in_ncols, c0 = A.in_col0 - mb;
   {
     const int lane = threadIdx.x & 31, i0 = i - lane;
     if (i0 >= A.rows) return;  // whole warp beyond the last row
     const bool active = i < A.rows;
-    const size_t c = (size_t)blockIdx.y * A.rows + (active ? i : 0);
+    const size_t c = ((unsigned)blockIdx.z * A.out_ncols + blockIdx.y) * (unsigned)A.rows + (active ? i : 0);  // < 2^32
     const double cx = A.X[active ? i : 0], cy = A.Y[j];
     // disk columns that exist in the map and in this slab's buffer.  l_lo is written as a negated minimum: ptxas of CUDA 12.9 for
     // sm_90a fuses max(-L, max(-j, in_col0 - j)) into one three-input VIMNMX3 that reads +L, and the loops bounded by l_hi then ran
@@ -440,7 +454,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
       const int w0 = max(i0 - A.L, 0) >> 5, w1 = min(i0 + 31 + A.L, A.rows - 1) >> 5;
       unsigned acc = 0;
       for (int l = l_lo + lane; l <= l_hi; l += 32) {  // a lane per disk column, at most four words each
-        const unsigned* wc = A.bits + (size_t)(j + l - A.in_col0) * A.words;
+        const unsigned* wc = A.bits + (size_t)(j + l - c0) * A.words;
         for (int w = w0; w <= w1; ++w) acc |= __ldg(wc + w);
       }
       warp_any = __any_sync(0xffffffffu, acc != 0u);
@@ -449,7 +463,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
     // ---- nearest blocked cell of the visited set, as a squared index distance ------------------------
     int best = 0x7fffffff;
     if (warp_any) {
-      const unsigned char* nr = A.near + (size_t)(j + l_lo - A.in_col0) * A.rows + i;
+      const unsigned char* nr = A.near + (size_t)(j + l_lo - c0) * A.rows + i;
       for (int l = l_lo; l <= l_hi; ++l, nr += A.rows) {
         const int g = (int)__ldg(nr);              // nearest blocked row offset in this column
         const int hw = A.halfw_c[l + A.L];
@@ -462,7 +476,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
         if (a < 0 || b < 0 || a >= A.rows || b >= A.cols_total || lb < 0 || lb >= A.in_ncols) continue;
         const double dx = A.X[a] - cx, dy = A.Y[b] - cy;
         if (!(dx * dx + dy * dy <= A.rmax2)) continue;
-        if (blocked[(size_t)lb * A.rows + a]) best = min(best, di * di + dj * dj);
+        if (blocked[(size_t)(mb + lb) * A.rows + a]) best = min(best, di * di + dj * dj);
       }
     }
     // ---- sums over the visited cells before the first blocked one --------------------------------------
@@ -482,7 +496,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
       // nothing blocked near this warp and no clipping along the rows: 2 loads and 2 additions per disk column, offsets from
       // the constant bank
       // biased base: the entry L columns and L rows before the centre's own, so that every table offset is a non-negative byte count
-      const char* pb = reinterpret_cast<const char*>(A.P + ((size_t)(j - A.in_col0) * ((size_t)A.rows + 1) + i)) -
+      const char* pb = reinterpret_cast<const char*>(A.P + ((size_t)(j - c0) * ((size_t)A.rows + 1) + i)) -
                        8 * ((ptrdiff_t)A.L * ((ptrdiff_t)A.rows + 1) + A.L);
       auto P8 = [&](unsigned off) { return __ldg(reinterpret_cast<const double*>(pb + off)); };
       int l = l_lo + A.L;
@@ -495,7 +509,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
       t += t_b;
       n = (int)A.cntp[l_end + 1] - (int)A.cntp[l_lo + A.L];
     } else {
-      const double* pc = A.P + (size_t)(j + l_lo - A.in_col0) * (A.rows + 1);
+      const double* pc = A.P + (size_t)(j + l_lo - c0) * (A.rows + 1);
       const size_t pstride = (size_t)A.rows + 1;
       if (i - A.L >= 0 && i + A.L < A.rows) {  // no clipping along the rows: two independent accumulators
         int l = l_lo;
@@ -528,7 +542,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
         if (a < 0 || b < 0 || a >= A.rows || b >= A.cols_total || lb < 0 || lb >= A.in_ncols) continue;
         const double dx = A.X[a] - cx, dy = A.Y[b] - cy;
         if (!(dx * dx + dy * dy <= A.rmax2)) continue;
-        const float v = __ldg(L.trav + (size_t)lb * A.rows + a);
+        const float v = __ldg(L.trav + (size_t)(mb + lb) * A.rows + a);
         t += finitef(v) ? (double)v : A.tdefault;
         ++n;
       }
@@ -547,7 +561,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
           const double dx = A.X[a] - cx, dy = A.Y[b] - cy;
           if (!(dx * dx + dy * dy <= A.rmax2)) continue;
         }
-        const size_t cc = (size_t)lb * A.rows + a;
+        const size_t cc = (size_t)(mb + lb) * A.rows + a;
         if (blocked[cc]) break;
         const float v = __ldg(L.trav + cc);
         t += finitef(v) ? (double)v : A.tdefault;
@@ -614,6 +628,8 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
   extern __shared__ double sP[];  // [NC][PS] prefix sums of t'; then [NC][PB] uint16 prefix counts of blocked cells
   const int Lr = Q.Lp, NR = PTR + 2 * Lr, NC = PTC + 2 * Lr, PS = NR + 1;
   unsigned short* sB = reinterpret_cast<unsigned short*>(sP + (size_t)NC * PS);
+  // map blockIdx.z of the batch: its input-buffer columns start mb columns into the batch's, its output columns mbo
+  const int mb = (int)blockIdx.z * A.in_ncols, mbo = (int)blockIdx.z * A.out_ncols;
   const int r0 = (int)blockIdx.x * PTR, c0 = A.out_col0 + (int)blockIdx.y * PTC;
   const int rb = r0 - Lr, cb = c0 - Lr;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -624,8 +640,8 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
   for (int cc = warp; cc < NC; cc += 8) {
     const int gcol = cb + cc, lb = gcol - A.in_col0;
     const bool col_ok = gcol >= 0 && gcol < A.cols_total && lb >= 0 && lb < A.in_ncols;
-    const float* tcol = trav + (size_t)(col_ok ? lb : 0) * A.rows;
-    const unsigned char* bcol = blocked + (size_t)(col_ok ? lb : 0) * A.rows;
+    const float* tcol = trav + (size_t)(mb + (col_ok ? lb : 0)) * A.rows;
+    const unsigned char* bcol = blocked + (size_t)(mb + (col_ok ? lb : 0)) * A.rows;
     double v[4];
     int cb4[4];
     unsigned bw = 0;
@@ -760,7 +776,7 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
     if (nblk > 0) result = 0.0f;                       // :297 / :301
     else if (n == 0) result = (float)A.tdefault;       // :625-628
     else result = (float)(t / (double)n);              // :630
-    out[(size_t)(j - A.out_col0) * A.rows + i] = result;
+    out[(size_t)(mbo + j - A.out_col0) * A.rows + i] = result;
   }
 }
 
@@ -2205,27 +2221,30 @@ int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, int
   return 0;
 }
 
-// isTraversableForFilters for every cell of the slab + halo into st.block (k_pred_classify + k_pred_heavy); fills the geometry /
-// parameter part of the kernel arguments.  Shared by the circular and the polygonal sweep.
-int run_predicates(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+// isTraversableForFilters for every cell of the slab + halo of each of the nmaps maps into st.block (k_pred_classify +
+// k_pred_heavy); fills the geometry / parameter part of the kernel arguments.  Shared by the circular and the polygonal sweep.
+int run_predicates(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int nmaps, const float* trav,
                    const float* slope, const float* step, const float* rough, const float* elev, float* slope_fp, float* step_fp,
                    float* rough_fp, int sms, cudaStream_t s, FpArgs* out_args) {
   const double rmax = p->radius + p->offset;
-  const size_t ncell_in = (size_t)v.rows * v.in_ncols;
+  if (nmaps < 1 || nmaps > 65535) { st.why = "number of maps outside 1 .. 65535"; return TE_ERR_UNSUPPORTED; }
+  const size_t ncell_in = (size_t)v.rows * v.in_ncols * nmaps;
+  if (ncell_in >= ((size_t)1 << 32)) { st.why = "slab or batch of 2^32 or more cells"; return TE_ERR_UNSUPPORTED; }
+  if ((size_t)v.in_ncols * nmaps >= ((size_t)1 << 31)) { st.why = "batch of 2^31 or more columns"; return TE_ERR_UNSUPPORTED; }
   if (st.block.reserve(ncell_in) != cudaSuccess) { st.why = "allocating the predicate bytes failed"; return TE_ERR_CUDA; }
   FpArgs a = filter_args(v, g, p, rough);
   a.rmin = p->radius; a.rmax = rmax; a.rmax2 = rmax * rmax;
   a.n_spiral = st.n_spiral; a.spiral = (const int*)st.spiral.p;
+  a.nmaps = nmaps;
   const Layers L{trav, slope, step, elev, rough};
   const long long t1 = (long long)ncell_in;
   const int g1 = (int)std::min<long long>((t1 + 127) / 128, (long long)sms * 16);
   {
-    if (ncell_in >= ((size_t)1 << 32)) { st.why = "slab of 2^32 or more cells"; return TE_ERR_UNSUPPORTED; }
     if (st.list.reserve(sizeof(unsigned) * (ncell_in + 1)) != cudaSuccess) { st.why = "allocating the predicate work list failed"; return TE_ERR_CUDA; }
     unsigned* cnt = (unsigned*)st.list.p;          // word 0: list length; entries follow
     unsigned* lst = cnt + 1;
     cudaMemsetAsync(cnt, 0, sizeof(unsigned), s);
-    const dim3 gc((unsigned)((v.rows + 255) / 256), (unsigned)v.in_ncols);
+    const dim3 gc((unsigned)((v.rows + 255) / 256), (unsigned)v.in_ncols, (unsigned)nmaps);
     k_pred_classify<<<gc, 256, 0, s>>>(a, L, (unsigned char*)st.block.p, slope_fp, step_fp, rough_fp, lst, cnt);
     k_pred_heavy<<<std::max(g1, 1), 128, 0, s>>>(a, L, (unsigned char*)st.block.p, slope_fp, step_fp, rough_fp, lst, cnt);
   }
@@ -2233,7 +2252,7 @@ int run_predicates(FootprintState& st, const SlabView& v, const te_geometry* g, 
   return 0;
 }
 
-int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int nmaps, const float* trav,
                      const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
                      float* step_fp, float* rough_fp, int sms, cudaStream_t s, int* launches) {
   const double rmax = p->radius + p->offset;
@@ -2250,10 +2269,10 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
     st.tables_valid = false;
   }
   FpArgs a{};
-  if (int rc = run_predicates(st, v, g, p, trav, slope, step, rough, elev, slope_fp, step_fp, rough_fp, sms, s, &a)) return rc;
-  const size_t ncell_in = (size_t)v.rows * v.in_ncols;
+  if (int rc = run_predicates(st, v, g, p, nmaps, trav, slope, step, rough, elev, slope_fp, step_fp, rough_fp, sms, s, &a)) return rc;
+  const size_t ncols_in = (size_t)v.in_ncols * nmaps, ncell_in = (size_t)v.rows * ncols_in;  // input-buffer columns / cells of the batch
   const Layers L{trav, slope, step, elev, rough};
-  const long long t1 = (long long)ncell_in, t2 = (long long)v.rows * v.out_ncols;
+  const long long t1 = (long long)ncell_in, t2 = (long long)v.rows * v.out_ncols * nmaps;
   const int g2 = (int)std::min<long long>((t2 + 255) / 256, (long long)sms * 8);
   const int Lmax = (int)std::floor(rmax / g->resolution + 1e-9);
   const bool fast = Lmax <= 31 && v.out_ncols <= 65535 && std::getenv("TE_FOOTPRINT_BRUTE") == nullptr;
@@ -2318,8 +2337,8 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
     st.tables_valid = true;
   }
   const int words = (v.rows + 31) / 32;
-  const size_t pbytes = sizeof(double) * (size_t)(v.rows + 1) * v.in_ncols;
-  const size_t wbytes = (sizeof(unsigned) * (size_t)words * v.in_ncols + 15) / 16 * 16;
+  const size_t pbytes = sizeof(double) * (size_t)(v.rows + 1) * ncols_in;
+  const size_t wbytes = (sizeof(unsigned) * (size_t)words * ncols_in + 15) / 16 * 16;
   const size_t gbytes = ncell_in;
   if (st.prefix.reserve(pbytes + wbytes + gbytes) != cudaSuccess) { st.why = "allocating the footprint prefix sums failed"; return TE_ERR_CUDA; }
   char* const prefix = (char*)st.prefix.p;
@@ -2346,11 +2365,12 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
       a.cntp[k + 1] = (short)(a.cntp[k] + (h >= 0 ? 2 * h + 1 : 0));
     }
   }
-  const int g3 = std::min(sms * 8, (v.in_ncols + 7) / 8);
+  const int g3 = (int)std::min<long long>((long long)sms * 8, ((long long)ncols_in + 7) / 8);
   const int g1b = (int)std::min<long long>((t1 + 255) / 256, (long long)sms * 8);
   k_fp_prepare_p<<<std::max(g3, 1), 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, (double*)prefix, (unsigned*)(prefix + pbytes));
   k_fp_nearest<<<std::max(g1b, 1), 256, 0, s>>>(a, (unsigned char*)prefix + pbytes + wbytes);
-  k_sweep_fast<<<dim3((unsigned)((v.rows + 255) / 256), (unsigned)v.out_ncols), 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
+  const dim3 gs((unsigned)((v.rows + 255) / 256), (unsigned)v.out_ncols, (unsigned)nmaps);
+  k_sweep_fast<<<gs, 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
   if (launches) *launches = 5;
   return 0;
 }
@@ -2429,12 +2449,13 @@ bool classify_polygon(double res, int Lp, int npts, const double* px, const doub
 // traversabilityFootprint(yaw): predicates once, then one tiled launch per polygon (unrotated -> out_x, rotated -> out_rot).
 int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int npts,
                              const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step,
-                             const float* rough, const float* elev, float* out_x, float* out_rot, int sms, cudaStream_t s, int* launches) {
+                             const float* rough, const float* elev, float* out_x, float* out_rot, int nmaps, int sms, cudaStream_t s,
+                             int* launches) {
   if (npts < 3 || npts > PMAXV) { st.why = "footprint polygon needs 3 to 16 vertices"; return TE_ERR_UNSUPPORTED; }
   const int Lp = polygon_reach(g, npts, pts_xy);
   if (Lp > 31) { st.why = "footprint polygon reaches further than 31 cells from its centre"; return TE_ERR_UNSUPPORTED; }
   FpArgs a{};
-  if (int rc = run_predicates(st, v, g, p, trav, slope, step, rough, elev, nullptr, nullptr, nullptr, sms, s, &a)) return rc;
+  if (int rc = run_predicates(st, v, g, p, nmaps, trav, slope, step, rough, elev, nullptr, nullptr, nullptr, sms, s, &a)) return rc;
   const size_t smem = sizeof(double) * (size_t)(PTC + 2 * Lp) * (PTR + 2 * Lp + 1) + (size_t)(PTC + 2 * Lp) * (PB * 2);
   if (!st.poly_attr) {
     const size_t smax = sizeof(double) * (size_t)(PTC + 62) * (PTR + 63) + (size_t)(PTC + 62) * (PB * 2);
@@ -2465,7 +2486,7 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
     q.runs = dr; q.fz = df; q.nruns = (int)tb.runs.size(); q.nfz = (int)tb.fz.size();
     q.ncert = 0;
     for (int rw : tb.runs) q.ncert += (int)(signed char)((rw >> 16) & 0xff) - (int)(signed char)((rw >> 8) & 0xff) + 1;
-    k_poly_tile<<<dim3((unsigned)((v.rows + PTR - 1) / PTR), (unsigned)((v.out_ncols + PTC - 1) / PTC)), 256, smem, s>>>(
+    k_poly_tile<<<dim3((unsigned)((v.rows + PTR - 1) / PTR), (unsigned)((v.out_ncols + PTC - 1) / PTC), (unsigned)nmaps), 256, smem, s>>>(
         a, q, trav, (const unsigned char*)st.block.p, which ? out_rot : out_x);
   }
   if (launches) *launches = 2 + nl;

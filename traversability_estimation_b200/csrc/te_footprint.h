@@ -39,7 +39,9 @@ struct FootprintState {
 
 int footprint_halo(const te_geometry* g, const te_footprint_params* p);
 
-int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
+// The sweeps run on `nmaps` (1 .. 65535) maps of the slab's shape stored back to back: map m's layers start m * rows * in_ncols
+// cells into every input, its outputs m * rows * out_ncols cells into every output.  The tables are built once per call.
+int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int nmaps, const float* trav,
                      const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
                      float* step_fp, float* rough_fp, int sms, cudaStream_t s, int* launches);
 
@@ -47,7 +49,8 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
 int footprint_polygon_halo(const te_geometry* g, const te_footprint_params* p, int npts, const double* pts_xy);
 int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int npts,
                              const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step,
-                             const float* rough, const float* elev, float* out_x, float* out_rot, int sms, cudaStream_t s, int* launches);
+                             const float* rough, const float* elev, float* out_x, float* out_rot, int nmaps, int sms, cudaStream_t s,
+                             int* launches);
 
 // TraversabilityMap::checkCircularFootprintPath for a batch of paths on a complete traversability_footprint layer (device pointers).
 void launch_check_paths(const SlabView& v, const te_geometry* g, double traversability_default, const float* footprint, const float* robot_slope, int npaths,
