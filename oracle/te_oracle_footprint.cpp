@@ -53,6 +53,25 @@ inline double cell_coord(double map_pos, double length, double res, int idx) {
   return (map_pos + offset) + res * (-(double)idx);
 }
 
+// OpenMP threads: nthreads > 0 as given, otherwise all.
+int thread_count(int nthreads) {
+#ifdef _OPENMP
+  return nthreads > 0 ? nthreads : omp_get_max_threads();
+#else
+  return (void)nthreads, 1;
+#endif
+}
+
+// The map and its cell-centre tables X (rows) and Y (columns), grid_map::getPosition.
+Map map_of(const teo_geometry* g, const float* trav, const float* slope, const float* step, const float* elev) {
+  Map m{g->rows, g->cols, g->resolution, {g->length_x, g->length_y}, {g->position_x, g->position_y}, trav, slope, step, elev, {}, {}};
+  m.X.resize(m.rows);
+  m.Y.resize(m.cols);
+  for (int i = 0; i < m.rows; ++i) m.X[i] = cell_coord(m.pos.x, m.len.x, m.res, i);
+  for (int j = 0; j < m.cols; ++j) m.Y[j] = cell_coord(m.pos.y, m.len.y, m.res, j);
+  return m;
+}
+
 // grid_map::checkIfPositionWithinMap (A.1): half-open box test in the flipped frame.
 inline bool is_inside(const Map& m, V2 p) {
   const double tx = -((p.x - m.pos.x) - 0.5 * m.len.x);
@@ -145,6 +164,77 @@ inline void for_line(int i0, int j0, int i1, int j1, F&& f) {
     if (num >= den) { num -= den; i += inc1x; j += inc1y; }
     i += inc2x; j += inc2y;
   }
+}
+
+// TraversabilityMap::checkInclination, TraversabilityMap.cpp:748-762, on the layer robotSlopeType_ names (robot.yaml:1); NULL is
+// checkRobotInclination_ off.  A single pose outside the map makes atPosition throw: reported unsafe here.  Invalid (NaN) cells
+// compare unequal to 0 and pass (:757).
+bool check_inclination(const Map& m, const float* robot_slope, V2 start, V2 end) {
+  if (!robot_slope) return true;
+  int si, sj, ei, ej;
+  if (!get_index(m, start, si, sj) || !get_index(m, end, ei, ej)) return false;       // poses must lie in the map
+  if (end.x == start.x && end.y == start.y) return !(robot_slope[(size_t)sj * m.rows + si] == 0.0f);  // :750-751
+  bool ok = true;
+  for_line(si, sj, ei, ej, [&](int a, int c) { return ok = !(robot_slope[(size_t)c * m.rows + a] == 0.0f); });  // :756-758
+  return ok;
+}
+
+using Polygon = std::vector<V2>;
+
+// TraversabilityMap::checkCircularFootprintPath, TraversabilityMap.cpp:345-462 (publishPolygons = true) for one path, pose k at
+// xy[stride * k].  isTraversable(center, t, polygon) is isTraversable(center, radius + offset, cup, t, polygon, radius) :654-746;
+// with `cup` set, `hull` is Polygon::convexHull and publish is publishUntraversablePolygon.  Returns is_safe, with
+// result.traversability in `result`.  Deviation noted: `lengthPath` (:443) is uninitialised there; the running length is used.
+template <class IsTraversable, class Publish>
+bool circular_footprint_path(const Map& m, const float* robot_slope, const double* xy, int stride, int arraySize, bool cup, double& result,
+                             Polygon (*hull)(const Polygon&, const Polygon&), IsTraversable&& isTraversable, Publish&& publish) {
+  if (arraySize <= 0) return false;                                                   // :330-334
+  double lengthPath = 0.0;
+  V2 start{0.0, 0.0}, end{0.0, 0.0};
+  Polygon untraversablePolygon;                                                       // :357
+  for (int i = 0; i < arraySize; i++) {                                               // :360
+    start = end;                                                                      // :361
+    end = V2{xy[(size_t)stride * i], xy[(size_t)stride * i + 1]};                     // :362-363
+    if (arraySize == 1) {                                                             // :365
+      if (!check_inclination(m, robot_slope, end, end)) return false;                 // :366-370 (returns before publishing)
+      const bool pathIsTraversable = isTraversable(end, result, untraversablePolygon);  // :371-372, :386
+      if (cup) publish(untraversablePolygon);                                         // :373-381
+      if (!pathIsTraversable) return false;                                           // :382-385
+    }
+    if (arraySize > 1 && i > 0) {                                                     // :389
+      if (!check_inclination(m, robot_slope, start, end)) return false;               // :390-394
+      int si, sj, ei, ej;
+      if (!get_index(m, start, si, sj) || !get_index(m, end, ei, ej)) return false;   // poses must lie in the map
+      double traversabilityTemp = 0.0, traversabilitySum = 0.0;                       // :395
+      int nLine = 0, visit = 0;
+      Polygon auxiliaryUntraversablePolygon;                                          // :402
+      bool pathIsTraversable = true;
+      for_line(ei, ej, si, sj, [&](int a, int c) {                                    // :404 LineIterator(endIndex, startIndex)
+        if ((visit++ & 3) != 0) return true;                                          // :421-425: nSkip = 3 cells skipped after a check
+        const V2 center{m.X[a], m.Y[c]};                                              // :406
+        pathIsTraversable = pathIsTraversable && isTraversable(center, traversabilityTemp, auxiliaryUntraversablePolygon);  // :407-408
+        if (cup && !auxiliaryUntraversablePolygon.empty())                            // :410-412
+          untraversablePolygon = hull(untraversablePolygon, auxiliaryUntraversablePolygon);
+        // :414-417 never returns early with publishPolygons; the && above skips every later isTraversable instead
+        traversabilitySum += traversabilityTemp;                                      // :419
+        nLine++;                                                                      // :420
+        return true;
+      });
+      if (cup) publish(untraversablePolygon);                                         // :429-439
+      if (!pathIsTraversable) return false;                                           // :453-456
+      const double t = traversabilitySum / (double)nLine;                             // :442
+      const double lengthSegment = std::sqrt((end.x - start.x) * (end.x - start.x) + (end.y - start.y) * (end.y - start.y));  // :444
+      if (i > 1) {                                                                    // :445-448
+        const double lengthPreviousPath = lengthPath;
+        lengthPath += lengthSegment;
+        result = (lengthSegment * t + lengthPreviousPath * result) / lengthPath;
+      } else {                                                                        // :449-452
+        lengthPath = lengthSegment;
+        result = t;
+      }
+    }
+  }
+  return true;                                                                        // :460
 }
 
 // TraversabilityMap::checkForStep, TraversabilityMap.cpp:794-865 (memoisation removed).
@@ -301,18 +391,8 @@ int teo_footprint2(const teo_geometry* g, const teo_footprint_params* p, const f
                    const float* rough, const float* elev, float* out, float* slope_fp, float* step_fp, float* rough_fp, int nthreads) {
   if (!g || g->rows <= 0 || g->cols <= 0 || !(g->resolution > 0.0) || !p || !trav || !slope || !step || !elev || !out) return 1;
   if (p->verify_roughness && !rough) return 1;
-  Map m{g->rows, g->cols, g->resolution, {g->length_x, g->length_y}, {g->position_x, g->position_y}, trav, slope, step, elev, {}, {}};
-  m.X.resize(m.rows);
-  m.Y.resize(m.cols);
-  for (int i = 0; i < m.rows; ++i) m.X[i] = cell_coord(m.pos.x, m.len.x, m.res, i);
-  for (int j = 0; j < m.cols; ++j) m.Y[j] = cell_coord(m.pos.y, m.len.y, m.res, j);
-  int nt = 1;
-#ifdef _OPENMP
-  nt = nthreads > 0 ? nthreads : omp_get_max_threads();
-#else
-  (void)nthreads;
-#endif
-  (void)nt;
+  const Map m = map_of(g, trav, slope, step, elev);
+  const int nt = thread_count(nthreads);
   std::vector<unsigned char> blocked;
   compute_blocked(m, *p, rough, blocked, slope_fp, step_fp, rough_fp, nt);
 
@@ -395,18 +475,8 @@ int teo_footprint_polygon(const teo_geometry* g, const teo_footprint_params* p, 
       !out_x || !out_rot)
     return 1;
   if (p->verify_roughness && !rough) return 1;
-  Map m{g->rows, g->cols, g->resolution, {g->length_x, g->length_y}, {g->position_x, g->position_y}, trav, slope, step, elev, {}, {}};
-  m.X.resize(m.rows);
-  m.Y.resize(m.cols);
-  for (int i = 0; i < m.rows; ++i) m.X[i] = cell_coord(m.pos.x, m.len.x, m.res, i);
-  for (int j = 0; j < m.cols; ++j) m.Y[j] = cell_coord(m.pos.y, m.len.y, m.res, j);
-  int nt = 1;
-#ifdef _OPENMP
-  nt = nthreads > 0 ? nthreads : omp_get_max_threads();
-#else
-  (void)nthreads;
-#endif
-  (void)nt;
+  const Map m = map_of(g, trav, slope, step, elev);
+  const int nt = thread_count(nthreads);
   std::vector<unsigned char> blocked;
   compute_blocked(m, *p, rough, blocked, nullptr, nullptr, nullptr, nt);
   // rotation matrices (Eigen::Quaternion::toRotationMatrix with x = y = 0)
@@ -468,105 +538,34 @@ int teo_footprint_polygon(const teo_geometry* g, const teo_footprint_params* p, 
   return 0;
 }
 
-// TraversabilityMap::checkCircularFootprintPath, TraversabilityMap.cpp:345-462, for a batch of paths, evaluated on a
-// traversability_footprint layer that is valid everywhere (i.e. after traversabilityFootprint(radius, offset), :307-318): every
-// isTraversable(center, ...) then takes the memoised branch :667-673 (traversability = layer value, traversable = value != 0);
-// centres outside the map take :660-666 (traversability = default).  checkRobotInclination_ (:359,:386) is off, no polygons.
-// Deviation noted: `lengthPath` (:441) is an uninitialised block-scope local in the reference; the intended running path
-// length is used here.
+// circular_footprint_path for a batch of paths on a traversability_footprint layer that is valid everywhere (after
+// traversabilityFootprint(radius, offset), :307-318): every isTraversable(center, ...) takes the memoised branch :673-678; centres
+// outside the map take :662-667 (traversability = default).  checkRobotInclination_ (:366, :390) is off, no polygons.
 int teo_check_circular_paths(const teo_geometry* g, const float* footprint, double traversability_default, int npaths,
                              const int32_t* path_begin, const double* poses_xy, uint8_t* is_safe, double* traversability) {
   return teo_check_circular_paths2(g, footprint, nullptr, traversability_default, npaths, path_begin, poses_xy, is_safe, traversability);
 }
 
-// The same with checkRobotInclination_ set (TraversabilityMap.cpp:359-363, :386-390): `robot_slope` is the layer robotSlopeType_
-// names (robot.yaml:1), NULL switches the check off.  checkInclination, TraversabilityMap.cpp:748-762: a single pose reads the
-// layer at the pose (a pose outside the map makes atPosition throw: reported unsafe here); two poses walk
-// LineIterator(startIndex, endIndex), skip invalid cells (:757) and fail on a cell that is exactly 0.0 (:758).
+// The same with checkRobotInclination_ set: `robot_slope` is check_inclination's layer, NULL switches the check off.
 int teo_check_circular_paths2(const teo_geometry* g, const float* footprint, const float* robot_slope, double traversability_default,
                               int npaths, const int32_t* path_begin, const double* poses_xy, uint8_t* is_safe, double* traversability) {
   if (!g || g->rows <= 0 || g->cols <= 0 || !footprint || npaths < 0 || !path_begin || !poses_xy || !is_safe || !traversability) return 1;
-  Map m{g->rows, g->cols, g->resolution, {g->length_x, g->length_y}, {g->position_x, g->position_y}, nullptr, nullptr, nullptr, nullptr, {}, {}};
-  m.X.resize(m.rows);
-  m.Y.resize(m.cols);
-  for (int i = 0; i < m.rows; ++i) m.X[i] = cell_coord(m.pos.x, m.len.x, m.res, i);
-  for (int j = 0; j < m.cols; ++j) m.Y[j] = cell_coord(m.pos.y, m.len.y, m.res, j);
-  auto circle = [&](V2 c, double& t) -> bool {  // isTraversable(center, ...) on the memoised layer
+  const Map m = map_of(g, nullptr, nullptr, nullptr, nullptr);
+  auto memoised = [&](V2 c, double& t, Polygon&) -> bool {                  // isTraversable(center, ...) on the memoised layer
     int i, j;
-    if (!is_inside(m, c) || !get_index(m, c, i, j)) {                       // :660-666
+    if (!is_inside(m, c) || !get_index(m, c, i, j)) {                       // :662-667
       t = traversability_default;
       return traversability_default != 0.0;
     }
-    t = (double)footprint[(size_t)j * m.rows + i];                          // :668
-    return t != 0.0;                                                         // :669
-  };
-  auto inclination_ok = [&](V2 start, V2 end) -> bool {                       // checkInclination, :748-762
-    if (!robot_slope) return true;                                           // checkRobotInclination_ off
-    if (end.x == start.x && end.y == start.y) {                              // :750
-      int i, j;
-      if (!is_inside(m, start) || !get_index(m, start, i, j)) return false;  // atPosition would throw
-      return !(robot_slope[(size_t)j * m.rows + i] == 0.0f);                 // :751
-    }
-    int si, sj, ei, ej;
-    if (!get_index(m, start, si, sj) || !get_index(m, end, ei, ej)) return false;  // poses must lie in the map
-    bool ok = true;
-    for_line(si, sj, ei, ej, [&](int a, int c2) {                            // :756 LineIterator(startIndex, endIndex)
-      const float v = robot_slope[(size_t)c2 * m.rows + a];
-      if (!std::isfinite(v)) return true;                                    // :757
-      if (v == 0.0f) { ok = false; return false; }                           // :758
-      return true;
-    });
-    return ok;
+    t = (double)footprint[(size_t)j * m.rows + i];                          // :674
+    return t != 0.0;                                                         // :675
   };
   for (int q = 0; q < npaths; ++q) {
-    const int b = path_begin[q], n = path_begin[q + 1] - b;
-    is_safe[q] = 0;                                                          // :352-353
-    traversability[q] = 0.0;
-    if (n <= 0) continue;                                                    // :330-334
-    double result = 0.0, lengthPath = 0.0;
-    bool ok = true;
-    V2 start{0.0, 0.0}, end{0.0, 0.0};
-    for (int k = 0; k < n && ok; ++k) {
-      start = end;                                                           // :361
-      end = V2{poses_xy[2 * (b + k)], poses_xy[2 * (b + k) + 1]};            // :362-363
-      if (n == 1) {                                                          // :365
-        if (!inclination_ok(end, end)) { ok = false; break; }                // :366-370
-        double t;
-        if (!circle(end, t)) { ok = false; break; }                          // :371-388
-        result = t;                                                          // :389
-      }
-      if (n > 1 && k > 0) {                                                  // :392
-        if (!inclination_ok(start, end)) { ok = false; break; }              // :393-397
-        int si, sj, ei, ej;
-        if (!get_index(m, start, si, sj) || !get_index(m, end, ei, ej)) { ok = false; break; }  // poses must lie in the map
-        double sum = 0.0;
-        int nLine = 0, visit = 0;
-        bool trav = true;
-        for_line(ei, ej, si, sj, [&](int a, int c2) {                        // :406 LineIterator(endIndex, startIndex)
-          if ((visit++ & 3) != 0) return true;                               // :424-428: three cells skipped after every check
-          double t;
-          trav = trav && circle(V2{m.X[a], m.Y[c2]}, t);                     // :407-410
-          if (!trav) return false;                                           // :416-419
-          sum += t;                                                          // :421
-          ++nLine;                                                           // :422
-          return true;
-        });
-        if (!trav) { ok = false; break; }                                    // :450-453
-        const double t = sum / (double)nLine;                                // :438
-        const double lengthSegment = std::sqrt((end.x - start.x) * (end.x - start.x) + (end.y - start.y) * (end.y - start.y));  // :440
-        if (k > 1) {                                                         // :441-445
-          const double lengthPreviousPath = lengthPath;
-          lengthPath += lengthSegment;
-          result = (lengthSegment * t + lengthPreviousPath * result) / lengthPath;
-        } else {
-          lengthPath = lengthSegment;                                        // :446-448
-          result = t;
-        }
-      }
-    }
-    if (!ok) continue;
-    is_safe[q] = 1;                                                          // :458
-    traversability[q] = result;
+    double result = 0.0;
+    const bool ok = circular_footprint_path(m, robot_slope, poses_xy + 2 * (size_t)path_begin[q], 2, path_begin[q + 1] - path_begin[q],
+                                            false, result, nullptr, memoised, [](const Polygon&) {});
+    is_safe[q] = ok;                                                         // :352-353, :460
+    traversability[q] = ok ? result : 0.0;
   }
   return 0;
 }

@@ -4,10 +4,10 @@ footprint.  Every path must get, bit for bit, what te_check_footprint_paths_fres
 import numpy as np
 import pytest
 
+import paths_oracle as po
 import synth
-import untraversable_oracle as uo
-from test_paths_fresh_gpu import _layers
-from test_polygon_paths_gpu import YAML, _footprint, _quat
+from helpers import (YAML, chain_layers, footprint_arrays, footprint_params, mixed_request, request_footprints, same,
+                     same_polygons)
 
 pytestmark = pytest.mark.gpu
 
@@ -20,81 +20,6 @@ CASES = [
 ]
 
 
-def _fps(te, oracle, verify):
-    ft, fo = te.FootprintParams.yaml_defaults(), oracle.FootprintParams.yaml_defaults()
-    ft.verify_roughness = fo.verify_roughness = verify
-    return ft, fo
-
-
-def _same(a, b):
-    return bool(np.all((a.view(np.uint64) == b.view(np.uint64)) | (np.isnan(a) & np.isnan(b))))
-
-
-def _same_polygons(cnt, xy, ref_cnt, ref_xy, what):
-    assert np.array_equal(cnt, ref_cnt), (what, np.nonzero(cnt != ref_cnt)[0][:10])
-    for q in np.nonzero(cnt > 0)[0]:
-        k = min(int(cnt[q]), xy.shape[1])
-        assert np.array_equal(xy[q, :k].view(np.uint64), ref_xy[q, :k].view(np.uint64)), (what, q)
-
-
-def _footprints(rng):
-    """The four footprints of a request: 1, 3, 4 (the YAML rectangle) and 16 vertices."""
-    return [_footprint(rng, 1), _footprint(rng, 3), np.asarray(YAML, np.float32), _footprint(rng, 16)]
-
-
-def _request(rng, og, npaths, fps, circular=0.4, planner=False, cap_path=True):
-    """A mixed request: per path its poses (7 wide), radius, footprint index (-1: circular), conservative and cup.  Circular
-    paths carry z / orientations the check must ignore (NaN in some); polygonal paths carry a NaN radius, which it ignores too."""
-    lx, ly = og.rows * og.resolution, og.cols * og.resolution
-    cx, cy = og.position_x, og.position_y
-    begin, poses, radius, kind = [0], [], [], []
-    for q in range(npaths):
-        k = -1 if rng.random() < circular else int(rng.integers(0, len(fps)))
-        if planner:
-            n = int(rng.integers(2, 9))
-        else:
-            n = int(rng.integers(0, 9)) if q > 5 else (0, 1, 2, 1, 5, 8)[q]
-        p = [rng.uniform([cx - 0.45 * lx, cy - 0.45 * ly], [cx + 0.45 * lx, cy + 0.45 * ly])]
-        for _ in range(n - 1):   # 0.1 - 0.5 m steps; a few paths turn back on themselves
-            a, d = rng.uniform(0, 2 * np.pi), rng.uniform(0.1, 0.5)
-            p.append(p[-1] + d * np.array([np.cos(a), np.sin(a)]) if rng.random() > 0.1 or len(p) < 2 else p[-2].copy())
-        p = np.asarray(p[:n]).reshape(-1, 2)
-        if not planner and q % 40 == 9 and n > 0:
-            p[0] = [cx + 0.6 * lx, cy]                        # a pose outside the map
-        qkind = 0 if planner else int(rng.integers(0, 3))
-        for x, y in p:
-            rest = [rng.uniform(-1, 1), *_quat(rng, qkind)]
-            if k < 0 and rng.random() < 0.2:
-                rest[-1] = np.nan
-            poses.append([x, y, *rest])
-        begin.append(len(poses))
-        radius.append(float(rng.uniform(0.1, 0.5)) if k < 0 else np.nan)
-        kind.append(k)
-    if cap_path:   # a conservative YAML path of 256 poses: polygon2 reaches the 1024-vertex cap
-        walk = np.cumsum(rng.uniform(-0.01, 0.01, (256, 2)), axis=0) + [cx + 0.1 * lx, cy - 0.1 * ly]
-        poses.extend(np.concatenate([walk, np.tile([0.0, 0.0, 0.0, 0.0, 1.0], (256, 1))], axis=1).tolist())
-        begin.append(len(poses))
-        radius.append(np.nan)
-        kind.append(2)
-    m = len(kind)
-    cons = (rng.random(m) < 0.3).astype(np.uint8)
-    cup = (rng.random(m) < 0.5).astype(np.uint8)
-    if cap_path:
-        cons[-1] = cup[-1] = 1
-    return dict(begin=np.asarray(begin, np.int32), poses=np.asarray(poses, np.float64).reshape(-1, 7),
-                radius=np.asarray(radius, np.float64), kind=np.asarray(kind), cons=cons, cup=cup)
-
-
-def _footprint_arrays(R, fps):
-    """footprint_begin / footprint_xyz of a request: path q's own copy of its footprint, none for circular paths."""
-    fb, fx = [0], []
-    for k in R["kind"]:
-        if k >= 0:
-            fx.extend(fps[k].tolist())
-        fb.append(len(fx))
-    return np.asarray(fb, np.int32), np.asarray(fx, np.float32).reshape(-1, 3)
-
-
 def _subset(R, idx):
     """path_begin and poses of the paths `idx` of a request, in that order."""
     b = R["begin"]
@@ -104,7 +29,7 @@ def _subset(R, idx):
 
 
 def _run(ctx, g, ft, L, R, fps, rs, cap, memory=0, **kw):
-    fb, fx = _footprint_arrays(R, fps)
+    fb, fx = footprint_arrays(R, fps)
     args = (g, ft, L["traversability"], L["slope"], L["step"], L["elevation"], R["begin"], R["poses"], R["radius"], fb, fx)
     return ctx.check_footprint_request(*args, robot_slope=rs, roughness=L["roughness"] if ft.verify_roughness else None,
                                        conservative=R["cons"], compute_untraversable_polygon=R["cup"], untraversable_capacity=cap,
@@ -143,16 +68,16 @@ def _split(ctx, g, ft, L, R, fps, rs, cap):
 
 def _assert_equal(got, want, what):
     assert np.array_equal(got[0], want[0]), (what, np.nonzero(got[0] != want[0])[0][:10])
-    assert _same(got[1], want[1]) and _same(got[2], want[2]), what
+    assert same(got[1], want[1]) and same(got[2], want[2]), what
     if len(want) > 3:
-        _same_polygons(got[3], got[4], want[3], want[4], what)
+        same_polygons(got[3], got[4], want[3], want[4], what)
 
 
 def _to_device(R, fps, L, rs):
     import torch
     dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
     lay = lambda a: None if a is None else torch.from_numpy(np.ascontiguousarray(a.T)).cuda()  # noqa: E731
-    fb, fx = _footprint_arrays(R, fps)
+    fb, fx = footprint_arrays(R, fps)
     D = {k: dev(R[k]) for k in ("begin", "poses", "radius", "cons", "cup")}
     D["fb"], D["fx"] = dev(fb), dev(fx)
     return D, {k: lay(v) for k, v in L.items()}, lay(rs)
@@ -191,10 +116,10 @@ def _mixed(te, oracle, case):
     res, pos = case["res"], case.get("position", (0.0, 0.0))
     z = synth.terrain(case["rows"], case["cols"], res, case["seed"], "mixed", pos)
     og, g = oracle.Geometry.make(case["rows"], case["cols"], res, pos), te.Geometry.make(case["rows"], case["cols"], res, pos)
-    L, rs = _layers(oracle, og, z, case["seed"])
+    L, rs = chain_layers(oracle, og, z, case["seed"])
     rng = np.random.default_rng(case["seed"])
-    fps = _footprints(rng)
-    R = _request(rng, og, 200, fps, planner=case["rows"] >= 2048)
+    fps = request_footprints(rng)
+    R = mixed_request(rng, og, 200, fps, planner=case["rows"] >= 2048)
     return dict(og=og, g=g, L=L, rs=rs, fps=fps, R=R)
 
 
@@ -204,7 +129,7 @@ def test_mixed_requests_equal_the_split_calls(te, ctx, oracle, mixed_case):
     assert (kinds < 0).sum() > 40 and all((kinds == k).sum() > 10 for k in range(4))
     D, Ld, rsd = _to_device(R, fps, L, rs)
     for verify in (0, 1):
-        ft, _ = _fps(te, oracle, verify)
+        ft, _ = footprint_params(te, oracle, verify)
         for slope_layer, slope_dev in ((None, None), (rs, rsd)):
             for cap in (None, CAP):
                 what = (verify, slope_layer is None, cap)
@@ -219,28 +144,10 @@ def test_mixed_requests_equal_the_split_calls(te, ctx, oracle, mixed_case):
 
 
 def _oracle(og, fo, L, R, fps, rs):
-    """The CPU oracles' answer to a request, path by path in request order: check_circular_paths_fresh2 for its circular paths
-    (area 0), check_polygonal_paths2 once per footprint for its polygonal paths."""
-    m = len(R["kind"])
-    out = (np.zeros(m, np.uint8), np.zeros(m), np.zeros(m), np.zeros(m, np.int32), np.zeros((m, CAP, 2)))
-    rough = L["roughness"] if fo.verify_roughness else None
-    for k in range(-1, len(fps)):
-        idx = np.nonzero(R["kind"] == k)[0]
-        if not len(idx):
-            continue
-        b, p = _subset(R, idx)
-        if k < 0:
-            w = uo.check_circular_paths_fresh2(og, fo, L["traversability"], L["slope"], L["step"], L["elevation"], b, p[:, :2].copy(),
-                                               R["radius"][idx], robot_slope=rs, roughness=rough,
-                                               compute_untraversable_polygon=R["cup"][idx], capacity=CAP)
-            w = (w[0], w[1], np.zeros(len(idx)), w[2], w[3])
-        else:
-            w = uo.check_polygonal_paths2(og, fo, L["traversability"], L["slope"], L["step"], L["elevation"], fps[k], b, p,
-                                          robot_slope=rs, roughness=rough, conservative=R["cons"][idx],
-                                          compute_untraversable_polygon=R["cup"][idx], capacity=CAP)
-        for a, v in zip(out, w):
-            a[idx] = v
-    return out
+    """The CPU oracle's answer to a request, in one call on a fresh map."""
+    fb, fx = footprint_arrays(R, fps)
+    return po.check_request(og, fo, dict(L, robot_slope=rs), R["begin"], R["poses"], R["radius"], footprint_begin=fb,
+                            footprint_xyz=fx, conservative=R["cons"], cup=R["cup"], capacity=CAP)
 
 
 def test_request_matches_the_cpu_oracles(te, ctx, oracle):
@@ -251,7 +158,7 @@ def test_request_matches_the_cpu_oracles(te, ctx, oracle):
         og, g, L, fps, R = (M[k] for k in ("og", "g", "L", "fps", "R"))
         assert R["cons"][-1] and R["cup"][-1] and R["begin"][-1] - R["begin"][-2] == 256
         for verify in (0, 1):
-            ft, fo = _fps(te, oracle, verify)
+            ft, fo = footprint_params(te, oracle, verify)
             for rs in (None, M["rs"]):
                 want = _oracle(og, fo, L, R, fps, rs)
                 for cap in (None, CAP):
@@ -264,15 +171,15 @@ def test_degenerate_requests(te, ctx, oracle):
     rows, cols = 160, 150
     z = synth.terrain(rows, cols, 0.02, 52, "mixed")
     og, g = oracle.Geometry.make(rows, cols, 0.02), te.Geometry.make(rows, cols, 0.02)
-    L, rs = _layers(oracle, og, z, 52)
+    L, rs = chain_layers(oracle, og, z, 52)
     rng = np.random.default_rng(52)
-    fps = _footprints(rng)
-    ft, _ = _fps(te, oracle, 1)
+    fps = request_footprints(rng)
+    ft, _ = footprint_params(te, oracle, 1)
     for circular in (1.0, 0.0):   # all circular; all polygonal over one footprint
-        R = _request(rng, og, 150, fps[2:3], circular=circular, cap_path=False)
+        R = mixed_request(rng, og, 150, fps[2:3], circular=circular, cap_path=False)
         for cap in (None, CAP):
             _assert_equal(_run(ctx, g, ft, L, R, fps[2:3], rs, cap), _split(ctx, g, ft, L, R, fps[2:3], rs, cap), (circular, cap))
-    empty = _request(rng, og, 0, fps, cap_path=False)
+    empty = mixed_request(rng, og, 0, fps, cap_path=False)
     got = _run(ctx, g, ft, L, empty, fps, None, CAP)
     assert all(len(a) == 0 for a in got)
 
@@ -282,12 +189,12 @@ def test_device_mode_on_a_torch_stream(te, oracle):
     rows, cols = 160, 150
     z = synth.terrain(rows, cols, 0.02, 53, "mixed")
     og, g = oracle.Geometry.make(rows, cols, 0.02), te.Geometry.make(rows, cols, 0.02)
-    L, rs = _layers(oracle, og, z, 53)
+    L, rs = chain_layers(oracle, og, z, 53)
     rng = np.random.default_rng(53)
-    fps = _footprints(rng)
-    R = _request(rng, og, 200, fps, cap_path=False)
+    fps = request_footprints(rng)
+    R = mixed_request(rng, og, 200, fps, cap_path=False)
     R["cup"][:] = 1
-    ft, _ = _fps(te, oracle, 1)
+    ft, _ = footprint_params(te, oracle, 1)
     ctx = te.Context(0)
     try:
         want = _run(ctx, g, ft, L, R, fps, rs, CAP)
@@ -315,11 +222,11 @@ def test_host_mode_with_start_index(te, ctx, oracle):
     rows, cols = 150, 140
     z = synth.terrain(rows, cols, 0.02, 54, "mixed")
     og, g = oracle.Geometry.make(rows, cols, 0.02), te.Geometry.make(rows, cols, 0.02)
-    L, rs = _layers(oracle, og, z, 54)
+    L, rs = chain_layers(oracle, og, z, 54)
     rng = np.random.default_rng(54)
-    fps = _footprints(rng)
-    R = _request(rng, og, 200, fps, cap_path=False)
-    ft, _ = _fps(te, oracle, 1)
+    fps = request_footprints(rng)
+    R = mixed_request(rng, og, 200, fps, cap_path=False)
+    ft, _ = footprint_params(te, oracle, 1)
     want = _run(ctx, g, ft, L, R, fps, rs, CAP)
     sr, sc = 37, 101
     wrap = lambda a: np.asfortranarray(np.roll(np.roll(a, sr, axis=0), sc, axis=1))  # noqa: E731
@@ -328,7 +235,7 @@ def test_host_mode_with_start_index(te, ctx, oracle):
     got = _run(ctx, gw, ft, {k: wrap(v) for k, v in L.items()}, R, fps, wrap(rs), CAP)
     for a, b in zip(got[:3], want[:3]):
         assert np.array_equal(a.view(np.uint8), b.view(np.uint8))
-    _same_polygons(got[3], got[4], want[3], want[4], "start index")
+    same_polygons(got[3], got[4], want[3], want[4], "start index")
     assert (want[3] > 3).any()
 
 
@@ -336,11 +243,11 @@ def test_launch_count_does_not_depend_on_the_footprints(te, ctx, oracle):
     rows, cols = 120, 120
     z = synth.terrain(rows, cols, 0.02, 55, "mixed")
     og, g = oracle.Geometry.make(rows, cols, 0.02), te.Geometry.make(rows, cols, 0.02)
-    L, rs = _layers(oracle, og, z, 55)
+    L, rs = chain_layers(oracle, og, z, 55)
     rng = np.random.default_rng(55)
-    fps = _footprints(rng)
-    R = _request(rng, og, 100, fps, cap_path=False)
-    ft, _ = _fps(te, oracle, 0)
+    fps = request_footprints(rng)
+    R = mixed_request(rng, og, 100, fps, cap_path=False)
+    ft, _ = footprint_params(te, oracle, 0)
     counts = []
     for footprints in (fps[2:3] * 4, fps):   # the same request over 1 and over 4 distinct footprints
         for cap in (None, CAP):
@@ -354,7 +261,7 @@ def test_error_codes(te, ctx, oracle):
     rows, cols = 64, 64
     g = te.Geometry.make(rows, cols, 0.02)
     one = np.ones((rows, cols), np.float32, order="F")
-    ft, _ = _fps(te, oracle, 0)
+    ft, _ = footprint_params(te, oracle, 0)
     lib = te.load_library()
     fn = lib.te_check_footprint_request
     pose = [0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 1.0]

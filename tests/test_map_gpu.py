@@ -1,12 +1,11 @@
-"""te_map on the GPU against the sequential CPU oracle (tests/map_oracle.cpp), bit for bit: is_safe, traversability, area,
-untraversable polygons and the traversability_footprint cache after every call."""
+"""te_map on the GPU against the CPU oracle on a persistent cache (tests/paths_oracle.cpp), bit for bit: is_safe, traversability,
+area, untraversable polygons and the traversability_footprint cache after every call."""
 import numpy as np
 import pytest
 
-import map_oracle as mo
+import paths_oracle as po
 import synth
-from test_footprint_request_gpu import _footprint_arrays, _footprints, _request, _same, _same_polygons
-from test_paths_fresh_gpu import _layers
+from helpers import chain_layers, footprint_arrays, mixed_request, request_footprints, same, same_polygons
 
 pytestmark = pytest.mark.gpu
 
@@ -16,7 +15,7 @@ CAP = 64
 def _setup(te, oracle, rows=200, cols=180, res=0.02, seed=61, position=(0.0, 0.0)):
     z = synth.terrain(rows, cols, res, seed, "mixed", position)
     og, g = oracle.Geometry.make(rows, cols, res, position), te.Geometry.make(rows, cols, res, position)
-    L, rs = _layers(oracle, og, z, seed)
+    L, rs = chain_layers(oracle, og, z, seed)
     return og, g, L, rs
 
 
@@ -30,20 +29,20 @@ def _params(te, oracle, verify=0, **kw):
 
 
 def _same_cache(a, b, what):
-    assert np.array_equal(a.view(np.uint32), b.view(np.uint32)) or _same(a.astype(np.float64), b.astype(np.float64)), \
+    assert np.array_equal(a.view(np.uint32), b.view(np.uint32)) or same(a.astype(np.float64), b.astype(np.float64)), \
         (what, int(np.sum(~((a == b) | (np.isnan(a) & np.isnan(b))))))
 
 
 def _both(m, og, ft, fo, OL, cache, R, fps):
     """One request on the map and on the oracle; asserts every output and the cache are identical."""
-    fb, fx = _footprint_arrays(R, fps)
+    fb, fx = footprint_arrays(R, fps)
     got = m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, max_footprint_vertices=16,
                                     conservative=R["cons"], compute_untraversable_polygon=R["cup"], untraversable_capacity=CAP)
-    want = mo.check_request(og, fo, OL, cache, R["begin"], R["poses"], R["radius"], fb, fx, conservative=R["cons"],
-                            compute_untraversable_polygon=R["cup"], capacity=CAP)
+    want = po.check_request(og, fo, OL, R["begin"], R["poses"], R["radius"], fb, fx, conservative=R["cons"], cup=R["cup"],
+                            cache=cache, capacity=CAP)
     assert np.array_equal(got[0], want[0]), np.nonzero(got[0] != want[0])[0][:10]
-    assert _same(got[1], want[1]) and _same(got[2], want[2])
-    _same_polygons(got[3], got[4], want[3], want[4], "polygons")
+    assert same(got[1], want[1]) and same(got[2], want[2])
+    same_polygons(got[3], got[4], want[3], want[4], "polygons")
     _same_cache(m.get_footprint(), cache, "cache")
     return got
 
@@ -64,11 +63,11 @@ def test_request_sequence_matches_oracle(te, ctx, oracle, verify, slope):
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"], roughness=L["roughness"],
                  robot_slope=rs if slope else None)
     OL = dict(L, robot_slope=rs if slope else None)
-    cache = mo.empty_cache(og)
+    cache = po.empty_cache(og)
     rng = np.random.default_rng(7 + verify)
-    fps = _footprints(rng)
-    R1 = _request(rng, og, 60, fps, circular=0.6, cap_path=False)
-    R2 = _request(rng, og, 80, fps, circular=0.7, planner=True, cap_path=False)
+    fps = request_footprints(rng)
+    R1 = mixed_request(rng, og, 60, fps, circular=0.6, cap_path=False)
+    R2 = mixed_request(rng, og, 80, fps, circular=0.7, planner=True, cap_path=False)
     for R in (R1, _repeat(R1, rng.permutation(len(R1["kind"]))), R2, _repeat(R2, np.arange(len(R2["kind"])) // 2)):
         _both(m, og, ft, fo, OL, cache, R, fps)
     cand, keys, stored = m.request_stats()
@@ -81,7 +80,7 @@ def test_annulus_blocker_revisit_and_single_poses_in_one_cell(te, ctx, oracle):
     ft, fo = _params(te, oracle)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"])
-    cache = mo.empty_cache(og)
+    cache = po.empty_cache(og)
     rng = np.random.default_rng(9)
     n = 300
     xy = rng.uniform([-1.8, -1.6], [1.8, 1.6], (n, 2))
@@ -108,7 +107,7 @@ def test_zero_mean_circle_then_fails(te, ctx, oracle):
     ft, fo = _params(te, oracle)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"])
-    cache = mo.empty_cache(og)
+    cache = po.empty_cache(og)
     poses = np.array([[0.1, 0.2, 0, 0, 0, 0, 1.0]])
     R = dict(begin=np.array([0, 1], np.int32), poses=poses, radius=np.array([0.2]), kind=np.array([-1]), cons=np.zeros(1, np.uint8),
              cup=np.ones(1, np.uint8))
@@ -123,10 +122,10 @@ def test_sweep_and_request_share_the_cache(te, ctx, oracle):
     ft, fo = _params(te, oracle)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"])
-    cache = mo.empty_cache(og)
+    cache = po.empty_cache(og)
     rng = np.random.default_rng(11)
-    fps = _footprints(rng)
-    _both(m, og, ft, fo, L, cache, _request(rng, og, 40, fps, circular=0.8, cap_path=False), fps)
+    fps = request_footprints(rng)
+    _both(m, og, ft, fo, L, cache, mixed_request(rng, og, 40, fps, circular=0.8, cap_path=False), fps)
     before = m.get_footprint()
     after = m.footprint(ft)
     sweep = np.empty_like(after)
@@ -137,7 +136,7 @@ def test_sweep_and_request_share_the_cache(te, ctx, oracle):
     assert np.array_equal(m.get_footprint().view(np.uint32), after.view(np.uint32))
     # a request after the sweep reads the swept cache: start the oracle from it
     cache = np.asfortranarray(after.copy())
-    _both(m, og, ft, fo, L, cache, _request(rng, og, 40, fps, circular=0.8, cap_path=False), fps)
+    _both(m, og, ft, fo, L, cache, mixed_request(rng, og, 40, fps, circular=0.8, cap_path=False), fps)
     m.close()
 
 
@@ -147,17 +146,17 @@ def test_new_layers_clear_cache_and_memo(te, ctx, oracle):
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"])
     rng = np.random.default_rng(13)
-    R = _request(rng, og, 40, [], circular=1.0, cap_path=False)
-    cache = mo.empty_cache(og)
+    R = mixed_request(rng, og, 40, [], circular=1.0, cap_path=False)
+    cache = po.empty_cache(og)
     _both(m, og, ft, fo, L, cache, R, [])
     # a changed max_gap_width rebuilds the memo and keeps the cache
     ft2, fo2 = _params(te, oracle, max_gap_width=0.1)
-    _both(m, og, ft2, fo2, L, cache, _request(rng, og, 40, [], circular=1.0, cap_path=False), [])
+    _both(m, og, ft2, fo2, L, cache, mixed_request(rng, og, 40, [], circular=1.0, cap_path=False), [])
     # new layers: empty cache, fresh memo
     L2 = dict(L, traversability=np.asfortranarray(L["traversability"] * np.float32(0.5)))
     m.set_layers(g, L2["traversability"], L2["slope"], L2["step"], L2["elevation"])
     assert np.isnan(m.get_footprint()).all()
-    cache = mo.empty_cache(og)
+    cache = po.empty_cache(og)
     _both(m, og, ft, fo, L2, cache, R, [])
     # te_map_chain: the chain's layers, an empty cache
     ch = m.chain(g, te.ChainParams.yaml_defaults(0), L["elevation"], outputs=True)
@@ -166,7 +165,7 @@ def test_new_layers_clear_cache_and_memo(te, ctx, oracle):
         assert np.array_equal(ch[k].view(np.uint32), want[k].view(np.uint32)), k
     assert np.isnan(m.get_footprint()).all()
     L3 = dict(traversability=ch["traversability"], slope=ch["slope"], step=ch["step"], elevation=L["elevation"])
-    cache = mo.empty_cache(og)
+    cache = po.empty_cache(og)
     _both(m, og, ft, fo, L3, cache, R, [])
     m.clear_footprint()
     assert np.isnan(m.get_footprint()).all()
@@ -179,7 +178,7 @@ def test_fresh_map_disjoint_cells_equal_stateless_request(te, ctx, oracle):
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"], roughness=L["roughness"], robot_slope=rs)
     rng = np.random.default_rng(15)
-    fps = _footprints(rng)
+    fps = request_footprints(rng)
     n = 150
     cells = rng.choice(og.rows * og.cols, n, replace=False)
     res = og.resolution
@@ -190,14 +189,14 @@ def test_fresh_map_disjoint_cells_equal_stateless_request(te, ctx, oracle):
     kind = np.where(rng.random(n) < 0.6, -1, rng.integers(0, len(fps), n))
     R = dict(begin=np.arange(n + 1, dtype=np.int32), poses=poses, radius=rng.choice([0.0, 0.1, 0.3], n), kind=kind,
              cons=np.zeros(n, np.uint8), cup=(rng.random(n) < 0.5).astype(np.uint8))
-    fb, fx = _footprint_arrays(R, fps)
+    fb, fx = footprint_arrays(R, fps)
     got = m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, compute_untraversable_polygon=R["cup"],
                                     untraversable_capacity=CAP)
     want = ctx.check_footprint_request(g, ft, L["traversability"], L["slope"], L["step"], L["elevation"], R["begin"], R["poses"],
                                        R["radius"], fb, fx, robot_slope=rs, roughness=L["roughness"],
                                        compute_untraversable_polygon=R["cup"], untraversable_capacity=CAP)
-    assert np.array_equal(got[0], want[0]) and _same(got[1], want[1]) and _same(got[2], want[2])
-    _same_polygons(got[3], got[4], want[3], want[4], "polygons")
+    assert np.array_equal(got[0], want[0]) and same(got[1], want[1]) and same(got[2], want[2])
+    same_polygons(got[3], got[4], want[3], want[4], "polygons")
     # te_map_footprint_polygon is te_footprint_polygon on the map's layers
     pts = np.array([[0.2, 0.1], [-0.2, 0.1], [-0.2, -0.1], [0.2, -0.1]])
     gx, gr = m.footprint_polygon(ft, pts, 0.3)
@@ -219,8 +218,8 @@ def test_start_index_layers(te, ctx, oracle):
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"], robot_slope=rs)
     mw.set_layers(gw, *(wrap(L[k]) for k in ("traversability", "slope", "step", "elevation")), robot_slope=wrap(rs))
     rng = np.random.default_rng(17)
-    R = _request(rng, og, 50, [], circular=1.0, cap_path=False)
-    fb, fx = _footprint_arrays(R, [])
+    R = mixed_request(rng, og, 50, [], circular=1.0, cap_path=False)
+    fb, fx = footprint_arrays(R, [])
     a = m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, compute_untraversable_polygon=R["cup"],
                                   untraversable_capacity=CAP)
     b = mw.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, compute_untraversable_polygon=R["cup"],

@@ -3,7 +3,7 @@ TraversabilityMap.cpp:345-462 with :679-736) in the CPU oracle, against answers 
 0.8 everywhere, cells blocked by patches of zero roughness traversability (verify_roughness, checkForRoughness :895-921)."""
 import numpy as np
 
-import paths_fresh_oracle as pfo
+import paths_oracle as po
 
 RES = 0.02
 
@@ -36,10 +36,7 @@ def _map(oracle, rows, cols, patches):
 def _fresh(g, fp, L, poses, radius=0.3, cup=None, begin=None):
     poses = np.asarray(poses, dtype=np.float64).reshape(-1, 2)
     begin = [0, len(poses)] if begin is None else begin
-    n = len(begin) - 1
-    return pfo.check_circular_paths_fresh(g, fp, L["traversability"], L["slope"], L["step"], L["elevation"], begin, poses,
-                                          [radius] * n, roughness=L["roughness"],
-                                          compute_untraversable_polygon=None if cup is None else [cup] * n)
+    return po.check_request(g, fp, L, begin, poses, radius, cup=cup)[:2]
 
 
 def _sweep_then_memo(oracle, g, fp, L, poses):

@@ -2,53 +2,11 @@
 import numpy as np
 import pytest
 
-import paths_fresh_oracle as pfo
+import paths_oracle as po
 import synth
+from helpers import chain_layers, circular_paths, footprint_params
 
 pytestmark = pytest.mark.gpu
-
-
-def _layers(oracle, og, z, seed):
-    ch = oracle.chain(og, oracle.ChainParams.yaml_defaults(0), z)
-    rng = np.random.default_rng(seed)
-    rough = ch["roughness"].copy()   # zero patches, so that checkForRoughness blocks cells the slope / step checks let through
-    for _ in range(40):
-        a, b = int(rng.integers(0, og.rows - 12)), int(rng.integers(0, og.cols - 12))
-        rough[a:a + int(rng.integers(1, 12)), b:b + int(rng.integers(1, 12))] = 0.0
-    rs = ch["slope"].copy()
-    rs[rng.random(rs.shape) < 0.0005] = 0.0
-    rs[rng.random(rs.shape) < 0.05] = np.nan
-    f = lambda a: np.asfortranarray(a, dtype=np.float32)  # noqa: E731
-    return dict(traversability=f(ch["traversability"]), slope=f(ch["slope"]), step=f(ch["step"]), elevation=f(z),
-                roughness=f(rough)), f(rs)
-
-
-def _paths(rng, og, npaths, radii=(0.0, 0.2, 0.3, 0.45), planner=False):
-    lx, ly = og.rows * og.resolution, og.cols * og.resolution
-    cx, cy = og.position_x, og.position_y
-    begin, poses, radius = [0], [], []
-    for q in range(npaths):
-        if planner:
-            n = int(rng.integers(2, 9))
-        else:
-            n = int(rng.integers(0, 7)) if q > 3 else (0, 1, 2, 5)[q]
-        p = [rng.uniform([cx - 0.45 * lx, cy - 0.45 * ly], [cx + 0.45 * lx, cy + 0.45 * ly])]
-        for _ in range(n - 1):   # 0.1 - 0.5 m steps, like a planner's poses; a few paths turn back on themselves
-            ang, d = rng.uniform(0, 2 * np.pi), rng.uniform(0.1, 0.5)
-            p.append(p[-1] + d * np.array([np.cos(ang), np.sin(ang)]) if rng.random() > 0.1 or len(p) < 2 else p[-2].copy())
-        p = np.asarray(p[:n]).reshape(-1, 2)
-        if not planner and q % 50 == 7 and n > 0:
-            p[0] = [cx + 0.6 * lx, cy]                            # a pose outside the map
-        poses.extend(p.tolist())
-        begin.append(len(poses))
-        radius.append(0.3 if planner else float(radii[int(rng.integers(0, len(radii)))]))
-    return np.asarray(begin, np.int32), np.asarray(poses, np.float64).reshape(-1, 2), np.asarray(radius, np.float64)
-
-
-def _fps(te, oracle, verify):
-    ft, fo = te.FootprintParams.yaml_defaults(), oracle.FootprintParams.yaml_defaults()
-    ft.verify_roughness = fo.verify_roughness = verify
-    return ft, fo
 
 
 def _gpu(ctx, g, ft, L, begin, poses, radius, rs, cup, **kw):
@@ -58,9 +16,7 @@ def _gpu(ctx, g, ft, L, begin, poses, radius, rs, cup, **kw):
 
 
 def _cpu(og, fo, L, begin, poses, radius, rs, cup):
-    return pfo.check_circular_paths_fresh(og, fo, L["traversability"], L["slope"], L["step"], L["elevation"], begin, poses, radius,
-                                          robot_slope=rs, roughness=L["roughness"] if fo.verify_roughness else None,
-                                          compute_untraversable_polygon=cup)
+    return po.check_request(og, fo, dict(L, robot_slope=rs), begin, poses, radius, cup=cup)[:2]
 
 
 @pytest.mark.parametrize("case", [
@@ -72,12 +28,12 @@ def test_fresh_paths_match_oracle(te, ctx, oracle, case):
     res, pos = case["res"], case.get("position", (0.0, 0.0))
     z = synth.terrain(case["rows"], case["cols"], res, case["seed"], "mixed", pos)
     og, g = oracle.Geometry.make(case["rows"], case["cols"], res, pos), te.Geometry.make(case["rows"], case["cols"], res, pos)
-    L, rs = _layers(oracle, og, z, case["seed"])
+    L, rs = chain_layers(oracle, og, z, case["seed"])
     rng = np.random.default_rng(case["seed"])
-    begin, poses, radius = _paths(rng, og, 400)
+    begin, poses, radius = circular_paths(rng, og, 400)
     cup = (rng.random(len(radius)) < 0.3).astype(np.uint8)
     for verify in (0, 1):
-        ft, fo = _fps(te, oracle, verify)
+        ft, fo = footprint_params(te, oracle, verify)
         for slope_layer in (None, rs):
             ref_safe, ref_t = _cpu(og, fo, L, begin, poses, radius, slope_layer, cup)
             safe, t = _gpu(ctx, g, ft, L, begin, poses, radius, slope_layer, cup)
@@ -85,7 +41,7 @@ def test_fresh_paths_match_oracle(te, ctx, oracle, case):
             assert np.array_equal(t.view(np.uint64), ref_t.view(np.uint64)), (verify, np.nonzero(t != ref_t)[0][:10])
             assert 10 < int(safe.sum()) < 390 and safe[0] == 0
     # the route of INTEGRATION.md (sweep at 0.3 m, then the memoised check) answers a different question for some paths
-    ft, fo = _fps(te, oracle, 1)
+    ft, fo = footprint_params(te, oracle, 1)
     sel = np.nonzero(radius == 0.3)[0]
     sb = np.concatenate([[0], np.cumsum(np.diff(begin)[sel])]).astype(np.int32)
     sp = np.concatenate([poses[begin[q]:begin[q + 1]] for q in sel]).reshape(-1, 2)
@@ -100,9 +56,9 @@ def test_fresh_planner_paths_2048(te, ctx, oracle):
     n = 2048
     z = synth.terrain(n, n, 0.02, 2048, "mixed")
     og, g = oracle.Geometry.make(n, n, 0.02), te.Geometry.make(n, n, 0.02)
-    L, _ = _layers(oracle, og, z, 2048)
-    begin, poses, radius = _paths(np.random.default_rng(2048), og, 2000, planner=True)
-    ft, fo = _fps(te, oracle, 0)
+    L, _ = chain_layers(oracle, og, z, 2048)
+    begin, poses, radius = circular_paths(np.random.default_rng(2048), og, 2000, planner=True)
+    ft, fo = footprint_params(te, oracle, 0)
     ref_safe, ref_t = _cpu(og, fo, L, begin, poses, radius, None, None)
     safe, t = _gpu(ctx, g, ft, L, begin, poses, radius, None, None)
     assert np.array_equal(safe, ref_safe) and np.array_equal(t.view(np.uint64), ref_t.view(np.uint64))
@@ -114,13 +70,13 @@ def test_fresh_device_mode_on_a_torch_stream(te, oracle):
     rows, cols = 160, 150
     z = synth.terrain(rows, cols, 0.02, 71, "mixed")
     og, g = oracle.Geometry.make(rows, cols, 0.02), te.Geometry.make(rows, cols, 0.02)
-    L, rs = _layers(oracle, og, z, 71)
+    L, rs = chain_layers(oracle, og, z, 71)
     rng = np.random.default_rng(71)
-    begin, poses, radius = _paths(rng, og, 300)
+    begin, poses, radius = circular_paths(rng, og, 300)
     radius[5] = 3.0                                          # 0.3 + 3.0 m at 0.02 m: 158 rings, more than the ring table holds
     radius[6] = -1.0
     cup = (rng.random(len(radius)) < 0.3).astype(np.uint8)
-    ft, _ = _fps(te, oracle, 1)
+    ft, _ = footprint_params(te, oracle, 1)
     ctx = te.Context(0)
     try:
         host_radius = radius.copy()
@@ -153,9 +109,9 @@ def test_fresh_host_mode_with_start_index(te, ctx, oracle):
     rows, cols = 150, 140
     z = synth.terrain(rows, cols, 0.02, 81, "mixed")
     og = oracle.Geometry.make(rows, cols, 0.02)
-    L, rs = _layers(oracle, og, z, 81)
-    begin, poses, radius = _paths(np.random.default_rng(81), og, 200)
-    ft, _ = _fps(te, oracle, 1)
+    L, rs = chain_layers(oracle, og, z, 81)
+    begin, poses, radius = circular_paths(np.random.default_rng(81), og, 200)
+    ft, _ = footprint_params(te, oracle, 1)
     g = te.Geometry.make(rows, cols, 0.02)
     want = _gpu(ctx, g, ft, L, begin, poses, radius, rs, None)
     sr, sc = 37, 101
@@ -174,7 +130,7 @@ def test_fresh_error_codes(te, ctx, oracle):
     one = np.ones((rows, cols), np.float32, order="F")
     L = dict(traversability=one, slope=one, step=one, elevation=one * 0, roughness=one)
     begin, poses, radius = np.array([0, 1], np.int32), np.zeros((1, 2)), np.array([0.3])
-    ft, _ = _fps(te, oracle, 0)
+    ft, _ = footprint_params(te, oracle, 0)
     assert _gpu(ctx, g, ft, L, begin, poses, radius, None, None)[0].tolist() == [1]
 
     def code(fn):
@@ -182,14 +138,14 @@ def test_fresh_error_codes(te, ctx, oracle):
             fn()
         return e.value.code
 
-    fv, _ = _fps(te, oracle, 1)
+    fv, _ = footprint_params(te, oracle, 1)
     assert code(lambda: ctx.check_footprint_paths_fresh(g, fv, one, one, one, one * 0, begin, poses, radius)) == -2   # no roughness
     assert code(lambda: ctx.check_footprint_paths_fresh(g, ft, None, one, one, one * 0, begin, poses, radius)) == -2
     assert code(lambda: _gpu(ctx, g, ft, L, begin, poses, np.array([np.nan]), None, None)) == -1
     assert code(lambda: _gpu(ctx, g, ft, L, begin, poses, np.array([-0.1]), None, None)) == -1
     assert code(lambda: _gpu(ctx, g, ft, L, begin, poses, np.array([2.4]), None, None)) == -4    # ceil(2.55 / 0.02) = 128 rings
     assert _gpu(ctx, g, ft, L, begin, poses, np.array([2.38]), None, None)[0].tolist() == [1]   # 127 rings
-    fneg, _ = _fps(te, oracle, 0)
+    fneg, _ = footprint_params(te, oracle, 0)
     fneg.offset = -0.1
     assert code(lambda: _gpu(ctx, g, fneg, L, begin, poses, radius, None, None)) == -1
     lib = te.load_library()

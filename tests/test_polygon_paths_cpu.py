@@ -4,7 +4,7 @@ the CPU oracle, against values derived by hand.  Dyadic geometry throughout: 0.2
 every expected value below is exact."""
 import numpy as np
 
-import polygon_paths_oracle as ppo
+import paths_oracle as po
 
 RES, N = 0.25, 32
 RECT = [(0.5, 0.25, 0.0), (-0.5, 0.25, 0.0), (-0.5, -0.25, 0.0), (0.5, -0.25, 0.0)]       # 1.0 x 0.5 m, centred
@@ -38,9 +38,8 @@ def _check(g, fp, L, footprint, paths, conservative=None, robot_slope=None):
             q = p[2:] if len(p) > 2 else IDENTITY
             poses.append([x, y, 0.0, *q])
         begin.append(len(poses))
-    return ppo.check_polygonal_paths(g, fp, L["traversability"], L["slope"], L["step"], L["elevation"], footprint, begin,
-                                     np.asarray(poses, np.float64).reshape(-1, 7), robot_slope=robot_slope,
-                                     roughness=L["roughness"], conservative=conservative)
+    return po.check_request(g, fp, dict(L, robot_slope=robot_slope), begin, np.asarray(poses, np.float64).reshape(-1, 7),
+                            footprint_xyz=footprint, conservative=conservative)[:3]
 
 
 def _mean_rows(rows):

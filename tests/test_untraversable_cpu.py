@@ -6,48 +6,21 @@ import math
 
 import numpy as np
 
-import paths_fresh_oracle as pfo
-import polygon_paths_oracle as ppo
-import untraversable_oracle as uo
-
-RES, N = 0.25, 64
-
-
-def X(i):
-    return (0.0 + (0.5 * N * RES - 0.5 * RES)) + RES * (-float(i))
-
+import paths_oracle as po
+from helpers import DYADIC_N as N, dyadic_cell as P, dyadic_map as _map, dyadic_x as X
 
 Y = X
-
-
-def P(i, j):
-    return (X(i), Y(j))
-
-
-def _map(oracle, blocked=(), trav=0.5):
-    g = oracle.Geometry.make(N, N, RES)
-    one = np.ones((N, N), np.float32, order="F")
-    slope = one.copy()
-    for a, b in blocked:
-        slope[a, b] = 0.0
-    t = trav if isinstance(trav, np.ndarray) else np.full((N, N), trav, np.float32, order="F")
-    fp = oracle.FootprintParams.yaml_defaults()
-    fp.max_gap_width, fp.offset, fp.traversability_default = 0.1, 0.5, 0.3
-    return g, fp, dict(traversability=np.asfortranarray(t), slope=slope, step=one, elevation=one * 0)
 
 
 def _circle(g, fp, L, paths, radius=1.0, cup=1, robot_slope=None, capacity=64):
     """paths: lists of (x, y) poses; returns (is_safe, traversability, [vertex list per path])."""
     begin = np.cumsum([0] + [len(p) for p in paths]).astype(np.int32)
     poses = np.asarray([q for p in paths for q in p], np.float64).reshape(-1, 2)
-    n = len(paths)
-    safe, t, cnt, xy = uo.check_circular_paths_fresh2(g, fp, L["traversability"], L["slope"], L["step"], L["elevation"], begin, poses,
-                                                       [radius] * n, robot_slope=robot_slope, compute_untraversable_polygon=[cup] * n,
-                                                       capacity=capacity)
-    ref_safe, ref_t = pfo.check_circular_paths_fresh(g, fp, L["traversability"], L["slope"], L["step"], L["elevation"], begin, poses,
-                                                     [radius] * n, robot_slope=robot_slope, compute_untraversable_polygon=[cup] * n)
+    Ls = dict(L, robot_slope=robot_slope)
+    safe, t, _, cnt, xy = po.check_request(g, fp, Ls, begin, poses, radius, cup=cup, capacity=capacity)
+    ref_safe, ref_t = po.check_request(g, fp, Ls, begin, poses, radius, cup=cup, capacity=0)[:2]   # no polygon outputs
     assert np.array_equal(safe, ref_safe) and np.array_equal(t.view(np.uint64), ref_t.view(np.uint64))
-    return safe, t, [[tuple(v) for v in xy[q, :min(cnt[q], capacity)]] for q in range(n)]
+    return safe, t, [[tuple(v) for v in xy[q, :min(cnt[q], capacity)]] for q in range(len(paths))]
 
 
 def from_circle(cx, cy, r):
@@ -167,8 +140,7 @@ def test_inclination_failure_publishes_nothing(oracle):
 def test_capacity_smaller_than_the_polygon(oracle):
     g, fp, L = _map(oracle, [(a, b) for a in range(31, 34) for b in range(31, 34)])
     begin, poses = np.array([0, 1], np.int32), np.array([P(32, 32)])
-    _, _, cnt, xy = uo.check_circular_paths_fresh2(g, fp, L["traversability"], L["slope"], L["step"], L["elevation"], begin, poses,
-                                                    [1.0], compute_untraversable_polygon=[1], capacity=2)
+    _, _, _, cnt, xy = po.check_request(g, fp, L, begin, poses, [1.0], cup=[1], capacity=2)
     assert cnt.tolist() == [4] and [tuple(v) for v in xy[0]] == [P(33, 33), P(31, 33)]
 
 
@@ -182,13 +154,11 @@ def _pose(x, y):
 def _polygonal(g, fp, L, paths, cup):
     begin = np.cumsum([0] + [len(p) for p in paths]).astype(np.int32)
     poses = np.asarray([_pose(*q) for p in paths for q in p], np.float64)
-    n = len(paths)
-    out = uo.check_polygonal_paths2(g, fp, L["traversability"], L["slope"], L["step"], L["elevation"], SQUARE, begin, poses,
-                                     compute_untraversable_polygon=[cup] * n)
-    ref = ppo.check_polygonal_paths(g, fp, L["traversability"], L["slope"], L["step"], L["elevation"], SQUARE, begin, poses)
-    for a, b in zip(out[:3], ref):
+    out = po.check_request(g, fp, L, begin, poses, footprint_xyz=SQUARE, cup=cup)
+    ref = po.check_request(g, fp, L, begin, poses, footprint_xyz=SQUARE, cup=1 - cup)   # is_safe, traversability, area: cup has no say
+    for a, b in zip(out[:3], ref[:3]):
         assert np.array_equal(a.view(np.uint8), b.view(np.uint8))
-    return out[0], [[tuple(v) for v in out[4][q, :out[3][q]]] for q in range(n)]
+    return out[0], [[tuple(v) for v in out[4][q, :out[3][q]]] for q in range(len(paths))]
 
 
 def test_polygonal_footprint_over_a_blocked_patch(oracle):

@@ -12,12 +12,12 @@ with the GPU name and its power limit.
 
 --footprint polygon times te_check_footprint_paths_polygon (TE_MEM_DEVICE) instead, with the YAML footprint polygon
 (robot_footprint_parameter.yaml:3) and planner-like paths with a random yaw per pose, conservative off and on, and the CPU oracle
-of the same call (tests/polygon_paths_oracle.cpp, all host threads, one run; it includes the oracle's whole-map
+of the same call (tests/paths_oracle.cpp, all host threads, one run; it includes the oracle's whole-map
 isTraversableForFilters pass, which the GPU evaluates only where a polygon looks).
 
 --untraversable times te_check_footprint_paths_fresh2 (radius 0.3 m) and te_check_footprint_paths_polygon2 (YAML footprint) in
 TE_MEM_DEVICE with compute_untraversable_polygon off and on for every path (room for 256 vertices per path), next to the CPU
-oracle of the same calls (tests/untraversable_oracle.cpp; all host threads, one run).
+oracle of the same calls (tests/paths_oracle.cpp; all host threads, one run).
 
 --request times te_check_footprint_request against the calls a node makes without it: te_check_footprint_paths_fresh on the
 circular paths and te_check_footprint_paths_polygon once per distinct footprint.  Every other path is circular (radius 0.3 m,
@@ -158,7 +158,7 @@ def main_polygon(args):
     import synth
     import traversability_estimation_b200 as te
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import polygon_paths_oracle as ppo
+    import paths_oracle as po
     from oracle import binding as ob
 
     n, res = args.size, 0.02
@@ -168,6 +168,7 @@ def main_polygon(args):
     ctx = te.Context(0)
     z = synth.terrain(n, n, res, 4096, "mixed")
     layers = ctx.chain_host(g, te.ChainParams.yaml_defaults(0), z)
+    oracle_layers = dict(traversability=layers["traversability"], slope=layers["slope"], step=layers["step"], elevation=z)
     dev = lambda a: torch.from_numpy(np.ascontiguousarray(np.asarray(a, np.float32).T)).cuda()  # noqa: E731
     trav, slope, step, elev = (dev(a) for a in (layers["traversability"], layers["slope"], layers["step"], z))
     stream = torch.cuda.Stream()
@@ -204,8 +205,8 @@ def main_polygon(args):
                 e1.synchronize()
                 ts.append(e0.elapsed_time(e1))
             t0 = time.perf_counter()
-            want = ppo.check_polygonal_paths(og, ofp, layers["traversability"], layers["slope"], layers["step"], z, fxyz, begin, poses,
-                                             conservative=cons if conservative else None)
+            want = po.check_request(og, ofp, oracle_layers, begin, poses, footprint_xyz=fxyz,
+                                    conservative=cons if conservative else None)[:3]
             cpu_ms = (time.perf_counter() - t0) * 1e3
             got = (safe.cpu().numpy(), tout.cpu().numpy(), aout.cpu().numpy())
             same = all(np.array_equal(a.view(np.uint8), b.view(np.uint8)) for a, b in zip(got, want))
@@ -224,7 +225,7 @@ def main_untraversable(args):
     import synth
     import traversability_estimation_b200 as te
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import untraversable_oracle as uo
+    import paths_oracle as po
     from oracle import binding as ob
 
     n, res, cap = args.size, 0.02, 256
@@ -234,6 +235,7 @@ def main_untraversable(args):
     ctx = te.Context(0)
     z = synth.terrain(n, n, res, 4096, "mixed")
     layers = ctx.chain_host(g, te.ChainParams.yaml_defaults(0), z)
+    oracle_layers = dict(traversability=layers["traversability"], slope=layers["slope"], step=layers["step"], elevation=z)
     dev = lambda a: torch.from_numpy(np.ascontiguousarray(np.asarray(a, np.float32).T)).cuda()  # noqa: E731
     trav, slope, step, elev = (dev(a) for a in (layers["traversability"], layers["slope"], layers["step"], z))
     stream = torch.cuda.Stream()
@@ -285,13 +287,10 @@ def main_untraversable(args):
                 med, mn = timed(run)
                 t0 = time.perf_counter()
                 if kind == "circle":
-                    want = uo.check_circular_paths_fresh2(og, ofp, layers["traversability"], layers["slope"], layers["step"], z, begin,
-                                                           xy, np.full(batch, 0.3), compute_untraversable_polygon=cup, capacity=cap)
-                    want_counts = want[2]
+                    want = po.check_request(og, ofp, oracle_layers, begin, xy, 0.3, cup=cup, capacity=cap)
                 else:
-                    want = uo.check_polygonal_paths2(og, ofp, layers["traversability"], layers["slope"], layers["step"], z, fxyz, begin,
-                                                      poses, compute_untraversable_polygon=cup, capacity=cap)
-                    want_counts = want[3]
+                    want = po.check_request(og, ofp, oracle_layers, begin, poses, footprint_xyz=fxyz, cup=cup, capacity=cap)
+                want_counts = want[3]
                 cpu_ms = (time.perf_counter() - t0) * 1e3
                 got = cnt.cpu().numpy()
                 print(json.dumps({"gpu": name, "power_limit_w": power, "map": f"{n}x{n}", "resolution": res, "footprint": kind,
