@@ -403,6 +403,28 @@ int te_check_footprint_request(te_ctx* ctx, const te_geometry* g, const te_footp
                                double* area_out, int32_t max_vertices, int32_t* untraversable_count_or_null,
                                double* untraversable_xy_or_null, int memory);
 
+/* te_check_footprint_request for the paths of a whole batch of maps in one call (multi-robot and MPC roll-out batches, after
+ * te_chain_batched).  Layers: nmaps whole maps of geometry g in the layout of te_chain_batched / te_footprint_batched, map m at
+ * offset m*rows*cols in every layer, robot_slope included.  Path q is on map path_map[q] (0..nmaps-1; any order, and a map may have
+ * no paths); poses are map-frame positions, the same for every map.  The other arguments and outputs are those of
+ * te_check_footprint_request, and path q gets, bit for bit, what te_check_footprint_request returns for it on map path_map[q]
+ * alone (is_safe, traversability, area and the untraversable polygon).  Each map has its own isTraversableForFilters memo; a path
+ * never reads the cells of another map.  Errors: those of te_check_footprint_request, per path, plus TE_ERR_BAD_ARG for nmaps < 1,
+ * a null path_map and, in TE_MEM_HOST, a path_map entry outside 0..nmaps-1; TE_ERR_UNSUPPORTED for a circular-buffer start index
+ * and for nmaps*cols >= 2^31.  TE_MEM_HOST stages the nmaps*cols columns of every layer once; TE_MEM_DEVICE is asynchronous on the
+ * context stream and cannot read path_map: a path on a map outside the batch gets is_safe = 0, NaN in traversability and area,
+ * and count -1 where its polygon was requested; the other paths are unaffected.  The launches are those of one
+ * te_check_footprint_request, whatever nmaps. */
+int te_check_footprint_request_batched(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, int32_t nmaps,
+                                       const float* traversability, const float* slope, const float* step,
+                                       const float* roughness_or_null, const float* elevation, const float* robot_slope_or_null,
+                                       const int32_t* path_map, int32_t npaths, int32_t nposes, const int32_t* path_begin,
+                                       const double* poses, const double* radius, int32_t nvertices, const int32_t* footprint_begin,
+                                       const float* footprint_xyz, int32_t max_footprint_vertices,
+                                       const uint8_t* conservative_or_null, const uint8_t* compute_untraversable_polygon_or_null,
+                                       uint8_t* is_safe, double* traversability_out, double* area_out, int32_t max_vertices,
+                                       int32_t* untraversable_count_or_null, double* untraversable_xy_or_null, int memory);
+
 /* ---- te_map: a traversability map that stays on the device between calls -------------------------------------------------------
  * The reference keeps its layers, the traversability_footprint cache and the isTraversableForFilters memo in one TraversabilityMap;
  * computeTraversability (TraversabilityMap.cpp:202-237) resets them and nothing else does (resetTraversabilityFootprintLayers,

@@ -24,6 +24,13 @@ circular paths and te_check_footprint_paths_polygon once per distinct footprint.
 offset 0.15 m), the rest polygonal over 1 or 4 distinct footprints, with a random yaw per pose.  Both in TE_MEM_DEVICE (CUDA
 events; the split calls write one output set each and nothing is scattered back) and in TE_MEM_HOST (host clock around the
 call, which ends in a synchronise; the split calls upload the layers once per call).  Outputs of the two are compared bit for bit.
+
+--batched times te_check_footprint_request_batched on a batch of maps against a loop of te_check_footprint_request, one call per
+map, both in TE_MEM_DEVICE on the same stream.  Maps: --maps (256 and 16) maps of 512 x 512 cells at 0.02 m (synth.terrain
+"mixed", 1 % holes, one seed per map) through te_chain_batched once.  Paths: --paths-per-map (4, 16, 64) planner-like paths per
+map, stored map by map; every other path circular (radius 0.3 m, offset 0.15 m), the others the YAML footprint with a random
+yaw per pose.  CUDA events around the whole batch (the batched call, or the loop), median of --reps after --warmup, the two
+alternating; the kernel launches of one batch (te_get_stats); whether the two output sets are identical bit for bit.
 """
 from __future__ import annotations
 
@@ -76,7 +83,12 @@ def main():
     ap.add_argument("--untraversable", action="store_true")
     ap.add_argument("--request", action="store_true")
     ap.add_argument("--map", action="store_true")
+    ap.add_argument("--batched", action="store_true")
+    ap.add_argument("--maps", type=int, nargs="+", default=[256, 16])
+    ap.add_argument("--paths-per-map", type=int, nargs="+", default=[4, 16, 64])
     args = ap.parse_args()
+    if args.batched:
+        return main_batched(args)
     if args.map:
         return main_map(args)
     if args.request:
@@ -511,6 +523,95 @@ def main_map(args):
             row[f"map_{label}_kernels_ms"] = round(sum(e.self_device_time_total for e in ev) / 1e3 / reps, 4)
         print(json.dumps(row), flush=True)
     m.close()
+    ctx.close()
+
+
+def main_batched(args):
+    import torch
+    import synth
+    import traversability_estimation_b200 as te
+
+    n, res = 512, 0.02
+    g = te.Geometry.make(n, n, res)
+    fp = te.FootprintParams.yaml_defaults()            # offset 0.15
+    fyaml = np.asarray(YAML_FOOTPRINT, np.float32)
+    ctx = te.Context(0)
+    stream = torch.cuda.Stream()   # torch's work, the library's calls and the events share one stream
+    torch.cuda.set_stream(stream)
+    ctx.set_stream(stream.cuda_stream)
+    name, power = gpu_info(torch)
+    for nmaps in args.maps:
+        z = torch.from_numpy(np.stack([np.ascontiguousarray(synth.terrain(n, n, res, 1000 + k, "mixed").T) for k in range(nmaps)])).cuda()
+        slope, step, rough, trav = (torch.empty_like(z) for _ in range(4))
+        ctx.chain_batched(g, te.ChainParams.yaml_defaults(0), nmaps, z, slope, step, rough, trav, te.MEM_DEVICE)
+        for per_map in args.paths_per_map:
+            rng = np.random.default_rng(per_map)
+            maps = []   # per map: path_begin, poses (7 wide), footprint_begin, footprint_xyz
+            for _ in range(nmaps):
+                begin, xy = planner_paths(rng, n, per_map, res)
+                yaw = rng.uniform(0, 2 * np.pi, len(xy))
+                poses = np.stack([xy[:, 0], xy[:, 1], np.zeros(len(xy)), np.zeros(len(xy)), np.zeros(len(xy)), np.sin(yaw / 2),
+                                  np.cos(yaw / 2)], axis=1)
+                circ = np.arange(per_map) % 2 == 1   # odd paths circular
+                fbeg = np.concatenate([[0], np.cumsum(np.where(circ, 0, len(fyaml)))]).astype(np.int32)
+                fxyz = np.concatenate([fyaml] * int((~circ).sum()) + [np.zeros((0, 3), np.float32)])
+                maps.append((begin, poses, fbeg, fxyz))
+            npaths = nmaps * per_map
+            # the whole batch, paths map by map
+            begin = np.concatenate([[0]] + [m[0][1:] + sum(len(p[1]) for p in maps[:k]) for k, m in enumerate(maps)]).astype(np.int32)
+            poses = np.concatenate([m[1] for m in maps])
+            fbeg = np.concatenate([[0]] + [m[2][1:] + sum(len(p[3]) for p in maps[:k]) for k, m in enumerate(maps)]).astype(np.int32)
+            fxyz = np.concatenate([m[3] for m in maps])
+            d = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
+            path_map = d(np.repeat(np.arange(nmaps, dtype=np.int32), per_map))
+            db, dp, dr, dfb, dfx = d(begin), d(poses), d(np.full(npaths, 0.3)), d(fbeg), d(fxyz)
+            per = [(d(m[0]), d(m[1]), d(np.full(per_map, 0.3)), d(m[2]), d(m[3])) for m in maps]
+            outs = lambda: dict(is_safe=torch.empty(npaths, dtype=torch.uint8, device="cuda"),  # noqa: E731
+                                traversability_out=torch.empty(npaths, dtype=torch.float64, device="cuda"),
+                                area_out=torch.empty(npaths, dtype=torch.float64, device="cuda"))
+            ob, ol = outs(), outs()
+
+            def batched():
+                ctx.check_footprint_request_batched(g, fp, nmaps, trav, slope, step, z, path_map, db, dp, dr, dfb, dfx,
+                                                    max_footprint_vertices=len(fyaml), memory=te.MEM_DEVICE, **ob)
+
+            def loop():
+                for k, (b, p, r, fb, fx) in enumerate(per):
+                    sl = slice(k * per_map, (k + 1) * per_map)
+                    ctx.check_footprint_request(g, fp, trav[k], slope[k], step[k], z[k], b, p, r, fb, fx, max_footprint_vertices=len(fyaml),
+                                                memory=te.MEM_DEVICE, **{key: v[sl] for key, v in ol.items()})
+
+            launches = {}
+            for key, fn in (("batched", batched), ("loop", loop)):
+                l0 = ctx.stats()[0]
+                fn()
+                stream.synchronize()
+                launches[key] = ctx.stats()[0] - l0
+            for _ in range(args.warmup):
+                batched()
+                loop()
+            stream.synchronize()
+            tb, tl = [], []
+            for _ in range(args.reps):
+                for fn, ts in ((batched, tb), (loop, tl)):
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record(stream)
+                    fn()
+                    e1.record(stream)
+                    e1.synchronize()
+                    ts.append(e0.elapsed_time(e1))
+            same = all(np.array_equal(ob[k].cpu().numpy().view(np.uint8), ol[k].cpu().numpy().view(np.uint8)) for k in ob)
+            mb, ml = float(np.median(tb)), float(np.median(tl))
+            print(json.dumps({"gpu": name, "power_limit_w": power, "maps": nmaps, "size": f"{n}x{n}", "resolution": res,
+                              "paths_per_map": per_map, "paths": npaths, "poses": int(begin[-1]), "circular": npaths // 2,
+                              "batched_ms": round(mb, 4), "loop_ms": round(ml, 4), "speedup": round(ml / mb, 3),
+                              "batched_ms_range": [round(min(tb), 4), round(max(tb), 4)],
+                              "loop_ms_range": [round(min(tl), 4), round(max(tl), 4)],
+                              "launches_batched": launches["batched"], "launches_loop": launches["loop"],
+                              "safe": int(ob["is_safe"].sum().item()), "bit_identical": bool(same)}), flush=True)
+        del z, slope, step, rough, trav
+        torch.cuda.empty_cache()
+    ctx.set_stream(None)
     ctx.close()
 
 

@@ -18,7 +18,7 @@ KERNEL_AUTO, KERNEL_GENERIC, KERNEL_FUSED = 0, 1, 2
 
 EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set_stream", "te_synchronize",
            "te_set_kernel", "te_get_stats", "te_enable_timing", "te_get_timing", "te_get_flag_counters", "te_get_escalation_stats", "te_fused_plan", "te_slope", "te_normals", "te_step", "te_roughness", "te_chain",
-           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_footprint_batched", "te_footprint_polygon_batched", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_check_footprint_paths_fresh2", "te_check_footprint_paths_polygon2", "te_check_footprint_request", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
+           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_footprint_batched", "te_footprint_polygon_batched", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_check_footprint_paths_fresh2", "te_check_footprint_paths_polygon2", "te_check_footprint_request", "te_check_footprint_request_batched", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
            "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free", "te_map_create", "te_map_destroy",
            "te_map_chain", "te_map_set_layers", "te_map_footprint", "te_map_footprint_polygon", "te_map_check_footprint_request",
            "te_map_get_footprint", "te_map_clear_footprint", "te_map_request_stats"]
@@ -454,36 +454,73 @@ class Context:
         float32, conservative / compute_untraversable_polygon uint8) and the results go to the caller's is_safe /
         traversability_out / area_out tensors.  untraversable_capacity=V: the tuple gains counts (int32[npaths]) and xy
         (float64[npaths, V, 2]) as in check_footprint_paths_fresh."""
-        fn = self._L.te_check_footprint_request
-        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + \
+        return self._request(None, g, fp, traversability, slope, step, elevation, path_begin, poses, radius, footprint_begin,
+                             footprint_xyz, max_footprint_vertices, robot_slope, roughness, conservative, compute_untraversable_polygon,
+                             memory, is_safe, traversability_out, area_out, untraversable_capacity, untraversable_count, untraversable_xy)
+
+    def check_footprint_request_batched(self, g, fp, nmaps, traversability, slope, step, elevation, path_map, path_begin, poses,
+                                        radius, footprint_begin, footprint_xyz, max_footprint_vertices=None, robot_slope=None,
+                                        roughness=None, conservative=None, compute_untraversable_polygon=None, memory=MEM_HOST,
+                                        is_safe=None, traversability_out=None, area_out=None, untraversable_capacity=None,
+                                        untraversable_count=None, untraversable_xy=None):
+        """te_check_footprint_request_batched: check_footprint_request() for the paths of nmaps whole maps of geometry g stored back
+        to back (the layout of chain_batched: layers shaped (nmaps, cols, rows)); path q is on map path_map[q] (int32 per path).
+        Keyword arguments and return values are those of check_footprint_request."""
+        return self._request((int(nmaps), path_map), g, fp, traversability, slope, step, elevation, path_begin, poses, radius,
+                             footprint_begin, footprint_xyz, max_footprint_vertices, robot_slope, roughness, conservative,
+                             compute_untraversable_polygon, memory, is_safe, traversability_out, area_out, untraversable_capacity,
+                             untraversable_count, untraversable_xy)
+
+    def _request(self, batch, g, fp, traversability, slope, step, elevation, path_begin, poses, radius, footprint_begin, footprint_xyz,
+                 max_footprint_vertices, robot_slope, roughness, conservative, compute_untraversable_polygon, memory, is_safe,
+                 traversability_out, area_out, untraversable_capacity, untraversable_count, untraversable_xy):
+        """The body of check_footprint_request (batch None) and check_footprint_request_batched (batch = (nmaps, path_map)): the
+        batched entry takes nmaps after the parameters and path_map after robot_slope."""
+        if batch is None:
+            fn = self._L.te_check_footprint_request
+            head, nlay = [], 6
+        else:
+            fn = self._L.te_check_footprint_request_batched
+            head, nlay = [C.c_int32], 7
+        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + head + [C.c_void_p] * nlay + \
             [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32] + \
             [C.c_void_p] * 5 + [C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
+        def lead(layers, path_map):
+            """The arguments up to the path count: parameters, (nmaps,) the layers in argument order, (path_map)."""
+            return [C.byref(g), C.byref(fp)] + ([] if batch is None else [batch[0]]) + [_addr(a) for a in layers] + \
+                ([] if batch is None else [_addr(path_map)])
+
         maxv = 0 if untraversable_capacity is None else int(untraversable_capacity)
         if memory == MEM_DEVICE:
             self._order_after_torch(memory)
             n = int(path_begin.numel()) - 1
             mfv = 16 if max_footprint_vertices is None else int(max_footprint_vertices)
             self._check(fn(
-                self._h, C.byref(g), C.byref(fp), _addr(traversability), _addr(slope), _addr(step), _addr(roughness), _addr(elevation),
-                _addr(robot_slope), n, int(poses.numel()) // 7, _addr(path_begin), _addr(poses), _addr(radius),
+                self._h, *lead([traversability, slope, step, roughness, elevation, robot_slope], None if batch is None else batch[1]),
+                n, int(poses.numel()) // 7, _addr(path_begin), _addr(poses), _addr(radius),
                 int(footprint_xyz.numel()) // 3, _addr(footprint_begin), _addr(footprint_xyz), mfv, _addr(conservative),
                 _addr(compute_untraversable_polygon), _addr(is_safe), _addr(traversability_out), _addr(area_out), maxv,
                 _addr(untraversable_count), _addr(untraversable_xy), MEM_DEVICE))
             if untraversable_capacity is None:
                 return is_safe, traversability_out, area_out
             return is_safe, traversability_out, area_out, untraversable_count, untraversable_xy
-        lay = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)  # noqa: E731
+        if batch is None:   # one column-major map
+            lay = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)  # noqa: E731
+        else:               # (nmaps, cols, rows)
+            lay = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float32)  # noqa: E731
         t, s, st, e, rs, r = (lay(a) for a in (traversability, slope, step, elevation, robot_slope, roughness))
         pb = np.ascontiguousarray(path_begin, dtype=np.int32)
         ps = np.ascontiguousarray(poses, dtype=np.float64).reshape(-1, 7)
         rad = np.ascontiguousarray(radius, dtype=np.float64)
         fb = np.ascontiguousarray(footprint_begin, dtype=np.int32)
         fxyz = np.ascontiguousarray(footprint_xyz, dtype=np.float32).reshape(-1, 3)
+        pm = None if batch is None or batch[1] is None else np.ascontiguousarray(batch[1], dtype=np.int32)
         n = len(pb) - 1
         per_path = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.uint8)  # noqa: E731
         cons, cup = per_path(conservative), per_path(compute_untraversable_polygon)
-        if len(rad) != n or len(fb) != n + 1 or any(a is not None and len(a) != n for a in (cons, cup)):
-            raise ValueError("radius / conservative / compute_untraversable_polygon need one entry per path, footprint_begin npaths + 1")
+        if len(rad) != n or len(fb) != n + 1 or any(a is not None and len(a) != n for a in (cons, cup, pm)):
+            raise ValueError("radius / conservative / compute_untraversable_polygon / path_map need one entry per path, "
+                             "footprint_begin npaths + 1")
         if max_footprint_vertices is None:
             max_footprint_vertices = int(np.diff(fb).max()) if n > 0 else 0
         safe = np.zeros(n, dtype=np.uint8) if is_safe is None else is_safe
@@ -491,8 +528,7 @@ class Context:
         area = np.zeros(n, dtype=np.float64) if area_out is None else area_out
         counts, uxy = (None, None) if untraversable_capacity is None else _untraversable_outputs(n, maxv)
         self._check(fn(
-            self._h, C.byref(g), C.byref(fp), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), n, len(ps), pb.ctypes.data,
-            ps.ctypes.data, rad.ctypes.data, len(fxyz), fb.ctypes.data, fxyz.ctypes.data, int(max_footprint_vertices), _addr(cons),
+            self._h, *lead([t, s, st, r, e, rs], pm), n, len(ps), pb.ctypes.data, ps.ctypes.data, rad.ctypes.data, len(fxyz), fb.ctypes.data, fxyz.ctypes.data, int(max_footprint_vertices), _addr(cons),
             _addr(cup), safe.ctypes.data, trav.ctypes.data, area.ctypes.data, maxv, _addr(counts), _addr(uxy), MEM_HOST))
         if untraversable_capacity is None:
             return safe, trav, area

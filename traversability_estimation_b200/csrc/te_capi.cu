@@ -70,7 +70,7 @@ struct te_ctx {
   DevBuf dX, dY;
   std::vector<double> hX, hY;
 
-  DevBuf stage[20];          // TE_MEM_HOST staging (handed out in order by Staging; te_check_footprint_request takes 18)
+  DevBuf stage[20];          // TE_MEM_HOST staging (handed out in order by Staging; te_check_footprint_request_batched takes 19)
   DevBuf worklist, worklist3, counter;  // fused-kernel fix-up lists (tier 2, tier 3) and their counters
   // The counters are two 512-byte blocks used alternately: the last kernel of a chain call (k_fixup_cells) zeroes the block of the
   // NEXT call, so a call needs no cudaMemsetAsync of its own (one stream operation and one launch gap less per map).
@@ -979,6 +979,7 @@ int te_check_footprint_paths_fresh(te_ctx* c, const te_geometry* g_in, const te_
 // Stages the path arrays of `r` and points `r` at the device copies (host memory; null stays null).
 static void stage_paths(Staging& st, te::PathChecks& r) {
   const size_t np = (size_t)r.npaths;
+  r.path_map = st.in(r.path_map, np);
   r.path_begin = st.in(r.path_begin, np + 1);
   r.poses = st.in(r.poses, (size_t)r.pose_stride * r.nposes);
   r.radius = st.in(r.radius, np);
@@ -993,15 +994,18 @@ static void stage_paths(Staging& st, te::PathChecks& r) {
   r.uxy = st.out(r.uxy, 2 * (size_t)r.max_vertices * np);
 }
 
-// The body of te_check_footprint_paths_fresh2, te_check_footprint_paths_polygon2 and te_check_footprint_request once the entry has
-// put its arguments into `r` (the caller's pointers): the checks the three share, then in host memory `host_checks(g, r)` (the
-// entry's validation of the path arrays; it sets r.nposes where the entry has none, and r.max_points), the staging, the launches
-// and the download.  Device memory reads nothing back: a path that cannot be checked gets is_safe 0 and NaN (te_b200.h).
+// The body of te_check_footprint_paths_fresh2, te_check_footprint_paths_polygon2, te_check_footprint_request and
+// te_check_footprint_request_batched once the entry has put its arguments into `r` (the caller's pointers): the checks they share,
+// then in host memory `host_checks(g, r)` (the entry's validation of the path arrays; it sets r.nposes where the entry has none,
+// and r.max_points), the staging of r.nmaps maps, the launches and the download.  Device memory reads nothing back: a path that
+// cannot be checked gets is_safe 0 and NaN (te_b200.h).  A batch (r.path_map) takes maps in default order only.
 static int run_path_checks(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, te::PathChecks r, int memory, const char* what,
                            const std::function<int(const te_geometry*, te::PathChecks&)>& host_checks) {
   te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE, &g0)) return rc;
+  if (int rc = unwrap_geometry(g_in, memory != TE_MEM_DEVICE && !r.path_map, &g0)) return rc;
   const te_geometry* g = &g0;
+  if (r.nmaps < 1) return fail(TE_ERR_BAD_ARG, "number of maps must be positive");
+  if ((long long)r.nmaps * g->cols >= (1LL << 31)) return fail(TE_ERR_UNSUPPORTED, "batch of 2^31 or more columns");
   if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
   const bool circular = r.footprint_begin || !r.footprint, polygonal = r.footprint_begin || r.footprint;
   if (circular && !(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
@@ -1017,12 +1021,13 @@ static int run_path_checks(te_ctx* c, const te_geometry* g_in, const te_footprin
     if (int rc = host_checks(g, r)) return rc;
   int32_t* const ucount = r.ucount;
   Staging st(c, host, g_in);
-  r.trav = st.in_layer(r.trav, g->cols);
-  r.slope = st.in_layer(r.slope, g->cols);
-  r.step = st.in_layer(r.step, g->cols);
-  r.elev = st.in_layer(r.elev, g->cols);
-  r.rough = st.in_layer(p->verify_roughness ? r.rough : nullptr, g->cols);
-  r.robot_slope = st.in_layer(r.robot_slope, g->cols);
+  const int ncols = g->cols * r.nmaps;
+  r.trav = st.in_layer(r.trav, ncols);
+  r.slope = st.in_layer(r.slope, ncols);
+  r.step = st.in_layer(r.step, ncols);
+  r.elev = st.in_layer(r.elev, ncols);
+  r.rough = st.in_layer(p->verify_roughness ? r.rough : nullptr, ncols);
+  r.robot_slope = st.in_layer(r.robot_slope, ncols);
   stage_paths(st, r);
   if (st.rc) return st.rc;
   const te_slab s{0, g->cols, 0, 0};
@@ -1045,7 +1050,7 @@ int te_check_footprint_paths_fresh2(te_ctx* c, const te_geometry* g_in, const te
                                     int memory) {
   TE_ENTER(c);
   te::PathChecks r{};
-  r.trav = trav; r.slope = slope; r.step = step; r.rough = rough; r.elev = elev; r.robot_slope = robot_slope;
+  r.trav = trav; r.slope = slope; r.step = step; r.rough = rough; r.elev = elev; r.robot_slope = robot_slope; r.nmaps = 1;
   r.npaths = npaths; r.nposes = -1; r.path_begin = path_begin; r.poses = poses_xy; r.pose_stride = 2; r.radius = radius; r.cup = cup;
   r.is_safe = is_safe; r.trav_out = traversability; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
   return run_path_checks(c, g_in, p, r, memory, "fresh path check", [&](const te_geometry* g, te::PathChecks& h) -> int {
@@ -1080,7 +1085,7 @@ int te_check_footprint_paths_polygon2(te_ctx* c, const te_geometry* g_in, const 
   for (int k = 0; k < 3 * nfootprint; ++k)
     if (!std::isfinite(footprint_xyz[k])) return fail(TE_ERR_BAD_ARG, "footprint vertex %d is not finite", k / 3);
   te::PathChecks r{};
-  r.trav = trav; r.slope = slope; r.step = step; r.rough = rough; r.elev = elev; r.robot_slope = robot_slope;
+  r.trav = trav; r.slope = slope; r.step = step; r.rough = rough; r.elev = elev; r.robot_slope = robot_slope; r.nmaps = 1;
   r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7;
   r.nfp = nfootprint; r.footprint = footprint_xyz; r.conservative = conservative; r.cup = ucount ? cup : nullptr;
   // the hull input bound of one item; host memory sizes it from the paths
@@ -1147,13 +1152,14 @@ static int check_request_host(const te_geometry* g, const te_footprint_params* p
   return TE_OK;
 }
 
-int te_check_footprint_request(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
-                               const float* step, const float* rough, const float* elev, const float* robot_slope, int32_t npaths,
-                               int32_t nposes, const int32_t* path_begin, const double* poses, const double* radius, int32_t nvertices,
-                               const int32_t* footprint_begin, const float* footprint_xyz, int32_t max_footprint_vertices,
-                               const uint8_t* conservative, const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area,
-                               int32_t max_vertices, int32_t* ucount, double* uxy, int memory) {
-  TE_ENTER(c);
+// te_check_footprint_request (one map, path_map null) and te_check_footprint_request_batched (nmaps maps, path q on path_map[q]).
+static int footprint_request_common(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, int32_t nmaps, const float* trav,
+                                    const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                                    const int32_t* path_map, int32_t npaths, int32_t nposes, const int32_t* path_begin, const double* poses,
+                                    const double* radius, int32_t nvertices, const int32_t* footprint_begin, const float* footprint_xyz,
+                                    int32_t max_footprint_vertices, const uint8_t* conservative, const uint8_t* cup, uint8_t* is_safe,
+                                    double* traversability, double* area, int32_t max_vertices, int32_t* ucount, double* uxy,
+                                    int memory) {
   if (nvertices < 0 || !footprint_begin || (nvertices > 0 && !footprint_xyz)) return fail(TE_ERR_BAD_ARG, "null argument or negative count");
   if (max_footprint_vertices < 0 || max_footprint_vertices > te::kPolyMaxVerts)
     return fail(TE_ERR_BAD_ARG, "max_footprint_vertices must be 0..%d, got %d", te::kPolyMaxVerts, max_footprint_vertices);
@@ -1161,15 +1167,45 @@ int te_check_footprint_request(te_ctx* c, const te_geometry* g_in, const te_foot
   // from the paths.
   te::PathChecks r{};
   r.trav = trav; r.slope = slope; r.step = step; r.rough = rough; r.elev = elev; r.robot_slope = robot_slope;
+  r.nmaps = nmaps; r.path_map = path_map;
   r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7; r.radius = radius;
   r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
   r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup;
   r.max_points = conservative && max_footprint_vertices > 0 ? 2 * te::kPolyConsCap : 2 * std::max(max_footprint_vertices, 1);
   r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
   return run_path_checks(c, g_in, p, r, memory, "footprint path request", [&](const te_geometry* g, te::PathChecks& h) {
+    for (int32_t q = 0; path_map && q < npaths; ++q)
+      if (path_map[q] < 0 || path_map[q] >= nmaps)
+        return fail(TE_ERR_BAD_ARG, "path_map[%d] = %d is outside 0..%d", q, path_map[q], nmaps - 1);
     return check_request_host(g, p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
                               max_footprint_vertices, conservative, &h.max_points);
   });
+}
+
+int te_check_footprint_request(te_ctx* c, const te_geometry* g_in, const te_footprint_params* p, const float* trav, const float* slope,
+                               const float* step, const float* rough, const float* elev, const float* robot_slope, int32_t npaths,
+                               int32_t nposes, const int32_t* path_begin, const double* poses, const double* radius, int32_t nvertices,
+                               const int32_t* footprint_begin, const float* footprint_xyz, int32_t max_footprint_vertices,
+                               const uint8_t* conservative, const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area,
+                               int32_t max_vertices, int32_t* ucount, double* uxy, int memory) {
+  TE_ENTER(c);
+  return footprint_request_common(c, g_in, p, 1, trav, slope, step, rough, elev, robot_slope, nullptr, npaths, nposes, path_begin, poses,
+                                  radius, nvertices, footprint_begin, footprint_xyz, max_footprint_vertices, conservative, cup, is_safe,
+                                  traversability, area, max_vertices, ucount, uxy, memory);
+}
+
+int te_check_footprint_request_batched(te_ctx* c, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, const float* trav,
+                                       const float* slope, const float* step, const float* rough, const float* elev,
+                                       const float* robot_slope, const int32_t* path_map, int32_t npaths, int32_t nposes,
+                                       const int32_t* path_begin, const double* poses, const double* radius, int32_t nvertices,
+                                       const int32_t* footprint_begin, const float* footprint_xyz, int32_t max_footprint_vertices,
+                                       const uint8_t* conservative, const uint8_t* cup, uint8_t* is_safe, double* traversability,
+                                       double* area, int32_t max_vertices, int32_t* ucount, double* uxy, int memory) {
+  TE_ENTER(c);
+  if (!path_map) return fail(TE_ERR_BAD_ARG, "path_map is null");
+  return footprint_request_common(c, g, p, nmaps, trav, slope, step, rough, elev, robot_slope, path_map, npaths, nposes, path_begin, poses,
+                                  radius, nvertices, footprint_begin, footprint_xyz, max_footprint_vertices, conservative, cup, is_safe,
+                                  traversability, area, max_vertices, ucount, uxy, memory);
 }
 
 // ---- te_map: the layers, the traversability_footprint cache and the isTraversableForFilters memo, resident on the device -------
@@ -1409,7 +1445,7 @@ int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int3
   if (nvertices > 0) {  // the polygonal paths (TraversabilityMap.cpp:464-584) read the memo and leave the cache alone
     te::PathChecks r{};
     r.trav = (const float*)m->trav.p; r.slope = (const float*)m->slope.p; r.step = (const float*)m->step.p; r.rough = rough;
-    r.elev = (const float*)m->elev.p; r.robot_slope = rslope;
+    r.elev = (const float*)m->elev.p; r.robot_slope = rslope; r.nmaps = 1;
     r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7;
     r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
     r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup; r.max_points = mp;

@@ -1180,6 +1180,9 @@ struct CircleTable {
 // k_check_paths_fresh*), any other count polygonal (checked by k_check_polygon_*).  Without fp_begin every path is circular for
 // k_check_paths_fresh* and uses the one footprint of PolyPathArgs for k_check_polygon_*.  Device memory cannot validate the arrays
 // on the host, so the kernels do (request_footprint_ok_d, the pose range).
+// A batch of maps (te_check_footprint_request_batched): path q is on map path_map[q], whose layers, robot_slope and memo start
+// path_map[q] * map_cells cells into theirs.  Each kernel shifts those pointers once it knows its path (map_offset_d), so one map
+// and a batch run the same code.
 struct RequestArgs {
   const int* fp_begin;   // [npaths + 1], nullptr: no per-path footprints
   const float* fp_xyz;   // 3 floats (x, y, z) per vertex
@@ -1187,7 +1190,22 @@ struct RequestArgs {
   int maxfp;             // max_footprint_vertices: a longer footprint is not checked
   int nposes;            // < 0: not known, the circular check does not test pose ranges
   double* area_out;      // the area of the circular paths: 0, NaN for a path that is not checked; nullptr: not wanted
+  const int* path_map;   // [npaths], nullptr: every path is on map 0
+  int nmaps;             // maps of the batch: a path on a map outside 0 .. nmaps-1 is not checked
+  long long map_cells;   // rows * cols
 };
+
+// The first cell of path q's map in the layers and the memo, or -1 for a map outside the batch.
+__device__ __forceinline__ long long map_offset_d(const RequestArgs& R, int q) {
+  if (!R.path_map) return 0;
+  const int m = R.path_map[q];
+  return (m >= 0 && m < R.nmaps) ? m * R.map_cells : -1;
+}
+
+// The layers of the map that starts `o` cells in (a null roughness layer stays null).
+__device__ __forceinline__ Layers shift_layers_d(const Layers& L, long long o) {
+  return Layers{L.trav + o, L.slope + o, L.step + o, L.elev + o, L.rough ? L.rough + o : nullptr};
+}
 
 // Whether path q's footprint can be checked: 1..maxfp vertices inside fp_xyz, all finite (host memory rejects the rest).  The
 // vertex components are read from `first` in steps of `step` (a warp: lane, 32; one thread: 0, 1).
@@ -1201,8 +1219,8 @@ __device__ __forceinline__ bool request_footprint_ok_d(const RequestArgs& R, int
 // The body of k_check_paths_fresh; POLY also produces the untraversable polygon (k_check_paths_fresh_poly).  With per-path
 // footprints (R.fp_begin) it checks the circular paths of a request and leaves its polygonal paths to k_check_polygon_*.
 template <bool POLY>
-__device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layers& L, const PathArgs& P, const UntravOut& O,
-                                                    const CircleTable& C, const UntravScratch& S, const RequestArgs& R) {
+__device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, Layers L, PathArgs P, const UntravOut& O, const CircleTable& C,
+                                                    const UntravScratch& S, const RequestArgs& R) {
   const int PS = P.pose_stride;  // x and y come first
   const int lane = threadIdx.x & 31;
   const int q = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
@@ -1212,9 +1230,10 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
   const double rmin = P.radius[q], rmax = rmin + P.offset;
   const bool cup = P.cup != nullptr && P.cup[q] != 0;
   const double rings = ceil(rmax / A.res);  // SpiralIterator nRings
+  const long long mo = map_offset_d(R, q);
   // not checkable here: marked so that no checked result looks alike (with a pose count: also a pose range outside it; written
   // b <= nposes - n, which ptxas compiles to fewer registers in the _poly kernel than a 64-bit b + n, see DESIGN.md)
-  if (!(rmin >= 0.0) || !(rings <= (double)kPathMaxRings) || (R.nposes >= 0 && !(b >= 0 && n >= 0 && b <= R.nposes - n))) {
+  if (!(rmin >= 0.0) || !(rings <= (double)kPathMaxRings) || (R.nposes >= 0 && !(b >= 0 && n >= 0 && b <= R.nposes - n)) || mo < 0) {
     if (lane == 0) {
       P.is_safe[q] = 0; P.trav_out[q] = nan("");
       if (R.area_out) R.area_out[q] = nan("");
@@ -1222,6 +1241,9 @@ __device__ __forceinline__ void check_paths_fresh_d(const FpArgs& A, const Layer
     }
     return;
   }
+  L = shift_layers_d(L, mo);  // path q's map
+  if (P.rslope) P.rslope += mo;
+  P.memo += mo;
   const int nr = (int)rings;
   double result = 0.0, lengthPath = 0.0;
   double sx = 0.0, sy = 0.0, ex = 0.0, ey = 0.0;
@@ -1505,7 +1527,7 @@ __host__ __device__ inline size_t poly_warp_smem(int mcap, bool poly) {
 // set for the item's path, the walk goes on past blocked cells and collects them (:602-608, :634-638).  With per-path footprints
 // (R.fp_begin) each polygonal path uses its own, and the poses of circular paths are no items.
 template <bool POLY>
-__device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Layers& L, const PolyPathArgs& P, const PolyUntravArgs& U,
+__device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, Layers L, const PolyPathArgs& P, const PolyUntravArgs& U,
                                                      const RequestArgs& R) {
   extern __shared__ double2 sPoly[];
   const int lane = threadIdx.x & 31;
@@ -1530,10 +1552,14 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
   }
   const int q = lo, b = P.path_begin[q], e = P.path_begin[q + 1], n = e - b, k = p - b;
   if (R.fp_begin && R.fp_begin[q + 1] == R.fp_begin[q]) return;  // a pose of a circular path
-  if (!(b >= 0 && b <= p && p < e && e <= P.nposes && (n == 1 || k >= 1))) {
+  const long long mo = map_offset_d(R, q);
+  if (!(b >= 0 && b <= p && p < e && e <= P.nposes && (n == 1 || k >= 1)) || mo < 0) {
     if (lane == 0) P.items[p] = it;
     return;
   }
+  L = shift_layers_d(L, mo);  // path q's map
+  const float* const rslope = P.rslope ? P.rslope + mo : nullptr;
+  unsigned char* const memo = P.memo + mo;
   it.q = q;
   const bool cup = POLY && U.cup != nullptr && U.cup[q] != 0;
   int ncollected = 0;  // POLY: blocked cells collected by the walk
@@ -1619,7 +1645,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
   }
   if (lane == 0) it.hull_area = polygon_area_d(sA, nh);
   // checkInclination (:524-526, :550-554), then isTraversable(polygon) (:592-645)
-  bool ok = inclination_ok_d(A, P.rslope, sx, sy, ex, ey);
+  bool ok = inclination_ok_d(A, rslope, sx, sy, ex, ey);
   double t = 0.0;
   if (ok) {
     double tlx = sA[0].x, tly = sA[0].y, brx = tlx, bry = tly;  // PolygonIterator::findSubmapParameters
@@ -1649,7 +1675,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, const Laye
         bb = sj + (int)(c % nc);
         if (a >= 0 && bb >= 0 && a < A.rows && bb < A.cols_total && polygon_inside_d(sA, nh, A.X[a], A.Y[bb])) {
           member = true;
-          blk = blocked_memo_d(A, L, P.memo, a, bb);
+          blk = blocked_memo_d(A, L, memo, a, bb);
           if (!blk) {
             const float f = __ldg(L.trav + (size_t)bb * A.rows + a);
             v = finitef(f) ? (double)f : A.tdefault;  // :613-619
@@ -1721,7 +1747,7 @@ __device__ __forceinline__ void check_polygon_combine_d(const PolyPathArgs& P, c
   }
   int failed = -1;  // POLY: pose index of the failing item
   const int b = P.path_begin[q], e = P.path_begin[q + 1], n = e - b;
-  bool checkable = fp_ok && b >= 0 && e >= b && e <= P.nposes;
+  bool checkable = fp_ok && b >= 0 && e >= b && e <= P.nposes && map_offset_d(R, q) >= 0;  // an empty path on no map too
   unsigned char safe = 0;
   double trav = 0.0, area = 0.0;
   if (checkable && n > 0) {
@@ -1854,9 +1880,10 @@ FpArgs filter_args(const SlabView& v, const te_geometry* g, const te_footprint_p
   return a;
 }
 
-// The per-call isTraversableForFilters memo of the path checks (blocked_memo_d): one byte per map cell, cleared on `s`.
-int reset_filter_memo(FootprintState& st, const SlabView& v, cudaStream_t s) {
-  const size_t ncell = (size_t)v.rows * v.cols_total;
+// The per-call isTraversableForFilters memo of the path checks (blocked_memo_d): one byte per map cell of each of `nmaps` maps,
+// cleared on `s`.
+int reset_filter_memo(FootprintState& st, const SlabView& v, int nmaps, cudaStream_t s) {
+  const size_t ncell = (size_t)v.rows * v.cols_total * nmaps;
   if (st.memo.reserve(ncell) != cudaSuccess) { st.why = "allocating the predicate memo failed"; return TE_ERR_CUDA; }
   if (cudaMemsetAsync(st.memo.p, 0, ncell, s) != cudaSuccess) { st.why = "cudaMemsetAsync(predicate memo) failed"; return TE_ERR_CUDA; }
   return 0;
@@ -1938,10 +1965,11 @@ int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry*
   if (circles)
     if (int rc = ensure_ring_table(st, s)) return rc;
   if (clear_memo)  // one memo for both kinds of path: it depends on the layers only
-    if (int rc = reset_filter_memo(st, v, s)) return rc;
+    if (int rc = reset_filter_memo(st, v, r.nmaps, s)) return rc;
   const FpArgs a = filter_args(v, g, p, r.rough);
   const Layers L{r.trav, r.slope, r.step, r.elev, r.rough};
-  const RequestArgs R{r.footprint_begin, r.footprint_xyz, r.nvertices, r.max_footprint_vertices, r.nposes, r.area_out};
+  const RequestArgs R{r.footprint_begin, r.footprint_xyz, r.nvertices, r.max_footprint_vertices, r.nposes, r.area_out,
+                      r.path_map, r.nmaps, (long long)v.rows * v.cols_total};
   if (circles) {
     PathArgs C = path_args(st, p, r.robot_slope);
     C.npaths = r.npaths; C.pose_stride = r.pose_stride; C.path_begin = r.path_begin; C.poses = r.poses; C.radius = r.radius;

@@ -68,6 +68,11 @@ constexpr int kUntravRows = 1024;
 struct PathChecks {
   const float *trav, *slope, *step, *rough, *elev;  // isTraversableForFilters' layers; rough null unless verify_roughness
   const float* robot_slope;                          // null: no checkRobotInclination
+  // A batch of maps of one geometry (te_check_footprint_request_batched): map m's cells start m * rows * cols cells into every
+  // layer and into the memo (nmaps maps' worth, cleared once), and path q is on map path_map[q] (device memory; null: every path
+  // is on map 0).  A path on a map outside 0 .. nmaps-1 is not checked.
+  int nmaps;
+  const int* path_map;
   int npaths;
   int nposes;                     // poses in `poses`; < 0: not known (circular paths then need no pose range check)
   const int* path_begin;          // [npaths + 1]
