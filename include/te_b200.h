@@ -226,6 +226,24 @@ int te_footprint_polygon_batched(te_ctx* ctx, const te_geometry* g, const te_foo
                                  const float* step, const float* roughness_or_null, const float* elevation, float* traversability_x,
                                  float* traversability_rot, int memory);
 
+/* traversabilityFootprint(footprintYaw) at a whole list of yaws in one call: the cost of a non-circular robot at every heading a
+ * lattice / hybrid-A* planner or a sampling MPC plans over.  Layer k of map m is at offset (k*nmaps + m)*rows*cols of
+ * traversability_yaws (column-major as every layer) and equals, bit for bit, the traversability_rot that
+ * te_footprint_polygon(..., footprint_yaw = yaws[k], ...) returns for map m alone; a yaw of exactly 0.0 therefore also equals its
+ * traversability_x.  The layers take the layout and limits of te_footprint_polygon_batched: nmaps whole maps back to back,
+ * 1 <= nmaps <= 65535 (nmaps = 1: a single map), the same cell and column bounds, and a circular-buffer start index is
+ * TE_ERR_UNSUPPORTED.  polygon_xy (3..16 vertices) and yaws are HOST arrays in both memory modes: the host classifies the
+ * polygon's cells once per yaw.  Parameters from p: exactly what te_footprint_polygon uses.  1 <= nyaws <= 1024: below 1
+ * TE_ERR_BAD_ARG, above 1024 TE_ERR_UNSUPPORTED (the cap bounds the host classification and table upload per call; 1024 headings
+ * are 0.35 degrees apart).  TE_ERR_BAD_ARG for a non-finite yaw and a null yaws or output; TE_ERR_UNSUPPORTED for a polygon that
+ * reaches further than 31 cells from its centre; TE_ERR_MISSING_LAYER for verify_roughness without roughness_or_null.  The
+ * predicates run once and one kernel sweeps every yaw.  TE_MEM_HOST stages the nyaws*nmaps*cols output columns; TE_MEM_DEVICE is
+ * asynchronous on the context stream. */
+int te_footprint_polygon_yaws(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, int32_t npts,
+                              const double* polygon_xy, int32_t nyaws, const double* yaws, const float* traversability,
+                              const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                              float* traversability_yaws, int memory);
+
 /* TraversabilityMap::checkFootprintPath for circular footprints — checkCircularFootprintPath, TraversabilityMap.cpp:345-462 —
  * for a BATCH of paths in one launch (one thread per path: the service callback of the reference checks one path per call;
  * planners and MPC roll-outs ask for hundreds).  It is evaluated on a complete traversability_footprint layer, i.e. the output

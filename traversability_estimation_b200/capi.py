@@ -18,7 +18,7 @@ KERNEL_AUTO, KERNEL_GENERIC, KERNEL_FUSED = 0, 1, 2
 
 EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set_stream", "te_synchronize",
            "te_set_kernel", "te_get_stats", "te_enable_timing", "te_get_timing", "te_get_flag_counters", "te_get_escalation_stats", "te_fused_plan", "te_slope", "te_normals", "te_step", "te_roughness", "te_chain",
-           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_footprint_batched", "te_footprint_polygon_batched", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_check_footprint_paths_fresh2", "te_check_footprint_paths_polygon2", "te_check_footprint_request", "te_check_footprint_request_batched", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
+           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_footprint_batched", "te_footprint_polygon_batched", "te_footprint_polygon_yaws", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_check_footprint_paths_fresh2", "te_check_footprint_paths_polygon2", "te_check_footprint_request", "te_check_footprint_request_batched", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
            "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free", "te_map_create", "te_map_destroy",
            "te_map_chain", "te_map_set_layers", "te_map_footprint", "te_map_footprint_polygon", "te_map_check_footprint_request",
            "te_map_get_footprint", "te_map_clear_footprint", "te_map_request_stats"]
@@ -308,6 +308,20 @@ class Context:
         self._check(self._L.te_footprint_polygon_batched(self._h, C.byref(g), C.byref(fp), nmaps, len(pts), pts.ctypes.data, float(yaw),
                                                          _addr(traversability), _addr(slope), _addr(step), _addr(roughness),
                                                          _addr(elevation), _addr(out_x), _addr(out_rot), memory))
+
+    def footprint_polygon_yaws(self, g, fp, nmaps, polygon_xy, yaws, traversability, slope, step, elevation, out, memory,
+                               roughness=None):
+        """footprint_polygon()'s traversability_rot at every yaw of `yaws` (host sequence) for nmaps whole maps of geometry g stored
+        back to back (the layout of chain_batched).  `out` is (nyaws, nmaps, cols, rows) C-contiguous: out[k, m] is map m's layer
+        at yaws[k]."""
+        self._order_after_torch(memory)
+        pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
+        ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
+        self._L.te_footprint_polygon_yaws.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams), C.c_int32, C.c_int32,
+                                                      C.c_void_p, C.c_int32, C.c_void_p] + [C.c_void_p] * 6 + [C.c_int]
+        self._check(self._L.te_footprint_polygon_yaws(self._h, C.byref(g), C.byref(fp), nmaps, len(pts), pts.ctypes.data, len(ys),
+                                                      ys.ctypes.data if len(ys) else None, _addr(traversability), _addr(slope),
+                                                      _addr(step), _addr(roughness), _addr(elevation), _addr(out), memory))
 
     def check_footprint_paths(self, g, footprint_layer, traversability_default, path_begin, poses_xy, robot_slope=None):
         """Host convenience: (is_safe uint8[npaths], traversability float64[npaths]); footprint_layer is a column-major host layer;

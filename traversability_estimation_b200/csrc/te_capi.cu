@@ -864,21 +864,34 @@ int te_footprint_batched(te_ctx* c, const te_geometry* g, const te_footprint_par
   return footprint_common(c, g, nullptr, p, nmaps, trav, slope, step, rough, elev, out, slope_fp, step_fp, rough_fp, memory);
 }
 
-// te_footprint_polygon (one map or slab) and te_footprint_polygon_batched (nmaps whole maps).
+// Output of a polygon footprint entry: `count` layers of the call's maps back to back from `out`, layer k rotated by yaws[k].
+struct PolygonOutputs {
+  float* out;
+  int count;
+  const double* yaws;
+};
+
+// te_footprint_polygon (one map or slab), te_footprint_polygon_batched (nmaps whole maps) and te_footprint_polygon_yaws (nmaps
+// whole maps, a list of yaws): every layer of `outs` from one sweep.  `start_index_ok`: in host memory the staging takes a
+// circular-buffer map (whole single maps of the two-layer entries).
 static int footprint_polygon_common(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const te_footprint_params* p, int nmaps,
-                                    int32_t npts, const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step,
-                                    const float* rough, const float* elev, float* out_x, float* out_rot, int memory) {
+                                    int32_t npts, const double* pts_xy, const float* trav, const float* slope, const float* step,
+                                    const float* rough, const float* elev, int nouts, const PolygonOutputs* outs, int memory,
+                                    bool start_index_ok) {
   te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && slab == nullptr && nmaps == 1, &g0)) return rc;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && start_index_ok, &g0)) return rc;
   const te_geometry* g = &g0;
   if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
   if (npts < 3 || npts > 16 || !pts_xy) return fail(TE_ERR_BAD_ARG, "footprint polygon needs 3 to 16 vertices");
-  if (!std::isfinite(yaw)) return fail(TE_ERR_BAD_ARG, "footprint yaw is not finite");
+  for (int k = 0; k < nouts; ++k)
+    for (int y = 0; y < outs[k].count; ++y)
+      if (!std::isfinite(outs[k].yaws[y])) return fail(TE_ERR_BAD_ARG, "footprint yaw is not finite");
   for (int k = 0; k < 2 * npts; ++k)
     if (!std::isfinite(pts_xy[k])) return fail(TE_ERR_BAD_ARG, "footprint polygon vertex is not finite");
   if (int rc = check_footprint_batch(g, nmaps)) return rc;
   if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
-  if (!out_x || !out_rot) return fail(TE_ERR_BAD_ARG, "output layer is null");
+  for (int k = 0; k < nouts; ++k)
+    if (!outs[k].out) return fail(TE_ERR_BAD_ARG, "output layer is null");
   const bool use_rough = p->verify_roughness != 0;
   te_slab s;
   if (int rc = resolve_slab(g, slab, te::footprint_polygon_halo(g, p, npts, pts_xy), &s)) return rc;
@@ -887,28 +900,54 @@ static int footprint_polygon_common(te_ctx* c, const te_geometry* g_in, const te
   const int in_cols = (s.halo_left + s.col_count + s.halo_right) * nmaps, out_cols = s.col_count * nmaps;
   const float* in[5] = {st.in_layer(trav, in_cols), st.in_layer(slope, in_cols), st.in_layer(step, in_cols), st.in_layer(elev, in_cols),
                         st.in_layer(use_rough ? rough : nullptr, in_cols)};
-  float* o[2] = {st.out_layer(out_x, out_cols), st.out_layer(out_rot, out_cols)};
+  std::vector<te::PolygonLayer> layers;
+  for (int k = 0; k < nouts; ++k) {
+    if ((long long)outs[k].count * out_cols >= (1LL << 31)) return fail(TE_ERR_UNSUPPORTED, "output of 2^31 or more columns");
+    float* const o = st.out_layer(outs[k].out, outs[k].count * out_cols);  // one staging buffer for all layers of an output
+    for (int y = 0; y < outs[k].count && o; ++y) layers.push_back(te::PolygonLayer{outs[k].yaws[y], o + (size_t)y * out_cols * g->rows});
+  }
   if (st.rc) return st.rc;
   int nl = 0;
-  int rc = te::launch_footprint_polygon(c->fp, make_view(c, g, s), g, p, npts, pts_xy, yaw, in[0], in[1], in[2], in[4], in[3], o[0], o[1],
-                                        nmaps, c->sms, c->stream, &nl);
+  int rc = te::launch_footprint_polygon(c->fp, make_view(c, g, s), g, p, npts, pts_xy, (int)layers.size(), layers.data(), in[0], in[1], in[2],
+                                        in[4], in[3], nmaps, c->sms, c->stream, &nl);
   if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", c->fp.why.c_str());
   if (int r2 = launch_check(c, "polygon footprint", nl)) return r2;
   return st.finish();
+}
+
+// traversability_x is the footprint at yaw 0: the rotation of yaw 0 is the identity, exactly (te::launch_footprint_polygon).
+static int footprint_polygon_pair(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, int nmaps,
+                                  int32_t npts, const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step,
+                                  const float* rough, const float* elev, float* out_x, float* out_rot, int memory) {
+  static const double identity = 0.0;
+  const PolygonOutputs outs[2] = {{out_x, 1, &identity}, {out_rot, 1, &yaw}};
+  return footprint_polygon_common(c, g, slab, p, nmaps, npts, pts_xy, trav, slope, step, rough, elev, 2, outs, memory,
+                                  slab == nullptr && nmaps == 1);
 }
 
 int te_footprint_polygon(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, int32_t npts,
                          const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step, const float* rough,
                          const float* elev, float* out_x, float* out_rot, int memory) {
   TE_ENTER(c);
-  return footprint_polygon_common(c, g, slab, p, 1, npts, pts_xy, yaw, trav, slope, step, rough, elev, out_x, out_rot, memory);
+  return footprint_polygon_pair(c, g, slab, p, 1, npts, pts_xy, yaw, trav, slope, step, rough, elev, out_x, out_rot, memory);
 }
 
 int te_footprint_polygon_batched(te_ctx* c, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, int32_t npts,
                                  const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step,
                                  const float* rough, const float* elev, float* out_x, float* out_rot, int memory) {
   TE_ENTER(c);
-  return footprint_polygon_common(c, g, nullptr, p, nmaps, npts, pts_xy, yaw, trav, slope, step, rough, elev, out_x, out_rot, memory);
+  return footprint_polygon_pair(c, g, nullptr, p, nmaps, npts, pts_xy, yaw, trav, slope, step, rough, elev, out_x, out_rot, memory);
+}
+
+int te_footprint_polygon_yaws(te_ctx* c, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, int32_t npts,
+                              const double* pts_xy, int32_t nyaws, const double* yaws, const float* trav, const float* slope,
+                              const float* step, const float* rough, const float* elev, float* out, int memory) {
+  TE_ENTER(c);
+  if (nyaws < 1 || !yaws) return fail(TE_ERR_BAD_ARG, "footprint yaws: need 1 or more");
+  if (nyaws > 1024) return fail(TE_ERR_UNSUPPORTED, "%d footprint yaws: at most 1024 per call", nyaws);
+  if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
+  const PolygonOutputs outs[1] = {{out, nyaws, yaws}};
+  return footprint_polygon_common(c, g, nullptr, p, nmaps, npts, pts_xy, trav, slope, step, rough, elev, 1, outs, memory, false);
 }
 
 int te_footprint(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, const float* trav,
@@ -1407,8 +1446,10 @@ int te_map_footprint_polygon(te_map* m, const te_footprint_params* p, int32_t np
   const te_slab s{0, g->cols, 0, 0};
   const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
   int nl = 0;
-  int rc = te::launch_footprint_polygon(m->fp, make_view(c, g, s), g, p, npts, pts_xy, yaw, (const float*)m->trav.p, (const float*)m->slope.p,
-                                        (const float*)m->step.p, rough, (const float*)m->elev.p, o[0], o[1], 1, c->sms, c->stream, &nl);
+  const te::PolygonLayer layers[2] = {{0.0, o[0]}, {yaw, o[1]}};  // traversability_x: yaw 0, the identity
+  int rc = te::launch_footprint_polygon(m->fp, make_view(c, g, s), g, p, npts, pts_xy, 2, layers, (const float*)m->trav.p,
+                                        (const float*)m->slope.p, (const float*)m->step.p, rough, (const float*)m->elev.p, 1, c->sms,
+                                        c->stream, &nl);
   if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", m->fp.why.c_str());
   if (int r2 = launch_check(c, "map polygon footprint", nl)) return r2;
   return st.finish();

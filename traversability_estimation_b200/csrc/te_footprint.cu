@@ -588,34 +588,50 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
 // polygon fails isTraversableForFilters, otherwise the mean of t' over the polygon's cells (traversabilityDefault_ when it covers
 // none).  The set of cells inside the polygon is the same offset pattern for every centre EXCEPT for offsets whose cell centre lies
 // on (within rounding of) an edge: grid_map::Polygon::isInside decides those on absolute double coordinates, differently from
-// centre to centre.  The host classifies the offsets once (launch_footprint_polygon): certain-in cells become per-column runs that
-// are summed from the tile's prefix sums; the few uncertain offsets are decided per centre with the reference's own arithmetic —
-// cooperatively when the decision does not depend on the centre's row (an edge parallel to the x axis through cell centres: the
-// YAML footprint at 0.02 m has 92 such offsets), 32 offsets per warp pass.
+// centre to centre.  The host classifies the offsets once per polygon (launch_footprint_polygon): certain-in cells become per-column
+// runs that are summed from the tile's prefix sums; the few uncertain offsets are decided per centre with the reference's own
+// arithmetic — cooperatively when the decision does not depend on the centre's row (an edge parallel to the x axis through cell
+// centres: the YAML footprint at 0.02 m has 92 such offsets), 32 offsets per warp pass.  One launch sweeps a list of polygons (the
+// footprint at several yaws): a block stages its tile once and sweeps a group of them.
 constexpr int PTR = 64, PTC = 16;  // tile of centres: rows x columns
 constexpr int PMAXV = 16;          // polygon vertices
 constexpr int PB = 130;            // pitch of a staged blocked-count column (uint16)
+// Eigen::Quaternion::toRotationMatrix of (cos(yaw/2), 0, 0, sin(yaw/2)), upper-left 2 x 2
+struct Rot2 {
+  double r00, r01, r10, r11;
+};
+// One polygon of a sweep: the footprint placed with rotation R, its slices of the call's run and uncertain-offset tables, and its
+// output layer (map m's starts m * rows * out_ncols cells into `out`).
+struct PolyDesc {
+  Rot2 R;
+  int run0, nruns;    // runs[run0 .. run0 + nruns)
+  int fz0, nfz;       // fz[fz0 .. fz0 + nfz)
+  int ncert;          // number of certain cells (sum of the run lengths)
+  float* out;
+};
 struct PolyArgs {
-  int Lp;             // reach of the polygon in cells (<= 31)
-  int nruns, nfz, npts;
+  int Lp;             // reach of the polygon in cells (<= 31), the same at every rotation
+  int npts;
+  int npoly;          // polygons of the launch
+  int group;          // polygons per block: blockIdx.x = g * row_tiles + row tile sweeps polygons g * group .. (g + 1) * group - 1
+  int row_tiles;
+  const PolyDesc* desc;  // [npoly]
   const int* runs;    // (dj & 0xff) | (lo & 0xff) << 8 | (hi & 0xff) << 16: rows i+lo .. i+hi of column j+dj are certainly inside
   const int* fz;      // (di & 0xff) | (dj & 0xff) << 8 | flags << 16: uncertain offsets, sorted by (dj, di); flag bit 0: the decision
                       // depends on the centre's row; bit 1: same column as the previous entry, next row, neither depends on the row
-  int ncert;          // number of certain cells (sum of the run lengths)
-  double r00, r01, r10, r11;  // Eigen::Quaternion::toRotationMatrix of (cos(yaw/2), 0, 0, sin(yaw/2)), upper-left 2 x 2
   double px[PMAXV], py[PMAXV];
 };
 
 // grid_map::Polygon::isInside for the polygon placed at (cx, cy): vertices = R * p + centre in the operand order of Eigen's
 // Transform * vector (oracle: teo_footprint_polygon), crossing-number test over (v[i], v[i-1]).
-__device__ bool poly_inside_d(const PolyArgs& Q, double cx, double cy, double ptx, double pty) {
+__device__ bool poly_inside_d(const PolyArgs& Q, const Rot2& R, double cx, double cy, double ptx, double pty) {
   int cross = 0;
   const int last = Q.npts - 1;
-  double jx = cx + ((Q.r00 * Q.px[last] + Q.r01 * Q.py[last]) + 0.0);
-  double jy = cy + ((Q.r10 * Q.px[last] + Q.r11 * Q.py[last]) + 0.0);
+  double jx = cx + ((R.r00 * Q.px[last] + R.r01 * Q.py[last]) + 0.0);
+  double jy = cy + ((R.r10 * Q.px[last] + R.r11 * Q.py[last]) + 0.0);
   for (int k = 0; k < Q.npts; ++k) {
-    const double ix = cx + ((Q.r00 * Q.px[k] + Q.r01 * Q.py[k]) + 0.0);
-    const double iy = cy + ((Q.r10 * Q.px[k] + Q.r11 * Q.py[k]) + 0.0);
+    const double ix = cx + ((R.r00 * Q.px[k] + R.r01 * Q.py[k]) + 0.0);
+    const double iy = cy + ((R.r10 * Q.px[k] + R.r11 * Q.py[k]) + 0.0);
     if (((iy > pty) != (jy > pty)) && (ptx < (jx - ix) * (pty - iy) / (jy - iy) + ix)) ++cross;
     jx = ix;
     jy = iy;
@@ -623,14 +639,16 @@ __device__ bool poly_inside_d(const PolyArgs& Q, double cx, double cy, double pt
   return (cross & 1) != 0;
 }
 
-__global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const float* __restrict__ trav, const unsigned char* __restrict__ blocked,
-                                                   float* __restrict__ out) {
+// The tile geometry (PTR x PTC centres, staging origin r0 - Lp, c0 - Lp) is part of the results: a sum over a run is a difference
+// of the staged prefix sums, whose float32 rounding depends on where the staged column starts.
+__global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const float* __restrict__ trav, const unsigned char* __restrict__ blocked) {
   extern __shared__ double sP[];  // [NC][PS] prefix sums of t'; then [NC][PB] uint16 prefix counts of blocked cells
   const int Lr = Q.Lp, NR = PTR + 2 * Lr, NC = PTC + 2 * Lr, PS = NR + 1;
   unsigned short* sB = reinterpret_cast<unsigned short*>(sP + (size_t)NC * PS);
   // map blockIdx.z of the batch: its input-buffer columns start mb columns into the batch's, its output columns mbo
   const int mb = (int)blockIdx.z * A.in_ncols, mbo = (int)blockIdx.z * A.out_ncols;
-  const int r0 = (int)blockIdx.x * PTR, c0 = A.out_col0 + (int)blockIdx.y * PTC;
+  const int tile_r = (int)blockIdx.x % Q.row_tiles, p0 = ((int)blockIdx.x / Q.row_tiles) * Q.group, p1 = min(p0 + Q.group, Q.npoly);
+  const int r0 = tile_r * PTR, c0 = A.out_col0 + (int)blockIdx.y * PTC;
   const int rb = r0 - Lr, cb = c0 - Lr;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // ---- phase 1: prefix sums of t' and of the blocked flags, one warp per staged column.  NR <= 4 * 32 (Lp <= 31): a lane takes
@@ -681,7 +699,8 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
     }
   }
   const bool tile_any = __syncthreads_or(anyb) != 0;
-  // ---- phase 2: a warp is 32 consecutive rows of one column at a time (4 columns per warp)
+  // ---- phase 2: a warp is 32 consecutive rows of one column at a time (4 columns per warp), each centre swept for every polygon
+  //      of the block's group
   const int i = r0 + (warp & 1) * 32 + lane;
   const int i0 = i - lane;
   if (i0 >= A.rows) return;
@@ -693,90 +712,96 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
     const int j = c0 + (warp >> 1) * (PTC / 4) + q;
     if (j >= A.out_col0 + A.out_ncols) break;
     const double cy = A.Y[j];
-    double t = 0.0;
-    int n = 0, nblk = 0;
     // certain cells: per-column runs from the prefix sums (cells outside the map were staged as t' = 0, not blocked)
     const double* pbase = sP + (size_t)(j - cb) * PS + k0;
     const unsigned short* bbase = sB + (size_t)(j - cb) * PB + k0;
     const bool interior = ic - Lr >= 0 && ic + Lr < A.rows && j - Lr >= max(0, A.in_col0) && j + Lr <= min(A.cols_total, A.in_col0 + A.in_ncols) - 1;
-    if (interior) {  // no clipping anywhere: the cell count is the table's
-      for (int r = 0; r < Q.nruns; ++r) {
-        const int w = __ldg(Q.runs + r);
-        const int dj = (int)(signed char)(w & 0xff), lo = (int)(signed char)((w >> 8) & 0xff), hi = (int)(signed char)((w >> 16) & 0xff);
-        const double* pc = pbase + dj * PS;
-        t += pc[hi + 1] - pc[lo];
-        if (tile_any) {
-          const unsigned short* bc = bbase + dj * PB;
-          nblk += (int)bc[hi + 1] - (int)bc[lo];
+    for (int y = p0; y < p1; ++y) {
+      const PolyDesc& D = Q.desc[y];
+      const Rot2 R = D.R;
+      const int* const runs = Q.runs + D.run0;
+      const int* const fz = Q.fz + D.fz0;
+      const int nruns = D.nruns, nfz = D.nfz;
+      double t = 0.0;
+      int n = 0, nblk = 0;
+      if (interior) {  // no clipping anywhere: the cell count is the table's
+        for (int r = 0; r < nruns; ++r) {
+          const int w = __ldg(runs + r);
+          const int dj = (int)(signed char)(w & 0xff), lo = (int)(signed char)((w >> 8) & 0xff), hi = (int)(signed char)((w >> 16) & 0xff);
+          const double* pc = pbase + dj * PS;
+          t += pc[hi + 1] - pc[lo];
+          if (tile_any) {
+            const unsigned short* bc = bbase + dj * PB;
+            nblk += (int)bc[hi + 1] - (int)bc[lo];
+          }
+        }
+        n = D.ncert;
+      } else {
+        for (int r = 0; r < nruns; ++r) {
+          const int w = __ldg(runs + r);
+          const int dj = (int)(signed char)(w & 0xff), lo = (int)(signed char)((w >> 8) & 0xff), hi = (int)(signed char)((w >> 16) & 0xff);
+          const int b = j + dj, lb = b - A.in_col0;
+          if (b < 0 || b >= A.cols_total || lb < 0 || lb >= A.in_ncols) continue;
+          const int a0 = max(ic + lo, 0), a1 = min(ic + hi, A.rows - 1);
+          if (a0 > a1) continue;
+          const double* pc = pbase + dj * PS;
+          t += pc[hi + 1] - pc[lo];
+          n += a1 - a0 + 1;
+          if (tile_any) {
+            const unsigned short* bc = bbase + dj * PB;
+            nblk += (int)bc[hi + 1] - (int)bc[lo];
+          }
         }
       }
-      n = Q.ncert;
-    } else {
-      for (int r = 0; r < Q.nruns; ++r) {
-        const int w = __ldg(Q.runs + r);
-        const int dj = (int)(signed char)(w & 0xff), lo = (int)(signed char)((w >> 8) & 0xff), hi = (int)(signed char)((w >> 16) & 0xff);
-        const int b = j + dj, lb = b - A.in_col0;
-        if (b < 0 || b >= A.cols_total || lb < 0 || lb >= A.in_ncols) continue;
-        const int a0 = max(ic + lo, 0), a1 = min(ic + hi, A.rows - 1);
-        if (a0 > a1) continue;
-        const double* pc = pbase + dj * PS;
-        t += pc[hi + 1] - pc[lo];
-        n += a1 - a0 + 1;
-        if (tile_any) {
-          const unsigned short* bc = bbase + dj * PB;
-          nblk += (int)bc[hi + 1] - (int)bc[lo];
+      // uncertain offsets, 32 per pass: lane l decides offset base + l when the decision is the same for every row of the column; the
+      // offsets that came out inside and follow each other down a column are then summed as ONE run from the prefix sums
+      for (int base = 0; base < nfz; base += 32) {
+        const int idx = base + lane;
+        int w = 0;
+        bool cand = false;
+        if (idx < nfz) {
+          w = __ldg(fz + idx);
+          const int di = (int)(signed char)(w & 0xff), dj = (int)(signed char)((w >> 8) & 0xff);
+          if ((w >> 16) & 1) {
+            cand = true;  // depends on the row: every lane decides for itself below
+          } else {
+            const int a = ic + di, b = j + dj;
+            // the decision does not depend on the row, so any row's coordinates will do — but they must exist
+            const int ar = min(max(a, 0), A.rows - 1), icr = ar - di;
+            if (b >= 0 && b < A.cols_total && icr >= 0 && icr < A.rows) cand = poly_inside_d(Q, R, A.X[icr], cy, A.X[ar], A.Y[b]);
+          }
+        }
+        unsigned m = __ballot_sync(0xffffffffu, cand);
+        const unsigned ext = m & __ballot_sync(0xffffffffu, ((w >> 17) & 1) != 0);  // inside AND continues its predecessor down the column
+        while (m) {
+          const int src = __ffs((int)m) - 1;
+          const unsigned tail = src == 31 ? 0u : (ext >> (src + 1));
+          const int len = __ffs((int)~tail) - 1;  // further entries of the run (0..31 - src)
+          m &= ~((len >= 31 ? 0xffffffffu : ((2u << len) - 1u)) << src);
+          const int wv = __shfl_sync(0xffffffffu, w, src);
+          const int di = (int)(signed char)(wv & 0xff), dj = (int)(signed char)((wv >> 8) & 0xff);
+          const int b = j + dj, lb = b - A.in_col0;
+          if (b < 0 || b >= A.cols_total || lb < 0 || lb >= A.in_ncols) continue;
+          const int a0 = ic + di, a1 = a0 + len;
+          const int a0c = max(a0, 0), a1c = min(a1, A.rows - 1);
+          if (a0c > a1c) continue;
+          if (((wv >> 16) & 1) && !poly_inside_d(Q, R, cx, cy, A.X[a0], A.Y[b])) continue;  // row-dependent entries never chain (len == 0)
+          const int cc = b - cb;
+          const double* pc = sP + (size_t)cc * PS + (a0 - rb);
+          t += pc[len + 1] - pc[0];
+          n += a1c - a0c + 1;
+          if (tile_any) {
+            const unsigned short* bc = sB + (size_t)cc * PB + (a0 - rb);
+            nblk += (int)bc[len + 1] - (int)bc[0];
+          }
         }
       }
+      float result;
+      if (nblk > 0) result = 0.0f;                       // :297 / :301
+      else if (n == 0) result = (float)A.tdefault;       // :625-628
+      else result = (float)(t / (double)n);              // :630
+      if (active) D.out[(size_t)(mbo + j - A.out_col0) * A.rows + i] = result;
     }
-    // uncertain offsets, 32 per pass: lane l decides offset base + l when the decision is the same for every row of the column; the
-    // offsets that came out inside and follow each other down a column are then summed as ONE run from the prefix sums
-    for (int base = 0; base < Q.nfz; base += 32) {
-      const int idx = base + lane;
-      int w = 0;
-      bool cand = false;
-      if (idx < Q.nfz) {
-        w = __ldg(Q.fz + idx);
-        const int di = (int)(signed char)(w & 0xff), dj = (int)(signed char)((w >> 8) & 0xff);
-        if ((w >> 16) & 1) {
-          cand = true;  // depends on the row: every lane decides for itself below
-        } else {
-          const int a = ic + di, b = j + dj;
-          // the decision does not depend on the row, so any row's coordinates will do — but they must exist
-          const int ar = min(max(a, 0), A.rows - 1), icr = ar - di;
-          if (b >= 0 && b < A.cols_total && icr >= 0 && icr < A.rows) cand = poly_inside_d(Q, A.X[icr], cy, A.X[ar], A.Y[b]);
-        }
-      }
-      unsigned m = __ballot_sync(0xffffffffu, cand);
-      const unsigned ext = m & __ballot_sync(0xffffffffu, ((w >> 17) & 1) != 0);  // inside AND continues its predecessor down the column
-      while (m) {
-        const int src = __ffs((int)m) - 1;
-        const unsigned tail = src == 31 ? 0u : (ext >> (src + 1));
-        const int len = __ffs((int)~tail) - 1;  // further entries of the run (0..31 - src)
-        m &= ~((len >= 31 ? 0xffffffffu : ((2u << len) - 1u)) << src);
-        const int wv = __shfl_sync(0xffffffffu, w, src);
-        const int di = (int)(signed char)(wv & 0xff), dj = (int)(signed char)((wv >> 8) & 0xff);
-        const int b = j + dj, lb = b - A.in_col0;
-        if (b < 0 || b >= A.cols_total || lb < 0 || lb >= A.in_ncols) continue;
-        const int a0 = ic + di, a1 = a0 + len;
-        const int a0c = max(a0, 0), a1c = min(a1, A.rows - 1);
-        if (a0c > a1c) continue;
-        if (((wv >> 16) & 1) && !poly_inside_d(Q, cx, cy, A.X[a0], A.Y[b])) continue;  // row-dependent entries never chain (len == 0)
-        const int cc = b - cb;
-        const double* pc = sP + (size_t)cc * PS + (a0 - rb);
-        t += pc[len + 1] - pc[0];
-        n += a1c - a0c + 1;
-        if (tile_any) {
-          const unsigned short* bc = sB + (size_t)cc * PB + (a0 - rb);
-          nblk += (int)bc[len + 1] - (int)bc[0];
-        }
-      }
-    }
-    if (!active) continue;
-    float result;
-    if (nblk > 0) result = 0.0f;                       // :297 / :301
-    else if (n == 0) result = (float)A.tdefault;       // :625-628
-    else result = (float)(t / (double)n);              // :630
-    out[(size_t)(mbo + j - A.out_col0) * A.rows + i] = result;
   }
 }
 
@@ -1836,7 +1861,7 @@ std::vector<int> build_spiral(double radius, double res) {
 }  // namespace
 
 void FootprintState::release() {
-  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly[0], &poly[1], &rings, &memo, &items, &upoly, &mapbuf}) b->release();
+  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly, &rings, &memo, &items, &upoly, &mapbuf}) b->release();
   tables_valid = false;
   valid = false;
 }
@@ -2472,18 +2497,69 @@ bool classify_polygon(double res, int Lp, int npts, const double* px, const doub
   }
   return true;
 }
+
+// Eigen::Quaternion::toRotationMatrix of AngleAxisd(yaw, UnitZ) = (w, 0, 0, z) = (cos(yaw/2), 0, 0, sin(yaw/2)), upper-left 2 x 2,
+// in Eigen's operation order.  Yaw 0 gives w = 1, z = 0 exactly: the identity that traversability_x uses.
+Rot2 yaw_rotation(double yaw) {
+  const double w = std::cos(0.5 * yaw), z = std::sin(0.5 * yaw);
+  const double tz = 2.0 * z, twz = tz * w, tzz = tz * z;
+  return Rot2{1.0 - (0.0 + tzz), 0.0 - twz, 0.0 + twz, 1.0 - (0.0 + tzz)};
+}
+
+// Yaw groups of a k_poly_tile launch: a block sweeps a group of consecutive polygons of its tile.  Tiles alone fill an H100 from
+// 4 * sms of them (at the largest reach two blocks are resident per SM: two waves); fewer tiles split the polygons into as many
+// groups as bring the launch to 4 * sms blocks, at most one per polygon.  A group restages its tile, so larger groups save
+// staging; which block sweeps a layer never changes its bits.
+int polygon_groups(long long tiles, int npoly, int sms) {
+  const long long want = std::max(1LL, (4LL * sms + tiles - 1) / tiles);
+  return (int)std::min<long long>(npoly, want);
+}
 }  // namespace
 
-// traversabilityFootprint(yaw): predicates once, then one tiled launch per polygon (unrotated -> out_x, rotated -> out_rot).
+// traversabilityFootprint(yaw) for every layer of `polys`: predicates once, the polygon tables of every rotation in one upload,
+// then one k_poly_tile launch for all of them.
 int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int npts,
-                             const double* pts_xy, double yaw, const float* trav, const float* slope, const float* step,
-                             const float* rough, const float* elev, float* out_x, float* out_rot, int nmaps, int sms, cudaStream_t s,
-                             int* launches) {
+                             const double* pts_xy, int npoly, const PolygonLayer* polys, const float* trav, const float* slope,
+                             const float* step, const float* rough, const float* elev, int nmaps, int sms, cudaStream_t s, int* launches) {
   if (npts < 3 || npts > PMAXV) { st.why = "footprint polygon needs 3 to 16 vertices"; return TE_ERR_UNSUPPORTED; }
+  if (npoly < 1) { st.why = "no polygon layer to sweep"; return TE_ERR_UNSUPPORTED; }
   const int Lp = polygon_reach(g, npts, pts_xy);
   if (Lp > 31) { st.why = "footprint polygon reaches further than 31 cells from its centre"; return TE_ERR_UNSUPPORTED; }
+  PolyArgs q{};
+  q.Lp = Lp; q.npts = npts; q.npoly = npoly;
+  for (int k = 0; k < npts; ++k) { q.px[k] = pts_xy[2 * k]; q.py[k] = pts_xy[2 * k + 1]; }
+  // the call's table: npoly descriptors, then the runs of every polygon, then their uncertain offsets
+  std::vector<PolyDesc> desc(npoly);
+  std::vector<int> runs, fz;
+  {
+    PolyTables tb;
+    for (int k = 0; k < npoly; ++k) {
+      PolyDesc& d = desc[k];
+      d.R = yaw_rotation(polys[k].yaw);
+      const double R[4] = {d.R.r00, d.R.r01, d.R.r10, d.R.r11};
+      if (!classify_polygon(g->resolution, Lp, npts, q.px, q.py, R, &tb, &st.why)) return TE_ERR_UNSUPPORTED;
+      d.run0 = (int)runs.size(); d.nruns = (int)tb.runs.size();
+      d.fz0 = (int)fz.size(); d.nfz = (int)tb.fz.size();
+      d.ncert = 0;
+      for (int rw : tb.runs) d.ncert += (int)(signed char)((rw >> 16) & 0xff) - (int)(signed char)((rw >> 8) & 0xff) + 1;
+      d.out = polys[k].out;
+      runs.insert(runs.end(), tb.runs.begin(), tb.runs.end());
+      fz.insert(fz.end(), tb.fz.begin(), tb.fz.end());
+    }
+  }
+  const size_t dbytes = sizeof(PolyDesc) * desc.size(), bytes = dbytes + sizeof(int) * (runs.size() + fz.size());
+  std::vector<char> blob(bytes);
+  std::memcpy(blob.data(), desc.data(), dbytes);
+  if (!runs.empty()) std::memcpy(blob.data() + dbytes, runs.data(), sizeof(int) * runs.size());
+  if (!fz.empty()) std::memcpy(blob.data() + dbytes + sizeof(int) * runs.size(), fz.data(), sizeof(int) * fz.size());
   FpArgs a{};
   if (int rc = run_predicates(st, v, g, p, nmaps, trav, slope, step, rough, elev, nullptr, nullptr, nullptr, sms, s, &a)) return rc;
+  if (st.poly.p && st.poly.cap < bytes) cudaStreamSynchronize(s);  // kernels of an earlier call may still read the old tables
+  if (st.poly.reserve(bytes) != cudaSuccess) { st.why = "allocating the polygon tables failed"; return TE_ERR_CUDA; }
+  if (cudaMemcpyAsync(st.poly.p, blob.data(), bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) { st.why = "polygon table upload failed"; return TE_ERR_CUDA; }
+  q.desc = (const PolyDesc*)st.poly.p;
+  q.runs = (const int*)((const char*)st.poly.p + dbytes);
+  q.fz = q.runs + runs.size();
   const size_t smem = sizeof(double) * (size_t)(PTC + 2 * Lp) * (PTR + 2 * Lp + 1) + (size_t)(PTC + 2 * Lp) * (PB * 2);
   if (!st.poly_attr) {
     const size_t smax = sizeof(double) * (size_t)(PTC + 62) * (PTR + 63) + (size_t)(PTC + 62) * (PB * 2);
@@ -2492,32 +2568,13 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
     }
     st.poly_attr = true;
   }
-  int nl = 2;
-  for (int which = 0; which < 2; ++which) {
-    PolyArgs q{};
-    q.Lp = Lp; q.npts = npts;
-    const double w = which ? std::cos(0.5 * yaw) : 1.0, z = which ? std::sin(0.5 * yaw) : 0.0;
-    const double tz = 2.0 * z, twz = tz * w, tzz = tz * z;
-    q.r00 = 1.0 - (0.0 + tzz); q.r01 = 0.0 - twz; q.r10 = 0.0 + twz; q.r11 = 1.0 - (0.0 + tzz);
-    for (int k = 0; k < npts; ++k) { q.px[k] = pts_xy[2 * k]; q.py[k] = pts_xy[2 * k + 1]; }
-    const double R[4] = {q.r00, q.r01, q.r10, q.r11};
-    PolyTables tb;
-    if (!classify_polygon(g->resolution, Lp, npts, q.px, q.py, R, &tb, &st.why)) return TE_ERR_UNSUPPORTED;
-    const size_t bytes = sizeof(int) * (tb.runs.size() + tb.fz.size() + 2);
-    DevBuf& d = st.poly[which];
-    if (d.p && d.cap < bytes) cudaStreamSynchronize(s);  // kernels of an earlier call may still read the old tables
-    if (d.reserve(bytes) != cudaSuccess) { st.why = "allocating the polygon tables failed"; return TE_ERR_CUDA; }
-    int* dr = (int*)d.p;
-    int* df = dr + tb.runs.size() + 1;
-    if (!tb.runs.empty() && cudaMemcpyAsync(dr, tb.runs.data(), sizeof(int) * tb.runs.size(), cudaMemcpyHostToDevice, s) != cudaSuccess) { st.why = "polygon table upload failed"; return TE_ERR_CUDA; }
-    if (!tb.fz.empty() && cudaMemcpyAsync(df, tb.fz.data(), sizeof(int) * tb.fz.size(), cudaMemcpyHostToDevice, s) != cudaSuccess) { st.why = "polygon table upload failed"; return TE_ERR_CUDA; }
-    q.runs = dr; q.fz = df; q.nruns = (int)tb.runs.size(); q.nfz = (int)tb.fz.size();
-    q.ncert = 0;
-    for (int rw : tb.runs) q.ncert += (int)(signed char)((rw >> 16) & 0xff) - (int)(signed char)((rw >> 8) & 0xff) + 1;
-    k_poly_tile<<<dim3((unsigned)((v.rows + PTR - 1) / PTR), (unsigned)((v.out_ncols + PTC - 1) / PTC), (unsigned)nmaps), 256, smem, s>>>(
-        a, q, trav, (const unsigned char*)st.block.p, which ? out_rot : out_x);
-  }
-  if (launches) *launches = 2 + nl;
+  q.row_tiles = (v.rows + PTR - 1) / PTR;
+  const int col_tiles = (v.out_ncols + PTC - 1) / PTC;
+  const int ngroups = polygon_groups((long long)q.row_tiles * col_tiles * nmaps, npoly, sms);
+  q.group = (npoly + ngroups - 1) / ngroups;
+  const int nblocks_x = q.row_tiles * ((npoly + q.group - 1) / q.group);
+  k_poly_tile<<<dim3((unsigned)nblocks_x, (unsigned)col_tiles, (unsigned)nmaps), 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p);
+  if (launches) *launches = 3;
   return 0;
 }
 
