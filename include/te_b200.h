@@ -244,6 +244,21 @@ int te_footprint_polygon_yaws(te_ctx* ctx, const te_geometry* g, const te_footpr
                               const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
                               float* traversability_yaws, int memory);
 
+/* Per-cell reductions of te_footprint_polygon_yaws over its yaws, without the stack: the worst heading (can the robot turn on the
+ * spot here? 0 as soon as any heading is blocked) and the best heading with its index (a hybrid-A* heuristic, a heading-free cost
+ * map).  With v_k the value te_footprint_polygon_yaws writes for yaws[k] at a cell of map m:
+ *   worst[m, cell] = v_j for the first j that minimises v_k over k;
+ *   best[m, cell] = v_k and best_yaw[m, cell] = k (int32) for the first k that maximises v_k.
+ * Comparisons are IEEE; a tie goes to the lower heading index, whose value bits are returned (-0.0 and +0.0 are not reordered).
+ * Each output is one layer per map, map m at offset m*rows*cols, or NULL when not wanted.  The reduction runs inside the sweep:
+ * device memory holds three layers, not nyaws.  Arguments, layout, limits and errors are those of te_footprint_polygon_yaws, plus
+ * TE_ERR_BAD_ARG when all three outputs are NULL or p->traversability_default is not finite (with a finite default every v_k is
+ * finite).  TE_MEM_HOST stages only the requested outputs; TE_MEM_DEVICE is asynchronous on the context stream. */
+int te_footprint_polygon_yaws_reduce(te_ctx* ctx, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, int32_t npts,
+                                     const double* polygon_xy, int32_t nyaws, const double* yaws, const float* traversability,
+                                     const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                                     float* worst_or_null, float* best_or_null, int32_t* best_yaw_or_null, int memory);
+
 /* TraversabilityMap::checkFootprintPath for circular footprints — checkCircularFootprintPath, TraversabilityMap.cpp:345-462 —
  * for a BATCH of paths in one launch (one thread per path: the service callback of the reference checks one path per call;
  * planners and MPC roll-outs ask for hundreds).  It is evaluated on a complete traversability_footprint layer, i.e. the output
@@ -482,6 +497,19 @@ int te_map_footprint(te_map* map, const te_footprint_params* p, float* traversab
 /* traversabilityFootprint(yaw) (:239-305): te_footprint_polygon on the map's layers.  Reads and changes no cache. */
 int te_map_footprint_polygon(te_map* map, const te_footprint_params* p, int32_t npts, const double* polygon_xy, double footprint_yaw,
                              float* traversability_x, float* traversability_rot, int memory);
+
+/* te_footprint_polygon_yaws on the map's layers: layer k (at k*rows*cols) is the traversability_rot of yaws[k].  Yaws, limits and
+ * errors as te_footprint_polygon_yaws; the map's start index is fine.  Reads and changes no cache.  In host memory every layer is
+ * re-wrapped to the map's start index, as te_map's other outputs; in device memory the layers are in the map's default (unwrapped)
+ * order, as te_map_footprint_polygon's. */
+int te_map_footprint_polygon_yaws(te_map* map, const te_footprint_params* p, int32_t npts, const double* polygon_xy, int32_t nyaws,
+                                  const double* yaws, float* traversability_yaws, int memory);
+
+/* te_footprint_polygon_yaws_reduce on the map's layers: one layer each, NULL when not wanted.  Outputs, errors and memory order as
+ * te_map_footprint_polygon_yaws (best_yaw is re-wrapped as the float layers are).  Reads and changes no cache. */
+int te_map_footprint_polygon_yaws_reduce(te_map* map, const te_footprint_params* p, int32_t npts, const double* polygon_xy,
+                                         int32_t nyaws, const double* yaws, float* worst_or_null, float* best_or_null,
+                                         int32_t* best_yaw_or_null, int memory);
 
 /* A CheckFootprintPath request on the map, as the reference service loop answers it (TraversabilityEstimation.cpp:278-295, with
  * publishPolygons = true).  Arguments, outputs, conventions, limits and errors are those of te_check_footprint_request, with the

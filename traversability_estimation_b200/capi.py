@@ -18,9 +18,10 @@ KERNEL_AUTO, KERNEL_GENERIC, KERNEL_FUSED = 0, 1, 2
 
 EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set_stream", "te_synchronize",
            "te_set_kernel", "te_get_stats", "te_enable_timing", "te_get_timing", "te_get_flag_counters", "te_get_escalation_stats", "te_fused_plan", "te_slope", "te_normals", "te_step", "te_roughness", "te_chain",
-           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_footprint_batched", "te_footprint_polygon_batched", "te_footprint_polygon_yaws", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_check_footprint_paths_fresh2", "te_check_footprint_paths_polygon2", "te_check_footprint_request", "te_check_footprint_request_batched", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
+           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_footprint_batched", "te_footprint_polygon_batched", "te_footprint_polygon_yaws", "te_footprint_polygon_yaws_reduce", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_check_footprint_paths_fresh2", "te_check_footprint_paths_polygon2", "te_check_footprint_request", "te_check_footprint_request_batched", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
            "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free", "te_map_create", "te_map_destroy",
-           "te_map_chain", "te_map_set_layers", "te_map_footprint", "te_map_footprint_polygon", "te_map_check_footprint_request",
+           "te_map_chain", "te_map_set_layers", "te_map_footprint", "te_map_footprint_polygon", "te_map_footprint_polygon_yaws", "te_map_footprint_polygon_yaws_reduce",
+           "te_map_check_footprint_request",
            "te_map_get_footprint", "te_map_clear_footprint", "te_map_request_stats"]
 
 
@@ -322,6 +323,21 @@ class Context:
         self._check(self._L.te_footprint_polygon_yaws(self._h, C.byref(g), C.byref(fp), nmaps, len(pts), pts.ctypes.data, len(ys),
                                                       ys.ctypes.data if len(ys) else None, _addr(traversability), _addr(slope),
                                                       _addr(step), _addr(roughness), _addr(elevation), _addr(out), memory))
+
+    def footprint_polygon_yaws_reduce(self, g, fp, nmaps, polygon_xy, yaws, traversability, slope, step, elevation, worst, best,
+                                      best_yaw, memory, roughness=None):
+        """Per-cell reductions of footprint_polygon_yaws over `yaws` without the stack: worst is the value of the first heading
+        that minimises it, best that of the first that maximises it, best_yaw (int32) that heading's index.  Each output is
+        (nmaps, cols, rows) C-contiguous, or None when not wanted (not all three)."""
+        self._order_after_torch(memory)
+        pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
+        ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
+        self._L.te_footprint_polygon_yaws_reduce.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams), C.c_int32,
+                                                             C.c_int32, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_void_p] * 8 + [C.c_int]
+        self._check(self._L.te_footprint_polygon_yaws_reduce(self._h, C.byref(g), C.byref(fp), nmaps, len(pts), pts.ctypes.data, len(ys),
+                                                             ys.ctypes.data if len(ys) else None, _addr(traversability), _addr(slope),
+                                                             _addr(step), _addr(roughness), _addr(elevation), _addr(worst), _addr(best),
+                                                             _addr(best_yaw), memory))
 
     def check_footprint_paths(self, g, footprint_layer, traversability_default, path_begin, poses_xy, robot_slope=None):
         """Host convenience: (is_safe uint8[npaths], traversability float64[npaths]); footprint_layer is a column-major host layer;
@@ -670,6 +686,29 @@ class Map:
         orot = np.empty(self._shape(), dtype=np.float32, order="F")
         self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, float(yaw), _addr(ox), _addr(orot), MEM_HOST))
         return ox, orot
+
+    def footprint_polygon_yaws(self, fp, polygon_xy, yaws):
+        """te_map_footprint_polygon_yaws: (nyaws, rows, cols), layer k the traversability_rot at yaws[k] of the map's layers."""
+        fn = self._L.te_map_footprint_polygon_yaws
+        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
+        pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
+        ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
+        out = np.empty((len(ys), self._g.cols, self._g.rows), dtype=np.float32)   # layer k column-major at k * rows * cols
+        self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data if len(ys) else None, _addr(out),
+                       MEM_HOST))
+        return out.transpose(0, 2, 1)
+
+    def footprint_polygon_yaws_reduce(self, fp, polygon_xy, yaws):
+        """te_map_footprint_polygon_yaws_reduce: (worst, best, best_yaw) over `yaws` of the map's layers, each (rows, cols)."""
+        fn = self._L.te_map_footprint_polygon_yaws_reduce
+        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_void_p] * 3 + [C.c_int]
+        pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
+        ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
+        worst, best = (np.empty(self._shape(), dtype=np.float32, order="F") for _ in range(2))
+        best_yaw = np.empty(self._shape(), dtype=np.int32, order="F")
+        self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data if len(ys) else None, _addr(worst),
+                       _addr(best), _addr(best_yaw), MEM_HOST))
+        return worst, best, best_yaw
 
     def check_footprint_request(self, fp, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices=None,
                                 conservative=None, compute_untraversable_polygon=None, untraversable_capacity=None):

@@ -297,7 +297,8 @@ struct Staging {
   int rows, cols, sr, sc;
   int rc = TE_OK;
   int used = 0;
-  struct Out { void* host; const void* dev; size_t bytes; int ncols; };  // ncols > 0: a layer of that many columns
+  // ncols > 0: nlayers layers of that many columns back to back (4-byte cells: float32, or int32 copied as they are)
+  struct Out { void* host; const void* dev; size_t bytes; int ncols, nlayers; };
   Out outs[sizeof(te_ctx::stage) / sizeof(DevBuf)];
   int nout = 0;
 
@@ -334,23 +335,34 @@ struct Staging {
     if (d && n) check(cudaMemcpyAsync(d, h, sizeof(T) * n, cudaMemcpyHostToDevice, c->stream), "upload");
     return d;
   }
-  // An output layer of `ncols` columns / an output array of `n` elements; null stays null.
-  float* out_layer(float* h, int ncols) { return (float*)record(h, layer_bytes(ncols), ncols); }
+  // `nlayers` output layers of `ncols` columns in one staging buffer / an output array of `n` elements; null stays null.
   template <class T>
-  T* out(T* h, size_t n) { return (T*)record(h, sizeof(T) * n, 0); }
-  void* record(void* h, size_t bytes, int ncols) {
+  T* out_layer(T* h, int ncols, int nlayers = 1) {
+    static_assert(sizeof(T) == sizeof(float), "layers have 4-byte cells");
+    return (T*)record(h, layer_bytes(ncols) * nlayers, ncols, nlayers);
+  }
+  template <class T>
+  T* out(T* h, size_t n) { return (T*)record(h, sizeof(T) * n, 0, 0); }
+  void* record(void* h, size_t bytes, int ncols, int nlayers) {
     if (!host || !h) return h;
     void* d = slot(bytes);
-    if (d) outs[nout++] = Out{h, d, bytes, ncols};
+    if (d) outs[nout++] = Out{h, d, bytes, ncols, nlayers};
     return d;
   }
   int finish() {
     if (!host || rc != TE_OK) return rc;
     for (int k = 0; k < nout; ++k) {
       const Out& o = outs[k];
-      check(o.ncols ? download_cols((float*)o.host, (const float*)o.dev, rows, cols, sr, sc, 0, o.ncols, c->stream)
-                    : cudaMemcpyAsync(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost, c->stream),
-            "download");
+      if (!o.ncols) {
+        check(cudaMemcpyAsync(o.host, o.dev, o.bytes, cudaMemcpyDeviceToHost, c->stream), "download");
+      } else if (sr == 0 && sc == 0) {  // default order: the layers are one run of columns
+        check(download_cols((float*)o.host, (const float*)o.dev, rows, cols, 0, 0, 0, o.ncols * o.nlayers, c->stream), "download");
+      } else {  // a start index wraps the columns of one map: re-wrap each layer on its own
+        for (int l = 0; l < o.nlayers; ++l) {
+          const size_t off = (size_t)l * rows * o.ncols;
+          check(download_cols((float*)o.host + off, (const float*)o.dev + off, rows, cols, sr, sc, 0, o.ncols, c->stream), "download");
+        }
+      }
     }
     check(cudaStreamSynchronize(c->stream), "cudaStreamSynchronize");
     return rc;
@@ -871,15 +883,18 @@ struct PolygonOutputs {
   const double* yaws;
 };
 
-// te_footprint_polygon (one map or slab), te_footprint_polygon_batched (nmaps whole maps) and te_footprint_polygon_yaws (nmaps
-// whole maps, a list of yaws): every layer of `outs` from one sweep.  `start_index_ok`: in host memory the staging takes a
-// circular-buffer map (whole single maps of the two-layer entries).
-static int footprint_polygon_common(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const te_footprint_params* p, int nmaps,
-                                    int32_t npts, const double* pts_xy, const float* trav, const float* slope, const float* step,
-                                    const float* rough, const float* elev, int nouts, const PolygonOutputs* outs, int memory,
-                                    bool start_index_ok) {
+// te_footprint_polygon (one map or slab), te_footprint_polygon_batched (nmaps whole maps), te_footprint_polygon_yaws(_reduce) (nmaps
+// whole maps, a list of yaws) and the te_map polygon entries: every layer of `outs` from one sweep or, with `reduce` (HOST or
+// device pointers as `memory` says), the reductions over the yaws of its one output, whose `out` is then unused.  `start_index_ok`:
+// in host memory the staging takes a circular-buffer map (whole single maps).  `resident`: the layers are a te_map's, on the device
+// in default order, swept with the map's own state; they are never staged, and a start index is then fine in either memory (device
+// outputs are in default order).
+static int footprint_polygon_common(te_ctx* c, te::FootprintState* resident, const te_geometry* g_in, const te_slab* slab,
+                                    const te_footprint_params* p, int nmaps, int32_t npts, const double* pts_xy, const float* trav,
+                                    const float* slope, const float* step, const float* rough, const float* elev, int nouts,
+                                    const PolygonOutputs* outs, const te::PolygonReduce* reduce, int memory, bool start_index_ok) {
   te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && start_index_ok, &g0)) return rc;
+  if (int rc = unwrap_geometry(g_in, resident || (memory == TE_MEM_HOST && start_index_ok), &g0)) return rc;
   const te_geometry* g = &g0;
   if (!p) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
   if (npts < 3 || npts > 16 || !pts_xy) return fail(TE_ERR_BAD_ARG, "footprint polygon needs 3 to 16 vertices");
@@ -888,29 +903,36 @@ static int footprint_polygon_common(te_ctx* c, const te_geometry* g_in, const te
       if (!std::isfinite(outs[k].yaws[y])) return fail(TE_ERR_BAD_ARG, "footprint yaw is not finite");
   for (int k = 0; k < 2 * npts; ++k)
     if (!std::isfinite(pts_xy[k])) return fail(TE_ERR_BAD_ARG, "footprint polygon vertex is not finite");
+  // with a finite default every value is finite, so the reductions need no NaN rule
+  if (reduce && !std::isfinite(p->traversability_default)) return fail(TE_ERR_BAD_ARG, "traversability_default is not finite (reductions over yaws)");
   if (int rc = check_footprint_batch(g, nmaps)) return rc;
   if (int rc = check_filter_layers(p, trav, slope, step, elev, rough)) return rc;
   for (int k = 0; k < nouts; ++k)
-    if (!outs[k].out) return fail(TE_ERR_BAD_ARG, "output layer is null");
+    if (!outs[k].out && !reduce) return fail(TE_ERR_BAD_ARG, "output layer is null");
   const bool use_rough = p->verify_roughness != 0;
   te_slab s;
   if (int rc = resolve_slab(g, slab, te::footprint_polygon_halo(g, p, npts, pts_xy), &s)) return rc;
   if (int rc = ensure_geometry(c, g)) return rc;
   Staging st(c, memory == TE_MEM_HOST, g_in);
   const int in_cols = (s.halo_left + s.col_count + s.halo_right) * nmaps, out_cols = s.col_count * nmaps;
-  const float* in[5] = {st.in_layer(trav, in_cols), st.in_layer(slope, in_cols), st.in_layer(step, in_cols), st.in_layer(elev, in_cols),
-                        st.in_layer(use_rough ? rough : nullptr, in_cols)};
+  const float* in[5] = {trav, slope, step, elev, use_rough ? rough : nullptr};
+  if (!resident)
+    for (const float*& l : in) l = st.in_layer(l, in_cols);
   std::vector<te::PolygonLayer> layers;
   for (int k = 0; k < nouts; ++k) {
     if ((long long)outs[k].count * out_cols >= (1LL << 31)) return fail(TE_ERR_UNSUPPORTED, "output of 2^31 or more columns");
-    float* const o = st.out_layer(outs[k].out, outs[k].count * out_cols);  // one staging buffer for all layers of an output
-    for (int y = 0; y < outs[k].count && o; ++y) layers.push_back(te::PolygonLayer{outs[k].yaws[y], o + (size_t)y * out_cols * g->rows});
+    float* const o = reduce ? nullptr : st.out_layer(outs[k].out, out_cols, outs[k].count);  // one staging buffer for all layers
+    for (int y = 0; y < outs[k].count; ++y)
+      layers.push_back(te::PolygonLayer{outs[k].yaws[y], o ? o + (size_t)y * out_cols * g->rows : nullptr});
   }
+  te::PolygonReduce red{};
+  if (reduce) red = {st.out_layer(reduce->worst, out_cols), st.out_layer(reduce->best, out_cols), st.out_layer(reduce->best_yaw, out_cols)};
   if (st.rc) return st.rc;
+  te::FootprintState& fp = resident ? *resident : c->fp;
   int nl = 0;
-  int rc = te::launch_footprint_polygon(c->fp, make_view(c, g, s), g, p, npts, pts_xy, (int)layers.size(), layers.data(), in[0], in[1], in[2],
-                                        in[4], in[3], nmaps, c->sms, c->stream, &nl);
-  if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", c->fp.why.c_str());
+  int rc = te::launch_footprint_polygon(fp, make_view(c, g, s), g, p, npts, pts_xy, (int)layers.size(), layers.data(), reduce ? &red : nullptr,
+                                        in[0], in[1], in[2], in[4], in[3], nmaps, c->sms, c->stream, &nl);
+  if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", fp.why.c_str());
   if (int r2 = launch_check(c, "polygon footprint", nl)) return r2;
   return st.finish();
 }
@@ -921,7 +943,7 @@ static int footprint_polygon_pair(te_ctx* c, const te_geometry* g, const te_slab
                                   const float* rough, const float* elev, float* out_x, float* out_rot, int memory) {
   static const double identity = 0.0;
   const PolygonOutputs outs[2] = {{out_x, 1, &identity}, {out_rot, 1, &yaw}};
-  return footprint_polygon_common(c, g, slab, p, nmaps, npts, pts_xy, trav, slope, step, rough, elev, 2, outs, memory,
+  return footprint_polygon_common(c, nullptr, g, slab, p, nmaps, npts, pts_xy, trav, slope, step, rough, elev, 2, outs, nullptr, memory,
                                   slab == nullptr && nmaps == 1);
 }
 
@@ -939,15 +961,40 @@ int te_footprint_polygon_batched(te_ctx* c, const te_geometry* g, const te_footp
   return footprint_polygon_pair(c, g, nullptr, p, nmaps, npts, pts_xy, yaw, trav, slope, step, rough, elev, out_x, out_rot, memory);
 }
 
+// The list of yaws of the yaws entries (the cap bounds the host classification and the table upload of one call).
+static int check_yaws(int32_t nyaws, const double* yaws) {
+  if (nyaws < 1 || !yaws) return fail(TE_ERR_BAD_ARG, "footprint yaws: need 1 or more");
+  if (nyaws > 1024) return fail(TE_ERR_UNSUPPORTED, "%d footprint yaws: at most 1024 per call", nyaws);
+  return TE_OK;
+}
+
+static int check_reduce_outputs(const te::PolygonReduce& r) {
+  if (!r.worst && !r.best && !r.best_yaw) return fail(TE_ERR_BAD_ARG, "no output: worst, best and best_yaw are all null");
+  return TE_OK;
+}
+
 int te_footprint_polygon_yaws(te_ctx* c, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, int32_t npts,
                               const double* pts_xy, int32_t nyaws, const double* yaws, const float* trav, const float* slope,
                               const float* step, const float* rough, const float* elev, float* out, int memory) {
   TE_ENTER(c);
-  if (nyaws < 1 || !yaws) return fail(TE_ERR_BAD_ARG, "footprint yaws: need 1 or more");
-  if (nyaws > 1024) return fail(TE_ERR_UNSUPPORTED, "%d footprint yaws: at most 1024 per call", nyaws);
+  if (int rc = check_yaws(nyaws, yaws)) return rc;
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
   const PolygonOutputs outs[1] = {{out, nyaws, yaws}};
-  return footprint_polygon_common(c, g, nullptr, p, nmaps, npts, pts_xy, trav, slope, step, rough, elev, 1, outs, memory, false);
+  return footprint_polygon_common(c, nullptr, g, nullptr, p, nmaps, npts, pts_xy, trav, slope, step, rough, elev, 1, outs, nullptr, memory,
+                                  false);
+}
+
+int te_footprint_polygon_yaws_reduce(te_ctx* c, const te_geometry* g, const te_footprint_params* p, int32_t nmaps, int32_t npts,
+                                     const double* pts_xy, int32_t nyaws, const double* yaws, const float* trav, const float* slope,
+                                     const float* step, const float* rough, const float* elev, float* worst, float* best,
+                                     int32_t* best_yaw, int memory) {
+  TE_ENTER(c);
+  if (int rc = check_yaws(nyaws, yaws)) return rc;
+  const te::PolygonReduce red{worst, best, best_yaw};
+  if (int rc = check_reduce_outputs(red)) return rc;
+  const PolygonOutputs outs[1] = {{nullptr, nyaws, yaws}};
+  return footprint_polygon_common(c, nullptr, g, nullptr, p, nmaps, npts, pts_xy, trav, slope, step, rough, elev, 1, outs, &red, memory,
+                                  false);
 }
 
 int te_footprint(te_ctx* c, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, const float* trav,
@@ -1428,31 +1475,42 @@ int te_map_footprint(te_map* m, const te_footprint_params* p, float* out, int me
   return TE_OK;
 }
 
+// The te_map polygon entries: footprint_polygon_common on the map's resident layers with the map's own state.  They neither read
+// nor change the traversability_footprint cache or the memo.
+static int map_footprint_polygon(te_map* m, const te_footprint_params* p, int32_t npts, const double* pts_xy, int nouts,
+                                 const PolygonOutputs* outs, const te::PolygonReduce* reduce, int memory) {
+  if (int rc = map_ready(m)) return rc;
+  if (int rc = map_footprint_params(m, p)) return rc;
+  return footprint_polygon_common(m->ctx, &m->fp, &m->geo_in, nullptr, p, 1, npts, pts_xy, (const float*)m->trav.p, (const float*)m->slope.p,
+                                  (const float*)m->step.p, m->have_rough ? (const float*)m->rough.p : nullptr, (const float*)m->elev.p,
+                                  nouts, outs, reduce, memory, true);
+}
+
 int te_map_footprint_polygon(te_map* m, const te_footprint_params* p, int32_t npts, const double* pts_xy, double yaw, float* out_x,
                              float* out_rot, int memory) {
   TE_MAP_ENTER(m);
-  if (int rc = map_ready(m)) return rc;
-  if (int rc = map_footprint_params(m, p)) return rc;
-  if (npts < 3 || npts > 16 || !pts_xy) return fail(TE_ERR_BAD_ARG, "footprint polygon needs 3 to 16 vertices");
-  if (!std::isfinite(yaw)) return fail(TE_ERR_BAD_ARG, "footprint yaw is not finite");
-  for (int k = 0; k < 2 * npts; ++k)
-    if (!std::isfinite(pts_xy[k])) return fail(TE_ERR_BAD_ARG, "footprint polygon vertex is not finite");
-  if (!out_x || !out_rot) return fail(TE_ERR_BAD_ARG, "output layer is null");
-  const te_geometry* g = &m->geo;
-  if (int rc = ensure_geometry(c, g)) return rc;
-  Staging st(c, memory == TE_MEM_HOST, &m->geo_in);
-  float* o[2] = {st.out_layer(out_x, g->cols), st.out_layer(out_rot, g->cols)};
-  if (st.rc) return st.rc;
-  const te_slab s{0, g->cols, 0, 0};
-  const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
-  int nl = 0;
-  const te::PolygonLayer layers[2] = {{0.0, o[0]}, {yaw, o[1]}};  // traversability_x: yaw 0, the identity
-  int rc = te::launch_footprint_polygon(m->fp, make_view(c, g, s), g, p, npts, pts_xy, 2, layers, (const float*)m->trav.p,
-                                        (const float*)m->slope.p, (const float*)m->step.p, rough, (const float*)m->elev.p, 1, c->sms,
-                                        c->stream, &nl);
-  if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", m->fp.why.c_str());
-  if (int r2 = launch_check(c, "map polygon footprint", nl)) return r2;
-  return st.finish();
+  static const double identity = 0.0;  // traversability_x: yaw 0, the identity
+  const PolygonOutputs outs[2] = {{out_x, 1, &identity}, {out_rot, 1, &yaw}};
+  return map_footprint_polygon(m, p, npts, pts_xy, 2, outs, nullptr, memory);
+}
+
+int te_map_footprint_polygon_yaws(te_map* m, const te_footprint_params* p, int32_t npts, const double* pts_xy, int32_t nyaws,
+                                  const double* yaws, float* out, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = check_yaws(nyaws, yaws)) return rc;
+  if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
+  const PolygonOutputs outs[1] = {{out, nyaws, yaws}};
+  return map_footprint_polygon(m, p, npts, pts_xy, 1, outs, nullptr, memory);
+}
+
+int te_map_footprint_polygon_yaws_reduce(te_map* m, const te_footprint_params* p, int32_t npts, const double* pts_xy, int32_t nyaws,
+                                         const double* yaws, float* worst, float* best, int32_t* best_yaw, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = check_yaws(nyaws, yaws)) return rc;
+  const te::PolygonReduce red{worst, best, best_yaw};
+  if (int rc = check_reduce_outputs(red)) return rc;
+  const PolygonOutputs outs[1] = {{nullptr, nyaws, yaws}};
+  return map_footprint_polygon(m, p, npts, pts_xy, 1, outs, &red, memory);
 }
 
 int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int32_t npaths, int32_t nposes, const int32_t* path_begin,

@@ -619,6 +619,13 @@ struct PolyArgs {
   const int* runs;    // (dj & 0xff) | (lo & 0xff) << 8 | (hi & 0xff) << 16: rows i+lo .. i+hi of column j+dj are certainly inside
   const int* fz;      // (di & 0xff) | (dj & 0xff) << 8 | flags << 16: uncertain offsets, sorted by (dj, di); flag bit 0: the decision
                       // depends on the centre's row; bit 1: same column as the previous entry, next row, neither depends on the row
+  // Reduce mode (k_poly_tile<true>; the descriptors' `out` is unused): per centre, the value of the first polygon of the block's
+  // group that minimises it (worst), of the first that maximises it (best) and that polygon's index (best_yaw); each null when not
+  // wanted.  Group g writes at g * rstride cells (0 without a split; a split leaves the folding to k_poly_combine).
+  float* worst;
+  float* best;
+  int* best_yaw;
+  size_t rstride;
   double px[PMAXV], py[PMAXV];
 };
 
@@ -640,7 +647,9 @@ __device__ bool poly_inside_d(const PolyArgs& Q, const Rot2& R, double cx, doubl
 }
 
 // The tile geometry (PTR x PTC centres, staging origin r0 - Lp, c0 - Lp) is part of the results: a sum over a run is a difference
-// of the staged prefix sums, whose float32 rounding depends on where the staged column starts.
+// of the staged prefix sums, whose float32 rounding depends on where the staged column starts.  kReduce: reduce over the block's
+// polygons in registers instead of storing a layer per polygon (PolyArgs::worst / best / best_yaw).
+template <bool kReduce>
 __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const float* __restrict__ trav, const unsigned char* __restrict__ blocked) {
   extern __shared__ double sP[];  // [NC][PS] prefix sums of t'; then [NC][PB] uint16 prefix counts of blocked cells
   const int Lr = Q.Lp, NR = PTR + 2 * Lr, NC = PTC + 2 * Lr, PS = NR + 1;
@@ -716,6 +725,10 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
     const double* pbase = sP + (size_t)(j - cb) * PS + k0;
     const unsigned short* bbase = sB + (size_t)(j - cb) * PB + k0;
     const bool interior = ic - Lr >= 0 && ic + Lr < A.rows && j - Lr >= max(0, A.in_col0) && j + Lr <= min(A.cols_total, A.in_col0 + A.in_ncols) - 1;
+    // reduce mode: every value is finite (the callers reject a non-finite traversability_default), so the infinities lose to the
+    // first polygon, and strict comparisons keep the earliest polygon of a tie with its own bits (-0.0 and +0.0 included)
+    float worst = __int_as_float(0x7f800000), best = __int_as_float(0xff800000);
+    int best_y = p0;
     for (int y = p0; y < p1; ++y) {
       const PolyDesc& D = Q.desc[y];
       const Rot2 R = D.R;
@@ -800,7 +813,47 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
       if (nblk > 0) result = 0.0f;                       // :297 / :301
       else if (n == 0) result = (float)A.tdefault;       // :625-628
       else result = (float)(t / (double)n);              // :630
-      if (active) D.out[(size_t)(mbo + j - A.out_col0) * A.rows + i] = result;
+      if constexpr (kReduce) {
+        if (result < worst) worst = result;
+        if (result > best) { best = result; best_y = y; }
+      } else {
+        if (active) D.out[(size_t)(mbo + j - A.out_col0) * A.rows + i] = result;
+      }
+    }
+    if constexpr (kReduce) {
+      if (active) {
+        const size_t o = (size_t)(p0 / Q.group) * Q.rstride + (size_t)(mbo + j - A.out_col0) * A.rows + i;
+        if (Q.worst) Q.worst[o] = worst;
+        if (Q.best) Q.best[o] = best;
+        if (Q.best_yaw) Q.best_yaw[o] = best_y;
+      }
+    }
+  }
+}
+
+// Reduce mode after a yaw-group split: k_poly_tile left group g's partial reduction at g * n cells of each scratch array (sw: worst,
+// sb: best, sk: best_yaw; sb is there when best or best_yaw is wanted).  The groups are runs of consecutive polygons in order, so
+// folding them in group order with the same strict comparisons gives the first minimum / maximum over all polygons.
+__global__ void k_poly_combine(const float* __restrict__ sw, const float* __restrict__ sb, const int* __restrict__ sk, int ngroups, size_t n,
+                               float* worst, float* best, int* best_yaw) {
+  for (size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x; c < n; c += (size_t)gridDim.x * blockDim.x) {
+    if (worst) {
+      float w = sw[c];
+      for (int g = 1; g < ngroups; ++g) {
+        const float v = sw[(size_t)g * n + c];
+        if (v < w) w = v;
+      }
+      worst[c] = w;
+    }
+    if (sb) {
+      float b = sb[c];
+      int k = sk ? sk[c] : 0;
+      for (int g = 1; g < ngroups; ++g) {
+        const float v = sb[(size_t)g * n + c];
+        if (v > b) { b = v; if (sk) k = sk[(size_t)g * n + c]; }
+      }
+      if (best) best[c] = b;
+      if (best_yaw) best_yaw[c] = k;
     }
   }
 }
@@ -1861,7 +1914,7 @@ std::vector<int> build_spiral(double radius, double res) {
 }  // namespace
 
 void FootprintState::release() {
-  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly, &rings, &memo, &items, &upoly, &mapbuf}) b->release();
+  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly, &reduce, &rings, &memo, &items, &upoly, &mapbuf}) b->release();
   tables_valid = false;
   valid = false;
 }
@@ -2517,12 +2570,14 @@ int polygon_groups(long long tiles, int npoly, int sms) {
 }  // namespace
 
 // traversabilityFootprint(yaw) for every layer of `polys`: predicates once, the polygon tables of every rotation in one upload,
-// then one k_poly_tile launch for all of them.
+// then one k_poly_tile launch for all of them (and, in reduce mode with yaw groups, one k_poly_combine).
 int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int npts,
-                             const double* pts_xy, int npoly, const PolygonLayer* polys, const float* trav, const float* slope,
-                             const float* step, const float* rough, const float* elev, int nmaps, int sms, cudaStream_t s, int* launches) {
+                             const double* pts_xy, int npoly, const PolygonLayer* polys, const PolygonReduce* reduce, const float* trav,
+                             const float* slope, const float* step, const float* rough, const float* elev, int nmaps, int sms,
+                             cudaStream_t s, int* launches) {
   if (npts < 3 || npts > PMAXV) { st.why = "footprint polygon needs 3 to 16 vertices"; return TE_ERR_UNSUPPORTED; }
   if (npoly < 1) { st.why = "no polygon layer to sweep"; return TE_ERR_UNSUPPORTED; }
+  if (reduce && !reduce->worst && !reduce->best && !reduce->best_yaw) { st.why = "no reduction output"; return TE_ERR_UNSUPPORTED; }
   const int Lp = polygon_reach(g, npts, pts_xy);
   if (Lp > 31) { st.why = "footprint polygon reaches further than 31 cells from its centre"; return TE_ERR_UNSUPPORTED; }
   PolyArgs q{};
@@ -2563,7 +2618,8 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
   const size_t smem = sizeof(double) * (size_t)(PTC + 2 * Lp) * (PTR + 2 * Lp + 1) + (size_t)(PTC + 2 * Lp) * (PB * 2);
   if (!st.poly_attr) {
     const size_t smax = sizeof(double) * (size_t)(PTC + 62) * (PTR + 63) + (size_t)(PTC + 62) * (PB * 2);
-    if (cudaFuncSetAttribute(k_poly_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess) {
+    if (cudaFuncSetAttribute(k_poly_tile<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
+        cudaFuncSetAttribute(k_poly_tile<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess) {
       st.why = "cudaFuncSetAttribute(max dynamic shared memory) failed"; return TE_ERR_CUDA;
     }
     st.poly_attr = true;
@@ -2572,9 +2628,36 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
   const int col_tiles = (v.out_ncols + PTC - 1) / PTC;
   const int ngroups = polygon_groups((long long)q.row_tiles * col_tiles * nmaps, npoly, sms);
   q.group = (npoly + ngroups - 1) / ngroups;
-  const int nblocks_x = q.row_tiles * ((npoly + q.group - 1) / q.group);
-  k_poly_tile<<<dim3((unsigned)nblocks_x, (unsigned)col_tiles, (unsigned)nmaps), 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p);
-  if (launches) *launches = 3;
+  const int nsplit = (npoly + q.group - 1) / q.group;  // groups actually launched
+  const int nblocks_x = q.row_tiles * nsplit;
+  const dim3 grid((unsigned)nblocks_x, (unsigned)col_tiles, (unsigned)nmaps);
+  if (!reduce) {
+    k_poly_tile<false><<<grid, 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p);
+    if (launches) *launches = 3;
+    return 0;
+  }
+  // Reduce mode.  Without a split the sweep writes the outputs.  With one, each group writes its partial results to st.reduce:
+  // the split only happens below 4 * sms tiles, so that is under (4 * sms + tiles) * PTR * PTC cells per array.
+  const size_t n = (size_t)nmaps * v.out_ncols * v.rows;
+  if (nsplit == 1) {
+    q.worst = reduce->worst; q.best = reduce->best; q.best_yaw = reduce->best_yaw;
+    k_poly_tile<true><<<grid, 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p);
+    if (launches) *launches = 3;
+    return 0;
+  }
+  const bool want_best = reduce->best || reduce->best_yaw;
+  const size_t per = (size_t)nsplit * n, sbytes = sizeof(float) * per * ((reduce->worst ? 1 : 0) + (want_best ? 1 : 0) + (reduce->best_yaw ? 1 : 0));
+  if (st.reduce.p && st.reduce.cap < sbytes) cudaStreamSynchronize(s);  // kernels of an earlier call may still use the old scratch
+  if (st.reduce.reserve(sbytes) != cudaSuccess) { st.why = "allocating the reduction scratch failed"; return TE_ERR_CUDA; }
+  float* next = (float*)st.reduce.p;
+  if (reduce->worst) { q.worst = next; next += per; }
+  if (want_best) { q.best = next; next += per; }
+  if (reduce->best_yaw) q.best_yaw = (int*)next;
+  q.rstride = n;
+  k_poly_tile<true><<<grid, 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p);
+  const int cblocks = (int)std::min<size_t>((n + 255) / 256, (size_t)sms * 8);
+  k_poly_combine<<<cblocks, 256, 0, s>>>(q.worst, q.best, q.best_yaw, nsplit, n, reduce->worst, reduce->best, reduce->best_yaw);
+  if (launches) *launches = 4;
   return 0;
 }
 

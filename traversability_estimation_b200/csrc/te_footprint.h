@@ -28,6 +28,7 @@ struct FootprintState {
   DevBuf list;    // work list of the cells whose predicates need the window / gap-walk code (word 0: length)
   DevBuf poly;    // polygon sweep: per-polygon descriptors, then the run / uncertain-offset tables of every polygon of the call
   bool poly_attr = false;
+  DevBuf reduce;  // polygon sweep in reduce mode with yaw groups: every group's partial worst / best / best_yaw of every cell
   DevBuf rings;   // fresh path checks: ring starts + SpiralIterator visit order of rings 0..127 (built once)
   DevBuf memo;    // fresh and polygonal path checks: per-cell isTraversableForFilters memo of one call
   DevBuf items;   // polygonal path checks: one result record per pose index
@@ -53,10 +54,21 @@ struct PolygonLayer {
   double yaw;
   float* out;
 };
+// Reduce mode: instead of one layer per polygon, per cell the value of the first polygon that minimises it (worst), of the first
+// that maximises it (best) and that polygon's index in `polys` (best_yaw); each null when not wanted, not all three.  Device
+// pointers laid out as a layer; the polygons' `out` is unused.  Needs a finite traversability_default.  The reduction runs in the
+// sweep; when the launch splits the polygons into yaw groups, the groups' partial results go to st.reduce and one more kernel
+// folds them.
+struct PolygonReduce {
+  float* worst;
+  float* best;
+  int* best_yaw;
+};
 int footprint_polygon_halo(const te_geometry* g, const te_footprint_params* p, int npts, const double* pts_xy);
 int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int npts,
-                             const double* pts_xy, int npoly, const PolygonLayer* polys, const float* trav, const float* slope,
-                             const float* step, const float* rough, const float* elev, int nmaps, int sms, cudaStream_t s, int* launches);
+                             const double* pts_xy, int npoly, const PolygonLayer* polys, const PolygonReduce* reduce, const float* trav,
+                             const float* slope, const float* step, const float* rough, const float* elev, int nmaps, int sms,
+                             cudaStream_t s, int* launches);
 
 // TraversabilityMap::checkCircularFootprintPath for a batch of paths on a complete traversability_footprint layer (device pointers).
 void launch_check_paths(const SlabView& v, const te_geometry* g, double traversability_default, const float* footprint, const float* robot_slope, int npaths,
