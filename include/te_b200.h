@@ -538,6 +538,63 @@ int te_map_clear_footprint(te_map* map);
  * circles among them (each is walked once on the device), out[2] cache cells the request stored.  No reference counterpart. */
 int te_map_request_stats(te_map* map, int64_t out[3]);
 
+/* ---- The read side of a te_map: the layers the reference node publishes and serves ----------------------------------------
+ * The layers, as bits of a mask; an output that holds several has them back to back in this order. */
+typedef enum te_layer {
+  TE_LAYER_TRAVERSABILITY = 1 << 0,
+  TE_LAYER_SLOPE = 1 << 1,      /* traversability_slope */
+  TE_LAYER_STEP = 1 << 2,       /* traversability_step */
+  TE_LAYER_ROUGHNESS = 1 << 3,  /* traversability_roughness: te_map_chain, or te_map_set_layers with one */
+  TE_LAYER_ELEVATION = 1 << 4,
+  TE_LAYER_ROBOT_SLOPE = 1 << 5,  /* te_map_set_layers with one */
+  TE_LAYER_FOOTPRINT = 1 << 6,  /* traversability_footprint: the cache (NaN = empty) */
+  TE_LAYER_ALL = 0x7f
+} te_layer;
+
+/* One window of GridMap::getSubmap(position, length, isSuccess) (TraversabilityEstimation.cpp:305, getSubmapInformation; SURVEY.md
+ * A.1, recalled from grid_map 1.6.x).  The submap is the block [top_row, top_row + rows) x [top_col, top_col + cols) of the map in
+ * default (unwrapped) order, with start index 0: a circular-buffer start index changes no field.  requested_row / requested_col
+ * is the requested position's index in the submap (indexInSubmap).  A failed window (success 0: isSuccess false, e.g. a position
+ * outside the map) has every field 0 but offset, as getSubmap returns an empty map.  offset: floats before the window's layers in
+ * te_map_get_submaps's output (te_submap_geometry: with one layer per window); a failed window takes no space. */
+typedef struct te_submap_info {
+  int32_t success;
+  int32_t rows, cols;
+  int32_t top_row, top_col;
+  int32_t requested_row, requested_col;
+  int32_t reserved;
+  double length_x, length_y;
+  double position_x, position_y;
+  int64_t offset;
+} te_submap_info;
+
+/* The submap geometry of n windows (position_xy, length_xy: n (x, y) pairs each) on the map `g`.  Host arithmetic, no GPU needed.
+ * TE_ERR_BAD_ARG for a negative or non-finite length or position (the reference does not check them: a negative length makes
+ * blocks of negative size), before any record is written. */
+int te_submap_geometry(const te_geometry* g, int32_t n, const double* position_xy, const double* length_xy, te_submap_info* info);
+
+/* publishTraversabilityMap (TraversabilityMap.cpp:172-186): the layers of `layer_mask` (te_layer bits), each rows x cols, back to
+ * back in bit order.  In host memory each is re-wrapped to the map's start index, as te_map's other outputs, and the call returns
+ * synchronised; in device memory they are in the map's default (unwrapped) order, asynchronously.  TE_ERR_MISSING_LAYER for a
+ * layer the map does not hold (roughness after te_map_set_layers without it, robot_slope after te_map_chain); TE_ERR_BAD_ARG
+ * for an empty mask or unknown bits. */
+int te_map_get_layers(te_map* map, uint32_t layer_mask, float* out, int memory);
+
+/* The get_traversability_map service (TraversabilityEstimation.cpp:297-316) for nwin windows in one call: info[k] as
+ * te_submap_geometry gives it, and window k's layers of `layer_mask` from out + info[k].offset on, in bit order, each
+ * rows_k x cols_k column-major with start index 0, as getSubmap returns them.  position_xy, length_xy and info are host arrays;
+ * `out` is in `memory` (host: returns synchronised; device: asynchronous on the context stream).  When the windows take more
+ * than out_capacity floats the call fills info, writes nothing else and returns TE_ERR_BAD_ARG: the total is the last record's
+ * offset plus its layers, so the caller can call again with more room.  One kernel launch for all windows and layers (none when
+ * every window fails).  Layer errors as te_map_get_layers; window errors as te_submap_geometry. */
+int te_map_get_submaps(te_map* map, int32_t nwin, const double* position_xy, const double* length_xy, uint32_t layer_mask,
+                       te_submap_info* info, float* out, int64_t out_capacity, int memory);
+
+/* mapHasValidTraversabilityAt (TraversabilityMap.cpp:971-983) for n positions (xy: n (x, y) pairs): valid[q] = 1 when getIndex
+ * finds the position in the map and traversability is finite there, else 0.  xy and valid are in `memory`; device memory is
+ * asynchronous on the context stream. */
+int te_map_valid_at(te_map* map, int32_t n, const double* xy, uint8_t* valid, int memory);
+
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the
  * neighbours' boundary columns of the INPUT layer(s) into this rank's halo.  The reference has no counterpart (it is a

@@ -22,10 +22,45 @@ EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set
            "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free", "te_map_create", "te_map_destroy",
            "te_map_chain", "te_map_set_layers", "te_map_footprint", "te_map_footprint_polygon", "te_map_footprint_polygon_yaws", "te_map_footprint_polygon_yaws_reduce",
            "te_map_check_footprint_request",
-           "te_map_get_footprint", "te_map_clear_footprint", "te_map_request_stats"]
+           "te_map_get_footprint", "te_map_clear_footprint", "te_map_request_stats", "te_submap_geometry", "te_map_get_layers",
+           "te_map_get_submaps", "te_map_valid_at"]
 
 
 IPC_HANDLE_BYTES = 80  # TE_IPC_HANDLE_BYTES
+
+# te_layer: bit k of a layer mask is LAYERS[k]; outputs that hold several layers have them in this order.
+LAYERS = ("traversability", "traversability_slope", "traversability_step", "traversability_roughness", "elevation", "robot_slope",
+          "traversability_footprint")
+
+
+def layer_mask(names) -> int:
+    """The te_layer mask of layer names (any order; each once)."""
+    names = list(names)
+    unknown = [n for n in names if n not in LAYERS]
+    if unknown or len(set(names)) != len(names):
+        raise ValueError(f"layer names {names}: each once, from {LAYERS}")
+    return sum(1 << LAYERS.index(n) for n in names)
+
+
+class SubmapInfo(C.Structure):
+    """te_submap_info."""
+    _fields_ = [("success", C.c_int32), ("rows", C.c_int32), ("cols", C.c_int32), ("top_row", C.c_int32), ("top_col", C.c_int32),
+                ("requested_row", C.c_int32), ("requested_col", C.c_int32), ("reserved", C.c_int32),
+                ("length_x", C.c_double), ("length_y", C.c_double), ("position_x", C.c_double), ("position_y", C.c_double),
+                ("offset", C.c_int64)]
+
+
+# te_submap_info as a numpy record, for arrays of them
+SUBMAP_INFO_DTYPE = np.dtype([(n, np.dtype(t._type_)) for n, t in SubmapInfo._fields_])
+assert SUBMAP_INFO_DTYPE.itemsize == C.sizeof(SubmapInfo)
+
+
+def _windows(positions, lengths):
+    p = np.ascontiguousarray(positions, dtype=np.float64).reshape(-1, 2)
+    ln = np.ascontiguousarray(lengths, dtype=np.float64).reshape(-1, 2)
+    if len(p) != len(ln):
+        raise ValueError(f"{len(p)} positions but {len(ln)} lengths")
+    return p, ln
 
 
 class TEError(RuntimeError):
@@ -147,6 +182,19 @@ def fused_plan(rows: int, out_ncols: int, nmaps: int = 1, sms: int = 132) -> dic
     nl = out[1]
     levels = [dict(unit0=out[2 + 4 * i], col0=out[3 + 4 * i], seg_len=out[4 + 4 * i], nseg=out[5 + 4 * i]) for i in range(nl)]
     return {"strips": out[0], "levels": levels, "units": out[2 + 4 * nl]}
+
+
+def submap_geometry(g, positions, lengths):
+    """te_submap_geometry: GridMap::getSubmap's geometry of each window ((x, y) position and length per row) on the map `g`, as
+    an array of SUBMAP_INFO_DTYPE records; offsets count one layer per window.  Host arithmetic, no GPU needed."""
+    L = load_library()
+    p, ln = _windows(positions, lengths)
+    info = np.zeros(len(p), dtype=SUBMAP_INFO_DTYPE)
+    L.te_submap_geometry.argtypes = [C.POINTER(Geometry), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    rc = L.te_submap_geometry(C.byref(g), len(p), p.ctypes.data, ln.ctypes.data, info.ctypes.data)
+    if rc != 0:
+        raise TEError(rc, L.te_last_error().decode())
+    return info
 
 
 def _addr(a):
@@ -756,3 +804,60 @@ class Map:
         self._L.te_map_request_stats.argtypes = [C.c_void_p, C.c_int64 * 3]
         self._check(self._L.te_map_request_stats(self._h, out))
         return tuple(int(v) for v in out)
+
+    def get_layers(self, names, out=None, memory=MEM_HOST):
+        """te_map_get_layers (publishTraversabilityMap): dict name -> (rows, cols) layer for `names` (LAYERS entries).  Host
+        memory: numpy arrays, re-wrapped to the map's start index.  Device memory: `out` is a float32 device tensor of
+        len(names) * rows * cols, filled asynchronously on the context stream in the map's default order; the dict holds views."""
+        mask = layer_mask(names)
+        order = [n for k, n in enumerate(LAYERS) if (mask >> k) & 1]
+        rows, cols = self._shape() if self._g else (0, 0)
+        if memory == MEM_HOST:
+            out = np.empty((len(order), cols, rows), dtype=np.float32)   # layer k column-major at k * rows * cols
+        fn = self._L.te_map_get_layers
+        fn.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_int]
+        self._ctx._order_after_torch(memory)
+        self._check(fn(self._h, mask, _addr(out), memory))
+        v = out.reshape(len(order), cols, rows)
+        return {n: v[k].T for k, n in enumerate(order)}
+
+    def get_submaps(self, positions, lengths, names, out=None, memory=MEM_HOST):
+        """te_map_get_submaps (the get_traversability_map service per window): one (info, layers) pair per window, info a
+        SUBMAP_INFO_DTYPE record and layers a dict name -> (rows_k, cols_k) submap layer, or None for a failed window.  Host
+        memory: numpy arrays (out=None: sized by submap_geometry).  Device memory: `out` is a float32 device tensor with room for
+        every window, filled asynchronously on the context stream; the layers are views of it."""
+        mask = layer_mask(names)
+        order = [n for k, n in enumerate(LAYERS) if (mask >> k) & 1]
+        p, ln = _windows(positions, lengths)
+        if out is None:
+            if memory != MEM_HOST:
+                raise ValueError("device memory needs an `out` tensor")
+            geo = submap_geometry(self._g, p, ln) if self._g is not None else np.zeros(0, dtype=SUBMAP_INFO_DTYPE)
+            out = np.empty(len(order) * int((geo["rows"].astype(np.int64) * geo["cols"]).sum()), dtype=np.float32)
+        cap = out.size if isinstance(out, np.ndarray) else out.numel()
+        info = np.zeros(len(p), dtype=SUBMAP_INFO_DTYPE)
+        fn = self._L.te_map_get_submaps
+        fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]
+        self._ctx._order_after_torch(memory)
+        self._check(fn(self._h, len(p), p.ctypes.data, ln.ctypes.data, mask, info.ctypes.data, _addr(out), cap, memory))
+        res = []
+        for r in info:
+            if not r["success"]:
+                res.append((r, None))
+                continue
+            nr, nc, o = int(r["rows"]), int(r["cols"]), int(r["offset"])
+            res.append((r, {n: out[o + k * nr * nc:o + (k + 1) * nr * nc].reshape(nc, nr).T for k, n in enumerate(order)}))
+        return res
+
+    def valid_at(self, xy, out=None, memory=MEM_HOST):
+        """te_map_valid_at (mapHasValidTraversabilityAt per position): uint8 per (x, y) row of `xy`, 1 where getIndex finds the
+        position in the map and traversability is finite there.  Device memory: xy a float64 (n, 2) device tensor and `out` a
+        uint8 device tensor of n, filled asynchronously on the context stream."""
+        if memory == MEM_HOST:
+            xy = np.ascontiguousarray(xy, dtype=np.float64).reshape(-1, 2)
+            out = np.zeros(len(xy), dtype=np.uint8)
+        fn = self._L.te_map_valid_at
+        fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
+        self._ctx._order_after_torch(memory)
+        self._check(fn(self._h, len(xy), _addr(xy), _addr(out), memory))
+        return out

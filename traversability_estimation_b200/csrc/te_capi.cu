@@ -1301,6 +1301,7 @@ struct te_map {
   te_geometry geo_in{};  // as the layers came (host memory: with their circular-buffer start index)
   te_geometry geo{};     // the same with the start index cleared: the device layers are in default order
   DevBuf trav, slope, step, rough, elev, rslope, cache, fresh;
+  DevBuf gather;  // te_map_get_submaps: the source-layer table, then the windows (te::SubmapWindow)
   bool have_rough = false, have_rslope = false;
   te::FootprintState fp;  // the map's own scratch; fp.memo is the resident memo
   bool memo_valid = false;
@@ -1371,6 +1372,22 @@ int map_footprint_params(const te_map* m, const te_footprint_params* p) {
   return TE_OK;
 }
 
+// The map's layers of `mask`, in te_layer bit order (the order of every output that holds several).
+int map_layers(const te_map* m, uint32_t mask, const float* out[7], int* n) {
+  if (mask == 0 || (mask & ~(uint32_t)TE_LAYER_ALL)) return fail(TE_ERR_BAD_ARG, "layer mask 0x%x: need a non-empty subset of 0x%x", mask, TE_LAYER_ALL);
+  static const char* const names[7] = {"traversability", "traversability_slope", "traversability_step", "traversability_roughness",
+                                       "elevation", "robot_slope", "traversability_footprint"};
+  const DevBuf* const src[7] = {&m->trav, &m->slope, &m->step, m->have_rough ? &m->rough : nullptr, &m->elev,
+                                m->have_rslope ? &m->rslope : nullptr, &m->cache};
+  *n = 0;
+  for (int b = 0; b < 7; ++b) {
+    if (!((mask >> b) & 1u)) continue;
+    if (!src[b]) return fail(TE_ERR_MISSING_LAYER, "layer %s is missing: the map does not hold it", names[b]);
+    out[(*n)++] = (const float*)src[b]->p;
+  }
+  return TE_OK;
+}
+
 #define TE_MAP_ENTER(map)                                   \
   if (!(map)) return fail(TE_ERR_BAD_ARG, "map is null");   \
   te_ctx* c = (map)->ctx;                                   \
@@ -1394,7 +1411,7 @@ int te_map_destroy(te_map* m) {
     Guard g(m->ctx);
     if (g.ok) {
       cudaStreamSynchronize(m->ctx->stream);
-      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh}) b->release();
+      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather}) b->release();
       m->fp.release();
     }
   }
@@ -1596,6 +1613,115 @@ int te_map_request_stats(te_map* m, int64_t out[3]) {
   out[1] = m->last.keys;
   out[2] = m->last.stored;
   return TE_OK;
+}
+
+// ---- The read side: GetGridMap submaps, the published layers and mapHasValidTraversabilityAt -----------------------------------
+namespace {
+
+// te_submap_geometry's records of `n` windows on the map `g` (its start index changes nothing: te::grid_submap), with offsets for
+// `nlayers` layers per window; *total receives the floats they take.  Every window is checked before any record is written.
+int submap_windows(const te_geometry* g, int32_t n, const double* pos, const double* len, int nlayers, te_submap_info* info,
+                   int64_t* total) {
+  if (n < 0) return fail(TE_ERR_BAD_ARG, "negative window count");
+  if (n > 0 && (!pos || !len || !info)) return fail(TE_ERR_BAD_ARG, "null argument");
+  for (int32_t k = 0; k < n; ++k) {  // the reference does not validate these; a negative length would make negative-sized blocks
+    if (!std::isfinite(pos[2 * k]) || !std::isfinite(pos[2 * k + 1])) return fail(TE_ERR_BAD_ARG, "window %d: position is not finite", k);
+    if (!(len[2 * k] >= 0.0 && len[2 * k + 1] >= 0.0) || !std::isfinite(len[2 * k]) || !std::isfinite(len[2 * k + 1]))
+      return fail(TE_ERR_BAD_ARG, "window %d: length must be finite and >= 0", k);
+  }
+  const te::GridGeo A{g->rows, g->cols, g->resolution, g->length_x, g->length_y, g->position_x, g->position_y};
+  int64_t off = 0;
+  for (int32_t k = 0; k < n; ++k) {
+    te_submap_info r{};
+    te::SubmapGeo s{};
+    if (te::grid_submap(A, pos[2 * k], pos[2 * k + 1], len[2 * k], len[2 * k + 1], s)) {
+      r.success = 1;
+      r.rows = s.rows; r.cols = s.cols; r.top_row = s.top_row; r.top_col = s.top_col;
+      r.requested_row = s.req_row; r.requested_col = s.req_col;
+      r.length_x = s.lenx; r.length_y = s.leny; r.position_x = s.posx; r.position_y = s.posy;
+    }
+    r.offset = off;
+    off += (int64_t)nlayers * r.rows * r.cols;
+    info[k] = r;
+  }
+  if (total) *total = off;
+  return TE_OK;
+}
+
+}  // namespace
+
+int te_submap_geometry(const te_geometry* g, int32_t n, const double* position_xy, const double* length_xy, te_submap_info* info) {
+  if (int rc = check_geometry(g, true)) return rc;
+  return submap_windows(g, n, position_xy, length_xy, 1, info, nullptr);
+}
+
+int te_map_get_layers(te_map* m, uint32_t layer_mask, float* out, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  const float* src[7];
+  int nl = 0;
+  if (int rc = map_layers(m, layer_mask, src, &nl)) return rc;
+  if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
+  for (int k = 0; k < nl; ++k)
+    if (int rc = map_get_layer(m, out + (size_t)k * map_cells(m), src[k], memory)) return rc;
+  if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));
+  return TE_OK;
+}
+
+int te_map_get_submaps(te_map* m, int32_t nwin, const double* position_xy, const double* length_xy, uint32_t layer_mask,
+                       te_submap_info* info, float* out, int64_t out_capacity, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  const float* src[7];
+  int nl = 0;
+  if (int rc = map_layers(m, layer_mask, src, &nl)) return rc;
+  int64_t total = 0;
+  if (int rc = submap_windows(&m->geo, nwin, position_xy, length_xy, nl, info, &total)) return rc;
+  if (out_capacity < total)
+    return fail(TE_ERR_BAD_ARG, "the submaps take %lld floats but out holds %lld: call again with more room", (long long)total,
+                (long long)out_capacity);
+  if (total == 0) return TE_OK;
+  if (!out) return fail(TE_ERR_BAD_ARG, "output is null");
+  // the table k_map_gather_submaps reads: the source layers in its first two records, then the windows that have cells
+  static_assert(sizeof(const float*) * 7 <= 2 * sizeof(te::SubmapWindow), "layer table");
+  std::vector<te::SubmapWindow> table(2);
+  std::memcpy((void*)table.data(), src, sizeof(const float*) * nl);
+  long long columns = 0;
+  for (int32_t k = 0; k < nwin; ++k) {
+    const te_submap_info& r = info[k];
+    if (!r.success) continue;
+    table.push_back(te::SubmapWindow{columns, (long long)r.top_col * m->geo.rows + r.top_row, r.offset, r.rows, r.cols});
+    columns += (long long)nl * r.cols;
+  }
+  const size_t bytes = sizeof(te::SubmapWindow) * table.size();
+  if (m->gather.p && m->gather.cap < bytes) TE_CUDA(cudaStreamSynchronize(c->stream));  // an earlier gather may still read it
+  TE_CUDA(m->gather.reserve(bytes));
+  TE_CUDA(cudaMemcpyAsync(m->gather.p, table.data(), bytes, cudaMemcpyHostToDevice, c->stream));
+  Staging st(c, memory == TE_MEM_HOST, &m->geo);  // host memory: gather into staging, then one copy of the packed floats
+  float* dout = st.out(out, (size_t)total);
+  if (st.rc) return st.rc;
+  const te::SubmapGather a{(const float* const*)m->gather.p, (const te::SubmapWindow*)m->gather.p + 2, (int)table.size() - 2,
+                           m->geo.rows, columns, dout};
+  te::launch_gather_submaps(a, c->sms, c->stream);
+  if (int rc = launch_check(c, "k_map_gather_submaps")) return rc;
+  return st.finish();
+}
+
+int te_map_valid_at(te_map* m, int32_t n, const double* xy, uint8_t* valid, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (n < 0) return fail(TE_ERR_BAD_ARG, "negative position count");
+  if (n == 0) return TE_OK;
+  if (!xy || !valid) return fail(TE_ERR_BAD_ARG, "null argument");
+  Staging st(c, memory == TE_MEM_HOST, &m->geo);
+  const double* dxy = st.in(xy, 2 * (size_t)n);
+  uint8_t* dvalid = st.out(valid, (size_t)n);
+  if (st.rc) return st.rc;
+  const te_geometry& g = m->geo;
+  te::launch_valid_at(te::GridGeo{g.rows, g.cols, g.resolution, g.length_x, g.length_y, g.position_x, g.position_y},
+                      (const float*)m->trav.p, n, dxy, dvalid, c->stream);
+  if (int rc = launch_check(c, "k_map_valid_at")) return rc;
+  return st.finish();
 }
 
 // A te IPC handle is the CUDA handle of the ALLOCATION that contains the pointer (cudaIpcGetMemHandle always describes the whole

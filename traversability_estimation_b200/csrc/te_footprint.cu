@@ -83,14 +83,7 @@ __device__ __forceinline__ bool get_index_d(const FpArgs& A, double px, double p
 }
 
 __device__ __forceinline__ void bound_position_d(const FpArgs& A, double& px, double& py) {
-  double sx = (px - A.posx) + 0.5 * A.lenx, sy = (py - A.posy) + 0.5 * A.leny;
-  double ex = 10.0 * 2.220446049250313e-16, ey = ex;
-  if (fabs(px) > 1.0) ex *= fabs(px);
-  if (fabs(py) > 1.0) ey *= fabs(py);
-  if (sx <= 0.0) sx = ex; else if (sx >= A.lenx) sx = A.lenx - ex;
-  if (sy <= 0.0) sy = ey; else if (sy >= A.leny) sy = A.leny - ey;
-  px = (sx + A.posx) - 0.5 * A.lenx;
-  py = (sy + A.posy) - 0.5 * A.leny;
+  grid_bound_position(A, px, py);
 }
 
 template <class F>

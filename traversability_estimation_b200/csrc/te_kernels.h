@@ -45,4 +45,25 @@ void launch_step(const SlabView& v, const ChainDev& p, const float* elev, float*
 void launch_roughness(const SlabView& v, const ChainDev& p, const float* elev, const float* nx, const float* ny, const float* nz,
                       float* out, int sms, cudaStream_t s);
 
+// te_submap.cu — the read side of a te_map.  A window of te_map_get_submaps that has cells: its block of the map and where its
+// layers go.  Columns are numbered flat over (window, layer, column), window by window.
+struct SubmapWindow {
+  long long col0;  // the window's first column in that numbering
+  long long src;   // cell offset of its top-left cell in a source layer: top_col * map rows + top_row
+  long long dst;   // float offset of its first layer in `out`
+  int rows, cols;
+};
+struct SubmapGather {
+  const float* const* layers;  // device table of the source layers (column-major, default order), in output order
+  const SubmapWindow* win;     // device, in column order
+  int nwin, map_rows;
+  long long ncolumns;          // windows x layers x columns
+  float* out;
+};
+// One k_map_gather_submaps launch for every column of every window (none when there is no column).
+void launch_gather_submaps(const SubmapGather& a, int sms, cudaStream_t s);
+struct GridGeo;
+// valid[q] = getIndex(xy[2q], xy[2q+1]) succeeds and traversability is finite there (device pointers; none launched for n = 0).
+void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, unsigned char* valid, cudaStream_t s);
+
 }  // namespace te
