@@ -42,7 +42,7 @@ def test_footprint_slope_threshold_constant():
     assert ncrit(0.02) == 29 and ncrit(0.03) == 20
 
 
-def test_slope_stream_acos_polynomial_meets_its_stated_error():
+def test_slope_stream_acos_constant_bank_coefficients_meet_their_stated_error():
     """k_slope_stream in te_generic.cu: acos(|x|) = sqrt(1 - |x|) * P14(|x|) in double.  The kernel rounds 1 - theta/critical
     to float32 only when it stands 1e-12 (times max(1, 1/critical)) clear of a rounding boundary and documents
     |error| <= 5.1e-14 rad for the polynomial, a 20-fold margin: check the coefficients the kernel holds in constant memory
@@ -65,7 +65,3 @@ def test_slope_stream_acos_polynomial_meets_its_stated_error():
     err = np.abs(theta.astype(np.longdouble) - exact)
     assert float(err.max()) <= 5.2e-14, float(err.max())
     assert theta[a == 1.0].max() == 0.0
-    # the literal branch of the old build and the constant-bank branch must hold the same numbers
-    lit = re.findall(r"fma\((?:a|p), (?:a, )?(-?[0-9.e-]+)(?:, (-?[0-9.e-]+))?\);", src[src.index("#else", src.index("TE_SLOPE_CONST_BANK\n")):])
-    flat = [float(t) for pair in lit for t in pair if t][:15]
-    assert flat == c, (flat, c)

@@ -1,6 +1,6 @@
 #!/bin/bash
 # Time several builds of the kernels in ONE GPU session.
-#   here (no GPU):   make -C traversability_estimation_b200/csrc variant NAME=a TE_WPC=8 EXTRA="-DX=1"   (one per variant)
+#   here (no GPU):   make -C traversability_estimation_b200/csrc variant NAME=a EXTRA="-DX=1"   (one per variant)
 #   under gpurun:    bash tools/dev_variants.sh a b c -- --holes 0
 # Every variant is libte_b200_<name>.so next to the product library; "base" means the product library itself.
 names=(); extra=()

@@ -431,9 +431,6 @@ __global__ void __launch_bounds__(256) k_slope(long long total, double crit, con
     out[c] = slope_literal(__ldg(nz + c), crit);
 }
 
-#ifndef TE_SLOPE_CONST_BANK
-#define TE_SLOPE_CONST_BANK 1
-#endif
 __constant__ double c_acos14[15] = {3.139129045303817e-05,  -0.0002719939971935411, 0.0011120542916517797, -0.002896219765138688,
                                     0.005523167239593235,   -0.008503457350174303,  0.01149382355518035,   -0.01466134286289636,
                                     0.018621724287455857,   -0.024366397045309886,  0.03368046433967888,   -0.050792762643682245,
@@ -449,27 +446,10 @@ __constant__ double c_acos14[15] = {3.139129045303817e-05,  -0.00027199399719354
 __device__ __forceinline__ float slope_stream(float x, double crit, double inv_crit, double band) {
   if (!finitef(x)) return nanf_();                      // no surface normal: the layer stays NaN (SlopeFilter.cpp:71)
   const double a = fabs((double)x);
-#if TE_SLOPE_CONST_BANK
   // coefficients as constant-bank operands of the DFMAs: as 64-bit literals they cost two UMOV each (28 of ~80 instructions per cell)
   double p = fma(a, c_acos14[0], c_acos14[1]);
 #pragma unroll
   for (int k = 2; k < 15; ++k) p = fma(p, a, c_acos14[k]);
-#else
-  double p = fma(a, 3.139129045303817e-05, -0.0002719939971935411);
-  p = fma(p, a, 0.0011120542916517797);
-  p = fma(p, a, -0.002896219765138688);
-  p = fma(p, a, 0.005523167239593235);
-  p = fma(p, a, -0.008503457350174303);
-  p = fma(p, a, 0.01149382355518035);
-  p = fma(p, a, -0.01466134286289636);
-  p = fma(p, a, 0.018621724287455857);
-  p = fma(p, a, -0.024366397045309886);
-  p = fma(p, a, 0.03368046433967888);
-  p = fma(p, a, -0.050792762643682245);
-  p = fma(p, a, 0.08904862081826843);
-  p = fma(p, a, -0.21460183657961013);
-  p = fma(p, a, 1.5707963267948457);
-#endif
   double th = sqrt(1.0 - a) * p;
   if (x < 0.0f) th = 3.141592653589793 - th;
   const double v = fma(-th, inv_crit, 1.0);
