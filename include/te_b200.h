@@ -473,7 +473,19 @@ int te_check_footprint_request_batched(te_ctx* ctx, const te_geometry* g, const 
  * memo, which is kept until the layers or one of max_gap_width, critical_step_height and verify_roughness change.  Whole maps only.
  * Host layers may carry a circular-buffer start index: they are unwrapped on upload and outputs are re-wrapped to the start index
  * of the last te_map_chain / te_map_set_layers.  Every entry but te_map_create / te_map_destroy fails with TE_ERR_BAD_ARG before
- * layers were set.  Host-memory entries return synchronised; device-memory ones are asynchronous on the context stream. */
+ * layers were set.  Host-memory entries return synchronised; device-memory ones are asynchronous on the context stream.
+ *
+ * Batches.  te_map_chain_batched / te_map_set_layers_batched give a te_map nmaps >= 1 maps of one geometry (a robot each, say),
+ * in the layout of te_chain_batched: map m at offset m*rows*cols in every layer, the cache and the memo.  Each map has its own
+ * cache and memo, and for each map m everything a call returns or stores is, bit for bit, what a separate single-map te_map
+ * holding map m returns or stores for the same calls restricted to map m (for a request: that map's paths, in their relative
+ * request order).  A path never reads or writes another map's cells, cache or memo.  Limits as te_footprint_batched: nmaps
+ * 1..65535 (TE_ERR_BAD_ARG below 1, TE_ERR_UNSUPPORTED above), nmaps*rows*cols < 2^32 and nmaps*cols < 2^31 (TE_ERR_UNSUPPORTED);
+ * a circular-buffer start index is TE_ERR_UNSUPPORTED for every _batched entry.  On a batch te_map_footprint, the polygon
+ * entries, te_map_get_layers, te_map_get_footprint and te_map_clear_footprint work on every map, their outputs holding the maps
+ * back to back per layer; te_map_check_footprint_request, te_map_get_submaps and te_map_valid_at need a map index and fail with
+ * TE_ERR_BAD_ARG on a te_map of more than one map (use their _batched entries).  The single-map entries on a te_map of one map
+ * are unchanged, start indices included. */
 typedef struct te_map te_map;
 int te_map_create(te_ctx* ctx, te_map** out);
 int te_map_destroy(te_map* map);
@@ -488,13 +500,28 @@ int te_map_chain(te_map* map, const te_geometry* g, const te_chain_params* p, co
 int te_map_set_layers(te_map* map, const te_geometry* g, const float* traversability, const float* slope, const float* step,
                       const float* roughness_or_null, const float* elevation, const float* robot_slope_or_null, int memory);
 
+/* computeTraversability for every map of a batch: te_chain_batched on nmaps elevation maps (layout and limits above) into the
+ * te_map's layers, each optionally copied out for every map.  Empties every cache and memo and leaves the batch without
+ * robot_slope, as te_map_chain does; te_map_chain is its nmaps = 1 case. */
+int te_map_chain_batched(te_map* map, const te_geometry* g, const te_chain_params* p, int32_t nmaps, const float* elevation,
+                         float* slope_or_null, float* step_or_null, float* roughness_or_null, float* traversability_or_null, int memory);
+
+/* setTraversabilityMap for every map of a batch: every layer holds nmaps maps back to back.  Empties every cache and memo; the only
+ * way to give a batch robot_slope.  te_map_set_layers is its nmaps = 1 case. */
+int te_map_set_layers_batched(te_map* map, const te_geometry* g, int32_t nmaps, const float* traversability, const float* slope,
+                              const float* step, const float* roughness_or_null, const float* elevation,
+                              const float* robot_slope_or_null, int memory);
+
 /* traversabilityFootprint(radius, offset) (:307-318) on the cache: a cached cell keeps its value (the memoised branch, :673-675),
  * every other cell gets te_footprint2's value for `p`; traversability_footprint_or_null receives the cache afterwards.  The
  * prefix-sum sweep may differ from the visit-by-visit one in the last float32 bit of a few cells (DESIGN.md §4.3); those values
- * then stay in the cache.  Errors as te_footprint2 (TE_ERR_MISSING_LAYER: verify_roughness without a roughness layer). */
+ * then stay in the cache.  Errors as te_footprint2 (TE_ERR_MISSING_LAYER: verify_roughness without a roughness layer).  On a
+ * batch: every map's cache, te_footprint_batched's sweep, nmaps layers out. */
 int te_map_footprint(te_map* map, const te_footprint_params* p, float* traversability_footprint_or_null, int memory);
 
-/* traversabilityFootprint(yaw) (:239-305): te_footprint_polygon on the map's layers.  Reads and changes no cache. */
+/* traversabilityFootprint(yaw) (:239-305): te_footprint_polygon on the map's layers.  Reads and changes no cache.  On a batch:
+ * te_footprint_polygon_batched's outputs (and te_footprint_polygon_yaws(_reduce)'s for the two entries below: layer k of map m at
+ * (k*nmaps + m)*rows*cols). */
 int te_map_footprint_polygon(te_map* map, const te_footprint_params* p, int32_t npts, const double* polygon_xy, double footprint_yaw,
                              float* traversability_x, float* traversability_rot, int memory);
 
@@ -529,13 +556,27 @@ int te_map_check_footprint_request(te_map* map, const te_footprint_params* p, in
                                    double* area_out, int32_t max_vertices, int32_t* untraversable_count_or_null,
                                    double* untraversable_xy_or_null);
 
+/* te_map_check_footprint_request on a batch: path q is on map path_map[q] (a host array, like every other request array; an
+ * entry outside 0..nmaps-1 is TE_ERR_BAD_ARG, as is a null path_map).  Paths run in request order, each on its own map's layers,
+ * cache and memo, so a map's answers and cache equal those of a single-map te_map given that map's paths in the same order; maps
+ * may interleave and may have no paths.  The launches are those of one te_map_check_footprint_request, whatever nmaps. */
+int te_map_check_footprint_request_batched(te_map* map, const te_footprint_params* p, const int32_t* path_map, int32_t npaths,
+                                           int32_t nposes, const int32_t* path_begin, const double* poses, const double* radius,
+                                           int32_t nvertices, const int32_t* footprint_begin, const float* footprint_xyz,
+                                           int32_t max_footprint_vertices, const uint8_t* conservative_or_null,
+                                           const uint8_t* compute_untraversable_polygon_or_null, uint8_t* is_safe,
+                                           double* traversability_out, double* area_out, int32_t max_vertices,
+                                           int32_t* untraversable_count_or_null, double* untraversable_xy_or_null);
+
 /* The cache as publishTraversabilityMap publishes its traversability_footprint layer (in host memory: in the map's buffer
- * order; device memory needs a map without a start index), and resetTraversabilityFootprintLayers (:195-200). */
+ * order; device memory needs a map without a start index), and resetTraversabilityFootprintLayers (:195-200).  On a batch: every
+ * map's cache, back to back. */
 int te_map_get_footprint(te_map* map, float* traversability_footprint, int memory);
 int te_map_clear_footprint(te_map* map);
 
-/* Counters of the last te_map_check_footprint_request: out[0] isTraversable calls its circular paths could make, out[1] distinct
- * circles among them (each is walked once on the device), out[2] cache cells the request stored.  No reference counterpart. */
+/* Counters of the last te_map_check_footprint_request(_batched): out[0] isTraversable calls its circular paths could make, out[1]
+ * distinct circles among them (each is walked once on the device), out[2] cache cells the request stored; totals over every map
+ * of a batch.  No reference counterpart. */
 int te_map_request_stats(te_map* map, int64_t out[3]);
 
 /* ---- The read side of a te_map: the layers the reference node publishes and serves ----------------------------------------
@@ -574,7 +615,7 @@ typedef struct te_submap_info {
 int te_submap_geometry(const te_geometry* g, int32_t n, const double* position_xy, const double* length_xy, te_submap_info* info);
 
 /* publishTraversabilityMap (TraversabilityMap.cpp:172-186): the layers of `layer_mask` (te_layer bits), each rows x cols, back to
- * back in bit order.  In host memory each is re-wrapped to the map's start index, as te_map's other outputs, and the call returns
+ * back in bit order (on a batch: per layer the nmaps maps back to back, nmaps*rows*cols floats a layer).  In host memory each is re-wrapped to the map's start index, as te_map's other outputs, and the call returns
  * synchronised; in device memory they are in the map's default (unwrapped) order, asynchronously.  TE_ERR_MISSING_LAYER for a
  * layer the map does not hold (roughness after te_map_set_layers without it, robot_slope after te_map_chain); TE_ERR_BAD_ARG
  * for an empty mask or unknown bits. */
@@ -590,10 +631,19 @@ int te_map_get_layers(te_map* map, uint32_t layer_mask, float* out, int memory);
 int te_map_get_submaps(te_map* map, int32_t nwin, const double* position_xy, const double* length_xy, uint32_t layer_mask,
                        te_submap_info* info, float* out, int64_t out_capacity, int memory);
 
+/* te_map_get_submaps on a batch: window k is taken from map win_map[k] (a host array; an entry outside 0..nmaps-1 is
+ * TE_ERR_BAD_ARG).  Output layout, te_submap_info and the capacity protocol are those of te_map_get_submaps. */
+int te_map_get_submaps_batched(te_map* map, int32_t nwin, const int32_t* win_map, const double* position_xy, const double* length_xy,
+                               uint32_t layer_mask, te_submap_info* info, float* out, int64_t out_capacity, int memory);
+
 /* mapHasValidTraversabilityAt (TraversabilityMap.cpp:971-983) for n positions (xy: n (x, y) pairs): valid[q] = 1 when getIndex
  * finds the position in the map and traversability is finite there, else 0.  xy and valid are in `memory`; device memory is
  * asynchronous on the context stream. */
 int te_map_valid_at(te_map* map, int32_t n, const double* xy, uint8_t* valid, int memory);
+
+/* te_map_valid_at on a batch: position q is on map pos_map[q]; pos_map, xy and valid are in `memory`.  In host memory a map
+ * outside 0..nmaps-1 is TE_ERR_BAD_ARG; in device memory (not read on the host) that position gets 0. */
+int te_map_valid_at_batched(te_map* map, int32_t n, const int32_t* pos_map, const double* xy, uint8_t* valid, int memory);
 
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the

@@ -31,6 +31,13 @@ map, both in TE_MEM_DEVICE on the same stream.  Maps: --maps (256 and 16) maps o
 map, stored map by map; every other path circular (radius 0.3 m, offset 0.15 m), the others the YAML footprint with a random
 yaw per pose.  CUDA events around the whole batch (the batched call, or the loop), median of --reps after --warmup, the two
 alternating; the kernel launches of one batch (te_get_stats); whether the two output sets are identical bit for bit.
+
+--map --batched times te_map_check_footprint_request_batched on one te_map holding a batch (--maps: 256 and 16 maps of 512 x 512
+at 0.02 m, te_map_chain_batched on synth.terrain) against a loop of te_map_check_footprint_request over one single-map te_map per
+map holding the same layers.  The path mix of --batched, --paths-per-map (16) per map, in host memory.  Two cases: "empty_cache"
+(every cache cleared before each call, not timed) and "again" (the same request on the cache it left).  Host clock around each
+call (they end synchronised), median of --reps after --warmup, the two alternating; the launches of one call; every output and
+every map's cache are asserted equal to the loop's bit for bit.
 """
 from __future__ import annotations
 
@@ -85,9 +92,13 @@ def main():
     ap.add_argument("--map", action="store_true")
     ap.add_argument("--batched", action="store_true")
     ap.add_argument("--maps", type=int, nargs="+", default=[256, 16])
-    ap.add_argument("--paths-per-map", type=int, nargs="+", default=[4, 16, 64])
+    ap.add_argument("--paths-per-map", type=int, nargs="+", default=None)
     args = ap.parse_args()
+    if args.batched and args.map:
+        args.paths_per_map = args.paths_per_map or [16]
+        return main_map_batched(args)
     if args.batched:
+        args.paths_per_map = args.paths_per_map or [4, 16, 64]
         return main_batched(args)
     if args.map:
         return main_map(args)
@@ -612,6 +623,102 @@ def main_batched(args):
         del z, slope, step, rough, trav
         torch.cuda.empty_cache()
     ctx.set_stream(None)
+    ctx.close()
+
+
+def main_map_batched(args):
+    """te_map_check_footprint_request_batched on one te_map holding a batch against a loop of te_map_check_footprint_request over
+    one single-map te_map per map holding the same layers, in host memory (host clock around each call, which ends synchronised)."""
+    import time
+    import torch
+    import synth
+    import traversability_estimation_b200 as te
+
+    n, res = 512, 0.02
+    g = te.Geometry.make(n, n, res)
+    fp = te.FootprintParams.yaml_defaults()            # offset 0.15
+    fyaml = np.asarray(YAML_FOOTPRINT, np.float32)
+    ctx = te.Context(0)
+    name, power = gpu_info(torch)
+    for nmaps in args.maps:
+        b = ctx.map()
+        L = b.chain_batched(g, te.ChainParams.yaml_defaults(0), nmaps,
+                            np.stack([synth.terrain(n, n, res, 1000 + k, "mixed") for k in range(nmaps)]), outputs=True)
+        elev = b.get_layers(["elevation"])["elevation"]
+        singles = []
+        for k in range(nmaps):
+            s = ctx.map()
+            s.set_layers(g, L["traversability"][k], L["slope"][k], L["step"][k], elev[k], roughness=L["roughness"][k])
+            singles.append(s)
+        for per_map in args.paths_per_map:
+            rng = np.random.default_rng(per_map)
+            maps = []   # per map: path_begin, poses (7 wide), radius, footprint_begin, footprint_xyz; odd paths circular
+            for _ in range(nmaps):
+                begin, xy = planner_paths(rng, n, per_map, res)
+                yaw = rng.uniform(0, 2 * np.pi, len(xy))
+                poses = np.stack([xy[:, 0], xy[:, 1], np.zeros(len(xy)), np.zeros(len(xy)), np.zeros(len(xy)), np.sin(yaw / 2),
+                                  np.cos(yaw / 2)], axis=1)
+                circ = np.arange(per_map) % 2 == 1
+                fbeg = np.concatenate([[0], np.cumsum(np.where(circ, 0, len(fyaml)))]).astype(np.int32)
+                fxyz = np.concatenate([fyaml] * int((~circ).sum()) + [np.zeros((0, 3), np.float32)])
+                maps.append((begin, poses, np.full(per_map, 0.3), fbeg, fxyz))
+            npaths = nmaps * per_map
+            begin = np.concatenate([[0]] + [m[0][1:] + sum(len(p[1]) for p in maps[:k]) for k, m in enumerate(maps)]).astype(np.int32)
+            fbeg = np.concatenate([[0]] + [m[3][1:] + sum(len(p[4]) for p in maps[:k]) for k, m in enumerate(maps)]).astype(np.int32)
+            poses, radius, fxyz = (np.concatenate([m[i] for m in maps]) for i in (1, 2, 4))
+            path_map = np.repeat(np.arange(nmaps, dtype=np.int32), per_map)
+
+            def batched():
+                return b.check_footprint_request_batched(fp, path_map, begin, poses, radius, fbeg, fxyz, max_footprint_vertices=len(fyaml))
+
+            def loop():
+                outs = [s.check_footprint_request(fp, *m, max_footprint_vertices=len(fyaml)) for s, m in zip(singles, maps)]
+                return tuple(np.concatenate(o) for o in zip(*outs))
+
+            def clear_batched():
+                b.clear_footprint()
+
+            def clear_loop():
+                for s in singles:
+                    s.clear_footprint()
+
+            row = {"gpu": name, "power_limit_w": power, "maps": nmaps, "size": f"{n}x{n}", "resolution": res, "paths_per_map": per_map,
+                   "paths": npaths, "poses": int(begin[-1]), "circular": npaths // 2, "memory": "host"}
+            same = True
+            for case, clear in (("empty_cache", True), ("again", False)):
+                if clear:
+                    clear_batched()
+                    clear_loop()
+                outs, launches = {}, {}
+                for key, fn in (("batched", batched), ("loop", loop)):
+                    l0 = ctx.stats()[0]
+                    outs[key] = fn()
+                    launches[key] = ctx.stats()[0] - l0
+                got, want = outs["batched"], outs["loop"]
+                same &= all(np.array_equal(a.view(np.uint8), w.view(np.uint8)) for a, w in zip(got, want))
+                caches = b.get_footprint()
+                same &= all(np.array_equal(caches[k].view(np.uint32), s.get_footprint().view(np.uint32)) for k, s in enumerate(singles))
+                ts = {"batched": [], "loop": []}
+                for rep in range(args.warmup + args.reps):
+                    for key, fn, before in (("batched", batched, clear_batched), ("loop", loop, clear_loop)):
+                        if clear:
+                            before()
+                        t = time.perf_counter()
+                        fn()
+                        if rep >= args.warmup:
+                            ts[key].append((time.perf_counter() - t) * 1e3)
+                mb, ml = float(np.median(ts["batched"])), float(np.median(ts["loop"]))
+                row[case] = {"batched_ms": round(mb, 3), "loop_ms": round(ml, 3), "speedup": round(ml / mb, 2),
+                             "batched_ms_range": [round(min(ts["batched"]), 3), round(max(ts["batched"]), 3)],
+                             "loop_ms_range": [round(min(ts["loop"]), 3), round(max(ts["loop"]), 3)],
+                             "launches_batched": launches["batched"], "launches_loop": launches["loop"],
+                             "safe": int(got[0].sum())}
+            row["reps"] = args.reps
+            row["bit_identical_outputs_and_caches"] = bool(same)
+            print(json.dumps(row), flush=True)
+            assert same, "the batched request differs from the loop over single maps"
+        for m in singles + [b]:
+            m.close()
     ctx.close()
 
 

@@ -23,7 +23,8 @@ EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set
            "te_map_chain", "te_map_set_layers", "te_map_footprint", "te_map_footprint_polygon", "te_map_footprint_polygon_yaws", "te_map_footprint_polygon_yaws_reduce",
            "te_map_check_footprint_request",
            "te_map_get_footprint", "te_map_clear_footprint", "te_map_request_stats", "te_submap_geometry", "te_map_get_layers",
-           "te_map_get_submaps", "te_map_valid_at"]
+           "te_map_get_submaps", "te_map_valid_at", "te_map_chain_batched", "te_map_set_layers_batched",
+           "te_map_check_footprint_request_batched", "te_map_get_submaps_batched", "te_map_valid_at_batched"]
 
 
 IPC_HANDLE_BYTES = 80  # TE_IPC_HANDLE_BYTES
@@ -667,7 +668,11 @@ class Map:
     """te_map: the traversability layers, the traversability_footprint cache and the isTraversableForFilters memo kept on the
     device between calls, so that check_footprint_request answers as the reference's check_footprint_path service does over a
     sequence of requests.  Layers are numpy arrays in host memory (rows x cols, any order; copied column-major); the geometry's
-    start index, if any, applies to them and to the layers read back."""
+    start index, if any, applies to them and to the layers read back.
+
+    A Map may hold a batch of nmaps maps of one geometry (chain_batched / set_layers_batched): their layers are (nmaps, rows, cols)
+    arrays, map k's layer a[k]; every output of the whole-map methods then has that leading nmaps axis, and the methods that address
+    one map by position take a map index per path, window or position (the *_batched methods)."""
 
     def __init__(self, ctx: Context):
         self._ctx = ctx
@@ -677,6 +682,28 @@ class Map:
         self._check(self._L.te_map_create(ctx._h, C.byref(h)))
         self._h = h
         self._g = None
+        self._n = 1
+
+    @property
+    def nmaps(self) -> int:
+        """Maps held (1 until chain_batched / set_layers_batched gives it a batch)."""
+        return self._n
+
+    def _layer_out(self, count=None, dtype=np.float32):
+        """An empty host output of `count` layers (None: one) of every map, laid out as the library writes them (per layer the
+        maps back to back, each column-major), and the view returned to the caller: (rows, cols) for one map, (nmaps, rows, cols)
+        for a batch, with a leading `count` axis when count is given."""
+        rows, cols = self._shape()
+        buf = np.empty((1 if count is None else count, self._n, cols, rows), dtype=dtype)
+        view = buf.transpose(0, 1, 3, 2)
+        if self._n == 1:
+            view = view[:, 0]
+        return buf, (view[0] if count is None else view)
+
+    @staticmethod
+    def _batch_layers(a):
+        """(nmaps, rows, cols) host layers as the library reads them: map after map, each column-major."""
+        return None if a is None else np.ascontiguousarray(np.asarray(a, dtype=np.float32).transpose(0, 2, 1))
 
     def _check(self, rc):
         self._ctx._check(rc)
@@ -705,8 +732,21 @@ class Map:
             if outputs else {}
         self._check(fn(self._h, C.byref(g), C.byref(p), _addr(e), *(_addr(out.get(k)) for k in ("slope", "step", "roughness",
                                                                                                  "traversability")), MEM_HOST))
-        self._g = g
+        self._g, self._n = g, 1
         return out if outputs else None
+
+    def chain_batched(self, g, p, nmaps, elevation, outputs=False):
+        """te_map_chain_batched (computeTraversability for every map): elevation (nmaps, rows, cols); empties every cache.
+        outputs=True also returns the four layers as a dict of (nmaps, rows, cols) arrays."""
+        fn = self._L.te_map_chain_batched
+        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(ChainParams), C.c_int32] + [C.c_void_p] * 5 + [C.c_int]
+        e = self._batch_layers(elevation)
+        out = {k: np.empty((int(nmaps), g.cols, g.rows), dtype=np.float32) for k in ("slope", "step", "roughness", "traversability")} \
+            if outputs else {}
+        self._check(fn(self._h, C.byref(g), C.byref(p), int(nmaps), _addr(e),
+                       *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")), MEM_HOST))
+        self._g, self._n = g, int(nmaps)
+        return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
 
     def set_layers(self, g, traversability, slope, step, elevation, roughness=None, robot_slope=None):
         """te_map_set_layers (setTraversabilityMap): empties the cache and the memo."""
@@ -715,14 +755,25 @@ class Map:
         lay = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)  # noqa: E731
         t, s, st, r, e, rs = (lay(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
         self._check(fn(self._h, C.byref(g), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST))
-        self._g = g
+        self._g, self._n = g, 1
+
+    def set_layers_batched(self, g, nmaps, traversability, slope, step, elevation, roughness=None, robot_slope=None):
+        """te_map_set_layers_batched (setTraversabilityMap for every map): each layer (nmaps, rows, cols); empties every cache and
+        memo."""
+        fn = self._L.te_map_set_layers_batched
+        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.c_int32] + [C.c_void_p] * 6 + [C.c_int]
+        t, s, st, r, e, rs = (self._batch_layers(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
+        self._check(fn(self._h, C.byref(g), int(nmaps), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST))
+        self._g, self._n = g, int(nmaps)
 
     def footprint(self, fp):
         """te_map_footprint (traversabilityFootprint(radius, offset) on the cache); returns the cache afterwards."""
         fn = self._L.te_map_footprint
         fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_void_p, C.c_int]
-        out = np.empty(self._shape() if self._g else (0, 0), dtype=np.float32, order="F")
-        self._check(fn(self._h, C.byref(fp), _addr(out) if self._g else None, MEM_HOST))
+        if not self._g:
+            self._check(fn(self._h, C.byref(fp), None, MEM_HOST))
+        buf, out = self._layer_out()
+        self._check(fn(self._h, C.byref(fp), _addr(buf), MEM_HOST))
         return out
 
     def footprint_polygon(self, fp, polygon_xy, yaw):
@@ -730,41 +781,60 @@ class Map:
         fn = self._L.te_map_footprint_polygon
         fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_int]
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
-        ox = np.empty(self._shape(), dtype=np.float32, order="F")
-        orot = np.empty(self._shape(), dtype=np.float32, order="F")
-        self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, float(yaw), _addr(ox), _addr(orot), MEM_HOST))
+        (bx, ox), (brot, orot) = self._layer_out(), self._layer_out()
+        self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, float(yaw), _addr(bx), _addr(brot), MEM_HOST))
         return ox, orot
 
     def footprint_polygon_yaws(self, fp, polygon_xy, yaws):
-        """te_map_footprint_polygon_yaws: (nyaws, rows, cols), layer k the traversability_rot at yaws[k] of the map's layers."""
+        """te_map_footprint_polygon_yaws: (nyaws, rows, cols), layer k the traversability_rot at yaws[k] of the map's layers; on a
+        batch (nyaws, nmaps, rows, cols)."""
         fn = self._L.te_map_footprint_polygon_yaws
         fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
         ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
-        out = np.empty((len(ys), self._g.cols, self._g.rows), dtype=np.float32)   # layer k column-major at k * rows * cols
-        self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data if len(ys) else None, _addr(out),
+        buf, out = self._layer_out(len(ys))   # layer k of map m column-major at (k * nmaps + m) * rows * cols
+        self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data if len(ys) else None, _addr(buf),
                        MEM_HOST))
-        return out.transpose(0, 2, 1)
+        return out
 
     def footprint_polygon_yaws_reduce(self, fp, polygon_xy, yaws):
-        """te_map_footprint_polygon_yaws_reduce: (worst, best, best_yaw) over `yaws` of the map's layers, each (rows, cols)."""
+        """te_map_footprint_polygon_yaws_reduce: (worst, best, best_yaw) over `yaws` of the map's layers, each (rows, cols) or, on
+        a batch, (nmaps, rows, cols)."""
         fn = self._L.te_map_footprint_polygon_yaws_reduce
         fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_void_p] * 3 + [C.c_int]
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
         ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
-        worst, best = (np.empty(self._shape(), dtype=np.float32, order="F") for _ in range(2))
-        best_yaw = np.empty(self._shape(), dtype=np.int32, order="F")
-        self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data if len(ys) else None, _addr(worst),
-                       _addr(best), _addr(best_yaw), MEM_HOST))
+        (bw, worst), (bb, best) = self._layer_out(), self._layer_out()
+        by, best_yaw = self._layer_out(dtype=np.int32)
+        self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data if len(ys) else None, _addr(bw),
+                       _addr(bb), _addr(by), MEM_HOST))
         return worst, best, best_yaw
 
     def check_footprint_request(self, fp, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices=None,
                                 conservative=None, compute_untraversable_polygon=None, untraversable_capacity=None):
         """te_map_check_footprint_request: Context.check_footprint_request in host memory on the map's layers and cache.
         Returns (is_safe, traversability, area) and, with untraversable_capacity=V, (counts, xy) too."""
-        fn = self._L.te_map_check_footprint_request
-        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
-                       C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p, C.c_void_p]
+        return self._request(fp, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices, conservative,
+                             compute_untraversable_polygon, untraversable_capacity)
+
+    def check_footprint_request_batched(self, fp, path_map, path_begin, poses, radius, footprint_begin, footprint_xyz,
+                                        max_footprint_vertices=None, conservative=None, compute_untraversable_polygon=None,
+                                        untraversable_capacity=None):
+        """te_map_check_footprint_request_batched: check_footprint_request with path q on map path_map[q] (int32 per path), each
+        path on its own map's layers and cache, in request order."""
+        return self._request(fp, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices, conservative,
+                             compute_untraversable_polygon, untraversable_capacity, path_map=path_map)
+
+    def _request(self, fp, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices, conservative,
+                 compute_untraversable_polygon, untraversable_capacity, path_map=None):
+        """The body of check_footprint_request (path_map None) and check_footprint_request_batched: the batched entry takes
+        path_map after the parameters."""
+        batched = path_map is not None
+        fn = self._L.te_map_check_footprint_request_batched if batched else self._L.te_map_check_footprint_request
+        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams)] + ([C.c_void_p] if batched else []) + \
+            [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+             C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p, C.c_void_p]
+        pm = [np.ascontiguousarray(path_map, dtype=np.int32)] if batched else []
         pb = np.ascontiguousarray(path_begin, dtype=np.int32)
         ps = np.ascontiguousarray(poses, dtype=np.float64).reshape(-1, 7)
         rad = np.ascontiguousarray(radius, dtype=np.float64)
@@ -778,19 +848,23 @@ class Map:
         maxv = 0 if untraversable_capacity is None else int(untraversable_capacity)
         safe, trav, area = np.zeros(n, dtype=np.uint8), np.zeros(n, dtype=np.float64), np.zeros(n, dtype=np.float64)
         counts, uxy = (None, None) if untraversable_capacity is None else _untraversable_outputs(n, maxv)
-        self._check(fn(self._h, C.byref(fp), n, len(ps), pb.ctypes.data, ps.ctypes.data, rad.ctypes.data, len(fxyz), fb.ctypes.data,
-                       fxyz.ctypes.data, int(max_footprint_vertices), _addr(cons), _addr(cup), safe.ctypes.data, trav.ctypes.data,
-                       area.ctypes.data, maxv, _addr(counts), _addr(uxy)))
+        if batched and len(pm[0]) != n:
+            raise ValueError("path_map needs one entry per path")
+        self._check(fn(self._h, C.byref(fp), *(a.ctypes.data for a in pm), n, len(ps), pb.ctypes.data, ps.ctypes.data,
+                       rad.ctypes.data, len(fxyz), fb.ctypes.data, fxyz.ctypes.data, int(max_footprint_vertices), _addr(cons),
+                       _addr(cup), safe.ctypes.data, trav.ctypes.data, area.ctypes.data, maxv, _addr(counts), _addr(uxy)))
         if untraversable_capacity is None:
             return safe, trav, area
         return safe, trav, area, counts, uxy
 
     def get_footprint(self):
-        """te_map_get_footprint: the traversability_footprint cache (NaN = empty)."""
+        """te_map_get_footprint: the traversability_footprint cache (NaN = empty); (nmaps, rows, cols) on a batch."""
         fn = self._L.te_map_get_footprint
         fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-        out = np.empty(self._shape() if self._g else (0, 0), dtype=np.float32, order="F")
-        self._check(fn(self._h, _addr(out) if self._g else None, MEM_HOST))
+        if not self._g:
+            self._check(fn(self._h, None, MEM_HOST))
+        buf, out = self._layer_out()
+        self._check(fn(self._h, _addr(buf), MEM_HOST))
         return out
 
     def clear_footprint(self):
@@ -808,24 +882,35 @@ class Map:
     def get_layers(self, names, out=None, memory=MEM_HOST):
         """te_map_get_layers (publishTraversabilityMap): dict name -> (rows, cols) layer for `names` (LAYERS entries).  Host
         memory: numpy arrays, re-wrapped to the map's start index.  Device memory: `out` is a float32 device tensor of
-        len(names) * rows * cols, filled asynchronously on the context stream in the map's default order; the dict holds views."""
+        len(names) * rows * cols, filled asynchronously on the context stream in the map's default order; the dict holds views.
+        On a batch every layer is (nmaps, rows, cols) (device memory: len(names) * nmaps * rows * cols floats)."""
         mask = layer_mask(names)
         order = [n for k, n in enumerate(LAYERS) if (mask >> k) & 1]
         rows, cols = self._shape() if self._g else (0, 0)
         if memory == MEM_HOST:
-            out = np.empty((len(order), cols, rows), dtype=np.float32)   # layer k column-major at k * rows * cols
+            out = np.empty((len(order), self._n, cols, rows), dtype=np.float32)   # per layer the maps back to back, column-major
         fn = self._L.te_map_get_layers
         fn.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_int]
         self._ctx._order_after_torch(memory)
         self._check(fn(self._h, mask, _addr(out), memory))
-        v = out.reshape(len(order), cols, rows)
-        return {n: v[k].T for k, n in enumerate(order)}
+        if self._n == 1:
+            v = out.reshape(len(order), cols, rows)
+            return {n: v[k].T for k, n in enumerate(order)}
+        v = out.reshape(len(order), self._n, cols, rows)
+        return {n: v[k].swapaxes(1, 2) for k, n in enumerate(order)}
 
     def get_submaps(self, positions, lengths, names, out=None, memory=MEM_HOST):
         """te_map_get_submaps (the get_traversability_map service per window): one (info, layers) pair per window, info a
         SUBMAP_INFO_DTYPE record and layers a dict name -> (rows_k, cols_k) submap layer, or None for a failed window.  Host
         memory: numpy arrays (out=None: sized by submap_geometry).  Device memory: `out` is a float32 device tensor with room for
         every window, filled asynchronously on the context stream; the layers are views of it."""
+        return self._submaps(None, positions, lengths, names, out, memory)
+
+    def get_submaps_batched(self, win_map, positions, lengths, names, out=None, memory=MEM_HOST):
+        """te_map_get_submaps_batched: get_submaps with window k taken from map win_map[k] (int32 per window)."""
+        return self._submaps(win_map, positions, lengths, names, out, memory)
+
+    def _submaps(self, win_map, positions, lengths, names, out, memory):
         mask = layer_mask(names)
         order = [n for k, n in enumerate(LAYERS) if (mask >> k) & 1]
         p, ln = _windows(positions, lengths)
@@ -836,10 +921,19 @@ class Map:
             out = np.empty(len(order) * int((geo["rows"].astype(np.int64) * geo["cols"]).sum()), dtype=np.float32)
         cap = out.size if isinstance(out, np.ndarray) else out.numel()
         info = np.zeros(len(p), dtype=SUBMAP_INFO_DTYPE)
-        fn = self._L.te_map_get_submaps
-        fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]
         self._ctx._order_after_torch(memory)
-        self._check(fn(self._h, len(p), p.ctypes.data, ln.ctypes.data, mask, info.ctypes.data, _addr(out), cap, memory))
+        if win_map is None:
+            fn = self._L.te_map_get_submaps
+            fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]
+            self._check(fn(self._h, len(p), p.ctypes.data, ln.ctypes.data, mask, info.ctypes.data, _addr(out), cap, memory))
+        else:
+            wm = np.ascontiguousarray(win_map, dtype=np.int32).reshape(-1)
+            if len(wm) != len(p):
+                raise ValueError("win_map needs one entry per window")
+            fn = self._L.te_map_get_submaps_batched
+            fn.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]
+            self._check(fn(self._h, len(p), wm.ctypes.data, p.ctypes.data, ln.ctypes.data, mask, info.ctypes.data, _addr(out), cap,
+                           memory))
         res = []
         for r in info:
             if not r["success"]:
@@ -860,4 +954,20 @@ class Map:
         fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
         self._ctx._order_after_torch(memory)
         self._check(fn(self._h, len(xy), _addr(xy), _addr(out), memory))
+        return out
+
+    def valid_at_batched(self, pos_map, xy, out=None, memory=MEM_HOST):
+        """te_map_valid_at_batched: valid_at with position q on map pos_map[q].  Host memory: numpy int32 pos_map (a map outside
+        the batch raises).  Device memory: pos_map an int32 device tensor of n (a map outside the batch gives 0), xy and out as in
+        valid_at."""
+        if memory == MEM_HOST:
+            xy = np.ascontiguousarray(xy, dtype=np.float64).reshape(-1, 2)
+            pos_map = np.ascontiguousarray(pos_map, dtype=np.int32).reshape(-1)
+            if len(pos_map) != len(xy):
+                raise ValueError("pos_map needs one entry per position")
+            out = np.zeros(len(xy), dtype=np.uint8)
+        fn = self._L.te_map_valid_at_batched
+        fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+        self._ctx._order_after_torch(memory)
+        self._check(fn(self._h, len(xy), _addr(pos_map), _addr(xy), _addr(out), memory))
         return out

@@ -1295,9 +1295,12 @@ int te_check_footprint_request_batched(te_ctx* c, const te_geometry* g, const te
 }
 
 // ---- te_map: the layers, the traversability_footprint cache and the isTraversableForFilters memo, resident on the device -------
+// A te_map holds nmaps maps of one geometry in the layout of te_chain_batched: map m starts m * rows * cols cells into every layer,
+// the cache and the memo.  The single-map entries are the nmaps = 1 case of the same bodies.
 struct te_map {
   te_ctx* ctx = nullptr;
   bool have_layers = false;
+  int nmaps = 1;
   te_geometry geo_in{};  // as the layers came (host memory: with their circular-buffer start index)
   te_geometry geo{};     // the same with the start index cleared: the device layers are in default order
   DevBuf trav, slope, step, rough, elev, rslope, cache, fresh;
@@ -1313,51 +1316,73 @@ struct te_map {
 namespace {
 
 size_t map_cells(const te_map* m) { return (size_t)m->geo.rows * m->geo.cols; }
+size_t batch_cells(const te_map* m) { return map_cells(m) * m->nmaps; }  // every map of the te_map
 
 int map_ready(const te_map* m) {
   if (!m->have_layers) return fail(TE_ERR_BAD_ARG, "the map has no layers yet: call te_map_chain or te_map_set_layers first");
   return TE_OK;
 }
 
-// New layers: the geometry, an empty cache and a memo to be rebuilt.
-int map_reset(te_map* m, const te_geometry* g_in, const te_geometry* g) {
+// The entries that address one map of a te_map by position take a map index on a batch (the `_batched` entry).
+int map_single(const te_map* m, const char* batched) {
+  if (m->nmaps > 1) return fail(TE_ERR_BAD_ARG, "the te_map holds %d maps: call %s with a map index", m->nmaps, batched);
+  return TE_OK;
+}
+
+// A host array of map indices of a batched entry: every entry in 0 .. nmaps-1.
+int check_map_indices(const te_map* m, const int32_t* idx, int32_t n, const char* what) {
+  if (n > 0 && !idx) return fail(TE_ERR_BAD_ARG, "%s is null", what);
+  for (int32_t k = 0; k < n; ++k)
+    if (idx[k] < 0 || idx[k] >= m->nmaps) return fail(TE_ERR_BAD_ARG, "%s[%d] = %d is outside 0..%d", what, k, idx[k], m->nmaps - 1);
+  return TE_OK;
+}
+
+// New layers for nmaps maps of geometry g: the geometry, an empty cache and a memo to be rebuilt.  Checks the batch limits of the
+// stateless batched entries (a start index on a batch is TE_ERR_UNSUPPORTED: unwrap_geometry).
+int map_reset(te_map* m, const te_geometry* g_in, const te_geometry* g, int nmaps) {
   te_ctx* c = m->ctx;
-  const size_t bytes = sizeof(float) * (size_t)g->rows * g->cols;
+  if (int rc = check_footprint_batch(g, nmaps)) return rc;
+  const size_t bytes = sizeof(float) * (size_t)g->rows * g->cols * nmaps;
   for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->elev, &m->cache}) TE_CUDA(b->reserve(bytes));
   TE_CUDA(cudaMemsetAsync(m->cache.p, 0xff, bytes, c->stream));  // all-ones bits: NaN, the empty cache of computeTraversability (:225-228)
   m->geo_in = *g_in;
   m->geo = *g;
+  m->nmaps = nmaps;
   m->memo_valid = false;
   m->have_layers = false;
   return TE_OK;
 }
 
-// One layer into the map: host layers are unwrapped from their start index; device layers are copied.
+// One layer of every map into the te_map: host layers are unwrapped from their start index (a single map only); device layers are
+// copied.
 int map_put_layer(te_map* m, DevBuf& dst, const float* src, int memory) {
   te_ctx* c = m->ctx;
   const te_geometry& g = m->geo_in;
-  TE_CUDA(dst.reserve(sizeof(float) * map_cells(m)));
-  if (memory == TE_MEM_HOST) TE_CUDA(upload_cols((float*)dst.p, src, g.rows, g.cols, g.start_row, g.start_col, 0, g.cols, c->stream));
-  else TE_CUDA(cudaMemcpyAsync(dst.p, src, sizeof(float) * map_cells(m), cudaMemcpyDeviceToDevice, c->stream));
+  TE_CUDA(dst.reserve(sizeof(float) * batch_cells(m)));
+  if (memory == TE_MEM_HOST)
+    TE_CUDA(upload_cols((float*)dst.p, src, g.rows, g.cols, g.start_row, g.start_col, 0, g.cols * m->nmaps, c->stream));
+  else TE_CUDA(cudaMemcpyAsync(dst.p, src, sizeof(float) * batch_cells(m), cudaMemcpyDeviceToDevice, c->stream));
   return TE_OK;
 }
 
-// A map layer out: host layers are re-wrapped to the map's start index (the caller synchronises); device layers are copied.
+// A layer of every map out: host layers are re-wrapped to the map's start index (the caller synchronises); device layers are copied.
 int map_get_layer(te_map* m, float* dst, const void* src, int memory) {
   te_ctx* c = m->ctx;
   const te_geometry& g = m->geo_in;
-  if (memory == TE_MEM_HOST) TE_CUDA(download_cols(dst, (const float*)src, g.rows, g.cols, g.start_row, g.start_col, 0, g.cols, c->stream));
-  else TE_CUDA(cudaMemcpyAsync(dst, src, sizeof(float) * map_cells(m), cudaMemcpyDeviceToDevice, c->stream));
+  if (memory == TE_MEM_HOST)
+    TE_CUDA(download_cols(dst, (const float*)src, g.rows, g.cols, g.start_row, g.start_col, 0, g.cols * m->nmaps, c->stream));
+  else TE_CUDA(cudaMemcpyAsync(dst, src, sizeof(float) * batch_cells(m), cudaMemcpyDeviceToDevice, c->stream));
   return TE_OK;
 }
 
 // The resident isTraversableForFilters memo for these parameters: kept while the layers and max_gap_width, critical_step_height
-// and verify_roughness (all that checkForStep / checkForSlope / checkForRoughness read) stay the same, cleared otherwise.
+// and verify_roughness (all that checkForStep / checkForSlope / checkForRoughness read) stay the same, cleared otherwise.  One byte
+// per cell of every map.
 int map_memo(te_map* m, const te_footprint_params* p) {
   const int rough = p->verify_roughness != 0;
   if (m->memo_valid && m->memo_gap == p->max_gap_width && m->memo_crit == p->critical_step_height && m->memo_rough == rough) return TE_OK;
-  TE_CUDA(m->fp.memo.reserve(map_cells(m)));
-  TE_CUDA(cudaMemsetAsync(m->fp.memo.p, 0, map_cells(m), m->ctx->stream));
+  TE_CUDA(m->fp.memo.reserve(batch_cells(m)));
+  TE_CUDA(cudaMemsetAsync(m->fp.memo.p, 0, batch_cells(m), m->ctx->stream));
   m->memo_valid = true;
   m->memo_gap = p->max_gap_width;
   m->memo_crit = p->critical_step_height;
@@ -1419,17 +1444,20 @@ int te_map_destroy(te_map* m) {
   return TE_OK;
 }
 
-int te_map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, const float* elev, float* slope, float* step, float* rough,
-                 float* trav, int memory) {
-  TE_MAP_ENTER(m);
+namespace {
+
+// te_map_chain (nmaps = 1) and te_map_chain_batched.
+int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int nmaps, const float* elev, float* slope, float* step,
+              float* rough, float* trav, int memory) {
+  te_ctx* c = m->ctx;
   te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST, &g0)) return rc;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) return rc;
   if (int rc = check_params(p)) return rc;
   if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
-  if (int rc = map_reset(m, g_in, &g0)) return rc;
-  TE_CUDA(m->rough.reserve(sizeof(float) * map_cells(m)));
+  if (int rc = map_reset(m, g_in, &g0, nmaps)) return rc;
+  TE_CUDA(m->rough.reserve(sizeof(float) * batch_cells(m)));
   if (int rc = map_put_layer(m, m->elev, elev, memory)) return rc;
-  if (int rc = chain_common(c, &g0, nullptr, p, 1, (const float*)m->elev.p, (float*)m->slope.p, (float*)m->step.p, (float*)m->rough.p,
+  if (int rc = chain_common(c, &g0, nullptr, p, nmaps, (const float*)m->elev.p, (float*)m->slope.p, (float*)m->step.p, (float*)m->rough.p,
                             (float*)m->trav.p, nullptr, nullptr, nullptr, TE_MEM_DEVICE))
     return rc;
   m->have_rough = true;
@@ -1443,16 +1471,17 @@ int te_map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, c
   return TE_OK;
 }
 
-int te_map_set_layers(te_map* m, const te_geometry* g_in, const float* trav, const float* slope, const float* step, const float* rough,
-                      const float* elev, const float* robot_slope, int memory) {
-  TE_MAP_ENTER(m);
+// te_map_set_layers (nmaps = 1) and te_map_set_layers_batched.
+int map_set_layers(te_map* m, const te_geometry* g_in, int nmaps, const float* trav, const float* slope, const float* step,
+                   const float* rough, const float* elev, const float* robot_slope, int memory) {
+  te_ctx* c = m->ctx;
   te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST, &g0)) return rc;
+  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) return rc;
   if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
   if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
   if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
   if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
-  if (int rc = map_reset(m, g_in, &g0)) return rc;
+  if (int rc = map_reset(m, g_in, &g0, nmaps)) return rc;
   if (int rc = map_put_layer(m, m->trav, trav, memory)) return rc;
   if (int rc = map_put_layer(m, m->slope, slope, memory)) return rc;
   if (int rc = map_put_layer(m, m->step, step, memory)) return rc;
@@ -1468,6 +1497,32 @@ int te_map_set_layers(te_map* m, const te_geometry* g_in, const float* trav, con
   return TE_OK;
 }
 
+}  // namespace
+
+int te_map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, const float* elev, float* slope, float* step, float* rough,
+                 float* trav, int memory) {
+  TE_MAP_ENTER(m);
+  return map_chain(m, g_in, p, 1, elev, slope, step, rough, trav, memory);
+}
+
+int te_map_chain_batched(te_map* m, const te_geometry* g, const te_chain_params* p, int32_t nmaps, const float* elev, float* slope,
+                         float* step, float* rough, float* trav, int memory) {
+  TE_MAP_ENTER(m);
+  return map_chain(m, g, p, nmaps, elev, slope, step, rough, trav, memory);
+}
+
+int te_map_set_layers(te_map* m, const te_geometry* g_in, const float* trav, const float* slope, const float* step, const float* rough,
+                      const float* elev, const float* robot_slope, int memory) {
+  TE_MAP_ENTER(m);
+  return map_set_layers(m, g_in, 1, trav, slope, step, rough, elev, robot_slope, memory);
+}
+
+int te_map_set_layers_batched(te_map* m, const te_geometry* g, int32_t nmaps, const float* trav, const float* slope, const float* step,
+                              const float* rough, const float* elev, const float* robot_slope, int memory) {
+  TE_MAP_ENTER(m);
+  return map_set_layers(m, g, nmaps, trav, slope, step, rough, elev, robot_slope, memory);
+}
+
 int te_map_footprint(te_map* m, const te_footprint_params* p, float* out, int memory) {
   TE_MAP_ENTER(m);
   if (int rc = map_ready(m)) return rc;
@@ -1475,15 +1530,16 @@ int te_map_footprint(te_map* m, const te_footprint_params* p, float* out, int me
   if (!(p->radius >= 0.0) || !(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint radius/offset must be >= 0");
   const te_geometry* g = &m->geo;
   if (int rc = ensure_geometry(c, g)) return rc;
-  TE_CUDA(m->fresh.reserve(sizeof(float) * map_cells(m)));
+  TE_CUDA(m->fresh.reserve(sizeof(float) * batch_cells(m)));
   const te_slab s{0, g->cols, 0, 0};
   const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
   int nl = 0;
-  int rc = te::launch_footprint(m->fp, make_view(c, g, s), g, p, 1, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p,
-                                rough, (const float*)m->elev.p, (float*)m->fresh.p, nullptr, nullptr, nullptr, c->sms, c->stream, &nl);
+  int rc = te::launch_footprint(m->fp, make_view(c, g, s), g, p, m->nmaps, (const float*)m->trav.p, (const float*)m->slope.p,
+                                (const float*)m->step.p, rough, (const float*)m->elev.p, (float*)m->fresh.p, nullptr, nullptr, nullptr,
+                                c->sms, c->stream, &nl);
   if (rc != 0) return fail(rc, "footprint sweep failed: %s", m->fp.why.c_str());
-  te::launch_map_merge((const float*)m->fresh.p, (float*)m->cache.p, (out && memory == TE_MEM_DEVICE) ? out : nullptr, map_cells(m), c->sms,
-                       c->stream);
+  te::launch_map_merge((const float*)m->fresh.p, (float*)m->cache.p, (out && memory == TE_MEM_DEVICE) ? out : nullptr, batch_cells(m),
+                       c->sms, c->stream);
   if (int r2 = launch_check(c, "map footprint", nl + 1)) return r2;
   if (out && memory == TE_MEM_HOST) {
     if (int r2 = map_get_layer(m, out, m->cache.p, memory)) return r2;
@@ -1498,7 +1554,7 @@ static int map_footprint_polygon(te_map* m, const te_footprint_params* p, int32_
                                  const PolygonOutputs* outs, const te::PolygonReduce* reduce, int memory) {
   if (int rc = map_ready(m)) return rc;
   if (int rc = map_footprint_params(m, p)) return rc;
-  return footprint_polygon_common(m->ctx, &m->fp, &m->geo_in, nullptr, p, 1, npts, pts_xy, (const float*)m->trav.p, (const float*)m->slope.p,
+  return footprint_polygon_common(m->ctx, &m->fp, &m->geo_in, nullptr, p, m->nmaps, npts, pts_xy, (const float*)m->trav.p, (const float*)m->slope.p,
                                   (const float*)m->step.p, m->have_rough ? (const float*)m->rough.p : nullptr, (const float*)m->elev.p,
                                   nouts, outs, reduce, memory, true);
 }
@@ -1530,13 +1586,14 @@ int te_map_footprint_polygon_yaws_reduce(te_map* m, const te_footprint_params* p
   return map_footprint_polygon(m, p, npts, pts_xy, 1, outs, &red, memory);
 }
 
-int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int32_t npaths, int32_t nposes, const int32_t* path_begin,
-                                   const double* poses, const double* radius, int32_t nvertices, const int32_t* footprint_begin,
-                                   const float* footprint_xyz, int32_t max_footprint_vertices, const uint8_t* conservative,
-                                   const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area, int32_t max_vertices,
-                                   int32_t* ucount, double* uxy) {
-  TE_MAP_ENTER(m);
-  if (int rc = map_ready(m)) return rc;
+// te_map_check_footprint_request (path_map null: a single map) and te_map_check_footprint_request_batched (path q on map
+// path_map[q], checked by the entry).
+static int map_request(te_map* m, const te_footprint_params* p, const int32_t* path_map, int32_t npaths, int32_t nposes,
+                       const int32_t* path_begin, const double* poses, const double* radius, int32_t nvertices,
+                       const int32_t* footprint_begin, const float* footprint_xyz, int32_t max_footprint_vertices,
+                       const uint8_t* conservative, const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area,
+                       int32_t max_vertices, int32_t* ucount, double* uxy) {
+  te_ctx* c = m->ctx;
   if (int rc = map_footprint_params(m, p)) return rc;
   if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
   if (npaths < 0 || nposes < 0 || nvertices < 0 || !path_begin || !poses || !radius || !footprint_begin ||
@@ -1561,7 +1618,7 @@ int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int3
   if (nvertices > 0) {  // the polygonal paths (TraversabilityMap.cpp:464-584) read the memo and leave the cache alone
     te::PathChecks r{};
     r.trav = (const float*)m->trav.p; r.slope = (const float*)m->slope.p; r.step = (const float*)m->step.p; r.rough = rough;
-    r.elev = (const float*)m->elev.p; r.robot_slope = rslope; r.nmaps = 1;
+    r.elev = (const float*)m->elev.p; r.robot_slope = rslope; r.nmaps = m->nmaps; r.path_map = path_map;
     r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7;
     r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
     r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup; r.max_points = mp;
@@ -1576,9 +1633,9 @@ int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int3
   }
   // the circular paths (TraversabilityMap.cpp:345-462) in request order on the cache; they write their own outputs on the host
   int rc = te::launch_map_circles(m->fp, v, g, p, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p, rough,
-                                  (const float*)m->elev.p, rslope, (float*)m->cache.p, c->hX.data(), c->hY.data(), npaths, path_begin,
-                                  poses, radius, footprint_begin, cup, is_safe, traversability, area, max_vertices, ucount, uxy, c->stream,
-                                  &nl, &m->last);
+                                  (const float*)m->elev.p, rslope, (float*)m->cache.p, m->nmaps, path_map, c->hX.data(), c->hY.data(),
+                                  npaths, path_begin, poses, radius, footprint_begin, cup, is_safe, traversability, area, max_vertices,
+                                  ucount, uxy, c->stream, &nl, &m->last);
   if (rc != 0) return fail(rc, "map request (circular paths) failed: %s", m->fp.why.c_str());
   if (int r2 = launch_check(c, "map request (circular paths)", nl)) return r2;
   if (ucount)  // the row bound of a polygonal path's polygon table (kUntravRows) is only known once the hulls are
@@ -1586,6 +1643,32 @@ int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int3
       if (ucount[q] < 0)
         return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);
   return TE_OK;
+}
+
+int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int32_t npaths, int32_t nposes, const int32_t* path_begin,
+                                   const double* poses, const double* radius, int32_t nvertices, const int32_t* footprint_begin,
+                                   const float* footprint_xyz, int32_t max_footprint_vertices, const uint8_t* conservative,
+                                   const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area, int32_t max_vertices,
+                                   int32_t* ucount, double* uxy) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (int rc = map_single(m, "te_map_check_footprint_request_batched")) return rc;
+  return map_request(m, p, nullptr, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+                     max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy);
+}
+
+int te_map_check_footprint_request_batched(te_map* m, const te_footprint_params* p, const int32_t* path_map, int32_t npaths,
+                                           int32_t nposes, const int32_t* path_begin, const double* poses, const double* radius,
+                                           int32_t nvertices, const int32_t* footprint_begin, const float* footprint_xyz,
+                                           int32_t max_footprint_vertices, const uint8_t* conservative, const uint8_t* cup,
+                                           uint8_t* is_safe, double* traversability, double* area, int32_t max_vertices, int32_t* ucount,
+                                           double* uxy) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (!path_map) return fail(TE_ERR_BAD_ARG, "path_map is null");
+  if (int rc = check_map_indices(m, path_map, std::max(npaths, 0), "path_map")) return rc;
+  return map_request(m, p, path_map, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+                     max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy);
 }
 
 int te_map_get_footprint(te_map* m, float* dst, int memory) {
@@ -1602,7 +1685,7 @@ int te_map_get_footprint(te_map* m, float* dst, int memory) {
 int te_map_clear_footprint(te_map* m) {
   TE_MAP_ENTER(m);
   if (int rc = map_ready(m)) return rc;
-  TE_CUDA(cudaMemsetAsync(m->cache.p, 0xff, sizeof(float) * map_cells(m), c->stream));
+  TE_CUDA(cudaMemsetAsync(m->cache.p, 0xff, sizeof(float) * batch_cells(m), c->stream));
   return TE_OK;
 }
 
@@ -1662,16 +1745,17 @@ int te_map_get_layers(te_map* m, uint32_t layer_mask, float* out, int memory) {
   int nl = 0;
   if (int rc = map_layers(m, layer_mask, src, &nl)) return rc;
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
-  for (int k = 0; k < nl; ++k)
-    if (int rc = map_get_layer(m, out + (size_t)k * map_cells(m), src[k], memory)) return rc;
+  for (int k = 0; k < nl; ++k)  // per layer every map, back to back
+    if (int rc = map_get_layer(m, out + (size_t)k * batch_cells(m), src[k], memory)) return rc;
   if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));
   return TE_OK;
 }
 
-int te_map_get_submaps(te_map* m, int32_t nwin, const double* position_xy, const double* length_xy, uint32_t layer_mask,
-                       te_submap_info* info, float* out, int64_t out_capacity, int memory) {
-  TE_MAP_ENTER(m);
-  if (int rc = map_ready(m)) return rc;
+// te_map_get_submaps (win_map null: map 0) and te_map_get_submaps_batched (window k on map win_map[k], checked by the entry): only
+// the source offset of a window's record depends on its map.
+static int map_submaps(te_map* m, int32_t nwin, const int32_t* win_map, const double* position_xy, const double* length_xy,
+                       uint32_t layer_mask, te_submap_info* info, float* out, int64_t out_capacity, int memory) {
+  te_ctx* c = m->ctx;
   const float* src[7];
   int nl = 0;
   if (int rc = map_layers(m, layer_mask, src, &nl)) return rc;
@@ -1690,7 +1774,8 @@ int te_map_get_submaps(te_map* m, int32_t nwin, const double* position_xy, const
   for (int32_t k = 0; k < nwin; ++k) {
     const te_submap_info& r = info[k];
     if (!r.success) continue;
-    table.push_back(te::SubmapWindow{columns, (long long)r.top_col * m->geo.rows + r.top_row, r.offset, r.rows, r.cols});
+    const long long map0 = win_map ? (long long)win_map[k] * (long long)map_cells(m) : 0;
+    table.push_back(te::SubmapWindow{columns, map0 + (long long)r.top_col * m->geo.rows + r.top_row, r.offset, r.rows, r.cols});
     columns += (long long)nl * r.cols;
   }
   const size_t bytes = sizeof(te::SubmapWindow) * table.size();
@@ -1707,21 +1792,54 @@ int te_map_get_submaps(te_map* m, int32_t nwin, const double* position_xy, const
   return st.finish();
 }
 
-int te_map_valid_at(te_map* m, int32_t n, const double* xy, uint8_t* valid, int memory) {
+int te_map_get_submaps(te_map* m, int32_t nwin, const double* position_xy, const double* length_xy, uint32_t layer_mask,
+                       te_submap_info* info, float* out, int64_t out_capacity, int memory) {
   TE_MAP_ENTER(m);
   if (int rc = map_ready(m)) return rc;
+  if (int rc = map_single(m, "te_map_get_submaps_batched")) return rc;
+  return map_submaps(m, nwin, nullptr, position_xy, length_xy, layer_mask, info, out, out_capacity, memory);
+}
+
+int te_map_get_submaps_batched(te_map* m, int32_t nwin, const int32_t* win_map, const double* position_xy, const double* length_xy,
+                               uint32_t layer_mask, te_submap_info* info, float* out, int64_t out_capacity, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (int rc = check_map_indices(m, win_map, std::max(nwin, 0), "win_map")) return rc;
+  return map_submaps(m, nwin, win_map, position_xy, length_xy, layer_mask, info, out, out_capacity, memory);
+}
+
+// te_map_valid_at (pos_map null: map 0) and te_map_valid_at_batched (position q on map pos_map[q], in `memory`).
+static int map_valid_at(te_map* m, int32_t n, const int32_t* pos_map, const double* xy, uint8_t* valid, int memory) {
+  te_ctx* c = m->ctx;
   if (n < 0) return fail(TE_ERR_BAD_ARG, "negative position count");
   if (n == 0) return TE_OK;
   if (!xy || !valid) return fail(TE_ERR_BAD_ARG, "null argument");
   Staging st(c, memory == TE_MEM_HOST, &m->geo);
   const double* dxy = st.in(xy, 2 * (size_t)n);
+  const int32_t* dmap = st.in(pos_map, (size_t)n);
   uint8_t* dvalid = st.out(valid, (size_t)n);
   if (st.rc) return st.rc;
   const te_geometry& g = m->geo;
   te::launch_valid_at(te::GridGeo{g.rows, g.cols, g.resolution, g.length_x, g.length_y, g.position_x, g.position_y},
-                      (const float*)m->trav.p, n, dxy, dvalid, c->stream);
+                      (const float*)m->trav.p, n, dxy, dmap, m->nmaps, dvalid, c->stream);
   if (int rc = launch_check(c, "k_map_valid_at")) return rc;
   return st.finish();
+}
+
+int te_map_valid_at(te_map* m, int32_t n, const double* xy, uint8_t* valid, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (int rc = map_single(m, "te_map_valid_at_batched")) return rc;
+  return map_valid_at(m, n, nullptr, xy, valid, memory);
+}
+
+int te_map_valid_at_batched(te_map* m, int32_t n, const int32_t* pos_map, const double* xy, uint8_t* valid, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (n > 0 && !pos_map) return fail(TE_ERR_BAD_ARG, "pos_map is null");
+  if (memory == TE_MEM_HOST)  // device memory cannot be read here: the kernel gives 0 for a map outside the batch
+    if (int rc = check_map_indices(m, pos_map, std::max(n, 0), "pos_map")) return rc;
+  return map_valid_at(m, n, pos_map, xy, valid, memory);
 }
 
 // A te IPC handle is the CUDA handle of the ALLOCATION that contains the pointer (cudaIpcGetMemHandle always describes the whole

@@ -1417,14 +1417,16 @@ __global__ void __launch_bounds__(128, 4) k_check_paths_fresh_poly(FpArgs A, Lay
 // ---------------------------------------------------------------------------------------------------------------------------
 // The circular paths of a request on a te_map (launch_map_circles).  The traversability_footprint cache there persists across the
 // paths of a request and across requests, so which isTraversable calls run, and what they read, depends on what earlier calls
-// stored.  The host lists every circle the paths could check (a MapKey per distinct centre, cell, radius and polygon flag);
+// stored.  The host lists every circle the paths could check (a MapKey per distinct map, centre, cell, radius and polygon flag);
 // k_map_eval_circles evaluates every key on the cache as the request found it, one warp per key; the host then replays the
-// service loop in order over these records and writes the cells it stored back with k_map_scatter.
+// service loop in order over these records and writes the cells it stored back with k_map_scatter.  A te_map may hold a batch of
+// maps of one geometry (map m's layers, cache and memo start m * rows * cols cells into theirs); a key belongs to one of them.
 struct MapKey {
   double cx, cy, rmin;  // isTraversable(center, rmin + offset, cup, ..., rmin)
   int ci, cj;           // getIndex(center)
   int cup;              // computeUntraversablePolygon
   int slot;             // row of the hull table for a cup key, -1: no polygon wanted
+  int map;              // the map of the batch (0 on a single map)
 };
 struct MapRecord {
   double t;       // the walk's traversability output (double), or the cached value
@@ -1446,18 +1448,29 @@ __global__ void __launch_bounds__(128) k_map_eval_circles(FpArgs A, Layers L, Pa
   if (k >= nkeys) return;  // whole warp
   const MapKey K = keys[k];
   MapRecord& R = recs[k];
-  const float c0 = __ldg(cache + (size_t)K.cj * A.rows + K.ci);
+  // The key's map: its layers, memo and cache start mo cells in.  The walks take the shifted layer and path arguments from a
+  // per-warp copy in shared memory (by reference, as they take the kernel's own), so no register holds them across the calls.
+  __shared__ Layers s_L[4];
+  __shared__ PathArgs s_P[4];
+  const long long mo = (long long)K.map * A.rows * A.cols_total;
+  const float c0 = __ldg(cache + mo + (size_t)K.cj * A.rows + K.ci);
   if (finitef(c0)) {  // :673-675
     if (lane == 0) { R.t = (double)c0; R.cache = c0; R.state = 2; R.cnt = 0; R.nv = 0; }
     return;
   }
+  if (lane == 0) {
+    s_L[w] = shift_layers_d(L, mo);
+    s_P[w] = P;
+    s_P[w].memo += mo;
+  }
+  __syncwarp();
   const double rmax = K.rmin + P.offset;
   const int nr = (int)ceil(rmax / A.res);
-  const FreshCircle f = fresh_circle_d(A, L, P, K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, nr, K.cup != 0);
+  const FreshCircle f = fresh_circle_d(A, s_L[w], s_P[w], K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, nr, K.cup != 0);
   int cnt = 0, nv = 0;
   if (K.cup && !f.ok && K.slot >= 0) {  // a cup walk fails only within rmin: it collects the blocked cells (:687-730)
     const UntravScratch S{s_min[w], s_max[w], s_stack[w], s_first[w]};
-    cnt = spiral_blockers_d(A, L, P, S, K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, nr);
+    cnt = spiral_blockers_d(A, s_L[w], s_P[w], S, K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, nr);
     if (lane == 0) {
       for (int v = 0; v < min(cnt, 3); ++v) R.first[v] = S.first[v];
       if (cnt >= 2) {
@@ -1474,16 +1487,18 @@ __global__ void __launch_bounds__(128) k_map_eval_circles(FpArgs A, Layers L, Pa
   if (lane == 0) { R.t = f.t; R.cache = f.cache; R.state = f.ok ? 0 : 1; R.cnt = cnt; R.nv = nv; }
 }
 
-// checkInclination of every pose (x, y, x, y) or segment (start, end) the host lists, one thread each.
+// checkInclination of every pose (x, y, x, y) or segment (start, end) the host lists, one thread each, on the robot_slope layer
+// of map seg_map[k] (null: map 0).
 __global__ void __launch_bounds__(128) k_map_inclination(FpArgs A, const float* __restrict__ rslope, const double4* __restrict__ seg,
-                                                         int nseg, unsigned char* __restrict__ ok) {
+                                                         const int* __restrict__ seg_map, int nseg, unsigned char* __restrict__ ok) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= nseg) return;
   const double4 s = seg[k];
+  if (seg_map) rslope += (long long)seg_map[k] * A.rows * A.cols_total;
   ok[k] = inclination_ok_d(A, rslope, s.x, s.y, s.z, s.w) ? 1 : 0;
 }
 
-// The cells the replay stored, written into the cache.
+// The cells the replay stored (cells of the whole batch: map * rows * cols + cell), written into the cache.
 __global__ void __launch_bounds__(256) k_map_scatter(float* __restrict__ cache, const unsigned long long* __restrict__ cell,
                                                      const float* __restrict__ value, int n) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2077,11 +2092,13 @@ int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry*
 }
 
 namespace {
-// The identity of an isTraversable call on an empty cell: its centre, cell, radius and polygon flag, bit for bit.
+// The identity of an isTraversable call on an empty cell: its map, centre, cell, radius and polygon flag, bit for bit.
 struct MapKeyBits {
   unsigned long long cx, cy, r;
-  int ci, cj, cup;
-  bool operator==(const MapKeyBits& o) const { return cx == o.cx && cy == o.cy && r == o.r && ci == o.ci && cj == o.cj && cup == o.cup; }
+  int ci, cj, cup, map;
+  bool operator==(const MapKeyBits& o) const {
+    return cx == o.cx && cy == o.cy && r == o.r && ci == o.ci && cj == o.cj && cup == o.cup && map == o.map;
+  }
 };
 struct MapKeyHash {
   size_t operator()(const MapKeyBits& k) const {
@@ -2089,6 +2106,7 @@ struct MapKeyHash {
     h = (h ^ (h >> 29)) + k.cy * 0xBF58476D1CE4E5B9ULL;
     h = (h ^ (h >> 31)) + k.r * 0x94D049BB133111EBULL;
     h ^= ((unsigned long long)(unsigned)k.ci << 33) ^ ((unsigned long long)(unsigned)k.cj << 1) ^ (unsigned long long)k.cup;
+    h += (unsigned long long)(unsigned)k.map * 0xD6E8FEB86659FD93ULL;
     return (size_t)(h ^ (h >> 32));
   }
 };
@@ -2102,53 +2120,62 @@ size_t align16(size_t b) { return (b + 15) / 16 * 16; }
 
 int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
                        const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                       float* cache, const double* hX, const double* hY, int npaths, const int* path_begin, const double* poses,
-                       const double* radius, const int* footprint_begin, const unsigned char* cup, unsigned char* is_safe,
-                       double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s, int* launches,
-                       MapRequestStats* stats) {
+                       float* cache, int nmaps, const int* path_map, const double* hX, const double* hY, int npaths,
+                       const int* path_begin, const double* poses, const double* radius, const int* footprint_begin,
+                       const unsigned char* cup, unsigned char* is_safe, double* trav_out, double* area_out, int max_vertices, int* ucount,
+                       double* uxy, cudaStream_t s, int* launches, MapRequestStats* stats) {
   *launches = 0;
   *stats = MapRequestStats{};
   const GridGeo G{g->rows, g->cols, g->resolution, g->length_x, g->length_y, g->position_x, g->position_y};
   const bool want_poly = ucount != nullptr;
   const int maxv = std::max(max_vertices, 1);
+  const unsigned long long map_cells = (unsigned long long)g->rows * g->cols;
   auto circular = [&](int q) { return footprint_begin[q + 1] == footprint_begin[q]; };
   auto pose = [&](int k) { return poses + 7 * (size_t)k; };
+  auto map_of = [&](int q) { return path_map ? path_map[q] : 0; };
+  if (nmaps < 1 || (!path_map && nmaps != 1)) { st.why = "a batch of maps needs a map per path"; return TE_ERR_BAD_ARG; }
 
   // 1. every circle the circular paths could check, deduplicated, and every pose / segment checkInclination could read
   std::unordered_map<MapKeyBits, int, MapKeyHash> index;
   std::vector<MapKey> keys;
   std::vector<double4> segs;
+  std::vector<int> seg_map;  // the map of each segment (a batch only)
   std::vector<int> seg_of_pose(robot_slope ? (size_t)path_begin[npaths] : 0, -1);
   int nslots = 0;
-  auto key_of = [&](double cx, double cy, int ci, int cj, double rmin, bool c, bool insert) -> int {
-    const MapKeyBits kb{dbits(cx), dbits(cy), dbits(rmin), ci, cj, c ? 1 : 0};
+  auto key_of = [&](int m, double cx, double cy, int ci, int cj, double rmin, bool c, bool insert) -> int {
+    const MapKeyBits kb{dbits(cx), dbits(cy), dbits(rmin), ci, cj, c ? 1 : 0, m};
     auto it = index.find(kb);
     if (it != index.end()) return it->second;
     if (!insert) return -1;
-    keys.push_back(MapKey{cx, cy, rmin, ci, cj, c ? 1 : 0, (c && want_poly) ? nslots++ : -1});
+    keys.push_back(MapKey{cx, cy, rmin, ci, cj, c ? 1 : 0, (c && want_poly) ? nslots++ : -1, m});
     index.emplace(kb, (int)keys.size() - 1);
     return (int)keys.size() - 1;
   };
+  auto add_seg = [&](int q, int k, double4 sg) {
+    seg_of_pose[k] = (int)segs.size();
+    segs.push_back(sg);
+    if (path_map) seg_map.push_back(path_map[q]);
+  };
   for (int q = 0; q < npaths; ++q) {
     if (!circular(q)) continue;
-    const int b = path_begin[q], n = path_begin[q + 1] - b;
+    const int b = path_begin[q], n = path_begin[q + 1] - b, m = map_of(q);
     const bool c = cup && cup[q];
     for (int k = 0; k < n; ++k) {
       const double ex = pose(b + k)[0], ey = pose(b + k)[1];
       if (n == 1) {
-        if (robot_slope) { seg_of_pose[b] = (int)segs.size(); segs.push_back(make_double4(ex, ey, ex, ey)); }
+        if (robot_slope) add_seg(q, b, make_double4(ex, ey, ex, ey));
         int i, j;
-        if (grid_get_index(G, ex, ey, i, j)) { key_of(ex, ey, i, j, radius[q], c, true); ++stats->candidates; }
+        if (grid_get_index(G, ex, ey, i, j)) { key_of(m, ex, ey, i, j, radius[q], c, true); ++stats->candidates; }
         continue;
       }
       if (k == 0) continue;
       const double sx = pose(b + k - 1)[0], sy = pose(b + k - 1)[1];
-      if (robot_slope) { seg_of_pose[b + k] = (int)segs.size(); segs.push_back(make_double4(sx, sy, ex, ey)); }
+      if (robot_slope) add_seg(q, b + k, make_double4(sx, sy, ex, ey));
       int si, sj, ei, ej;
       if (!grid_get_index(G, sx, sy, si, sj) || !grid_get_index(G, ex, ey, ei, ej)) continue;
       LineD line(ei, ej, si, sj);
       for (int cc = 0; cc < line.n; ++cc, line.next())
-        if ((cc & 3) == 0) { key_of(hX[line.li], hY[line.lj], line.li, line.lj, radius[q], c, true); ++stats->candidates; }
+        if ((cc & 3) == 0) { key_of(m, hX[line.li], hY[line.lj], line.li, line.lj, radius[q], c, true); ++stats->candidates; }
     }
   }
   stats->keys = (long long)keys.size();
@@ -2160,13 +2187,15 @@ int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry*
   std::vector<double> hulls(want_poly ? 2 * (size_t)maxv * nslots : 0);
   if (nkeys > 0 || nseg > 0) {
     if (int rc = ensure_ring_table(st, s)) return rc;
-    const size_t o_keys = 0, o_segs = align16(o_keys + sizeof(MapKey) * nkeys), o_recs = align16(o_segs + sizeof(double4) * nseg);
+    const size_t o_keys = 0, o_segs = align16(o_keys + sizeof(MapKey) * nkeys), o_smap = align16(o_segs + sizeof(double4) * nseg);
+    const size_t o_recs = align16(o_smap + sizeof(int) * seg_map.size());
     const size_t o_incl = align16(o_recs + sizeof(MapRecord) * nkeys), o_hull = align16(o_incl + nseg);
     const size_t bytes = o_hull + sizeof(double) * hulls.size();
     if (st.mapbuf.reserve(std::max<size_t>(bytes, 16)) != cudaSuccess) { st.why = "allocating the map request records failed"; return TE_ERR_CUDA; }
     char* base = (char*)st.mapbuf.p;
     if (cudaMemcpyAsync(base + o_keys, keys.data(), sizeof(MapKey) * nkeys, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-        cudaMemcpyAsync(base + o_segs, segs.data(), sizeof(double4) * nseg, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+        cudaMemcpyAsync(base + o_segs, segs.data(), sizeof(double4) * nseg, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+        cudaMemcpyAsync(base + o_smap, seg_map.data(), sizeof(int) * seg_map.size(), cudaMemcpyHostToDevice, s) != cudaSuccess) {
       st.why = "map request upload failed";
       return TE_ERR_CUDA;
     }
@@ -2179,7 +2208,8 @@ int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry*
       ++*launches;
     }
     if (nseg > 0) {
-      k_map_inclination<<<(unsigned)((nseg + 127) / 128), 128, 0, s>>>(a, robot_slope, (const double4*)(base + o_segs), nseg,
+      k_map_inclination<<<(unsigned)((nseg + 127) / 128), 128, 0, s>>>(a, robot_slope, (const double4*)(base + o_segs),
+                                                                      path_map ? (const int*)(base + o_smap) : nullptr, nseg,
                                                                       (unsigned char*)(base + o_incl));
       ++*launches;
     }
@@ -2193,14 +2223,15 @@ int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry*
   }
 
   // 3. the service loop in request order (checkCircularFootprintPath, TraversabilityMap.cpp:345-462, with publishPolygons = true)
-  // over the records: a cell this request stored reads the overlay, any other cell its own key's record
+  // over the records: a cell this request stored reads the overlay, any other cell its own key's record.  Cells are cells of the
+  // batch (map * rows * cols + cell), so a path sees its own map's cache only.
   std::unordered_map<unsigned long long, float> overlay;
   std::vector<unsigned long long> order;  // overlay cells in the order they were stored
   const CircleTable CT = circle_table();
   const double tdefault = p->traversability_default, offset = p->offset;
   for (int q = 0; q < npaths; ++q) {
     if (!circular(q)) continue;
-    const int b = path_begin[q], n = path_begin[q + 1] - b;
+    const int b = path_begin[q], n = path_begin[q + 1] - b, m = map_of(q);
     const double rmin = radius[q], rmax = rmin + offset;
     const bool c = cup && cup[q];
     // isTraversable(center, rmax, c, t, ..., rmin) (:654-746); `cell` < 0: the centre is outside the map
@@ -2212,11 +2243,11 @@ int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry*
         if (tdefault == 0.0) { fkind = 1; fx = cx; fy = cy; }
         return tdefault != 0.0;
       }
-      const unsigned long long cell = (unsigned long long)cj * g->rows + ci;
+      const unsigned long long cell = (unsigned long long)m * map_cells + (unsigned long long)cj * g->rows + ci;
       float cached;
       bool have = false;
       auto ov = overlay.find(cell);
-      const int k = key_of(cx, cy, ci, cj, rmin, c, false);
+      const int k = key_of(m, cx, cy, ci, cj, rmin, c, false);
       if (ov != overlay.end()) { cached = ov->second; have = true; }
       else if (recs[k].state == 2) { cached = recs[k].cache; have = true; }
       if (have) {  // :673-678

@@ -127,7 +127,9 @@ int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry*
 // A request on a te_map (te_map_check_footprint_request): its polygonal paths run launch_path_checks on the memo the map keeps.
 // Its circular paths: launch_map_circles reads and fills the traversability_footprint cache `cache` (device, NaN = empty) in the
 // reference's order; every path array and output is in HOST memory, hX / hY are the host copies of the cell-centre tables, and
-// the call returns synchronised.
+// the call returns synchronised.  A batch of `nmaps` maps (te_map_check_footprint_request_batched): the layers, robot_slope, the
+// cache and the memo hold map m from m * rows * cols cells on, and path q is on map path_map[q] (HOST memory, checked by the
+// caller); path_map null: one map.
 struct MapRequestStats {
   long long candidates = 0;  // isTraversable calls the circular paths could make
   long long keys = 0;        // distinct circles among them (what k_map_eval_circles evaluates)
@@ -135,10 +137,10 @@ struct MapRequestStats {
 };
 int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
                        const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                       float* cache, const double* hX, const double* hY, int npaths, const int* path_begin, const double* poses,
-                       const double* radius, const int* footprint_begin, const unsigned char* cup, unsigned char* is_safe,
-                       double* trav_out, double* area_out, int max_vertices, int* ucount, double* uxy, cudaStream_t s, int* launches,
-                       MapRequestStats* stats);
+                       float* cache, int nmaps, const int* path_map, const double* hX, const double* hY, int npaths,
+                       const int* path_begin, const double* poses, const double* radius, const int* footprint_begin,
+                       const unsigned char* cup, unsigned char* is_safe, double* trav_out, double* area_out, int max_vertices, int* ucount,
+                       double* uxy, cudaStream_t s, int* launches, MapRequestStats* stats);
 // traversabilityFootprint(radius, offset) on a cache: cache = finite(cache) ? cache : fresh over n cells; `out` (device, may be
 // null) receives the result too.
 int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, int sms, cudaStream_t s);

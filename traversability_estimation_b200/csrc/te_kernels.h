@@ -64,6 +64,9 @@ struct SubmapGather {
 void launch_gather_submaps(const SubmapGather& a, int sms, cudaStream_t s);
 struct GridGeo;
 // valid[q] = getIndex(xy[2q], xy[2q+1]) succeeds and traversability is finite there (device pointers; none launched for n = 0).
-void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, unsigned char* valid, cudaStream_t s);
+// A batch of nmaps maps of geometry g back to back in `trav`: position q is on map pos_map[q] (null: map 0), and a map outside
+// 0 .. nmaps-1 gives 0.
+void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, const int* pos_map, int nmaps, unsigned char* valid,
+                     cudaStream_t s);
 
 }  // namespace te

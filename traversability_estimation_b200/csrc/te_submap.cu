@@ -43,10 +43,16 @@ __global__ void __launch_bounds__(kGatherWarps * 32) k_map_gather_submaps(Submap
   }
 }
 
+// Position q on map pos_map[q] of a batch of nmaps maps (pos_map null: map 0); a map outside the batch gives 0.
 __global__ void k_map_valid_at(GridGeo g, const float* __restrict__ trav, int n, const double* __restrict__ xy,
-                               unsigned char* __restrict__ valid) {
+                               const int* __restrict__ pos_map, int nmaps, unsigned char* __restrict__ valid) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n) return;
+  if (pos_map) {
+    const int m = pos_map[q];
+    if (m < 0 || m >= nmaps) { valid[q] = 0; return; }
+    trav += (size_t)m * g.rows * g.cols_total;
+  }
   int i, j;
   const bool in = grid_get_index(g, xy[2 * q], xy[2 * q + 1], i, j);
   valid[q] = in && finitef(__ldg(trav + (size_t)j * g.rows + i)) ? 1 : 0;
@@ -60,9 +66,10 @@ void launch_gather_submaps(const SubmapGather& a, int sms, cudaStream_t s) {
   k_map_gather_submaps<<<(unsigned)blocks, kGatherWarps * 32, 0, s>>>(a);
 }
 
-void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, unsigned char* valid, cudaStream_t s) {
+void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, const int* pos_map, int nmaps, unsigned char* valid,
+                     cudaStream_t s) {
   if (n <= 0) return;
-  k_map_valid_at<<<(n + 255) / 256, 256, 0, s>>>(g, trav, n, xy, valid);
+  k_map_valid_at<<<(n + 255) / 256, 256, 0, s>>>(g, trav, n, xy, pos_map, nmaps, valid);
 }
 
 }  // namespace te
