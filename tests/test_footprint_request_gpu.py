@@ -282,8 +282,6 @@ def test_error_codes(te, ctx, oracle):
                   len(fx) if nvertices is None else nvertices, fbeg.ctypes.data, fx.ctypes.data, mfv, ad(cons), ad(cup),
                   *(a.ctypes.data for a in out[:3]), maxv, out[3].ctypes.data, out[4].ctypes.data, memory)
 
-    # sets argtypes
-    ctx.check_footprint_request(g, ft, one, one, one, one * 0, [0, 1], [pose], [0.3], [0, 0], np.zeros((0, 3), np.float32))
     assert call([0, 4, 3]) == 0
     assert call([]) == 0                                            # npaths = 0
     # new: max_footprint_vertices, footprint_begin, vertex bound, non-finite vertex

@@ -250,10 +250,6 @@ def test_map_entries(te, ctx):
     rd = (torch.full((cols, rows), SENTINEL, device="cuda"), torch.full((cols, rows), SENTINEL, device="cuda"),
           torch.full((cols, rows), -7, dtype=torch.int32, device="cuda"))
     Lb = ctx._L
-    Lb.te_map_footprint_polygon_yaws.argtypes = [C.c_void_p, C.POINTER(te.FootprintParams), C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
-                                                 C.c_void_p, C.c_int]
-    Lb.te_map_footprint_polygon_yaws_reduce.argtypes = [C.c_void_p, C.POINTER(te.FootprintParams), C.c_int32, C.c_void_p, C.c_int32,
-                                                        C.c_void_p] + [C.c_void_p] * 3 + [C.c_int]
     assert Lb.te_map_footprint_polygon_yaws(mw._h, C.byref(p), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data, od.data_ptr(),
                                             te.MEM_DEVICE) == 0
     assert Lb.te_map_footprint_polygon_yaws_reduce(mw._h, C.byref(p), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data,

@@ -97,7 +97,6 @@ def test_submap_geometry_rejects_bad_windows_before_writing(te, pos, length):
     p = np.array([[0.1, 0.1], pos], dtype=np.float64)
     ln = np.array([[0.2, 0.2], length], dtype=np.float64)
     info = np.full(2, 7, dtype=te.capi.SUBMAP_INFO_DTYPE)
-    L.te_submap_geometry.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     assert L.te_submap_geometry(C.byref(g), 2, p.ctypes.data, ln.ctypes.data, info.ctypes.data) == -1
     assert (info["rows"] == 7).all() and (info["offset"] == 7).all()   # nothing written
     with pytest.raises(te.TEError) as e:
@@ -107,7 +106,6 @@ def test_submap_geometry_rejects_bad_windows_before_writing(te, pos, length):
 
 def test_submap_geometry_argument_errors(te):
     L = te.load_library()
-    L.te_submap_geometry.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     g = te.Geometry.make(50, 50, 0.02)
     p = np.zeros(2)
     info = np.zeros(1, dtype=te.capi.SUBMAP_INFO_DTYPE)
@@ -130,7 +128,5 @@ def test_layer_mask_and_map_entries_without_a_map(te):
         with pytest.raises(ValueError):
             te.capi.layer_mask(names)
     L = te.load_library()
-    L.te_map_get_layers.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_int]
-    L.te_map_valid_at.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
     assert L.te_map_get_layers(None, 1, None, 0) == -1
     assert L.te_map_valid_at(None, 0, None, None, 0) == -1

@@ -1,8 +1,6 @@
 """The read side of a te_map on the GPU, bit for bit: te_map_get_layers against the layers that went in or came out of the chain,
 te_map_get_submaps against numpy slices at the CPU oracle's getSubmap geometry (tests/submap_oracle.cpp), and te_map_valid_at
 against the oracle's getIndex + isfinite."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -123,7 +121,6 @@ def test_layer_errors(te, ctx):
             m.get_submaps([[0.3, -0.2]], [[0.5, 0.5]], [name])
         assert e.value.code == -2
     L = te.load_library()
-    L.te_map_get_layers.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_int]
     buf = np.zeros(ROWS * COLS, dtype=np.float32)
     assert L.te_map_get_layers(m._h, 0, buf.ctypes.data, 0) == -1          # empty mask
     assert L.te_map_get_layers(m._h, 0x80, buf.ctypes.data, 0) == -1       # unknown bit
@@ -213,7 +210,6 @@ def test_capacity_retry_failed_windows_and_launch_count(te, ctx):
     m, L = _set(te, ctx, seed=9)
     Lib = te.load_library()
     fn = Lib.te_map_get_submaps
-    fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]
     pos = np.array([[0.37, -0.21], [50.0, 50.0], [0.2, -0.1], [-50.0, 0.0]])      # windows 1 and 3 lie outside the map
     length = np.array([[0.5, 0.4], [1.0, 1.0], [0.1, 0.3], [1.0, 1.0]])
     mask = 0x11

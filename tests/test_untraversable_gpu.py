@@ -295,7 +295,6 @@ def test_error_codes(te, ctx, oracle):
     begin, poses, radius = np.array([0, 1], np.int32), np.zeros((1, 2)), np.array([0.3])
     ft, _ = footprint_params(te, oracle, 0)
     lib = te.load_library()
-    ctx.check_footprint_paths_fresh(g, ft, one, one, one, one * 0, begin, poses, radius, untraversable_capacity=4)  # sets argtypes
     fresh = lib.te_check_footprint_paths_fresh2
     s8, d1, c1, xy = np.zeros(1, np.uint8), np.zeros(1), np.zeros(1, np.int32), np.zeros(8)
     L = [one.ctypes.data, one.ctypes.data, one.ctypes.data, None, one.ctypes.data, None]
@@ -309,8 +308,6 @@ def test_error_codes(te, ctx, oracle):
     assert f(0, c1.ctypes.data, None) == 0 and c1[0] == 0       # counts only
     assert f(0, None, None) == 0                                # exactly te_check_footprint_paths_fresh
     fxyz = np.asarray(YAML, np.float32)
-    ctx.check_footprint_paths_polygon(g, ft, one, one, one, one * 0, fxyz, begin, np.array([[0.0, 0, 0, 0, 0, 0, 1]]),
-                                      untraversable_capacity=4)
     poly = lib.te_check_footprint_paths_polygon2
     pose = np.array([[0.0, 0, 0, 0, 0, 0, 1]])
     cup = np.ones(1, np.uint8)

@@ -124,8 +124,6 @@ def main():
     stream = torch.cuda.Stream()
     ctx.set_stream(stream.cuda_stream)
     L = te.load_library()
-    L.te_check_footprint_paths2.argtypes = [C.c_void_p, C.POINTER(te.Geometry), C.c_void_p, C.c_void_p, C.c_double, C.c_int32] + \
-        [C.c_void_p] * 4 + [C.c_int]
     name, power = gpu_info(torch)
     rng = np.random.default_rng(1)
     for batch in (1, 100, 1000):

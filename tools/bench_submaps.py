@@ -93,9 +93,7 @@ def main():
     elev = torch.from_numpy(np.ascontiguousarray(synth.terrain(n, n, RES, 7, "mixed").T)).pin_memory()
     outs = [torch.empty((n, n), dtype=torch.float32).pin_memory() for _ in range(4)]
     chain = L.te_map_chain
-    chain.argtypes = [C.c_void_p, C.POINTER(te.Geometry), C.POINTER(te.ChainParams)] + [C.c_void_p] * 5 + [C.c_int]
     get = L.te_map_get_submaps
-    get.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]
     mask = te.capi.layer_mask(HELD)
     cell_bytes = 4 * n * n
     rng = np.random.default_rng(3)

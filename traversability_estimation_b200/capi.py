@@ -16,17 +16,6 @@ _LIB = os.environ.get("TE_B200_LIBRARY") or os.path.join(_HERE, "libte_b200.so")
 MEM_HOST, MEM_DEVICE = 0, 1
 KERNEL_AUTO, KERNEL_GENERIC, KERNEL_FUSED = 0, 1, 2
 
-EXPORTS = ["te_create", "te_destroy", "te_last_error", "te_abi_version", "te_set_stream", "te_synchronize",
-           "te_set_kernel", "te_get_stats", "te_enable_timing", "te_get_timing", "te_get_flag_counters", "te_get_escalation_stats", "te_fused_plan", "te_slope", "te_normals", "te_step", "te_roughness", "te_chain",
-           "te_chain_batched", "te_footprint", "te_footprint2", "te_footprint_polygon", "te_footprint_batched", "te_footprint_polygon_batched", "te_footprint_polygon_yaws", "te_footprint_polygon_yaws_reduce", "te_check_footprint_paths", "te_check_footprint_paths2", "te_check_footprint_paths_fresh", "te_check_footprint_paths_polygon", "te_check_footprint_paths_fresh2", "te_check_footprint_paths_polygon2", "te_check_footprint_request", "te_check_footprint_request_batched", "te_ipc_export", "te_ipc_open", "te_ipc_close", "te_event_create_ipc", "te_event_open_ipc",
-           "te_event_record", "te_event_destroy", "te_halo_pull", "te_host_alloc", "te_host_free", "te_map_create", "te_map_destroy",
-           "te_map_chain", "te_map_set_layers", "te_map_footprint", "te_map_footprint_polygon", "te_map_footprint_polygon_yaws", "te_map_footprint_polygon_yaws_reduce",
-           "te_map_check_footprint_request",
-           "te_map_get_footprint", "te_map_clear_footprint", "te_map_request_stats", "te_submap_geometry", "te_map_get_layers",
-           "te_map_get_submaps", "te_map_valid_at", "te_map_chain_batched", "te_map_set_layers_batched",
-           "te_map_check_footprint_request_batched", "te_map_get_submaps_batched", "te_map_valid_at_batched"]
-
-
 IPC_HANDLE_BYTES = 80  # TE_IPC_HANDLE_BYTES
 
 # te_layer: bit k of a layer mask is LAYERS[k]; outputs that hold several layers have them in this order.
@@ -117,6 +106,83 @@ class FootprintParams(C.Structure):
         return cls(0.30, 0.15, 0.3, 0.3, 0.12, 1, 0)
 
 
+# Every entry point of include/te_b200.h in header order: name -> (restype, argtypes), applied once by load_library().  Without
+# argtypes ctypes passes a Python int as a C int, so an undeclared entry would get truncated addresses.  Kinds: handles (te_ctx*,
+# te_map*), void* and every data pointer or array, host or device, are c_void_p; a parameter struct is a POINTER to its Structure
+# (pass byref(s) or s); int and int32_t are c_int32.  tests/test_capi_signatures_cpu.py checks the table against the header.
+_P, _I, _U, _L, _Z, _D = C.c_void_p, C.c_int32, C.c_uint32, C.c_int64, C.c_size_t, C.c_double
+_G, _S, _CP, _FP, _HP = (C.POINTER(s) for s in (Geometry, Slab, ChainParams, FootprintParams, HaloPeer))
+_R = C.c_int
+SIGNATURES = {
+    "te_create": (_R, [_P, _I]),
+    "te_destroy": (_R, [_P]),
+    "te_last_error": (C.c_char_p, []),
+    "te_abi_version": (_R, []),
+    "te_host_alloc": (_R, [_P, _Z]),
+    "te_host_free": (_R, [_P]),
+    "te_set_stream": (_R, [_P, _P]),
+    "te_synchronize": (_R, [_P]),
+    "te_set_kernel": (_R, [_P, _I]),
+    "te_get_stats": (_R, [_P, _P, _P]),
+    "te_enable_timing": (_R, [_P, _I]),
+    "te_get_timing": (_R, [_P, _P, _P, _P]),
+    "te_get_flag_counters": (_R, [_P, _P]),
+    "te_get_escalation_stats": (_R, [_P, _P, _P]),
+    "te_fused_plan": (_R, [_I, _I, _I, _I, _P]),
+    "te_slope": (_R, [_P, _G, _D, _P, _P, _I]),
+    "te_normals": (_R, [_P, _G, _CP, _P, _P, _P, _P, _I]),
+    "te_step": (_R, [_P, _G, _CP, _P, _P, _I]),
+    "te_roughness": (_R, [_P, _G, _CP, _P, _P, _P, _P, _P, _I]),
+    "te_chain": (_R, [_P, _G, _S, _CP, _P, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_chain_batched": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _I]),
+    "te_footprint": (_R, [_P, _G, _S, _FP, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_footprint2": (_R, [_P, _G, _S, _FP, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_footprint_polygon": (_R, [_P, _G, _S, _FP, _I, _P, _D, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_footprint_batched": (_R, [_P, _G, _FP, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_footprint_polygon_batched": (_R, [_P, _G, _FP, _I, _I, _P, _D, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_footprint_polygon_yaws": (_R, [_P, _G, _FP, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_footprint_polygon_yaws_reduce": (_R, [_P, _G, _FP, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_check_footprint_paths": (_R, [_P, _G, _P, _D, _I, _P, _P, _P, _P, _I]),
+    "te_check_footprint_paths2": (_R, [_P, _G, _P, _P, _D, _I, _P, _P, _P, _P, _I]),
+    "te_check_footprint_paths_fresh": (_R, [_P, _G, _FP, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I]),
+    "te_check_footprint_paths_polygon": (_R, [_P, _G, _FP, _P, _P, _P, _P, _P, _P, _I, _P, _I, _I, _P, _P, _P, _P, _P, _P, _I]),
+    "te_check_footprint_paths_fresh2": (_R, [_P, _G, _FP, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _P, _P, _I]),
+    "te_check_footprint_paths_polygon2": (_R, [_P, _G, _FP, _P, _P, _P, _P, _P, _P, _I, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _I]),
+    "te_check_footprint_request": (_R, [_P, _G, _FP, _P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P, _I]),
+    "te_check_footprint_request_batched": (_R, [_P, _G, _FP, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P, _I]),
+    "te_map_create": (_R, [_P, _P]),
+    "te_map_destroy": (_R, [_P]),
+    "te_map_chain": (_R, [_P, _G, _CP, _P, _P, _P, _P, _P, _I]),
+    "te_map_set_layers": (_R, [_P, _G, _P, _P, _P, _P, _P, _P, _I]),
+    "te_map_chain_batched": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _I]),
+    "te_map_set_layers_batched": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _I]),
+    "te_map_footprint": (_R, [_P, _FP, _P, _I]),
+    "te_map_footprint_polygon": (_R, [_P, _FP, _I, _P, _D, _P, _P, _I]),
+    "te_map_footprint_polygon_yaws": (_R, [_P, _FP, _I, _P, _I, _P, _P, _I]),
+    "te_map_footprint_polygon_yaws_reduce": (_R, [_P, _FP, _I, _P, _I, _P, _P, _P, _P, _I]),
+    "te_map_check_footprint_request": (_R, [_P, _FP, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
+    "te_map_check_footprint_request_batched": (_R, [_P, _FP, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
+    "te_map_get_footprint": (_R, [_P, _P, _I]),
+    "te_map_clear_footprint": (_R, [_P]),
+    "te_map_request_stats": (_R, [_P, _P]),
+    "te_submap_geometry": (_R, [_G, _I, _P, _P, _P]),
+    "te_map_get_layers": (_R, [_P, _U, _P, _I]),
+    "te_map_get_submaps": (_R, [_P, _I, _P, _P, _U, _P, _P, _L, _I]),
+    "te_map_get_submaps_batched": (_R, [_P, _I, _P, _P, _P, _U, _P, _P, _L, _I]),
+    "te_map_valid_at": (_R, [_P, _I, _P, _P, _I]),
+    "te_map_valid_at_batched": (_R, [_P, _I, _P, _P, _P, _I]),
+    "te_ipc_export": (_R, [_P, _P]),
+    "te_ipc_open": (_R, [_P, _P]),
+    "te_ipc_close": (_R, [_P]),
+    "te_event_create_ipc": (_R, [_P, _P, _P]),
+    "te_event_open_ipc": (_R, [_P, _P]),
+    "te_event_record": (_R, [_P, _P]),
+    "te_event_destroy": (_R, [_P]),
+    "te_halo_pull": (_R, [_P, _G, _S, _P, _HP, _HP]),
+}
+EXPORTS = list(SIGNATURES)
+
+
 def library_path() -> str:
     return _LIB
 
@@ -140,34 +206,10 @@ def load_library():
             raise ImportError(f"{_LIB} is missing: run traversability_estimation_b200.build_library() "
                               "(there is no CPU fallback)")
         L = C.CDLL(_LIB)
-        vp, fp = C.c_void_p, C.c_void_p  # layers are passed as raw addresses (host or device)
-        G, S = C.POINTER(Geometry), C.POINTER(Slab)
-        P, F = C.POINTER(ChainParams), C.POINTER(FootprintParams)
-        L.te_create.argtypes = [C.POINTER(vp), C.c_int]
-        L.te_destroy.argtypes = [vp]
-        L.te_last_error.restype = C.c_char_p
-        L.te_set_stream.argtypes = [vp, vp]
-        L.te_synchronize.argtypes = [vp]
-        L.te_set_kernel.argtypes = [vp, C.c_int]
-        L.te_get_stats.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
-        L.te_enable_timing.argtypes = [vp, C.c_int]
-        L.te_get_timing.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
-        L.te_slope.argtypes = [vp, G, C.c_double, fp, fp, C.c_int]
-        L.te_normals.argtypes = [vp, G, P, fp, fp, fp, fp, C.c_int]
-        L.te_step.argtypes = [vp, G, P, fp, fp, C.c_int]
-        L.te_roughness.argtypes = [vp, G, P, fp, fp, fp, fp, fp, C.c_int]
-        L.te_chain.argtypes = [vp, G, S, P, fp, fp, fp, fp, fp, fp, fp, fp, C.c_int]
-        L.te_chain_batched.argtypes = [vp, G, P, C.c_int32, fp, fp, fp, fp, fp, C.c_int]
-        L.te_footprint.argtypes = [vp, G, S, F, fp, fp, fp, fp, fp, fp, fp, C.c_int]
-        L.te_footprint2.argtypes = [vp, G, S, F, fp, fp, fp, fp, fp, fp, fp, fp, fp, C.c_int]
-        L.te_ipc_export.argtypes = [vp, vp]
-        L.te_ipc_open.argtypes = [vp, C.POINTER(vp)]
-        L.te_ipc_close.argtypes = [vp]
-        L.te_event_create_ipc.argtypes = [vp, C.POINTER(vp), vp]
-        L.te_event_open_ipc.argtypes = [vp, C.POINTER(vp)]
-        L.te_event_record.argtypes = [vp, vp]
-        L.te_event_destroy.argtypes = [vp]
-        L.te_halo_pull.argtypes = [vp, G, S, fp, C.POINTER(HaloPeer), C.POINTER(HaloPeer)]
+        for name, (restype, argtypes) in SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype = restype
+            fn.argtypes = argtypes
         _lib = L
     return _lib
 
@@ -176,7 +218,6 @@ def fused_plan(rows: int, out_ncols: int, nmaps: int = 1, sms: int = 132) -> dic
     """te_fused_plan: the (level, map, segment, strip) work units of the fused launch; host arithmetic, no GPU needed."""
     L = load_library()
     out = (C.c_int32 * 19)()
-    L.te_fused_plan.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32)]
     rc = L.te_fused_plan(rows, out_ncols, nmaps, sms, out)
     if rc != 0:
         raise TEError(rc, "te_fused_plan: invalid argument")
@@ -191,7 +232,6 @@ def submap_geometry(g, positions, lengths):
     L = load_library()
     p, ln = _windows(positions, lengths)
     info = np.zeros(len(p), dtype=SUBMAP_INFO_DTYPE)
-    L.te_submap_geometry.argtypes = [C.POINTER(Geometry), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     rc = L.te_submap_geometry(C.byref(g), len(p), p.ctypes.data, ln.ctypes.data, info.ctypes.data)
     if rc != 0:
         raise TEError(rc, L.te_last_error().decode())
@@ -278,14 +318,12 @@ class Context:
 
     def flag_counters(self):
         a = (C.c_uint32 * 5)()
-        self._L.te_get_flag_counters.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
         self._check(self._L.te_get_flag_counters(self._h, a))
         return list(a)
 
     def escalation_stats(self):
         """(cells by escalation reason [16], cells by number of valid window cells [26]) of the last fused launch."""
         a, b = (C.c_uint32 * 16)(), (C.c_uint32 * 26)()
-        self._L.te_get_escalation_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
         self._check(self._L.te_get_escalation_stats(self._h, a, b))
         return list(a), list(b)
 
@@ -331,9 +369,8 @@ class Context:
 
     def footprint_polygon(self, g, fp, polygon_xy, yaw, traversability, slope, step, elevation, out_x, out_rot, memory, slab=None, roughness=None):
         """TraversabilityMap::traversabilityFootprint(yaw): layers traversability_x / traversability_rot for the footprint polygon."""
+        self._order_after_torch(memory)
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
-        self._L.te_footprint_polygon.argtypes = [C.c_void_p, C.POINTER(Geometry), C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p,
-                                                 C.c_double] + [C.c_void_p] * 7 + [C.c_int]
         self._check(self._L.te_footprint_polygon(self._h, C.byref(g), C.byref(slab) if slab is not None else None, C.byref(fp), len(pts),
                                                  pts.ctypes.data, float(yaw), _addr(traversability), _addr(slope), _addr(step), _addr(roughness),
                                                  _addr(elevation), _addr(out_x), _addr(out_rot), memory))
@@ -342,8 +379,6 @@ class Context:
                           roughness=None, roughness_fp=None):
         """footprint() for nmaps whole maps of geometry g stored back to back (the layout of chain_batched)."""
         self._order_after_torch(memory)
-        self._L.te_footprint_batched.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams), C.c_int32] + \
-            [C.c_void_p] * 9 + [C.c_int]
         self._check(self._L.te_footprint_batched(self._h, C.byref(g), C.byref(fp), nmaps, _addr(traversability), _addr(slope),
                                                  _addr(step), _addr(roughness), _addr(elevation), _addr(out), _addr(slope_fp),
                                                  _addr(step_fp), _addr(roughness_fp), memory))
@@ -353,8 +388,6 @@ class Context:
         """footprint_polygon() for nmaps whole maps of geometry g stored back to back (the layout of chain_batched)."""
         self._order_after_torch(memory)
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
-        self._L.te_footprint_polygon_batched.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams), C.c_int32,
-                                                         C.c_int32, C.c_void_p, C.c_double] + [C.c_void_p] * 7 + [C.c_int]
         self._check(self._L.te_footprint_polygon_batched(self._h, C.byref(g), C.byref(fp), nmaps, len(pts), pts.ctypes.data, float(yaw),
                                                          _addr(traversability), _addr(slope), _addr(step), _addr(roughness),
                                                          _addr(elevation), _addr(out_x), _addr(out_rot), memory))
@@ -367,8 +400,6 @@ class Context:
         self._order_after_torch(memory)
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
         ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
-        self._L.te_footprint_polygon_yaws.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams), C.c_int32, C.c_int32,
-                                                      C.c_void_p, C.c_int32, C.c_void_p] + [C.c_void_p] * 6 + [C.c_int]
         self._check(self._L.te_footprint_polygon_yaws(self._h, C.byref(g), C.byref(fp), nmaps, len(pts), pts.ctypes.data, len(ys),
                                                       ys.ctypes.data if len(ys) else None, _addr(traversability), _addr(slope),
                                                       _addr(step), _addr(roughness), _addr(elevation), _addr(out), memory))
@@ -381,8 +412,6 @@ class Context:
         self._order_after_torch(memory)
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
         ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
-        self._L.te_footprint_polygon_yaws_reduce.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams), C.c_int32,
-                                                             C.c_int32, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_void_p] * 8 + [C.c_int]
         self._check(self._L.te_footprint_polygon_yaws_reduce(self._h, C.byref(g), C.byref(fp), nmaps, len(pts), pts.ctypes.data, len(ys),
                                                              ys.ctypes.data if len(ys) else None, _addr(traversability), _addr(slope),
                                                              _addr(step), _addr(roughness), _addr(elevation), _addr(worst), _addr(best),
@@ -397,8 +426,6 @@ class Context:
         xy = np.ascontiguousarray(poses_xy, dtype=np.float64)
         n = len(pb) - 1
         safe, trav = np.zeros(n, dtype=np.uint8), np.zeros(n, dtype=np.float64)
-        self._L.te_check_footprint_paths2.argtypes = [C.c_void_p, C.POINTER(Geometry), C.c_void_p, C.c_void_p, C.c_double, C.c_int32, C.c_void_p,
-                                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         self._check(self._L.te_check_footprint_paths2(self._h, C.byref(g), f.ctypes.data, rs.ctypes.data if rs is not None else None,
                                                       traversability_default, n, pb.ctypes.data, xy.ctypes.data, safe.ctypes.data,
                                                       trav.ctypes.data, MEM_HOST))
@@ -418,14 +445,10 @@ class Context:
         (int32[npaths]: vertex count, 0 none, -1 not computed) and xy (float64[npaths, V, 2]: the first min(count, V) vertices);
         in MEM_DEVICE they are the caller's untraversable_count / untraversable_xy tensors."""
         if untraversable_capacity is None:
-            sig = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + [C.c_int32] + [C.c_void_p] * 6 + [C.c_int]
             fn = self._L.te_check_footprint_paths_fresh
             extra = ()
         else:
-            sig = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + [C.c_int32] + [C.c_void_p] * 6 + \
-                [C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
             fn = self._L.te_check_footprint_paths_fresh2
-        fn.argtypes = sig
         if memory == MEM_DEVICE:
             self._order_after_torch(memory)
             n = int(path_begin.numel()) - 1
@@ -473,13 +496,9 @@ class Context:
         in check_footprint_paths_fresh."""
         if untraversable_capacity is None:
             fn = self._L.te_check_footprint_paths_polygon
-            tail = []
             extra = ()
         else:
             fn = self._L.te_check_footprint_paths_polygon2
-            tail = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
-        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + [C.c_void_p] * 6 + \
-            [C.c_int32, C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 6 + tail + [C.c_int]
         fxyz = np.ascontiguousarray(footprint_xyz, dtype=np.float32).reshape(-1, 3)
         if memory == MEM_DEVICE:
             self._order_after_torch(memory)
@@ -555,15 +574,8 @@ class Context:
                  traversability_out, area_out, untraversable_capacity, untraversable_count, untraversable_xy):
         """The body of check_footprint_request (batch None) and check_footprint_request_batched (batch = (nmaps, path_map)): the
         batched entry takes nmaps after the parameters and path_map after robot_slope."""
-        if batch is None:
-            fn = self._L.te_check_footprint_request
-            head, nlay = [], 6
-        else:
-            fn = self._L.te_check_footprint_request_batched
-            head, nlay = [C.c_int32], 7
-        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(FootprintParams)] + head + [C.c_void_p] * nlay + \
-            [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32] + \
-            [C.c_void_p] * 5 + [C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
+        fn = self._L.te_check_footprint_request if batch is None else self._L.te_check_footprint_request_batched
+
         def lead(layers, path_map):
             """The arguments up to the path count: parameters, (nmaps,) the layers in argument order, (path_map)."""
             return [C.byref(g), C.byref(fp)] + ([] if batch is None else [batch[0]]) + [_addr(a) for a in layers] + \
@@ -678,7 +690,6 @@ class Map:
         self._ctx = ctx
         self._L = ctx._L
         h = C.c_void_p()
-        self._L.te_map_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
         self._check(self._L.te_map_create(ctx._h, C.byref(h)))
         self._h = h
         self._g = None
@@ -710,7 +721,6 @@ class Map:
 
     def close(self):
         if getattr(self, "_h", None):
-            self._L.te_map_destroy.argtypes = [C.c_void_p]
             self._L.te_map_destroy(self._h)
             self._h = None
 
@@ -726,7 +736,6 @@ class Map:
     def chain(self, g, p, elevation, outputs=False):
         """te_map_chain (computeTraversability): empties the cache.  outputs=True also returns the four layers as a dict."""
         fn = self._L.te_map_chain
-        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(ChainParams)] + [C.c_void_p] * 5 + [C.c_int]
         e = np.asfortranarray(elevation, dtype=np.float32)
         out = {k: np.empty((g.rows, g.cols), dtype=np.float32, order="F") for k in ("slope", "step", "roughness", "traversability")} \
             if outputs else {}
@@ -739,7 +748,6 @@ class Map:
         """te_map_chain_batched (computeTraversability for every map): elevation (nmaps, rows, cols); empties every cache.
         outputs=True also returns the four layers as a dict of (nmaps, rows, cols) arrays."""
         fn = self._L.te_map_chain_batched
-        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.POINTER(ChainParams), C.c_int32] + [C.c_void_p] * 5 + [C.c_int]
         e = self._batch_layers(elevation)
         out = {k: np.empty((int(nmaps), g.cols, g.rows), dtype=np.float32) for k in ("slope", "step", "roughness", "traversability")} \
             if outputs else {}
@@ -751,7 +759,6 @@ class Map:
     def set_layers(self, g, traversability, slope, step, elevation, roughness=None, robot_slope=None):
         """te_map_set_layers (setTraversabilityMap): empties the cache and the memo."""
         fn = self._L.te_map_set_layers
-        fn.argtypes = [C.c_void_p, C.POINTER(Geometry)] + [C.c_void_p] * 6 + [C.c_int]
         lay = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)  # noqa: E731
         t, s, st, r, e, rs = (lay(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
         self._check(fn(self._h, C.byref(g), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST))
@@ -761,7 +768,6 @@ class Map:
         """te_map_set_layers_batched (setTraversabilityMap for every map): each layer (nmaps, rows, cols); empties every cache and
         memo."""
         fn = self._L.te_map_set_layers_batched
-        fn.argtypes = [C.c_void_p, C.POINTER(Geometry), C.c_int32] + [C.c_void_p] * 6 + [C.c_int]
         t, s, st, r, e, rs = (self._batch_layers(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
         self._check(fn(self._h, C.byref(g), int(nmaps), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST))
         self._g, self._n = g, int(nmaps)
@@ -769,7 +775,6 @@ class Map:
     def footprint(self, fp):
         """te_map_footprint (traversabilityFootprint(radius, offset) on the cache); returns the cache afterwards."""
         fn = self._L.te_map_footprint
-        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_void_p, C.c_int]
         if not self._g:
             self._check(fn(self._h, C.byref(fp), None, MEM_HOST))
         buf, out = self._layer_out()
@@ -779,7 +784,6 @@ class Map:
     def footprint_polygon(self, fp, polygon_xy, yaw):
         """te_map_footprint_polygon: (traversability_x, traversability_rot) of the map's layers."""
         fn = self._L.te_map_footprint_polygon
-        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_int]
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
         (bx, ox), (brot, orot) = self._layer_out(), self._layer_out()
         self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, float(yaw), _addr(bx), _addr(brot), MEM_HOST))
@@ -789,7 +793,6 @@ class Map:
         """te_map_footprint_polygon_yaws: (nyaws, rows, cols), layer k the traversability_rot at yaws[k] of the map's layers; on a
         batch (nyaws, nmaps, rows, cols)."""
         fn = self._L.te_map_footprint_polygon_yaws
-        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
         ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
         buf, out = self._layer_out(len(ys))   # layer k of map m column-major at (k * nmaps + m) * rows * cols
@@ -801,7 +804,6 @@ class Map:
         """te_map_footprint_polygon_yaws_reduce: (worst, best, best_yaw) over `yaws` of the map's layers, each (rows, cols) or, on
         a batch, (nmaps, rows, cols)."""
         fn = self._L.te_map_footprint_polygon_yaws_reduce
-        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams), C.c_int32, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_void_p] * 3 + [C.c_int]
         pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
         ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
         (bw, worst), (bb, best) = self._layer_out(), self._layer_out()
@@ -831,9 +833,6 @@ class Map:
         path_map after the parameters."""
         batched = path_map is not None
         fn = self._L.te_map_check_footprint_request_batched if batched else self._L.te_map_check_footprint_request
-        fn.argtypes = [C.c_void_p, C.POINTER(FootprintParams)] + ([C.c_void_p] if batched else []) + \
-            [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
-             C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p, C.c_void_p]
         pm = [np.ascontiguousarray(path_map, dtype=np.int32)] if batched else []
         pb = np.ascontiguousarray(path_begin, dtype=np.int32)
         ps = np.ascontiguousarray(poses, dtype=np.float64).reshape(-1, 7)
@@ -860,7 +859,6 @@ class Map:
     def get_footprint(self):
         """te_map_get_footprint: the traversability_footprint cache (NaN = empty); (nmaps, rows, cols) on a batch."""
         fn = self._L.te_map_get_footprint
-        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
         if not self._g:
             self._check(fn(self._h, None, MEM_HOST))
         buf, out = self._layer_out()
@@ -869,13 +867,11 @@ class Map:
 
     def clear_footprint(self):
         """te_map_clear_footprint (resetTraversabilityFootprintLayers)."""
-        self._L.te_map_clear_footprint.argtypes = [C.c_void_p]
         self._check(self._L.te_map_clear_footprint(self._h))
 
     def request_stats(self):
         """(candidate checks, distinct circles walked, cache cells stored) of the last request."""
         out = (C.c_int64 * 3)()
-        self._L.te_map_request_stats.argtypes = [C.c_void_p, C.c_int64 * 3]
         self._check(self._L.te_map_request_stats(self._h, out))
         return tuple(int(v) for v in out)
 
@@ -889,10 +885,8 @@ class Map:
         rows, cols = self._shape() if self._g else (0, 0)
         if memory == MEM_HOST:
             out = np.empty((len(order), self._n, cols, rows), dtype=np.float32)   # per layer the maps back to back, column-major
-        fn = self._L.te_map_get_layers
-        fn.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_int]
         self._ctx._order_after_torch(memory)
-        self._check(fn(self._h, mask, _addr(out), memory))
+        self._check(self._L.te_map_get_layers(self._h, mask, _addr(out), memory))
         if self._n == 1:
             v = out.reshape(len(order), cols, rows)
             return {n: v[k].T for k, n in enumerate(order)}
@@ -924,14 +918,12 @@ class Map:
         self._ctx._order_after_torch(memory)
         if win_map is None:
             fn = self._L.te_map_get_submaps
-            fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]
             self._check(fn(self._h, len(p), p.ctypes.data, ln.ctypes.data, mask, info.ctypes.data, _addr(out), cap, memory))
         else:
             wm = np.ascontiguousarray(win_map, dtype=np.int32).reshape(-1)
             if len(wm) != len(p):
                 raise ValueError("win_map needs one entry per window")
             fn = self._L.te_map_get_submaps_batched
-            fn.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 3 + [C.c_uint32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]
             self._check(fn(self._h, len(p), wm.ctypes.data, p.ctypes.data, ln.ctypes.data, mask, info.ctypes.data, _addr(out), cap,
                            memory))
         res = []
@@ -950,10 +942,8 @@ class Map:
         if memory == MEM_HOST:
             xy = np.ascontiguousarray(xy, dtype=np.float64).reshape(-1, 2)
             out = np.zeros(len(xy), dtype=np.uint8)
-        fn = self._L.te_map_valid_at
-        fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int]
         self._ctx._order_after_torch(memory)
-        self._check(fn(self._h, len(xy), _addr(xy), _addr(out), memory))
+        self._check(self._L.te_map_valid_at(self._h, len(xy), _addr(xy), _addr(out), memory))
         return out
 
     def valid_at_batched(self, pos_map, xy, out=None, memory=MEM_HOST):
@@ -966,8 +956,6 @@ class Map:
             if len(pos_map) != len(xy):
                 raise ValueError("pos_map needs one entry per position")
             out = np.zeros(len(xy), dtype=np.uint8)
-        fn = self._L.te_map_valid_at_batched
-        fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         self._ctx._order_after_torch(memory)
-        self._check(fn(self._h, len(xy), _addr(pos_map), _addr(xy), _addr(out), memory))
+        self._check(self._L.te_map_valid_at_batched(self._h, len(xy), _addr(pos_map), _addr(xy), _addr(out), memory))
         return out
