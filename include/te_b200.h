@@ -568,6 +568,39 @@ int te_map_check_footprint_request_batched(te_map* map, const te_footprint_param
                                            double* traversability_out, double* area_out, int32_t max_vertices,
                                            int32_t* untraversable_count_or_null, double* untraversable_xy_or_null);
 
+/* te_map_check_footprint_request(_batched) with every array in DEVICE memory, for planners whose paths are made on the GPU: the
+ * call is asynchronous on the context stream (te_set_stream), makes no host synchronisation and reads no request array on the
+ * host, so it can be captured in a CUDA graph.  path_map_or_null: path q is on map path_map[q]; NULL only on a te_map of one map.
+ * For a valid request every output, the cache afterwards and te_map_request_stats are, bit for bit, what the host entry returns
+ * and leaves for the same request on the same map state.  Paths run in request order, each on its own map's layers, cache and
+ * memo; a start index on the map's layers changes nothing (poses are map-frame positions, the layers are resident unwrapped).
+ * Device-memory conventions, as te_check_footprint_request's: a path the library cannot check (a negative or NaN radius, more
+ * than 127 rings, a non-finite x or y, a pose range outside 0..nposes, a map outside 0..nmaps-1, a bad footprint) gets is_safe
+ * = 0, NaN traversability and area, and count -1 where its polygon was requested; it reads and stores nothing, so the other
+ * paths and the cache equal a host request without it.
+ * max_checks sizes the device work list of circle checks: one entry per isTraversable call a circular path could make (every
+ * fourth LineIterator cell of an in-map segment, every single pose), plus one per check the host loop skips (a failed
+ * checkInclination, a segment with an end outside the map), in request order.  When the request needs more, the first circular
+ * path whose entries do not fit and every circular path after it get the convention above and store nothing; everything before
+ * them is exact, so outputs and cache equal a host request of the paths that fit.  Polygonal paths do not use the list and are
+ * always answered; max_checks = 0 answers only them.  The workspace is reserved from npaths, nposes, the maps and max_checks
+ * (about 160 bytes per entry): a call with the same or smaller sizes allocates nothing.  Every call clears a hash table of
+ * 2 * max_checks slots (8 bytes per entry), so a generous max_checks costs that memset on each call.  te_map_request_stats after a device
+ * request synchronises the context stream and returns the counters the request left on the device (candidates, distinct keys,
+ * stored cells; those of the host entry for the same request).
+ * Errors, returned synchronously as by the host entry: TE_ERR_BAD_ARG for a map without layers, a NULL path_map on a batch, null
+ * pointers, negative counts, max_footprint_vertices outside 0..16, max_vertices / polygon pointer mismatches, p->offset < 0 and
+ * max_checks < 0; TE_ERR_UNSUPPORTED for max_checks > 2^30; TE_ERR_MISSING_LAYER for verify_roughness without a roughness layer.
+ * Launches: the same kernels whatever npaths, nposes and the maps; te_get_stats counts 12 (13 with polygons, plus the polygonal
+ * paths' 1-2), each of the three CUB scan / sort calls as one. */
+int te_map_check_footprint_request_device(te_map* map, const te_footprint_params* p, const int32_t* path_map_or_null,
+                                          int32_t npaths, int32_t nposes, const int32_t* path_begin, const double* poses,
+                                          const double* radius, int32_t nvertices, const int32_t* footprint_begin,
+                                          const float* footprint_xyz, int32_t max_footprint_vertices,
+                                          const uint8_t* conservative_or_null, const uint8_t* compute_untraversable_polygon_or_null,
+                                          uint8_t* is_safe, double* traversability_out, double* area_out, int32_t max_vertices,
+                                          int32_t* untraversable_count_or_null, double* untraversable_xy_or_null, int64_t max_checks);
+
 /* The cache as publishTraversabilityMap publishes its traversability_footprint layer (in host memory: in the map's buffer
  * order; device memory needs a map without a start index), and resetTraversabilityFootprintLayers (:195-200).  On a batch: every
  * map's cache, back to back. */

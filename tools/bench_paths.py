@@ -38,6 +38,13 @@ map holding the same layers.  The path mix of --batched, --paths-per-map (16) pe
 (every cache cleared before each call, not timed) and "again" (the same request on the cache it left).  Host clock around each
 call (they end synchronised), median of --reps after --warmup, the two alternating; the launches of one call; every output and
 every map's cache are asserted equal to the loop's bit for bit.
+
+--map --device times te_map_check_footprint_request_device against the host entry on twin te_maps holding the same layers: the
+--map workloads (a --size map, 1 / 100 / 1000 planner paths, every other one circular) and the --map --batched one (--maps maps
+of 512 x 512, 16 paths per map), each in the cases "empty_cache" and "again".  The device call is timed with CUDA events on
+torch's stream (set with te_set_stream), the host call with the host clock (it ends synchronised); the two alternate, median of
+--reps after --warmup.  The kernels of each call are summed with torch.profiler in a separate run.  Every output, the caches
+and request_stats of the two are asserted equal bit for bit.
 """
 from __future__ import annotations
 
@@ -91,9 +98,12 @@ def main():
     ap.add_argument("--request", action="store_true")
     ap.add_argument("--map", action="store_true")
     ap.add_argument("--batched", action="store_true")
+    ap.add_argument("--device", action="store_true")
     ap.add_argument("--maps", type=int, nargs="+", default=[256, 16])
     ap.add_argument("--paths-per-map", type=int, nargs="+", default=None)
     args = ap.parse_args()
+    if args.device and args.map:
+        return main_map_device(args)
     if args.batched and args.map:
         args.paths_per_map = args.paths_per_map or [16]
         return main_map_batched(args)
@@ -717,6 +727,138 @@ def main_map_batched(args):
             assert same, "the batched request differs from the loop over single maps"
         for m in singles + [b]:
             m.close()
+    ctx.close()
+
+
+def main_map_device(args):
+    """te_map_check_footprint_request_device against te_map_check_footprint_request(_batched) on twin maps (see the docstring)."""
+    import time
+    import torch
+    import synth
+    import traversability_estimation_b200 as te
+
+    fp = te.FootprintParams.yaml_defaults()            # offset 0.15
+    fyaml = np.asarray(YAML_FOOTPRINT, np.float32)
+    ctx = te.Context(0)
+    stream = torch.cuda.Stream()
+    torch.cuda.set_stream(stream)
+    ctx.set_stream(stream.cuda_stream)
+    name, power = gpu_info(torch)
+
+    def request(rng, n, res, npaths):
+        begin, xy = planner_paths(rng, n, npaths, res)
+        yaw = rng.uniform(0, 2 * np.pi, len(xy))
+        poses = np.stack([xy[:, 0], xy[:, 1], np.zeros(len(xy)), np.zeros(len(xy)), np.zeros(len(xy)), np.sin(yaw / 2),
+                          np.cos(yaw / 2)], axis=1)
+        circ = np.arange(npaths) % 2 == 1
+        fbeg = np.concatenate([[0], np.cumsum(np.where(circ, 0, len(fyaml)))]).astype(np.int32)
+        fxyz = np.concatenate([fyaml] * int((~circ).sum()) + [np.zeros((0, 3), np.float32)])
+        return begin, poses, np.full(npaths, 0.3), fbeg, fxyz
+
+    def workload(label, H, D, nmaps, begin, poses, radius, fbeg, fxyz, path_map):
+        npaths = len(begin) - 1
+        d = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
+        dargs = (d(begin), d(poses), d(radius), d(fbeg), d(fxyz))
+        dpm = None if path_map is None else d(path_map)
+        out = dict(is_safe=torch.empty(npaths, dtype=torch.uint8, device="cuda"),
+                   traversability_out=torch.empty(npaths, dtype=torch.float64, device="cuda"),
+                   area_out=torch.empty(npaths, dtype=torch.float64, device="cuda"))
+        max_checks = 16 * len(poses) + 1024   # a segment of 0.5 m checks at most 8 cells at 0.02 m, plus a gate
+        stream.synchronize()
+
+        def host():
+            if path_map is None:
+                return H.check_footprint_request(fp, begin, poses, radius, fbeg, fxyz, max_footprint_vertices=len(fyaml))
+            return H.check_footprint_request_batched(fp, path_map, begin, poses, radius, fbeg, fxyz, max_footprint_vertices=len(fyaml))
+
+        def device():
+            D.check_footprint_request_device(fp, *dargs, max_checks=max_checks, path_map=dpm, max_footprint_vertices=len(fyaml), **out)
+
+        row = {"gpu": name, "power_limit_w": power, "workload": label, "maps": nmaps, "paths": npaths, "poses": int(begin[-1]),
+               "circular": int((np.diff(fbeg) == 0).sum()), "max_checks": max_checks}
+        for case, clear in (("empty_cache", True), ("again", False)):
+            if clear:
+                H.clear_footprint()
+                D.clear_footprint()
+            want = host()
+            l0 = ctx.stats()[0]
+            device()
+            launches = ctx.stats()[0] - l0
+            stream.synchronize()
+            got = [out[k].cpu().numpy() for k in ("is_safe", "traversability_out", "area_out")]
+            same = all(np.array_equal(a.view(np.uint8), w.view(np.uint8)) for a, w in zip(got, want))
+            same &= np.array_equal(H.get_footprint().view(np.uint32), D.get_footprint().view(np.uint32))
+            same &= H.request_stats() == D.request_stats()
+            assert same, f"{label} {case}: the device request differs from the host entry"
+            th, td = [], []
+            for rep in range(args.warmup + args.reps):
+                if clear:
+                    H.clear_footprint()
+                t = time.perf_counter()
+                host()
+                if rep >= args.warmup:
+                    th.append((time.perf_counter() - t) * 1e3)
+                if clear:
+                    D.clear_footprint()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(stream)
+                device()
+                e1.record(stream)
+                e1.synchronize()
+                if rep >= args.warmup:
+                    td.append(e0.elapsed_time(e1))
+            kernels = {}
+            for key, fn, m in (("host", host, H), ("device", device, D)):
+                reps = 5
+                with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+                    for _ in range(reps):
+                        if clear:
+                            m.clear_footprint()
+                        fn()
+                    stream.synchronize()
+                ev = [e for e in prof.key_averages() if "memset" not in e.key.lower() and "memcpy" not in e.key.lower()]
+                kernels[key] = round(sum(e.self_device_time_total for e in ev) / 1e3 / reps, 4)
+            mh, md = float(np.median(th)), float(np.median(td))
+            row[case] = {"host_ms": round(mh, 3), "device_ms": round(md, 3), "host_over_device": round(mh / md, 2),
+                         "host_ms_range": [round(min(th), 3), round(max(th), 3)], "device_ms_range": [round(min(td), 3), round(max(td), 3)],
+                         "host_kernels_ms": kernels["host"], "device_kernels_ms": kernels["device"], "device_launches": launches,
+                         "stats": list(D.request_stats()), "safe": int(got[0].sum())}
+        row["reps"] = args.reps
+        row["bit_identical"] = True
+        print(json.dumps(row), flush=True)
+
+    # one map of --size cells, 1 / 100 / 1000 paths
+    n, res = args.size, 0.02
+    g = te.Geometry.make(n, n, res)
+    z = synth.terrain(n, n, res, 4096, "mixed")
+    layers = ctx.chain_host(g, te.ChainParams.yaml_defaults(0), z)
+    H, D = ctx.map(), ctx.map()
+    for m in (H, D):
+        m.set_layers(g, layers["traversability"], layers["slope"], layers["step"], z)
+    rng = np.random.default_rng(1)
+    for batch in (1, 100, 1000):
+        workload(f"{n}x{n}", H, D, 1, *request(rng, n, res, batch), None)
+    H.close()
+    D.close()
+    del layers, z
+    # a batch of maps of 512 x 512, 16 paths per map
+    n = 512
+    g = te.Geometry.make(n, n, res)
+    for nmaps in args.maps:
+        H, D = ctx.map(), ctx.map()
+        zb = np.stack([synth.terrain(n, n, res, 1000 + k, "mixed") for k in range(nmaps)])
+        for m in (H, D):
+            m.chain_batched(g, te.ChainParams.yaml_defaults(0), nmaps, zb)
+        rng = np.random.default_rng(16)
+        maps = [request(rng, n, res, 16) for _ in range(nmaps)]
+        begin = np.concatenate([[0]] + [m[0][1:] + sum(len(p[1]) for p in maps[:k]) for k, m in enumerate(maps)]).astype(np.int32)
+        fbeg = np.concatenate([[0]] + [m[3][1:] + sum(len(p[4]) for p in maps[:k]) for k, m in enumerate(maps)]).astype(np.int32)
+        poses, radius, fxyz = (np.concatenate([m[i] for m in maps]) for i in (1, 2, 4))
+        path_map = np.repeat(np.arange(nmaps, dtype=np.int32), 16)
+        workload(f"{nmaps}x{n}x{n}", H, D, nmaps, begin, poses, radius, fbeg, fxyz, path_map)
+        H.close()
+        D.close()
+    ctx.set_stream(None)
     ctx.close()
 
 

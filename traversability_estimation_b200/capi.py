@@ -162,6 +162,7 @@ SIGNATURES = {
     "te_map_footprint_polygon_yaws_reduce": (_R, [_P, _FP, _I, _P, _I, _P, _P, _P, _P, _I]),
     "te_map_check_footprint_request": (_R, [_P, _FP, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
     "te_map_check_footprint_request_batched": (_R, [_P, _FP, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
+    "te_map_check_footprint_request_device": (_R, [_P, _FP, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P, _L]),
     "te_map_get_footprint": (_R, [_P, _P, _I]),
     "te_map_clear_footprint": (_R, [_P]),
     "te_map_request_stats": (_R, [_P, _P]),
@@ -855,6 +856,27 @@ class Map:
         if untraversable_capacity is None:
             return safe, trav, area
         return safe, trav, area, counts, uxy
+
+    def check_footprint_request_device(self, fp, path_begin, poses, radius, footprint_begin, footprint_xyz, is_safe,
+                                       traversability_out, area_out, max_checks, path_map=None, max_footprint_vertices=None,
+                                       conservative=None, compute_untraversable_polygon=None, untraversable_capacity=None,
+                                       untraversable_count=None, untraversable_xy=None):
+        """te_map_check_footprint_request_device: check_footprint_request(_batched) with every argument a device tensor, as
+        Context.check_footprint_request(memory=MEM_DEVICE) takes them (path_map int32 per path, None on a map of one map), results
+        in the caller's tensors.  Asynchronous: ordered after torch's current stream, no host synchronisation.  max_checks sizes
+        the work list of circle checks (te_b200.h).  max_footprint_vertices defaults to 16."""
+        self._ctx._order_after_torch(MEM_DEVICE)
+        n = int(path_begin.numel()) - 1
+        mfv = 16 if max_footprint_vertices is None else int(max_footprint_vertices)
+        maxv = 0 if untraversable_capacity is None else int(untraversable_capacity)
+        self._check(self._L.te_map_check_footprint_request_device(
+            self._h, C.byref(fp), _addr(path_map), n, int(poses.numel()) // 7, _addr(path_begin), _addr(poses), _addr(radius),
+            int(footprint_xyz.numel()) // 3, _addr(footprint_begin), _addr(footprint_xyz), mfv, _addr(conservative),
+            _addr(compute_untraversable_polygon), _addr(is_safe), _addr(traversability_out), _addr(area_out), maxv,
+            _addr(untraversable_count), _addr(untraversable_xy), int(max_checks)))
+        if untraversable_capacity is None:
+            return is_safe, traversability_out, area_out
+        return is_safe, traversability_out, area_out, untraversable_count, untraversable_xy
 
     def get_footprint(self):
         """te_map_get_footprint: the traversability_footprint cache (NaN = empty); (nmaps, rows, cols) on a batch."""

@@ -1311,6 +1311,7 @@ struct te_map {
   double memo_gap = 0.0, memo_crit = 0.0;
   int memo_rough = 0;
   te::MapRequestStats last{};
+  bool last_device = false;  // the last request ran in device memory: its counters are on the device (fp.req_counters)
 };
 
 namespace {
@@ -1603,6 +1604,7 @@ static int map_request(te_map* m, const te_footprint_params* p, const int32_t* p
     return fail(TE_ERR_BAD_ARG, "max_footprint_vertices must be 0..%d, got %d", te::kPolyMaxVerts, max_footprint_vertices);
   if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
   m->last = te::MapRequestStats{};
+  m->last_device = false;
   if (npaths == 0) return TE_OK;
   const te_geometry* g = &m->geo;
   int mp = 2;
@@ -1671,6 +1673,59 @@ int te_map_check_footprint_request_batched(te_map* m, const te_footprint_params*
                      max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy);
 }
 
+int te_map_check_footprint_request_device(te_map* m, const te_footprint_params* p, const int32_t* path_map, int32_t npaths,
+                                          int32_t nposes, const int32_t* path_begin, const double* poses, const double* radius,
+                                          int32_t nvertices, const int32_t* footprint_begin, const float* footprint_xyz,
+                                          int32_t max_footprint_vertices, const uint8_t* conservative, const uint8_t* cup,
+                                          uint8_t* is_safe, double* traversability, double* area, int32_t max_vertices, int32_t* ucount,
+                                          double* uxy, int64_t max_checks) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (!path_map && m->nmaps > 1) return fail(TE_ERR_BAD_ARG, "path_map is null on a te_map of %d maps", m->nmaps);
+  if (int rc = map_footprint_params(m, p)) return rc;
+  if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
+  if (npaths < 0 || nposes < 0 || nvertices < 0 || !path_begin || !poses || !radius || !footprint_begin ||
+      (nvertices > 0 && !footprint_xyz) || !is_safe || !traversability || !area)
+    return fail(TE_ERR_BAD_ARG, "null argument or negative count");
+  if (max_footprint_vertices < 0 || max_footprint_vertices > te::kPolyMaxVerts)
+    return fail(TE_ERR_BAD_ARG, "max_footprint_vertices must be 0..%d, got %d", te::kPolyMaxVerts, max_footprint_vertices);
+  if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
+  if (max_checks < 0) return fail(TE_ERR_BAD_ARG, "max_checks must be >= 0, got %lld", (long long)max_checks);
+  if (max_checks > (1LL << 30)) return fail(TE_ERR_UNSUPPORTED, "max_checks above 2^30");
+  m->last = te::MapRequestStats{};
+  m->last_device = false;
+  if (npaths == 0) return TE_OK;
+  const te_geometry* g = &m->geo;
+  if (int rc = ensure_geometry(c, g)) return rc;
+  if (int rc = map_memo(m, p)) return rc;
+  const te::SlabView v = make_view(c, g, te_slab{0, g->cols, 0, 0});
+  const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
+  const float* rslope = m->have_rslope ? (const float*)m->rslope.p : nullptr;
+  int nl = 0;
+  if (nvertices > 0) {  // the polygonal paths, as te_check_footprint_request_batched in device memory, on the resident memo
+    te::PathChecks r{};
+    r.trav = (const float*)m->trav.p; r.slope = (const float*)m->slope.p; r.step = (const float*)m->step.p; r.rough = rough;
+    r.elev = (const float*)m->elev.p; r.robot_slope = rslope; r.nmaps = m->nmaps; r.path_map = path_map;
+    r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7;
+    r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
+    r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup;
+    r.max_points = conservative && max_footprint_vertices > 0 ? 2 * te::kPolyConsCap : 2 * std::max(max_footprint_vertices, 1);
+    r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
+    int rc = te::launch_path_checks(m->fp, v, g, p, r, false, false, c->stream, &nl);
+    if (rc != 0) return fail(rc, "map request (polygonal paths) failed: %s", m->fp.why.c_str());
+    if (int r2 = launch_check(c, "map request (polygonal paths)", nl)) return r2;
+  }
+  // the circular paths: work list, keys, walks, replay and polygons on the device
+  int rc = te::launch_map_request_device(m->fp, v, g, p, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p,
+                                         rough, (const float*)m->elev.p, rslope, (float*)m->cache.p, m->nmaps, path_map, npaths, nposes,
+                                         path_begin, poses, radius, footprint_begin, cup, is_safe, traversability, area, max_vertices,
+                                         ucount, uxy, (long long)max_checks, c->sms, c->stream, &nl);
+  if (rc != 0) return fail(rc, "map request (circular paths) failed: %s", m->fp.why.c_str());
+  if (int r2 = launch_check(c, "map request (circular paths)", nl)) return r2;
+  m->last_device = true;
+  return TE_OK;
+}
+
 int te_map_get_footprint(te_map* m, float* dst, int memory) {
   TE_MAP_ENTER(m);
   if (int rc = map_ready(m)) return rc;
@@ -1692,6 +1747,13 @@ int te_map_clear_footprint(te_map* m) {
 int te_map_request_stats(te_map* m, int64_t out[3]) {
   TE_MAP_ENTER(m);
   if (!out) return fail(TE_ERR_BAD_ARG, "null argument");
+  if (m->last_device) {  // the counters a device request left on the device
+    unsigned long long dev[3];
+    TE_CUDA(cudaStreamSynchronize(c->stream));
+    TE_CUDA(cudaMemcpy(dev, m->fp.req_counters, sizeof(dev), cudaMemcpyDeviceToHost));
+    m->last = te::MapRequestStats{(long long)dev[0], (long long)dev[1], (long long)dev[2]};
+    m->last_device = false;
+  }
   out[0] = m->last.candidates;
   out[1] = m->last.keys;
   out[2] = m->last.stored;

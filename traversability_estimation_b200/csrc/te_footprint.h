@@ -34,6 +34,8 @@ struct FootprintState {
   DevBuf items;   // polygonal path checks: one result record per pose index
   DevBuf upoly;   // polygonal path checks with untraversable polygons: per pose index a vertex count and max_vertices points
   DevBuf mapbuf;  // map requests: circle keys, inclination segments, their records and hulls; then the cache cells to store
+  DevBuf devreq;  // map requests in device memory: the work list, its keys and records, the hash table and the scan / sort scratch
+  const unsigned long long* req_counters = nullptr;  // in devreq: candidates, keys, stored of the last device request
   void invalidate() { valid = false; tables_valid = false; }
   void release();
 };
@@ -141,6 +143,20 @@ int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry*
                        const int* path_begin, const double* poses, const double* radius, const int* footprint_begin,
                        const unsigned char* cup, unsigned char* is_safe, double* trav_out, double* area_out, int max_vertices, int* ucount,
                        double* uxy, cudaStream_t s, int* launches, MapRequestStats* stats);
+// The circular paths of a request on a te_map with every path array and output in DEVICE memory (te_map_check_footprint_request_
+// device): what launch_map_circles returns and stores for the same request, asynchronous on `s` and without a host
+// synchronisation.  A path the kernels cannot check (radius, rings, pose range, non-finite position, map outside the batch), and
+// every circular path from the first whose work-list entries end past `max_checks` on, gets is_safe 0, NaN traversability and
+// area and count -1 where its polygon was requested, and reads and stores nothing.  The workspace (st.devreq) is sized from
+// npaths, nposes, nmaps and max_checks; the request's counters stay on the device at st.req_counters.  Launches: 12 (nine
+// kernels, three CUB calls counted as one each), and one more with polygons, whatever the paths and maps.  Every call clears a
+// hash table of 2 * max_checks slots (rounded up to a power of two; 8 bytes per entry of max_checks).
+int launch_map_request_device(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p,
+                              const float* trav, const float* slope, const float* step, const float* rough, const float* elev,
+                              const float* robot_slope, float* cache, int nmaps, const int* path_map, int npaths, int nposes,
+                              const int* path_begin, const double* poses, const double* radius, const int* footprint_begin,
+                              const unsigned char* cup, unsigned char* is_safe, double* trav_out, double* area_out, int max_vertices,
+                              int* ucount, double* uxy, long long max_checks, int sms, cudaStream_t s, int* launches);
 // traversabilityFootprint(radius, offset) on a cache: cache = finite(cache) ? cache : fresh over n cells; `out` (device, may be
 // null) receives the result too.
 int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, int sms, cudaStream_t s);
