@@ -540,9 +540,12 @@ int te_map_footprint_polygon_yaws_reduce(te_map* map, const te_footprint_params*
 
 /* A CheckFootprintPath request on the map, as the reference service loop answers it (TraversabilityEstimation.cpp:278-295, with
  * publishPolygons = true).  Arguments, outputs, conventions, limits and errors are those of te_check_footprint_request, with the
- * layers and the memory mode taken from the map: every array is in HOST memory (requests come from a ROS message, and which checks
- * run depends on values earlier checks cached, which the host resolves); the call returns synchronised.  Planners whose requests
- * live on the device use te_check_footprint_request.  Paths run in request order.  A circular path's isTraversable calls
+ * layers and the memory mode taken from the map: every array is in HOST memory (requests come from a ROS message); the call
+ * validates the request, stages it to the device, runs the kernels of te_map_check_footprint_request_device with a work list
+ * sized so that no path is cut, and returns synchronised.  One more limit: TE_ERR_UNSUPPORTED when the circular paths could make
+ * more than 2^30 circle checks (see max_checks there; the work list would need over 100 GB).  Launches: those of
+ * te_map_check_footprint_request_device, without the circular paths' when the request has none.  Planners whose requests live
+ * on the device use te_map_check_footprint_request_device.  Paths run in request order.  A circular path's isTraversable calls
  * (:654-746) read and fill the cache exactly as the reference's do: a centre outside the map gives the default and stores
  * nothing; a cached cell gives its float32 value and is traversable iff it is != 0 (with compute_untraversable_polygon, a cached 0
  * publishes Polygon::fromCircle); any other cell walks the spiral with this check's radius, offset and flag, returns the double
@@ -571,8 +574,9 @@ int te_map_check_footprint_request_batched(te_map* map, const te_footprint_param
 /* te_map_check_footprint_request(_batched) with every array in DEVICE memory, for planners whose paths are made on the GPU: the
  * call is asynchronous on the context stream (te_set_stream), makes no host synchronisation and reads no request array on the
  * host, so it can be captured in a CUDA graph.  path_map_or_null: path q is on map path_map[q]; NULL only on a te_map of one map.
- * For a valid request every output, the cache afterwards and te_map_request_stats are, bit for bit, what the host entry returns
- * and leaves for the same request on the same map state.  Paths run in request order, each on its own map's layers, cache and
+ * The host entries stage their arrays and run this same implementation, so for a valid request every output, the cache
+ * afterwards and te_map_request_stats are, bit for bit, what the host entry returns and leaves for the same request on the same
+ * map state.  Paths run in request order, each on its own map's layers, cache and
  * memo; a start index on the map's layers changes nothing (poses are map-frame positions, the layers are resident unwrapped).
  * Device-memory conventions, as te_check_footprint_request's: a path the library cannot check (a negative or NaN radius, more
  * than 127 rings, a non-finite x or y, a pose range outside 0..nposes, a map outside 0..nmaps-1, a bad footprint) gets is_safe
@@ -584,7 +588,7 @@ int te_map_check_footprint_request_batched(te_map* map, const te_footprint_param
  * path whose entries do not fit and every circular path after it get the convention above and store nothing; everything before
  * them is exact, so outputs and cache equal a host request of the paths that fit.  Polygonal paths do not use the list and are
  * always answered; max_checks = 0 answers only them.  The workspace is reserved from npaths, nposes, the maps and max_checks
- * (about 160 bytes per entry): a call with the same or smaller sizes allocates nothing.  Every call clears a hash table of
+ * (about 120 bytes per entry): a call with the same or smaller sizes allocates nothing.  Every call clears a hash table of
  * 2 * max_checks slots (8 bytes per entry), so a generous max_checks costs that memset on each call.  te_map_request_stats after a device
  * request synchronises the context stream and returns the counters the request left on the device (candidates, distinct keys,
  * stored cells; those of the host entry for the same request).

@@ -117,6 +117,36 @@ def test_zero_mean_circle_then_fails(te, ctx, oracle):
     m.close()
 
 
+@pytest.mark.parametrize("cup", [0, 1])
+@pytest.mark.parametrize("slope", [False, True])
+def test_nonfinite_circular_poses(te, ctx, oracle, cup, slope):
+    """A NaN or Inf x or y on a circular path: a single pose there is checked as outside the map (the default), and a segment
+    with such an end fails without a polygon after the earlier segments stored their cells.  Asked twice, on the cache the
+    first request left."""
+    og, g, L, rs = _setup(te, oracle, seed=68)
+    ft, fo = _params(te, oracle)
+    m = ctx.map()
+    m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"], robot_slope=rs if slope else None)
+    OL = dict(L, robot_slope=rs if slope else None)
+    cache = po.empty_cache(og)
+    nan, inf = np.nan, np.inf
+    paths = [[(nan, 0.1)], [(0.2, inf)], [(-inf, nan)],
+             [(-0.6, -0.4), (-0.3, -0.2), (0.1, -0.3), (nan, 0.2), (0.4, 0.4)],   # the fourth pose ends the third segment
+             [(0.5, -0.5), (0.7, -0.2), (0.9, nan)]]
+    xy = np.array([p for path in paths for p in path])
+    poses = np.zeros((len(xy), 7))
+    poses[:, :2], poses[:, 6] = xy, 1.0
+    n = len(paths)
+    R = dict(begin=np.concatenate([[0], np.cumsum([len(p) for p in paths])]).astype(np.int32), poses=poses,
+             radius=np.full(n, 0.1), kind=np.full(n, -1), cons=np.zeros(n, np.uint8), cup=np.full(n, cup, np.uint8))
+    first = _both(m, og, ft, fo, OL, cache, R, [])
+    if not slope:
+        assert first[0][0] == 1 and first[1][0] == fo.traversability_default   # outside the map: the default
+        assert first[0][3] == 0 and first[0][4] == 0 and np.isfinite(cache).any()
+    _both(m, og, ft, fo, OL, cache, R, [])
+    m.close()
+
+
 def test_sweep_and_request_share_the_cache(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, rows=160, cols=150, seed=63)
     ft, fo = _params(te, oracle)

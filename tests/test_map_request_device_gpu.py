@@ -1,6 +1,9 @@
 """te_map_check_footprint_request_device: a request on a te_map with every array in device memory.  Unless a case says otherwise,
 every output, the traversability_footprint cache after each request and request_stats must be bit-identical to what the host
-entry (te_map_check_footprint_request(_batched)) returns and leaves on a twin te_map holding the same layers."""
+entry (te_map_check_footprint_request(_batched)) returns and leaves on a twin te_map holding the same layers.  Both entries run
+the same kernels, so those comparisons check the host entry's staging (and its max_checks, which must cut no path); the cases
+that compare with the sequential CPU oracle (tests/paths_oracle.cpp) check the kernels themselves, as do test_map_gpu.py and
+test_map_batched_gpu.py for the host entry."""
 import ctypes as C
 
 import numpy as np

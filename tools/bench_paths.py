@@ -41,10 +41,12 @@ every map's cache are asserted equal to the loop's bit for bit.
 
 --map --device times te_map_check_footprint_request_device against the host entry on twin te_maps holding the same layers: the
 --map workloads (a --size map, 1 / 100 / 1000 planner paths, every other one circular) and the --map --batched one (--maps maps
-of 512 x 512, 16 paths per map), each in the cases "empty_cache" and "again".  The device call is timed with CUDA events on
-torch's stream (set with te_set_stream), the host call with the host clock (it ends synchronised); the two alternate, median of
---reps after --warmup.  The kernels of each call are summed with torch.profiler in a separate run.  Every output, the caches
-and request_stats of the two are asserted equal bit for bit.
+of 512 x 512, 16 paths per map), each in the cases "empty_cache" and "again".  Both entries run the same kernels, so the
+difference is the host entry's staging: the validation and work-list sizing on the host, the upload of the path arrays, the
+download of the outputs and the synchronisation.  The device call is timed with CUDA events on torch's stream (set with
+te_set_stream), the host call with the host clock (it ends synchronised); the two alternate, median of --reps after --warmup.
+The kernels of each call are summed with torch.profiler in a separate run.  Every output, the caches and request_stats of the
+two are asserted equal bit for bit.
 """
 from __future__ import annotations
 
@@ -465,7 +467,8 @@ def main_map(args):
     """te_map_check_footprint_request against te_check_footprint_request, both in host memory, on planner-like batches with every
     other path circular (radius 0.3) and the YAML footprint on the others.  `map_cleared_ms`: the map request on an empty cache
     (te_map_clear_footprint before each call, not timed); `map_repeat_ms`: the same request again on the cache it left.  The
-    device time is the sum of the map request's kernels (torch.profiler, CUDA activities) per call."""
+    device time is the sum of the map request's kernels (torch.profiler, CUDA activities: every kernel of the call, CUB's scans
+    and sort included, but no copy or memset) per call."""
     import time
     import torch
     import synth
@@ -538,7 +541,7 @@ def main_map(args):
                     if before:
                         before()
                     on_map()
-            ev = [e for e in prof.key_averages() if "k_map_" in e.key or "k_check_polygon" in e.key]
+            ev = [e for e in prof.key_averages() if "memset" not in e.key.lower() and "memcpy" not in e.key.lower()]
             row[f"map_{label}_kernels_ms"] = round(sum(e.self_device_time_total for e in ev) / 1e3 / reps, 4)
         print(json.dumps(row), flush=True)
     m.close()

@@ -1587,14 +1587,41 @@ int te_map_footprint_polygon_yaws_reduce(te_map* m, const te_footprint_params* p
   return map_footprint_polygon(m, p, npts, pts_xy, 1, outs, &red, memory);
 }
 
-// te_map_check_footprint_request (path_map null: a single map) and te_map_check_footprint_request_batched (path q on map
-// path_map[q], checked by the entry).
+// The work-list entries launch_map_request_device needs at most for the circular paths of a validated host request: the count of
+// req_pose_entries_d with every checkInclination gate counted when the map has robot_slope, so that no path is cut.  It walks no
+// line.  *circles: whether the request has a circular path.
+static long long map_request_checks(const te_geometry* g, bool rslope, int32_t npaths, const int32_t* path_begin, const double* poses,
+                                    const int32_t* footprint_begin, bool* circles) {
+  const te::GridGeo G{g->rows, g->cols, g->resolution, g->length_x, g->length_y, g->position_x, g->position_y};
+  long long total = 0;
+  *circles = false;
+  for (int32_t q = 0; q < npaths; ++q) {
+    if (footprint_begin[q + 1] != footprint_begin[q]) continue;  // polygonal
+    *circles = true;
+    const int32_t b = path_begin[q], n = path_begin[q + 1] - b;
+    for (int32_t k = n == 1 ? 0 : 1; k < n; ++k) {  // pose 0 of a longer path adds nothing
+      const double* e = poses + 7 * (size_t)(b + k);
+      int si, sj, ei, ej;
+      if (n > 1 && te::grid_get_index(G, e[-7], e[-6], si, sj) && te::grid_get_index(G, e[0], e[1], ei, ej))
+        total += (te::LineD(ei, ej, si, sj).n + 3) / 4;  // every fourth LineIterator cell
+      else
+        total += 1;  // a single pose, or a segment's gate
+      if (rslope) total += 1;
+    }
+  }
+  return total;
+}
+
+// te_map_check_footprint_request(_batched) in host memory (path_map null: a single map; else checked by the entry) and
+// te_map_check_footprint_request_device.  Host memory validates the paths, sizes max_checks so that no path is cut and stages
+// the arrays; then both run the same launches, and host memory downloads the outputs.
 static int map_request(te_map* m, const te_footprint_params* p, const int32_t* path_map, int32_t npaths, int32_t nposes,
                        const int32_t* path_begin, const double* poses, const double* radius, int32_t nvertices,
                        const int32_t* footprint_begin, const float* footprint_xyz, int32_t max_footprint_vertices,
                        const uint8_t* conservative, const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area,
-                       int32_t max_vertices, int32_t* ucount, double* uxy) {
+                       int32_t max_vertices, int32_t* ucount, double* uxy, long long max_checks, int memory) {
   te_ctx* c = m->ctx;
+  const bool host = memory == TE_MEM_HOST;
   if (int rc = map_footprint_params(m, p)) return rc;
   if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
   if (npaths < 0 || nposes < 0 || nvertices < 0 || !path_begin || !poses || !radius || !footprint_begin ||
@@ -1603,44 +1630,57 @@ static int map_request(te_map* m, const te_footprint_params* p, const int32_t* p
   if (max_footprint_vertices < 0 || max_footprint_vertices > te::kPolyMaxVerts)
     return fail(TE_ERR_BAD_ARG, "max_footprint_vertices must be 0..%d, got %d", te::kPolyMaxVerts, max_footprint_vertices);
   if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
+  if (!host) {
+    if (max_checks < 0) return fail(TE_ERR_BAD_ARG, "max_checks must be >= 0, got %lld", max_checks);
+    if (max_checks > (1LL << 30)) return fail(TE_ERR_UNSUPPORTED, "max_checks above 2^30");
+  }
   m->last = te::MapRequestStats{};
   m->last_device = false;
   if (npaths == 0) return TE_OK;
   const te_geometry* g = &m->geo;
-  int mp = 2;
-  if (int rc = check_request_host(g, p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
-                                  max_footprint_vertices, conservative, &mp))
-    return rc;
+  // the hull input bound of a polygonal item: as te_check_footprint_request; host memory sizes it from the paths
+  int mp = conservative && max_footprint_vertices > 0 ? 2 * te::kPolyConsCap : 2 * std::max(max_footprint_vertices, 1);
+  bool circles = true;  // device memory cannot tell: the circular kernels run and find none
+  if (host) {
+    if (int rc = check_request_host(g, p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+                                    max_footprint_vertices, conservative, &mp))
+      return rc;
+    max_checks = map_request_checks(g, m->have_rslope, npaths, path_begin, poses, footprint_begin, &circles);
+    if (max_checks > (1LL << 30))
+      return fail(TE_ERR_UNSUPPORTED, "the circular paths need %lld circle checks, more than 2^30", max_checks);
+  }
   if (int rc = ensure_geometry(c, g)) return rc;
   if (int rc = map_memo(m, p)) return rc;
   const te::SlabView v = make_view(c, g, te_slab{0, g->cols, 0, 0});
   const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
   const float* rslope = m->have_rslope ? (const float*)m->rslope.p : nullptr;
+  te::PathChecks r{};
+  r.trav = (const float*)m->trav.p; r.slope = (const float*)m->slope.p; r.step = (const float*)m->step.p; r.rough = rough;
+  r.elev = (const float*)m->elev.p; r.robot_slope = rslope; r.nmaps = m->nmaps; r.path_map = path_map;
+  r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7; r.radius = radius;
+  r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
+  r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup; r.max_points = mp;
+  r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
+  Staging st(c, host, g);
+  stage_paths(st, r);
+  if (st.rc) return st.rc;
   int nl = 0;
   if (nvertices > 0) {  // the polygonal paths (TraversabilityMap.cpp:464-584) read the memo and leave the cache alone
-    te::PathChecks r{};
-    r.trav = (const float*)m->trav.p; r.slope = (const float*)m->slope.p; r.step = (const float*)m->step.p; r.rough = rough;
-    r.elev = (const float*)m->elev.p; r.robot_slope = rslope; r.nmaps = m->nmaps; r.path_map = path_map;
-    r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7;
-    r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
-    r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup; r.max_points = mp;
-    r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
-    Staging st(c, true, g);
-    stage_paths(st, r);
-    if (st.rc) return st.rc;
     int rc = te::launch_path_checks(m->fp, v, g, p, r, false, false, c->stream, &nl);
     if (rc != 0) return fail(rc, "map request (polygonal paths) failed: %s", m->fp.why.c_str());
     if (int r2 = launch_check(c, "map request (polygonal paths)", nl)) return r2;
-    if (int r2 = st.finish()) return r2;
   }
-  // the circular paths (TraversabilityMap.cpp:345-462) in request order on the cache; they write their own outputs on the host
-  int rc = te::launch_map_circles(m->fp, v, g, p, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p, rough,
-                                  (const float*)m->elev.p, rslope, (float*)m->cache.p, m->nmaps, path_map, c->hX.data(), c->hY.data(),
-                                  npaths, path_begin, poses, radius, footprint_begin, cup, is_safe, traversability, area, max_vertices,
-                                  ucount, uxy, c->stream, &nl, &m->last);
-  if (rc != 0) return fail(rc, "map request (circular paths) failed: %s", m->fp.why.c_str());
-  if (int r2 = launch_check(c, "map request (circular paths)", nl)) return r2;
-  if (ucount)  // the row bound of a polygonal path's polygon table (kUntravRows) is only known once the hulls are
+  if (circles) {  // the circular paths (TraversabilityMap.cpp:345-462) in request order on the cache
+    int rc = te::launch_map_request_device(m->fp, v, g, p, r.trav, r.slope, r.step, rough, r.elev, rslope, (float*)m->cache.p,
+                                           m->nmaps, r.path_map, npaths, nposes, r.path_begin, r.poses, r.radius, r.footprint_begin,
+                                           r.cup, r.is_safe, r.trav_out, r.area_out, max_vertices, r.ucount, r.uxy, max_checks, host,
+                                           c->sms, c->stream, &nl);
+    if (rc != 0) return fail(rc, "map request (circular paths) failed: %s", m->fp.why.c_str());
+    if (int r2 = launch_check(c, "map request (circular paths)", nl)) return r2;
+    m->last_device = true;
+  }
+  if (int rc = st.finish()) return rc;
+  if (host && ucount)  // the row bound of a polygonal path's polygon table (kUntravRows) is only known once the hulls are
     for (int32_t q = 0; q < npaths; ++q)
       if (ucount[q] < 0)
         return fail(TE_ERR_UNSUPPORTED, "the untraversable polygon of path %d spans more than %d map rows", q, te::kUntravRows);
@@ -1656,7 +1696,8 @@ int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int3
   if (int rc = map_ready(m)) return rc;
   if (int rc = map_single(m, "te_map_check_footprint_request_batched")) return rc;
   return map_request(m, p, nullptr, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
-                     max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy);
+                     max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy, 0,
+                     TE_MEM_HOST);
 }
 
 int te_map_check_footprint_request_batched(te_map* m, const te_footprint_params* p, const int32_t* path_map, int32_t npaths,
@@ -1670,7 +1711,8 @@ int te_map_check_footprint_request_batched(te_map* m, const te_footprint_params*
   if (!path_map) return fail(TE_ERR_BAD_ARG, "path_map is null");
   if (int rc = check_map_indices(m, path_map, std::max(npaths, 0), "path_map")) return rc;
   return map_request(m, p, path_map, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
-                     max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy);
+                     max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy, 0,
+                     TE_MEM_HOST);
 }
 
 int te_map_check_footprint_request_device(te_map* m, const te_footprint_params* p, const int32_t* path_map, int32_t npaths,
@@ -1682,48 +1724,9 @@ int te_map_check_footprint_request_device(te_map* m, const te_footprint_params* 
   TE_MAP_ENTER(m);
   if (int rc = map_ready(m)) return rc;
   if (!path_map && m->nmaps > 1) return fail(TE_ERR_BAD_ARG, "path_map is null on a te_map of %d maps", m->nmaps);
-  if (int rc = map_footprint_params(m, p)) return rc;
-  if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
-  if (npaths < 0 || nposes < 0 || nvertices < 0 || !path_begin || !poses || !radius || !footprint_begin ||
-      (nvertices > 0 && !footprint_xyz) || !is_safe || !traversability || !area)
-    return fail(TE_ERR_BAD_ARG, "null argument or negative count");
-  if (max_footprint_vertices < 0 || max_footprint_vertices > te::kPolyMaxVerts)
-    return fail(TE_ERR_BAD_ARG, "max_footprint_vertices must be 0..%d, got %d", te::kPolyMaxVerts, max_footprint_vertices);
-  if (int rc = check_polygon_outputs(max_vertices, ucount, uxy)) return rc;
-  if (max_checks < 0) return fail(TE_ERR_BAD_ARG, "max_checks must be >= 0, got %lld", (long long)max_checks);
-  if (max_checks > (1LL << 30)) return fail(TE_ERR_UNSUPPORTED, "max_checks above 2^30");
-  m->last = te::MapRequestStats{};
-  m->last_device = false;
-  if (npaths == 0) return TE_OK;
-  const te_geometry* g = &m->geo;
-  if (int rc = ensure_geometry(c, g)) return rc;
-  if (int rc = map_memo(m, p)) return rc;
-  const te::SlabView v = make_view(c, g, te_slab{0, g->cols, 0, 0});
-  const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
-  const float* rslope = m->have_rslope ? (const float*)m->rslope.p : nullptr;
-  int nl = 0;
-  if (nvertices > 0) {  // the polygonal paths, as te_check_footprint_request_batched in device memory, on the resident memo
-    te::PathChecks r{};
-    r.trav = (const float*)m->trav.p; r.slope = (const float*)m->slope.p; r.step = (const float*)m->step.p; r.rough = rough;
-    r.elev = (const float*)m->elev.p; r.robot_slope = rslope; r.nmaps = m->nmaps; r.path_map = path_map;
-    r.npaths = npaths; r.nposes = nposes; r.path_begin = path_begin; r.poses = poses; r.pose_stride = 7;
-    r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
-    r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup;
-    r.max_points = conservative && max_footprint_vertices > 0 ? 2 * te::kPolyConsCap : 2 * std::max(max_footprint_vertices, 1);
-    r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
-    int rc = te::launch_path_checks(m->fp, v, g, p, r, false, false, c->stream, &nl);
-    if (rc != 0) return fail(rc, "map request (polygonal paths) failed: %s", m->fp.why.c_str());
-    if (int r2 = launch_check(c, "map request (polygonal paths)", nl)) return r2;
-  }
-  // the circular paths: work list, keys, walks, replay and polygons on the device
-  int rc = te::launch_map_request_device(m->fp, v, g, p, (const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p,
-                                         rough, (const float*)m->elev.p, rslope, (float*)m->cache.p, m->nmaps, path_map, npaths, nposes,
-                                         path_begin, poses, radius, footprint_begin, cup, is_safe, traversability, area, max_vertices,
-                                         ucount, uxy, (long long)max_checks, c->sms, c->stream, &nl);
-  if (rc != 0) return fail(rc, "map request (circular paths) failed: %s", m->fp.why.c_str());
-  if (int r2 = launch_check(c, "map request (circular paths)", nl)) return r2;
-  m->last_device = true;
-  return TE_OK;
+  return map_request(m, p, path_map, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+                     max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy,
+                     (long long)max_checks, TE_MEM_DEVICE);
 }
 
 int te_map_get_footprint(te_map* m, float* dst, int memory) {

@@ -21,7 +21,6 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
-#include <unordered_map>
 
 namespace te {
 namespace {
@@ -890,7 +889,7 @@ __device__ bool inclination_ok_d(const FpArgs& A, const float* rslope, double ax
 
 // The running, length-weighted mean of the segment means (TraversabilityMap.cpp:440-452); `lengthPath` (an uninitialised local
 // in the reference) is the running path length.
-__host__ __device__ __forceinline__ void add_segment_d(double t, double lx, double ly, int k, double& lengthPath, double& result) {
+__device__ __forceinline__ void add_segment_d(double t, double lx, double ly, int k, double& lengthPath, double& result) {
   const double lengthSegment = sqrt(lx * lx + ly * ly);
   if (k > 1) {
     const double lengthPreviousPath = lengthPath;
@@ -1057,11 +1056,11 @@ __device__ FreshCircle fresh_circle_d(const FpArgs& A, const Layers& L, const Pa
   return FreshCircle{true, t, (float)t};
 }
 
-__host__ __device__ __forceinline__ bool lex_less_d(double2 a, double2 b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
+__device__ __forceinline__ bool lex_less_d(double2 a, double2 b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
 
 // grid_map::Polygon::monotoneChainConvexHullOfPoints (recalled) of the m > 3 points `sorted` (already in lexicographic order) into
 // `hull` (2m entries, the reference's own allocation); returns the vertex count.  One thread.
-__host__ __device__ int monotone_chain_d(const double2* sorted, int m, double2* hull) {
+__device__ int monotone_chain_d(const double2* sorted, int m, double2* hull) {
   auto clockwise = [](double2 o, double2 a, double2 b) {
     const double ux = a.x - o.x, uy = a.y - o.y, wx = b.x - o.x, wy = b.y - o.y;
     return (ux * wy - uy * wx) <= 0;
@@ -1228,7 +1227,7 @@ __device__ int spiral_blockers_d(const FpArgs& A, const Layers& L, const PathArg
 // grid_map::Polygon::fromCircle(center, radius) (recalled): vertex j = center + Rotation2D(j * 2 * M_PI / 19) * (radius, 0); the
 // 20 cosines and sines come from the host's libm (circle_table).  A single pose publishes it as it is; a segment
 // hulls it: 20 points, so every later convexHull with it is the same chain (see write_cells_polygon_d).  One thread.
-__host__ __device__ void write_circle_polygon_d(const double* cs, const double* sn, double cx, double cy, double radius, bool hulled,
+__device__ void write_circle_polygon_d(const double* cs, const double* sn, double cx, double cy, double radius, bool hulled,
                                        double2* pts, const UntravOut& O, int q) {
   const int nc = kFromCircleVertices;
   double2* hull = pts + nc;
@@ -1418,47 +1417,38 @@ __global__ void __launch_bounds__(128, 4) k_check_paths_fresh_poly(FpArgs A, Lay
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// The circular paths of a request on a te_map (launch_map_circles).  The traversability_footprint cache there persists across the
-// paths of a request and across requests, so which isTraversable calls run, and what they read, depends on what earlier calls
-// stored.  The host lists every circle the paths could check (a MapKey per distinct map, centre, cell, radius and polygon flag);
-// k_map_eval_circles evaluates every key on the cache as the request found it, one warp per key; the host then replays the
-// service loop in order over these records and writes the cells it stored back with k_map_scatter.  A te_map may hold a batch of
-// maps of one geometry (map m's layers, cache and memo start m * rows * cols cells into theirs); a key belongs to one of them.
+// The circular paths of a request on a te_map (launch_map_request_device).  The traversability_footprint cache there persists
+// across the paths of a request and across requests, so which isTraversable calls run, and what they read, depends on what
+// earlier calls stored.  Every circle the paths could check is a MapKey (one per distinct map, centre, cell, radius and polygon
+// flag); k_map_eval_circles_dev evaluates every key on the cache as the request found it, one warp per key, and k_req_replay
+// then runs the service loop in order over these records.  A te_map may hold a batch of maps of one geometry (map m's layers,
+// cache and memo start m * rows * cols cells into theirs); a key belongs to one of them.
 struct MapKey {
   double cx, cy, rmin;  // isTraversable(center, rmin + offset, cup, ..., rmin)
   int ci, cj;           // getIndex(center)
   int cup;              // computeUntraversablePolygon
-  int slot;             // row of the hull table for a cup key, -1: no polygon wanted
   int map;              // the map of the batch (0 on a single map)
 };
 struct MapRecord {
   double t;       // the walk's traversability output (double), or the cached value
   float cache;    // what the walk stores at (ci, cj), or the cached value
   int state;      // 0: walked, traversable; 1: walked, untraversable; 2: the cell was cached when the request began
-  int cnt;        // an untraversable cup walk: the blocked cells it collects (spiral_blockers_d)
-  int nv;         // ... the vertex count of their monotone chain (cnt >= 2; the first min(nv, maxv) vertices are in the hull table)
-  int2 first[3];  // ... the first three of them (map row, map column) in visit order
 };
 
-// Key k of the request, by the whole warp w of a block of four: the record and, for a cup key with a hull slot, its hull
-// (k_map_eval_circles, k_map_eval_circles_dev).
+// Key k of the request, by the whole warp w of a block of four: its record (k_map_eval_circles_dev).
 __device__ __forceinline__ void map_eval_circle_d(const FpArgs& A, const Layers& L, const PathArgs& P, const MapKey* __restrict__ keys,
-                                                  int k, const float* __restrict__ cache, MapRecord* __restrict__ recs, int maxv,
-                                                  double* __restrict__ hulls) {
-  __shared__ int s_min[4][kFreshTableRows + 1], s_max[4][kFreshTableRows + 1];
-  __shared__ int2 s_stack[4][2 * kFreshTableRows + 4];
-  __shared__ int2 s_first[4][3];
+                                                  int k, const float* __restrict__ cache, MapRecord* __restrict__ recs) {
   __shared__ Layers s_L[4];
   __shared__ PathArgs s_P[4];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const MapKey K = keys[k];
   MapRecord& R = recs[k];
-  // The key's map: its layers, memo and cache start mo cells in.  The walks take the shifted layer and path arguments from a
-  // per-warp copy in shared memory (by reference, as they take the kernel's own), so no register holds them across the calls.
+  // The key's map: its layers, memo and cache start mo cells in.  The walk takes the shifted layer and path arguments from a
+  // per-warp copy in shared memory (by reference, as it takes the kernel's own), so no register holds them across the call.
   const long long mo = (long long)K.map * A.rows * A.cols_total;
   const float c0 = __ldg(cache + mo + (size_t)K.cj * A.rows + K.ci);
   if (finitef(c0)) {  // :673-675
-    if (lane == 0) { R.t = (double)c0; R.cache = c0; R.state = 2; R.cnt = 0; R.nv = 0; }
+    if (lane == 0) { R.t = (double)c0; R.cache = c0; R.state = 2; }
     return;
   }
   if (lane == 0) {
@@ -1470,60 +1460,17 @@ __device__ __forceinline__ void map_eval_circle_d(const FpArgs& A, const Layers&
   const double rmax = K.rmin + P.offset;
   const int nr = (int)ceil(rmax / A.res);
   const FreshCircle f = fresh_circle_d(A, s_L[w], s_P[w], K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, nr, K.cup != 0);
-  int cnt = 0, nv = 0;
-  if (K.cup && !f.ok && K.slot >= 0) {  // a cup walk fails only within rmin: it collects the blocked cells (:687-730)
-    const UntravScratch S{s_min[w], s_max[w], s_stack[w], s_first[w]};
-    cnt = spiral_blockers_d(A, s_L[w], s_P[w], S, K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, nr);
-    if (lane == 0) {
-      for (int v = 0; v < min(cnt, 3); ++v) R.first[v] = S.first[v];
-      if (cnt >= 2) {
-        const int a0 = K.ci - nr;
-        nv = table_chain_d(A, S.tmin, S.tmax, 2 * nr + 1, a0, S.stack);
-        double* xy = hulls + 2 * (size_t)maxv * K.slot;
-        for (int v = 0; v < min(nv, maxv); ++v) {
-          xy[2 * v] = A.X[a0 + S.stack[v].x];
-          xy[2 * v + 1] = A.Y[S.stack[v].y];
-        }
-      }
-    }
-  }
-  if (lane == 0) { R.t = f.t; R.cache = f.cache; R.state = f.ok ? 0 : 1; R.cnt = cnt; R.nv = nv; }
+  if (lane == 0) { R.t = f.t; R.cache = f.cache; R.state = f.ok ? 0 : 1; }
 }
 
-__global__ void __launch_bounds__(128) k_map_eval_circles(FpArgs A, Layers L, PathArgs P, const MapKey* __restrict__ keys, int nkeys,
-                                                          const float* __restrict__ cache, MapRecord* __restrict__ recs, int maxv,
-                                                          double* __restrict__ hulls) {
-  const int k = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
-  if (k >= nkeys) return;  // whole warp
-  map_eval_circle_d(A, L, P, keys, k, cache, recs, maxv, hulls);
-}
-
-// k_map_eval_circles for the device request: the key count is on the device (*nkeys), so the warps stride over the keys.  No hull
-// slots: the request computes its polygons after the replay (k_req_polygons).
+// The key count is on the device (*nkeys), so the warps stride over the keys.  The polygons of the failed paths come after the
+// replay (k_req_polygons).
 __global__ void __launch_bounds__(128, 4) k_map_eval_circles_dev(FpArgs A, Layers L, PathArgs P, const MapKey* __restrict__ keys,
                                                               const unsigned long long* __restrict__ nkeys, const float* __restrict__ cache,
                                                               MapRecord* __restrict__ recs) {
   const long long n = (long long)*nkeys;
   for (long long k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; k < n; k += (gridDim.x * blockDim.x) >> 5)  // whole warps
-    map_eval_circle_d(A, L, P, keys, (int)k, cache, recs, 1, nullptr);
-}
-
-// checkInclination of every pose (x, y, x, y) or segment (start, end) the host lists, one thread each, on the robot_slope layer
-// of map seg_map[k] (null: map 0).
-__global__ void __launch_bounds__(128) k_map_inclination(FpArgs A, const float* __restrict__ rslope, const double4* __restrict__ seg,
-                                                         const int* __restrict__ seg_map, int nseg, unsigned char* __restrict__ ok) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= nseg) return;
-  const double4 s = seg[k];
-  if (seg_map) rslope += (long long)seg_map[k] * A.rows * A.cols_total;
-  ok[k] = inclination_ok_d(A, rslope, s.x, s.y, s.z, s.w) ? 1 : 0;
-}
-
-// The cells the replay stored (cells of the whole batch: map * rows * cols + cell), written into the cache.
-__global__ void __launch_bounds__(256) k_map_scatter(float* __restrict__ cache, const unsigned long long* __restrict__ cell,
-                                                     const float* __restrict__ value, int n) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k < n) cache[cell[k]] = value[k];
+    map_eval_circle_d(A, L, P, keys, (int)k, cache, recs);
 }
 
 // traversabilityFootprint(radius, offset) on a cache: a cached cell takes the memoised branch and keeps its value, every other cell
@@ -1537,12 +1484,12 @@ __global__ void __launch_bounds__(256) k_map_merge(float* cache, const float* __
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// The circular paths of a request in device memory (launch_map_request_device): the steps of launch_map_circles without the
-// host.  A work list holds one entry per isTraversable call a circular path could make (a single pose; every fourth LineIterator
-// cell of an in-map segment) and a "gate" wherever the host loop breaks without a check (a failed checkInclination, a segment
-// with an end outside the map).  The list is laid out per map, each map's entries contiguous and in request order
-// (k_req_count .. k_req_list); the key entries are deduplicated on MapKeyBits (k_req_dedup) and every distinct key is walked once
-// on the cache as the request found it (k_map_eval_circles_dev); k_req_replay then runs the service loop, one warp per map, and
+// The work list of the circular paths of a request on a te_map (launch_map_request_device), whichever memory the request came
+// from.  It holds one entry per isTraversable call a circular path could make (a single pose; every fourth LineIterator cell of an
+// in-map segment) and a "gate" wherever the service loop breaks without a check (a failed checkInclination, a segment with an end
+// outside the map).  The list is laid out per map, each map's entries contiguous and in request order (k_req_count ..
+// k_req_list); the key entries are deduplicated on their key's bits (k_req_dedup) and every distinct key is walked once on the
+// cache as the request found it (k_map_eval_circles_dev); k_req_replay then runs the service loop, one warp per map, and
 // k_req_polygons publishes the polygons of the failed paths.
 enum : int { kEntKey = 1, kEntOutside = 2, kEntGate = 4, kEntSegEnd = 8, kEntPathEnd = 16 };
 struct ReqEntry {
@@ -1599,6 +1546,9 @@ struct DevReq {
   MapRecord* recs;
   ReqFail* fails;               // per path
   unsigned long long* counters; // candidates, keys, stored
+  // host memory: a non-finite x or y is checked as the service loop checks it (a single pose outside the map, a segment gate)
+  // instead of leaving its path unchecked; only k_req_paths reads it (last, so the other kernels' parameters keep their offsets)
+  bool nonfinite_ok;
 };
 
 // The path of pose p: the last q with path_begin[q] <= p (k_check_polygon_items' search).
@@ -1613,8 +1563,8 @@ __device__ __forceinline__ int req_path_of_d(const DevReq& D, int p) {
 
 __device__ __forceinline__ bool req_circular_d(const DevReq& D, int q) { return D.fp_begin[q + 1] == D.fp_begin[q]; }
 
-// One thread per path: whether circular path q can be checked (radius, rings, pose range, finite positions, map) and every pose
-// of it is found by req_path_of_d.
+// One thread per path: whether circular path q can be checked (radius, rings, pose range, finite positions unless
+// D.nonfinite_ok, map) and every pose of it is found by req_path_of_d.
 __global__ void __launch_bounds__(128) k_req_paths(FpArgs A, DevReq D) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= D.npaths) return;
@@ -1624,7 +1574,8 @@ __global__ void __launch_bounds__(128) k_req_paths(FpArgs A, DevReq D) {
   bool ok = rmin >= 0.0 && ceil((rmin + D.offset) / A.res) <= (double)kPathMaxRings && b >= 0 && n >= 0 && b <= D.nposes - n;
   if (ok && D.path_map) ok = D.path_map[q] >= 0 && D.path_map[q] < D.nmaps;
   for (int k = 0; k < n && ok; ++k)
-    ok = isfinite(D.poses[7 * (size_t)(b + k)]) && isfinite(D.poses[7 * (size_t)(b + k) + 1]) && req_path_of_d(D, b + k) == q;
+    ok = (D.nonfinite_ok || (isfinite(D.poses[7 * (size_t)(b + k)]) && isfinite(D.poses[7 * (size_t)(b + k) + 1]))) &&
+         req_path_of_d(D, b + k) == q;
   D.status[q] = !ok ? 2 : n == 0 ? 3 : 1;
 }
 
@@ -1646,7 +1597,7 @@ __device__ long long req_pose_entries_d(const FpArgs& A, const DevReq& D, int p,
     if (E && c < room) E[c] = ReqEntry{cx, cy, q, flags, ci, cj, n > 1 ? k : 0, freps, m, -1};
     ++c;
   };
-  // the host enumeration lists a check's circles whatever checkInclination says: the gate goes in front of them
+  // the candidates count a check's circles whatever checkInclination says: the gate goes in front of them
   if (rslope && !inclination_ok_d(A, rslope, sx, sy, ex, ey)) put(ex, ey, kEntGate, 0, 0, 1);
   if (n == 1) {
     int i, j;
@@ -1729,7 +1680,7 @@ __global__ void __launch_bounds__(128) k_req_list(FpArgs A, DevReq D) {
 
 __device__ __forceinline__ unsigned long long dbits_d(double d) { return (unsigned long long)__double_as_longlong(d); }
 
-// The identity of a key entry's isTraversable call (MapKeyBits): map, centre, cell, radius and polygon flag, bit for bit.
+// The identity of a key entry's isTraversable call: map, centre, cell, radius and polygon flag, bit for bit.
 __device__ __forceinline__ bool req_same_key_d(const DevReq& D, const ReqEntry& a, const ReqEntry& b) {
   const bool ca = D.cup && D.cup[a.q], cb = D.cup && D.cup[b.q];
   return a.map == b.map && dbits_d(a.cx) == dbits_d(b.cx) && dbits_d(a.cy) == dbits_d(b.cy) && a.ci == b.ci && a.cj == b.cj &&
@@ -1765,7 +1716,7 @@ __device__ __forceinline__ void req_dedup_entry_d(const DevReq& D, int e) {
   if (canon == e) {
     const int id = (int)atomicAdd(D.counters + 1, 1ULL);  // distinct keys
     D.kid[e] = id;
-    D.keys[id] = MapKey{E.cx, E.cy, rmin, E.ci, E.cj, cup ? 1 : 0, -1, E.map};
+    D.keys[id] = MapKey{E.cx, E.cy, rmin, E.ci, E.cj, cup ? 1 : 0, E.map};
   }
 }
 
@@ -1774,21 +1725,22 @@ __global__ void __launch_bounds__(256) k_req_dedup(DevReq D) {
   for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total; e += gridDim.x * blockDim.x) req_dedup_entry_d(D, e);
 }
 
-// 5. Replay: the service loop of one map (launch_map_circles' step 3), one warp per map, over the map's entries in request order,
-// 32 at a time.  Why this is the host loop exactly:
-//   - Which value a check reads depends only on the checks before it in its map: a cell is in the overlay iff an executed earlier
-//     check of the request walked it, and then holds that walk's float.  The live cache is that overlay: a cell the request
-//     stored, or one cached when it began, is finite (the walks store finite values); an empty cell was empty when the request
-//     began, so its key's record is a walk.
+// 5. Replay: the service loop of one map, one warp per map, over the map's entries in request order, 32 at a time.  Why this is
+// the sequential loop (one check after the other, as the reference runs it) exactly:
+//   - Which value a check reads depends only on the checks before it in its map: in the sequential loop a cell holds a value this
+//     request stored iff an executed earlier check of the request walked it, and then that walk's float.  The live cache holds
+//     exactly those: a cell the request stored, or one cached when it began, is finite (the walks store finite values); an empty
+//     cell was empty when the request began, so its key's record is a walk.
 //   - Within a window every lane assumes that all lanes before it run.  Among lanes of one cell only the first can find the cell
 //     empty and walk; every later one reads the first one's float (the live value, or the float its record stores).  So under
-//     that assumption each lane's value and verdict are the host's.
+//     that assumption each lane's value and verdict are the sequential loop's.
 //   - The assumption holds up to and including the first failing lane f: no lane before it fails, and entries of one path are
-//     consecutive, so the host runs lanes 0 .. f in this order.  They commit: first touches store their float, and one lane
-//     folds the values in visit order, so sums, add_segment_d and the verdicts are the host's bit for bit.
-//   - The host then skips the rest of f's path (the `break`s); the next window starts at the first entry of a later path.  Lanes
-//     after f that belong to later paths are evaluated again there: their assumption included dropped lanes, which store nothing.
-//   - Gates fail without a polygon, as the host's `break`.  Maps share nothing, so their warps run independently.
+//     consecutive, so the sequential loop runs lanes 0 .. f in this order.  They commit: first touches store their float, and one
+//     lane folds the values in visit order, so sums, add_segment_d and the verdicts are the sequential loop's bit for bit.
+//   - The sequential loop then skips the rest of f's path (the `break`s); the next window starts at the first entry of a later
+//     path.  Lanes after f that belong to later paths are evaluated again there: their assumption included dropped lanes, which
+//     store nothing.
+//   - Gates fail without a polygon, as the loop's `break`.  Maps share nothing, so their warps run independently.
 __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* cache) {
   __shared__ double s_t[4][32];
   __shared__ int s_v[4][32];
@@ -2341,7 +2293,7 @@ std::vector<int> build_spiral(double radius, double res) {
 }  // namespace
 
 void FootprintState::release() {
-  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly, &reduce, &rings, &memo, &items, &upoly, &mapbuf, &devreq}) b->release();
+  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly, &reduce, &rings, &memo, &items, &upoly, &devreq}) b->release();
   req_counters = nullptr;
   tables_valid = false;
   valid = false;
@@ -2512,265 +2464,16 @@ int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry*
 }
 
 namespace {
-// The identity of an isTraversable call on an empty cell: its map, centre, cell, radius and polygon flag, bit for bit.
-struct MapKeyBits {
-  unsigned long long cx, cy, r;
-  int ci, cj, cup, map;
-  bool operator==(const MapKeyBits& o) const {
-    return cx == o.cx && cy == o.cy && r == o.r && ci == o.ci && cj == o.cj && cup == o.cup && map == o.map;
-  }
-};
-struct MapKeyHash {
-  size_t operator()(const MapKeyBits& k) const {
-    unsigned long long h = k.cx * 0x9E3779B97F4A7C15ULL;
-    h = (h ^ (h >> 29)) + k.cy * 0xBF58476D1CE4E5B9ULL;
-    h = (h ^ (h >> 31)) + k.r * 0x94D049BB133111EBULL;
-    h ^= ((unsigned long long)(unsigned)k.ci << 33) ^ ((unsigned long long)(unsigned)k.cj << 1) ^ (unsigned long long)k.cup;
-    h += (unsigned long long)(unsigned)k.map * 0xD6E8FEB86659FD93ULL;
-    return (size_t)(h ^ (h >> 32));
-  }
-};
-unsigned long long dbits(double d) {
-  unsigned long long u;
-  std::memcpy(&u, &d, sizeof(u));
-  return u;
-}
 size_t align16(size_t b) { return (b + 15) / 16 * 16; }
 }  // namespace
-
-int launch_map_circles(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* trav,
-                       const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
-                       float* cache, int nmaps, const int* path_map, const double* hX, const double* hY, int npaths,
-                       const int* path_begin, const double* poses, const double* radius, const int* footprint_begin,
-                       const unsigned char* cup, unsigned char* is_safe, double* trav_out, double* area_out, int max_vertices, int* ucount,
-                       double* uxy, cudaStream_t s, int* launches, MapRequestStats* stats) {
-  *launches = 0;
-  *stats = MapRequestStats{};
-  const GridGeo G{g->rows, g->cols, g->resolution, g->length_x, g->length_y, g->position_x, g->position_y};
-  const bool want_poly = ucount != nullptr;
-  const int maxv = std::max(max_vertices, 1);
-  const unsigned long long map_cells = (unsigned long long)g->rows * g->cols;
-  auto circular = [&](int q) { return footprint_begin[q + 1] == footprint_begin[q]; };
-  auto pose = [&](int k) { return poses + 7 * (size_t)k; };
-  auto map_of = [&](int q) { return path_map ? path_map[q] : 0; };
-  if (nmaps < 1 || (!path_map && nmaps != 1)) { st.why = "a batch of maps needs a map per path"; return TE_ERR_BAD_ARG; }
-
-  // 1. every circle the circular paths could check, deduplicated, and every pose / segment checkInclination could read
-  std::unordered_map<MapKeyBits, int, MapKeyHash> index;
-  std::vector<MapKey> keys;
-  std::vector<double4> segs;
-  std::vector<int> seg_map;  // the map of each segment (a batch only)
-  std::vector<int> seg_of_pose(robot_slope ? (size_t)path_begin[npaths] : 0, -1);
-  int nslots = 0;
-  auto key_of = [&](int m, double cx, double cy, int ci, int cj, double rmin, bool c, bool insert) -> int {
-    const MapKeyBits kb{dbits(cx), dbits(cy), dbits(rmin), ci, cj, c ? 1 : 0, m};
-    auto it = index.find(kb);
-    if (it != index.end()) return it->second;
-    if (!insert) return -1;
-    keys.push_back(MapKey{cx, cy, rmin, ci, cj, c ? 1 : 0, (c && want_poly) ? nslots++ : -1, m});
-    index.emplace(kb, (int)keys.size() - 1);
-    return (int)keys.size() - 1;
-  };
-  auto add_seg = [&](int q, int k, double4 sg) {
-    seg_of_pose[k] = (int)segs.size();
-    segs.push_back(sg);
-    if (path_map) seg_map.push_back(path_map[q]);
-  };
-  for (int q = 0; q < npaths; ++q) {
-    if (!circular(q)) continue;
-    const int b = path_begin[q], n = path_begin[q + 1] - b, m = map_of(q);
-    const bool c = cup && cup[q];
-    for (int k = 0; k < n; ++k) {
-      const double ex = pose(b + k)[0], ey = pose(b + k)[1];
-      if (n == 1) {
-        if (robot_slope) add_seg(q, b, make_double4(ex, ey, ex, ey));
-        int i, j;
-        if (grid_get_index(G, ex, ey, i, j)) { key_of(m, ex, ey, i, j, radius[q], c, true); ++stats->candidates; }
-        continue;
-      }
-      if (k == 0) continue;
-      const double sx = pose(b + k - 1)[0], sy = pose(b + k - 1)[1];
-      if (robot_slope) add_seg(q, b + k, make_double4(sx, sy, ex, ey));
-      int si, sj, ei, ej;
-      if (!grid_get_index(G, sx, sy, si, sj) || !grid_get_index(G, ex, ey, ei, ej)) continue;
-      LineD line(ei, ej, si, sj);
-      for (int cc = 0; cc < line.n; ++cc, line.next())
-        if ((cc & 3) == 0) { key_of(m, hX[line.li], hY[line.lj], line.li, line.lj, radius[q], c, true); ++stats->candidates; }
-    }
-  }
-  stats->keys = (long long)keys.size();
-
-  // 2. one launch walks every key on the cache as the request found it; a second checks the inclinations
-  const int nkeys = (int)keys.size(), nseg = (int)segs.size();
-  std::vector<MapRecord> recs(nkeys);
-  std::vector<unsigned char> incl(nseg);
-  std::vector<double> hulls(want_poly ? 2 * (size_t)maxv * nslots : 0);
-  if (nkeys > 0 || nseg > 0) {
-    if (int rc = ensure_ring_table(st, s)) return rc;
-    const size_t o_keys = 0, o_segs = align16(o_keys + sizeof(MapKey) * nkeys), o_smap = align16(o_segs + sizeof(double4) * nseg);
-    const size_t o_recs = align16(o_smap + sizeof(int) * seg_map.size());
-    const size_t o_incl = align16(o_recs + sizeof(MapRecord) * nkeys), o_hull = align16(o_incl + nseg);
-    const size_t bytes = o_hull + sizeof(double) * hulls.size();
-    if (st.mapbuf.reserve(std::max<size_t>(bytes, 16)) != cudaSuccess) { st.why = "allocating the map request records failed"; return TE_ERR_CUDA; }
-    char* base = (char*)st.mapbuf.p;
-    if (cudaMemcpyAsync(base + o_keys, keys.data(), sizeof(MapKey) * nkeys, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-        cudaMemcpyAsync(base + o_segs, segs.data(), sizeof(double4) * nseg, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-        cudaMemcpyAsync(base + o_smap, seg_map.data(), sizeof(int) * seg_map.size(), cudaMemcpyHostToDevice, s) != cudaSuccess) {
-      st.why = "map request upload failed";
-      return TE_ERR_CUDA;
-    }
-    FpArgs a = filter_args(v, g, p, rough);
-    const Layers L{trav, slope, step, elev, rough};
-    const PathArgs P = path_args(st, p, robot_slope);
-    if (nkeys > 0) {
-      k_map_eval_circles<<<(unsigned)((32LL * nkeys + 127) / 128), 128, 0, s>>>(a, L, P, (const MapKey*)(base + o_keys), nkeys, cache,
-                                                                               (MapRecord*)(base + o_recs), maxv, (double*)(base + o_hull));
-      ++*launches;
-    }
-    if (nseg > 0) {
-      k_map_inclination<<<(unsigned)((nseg + 127) / 128), 128, 0, s>>>(a, robot_slope, (const double4*)(base + o_segs),
-                                                                      path_map ? (const int*)(base + o_smap) : nullptr, nseg,
-                                                                      (unsigned char*)(base + o_incl));
-      ++*launches;
-    }
-    if (cudaMemcpyAsync(recs.data(), base + o_recs, sizeof(MapRecord) * nkeys, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-        cudaMemcpyAsync(incl.data(), base + o_incl, nseg, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-        cudaMemcpyAsync(hulls.data(), base + o_hull, sizeof(double) * hulls.size(), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-        cudaStreamSynchronize(s) != cudaSuccess) {
-      st.why = "map request records failed";
-      return TE_ERR_CUDA;
-    }
-  }
-
-  // 3. the service loop in request order (checkCircularFootprintPath, TraversabilityMap.cpp:345-462, with publishPolygons = true)
-  // over the records: a cell this request stored reads the overlay, any other cell its own key's record.  Cells are cells of the
-  // batch (map * rows * cols + cell), so a path sees its own map's cache only.
-  std::unordered_map<unsigned long long, float> overlay;
-  std::vector<unsigned long long> order;  // overlay cells in the order they were stored
-  const CircleTable CT = circle_table();
-  const double tdefault = p->traversability_default, offset = p->offset;
-  for (int q = 0; q < npaths; ++q) {
-    if (!circular(q)) continue;
-    const int b = path_begin[q], n = path_begin[q + 1] - b, m = map_of(q);
-    const double rmin = radius[q], rmax = rmin + offset;
-    const bool c = cup && cup[q];
-    // isTraversable(center, rmax, c, t, ..., rmin) (:654-746); `cell` < 0: the centre is outside the map
-    int fkind = 0, fkey = -1, freps = 1;  // the failing circle: 0 none, 1 fromCircle(fx, fy), 2 the blocked cells of key fkey
-    double fx = 0.0, fy = 0.0;
-    auto check = [&](double cx, double cy, int ci, int cj, bool inside, double& t) -> bool {
-      if (!inside) {  // :662-667
-        t = tdefault;
-        if (tdefault == 0.0) { fkind = 1; fx = cx; fy = cy; }
-        return tdefault != 0.0;
-      }
-      const unsigned long long cell = (unsigned long long)m * map_cells + (unsigned long long)cj * g->rows + ci;
-      float cached;
-      bool have = false;
-      auto ov = overlay.find(cell);
-      const int k = key_of(m, cx, cy, ci, cj, rmin, c, false);
-      if (ov != overlay.end()) { cached = ov->second; have = true; }
-      else if (recs[k].state == 2) { cached = recs[k].cache; have = true; }
-      if (have) {  // :673-678
-        t = (double)cached;
-        if (cached == 0.0f) { fkind = 1; fx = cx; fy = cy; }
-        return cached != 0.0f;
-      }
-      const MapRecord& r = recs[k];  // the first check of the cell: the walk (:679-736) stores its value
-      overlay.emplace(cell, r.cache);
-      order.push_back(cell);
-      t = r.t;
-      if (r.state == 1) { fkind = 2; fkey = k; fx = cx; fy = cy; }
-      return r.state == 0;
-    };
-    double result = 0.0, lengthPath = 0.0;
-    double sx = 0.0, sy = 0.0, ex = 0.0, ey = 0.0;
-    bool ok = n > 0;
-    for (int k = 0; k < n && ok; ++k) {
-      sx = ex; sy = ey;
-      ex = pose(b + k)[0]; ey = pose(b + k)[1];
-      if (n == 1) {  // :365-387
-        if (robot_slope && !incl[seg_of_pose[b]]) { ok = false; break; }
-        int i, j;
-        const bool inside = grid_get_index(G, ex, ey, i, j);
-        ok = check(ex, ey, i, j, inside, result);
-      }
-      if (n > 1 && k > 0) {  // :389-457
-        if (robot_slope && !incl[seg_of_pose[b + k]]) { ok = false; break; }
-        int si, sj, ei, ej;
-        if (!grid_get_index(G, sx, sy, si, sj) || !grid_get_index(G, ex, ey, ei, ej)) { ok = false; break; }
-        LineD line(ei, ej, si, sj);
-        int nLine = 0;
-        double sum = 0.0;
-        for (int cc = 0; cc < line.n && ok; ++cc, line.next()) {
-          if (cc & 3) continue;
-          double t;
-          ok = check(hX[line.li], hY[line.lj], line.li, line.lj, true, t);
-          // the failing circle's polygon is hulled into the path's once for itself and once per later checked cell (:407-412)
-          if (!ok) freps = (line.n - 1) / 4 - cc / 4 + 1;
-          sum += t;
-          ++nLine;
-        }
-        if (!ok) break;  // :414-417, :453-456
-        add_segment_d(sum / (double)nLine, ex - sx, ey - sy, k, lengthPath, result);
-      }
-    }
-    is_safe[q] = ok ? 1 : 0;
-    trav_out[q] = ok ? result : 0.0;
-    area_out[q] = 0.0;
-    if (!want_poly) continue;
-    // the last non-empty polygon published for the path: only an untraversable circle has one (inclination failures return first)
-    if (!c || ok || fkind == 0) {
-      ucount[q] = 0;
-    } else if (fkind == 1) {
-      double2 pts[3 * kFromCircleVertices];
-      write_circle_polygon_d(CT.cs, CT.sn, fx, fy, rmax, n > 1, pts, UntravOut{max_vertices, ucount, uxy}, q);
-    } else {  // as write_cells_polygon_d, from the record
-      const MapRecord& r = recs[fkey];
-      double* xy = uxy + 2 * (size_t)max_vertices * q;
-      if (r.cnt >= 4 || (r.cnt >= 2 && freps >= 2)) {
-        ucount[q] = r.nv;
-        const double* h = hulls.data() + 2 * (size_t)maxv * keys[fkey].slot;
-        for (int u = 0; u < std::min(r.nv, max_vertices); ++u) { xy[2 * u] = h[2 * u]; xy[2 * u + 1] = h[2 * u + 1]; }
-      } else {
-        const int nv = (r.cnt == 1 && freps >= 2) ? 2 + (freps & 1) : r.cnt;
-        ucount[q] = nv;
-        for (int u = 0; u < std::min(nv, max_vertices); ++u) {
-          const int2 cl = r.first[r.cnt == 1 ? 0 : u];
-          xy[2 * u] = hX[cl.x];
-          xy[2 * u + 1] = hY[cl.y];
-        }
-      }
-    }
-  }
-
-  // 4. the cells the replay stored go into the device cache
-  const int nw = (int)order.size();
-  stats->stored = nw;
-  if (nw > 0) {
-    std::vector<unsigned long long> cells(order);
-    std::vector<float> vals(nw);
-    for (int k = 0; k < nw; ++k) vals[k] = overlay.at(order[k]);
-    const size_t o_vals = align16(sizeof(unsigned long long) * nw);
-    if (st.mapbuf.reserve(o_vals + sizeof(float) * nw) != cudaSuccess) { st.why = "allocating the cache update failed"; return TE_ERR_CUDA; }
-    char* base = (char*)st.mapbuf.p;
-    if (cudaMemcpyAsync(base, cells.data(), sizeof(unsigned long long) * nw, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-        cudaMemcpyAsync(base + o_vals, vals.data(), sizeof(float) * nw, cudaMemcpyHostToDevice, s) != cudaSuccess) {
-      st.why = "cache update upload failed";
-      return TE_ERR_CUDA;
-    }
-    k_map_scatter<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(cache, (const unsigned long long*)base, (const float*)(base + o_vals), nw);
-    ++*launches;
-    if (cudaStreamSynchronize(s) != cudaSuccess) { st.why = "cache update failed"; return TE_ERR_CUDA; }  // cells / vals are freed
-  }
-  return 0;
-}
 
 int launch_map_request_device(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p,
                               const float* trav, const float* slope, const float* step, const float* rough, const float* elev,
                               const float* robot_slope, float* cache, int nmaps, const int* path_map, int npaths, int nposes,
                               const int* path_begin, const double* poses, const double* radius, const int* footprint_begin,
                               const unsigned char* cup, unsigned char* is_safe, double* trav_out, double* area_out, int max_vertices,
-                              int* ucount, double* uxy, long long max_checks, int sms, cudaStream_t s, int* launches) {
+                              int* ucount, double* uxy, long long max_checks, bool nonfinite_ok, int sms, cudaStream_t s,
+                              int* launches) {
   *launches = 0;
   if (nmaps < 1 || (!path_map && nmaps != 1)) { st.why = "a batch of maps needs a map per path"; return TE_ERR_BAD_ARG; }
   if (int rc = ensure_ring_table(st, s)) return rc;
@@ -2813,6 +2516,7 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
   D.map_range = (int*)(base + o_range); D.entries = (ReqEntry*)(base + o_entries); D.kid = (int*)(base + o_kid);
   D.table = (int*)(base + o_table); D.tmask = tslots - 1; D.keys = (MapKey*)(base + o_keys); D.recs = (MapRecord*)(base + o_recs);
   D.counters = (unsigned long long*)(base + o_counters);
+  D.nonfinite_ok = nonfinite_ok;
   st.req_counters = D.counters;
   void* tmp = base + o_cub;
   if (cudaMemsetAsync(base + o_counters, 0, o_status - o_counters, s) != cudaSuccess ||  // counters and map ranges

@@ -1,7 +1,8 @@
 // te_grid.cuh — the grid_map index arithmetic that the host and the kernels must agree on bit for bit: cell centres, isInside,
-// getIndex, boundPositionToRange, getSubmap's geometry and the LineIterator walk.  The map request (te_map_check_footprint_request)
-// enumerates on the host the circles the kernels then walk, so both sides compile this one definition (the literal translation units build with --fmad=false; the host
-// compiler targets x86-64 without FMA, so neither side contracts a*b+c).
+// getIndex, boundPositionToRange, getSubmap's geometry and the LineIterator walk.  A map request in host memory
+// (te_map_check_footprint_request) sizes on the host the work list of circle checks the kernels then fill, and the submap entries
+// compute their windows on the host, so both sides compile this one definition (the literal translation units build with
+// --fmad=false; the host compiler targets x86-64 without FMA, so neither side contracts a*b+c).
 #pragma once
 #include <cmath>
 #include <cstdlib>
