@@ -512,12 +512,52 @@ int te_map_set_layers_batched(te_map* map, const te_geometry* g, int32_t nmaps, 
                               const float* step, const float* roughness_or_null, const float* elevation,
                               const float* robot_slope_or_null, int memory);
 
+/* Updates of some maps of a batch: te_map_chain_maps, te_map_set_layers_maps and te_map_footprint_maps act on the maps
+ * map_index[0..nsel) only, as the single-map entry would on a te_map holding that map alone, and leave every bit of the other maps'
+ * layers, caches and memos as it was.  So a batch keeps modelling one reference node per map when the maps are updated
+ * independently (a robot receives a new elevation map, a simulated environment resets its terrain).  Rules:
+ *   - map_index is a HOST array in both memory modes, read before the call returns (pageable or page-locked, the caller may reuse
+ *     it at once); nsel is 1..nmaps and the entries are distinct and in 0..nmaps-1, in any order.  Layer arguments and outputs
+ *     hold the nsel maps back to back in map_index order.
+ *   - g must equal the batch's geometry bit for bit (TE_ERR_BAD_ARG otherwise).  A start index, in g or on the te_map's layers, is
+ *     TE_ERR_UNSUPPORTED, as for every _batched entry (use te_map_chain there).  A te_map without layers is TE_ERR_BAD_ARG.
+ *   - Every map of a batch holds the same layers, so the optional layers stay those the batch holds: te_map_chain_maps, which gives
+ *     a map roughness and no robot_slope as te_map_chain does, is TE_ERR_UNSUPPORTED on a batch that holds robot_slope or lacks
+ *     roughness; te_map_set_layers_maps must be given exactly the batch's optional layers (TE_ERR_MISSING_LAYER for a missing one,
+ *     TE_ERR_BAD_ARG for an extra one).
+ *   - Every argument error is found before anything is written: the te_map is then unchanged.
+ *   - The selected maps' caches are emptied and their memo bytes cleared; the memo of the other maps and its parameter key stay.
+ * The selected maps move through scratch the te_map keeps, grown to the largest nsel seen and released by te_map_destroy, in bytes
+ * per cell of the selected maps: te_map_chain_maps 20 in host memory, 16 in device memory (the elevation is read in place);
+ * te_map_set_layers_maps 4 per layer given in host memory, none in device memory; te_map_footprint_maps 4 per layer the sweep
+ * reads (16, or 20 with verify_roughness) plus 4 for the sweep's values, a buffer te_map_footprint shares (it holds the whole
+ * batch once te_map_footprint has run).  Plus 4 bytes per selected map for the slot table.  Launches: those of te_chain_batched
+ * (te_map_chain_maps) or te_footprint_batched (te_map_footprint_maps) on nsel maps, plus one kernel that puts the maps in place
+ * (te_map_set_layers_maps: that kernel alone) or, for the sweep, one that gathers them and the merge into the caches; none per
+ * selected map. */
+
+/* computeTraversability for the maps map_index[0..nsel) of a batch: te_chain_batched on nsel elevation maps (back to back in
+ * map_index order) into those maps' layers; each output optionally copied out, nsel maps back to back in map_index order. */
+int te_map_chain_maps(te_map* map, const te_geometry* g, const te_chain_params* p, int32_t nsel, const int32_t* map_index,
+                      const float* elevation, float* slope_or_null, float* step_or_null, float* roughness_or_null,
+                      float* traversability_or_null, int memory);
+
+/* setTraversabilityMap for those maps only: every layer holds nsel maps back to back in map_index order. */
+int te_map_set_layers_maps(te_map* map, const te_geometry* g, int32_t nsel, const int32_t* map_index, const float* traversability,
+                           const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                           const float* robot_slope_or_null, int memory);
+
 /* traversabilityFootprint(radius, offset) (:307-318) on the cache: a cached cell keeps its value (the memoised branch, :673-675),
  * every other cell gets te_footprint2's value for `p`; traversability_footprint_or_null receives the cache afterwards.  The
  * prefix-sum sweep may differ from the visit-by-visit one in the last float32 bit of a few cells (DESIGN.md §4.3); those values
  * then stay in the cache.  Errors as te_footprint2 (TE_ERR_MISSING_LAYER: verify_roughness without a roughness layer).  On a
  * batch: every map's cache, te_footprint_batched's sweep, nmaps layers out. */
 int te_map_footprint(te_map* map, const te_footprint_params* p, float* traversability_footprint_or_null, int memory);
+
+/* traversabilityFootprint(radius, offset) on the caches of the maps map_index[0..nsel) only (rules above te_map_chain_maps): each
+ * selected cache becomes what te_map_footprint gives that map; the output holds the nsel caches afterwards in map_index order. */
+int te_map_footprint_maps(te_map* map, const te_footprint_params* p, int32_t nsel, const int32_t* map_index,
+                          float* traversability_footprint_or_null, int memory);
 
 /* traversabilityFootprint(yaw) (:239-305): te_footprint_polygon on the map's layers.  Reads and changes no cache.  On a batch:
  * te_footprint_polygon_batched's outputs (and te_footprint_polygon_yaws(_reduce)'s for the two entries below: layer k of map m at

@@ -156,7 +156,10 @@ SIGNATURES = {
     "te_map_set_layers": (_R, [_P, _G, _P, _P, _P, _P, _P, _P, _I]),
     "te_map_chain_batched": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _I]),
     "te_map_set_layers_batched": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _I]),
+    "te_map_chain_maps": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _P, _I]),
+    "te_map_set_layers_maps": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _P, _I]),
     "te_map_footprint": (_R, [_P, _FP, _P, _I]),
+    "te_map_footprint_maps": (_R, [_P, _FP, _I, _P, _P, _I]),
     "te_map_footprint_polygon": (_R, [_P, _FP, _I, _P, _D, _P, _P, _I]),
     "te_map_footprint_polygon_yaws": (_R, [_P, _FP, _I, _P, _I, _P, _P, _I]),
     "te_map_footprint_polygon_yaws_reduce": (_R, [_P, _FP, _I, _P, _I, _P, _P, _P, _P, _I]),
@@ -772,6 +775,40 @@ class Map:
         t, s, st, r, e, rs = (self._batch_layers(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
         self._check(fn(self._h, C.byref(g), int(nmaps), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST))
         self._g, self._n = g, int(nmaps)
+
+    @staticmethod
+    def _map_index(map_index):
+        return np.ascontiguousarray(map_index, dtype=np.int32).reshape(-1)
+
+    def chain_maps(self, g, p, map_index, elevation, outputs=False):
+        """te_map_chain_maps (computeTraversability for the maps map_index of the batch only): elevation (nsel, rows, cols), map
+        j of it going to map map_index[j]; empties those maps' caches and keeps every other map as it was.  outputs=True also
+        returns the four layers as a dict of (nsel, rows, cols) arrays in map_index order."""
+        idx = self._map_index(map_index)
+        e = self._batch_layers(elevation)
+        out = {k: np.empty((len(idx), g.cols, g.rows), dtype=np.float32) for k in ("slope", "step", "roughness", "traversability")} \
+            if outputs else {}
+        self._check(self._L.te_map_chain_maps(self._h, C.byref(g), C.byref(p), len(idx), _addr(idx), _addr(e),
+                                              *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")),
+                                              MEM_HOST))
+        return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
+
+    def set_layers_maps(self, g, map_index, traversability, slope, step, elevation, roughness=None, robot_slope=None):
+        """te_map_set_layers_maps (setTraversabilityMap for the maps map_index only): each layer (nsel, rows, cols) in map_index
+        order; the optional layers must be those the batch holds.  Empties those maps' caches and memos."""
+        idx = self._map_index(map_index)
+        t, s, st, r, e, rs = (self._batch_layers(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
+        self._check(self._L.te_map_set_layers_maps(self._h, C.byref(g), len(idx), _addr(idx), _addr(t), _addr(s), _addr(st), _addr(r),
+                                                   _addr(e), _addr(rs), MEM_HOST))
+
+    def footprint_maps(self, fp, map_index):
+        """te_map_footprint_maps (traversabilityFootprint(radius, offset) on the caches of the maps map_index only); returns those
+        caches afterwards, (nsel, rows, cols) in map_index order."""
+        idx = self._map_index(map_index)
+        rows, cols = self._shape() if self._g else (0, 0)
+        buf = np.empty((len(idx), cols, rows), dtype=np.float32)
+        self._check(self._L.te_map_footprint_maps(self._h, C.byref(fp), len(idx), _addr(idx), _addr(buf), MEM_HOST))
+        return buf.transpose(0, 2, 1)
 
     def footprint(self, fp):
         """te_map_footprint (traversabilityFootprint(radius, offset) on the cache); returns the cache afterwards."""

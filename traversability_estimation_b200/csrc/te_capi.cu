@@ -1305,6 +1305,8 @@ struct te_map {
   te_geometry geo{};     // the same with the start index cleared: the device layers are in default order
   DevBuf trav, slope, step, rough, elev, rslope, cache, fresh;
   DevBuf gather;  // te_map_get_submaps: the source-layer table, then the windows (te::SubmapWindow)
+  // The _maps entries: the selected maps' layers packed back to back (grown to the largest selection) and their slot table
+  DevBuf sel[te::kMapSlotLayers], slots;
   bool have_rough = false, have_rslope = false;
   te::FootprintState fp;  // the map's own scratch; fp.memo is the resident memo
   bool memo_valid = false;
@@ -1414,6 +1416,79 @@ int map_layers(const te_map* m, uint32_t mask, const float* out[7], int* n) {
   return TE_OK;
 }
 
+// The maps a _maps entry updates: n distinct indices of the batch, a host array.  The whole-batch entries pass none.
+struct MapSel {
+  int32_t n;
+  const int32_t* idx;
+};
+
+// Validates a selection on a te_map that has layers and, when the entry takes one (with_geometry), g against the batch's
+// geometry.  Writes nothing.
+int map_select(const te_map* m, bool with_geometry, const te_geometry* g, const MapSel& s) {
+  if (int rc = map_ready(m)) return rc;
+  if (with_geometry) {
+    if (int rc = check_geometry(g, true)) return rc;
+    if (g->start_row != 0 || g->start_col != 0)
+      return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0) is unsupported for the _maps entries", g->start_row,
+                  g->start_col);
+  }
+  if (m->geo_in.start_row != 0 || m->geo_in.start_col != 0)
+    return fail(TE_ERR_UNSUPPORTED, "the te_map's layers came with a circular-buffer start index: use te_map_chain / te_map_set_layers");
+  if (with_geometry && std::memcmp(g, &m->geo, sizeof(te_geometry)) != 0)
+    return fail(TE_ERR_BAD_ARG, "the geometry differs from the te_map's: reload the whole batch to change it");
+  if (s.n < 1 || s.n > m->nmaps) return fail(TE_ERR_BAD_ARG, "nsel = %d: need 1..%d", s.n, m->nmaps);
+  if (!s.idx) return fail(TE_ERR_BAD_ARG, "map_index is null");
+  std::vector<char> seen(m->nmaps, 0);
+  for (int32_t k = 0; k < s.n; ++k) {
+    const int32_t v = s.idx[k];
+    if (v < 0 || v >= m->nmaps) return fail(TE_ERR_BAD_ARG, "map_index[%d] = %d is outside 0..%d", k, v, m->nmaps - 1);
+    if (seen[v]++) return fail(TE_ERR_BAD_ARG, "map_index[%d] = %d is selected twice", k, v);
+  }
+  return TE_OK;
+}
+
+// Scratch for the packed layers m->sel[l] of the selection with bit l of `layers` set, and its slot table on the device.  A buffer
+// that grows first waits for the kernels that may still read it.  The slot table is uploaded from a copy of map_index made here,
+// so the caller may reuse its array as soon as the call returns, whatever kind of host memory it is: a copy from pageable memory
+// has read its source when cudaMemcpyAsync returns, one from page-locked memory only when the stream reaches it.
+int map_stage_selection(te_map* m, const MapSel& s, unsigned layers) {
+  te_ctx* c = m->ctx;
+  const size_t bytes = sizeof(float) * map_cells(m) * s.n, tbytes = sizeof(int32_t) * s.n;
+  bool grow = m->slots.p && m->slots.cap < tbytes;
+  for (int l = 0; l < te::kMapSlotLayers; ++l) grow = grow || (((layers >> l) & 1u) && m->sel[l].p && m->sel[l].cap < bytes);
+  if (grow) TE_CUDA(cudaStreamSynchronize(c->stream));
+  for (int l = 0; l < te::kMapSlotLayers; ++l)
+    if ((layers >> l) & 1u) TE_CUDA(m->sel[l].reserve(bytes));
+  TE_CUDA(m->slots.reserve(tbytes));
+  const std::vector<int32_t> idx(s.idx, s.idx + s.n);  // pageable: consumed before cudaMemcpyAsync returns
+  TE_CUDA(cudaMemcpyAsync(m->slots.p, idx.data(), tbytes, cudaMemcpyHostToDevice, c->stream));
+  return TE_OK;
+}
+
+// n cells between a packed device buffer and the caller's array in `memory` (selected maps back to back, no start index).
+cudaError_t map_copy_packed(te_map* m, float* dst, const float* src, size_t n, bool to_caller, int memory) {
+  const cudaMemcpyKind kind = memory == TE_MEM_DEVICE ? cudaMemcpyDeviceToDevice : to_caller ? cudaMemcpyDeviceToHost : cudaMemcpyHostToDevice;
+  return cudaMemcpyAsync(dst, src, sizeof(float) * n, kind, m->ctx->stream);
+}
+
+// The packed layers src (each null or nsel maps back to back) into the selected maps' resident layers dst, in one launch that also
+// empties those maps' caches and, when the memo is live, clears their memo bytes.  The te_map-wide memo key stays.
+int map_put_selected(te_map* m, const MapSel& s, const float* const src[te::kMapSlotLayers], DevBuf* const dst[te::kMapSlotLayers]) {
+  te_ctx* c = m->ctx;
+  te::MapSlots a{};
+  for (int l = 0; l < te::kMapSlotLayers; ++l) {
+    a.src[l] = dst[l] ? src[l] : nullptr;
+    a.dst[l] = dst[l] ? (float*)dst[l]->p : nullptr;
+  }
+  a.cache = (float*)m->cache.p;
+  a.memo = m->memo_valid ? (unsigned char*)m->fp.memo.p : nullptr;  // reserved for the whole batch while valid (map_memo)
+  a.slot = (const int*)m->slots.p;
+  a.nsel = s.n;
+  a.cells = map_cells(m);
+  te::launch_map_slots(a, true, c->sms, c->stream);
+  return launch_check(c, "k_map_slots (put)");
+}
+
 #define TE_MAP_ENTER(map)                                   \
   if (!(map)) return fail(TE_ERR_BAD_ARG, "map is null");   \
   te_ctx* c = (map)->ctx;                                   \
@@ -1437,7 +1512,8 @@ int te_map_destroy(te_map* m) {
     Guard g(m->ctx);
     if (g.ok) {
       cudaStreamSynchronize(m->ctx->stream);
-      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather}) b->release();
+      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather, &m->slots}) b->release();
+      for (DevBuf& b : m->sel) b.release();
       m->fp.release();
     }
   }
@@ -1447,41 +1523,106 @@ int te_map_destroy(te_map* m) {
 
 namespace {
 
-// te_map_chain (nmaps = 1) and te_map_chain_batched.
+// te_map_chain (nmaps = 1), te_map_chain_batched and, with a selection, te_map_chain_maps: the selected maps' layers are chained
+// into scratch (the elevation staged there in host memory, read in place in device memory) and k_map_slots puts them in place.
 int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int nmaps, const float* elev, float* slope, float* step,
-              float* rough, float* trav, int memory) {
+              float* rough, float* trav, int memory, const MapSel* sel = nullptr) {
   te_ctx* c = m->ctx;
   te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) return rc;
+  if (sel) {
+    if (int rc = map_select(m, true, g_in, *sel)) return rc;
+    g0 = m->geo;
+    nmaps = sel->n;
+  } else if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) {
+    return rc;
+  }
   if (int rc = check_params(p)) return rc;
   if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
-  if (int rc = map_reset(m, g_in, &g0, nmaps)) return rc;
-  TE_CUDA(m->rough.reserve(sizeof(float) * batch_cells(m)));
-  if (int rc = map_put_layer(m, m->elev, elev, memory)) return rc;
-  if (int rc = chain_common(c, &g0, nullptr, p, nmaps, (const float*)m->elev.p, (float*)m->slope.p, (float*)m->step.p, (float*)m->rough.p,
-                            (float*)m->trav.p, nullptr, nullptr, nullptr, TE_MEM_DEVICE))
+  if (sel && (m->have_rslope || !m->have_rough))
+    return fail(TE_ERR_UNSUPPORTED, "the batch %s, and te_map_chain_maps gives a map roughness and no robot_slope: every map of a batch holds "
+                "the same layers, so use te_map_set_layers_maps or reload the whole batch",
+                m->have_rslope ? "holds robot_slope" : "has no roughness");
+  DevBuf* const lay[5] = {sel ? &m->sel[0] : &m->elev, sel ? &m->sel[1] : &m->slope, sel ? &m->sel[2] : &m->step,
+                          sel ? &m->sel[3] : &m->rough, sel ? &m->sel[4] : &m->trav};  // where the chain reads and writes
+  const size_t cells = map_cells(m) * (sel ? sel->n : 0);
+  const float* din = elev;
+  if (sel) {
+    if (int rc = map_stage_selection(m, *sel, memory == TE_MEM_HOST ? 0x1fu : 0x1eu)) return rc;  // sel[0]: the staged elevation
+    if (memory == TE_MEM_HOST) {
+      TE_CUDA(map_copy_packed(m, (float*)lay[0]->p, elev, cells, false, memory));
+      din = (const float*)lay[0]->p;
+    }
+  } else {
+    if (int rc = map_reset(m, g_in, &g0, nmaps)) return rc;
+    TE_CUDA(m->rough.reserve(sizeof(float) * batch_cells(m)));
+    if (int rc = map_put_layer(m, m->elev, elev, memory)) return rc;
+    din = (const float*)m->elev.p;
+  }
+  if (int rc = chain_common(c, &g0, nullptr, p, nmaps, din, (float*)lay[1]->p, (float*)lay[2]->p, (float*)lay[3]->p, (float*)lay[4]->p,
+                            nullptr, nullptr, nullptr, TE_MEM_DEVICE))
     return rc;
-  m->have_rough = true;
-  m->have_rslope = false;  // computeTraversability leaves robot_slope to a later setTraversabilityMap
-  m->have_layers = true;
-  const std::pair<float*, DevBuf*> outs[4] = {{slope, &m->slope}, {step, &m->step}, {rough, &m->rough}, {trav, &m->trav}};
+  if (sel) {
+    const float* const src[te::kMapSlotLayers] = {(const float*)lay[4]->p, (const float*)lay[1]->p, (const float*)lay[2]->p,
+                                                  (const float*)lay[3]->p, din, nullptr};
+    DevBuf* const dst[te::kMapSlotLayers] = {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, nullptr};
+    if (int rc = map_put_selected(m, *sel, src, dst)) return rc;
+  } else {
+    m->have_rough = true;
+    m->have_rslope = false;  // computeTraversability leaves robot_slope to a later setTraversabilityMap
+    m->have_layers = true;
+  }
+  const std::pair<float*, DevBuf*> outs[4] = {{slope, lay[1]}, {step, lay[2]}, {rough, lay[3]}, {trav, lay[4]}};
   for (const auto& o : outs)
-    if (o.first)
-      if (int rc = map_get_layer(m, o.first, o.second->p, memory)) return rc;
+    if (o.first) {
+      if (sel) TE_CUDA(map_copy_packed(m, o.first, (const float*)o.second->p, cells, true, memory));
+      else if (int rc = map_get_layer(m, o.first, o.second->p, memory)) return rc;
+    }
   if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));
   return TE_OK;
 }
 
-// te_map_set_layers (nmaps = 1) and te_map_set_layers_batched.
+// te_map_set_layers (nmaps = 1), te_map_set_layers_batched and, with a selection, te_map_set_layers_maps: the selected maps'
+// layers (staged in host memory, read in place in device memory) go to their slots in one k_map_slots launch.  The optional
+// layers must then be those the batch holds.
 int map_set_layers(te_map* m, const te_geometry* g_in, int nmaps, const float* trav, const float* slope, const float* step,
-                   const float* rough, const float* elev, const float* robot_slope, int memory) {
+                   const float* rough, const float* elev, const float* robot_slope, int memory, const MapSel* sel = nullptr) {
   te_ctx* c = m->ctx;
   te_geometry g0;
-  if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) return rc;
+  if (sel) {
+    if (int rc = map_select(m, true, g_in, *sel)) return rc;
+  } else if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) {
+    return rc;
+  }
   if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
   if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
   if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
   if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
+  if (sel) {
+    const std::pair<bool, bool> opt[2] = {{m->have_rough, rough != nullptr}, {m->have_rslope, robot_slope != nullptr}};
+    static const char* const names[2] = {"traversability_roughness", "robot_slope"};
+    for (int k = 0; k < 2; ++k) {
+      if (opt[k].first && !opt[k].second)
+        return fail(TE_ERR_MISSING_LAYER, "layer %s is missing: the batch holds it, so every map needs it", names[k]);
+      if (!opt[k].first && opt[k].second)
+        return fail(TE_ERR_BAD_ARG, "layer %s is given but the batch does not hold it: reload the whole batch to add it", names[k]);
+    }
+    const float* src[te::kMapSlotLayers] = {trav, slope, step, rough, elev, robot_slope};
+    DevBuf* const dst[te::kMapSlotLayers] = {&m->trav, &m->slope, &m->step, rough ? &m->rough : nullptr, &m->elev,
+                                             robot_slope ? &m->rslope : nullptr};
+    unsigned staged = 0;  // host memory: the layers given, staged; device memory: read in place
+    for (int l = 0; l < te::kMapSlotLayers; ++l)
+      if (memory == TE_MEM_HOST && src[l]) staged |= 1u << l;
+    if (int rc = map_stage_selection(m, *sel, staged)) return rc;
+    if (memory == TE_MEM_HOST)
+      for (int l = 0; l < te::kMapSlotLayers; ++l)
+        if (src[l]) {
+          TE_CUDA(map_copy_packed(m, (float*)m->sel[l].p, src[l], map_cells(m) * sel->n, false, memory));
+          src[l] = (const float*)m->sel[l].p;
+        }
+    if (int rc = map_put_selected(m, *sel, src, dst)) return rc;
+    if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));  // the caller may reuse its layers on return
+    return TE_OK;
+  }
   if (int rc = map_reset(m, g_in, &g0, nmaps)) return rc;
   if (int rc = map_put_layer(m, m->trav, trav, memory)) return rc;
   if (int rc = map_put_layer(m, m->slope, slope, memory)) return rc;
@@ -1524,29 +1665,80 @@ int te_map_set_layers_batched(te_map* m, const te_geometry* g, int32_t nmaps, co
   return map_set_layers(m, g, nmaps, trav, slope, step, rough, elev, robot_slope, memory);
 }
 
-int te_map_footprint(te_map* m, const te_footprint_params* p, float* out, int memory) {
+int te_map_chain_maps(te_map* m, const te_geometry* g, const te_chain_params* p, int32_t nsel, const int32_t* map_index, const float* elev,
+                      float* slope, float* step, float* rough, float* trav, int memory) {
   TE_MAP_ENTER(m);
-  if (int rc = map_ready(m)) return rc;
+  const MapSel sel{nsel, map_index};
+  return map_chain(m, g, p, nsel, elev, slope, step, rough, trav, memory, &sel);
+}
+
+int te_map_set_layers_maps(te_map* m, const te_geometry* g, int32_t nsel, const int32_t* map_index, const float* trav, const float* slope,
+                           const float* step, const float* rough, const float* elev, const float* robot_slope, int memory) {
+  TE_MAP_ENTER(m);
+  const MapSel sel{nsel, map_index};
+  return map_set_layers(m, g, nsel, trav, slope, step, rough, elev, robot_slope, memory, &sel);
+}
+
+// te_map_footprint (sel null: every map, swept in place) and te_map_footprint_maps (the selected maps' input layers gathered
+// into scratch by one k_map_slots launch, swept as a batch of nsel maps and merged into their cache slots).  A map's sweep reads
+// only its own cells, so each selected map gets the values a whole-batch sweep gives it.
+static int map_footprint(te_map* m, const te_footprint_params* p, const MapSel* sel, float* out, int memory) {
+  te_ctx* c = m->ctx;
+  if (int rc = sel ? map_select(m, false, nullptr, *sel) : map_ready(m)) return rc;
   if (int rc = map_footprint_params(m, p)) return rc;
   if (!(p->radius >= 0.0) || !(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint radius/offset must be >= 0");
   const te_geometry* g = &m->geo;
   if (int rc = ensure_geometry(c, g)) return rc;
-  TE_CUDA(m->fresh.reserve(sizeof(float) * batch_cells(m)));
+  const int n = sel ? sel->n : m->nmaps;
+  TE_CUDA(m->fresh.reserve(sizeof(float) * map_cells(m) * n));
   const te_slab s{0, g->cols, 0, 0};
-  const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
+  // trav, slope, step, rough (verify_roughness only), elev: resident, or gathered for the selection
+  const float* in[5] = {(const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p,
+                        p->verify_roughness ? (const float*)m->rough.p : nullptr, (const float*)m->elev.p};
+  int fixed = 1;  // k_map_merge, and k_map_slots for a selection
+  if (sel) {
+    unsigned gathered = 0;
+    for (int l = 0; l < 5; ++l)
+      if (in[l]) gathered |= 1u << l;
+    if (int rc = map_stage_selection(m, *sel, gathered)) return rc;
+    te::MapSlots a{};
+    for (int l = 0; l < 5; ++l) {
+      a.src[l] = in[l];
+      a.dst[l] = in[l] ? (float*)m->sel[l].p : nullptr;
+      in[l] = a.dst[l];
+    }
+    a.slot = (const int*)m->slots.p;
+    a.nsel = n;
+    a.cells = map_cells(m);
+    te::launch_map_slots(a, false, c->sms, c->stream);
+    ++fixed;
+  }
   int nl = 0;
-  int rc = te::launch_footprint(m->fp, make_view(c, g, s), g, p, m->nmaps, (const float*)m->trav.p, (const float*)m->slope.p,
-                                (const float*)m->step.p, rough, (const float*)m->elev.p, (float*)m->fresh.p, nullptr, nullptr, nullptr,
-                                c->sms, c->stream, &nl);
+  int rc = te::launch_footprint(m->fp, make_view(c, g, s), g, p, n, in[0], in[1], in[2], in[3], in[4], (float*)m->fresh.p, nullptr,
+                                nullptr, nullptr, c->sms, c->stream, &nl);
   if (rc != 0) return fail(rc, "footprint sweep failed: %s", m->fp.why.c_str());
-  te::launch_map_merge((const float*)m->fresh.p, (float*)m->cache.p, (out && memory == TE_MEM_DEVICE) ? out : nullptr, batch_cells(m),
-                       c->sms, c->stream);
-  if (int r2 = launch_check(c, "map footprint", nl + 1)) return r2;
+  // host memory: the whole cache is read back from its resident layer, a selection's from packed scratch (its trav slot)
+  float* const dout = !out ? nullptr : memory == TE_MEM_DEVICE ? out : sel ? (float*)m->sel[0].p : nullptr;
+  te::launch_map_merge((const float*)m->fresh.p, (float*)m->cache.p, dout, sel ? map_cells(m) : batch_cells(m),
+                       sel ? (const int*)m->slots.p : nullptr, sel ? n : 1, c->sms, c->stream);
+  if (int r2 = launch_check(c, "map footprint", nl + fixed)) return r2;
   if (out && memory == TE_MEM_HOST) {
-    if (int r2 = map_get_layer(m, out, m->cache.p, memory)) return r2;
+    if (sel) TE_CUDA(map_copy_packed(m, out, dout, map_cells(m) * n, true, memory));
+    else if (int r2 = map_get_layer(m, out, m->cache.p, memory)) return r2;
     TE_CUDA(cudaStreamSynchronize(c->stream));
   }
   return TE_OK;
+}
+
+int te_map_footprint(te_map* m, const te_footprint_params* p, float* out, int memory) {
+  TE_MAP_ENTER(m);
+  return map_footprint(m, p, nullptr, out, memory);
+}
+
+int te_map_footprint_maps(te_map* m, const te_footprint_params* p, int32_t nsel, const int32_t* map_index, float* out, int memory) {
+  TE_MAP_ENTER(m);
+  const MapSel sel{nsel, map_index};
+  return map_footprint(m, p, &sel, out, memory);
 }
 
 // The te_map polygon entries: footprint_polygon_common on the map's resident layers with the map's own state.  They neither read

@@ -21,6 +21,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 namespace te {
 namespace {
@@ -1474,12 +1475,45 @@ __global__ void __launch_bounds__(128, 4) k_map_eval_circles_dev(FpArgs A, Layer
 }
 
 // traversabilityFootprint(radius, offset) on a cache: a cached cell takes the memoised branch and keeps its value, every other cell
-// gets the sweep's.  `out` (may be null or `cache` itself) receives the cache afterwards.
-__global__ void __launch_bounds__(256) k_map_merge(float* cache, const float* __restrict__ fresh, float* out, size_t n) {
+// gets the sweep's.  `out` (may be null or `cache` itself) receives the cache afterwards.  Block row y merges n cells: `fresh` and
+// `out` from y * n on, the cache from slot[y] * n on (slot null: y * n).
+__global__ void __launch_bounds__(256) k_map_merge(float* cache, const float* __restrict__ fresh, float* out, size_t n,
+                                                   const int* __restrict__ slot) {
+  const size_t y = blockIdx.y;
+  cache += (slot ? (size_t)slot[y] : y) * n;
+  fresh += y * n;
+  if (out) out += y * n;
   for (size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x; c < n; c += (size_t)gridDim.x * blockDim.x) {
     const float v = finitef(cache[c]) ? cache[c] : fresh[c];
     cache[c] = v;
     if (out) out[c] = v;
+  }
+}
+
+// Selected maps between their slots of a te_map and packed scratch (launch_map_slots).  PUT: layer l of packed map j goes to
+// dst[l] + slot[j] * cells, and the cache / memo slots of the map are emptied (NaN bits 0xffffffff, memo 0: not evaluated).  Not
+// PUT: src[l] + slot[j] * cells goes to packed map j of dst[l].  V cells per thread and access (V = 4: 16-byte accesses).
+template <bool PUT, int V>
+__global__ void __launch_bounds__(256) k_map_slots(MapSlots a) {
+  using Vec = typename std::conditional<V == 4, float4, float>::type;
+  using Bytes = typename std::conditional<V == 4, unsigned, unsigned char>::type;
+  const size_t step = (size_t)gridDim.x * blockDim.x * V;
+  for (int j = blockIdx.y; j < a.nsel; j += gridDim.y) {
+    const size_t packed = (size_t)j * a.cells, resident = (size_t)a.slot[j] * a.cells;
+    const size_t s0 = PUT ? packed : resident, d0 = PUT ? resident : packed;
+    for (size_t c = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * V; c < a.cells; c += step) {
+#pragma unroll
+      for (int l = 0; l < kMapSlotLayers; ++l)
+        if (a.dst[l]) *reinterpret_cast<Vec*>(a.dst[l] + d0 + c) = __ldg(reinterpret_cast<const Vec*>(a.src[l] + s0 + c));
+      if (PUT) {
+        const float nan = __int_as_float(-1);
+        Vec e;
+        if constexpr (V == 4) e = make_float4(nan, nan, nan, nan);
+        else e = nan;
+        *reinterpret_cast<Vec*>(a.cache + resident + c) = e;
+        if (a.memo) *reinterpret_cast<Bytes*>(a.memo + resident + c) = 0;
+      }
+    }
   }
 }
 
@@ -2552,10 +2586,29 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
   return 0;
 }
 
-int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, int sms, cudaStream_t s) {
-  const long long blocks = std::min<long long>((long long)((n + 255) / 256), (long long)sms * 8);
-  k_map_merge<<<(unsigned)std::max(blocks, 1LL), 256, 0, s>>>(cache, fresh, out, n);
+int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, const int* slot, int nsel, int sms, cudaStream_t s) {
+  const long long per_map = std::max<long long>((long long)sms * 8 / nsel, 1);
+  const long long blocks = std::min<long long>((long long)((n + 255) / 256), per_map);
+  k_map_merge<<<dim3((unsigned)std::max(blocks, 1LL), (unsigned)nsel), 256, 0, s>>>(cache, fresh, out, n, slot);
   return 0;
+}
+
+void launch_map_slots(const MapSlots& a, bool put, int sms, cudaStream_t s) {
+  // 16-byte accesses when every map slot and every layer starts on a 16-byte boundary
+  bool vec = a.cells % 4 == 0 && (reinterpret_cast<uintptr_t>(a.cache) & 15u) == 0;
+  for (int l = 0; l < kMapSlotLayers; ++l)
+    vec = vec && ((reinterpret_cast<uintptr_t>(a.src[l]) | reinterpret_cast<uintptr_t>(a.dst[l])) & 15u) == 0;
+  const int V = vec ? 4 : 1;
+  const long long per_map = std::max<long long>((long long)sms * 8 / a.nsel, 1);
+  const long long bx = std::max(std::min<long long>((long long)((a.cells / V + 255) / 256), per_map), 1LL);
+  const dim3 grid((unsigned)bx, (unsigned)std::min(a.nsel, 65535));
+  if (put) {
+    if (vec) k_map_slots<true, 4><<<grid, 256, 0, s>>>(a);
+    else k_map_slots<true, 1><<<grid, 256, 0, s>>>(a);
+  } else {
+    if (vec) k_map_slots<false, 4><<<grid, 256, 0, s>>>(a);
+    else k_map_slots<false, 1><<<grid, 256, 0, s>>>(a);
+  }
 }
 
 // isTraversableForFilters for every cell of the slab + halo of each of the nmaps maps into st.block (k_pred_classify +

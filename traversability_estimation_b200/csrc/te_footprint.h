@@ -150,8 +150,26 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
                               const unsigned char* cup, unsigned char* is_safe, double* trav_out, double* area_out, int max_vertices,
                               int* ucount, double* uxy, long long max_checks, bool nonfinite_ok, int sms, cudaStream_t s,
                               int* launches);
-// traversabilityFootprint(radius, offset) on a cache: cache = finite(cache) ? cache : fresh over n cells; `out` (device, may be
-// null) receives the result too.
-int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, int sms, cudaStream_t s);
+// traversabilityFootprint(radius, offset) on a cache: cache = finite(cache) ? cache : fresh over nsel blocks of n cells; `out`
+// (device, may be null) receives the result too.  Block j of `fresh` and `out` starts at j * n, its cache block at slot[j] * n
+// (slot: a device table of nsel map slots; null: j * n, the whole batch as nsel = 1 block of every cell).  One launch.
+int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, const int* slot, int nsel, int sms, cudaStream_t s);
+
+// Selected maps of a te_map (te_map_chain_maps, te_map_set_layers_maps, te_map_footprint_maps): packed map j is at j * cells in
+// scratch, its resident copy at slot[j] * cells in the te_map's layers, cache and memo.  Up to kMapSlotLayers layers move in one
+// launch; a layer with a null dst is skipped.  put: packed src -> resident dst, and the maps' cache slots become NaN (empty) and
+// their memo slots 0 (memo may be null); otherwise resident src -> packed dst (cache and memo unused).  Grid-stride over maps and
+// cells, 16-byte accesses when cells % 4 == 0 and every pointer is 16-byte aligned.  One launch, whatever nsel and the layers.
+constexpr int kMapSlotLayers = 6;
+struct MapSlots {
+  const float* src[kMapSlotLayers];
+  float* dst[kMapSlotLayers];
+  float* cache;
+  unsigned char* memo;
+  const int* slot;  // device, nsel entries
+  int nsel;
+  size_t cells;     // per map
+};
+void launch_map_slots(const MapSlots& a, bool put, int sms, cudaStream_t s);
 
 }  // namespace te
