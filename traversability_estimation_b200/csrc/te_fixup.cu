@@ -264,14 +264,15 @@ __device__ bool normals_t2(const FixupArgs& A, const Elev& E, int i, int j, floa
     if (nz < 0.0) { nx = -nx; ny = -ny; nz = -nz; }
     why = 8u | ((unsigned)cnt << 8);
     if (nz == 0.0) return false;
-    // float32 rounding of n_z: where acos amplifies one ulp beyond the tolerance (theta < ~0.02 rad) the rounding must be
-    // certain: escalate when n_z is within A.nz_guard ulps of a rounding boundary (make_fixup_args: 100 x the error the
-    // reference's absolute-coordinate arithmetic can carry into its own n_z)
-    if (nz > 0.9998) {
+    // float32 rounding of n_z: where acos amplifies one ulp beyond the tolerance (theta < ~0.02 rad at crit = 1 rad, up to
+    // just past crit for small crit: A.nz_check) the rounding must be certain: escalate when n_z is within A.nz_guard ulps of a
+    // rounding boundary (make_fixup_args: 100 x the error the reference's absolute-coordinate arithmetic can carry into its own n_z)
+    if (nz > A.nz_check) {
       const float f = (float)nz;
       const float up = __uint_as_float(__float_as_uint(f) + 1u), dn = __uint_as_float(__float_as_uint(f) - 1u);
       const double bu = 0.5 * ((double)f + (double)up), bd = 0.5 * ((double)f + (double)dn);
-      const double guard = A.nz_guard * (bu - bd);
+      // the reference's error grows with the cell's own s = 1 - n_z: nz_guard holds for s <= 2e-4
+      const double guard = A.nz_guard * fmax(1.0, (1.0 - nz) * 5e3) * (bu - bd);
       why = 9u | ((unsigned)cnt << 8);
       if (fabs(nz - bu) < guard || fabs(nz - bd) < guard) return false;
     }

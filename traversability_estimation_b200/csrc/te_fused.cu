@@ -114,6 +114,7 @@ struct FusedArgs {
   unsigned* list;
   unsigned* count;
   unsigned cap;
+  float k_nz_check;  // s = 1 - n_z below which the float32 rounding of n_z is certified: nz_check_limit(slope_crit)
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -405,10 +406,11 @@ __device__ __forceinline__ Normal2 finish_normal2(const FusedArgs& A, f2 Sw, f2 
   const bool fail0 = !(min2n(lo(t1), lo(t2)) > 0.f) & (lo(Sww) != 0.f) & (lo(inval) == 0.f);
   const bool fail1 = !(min2n(hi(t1), hi(t2)) > 0.f) & (hi(Sww) != 0.f) & (hi(inval) == 0.f);
   unsigned flag = (unsigned)fail0 | ((unsigned)fail1 << 1);
-  // where acos amplifies one ulp of n_z beyond the tolerance (theta < ~0.012 rad) certify its float32 rounding
+  // where acos amplifies one ulp of n_z beyond half the slope layer's tolerance (s < k_nz_check: theta < 0.012 rad at crit
+  // >= 1 rad, every theta up to just past crit below crit ~0.35 rad) certify its float32 rounding.
   // n_z = 1 - s is rounded to float32 with spacing 2^-24: flag when s, known to relative error eps, may sit on the other
   // side of a rounding boundary (eps: the first moments carry <= 2.5e-6*sqrt(Sww) absolute error).  Both rows at once.
-  const bool cx = lo(s) < 7.2e-5f && lo(Sww) > 0.f, cy = hi(s) < 7.2e-5f && hi(Sww) > 0.f;
+  const bool cx = lo(s) < A.k_nz_check && lo(Sww) > 0.f, cy = hi(s) < A.k_nz_check && hi(Sww) > 0.f;
   if (cx || cy) {
     const f2 qv = mul2c(s, A.k_2p24);
     const f2 fr = sub2(qv, mk(floorf(lo(qv)), floorf(hi(qv))));
@@ -866,6 +868,44 @@ WindowClass classify(double radius, double res) {
   return c;
 }
 
+// s = 1 - n_z below which the float32 rounding of n_z has to be certain (finish_normal2's k_nz_check; tier 2 widens its guard
+// band to it).  One float32 ulp of n_z (2^-24 on [0.5, 1)) moves theta = acos(n_z) by ~2^-24 / sin(theta) and the slope layer
+// 1 - theta/crit by that over crit, while the layer's tolerance 1e-5 |layer| + 1e-6 does not scale with crit; and away from a
+// rounding boundary the fp32 n_z may be several ulps off (s carries the relative error of the moments), which near theta = crit,
+// where the tolerance is 1e-6, the layer does not absorb either once crit < 1 rad.  So below 1 rad the band is every theta up to
+// just past crit (2 % and 4 ulps of n_z past it, where the layer could otherwise step across its 0 branch): inside it a cell is
+// either rounded exactly like the reference or flagged.  From 1 rad up it stays the 7.2e-5 (theta = 0.012 rad) calibrated at
+// the YAML's crit = 1 rad (DESIGN.md §4.1: worst slope error 0.45 x tolerance on the 8192^2 map), so the YAML outputs keep every
+// bit; there one ulp moves the layer by at most half its tolerance above the band.  s < 0.48: n_z > 0.5, the 2^-24 spacing the
+// check assumes.  tests/test_kernel_constants_cpu.py restates this and checks it against every float32 n_z.
+double nz_check_limit(double crit) {
+  if (!(crit < 1.0)) return 7.2e-5;
+  const double t = 1.02 * crit + std::ldexp(1.0, -22) / std::sin(crit);
+  const double sh = std::sin(0.5 * t);
+  return std::max(7.2e-5, 2.0 * sh * sh);  // 1 - cos(t) without cancellation
+}
+
+// roughness_critical of the YAML, where the roughness certification (rough_k = 0.06) was calibrated
+constexpr double ROUGH_CRIT_YAML = 0.05;
+
+// 1/step_crit as the kernel multiplies it (step layer = sat(1 - st * m)): for a step_critical_cells that is not a power of two,
+// rounded up from float32(1/crit) until every st that may stand for a reference step >= crit gives st * m >= 1, i.e. exactly the
+// reference's 0 branch (StepFilter.cpp:172-176): CNT * (1/ncrit) * stepMax carries up to three float32 roundings, so st may lie
+// 4 ulps below crit.  A reference step below crit whose st passes that bound has a layer below 2.4e-7, inside the tolerance of
+// 0.  With a power of two only the last product rounds; m stays float32(1/crit), so that the YAML outputs (0.12, 4 cells) keep
+// every bit.  There the 0 branch is exact where st >= the smallest float >= crit, but CNT * stepMax / ncrit with CNT not a multiple
+// of ncrit (3/4 stepMax at the YAML's 4 cells) can round to float32(crit) < crit where the reference's double step is >= crit: a
+// layer of ~1e-7 instead of 0, at the YAML values too (a 1e-9 m wide window of stepMax at 0.12 m).  Open: deciding the branch
+// exactly (the residual of the exact CNT * (1/ncrit) times stepMax) costs march-step instructions at the 168-register limit.
+float step_layer_scale(double crit, int ncrit) {
+  float m = (float)(1.0 / crit);
+  if (ncrit > 0 && (ncrit & (ncrit - 1)) == 0) return m;
+  float lo = (float)(crit * (1.0 - std::ldexp(4.0, -24)));
+  if ((double)lo > crit * (1.0 - std::ldexp(4.0, -24))) lo = std::nextafterf(lo, 0.0f);
+  while ((double)lo * (double)m < 1.0) m = std::nextafterf(m, INFINITY);  // the product of two floats is exact in double
+  return m;
+}
+
 using ShapeA = Shape<2, 2, 1, 1, 1, -1, true, 1, 1, -1, true>;    // YAML radii at 0.02 m
 using ShapeB = Shape<1, 1, -1, 1, 0, -1, false, 1, 0, -1, false>; // YAML radii at 0.03 m (fixture)
 
@@ -1095,7 +1135,11 @@ void make_fixup_args(const FusedState& st, const SlabView& v, const ChainDev& p,
   // could put its double result on the other side.  The reference forms the window offsets from absolute coordinates
   // (X[a] - mean): relative error eps_off <= 4 * 2^-53 * |X|max / res; the small-angle term s = 1 - n_z <= 2e-4 inherits ~4 eps_off,
   // i.e. 2e-4 * 16 * 2^-53 * (|X|max / res) / 2^-24 = 6e-12 * |X|max / res float32 ulps (6e-9 for the 8192^2 map at 0.02 m, with
-  // tier 2's own error on centred coordinates an order below).  The band is 100 times that, at least 1e-6 ulp.
+  // tier 2's own error on centred coordinates an order below).  The band is 100 times that, at least 1e-6 ulp.  It applies to
+  // n_z > 0.9998, or down to the band tier 1 certifies when that is wider (small slope_critical, nz_check_limit); past s = 2e-4
+  // tier 2 scales it by the cell's own s / 2e-4, as the error grows in proportion to s.
+  const double s_check = nz_check_limit(p.slope_crit);
+  a.nz_check = s_check > 2e-4 ? 1.0 - s_check : 0.9998;
   a.nz_guard = std::max(1e-6, 100.0 * 6e-12 * v.coord_max / v.res);
   a.fuse_w = p.fuse_w;
   a.rowmask = (const unsigned char*)st.rowmask.p;
@@ -1150,12 +1194,19 @@ int launch_chain_fused(FusedState& st, const SlabView& v, const ChainDev& p, int
   if (const char* e = std::getenv("TE_FUSED_COND_K")) cond_k = std::atof(e);
 #endif
   a.cond_k = (float)cond_k;
-  a.rough_thr = (float)((rough_k / p.rough_crit) * (rough_k / p.rough_crit) * (N - 1.0) / N);
+  // Below the YAML's roughness_critical (0.05 m) rough_k is 1.5.  A cell at r ~ crit has a layer tolerance of 1e-6 absolute, and the
+  // fp32 error of lambda0 moves the layer by about that error over 2 crit^2: in windows of nearly isotropic noise (cmag ~ lambda0)
+  // fp32 lambda0 is off by up to ~2.5e-6 relative, and with 0.06 such cells at 0.02 ... 0.005 m on rough terrain left the
+  // tolerance (1-5 per 1024^2 map; the flag lambda0 < rough_thr cmag^2 needs rough_k > crit r / cmag ~ 1.03 for the worst of
+  // them).  With 1.5 every cell from r = 0.82 crit up is flagged (cmag >= lambda0), and below it the tolerance is 2.8e-6 or more.
+  // At 0.05 m and above rough_k is the calibrated 0.06, so the YAML outputs keep every bit.
+  if (p.rough_crit < ROUGH_CRIT_YAML) rough_k = std::max(rough_k, 1.5);
+  a.rough_thr =(float)((rough_k / p.rough_crit) * (rough_k / p.rough_crit) * (N - 1.0) / N);
   a.kp = (float)(-res / N);
   a.invN = (float)(1.0 / N);
   a.n_over_nm1 = (float)(N / (N - 1.0));
   a.slope_crit = (float)p.slope_crit; a.inv_slope_crit = (float)(1.0 / p.slope_crit); a.minv_slope_crit = (float)(-1.0 / p.slope_crit);
-  a.minv_step_crit = -(float)(1.0 / p.step_crit); a.minv_rough_crit = (float)(-1.0 / p.rough_crit);
+  a.minv_step_crit = -step_layer_scale(p.step_crit, p.ncrit); a.minv_rough_crit = (float)(-1.0 / p.rough_crit);
   a.step_crit = (float)p.step_crit; a.inv_step_crit = (float)(1.0 / p.step_crit);
   a.step_cmp = (float)p.step_crit;
   if ((double)a.step_cmp > p.step_crit) a.step_cmp = std::nextafterf(a.step_cmp, -INFINITY);
@@ -1175,6 +1226,7 @@ int launch_chain_fused(FusedState& st, const SlabView& v, const ChainDev& p, int
   // stays 0 here so that the outputs stay bit-identical; restoring the 1e-3 floor is an open certification question (it would
   // send more cells near a rounding boundary to the fp64 fix-up and can change their float32 rounding).
   a.k_bmargin = B2(0.0);
+  a.k_nz_check = B2(nz_check_limit(p.slope_crit));
   a.k_one = B2(1.0); a.k_two = B2(2.0); a.k_half = B2(0.5);
   a.k_p0 = B2(1.570796251296997); a.k_p1 = B2(-0.21459604799747467); a.k_p2 = B2(0.08894557505846024);
   a.k_p3 = B2(-0.05000271648168564); a.k_p4 = B2(0.03044925443828106); a.k_p5 = B2(-0.016484638676047325);

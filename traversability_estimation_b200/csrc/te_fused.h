@@ -42,6 +42,7 @@ struct FixupArgs {
   double res, slope_crit, step_crit, rough_crit;
   double inv_slope_crit, inv_rough_crit;
   double nz_guard;          // half-width, in float32 ulps, of the band around a rounding boundary of n_z that tier 2 leaves to tier 3
+  double nz_check;          // the guard applies to n_z above this (where one ulp of n_z matters to the slope layer)
   float fuse_w;
   const unsigned char* rowmask;
   const unsigned char* colmask;
