@@ -547,6 +547,61 @@ int te_map_set_layers_maps(te_map* map, const te_geometry* g, int32_t nsel, cons
                            const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
                            const float* robot_slope_or_null, int memory);
 
+/* ---- Elevation images: the reference node's image topic (TraversabilityEstimation::imageCallback) ------------------------------
+ * The node turns a grayscale height image into the elevation layer (GridMapRosConverter::initializeFromImage on the first image,
+ * then addLayerFromImage(image, "elevation", map, min_height, max_height)) and runs computeTraversability on it.  The entries
+ * below do the same: the per-pixel arithmetic runs on the GPU, on the image's own 1 or 2 bytes per cell, and the rest is
+ * te_map_chain(_batched/_maps).  The node keeps the sensor_msgs header, encoding string and byte order: it passes an encoding
+ * code and, for an is_bigendian mono16 image, swaps the bytes itself (pixels are read in host byte order).
+ *
+ * Encodings.  Mono only: TE_IMAGE_MONO8 (mono8, 8UC1) and TE_IMAGE_MONO16 (mono16, 16UC1), elevation(i, j) = lower + (upper -
+ * lower) * ((float)pixel(i, j) / maxv) with lower = (float)min_height, upper = (float)max_height and maxv = 255 or 65535, every
+ * operation float32 and IEEE-rounded, as GridMapCvConverter::addLayerFromImage does it.  So pixel 0 gives lower, and the top
+ * pixel gives lower + (upper - lower) * 1.0f, which need not equal upper.  min_height and max_height are not checked: a reversed,
+ * equal or overflowing pair gives the bits the reference's formula gives.  The colour encodings are TE_ERR_UNSUPPORTED: the
+ * reference first greys them with OpenCV's cvtColor, whose fixed-point coefficients depend on the OpenCV version and build, so no
+ * result here could be pinned to the reference's. */
+enum {
+  TE_IMAGE_MONO8 = 0,
+  TE_IMAGE_MONO16 = 1,
+  /* TE_ERR_UNSUPPORTED (see above) */
+  TE_IMAGE_RGB8 = 2, TE_IMAGE_BGR8 = 3, TE_IMAGE_RGBA8 = 4, TE_IMAGE_BGRA8 = 5,
+  TE_IMAGE_RGB16 = 6, TE_IMAGE_BGR16 = 7, TE_IMAGE_RGBA16 = 8, TE_IMAGE_BGRA16 = 9
+};
+
+/* initializeFromImage(image, resolution, map, position): GridMap::setGeometry(Length(resolution * height, resolution * width),
+ * resolution, position), i.e. rows = (int)round(resolution * height / resolution), cols likewise with width, length = size *
+ * resolution, the position as given and start index 0.  Host arithmetic, no GPU needed.  TE_ERR_BAD_ARG (out untouched) for a
+ * null out, height or width < 1, a resolution that is not finite and > 0, and a position that is not finite. */
+int te_image_geometry(int32_t height, int32_t width, double resolution, double position_x, double position_y, te_geometry* out);
+
+/* imageCallback's addLayerFromImage followed by computeTraversability, for nmaps images (nmaps = 1: a single map): te_map_chain
+ * (nmaps = 1) or te_map_chain_batched on the elevation the images give, with the same outputs, limits, cache and memo reset and
+ * no robot_slope afterwards; te_map_get_layers(TE_LAYER_ELEVATION) returns that elevation.
+ *   - Images are row-major, as sensor_msgs/Image: g->rows x g->cols pixels, image row i being map row i (so the layer, column-major,
+ *     is the image transposed); row i of image m starts at images + m * image_stride_bytes + i * row_stride_bytes.
+ *     image_stride_bytes is ignored for nmaps = 1.  The images are in `memory`.
+ *   - TE_ERR_UNSUPPORTED for a start index in g (an image map has none) and a colour encoding; TE_ERR_BAD_ARG for an unknown
+ *     encoding, row_stride_bytes < cols * bytes per pixel, image_stride_bytes < rows * row_stride_bytes (nmaps > 1) and, for
+ *     mono16, an odd images address or stride (checked in both memory modes); TE_ERR_MISSING_LAYER for null images.  Every
+ *     argument error is found before anything is written: the te_map is then unchanged.
+ *   - Host memory stages the image bytes only (1 or 2 per cell, not 4) and returns synchronised; device memory reads the images
+ *     in place and is asynchronous on the context stream.  Scratch the te_map keeps, grown to the largest call and released by
+ *     te_map_destroy: 1 or 2 bytes per cell of the nmaps maps in host memory (the staged images), none in device memory.
+ *   - Launches: those of te_map_chain(_batched) plus one conversion kernel, whatever nmaps. */
+int te_map_chain_image(te_map* map, const te_geometry* g, const te_chain_params* p, int32_t nmaps, int32_t encoding,
+                       const void* images, int64_t row_stride_bytes, int64_t image_stride_bytes, double min_height, double max_height,
+                       float* slope_or_null, float* step_or_null, float* roughness_or_null, float* traversability_or_null, int memory);
+
+/* The same for the maps map_index[0..nsel) of a batch only: te_map_chain_maps on the elevation the nsel images give (image k goes
+ * to map map_index[k]), under the rules of the _maps entries above and the image rules of te_map_chain_image.  Scratch: that of
+ * te_map_chain_maps in host memory (20 bytes per selected cell) plus the staged images (1 or 2), and 20 in device memory (the
+ * converted elevation is packed before it is put in place).  Launches: those of te_map_chain_maps plus one. */
+int te_map_chain_image_maps(te_map* map, const te_geometry* g, const te_chain_params* p, int32_t nsel, const int32_t* map_index,
+                            int32_t encoding, const void* images, int64_t row_stride_bytes, int64_t image_stride_bytes,
+                            double min_height, double max_height, float* slope_or_null, float* step_or_null,
+                            float* roughness_or_null, float* traversability_or_null, int memory);
+
 /* traversabilityFootprint(radius, offset) (:307-318) on the cache: a cached cell keeps its value (the memoised branch, :673-675),
  * every other cell gets te_footprint2's value for `p`; traversability_footprint_or_null receives the cache afterwards.  The
  * prefix-sum sweep may differ from the visit-by-visit one in the last float32 bit of a few cells (DESIGN.md §4.3); those values

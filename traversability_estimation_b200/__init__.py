@@ -6,5 +6,5 @@ tests, `bench.py` and multi-process launch via torch.distributed — it adds no 
 and there is no CPU fallback: loading fails loudly when the library is missing.
 """
 from .capi import (ChainParams, Context, FootprintParams, Geometry, HaloPeer, Map, Slab, TEError,  # noqa: F401
-                   KERNEL_AUTO, KERNEL_FUSED, KERNEL_GENERIC, MEM_DEVICE, MEM_HOST, build_library,
-                   library_path, load_library)
+                   IMAGE_MONO8, IMAGE_MONO16, KERNEL_AUTO, KERNEL_FUSED, KERNEL_GENERIC, MEM_DEVICE, MEM_HOST,
+                   build_library, image_geometry, library_path, load_library)

@@ -158,6 +158,9 @@ SIGNATURES = {
     "te_map_set_layers_batched": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _I]),
     "te_map_chain_maps": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _P, _I]),
     "te_map_set_layers_maps": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_image_geometry": (_R, [_I, _I, _D, _D, _D, _G]),
+    "te_map_chain_image": (_R, [_P, _G, _CP, _I, _I, _P, _L, _L, _D, _D, _P, _P, _P, _P, _I]),
+    "te_map_chain_image_maps": (_R, [_P, _G, _CP, _I, _P, _I, _P, _L, _L, _D, _D, _P, _P, _P, _P, _I]),
     "te_map_footprint": (_R, [_P, _FP, _P, _I]),
     "te_map_footprint_maps": (_R, [_P, _FP, _I, _P, _P, _I]),
     "te_map_footprint_polygon": (_R, [_P, _FP, _I, _P, _D, _P, _P, _I]),
@@ -240,6 +243,36 @@ def submap_geometry(g, positions, lengths):
     if rc != 0:
         raise TEError(rc, L.te_last_error().decode())
     return info
+
+
+IMAGE_MONO8, IMAGE_MONO16 = 0, 1  # te_image encodings
+
+
+def image_geometry(height, width, resolution, position=(0.0, 0.0)) -> Geometry:
+    """te_image_geometry: the geometry initializeFromImage gives a height x width image (GridMap::setGeometry); host arithmetic,
+    no GPU needed."""
+    L = load_library()
+    g = Geometry()
+    rc = L.te_image_geometry(int(height), int(width), float(resolution), float(position[0]), float(position[1]), C.byref(g))
+    if rc != 0:
+        raise TEError(rc, L.te_last_error().decode())
+    return g
+
+
+def _images(images):
+    """(array, nmaps, encoding, row_stride_bytes, image_stride_bytes) of uint8 / uint16 images shaped (rows, cols) or (n, rows,
+    cols), row-major as an image is.  A view whose pixels are contiguous along each row (sliced, padded) is passed as it is; any
+    other layout and a non-native byte order are copied."""
+    a = np.asarray(images)
+    if a.dtype.kind != "u" or a.dtype.itemsize not in (1, 2) or a.ndim not in (2, 3):
+        raise ValueError(f"images: need uint8 or uint16 of shape (rows, cols) or (n, rows, cols), got {a.dtype} {a.shape}")
+    if not a.dtype.isnative:
+        a = a.astype(a.dtype.newbyteorder("="))
+    if (a.strides[-1] != a.itemsize or a.strides[-2] < a.shape[-1] * a.itemsize
+            or (a.ndim == 3 and a.strides[0] < a.shape[1] * a.strides[1])):  # also broadcast and reversed views
+        a = np.ascontiguousarray(a)
+    n = 1 if a.ndim == 2 else a.shape[0]
+    return a, n, IMAGE_MONO8 if a.itemsize == 1 else IMAGE_MONO16, a.strides[-2], a.strides[0] if a.ndim == 3 else 0
 
 
 def _addr(a):
@@ -791,6 +824,31 @@ class Map:
         self._check(self._L.te_map_chain_maps(self._h, C.byref(g), C.byref(p), len(idx), _addr(idx), _addr(e),
                                               *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")),
                                               MEM_HOST))
+        return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
+
+    _CHAIN_OUTPUTS = ("slope", "step", "roughness", "traversability")
+
+    def chain_image(self, g, p, images, min_height, max_height, outputs=False):
+        """te_map_chain_image (imageCallback: addLayerFromImage, then computeTraversability): images uint8 (mono8) or uint16 (mono16)
+        of shape (rows, cols), or (n, rows, cols) for a batch of n maps.  outputs=True also returns the four layers as a dict, shaped
+        as the images."""
+        a, n, enc, rs, ims = _images(images)
+        out = {k: np.empty((n, g.cols, g.rows), dtype=np.float32) for k in self._CHAIN_OUTPUTS} if outputs else {}
+        self._check(self._L.te_map_chain_image(self._h, C.byref(g), C.byref(p), n, enc, _addr(a), rs, ims, float(min_height),
+                                               float(max_height), *(_addr(out.get(k)) for k in self._CHAIN_OUTPUTS), MEM_HOST))
+        self._g, self._n = g, n
+        return {k: (v.transpose(0, 2, 1) if a.ndim == 3 else v[0].T) for k, v in out.items()} if outputs else None
+
+    def chain_image_maps(self, g, p, map_index, images, min_height, max_height, outputs=False):
+        """te_map_chain_image_maps (chain_image for the maps map_index of the batch only): images (nsel, rows, cols), image j
+        going to map map_index[j]; keeps every other map as it was.  outputs=True also returns the four layers as a dict of
+        (nsel, rows, cols) arrays in map_index order."""
+        idx = self._map_index(map_index)
+        a, _, enc, rs, ims = _images(images)
+        out = {k: np.empty((len(idx), g.cols, g.rows), dtype=np.float32) for k in self._CHAIN_OUTPUTS} if outputs else {}
+        self._check(self._L.te_map_chain_image_maps(self._h, C.byref(g), C.byref(p), len(idx), _addr(idx), enc, _addr(a), rs, ims,
+                                                    float(min_height), float(max_height),
+                                                    *(_addr(out.get(k)) for k in self._CHAIN_OUTPUTS), MEM_HOST))
         return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
 
     def set_layers_maps(self, g, map_index, traversability, slope, step, elevation, roughness=None, robot_slope=None):

@@ -271,11 +271,19 @@ cudaError_t for_wrapped_pieces(int rows, int cols, int sr, int sc, int c0, int n
   return cudaSuccess;
 }
 
-cudaError_t upload_cols(float* dev, const float* host, int rows, int cols, int sr, int sc, int c0, int n, cudaStream_t s) {
-  const size_t pitch = sizeof(float) * (size_t)rows;
-  if (sr == 0 && sc == 0) return cudaMemcpyAsync(dev + (size_t)c0 * rows, host + (size_t)c0 * rows, pitch * n, cudaMemcpyHostToDevice, s);
+// Cells are `elem` bytes (float32 layers: 4; image bytes, whose "columns" are image rows: 1 or 2).  The host columns lie
+// `host_pitch` bytes apart (0: packed, elem * rows; a padded pitch needs start index 0); the device columns are packed.
+cudaError_t upload_cols(void* dev, const void* host, int rows, int cols, int sr, int sc, int c0, int n, cudaStream_t s,
+                        size_t elem = sizeof(float), size_t host_pitch = 0) {
+  const size_t pitch = elem * (size_t)rows;
+  char* d0 = (char*)dev;
+  const char* h0 = (const char*)host;
+  if (sr == 0 && sc == 0) {
+    if (!host_pitch || host_pitch == pitch) return cudaMemcpyAsync(d0 + c0 * pitch, h0 + c0 * pitch, pitch * n, cudaMemcpyHostToDevice, s);
+    return cudaMemcpy2DAsync(d0 + c0 * pitch, pitch, h0 + c0 * host_pitch, host_pitch, pitch, n, cudaMemcpyHostToDevice, s);
+  }
   return for_wrapped_pieces(rows, cols, sr, sc, c0, n, [&](size_t d, size_t h, int r, int m) {
-    return cudaMemcpy2DAsync(dev + d, pitch, host + h, pitch, sizeof(float) * r, m, cudaMemcpyHostToDevice, s);
+    return cudaMemcpy2DAsync(d0 + elem * d, pitch, h0 + elem * h, pitch, elem * r, m, cudaMemcpyHostToDevice, s);
   });
 }
 
@@ -1307,6 +1315,7 @@ struct te_map {
   DevBuf gather;  // te_map_get_submaps: the source-layer table, then the windows (te::SubmapWindow)
   // The _maps entries: the selected maps' layers packed back to back (grown to the largest selection) and their slot table
   DevBuf sel[te::kMapSlotLayers], slots;
+  DevBuf image;  // te_map_chain_image(_maps) in host memory: the staged image bytes, packed
   bool have_rough = false, have_rslope = false;
   te::FootprintState fp;  // the map's own scratch; fp.memo is the resident memo
   bool memo_valid = false;
@@ -1512,7 +1521,8 @@ int te_map_destroy(te_map* m) {
     Guard g(m->ctx);
     if (g.ok) {
       cudaStreamSynchronize(m->ctx->stream);
-      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather, &m->slots}) b->release();
+      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather, &m->slots, &m->image})
+        b->release();
       for (DevBuf& b : m->sel) b.release();
       m->fp.release();
     }
@@ -1523,12 +1533,73 @@ int te_map_destroy(te_map* m) {
 
 namespace {
 
-// te_map_chain (nmaps = 1), te_map_chain_batched and, with a selection, te_map_chain_maps: the selected maps' layers are chained
-// into scratch (the elevation staged there in host memory, read in place in device memory) and k_map_slots puts them in place.
-int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int nmaps, const float* elev, float* slope, float* step,
+// te_map_chain_image(_maps)'s images, as the caller passed them.
+struct ImageIn {
+  int32_t encoding;
+  const void* px;
+  int64_t row_stride, image_stride;
+  double min_height, max_height;
+};
+
+// Where map_chain's elevation comes from: a float32 layer, or images that k_image_to_layer turns into one.
+struct ElevSource {
+  const float* layer;
+  const ImageIn* image;
+};
+
+// Validates nmaps images of geometry g and returns their bytes per pixel.  Writes nothing.
+int check_image(const ImageIn& im, const te_geometry& g, int nmaps, int* bpp) {
+  if (im.encoding >= TE_IMAGE_RGB8 && im.encoding <= TE_IMAGE_BGRA16)
+    return fail(TE_ERR_UNSUPPORTED, "colour image encoding %d: only mono8 and mono16 images are taken (the reference greys colour "
+                "images with OpenCV's cvtColor, whose coefficients depend on the OpenCV version and build)", im.encoding);
+  if (im.encoding != TE_IMAGE_MONO8 && im.encoding != TE_IMAGE_MONO16) return fail(TE_ERR_BAD_ARG, "unknown image encoding %d", im.encoding);
+  if (!im.px) return fail(TE_ERR_MISSING_LAYER, "the images that give layer elevation are missing");
+  const int b = im.encoding == TE_IMAGE_MONO16 ? 2 : 1;
+  if (im.row_stride < (int64_t)g.cols * b)
+    return fail(TE_ERR_BAD_ARG, "row_stride_bytes = %lld is less than a row of %d pixels of %d bytes", (long long)im.row_stride, g.cols, b);
+  if (nmaps > 1 && (im.row_stride > INT64_MAX / g.rows || im.image_stride < im.row_stride * g.rows))
+    return fail(TE_ERR_BAD_ARG, "image_stride_bytes = %lld is less than %d rows of %lld bytes", (long long)im.image_stride, g.rows,
+                (long long)im.row_stride);
+  if (b == 2 && (((uintptr_t)im.px | (uint64_t)im.row_stride | (uint64_t)(nmaps > 1 ? im.image_stride : 0)) & 1))
+    return fail(TE_ERR_BAD_ARG, "mono16 images need an even address, row_stride_bytes and image_stride_bytes");
+  *bpp = b;
+  return TE_OK;
+}
+
+// addLayerFromImage: nmaps images of geometry g into the float32 elevation `out` (nmaps maps back to back), one launch.  In host
+// memory only the image bytes are staged, packed in m->image; device images are read in place.
+int map_convert_image(te_map* m, const te_geometry& g, const ImageIn& im, int bpp, int nmaps, int memory, float* out) {
+  te_ctx* c = m->ctx;
+  te::ImageToLayer a{im.px, im.row_stride, im.image_stride, g.rows, g.cols, nmaps, bpp, (float)im.min_height, 0.0f, out};
+  a.diff = (float)im.max_height - a.lower;  // float32 operands and result: mapValueDifference
+  if (memory == TE_MEM_HOST) {  // the image rows are the columns of the staged bytes
+    const size_t row = (size_t)bpp * g.cols, image = row * g.rows;
+    TE_CUDA(m->image.reserve(image * nmaps));
+    char* dst = (char*)m->image.p;
+    if (nmaps == 1 || (im.image_stride == im.row_stride * g.rows && (int64_t)g.rows * nmaps <= INT32_MAX)) {
+      TE_CUDA(upload_cols(dst, im.px, g.cols, g.rows * nmaps, 0, 0, 0, g.rows * nmaps, c->stream, bpp, im.row_stride));
+    } else {
+      for (int k = 0; k < nmaps; ++k)
+        TE_CUDA(upload_cols(dst + k * image, (const char*)im.px + k * im.image_stride, g.cols, g.rows, 0, 0, 0, g.rows, c->stream, bpp,
+                            im.row_stride));
+    }
+    a.px = dst;
+    a.row_stride = (long long)row;
+    a.image_stride = (long long)image;
+  }
+  te::launch_image_to_layer(a, c->stream);
+  return launch_check(c, "k_image_to_layer");
+}
+
+// te_map_chain (nmaps = 1), te_map_chain_batched and, with a selection, te_map_chain_maps, from an elevation layer or from images
+// (te_map_chain_image(_maps)): the selected maps' layers are chained into scratch (the elevation staged there in host memory,
+// read in place in device memory; images converted there in both) and k_map_slots puts them in place.
+int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int nmaps, const ElevSource& src, float* slope, float* step,
               float* rough, float* trav, int memory, const MapSel* sel = nullptr) {
   te_ctx* c = m->ctx;
   te_geometry g0;
+  if (src.image && g_in && (g_in->start_row != 0 || g_in->start_col != 0))
+    return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0): an image map has none", g_in->start_row, g_in->start_col);
   if (sel) {
     if (int rc = map_select(m, true, g_in, *sel)) return rc;
     g0 = m->geo;
@@ -1537,35 +1608,44 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
     return rc;
   }
   if (int rc = check_params(p)) return rc;
-  if (!elev) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
+  if (!src.layer && !src.image) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
   if (sel && (m->have_rslope || !m->have_rough))
     return fail(TE_ERR_UNSUPPORTED, "the batch %s, and te_map_chain_maps gives a map roughness and no robot_slope: every map of a batch holds "
                 "the same layers, so use te_map_set_layers_maps or reload the whole batch",
                 m->have_rslope ? "holds robot_slope" : "has no roughness");
+  int bpp = 0;
+  if (src.image)
+    if (int rc = check_image(*src.image, g0, nmaps, &bpp)) return rc;
   DevBuf* const lay[5] = {sel ? &m->sel[0] : &m->elev, sel ? &m->sel[1] : &m->slope, sel ? &m->sel[2] : &m->step,
                           sel ? &m->sel[3] : &m->rough, sel ? &m->sel[4] : &m->trav};  // where the chain reads and writes
   const size_t cells = map_cells(m) * (sel ? sel->n : 0);
-  const float* din = elev;
+  const float* din = src.layer;
   if (sel) {
-    if (int rc = map_stage_selection(m, *sel, memory == TE_MEM_HOST ? 0x1fu : 0x1eu)) return rc;  // sel[0]: the staged elevation
-    if (memory == TE_MEM_HOST) {
-      TE_CUDA(map_copy_packed(m, (float*)lay[0]->p, elev, cells, false, memory));
+    const bool packed = memory == TE_MEM_HOST || src.image;  // sel[0]: the staged or converted elevation
+    if (int rc = map_stage_selection(m, *sel, packed ? 0x1fu : 0x1eu)) return rc;
+    if (memory == TE_MEM_HOST && src.layer) {
+      TE_CUDA(map_copy_packed(m, (float*)lay[0]->p, src.layer, cells, false, memory));
       din = (const float*)lay[0]->p;
     }
   } else {
     if (int rc = map_reset(m, g_in, &g0, nmaps)) return rc;
     TE_CUDA(m->rough.reserve(sizeof(float) * batch_cells(m)));
-    if (int rc = map_put_layer(m, m->elev, elev, memory)) return rc;
+    if (src.layer)
+      if (int rc = map_put_layer(m, m->elev, src.layer, memory)) return rc;
     din = (const float*)m->elev.p;
+  }
+  if (src.image) {
+    if (int rc = map_convert_image(m, g0, *src.image, bpp, nmaps, memory, (float*)lay[0]->p)) return rc;
+    din = (const float*)lay[0]->p;
   }
   if (int rc = chain_common(c, &g0, nullptr, p, nmaps, din, (float*)lay[1]->p, (float*)lay[2]->p, (float*)lay[3]->p, (float*)lay[4]->p,
                             nullptr, nullptr, nullptr, TE_MEM_DEVICE))
     return rc;
   if (sel) {
-    const float* const src[te::kMapSlotLayers] = {(const float*)lay[4]->p, (const float*)lay[1]->p, (const float*)lay[2]->p,
-                                                  (const float*)lay[3]->p, din, nullptr};
+    const float* const src_l[te::kMapSlotLayers] = {(const float*)lay[4]->p, (const float*)lay[1]->p, (const float*)lay[2]->p,
+                                                    (const float*)lay[3]->p, din, nullptr};
     DevBuf* const dst[te::kMapSlotLayers] = {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, nullptr};
-    if (int rc = map_put_selected(m, *sel, src, dst)) return rc;
+    if (int rc = map_put_selected(m, *sel, src_l, dst)) return rc;
   } else {
     m->have_rough = true;
     m->have_rslope = false;  // computeTraversability leaves robot_slope to a later setTraversabilityMap
@@ -1644,13 +1724,13 @@ int map_set_layers(te_map* m, const te_geometry* g_in, int nmaps, const float* t
 int te_map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, const float* elev, float* slope, float* step, float* rough,
                  float* trav, int memory) {
   TE_MAP_ENTER(m);
-  return map_chain(m, g_in, p, 1, elev, slope, step, rough, trav, memory);
+  return map_chain(m, g_in, p, 1, ElevSource{elev, nullptr}, slope, step, rough, trav, memory);
 }
 
 int te_map_chain_batched(te_map* m, const te_geometry* g, const te_chain_params* p, int32_t nmaps, const float* elev, float* slope,
                          float* step, float* rough, float* trav, int memory) {
   TE_MAP_ENTER(m);
-  return map_chain(m, g, p, nmaps, elev, slope, step, rough, trav, memory);
+  return map_chain(m, g, p, nmaps, ElevSource{elev, nullptr}, slope, step, rough, trav, memory);
 }
 
 int te_map_set_layers(te_map* m, const te_geometry* g_in, const float* trav, const float* slope, const float* step, const float* rough,
@@ -1669,7 +1749,44 @@ int te_map_chain_maps(te_map* m, const te_geometry* g, const te_chain_params* p,
                       float* slope, float* step, float* rough, float* trav, int memory) {
   TE_MAP_ENTER(m);
   const MapSel sel{nsel, map_index};
-  return map_chain(m, g, p, nsel, elev, slope, step, rough, trav, memory, &sel);
+  return map_chain(m, g, p, nsel, ElevSource{elev, nullptr}, slope, step, rough, trav, memory, &sel);
+}
+
+int te_image_geometry(int32_t height, int32_t width, double resolution, double position_x, double position_y, te_geometry* out) {
+  if (!out) return fail(TE_ERR_BAD_ARG, "out is null");
+  if (height < 1 || width < 1) return fail(TE_ERR_BAD_ARG, "image size %d x %d: need at least 1 x 1", height, width);
+  if (!(resolution > 0.0) || !std::isfinite(resolution)) return fail(TE_ERR_BAD_ARG, "resolution must be finite and positive");
+  if (!std::isfinite(position_x) || !std::isfinite(position_y)) return fail(TE_ERR_BAD_ARG, "position must be finite");
+  // initializeFromImage: setGeometry(Length(resolution * height, resolution * width), resolution, position)
+  const double length_x = resolution * height, length_y = resolution * width;
+  if (!std::isfinite(length_x) || !std::isfinite(length_y)) return fail(TE_ERR_BAD_ARG, "resolution * image size is not finite");
+  te_geometry g{};
+  g.rows = (int)std::round(length_x / resolution);  // setGeometry: size = round(length / resolution), length = size * resolution
+  g.cols = (int)std::round(length_y / resolution);
+  g.resolution = resolution;
+  g.length_x = g.rows * resolution;
+  g.length_y = g.cols * resolution;
+  g.position_x = position_x;
+  g.position_y = position_y;
+  *out = g;
+  return TE_OK;
+}
+
+int te_map_chain_image(te_map* m, const te_geometry* g, const te_chain_params* p, int32_t nmaps, int32_t encoding, const void* images,
+                       int64_t row_stride_bytes, int64_t image_stride_bytes, double min_height, double max_height, float* slope,
+                       float* step, float* rough, float* trav, int memory) {
+  TE_MAP_ENTER(m);
+  const ImageIn im{encoding, images, row_stride_bytes, image_stride_bytes, min_height, max_height};
+  return map_chain(m, g, p, nmaps, ElevSource{nullptr, &im}, slope, step, rough, trav, memory);
+}
+
+int te_map_chain_image_maps(te_map* m, const te_geometry* g, const te_chain_params* p, int32_t nsel, const int32_t* map_index,
+                            int32_t encoding, const void* images, int64_t row_stride_bytes, int64_t image_stride_bytes, double min_height,
+                            double max_height, float* slope, float* step, float* rough, float* trav, int memory) {
+  TE_MAP_ENTER(m);
+  const MapSel sel{nsel, map_index};
+  const ImageIn im{encoding, images, row_stride_bytes, image_stride_bytes, min_height, max_height};
+  return map_chain(m, g, p, nsel, ElevSource{nullptr, &im}, slope, step, rough, trav, memory, &sel);
 }
 
 int te_map_set_layers_maps(te_map* m, const te_geometry* g, int32_t nsel, const int32_t* map_index, const float* trav, const float* slope,

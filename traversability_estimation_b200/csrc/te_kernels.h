@@ -69,4 +69,18 @@ struct GridGeo;
 void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, const int* pos_map, int nmaps, unsigned char* valid,
                      cudaStream_t s);
 
+// te_image.cu — addLayerFromImage for mono images: nmaps row-major images of rows x cols pixels (image m at px + m * image_stride
+// bytes, its row i at + i * row_stride bytes; device memory, 2-byte pixels at even addresses and strides) into nmaps column-major
+// float32 layers back to back at out: out[m*rows*cols + j*rows + i] = lower + diff * (pixel(m, i, j) / max pixel value).
+struct ImageToLayer {
+  const void* px;
+  long long row_stride, image_stride;
+  int rows, cols, nmaps;  // nmaps 1..65535
+  int bpp;                // 1: mono8, 2: mono16 (host byte order)
+  float lower, diff;      // lowerValue and mapValueDifference = upperValue - lowerValue
+  float* out;
+};
+// One k_image_to_layer launch for every map.
+void launch_image_to_layer(const ImageToLayer& a, cudaStream_t s);
+
 }  // namespace te
