@@ -23,7 +23,7 @@ def _bits(a):
 
 
 def _groups(tiles, nyaws, sms):
-    """The launcher's yaw-group rule (polygon_groups in te_footprint.cu): as many groups as bring the launch to 4 * sms blocks."""
+    """The launcher's yaw-group rule (polygon_groups in te_footprint_polygon.cu): as many groups as bring the launch to 4 * sms blocks."""
     return min(nyaws, max(1, -(-4 * sms // tiles)))
 
 

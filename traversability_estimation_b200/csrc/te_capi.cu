@@ -1980,10 +1980,7 @@ static int map_request(te_map* m, const te_footprint_params* p, const int32_t* p
     if (int r2 = launch_check(c, "map request (polygonal paths)", nl)) return r2;
   }
   if (circles) {  // the circular paths (TraversabilityMap.cpp:345-462) in request order on the cache
-    int rc = te::launch_map_request_device(m->fp, v, g, p, r.trav, r.slope, r.step, rough, r.elev, rslope, (float*)m->cache.p,
-                                           m->nmaps, r.path_map, npaths, nposes, r.path_begin, r.poses, r.radius, r.footprint_begin,
-                                           r.cup, r.is_safe, r.trav_out, r.area_out, max_vertices, r.ucount, r.uxy, max_checks, host,
-                                           c->sms, c->stream, &nl);
+    int rc = te::launch_map_request_device(m->fp, v, g, p, r, (float*)m->cache.p, max_checks, host, c->sms, c->stream, &nl);
     if (rc != 0) return fail(rc, "map request (circular paths) failed: %s", m->fp.why.c_str());
     if (int r2 = launch_check(c, "map request (circular paths)", nl)) return r2;
     m->last_device = true;

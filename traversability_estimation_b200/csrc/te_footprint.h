@@ -1,4 +1,5 @@
-// te_footprint.h — host interface of the footprint sweep (te_footprint.cu).
+// te_footprint.h — host interface of the footprint sweeps (te_footprint.cu, te_footprint_polygon.cu), the footprint path checks
+// (te_paths.cu) and the te_map footprint cache (te_map_request.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <string>
@@ -127,28 +128,25 @@ int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry*
 
 // A request on a te_map (te_map_check_footprint_request(_batched, _device)): its polygonal paths run launch_path_checks on the
 // memo the map keeps.  Its circular paths: launch_map_request_device reads and fills the traversability_footprint cache `cache`
-// (device, NaN = empty) in the reference's order; every path array and output is in DEVICE memory (a host request stages them),
-// and the call is asynchronous on `s`, without a host synchronisation.  A batch of `nmaps` maps: the layers, robot_slope, the
-// cache and the memo hold map m from m * rows * cols cells on, and path q is on map path_map[q] (path_map null: one map).  A
-// path the kernels cannot check (radius, rings, pose range, non-finite position unless `nonfinite_ok`, map outside the batch),
-// and every circular path from the first whose work-list entries end past `max_checks` on, gets is_safe 0, NaN traversability
-// and area and count -1 where its polygon was requested, and reads and stores nothing.  `nonfinite_ok` (host memory, where the
-// request was validated): a non-finite x or y is answered as the service loop answers it, a single pose there as outside the
-// map and a segment with such an end as a failed check without a polygon.  The workspace (st.devreq) is sized from npaths,
-// nposes, nmaps and max_checks; the request's counters stay on the device at st.req_counters.  Launches: 12 (nine kernels, three
-// CUB calls counted as one each), and one more with polygons, whatever the paths and maps.  Every call clears a hash table of
-// 2 * max_checks slots (rounded up to a power of two; 8 bytes per entry of max_checks).
+// (device, NaN = empty) in the reference's order.  It takes the layers, the map batch, the path arrays and the outputs from `r`,
+// every array in DEVICE memory (a host request stages them; poses of 7 doubles, footprint_begin set), and is asynchronous on `s`,
+// without a host synchronisation.  A batch of r.nmaps maps: the layers, robot_slope, the cache and the memo hold map m from
+// m * rows * cols cells on, and path q is on map r.path_map[q] (path_map null: one map).  A path the kernels cannot check
+// (radius, rings, pose range, non-finite position unless `nonfinite_ok`, map outside the batch), and every circular path from
+// the first whose work-list entries end past `max_checks` on, gets is_safe 0, NaN traversability and area and count -1 where its
+// polygon was requested, and reads and stores nothing.  `nonfinite_ok` (host memory, where the request was validated): a
+// non-finite x or y is answered as the service loop answers it, a single pose there as outside the map and a segment with such an
+// end as a failed check without a polygon.  The workspace (st.devreq) is sized from npaths, nposes, nmaps and max_checks; the
+// request's counters stay on the device at st.req_counters.  Launches: 12 (nine kernels, three CUB calls counted as one each),
+// and one more with polygons (r.ucount), whatever the paths and maps.  Every call clears a hash table of 2 * max_checks slots
+// (rounded up to a power of two; 8 bytes per entry of max_checks).
 struct MapRequestStats {
   long long candidates = 0;  // isTraversable calls the circular paths could make
   long long keys = 0;        // distinct circles among them (what k_map_eval_circles_dev evaluates)
   long long stored = 0;      // cache cells the request stored
 };
 int launch_map_request_device(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p,
-                              const float* trav, const float* slope, const float* step, const float* rough, const float* elev,
-                              const float* robot_slope, float* cache, int nmaps, const int* path_map, int npaths, int nposes,
-                              const int* path_begin, const double* poses, const double* radius, const int* footprint_begin,
-                              const unsigned char* cup, unsigned char* is_safe, double* trav_out, double* area_out, int max_vertices,
-                              int* ucount, double* uxy, long long max_checks, bool nonfinite_ok, int sms, cudaStream_t s,
+                              const PathChecks& r, float* cache, long long max_checks, bool nonfinite_ok, int sms, cudaStream_t s,
                               int* launches);
 // traversabilityFootprint(radius, offset) on a cache: cache = finite(cache) ? cache : fresh over nsel blocks of n cells; `out`
 // (device, may be null) receives the result too.  Block j of `fresh` and `out` starts at j * n, its cache block at slot[j] * n
