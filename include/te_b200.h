@@ -469,7 +469,8 @@ int te_check_footprint_request_batched(te_ctx* ctx, const te_geometry* g, const 
  *
  * A te_map belongs to one te_ctx: it runs on that context's stream under its lock and must be destroyed before the context.  It
  * owns, on the device, the layers traversability, traversability_slope, traversability_step, traversability_roughness (optional),
- * elevation and robot_slope (optional); the traversability_footprint cache (float32, NaN = empty); and the isTraversableForFilters
+ * elevation, robot_slope (optional) and the elevation map's carried layers (optional, te_map_carry_layers below); the
+ * traversability_footprint cache (float32, NaN = empty); and the isTraversableForFilters
  * memo, which is kept until the layers or one of max_gap_width, critical_step_height and verify_roughness change.  Whole maps only.
  * Host layers may carry a circular-buffer start index: they are unwrapped on upload and outputs are re-wrapped to the start index
  * of the last te_map_chain / te_map_set_layers.  Every entry but te_map_create / te_map_destroy fails with TE_ERR_BAD_ARG before
@@ -491,7 +492,8 @@ int te_map_create(te_ctx* ctx, te_map** out);
 int te_map_destroy(te_map* map);
 
 /* computeTraversability (:202-237): te_chain on `elevation` into the map's layers, each optionally copied out (NULL: kept on the
- * device only).  Empties the cache and the memo and leaves the map without robot_slope. */
+ * device only).  Empties the cache and the memo and leaves the map without robot_slope and carried layers (te_map_carry_layers
+ * adds them). */
 int te_map_chain(te_map* map, const te_geometry* g, const te_chain_params* p, const float* elevation, float* slope_or_null,
                  float* step_or_null, float* roughness_or_null, float* traversability_or_null, int memory);
 
@@ -721,8 +723,53 @@ typedef enum te_layer {
   TE_LAYER_ELEVATION = 1 << 4,
   TE_LAYER_ROBOT_SLOPE = 1 << 5,  /* te_map_set_layers with one */
   TE_LAYER_FOOTPRINT = 1 << 6,  /* traversability_footprint: the cache (NaN = empty) */
-  TE_LAYER_ALL = 0x7f
+  TE_LAYER_ALL = 0x7f,
+  /* 1 << 7 is unassigned.  The elevation map's own layers, which the reference's filter chain carries into the traversability
+   * map unchanged (mapOut = mapIn): te_map_carry_layers gives them.  The node asks the elevation mapping's submap service for
+   * elevation plus upper_bound / lower_bound, or with a raw map for the variances and time (TraversabilityEstimation.cpp:60-69,
+   * 264), and setElevationMap refuses a map without them (TraversabilityMap.cpp:145-150). */
+  TE_LAYER_UPPER_BOUND = 1 << 8,
+  TE_LAYER_LOWER_BOUND = 1 << 9,
+  TE_LAYER_VARIANCE = 1 << 10,
+  TE_LAYER_HORIZONTAL_VARIANCE_X = 1 << 11,
+  TE_LAYER_HORIZONTAL_VARIANCE_Y = 1 << 12,
+  TE_LAYER_HORIZONTAL_VARIANCE_XY = 1 << 13,
+  TE_LAYER_TIME = 1 << 14,
+  TE_LAYER_CARRIED = 0x7f00,  /* the seven bits above */
+  /* upper_bound - lower_bound, derived when read: publishTraversabilityMap adds it to the copy it publishes
+   * (TraversabilityMap.cpp:178-180).  te_map_get_layers only. */
+  TE_LAYER_UNCERTAINTY_RANGE = 1 << 15
 } te_layer;
+
+/* mapOut = mapIn for the layers the chain does not make: the carried layers of `layer_mask` (TE_LAYER_CARRIED bits) and
+ * robot_slope (TE_LAYER_ROBOT_SLOPE) into the te_map, next to the layers te_map_chain / te_map_set_layers gave it.  A node that
+ * initialises from a grid map with robot_slope (initializeTraversabilityMapFromGridMap, TraversabilityEstimation.cpp:331-362:
+ * the layer survives computeTraversability, and checkInclination reads it, TraversabilityMap.cpp:748-762) calls te_map_chain and
+ * then this, instead of copying the chain's outputs out and back through te_map_set_layers.  The image and init paths add
+ * missing bounds as 0.0 (TraversabilityEstimation.cpp:159-161, 340-345): a NULL layer pointer does that.
+ *   - layers: a HOST array of one pointer per set bit of layer_mask, in bit order; each is in `memory` or NULL (the layer is then
+ *     filled with 0.0f on the device, as GridMap::add(layer, 0.0)).
+ *   - nsel = 0 with map_index NULL: every map, each layer holding the nmaps maps back to back.  Host layers may carry the map's
+ *     circular-buffer start index (unwrapped on upload, as te_map_set_layers); device layers are in default order.  Otherwise the
+ *     maps map_index[0..nsel) only, under the rules of the _maps entries above (a host map_index of distinct entries, layers nsel
+ *     maps back to back in map_index order, no start index), and only layers the batch already holds: every map of a batch
+ *     holds the same layers, so a new layer is given to every map at once.
+ *   - Leaves the cache and the memo as they are: no carried layer feeds isTraversableForFilters, and robot_slope only gates the
+ *     later path checks (checkInclination).
+ *   - Lifetime, as the reference's map is replaced wholesale by each new one: te_map_chain(_batched), te_map_set_layers(_batched)
+ *     and te_map_chain_image drop every carried layer (as they drop robot_slope); te_map_chain_maps, te_map_set_layers_maps and
+ *     te_map_chain_image_maps keep the batch's carried layers and fill the selected maps' with NaN (robot_slope keeps the rules
+ *     of those entries).
+ *   - Errors: TE_ERR_BAD_ARG for a map without layers, an empty mask or any other bit (the chain's layers, the cache,
+ *     uncertainty_range, 1 << 7, unknown bits), a null layers array, an unknown memory mode, a bad selection and a layer the
+ *     batch does not hold given to a selection; TE_ERR_UNSUPPORTED for a selection on a map with a start index.  Every argument
+ *     error is found before anything is written: the te_map is then unchanged.
+ *   - Memory: a resident buffer of 4 bytes per cell and map per carried layer, allocated on first use and released by
+ *     te_map_destroy.  A selection in host memory stages its layers in the _maps scratch (4 bytes per given layer and selected
+ *     cell).  Launches: one kernel that puts a selection in place and fills its NULL layers, or for every map one fill kernel
+ *     when a pointer is NULL (none otherwise).  Host memory returns synchronised; device memory is asynchronous. */
+int te_map_carry_layers(te_map* map, int32_t nsel, const int32_t* map_index_or_null, uint32_t layer_mask, const float* layers[],
+                        int memory);
 
 /* One window of GridMap::getSubmap(position, length, isSuccess) (TraversabilityEstimation.cpp:305, getSubmapInformation; SURVEY.md
  * A.1, recalled from grid_map 1.6.x).  The submap is the block [top_row, top_row + rows) x [top_col, top_col + cols) of the map in
@@ -749,8 +796,12 @@ int te_submap_geometry(const te_geometry* g, int32_t n, const double* position_x
 /* publishTraversabilityMap (TraversabilityMap.cpp:172-186): the layers of `layer_mask` (te_layer bits), each rows x cols, back to
  * back in bit order (on a batch: per layer the nmaps maps back to back, nmaps*rows*cols floats a layer).  In host memory each is re-wrapped to the map's start index, as te_map's other outputs, and the call returns
  * synchronised; in device memory they are in the map's default (unwrapped) order, asynchronously.  TE_ERR_MISSING_LAYER for a
- * layer the map does not hold (roughness after te_map_set_layers without it, robot_slope after te_map_chain); TE_ERR_BAD_ARG
- * for an empty mask or unknown bits. */
+ * layer the map does not hold (roughness after te_map_set_layers without it, robot_slope after te_map_chain, a carried layer
+ * te_map_carry_layers did not give since the last whole-map update); TE_ERR_BAD_ARG for an empty mask or unknown bits.
+ * TE_LAYER_UNCERTAINTY_RANGE is upper_bound - lower_bound, one IEEE float32 subtraction per cell computed on the device
+ * (TraversabilityMap.cpp:178-180), with NaN results carrying the payload an x86-64 host's subtraction gives them (the first NaN
+ * operand, quieted; 0xffc00000 for Inf - Inf), so bit for bit what the reference publishes there.  It needs both bounds
+ * (TE_ERR_MISSING_LAYER otherwise).  In host memory it goes through a staging buffer of 4 bytes per cell of every map. */
 int te_map_get_layers(te_map* map, uint32_t layer_mask, float* out, int memory);
 
 /* The get_traversability_map service (TraversabilityEstimation.cpp:297-316) for nwin windows in one call: info[k] as
@@ -759,7 +810,9 @@ int te_map_get_layers(te_map* map, uint32_t layer_mask, float* out, int memory);
  * `out` is in `memory` (host: returns synchronised; device: asynchronous on the context stream).  When the windows take more
  * than out_capacity floats the call fills info, writes nothing else and returns TE_ERR_BAD_ARG: the total is the last record's
  * offset plus its layers, so the caller can call again with more room.  One kernel launch for all windows and layers (none when
- * every window fails).  Layer errors as te_map_get_layers; window errors as te_submap_geometry. */
+ * every window fails).  Layer errors as te_map_get_layers, except that TE_LAYER_UNCERTAINTY_RANGE is TE_ERR_BAD_ARG: the
+ * service cuts its submaps from the traversability map itself (TraversabilityEstimation.cpp:303-313), which has no such layer.
+ * Window errors as te_submap_geometry. */
 int te_map_get_submaps(te_map* map, int32_t nwin, const double* position_xy, const double* length_xy, uint32_t layer_mask,
                        te_submap_info* info, float* out, int64_t out_capacity, int memory);
 

@@ -18,18 +18,29 @@ KERNEL_AUTO, KERNEL_GENERIC, KERNEL_FUSED = 0, 1, 2
 
 IPC_HANDLE_BYTES = 80  # TE_IPC_HANDLE_BYTES
 
-# te_layer: bit k of a layer mask is LAYERS[k]; outputs that hold several layers have them in this order.
+# te_layer: bit k of a layer mask is LAYERS[k]; outputs that hold several layers have them in bit order.
 LAYERS = ("traversability", "traversability_slope", "traversability_step", "traversability_roughness", "elevation", "robot_slope",
           "traversability_footprint")
+# The elevation map's layers a te_map carries (Map.carry_layers), bits 8 .. 14 (bit 7 is unassigned), and uncertainty_range (bit
+# 15: upper_bound - lower_bound, derived by Map.get_layers).
+CARRIED_LAYERS = ("upper_bound", "lower_bound", "variance", "horizontal_variance_x", "horizontal_variance_y", "horizontal_variance_xy",
+                  "time")
+UNCERTAINTY_RANGE = "uncertainty_range"
+LAYER_BITS = {**{n: k for k, n in enumerate(LAYERS)}, **{n: 8 + k for k, n in enumerate(CARRIED_LAYERS)}, UNCERTAINTY_RANGE: 15}
 
 
 def layer_mask(names) -> int:
     """The te_layer mask of layer names (any order; each once)."""
     names = list(names)
-    unknown = [n for n in names if n not in LAYERS]
+    unknown = [n for n in names if n not in LAYER_BITS]
     if unknown or len(set(names)) != len(names):
-        raise ValueError(f"layer names {names}: each once, from {LAYERS}")
-    return sum(1 << LAYERS.index(n) for n in names)
+        raise ValueError(f"layer names {names}: each once, from {tuple(LAYER_BITS)}")
+    return sum(1 << LAYER_BITS[n] for n in names)
+
+
+def layer_order(mask) -> list:
+    """The layer names of a te_layer mask in bit order, the order of every output that holds several."""
+    return [n for n, b in sorted(LAYER_BITS.items(), key=lambda x: x[1]) if (mask >> b) & 1]
 
 
 class SubmapInfo(C.Structure):
@@ -172,6 +183,7 @@ SIGNATURES = {
     "te_map_get_footprint": (_R, [_P, _P, _I]),
     "te_map_clear_footprint": (_R, [_P]),
     "te_map_request_stats": (_R, [_P, _P]),
+    "te_map_carry_layers": (_R, [_P, _I, _P, _U, _P, _I]),
     "te_submap_geometry": (_R, [_G, _I, _P, _P, _P]),
     "te_map_get_layers": (_R, [_P, _U, _P, _I]),
     "te_map_get_submaps": (_R, [_P, _I, _P, _P, _U, _P, _P, _L, _I]),
@@ -859,6 +871,35 @@ class Map:
         self._check(self._L.te_map_set_layers_maps(self._h, C.byref(g), len(idx), _addr(idx), _addr(t), _addr(s), _addr(st), _addr(r),
                                                    _addr(e), _addr(rs), MEM_HOST))
 
+    def carry_layers(self, names, layers, map_index=None, memory=MEM_HOST):
+        """te_map_carry_layers (mapOut = mapIn for the layers the chain does not make): layers[k] becomes the map's layer names[k]
+        ("robot_slope" or CARRIED_LAYERS entries, any order); None fills it with 0.0.  Leaves the cache and the memo as they are.
+        map_index None: every map; otherwise the maps map_index only, and only layers the batch already holds.  Host memory: numpy
+        layers, (rows, cols) for one map or (n, rows, cols) for n maps (the batch, or the selection in map_index order), in the
+        map's start index.  Device memory: float32 device tensors of n * rows * cols, each map column-major in default order,
+        read asynchronously on the context stream."""
+        names, layers = list(names), list(layers)
+        if len(names) != len(layers):
+            raise ValueError(f"{len(names)} names but {len(layers)} layers")
+        mask = layer_mask(names)
+        given = dict(zip(names, layers))
+        if memory == MEM_HOST:
+            def host(a):
+                if a is None:
+                    return None
+                a = np.asarray(a, dtype=np.float32)
+                return np.asfortranarray(a) if a.ndim == 2 else self._batch_layers(a)
+            given = {n: host(a) for n, a in given.items()}
+        else:
+            self._ctx._order_after_torch(memory)
+        ordered = [given[n] for n in layer_order(mask)]   # the host pointer array holds them in bit order
+        ptrs = (C.c_void_p * len(ordered))(*(_addr(a) for a in ordered))
+        if map_index is None:
+            self._check(self._L.te_map_carry_layers(self._h, 0, None, mask, ptrs, memory))
+        else:
+            idx = self._map_index(map_index)
+            self._check(self._L.te_map_carry_layers(self._h, len(idx), _addr(idx), mask, ptrs, memory))
+
     def footprint_maps(self, fp, map_index):
         """te_map_footprint_maps (traversabilityFootprint(radius, offset) on the caches of the maps map_index only); returns those
         caches afterwards, (nsel, rows, cols) in map_index order."""
@@ -993,12 +1034,13 @@ class Map:
         return tuple(int(v) for v in out)
 
     def get_layers(self, names, out=None, memory=MEM_HOST):
-        """te_map_get_layers (publishTraversabilityMap): dict name -> (rows, cols) layer for `names` (LAYERS entries).  Host
+        """te_map_get_layers (publishTraversabilityMap): dict name -> (rows, cols) layer for `names` (LAYER_BITS entries; the
+        carried layers once carry_layers gave them, uncertainty_range = upper_bound - lower_bound computed on the device).  Host
         memory: numpy arrays, re-wrapped to the map's start index.  Device memory: `out` is a float32 device tensor of
         len(names) * rows * cols, filled asynchronously on the context stream in the map's default order; the dict holds views.
         On a batch every layer is (nmaps, rows, cols) (device memory: len(names) * nmaps * rows * cols floats)."""
         mask = layer_mask(names)
-        order = [n for k, n in enumerate(LAYERS) if (mask >> k) & 1]
+        order = layer_order(mask)
         rows, cols = self._shape() if self._g else (0, 0)
         if memory == MEM_HOST:
             out = np.empty((len(order), self._n, cols, rows), dtype=np.float32)   # per layer the maps back to back, column-major
@@ -1023,7 +1065,7 @@ class Map:
 
     def _submaps(self, win_map, positions, lengths, names, out, memory):
         mask = layer_mask(names)
-        order = [n for k, n in enumerate(LAYERS) if (mask >> k) & 1]
+        order = layer_order(mask)
         p, ln = _windows(positions, lengths)
         if out is None:
             if memory != MEM_HOST:

@@ -1312,6 +1312,8 @@ struct te_map {
   te_geometry geo_in{};  // as the layers came (host memory: with their circular-buffer start index)
   te_geometry geo{};     // the same with the start index cleared: the device layers are in default order
   DevBuf trav, slope, step, rough, elev, rslope, cache, fresh;
+  DevBuf carry[7];        // the carried layers, TE_LAYER_UPPER_BOUND (carry[0]) .. TE_LAYER_TIME (carry[6]): te_map_carry_layers
+  uint32_t carried = 0;   // the TE_LAYER_CARRIED bits the map holds
   DevBuf gather;  // te_map_get_submaps: the source-layer table, then the windows (te::SubmapWindow)
   // The _maps entries: the selected maps' layers packed back to back (grown to the largest selection) and their slot table
   DevBuf sel[te::kMapSlotLayers], slots;
@@ -1362,6 +1364,7 @@ int map_reset(te_map* m, const te_geometry* g_in, const te_geometry* g, int nmap
   m->nmaps = nmaps;
   m->memo_valid = false;
   m->have_layers = false;
+  m->carried = 0;  // a new map replaces the old one wholesale, its elevation map's layers included
   return TE_OK;
 }
 
@@ -1409,18 +1412,46 @@ int map_footprint_params(const te_map* m, const te_footprint_params* p) {
   return TE_OK;
 }
 
-// The map's layers of `mask`, in te_layer bit order (the order of every output that holds several).
-int map_layers(const te_map* m, uint32_t mask, const float* out[7], int* n) {
-  if (mask == 0 || (mask & ~(uint32_t)TE_LAYER_ALL)) return fail(TE_ERR_BAD_ARG, "layer mask 0x%x: need a non-empty subset of 0x%x", mask, TE_LAYER_ALL);
-  static const char* const names[7] = {"traversability", "traversability_slope", "traversability_step", "traversability_roughness",
-                                       "elevation", "robot_slope", "traversability_footprint"};
-  const DevBuf* const src[7] = {&m->trav, &m->slope, &m->step, m->have_rough ? &m->rough : nullptr, &m->elev,
-                                m->have_rslope ? &m->rslope : nullptr, &m->cache};
+constexpr int kLayerBits = 16;  // te_layer bits 0 .. 15 (1 << 7 unassigned)
+constexpr int kCarryBit0 = 8;   // TE_LAYER_UPPER_BOUND: carry[b - kCarryBit0] holds layer bit b of TE_LAYER_CARRIED
+const char* const kLayerNames[kLayerBits] = {"traversability", "traversability_slope", "traversability_step", "traversability_roughness",
+                                             "elevation", "robot_slope", "traversability_footprint", nullptr, "upper_bound", "lower_bound",
+                                             "variance", "horizontal_variance_x", "horizontal_variance_y", "horizontal_variance_xy",
+                                             "time", "uncertainty_range"};
+
+// The resident buffer of te_layer bit b when the map holds that layer, else null (uncertainty_range is derived: null).
+DevBuf* map_layer_buf(te_map* m, int b) {
+  switch (b) {
+    case 0: return &m->trav;
+    case 1: return &m->slope;
+    case 2: return &m->step;
+    case 3: return m->have_rough ? &m->rough : nullptr;
+    case 4: return &m->elev;
+    case 5: return m->have_rslope ? &m->rslope : nullptr;
+    case 6: return &m->cache;
+    default: return b >= kCarryBit0 && b < kCarryBit0 + 7 && ((m->carried >> b) & 1u) ? &m->carry[b - kCarryBit0] : nullptr;
+  }
+}
+
+// The map's layers of `mask`, in te_layer bit order (the order of every output that holds several).  with_range: the mask may
+// ask for TE_LAYER_UNCERTAINTY_RANGE (te_map_get_layers), whose entry is then null: the caller derives it from the bounds.
+int map_layers(te_map* m, uint32_t mask, bool with_range, const float* out[kLayerBits], int* n) {
+  if (!with_range && (mask & TE_LAYER_UNCERTAINTY_RANGE))
+    return fail(TE_ERR_BAD_ARG, "layer uncertainty_range is published with the map, not held by it: submaps have no such layer");
+  const uint32_t known = TE_LAYER_ALL | TE_LAYER_CARRIED | (with_range ? (uint32_t)TE_LAYER_UNCERTAINTY_RANGE : 0u);
+  if (mask == 0 || (mask & ~known)) return fail(TE_ERR_BAD_ARG, "layer mask 0x%x: need a non-empty subset of 0x%x", mask, known);
   *n = 0;
-  for (int b = 0; b < 7; ++b) {
+  for (int b = 0; b < kLayerBits; ++b) {
     if (!((mask >> b) & 1u)) continue;
-    if (!src[b]) return fail(TE_ERR_MISSING_LAYER, "layer %s is missing: the map does not hold it", names[b]);
-    out[(*n)++] = (const float*)src[b]->p;
+    if (b == 15) {
+      if ((m->carried & (TE_LAYER_UPPER_BOUND | TE_LAYER_LOWER_BOUND)) != (TE_LAYER_UPPER_BOUND | TE_LAYER_LOWER_BOUND))
+        return fail(TE_ERR_MISSING_LAYER, "layer uncertainty_range needs upper_bound and lower_bound: the map does not hold both");
+      out[(*n)++] = nullptr;
+      continue;
+    }
+    const DevBuf* src = map_layer_buf(m, b);
+    if (!src) return fail(TE_ERR_MISSING_LAYER, "layer %s is missing: the map does not hold it", kLayerNames[b]);
+    out[(*n)++] = (const float*)src->p;
   }
   return TE_OK;
 }
@@ -1481,7 +1512,8 @@ cudaError_t map_copy_packed(te_map* m, float* dst, const float* src, size_t n, b
 }
 
 // The packed layers src (each null or nsel maps back to back) into the selected maps' resident layers dst, in one launch that also
-// empties those maps' caches and, when the memo is live, clears their memo bytes.  The te_map-wide memo key stays.
+// empties those maps' caches, fills their carried layers with NaN (the new maps come without them, but every map of a batch
+// holds the same layers) and, when the memo is live, clears their memo bytes.  The te_map-wide memo key stays.
 int map_put_selected(te_map* m, const MapSel& s, const float* const src[te::kMapSlotLayers], DevBuf* const dst[te::kMapSlotLayers]) {
   te_ctx* c = m->ctx;
   te::MapSlots a{};
@@ -1489,6 +1521,9 @@ int map_put_selected(te_map* m, const MapSel& s, const float* const src[te::kMap
     a.src[l] = dst[l] ? src[l] : nullptr;
     a.dst[l] = dst[l] ? (float*)dst[l]->p : nullptr;
   }
+  for (int k = 0; k < 7; ++k)
+    if ((m->carried >> (kCarryBit0 + k)) & 1u) a.fill[k] = (float*)m->carry[k].p;
+  a.fill_bits = 0xffffffffu;
   a.cache = (float*)m->cache.p;
   a.memo = m->memo_valid ? (unsigned char*)m->fp.memo.p : nullptr;  // reserved for the whole batch while valid (map_memo)
   a.slot = (const int*)m->slots.p;
@@ -1524,6 +1559,7 @@ int te_map_destroy(te_map* m) {
       for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather, &m->slots, &m->image})
         b->release();
       for (DevBuf& b : m->sel) b.release();
+      for (DevBuf& b : m->carry) b.release();
       m->fp.release();
     }
   }
@@ -1794,6 +1830,85 @@ int te_map_set_layers_maps(te_map* m, const te_geometry* g, int32_t nsel, const 
   TE_MAP_ENTER(m);
   const MapSel sel{nsel, map_index};
   return map_set_layers(m, g, nsel, trav, slope, step, rough, elev, robot_slope, memory, &sel);
+}
+
+// mapOut = mapIn for robot_slope and the carried layers.  Every map: given layers are copied in as map_put_layer does (host layers
+// unwrapped), and one k_map_slots launch with the identity slot table fills the NULL ones with 0.0f.  A selection: given layers
+// (staged in host memory, read in place in device memory) go to their slots and the NULL ones are filled, in one k_map_slots
+// launch.  Neither touches the cache or the memo.
+int te_map_carry_layers(te_map* m, int32_t nsel, const int32_t* map_index, uint32_t layer_mask, const float* layers[], int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  const uint32_t allowed = (uint32_t)TE_LAYER_ROBOT_SLOPE | (uint32_t)TE_LAYER_CARRIED;
+  if (layer_mask == 0 || (layer_mask & ~allowed))
+    return fail(TE_ERR_BAD_ARG, "layer mask 0x%x: te_map_carry_layers takes a non-empty subset of 0x%x (robot_slope and the elevation "
+                "map's layers)", layer_mask, allowed);
+  if (!layers) return fail(TE_ERR_BAD_ARG, "layers is null");
+  if (memory != TE_MEM_HOST && memory != TE_MEM_DEVICE) return fail(TE_ERR_BAD_ARG, "unknown memory mode %d", memory);
+  const bool whole = nsel == 0 && !map_index;
+  const MapSel sel{nsel, map_index};
+  if (!whole) {
+    if (int rc = map_select(m, false, nullptr, sel)) return rc;
+    const uint32_t held = m->carried | (m->have_rslope ? (uint32_t)TE_LAYER_ROBOT_SLOPE : 0u);
+    if (const uint32_t extra = layer_mask & ~held)
+      return fail(TE_ERR_BAD_ARG, "layer %s is given to some maps but the batch does not hold it: every map of a batch holds the same "
+                  "layers, so give it to every map (nsel = 0, map_index NULL)", kLayerNames[__builtin_ctz(extra)]);
+  }
+  // the layers in bit order: the slots of MapSlots, and where each goes
+  const float* src[te::kMapSlotLayers] = {};
+  DevBuf* dst[te::kMapSlotLayers] = {};
+  int n = 0;
+  for (int b = 0; b < kLayerBits; ++b)
+    if ((layer_mask >> b) & 1u) {
+      src[n] = layers[n];
+      dst[n++] = b == 5 ? &m->rslope : &m->carry[b - kCarryBit0];
+    }
+  const size_t cells = whole ? batch_cells(m) : map_cells(m) * sel.n;
+  te::MapSlots a{};
+  a.nsel = whole ? m->nmaps : sel.n;
+  a.cells = map_cells(m);
+  a.fill_bits = 0u;  // GridMap::add(layer, 0.0)
+  bool fills = false;
+  if (whole) {
+    for (int k = 0; k < n; ++k) TE_CUDA(dst[k]->reserve(sizeof(float) * batch_cells(m)));
+    for (int k = 0; k < n; ++k) {
+      if (src[k]) {
+        if (int rc = map_put_layer(m, *dst[k], src[k], memory)) return rc;
+      } else {
+        a.fill[k] = (float*)dst[k]->p;
+        fills = true;
+      }
+    }
+  } else {
+    unsigned staged = 0;  // host memory: the layers given, staged; device memory: read in place
+    for (int k = 0; k < n; ++k)
+      if (memory == TE_MEM_HOST && src[k]) staged |= 1u << k;
+    if (int rc = map_stage_selection(m, sel, staged)) return rc;
+    for (int k = 0; k < n; ++k) {
+      if (src[k] && memory == TE_MEM_HOST) {
+        TE_CUDA(map_copy_packed(m, (float*)m->sel[k].p, src[k], cells, false, memory));
+        src[k] = (const float*)m->sel[k].p;
+      }
+      if (src[k]) {
+        a.src[k] = src[k];
+        a.dst[k] = (float*)dst[k]->p;
+      } else {
+        a.fill[k] = (float*)dst[k]->p;
+      }
+    }
+    a.slot = (const int*)m->slots.p;
+    fills = true;  // the one launch that puts the selection in place
+  }
+  if (fills) {
+    te::launch_map_slots(a, true, c->sms, c->stream);
+    if (int rc = launch_check(c, "k_map_slots (carry)")) return rc;
+  }
+  if (whole) {
+    m->carried |= layer_mask & TE_LAYER_CARRIED;
+    if (layer_mask & TE_LAYER_ROBOT_SLOPE) m->have_rslope = true;
+  }
+  if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));  // the caller may reuse its layers on return
+  return TE_OK;
 }
 
 // te_map_footprint (sel null: every map, swept in place) and te_map_footprint_maps (the selected maps' input layers gathered
@@ -2112,14 +2227,25 @@ int te_submap_geometry(const te_geometry* g, int32_t n, const double* position_x
 int te_map_get_layers(te_map* m, uint32_t layer_mask, float* out, int memory) {
   TE_MAP_ENTER(m);
   if (int rc = map_ready(m)) return rc;
-  const float* src[7];
+  const float* src[kLayerBits];
   int nl = 0;
-  if (int rc = map_layers(m, layer_mask, src, &nl)) return rc;
+  if (int rc = map_layers(m, layer_mask, true, src, &nl)) return rc;
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
-  for (int k = 0; k < nl; ++k)  // per layer every map, back to back
-    if (int rc = map_get_layer(m, out + (size_t)k * batch_cells(m), src[k], memory)) return rc;
-  if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));
-  return TE_OK;
+  // uncertainty_range (a null entry, the last in bit order) is computed straight into a device output; in host memory into staging,
+  // which finish() re-wraps and copies back after the other layers
+  Staging st(c, memory == TE_MEM_HOST, &m->geo_in);
+  for (int k = 0; k < nl; ++k) {  // per layer every map, back to back
+    float* dst = out + (size_t)k * batch_cells(m);
+    if (src[k]) {
+      if (int rc = map_get_layer(m, dst, src[k], memory)) return rc;
+      continue;
+    }
+    float* d = st.out_layer(dst, m->geo.cols * m->nmaps);
+    if (st.rc) return st.rc;
+    te::launch_uncertainty_range((const float*)m->carry[0].p, (const float*)m->carry[1].p, d, batch_cells(m), c->sms, c->stream);
+    if (int rc = launch_check(c, "k_uncertainty_range")) return rc;
+  }
+  return st.finish();  // host memory: returns synchronised
 }
 
 // te_map_get_submaps (win_map null: map 0) and te_map_get_submaps_batched (window k on map win_map[k], checked by the entry): only
@@ -2127,9 +2253,9 @@ int te_map_get_layers(te_map* m, uint32_t layer_mask, float* out, int memory) {
 static int map_submaps(te_map* m, int32_t nwin, const int32_t* win_map, const double* position_xy, const double* length_xy,
                        uint32_t layer_mask, te_submap_info* info, float* out, int64_t out_capacity, int memory) {
   te_ctx* c = m->ctx;
-  const float* src[7];
+  const float* src[kLayerBits];
   int nl = 0;
-  if (int rc = map_layers(m, layer_mask, src, &nl)) return rc;
+  if (int rc = map_layers(m, layer_mask, false, src, &nl)) return rc;
   int64_t total = 0;
   if (int rc = submap_windows(&m->geo, nwin, position_xy, length_xy, nl, info, &total)) return rc;
   if (out_capacity < total)
@@ -2137,9 +2263,10 @@ static int map_submaps(te_map* m, int32_t nwin, const int32_t* win_map, const do
                 (long long)out_capacity);
   if (total == 0) return TE_OK;
   if (!out) return fail(TE_ERR_BAD_ARG, "output is null");
-  // the table k_map_gather_submaps reads: the source layers in its first two records, then the windows that have cells
-  static_assert(sizeof(const float*) * 7 <= 2 * sizeof(te::SubmapWindow), "layer table");
-  std::vector<te::SubmapWindow> table(2);
+  // the table k_map_gather_submaps reads: the source layers in its first kHead records, then the windows that have cells
+  constexpr int kHead = 4;
+  static_assert(sizeof(const float*) * (kLayerBits - 1) <= kHead * sizeof(te::SubmapWindow), "layer table");
+  std::vector<te::SubmapWindow> table(kHead);
   std::memcpy((void*)table.data(), src, sizeof(const float*) * nl);
   long long columns = 0;
   for (int32_t k = 0; k < nwin; ++k) {
@@ -2156,7 +2283,7 @@ static int map_submaps(te_map* m, int32_t nwin, const int32_t* win_map, const do
   Staging st(c, memory == TE_MEM_HOST, &m->geo);  // host memory: gather into staging, then one copy of the packed floats
   float* dout = st.out(out, (size_t)total);
   if (st.rc) return st.rc;
-  const te::SubmapGather a{(const float* const*)m->gather.p, (const te::SubmapWindow*)m->gather.p + 2, (int)table.size() - 2,
+  const te::SubmapGather a{(const float* const*)m->gather.p, (const te::SubmapWindow*)m->gather.p + kHead, (int)table.size() - kHead,
                            m->geo.rows, columns, dout};
   te::launch_gather_submaps(a, c->sms, c->stream);
   if (int rc = launch_check(c, "k_map_gather_submaps")) return rc;

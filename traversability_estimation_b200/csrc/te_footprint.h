@@ -153,18 +153,22 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
 // (slot: a device table of nsel map slots; null: j * n, the whole batch as nsel = 1 block of every cell).  One launch.
 int launch_map_merge(const float* fresh, float* cache, float* out, size_t n, const int* slot, int nsel, int sms, cudaStream_t s);
 
-// Selected maps of a te_map (te_map_chain_maps, te_map_set_layers_maps, te_map_footprint_maps): packed map j is at j * cells in
-// scratch, its resident copy at slot[j] * cells in the te_map's layers, cache and memo.  Up to kMapSlotLayers layers move in one
-// launch; a layer with a null dst is skipped.  put: packed src -> resident dst, and the maps' cache slots become NaN (empty) and
-// their memo slots 0 (memo may be null); otherwise resident src -> packed dst (cache and memo unused).  Grid-stride over maps and
-// cells, 16-byte accesses when cells % 4 == 0 and every pointer is 16-byte aligned.  One launch, whatever nsel and the layers.
-constexpr int kMapSlotLayers = 6;
+// Selected maps of a te_map (te_map_chain_maps, te_map_set_layers_maps, te_map_footprint_maps, te_map_carry_layers): packed map j
+// is at j * cells in scratch, its resident copy at slot[j] * cells in the te_map's layers, cache and memo.  Up to kMapSlotLayers
+// layers move in one launch; a layer with a null dst is skipped.  put: packed src -> resident dst, the maps' cache slots become
+// NaN (empty; cache may be null) and their memo slots 0 (memo may be null), and their slots of every non-null fill layer take the
+// bits fill_bits; otherwise resident src -> packed dst (cache, memo and fill unused).  A null slot table is the identity (slot[j]
+// = j: every map of the te_map when nsel = nmaps).  Grid-stride over maps and cells, 16-byte accesses when cells % 4 == 0 and
+// every pointer is 16-byte aligned.  One launch, whatever nsel and the layers.
+constexpr int kMapSlotLayers = 8;
 struct MapSlots {
   const float* src[kMapSlotLayers];
   float* dst[kMapSlotLayers];
+  float* fill[kMapSlotLayers];
+  unsigned fill_bits;
   float* cache;
   unsigned char* memo;
-  const int* slot;  // device, nsel entries
+  const int* slot;  // device, nsel entries, or null
   int nsel;
   size_t cells;     // per map
 };

@@ -62,6 +62,9 @@ struct SubmapGather {
 };
 // One k_map_gather_submaps launch for every column of every window (none when there is no column).
 void launch_gather_submaps(const SubmapGather& a, int sms, cudaStream_t s);
+// out[c] = upper[c] - lower[c] for n cells (device pointers), IEEE float32: publishTraversabilityMap's uncertainty_range.  One
+// k_uncertainty_range launch (none for n = 0).
+void launch_uncertainty_range(const float* upper, const float* lower, float* out, size_t n, int sms, cudaStream_t s);
 struct GridGeo;
 // valid[q] = getIndex(xy[2q], xy[2q+1]) succeeds and traversability is finite there (device pointers; none launched for n = 0).
 // A batch of nmaps maps of geometry g back to back in `trav`: position q is on map pos_map[q] (null: map 0), and a map outside

@@ -88,27 +88,36 @@ __global__ void __launch_bounds__(256) k_map_merge(float* cache, const float* __
 }
 
 // Selected maps between their slots of a te_map and packed scratch (launch_map_slots).  PUT: layer l of packed map j goes to
-// dst[l] + slot[j] * cells, and the cache / memo slots of the map are emptied (NaN bits 0xffffffff, memo 0: not evaluated).  Not
-// PUT: src[l] + slot[j] * cells goes to packed map j of dst[l].  V cells per thread and access (V = 4: 16-byte accesses).
+// dst[l] + slot[j] * cells, the cache / memo slots of the map are emptied (NaN bits 0xffffffff, memo 0: not evaluated) and its
+// slots of the fill layers take fill_bits.  Not PUT: src[l] + slot[j] * cells goes to packed map j of dst[l].  V cells per thread
+// and access (V = 4: 16-byte accesses).
 template <bool PUT, int V>
 __global__ void __launch_bounds__(256) k_map_slots(MapSlots a) {
   using Vec = typename std::conditional<V == 4, float4, float>::type;
   using Bytes = typename std::conditional<V == 4, unsigned, unsigned char>::type;
   const size_t step = (size_t)gridDim.x * blockDim.x * V;
   for (int j = blockIdx.y; j < a.nsel; j += gridDim.y) {
-    const size_t packed = (size_t)j * a.cells, resident = (size_t)a.slot[j] * a.cells;
+    const size_t packed = (size_t)j * a.cells, resident = (size_t)(a.slot ? a.slot[j] : j) * a.cells;
     const size_t s0 = PUT ? packed : resident, d0 = PUT ? resident : packed;
     for (size_t c = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * V; c < a.cells; c += step) {
 #pragma unroll
       for (int l = 0; l < kMapSlotLayers; ++l)
         if (a.dst[l]) *reinterpret_cast<Vec*>(a.dst[l] + d0 + c) = __ldg(reinterpret_cast<const Vec*>(a.src[l] + s0 + c));
       if (PUT) {
-        const float nan = __int_as_float(-1);
-        Vec e;
-        if constexpr (V == 4) e = make_float4(nan, nan, nan, nan);
-        else e = nan;
-        *reinterpret_cast<Vec*>(a.cache + resident + c) = e;
+        const float nan = __int_as_float(-1), f = __uint_as_float(a.fill_bits);
+        Vec e, v;
+        if constexpr (V == 4) {
+          e = make_float4(nan, nan, nan, nan);
+          v = make_float4(f, f, f, f);
+        } else {
+          e = nan;
+          v = f;
+        }
+        if (a.cache) *reinterpret_cast<Vec*>(a.cache + resident + c) = e;
         if (a.memo) *reinterpret_cast<Bytes*>(a.memo + resident + c) = 0;
+#pragma unroll
+        for (int l = 0; l < kMapSlotLayers; ++l)
+          if (a.fill[l]) *reinterpret_cast<Vec*>(a.fill[l] + resident + c) = v;
       }
     }
   }
@@ -614,7 +623,8 @@ void launch_map_slots(const MapSlots& a, bool put, int sms, cudaStream_t s) {
   // 16-byte accesses when every map slot and every layer starts on a 16-byte boundary
   bool vec = a.cells % 4 == 0 && (reinterpret_cast<uintptr_t>(a.cache) & 15u) == 0;
   for (int l = 0; l < kMapSlotLayers; ++l)
-    vec = vec && ((reinterpret_cast<uintptr_t>(a.src[l]) | reinterpret_cast<uintptr_t>(a.dst[l])) & 15u) == 0;
+    vec = vec && ((reinterpret_cast<uintptr_t>(a.src[l]) | reinterpret_cast<uintptr_t>(a.dst[l]) | reinterpret_cast<uintptr_t>(a.fill[l])) &
+                  15u) == 0;
   const int V = vec ? 4 : 1;
   const long long per_map = std::max<long long>((long long)sms * 8 / a.nsel, 1);
   const long long bx = std::max(std::min<long long>((long long)((a.cells / V + 255) / 256), per_map), 1LL);

@@ -58,7 +58,42 @@ __global__ void k_map_valid_at(GridGeo g, const float* __restrict__ trav, int n,
   valid[q] = in && finitef(__ldg(trav + (size_t)j * g.rows + i)) ? 1 : 0;
 }
 
+// upper - lower as the reference's host computes it: one IEEE float32 subtraction, round to nearest, never contracted.  Its NaN
+// results differ in payload only: the GPU returns its canonical NaN, x86-64's SSE / AVX subtraction (the reference node's, and
+// numpy's) returns the first NaN operand quieted, or the default NaN 0xffc00000 for Inf - Inf.  That rule is applied here, so the
+// layer is the reference's bit for bit.
+__device__ __forceinline__ float range_sub(float u, float l) {
+  const float r = __fsub_rn(u, l);
+  if (!isnan(r)) return r;
+  const unsigned q = isnan(u) ? __float_as_uint(u) : isnan(l) ? __float_as_uint(l) : 0xffc00000u;
+  return __uint_as_float(q | 0x00400000u);
+}
+
+// uncertainty_range = upper_bound - lower_bound per cell (publishTraversabilityMap).  V cells per thread and access (V = 4: 16-byte).
+template <int V>
+__global__ void __launch_bounds__(256) k_uncertainty_range(const float* __restrict__ upper, const float* __restrict__ lower,
+                                                           float* __restrict__ out, size_t n) {
+  const size_t step = (size_t)gridDim.x * blockDim.x * V;
+  for (size_t c = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * V; c < n; c += step) {
+    if constexpr (V == 4) {
+      const float4 u = __ldg(reinterpret_cast<const float4*>(upper + c)), l = __ldg(reinterpret_cast<const float4*>(lower + c));
+      *reinterpret_cast<float4*>(out + c) = make_float4(range_sub(u.x, l.x), range_sub(u.y, l.y), range_sub(u.z, l.z), range_sub(u.w, l.w));
+    } else {
+      out[c] = range_sub(__ldg(upper + c), __ldg(lower + c));
+    }
+  }
+}
+
 }  // namespace
+
+void launch_uncertainty_range(const float* upper, const float* lower, float* out, size_t n, int sms, cudaStream_t s) {
+  if (n == 0) return;
+  const bool vec = n % 4 == 0 && ((reinterpret_cast<uintptr_t>(upper) | reinterpret_cast<uintptr_t>(lower) | reinterpret_cast<uintptr_t>(out)) & 15u) == 0;
+  const int V = vec ? 4 : 1;
+  const size_t blocks = std::min<size_t>((n / V + 255) / 256, (size_t)sms * 16);
+  if (vec) k_uncertainty_range<4><<<(unsigned)blocks, 256, 0, s>>>(upper, lower, out, n);
+  else k_uncertainty_range<1><<<(unsigned)blocks, 256, 0, s>>>(upper, lower, out, n);
+}
 
 void launch_gather_submaps(const SubmapGather& a, int sms, cudaStream_t s) {
   if (a.ncolumns <= 0) return;
