@@ -486,7 +486,8 @@ int te_check_footprint_request_batched(te_ctx* ctx, const te_geometry* g, const 
  * entries, te_map_get_layers, te_map_get_footprint and te_map_clear_footprint work on every map, their outputs holding the maps
  * back to back per layer; te_map_check_footprint_request, te_map_get_submaps and te_map_valid_at need a map index and fail with
  * TE_ERR_BAD_ARG on a te_map of more than one map (use their _batched entries).  The single-map entries on a te_map of one map
- * are unchanged, start indices included. */
+ * are unchanged, start indices included.  The maps of a batch may also sit at their own positions (te_map_chain_batched_at and the
+ * other _at entries below): the rule above then holds with a single-map te_map holding map m at map m's position. */
 typedef struct te_map te_map;
 int te_map_create(te_ctx* ctx, te_map** out);
 int te_map_destroy(te_map* map);
@@ -548,6 +549,42 @@ int te_map_chain_maps(te_map* map, const te_geometry* g, const te_chain_params* 
 int te_map_set_layers_maps(te_map* map, const te_geometry* g, int32_t nsel, const int32_t* map_index, const float* traversability,
                            const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
                            const float* robot_slope_or_null, int memory);
+
+/* Maps at their own positions (a fleet, simulated environments with their own origins, robot-centric submaps around each robot).
+ * The four entries below take the arguments of the entry of the same name plus position_xy, a HOST array of one (x, y) pair per map
+ * the call updates (nmaps pairs, or nsel in map_index order), read before the call returns: map m then sits at that position
+ * instead of g's, with g's rows, cols, resolution and length.  position_xy NULL puts every map it updates at g's position: the
+ * entry of the same name is that case.  Everything a te_map entry returns or stores for a map (layers, cache, memo, request outputs
+ * and untraversable polygons, te_map_request_stats, submaps and their te_submap_info, te_map_valid_at_batched, the footprint sweeps
+ * and their reductions) is then, bit for bit, what a single-map te_map
+ * holding that map at its position returns or stores.  Rules:
+ *   - A non-finite position is TE_ERR_BAD_ARG, found before anything is written (the te_map is then unchanged).
+ *   - The _maps_at entries move only the selected maps; they check g against the batch bit for bit except for position_x /
+ *     position_y, as the _maps entries check all of it.  Every other rule of the _maps entries applies.
+ *   - te_map_chain_image(_maps) puts the maps it updates at g's position; te_map_carry_layers does not move a map.
+ *   - Requests (te_map_check_footprint_request_batched, _device) take each path's centres, getIndex and checkInclination from its
+ *     map's position, in the work list, the dedup keys (the map is part of a key), the walks, the replay and the polygonal paths.
+ *     The polygon entries (te_map_footprint_polygon(_yaws, _yaws_reduce)) classify the polygon's offsets per position: on maps at
+ *     several positions they sweep one map at a time (one sweep per map, outputs in the batch layout).
+ *   - Memory: when the maps of a call do not all sit at one position the te_map keeps per-map tables on the device, 8 bytes per
+ *     row and per column of every map of the call (cell-centre coordinates) plus 16 per map (the position), and for a chain call
+ *     1 byte more per row and column (the fused kernel's on-circle masks); they are rebuilt when the positions change.
+ * The kernels read a map's tables through a per-map stride that is 0 when every map sits at one position, so that case reads what
+ * it reads without positions. */
+int te_map_chain_batched_at(te_map* map, const te_geometry* g, const te_chain_params* p, int32_t nmaps, const float* elevation,
+                            float* slope_or_null, float* step_or_null, float* roughness_or_null, float* traversability_or_null, int memory,
+                            const double* position_xy);
+int te_map_set_layers_batched_at(te_map* map, const te_geometry* g, int32_t nmaps, const float* traversability, const float* slope,
+                                 const float* step, const float* roughness_or_null, const float* elevation,
+                                 const float* robot_slope_or_null, int memory, const double* position_xy);
+int te_map_chain_maps_at(te_map* map, const te_geometry* g, const te_chain_params* p, int32_t nsel, const int32_t* map_index,
+                         const float* elevation, float* slope_or_null, float* step_or_null, float* roughness_or_null,
+                         float* traversability_or_null, int memory, const double* position_xy);
+int te_map_set_layers_maps_at(te_map* map, const te_geometry* g, int32_t nsel, const int32_t* map_index, const float* traversability,
+                              const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                              const float* robot_slope_or_null, int memory, const double* position_xy);
+/* Where the maps sit: position_xy[2m], position_xy[2m + 1] for map m (nmaps pairs).  TE_ERR_BAD_ARG before layers were set. */
+int te_map_positions(te_map* map, double* position_xy);
 
 /* ---- Elevation images: the reference node's image topic (TraversabilityEstimation::imageCallback) ------------------------------
  * The node turns a grayscale height image into the elevation layer (GridMapRosConverter::initializeFromImage on the first image,

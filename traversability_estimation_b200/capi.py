@@ -169,6 +169,11 @@ SIGNATURES = {
     "te_map_set_layers_batched": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _I]),
     "te_map_chain_maps": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _P, _I]),
     "te_map_set_layers_maps": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _P, _I]),
+    "te_map_chain_batched_at": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _I, _P]),
+    "te_map_set_layers_batched_at": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "te_map_chain_maps_at": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "te_map_set_layers_maps_at": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "te_map_positions": (_R, [_P, _P]),
     "te_image_geometry": (_R, [_I, _I, _D, _D, _D, _G]),
     "te_map_chain_image": (_R, [_P, _G, _CP, _I, _I, _P, _L, _L, _D, _D, _P, _P, _P, _P, _I]),
     "te_map_chain_image_maps": (_R, [_P, _G, _CP, _I, _P, _I, _P, _L, _L, _D, _D, _P, _P, _P, _P, _I]),
@@ -793,15 +798,27 @@ class Map:
         self._g, self._n = g, 1
         return out if outputs else None
 
-    def chain_batched(self, g, p, nmaps, elevation, outputs=False):
+    @staticmethod
+    def _positions(positions, n):
+        """(n, 2) map positions (x, y) as the _at entries read them, or None."""
+        if positions is None:
+            return None
+        xy = np.ascontiguousarray(positions, dtype=np.float64).reshape(-1)
+        if xy.size != 2 * n:
+            raise ValueError(f"positions: need {n} (x, y) pairs, got {xy.size} values")
+        return xy
+
+    def chain_batched(self, g, p, nmaps, elevation, outputs=False, positions=None):
         """te_map_chain_batched (computeTraversability for every map): elevation (nmaps, rows, cols); empties every cache.
-        outputs=True also returns the four layers as a dict of (nmaps, rows, cols) arrays."""
-        fn = self._L.te_map_chain_batched
+        outputs=True also returns the four layers as a dict of (nmaps, rows, cols) arrays.  positions (nmaps, 2): map m sits at
+        positions[m] instead of g's position (te_map_chain_batched_at)."""
         e = self._batch_layers(elevation)
         out = {k: np.empty((int(nmaps), g.cols, g.rows), dtype=np.float32) for k in ("slope", "step", "roughness", "traversability")} \
             if outputs else {}
-        self._check(fn(self._h, C.byref(g), C.byref(p), int(nmaps), _addr(e),
-                       *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")), MEM_HOST))
+        xy = self._positions(positions, int(nmaps))
+        args = (self._h, C.byref(g), C.byref(p), int(nmaps), _addr(e),
+                *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")), MEM_HOST)
+        self._check(self._L.te_map_chain_batched(*args) if xy is None else self._L.te_map_chain_batched_at(*args, _addr(xy)))
         self._g, self._n = g, int(nmaps)
         return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
 
@@ -813,29 +830,32 @@ class Map:
         self._check(fn(self._h, C.byref(g), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST))
         self._g, self._n = g, 1
 
-    def set_layers_batched(self, g, nmaps, traversability, slope, step, elevation, roughness=None, robot_slope=None):
+    def set_layers_batched(self, g, nmaps, traversability, slope, step, elevation, roughness=None, robot_slope=None, positions=None):
         """te_map_set_layers_batched (setTraversabilityMap for every map): each layer (nmaps, rows, cols); empties every cache and
-        memo."""
-        fn = self._L.te_map_set_layers_batched
+        memo.  positions (nmaps, 2): map m sits at positions[m] (te_map_set_layers_batched_at)."""
         t, s, st, r, e, rs = (self._batch_layers(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
-        self._check(fn(self._h, C.byref(g), int(nmaps), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST))
+        xy = self._positions(positions, int(nmaps))
+        args = (self._h, C.byref(g), int(nmaps), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST)
+        self._check(self._L.te_map_set_layers_batched(*args) if xy is None else self._L.te_map_set_layers_batched_at(*args, _addr(xy)))
         self._g, self._n = g, int(nmaps)
 
     @staticmethod
     def _map_index(map_index):
         return np.ascontiguousarray(map_index, dtype=np.int32).reshape(-1)
 
-    def chain_maps(self, g, p, map_index, elevation, outputs=False):
+    def chain_maps(self, g, p, map_index, elevation, outputs=False, positions=None):
         """te_map_chain_maps (computeTraversability for the maps map_index of the batch only): elevation (nsel, rows, cols), map
         j of it going to map map_index[j]; empties those maps' caches and keeps every other map as it was.  outputs=True also
-        returns the four layers as a dict of (nsel, rows, cols) arrays in map_index order."""
+        returns the four layers as a dict of (nsel, rows, cols) arrays in map_index order.  positions (nsel, 2): map map_index[j]
+        moves to positions[j] (te_map_chain_maps_at)."""
         idx = self._map_index(map_index)
         e = self._batch_layers(elevation)
         out = {k: np.empty((len(idx), g.cols, g.rows), dtype=np.float32) for k in ("slope", "step", "roughness", "traversability")} \
             if outputs else {}
-        self._check(self._L.te_map_chain_maps(self._h, C.byref(g), C.byref(p), len(idx), _addr(idx), _addr(e),
-                                              *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")),
-                                              MEM_HOST))
+        xy = self._positions(positions, len(idx))
+        args = (self._h, C.byref(g), C.byref(p), len(idx), _addr(idx), _addr(e),
+                *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")), MEM_HOST)
+        self._check(self._L.te_map_chain_maps(*args) if xy is None else self._L.te_map_chain_maps_at(*args, _addr(xy)))
         return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
 
     _CHAIN_OUTPUTS = ("slope", "step", "roughness", "traversability")
@@ -863,13 +883,21 @@ class Map:
                                                     *(_addr(out.get(k)) for k in self._CHAIN_OUTPUTS), MEM_HOST))
         return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
 
-    def set_layers_maps(self, g, map_index, traversability, slope, step, elevation, roughness=None, robot_slope=None):
+    def set_layers_maps(self, g, map_index, traversability, slope, step, elevation, roughness=None, robot_slope=None, positions=None):
         """te_map_set_layers_maps (setTraversabilityMap for the maps map_index only): each layer (nsel, rows, cols) in map_index
-        order; the optional layers must be those the batch holds.  Empties those maps' caches and memos."""
+        order; the optional layers must be those the batch holds.  Empties those maps' caches and memos.  positions (nsel, 2): map
+        map_index[j] moves to positions[j] (te_map_set_layers_maps_at)."""
         idx = self._map_index(map_index)
         t, s, st, r, e, rs = (self._batch_layers(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
-        self._check(self._L.te_map_set_layers_maps(self._h, C.byref(g), len(idx), _addr(idx), _addr(t), _addr(s), _addr(st), _addr(r),
-                                                   _addr(e), _addr(rs), MEM_HOST))
+        xy = self._positions(positions, len(idx))
+        args = (self._h, C.byref(g), len(idx), _addr(idx), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST)
+        self._check(self._L.te_map_set_layers_maps(*args) if xy is None else self._L.te_map_set_layers_maps_at(*args, _addr(xy)))
+
+    def positions(self):
+        """te_map_positions: where the maps sit, an (nmaps, 2) float64 array of (x, y)."""
+        xy = np.empty((self._n, 2), dtype=np.float64)
+        self._check(self._L.te_map_positions(self._h, _addr(xy)))
+        return xy
 
     def carry_layers(self, names, layers, map_index=None, memory=MEM_HOST):
         """te_map_carry_layers (mapOut = mapIn for the layers the chain does not make): layers[k] becomes the map's layer names[k]
@@ -1070,7 +1098,19 @@ class Map:
         if out is None:
             if memory != MEM_HOST:
                 raise ValueError("device memory needs an `out` tensor")
-            geo = submap_geometry(self._g, p, ln) if self._g is not None else np.zeros(0, dtype=SUBMAP_INFO_DTYPE)
+            if self._g is None:
+                geo = np.zeros(0, dtype=SUBMAP_INFO_DTYPE)
+            else:   # each window on its own map's position (te_map_positions: g's unless an _at entry placed the map)
+                wm = np.zeros(len(p), np.int64) if win_map is None else np.asarray(win_map, dtype=np.int64).reshape(-1)
+                xy = self.positions()
+                geo = np.zeros(len(p), dtype=SUBMAP_INFO_DTYPE)
+                for m in np.unique(wm) if len(p) else ():
+                    if not 0 <= m < self._n:   # the library refuses the call: nothing to size
+                        continue
+                    gm = Geometry.from_buffer_copy(self._g)
+                    gm.position_x, gm.position_y = float(xy[m, 0]), float(xy[m, 1])
+                    k = np.nonzero(wm == m)[0]
+                    geo[k] = submap_geometry(gm, p[k], ln[k])
             out = np.empty(len(order) * int((geo["rows"].astype(np.int64) * geo["cols"]).sum()), dtype=np.float32)
         cap = out.size if isinstance(out, np.ndarray) else out.numel()
         info = np.zeros(len(p), dtype=SUBMAP_INFO_DTYPE)

@@ -8,7 +8,9 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <algorithm>
 #include <functional>
+#include <limits>
 #include <map>
 #include <mutex>
 #include <string>
@@ -389,8 +391,9 @@ int next_timing_slot(te_ctx* c, te_ctx::Ev3** out) {
 }
 
 // Device-memory chain on one slab: picks the kernel.
+// mm: the per-map mask tables of a batch whose maps sit at their own positions (v then holds their coordinate tables), or null.
 int run_chain_device(te_ctx* c, const te_geometry* g, const te::SlabView& v, const te_chain_params* p, const float* elev,
-                     const te::ChainOut& o, int nmaps) {
+                     const te::ChainOut& o, int nmaps, const te::MapMasks* mm = nullptr) {
   const te::ChainDev d = make_chain_dev(g, p);
   bool use_fused = false;
   if (c->kernel_choice != TE_KERNEL_GENERIC) {
@@ -433,12 +436,12 @@ int run_chain_device(te_ctx* c, const te_geometry* g, const te::SlabView& v, con
         if (int rc = next_timing_slot(c, &ev)) return rc;
         TE_CUDA(cudaEventRecord(ev->a, c->stream));
       }
-      int rc = te::launch_chain_fused(c->fused, v, d, nmaps, elev, om, (unsigned*)c->worklist.p, cnt, (unsigned)cap, c->sms, c->stream);
+      int rc = te::launch_chain_fused(c->fused, v, d, nmaps, elev, om, (unsigned*)c->worklist.p, cnt, (unsigned)cap, c->sms, c->stream, mm);
       if (rc != 0) return fail(TE_ERR_CUDA, "fused chain launch failed: %s", c->fused.why.c_str());
       if (int r2 = launch_check(c, "k_chain_fused")) return r2;
       if (c->timing) TE_CUDA(cudaEventRecord(ev->b, c->stream));
       te::FixupArgs fa;
-      te::make_fixup_args(c->fused, v, d, &fa);
+      te::make_fixup_args(c->fused, v, d, mm, &fa);
       // tiers 2 and 3 are programmatic dependent launches unless events are recorded in between (timing): their grids are set
       // up while the predecessor drains and wait on griddepcontrol.wait before they read the lists
       te::launch_fixup_t2(fa, elev, om, (const unsigned*)c->worklist.p, cnt, (unsigned)cap, (unsigned*)c->worklist3.p, cnt + 4,
@@ -464,7 +467,10 @@ int run_chain_device(te_ctx* c, const te_geometry* g, const te::SlabView& v, con
         if (int rc = next_timing_slot(c, &ev)) return rc;
         TE_CUDA(cudaEventRecord(ev->a, c->stream));
       }
-      te::launch_chain_generic(v, d, elev + m * in_stride, om, c->sms, c->stream);
+      te::SlabView vm = v;  // the map's coordinate tables
+      vm.X += (size_t)m * v.xs;
+      vm.Y += (size_t)m * v.ys;
+      te::launch_chain_generic(vm, d, elev + m * in_stride, om, c->sms, c->stream);
       if (int r2 = launch_check(c, "k_chain_generic")) return r2;
       if (c->timing) {
         TE_CUDA(cudaEventRecord(ev->b, c->stream));
@@ -792,8 +798,26 @@ static int chain_host_pipelined(te_ctx* c, Staging& st, const te_geometry* g, co
   return rc;
 }
 
+// The coordinate tables of a launch over maps at their own positions (device, built by map_tables): map k of the launch has X at
+// X + k * rows, Y at Y + k * cols and its position at pos[2k], pos[2k + 1]; masks: its fused mask tables (chain launches).
+struct PosTables {
+  const double* X;
+  const double* Y;
+  const double* pos;
+  double coord_max;  // the largest |cell-centre coordinate| over the maps
+  te::MapMasks masks;
+};
+
+static te::SlabView view_at(te::SlabView v, const te_geometry* g, const PosTables* t) {
+  if (!t) return v;
+  v.X = t->X; v.Y = t->Y; v.xs = g->rows; v.ys = g->cols; v.pos = t->pos;
+  v.coord_max = t->coord_max;
+  return v;
+}
+
 static int chain_common(te_ctx* c, const te_geometry* g_in, const te_slab* slab, const te_chain_params* p, int nmaps, const float* elev,
-                        float* slope, float* step, float* rough, float* trav, float* nx, float* ny, float* nz, int memory) {
+                        float* slope, float* step, float* rough, float* trav, float* nx, float* ny, float* nz, int memory,
+                        const PosTables* tab = nullptr) {
   te_geometry g0;
   if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && slab == nullptr && nmaps == 1, &g0)) return rc;
   const te_geometry* g = &g0;
@@ -812,7 +836,9 @@ static int chain_common(te_ctx* c, const te_geometry* g_in, const te_slab* slab,
   float* o[7];
   for (int k = 0; k < 7; ++k) o[k] = st.out_layer(host_out[k], s.col_count * nmaps);
   if (st.rc) return st.rc;
-  if (int rc = run_chain_device(c, g, make_view(c, g, s), p, din, te::ChainOut{o[0], o[1], o[2], o[3], o[4], o[5], o[6]}, nmaps)) return rc;
+  if (int rc = run_chain_device(c, g, view_at(make_view(c, g, s), g, tab), p, din, te::ChainOut{o[0], o[1], o[2], o[3], o[4], o[5], o[6]},
+                                nmaps, tab ? &tab->masks : nullptr))
+    return rc;
   return st.finish();
 }
 
@@ -1325,12 +1351,138 @@ struct te_map {
   int memo_rough = 0;
   te::MapRequestStats last{};
   bool last_device = false;  // the last request ran in device memory: its counters are on the device (fp.req_counters)
+  // Where each map sits: pos[2m], pos[2m + 1] (te_map_positions).  geo's position for every map unless an _at entry put maps
+  // elsewhere.  spread: the maps do not all sit at one position, so the kernels read per-map tables (map_tables).
+  std::vector<double> pos;
+  bool spread = false;
+  // Per-map device tables (map_tables), cached with what they were built from: tab_all for every map in index order, tab_launch
+  // for a chain launch (with the fused mask tables) or a selection.
+  struct PosTab {
+    std::vector<double> key;
+    double coord_max = 0.0;
+    size_t mask_off = 0;
+    DevBuf buf;
+  } tab_all, tab_launch;
 };
 
 namespace {
 
 size_t map_cells(const te_map* m) { return (size_t)m->geo.rows * m->geo.cols; }
 size_t batch_cells(const te_map* m) { return map_cells(m) * m->nmaps; }  // every map of the te_map
+
+// The maps a _maps entry updates: n distinct indices of the batch, a host array.  The whole-batch entries pass none.
+struct MapSel {
+  int32_t n;
+  const int32_t* idx;
+};
+
+// Validates n (x, y) map positions of an _at entry (null: none given).  Writes nothing.
+int check_positions(const double* xy, int n) {
+  if (!xy) return TE_OK;
+  for (int k = 0; k < 2 * n; ++k)
+    if (!std::isfinite(xy[k])) return fail(TE_ERR_BAD_ARG, "position_xy[%d] (map %d's %c) is not finite", k, k / 2, k % 2 ? 'y' : 'x');
+  return TE_OK;
+}
+
+// The positions of n maps of a launch: position_xy as given, or (x, y) for every map when it is null.
+std::vector<double> launch_positions(const double* xy, int n, double x, double y) {
+  std::vector<double> v(2 * (size_t)n);
+  for (int k = 0; k < n; ++k) {
+    v[2 * k] = xy ? xy[2 * k] : x;
+    v[2 * k + 1] = xy ? xy[2 * k + 1] : y;
+  }
+  return v;
+}
+
+// Whether every one of the n positions xy is (x, y), bit for bit.
+bool all_at(const double* xy, int n, double x, double y) {
+  for (int k = 0; k < n; ++k)
+    if (std::memcmp(xy + 2 * k, &x, sizeof(double)) != 0 || std::memcmp(xy + 2 * k + 1, &y, sizeof(double)) != 0) return false;
+  return true;
+}
+
+// The geometry the kernels see when every map of the te_map sits at one position: the te_map's, at that position.  False when the
+// maps are spread over several positions (the per-map tables then apply).
+bool map_geometry(const te_map* m, te_geometry* g) {
+  if (m->spread) return false;
+  *g = m->geo;
+  if (!m->pos.empty()) { g->position_x = m->pos[0]; g->position_y = m->pos[1]; }
+  return true;
+}
+// The same with the start index of the layers as they came (geo_in).
+te_geometry map_geometry_in(const te_map* m) {
+  te_geometry g = m->geo_in;
+  if (!m->pos.empty()) { g.position_x = m->pos[0]; g.position_y = m->pos[1]; }
+  return g;
+}
+
+// Device tables of n maps of geometry g at the positions xy (2n doubles, launch order): the cell-centre coordinates (X: n * rows,
+// Y: n * cols, as getPositionFromIndex gives them at each map's position) and the positions, plus for a chain launch (p set) the
+// fused mask tables of every map.  Cached in t while the geometry, the positions and the step radii stay the same; a rebuild is
+// ordered after the kernels that may still read the old tables.
+int map_tables(te_ctx* c, te_map::PosTab& t, const te_geometry& g, const double* xy, int n, const te_chain_params* p, PosTables* out) {
+  const double none = std::numeric_limits<double>::quiet_NaN();
+  std::vector<double> key = {(double)g.rows, (double)g.cols, g.resolution, g.length_x, g.length_y,
+                             p ? p->step_first_radius : none, p ? p->step_second_radius : none};
+  key.insert(key.end(), xy, xy + 2 * (size_t)n);
+  const size_t R = g.rows, C = g.cols;
+  const size_t dbytes = sizeof(double) * ((R + C) * n + 2 * (size_t)n);
+  if (!t.buf.p || t.key.size() != key.size() || std::memcmp(t.key.data(), key.data(), sizeof(double) * key.size()) != 0) {
+    std::vector<double> h((R + C) * n + 2 * (size_t)n);
+    double cmax = 0.0;
+    for (int k = 0; k < n; ++k) {
+      const double px = xy[2 * k], py = xy[2 * k + 1];
+      for (size_t i = 0; i < R; ++i) h[k * R + i] = cell_coord(px, g.length_x, g.resolution, (int)i);
+      for (size_t j = 0; j < C; ++j) h[R * n + k * C + j] = cell_coord(py, g.length_y, g.resolution, (int)j);
+      h[(R + C) * n + 2 * k] = px;
+      h[(R + C) * n + 2 * k + 1] = py;
+      cmax = std::max(cmax, std::max(std::fabs(px) + 0.5 * g.length_x, std::fabs(py) + 0.5 * g.length_y));
+    }
+    std::vector<unsigned char> mk;
+    if (p) {
+      mk.resize((R + C) * n);
+      for (int k = 0; k < n; ++k) {
+        te::fused_mask_bits(p, h.data() + k * R, (int)R, mk.data() + k * R);
+        te::fused_mask_bits(p, h.data() + R * n + k * C, (int)C, mk.data() + R * n + k * C);
+      }
+    }
+    const size_t bytes = dbytes + mk.size();
+    if (t.buf.p && t.buf.cap < bytes) TE_CUDA(cudaStreamSynchronize(c->stream));  // earlier kernels may still read the tables
+    TE_CUDA(t.buf.reserve(bytes));
+    // pageable sources: consumed before cudaMemcpyAsync returns, ordered after the kernels queued before on the stream
+    TE_CUDA(cudaMemcpyAsync(t.buf.p, h.data(), dbytes, cudaMemcpyHostToDevice, c->stream));
+    if (!mk.empty()) TE_CUDA(cudaMemcpyAsync((char*)t.buf.p + dbytes, mk.data(), mk.size(), cudaMemcpyHostToDevice, c->stream));
+    t.key = std::move(key);
+    t.coord_max = cmax;
+    t.mask_off = dbytes;
+  }
+  const double* base = (const double*)t.buf.p;
+  out->X = base;
+  out->Y = base + R * n;
+  out->pos = base + (R + C) * n;
+  out->coord_max = t.coord_max;
+  const unsigned char* mk = p ? (const unsigned char*)t.buf.p + t.mask_off : nullptr;
+  out->masks = te::MapMasks{mk, mk ? mk + R * n : nullptr, (unsigned)R, (unsigned)C};
+  return TE_OK;
+}
+
+// The tables of the maps s.idx[0..s.n) (idx null: every map, in index order) at their positions.
+int map_tables_of(te_map* m, const MapSel& s, PosTables* out) {
+  if (!s.idx) return map_tables(m->ctx, m->tab_all, m->geo, m->pos.data(), m->nmaps, nullptr, out);
+  std::vector<double> xy(2 * (size_t)s.n);
+  for (int k = 0; k < s.n; ++k) { xy[2 * k] = m->pos[2 * s.idx[k]]; xy[2 * k + 1] = m->pos[2 * s.idx[k] + 1]; }
+  return map_tables(m->ctx, m->tab_launch, m->geo, xy.data(), s.n, nullptr, out);
+}
+
+// Records where the maps of an update now sit: every map (idx null) or the maps idx[0..n) at the launch positions xy.
+void map_place(te_map* m, const int32_t* idx, int n, const std::vector<double>& xy) {
+  if (!idx) {
+    m->pos = xy;
+  } else {
+    for (int k = 0; k < n; ++k) { m->pos[2 * idx[k]] = xy[2 * k]; m->pos[2 * idx[k] + 1] = xy[2 * k + 1]; }
+  }
+  m->spread = !all_at(m->pos.data(), m->nmaps, m->pos[0], m->pos[1]);
+}
 
 int map_ready(const te_map* m) {
   if (!m->have_layers) return fail(TE_ERR_BAD_ARG, "the map has no layers yet: call te_map_chain or te_map_set_layers first");
@@ -1456,15 +1608,9 @@ int map_layers(te_map* m, uint32_t mask, bool with_range, const float* out[kLaye
   return TE_OK;
 }
 
-// The maps a _maps entry updates: n distinct indices of the batch, a host array.  The whole-batch entries pass none.
-struct MapSel {
-  int32_t n;
-  const int32_t* idx;
-};
-
 // Validates a selection on a te_map that has layers and, when the entry takes one (with_geometry), g against the batch's
-// geometry.  Writes nothing.
-int map_select(const te_map* m, bool with_geometry, const te_geometry* g, const MapSel& s) {
+// geometry; any_position: except its position (the _at entries).  Writes nothing.
+int map_select(const te_map* m, bool with_geometry, const te_geometry* g, const MapSel& s, bool any_position = false) {
   if (int rc = map_ready(m)) return rc;
   if (with_geometry) {
     if (int rc = check_geometry(g, true)) return rc;
@@ -1474,8 +1620,12 @@ int map_select(const te_map* m, bool with_geometry, const te_geometry* g, const 
   }
   if (m->geo_in.start_row != 0 || m->geo_in.start_col != 0)
     return fail(TE_ERR_UNSUPPORTED, "the te_map's layers came with a circular-buffer start index: use te_map_chain / te_map_set_layers");
-  if (with_geometry && std::memcmp(g, &m->geo, sizeof(te_geometry)) != 0)
-    return fail(TE_ERR_BAD_ARG, "the geometry differs from the te_map's: reload the whole batch to change it");
+  if (with_geometry) {
+    te_geometry gc = *g;
+    if (any_position) { gc.position_x = m->geo.position_x; gc.position_y = m->geo.position_y; }
+    if (std::memcmp(&gc, &m->geo, sizeof(te_geometry)) != 0)
+      return fail(TE_ERR_BAD_ARG, "the geometry differs from the te_map's: reload the whole batch to change it");
+  }
   if (s.n < 1 || s.n > m->nmaps) return fail(TE_ERR_BAD_ARG, "nsel = %d: need 1..%d", s.n, m->nmaps);
   if (!s.idx) return fail(TE_ERR_BAD_ARG, "map_index is null");
   std::vector<char> seen(m->nmaps, 0);
@@ -1560,6 +1710,8 @@ int te_map_destroy(te_map* m) {
         b->release();
       for (DevBuf& b : m->sel) b.release();
       for (DevBuf& b : m->carry) b.release();
+      m->tab_all.buf.release();
+      m->tab_launch.buf.release();
       m->fp.release();
     }
   }
@@ -1630,20 +1782,23 @@ int map_convert_image(te_map* m, const te_geometry& g, const ImageIn& im, int bp
 // te_map_chain (nmaps = 1), te_map_chain_batched and, with a selection, te_map_chain_maps, from an elevation layer or from images
 // (te_map_chain_image(_maps)): the selected maps' layers are chained into scratch (the elevation staged there in host memory,
 // read in place in device memory; images converted there in both) and k_map_slots puts them in place.
+// at: an _at entry, whose maps go to position_xy (null: g's position) and whose g may differ from the batch's in its position.
 int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int nmaps, const ElevSource& src, float* slope, float* step,
-              float* rough, float* trav, int memory, const MapSel* sel = nullptr) {
+              float* rough, float* trav, int memory, const MapSel* sel = nullptr, bool at = false, const double* position_xy = nullptr) {
   te_ctx* c = m->ctx;
   te_geometry g0;
   if (src.image && g_in && (g_in->start_row != 0 || g_in->start_col != 0))
     return fail(TE_ERR_UNSUPPORTED, "circular-buffer start index (%d,%d) != (0,0): an image map has none", g_in->start_row, g_in->start_col);
   if (sel) {
-    if (int rc = map_select(m, true, g_in, *sel)) return rc;
+    if (int rc = map_select(m, true, g_in, *sel, at)) return rc;
     g0 = m->geo;
     nmaps = sel->n;
   } else if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) {
     return rc;
   }
   if (int rc = check_params(p)) return rc;
+  if (nmaps > 0)
+    if (int rc = check_positions(position_xy, nmaps)) return rc;
   if (!src.layer && !src.image) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
   if (sel && (m->have_rslope || !m->have_rough))
     return fail(TE_ERR_UNSUPPORTED, "the batch %s, and te_map_chain_maps gives a map roughness and no robot_slope: every map of a batch holds "
@@ -1674,9 +1829,16 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
     if (int rc = map_convert_image(m, g0, *src.image, bpp, nmaps, memory, (float*)lay[0]->p)) return rc;
     din = (const float*)lay[0]->p;
   }
+  // where the launch's maps go; maps away from g0's position take per-map tables
+  const std::vector<double> at_xy = launch_positions(position_xy, nmaps, g_in->position_x, g_in->position_y);
+  PosTables tab{};
+  const bool spread = !all_at(at_xy.data(), nmaps, g0.position_x, g0.position_y);
+  if (spread)
+    if (int rc = map_tables(c, m->tab_launch, g0, at_xy.data(), nmaps, p, &tab)) return rc;
   if (int rc = chain_common(c, &g0, nullptr, p, nmaps, din, (float*)lay[1]->p, (float*)lay[2]->p, (float*)lay[3]->p, (float*)lay[4]->p,
-                            nullptr, nullptr, nullptr, TE_MEM_DEVICE))
+                            nullptr, nullptr, nullptr, TE_MEM_DEVICE, spread ? &tab : nullptr))
     return rc;
+  map_place(m, sel ? sel->idx : nullptr, nmaps, at_xy);
   if (sel) {
     const float* const src_l[te::kMapSlotLayers] = {(const float*)lay[4]->p, (const float*)lay[1]->p, (const float*)lay[2]->p,
                                                     (const float*)lay[3]->p, din, nullptr};
@@ -1701,14 +1863,19 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
 // layers (staged in host memory, read in place in device memory) go to their slots in one k_map_slots launch.  The optional
 // layers must then be those the batch holds.
 int map_set_layers(te_map* m, const te_geometry* g_in, int nmaps, const float* trav, const float* slope, const float* step,
-                   const float* rough, const float* elev, const float* robot_slope, int memory, const MapSel* sel = nullptr) {
+                   const float* rough, const float* elev, const float* robot_slope, int memory, const MapSel* sel = nullptr,
+                   bool at = false, const double* position_xy = nullptr) {
   te_ctx* c = m->ctx;
   te_geometry g0;
   if (sel) {
-    if (int rc = map_select(m, true, g_in, *sel)) return rc;
+    if (int rc = map_select(m, true, g_in, *sel, at)) return rc;
+    nmaps = sel->n;
   } else if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) {
     return rc;
   }
+  if (nmaps > 0)
+    if (int rc = check_positions(position_xy, nmaps)) return rc;
+  const std::vector<double> at_xy = launch_positions(position_xy, std::max(nmaps, 0), g_in->position_x, g_in->position_y);
   if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
   if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
   if (!step) return fail(TE_ERR_MISSING_LAYER, "layer traversability_step is missing");
@@ -1736,6 +1903,7 @@ int map_set_layers(te_map* m, const te_geometry* g_in, int nmaps, const float* t
           src[l] = (const float*)m->sel[l].p;
         }
     if (int rc = map_put_selected(m, *sel, src, dst)) return rc;
+    map_place(m, sel->idx, sel->n, at_xy);
     if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));  // the caller may reuse its layers on return
     return TE_OK;
   }
@@ -1750,6 +1918,7 @@ int map_set_layers(te_map* m, const te_geometry* g_in, int nmaps, const float* t
     if (int rc = map_put_layer(m, m->rslope, robot_slope, memory)) return rc;
   m->have_rough = rough != nullptr;
   m->have_rslope = robot_slope != nullptr;
+  map_place(m, nullptr, nmaps, at_xy);
   if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));  // the caller may reuse its layers on return
   m->have_layers = true;
   return TE_OK;
@@ -1786,6 +1955,41 @@ int te_map_chain_maps(te_map* m, const te_geometry* g, const te_chain_params* p,
   TE_MAP_ENTER(m);
   const MapSel sel{nsel, map_index};
   return map_chain(m, g, p, nsel, ElevSource{elev, nullptr}, slope, step, rough, trav, memory, &sel);
+}
+
+int te_map_chain_batched_at(te_map* m, const te_geometry* g, const te_chain_params* p, int32_t nmaps, const float* elev, float* slope,
+                            float* step, float* rough, float* trav, int memory, const double* position_xy) {
+  TE_MAP_ENTER(m);
+  return map_chain(m, g, p, nmaps, ElevSource{elev, nullptr}, slope, step, rough, trav, memory, nullptr, true, position_xy);
+}
+
+int te_map_set_layers_batched_at(te_map* m, const te_geometry* g, int32_t nmaps, const float* trav, const float* slope, const float* step,
+                                 const float* rough, const float* elev, const float* robot_slope, int memory, const double* position_xy) {
+  TE_MAP_ENTER(m);
+  return map_set_layers(m, g, nmaps, trav, slope, step, rough, elev, robot_slope, memory, nullptr, true, position_xy);
+}
+
+int te_map_chain_maps_at(te_map* m, const te_geometry* g, const te_chain_params* p, int32_t nsel, const int32_t* map_index,
+                         const float* elev, float* slope, float* step, float* rough, float* trav, int memory, const double* position_xy) {
+  TE_MAP_ENTER(m);
+  const MapSel sel{nsel, map_index};
+  return map_chain(m, g, p, nsel, ElevSource{elev, nullptr}, slope, step, rough, trav, memory, &sel, true, position_xy);
+}
+
+int te_map_set_layers_maps_at(te_map* m, const te_geometry* g, int32_t nsel, const int32_t* map_index, const float* trav,
+                              const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                              int memory, const double* position_xy) {
+  TE_MAP_ENTER(m);
+  const MapSel sel{nsel, map_index};
+  return map_set_layers(m, g, nsel, trav, slope, step, rough, elev, robot_slope, memory, &sel, true, position_xy);
+}
+
+int te_map_positions(te_map* m, double* position_xy) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (!position_xy) return fail(TE_ERR_BAD_ARG, "position_xy is null");
+  std::memcpy(position_xy, m->pos.data(), sizeof(double) * m->pos.size());
+  return TE_OK;
 }
 
 int te_image_geometry(int32_t height, int32_t width, double resolution, double position_x, double position_y, te_geometry* out) {
@@ -1919,9 +2123,15 @@ static int map_footprint(te_map* m, const te_footprint_params* p, const MapSel* 
   if (int rc = sel ? map_select(m, false, nullptr, *sel) : map_ready(m)) return rc;
   if (int rc = map_footprint_params(m, p)) return rc;
   if (!(p->radius >= 0.0) || !(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint radius/offset must be >= 0");
-  const te_geometry* g = &m->geo;
+  te_geometry gm;
+  PosTables tab{};
+  const bool spread = !map_geometry(m, &gm);  // the maps at several positions: their own tables
+  if (spread) gm = m->geo;
+  const te_geometry* g = &gm;
   if (int rc = ensure_geometry(c, g)) return rc;
   const int n = sel ? sel->n : m->nmaps;
+  if (spread)
+    if (int rc = map_tables_of(m, MapSel{n, sel ? sel->idx : nullptr}, &tab)) return rc;
   TE_CUDA(m->fresh.reserve(sizeof(float) * map_cells(m) * n));
   const te_slab s{0, g->cols, 0, 0};
   // trav, slope, step, rough (verify_roughness only), elev: resident, or gathered for the selection
@@ -1946,8 +2156,8 @@ static int map_footprint(te_map* m, const te_footprint_params* p, const MapSel* 
     ++fixed;
   }
   int nl = 0;
-  int rc = te::launch_footprint(m->fp, make_view(c, g, s), g, p, n, in[0], in[1], in[2], in[3], in[4], (float*)m->fresh.p, nullptr,
-                                nullptr, nullptr, c->sms, c->stream, &nl);
+  int rc = te::launch_footprint(m->fp, view_at(make_view(c, g, s), g, spread ? &tab : nullptr), g, p, n, in[0], in[1], in[2], in[3], in[4],
+                                (float*)m->fresh.p, nullptr, nullptr, nullptr, c->sms, c->stream, &nl);
   if (rc != 0) return fail(rc, "footprint sweep failed: %s", m->fp.why.c_str());
   // host memory: the whole cache is read back from its resident layer, a selection's from packed scratch (its trav slot)
   float* const dout = !out ? nullptr : memory == TE_MEM_DEVICE ? out : sel ? (float*)m->sel[0].p : nullptr;
@@ -1979,7 +2189,37 @@ static int map_footprint_polygon(te_map* m, const te_footprint_params* p, int32_
                                  const PolygonOutputs* outs, const te::PolygonReduce* reduce, int memory) {
   if (int rc = map_ready(m)) return rc;
   if (int rc = map_footprint_params(m, p)) return rc;
-  return footprint_polygon_common(m->ctx, &m->fp, &m->geo_in, nullptr, p, m->nmaps, npts, pts_xy, (const float*)m->trav.p, (const float*)m->slope.p,
+  if (m->spread) {
+    // Maps at several positions: the sweep classifies the polygon's offsets against absolute positions on the host, so each map
+    // is swept on its own geometry (one sweep per map, every output in the batch's layout).  Map m's layers and its layer of
+    // each output start m * rows * cols floats in; layer y of a list of yaws is at (y * nmaps + m) * rows * cols.
+    const size_t cells = map_cells(m);
+    const float* rough = m->have_rough ? (const float*)m->rough.p : nullptr;
+    for (int mi = 0; mi < m->nmaps; ++mi) {
+      te_geometry g = m->geo;
+      g.position_x = m->pos[2 * mi];
+      g.position_y = m->pos[2 * mi + 1];
+      std::vector<PolygonOutputs> om;
+      for (int k = 0; k < nouts; ++k)
+        for (int y = 0; y < outs[k].count; ++y)
+          om.push_back(PolygonOutputs{outs[k].out ? outs[k].out + (y * (size_t)m->nmaps + mi) * cells : nullptr, 1, outs[k].yaws + y});
+      te::PolygonReduce rm{};
+      if (reduce)
+        rm = te::PolygonReduce{reduce->worst ? reduce->worst + mi * cells : nullptr, reduce->best ? reduce->best + mi * cells : nullptr,
+                               reduce->best_yaw ? reduce->best_yaw + mi * cells : nullptr};
+      // the reductions run over the yaws of one output: keep it one output of every yaw
+      const PolygonOutputs one{nullptr, reduce ? outs[0].count : 0, reduce ? outs[0].yaws : nullptr};
+      const size_t o = mi * cells;
+      if (int rc = footprint_polygon_common(m->ctx, &m->fp, &g, nullptr, p, 1, npts, pts_xy, (const float*)m->trav.p + o,
+                                            (const float*)m->slope.p + o, (const float*)m->step.p + o, rough ? rough + o : nullptr,
+                                            (const float*)m->elev.p + o, reduce ? 1 : (int)om.size(), reduce ? &one : om.data(),
+                                            reduce ? &rm : nullptr, memory, true))
+        return rc;
+    }
+    return TE_OK;
+  }
+  const te_geometry g = map_geometry_in(m);
+  return footprint_polygon_common(m->ctx, &m->fp, &g, nullptr, p, m->nmaps, npts, pts_xy, (const float*)m->trav.p, (const float*)m->slope.p,
                                   (const float*)m->step.p, m->have_rough ? (const float*)m->rough.p : nullptr, (const float*)m->elev.p,
                                   nouts, outs, reduce, memory, true);
 }
@@ -2014,14 +2254,21 @@ int te_map_footprint_polygon_yaws_reduce(te_map* m, const te_footprint_params* p
 // The work-list entries launch_map_request_device needs at most for the circular paths of a validated host request: the count of
 // req_pose_entries_d with every checkInclination gate counted when the map has robot_slope, so that no path is cut.  It walks no
 // line.  *circles: whether the request has a circular path.
+// map_pos: the maps' own positions (x, y per map; path q on map path_map[q], or map 0), or null: every map at g's.
 static long long map_request_checks(const te_geometry* g, bool rslope, int32_t npaths, const int32_t* path_begin, const double* poses,
-                                    const int32_t* footprint_begin, bool* circles) {
-  const te::GridGeo G{g->rows, g->cols, g->resolution, g->length_x, g->length_y, g->position_x, g->position_y};
+                                    const int32_t* footprint_begin, bool* circles, const int32_t* path_map = nullptr,
+                                    const double* map_pos = nullptr) {
+  te::GridGeo G{g->rows, g->cols, g->resolution, g->length_x, g->length_y, g->position_x, g->position_y};
   long long total = 0;
   *circles = false;
   for (int32_t q = 0; q < npaths; ++q) {
     if (footprint_begin[q + 1] != footprint_begin[q]) continue;  // polygonal
     *circles = true;
+    if (map_pos) {
+      const int32_t mq = path_map ? path_map[q] : 0;
+      G.posx = map_pos[2 * mq];
+      G.posy = map_pos[2 * mq + 1];
+    }
     const int32_t b = path_begin[q], n = path_begin[q + 1] - b;
     for (int32_t k = n == 1 ? 0 : 1; k < n; ++k) {  // pose 0 of a longer path adds nothing
       const double* e = poses + 7 * (size_t)(b + k);
@@ -2061,7 +2308,10 @@ static int map_request(te_map* m, const te_footprint_params* p, const int32_t* p
   m->last = te::MapRequestStats{};
   m->last_device = false;
   if (npaths == 0) return TE_OK;
-  const te_geometry* g = &m->geo;
+  te_geometry gm;
+  const bool spread = !map_geometry(m, &gm);  // the maps at several positions: the kernels read each map's tables
+  if (spread) gm = m->geo;
+  const te_geometry* g = &gm;
   // the hull input bound of a polygonal item: as te_check_footprint_request; host memory sizes it from the paths
   int mp = conservative && max_footprint_vertices > 0 ? 2 * te::kPolyConsCap : 2 * std::max(max_footprint_vertices, 1);
   bool circles = true;  // device memory cannot tell: the circular kernels run and find none
@@ -2069,13 +2319,17 @@ static int map_request(te_map* m, const te_footprint_params* p, const int32_t* p
     if (int rc = check_request_host(g, p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
                                     max_footprint_vertices, conservative, &mp))
       return rc;
-    max_checks = map_request_checks(g, m->have_rslope, npaths, path_begin, poses, footprint_begin, &circles);
+    max_checks = map_request_checks(g, m->have_rslope, npaths, path_begin, poses, footprint_begin, &circles, path_map,
+                                    spread ? m->pos.data() : nullptr);
     if (max_checks > (1LL << 30))
       return fail(TE_ERR_UNSUPPORTED, "the circular paths need %lld circle checks, more than 2^30", max_checks);
   }
   if (int rc = ensure_geometry(c, g)) return rc;
   if (int rc = map_memo(m, p)) return rc;
-  const te::SlabView v = make_view(c, g, te_slab{0, g->cols, 0, 0});
+  PosTables tab{};
+  if (spread)
+    if (int rc = map_tables_of(m, MapSel{m->nmaps, nullptr}, &tab)) return rc;
+  const te::SlabView v = view_at(make_view(c, g, te_slab{0, g->cols, 0, 0}), g, spread ? &tab : nullptr);
   const float* rough = p->verify_roughness ? (const float*)m->rough.p : nullptr;
   const float* rslope = m->have_rslope ? (const float*)m->rslope.p : nullptr;
   te::PathChecks r{};
@@ -2189,8 +2443,9 @@ namespace {
 
 // te_submap_geometry's records of `n` windows on the map `g` (its start index changes nothing: te::grid_submap), with offsets for
 // `nlayers` layers per window; *total receives the floats they take.  Every window is checked before any record is written.
+// map_pos: the position of window k's map is map_pos[2 * win_map[k]], map_pos[... + 1] (null: g's for every window).
 int submap_windows(const te_geometry* g, int32_t n, const double* pos, const double* len, int nlayers, te_submap_info* info,
-                   int64_t* total) {
+                   int64_t* total, const int32_t* win_map = nullptr, const double* map_pos = nullptr) {
   if (n < 0) return fail(TE_ERR_BAD_ARG, "negative window count");
   if (n > 0 && (!pos || !len || !info)) return fail(TE_ERR_BAD_ARG, "null argument");
   for (int32_t k = 0; k < n; ++k) {  // the reference does not validate these; a negative length would make negative-sized blocks
@@ -2203,7 +2458,13 @@ int submap_windows(const te_geometry* g, int32_t n, const double* pos, const dou
   for (int32_t k = 0; k < n; ++k) {
     te_submap_info r{};
     te::SubmapGeo s{};
-    if (te::grid_submap(A, pos[2 * k], pos[2 * k + 1], len[2 * k], len[2 * k + 1], s)) {
+    te::GridGeo Ak = A;
+    if (map_pos) {
+      const int32_t mk = win_map ? win_map[k] : 0;
+      Ak.posx = map_pos[2 * mk];
+      Ak.posy = map_pos[2 * mk + 1];
+    }
+    if (te::grid_submap(Ak, pos[2 * k], pos[2 * k + 1], len[2 * k], len[2 * k + 1], s)) {
       r.success = 1;
       r.rows = s.rows; r.cols = s.cols; r.top_row = s.top_row; r.top_col = s.top_col;
       r.requested_row = s.req_row; r.requested_col = s.req_col;
@@ -2257,7 +2518,7 @@ static int map_submaps(te_map* m, int32_t nwin, const int32_t* win_map, const do
   int nl = 0;
   if (int rc = map_layers(m, layer_mask, false, src, &nl)) return rc;
   int64_t total = 0;
-  if (int rc = submap_windows(&m->geo, nwin, position_xy, length_xy, nl, info, &total)) return rc;
+  if (int rc = submap_windows(&m->geo, nwin, position_xy, length_xy, nl, info, &total, win_map, m->pos.data())) return rc;
   if (out_capacity < total)
     return fail(TE_ERR_BAD_ARG, "the submaps take %lld floats but out holds %lld: call again with more room", (long long)total,
                 (long long)out_capacity);
@@ -2317,9 +2578,15 @@ static int map_valid_at(te_map* m, int32_t n, const int32_t* pos_map, const doub
   const int32_t* dmap = st.in(pos_map, (size_t)n);
   uint8_t* dvalid = st.out(valid, (size_t)n);
   if (st.rc) return st.rc;
-  const te_geometry& g = m->geo;
+  te_geometry g;
+  PosTables tab{};
+  const bool spread = !map_geometry(m, &g);  // the maps at several positions: the kernel takes each map's
+  if (spread) {
+    g = m->geo;
+    if (int rc = map_tables_of(m, MapSel{m->nmaps, nullptr}, &tab)) return rc;
+  }
   te::launch_valid_at(te::GridGeo{g.rows, g.cols, g.resolution, g.length_x, g.length_y, g.position_x, g.position_y},
-                      (const float*)m->trav.p, n, dxy, dmap, m->nmaps, dvalid, c->stream);
+                      (const float*)m->trav.p, n, dxy, dmap, m->nmaps, spread ? tab.pos : nullptr, dvalid, c->stream);
   if (int rc = launch_check(c, "k_map_valid_at")) return rc;
   return st.finish();
 }

@@ -19,7 +19,11 @@ struct SlabView {
   const double* Y;  // [cols_total]
   double res;
   double coord_max;  // largest |cell-centre coordinate| of the global map (host-side use: error bounds of the reference's
-                     // absolute-coordinate arithmetic)
+                     // absolute-coordinate arithmetic); of every map of a batch at per-map positions
+  // A batch whose maps sit at their own positions (a te_map given positions): map m's tables start m * xs entries into X and
+  // m * ys into Y, and its position is pos[2m], pos[2m + 1].  xs = ys = 0 and pos = nullptr: every map at the one position.
+  int xs, ys;
+  const double* pos;
 };
 
 // Chain parameters in the form the kernels want them.

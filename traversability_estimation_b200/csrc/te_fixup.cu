@@ -329,7 +329,14 @@ __global__ void __launch_bounds__(128, 8) k_fixup_t2(FixupArgs A, const float* _
       r = o.rough[c];
     }
     if (do_s) {
-      t = step_t2(A, E, i, j);
+      if (A.rowmask_stride | A.colmask_stride) {  // the maps sit at their own positions: the cell's map's masks
+        FixupArgs Am = A;
+        Am.rowmask += (size_t)mapi * A.rowmask_stride;
+        Am.colmask += (size_t)mapi * A.colmask_stride;
+        t = step_t2(Am, E, i, j);
+      } else {
+        t = step_t2(A, E, i, j);
+      }
       o.step[c] = t;
     } else {
       t = o.step[c];

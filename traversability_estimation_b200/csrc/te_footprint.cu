@@ -60,6 +60,8 @@ __global__ void __launch_bounds__(256) k_pred_classify(FpArgs A, Layers L, unsig
   }
 }
 
+// AT: the maps sit at their own positions (FpArgs::pos); the shared-position instantiation reads A as it always did.
+template <bool AT>
 __global__ void __launch_bounds__(128) k_pred_heavy(FpArgs A, Layers L, unsigned char* __restrict__ blocked, float* slope_fp, float* step_fp,
                                                     float* rough_fp, const unsigned* __restrict__ list, const unsigned* __restrict__ count) {
   const unsigned n = *count;
@@ -71,7 +73,9 @@ __global__ void __launch_bounds__(128) k_pred_heavy(FpArgs A, Layers L, unsigned
     const int j = A.in_col0 + (int)(col - m * (unsigned)A.in_ncols);
     const size_t mc = (size_t)m * A.in_ncols * A.rows;    // the map's first cell: filters_d reads its layers only
     const Layers Lm{L.trav + mc, L.slope + mc, L.step + mc, L.elev + mc, L.rough ? L.rough + mc : nullptr};
-    const FilterVerdict v = filters_d(A, Lm, i, j);
+    FilterVerdict v;
+    if constexpr (AT) v = filters_d(map_args_d(A, m), Lm, i, j);
+    else v = filters_d(A, Lm, i, j);
     blocked[c] = v.ok ? 0 : 1;
     const int oj = j - A.out_col0;
     if (oj >= 0 && oj < A.out_ncols) {
@@ -83,6 +87,7 @@ __global__ void __launch_bounds__(128) k_pred_heavy(FpArgs A, Layers L, unsigned
   }
 }
 
+template <bool AT>
 __global__ void __launch_bounds__(256) k_sweep(FpArgs A, Layers L, const unsigned char* __restrict__ blocked, float* __restrict__ out) {
   const long long total = (long long)A.rows * A.out_ncols * A.nmaps;
   for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < total; c += (long long)gridDim.x * blockDim.x) {
@@ -91,7 +96,9 @@ __global__ void __launch_bounds__(256) k_sweep(FpArgs A, Layers L, const unsigne
     const unsigned m = col / (unsigned)A.out_ncols;
     const int j = A.out_col0 + (int)(col - m * (unsigned)A.out_ncols);
     const size_t mc = (size_t)m * A.in_ncols * A.rows;  // the map's first input cell
-    const double cx = A.X[i], cy = A.Y[j];
+    const double* const X = AT ? A.X + (size_t)m * A.xs : A.X;  // the map's coordinate tables
+    const double* const Y = AT ? A.Y + (size_t)m * A.ys : A.Y;
+    const double cx = X[i], cy = Y[j];
     int n = 0;
     double t = 0.0;
     float result = nanf_();
@@ -102,7 +109,7 @@ __global__ void __launch_bounds__(256) k_sweep(FpArgs A, Layers L, const unsigne
       const int a = i + di, b = j + dj;
       if (a < 0 || b < 0 || a >= A.rows || b >= A.cols_total) continue;
       if (w & 0x10000) {
-        const double dx = A.X[a] - cx, dy = A.Y[b] - cy;
+        const double dx = X[a] - cx, dy = Y[b] - cy;
         if (!(dx * dx + dy * dy <= A.rmax2)) continue;
       }
       const int lb = b - A.in_col0;
@@ -195,6 +202,7 @@ __global__ void __launch_bounds__(256) k_fp_prepare_p(FpArgs A, Layers L, const 
 // isTraversable for every cell on prefix sums: the visited set is a lattice disk, so "is anything blocked in it"
 // and "sum / count of the visited cells" are 2L+1 column queries instead of ~pi r^2 visits; only when a blocker
 // exists is the ring that holds the first one walked in SpiralIterator order.
+template <bool AT>
 __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const unsigned char* __restrict__ blocked, float* __restrict__ out) {
   const int W = 2 * A.L + 1;
   // one block = 256 consecutive rows of ONE output column (blockIdx.y): a warp's centres share their column, so everything that
@@ -209,7 +217,9 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
     if (i0 >= A.rows) return;  // whole warp beyond the last row
     const bool active = i < A.rows;
     const size_t c = ((unsigned)blockIdx.z * A.out_ncols + blockIdx.y) * (unsigned)A.rows + (active ? i : 0);  // < 2^32
-    const double cx = A.X[active ? i : 0], cy = A.Y[j];
+    const double* const X = AT ? A.X + (size_t)blockIdx.z * A.xs : A.X;  // the map's coordinate tables
+    const double* const Y = AT ? A.Y + (size_t)blockIdx.z * A.ys : A.Y;
+    const double cx = X[active ? i : 0], cy = Y[j];
     // disk columns that exist in the map and in this slab's buffer.  l_lo is written as a negated minimum: ptxas of CUDA 12.9 for
     // sm_90a fuses max(-L, max(-j, in_col0 - j)) into one three-input VIMNMX3 that reads +L, and the loops bounded by l_hi then ran
     // past it whenever the disk is clipped on the right
@@ -241,7 +251,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
         const int di = (int)(signed char)(w & 0xff), dj = (int)(signed char)((w >> 8) & 0xff);
         const int a = i + di, b = j + dj, lb = b - A.in_col0;
         if (a < 0 || b < 0 || a >= A.rows || b >= A.cols_total || lb < 0 || lb >= A.in_ncols) continue;
-        const double dx = A.X[a] - cx, dy = A.Y[b] - cy;
+        const double dx = X[a] - cx, dy = Y[b] - cy;
         if (!(dx * dx + dy * dy <= A.rmax2)) continue;
         if (blocked[(size_t)(mb + lb) * A.rows + a]) best = min(best, di * di + dj * dj);
       }
@@ -307,7 +317,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
         const int di = (int)(signed char)(w & 0xff), dj = (int)(signed char)((w >> 8) & 0xff);
         const int a = i + di, b = j + dj, lb = b - A.in_col0;
         if (a < 0 || b < 0 || a >= A.rows || b >= A.cols_total || lb < 0 || lb >= A.in_ncols) continue;
-        const double dx = A.X[a] - cx, dy = A.Y[b] - cy;
+        const double dx = X[a] - cx, dy = Y[b] - cy;
         if (!(dx * dx + dy * dy <= A.rmax2)) continue;
         const float v = __ldg(L.trav + (size_t)(mb + lb) * A.rows + a);
         t += finitef(v) ? (double)v : A.tdefault;
@@ -325,7 +335,7 @@ __global__ void __launch_bounds__(256) k_sweep_fast(FpArgs A, Layers L, const un
         const int a = i + di, b = j + dj, lb = b - A.in_col0;
         if (a < 0 || b < 0 || a >= A.rows || b >= A.cols_total || lb < 0 || lb >= A.in_ncols) continue;
         if (w & 0x10000) {
-          const double dx = A.X[a] - cx, dy = A.Y[b] - cy;
+          const double dx = X[a] - cx, dy = Y[b] - cy;
           if (!(dx * dx + dy * dy <= A.rmax2)) continue;
         }
         const size_t cc = (size_t)(mb + lb) * A.rows + a;
@@ -375,6 +385,7 @@ FpArgs geometry_args(const SlabView& v, const te_geometry* g) {
   a.out_col0 = v.out_col0; a.out_ncols = v.out_ncols;
   a.res = g->resolution; a.lenx = g->length_x; a.leny = g->length_y; a.posx = g->position_x; a.posy = g->position_y;
   a.X = v.X; a.Y = v.Y;
+  a.xs = v.xs; a.ys = v.ys; a.pos = v.pos;
   return a;
 }
 
@@ -422,7 +433,7 @@ int run_predicates(FootprintState& st, const SlabView& v, const te_geometry* g, 
     cudaMemsetAsync(cnt, 0, sizeof(unsigned), s);
     const dim3 gc((unsigned)((v.rows + 255) / 256), (unsigned)v.in_ncols, (unsigned)nmaps);
     k_pred_classify<<<gc, 256, 0, s>>>(a, L, (unsigned char*)st.block.p, slope_fp, step_fp, rough_fp, lst, cnt);
-    k_pred_heavy<<<std::max(g1, 1), 128, 0, s>>>(a, L, (unsigned char*)st.block.p, slope_fp, step_fp, rough_fp, lst, cnt);
+    (a.pos ? k_pred_heavy<true> : k_pred_heavy<false>)<<<std::max(g1, 1), 128, 0, s>>>(a, L, (unsigned char*)st.block.p, slope_fp, step_fp, rough_fp, lst, cnt);
   }
   *out_args = a;
   return 0;
@@ -453,7 +464,7 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
   const int Lmax = (int)std::floor(rmax / g->resolution + 1e-9);
   const bool fast = Lmax <= 31 && v.out_ncols <= 65535 && std::getenv("TE_FOOTPRINT_BRUTE") == nullptr;
   if (!fast) {
-    k_sweep<<<std::max(g2, 1), 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
+    (a.pos ? k_sweep<true> : k_sweep<false>)<<<std::max(g2, 1), 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
     if (launches) *launches = 3;
     return 0;
   }
@@ -546,7 +557,7 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
   k_fp_prepare_p<<<std::max(g3, 1), 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, (double*)prefix, (unsigned*)(prefix + pbytes));
   k_fp_nearest<<<std::max(g1b, 1), 256, 0, s>>>(a, (unsigned char*)prefix + pbytes + wbytes);
   const dim3 gs((unsigned)((v.rows + 255) / 256), (unsigned)v.out_ncols, (unsigned)nmaps);
-  k_sweep_fast<<<gs, 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
+  (a.pos ? k_sweep_fast<true> : k_sweep_fast<false>)<<<gs, 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
   if (launches) *launches = 5;
   return 0;
 }

@@ -59,6 +59,10 @@ struct FpArgs {
   // m * in_ncols columns into theirs, its outputs m * out_ncols columns into theirs.  The sweep kernels take m from blockIdx.z or
   // decode it from their flat index.  Kept last so that the path-check kernels, which do not read it, keep their parameter layout.
   int nmaps;
+  // maps at their own positions (SlabView::xs / ys / pos): map m's coordinate tables start m * xs entries into X and m * ys into Y,
+  // its position is pos[2m], pos[2m + 1]; xs = ys = 0 and pos null: every map at (posx, posy)
+  int xs, ys;
+  const double* pos;
 };
 
 constexpr int kPathMaxRings = 127;  // the signed-byte packing of the ring table
@@ -104,6 +108,16 @@ __device__ __forceinline__ float lay(const FpArgs& A, const float* l, int i, int
   const int lb = j - A.in_col0;
   if (lb < 0 || lb >= A.in_ncols) return nanf_();
   return __ldg(l + (size_t)lb * A.rows + i);
+}
+
+// The arguments of map m of a batch whose maps sit at their own positions: its coordinate tables and position.
+__device__ __forceinline__ FpArgs map_args_d(const FpArgs& A, unsigned m) {
+  FpArgs a = A;
+  a.X += (size_t)m * A.xs;
+  a.Y += (size_t)m * A.ys;
+  a.posx = A.pos[2 * (size_t)m];
+  a.posy = A.pos[2 * (size_t)m + 1];
+  return a;
 }
 
 __device__ __forceinline__ bool is_inside_d(const FpArgs& A, double px, double py) {

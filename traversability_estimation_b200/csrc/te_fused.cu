@@ -104,6 +104,7 @@ struct FusedArgs {
   float k_one, k_two, k_half, k_1p5, k_0375, k_m03125, k_p0, k_p1, k_p2, k_p3, k_p4, k_p5, k_p6, k_p7;
   const unsigned char* rowmask;  // per global row: bit0/1 pass-1 tips (-2,0)/(+2,0); bit2/3 pass-2 tips
   const unsigned char* colmask;  // per global column, same bits for (0,-2)/(0,+2)
+  unsigned rowmask_stride, colmask_stride;  // map m's masks start m * stride bytes in (0: every map at one position)
   float* slope;
   float* step;
   float* rough;
@@ -486,11 +487,12 @@ __device__ __noinline__ void store_normals(float* pnx, float* pny, float* pnz, b
 // Column tips of a chunk (CH march steps; column `cb` arrives at phase 0).  Lane ph < CH writes the word of phase ph into the
 // padding of the chunk's TMA stage: byte 0/1 = pass-1 tips (0,-2)/(0,+2) of column js = cb + ph - 2, byte 2/3 = pass-2 tips of
 // column jo = cb + ph - 4; 0x00 where the on-circle offset belongs to the window (colmask bit set), 0xff where it does not.
-__device__ __forceinline__ void fill_colmask(const FusedArgs& A, unsigned stage_addr, int cb, int lane) {
+// `colmask` is the unit's map's table.
+__device__ __forceinline__ void fill_colmask(const FusedArgs& A, const unsigned char* colmask, unsigned stage_addr, int cb, int lane) {
   if (lane < CH) {
     const int js = cb + lane - 2, jo = js - 2;
-    const unsigned x = (js >= 0 && js < A.cols_total) ? A.colmask[js] : 0u;
-    const unsigned y = (jo >= 0 && jo < A.cols_total) ? A.colmask[jo] : 0u;
+    const unsigned x = (js >= 0 && js < A.cols_total) ? colmask[js] : 0u;
+    const unsigned y = (jo >= 0 && jo < A.cols_total) ? colmask[jo] : 0u;
     const unsigned w = ((x & 1u) ? 0u : 0xffu) | ((x & 2u) ? 0u : 0xff00u) | ((y & 4u) ? 0u : 0xff0000u) | ((y & 8u) ? 0u : 0xff000000u);
     asm volatile("st.shared.u32 [%0], %1;" ::"r"(stage_addr + STAGE_PAD + lane * 4), "r"(w) : "memory");
   }
@@ -790,9 +792,12 @@ __global__ void __maxnreg__(168) k_chain_fused(const __grid_constant__ CUtensorM
     const int row0 = C.s0 + 2 * lane;
     C.out_len = (lane >= 1 && lane <= 30 && row0 < A.rows) ? (unsigned)(C.q1 - C.q0) : 0u;
     C.oc = (unsigned)mapi * A.map_cells + (unsigned)(C.q0 - A.out_col0 - 8) * (unsigned)A.rows + (unsigned)row0;
+    // the unit's map's mask tables (one per map when the maps sit at their own positions): looked up once per unit
+    const unsigned char* const colmask = A.colmask + (size_t)mapi * A.colmask_stride;
     if constexpr (S::MASKS) {
-      const unsigned rm0 = (row0 >= 0 && row0 < A.rows) ? A.rowmask[row0] : 0u;
-      const unsigned rm1 = (row0 + 1 >= 0 && row0 + 1 < A.rows) ? A.rowmask[row0 + 1] : 0u;
+      const unsigned char* const rowmask = A.rowmask + (size_t)mapi * A.rowmask_stride;
+      const unsigned rm0 = (row0 >= 0 && row0 < A.rows) ? rowmask[row0] : 0u;
+      const unsigned rm1 = (row0 + 1 >= 0 && row0 + 1 < A.rows) ? rowmask[row0 + 1] : 0u;
       const float qn = __int_as_float(0x7fc00000);
       C.tipU1 = mk((rm0 & 1u) ? 0.f : qn, (rm1 & 1u) ? 0.f : qn);
       C.tipD1 = mk((rm0 & 2u) ? 0.f : qn, (rm1 & 2u) ? 0.f : qn);
@@ -811,7 +816,7 @@ __global__ void __maxnreg__(168) k_chain_fused(const __grid_constant__ CUtensorM
       }
     }
     // column masks of the first chunk
-    if constexpr (S::MASKS) fill_colmask(A, ering + (kbase % NST) * STAGE_BYTES, C.q0 - 4, lane);
+    if constexpr (S::MASKS) fill_colmask(A, colmask, ering + (kbase % NST) * STAGE_BYTES, C.q0 - 4, lane);
     for (int kc = 0; kc < nchunks; ++kc) {
       const unsigned st = (kbase + kc) % NST;
       __syncwarp();  // all lanes finished the previous chunk: its predecessor's stage may be refilled
@@ -820,7 +825,7 @@ __global__ void __maxnreg__(168) k_chain_fused(const __grid_constant__ CUtensorM
         mbar_expect_tx(bar0 + 8 * sn, EROWS * CH * 4);
         tma_load_3d(ering + sn * STAGE_BYTES, &map, C.s0 - 2, (C.q0 - 4 + CH * (kc + NST - 2)) - A.in_col0, mapi, bar0 + 8 * sn);
       }
-      if constexpr (S::MASKS) fill_colmask(A, ering + ((kbase + kc + 1) % NST) * STAGE_BYTES, C.q0 - 4 + CH * (kc + 1), lane);  // next chunk's
+      if constexpr (S::MASKS) fill_colmask(A, colmask, ering + ((kbase + kc + 1) % NST) * STAGE_BYTES, C.q0 - 4 + CH * (kc + 1), lane);  // next chunk's
       mbar_wait(bar0 + 8 * st, ((kbase + kc) / NST) & 1u);
       const int t0 = kc * CH;
       march_step<S, 0, KN>(C, L, t0 + 0, st);
@@ -1059,6 +1064,24 @@ void FusedState::release() {
   valid = false;
 }
 
+void fused_mask_bits(const te_chain_params* p, const double* P, int n, unsigned char* out) {
+  const double r1sq = p->step_first_radius * p->step_first_radius, r2sq = p->step_second_radius * p->step_second_radius;
+  for (int i = 0; i < n; ++i) {
+    unsigned b = 0;
+    if (i - 2 >= 0) {
+      const double d = P[i - 2] - P[i];
+      if (d * d + 0.0 <= r1sq) b |= 1u;
+      if (d * d + 0.0 <= r2sq) b |= 4u;
+    }
+    if (i + 2 < n) {
+      const double d = P[i + 2] - P[i];
+      if (d * d + 0.0 <= r1sq) b |= 2u;
+      if (d * d + 0.0 <= r2sq) b |= 8u;
+    }
+    out[i] = (unsigned char)b;
+  }
+}
+
 bool fused_eligible(FusedState& st, const std::vector<double>& X, const std::vector<double>& Y, const te_geometry* g,
                     const te_chain_params* p, cudaStream_t stream) {
   if (st.valid && std::memcmp(&st.key_geo, g, sizeof(*g)) == 0 && std::memcmp(&st.key_par, p, sizeof(*p)) == 0) return st.shape_id >= 0;
@@ -1083,26 +1106,11 @@ bool fused_eligible(FusedState& st, const std::vector<double>& X, const std::vec
   const int id = match_shape(wn, w1, w2);
   if (id < 0) return no("no fused instantiation for these window shapes");
   // on-circle tip membership, decided exactly like CircleIterator does (double, absolute positions)
-  const double r1sq = p->step_first_radius * p->step_first_radius, r2sq = p->step_second_radius * p->step_second_radius;
   std::vector<unsigned char>&rm = st.h_rowmask, &cm = st.h_colmask;  // owned by the state: the uploads below are asynchronous
   rm.assign(g->rows, 0);
   cm.assign(g->cols, 0);
-  auto bits = [&](const std::vector<double>& P, int i, int n) {
-    unsigned b = 0;
-    if (i - 2 >= 0) {
-      const double d = P[i - 2] - P[i];
-      if (d * d + 0.0 <= r1sq) b |= 1u;
-      if (d * d + 0.0 <= r2sq) b |= 4u;
-    }
-    if (i + 2 < n) {
-      const double d = P[i + 2] - P[i];
-      if (d * d + 0.0 <= r1sq) b |= 2u;
-      if (d * d + 0.0 <= r2sq) b |= 8u;
-    }
-    return (unsigned char)b;
-  };
-  for (int i = 0; i < g->rows; ++i) rm[i] = bits(X, i, g->rows);
-  for (int j = 0; j < g->cols; ++j) cm[j] = bits(Y, j, g->cols);
+  fused_mask_bits(p, X.data(), g->rows, rm.data());
+  fused_mask_bits(p, Y.data(), g->cols, cm.data());
   // Kernels of an earlier asynchronous call may still read the tables: the overwrite is ordered after them on the context
   // stream (a reallocation waits for the stream first).
   auto upload = [&](DevBuf& d, const std::vector<unsigned char>& h) {
@@ -1118,7 +1126,7 @@ bool fused_eligible(FusedState& st, const std::vector<double>& X, const std::vec
   return true;
 }
 
-void make_fixup_args(const FusedState& st, const SlabView& v, const ChainDev& p, FixupArgs* out) {
+void make_fixup_args(const FusedState& st, const SlabView& v, const ChainDev& p, const MapMasks* mm, FixupArgs* out) {
   const WindowClass wn = classify(p.rn, v.res), w1 = classify(p.r1, v.res), w2 = classify(p.r2, v.res);
   FixupArgs a{};
   a.rows = v.rows; a.cols_total = v.cols_total; a.in_col0 = v.in_col0; a.in_ncols = v.in_ncols; a.out_col0 = v.out_col0;
@@ -1142,8 +1150,10 @@ void make_fixup_args(const FusedState& st, const SlabView& v, const ChainDev& p,
   a.nz_check = s_check > 2e-4 ? 1.0 - s_check : 0.9998;
   a.nz_guard = std::max(1e-6, 100.0 * 6e-12 * v.coord_max / v.res);
   a.fuse_w = p.fuse_w;
-  a.rowmask = (const unsigned char*)st.rowmask.p;
-  a.colmask = (const unsigned char*)st.colmask.p;
+  a.rowmask = mm ? mm->rowmask : (const unsigned char*)st.rowmask.p;
+  a.colmask = mm ? mm->colmask : (const unsigned char*)st.colmask.p;
+  a.rowmask_stride = mm ? mm->row_stride : 0u;
+  a.colmask_stride = mm ? mm->col_stride : 0u;
   *out = a;
 }
 
@@ -1159,7 +1169,7 @@ const char* fused_launch_obstacle(const SlabView& v, int nmaps, const float* ele
 }
 
 int launch_chain_fused(FusedState& st, const SlabView& v, const ChainDev& p, int nmaps, const float* elev, const ChainOut& o,
-                       unsigned* list, unsigned* count, unsigned cap, int sms, cudaStream_t s) {
+                       unsigned* list, unsigned* count, unsigned cap, int sms, cudaStream_t s, const MapMasks* mm) {
   if (st.shape_id < 0) { st.why = "fused stencil not eligible"; return 1; }
   if (const char* why = fused_launch_obstacle(v, nmaps, elev, o)) { st.why = why; return 1; }
   PFN_encodeTiled enc = get_encode();
@@ -1231,8 +1241,10 @@ int launch_chain_fused(FusedState& st, const SlabView& v, const ChainDev& p, int
   a.k_p0 = B2(1.570796251296997); a.k_p1 = B2(-0.21459604799747467); a.k_p2 = B2(0.08894557505846024);
   a.k_p3 = B2(-0.05000271648168564); a.k_p4 = B2(0.03044925443828106); a.k_p5 = B2(-0.016484638676047325);
   a.k_p6 = B2(0.006254698149859905); a.k_p7 = B2(-0.0011488182935863733);
-  a.rowmask = (const unsigned char*)st.rowmask.p;
-  a.colmask = (const unsigned char*)st.colmask.p;
+  a.rowmask = mm ? mm->rowmask : (const unsigned char*)st.rowmask.p;
+  a.colmask = mm ? mm->colmask : (const unsigned char*)st.colmask.p;
+  a.rowmask_stride = mm ? mm->row_stride : 0u;
+  a.colmask_stride = mm ? mm->col_stride : 0u;
   a.slope = o.slope; a.step = o.step; a.rough = o.rough; a.trav = o.trav;
   a.nx = (o.nx && o.ny && o.nz) ? o.nx : nullptr; a.ny = o.ny; a.nz = o.nz;
   a.list = list; a.count = count; a.cap = cap;

@@ -22,6 +22,18 @@ struct FusedState {
   void release();
 };
 
+// The on-circle tip bits of the mask tables for the n cell-centre coordinates P (one axis of one map), as CircleIterator decides
+// them: bit 0/1 the pass-1 tips at index offsets -2/+2, bit 2/3 the pass-2 tips.
+void fused_mask_bits(const te_chain_params* p, const double* P, int n, unsigned char* out);
+
+// Per-map mask tables of a batch whose maps sit at their own positions (a te_map given positions): map m's row masks start
+// m * row_stride bytes into rowmask, its column masks m * col_stride into colmask.  Device pointers.
+struct MapMasks {
+  const unsigned char* rowmask;
+  const unsigned char* colmask;
+  unsigned row_stride, col_stride;
+};
+
 // True when the fused stencil has an instantiation for these window shapes (fills the tables).
 bool fused_eligible(FusedState& st, const std::vector<double>& X, const std::vector<double>& Y, const te_geometry* g,
                     const te_chain_params* p, cudaStream_t stream);
@@ -46,10 +58,12 @@ struct FixupArgs {
   float fuse_w;
   const unsigned char* rowmask;
   const unsigned char* colmask;
+  unsigned rowmask_stride, colmask_stride;  // map m's masks start m * stride bytes in (0: every map at one position)
 };
 
 // Fills the tier-2 arguments for the shape the fused stencil was found eligible for.
-void make_fixup_args(const FusedState& st, const SlabView& v, const ChainDev& p, FixupArgs* out);
+// mm: per-map masks (null: the state's tables, every map at one position).
+void make_fixup_args(const FusedState& st, const SlabView& v, const ChainDev& p, const MapMasks* mm, FixupArgs* out);
 // pdl: launch as a programmatic dependent of the preceding kernel of the stream (the kernel waits on griddepcontrol.wait)
 void launch_fixup_t2(const FixupArgs& a, const float* elev, const ChainOut& o, const unsigned* list, const unsigned* count,
                      unsigned cap, unsigned* list3, unsigned* count3, unsigned cap3, int sms, cudaStream_t s, bool pdl);
@@ -65,6 +79,6 @@ size_t fused_list_capacity(size_t cells, int sms);
 void fused_plan(int rows, int out_ncols, int nmaps, int sms, int out[19]);
 
 int launch_chain_fused(FusedState& st, const SlabView& v, const ChainDev& p, int nmaps, const float* elev, const ChainOut& o,
-                       unsigned* list, unsigned* count, unsigned cap, int sms, cudaStream_t s);
+                       unsigned* list, unsigned* count, unsigned cap, int sms, cudaStream_t s, const MapMasks* mm = nullptr);
 
 }  // namespace te

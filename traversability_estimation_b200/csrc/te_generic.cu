@@ -406,7 +406,10 @@ __global__ void __launch_bounds__(128) k_fixup_cells(SlabView v, ChainDev p, con
     const size_t off = (size_t)mapi * map_cells;
     om.slope += off; om.step += off; om.rough += off; om.trav += off;
     if (om.nx) { om.nx += off; om.ny += off; om.nz += off; }
-    chain_cell_literal(v, p, elev + (size_t)mapi * v.rows * v.in_ncols, i, j, om, (w >> 30) & 1u, (w >> 31) & 1u, true);
+    SlabView vm = v;  // the cell's map's coordinate tables (the same tables for every map unless the maps sit at their own positions)
+    vm.X += (size_t)mapi * v.xs;
+    vm.Y += (size_t)mapi * v.ys;
+    chain_cell_literal(vm, p, elev + (size_t)mapi * v.rows * v.in_ncols, i, j, om, (w >> 30) & 1u, (w >> 31) & 1u, true);
   }
 }
 

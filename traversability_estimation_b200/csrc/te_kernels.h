@@ -68,9 +68,10 @@ void launch_uncertainty_range(const float* upper, const float* lower, float* out
 struct GridGeo;
 // valid[q] = getIndex(xy[2q], xy[2q+1]) succeeds and traversability is finite there (device pointers; none launched for n = 0).
 // A batch of nmaps maps of geometry g back to back in `trav`: position q is on map pos_map[q] (null: map 0), and a map outside
-// 0 .. nmaps-1 gives 0.
-void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, const int* pos_map, int nmaps, unsigned char* valid,
-                     cudaStream_t s);
+// 0 .. nmaps-1 gives 0.  map_pos (device, 2 * nmaps doubles, or null: every map at g's position): map m sits at map_pos[2m],
+// map_pos[2m + 1] (needs pos_map).
+void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, const int* pos_map, int nmaps, const double* map_pos,
+                     unsigned char* valid, cudaStream_t s);
 
 // te_image.cu — addLayerFromImage for mono images: nmaps row-major images of rows x cols pixels (image m at px + m * image_stride
 // bytes, its row i at + i * row_stride bytes; device memory, 2-byte pixels at even addresses and strides) into nmaps column-major

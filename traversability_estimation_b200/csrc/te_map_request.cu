@@ -34,12 +34,17 @@ struct MapRecord {
 };
 
 // Key k of the request, by the whole warp w of a block of four: its record (k_map_eval_circles_dev).
-__device__ __forceinline__ void map_eval_circle_d(const FpArgs& A, const Layers& L, const PathArgs& P, const MapKey* __restrict__ keys,
+// AT: the maps sit at their own positions (FpArgs::pos), and the walk takes the key's map's tables and position.
+template <bool AT>
+__device__ __forceinline__ void map_eval_circle_d(const FpArgs& A0, const Layers& L, const PathArgs& P, const MapKey* __restrict__ keys,
                                                   int k, const float* __restrict__ cache, MapRecord* __restrict__ recs) {
   __shared__ Layers s_L[4];
   __shared__ PathArgs s_P[4];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const MapKey K = keys[k];
+  FpArgs Am;
+  if constexpr (AT) Am = map_args_d(A0, K.map);
+  const FpArgs& A = AT ? Am : A0;
   MapRecord& R = recs[k];
   // The key's map: its layers, memo and cache start mo cells in.  The walk takes the shifted layer and path arguments from a
   // per-warp copy in shared memory (by reference, as it takes the kernel's own), so no register holds them across the call.
@@ -63,12 +68,13 @@ __device__ __forceinline__ void map_eval_circle_d(const FpArgs& A, const Layers&
 
 // The key count is on the device (*nkeys), so the warps stride over the keys.  The polygons of the failed paths come after the
 // replay (k_req_polygons).
+template <bool AT>
 __global__ void __launch_bounds__(128, 4) k_map_eval_circles_dev(FpArgs A, Layers L, PathArgs P, const MapKey* __restrict__ keys,
                                                               const unsigned long long* __restrict__ nkeys, const float* __restrict__ cache,
                                                               MapRecord* __restrict__ recs) {
   const long long n = (long long)*nkeys;
   for (long long k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; k < n; k += (gridDim.x * blockDim.x) >> 5)  // whole warps
-    map_eval_circle_d(A, L, P, keys, (int)k, cache, recs);
+    map_eval_circle_d<AT>(A, L, P, keys, (int)k, cache, recs);
 }
 
 // traversabilityFootprint(radius, offset) on a cache: a cached cell takes the memoised branch and keeps its value, every other cell
@@ -221,13 +227,18 @@ __global__ void __launch_bounds__(128) k_req_paths(FpArgs A, DevReq D) {
 
 // The entries pose p of a replayed path adds, written to E when E is not null (at most max_checks - off of them).  Returns their
 // count.  Request order: a failed inclination's gate first, then the pose's circle (a single pose) or the segment's cells.
-__device__ long long req_pose_entries_d(const FpArgs& A, const DevReq& D, int p, ReqEntry* E, long long room) {
+// AT: the maps sit at their own positions, and the path's map's tables and position apply.
+template <bool AT>
+__device__ long long req_pose_entries_d(const FpArgs& A0, const DevReq& D, int p, ReqEntry* E, long long room) {
   const int q = req_path_of_d(D, p);
   if (D.status[q] != 1) return 0;
   const int b = D.path_begin[q], n = D.path_begin[q + 1] - b, k = p - b;
   // poses before the first path or after the last belong to no path; the search gives them path 0 or npaths - 1
   if (!(k >= 0 && k < n) || (n > 1 && k == 0)) return 0;
   const int m = D.path_map ? D.path_map[q] : 0;
+  FpArgs Am;
+  if constexpr (AT) Am = map_args_d(A0, m);
+  const FpArgs& A = AT ? Am : A0;
   const float* rslope = D.rslope ? D.rslope + m * D.map_cells : nullptr;
   const double ex = D.poses[7 * (size_t)p], ey = D.poses[7 * (size_t)p + 1];
   const double sx = n > 1 ? D.poses[7 * (size_t)(p - 1)] : ex, sy = n > 1 ? D.poses[7 * (size_t)(p - 1) + 1] : ey;
@@ -262,10 +273,11 @@ __device__ long long req_pose_entries_d(const FpArgs& A, const DevReq& D, int p,
 }
 
 // 1. Count: one thread per pose index (and one more for the scan's total).
+template <bool AT>
 __global__ void __launch_bounds__(128) k_req_count(FpArgs A, DevReq D) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p > D.nposes) return;
-  D.cnt[p] = p < D.nposes ? req_pose_entries_d(A, D, p, nullptr, 0) : 0;
+  D.cnt[p] = p < D.nposes ? req_pose_entries_d<AT>(A, D, p, nullptr, 0) : 0;
 }
 
 // One thread per path after the scan: the capacity cut (a replayed or empty circular path whose entries end past max_checks, and
@@ -311,11 +323,12 @@ __global__ void __launch_bounds__(128) k_req_sorted(DevReq D) {
 }
 
 // 2. List: one thread per sorted pose index writes its entries at its offset.
+template <bool AT>
 __global__ void __launch_bounds__(128) k_req_list(FpArgs A, DevReq D) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= D.nposes || D.skey[i] == kReqNoMap) return;
   const int off = D.lofs[i];
-  req_pose_entries_d(A, D, D.order[i], D.entries + off, D.max_checks - off);
+  req_pose_entries_d<AT>(A, D, D.order[i], D.entries + off, D.max_checks - off);
 }
 
 __device__ __forceinline__ unsigned long long dbits_d(double d) { return (unsigned long long)__double_as_longlong(d); }
@@ -501,7 +514,8 @@ __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* c
 
 // 6. Polygons: one warp per path; a path the replay did not leave a failing circle to publish exits at once.  The pair
 // k_check_paths_fresh_poly calls: fromCircle, or spiral_blockers_d on the failing key and write_cells_polygon_d with its freps.
-__global__ void __launch_bounds__(128, 4) k_req_polygons(FpArgs A, Layers L, PathArgs P, DevReq D, CircleTable C) {
+template <bool AT>
+__global__ void __launch_bounds__(128, 4) k_req_polygons(FpArgs A0, Layers L, PathArgs P, DevReq D, CircleTable C) {
   __shared__ int s_min[4][kFreshTableRows + 1], s_max[4][kFreshTableRows + 1];
   __shared__ int2 s_stack[4][2 * kFreshTableRows + 4];
   __shared__ int2 s_first[4][3];
@@ -518,6 +532,9 @@ __global__ void __launch_bounds__(128, 4) k_req_polygons(FpArgs A, Layers L, Pat
     return;
   }
   const MapKey K = D.keys[F.key];
+  FpArgs Am;  // AT: the key's map's tables and position
+  if constexpr (AT) Am = map_args_d(A0, K.map);
+  const FpArgs& A = AT ? Am : A0;
   const long long mo = (long long)K.map * D.map_cells;
   L = shift_layers_d(L, mo);
   P.memo += mo;
@@ -590,7 +607,9 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
   auto blocks = [](long long n, int per) { return (unsigned)std::max((n + per - 1) / per, 1LL); };
   size_t b1 = cub_bytes, b2 = cub_bytes, b3 = cub_bytes;
   k_req_paths<<<blocks(npaths, 128), 128, 0, s>>>(a, D);
-  k_req_count<<<blocks(nposes + 1, 128), 128, 0, s>>>(a, D);
+  const bool at = a.pos != nullptr;  // maps at their own positions: the instantiations that read each map's tables
+  if (at) k_req_count<true><<<blocks(nposes + 1, 128), 128, 0, s>>>(a, D);
+  else k_req_count<false><<<blocks(nposes + 1, 128), 128, 0, s>>>(a, D);
   cudaError_t e = cub::DeviceScan::ExclusiveSum(tmp, b1, (const long long*)D.cnt, D.gofs, (int)np1, s);
   k_req_cut<<<blocks(npaths, 128), 128, 0, s>>>(D);
   k_req_keys<<<blocks(nsort, 128), 128, 0, s>>>(D);
@@ -598,14 +617,17 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
     e = cub::DeviceRadixSort::SortPairs(tmp, b2, (const unsigned short*)D.pkey, D.skey, (const int*)D.pidx, D.order, nsort, 0, 16, s);
   k_req_sorted<<<blocks(nposes + 1, 128), 128, 0, s>>>(D);
   if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(tmp, b3, (const int*)D.lcnt, D.lofs, (int)np1, s);
-  k_req_list<<<blocks(nposes, 128), 128, 0, s>>>(a, D);
+  if (at) k_req_list<true><<<blocks(nposes, 128), 128, 0, s>>>(a, D);
+  else k_req_list<false><<<blocks(nposes, 128), 128, 0, s>>>(a, D);
   k_req_dedup<<<(unsigned)std::min<long long>(blocks((long long)nc, 256), 8LL * sms), 256, 0, s>>>(D);
-  k_map_eval_circles_dev<<<(unsigned)std::min<long long>(blocks((long long)nc, 4), 16LL * sms), 128, 0, s>>>(
-      a, L, P, D.keys, D.counters + 1, cache, D.recs);
+  const unsigned ge = (unsigned)std::min<long long>(blocks((long long)nc, 4), 16LL * sms);
+  if (at) k_map_eval_circles_dev<true><<<ge, 128, 0, s>>>(a, L, P, D.keys, D.counters + 1, cache, D.recs);
+  else k_map_eval_circles_dev<false><<<ge, 128, 0, s>>>(a, L, P, D.keys, D.counters + 1, cache, D.recs);
   k_req_replay<<<blocks(nmaps, 4), 128, 0, s>>>(a, D, cache);
   *launches = 12;  // nine kernels and three CUB calls, each counted as one launch (a CUB call runs two or more kernels)
   if (r.ucount) {
-    k_req_polygons<<<blocks(npaths, 4), 128, 0, s>>>(a, L, P, D, circle_table());
+    if (at) k_req_polygons<true><<<blocks(npaths, 4), 128, 0, s>>>(a, L, P, D, circle_table());
+    else k_req_polygons<false><<<blocks(npaths, 4), 128, 0, s>>>(a, L, P, D, circle_table());
     ++*launches;
   }
   if (e != cudaSuccess) { st.why = std::string("scan / sort failed: ") + cudaGetErrorString(e); return TE_ERR_CUDA; }

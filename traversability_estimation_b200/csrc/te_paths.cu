@@ -348,9 +348,10 @@ __host__ __device__ inline size_t poly_warp_smem(int mcap, bool poly) {
 // One warp per pose index p.  Shared memory per warp: sA (2 mcap points: the hull input polygon1 ++ polygon2, then the hull) and
 // sB (mcap points: a conservative path's earlier polygon2, then the sorted hull input).  POLY: with compute_untraversable_polygon
 // set for the item's path, the walk goes on past blocked cells and collects them (:602-608, :634-638).  With per-path footprints
-// (R.fp_begin) each polygonal path uses its own, and the poses of circular paths are no items.
-template <bool POLY>
-__device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, Layers L, const PolyPathArgs& P, const PolyUntravArgs& U,
+// (R.fp_begin) each polygonal path uses its own, and the poses of circular paths are no items.  AT: the maps sit at their own
+// positions (FpArgs::pos), and the item takes its path's map's tables and position.
+template <bool POLY, bool AT>
+__device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L, const PolyPathArgs& P, const PolyUntravArgs& U,
                                                      const RequestArgs& R) {
   extern __shared__ double2 sPoly[];
   const int lane = threadIdx.x & 31;
@@ -381,6 +382,9 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, Layers L, 
     return;
   }
   L = shift_layers_d(L, mo);  // path q's map
+  FpArgs Am;
+  if constexpr (AT) Am = map_args_d(A0, R.path_map ? R.path_map[q] : 0);
+  const FpArgs& A = AT ? Am : A0;
   const float* const rslope = P.rslope ? P.rslope + mo : nullptr;
   unsigned char* const memo = P.memo + mo;
   it.q = q;
@@ -544,12 +548,14 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A, Layers L, 
   }
 }
 
+template <bool AT>
 __global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L, PolyPathArgs P, RequestArgs R) {
-  check_polygon_item_d<false>(A, L, P, PolyUntravArgs{}, R);
+  check_polygon_item_d<false, AT>(A, L, P, PolyUntravArgs{}, R);
 }
 
+template <bool AT>
 __global__ void __launch_bounds__(128) k_check_polygon_items_poly(FpArgs A, Layers L, PolyPathArgs P, PolyUntravArgs U, RequestArgs R) {
-  check_polygon_item_d<true>(A, L, P, U, R);
+  check_polygon_item_d<true, AT>(A, L, P, U, R);
 }
 
 // One thread per path: the area-weighted combination of the segment results in path order (:522-579).  An unsafe path reports 0;
@@ -771,16 +777,19 @@ int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry*
   for (int k = 0; r.footprint && k < r.nfp; ++k) {
     P.fx[k] = r.footprint[3 * k]; P.fy[k] = r.footprint[3 * k + 1]; P.fz[k] = r.footprint[3 * k + 2];
   }
-  if (!r.ucount) return launch_polygon_kernels(st, k_check_polygon_items, k_check_polygon_combine, "k_check_polygon_items", false, a, L, P, s,
-                                               launches, R);
+  // maps at their own positions (a te_map): the instantiations that read each path's map's tables
+  const bool at = a.pos != nullptr;
+  if (!r.ucount)
+    return launch_polygon_kernels(st, at ? k_check_polygon_items<true> : k_check_polygon_items<false>, k_check_polygon_combine,
+                                  "k_check_polygon_items", false, a, L, P, s, launches, R);
   const size_t cbytes = (sizeof(int) * nitems + 15) / 16 * 16;
   if (st.upoly.reserve(cbytes + sizeof(double2) * nitems * (size_t)std::max(r.max_vertices, 1)) != cudaSuccess) {
     st.why = "allocating the untraversable polygons failed";
     return TE_ERR_CUDA;
   }
   const PolyUntravArgs U{r.cup, (int*)st.upoly.p, (double*)((char*)st.upoly.p + cbytes), UntravOut{r.max_vertices, r.ucount, r.uxy}};
-  return launch_polygon_kernels(st, k_check_polygon_items_poly, k_check_polygon_combine_poly, "k_check_polygon_items_poly", true, a, L, P, s,
-                                launches, U, R);
+  return launch_polygon_kernels(st, at ? k_check_polygon_items_poly<true> : k_check_polygon_items_poly<false>, k_check_polygon_combine_poly,
+                                "k_check_polygon_items_poly", true, a, L, P, s, launches, U, R);
 }
 
 }  // namespace te

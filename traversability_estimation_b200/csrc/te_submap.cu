@@ -43,15 +43,18 @@ __global__ void __launch_bounds__(kGatherWarps * 32) k_map_gather_submaps(Submap
   }
 }
 
-// Position q on map pos_map[q] of a batch of nmaps maps (pos_map null: map 0); a map outside the batch gives 0.
+// Position q on map pos_map[q] of a batch of nmaps maps (pos_map null: map 0); a map outside the batch gives 0.  map_pos: the maps'
+// own positions (x, y per map), or null: every map at g's.
 __global__ void k_map_valid_at(GridGeo g, const float* __restrict__ trav, int n, const double* __restrict__ xy,
-                               const int* __restrict__ pos_map, int nmaps, unsigned char* __restrict__ valid) {
+                               const int* __restrict__ pos_map, int nmaps, const double* __restrict__ map_pos,
+                               unsigned char* __restrict__ valid) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n) return;
   if (pos_map) {
     const int m = pos_map[q];
     if (m < 0 || m >= nmaps) { valid[q] = 0; return; }
     trav += (size_t)m * g.rows * g.cols_total;
+    if (map_pos) { g.posx = map_pos[2 * m]; g.posy = map_pos[2 * m + 1]; }
   }
   int i, j;
   const bool in = grid_get_index(g, xy[2 * q], xy[2 * q + 1], i, j);
@@ -101,10 +104,10 @@ void launch_gather_submaps(const SubmapGather& a, int sms, cudaStream_t s) {
   k_map_gather_submaps<<<(unsigned)blocks, kGatherWarps * 32, 0, s>>>(a);
 }
 
-void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, const int* pos_map, int nmaps, unsigned char* valid,
-                     cudaStream_t s) {
+void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, const int* pos_map, int nmaps, const double* map_pos,
+                     unsigned char* valid, cudaStream_t s) {
   if (n <= 0) return;
-  k_map_valid_at<<<(n + 255) / 256, 256, 0, s>>>(g, trav, n, xy, pos_map, nmaps, valid);
+  k_map_valid_at<<<(n + 255) / 256, 256, 0, s>>>(g, trav, n, xy, pos_map, nmaps, map_pos, valid);
 }
 
 }  // namespace te
