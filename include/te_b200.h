@@ -469,7 +469,8 @@ int te_check_footprint_request_batched(te_ctx* ctx, const te_geometry* g, const 
  *
  * A te_map belongs to one te_ctx: it runs on that context's stream under its lock and must be destroyed before the context.  It
  * owns, on the device, the layers traversability, traversability_slope, traversability_step, traversability_roughness (optional),
- * elevation, robot_slope (optional) and the elevation map's carried layers (optional, te_map_carry_layers below); the
+ * elevation, robot_slope (optional), the elevation map's carried layers (optional, te_map_carry_layers below) and
+ * traversability_x / traversability_rot (optional, te_map_footprint_polygon_keep); the
  * traversability_footprint cache (float32, NaN = empty); and the isTraversableForFilters
  * memo, which is kept until the layers or one of max_gap_width, critical_step_height and verify_roughness change.  Whole maps only.
  * Host layers may carry a circular-buffer start index: they are unwrapped on upload and outputs are re-wrapped to the start index
@@ -566,6 +567,7 @@ int te_map_set_layers_maps(te_map* map, const te_geometry* g, int32_t nsel, cons
  *     map's position, in the work list, the dedup keys (the map is part of a key), the walks, the replay and the polygonal paths.
  *     The polygon entries (te_map_footprint_polygon(_yaws, _yaws_reduce)) classify the polygon's offsets per position: on maps at
  *     several positions they sweep one map at a time (one sweep per map, outputs in the batch layout).
+ *     te_map_footprint_polygon_keep sweeps maps at several positions in one launch, each on its own tables.
  *   - Memory: when the maps of a call do not all sit at one position the te_map keeps per-map tables on the device, 8 bytes per
  *     row and per column of every map of the call (cell-centre coordinates) plus 16 per map (the position), and for a chain call
  *     1 byte more per row and column (the fused kernel's on-circle masks); they are rebuilt when the positions change.
@@ -672,6 +674,40 @@ int te_map_footprint_polygon_yaws_reduce(te_map* map, const te_footprint_params*
                                          int32_t nyaws, const double* yaws, float* worst_or_null, float* best_or_null,
                                          int32_t* best_yaw_or_null, int memory);
 
+/* The reference's traversability_footprint service (TraversabilityEstimation.cpp:272-276, TraversabilityMap::traversabilityFootprint
+ * (footprintYaw), :239-305) kept on the map: traversability_x and traversability_rot become layers the te_map holds
+ * (TE_LAYER_TRAVERSABILITY_X / _ROT), published by te_map_get_layers and served by te_map_get_submaps(_batched), as the reference
+ * adds them to the map it publishes and cuts submaps from.
+ *   - Swept maps: nsel = 0 with map_index_or_null NULL sweeps every map; otherwise the maps map_index[0..nsel), under the rules of
+ *     the _maps entries above (a host array of distinct indices, outputs back to back in map_index order, TE_ERR_UNSUPPORTED for a
+ *     start index).
+ *   - footprint_yaw is a HOST array: nyaws = 1 gives every swept map that yaw, nyaws = the number of swept maps gives map k the
+ *     k-th (in map_index order for a selection); any other count is TE_ERR_BAD_ARG.  Yaws are taken as te_map_footprint_polygon
+ *     takes its yaw.  More than 1024 distinct yaws (compared by bits) is TE_ERR_UNSUPPORTED.
+ *   - Each swept map then holds, bit for bit, the traversability_x / traversability_rot that te_map_footprint_polygon(p,
+ *     polygon, its yaw) returns on a single-map te_map holding that map at its position.  Maps not swept keep their two layers
+ *     bit for bit; a map never swept holds NaN with bits 0xffffffff (the first call gives the two layers to every map of the
+ *     batch, as every map of a batch holds the same layers).  The cache, the memo and every other layer are left alone.
+ *   - traversability_x_or_null / traversability_rot_or_null receive copies of the swept maps' new layers: in host memory
+ *     re-wrapped to a single map's start index, and the call returns synchronised; in device memory in default order, and the
+ *     call is asynchronous on the context stream.
+ *   - Errors as te_map_footprint_polygon (TE_ERR_BAD_ARG for a map without layers, a polygon without 3..16 finite vertices and a
+ *     non-finite yaw; TE_ERR_UNSUPPORTED for a polygon that reaches further than 31 cells; TE_ERR_MISSING_LAYER for
+ *     verify_roughness without roughness), plus those of the selection and the yaws above and TE_ERR_BAD_ARG for an unknown
+ *     memory mode.  Every argument error is found before anything is written: the te_map is then unchanged.
+ *   - Lifetime, as each new map of the reference replaces the old one wholesale: te_map_chain(_batched, _batched_at),
+ *     te_map_set_layers(_batched, _batched_at) and te_map_chain_image drop both layers (TE_ERR_MISSING_LAYER until the next
+ *     call here); te_map_chain_maps(_at), te_map_set_layers_maps(_at) and te_map_chain_image_maps keep the batch's layers and fill
+ *     the selected maps' with 0xffffffff, as for carried layers; every other entry leaves them as they are (te_map_clear_footprint
+ *     too: resetTraversabilityFootprintLayers does not clear them).
+ *   - Memory: 8 bytes per cell and map, resident from the first call until te_map_destroy; a selection uses the _maps scratch as
+ *     te_map_footprint_maps does (plus 8 bytes per selected cell for host outputs).  Launches, whatever the maps, yaws and
+ *     positions: the two predicate kernels and one sweep, plus for a selection the kernel that gathers its layers and, with
+ *     outputs, the one that gathers those. */
+int te_map_footprint_polygon_keep(te_map* map, const te_footprint_params* p, int32_t nsel, const int32_t* map_index_or_null,
+                                  int32_t npts, const double* polygon_xy, int32_t nyaws, const double* footprint_yaw,
+                                  float* traversability_x_or_null, float* traversability_rot_or_null, int memory);
+
 /* A CheckFootprintPath request on the map, as the reference service loop answers it (TraversabilityEstimation.cpp:278-295, with
  * publishPolygons = true).  Arguments, outputs, conventions, limits and errors are those of te_check_footprint_request, with the
  * layers and the memory mode taken from the map: every array is in HOST memory (requests come from a ROS message); the call
@@ -775,7 +811,10 @@ typedef enum te_layer {
   TE_LAYER_CARRIED = 0x7f00,  /* the seven bits above */
   /* upper_bound - lower_bound, derived when read: publishTraversabilityMap adds it to the copy it publishes
    * (TraversabilityMap.cpp:178-180).  te_map_get_layers only. */
-  TE_LAYER_UNCERTAINTY_RANGE = 1 << 15
+  TE_LAYER_UNCERTAINTY_RANGE = 1 << 15,
+  /* The traversability_footprint service's layers (TraversabilityMap.cpp:239-305): te_map_footprint_polygon_keep gives them. */
+  TE_LAYER_TRAVERSABILITY_X = 1 << 16,
+  TE_LAYER_TRAVERSABILITY_ROT = 1 << 17
 } te_layer;
 
 /* mapOut = mapIn for the layers the chain does not make: the carried layers of `layer_mask` (TE_LAYER_CARRIED bits) and
@@ -834,7 +873,8 @@ int te_submap_geometry(const te_geometry* g, int32_t n, const double* position_x
  * back in bit order (on a batch: per layer the nmaps maps back to back, nmaps*rows*cols floats a layer).  In host memory each is re-wrapped to the map's start index, as te_map's other outputs, and the call returns
  * synchronised; in device memory they are in the map's default (unwrapped) order, asynchronously.  TE_ERR_MISSING_LAYER for a
  * layer the map does not hold (roughness after te_map_set_layers without it, robot_slope after te_map_chain, a carried layer
- * te_map_carry_layers did not give since the last whole-map update); TE_ERR_BAD_ARG for an empty mask or unknown bits.
+ * te_map_carry_layers did not give since the last whole-map update, traversability_x / _rot before te_map_footprint_polygon_keep);
+ * TE_ERR_BAD_ARG for an empty mask or unknown bits.
  * TE_LAYER_UNCERTAINTY_RANGE is upper_bound - lower_bound, one IEEE float32 subtraction per cell computed on the device
  * (TraversabilityMap.cpp:178-180), with NaN results carrying the payload an x86-64 host's subtraction gives them (the first NaN
  * operand, quieted; 0xffc00000 for Inf - Inf), so bit for bit what the reference publishes there.  It needs both bounds

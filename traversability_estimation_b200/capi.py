@@ -26,7 +26,10 @@ LAYERS = ("traversability", "traversability_slope", "traversability_step", "trav
 CARRIED_LAYERS = ("upper_bound", "lower_bound", "variance", "horizontal_variance_x", "horizontal_variance_y", "horizontal_variance_xy",
                   "time")
 UNCERTAINTY_RANGE = "uncertainty_range"
-LAYER_BITS = {**{n: k for k, n in enumerate(LAYERS)}, **{n: 8 + k for k, n in enumerate(CARRIED_LAYERS)}, UNCERTAINTY_RANGE: 15}
+# The traversability_footprint service's layers a te_map keeps (Map.footprint_polygon_keep), bits 16 and 17.
+POLYGON_LAYERS = ("traversability_x", "traversability_rot")
+LAYER_BITS = {**{n: k for k, n in enumerate(LAYERS)}, **{n: 8 + k for k, n in enumerate(CARRIED_LAYERS)}, UNCERTAINTY_RANGE: 15,
+              **{n: 16 + k for k, n in enumerate(POLYGON_LAYERS)}}
 
 
 def layer_mask(names) -> int:
@@ -182,6 +185,7 @@ SIGNATURES = {
     "te_map_footprint_polygon": (_R, [_P, _FP, _I, _P, _D, _P, _P, _I]),
     "te_map_footprint_polygon_yaws": (_R, [_P, _FP, _I, _P, _I, _P, _P, _I]),
     "te_map_footprint_polygon_yaws_reduce": (_R, [_P, _FP, _I, _P, _I, _P, _P, _P, _P, _I]),
+    "te_map_footprint_polygon_keep": (_R, [_P, _FP, _I, _P, _I, _P, _I, _P, _P, _P, _I]),
     "te_map_check_footprint_request": (_R, [_P, _FP, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
     "te_map_check_footprint_request_batched": (_R, [_P, _FP, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
     "te_map_check_footprint_request_device": (_R, [_P, _FP, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P, _L]),
@@ -976,6 +980,32 @@ class Map:
         self._check(fn(self._h, C.byref(fp), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data if len(ys) else None, _addr(bw),
                        _addr(bb), _addr(by), MEM_HOST))
         return worst, best, best_yaw
+
+    def footprint_polygon_keep(self, fp, polygon_xy, yaws, map_index=None, outputs=False, memory=MEM_HOST):
+        """te_map_footprint_polygon_keep (the traversability_footprint service, kept on the map): the swept maps (map_index None:
+        every map) then hold traversability_x and traversability_rot at their yaws (a scalar for every swept map, or one per swept
+        map in map_index order), which get_layers / get_submaps return.  Host memory: outputs=True returns copies of the swept
+        maps' new layers (x, rot), each (rows, cols) for one map or (n, rows, cols) for n swept maps, in the map's start index.
+        Device memory: outputs is False or a pair of float32 device tensors of n * rows * cols (None for one not wanted), filled
+        asynchronously on the context stream in default order and returned."""
+        pts = np.ascontiguousarray(polygon_xy, dtype=np.float64).reshape(-1, 2)
+        ys = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
+        idx = None if map_index is None else self._map_index(map_index)
+        n = self._n if idx is None else len(idx)
+        res = None
+        if memory == MEM_HOST:
+            rows, cols = self._shape() if self._g else (0, 0)
+            bufs = (np.empty((n, cols, rows), np.float32), np.empty((n, cols, rows), np.float32)) if outputs else (None, None)
+            if outputs:
+                res = tuple(b.transpose(0, 2, 1)[0] if idx is None and self._n == 1 else b.transpose(0, 2, 1) for b in bufs)
+        else:
+            self._ctx._order_after_torch(memory)
+            bufs = tuple(outputs) if outputs else (None, None)
+            res = bufs if outputs else None
+        self._check(self._L.te_map_footprint_polygon_keep(self._h, C.byref(fp), 0 if idx is None else len(idx), _addr(idx), len(pts),
+                                                          pts.ctypes.data, len(ys), ys.ctypes.data if len(ys) else None,
+                                                          _addr(bufs[0]), _addr(bufs[1]), memory))
+        return res
 
     def check_footprint_request(self, fp, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices=None,
                                 conservative=None, compute_untraversable_polygon=None, untraversable_capacity=None):

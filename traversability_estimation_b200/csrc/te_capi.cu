@@ -965,7 +965,7 @@ static int footprint_polygon_common(te_ctx* c, te::FootprintState* resident, con
   te::FootprintState& fp = resident ? *resident : c->fp;
   int nl = 0;
   int rc = te::launch_footprint_polygon(fp, make_view(c, g, s), g, p, npts, pts_xy, (int)layers.size(), layers.data(), reduce ? &red : nullptr,
-                                        in[0], in[1], in[2], in[4], in[3], nmaps, c->sms, c->stream, &nl);
+                                        nullptr, in[0], in[1], in[2], in[4], in[3], nmaps, c->sms, c->stream, &nl);
   if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", fp.why.c_str());
   if (int r2 = launch_check(c, "polygon footprint", nl)) return r2;
   return st.finish();
@@ -1340,6 +1340,8 @@ struct te_map {
   DevBuf trav, slope, step, rough, elev, rslope, cache, fresh;
   DevBuf carry[7];        // the carried layers, TE_LAYER_UPPER_BOUND (carry[0]) .. TE_LAYER_TIME (carry[6]): te_map_carry_layers
   uint32_t carried = 0;   // the TE_LAYER_CARRIED bits the map holds
+  DevBuf fpoly[2];        // traversability_x, traversability_rot: te_map_footprint_polygon_keep
+  bool have_fpoly = false;
   DevBuf gather;  // te_map_get_submaps: the source-layer table, then the windows (te::SubmapWindow)
   // The _maps entries: the selected maps' layers packed back to back (grown to the largest selection) and their slot table
   DevBuf sel[te::kMapSlotLayers], slots;
@@ -1517,6 +1519,7 @@ int map_reset(te_map* m, const te_geometry* g_in, const te_geometry* g, int nmap
   m->memo_valid = false;
   m->have_layers = false;
   m->carried = 0;  // a new map replaces the old one wholesale, its elevation map's layers included
+  m->have_fpoly = false;
   return TE_OK;
 }
 
@@ -1564,12 +1567,13 @@ int map_footprint_params(const te_map* m, const te_footprint_params* p) {
   return TE_OK;
 }
 
-constexpr int kLayerBits = 16;  // te_layer bits 0 .. 15 (1 << 7 unassigned)
+constexpr int kLayerBits = 18;  // te_layer bits 0 .. 17 (1 << 7 unassigned)
 constexpr int kCarryBit0 = 8;   // TE_LAYER_UPPER_BOUND: carry[b - kCarryBit0] holds layer bit b of TE_LAYER_CARRIED
+constexpr int kPolyBit0 = 16;   // TE_LAYER_TRAVERSABILITY_X: fpoly[b - kPolyBit0] holds layer bit b
 const char* const kLayerNames[kLayerBits] = {"traversability", "traversability_slope", "traversability_step", "traversability_roughness",
                                              "elevation", "robot_slope", "traversability_footprint", nullptr, "upper_bound", "lower_bound",
                                              "variance", "horizontal_variance_x", "horizontal_variance_y", "horizontal_variance_xy",
-                                             "time", "uncertainty_range"};
+                                             "time", "uncertainty_range", "traversability_x", "traversability_rot"};
 
 // The resident buffer of te_layer bit b when the map holds that layer, else null (uncertainty_range is derived: null).
 DevBuf* map_layer_buf(te_map* m, int b) {
@@ -1581,6 +1585,7 @@ DevBuf* map_layer_buf(te_map* m, int b) {
     case 4: return &m->elev;
     case 5: return m->have_rslope ? &m->rslope : nullptr;
     case 6: return &m->cache;
+    case kPolyBit0: case kPolyBit0 + 1: return m->have_fpoly ? &m->fpoly[b - kPolyBit0] : nullptr;
     default: return b >= kCarryBit0 && b < kCarryBit0 + 7 && ((m->carried >> b) & 1u) ? &m->carry[b - kCarryBit0] : nullptr;
   }
 }
@@ -1590,7 +1595,8 @@ DevBuf* map_layer_buf(te_map* m, int b) {
 int map_layers(te_map* m, uint32_t mask, bool with_range, const float* out[kLayerBits], int* n) {
   if (!with_range && (mask & TE_LAYER_UNCERTAINTY_RANGE))
     return fail(TE_ERR_BAD_ARG, "layer uncertainty_range is published with the map, not held by it: submaps have no such layer");
-  const uint32_t known = TE_LAYER_ALL | TE_LAYER_CARRIED | (with_range ? (uint32_t)TE_LAYER_UNCERTAINTY_RANGE : 0u);
+  const uint32_t known = TE_LAYER_ALL | TE_LAYER_CARRIED | TE_LAYER_TRAVERSABILITY_X | TE_LAYER_TRAVERSABILITY_ROT |
+                         (with_range ? (uint32_t)TE_LAYER_UNCERTAINTY_RANGE : 0u);
   if (mask == 0 || (mask & ~known)) return fail(TE_ERR_BAD_ARG, "layer mask 0x%x: need a non-empty subset of 0x%x", mask, known);
   *n = 0;
   for (int b = 0; b < kLayerBits; ++b) {
@@ -1662,8 +1668,9 @@ cudaError_t map_copy_packed(te_map* m, float* dst, const float* src, size_t n, b
 }
 
 // The packed layers src (each null or nsel maps back to back) into the selected maps' resident layers dst, in one launch that also
-// empties those maps' caches, fills their carried layers with NaN (the new maps come without them, but every map of a batch
-// holds the same layers) and, when the memo is live, clears their memo bytes.  The te_map-wide memo key stays.
+// empties those maps' caches, fills their carried and polygon layers with NaN (the new maps come without them, but every map of a
+// batch holds the same layers) and, when the memo is live, clears their memo bytes.  The te_map-wide memo key stays.  A batch
+// that holds more than kMapSlotLayers such layers fills the rest in a second launch.
 int map_put_selected(te_map* m, const MapSel& s, const float* const src[te::kMapSlotLayers], DevBuf* const dst[te::kMapSlotLayers]) {
   te_ctx* c = m->ctx;
   te::MapSlots a{};
@@ -1671,8 +1678,13 @@ int map_put_selected(te_map* m, const MapSel& s, const float* const src[te::kMap
     a.src[l] = dst[l] ? src[l] : nullptr;
     a.dst[l] = dst[l] ? (float*)dst[l]->p : nullptr;
   }
+  std::vector<float*> fill;
   for (int k = 0; k < 7; ++k)
-    if ((m->carried >> (kCarryBit0 + k)) & 1u) a.fill[k] = (float*)m->carry[k].p;
+    if ((m->carried >> (kCarryBit0 + k)) & 1u) fill.push_back((float*)m->carry[k].p);
+  if (m->have_fpoly)
+    for (DevBuf& b : m->fpoly) fill.push_back((float*)b.p);
+  const int nf = std::min((int)fill.size(), te::kMapSlotLayers);
+  std::copy(fill.begin(), fill.begin() + nf, a.fill);
   a.fill_bits = 0xffffffffu;
   a.cache = (float*)m->cache.p;
   a.memo = m->memo_valid ? (unsigned char*)m->fp.memo.p : nullptr;  // reserved for the whole batch while valid (map_memo)
@@ -1680,7 +1692,15 @@ int map_put_selected(te_map* m, const MapSel& s, const float* const src[te::kMap
   a.nsel = s.n;
   a.cells = map_cells(m);
   te::launch_map_slots(a, true, c->sms, c->stream);
-  return launch_check(c, "k_map_slots (put)");
+  if (nf == (int)fill.size()) return launch_check(c, "k_map_slots (put)");
+  te::MapSlots f{};
+  std::copy(fill.begin() + nf, fill.end(), f.fill);
+  f.fill_bits = a.fill_bits;
+  f.slot = a.slot;
+  f.nsel = a.nsel;
+  f.cells = a.cells;
+  te::launch_map_slots(f, true, c->sms, c->stream);
+  return launch_check(c, "k_map_slots (put)", 2);
 }
 
 #define TE_MAP_ENTER(map)                                   \
@@ -1710,6 +1730,7 @@ int te_map_destroy(te_map* m) {
         b->release();
       for (DevBuf& b : m->sel) b.release();
       for (DevBuf& b : m->carry) b.release();
+      for (DevBuf& b : m->fpoly) b.release();
       m->tab_all.buf.release();
       m->tab_launch.buf.release();
       m->fp.release();
@@ -2251,6 +2272,111 @@ int te_map_footprint_polygon_yaws_reduce(te_map* m, const te_footprint_params* p
   return map_footprint_polygon(m, p, npts, pts_xy, 1, outs, &red, memory);
 }
 
+// traversabilityFootprint(footprintYaw) kept on the map: every map (whole) or the maps sel.idx[0..sel.n) of the batch, each at its
+// own yaw, swept by one k_poly_tile_maps launch on the resident layers (a selection's gathered into the _maps scratch by one
+// k_map_slots launch) straight into the map slots of the resident traversability_x / traversability_rot.  The outputs are copies
+// of the swept maps' layers: a whole batch's read back as te_map_get_layers does, a selection's gathered by one more k_map_slots
+// launch.
+int te_map_footprint_polygon_keep(te_map* m, const te_footprint_params* p, int32_t nsel, const int32_t* map_index, int32_t npts,
+                                  const double* pts_xy, int32_t nyaws, const double* yaws, float* out_x, float* out_rot, int memory) {
+  TE_MAP_ENTER(m);
+  const bool whole = nsel == 0 && !map_index;
+  const MapSel sel{nsel, map_index};
+  if (int rc = whole ? map_ready(m) : map_select(m, false, nullptr, sel)) return rc;
+  if (int rc = map_footprint_params(m, p)) return rc;
+  if (memory != TE_MEM_HOST && memory != TE_MEM_DEVICE) return fail(TE_ERR_BAD_ARG, "unknown memory mode %d", memory);
+  if (npts < 3 || npts > 16 || !pts_xy) return fail(TE_ERR_BAD_ARG, "footprint polygon needs 3 to 16 vertices");
+  for (int k = 0; k < 2 * npts; ++k)
+    if (!std::isfinite(pts_xy[k])) return fail(TE_ERR_BAD_ARG, "footprint polygon vertex is not finite");
+  const int n = whole ? m->nmaps : sel.n;
+  if (!yaws) return fail(TE_ERR_BAD_ARG, "footprint_yaw is null");
+  if (nyaws != 1 && nyaws != n) return fail(TE_ERR_BAD_ARG, "%d footprint yaws for %d maps: need 1, or one per swept map", nyaws, n);
+  // polygon 0: the identity (traversability_x); polygon 1 + k: the k-th distinct yaw, by bits (traversability_rot)
+  std::vector<te::PolygonLayer> polys(1, te::PolygonLayer{0.0, nullptr});
+  std::vector<int> poly_of(n);
+  std::map<uint64_t, int> index;
+  for (int k = 0; k < n; ++k) {
+    const double y = yaws[nyaws == 1 ? 0 : k];
+    if (!std::isfinite(y)) return fail(TE_ERR_BAD_ARG, "footprint yaw %d is not finite", nyaws == 1 ? 0 : k);
+    uint64_t bits;
+    std::memcpy(&bits, &y, sizeof bits);
+    const auto it = index.emplace(bits, (int)polys.size());
+    if (it.second) {
+      if (polys.size() > 1024) return fail(TE_ERR_UNSUPPORTED, "more than 1024 distinct footprint yaws: at most 1024 per call");
+      polys.push_back(te::PolygonLayer{y, nullptr});
+    }
+    poly_of[k] = it.first->second;
+  }
+  te_geometry gm;
+  PosTables tab{};
+  const bool spread = !map_geometry(m, &gm);  // the maps at several positions: their own tables
+  if (spread) gm = m->geo;
+  const te_geometry* g = &gm;
+  if (int rc = ensure_geometry(c, g)) return rc;
+  if (spread)
+    if (int rc = map_tables_of(m, MapSel{n, whole ? nullptr : sel.idx}, &tab)) return rc;
+  // trav, slope, step, rough (verify_roughness only), elev: resident, or gathered for the selection
+  const float* in[5] = {(const float*)m->trav.p, (const float*)m->slope.p, (const float*)m->step.p,
+                        p->verify_roughness ? (const float*)m->rough.p : nullptr, (const float*)m->elev.p};
+  const bool host_out = memory == TE_MEM_HOST && (out_x || out_rot);
+  int fixed = 0;
+  if (!whole) {
+    unsigned staged = host_out ? 0x60u : 0u;  // sel[5], sel[6]: the outputs before their copy to the host
+    for (int l = 0; l < 5; ++l)
+      if (in[l]) staged |= 1u << l;
+    if (int rc = map_stage_selection(m, sel, staged)) return rc;
+    te::MapSlots a{};
+    for (int l = 0; l < 5; ++l) {
+      a.src[l] = in[l];
+      a.dst[l] = in[l] ? (float*)m->sel[l].p : nullptr;
+      in[l] = a.dst[l];
+    }
+    a.slot = (const int*)m->slots.p;
+    a.nsel = n;
+    a.cells = map_cells(m);
+    te::launch_map_slots(a, false, c->sms, c->stream);
+    ++fixed;
+  }
+  // the first sweep gives every map of the batch the two layers: the maps it does not sweep hold NaN (0xffffffff)
+  const size_t lbytes = sizeof(float) * batch_cells(m);
+  for (DevBuf& b : m->fpoly) {
+    TE_CUDA(b.reserve(lbytes));
+    if (!m->have_fpoly && !whole) TE_CUDA(cudaMemsetAsync(b.p, 0xff, lbytes, c->stream));
+  }
+  polys[0].out = (float*)m->fpoly[0].p;
+  for (size_t k = 1; k < polys.size(); ++k) polys[k].out = (float*)m->fpoly[1].p;
+  const te::PolygonMaps pm{poly_of.data(), whole ? nullptr : (const int*)m->slots.p};
+  const te_slab s{0, g->cols, 0, 0};
+  int nl = 0;
+  int rc = te::launch_footprint_polygon(m->fp, view_at(make_view(c, g, s), g, spread ? &tab : nullptr), g, p, npts, pts_xy, (int)polys.size(),
+                                        polys.data(), nullptr, &pm, in[0], in[1], in[2], in[3], in[4], n, c->sms, c->stream, &nl);
+  if (rc != 0) return fail(rc, "polygon footprint sweep failed: %s", m->fp.why.c_str());
+  if (int r2 = launch_check(c, "map polygon footprint", nl + fixed)) return r2;
+  m->have_fpoly = true;
+  float* const outs[2] = {out_x, out_rot};
+  if (whole) {
+    for (int l = 0; l < 2; ++l)
+      if (outs[l])
+        if (int r2 = map_get_layer(m, outs[l], m->fpoly[l].p, memory)) return r2;
+  } else if (out_x || out_rot) {
+    te::MapSlots a{};
+    for (int l = 0; l < 2; ++l) {
+      a.src[l] = outs[l] ? (const float*)m->fpoly[l].p : nullptr;
+      a.dst[l] = !outs[l] ? nullptr : host_out ? (float*)m->sel[5 + l].p : outs[l];
+    }
+    a.slot = (const int*)m->slots.p;
+    a.nsel = n;
+    a.cells = map_cells(m);
+    te::launch_map_slots(a, false, c->sms, c->stream);
+    if (int r2 = launch_check(c, "k_map_slots (get)")) return r2;
+    if (host_out)
+      for (int l = 0; l < 2; ++l)
+        if (outs[l]) TE_CUDA(map_copy_packed(m, outs[l], a.dst[l], map_cells(m) * n, true, memory));
+  }
+  if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));
+  return TE_OK;
+}
+
 // The work-list entries launch_map_request_device needs at most for the circular paths of a validated host request: the count of
 // req_pose_entries_d with every checkInclination gate counted when the map has robot_slope, so that no path is cut.  It walks no
 // line.  *circles: whether the request has a circular path.
@@ -2492,8 +2618,8 @@ int te_map_get_layers(te_map* m, uint32_t layer_mask, float* out, int memory) {
   int nl = 0;
   if (int rc = map_layers(m, layer_mask, true, src, &nl)) return rc;
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
-  // uncertainty_range (a null entry, the last in bit order) is computed straight into a device output; in host memory into staging,
-  // which finish() re-wraps and copies back after the other layers
+  // uncertainty_range (a null entry) is computed straight into a device output; in host memory into staging, which finish()
+  // re-wraps and copies back after the other layers
   Staging st(c, memory == TE_MEM_HOST, &m->geo_in);
   for (int k = 0; k < nl; ++k) {  // per layer every map, back to back
     float* dst = out + (size_t)k * batch_cells(m);
@@ -2526,7 +2652,7 @@ static int map_submaps(te_map* m, int32_t nwin, const int32_t* win_map, const do
   if (!out) return fail(TE_ERR_BAD_ARG, "output is null");
   // the table k_map_gather_submaps reads: the source layers in its first kHead records, then the windows that have cells
   constexpr int kHead = 4;
-  static_assert(sizeof(const float*) * (kLayerBits - 1) <= kHead * sizeof(te::SubmapWindow), "layer table");
+  static_assert(sizeof(const float*) * (kLayerBits - 2) <= kHead * sizeof(te::SubmapWindow), "layer table");  // not 1 << 7, range
   std::vector<te::SubmapWindow> table(kHead);
   std::memcpy((void*)table.data(), src, sizeof(const float*) * nl);
   long long columns = 0;

@@ -66,11 +66,20 @@ struct PolygonReduce {
   float* best;
   int* best_yaw;
 };
+// Per-map polygons (te_map_footprint_polygon_keep): map k of the launch sweeps two layers, polys[0] (yaw 0: traversability_x) and
+// polys[poly_of[k]] (its own yaw: traversability_rot), each into its polygon's `out` at map slot[k] instead of k.  poly_of: a
+// host array of nmaps entries in 1 .. npoly-1; slot: a device table of nmaps map slots, or null (slot k is k).  Maps at their own
+// positions (v.pos) read their own coordinate tables.  One sweep launch whatever the maps, yaws and positions; each layer equals,
+// bit for bit, what a call with that map and yaw alone gives.  No reduction.
+struct PolygonMaps {
+  const int* poly_of;
+  const int* slot;
+};
 int footprint_polygon_halo(const te_geometry* g, const te_footprint_params* p, int npts, const double* pts_xy);
 int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int npts,
-                             const double* pts_xy, int npoly, const PolygonLayer* polys, const PolygonReduce* reduce, const float* trav,
-                             const float* slope, const float* step, const float* rough, const float* elev, int nmaps, int sms,
-                             cudaStream_t s, int* launches);
+                             const double* pts_xy, int npoly, const PolygonLayer* polys, const PolygonReduce* reduce,
+                             const PolygonMaps* maps, const float* trav, const float* slope, const float* step, const float* rough,
+                             const float* elev, int nmaps, int sms, cudaStream_t s, int* launches);
 
 // TraversabilityMap::checkCircularFootprintPath for a batch of paths on a complete traversability_footprint layer (device pointers).
 void launch_check_paths(const SlabView& v, const te_geometry* g, double traversability_default, const float* footprint, const float* robot_slope, int npaths,

@@ -75,14 +75,24 @@ __device__ bool poly_inside_d(const PolyArgs& Q, const Rot2& R, double cx, doubl
 
 // The tile geometry (PTR x PTC centres, staging origin r0 - Lp, c0 - Lp) is part of the results: a sum over a run is a difference
 // of the staged prefix sums, whose float32 rounding depends on where the staged column starts.  kReduce: reduce over the block's
-// polygons in registers instead of storing a layer per polygon (PolyArgs::worst / best / best_yaw).
-template <bool kReduce>
-__global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const float* __restrict__ trav, const unsigned char* __restrict__ blocked) {
+// polygons in registers instead of storing a layer per polygon (PolyArgs::worst / best / best_yaw).  kAt: map z sits at its own
+// position and reads its coordinate tables at A.X + z * A.xs, A.Y + z * A.ys.  kMaps (Q.npoly = 2, the polygons of each map):
+// map z sweeps its own pair of polygons, desc[0] and desc[map_poly[z]], into map slot slot[z] of their layers (slot null: z);
+// device arrays of one entry per map, unused otherwise.  A and Q are taken by value: k_poly_tile then compiles to the code it had
+// as a kernel of its own (by reference it does not).
+template <bool kReduce, bool kAt, bool kMaps>
+__device__ __forceinline__ void poly_tile(FpArgs A, PolyArgs Q, const float* __restrict__ trav,
+                                          const unsigned char* __restrict__ blocked, const int* __restrict__ map_poly,
+                                          const int* __restrict__ slot) {
   extern __shared__ double sP[];  // [NC][PS] prefix sums of t'; then [NC][PB] uint16 prefix counts of blocked cells
   const int Lr = Q.Lp, NR = PTR + 2 * Lr, NC = PTC + 2 * Lr, PS = NR + 1;
   unsigned short* sB = reinterpret_cast<unsigned short*>(sP + (size_t)NC * PS);
   // map blockIdx.z of the batch: its input-buffer columns start mb columns into the batch's, its output columns mbo
-  const int mb = (int)blockIdx.z * A.in_ncols, mbo = (int)blockIdx.z * A.out_ncols;
+  const int mb = (int)blockIdx.z * A.in_ncols, mbo = (kMaps && slot ? slot[blockIdx.z] : (int)blockIdx.z) * A.out_ncols;
+  if constexpr (kAt) {  // the map's coordinate tables
+    A.X += (size_t)blockIdx.z * A.xs;
+    A.Y += (size_t)blockIdx.z * A.ys;
+  }
   const int tile_r = (int)blockIdx.x % Q.row_tiles, p0 = ((int)blockIdx.x / Q.row_tiles) * Q.group, p1 = min(p0 + Q.group, Q.npoly);
   const int r0 = tile_r * PTR, c0 = A.out_col0 + (int)blockIdx.y * PTC;
   const int rb = r0 - Lr, cb = c0 - Lr;
@@ -144,6 +154,7 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
   const int ic = active ? i : A.rows - 1;
   const double cx = A.X[ic];
   const int k0 = ic - rb;
+  const int mpoly = kMaps ? map_poly[blockIdx.z] : 0;
   for (int q = 0; q < PTC / 4; ++q) {
     const int j = c0 + (warp >> 1) * (PTC / 4) + q;
     if (j >= A.out_col0 + A.out_ncols) break;
@@ -157,7 +168,7 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
     float worst = __int_as_float(0x7f800000), best = __int_as_float(0xff800000);
     int best_y = p0;
     for (int y = p0; y < p1; ++y) {
-      const PolyDesc& D = Q.desc[y];
+      const PolyDesc& D = Q.desc[kMaps ? (y == 0 ? 0 : mpoly) : y];
       const Rot2 R = D.R;
       const int* const runs = Q.runs + D.run0;
       const int* const fz = Q.fz + D.fz0;
@@ -256,6 +267,19 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
       }
     }
   }
+}
+
+template <bool kReduce>
+__global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const float* __restrict__ trav, const unsigned char* __restrict__ blocked) {
+  poly_tile<kReduce, false, false>(A, Q, trav, blocked, nullptr, nullptr);
+}
+
+// The polygon layers a te_map keeps (launch_footprint_polygon with PolygonMaps): every map of the launch sweeps the identity and
+// its own yaw's rotation on its own coordinate tables (kAt) or on the shared ones.
+template <bool kAt>
+__global__ void __launch_bounds__(256) k_poly_tile_maps(FpArgs A, PolyArgs Q, const float* __restrict__ trav, const unsigned char* __restrict__ blocked,
+                                                        const int* __restrict__ map_poly, const int* __restrict__ slot) {
+  poly_tile<false, kAt, true>(A, Q, trav, blocked, map_poly, slot);
 }
 
 // Reduce mode after a yaw-group split: k_poly_tile left group g's partial reduction at g * n cells of each scratch array (sw: worst,
@@ -376,13 +400,15 @@ int polygon_groups(long long tiles, int npoly, int sms) {
 }  // namespace
 
 // traversabilityFootprint(yaw) for every layer of `polys`: predicates once, the polygon tables of every rotation in one upload,
-// then one k_poly_tile launch for all of them (and, in reduce mode with yaw groups, one k_poly_combine).
+// then one k_poly_tile launch for all of them (and, in reduce mode with yaw groups, one k_poly_combine), or with `maps` one
+// k_poly_tile_maps launch for each map's pair.
 int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int npts,
-                             const double* pts_xy, int npoly, const PolygonLayer* polys, const PolygonReduce* reduce, const float* trav,
-                             const float* slope, const float* step, const float* rough, const float* elev, int nmaps, int sms,
-                             cudaStream_t s, int* launches) {
+                             const double* pts_xy, int npoly, const PolygonLayer* polys, const PolygonReduce* reduce,
+                             const PolygonMaps* maps, const float* trav, const float* slope, const float* step, const float* rough,
+                             const float* elev, int nmaps, int sms, cudaStream_t s, int* launches) {
   if (npts < 3 || npts > PMAXV) { st.why = "footprint polygon needs 3 to 16 vertices"; return TE_ERR_UNSUPPORTED; }
-  if (npoly < 1) { st.why = "no polygon layer to sweep"; return TE_ERR_UNSUPPORTED; }
+  if (npoly < (maps ? 2 : 1)) { st.why = "no polygon layer to sweep"; return TE_ERR_UNSUPPORTED; }
+  if (maps && reduce) { st.why = "per-map polygons have no reduction"; return TE_ERR_UNSUPPORTED; }
   if (reduce && !reduce->worst && !reduce->best && !reduce->best_yaw) { st.why = "no reduction output"; return TE_ERR_UNSUPPORTED; }
   const int Lp = polygon_reach(g, npts, pts_xy);
   if (Lp > 31) { st.why = "footprint polygon reaches further than 31 cells from its centre"; return TE_ERR_UNSUPPORTED; }
@@ -408,11 +434,14 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
       fz.insert(fz.end(), tb.fz.begin(), tb.fz.end());
     }
   }
-  const size_t dbytes = sizeof(PolyDesc) * desc.size(), bytes = dbytes + sizeof(int) * (runs.size() + fz.size());
+  // with per-map polygons, each map's polygon index follows the tables
+  const size_t nmp = maps ? (size_t)nmaps : 0;
+  const size_t dbytes = sizeof(PolyDesc) * desc.size(), bytes = dbytes + sizeof(int) * (runs.size() + fz.size() + nmp);
   std::vector<char> blob(bytes);
   std::memcpy(blob.data(), desc.data(), dbytes);
   if (!runs.empty()) std::memcpy(blob.data() + dbytes, runs.data(), sizeof(int) * runs.size());
   if (!fz.empty()) std::memcpy(blob.data() + dbytes + sizeof(int) * runs.size(), fz.data(), sizeof(int) * fz.size());
+  if (maps) std::memcpy(blob.data() + dbytes + sizeof(int) * (runs.size() + fz.size()), maps->poly_of, sizeof(int) * nmp);
   FpArgs a{};
   if (int rc = run_predicates(st, v, g, p, nmaps, trav, slope, step, rough, elev, nullptr, nullptr, nullptr, sms, s, &a)) return rc;
   if (st.poly.p && st.poly.cap < bytes) cudaStreamSynchronize(s);  // kernels of an earlier call may still read the old tables
@@ -421,22 +450,31 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
   q.desc = (const PolyDesc*)st.poly.p;
   q.runs = (const int*)((const char*)st.poly.p + dbytes);
   q.fz = q.runs + runs.size();
+  if (maps) q.npoly = 2;  // per map: the identity and the map's own rotation
   const size_t smem = sizeof(double) * (size_t)(PTC + 2 * Lp) * (PTR + 2 * Lp + 1) + (size_t)(PTC + 2 * Lp) * (PB * 2);
   if (!st.poly_attr) {
     const size_t smax = sizeof(double) * (size_t)(PTC + 62) * (PTR + 63) + (size_t)(PTC + 62) * (PB * 2);
     if (cudaFuncSetAttribute(k_poly_tile<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
-        cudaFuncSetAttribute(k_poly_tile<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess) {
+        cudaFuncSetAttribute(k_poly_tile<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
+        cudaFuncSetAttribute(k_poly_tile_maps<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
+        cudaFuncSetAttribute(k_poly_tile_maps<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess) {
       st.why = "cudaFuncSetAttribute(max dynamic shared memory) failed"; return TE_ERR_CUDA;
     }
     st.poly_attr = true;
   }
   q.row_tiles = (v.rows + PTR - 1) / PTR;
   const int col_tiles = (v.out_ncols + PTC - 1) / PTC;
-  const int ngroups = polygon_groups((long long)q.row_tiles * col_tiles * nmaps, npoly, sms);
-  q.group = (npoly + ngroups - 1) / ngroups;
-  const int nsplit = (npoly + q.group - 1) / q.group;  // groups actually launched
+  const int ngroups = polygon_groups((long long)q.row_tiles * col_tiles * nmaps, q.npoly, sms);
+  q.group = (q.npoly + ngroups - 1) / ngroups;
+  const int nsplit = (q.npoly + q.group - 1) / q.group;  // groups actually launched
   const int nblocks_x = q.row_tiles * nsplit;
   const dim3 grid((unsigned)nblocks_x, (unsigned)col_tiles, (unsigned)nmaps);
+  if (maps) {
+    (a.pos ? k_poly_tile_maps<true> : k_poly_tile_maps<false>)<<<grid, 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p,
+                                                                                      q.fz + fz.size(), maps->slot);
+    if (launches) *launches = 3;
+    return 0;
+  }
   if (!reduce) {
     k_poly_tile<false><<<grid, 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p);
     if (launches) *launches = 3;
