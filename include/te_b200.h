@@ -907,6 +907,31 @@ int te_map_valid_at(te_map* map, int32_t n, const double* xy, uint8_t* valid, in
  * outside 0..nmaps-1 is TE_ERR_BAD_ARG; in device memory (not read on the host) that position gets 0. */
 int te_map_valid_at_batched(te_map* map, int32_t n, const int32_t* pos_map, const double* xy, uint8_t* valid, int memory);
 
+/* GridMap::atPosition(layer, position), as checkInclination reads robot_slope (TraversabilityMap.cpp:751), at npoints robot-frame
+ * points around each of nposes poses, for every layer of `layer_mask`, in one kernel launch.
+ *   - poses: 7 doubles per pose, x y z qx qy qz qw (geometry_msgs/Pose order).  points_xyz: 3 floats per point, x y z
+ *     (geometry_msgs/Point32 order).  Point t of pose k lies at `toPosition * orientation * point`, computed as
+ *     checkPolygonalFootprintPath places a footprint vertex (:488-507): the quaternion as given, not normalised, and the z of the
+ *     result dropped.  The single point (0, 0, 0) gives the pose's (x, y) exactly, so that is plain atPosition at a list of
+ *     positions.
+ *   - pose k is on map pose_map[k], at that map's own position (te_map_positions); pose_map may be NULL on a te_map of one map.
+ *     Positions are map-frame: a start index changes nothing, as in grid_map, since the layers are resident unwrapped.
+ *   - layer_mask: any te_layer bits the map holds, TE_LAYER_FOOTPRINT (the cache, NaN where empty), the carried layers,
+ *     TE_LAYER_TRAVERSABILITY_X / _ROT and TE_LAYER_UNCERTAINTY_RANGE (upper_bound - lower_bound at the cell, bit for bit as
+ *     te_map_get_layers computes it) included.
+ *   - out: per layer in bit order nposes * npoints floats, pose-major: layer l of point t of pose k at out[(l * nposes + k) *
+ *     npoints + t].  A valid point (its pose's map in the batch, x and y finite, getIndex finds the cell) gets the cell's float32
+ *     bits exactly, NaN payloads included; any other point, where atPosition would throw, gets NaN 0x7fc00000.
+ *     valid_or_null[k * npoints + t] is 1 for a valid point and 0 otherwise.
+ * Every array is in `memory`.  Host memory returns synchronised.  Device memory is asynchronous on the context stream: no host
+ * synchronisation and no argument array read on the host, so the call can be captured in a CUDA graph.  nposes = 0 launches
+ * nothing.  Errors, all found before anything is written: TE_ERR_BAD_ARG for a map without layers, an empty mask or unknown bits,
+ * null poses / points_xyz / out, nposes < 0, npoints < 1, an unknown memory mode, a NULL pose_map on a batch and, in host memory
+ * only, a pose_map entry outside 0..nmaps-1 (in device memory that pose's points are invalid, as in te_map_valid_at_batched);
+ * TE_ERR_MISSING_LAYER as te_map_get_layers; TE_ERR_UNSUPPORTED for nposes * npoints >= 2^31. */
+int te_map_at_poses(te_map* map, const int32_t* pose_map_or_null, int32_t nposes, const double* poses, int32_t npoints,
+                    const float* points_xyz, uint32_t layer_mask, float* out, uint8_t* valid_or_null, int memory);
+
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the
  * neighbours' boundary columns of the INPUT layer(s) into this rank's halo.  The reference has no counterpart (it is a

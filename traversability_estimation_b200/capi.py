@@ -41,6 +41,9 @@ def layer_mask(names) -> int:
     return sum(1 << LAYER_BITS[n] for n in names)
 
 
+_layer_mask_of = layer_mask  # for methods whose argument is named layer_mask
+
+
 def layer_order(mask) -> list:
     """The layer names of a te_layer mask in bit order, the order of every output that holds several."""
     return [n for n, b in sorted(LAYER_BITS.items(), key=lambda x: x[1]) if (mask >> b) & 1]
@@ -199,6 +202,7 @@ SIGNATURES = {
     "te_map_get_submaps_batched": (_R, [_P, _I, _P, _P, _P, _U, _P, _P, _L, _I]),
     "te_map_valid_at": (_R, [_P, _I, _P, _P, _I]),
     "te_map_valid_at_batched": (_R, [_P, _I, _P, _P, _P, _I]),
+    "te_map_at_poses": (_R, [_P, _P, _I, _P, _I, _P, _U, _P, _P, _I]),
     "te_ipc_export": (_R, [_P, _P]),
     "te_ipc_open": (_R, [_P, _P]),
     "te_ipc_close": (_R, [_P]),
@@ -1188,3 +1192,34 @@ class Map:
         self._ctx._order_after_torch(memory)
         self._check(self._L.te_map_valid_at_batched(self._h, len(xy), _addr(pos_map), _addr(xy), _addr(out), memory))
         return out
+
+    def at_poses(self, poses, points, layer_mask, pose_map=None, out=None, valid=None, memory=MEM_HOST):
+        """te_map_at_poses (GridMap::atPosition at robot-frame points around poses): returns (layers, valid), layers a dict name ->
+        (nposes, npoints) values in te_layer bit order and valid (nposes, npoints) uint8 (1 where the point lies on its pose's
+        map; the value is then the cell's, else NaN).  layer_mask: a te_layer mask or layer names.  poses: (nposes, 7) x y z qx qy
+        qz qw; points: (npoints, 3) x y z; pose_map: map per pose (None on a map of one map).  Host memory: numpy arguments, out /
+        valid allocated when None.  Device memory: poses float64, points float32 and pose_map int32 device tensors, `out` a
+        float32 device tensor of nlayers * nposes * npoints and `valid` a uint8 device tensor of nposes * npoints or None, filled
+        asynchronously on the context stream; the dict holds views of `out`."""
+        mask = int(layer_mask) if isinstance(layer_mask, (int, np.integer)) else _layer_mask_of(layer_mask)
+        order = layer_order(mask)
+        if memory == MEM_HOST:
+            poses = np.ascontiguousarray(poses, dtype=np.float64).reshape(-1, 7)
+            points = np.ascontiguousarray(points, dtype=np.float32).reshape(-1, 3)
+            if pose_map is not None:
+                pose_map = np.ascontiguousarray(pose_map, dtype=np.int32).reshape(-1)
+                if len(pose_map) != len(poses):
+                    raise ValueError("pose_map needs one entry per pose")
+            n, npts = len(poses), len(points)
+            if out is None:
+                out = np.empty(len(order) * n * npts, dtype=np.float32)
+            if valid is None:
+                valid = np.empty(n * npts, dtype=np.uint8)
+        else:
+            n, npts = int(poses.numel()) // 7, int(points.numel()) // 3
+        self._ctx._order_after_torch(memory)
+        self._check(self._L.te_map_at_poses(self._h, _addr(pose_map), n, _addr(poses), npts, _addr(points), mask, _addr(out),
+                                            _addr(valid), memory))
+        flat = out.reshape(-1)
+        layers = {name: flat[k * n * npts:(k + 1) * n * npts].reshape(n, npts) for k, name in enumerate(order)}
+        return layers, (None if valid is None else valid.reshape(n, npts))

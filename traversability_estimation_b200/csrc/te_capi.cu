@@ -2733,6 +2733,57 @@ int te_map_valid_at_batched(te_map* m, int32_t n, const int32_t* pos_map, const 
   return map_valid_at(m, n, pos_map, xy, valid, memory);
 }
 
+int te_map_at_poses(te_map* m, const int32_t* pose_map, int32_t nposes, const double* poses, int32_t npoints, const float* points_xyz,
+                    uint32_t layer_mask, float* out, uint8_t* valid, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (!poses || !points_xyz || !out) return fail(TE_ERR_BAD_ARG, "poses, points_xyz or out is null");
+  if (nposes < 0) return fail(TE_ERR_BAD_ARG, "negative pose count");
+  if (npoints < 1) return fail(TE_ERR_BAD_ARG, "need at least one point, got %d", npoints);
+  if (memory != TE_MEM_HOST && memory != TE_MEM_DEVICE) return fail(TE_ERR_BAD_ARG, "unknown memory mode %d", memory);
+  if (!pose_map && m->nmaps > 1) return fail(TE_ERR_BAD_ARG, "pose_map is null on a te_map of %d maps", m->nmaps);
+  // device memory cannot be read here: the kernel gives NaN and valid 0 for a map outside the batch
+  if (pose_map && memory == TE_MEM_HOST)
+    if (int rc = check_map_indices(m, pose_map, nposes, "pose_map")) return rc;
+  const float* src[kLayerBits];
+  int nl = 0;
+  if (int rc = map_layers(m, layer_mask, true, src, &nl)) return rc;
+  const long long total = (long long)nposes * npoints;
+  if (total >= (1LL << 31)) return fail(TE_ERR_UNSUPPORTED, "%d poses x %d points: 2^31 samples or more", nposes, npoints);
+  if (total == 0) return TE_OK;
+  te::MapAtPoses a{};
+  a.range_l = -1;
+  for (int l = 0; l < nl; ++l) {
+    if (src[l]) {
+      a.layer[l] = src[l];
+    } else {  // uncertainty_range: upper_bound - lower_bound at the cell, as te_map_get_layers computes it
+      a.layer[l] = (const float*)m->carry[0].p;
+      a.lower = (const float*)m->carry[1].p;
+      a.range_l = l;
+    }
+  }
+  a.nlayers = nl;
+  Staging st(c, memory == TE_MEM_HOST, &m->geo);
+  a.poses = st.in(poses, 7 * (size_t)nposes);
+  a.pose_map = st.in(pose_map, (size_t)nposes);
+  a.points = st.in(points_xyz, 3 * (size_t)npoints);
+  a.out = st.out(out, (size_t)nl * total);
+  a.valid = st.out(valid, (size_t)total);
+  if (st.rc) return st.rc;
+  te_geometry g;
+  PosTables tab{};
+  if (!map_geometry(m, &g)) {  // the maps at several positions: the kernel takes each map's
+    g = m->geo;
+    if (int rc = map_tables_of(m, MapSel{m->nmaps, nullptr}, &tab)) return rc;
+    a.map_pos = tab.pos;
+  }
+  a.rows = g.rows; a.cols = g.cols; a.nmaps = m->nmaps; a.nposes = nposes; a.npoints = npoints;
+  a.res = g.resolution; a.lenx = g.length_x; a.leny = g.length_y; a.posx = g.position_x; a.posy = g.position_y;
+  te::launch_map_at_poses(a, c->sms, c->stream);
+  if (int rc = launch_check(c, "k_map_at_poses")) return rc;
+  return st.finish();  // host memory: returns synchronised
+}
+
 // A te IPC handle is the CUDA handle of the ALLOCATION that contains the pointer (cudaIpcGetMemHandle always describes the whole
 // allocation; sub-allocating pools such as torch's caching allocator hand out interior pointers) plus the offset into it.
 struct TeIpcHandle {

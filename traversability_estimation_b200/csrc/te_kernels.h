@@ -72,6 +72,26 @@ struct GridGeo;
 // map_pos[2m + 1] (needs pos_map).
 void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, const int* pos_map, int nmaps, const double* map_pos,
                      unsigned char* valid, cudaStream_t s);
+// te_map_at_poses: layers of a batch at npoints robot-frame points around each of nposes poses (device pointers).  Point t of
+// pose k lands at pose_point_d (te_pose.cuh) on map pose_map[k] (null: map 0) and is read at the cell grid_get_index finds there,
+// on that map's position (map_pos as in launch_valid_at); a map outside 0 .. nmaps-1, a non-finite position or one outside the
+// map gives NaN (0x7fc00000) and valid 0.  Layer l of sample s = k * npoints + t goes to out[l * nposes * npoints + s].
+constexpr int kAtPosesMaxLayers = 17;  // te_layer bits 0 .. 17 but the unassigned 7
+struct MapAtPoses {
+  const float* layer[kAtPosesMaxLayers];  // resident layers in output order, each nmaps maps back to back, column-major
+  const float* lower;                     // lower_bound: layer[range_l] (upper_bound) - lower is uncertainty_range
+  int nlayers, range_l;                   // range_l: output index of uncertainty_range, or -1
+  int rows, cols, nmaps, nposes, npoints; // nposes * npoints < 2^31
+  double res, lenx, leny, posx, posy;     // geometry, at the position of every map when map_pos is null
+  const double* map_pos;
+  const int* pose_map;
+  const double* poses;                    // 7 per pose: x y z qx qy qz qw
+  const float* points;                    // 3 per point: x y z
+  float* out;
+  unsigned char* valid;                   // may be null
+};
+// One k_map_at_poses launch (none for nposes = 0).
+void launch_map_at_poses(const MapAtPoses& a, int sms, cudaStream_t s);
 
 // te_image.cu — addLayerFromImage for mono images: nmaps row-major images of rows x cols pixels (image m at px + m * image_stride
 // bytes, its row i at + i * row_stride bytes; device memory, 2-byte pixels at even addresses and strides) into nmaps column-major

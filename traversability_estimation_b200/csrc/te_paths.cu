@@ -4,6 +4,7 @@
 // (launch_path_checks).  A te_map's circular paths share one cache instead and run in te_map_request.cu; both walk the circle
 // with fresh_circle_d (te_fp_device.cuh).  Compiled with --fmad=false: the checks replay the reference's double arithmetic.
 #include "te_fp_device.cuh"
+#include "te_pose.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -280,26 +281,8 @@ struct PolyPathArgs {
   float fx[kPolyMaxVerts], fy[kPolyMaxVerts], fz[kPolyMaxVerts];  // footprint vertices (geometry_msgs/Point32)
 };
 
-// Translation * Quaternion of a pose: Eigen::QuaternionBase::toRotationMatrix of the quaternion as given (not normalised), rows 0
-// and 1 (the z of a transformed vertex is dropped, :505-507).
-struct PoseRT {
-  double tx, ty, r00, r01, r02, r10, r11, r12;
-};
-__device__ __forceinline__ PoseRT pose_rt_d(const double* p) {
-  const double qx = p[3], qy = p[4], qz = p[5], qw = p[6];
-  const double tx = 2.0 * qx, ty = 2.0 * qy, tz = 2.0 * qz;
-  const double twx = tx * qw, twy = ty * qw, twz = tz * qw;
-  const double txx = tx * qx, txy = ty * qx, txz = tz * qx;
-  const double tyy = ty * qy, tyz = tz * qy, tzz = tz * qz;
-  PoseRT T;
-  T.tx = p[0]; T.ty = p[1];
-  T.r00 = 1.0 - (tyy + tzz); T.r01 = txy - twz; T.r02 = txz + twy;
-  T.r10 = txy + twz; T.r11 = 1.0 - (txx + tzz); T.r12 = tyz - twx;
-  return T;
-}
-
-// `toPosition * orientation * positionToVertex` (:496-500) for footprint vertex v, in the operand order of Eigen's Transform * vector.
-// The vertex comes from the path's own footprint `fxyz` in global memory, or without one from the kernel parameters.
+// Footprint vertex v placed at the pose T (te_pose.cuh).  The vertex comes from the path's own footprint `fxyz` in global memory, or
+// without one from the kernel parameters.
 __device__ __forceinline__ double2 footprint_vertex_d(const PolyPathArgs& P, const float* fxyz, const PoseRT& T, int v) {
   double vx, vy, vz;
   if (fxyz) {
@@ -307,7 +290,7 @@ __device__ __forceinline__ double2 footprint_vertex_d(const PolyPathArgs& P, con
   } else {
     vx = (double)P.fx[v]; vy = (double)P.fy[v]; vz = (double)P.fz[v];
   }
-  return make_double2(((T.r00 * vx + T.r01 * vy) + T.r02 * vz) + T.tx, ((T.r10 * vx + T.r11 * vy) + T.r12 * vz) + T.ty);
+  return pose_point_d(T, vx, vy, vz);
 }
 
 // grid_map::Polygon::getArea (recalled, see the oracle): the shoelace sum in vertex order, one thread.

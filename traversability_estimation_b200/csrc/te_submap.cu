@@ -1,10 +1,12 @@
-// te_submap.cu — the read side of a te_map: GetGridMap submaps of its resident layers (k_map_gather_submaps) and
-// mapHasValidTraversabilityAt for a batch of positions (k_map_valid_at).  Compiled with --fmad=false: k_map_valid_at indexes
-// positions with te_grid.cuh's getIndex, which the host and the oracle evaluate without contraction.
+// te_submap.cu — the read side of a te_map: GetGridMap submaps of its resident layers (k_map_gather_submaps),
+// mapHasValidTraversabilityAt for a batch of positions (k_map_valid_at) and GridMap::atPosition at points around poses
+// (k_map_at_poses).  Compiled with --fmad=false: k_map_valid_at and k_map_at_poses index positions with te_grid.cuh's getIndex,
+// which the host and the oracle evaluate without contraction, and k_map_at_poses places points as the polygonal paths do.
 #include <algorithm>
 
 #include "te_kernels.h"
 #include "te_grid.cuh"
+#include "te_pose.cuh"
 
 namespace te {
 namespace {
@@ -87,7 +89,45 @@ __global__ void __launch_bounds__(256) k_uncertainty_range(const float* __restri
   }
 }
 
+// GridMap::atPosition(layer, position) for every (pose, point) sample: one thread per sample (grid-stride), which places its
+// point once, indexes it once on its map, then reads every requested layer at that cell.  Consecutive threads take consecutive
+// points of a pose, so the stores of each layer coalesce; the layer reads are scattered 4-byte loads.
+__global__ void __launch_bounds__(256) k_map_at_poses(const __grid_constant__ MapAtPoses a) {
+  const long long total = (long long)a.nposes * a.npoints;
+  const size_t cells = (size_t)a.rows * a.cols;
+  const float nan = __uint_as_float(0x7fc00000u);
+  for (long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x; s < total; s += (long long)gridDim.x * blockDim.x) {
+    const int k = (int)s / a.npoints, t = (int)s - k * a.npoints;
+    const int m = a.pose_map ? __ldg(a.pose_map + k) : 0;
+    GridGeo g{a.rows, a.cols, a.res, a.lenx, a.leny, a.posx, a.posy};
+    bool ok = m >= 0 && m < a.nmaps;
+    if (ok && a.map_pos) { g.posx = __ldg(a.map_pos + 2 * m); g.posy = __ldg(a.map_pos + 2 * m + 1); }
+    const PoseRT T = pose_rt_d(a.poses + 7 * (size_t)k);
+    const double2 p = pose_point_d(T, (double)__ldg(a.points + 3 * t), (double)__ldg(a.points + 3 * t + 1),
+                                   (double)__ldg(a.points + 3 * t + 2));
+    int i = 0, j = 0;
+    ok = ok && isfinite(p.x) && isfinite(p.y) && grid_get_index(g, p.x, p.y, i, j);
+    const size_t cell = ok ? (size_t)m * cells + (size_t)j * a.rows + i : 0;
+    for (int l = 0; l < a.nlayers; ++l) {
+      float v = nan;
+      if (ok) {
+        v = __ldg(a.layer[l] + cell);
+        if (l == a.range_l) v = range_sub(v, __ldg(a.lower + cell));
+      }
+      a.out[(size_t)l * total + s] = v;
+    }
+    if (a.valid) a.valid[s] = ok ? 1 : 0;
+  }
+}
+
 }  // namespace
+
+void launch_map_at_poses(const MapAtPoses& a, int sms, cudaStream_t s) {
+  const long long total = (long long)a.nposes * a.npoints;
+  if (total <= 0) return;
+  const long long blocks = std::min<long long>((total + 255) / 256, (long long)sms * 16);
+  k_map_at_poses<<<(unsigned)blocks, 256, 0, s>>>(a);
+}
 
 void launch_uncertainty_range(const float* upper, const float* lower, float* out, size_t n, int sms, cudaStream_t s) {
   if (n == 0) return;
