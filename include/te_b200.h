@@ -869,6 +869,59 @@ typedef struct te_submap_info {
  * blocks of negative size), before any record is written. */
 int te_submap_geometry(const te_geometry* g, int32_t n, const double* position_xy, const double* length_xy, te_submap_info* info);
 
+/* ---- Updates from a larger elevation map: the reference node's main update path --------------------------------------------
+ * updateTraversability (TraversabilityEstimation.cpp:202-222) asks elevation mapping for getSubmap(robot position, mapLength_) with
+ * the layers of elevationMapLayers_ (elevation plus upper_bound / lower_bound, or the variances and time for a raw map,
+ * TraversabilityMap.cpp:64-76), and setElevationMap (:135-154) hands that submap to computeTraversability (mapOut = mapIn).  The two
+ * entries below cut the windows out of the larger map on the GPU and chain them, in one call.
+ *   - src: the elevation map, with any circular-buffer start index (elevation mapping's moves).  src_mask: TE_LAYER_ELEVATION
+ *     (required) and any of TE_LAYER_CARRIED; src_layers: a HOST array of one pointer per set bit, in bit order, each a whole map
+ *     of src's size in its buffer order, in `memory`.  robot_slope is not a source layer: elevationMapLayers_ never holds it.
+ *   - Device memory reads the source in place and is asynchronous on the context stream.  Host memory stages only the source
+ *     columns the windows touch (one copy per contiguous run of stored columns and layer, through the context's staging buffers)
+ *     and returns synchronised.  Neither can be captured in a CUDA graph: the chain synchronises for its escalation counters.
+ *   - Errors, every argument error found before anything is written (the te_map is then unchanged): TE_ERR_BAD_ARG for a bad src
+ *     geometry or start index, a src_mask without elevation or with other bits, a null src_layers, an unknown memory mode, a
+ *     non-finite position, a non-finite or negative length, and a window whose indices on the source do not fit in int32;
+ *     TE_ERR_MISSING_LAYER for a NULL layer the mask names; those of the chain parameters.
+ *   - Launches: those of the chain entry the call stands for (below), plus one k_map_cut_windows, whatever the windows and layers:
+ *     the carried layers are cut straight into their place. */
+
+/* getSubmap(position, length) on src, then te_map_chain on the submap's elevation and te_map_carry_layers on its other layers: the
+ * te_map becomes one map of the submap's geometry (start index 0) and holds, bit for bit, the layers, cache, memo, requests,
+ * submaps and te_map_get_layers that te_map_chain(g_sub, elevation) followed by te_map_carry_layers(its carried layers) give, g_sub
+ * and the layers being getSubmap's (te_submap_geometry: bounding at the edges, so clipped there).  info receives te_submap_geometry's
+ * record.  When getSubmap's isSuccess is false (info->success = 0) the call returns TE_ERR_BAD_ARG and leaves the te_map as it was,
+ * as the reference node skips the update when its submap request fails. */
+int te_map_chain_submap(te_map* map, const te_geometry* src, uint32_t src_mask, const float* src_layers[], double position_x,
+                        double position_y, double length_x, double length_y, const te_chain_params* p, te_submap_info* info, int memory);
+
+/* One window of src per map of a batch, in one call: a fleet of robot-centric maps cut out of one shared map (a GPU elevation
+ * mapper, a global map, a simulator's terrain).  map_index_or_null NULL reloads the whole batch with nmaps maps, under the rules of
+ * te_map_chain_batched_at; otherwise the nmaps maps map_index[0..nmaps) are updated under the rules of te_map_chain_maps_at (distinct
+ * host indices, g checked against the batch except for its position, the robot_slope / roughness refusal, the traversability_x /
+ * _rot fill) and every other map keeps its layers, cache and memo.  position_xy: a HOST array of the requested (robot) positions,
+ * one (x, y) pair per map updated.
+ *   - Window rule.  A batch has one size (rows n, cols m of g), while getSubmap's size moves by a cell with the position, so a
+ *     window is getSubmap's top-left with the batch's size.  g->resolution must equal src's bit for bit (TE_ERR_BAD_ARG): cells are
+ *     copied, not resampled.  The top-left corner (x + 0.5 g->length_x, y + 0.5 g->length_y) is indexed with getIndex's
+ *     expressions, floored and not checked against the source: (ti, tj), which may be negative or past the source.  Map cell (i, j)
+ *     is source cell (ti + i, tj + j), NaN 0x7fc00000 (the unknown cell) outside the source.  The map's position is getSubmap's at
+ *     that size: getPosition(ti, tj) + 0.5 res - 0.5 (n res), likewise in y (te_map_positions returns it).  For a window at least
+ *     one cell inside the source on every side, where te_submap_geometry(src, (x, y), g's length) has size (n, m), top-left,
+ *     position and cells are getSubmap's, bit for bit.
+ *   - Carried layers as te_map_carry_layers gives them: a whole-batch reload holds exactly those of src_mask; a selection may give
+ *     only layers the batch holds (TE_ERR_BAD_ARG otherwise), and the batch's other carried layers of the selected maps are filled
+ *     with NaN as te_map_chain_maps_at fills them.
+ *   - For every map, everything the te_map returns or stores equals, bit for bit, what te_map_chain_batched_at /
+ *     te_map_chain_maps_at at the window positions, followed by te_map_carry_layers, give on the cut layers.
+ *   - Launches: those of te_map_chain_batched_at / te_map_chain_maps_at on the same maps and positions plus one (on a selection of a
+ *     batch that holds more than eight carried and traversability_x / _rot layers, one fill launch fewer when the given layers bring
+ *     the fill under nine).  A selection uses the scratch of te_map_chain_maps (16 bytes per selected cell) plus the cut elevation
+ *     (4); the window table is 8 bytes per window and layer plus 8 per window, and 4 per source column in host memory. */
+int te_map_chain_windows(te_map* map, const te_geometry* g, const te_geometry* src, uint32_t src_mask, const float* src_layers[],
+                         int32_t nmaps, const int32_t* map_index_or_null, const double* position_xy, const te_chain_params* p, int memory);
+
 /* publishTraversabilityMap (TraversabilityMap.cpp:172-186): the layers of `layer_mask` (te_layer bits), each rows x cols, back to
  * back in bit order (on a batch: per layer the nmaps maps back to back, nmaps*rows*cols floats a layer).  In host memory each is re-wrapped to the map's start index, as te_map's other outputs, and the call returns
  * synchronised; in device memory they are in the map's default (unwrapped) order, asynchronously.  TE_ERR_MISSING_LAYER for a

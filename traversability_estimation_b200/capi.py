@@ -197,6 +197,8 @@ SIGNATURES = {
     "te_map_request_stats": (_R, [_P, _P]),
     "te_map_carry_layers": (_R, [_P, _I, _P, _U, _P, _I]),
     "te_submap_geometry": (_R, [_G, _I, _P, _P, _P]),
+    "te_map_chain_submap": (_R, [_P, _G, _U, _P, _D, _D, _D, _D, _CP, _P, _I]),
+    "te_map_chain_windows": (_R, [_P, _G, _G, _U, _P, _I, _P, _P, _CP, _I]),
     "te_map_get_layers": (_R, [_P, _U, _P, _I]),
     "te_map_get_submaps": (_R, [_P, _I, _P, _P, _U, _P, _P, _L, _I]),
     "te_map_get_submaps_batched": (_R, [_P, _I, _P, _P, _P, _U, _P, _P, _L, _I]),
@@ -935,6 +937,52 @@ class Map:
         else:
             idx = self._map_index(map_index)
             self._check(self._L.te_map_carry_layers(self._h, len(idx), _addr(idx), mask, ptrs, memory))
+
+    def _source(self, layers, memory):
+        """(mask, pointer array) of a source map's layers for chain_submap / chain_windows: layers a dict name -> layer, elevation
+        and CARRIED_LAYERS entries.  Host memory: numpy (rows, cols) arrays in the source's buffer order (its start index), kept
+        alive in the returned tuple.  Device memory: float32 device tensors of rows * cols, column-major in buffer order."""
+        mask = layer_mask(list(layers))
+        if memory == MEM_HOST:
+            given = {n: np.asfortranarray(a, dtype=np.float32) for n, a in layers.items()}
+        else:
+            given = dict(layers)
+            self._ctx._order_after_torch(memory)
+        ordered = [given[n] for n in layer_order(mask)]
+        return mask, (C.c_void_p * len(ordered))(*(_addr(a) for a in ordered)), ordered
+
+    def chain_submap(self, src_g, layers, position, length, p, memory=MEM_HOST):
+        """te_map_chain_submap (requestElevationMap -> setElevationMap -> computeTraversability): getSubmap(position, length) of
+        the source map `src_g` (any start index), then the chain on its elevation and its other layers carried.  layers: a dict
+        name -> source layer, "elevation" and any CARRIED_LAYERS (see _source).  Returns the window's SubmapInfo; when getSubmap
+        fails (info.success == 0) the map is left as it was and nothing is raised, as the reference node skips that update.  The
+        map then holds one map of the submap's geometry (start index 0)."""
+        mask, ptrs, _keep = self._source(layers, memory)
+        info = SubmapInfo()
+        info.success = -1   # the library writes the record once every argument is checked
+        rc = self._L.te_map_chain_submap(self._h, C.byref(src_g), mask, ptrs, float(position[0]), float(position[1]), float(length[0]),
+                                         float(length[1]), C.byref(p), C.byref(info), memory)
+        if rc != 0 and info.success != 0:
+            self._check(rc)
+        if rc == 0:
+            self._g = Geometry(info.rows, info.cols, src_g.resolution, info.length_x, info.length_y, info.position_x, info.position_y,
+                               0, 0)
+            self._n = 1
+        return info
+
+    def chain_windows(self, g, src_g, layers, positions, p, map_index=None, memory=MEM_HOST):
+        """te_map_chain_windows: one window of g's size per map, cut out of the source map `src_g` at the requested (robot)
+        positions (n, 2) and chained, its other layers carried.  layers as in chain_submap.  map_index None reloads the whole batch
+        with n maps; otherwise the maps map_index[j] get the window at positions[j] and every other map keeps its state."""
+        mask, ptrs, _keep = self._source(layers, memory)
+        xy = np.ascontiguousarray(positions, dtype=np.float64).reshape(-1, 2)
+        idx = None if map_index is None else self._map_index(map_index)
+        if idx is not None and len(idx) != len(xy):
+            raise ValueError(f"{len(idx)} map indices but {len(xy)} positions")
+        self._check(self._L.te_map_chain_windows(self._h, C.byref(g), C.byref(src_g), mask, ptrs, len(xy), _addr(idx), _addr(xy),
+                                                 C.byref(p), memory))
+        if idx is None:
+            self._g, self._n = g, len(xy)
 
     def footprint_maps(self, fp, map_index):
         """te_map_footprint_maps (traversabilityFootprint(radius, offset) on the caches of the maps map_index only); returns those

@@ -1346,6 +1346,7 @@ struct te_map {
   // The _maps entries: the selected maps' layers packed back to back (grown to the largest selection) and their slot table
   DevBuf sel[te::kMapSlotLayers], slots;
   DevBuf image;  // te_map_chain_image(_maps) in host memory: the staged image bytes, packed
+  DevBuf cut;    // te_map_chain_submap / te_map_chain_windows: the window table of k_map_cut_windows
   bool have_rough = false, have_rslope = false;
   te::FootprintState fp;  // the map's own scratch; fp.memo is the resident memo
   bool memo_valid = false;
@@ -1670,8 +1671,10 @@ cudaError_t map_copy_packed(te_map* m, float* dst, const float* src, size_t n, b
 // The packed layers src (each null or nsel maps back to back) into the selected maps' resident layers dst, in one launch that also
 // empties those maps' caches, fills their carried and polygon layers with NaN (the new maps come without them, but every map of a
 // batch holds the same layers) and, when the memo is live, clears their memo bytes.  The te_map-wide memo key stays.  A batch
-// that holds more than kMapSlotLayers such layers fills the rest in a second launch.
-int map_put_selected(te_map* m, const MapSel& s, const float* const src[te::kMapSlotLayers], DevBuf* const dst[te::kMapSlotLayers]) {
+// that holds more than kMapSlotLayers such layers fills the rest in a second launch.  keep: carried layer bits whose slots of the
+// selected maps the caller has already written (te_map_chain_windows): those are not filled.
+int map_put_selected(te_map* m, const MapSel& s, const float* const src[te::kMapSlotLayers], DevBuf* const dst[te::kMapSlotLayers],
+                     uint32_t keep = 0) {
   te_ctx* c = m->ctx;
   te::MapSlots a{};
   for (int l = 0; l < te::kMapSlotLayers; ++l) {
@@ -1680,7 +1683,7 @@ int map_put_selected(te_map* m, const MapSel& s, const float* const src[te::kMap
   }
   std::vector<float*> fill;
   for (int k = 0; k < 7; ++k)
-    if ((m->carried >> (kCarryBit0 + k)) & 1u) fill.push_back((float*)m->carry[k].p);
+    if (((m->carried & ~keep) >> (kCarryBit0 + k)) & 1u) fill.push_back((float*)m->carry[k].p);
   if (m->have_fpoly)
     for (DevBuf& b : m->fpoly) fill.push_back((float*)b.p);
   const int nf = std::min((int)fill.size(), te::kMapSlotLayers);
@@ -1726,7 +1729,7 @@ int te_map_destroy(te_map* m) {
     Guard g(m->ctx);
     if (g.ok) {
       cudaStreamSynchronize(m->ctx->stream);
-      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather, &m->slots, &m->image})
+      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather, &m->slots, &m->image, &m->cut})
         b->release();
       for (DevBuf& b : m->sel) b.release();
       for (DevBuf& b : m->carry) b.release();
@@ -1750,10 +1753,23 @@ struct ImageIn {
   double min_height, max_height;
 };
 
-// Where map_chain's elevation comes from: a float32 layer, or images that k_image_to_layer turns into one.
+// te_map_chain_submap / te_map_chain_windows' source: a larger elevation map (any start index) with the layers of `mask`
+// (elevation and carried layers, in bit order, in `memory`), and where each window of the call starts in it, in launch order.
+struct CutIn {
+  const te_geometry* src;
+  uint32_t mask;
+  int nlayers;
+  const float* layers[te::kCutMaxLayers];
+  int memory;
+  std::vector<int2> top;
+};
+
+// Where map_chain's elevation comes from: a float32 layer, images that k_image_to_layer turns into one, or windows that
+// k_map_cut_windows cuts out of a larger map together with its carried layers.
 struct ElevSource {
   const float* layer;
   const ImageIn* image;
+  const CutIn* cut;
 };
 
 // Validates nmaps images of geometry g and returns their bytes per pixel.  Writes nothing.
@@ -1800,9 +1816,88 @@ int map_convert_image(te_map* m, const te_geometry& g, const ImageIn& im, int bp
   return launch_check(c, "k_image_to_layer");
 }
 
-// te_map_chain (nmaps = 1), te_map_chain_batched and, with a selection, te_map_chain_maps, from an elevation layer or from images
-// (te_map_chain_image(_maps)): the selected maps' layers are chained into scratch (the elevation staged there in host memory,
-// read in place in device memory; images converted there in both) and k_map_slots puts them in place.
+// The windows of `cut` into the maps of a chain launch of geometry m->geo, in one launch: the elevation of map k of the launch to
+// elev + k * cells (the te_map's layer on a whole-batch update, the selection's packed scratch otherwise), each carried layer
+// straight to its resident slot (map k, or sel->idx[k]).  Device sources are read in place; host sources stage only the source
+// columns the windows touch, one copy per contiguous run of stored columns and layer, and the kernel finds them through a
+// column table.
+int map_cut(te_map* m, const CutIn& cut, const MapSel* sel, float* elev) {
+  te_ctx* c = m->ctx;
+  const te_geometry& s = *cut.src;
+  const int n = (int)cut.top.size(), nl = cut.nlayers, rows = m->geo.rows, cols = m->geo.cols;
+  const size_t cells = map_cells(m);
+  std::vector<float*> dst((size_t)n * nl);
+  int l = 0;
+  for (int b = 0; b < kLayerBits; ++b) {
+    if (!((cut.mask >> b) & 1u)) continue;
+    float* base = elev;
+    if (b != 4) {
+      DevBuf& buf = m->carry[b - kCarryBit0];
+      if (!sel) TE_CUDA(buf.reserve(sizeof(float) * batch_cells(m)));
+      base = (float*)buf.p;
+    }
+    for (int k = 0; k < n; ++k) dst[(size_t)k * nl + l] = base + (size_t)(b != 4 && sel ? sel->idx[k] : k) * cells;
+    ++l;
+  }
+  te::WindowCut a{};
+  std::vector<int> col_of;
+  for (int k = 0; k < nl; ++k) a.src[k] = cut.layers[k];
+  if (cut.memory == TE_MEM_HOST) {
+    std::vector<char> touched(s.cols, 0);
+    for (const int2& t : cut.top)
+      for (long long J = std::max(0LL, (long long)t.y); J < std::min((long long)s.cols, (long long)t.y + cols); ++J)
+        touched[(J + s.start_col) % s.cols] = 1;
+    col_of.assign(s.cols, -1);
+    int nst = 0;
+    for (int j = 0; j < s.cols; ++j)
+      if (touched[j]) col_of[j] = nst++;
+    Staging st(c, true, &s);
+    float* staged = (float*)st.slot(sizeof(float) * s.rows * (size_t)nst * nl);
+    if (st.rc) return st.rc;
+    for (int j = 0; j < s.cols;) {  // runs of touched stored columns
+      if (!touched[j]) { ++j; continue; }
+      int e = j;
+      while (e < s.cols && touched[e]) ++e;
+      for (int k = 0; k < nl; ++k)
+        TE_CUDA(cudaMemcpyAsync(staged + ((size_t)k * nst + col_of[j]) * s.rows, cut.layers[k] + (size_t)j * s.rows,
+                                sizeof(float) * s.rows * (size_t)(e - j), cudaMemcpyHostToDevice, c->stream));
+      j = e;
+    }
+    for (int k = 0; k < nl; ++k) a.src[k] = staged + (size_t)k * nst * s.rows;
+  }
+  // the table: destination pointers, then the windows' top-left cells, then (host sources) the staged column of each stored one
+  const size_t pbytes = sizeof(float*) * dst.size(), tbytes = sizeof(int2) * n, cbytes = sizeof(int) * col_of.size();
+  std::vector<char> h(pbytes + tbytes + cbytes);
+  std::memcpy(h.data(), dst.data(), pbytes);
+  std::memcpy(h.data() + pbytes, cut.top.data(), tbytes);
+  if (cbytes) std::memcpy(h.data() + pbytes + tbytes, col_of.data(), cbytes);
+  if (m->cut.p && m->cut.cap < h.size()) TE_CUDA(cudaStreamSynchronize(c->stream));  // an earlier cut may still read it
+  TE_CUDA(m->cut.reserve(h.size()));
+  // pageable source: consumed before cudaMemcpyAsync returns, ordered after the kernels queued before on the stream
+  TE_CUDA(cudaMemcpyAsync(m->cut.p, h.data(), h.size(), cudaMemcpyHostToDevice, c->stream));
+  const char* t = (const char*)m->cut.p;
+  a.dst = (float* const*)t;
+  a.top = (const int2*)(t + pbytes);
+  a.col_of = cbytes ? (const int*)(t + pbytes + tbytes) : nullptr;
+  a.nlayers = nl;
+  a.nmaps = n;
+  a.rows = rows;
+  a.cols = cols;
+  a.src_rows = s.rows;
+  a.src_cols = s.cols;
+  a.start_row = s.start_row;
+  a.start_col = s.start_col;
+  a.ncolumns = (long long)n * nl * cols;
+  te::launch_cut_windows(a, c->sms, c->stream);
+  return launch_check(c, "k_map_cut_windows");
+}
+
+// te_map_chain (nmaps = 1), te_map_chain_batched and, with a selection, te_map_chain_maps, from an elevation layer, from images
+// (te_map_chain_image(_maps)) or from windows of a larger map (te_map_chain_submap / _windows): the selected maps' layers are
+// chained into scratch (the elevation staged there in host memory, read in place in device memory; images converted and windows
+// cut there in both) and k_map_slots puts them in place.  Windows also carry the source's carried layers: on a whole batch they
+// replace the batch's, on a selection they go straight to the selected maps' slots and only the batch's other carried layers are
+// filled with NaN.
 // at: an _at entry, whose maps go to position_xy (null: g's position) and whose g may differ from the batch's in its position.
 int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int nmaps, const ElevSource& src, float* slope, float* step,
               float* rough, float* trav, int memory, const MapSel* sel = nullptr, bool at = false, const double* position_xy = nullptr) {
@@ -1814,13 +1909,17 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
     if (int rc = map_select(m, true, g_in, *sel, at)) return rc;
     g0 = m->geo;
     nmaps = sel->n;
-  } else if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) {
+  } else if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1 && !src.cut, &g0)) {
     return rc;
   }
   if (int rc = check_params(p)) return rc;
   if (nmaps > 0)
     if (int rc = check_positions(position_xy, nmaps)) return rc;
-  if (!src.layer && !src.image) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
+  if (!src.layer && !src.image && !src.cut) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
+  if (sel && src.cut)
+    if (const uint32_t extra = src.cut->mask & TE_LAYER_CARRIED & ~m->carried)
+      return fail(TE_ERR_BAD_ARG, "layer %s is given to some maps but the batch does not hold it: every map of a batch holds the same "
+                  "layers, so give it to every map (map_index NULL)", kLayerNames[__builtin_ctz(extra)]);
   if (sel && (m->have_rslope || !m->have_rough))
     return fail(TE_ERR_UNSUPPORTED, "the batch %s, and te_map_chain_maps gives a map roughness and no robot_slope: every map of a batch holds "
                 "the same layers, so use te_map_set_layers_maps or reload the whole batch",
@@ -1833,7 +1932,7 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
   const size_t cells = map_cells(m) * (sel ? sel->n : 0);
   const float* din = src.layer;
   if (sel) {
-    const bool packed = memory == TE_MEM_HOST || src.image;  // sel[0]: the staged or converted elevation
+    const bool packed = memory == TE_MEM_HOST || src.image || src.cut;  // sel[0]: the staged, converted or cut elevation
     if (int rc = map_stage_selection(m, *sel, packed ? 0x1fu : 0x1eu)) return rc;
     if (memory == TE_MEM_HOST && src.layer) {
       TE_CUDA(map_copy_packed(m, (float*)lay[0]->p, src.layer, cells, false, memory));
@@ -1850,6 +1949,11 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
     if (int rc = map_convert_image(m, g0, *src.image, bpp, nmaps, memory, (float*)lay[0]->p)) return rc;
     din = (const float*)lay[0]->p;
   }
+  if (src.cut) {
+    if (int rc = map_cut(m, *src.cut, sel, (float*)lay[0]->p)) return rc;
+    din = (const float*)lay[0]->p;
+    if (!sel) m->carried = src.cut->mask & TE_LAYER_CARRIED;
+  }
   // where the launch's maps go; maps away from g0's position take per-map tables
   const std::vector<double> at_xy = launch_positions(position_xy, nmaps, g_in->position_x, g_in->position_y);
   PosTables tab{};
@@ -1864,7 +1968,7 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
     const float* const src_l[te::kMapSlotLayers] = {(const float*)lay[4]->p, (const float*)lay[1]->p, (const float*)lay[2]->p,
                                                     (const float*)lay[3]->p, din, nullptr};
     DevBuf* const dst[te::kMapSlotLayers] = {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, nullptr};
-    if (int rc = map_put_selected(m, *sel, src_l, dst)) return rc;
+    if (int rc = map_put_selected(m, *sel, src_l, dst, src.cut ? src.cut->mask & TE_LAYER_CARRIED : 0u)) return rc;
   } else {
     m->have_rough = true;
     m->have_rslope = false;  // computeTraversability leaves robot_slope to a later setTraversabilityMap
@@ -2609,6 +2713,85 @@ int submap_windows(const te_geometry* g, int32_t n, const double* pos, const dou
 int te_submap_geometry(const te_geometry* g, int32_t n, const double* position_xy, const double* length_xy, te_submap_info* info) {
   if (int rc = check_geometry(g, true)) return rc;
   return submap_windows(g, n, position_xy, length_xy, 1, info, nullptr);
+}
+
+// ---- The update from a larger elevation map: requestElevationMap's getSubmap, then setElevationMap and computeTraversability ----
+namespace {
+
+// Validates the source of te_map_chain_submap / _windows into `out` (windows still empty).  Writes nothing.
+int cut_source(const te_geometry* src, uint32_t mask, const float* layers[], int memory, CutIn* out) {
+  if (memory != TE_MEM_HOST && memory != TE_MEM_DEVICE) return fail(TE_ERR_BAD_ARG, "unknown memory mode %d", memory);
+  if (int rc = check_geometry(src, true)) return rc;
+  const uint32_t allowed = (uint32_t)TE_LAYER_ELEVATION | (uint32_t)TE_LAYER_CARRIED;
+  if (!(mask & TE_LAYER_ELEVATION) || (mask & ~allowed))
+    return fail(TE_ERR_BAD_ARG, "source mask 0x%x: need elevation (0x%x) and any of the elevation map's carried layers (0x%x)", mask,
+                (unsigned)TE_LAYER_ELEVATION, (unsigned)TE_LAYER_CARRIED);
+  if (!layers) return fail(TE_ERR_BAD_ARG, "layers is null");
+  out->src = src;
+  out->mask = mask;
+  out->memory = memory;
+  out->nlayers = 0;
+  for (int b = 0; b < kLayerBits; ++b) {
+    if (!((mask >> b) & 1u)) continue;
+    const float* l = layers[out->nlayers];
+    if (!l) return fail(TE_ERR_MISSING_LAYER, "layer %s is missing: the source mask names it", kLayerNames[b]);
+    out->layers[out->nlayers++] = l;
+  }
+  return TE_OK;
+}
+
+}  // namespace
+
+int te_map_chain_submap(te_map* m, const te_geometry* src, uint32_t src_mask, const float* src_layers[], double position_x,
+                        double position_y, double length_x, double length_y, const te_chain_params* p, te_submap_info* info,
+                        int memory) {
+  TE_MAP_ENTER(m);
+  CutIn cut;
+  if (int rc = cut_source(src, src_mask, src_layers, memory, &cut)) return rc;
+  if (int rc = check_params(p)) return rc;
+  if (!info) return fail(TE_ERR_BAD_ARG, "info is null");
+  const double pos[2] = {position_x, position_y}, len[2] = {length_x, length_y};
+  te_submap_info r{};
+  if (int rc = submap_windows(src, 1, pos, len, 1, &r, nullptr)) return rc;
+  *info = r;
+  if (!r.success)
+    return fail(TE_ERR_BAD_ARG, "getSubmap((%g, %g), (%g, %g)) fails on the source map: the te_map is left as it was", position_x,
+                position_y, length_x, length_y);
+  const te_geometry g{r.rows, r.cols, src->resolution, r.length_x, r.length_y, r.position_x, r.position_y, 0, 0};
+  cut.top.push_back(int2{r.top_row, r.top_col});
+  return map_chain(m, &g, p, 1, ElevSource{nullptr, nullptr, &cut}, nullptr, nullptr, nullptr, nullptr, memory);
+}
+
+int te_map_chain_windows(te_map* m, const te_geometry* g, const te_geometry* src, uint32_t src_mask, const float* src_layers[],
+                         int32_t nmaps, const int32_t* map_index, const double* position_xy, const te_chain_params* p, int memory) {
+  TE_MAP_ENTER(m);
+  CutIn cut;
+  if (int rc = cut_source(src, src_mask, src_layers, memory, &cut)) return rc;
+  if (int rc = check_geometry(g, true)) return rc;
+  if (std::memcmp(&g->resolution, &src->resolution, sizeof(double)) != 0)
+    return fail(TE_ERR_BAD_ARG, "resolution %.17g differs from the source's %.17g: windows copy cells, they do not resample", g->resolution,
+                src->resolution);
+  if (nmaps < 1) return fail(TE_ERR_BAD_ARG, "number of maps must be positive");
+  if (!position_xy) return fail(TE_ERR_BAD_ARG, "position_xy is null");
+  if (int rc = check_positions(position_xy, nmaps)) return rc;
+  // getSubmap's top-left index with the batch's size: floored, so that it may lie outside the source, and within int32
+  const te::GridGeo A{src->rows, src->cols, src->resolution, src->length_x, src->length_y, src->position_x, src->position_y};
+  std::vector<double> at(2 * (size_t)nmaps);
+  cut.top.resize(nmaps);
+  for (int32_t k = 0; k < nmaps; ++k) {
+    double ti, tj;
+    te::grid_window_top(A, position_xy[2 * k] + 0.5 * g->length_x, position_xy[2 * k + 1] + 0.5 * g->length_y, ti, tj);
+    if (!(ti >= (double)INT32_MIN && ti + (g->rows - 1) <= (double)INT32_MAX && tj >= (double)INT32_MIN &&
+          tj + (g->cols - 1) <= (double)INT32_MAX))
+      return fail(TE_ERR_BAD_ARG, "window %d at (%g, %g): its cells' indices on the source do not fit in int32", k, position_xy[2 * k],
+                  position_xy[2 * k + 1]);
+    cut.top[k] = int2{(int)ti, (int)tj};
+    te::grid_window_position(A, (int)ti, (int)tj, g->rows, g->cols, at[2 * k], at[2 * k + 1]);
+  }
+  if (!map_index) return map_chain(m, g, p, nmaps, ElevSource{nullptr, nullptr, &cut}, nullptr, nullptr, nullptr, nullptr, memory, nullptr,
+                                   true, at.data());
+  const MapSel sel{nmaps, map_index};
+  return map_chain(m, g, p, nmaps, ElevSource{nullptr, nullptr, &cut}, nullptr, nullptr, nullptr, nullptr, memory, &sel, true, at.data());
 }
 
 int te_map_get_layers(te_map* m, uint32_t layer_mask, float* out, int memory) {

@@ -86,6 +86,24 @@ __host__ __device__ __forceinline__ bool grid_submap(const G& A, double px, doub
   return true;
 }
 
+// te_map_chain_windows' window of a fixed size rows x cols whose top-left corner is (px, py): the index getIndex finds for the
+// corner, floored instead of truncated and not checked against the map (so -1, not 0, for a corner less than a cell above the
+// map), as doubles that may lie outside the map or int32; and the window's position, grid_submap's expressions at that index and
+// size.  For a window inside the map whose getSubmap has that size, both are getSubmap's.
+template <class G>
+__host__ __device__ __forceinline__ void grid_window_top(const G& A, double px, double py, double& ti, double& tj) {
+  const double vx = ((px - 0.5 * A.lenx) - A.posx) / A.res;
+  const double vy = ((py - 0.5 * A.leny) - A.posy) / A.res;
+  ti = floor(-vx);
+  tj = floor(-vy);
+}
+template <class G>
+__host__ __device__ __forceinline__ void grid_window_position(const G& A, int ti, int tj, int rows, int cols, double& px, double& py) {
+  const double cornx = cell_coord(A.posx, A.lenx, A.res, ti) + 0.5 * A.res, corny = cell_coord(A.posy, A.leny, A.res, tj) + 0.5 * A.res;
+  px = cornx - 0.5 * ((double)rows * A.res);
+  py = corny - 0.5 * ((double)cols * A.res);
+}
+
 // grid_map::LineIterator (Bresenham) from index (i0, j0) to (i1, j1): `n` cells, (li, lj) the current one.
 struct LineD {
   int li, lj, i1x, i2x, i1y, i2y, den, num, numAdd, n;

@@ -93,6 +93,24 @@ struct MapAtPoses {
 // One k_map_at_poses launch (none for nposes = 0).
 void launch_map_at_poses(const MapAtPoses& a, int sms, cudaStream_t s);
 
+// te_map_chain_submap / te_map_chain_windows: nmaps windows of rows x cols cells cut out of the layers of a larger map (device
+// pointers).  Window k starts at source cell top[k] = (row, col), which may lie outside the source; layer l of window k goes
+// column-major to dst[k * nlayers + l].  Source cell (I, J) is stored at src[l][col_of(Jb) * src_rows + Ib], (Ib, Jb) = (I +
+// start_row, J + start_col) modulo the source size and col_of the identity, or the table col_of when only some source columns
+// were staged; a cell outside the source is NaN 0x7fc00000.
+constexpr int kCutMaxLayers = 8;  // elevation and the seven carried layers
+struct WindowCut {
+  const float* src[kCutMaxLayers];
+  const int2* top;         // device, nmaps
+  float* const* dst;       // device, nmaps * nlayers
+  const int* col_of;       // device, src_cols entries, or null
+  int nlayers, nmaps, rows, cols;
+  int src_rows, src_cols, start_row, start_col;
+  long long ncolumns;      // nmaps * nlayers * cols
+};
+// One k_map_cut_windows launch for every column of every window and layer (none when there is no column).
+void launch_cut_windows(const WindowCut& a, int sms, cudaStream_t s);
+
 // te_image.cu — addLayerFromImage for mono images: nmaps row-major images of rows x cols pixels (image m at px + m * image_stride
 // bytes, its row i at + i * row_stride bytes; device memory, 2-byte pixels at even addresses and strides) into nmaps column-major
 // float32 layers back to back at out: out[m*rows*cols + j*rows + i] = lower + diff * (pixel(m, i, j) / max pixel value).

@@ -1,6 +1,6 @@
 // te_submap.cu — the read side of a te_map: GetGridMap submaps of its resident layers (k_map_gather_submaps),
 // mapHasValidTraversabilityAt for a batch of positions (k_map_valid_at) and GridMap::atPosition at points around poses
-// (k_map_at_poses).  Compiled with --fmad=false: k_map_valid_at and k_map_at_poses index positions with te_grid.cuh's getIndex,
+// (k_map_at_poses); and the windows a te_map update cuts out of a larger elevation map (k_map_cut_windows).  Compiled with --fmad=false: k_map_valid_at and k_map_at_poses index positions with te_grid.cuh's getIndex,
 // which the host and the oracle evaluate without contraction, and k_map_at_poses places points as the polygonal paths do.
 #include <algorithm>
 
@@ -42,6 +42,67 @@ __global__ void __launch_bounds__(kGatherWarps * 32) k_map_gather_submaps(Submap
       for (int e = lane; e < nv; e += 32) d4[e] = __ldg(s4 + e);
       for (int e = head + 4 * nv + lane; e < n; e += 32) dst[e] = __ldg(src + e);
     }
+  }
+}
+
+// n floats from src to dst by one warp: 16-byte accesses where the two agree modulo 16 bytes, 4-byte ones otherwise.
+__device__ __forceinline__ void warp_copy_run(float* __restrict__ dst, const float* __restrict__ src, int n, int lane) {
+  int head = n;  // elements copied one by one before the 16-byte body
+  if ((((uintptr_t)src ^ (uintptr_t)dst) & 15) == 0) head = min(n, (int)(((16 - ((uintptr_t)src & 15)) & 15) >> 2));
+  for (int e = lane; e < head; e += 32) dst[e] = __ldg(src + e);
+  if (head < n) {
+    const int nv = (n - head) >> 2;
+    const float4* __restrict__ s4 = reinterpret_cast<const float4*>(src + head);
+    float4* __restrict__ d4 = reinterpret_cast<float4*>(dst + head);
+    for (int e = lane; e < nv; e += 32) d4[e] = __ldg(s4 + e);
+    for (int e = head + 4 * nv + lane; e < n; e += 32) dst[e] = __ldg(src + e);
+  }
+}
+
+// n copies of v at dst by one warp, 16-byte stores from the first 16-byte boundary on.
+__device__ __forceinline__ void warp_fill_run(float* __restrict__ dst, float v, int n, int lane) {
+  const int head = min(n, (int)(((16 - ((uintptr_t)dst & 15)) & 15) >> 2));
+  for (int e = lane; e < head; e += 32) dst[e] = v;
+  const int nv = (n - head) >> 2;
+  float4* __restrict__ d4 = reinterpret_cast<float4*>(dst + head);
+  for (int e = lane; e < nv; e += 32) d4[e] = make_float4(v, v, v, v);
+  for (int e = head + 4 * nv + lane; e < n; e += 32) dst[e] = v;
+}
+
+// One warp per destination column, numbered flat over (map, layer, column): column j of layer l of map k is the source column
+// top[k].y + j from source row top[k].x on, read through the source's circular-buffer start index, so at most two contiguous
+// runs of the stored column (before and after the row wrap), and NaN 0x7fc00000 (grid_map's unknown cell) for the rows and columns
+// the window takes from outside the source.  Integer arithmetic only: the host placed the windows.
+__global__ void __launch_bounds__(kGatherWarps * 32) k_map_cut_windows(const __grid_constant__ WindowCut a) {
+  const int lane = threadIdx.x & 31;
+  const float nan = __uint_as_float(0x7fc00000u);
+  const long long per_map = (long long)a.nlayers * a.cols;
+  const long long nwarps = (long long)gridDim.x * kGatherWarps;
+  for (long long c = (long long)blockIdx.x * kGatherWarps + (threadIdx.x >> 5); c < a.ncolumns; c += nwarps) {
+    const int k = (int)(c / per_map);
+    const int r = (int)(c - (long long)k * per_map);
+    const int l = r / a.cols, j = r - l * a.cols;
+    const int2 t = __ldg(a.top + k);
+    float* __restrict__ dst = a.dst[(size_t)k * a.nlayers + l] + (size_t)j * a.rows;
+    const long long J = (long long)t.y + j;  // the source column
+    int i0 = 0, i1 = 0;                      // window rows [i0, i1) lie in the source
+    if (J >= 0 && J < a.src_cols) {
+      i0 = (int)max(0LL, -(long long)t.x);
+      i1 = (int)min((long long)a.rows, (long long)a.src_rows - t.x);
+      if (i1 <= i0) i0 = i1 = 0;
+    }
+    warp_fill_run(dst, nan, i0, lane);
+    if (i1 > i0) {
+      int sc = (int)J + a.start_col;
+      if (sc >= a.src_cols) sc -= a.src_cols;
+      const float* __restrict__ col = a.src[l] + (size_t)(a.col_of ? __ldg(a.col_of + sc) : sc) * a.src_rows;
+      int s0 = t.x + i0 + a.start_row;  // stored row of window row i0
+      if (s0 >= a.src_rows) s0 -= a.src_rows;
+      const int n = i1 - i0, n1 = min(n, a.src_rows - s0);
+      warp_copy_run(dst + i0, col + s0, n1, lane);
+      if (n1 < n) warp_copy_run(dst + i0 + n1, col, n - n1, lane);
+    }
+    warp_fill_run(dst + i1, nan, a.rows - i1, lane);
   }
 }
 
@@ -142,6 +203,12 @@ void launch_gather_submaps(const SubmapGather& a, int sms, cudaStream_t s) {
   if (a.ncolumns <= 0) return;
   const long long blocks = std::min<long long>((a.ncolumns + kGatherWarps - 1) / kGatherWarps, (long long)sms * 16);
   k_map_gather_submaps<<<(unsigned)blocks, kGatherWarps * 32, 0, s>>>(a);
+}
+
+void launch_cut_windows(const WindowCut& a, int sms, cudaStream_t s) {
+  if (a.ncolumns <= 0) return;
+  const long long blocks = std::min<long long>((a.ncolumns + kGatherWarps - 1) / kGatherWarps, (long long)sms * 16);
+  k_map_cut_windows<<<(unsigned)blocks, kGatherWarps * 32, 0, s>>>(a);
 }
 
 void launch_valid_at(const GridGeo& g, const float* trav, int n, const double* xy, const int* pos_map, int nmaps, const double* map_pos,
