@@ -52,8 +52,9 @@ inline int reach_generous(double radius, double res) {
   const int R = (int)std::floor(q);
   return (q - (double)R > 1.0 - 1e-6) ? R + 1 : R;
 }
-// Dependency radius in cells (what a slab halo must provide).
-inline int reach_true(double radius, double res) { return (int)std::floor(radius / res + 1e-9); }
+// Dependency radius in cells (what a slab halo must provide): the largest offset the reference's circle test on absolute cell
+// centres can admit, for coordinates of spacing cu (lattice_reach).
+inline int reach_true(double radius, double res, double cu) { return te::lattice_reach(radius, res, cu); }
 
 }  // namespace
 
@@ -162,8 +163,10 @@ te::ChainDev make_chain_dev(const te_geometry* g, const te_chain_params* p) {
 
 int chain_halo(const te_geometry* g, const te_chain_params* p) {
   const double res = g->resolution;
-  const int hn = reach_true(p->normals_radius, res), hr = reach_true(p->roughness_radius, res);
-  const int hs = reach_true(p->step_first_radius, res) + reach_true(p->step_second_radius, res);
+  const double rmax = std::max(std::max(p->normals_radius, p->roughness_radius), p->step_first_radius + p->step_second_radius);
+  const double cu = te::coord_ulp(std::max(std::fabs(g->position_x) + 0.5 * g->length_x, std::fabs(g->position_y) + 0.5 * g->length_y) + rmax);
+  const int hn = reach_true(p->normals_radius, res, cu), hr = reach_true(p->roughness_radius, res, cu);
+  const int hs = reach_true(p->step_first_radius, res, cu) + reach_true(p->step_second_radius, res, cu);
   return std::max(hn, std::max(hr, hs));
 }
 
@@ -397,7 +400,7 @@ int run_chain_device(te_ctx* c, const te_geometry* g, const te::SlabView& v, con
   const te::ChainDev d = make_chain_dev(g, p);
   bool use_fused = false;
   if (c->kernel_choice != TE_KERNEL_GENERIC) {
-    use_fused = te::fused_eligible(c->fused, c->hX, c->hY, g, p, c->stream);
+    use_fused = te::fused_eligible(c->fused, c->hX, c->hY, g, p, v.coord_max, c->stream);
     if (!use_fused && c->kernel_choice == TE_KERNEL_FUSED)
       return fail(TE_ERR_UNSUPPORTED, "fused stencil has no instantiation for these window shapes: %s", c->fused.why.c_str());
     if (use_fused) {

@@ -461,7 +461,18 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
   const Layers L{trav, slope, step, elev, rough};
   const long long t1 = (long long)ncell_in, t2 = (long long)v.rows * v.out_ncols * nmaps;
   const int g2 = (int)std::min<long long>((t2 + 255) / 256, (long long)sms * 8);
-  const int Lmax = (int)std::floor(rmax / g->resolution + 1e-9);
+  // The tables classify lattice offsets (k, l) by d2 = (k^2 + l^2) res^2 against r2 = rmax^2; the reference tests the same cell with
+  // dx * dx + dy * dy <= r2 on absolute cell centres, dx = X[a] - X[i] (likewise dy).  Each centre is (B + res * (-idx)) rounded,
+  // B = (position + offset) rounded once per map and so common to both, and res * (-idx) is below 2M in magnitude: dx is
+  // -k res + e with |e| <= 2 ulp(M) (two products and two sums, half an ulp each), M the largest |coordinate| the call touches.
+  // Then dx^2 + dy^2 = d2 + 2 res (|k| + |l|) * 2 ulp(M) at most = d2 + 4 sqrt(2) r ulp(M) near the circle, plus relative roundings
+  // of a few 2^-53 that 1e-9 r2 covers.  tol = max(1e-9 r2, 8 r ulp(M)): an offset closer than that to the circle goes to the
+  // uncertain list and is decided per centre on absolute doubles.  Near the origin 1e-9 r2 is the larger one, so the tables are
+  // what they always were; far out (a UTM or LV95 map) more offsets become uncertain.  Lmax, the largest |offset| that can be
+  // inside, widens with the same bound.
+  const double res = g->resolution, r2 = rmax * rmax, cu = coord_ulp(v.coord_max + rmax);
+  const double tol_far = 8.0 * rmax * cu, tol = std::max(1e-9 * r2, tol_far) + 1e-300;
+  const int Lmax = lattice_reach(rmax, res, cu);
   const bool fast = Lmax <= 31 && v.out_ncols <= 65535 && std::getenv("TE_FOOTPRINT_BRUTE") == nullptr;
   if (!fast) {
     (a.pos ? k_sweep<true> : k_sweep<false>)<<<std::max(g2, 1), 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
@@ -469,8 +480,7 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
     return 0;
   }
   // ---- prefix-sum sweep: tables (cached with the spiral) + per-call prefix/bit arrays -----------------
-  if (!st.tables_valid) {
-    const double res = g->resolution, r2 = rmax * rmax, tol = 1e-9 * r2 + 1e-300;
+  if (!st.tables_valid || st.tables_ulp != cu) {  // maps of an _at entry move M: the tables follow the tolerance
     const int nR = (int)std::ceil(rmax / res), Wd = 2 * Lmax + 1;
     std::vector<signed char> halfw(Wd, -1), inner((size_t)(nR + 2) * Wd, -1);
     std::vector<int> fuzzy, ring_start(nR + 2, 0);
@@ -521,6 +531,7 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
     st.n_fuzzy = (int)fuzzy.size();
     st.L = Lmax;
     st.nrings = nR;
+    st.tables_ulp = cu;
     st.tables_valid = true;
   }
   const int words = (v.rows + 31) / 32;

@@ -22,6 +22,7 @@ struct FootprintState {
   // prefix-sum sweep: half-width / ring tables (depend on radius and resolution) and per-call prefix sums + bit columns
   DevBuf tables;
   bool tables_valid = false;
+  double tables_ulp = 0.0;  // coord_ulp of the coordinates the tables' tolerance was sized for
   size_t off_ring = 0, off_fuzzy = 0, off_halfw = 0, off_inner = 0;
   int n_fuzzy = 0, L = 0, nrings = 0;
   signed char h_halfw[64] = {0};

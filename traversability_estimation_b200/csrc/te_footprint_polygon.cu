@@ -328,13 +328,26 @@ namespace {
 struct PolyTables {
   std::vector<int> runs, fz;
 };
-bool classify_polygon(double res, int Lp, int npts, const double* px, const double* py, const double R[4], PolyTables* out, std::string* why) {
+//
+// The reference compares absolute doubles: vertex v + c (rounded) against cell centre c' with c, c' cell centres of coordinates up
+// to M = |position| + half length + reach; cu = ulp(M).  A centre is (B + res * (-idx)) rounded with B common to the map, so
+// c' - c is the lattice offset plus at most 2 cu (two products, two sums), and placing the vertex adds half a cu:
+//   - y comparison v.y > pt.y: moved by at most 2.5 cu.  tol = max(1e-7 res, 4 cu).
+//   - x threshold thr = (vj.x - vi.x) (pt.y - vi.y) / (vj.y - vi.y) + vi.x against pt.x: the three differences carry 1, 2.5 and
+//     1 cu; with s = (vj.x - vi.x) / (vj.y - vi.y) and (pt.y - vi.y) / (vj.y - vi.y) in [0, 1] on a straddling edge, the quotient
+//     moves by (1 + 3.5 |s|) cu to first order; placing vi.x (0.5 cu), rounding the final sum (0.5 cu) and pt.x against the
+//     centre (2 cu) add 3 cu: (4 + 3.5 |s|) cu in all.  tol_x = max(tol, 8 (1 + |s|) cu), twice that first-order bound, covers
+//     the second-order terms (|vj.y - vi.y| >= 1e3 tol >= 4e3 cu, or the edge is uncertain anyway).
+// Near the origin 1e-7 res is the larger term, so the tables are what they always were; far out (a UTM or LV95 map) more offsets
+// become uncertain and are decided per centre.
+bool classify_polygon(double res, double cu, int Lp, int npts, const double* px, const double* py, const double R[4], PolyTables* out,
+                      std::string* why) {
   std::vector<double> vx(npts), vy(npts);
   for (int k = 0; k < npts; ++k) {
     vx[k] = (R[0] * px[k] + R[1] * py[k]) + 0.0;
     vy[k] = (R[2] * px[k] + R[3] * py[k]) + 0.0;
   }
-  const double tol = 1e-7 * res;  // rounding moves a comparison by ~1e-13 m at most; anything closer than this is decided per centre
+  const double tol = std::max(1e-7 * res, 4.0 * cu);
   out->runs.clear();
   out->fz.clear();
   for (int dj = -Lp; dj <= Lp; ++dj) {
@@ -354,8 +367,9 @@ bool classify_polygon(double res, int Lp, int npts, const double* px, const doub
           const bool ci = vy[i] > pty, cj = vy[j] > pty;
           if ((ci != cj) || ui || uj) {
             const double thr = (vx[j] - vx[i]) * (pty - vy[i]) / (vy[j] - vy[i]) + vx[i];
+            const double tol_x = std::max(tol, 8.0 * (1.0 + std::fabs((vx[j] - vx[i]) / (vy[j] - vy[i]))) * cu);
             // the x comparison involves the centre's row; so does a threshold that is a quotient of two rounding-sized numbers
-            if (std::fabs(ptx - thr) < tol || std::fabs(vy[j] - vy[i]) < 1e3 * tol) { fuzzy = true; row_dep = true; }
+            if (std::fabs(ptx - thr) < tol_x || std::fabs(vy[j] - vy[i]) < 1e3 * tol) { fuzzy = true; row_dep = true; }
             if ((ci != cj) && ptx < thr) ++cross;
           }
         }
@@ -420,11 +434,12 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
   std::vector<int> runs, fz;
   {
     PolyTables tb;
+    const double cu = coord_ulp(v.coord_max + Lp * g->resolution);
     for (int k = 0; k < npoly; ++k) {
       PolyDesc& d = desc[k];
       d.R = yaw_rotation(polys[k].yaw);
       const double R[4] = {d.R.r00, d.R.r01, d.R.r10, d.R.r11};
-      if (!classify_polygon(g->resolution, Lp, npts, q.px, q.py, R, &tb, &st.why)) return TE_ERR_UNSUPPORTED;
+      if (!classify_polygon(g->resolution, cu, Lp, npts, q.px, q.py, R, &tb, &st.why)) return TE_ERR_UNSUPPORTED;
       d.run0 = (int)runs.size(); d.nruns = (int)tb.runs.size();
       d.fz0 = (int)fz.size(); d.nfz = (int)tb.fz.size();
       d.ncert = 0;

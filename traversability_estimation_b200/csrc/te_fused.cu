@@ -33,6 +33,7 @@
 #include <cstring>
 
 #include "te_fused.h"
+#include "te_grid.cuh"
 
 namespace te {
 namespace {
@@ -851,10 +852,16 @@ struct WindowClass {
   int k2 = 0;                   // sum of k^2 over certain cells
 };
 
-WindowClass classify(double radius, double res) {
+// The window offsets within 4 cells, classified against the circle of `radius` as the fused kernel needs them.  The reference
+// decides membership on absolute cell centres (CircleIterator: dx * dx + dy * dy <= r2 with dx = X[a] - X[i]); dx is the lattice
+// offset plus at most 2 cu, cu = ulp of the largest |coordinate| (te_footprint.cu's launch_footprint derives it), which moves
+// dx^2 + dy^2 by up to 4 sqrt(2) r cu near the circle.  An offset closer to the circle than tol = max(1e-9 r2, 8 r cu) is "on" it:
+// the tips the mask tables decide per row and column, anything else not representable.  Near the origin 1e-9 r2 is the larger
+// term, so the YAML shapes and their outputs are unchanged; far out a radius in the band leaves the fused kernel.
+WindowClass classify(double radius, double res, double cu) {
   WindowClass c;
   const double r2 = radius * radius;
-  const double tol = 1e-9 * r2 + 1e-300;
+  const double tol = std::max(1e-9 * r2, 8.0 * radius * cu) + 1e-300;
   for (int l = -4; l <= 4; ++l)
     for (int k = -4; k <= 4; ++k) {
       const double d2 = (double)(k * k + l * l) * res * res;
@@ -1083,12 +1090,15 @@ void fused_mask_bits(const te_chain_params* p, const double* P, int n, unsigned 
 }
 
 bool fused_eligible(FusedState& st, const std::vector<double>& X, const std::vector<double>& Y, const te_geometry* g,
-                    const te_chain_params* p, cudaStream_t stream) {
-  if (st.valid && std::memcmp(&st.key_geo, g, sizeof(*g)) == 0 && std::memcmp(&st.key_par, p, sizeof(*p)) == 0) return st.shape_id >= 0;
+                    const te_chain_params* p, double coord_max, cudaStream_t stream) {
+  const double cu = coord_ulp(coord_max + 4.0 * g->resolution);
+  if (st.valid && std::memcmp(&st.key_geo, g, sizeof(*g)) == 0 && std::memcmp(&st.key_par, p, sizeof(*p)) == 0 && st.key_cu == cu)
+    return st.shape_id >= 0;
   st.valid = false;
   st.shape_id = -1;
   st.key_geo = *g;
   st.key_par = *p;
+  st.key_cu = cu;
   auto no = [&](const char* why) {
     st.why = why;
     st.valid = true;
@@ -1099,8 +1109,8 @@ bool fused_eligible(FusedState& st, const std::vector<double>& X, const std::vec
   if (g->rows % 4 != 0) return no("row count is not a multiple of 4 (TMA needs 16-byte column pitch)");
   if (!(p->slope_critical > 0.0) || !(p->step_critical > 0.0) || !(p->roughness_critical > 0.0)) return no("a critical value is zero");
   const double res = g->resolution;
-  const WindowClass wn = classify(p->normals_radius, res), wr = classify(p->roughness_radius, res);
-  const WindowClass w1 = classify(p->step_first_radius, res), w2 = classify(p->step_second_radius, res);
+  const WindowClass wn = classify(p->normals_radius, res, cu), wr = classify(p->roughness_radius, res, cu);
+  const WindowClass w1 = classify(p->step_first_radius, res, cu), w2 = classify(p->step_second_radius, res, cu);
   if (!wn.ok || wn.tips_on_circle) return no("normals window not representable (reach > 2 cells or on-circle offsets)");
   if (!wr.ok || wr.tips_on_circle || std::memcmp(wn.w, wr.w, sizeof(wn.w)) != 0) return no("roughness window differs from the normals window");
   const int id = match_shape(wn, w1, w2);
@@ -1127,7 +1137,7 @@ bool fused_eligible(FusedState& st, const std::vector<double>& X, const std::vec
 }
 
 void make_fixup_args(const FusedState& st, const SlabView& v, const ChainDev& p, const MapMasks* mm, FixupArgs* out) {
-  const WindowClass wn = classify(p.rn, v.res), w1 = classify(p.r1, v.res), w2 = classify(p.r2, v.res);
+  const WindowClass wn = classify(p.rn, v.res, st.key_cu), w1 = classify(p.r1, v.res, st.key_cu), w2 = classify(p.r2, v.res, st.key_cu);
   FixupArgs a{};
   a.rows = v.rows; a.cols_total = v.cols_total; a.in_col0 = v.in_col0; a.in_ncols = v.in_ncols; a.out_col0 = v.out_col0;
   a.map_cells = (unsigned)((size_t)v.rows * v.out_ncols);
@@ -1185,7 +1195,7 @@ int launch_chain_fused(FusedState& st, const SlabView& v, const ChainDev& p, int
   if (cr != CUDA_SUCCESS) { st.why = "cuTensorMapEncodeTiled failed (" + std::to_string((int)cr) + ")"; return 1; }
 
   const double res = v.res;
-  const WindowClass wn = classify(p.rn, res);
+  const WindowClass wn = classify(p.rn, res, st.key_cu);
   FusedArgs a{};
   a.rows = v.rows; a.cols_total = v.cols_total;
   a.in_col0 = v.in_col0; a.in_ncols = v.in_ncols; a.out_col0 = v.out_col0; a.out_ncols = v.out_ncols;

@@ -13,6 +13,7 @@ struct FusedState {
   bool valid = false;     // tables below match (geometry, params) of `key_*`
   te_geometry key_geo{};
   te_chain_params key_par{};
+  double key_cu = 0.0;    // coord_ulp of the coordinates the windows were classified for (see classify)
   int shape_id = -1;
   std::vector<unsigned char> h_rowmask, h_colmask;  // host copies of the tables below
   DevBuf rowmask, colmask;  // per-row / per-column on-circle membership bits
@@ -34,9 +35,10 @@ struct MapMasks {
   unsigned row_stride, col_stride;
 };
 
-// True when the fused stencil has an instantiation for these window shapes (fills the tables).
+// True when the fused stencil has an instantiation for these window shapes (fills the tables).  coord_max: the largest
+// |cell-centre coordinate| of the launch (SlabView::coord_max), which sizes the tolerance of the window classification.
 bool fused_eligible(FusedState& st, const std::vector<double>& X, const std::vector<double>& Y, const te_geometry* g,
-                    const te_chain_params* p, cudaStream_t stream);
+                    const te_chain_params* p, double coord_max, cudaStream_t stream);
 // Why this particular launch cannot use the fused stencil although the window shapes are eligible (pointer alignment, size,
 // partial normal outputs), or nullptr.  TE_KERNEL_AUTO runs the generic kernel instead.
 const char* fused_launch_obstacle(const SlabView& v, int nmaps, const float* elev, const ChainOut& o);

@@ -15,6 +15,19 @@ __host__ __device__ __forceinline__ double cell_coord(double map_pos, double len
   return (map_pos + offset) + res * (-(double)idx);
 }
 
+// The spacing of the doubles around |x| <= m (at least the spacing at 1): the rounding unit of the absolute coordinates that the
+// reference forms its membership decisions on.  Host only: it sizes the tolerances of the relative-offset tables.
+inline double coord_ulp(double m) { return std::ldexp(1.0, std::ilogb(std::fmax(m, 1.0)) - 52); }
+
+// The largest index offset n along one axis that a circle of radius r can hold when the reference tests membership on absolute
+// cell centres whose coordinates have spacing cu: n with n^2 res^2 <= r^2 + 8 r cu (the bound launch_footprint derives), and at
+// least floor(r / res + 1e-9).  Near the origin 8 r cu is below a rounding of r^2 and this is floor(r / res + 1e-9).  Host only.
+inline int lattice_reach(double r, double res, double cu) {
+  int n = (int)std::floor(r / res + 1e-9);
+  while ((double)((n + 1) * (n + 1)) * res * res <= r * r + 8.0 * r * cu) ++n;
+  return n;
+}
+
 // GridMap::isInside and GridMap::getIndex on a map in the default start index: the index (i, j) and whether the position lies in
 // the map.  G is any geometry with the members rows, cols_total, res, lenx, leny, posx and posy (the kernels' FpArgs, the host's
 // GridGeo); reading them in place keeps the kernels' code as it was.
