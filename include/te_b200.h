@@ -483,7 +483,8 @@ int te_check_footprint_request_batched(te_ctx* ctx, const te_geometry* g, const 
  * holding map m returns or stores for the same calls restricted to map m (for a request: that map's paths, in their relative
  * request order).  A path never reads or writes another map's cells, cache or memo.  Limits as te_footprint_batched: nmaps
  * 1..65535 (TE_ERR_BAD_ARG below 1, TE_ERR_UNSUPPORTED above), nmaps*rows*cols < 2^32 and nmaps*cols < 2^31 (TE_ERR_UNSUPPORTED);
- * a circular-buffer start index is TE_ERR_UNSUPPORTED for every _batched entry.  On a batch te_map_footprint, the polygon
+ * a circular-buffer start index in g is TE_ERR_UNSUPPORTED for every _batched entry (the _wrapped entries below take one per
+ * map).  On a batch te_map_footprint, the polygon
  * entries, te_map_get_layers, te_map_get_footprint and te_map_clear_footprint work on every map, their outputs holding the maps
  * back to back per layer; te_map_check_footprint_request, te_map_get_submaps and te_map_valid_at need a map index and fail with
  * TE_ERR_BAD_ARG on a te_map of more than one map (use their _batched entries).  The single-map entries on a te_map of one map
@@ -524,7 +525,8 @@ int te_map_set_layers_batched(te_map* map, const te_geometry* g, int32_t nmaps, 
  *     it at once); nsel is 1..nmaps and the entries are distinct and in 0..nmaps-1, in any order.  Layer arguments and outputs
  *     hold the nsel maps back to back in map_index order.
  *   - g must equal the batch's geometry bit for bit (TE_ERR_BAD_ARG otherwise).  A start index, in g or on the te_map's layers, is
- *     TE_ERR_UNSUPPORTED, as for every _batched entry (use te_map_chain there).  A te_map without layers is TE_ERR_BAD_ARG.
+ *     TE_ERR_UNSUPPORTED, as for every _batched entry (use te_map_chain there, or the _wrapped entries below, whose start indices
+ *     these entries accept).  A te_map without layers is TE_ERR_BAD_ARG.
  *   - Every map of a batch holds the same layers, so the optional layers stay those the batch holds: te_map_chain_maps, which gives
  *     a map roughness and no robot_slope as te_map_chain does, is TE_ERR_UNSUPPORTED on a batch that holds robot_slope or lacks
  *     roughness; te_map_set_layers_maps must be given exactly the batch's optional layers (TE_ERR_MISSING_LAYER for a missing one,
@@ -587,6 +589,47 @@ int te_map_set_layers_maps_at(te_map* map, const te_geometry* g, int32_t nsel, c
                               const float* robot_slope_or_null, int memory, const double* position_xy);
 /* Where the maps sit: position_xy[2m], position_xy[2m + 1] for map m (nmaps pairs).  TE_ERR_BAD_ARG before layers were set. */
 int te_map_positions(te_map* map, double* position_xy);
+
+/* Maps in their own circular-buffer order (robot-centric maps moved with GridMap::move, each published with its own outer / inner
+ * start index).  The four entries below take the arguments of the _at entry of the same stem plus start_index, a HOST array of one
+ * (start_row, start_col) pair per map the call updates (nmaps pairs, or nsel in map_index order), read before the call returns.
+ * Each map's block of every layer argument is in the buffer order of its pair: cell (i, j) of the map is stored at
+ * ((j + start_col) % cols) * rows + (i + start_row) % rows of the block, in both memory modes.  start_index NULL means (0, 0) for
+ * every map, and the entry is then its _at entry bit for bit.  Rules:
+ *   - g's start_row / start_col must be 0 (the array is the only source of the index) and every pair must lie in 0 .. rows-1,
+ *     0 .. cols-1: TE_ERR_BAD_ARG otherwise, found before anything is written.  Every other rule of the _at entry applies.
+ *   - The te_map keeps each map's start index until that map is reloaded: a whole-batch _wrapped call sets every map's, a _wrapped
+ *     selection the selected maps'; te_map_chain_maps(_at), te_map_set_layers_maps(_at), te_map_chain_image_maps and a
+ *     te_map_chain_windows selection give the maps they load (0, 0), and the other whole-batch entries give every map (0, 0).
+ *   - While a map has a start index, these HOST outputs hold its block in that buffer order: the chain outputs of these entries,
+ *     te_map_get_layers (uncertainty_range included), te_map_get_footprint, te_map_footprint(_maps),
+ *     te_map_footprint_polygon(_yaws, _yaws_reduce) (best_yaw included) and te_map_footprint_polygon_keep; te_map_carry_layers takes
+ *     its block in that order in both memory modes.  DEVICE outputs stay in default order.  Everything that depends on positions
+ *     (requests, submaps, te_map_valid_at_batched, te_map_at_poses) is unaffected, as in grid_map.
+ *   - The selection entries (_maps, te_map_footprint_maps, te_map_carry_layers and te_map_footprint_polygon_keep with map_index)
+ *     work on such a te_map; a te_map whose start index came in g (te_map_chain / te_map_set_layers) keeps refusing them.
+ *   - The moves run on the GPU: one k_map_cut_windows launch puts every map and layer of an input call in default order (device
+ *     inputs are read in place; host inputs take one copy per layer into scratch the te_map keeps first), and one re-wraps every
+ *     map's block of the host outputs into that scratch before one copy back per output array.  So a whole-batch _wrapped update
+ *     costs the launches of its _at entry plus one, whatever nmaps, and one more when it also returns host outputs.  Scratch: 4 bytes
+ *     per cell of every layer moved, grown to the largest call and released by te_map_destroy. */
+int te_map_chain_batched_wrapped(te_map* map, const te_geometry* g, const te_chain_params* p, int32_t nmaps, const float* elevation,
+                                 float* slope_or_null, float* step_or_null, float* roughness_or_null, float* traversability_or_null,
+                                 int memory, const double* position_xy_or_null, const int32_t* start_index);
+int te_map_set_layers_batched_wrapped(te_map* map, const te_geometry* g, int32_t nmaps, const float* traversability, const float* slope,
+                                      const float* step, const float* roughness_or_null, const float* elevation,
+                                      const float* robot_slope_or_null, int memory, const double* position_xy_or_null,
+                                      const int32_t* start_index);
+int te_map_chain_maps_wrapped(te_map* map, const te_geometry* g, const te_chain_params* p, int32_t nsel, const int32_t* map_index,
+                              const float* elevation, float* slope_or_null, float* step_or_null, float* roughness_or_null,
+                              float* traversability_or_null, int memory, const double* position_xy_or_null, const int32_t* start_index);
+int te_map_set_layers_maps_wrapped(te_map* map, const te_geometry* g, int32_t nsel, const int32_t* map_index, const float* traversability,
+                                   const float* slope, const float* step, const float* roughness_or_null, const float* elevation,
+                                   const float* robot_slope_or_null, int memory, const double* position_xy_or_null,
+                                   const int32_t* start_index);
+/* Each map's start index: start_index[2m], start_index[2m + 1] for map m (nmaps pairs; a single map whose start index came in g
+ * reports g's).  TE_ERR_BAD_ARG before layers were set. */
+int te_map_start_indices(te_map* map, int32_t* start_index);
 
 /* ---- Elevation images: the reference node's image topic (TraversabilityEstimation::imageCallback) ------------------------------
  * The node turns a grayscale height image into the elevation layer (GridMapRosConverter::initializeFromImage on the first image,

@@ -180,6 +180,11 @@ SIGNATURES = {
     "te_map_chain_maps_at": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _P, _I, _P]),
     "te_map_set_layers_maps_at": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
     "te_map_positions": (_R, [_P, _P]),
+    "te_map_chain_batched_wrapped": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
+    "te_map_set_layers_batched_wrapped": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _I, _P, _P]),
+    "te_map_chain_maps_wrapped": (_R, [_P, _G, _CP, _I, _P, _P, _P, _P, _P, _P, _I, _P, _P]),
+    "te_map_set_layers_maps_wrapped": (_R, [_P, _G, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P]),
+    "te_map_start_indices": (_R, [_P, _P]),
     "te_image_geometry": (_R, [_I, _I, _D, _D, _D, _G]),
     "te_map_chain_image": (_R, [_P, _G, _CP, _I, _I, _P, _L, _L, _D, _D, _P, _P, _P, _P, _I]),
     "te_map_chain_image_maps": (_R, [_P, _G, _CP, _I, _P, _I, _P, _L, _L, _D, _D, _P, _P, _P, _P, _I]),
@@ -818,17 +823,18 @@ class Map:
             raise ValueError(f"positions: need {n} (x, y) pairs, got {xy.size} values")
         return xy
 
-    def chain_batched(self, g, p, nmaps, elevation, outputs=False, positions=None):
+    def chain_batched(self, g, p, nmaps, elevation, outputs=False, positions=None, start_index=None):
         """te_map_chain_batched (computeTraversability for every map): elevation (nmaps, rows, cols); empties every cache.
         outputs=True also returns the four layers as a dict of (nmaps, rows, cols) arrays.  positions (nmaps, 2): map m sits at
-        positions[m] instead of g's position (te_map_chain_batched_at)."""
+        positions[m] instead of g's position (te_map_chain_batched_at).  start_index (nmaps, 2): map m's layers (input and
+        output) are in the circular-buffer order of start_index[m] (te_map_chain_batched_wrapped)."""
         e = self._batch_layers(elevation)
         out = {k: np.empty((int(nmaps), g.cols, g.rows), dtype=np.float32) for k in ("slope", "step", "roughness", "traversability")} \
             if outputs else {}
         xy = self._positions(positions, int(nmaps))
         args = (self._h, C.byref(g), C.byref(p), int(nmaps), _addr(e),
                 *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")), MEM_HOST)
-        self._check(self._L.te_map_chain_batched(*args) if xy is None else self._L.te_map_chain_batched_at(*args, _addr(xy)))
+        self._update("te_map_chain_batched", args, xy, start_index, int(nmaps))
         self._g, self._n = g, int(nmaps)
         return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
 
@@ -840,24 +846,27 @@ class Map:
         self._check(fn(self._h, C.byref(g), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST))
         self._g, self._n = g, 1
 
-    def set_layers_batched(self, g, nmaps, traversability, slope, step, elevation, roughness=None, robot_slope=None, positions=None):
+    def set_layers_batched(self, g, nmaps, traversability, slope, step, elevation, roughness=None, robot_slope=None, positions=None,
+                           start_index=None):
         """te_map_set_layers_batched (setTraversabilityMap for every map): each layer (nmaps, rows, cols); empties every cache and
-        memo.  positions (nmaps, 2): map m sits at positions[m] (te_map_set_layers_batched_at)."""
+        memo.  positions (nmaps, 2): map m sits at positions[m] (te_map_set_layers_batched_at).  start_index (nmaps, 2): map m's
+        layers are in the circular-buffer order of start_index[m] (te_map_set_layers_batched_wrapped)."""
         t, s, st, r, e, rs = (self._batch_layers(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
         xy = self._positions(positions, int(nmaps))
         args = (self._h, C.byref(g), int(nmaps), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST)
-        self._check(self._L.te_map_set_layers_batched(*args) if xy is None else self._L.te_map_set_layers_batched_at(*args, _addr(xy)))
+        self._update("te_map_set_layers_batched", args, xy, start_index, int(nmaps))
         self._g, self._n = g, int(nmaps)
 
     @staticmethod
     def _map_index(map_index):
         return np.ascontiguousarray(map_index, dtype=np.int32).reshape(-1)
 
-    def chain_maps(self, g, p, map_index, elevation, outputs=False, positions=None):
+    def chain_maps(self, g, p, map_index, elevation, outputs=False, positions=None, start_index=None):
         """te_map_chain_maps (computeTraversability for the maps map_index of the batch only): elevation (nsel, rows, cols), map
         j of it going to map map_index[j]; empties those maps' caches and keeps every other map as it was.  outputs=True also
         returns the four layers as a dict of (nsel, rows, cols) arrays in map_index order.  positions (nsel, 2): map map_index[j]
-        moves to positions[j] (te_map_chain_maps_at)."""
+        moves to positions[j] (te_map_chain_maps_at).  start_index (nsel, 2): map map_index[j] comes (and its outputs go back)
+        in the circular-buffer order of start_index[j] (te_map_chain_maps_wrapped)."""
         idx = self._map_index(map_index)
         e = self._batch_layers(elevation)
         out = {k: np.empty((len(idx), g.cols, g.rows), dtype=np.float32) for k in ("slope", "step", "roughness", "traversability")} \
@@ -865,7 +874,7 @@ class Map:
         xy = self._positions(positions, len(idx))
         args = (self._h, C.byref(g), C.byref(p), len(idx), _addr(idx), _addr(e),
                 *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")), MEM_HOST)
-        self._check(self._L.te_map_chain_maps(*args) if xy is None else self._L.te_map_chain_maps_at(*args, _addr(xy)))
+        self._update("te_map_chain_maps", args, xy, start_index, len(idx))
         return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
 
     _CHAIN_OUTPUTS = ("slope", "step", "roughness", "traversability")
@@ -893,15 +902,32 @@ class Map:
                                                     *(_addr(out.get(k)) for k in self._CHAIN_OUTPUTS), MEM_HOST))
         return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
 
-    def set_layers_maps(self, g, map_index, traversability, slope, step, elevation, roughness=None, robot_slope=None, positions=None):
+    def set_layers_maps(self, g, map_index, traversability, slope, step, elevation, roughness=None, robot_slope=None, positions=None,
+                        start_index=None):
         """te_map_set_layers_maps (setTraversabilityMap for the maps map_index only): each layer (nsel, rows, cols) in map_index
         order; the optional layers must be those the batch holds.  Empties those maps' caches and memos.  positions (nsel, 2): map
-        map_index[j] moves to positions[j] (te_map_set_layers_maps_at)."""
+        map_index[j] moves to positions[j] (te_map_set_layers_maps_at).  start_index (nsel, 2): map map_index[j]'s layers are in
+        the circular-buffer order of start_index[j] (te_map_set_layers_maps_wrapped)."""
         idx = self._map_index(map_index)
         t, s, st, r, e, rs = (self._batch_layers(a) for a in (traversability, slope, step, roughness, elevation, robot_slope))
         xy = self._positions(positions, len(idx))
         args = (self._h, C.byref(g), len(idx), _addr(idx), _addr(t), _addr(s), _addr(st), _addr(r), _addr(e), _addr(rs), MEM_HOST)
-        self._check(self._L.te_map_set_layers_maps(*args) if xy is None else self._L.te_map_set_layers_maps_at(*args, _addr(xy)))
+        self._update("te_map_set_layers_maps", args, xy, start_index, len(idx))
+
+    def _update(self, entry, args, xy, start_index, n):
+        """`entry`, or its _at entry when positions are given, or its _wrapped entry when start indices (n pairs) are given."""
+        if start_index is None:
+            return self._check(getattr(self._L, entry)(*args) if xy is None else getattr(self._L, entry + "_at")(*args, _addr(xy)))
+        si = np.ascontiguousarray(start_index, dtype=np.int32).reshape(-1)
+        if si.size != 2 * n:
+            raise ValueError(f"start_index: need {n} (row, col) pairs, got {si.size} values")
+        self._check(getattr(self._L, entry + "_wrapped")(*args, _addr(xy), _addr(si)))
+
+    def start_indices(self):
+        """te_map_start_indices: each map's circular-buffer start index, an (nmaps, 2) int32 array of (row, col)."""
+        si = np.empty((self._n, 2), dtype=np.int32)
+        self._check(self._L.te_map_start_indices(self._h, _addr(si)))
+        return si
 
     def positions(self):
         """te_map_positions: where the maps sit, an (nmaps, 2) float64 array of (x, y)."""

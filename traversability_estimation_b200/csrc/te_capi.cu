@@ -1349,7 +1349,8 @@ struct te_map {
   // The _maps entries: the selected maps' layers packed back to back (grown to the largest selection) and their slot table
   DevBuf sel[te::kMapSlotLayers], slots;
   DevBuf image;  // te_map_chain_image(_maps) in host memory: the staged image bytes, packed
-  DevBuf cut;    // te_map_chain_submap / te_map_chain_windows: the window table of k_map_cut_windows
+  DevBuf cut;    // the window table of k_map_cut_windows (te_map_chain_submap / _windows, and the moves of `start` below)
+  DevBuf wrap;   // maps in their buffer order on the device: host inputs before they are unwrapped, host outputs once re-wrapped
   bool have_rough = false, have_rslope = false;
   te::FootprintState fp;  // the map's own scratch; fp.memo is the resident memo
   bool memo_valid = false;
@@ -1361,6 +1362,11 @@ struct te_map {
   // elsewhere.  spread: the maps do not all sit at one position, so the kernels read per-map tables (map_tables).
   std::vector<double> pos;
   bool spread = false;
+  // Each map's circular-buffer start index (start[2m], start[2m + 1]: te_map_start_indices), as the _wrapped entries gave it; (0, 0)
+  // for maps the other entries loaded.  The device layers stay in default order; host inputs of a map with a start index are
+  // unwrapped and its host outputs re-wrapped by k_map_cut_windows (a single map whose start index came in g, geo_in, keeps the
+  // staging copies of upload_cols / download_cols instead, and all zeros here).
+  std::vector<int32_t> start;
   // Per-map device tables (map_tables), cached with what they were built from: tab_all for every map in index order, tab_launch
   // for a chain launch (with the fused mask tables) or a selection.
   struct PosTab {
@@ -1520,6 +1526,7 @@ int map_reset(te_map* m, const te_geometry* g_in, const te_geometry* g, int nmap
   m->geo_in = *g_in;
   m->geo = *g;
   m->nmaps = nmaps;
+  m->start.assign(2 * (size_t)nmaps, 0);  // a _wrapped entry sets the maps' start indices once their layers are in
   m->memo_valid = false;
   m->have_layers = false;
   m->carried = 0;  // a new map replaces the old one wholesale, its elevation map's layers included
@@ -1732,7 +1739,8 @@ int te_map_destroy(te_map* m) {
     Guard g(m->ctx);
     if (g.ok) {
       cudaStreamSynchronize(m->ctx->stream);
-      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather, &m->slots, &m->image, &m->cut})
+      for (DevBuf* b : {&m->trav, &m->slope, &m->step, &m->rough, &m->elev, &m->rslope, &m->cache, &m->fresh, &m->gather, &m->slots, &m->image,
+                        &m->cut, &m->wrap})
         b->release();
       for (DevBuf& b : m->sel) b.release();
       for (DevBuf& b : m->carry) b.release();
@@ -1819,6 +1827,157 @@ int map_convert_image(te_map* m, const te_geometry& g, const ImageIn& im, int bp
   return launch_check(c, "k_image_to_layer");
 }
 
+// One k_map_cut_windows launch (te_kernels.h WindowCut) of the windows `win`, nl layers each, from sources of src_rows x src_cols
+// cells: its table goes to m->cut (the windows, the source pointers, the destination pointers, then col_of).  A table that grows
+// first waits for the launches that may still read it.
+int map_launch_cut(te_map* m, const std::vector<int4>& win, const std::vector<const float*>& src, const std::vector<float*>& dst,
+                   const std::vector<int>& col_of, int nl, int rows, int cols, int src_rows, int src_cols) {
+  te_ctx* c = m->ctx;
+  const int n = (int)win.size();
+  const size_t wbytes = sizeof(int4) * n, pbytes = sizeof(float*) * src.size(), cbytes = sizeof(int) * col_of.size();
+  std::vector<char> h(wbytes + 2 * pbytes + cbytes);
+  std::memcpy(h.data(), win.data(), wbytes);
+  std::memcpy(h.data() + wbytes, src.data(), pbytes);
+  std::memcpy(h.data() + wbytes + pbytes, dst.data(), pbytes);
+  if (cbytes) std::memcpy(h.data() + wbytes + 2 * pbytes, col_of.data(), cbytes);
+  if (m->cut.p && m->cut.cap < h.size()) TE_CUDA(cudaStreamSynchronize(c->stream));  // an earlier launch may still read it
+  TE_CUDA(m->cut.reserve(h.size()));
+  // pageable source: consumed before cudaMemcpyAsync returns, ordered after the kernels queued before on the stream
+  TE_CUDA(cudaMemcpyAsync(m->cut.p, h.data(), h.size(), cudaMemcpyHostToDevice, c->stream));
+  const char* t = (const char*)m->cut.p;
+  te::WindowCut a{};
+  a.win = (const int4*)t;
+  a.src = (const float* const*)(t + wbytes);
+  a.dst = (float* const*)(t + wbytes + pbytes);
+  a.col_of = cbytes ? (const int*)(t + wbytes + 2 * pbytes) : nullptr;
+  a.nlayers = nl;
+  a.nmaps = n;
+  a.rows = rows;
+  a.cols = cols;
+  a.src_rows = src_rows;
+  a.src_cols = src_cols;
+  a.ncolumns = (long long)n * nl * cols;
+  te::launch_cut_windows(a, c->sms, c->stream);
+  return launch_check(c, "k_map_cut_windows");
+}
+
+// One map's layer of the te_map's geometry moved whole: from src, read through the start index (sr, sc), to dst (device pointers).
+struct MapBlock {
+  const float* src;
+  float* dst;
+  int32_t sr, sc;
+};
+
+// Every block in one k_map_cut_windows launch (none for no block).
+int map_move_blocks(te_map* m, const std::vector<MapBlock>& b) {
+  if (b.empty()) return TE_OK;
+  std::vector<int4> win(b.size());
+  std::vector<const float*> src(b.size());
+  std::vector<float*> dst(b.size());
+  for (size_t k = 0; k < b.size(); ++k) {
+    win[k] = int4{0, 0, b[k].sr, b[k].sc};
+    src[k] = b[k].src;
+    dst[k] = b[k].dst;
+  }
+  const int rows = m->geo.rows, cols = m->geo.cols;
+  return map_launch_cut(m, win, src, dst, {}, 1, rows, cols, rows, cols);
+}
+
+// Whether any of the n (start_row, start_col) pairs st is not (0, 0) (st null: none).
+bool any_start(const int32_t* st, int n) {
+  if (!st) return false;
+  for (int k = 0; k < 2 * n; ++k)
+    if (st[k] != 0) return true;
+  return false;
+}
+
+// The start indices of the maps s->idx[0..s->n) (s null: every map), pairs in that order.
+std::vector<int32_t> map_starts(const te_map* m, const MapSel* s) {
+  if (!s) return m->start;
+  std::vector<int32_t> st(2 * (size_t)s->n);
+  for (int k = 0; k < s->n; ++k) { st[2 * k] = m->start[2 * s->idx[k]]; st[2 * k + 1] = m->start[2 * s->idx[k] + 1]; }
+  return st;
+}
+
+// Validates the start_index of a _wrapped entry: n pairs inside a map of rows x cols (null: none).  Writes nothing.
+int check_start_indices(const int32_t* st, int n, int rows, int cols) {
+  if (!st) return TE_OK;
+  for (int k = 0; k < n; ++k)
+    if (st[2 * k] < 0 || st[2 * k] >= rows || st[2 * k + 1] < 0 || st[2 * k + 1] >= cols)
+      return fail(TE_ERR_BAD_ARG, "start_index[%d] = (%d, %d) is outside the map of %d x %d cells", k, st[2 * k], st[2 * k + 1], rows, cols);
+  return TE_OK;
+}
+
+// Records the start indices of an update's maps: every map (idx null) or the maps idx[0..n), from the pairs st in call order
+// (null: (0, 0)).
+void map_set_starts(te_map* m, const int32_t* idx, int n, const int32_t* st) {
+  for (int k = 0; k < n; ++k) {
+    const int t = idx ? idx[k] : k;
+    m->start[2 * t] = st ? st[2 * k] : 0;
+    m->start[2 * t + 1] = st ? st[2 * k + 1] : 0;
+  }
+}
+
+// m->wrap, at least `bytes` long; growing it first waits for the launches that may still read it.
+int map_wrap_reserve(te_map* m, size_t bytes) {
+  if (m->wrap.p && m->wrap.cap < bytes) TE_CUDA(cudaStreamSynchronize(m->ctx->stream));
+  TE_CUDA(m->wrap.reserve(bytes));
+  return TE_OK;
+}
+
+// nl layers of the n maps of an update, each map in its own buffer order (map k read through the start index st[2k], st[2k + 1]),
+// into default order at dst[l] + k * cells, in one launch.  Layer l holds the n maps back to back at in[l]: device layers are
+// read in place, host layers go to m->wrap first (one copy each).
+int map_unwrap_in(te_map* m, int n, const int32_t* st, int nl, const float* const* in, float* const* dst, int memory) {
+  const size_t cells = map_cells(m), lcells = cells * n;
+  std::vector<const float*> src(in, in + nl);
+  if (memory == TE_MEM_HOST) {
+    if (int rc = map_wrap_reserve(m, sizeof(float) * lcells * nl)) return rc;
+    for (int l = 0; l < nl; ++l) {
+      float* d = (float*)m->wrap.p + l * lcells;
+      TE_CUDA(cudaMemcpyAsync(d, in[l], sizeof(float) * lcells, cudaMemcpyHostToDevice, m->ctx->stream));
+      src[l] = d;
+    }
+  }
+  std::vector<MapBlock> b;
+  for (int l = 0; l < nl; ++l)
+    for (int k = 0; k < n; ++k) b.push_back(MapBlock{src[l] + k * cells, dst[l] + k * cells, st[2 * k], st[2 * k + 1]});
+  return map_move_blocks(m, b);
+}
+
+// Host outputs in buffer order: block b's src is a map in default order on the device, its dst the HOST array that takes it in the
+// buffer order of the block's start index.  One launch re-wraps every block into m->wrap, then one copy per run of blocks that
+// are contiguous on the host brings them back.  The caller synchronises.
+int map_wrap_out(te_map* m, const std::vector<MapBlock>& b) {
+  if (b.empty()) return TE_OK;
+  const size_t cells = map_cells(m);
+  const int rows = m->geo.rows, cols = m->geo.cols;
+  if (int rc = map_wrap_reserve(m, sizeof(float) * cells * b.size())) return rc;
+  float* const w = (float*)m->wrap.p;
+  std::vector<MapBlock> d(b.size());
+  for (size_t k = 0; k < b.size(); ++k)
+    d[k] = MapBlock{b[k].src, w + k * cells, (rows - b[k].sr) % rows, (cols - b[k].sc) % cols};
+  if (int rc = map_move_blocks(m, d)) return rc;
+  for (size_t k = 0; k < b.size();) {
+    size_t e = k + 1;
+    while (e < b.size() && b[e].dst == b[e - 1].dst + cells) ++e;
+    TE_CUDA(cudaMemcpyAsync(b[k].dst, w + k * cells, sizeof(float) * cells * (e - k), cudaMemcpyDeviceToHost, m->ctx->stream));
+    k = e;
+  }
+  return TE_OK;
+}
+
+// The host outputs out[0..n) (each null or nmaps maps back to back) of the device layers src[0..n) (the same layout), each map's
+// block re-wrapped to st[2k], st[2k + 1]: map_wrap_out's blocks.
+std::vector<MapBlock> wrap_blocks(te_map* m, int nmaps, const int32_t* st, int n, float* const* out, const float* const* src) {
+  const size_t cells = map_cells(m);
+  std::vector<MapBlock> b;
+  for (int l = 0; l < n; ++l)
+    if (out[l])
+      for (int k = 0; k < nmaps; ++k) b.push_back(MapBlock{src[l] + k * cells, out[l] + k * cells, st[2 * k], st[2 * k + 1]});
+  return b;
+}
+
 // The windows of `cut` into the maps of a chain launch of geometry m->geo, in one launch: the elevation of map k of the launch to
 // elev + k * cells (the te_map's layer on a whole-batch update, the selection's packed scratch otherwise), each carried layer
 // straight to its resident slot (map k, or sel->idx[k]).  Device sources are read in place; host sources stage only the source
@@ -1842,9 +2001,9 @@ int map_cut(te_map* m, const CutIn& cut, const MapSel* sel, float* elev) {
     for (int k = 0; k < n; ++k) dst[(size_t)k * nl + l] = base + (size_t)(b != 4 && sel ? sel->idx[k] : k) * cells;
     ++l;
   }
-  te::WindowCut a{};
+  const float* srcl[te::kCutMaxLayers];
   std::vector<int> col_of;
-  for (int k = 0; k < nl; ++k) a.src[k] = cut.layers[k];
+  for (int k = 0; k < nl; ++k) srcl[k] = cut.layers[k];
   if (cut.memory == TE_MEM_HOST) {
     std::vector<char> touched(s.cols, 0);
     for (const int2& t : cut.top)
@@ -1866,33 +2025,15 @@ int map_cut(te_map* m, const CutIn& cut, const MapSel* sel, float* elev) {
                                 sizeof(float) * s.rows * (size_t)(e - j), cudaMemcpyHostToDevice, c->stream));
       j = e;
     }
-    for (int k = 0; k < nl; ++k) a.src[k] = staged + (size_t)k * nst * s.rows;
+    for (int k = 0; k < nl; ++k) srcl[k] = staged + (size_t)k * nst * s.rows;
   }
-  // the table: destination pointers, then the windows' top-left cells, then (host sources) the staged column of each stored one
-  const size_t pbytes = sizeof(float*) * dst.size(), tbytes = sizeof(int2) * n, cbytes = sizeof(int) * col_of.size();
-  std::vector<char> h(pbytes + tbytes + cbytes);
-  std::memcpy(h.data(), dst.data(), pbytes);
-  std::memcpy(h.data() + pbytes, cut.top.data(), tbytes);
-  if (cbytes) std::memcpy(h.data() + pbytes + tbytes, col_of.data(), cbytes);
-  if (m->cut.p && m->cut.cap < h.size()) TE_CUDA(cudaStreamSynchronize(c->stream));  // an earlier cut may still read it
-  TE_CUDA(m->cut.reserve(h.size()));
-  // pageable source: consumed before cudaMemcpyAsync returns, ordered after the kernels queued before on the stream
-  TE_CUDA(cudaMemcpyAsync(m->cut.p, h.data(), h.size(), cudaMemcpyHostToDevice, c->stream));
-  const char* t = (const char*)m->cut.p;
-  a.dst = (float* const*)t;
-  a.top = (const int2*)(t + pbytes);
-  a.col_of = cbytes ? (const int*)(t + pbytes + tbytes) : nullptr;
-  a.nlayers = nl;
-  a.nmaps = n;
-  a.rows = rows;
-  a.cols = cols;
-  a.src_rows = s.rows;
-  a.src_cols = s.cols;
-  a.start_row = s.start_row;
-  a.start_col = s.start_col;
-  a.ncolumns = (long long)n * nl * cols;
-  te::launch_cut_windows(a, c->sms, c->stream);
-  return launch_check(c, "k_map_cut_windows");
+  std::vector<int4> win(n);
+  std::vector<const float*> src((size_t)n * nl);
+  for (int k = 0; k < n; ++k) {
+    win[k] = int4{cut.top[k].x, cut.top[k].y, s.start_row, s.start_col};
+    for (int l2 = 0; l2 < nl; ++l2) src[(size_t)k * nl + l2] = srcl[l2];
+  }
+  return map_launch_cut(m, win, src, dst, col_of, nl, rows, cols, s.rows, s.cols);
 }
 
 // te_map_chain (nmaps = 1), te_map_chain_batched and, with a selection, te_map_chain_maps, from an elevation layer, from images
@@ -1902,8 +2043,11 @@ int map_cut(te_map* m, const CutIn& cut, const MapSel* sel, float* elev) {
 // replace the batch's, on a selection they go straight to the selected maps' slots and only the batch's other carried layers are
 // filled with NaN.
 // at: an _at entry, whose maps go to position_xy (null: g's position) and whose g may differ from the batch's in its position.
+// start_index (the _wrapped entries): the start index of each map of the call (null: (0, 0)), which its elevation comes in and
+// its host outputs go back in.
 int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int nmaps, const ElevSource& src, float* slope, float* step,
-              float* rough, float* trav, int memory, const MapSel* sel = nullptr, bool at = false, const double* position_xy = nullptr) {
+              float* rough, float* trav, int memory, const MapSel* sel = nullptr, bool at = false, const double* position_xy = nullptr,
+              const int32_t* start_index = nullptr) {
   te_ctx* c = m->ctx;
   te_geometry g0;
   if (src.image && g_in && (g_in->start_row != 0 || g_in->start_col != 0))
@@ -1916,8 +2060,11 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
     return rc;
   }
   if (int rc = check_params(p)) return rc;
-  if (nmaps > 0)
+  if (nmaps > 0) {
     if (int rc = check_positions(position_xy, nmaps)) return rc;
+    if (int rc = check_start_indices(start_index, nmaps, g0.rows, g0.cols)) return rc;
+  }
+  const bool wrapped = any_start(start_index, nmaps);  // the elevation comes in, and host outputs go back, in buffer order
   if (!src.layer && !src.image && !src.cut) return fail(TE_ERR_MISSING_LAYER, "layer elevation is missing");
   if (sel && src.cut)
     if (const uint32_t extra = src.cut->mask & TE_LAYER_CARRIED & ~m->carried)
@@ -1935,17 +2082,27 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
   const size_t cells = map_cells(m) * (sel ? sel->n : 0);
   const float* din = src.layer;
   if (sel) {
-    const bool packed = memory == TE_MEM_HOST || src.image || src.cut;  // sel[0]: the staged, converted or cut elevation
+    // sel[0]: the staged, unwrapped, converted or cut elevation
+    const bool packed = memory == TE_MEM_HOST || src.image || src.cut || wrapped;
     if (int rc = map_stage_selection(m, *sel, packed ? 0x1fu : 0x1eu)) return rc;
-    if (memory == TE_MEM_HOST && src.layer) {
+    if (src.layer && wrapped) {
+      float* const d = (float*)lay[0]->p;
+      if (int rc = map_unwrap_in(m, nmaps, start_index, 1, &src.layer, &d, memory)) return rc;
+      din = d;
+    } else if (memory == TE_MEM_HOST && src.layer) {
       TE_CUDA(map_copy_packed(m, (float*)lay[0]->p, src.layer, cells, false, memory));
       din = (const float*)lay[0]->p;
     }
   } else {
     if (int rc = map_reset(m, g_in, &g0, nmaps)) return rc;
     TE_CUDA(m->rough.reserve(sizeof(float) * batch_cells(m)));
-    if (src.layer)
+    if (src.layer && wrapped) {
+      TE_CUDA(m->elev.reserve(sizeof(float) * batch_cells(m)));
+      float* const d = (float*)m->elev.p;
+      if (int rc = map_unwrap_in(m, nmaps, start_index, 1, &src.layer, &d, memory)) return rc;
+    } else if (src.layer) {
       if (int rc = map_put_layer(m, m->elev, src.layer, memory)) return rc;
+    }
     din = (const float*)m->elev.p;
   }
   if (src.image) {
@@ -1967,6 +2124,7 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
                             nullptr, nullptr, nullptr, TE_MEM_DEVICE, spread ? &tab : nullptr))
     return rc;
   map_place(m, sel ? sel->idx : nullptr, nmaps, at_xy);
+  map_set_starts(m, sel ? sel->idx : nullptr, nmaps, start_index);
   if (sel) {
     const float* const src_l[te::kMapSlotLayers] = {(const float*)lay[4]->p, (const float*)lay[1]->p, (const float*)lay[2]->p,
                                                     (const float*)lay[3]->p, din, nullptr};
@@ -1978,11 +2136,17 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
     m->have_layers = true;
   }
   const std::pair<float*, DevBuf*> outs[4] = {{slope, lay[1]}, {step, lay[2]}, {rough, lay[3]}, {trav, lay[4]}};
-  for (const auto& o : outs)
-    if (o.first) {
-      if (sel) TE_CUDA(map_copy_packed(m, o.first, (const float*)o.second->p, cells, true, memory));
-      else if (int rc = map_get_layer(m, o.first, o.second->p, memory)) return rc;
-    }
+  if (wrapped && memory == TE_MEM_HOST) {  // the launch's maps are back to back in lay[] on a whole batch and on a selection
+    float* const out[4] = {slope, step, rough, trav};
+    const float* const dev[4] = {(const float*)lay[1]->p, (const float*)lay[2]->p, (const float*)lay[3]->p, (const float*)lay[4]->p};
+    if (int rc = map_wrap_out(m, wrap_blocks(m, nmaps, start_index, 4, out, dev))) return rc;
+  } else {
+    for (const auto& o : outs)
+      if (o.first) {
+        if (sel) TE_CUDA(map_copy_packed(m, o.first, (const float*)o.second->p, cells, true, memory));
+        else if (int rc = map_get_layer(m, o.first, o.second->p, memory)) return rc;
+      }
+  }
   if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));
   return TE_OK;
 }
@@ -1992,17 +2156,21 @@ int map_chain(te_map* m, const te_geometry* g_in, const te_chain_params* p, int 
 // layers must then be those the batch holds.
 int map_set_layers(te_map* m, const te_geometry* g_in, int nmaps, const float* trav, const float* slope, const float* step,
                    const float* rough, const float* elev, const float* robot_slope, int memory, const MapSel* sel = nullptr,
-                   bool at = false, const double* position_xy = nullptr) {
+                   bool at = false, const double* position_xy = nullptr, const int32_t* start_index = nullptr) {
   te_ctx* c = m->ctx;
   te_geometry g0;
   if (sel) {
     if (int rc = map_select(m, true, g_in, *sel, at)) return rc;
     nmaps = sel->n;
+    g0 = m->geo;
   } else if (int rc = unwrap_geometry(g_in, memory == TE_MEM_HOST && nmaps == 1, &g0)) {
     return rc;
   }
-  if (nmaps > 0)
+  if (nmaps > 0) {
     if (int rc = check_positions(position_xy, nmaps)) return rc;
+    if (int rc = check_start_indices(start_index, nmaps, g0.rows, g0.cols)) return rc;
+  }
+  const bool wrapped = any_start(start_index, nmaps);  // the layers come in buffer order
   const std::vector<double> at_xy = launch_positions(position_xy, std::max(nmaps, 0), g_in->position_x, g_in->position_y);
   if (!trav) return fail(TE_ERR_MISSING_LAYER, "layer traversability is missing");
   if (!slope) return fail(TE_ERR_MISSING_LAYER, "layer traversability_slope is missing");
@@ -2020,33 +2188,55 @@ int map_set_layers(te_map* m, const te_geometry* g_in, int nmaps, const float* t
     const float* src[te::kMapSlotLayers] = {trav, slope, step, rough, elev, robot_slope};
     DevBuf* const dst[te::kMapSlotLayers] = {&m->trav, &m->slope, &m->step, rough ? &m->rough : nullptr, &m->elev,
                                              robot_slope ? &m->rslope : nullptr};
-    unsigned staged = 0;  // host memory: the layers given, staged; device memory: read in place
+    unsigned staged = 0;  // host memory or buffer order: the layers given, staged or unwrapped; device memory: read in place
     for (int l = 0; l < te::kMapSlotLayers; ++l)
-      if (memory == TE_MEM_HOST && src[l]) staged |= 1u << l;
+      if ((memory == TE_MEM_HOST || wrapped) && src[l]) staged |= 1u << l;
     if (int rc = map_stage_selection(m, *sel, staged)) return rc;
-    if (memory == TE_MEM_HOST)
+    if (wrapped) {
+      std::vector<const float*> in;
+      std::vector<float*> to;
+      for (int l = 0; l < te::kMapSlotLayers; ++l)
+        if (src[l]) {
+          in.push_back(src[l]);
+          to.push_back((float*)m->sel[l].p);
+          src[l] = (const float*)m->sel[l].p;
+        }
+      if (int rc = map_unwrap_in(m, sel->n, start_index, (int)in.size(), in.data(), to.data(), memory)) return rc;
+    } else if (memory == TE_MEM_HOST) {
       for (int l = 0; l < te::kMapSlotLayers; ++l)
         if (src[l]) {
           TE_CUDA(map_copy_packed(m, (float*)m->sel[l].p, src[l], map_cells(m) * sel->n, false, memory));
           src[l] = (const float*)m->sel[l].p;
         }
+    }
     if (int rc = map_put_selected(m, *sel, src, dst)) return rc;
     map_place(m, sel->idx, sel->n, at_xy);
+    map_set_starts(m, sel->idx, sel->n, start_index);
     if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));  // the caller may reuse its layers on return
     return TE_OK;
   }
   if (int rc = map_reset(m, g_in, &g0, nmaps)) return rc;
-  if (int rc = map_put_layer(m, m->trav, trav, memory)) return rc;
-  if (int rc = map_put_layer(m, m->slope, slope, memory)) return rc;
-  if (int rc = map_put_layer(m, m->step, step, memory)) return rc;
-  if (int rc = map_put_layer(m, m->elev, elev, memory)) return rc;
-  if (rough)
-    if (int rc = map_put_layer(m, m->rough, rough, memory)) return rc;
-  if (robot_slope)
-    if (int rc = map_put_layer(m, m->rslope, robot_slope, memory)) return rc;
+  const std::pair<const float*, DevBuf*> put[6] = {{trav, &m->trav}, {slope, &m->slope}, {step, &m->step}, {elev, &m->elev},
+                                                   {rough, &m->rough}, {robot_slope, &m->rslope}};
+  if (wrapped) {  // every layer given, unwrapped in one launch
+    std::vector<const float*> in;
+    std::vector<float*> to;
+    for (const auto& q : put)
+      if (q.first) {
+        TE_CUDA(q.second->reserve(sizeof(float) * batch_cells(m)));
+        in.push_back(q.first);
+        to.push_back((float*)q.second->p);
+      }
+    if (int rc = map_unwrap_in(m, nmaps, start_index, (int)in.size(), in.data(), to.data(), memory)) return rc;
+  } else {
+    for (const auto& q : put)
+      if (q.first)
+        if (int rc = map_put_layer(m, *q.second, q.first, memory)) return rc;
+  }
   m->have_rough = rough != nullptr;
   m->have_rslope = robot_slope != nullptr;
   map_place(m, nullptr, nmaps, at_xy);
+  map_set_starts(m, nullptr, nmaps, start_index);
   if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));  // the caller may reuse its layers on return
   m->have_layers = true;
   return TE_OK;
@@ -2117,6 +2307,64 @@ int te_map_positions(te_map* m, double* position_xy) {
   if (int rc = map_ready(m)) return rc;
   if (!position_xy) return fail(TE_ERR_BAD_ARG, "position_xy is null");
   std::memcpy(position_xy, m->pos.data(), sizeof(double) * m->pos.size());
+  return TE_OK;
+}
+
+namespace {
+
+// The _wrapped entries take the start index in their own array only.
+int check_wrapped_geometry(const te_geometry* g) {
+  if (g && (g->start_row != 0 || g->start_col != 0))
+    return fail(TE_ERR_BAD_ARG, "g has start index (%d,%d): the _wrapped entries take each map's start index in start_index, and g's "
+                "must be (0,0)", g->start_row, g->start_col);
+  return TE_OK;
+}
+
+}  // namespace
+
+int te_map_chain_batched_wrapped(te_map* m, const te_geometry* g, const te_chain_params* p, int32_t nmaps, const float* elev, float* slope,
+                                 float* step, float* rough, float* trav, int memory, const double* position_xy, const int32_t* start_index) {
+  TE_MAP_ENTER(m);
+  if (int rc = check_wrapped_geometry(g)) return rc;
+  return map_chain(m, g, p, nmaps, ElevSource{elev, nullptr}, slope, step, rough, trav, memory, nullptr, true, position_xy, start_index);
+}
+
+int te_map_set_layers_batched_wrapped(te_map* m, const te_geometry* g, int32_t nmaps, const float* trav, const float* slope, const float* step,
+                                      const float* rough, const float* elev, const float* robot_slope, int memory, const double* position_xy,
+                                      const int32_t* start_index) {
+  TE_MAP_ENTER(m);
+  if (int rc = check_wrapped_geometry(g)) return rc;
+  return map_set_layers(m, g, nmaps, trav, slope, step, rough, elev, robot_slope, memory, nullptr, true, position_xy, start_index);
+}
+
+int te_map_chain_maps_wrapped(te_map* m, const te_geometry* g, const te_chain_params* p, int32_t nsel, const int32_t* map_index,
+                              const float* elev, float* slope, float* step, float* rough, float* trav, int memory, const double* position_xy,
+                              const int32_t* start_index) {
+  TE_MAP_ENTER(m);
+  if (int rc = check_wrapped_geometry(g)) return rc;
+  const MapSel sel{nsel, map_index};
+  return map_chain(m, g, p, nsel, ElevSource{elev, nullptr}, slope, step, rough, trav, memory, &sel, true, position_xy, start_index);
+}
+
+int te_map_set_layers_maps_wrapped(te_map* m, const te_geometry* g, int32_t nsel, const int32_t* map_index, const float* trav,
+                                   const float* slope, const float* step, const float* rough, const float* elev, const float* robot_slope,
+                                   int memory, const double* position_xy, const int32_t* start_index) {
+  TE_MAP_ENTER(m);
+  if (int rc = check_wrapped_geometry(g)) return rc;
+  const MapSel sel{nsel, map_index};
+  return map_set_layers(m, g, nsel, trav, slope, step, rough, elev, robot_slope, memory, &sel, true, position_xy, start_index);
+}
+
+int te_map_start_indices(te_map* m, int32_t* start_index) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (!start_index) return fail(TE_ERR_BAD_ARG, "start_index is null");
+  if (m->geo_in.start_row != 0 || m->geo_in.start_col != 0) {  // a single map whose start index came in g
+    start_index[0] = m->geo_in.start_row;
+    start_index[1] = m->geo_in.start_col;
+    return TE_OK;
+  }
+  std::memcpy(start_index, m->start.data(), sizeof(int32_t) * m->start.size());
   return TE_OK;
 }
 
@@ -2196,6 +2444,11 @@ int te_map_carry_layers(te_map* m, int32_t nsel, const int32_t* map_index, uint3
       dst[n++] = b == 5 ? &m->rslope : &m->carry[b - kCarryBit0];
     }
   const size_t cells = whole ? batch_cells(m) : map_cells(m) * sel.n;
+  // maps with a start index of their own (the _wrapped entries) take their layers in that buffer order: unwrapped in one launch
+  const std::vector<int32_t> starts = map_starts(m, whole ? nullptr : &sel);
+  const bool wrapped = any_start(starts.data(), whole ? m->nmaps : sel.n);
+  std::vector<const float*> win;
+  std::vector<float*> wto;
   te::MapSlots a{};
   a.nsel = whole ? m->nmaps : sel.n;
   a.cells = map_cells(m);
@@ -2204,20 +2457,33 @@ int te_map_carry_layers(te_map* m, int32_t nsel, const int32_t* map_index, uint3
   if (whole) {
     for (int k = 0; k < n; ++k) TE_CUDA(dst[k]->reserve(sizeof(float) * batch_cells(m)));
     for (int k = 0; k < n; ++k) {
-      if (src[k]) {
+      if (src[k] && wrapped) {
+        win.push_back(src[k]);
+        wto.push_back((float*)dst[k]->p);
+      } else if (src[k]) {
         if (int rc = map_put_layer(m, *dst[k], src[k], memory)) return rc;
       } else {
         a.fill[k] = (float*)dst[k]->p;
         fills = true;
       }
     }
+    if (!win.empty())
+      if (int rc = map_unwrap_in(m, m->nmaps, starts.data(), (int)win.size(), win.data(), wto.data(), memory)) return rc;
   } else {
-    unsigned staged = 0;  // host memory: the layers given, staged; device memory: read in place
+    unsigned staged = 0;  // host memory or buffer order: the layers given, staged or unwrapped; device memory: read in place
     for (int k = 0; k < n; ++k)
-      if (memory == TE_MEM_HOST && src[k]) staged |= 1u << k;
+      if ((memory == TE_MEM_HOST || wrapped) && src[k]) staged |= 1u << k;
     if (int rc = map_stage_selection(m, sel, staged)) return rc;
+    for (int k = 0; k < n; ++k)
+      if (src[k] && wrapped) {
+        win.push_back(src[k]);
+        wto.push_back((float*)m->sel[k].p);
+        src[k] = (const float*)m->sel[k].p;
+      }
+    if (!win.empty())
+      if (int rc = map_unwrap_in(m, sel.n, starts.data(), (int)win.size(), win.data(), wto.data(), memory)) return rc;
     for (int k = 0; k < n; ++k) {
-      if (src[k] && memory == TE_MEM_HOST) {
+      if (src[k] && memory == TE_MEM_HOST && !wrapped) {
         TE_CUDA(map_copy_packed(m, (float*)m->sel[k].p, src[k], cells, false, memory));
         src[k] = (const float*)m->sel[k].p;
       }
@@ -2293,8 +2559,15 @@ static int map_footprint(te_map* m, const te_footprint_params* p, const MapSel* 
                        sel ? (const int*)m->slots.p : nullptr, sel ? n : 1, c->sms, c->stream);
   if (int r2 = launch_check(c, "map footprint", nl + fixed)) return r2;
   if (out && memory == TE_MEM_HOST) {
-    if (sel) TE_CUDA(map_copy_packed(m, out, dout, map_cells(m) * n, true, memory));
-    else if (int r2 = map_get_layer(m, out, m->cache.p, memory)) return r2;
+    const std::vector<int32_t> st = map_starts(m, sel);
+    const float* const from = sel ? dout : (const float*)m->cache.p;  // the swept maps back to back
+    if (any_start(st.data(), n)) {
+      if (int r2 = map_wrap_out(m, wrap_blocks(m, n, st.data(), 1, &out, &from))) return r2;
+    } else if (sel) {
+      TE_CUDA(map_copy_packed(m, out, dout, map_cells(m) * n, true, memory));
+    } else if (int r2 = map_get_layer(m, out, m->cache.p, memory)) {
+      return r2;
+    }
     TE_CUDA(cudaStreamSynchronize(c->stream));
   }
   return TE_OK;
@@ -2317,6 +2590,32 @@ static int map_footprint_polygon(te_map* m, const te_footprint_params* p, int32_
                                  const PolygonOutputs* outs, const te::PolygonReduce* reduce, int memory) {
   if (int rc = map_ready(m)) return rc;
   if (int rc = map_footprint_params(m, p)) return rc;
+  if (memory == TE_MEM_HOST && any_start(m->start.data(), m->nmaps)) {
+    // maps with start indices of their own: the sweep writes device staging in default order, then every map's block of every
+    // output is re-wrapped to its map's start index in one launch (best_yaw moves as 4-byte cells like the float layers)
+    Staging st(m->ctx, true, &m->geo);
+    const size_t bc = batch_cells(m), cells = map_cells(m);
+    std::vector<MapBlock> blocks;
+    auto stage = [&](float* host, int count) -> float* {
+      if (!host) return nullptr;
+      float* d = (float*)st.slot(sizeof(float) * bc * count);
+      if (d)
+        for (size_t q = 0; q < (size_t)count * m->nmaps; ++q) {
+          const size_t mi = q % m->nmaps;
+          blocks.push_back(MapBlock{d + q * cells, host + q * cells, m->start[2 * mi], m->start[2 * mi + 1]});
+        }
+      return d;
+    };
+    std::vector<PolygonOutputs> dev(outs, outs + nouts);
+    for (PolygonOutputs& o : dev) o.out = stage(o.out, o.count);
+    te::PolygonReduce red{};
+    if (reduce) red = te::PolygonReduce{stage(reduce->worst, 1), stage(reduce->best, 1), (int32_t*)stage((float*)reduce->best_yaw, 1)};
+    if (st.rc) return st.rc;
+    if (int rc = map_footprint_polygon(m, p, npts, pts_xy, nouts, dev.data(), reduce ? &red : nullptr, TE_MEM_DEVICE)) return rc;
+    if (int rc = map_wrap_out(m, blocks)) return rc;
+    TE_CUDA(cudaStreamSynchronize(m->ctx->stream));
+    return TE_OK;
+  }
   if (m->spread) {
     // Maps at several positions: the sweep classifies the polygon's offsets against absolute positions on the host, so each map
     // is swept on its own geometry (one sweep per map, every output in the batch's layout).  Map m's layers and its layer of
@@ -2461,7 +2760,16 @@ int te_map_footprint_polygon_keep(te_map* m, const te_footprint_params* p, int32
   if (int r2 = launch_check(c, "map polygon footprint", nl + fixed)) return r2;
   m->have_fpoly = true;
   float* const outs[2] = {out_x, out_rot};
-  if (whole) {
+  const std::vector<int32_t> starts = map_starts(m, whole ? nullptr : &sel);
+  if (host_out && any_start(starts.data(), n)) {  // the swept maps' blocks, re-wrapped straight from their resident slots
+    std::vector<MapBlock> b;
+    for (int l = 0; l < 2; ++l)
+      if (outs[l])
+        for (int k = 0; k < n; ++k)
+          b.push_back(MapBlock{(const float*)m->fpoly[l].p + (size_t)(whole ? k : sel.idx[k]) * map_cells(m), outs[l] + k * map_cells(m),
+                               starts[2 * k], starts[2 * k + 1]});
+    if (int r2 = map_wrap_out(m, b)) return r2;
+  } else if (whole) {
     for (int l = 0; l < 2; ++l)
       if (outs[l])
         if (int r2 = map_get_layer(m, outs[l], m->fpoly[l].p, memory)) return r2;
@@ -2643,7 +2951,12 @@ int te_map_get_footprint(te_map* m, float* dst, int memory) {
   if (!dst) return fail(TE_ERR_BAD_ARG, "output layer is null");
   if (memory != TE_MEM_HOST && (m->geo_in.start_row != 0 || m->geo_in.start_col != 0))
     return fail(TE_ERR_UNSUPPORTED, "the map's layers came with a circular-buffer start index: read its cache into host memory");
-  if (int rc = map_get_layer(m, dst, m->cache.p, memory)) return rc;
+  if (memory == TE_MEM_HOST && any_start(m->start.data(), m->nmaps)) {
+    const float* const from = (const float*)m->cache.p;
+    if (int rc = map_wrap_out(m, wrap_blocks(m, m->nmaps, m->start.data(), 1, &dst, &from))) return rc;
+  } else if (int rc = map_get_layer(m, dst, m->cache.p, memory)) {
+    return rc;
+  }
   if (memory == TE_MEM_HOST) TE_CUDA(cudaStreamSynchronize(c->stream));
   return TE_OK;
 }
@@ -2806,6 +3119,24 @@ int te_map_get_layers(te_map* m, uint32_t layer_mask, float* out, int memory) {
   if (!out) return fail(TE_ERR_BAD_ARG, "output layer is null");
   // uncertainty_range (a null entry) is computed straight into a device output; in host memory into staging, which finish()
   // re-wraps and copies back after the other layers
+  if (memory == TE_MEM_HOST && any_start(m->start.data(), m->nmaps)) {
+    // maps with start indices of their own: uncertainty_range into staging, then every map's block of every layer re-wrapped in
+    // one launch and read back in one copy
+    Staging st(c, true, &m->geo);
+    std::vector<float*> outs(nl);
+    for (int k = 0; k < nl; ++k) {
+      outs[k] = out + (size_t)k * batch_cells(m);
+      if (src[k]) continue;
+      float* d = (float*)st.slot(sizeof(float) * batch_cells(m));
+      if (st.rc) return st.rc;
+      te::launch_uncertainty_range((const float*)m->carry[0].p, (const float*)m->carry[1].p, d, batch_cells(m), c->sms, c->stream);
+      if (int rc = launch_check(c, "k_uncertainty_range")) return rc;
+      src[k] = d;
+    }
+    if (int rc = map_wrap_out(m, wrap_blocks(m, m->nmaps, m->start.data(), nl, outs.data(), src))) return rc;
+    TE_CUDA(cudaStreamSynchronize(c->stream));
+    return TE_OK;
+  }
   Staging st(c, memory == TE_MEM_HOST, &m->geo_in);
   for (int k = 0; k < nl; ++k) {  // per layer every map, back to back
     float* dst = out + (size_t)k * batch_cells(m);

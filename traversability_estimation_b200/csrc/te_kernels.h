@@ -93,20 +93,25 @@ struct MapAtPoses {
 // One k_map_at_poses launch (none for nposes = 0).
 void launch_map_at_poses(const MapAtPoses& a, int sms, cudaStream_t s);
 
-// te_map_chain_submap / te_map_chain_windows: nmaps windows of rows x cols cells cut out of the layers of a larger map (device
-// pointers).  Window k starts at source cell top[k] = (row, col), which may lie outside the source; layer l of window k goes
-// column-major to dst[k * nlayers + l].  Source cell (I, J) is stored at src[l][col_of(Jb) * src_rows + Ib], (Ib, Jb) = (I +
-// start_row, J + start_col) modulo the source size and col_of the identity, or the table col_of when only some source columns
-// were staged; a cell outside the source is NaN 0x7fc00000.
-constexpr int kCutMaxLayers = 8;  // elevation and the seven carried layers
+// nmaps windows of rows x cols cells, each read out of a source of src_rows x src_cols cells through that source's circular-buffer
+// start index (device pointers).  Window k is win[k] = (top_row, top_col, start_row, start_col): it starts at source cell (top_row,
+// top_col), which may lie outside the source, and layer l of it goes column-major to dst[k * nlayers + l].  Source cell (I, J) of
+// window k's layer l is stored at src[k * nlayers + l][col_of(Jb) * src_rows + Ib], (Ib, Jb) = (I + start_row, J + start_col)
+// modulo the source size and col_of the identity, or the table col_of when only some source columns were staged; a cell outside
+// the source is NaN 0x7fc00000.  One kernel serves three moves:
+//   - te_map_chain_submap / te_map_chain_windows: every window on the one larger map, at its top-left, with that map's start index;
+//   - unwrapping a map that came in its own buffer order: top-left (0, 0), the map's block as source, its start index (sr, sc);
+//   - re-wrapping a resident default-order map to that order: top-left (0, 0), start index ((rows - sr) % rows, (cols - sc) % cols).
+// Cells move as 4-byte words, unchanged (NaN payloads and int32 layers included).
+constexpr int kCutMaxLayers = 8;  // a cut's source layers: elevation and the seven carried layers
 struct WindowCut {
-  const float* src[kCutMaxLayers];
-  const int2* top;         // device, nmaps
-  float* const* dst;       // device, nmaps * nlayers
-  const int* col_of;       // device, src_cols entries, or null
+  const int4* win;          // device, nmaps
+  const float* const* src;  // device, nmaps * nlayers
+  float* const* dst;        // device, nmaps * nlayers
+  const int* col_of;        // device, src_cols entries, or null
   int nlayers, nmaps, rows, cols;
-  int src_rows, src_cols, start_row, start_col;
-  long long ncolumns;      // nmaps * nlayers * cols
+  int src_rows, src_cols;
+  long long ncolumns;       // nmaps * nlayers * cols
 };
 // One k_map_cut_windows launch for every column of every window and layer (none when there is no column).
 void launch_cut_windows(const WindowCut& a, int sms, cudaStream_t s);

@@ -69,21 +69,22 @@ __device__ __forceinline__ void warp_fill_run(float* __restrict__ dst, float v, 
   for (int e = head + 4 * nv + lane; e < n; e += 32) dst[e] = v;
 }
 
-// One warp per destination column, numbered flat over (map, layer, column): column j of layer l of map k is the source column
-// top[k].y + j from source row top[k].x on, read through the source's circular-buffer start index, so at most two contiguous
-// runs of the stored column (before and after the row wrap), and NaN 0x7fc00000 (grid_map's unknown cell) for the rows and columns
-// the window takes from outside the source.  Integer arithmetic only: the host placed the windows.
+// One warp per destination column, numbered flat over (window, layer, column): column j of layer l of window k is the column
+// win[k].y + j of its source from source row win[k].x on, read through the window's start index (win[k].z, win[k].w), so at most
+// two contiguous runs of the stored column (before and after the row wrap), and NaN 0x7fc00000 (grid_map's unknown cell) for the
+// rows and columns the window takes from outside the source.  Integer arithmetic only: the host placed the windows.
 __global__ void __launch_bounds__(kGatherWarps * 32) k_map_cut_windows(const __grid_constant__ WindowCut a) {
   const int lane = threadIdx.x & 31;
   const float nan = __uint_as_float(0x7fc00000u);
   const long long per_map = (long long)a.nlayers * a.cols;
-  const long long nwarps = (long long)gridDim.x * kGatherWarps;
-  for (long long c = (long long)blockIdx.x * kGatherWarps + (threadIdx.x >> 5); c < a.ncolumns; c += nwarps) {
+  for (long long c = (long long)blockIdx.x * kGatherWarps + (threadIdx.x >> 5); c < a.ncolumns; c += (long long)gridDim.x * kGatherWarps) {
     const int k = (int)(c / per_map);
     const int r = (int)(c - (long long)k * per_map);
     const int l = r / a.cols, j = r - l * a.cols;
-    const int2 t = __ldg(a.top + k);
-    float* __restrict__ dst = a.dst[(size_t)k * a.nlayers + l] + (size_t)j * a.rows;
+    const int4 t = a.win[k];
+    const size_t kl = (size_t)k * a.nlayers + l;
+    float* __restrict__ dst = a.dst[kl] + (size_t)j * a.rows;
+    const float* __restrict__ src = a.src[kl];
     const long long J = (long long)t.y + j;  // the source column
     int i0 = 0, i1 = 0;                      // window rows [i0, i1) lie in the source
     if (J >= 0 && J < a.src_cols) {
@@ -93,10 +94,10 @@ __global__ void __launch_bounds__(kGatherWarps * 32) k_map_cut_windows(const __g
     }
     warp_fill_run(dst, nan, i0, lane);
     if (i1 > i0) {
-      int sc = (int)J + a.start_col;
+      int sc = (int)J + t.w;
       if (sc >= a.src_cols) sc -= a.src_cols;
-      const float* __restrict__ col = a.src[l] + (size_t)(a.col_of ? __ldg(a.col_of + sc) : sc) * a.src_rows;
-      int s0 = t.x + i0 + a.start_row;  // stored row of window row i0
+      const float* __restrict__ col = src + (size_t)(a.col_of ? __ldg(a.col_of + sc) : sc) * a.src_rows;
+      int s0 = t.x + i0 + t.z;  // stored row of window row i0
       if (s0 >= a.src_rows) s0 -= a.src_rows;
       const int n = i1 - i0, n1 = min(n, a.src_rows - s0);
       warp_copy_run(dst + i0, col + s0, n1, lane);
