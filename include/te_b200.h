@@ -1028,6 +1028,50 @@ int te_map_valid_at_batched(te_map* map, int32_t n, const int32_t* pos_map, cons
 int te_map_at_poses(te_map* map, const int32_t* pose_map_or_null, int32_t nposes, const double* poses, int32_t npoints,
                     const float* points_xyz, uint32_t layer_mask, float* out, uint8_t* valid_or_null, int memory);
 
+/* ---- Occupancy grids (GridMapRosConverter::toOccupancyGrid), as grid_map_visualization publishes a traversability map -------
+ * visualization.launch with config/visualization/traversability.yaml publishes traversability, traversability_slope,
+ * traversability_step and traversability_roughness as nav_msgs/OccupancyGrid, each with data_min 1.0 and data_max 0.0 (SURVEY.md
+ * A.7).  The entries below give the grids' data and MapMetaData; headers, stamps and frame ids stay the caller's. */
+
+/* nav_msgs/MapMetaData of a grid (its map_load_time is the caller's). */
+typedef struct te_occupancy_info {
+  int32_t width, height;      /* getSize(): rows, cols */
+  float resolution;           /* (float)resolution */
+  int32_t reserved;
+  double origin_x, origin_y;  /* getPosition() - 0.5 * getLength(), per axis in double; z 0, orientation identity */
+} te_occupancy_info;
+
+/* The MapMetaData of n grids of maps of geometry g: record k at position (position_xy[2k], position_xy[2k + 1]), or, with
+ * position_xy_or_null NULL, n records at g's position (te_map_positions gives a batch's positions).  g's start index changes
+ * nothing.  Host arithmetic, no GPU needed.  TE_ERR_BAD_ARG for a null or bad geometry, n < 0, a null out (n > 0) and a non-finite
+ * position, before any record is written. */
+int te_occupancy_grid_info(const te_geometry* g, int32_t n, const double* position_xy_or_null, te_occupancy_info* out);
+
+/* toOccupancyGrid of every layer of layer_mask for the maps of the call, in one kernel launch.
+ *   - Maps: nsel 0 with map_index_or_null NULL is every map of the batch; otherwise the maps map_index[0..nsel), a HOST array of
+ *     distinct indices in 0..nmaps-1 in any order, read before the call returns, as for the _maps entries.  Start indices never
+ *     matter, so every te_map takes a selection, one whose start index came in g included.
+ *   - Layers: any bits te_map_get_layers accepts, with its TE_ERR_MISSING_LAYER rules: the carried layers, robot_slope, the
+ *     traversability_footprint cache (NaN where empty), traversability_x / _rot, and TE_LAYER_UNCERTAINTY_RANGE (upper_bound -
+ *     lower_bound, one IEEE float32 subtraction per cell; its NaN payload does not matter, NaN gives -1).
+ *   - Ranges: data_min and data_max are HOST arrays of one float per set bit, in bit order: each layer has its own range.
+ *   - Cells: value = (v - data_min) / (data_max - data_min), each step one IEEE float32 operation rounded to nearest; NaN gives -1,
+ *     anything else 0 + min(max(0, value), 1) * 100, truncated toward zero.  So data_max == data_min gives 0 or 100 (+-Inf clamped),
+ *     or -1 where v equals data_min; a NaN or Inf bound is not checked and gives the formula's result.
+ *   - Output: per layer in bit order, the call's maps back to back in call order, rows*cols bytes each: map block k of layer l
+ *     starts at byte (l * n + k) * rows * cols, n the maps of the call.  A block is the map's grid: cell (i, j) of the map in
+ *     default (unwrapped) order at byte rows*cols - 1 - (j*rows + i), whatever its start index (unlike te_map_get_layers, whose
+ *     host output is re-wrapped).  Reshaped (cols, rows) in C order it is OccupancyGrid.data as (height, width).
+ *   - Memory: host memory writes the grids into staging and copies them back once; the call returns synchronised.  Device
+ *     memory is asynchronous on the context stream, with no host synchronisation and no allocation once the scratch exists.  A
+ *     whole-batch device call passes everything to the kernel by value, so it can be captured in a CUDA graph; a selection
+ *     uploads its slot table as the _maps entries do, and is not promised to be capturable.
+ *   - Errors, every one found before anything is written (out is then untouched): TE_ERR_BAD_ARG for a map without layers, an
+ *     empty mask or unknown bits, a null data_min, data_max or out, an unknown memory mode and a bad selection;
+ *     TE_ERR_MISSING_LAYER as te_map_get_layers. */
+int te_map_get_occupancy(te_map* map, int32_t nsel, const int32_t* map_index_or_null, uint32_t layer_mask, const float* data_min,
+                         const float* data_max, int8_t* out, int memory);
+
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the
  * neighbours' boundary columns of the INPUT layer(s) into this rank's halo.  The reference has no counterpart (it is a

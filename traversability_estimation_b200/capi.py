@@ -62,6 +62,16 @@ SUBMAP_INFO_DTYPE = np.dtype([(n, np.dtype(t._type_)) for n, t in SubmapInfo._fi
 assert SUBMAP_INFO_DTYPE.itemsize == C.sizeof(SubmapInfo)
 
 
+class OccupancyInfo(C.Structure):
+    """te_occupancy_info: an OccupancyGrid's MapMetaData (width = rows, height = cols, origin = position - 0.5 * length)."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("resolution", C.c_float), ("reserved", C.c_int32),
+                ("origin_x", C.c_double), ("origin_y", C.c_double)]
+
+
+OCCUPANCY_INFO_DTYPE = np.dtype([(n, np.dtype(t._type_)) for n, t in OccupancyInfo._fields_])
+assert OCCUPANCY_INFO_DTYPE.itemsize == C.sizeof(OccupancyInfo)
+
+
 def _windows(positions, lengths):
     p = np.ascontiguousarray(positions, dtype=np.float64).reshape(-1, 2)
     ln = np.ascontiguousarray(lengths, dtype=np.float64).reshape(-1, 2)
@@ -210,6 +220,8 @@ SIGNATURES = {
     "te_map_valid_at": (_R, [_P, _I, _P, _P, _I]),
     "te_map_valid_at_batched": (_R, [_P, _I, _P, _P, _P, _I]),
     "te_map_at_poses": (_R, [_P, _P, _I, _P, _I, _P, _U, _P, _P, _I]),
+    "te_occupancy_grid_info": (_R, [_G, _I, _P, _P]),
+    "te_map_get_occupancy": (_R, [_P, _I, _P, _U, _P, _P, _P, _I]),
     "te_ipc_export": (_R, [_P, _P]),
     "te_ipc_open": (_R, [_P, _P]),
     "te_ipc_close": (_R, [_P]),
@@ -272,6 +284,20 @@ def submap_geometry(g, positions, lengths):
     p, ln = _windows(positions, lengths)
     info = np.zeros(len(p), dtype=SUBMAP_INFO_DTYPE)
     rc = L.te_submap_geometry(C.byref(g), len(p), p.ctypes.data, ln.ctypes.data, info.ctypes.data)
+    if rc != 0:
+        raise TEError(rc, L.te_last_error().decode())
+    return info
+
+
+def occupancy_grid_info(g, positions=None):
+    """te_occupancy_grid_info: the MapMetaData of the occupancy grids of maps of geometry `g`, as an array of OCCUPANCY_INFO_DTYPE
+    records: one at g's position (positions None), or one per (x, y) row of `positions` (Map.positions() gives a batch's).  Host
+    arithmetic, no GPU needed."""
+    L = load_library()
+    p = None if positions is None else np.ascontiguousarray(positions, dtype=np.float64).reshape(-1, 2)
+    n = 1 if p is None else len(p)
+    info = np.zeros(n, dtype=OCCUPANCY_INFO_DTYPE)
+    rc = L.te_occupancy_grid_info(C.byref(g), n, _addr(p), info.ctypes.data)
     if rc != 0:
         raise TEError(rc, L.te_last_error().decode())
     return info
@@ -1297,3 +1323,37 @@ class Map:
         flat = out.reshape(-1)
         layers = {name: flat[k * n * npts:(k + 1) * n * npts].reshape(n, npts) for k, name in enumerate(order)}
         return layers, (None if valid is None else valid.reshape(n, npts))
+
+    def get_occupancy(self, names, data_min, data_max, maps=None, out=None, memory=MEM_HOST):
+        """te_map_get_occupancy (GridMapRosConverter::toOccupancyGrid): dict name -> int8 grid for `names` (LAYER_BITS entries),
+        each (height, width) = (cols, rows) in C order, as OccupancyGrid.data reshapes, whatever the map's start index.  data_min /
+        data_max: one float for every layer, or one per entry of `names`.  maps None: every map; otherwise the maps `maps` in that
+        order.  On a batch, or with `maps`, every grid is (n, cols, rows).  Host memory: numpy arrays.  Device memory: `out` is an
+        int8 device tensor of len(names) * n * rows * cols bytes, filled asynchronously on the context stream; the dict holds
+        views."""
+        names = list(names)
+        mask = layer_mask(names)
+        order = layer_order(mask)
+
+        def per_layer(v, what):
+            a = np.asarray(v, dtype=np.float32)
+            if a.ndim == 0:
+                return np.full(len(order), a, dtype=np.float32)
+            if a.shape != (len(names),):
+                raise ValueError(f"{what}: need one float or one per name ({len(names)}), got shape {a.shape}")
+            return np.ascontiguousarray([a[names.index(n)] for n in order], dtype=np.float32)   # bit order
+
+        lo, hi = per_layer(data_min, "data_min"), per_layer(data_max, "data_max")
+        idx = None if maps is None else self._map_index(maps)
+        n = self._n if idx is None else len(idx)
+        rows, cols = self._shape() if self._g else (0, 0)
+        if memory == MEM_HOST:
+            out = np.empty(len(order) * n * rows * cols, dtype=np.int8)
+        self._ctx._order_after_torch(memory)
+        self._check(self._L.te_map_get_occupancy(self._h, 0 if idx is None else len(idx), _addr(idx), mask, _addr(lo), _addr(hi),
+                                                 _addr(out), memory))
+        if idx is None and self._n == 1:
+            v = out.reshape(len(order), cols, rows)
+        else:
+            v = out.reshape(len(order), n, cols, rows)
+        return {name: v[k] for k, name in enumerate(order)}

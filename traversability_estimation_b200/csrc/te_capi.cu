@@ -1625,6 +1625,8 @@ int map_layers(te_map* m, uint32_t mask, bool with_range, const float* out[kLaye
   return TE_OK;
 }
 
+int check_selection(const te_map* m, const MapSel& s);
+
 // Validates a selection on a te_map that has layers and, when the entry takes one (with_geometry), g against the batch's
 // geometry; any_position: except its position (the _at entries).  Writes nothing.
 int map_select(const te_map* m, bool with_geometry, const te_geometry* g, const MapSel& s, bool any_position = false) {
@@ -1643,6 +1645,11 @@ int map_select(const te_map* m, bool with_geometry, const te_geometry* g, const 
     if (std::memcmp(&gc, &m->geo, sizeof(te_geometry)) != 0)
       return fail(TE_ERR_BAD_ARG, "the geometry differs from the te_map's: reload the whole batch to change it");
   }
+  return check_selection(m, s);
+}
+
+// Validates the selection s on a te_map: 1..nmaps distinct indices of the batch.  Writes nothing.
+int check_selection(const te_map* m, const MapSel& s) {
   if (s.n < 1 || s.n > m->nmaps) return fail(TE_ERR_BAD_ARG, "nsel = %d: need 1..%d", s.n, m->nmaps);
   if (!s.idx) return fail(TE_ERR_BAD_ARG, "map_index is null");
   std::vector<char> seen(m->nmaps, 0);
@@ -3298,6 +3305,64 @@ int te_map_at_poses(te_map* m, const int32_t* pose_map, int32_t nposes, const do
   a.res = g.resolution; a.lenx = g.length_x; a.leny = g.length_y; a.posx = g.position_x; a.posy = g.position_y;
   te::launch_map_at_poses(a, c->sms, c->stream);
   if (int rc = launch_check(c, "k_map_at_poses")) return rc;
+  return st.finish();  // host memory: returns synchronised
+}
+
+int te_occupancy_grid_info(const te_geometry* g, int32_t n, const double* position_xy, te_occupancy_info* out) {
+  if (int rc = check_geometry(g, true)) return rc;
+  if (n < 0) return fail(TE_ERR_BAD_ARG, "negative record count");
+  if (n == 0) return TE_OK;
+  if (!out) return fail(TE_ERR_BAD_ARG, "out is null");
+  if (position_xy) {
+    if (int rc = check_positions(position_xy, n)) return rc;
+  } else if (!std::isfinite(g->position_x) || !std::isfinite(g->position_y)) {
+    return fail(TE_ERR_BAD_ARG, "the geometry's position is not finite");
+  }
+  for (int32_t k = 0; k < n; ++k) {  // MapMetaData: origin = getPosition() - 0.5 * getLength(), per axis in double
+    const double px = position_xy ? position_xy[2 * k] : g->position_x, py = position_xy ? position_xy[2 * k + 1] : g->position_y;
+    out[k] = te_occupancy_info{g->rows, g->cols, (float)g->resolution, 0, px - 0.5 * g->length_x, py - 0.5 * g->length_y};
+  }
+  return TE_OK;
+}
+
+int te_map_get_occupancy(te_map* m, int32_t nsel, const int32_t* map_index, uint32_t layer_mask, const float* data_min,
+                         const float* data_max, int8_t* out, int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  const float* src[kLayerBits];
+  int nl = 0;
+  if (int rc = map_layers(m, layer_mask, true, src, &nl)) return rc;
+  if (!data_min || !data_max || !out) return fail(TE_ERR_BAD_ARG, "data_min, data_max or out is null");
+  if (memory != TE_MEM_HOST && memory != TE_MEM_DEVICE) return fail(TE_ERR_BAD_ARG, "unknown memory mode %d", memory);
+  const bool whole = nsel == 0 && !map_index;
+  // the grids never depend on a start index (toOccupancyGrid walks the unwrapped index), so any te_map takes a selection
+  if (!whole)
+    if (int rc = check_selection(m, MapSel{nsel, map_index})) return rc;
+  te::MapOccupancy a{};
+  a.range_l = -1;
+  for (int l = 0; l < nl; ++l) {
+    if (src[l]) {
+      a.layer[l] = src[l];
+    } else {  // uncertainty_range: upper_bound - lower_bound per cell, as te_map_get_layers computes it
+      a.layer[l] = (const float*)m->carry[0].p;
+      a.lower = (const float*)m->carry[1].p;
+      a.range_l = l;
+    }
+    a.data_min[l] = data_min[l];
+    a.data_max[l] = data_max[l];
+  }
+  a.nlayers = nl;
+  a.nmaps = whole ? m->nmaps : nsel;
+  a.cells = (long long)map_cells(m);
+  if (!whole) {  // the slot table of the _maps entries
+    if (int rc = map_stage_selection(m, MapSel{nsel, map_index}, 0)) return rc;
+    a.slot = (const int*)m->slots.p;
+  }
+  Staging st(c, memory == TE_MEM_HOST, &m->geo);  // host memory: the grids into staging, then one copy back
+  a.out = (unsigned char*)st.out(out, (size_t)nl * a.nmaps * a.cells);
+  if (st.rc) return st.rc;
+  te::launch_map_occupancy(a, c->sms, c->stream);
+  if (int rc = launch_check(c, "k_map_occupancy")) return rc;
   return st.finish();  // host memory: returns synchronised
 }
 

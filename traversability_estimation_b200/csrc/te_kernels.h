@@ -65,6 +65,22 @@ void launch_gather_submaps(const SubmapGather& a, int sms, cudaStream_t s);
 // out[c] = upper[c] - lower[c] for n cells (device pointers), IEEE float32: publishTraversabilityMap's uncertainty_range.  One
 // k_uncertainty_range launch (none for n = 0).
 void launch_uncertainty_range(const float* upper, const float* lower, float* out, size_t n, int sms, cudaStream_t s);
+// te_map_get_occupancy: GridMapRosConverter::toOccupancyGrid of nlayers layers of nmaps maps (device pointers).  Block q = l * nmaps
+// + k of `out` (cells bytes at out + q * cells) is layer l of map slot[k] (slot null: map k) in grid order: out[q * cells + p] is
+// the cell of source index cells - 1 - p of that map's column-major, default-order block, with layer l's data_min / data_max.
+constexpr int kOccupancyMaxLayers = 17;  // te_layer bits 0 .. 17 but the unassigned 7
+struct MapOccupancy {
+  const float* layer[kOccupancyMaxLayers];  // resident layers in output order, every map of the te_map back to back
+  const float* lower;                       // lower_bound: layer[range_l] (upper_bound) - lower is uncertainty_range
+  float data_min[kOccupancyMaxLayers], data_max[kOccupancyMaxLayers];
+  int nlayers, range_l;                     // range_l: output index of uncertainty_range, or -1
+  int nmaps;                                // maps of the call
+  const int* slot;                          // device, nmaps map indices, or null
+  long long cells;                          // rows * cols
+  unsigned char* out;
+};
+// One k_map_occupancy launch for every layer and map (none when there is no cell).
+void launch_map_occupancy(const MapOccupancy& a, int sms, cudaStream_t s);
 struct GridGeo;
 // valid[q] = getIndex(xy[2q], xy[2q+1]) succeeds and traversability is finite there (device pointers; none launched for n = 0).
 // A batch of nmaps maps of geometry g back to back in `trav`: position q is on map pos_map[q] (null: map 0), and a map outside

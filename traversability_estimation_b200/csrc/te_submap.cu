@@ -1,6 +1,6 @@
 // te_submap.cu — the read side of a te_map: GetGridMap submaps of its resident layers (k_map_gather_submaps),
-// mapHasValidTraversabilityAt for a batch of positions (k_map_valid_at) and GridMap::atPosition at points around poses
-// (k_map_at_poses); and the windows a te_map update cuts out of a larger elevation map (k_map_cut_windows).  Compiled with --fmad=false: k_map_valid_at and k_map_at_poses index positions with te_grid.cuh's getIndex,
+// mapHasValidTraversabilityAt for a batch of positions (k_map_valid_at), GridMap::atPosition at points around poses
+// (k_map_at_poses) and GridMapRosConverter::toOccupancyGrid of its layers (k_map_occupancy); and the windows a te_map update cuts out of a larger elevation map (k_map_cut_windows).  Compiled with --fmad=false: k_map_valid_at and k_map_at_poses index positions with te_grid.cuh's getIndex,
 // which the host and the oracle evaluate without contraction, and k_map_at_poses places points as the polygonal paths do.
 #include <algorithm>
 
@@ -182,7 +182,73 @@ __global__ void __launch_bounds__(256) k_map_at_poses(const __grid_constant__ Ma
   }
 }
 
+// One cell of GridMapRosConverter::toOccupancyGrid: (v - dataMin) / (dataMax - dataMin), NaN -> -1, else 0 + clamp(., 0, 1) * 100
+// truncated toward zero, every step one IEEE float32 operation rounded to nearest (den = dataMax - dataMin).  The result's low
+// byte is the int8 cell: 0 .. 100, or 0xff (-1).
+__device__ __forceinline__ unsigned occupancy_cell(float v, float mn, float den) {
+  const float q = __fdiv_rn(__fsub_rn(v, mn), den);
+  if (isnan(q)) return 0xffu;
+  return (unsigned)__float2int_rz(__fadd_rn(0.0f, __fmul_rn(fminf(fmaxf(0.0f, q), 1.0f), 100.0f)));
+}
+
+// toOccupancyGrid of every (layer, map) block of a call: blockIdx.y walks the blocks q = l * nmaps + k, blockIdx.x / threadIdx.x the
+// cells of one block.  Block q's grid is its map's column-major layer reversed: out[q * cells + p] is the cell of source index
+// cells - 1 - p.  Each thread writes 4-byte words of the block (from its first 4-byte boundary on) from 4 consecutive source cells,
+// read as one 16-byte load where that is aligned; up to 3 head and 3 tail bytes per block are written one by one.
+__global__ void __launch_bounds__(256) k_map_occupancy(const __grid_constant__ MapOccupancy a) {
+  const long long N = a.cells, nblocks = (long long)a.nlayers * a.nmaps;
+  for (long long q = blockIdx.y; q < nblocks; q += gridDim.y) {
+    const int l = (int)(q / a.nmaps), k = (int)(q - (long long)l * a.nmaps);
+    const int m = a.slot ? __ldg(a.slot + k) : k;
+    const float* __restrict__ src = a.layer[l] + (size_t)m * N;
+    const float* __restrict__ low = l == a.range_l ? a.lower + (size_t)m * N : nullptr;
+    const float mn = a.data_min[l], den = __fsub_rn(a.data_max[l], mn);
+    unsigned char* __restrict__ dst = a.out + (size_t)q * N;
+    const long long head = min(N, (long long)((4u - ((unsigned)(uintptr_t)dst & 3u)) & 3u));
+    const long long nw = (N - head) >> 2, tail0 = head + 4 * nw;
+    // word u covers output bytes head + 4u .. + 3, i.e. source cells s0 .. s0 + 3 with s0 = N - 4 - head - 4u
+    const bool vec = (((uintptr_t)(src + (N - 4 - head)) | (low ? (uintptr_t)(low + (N - 4 - head)) : 0)) & 15u) == 0;
+    for (long long u = (long long)blockIdx.x * blockDim.x + threadIdx.x; u < nw + 8; u += (long long)gridDim.x * blockDim.x) {
+      if (u < nw) {
+        const long long s0 = N - 4 - head - 4 * u;
+        float4 v;
+        if (vec) {
+          v = __ldg(reinterpret_cast<const float4*>(src + s0));
+          if (low) {
+            const float4 w = __ldg(reinterpret_cast<const float4*>(low + s0));
+            v = make_float4(__fsub_rn(v.x, w.x), __fsub_rn(v.y, w.y), __fsub_rn(v.z, w.z), __fsub_rn(v.w, w.w));
+          }
+        } else {
+          v = make_float4(__ldg(src + s0), __ldg(src + s0 + 1), __ldg(src + s0 + 2), __ldg(src + s0 + 3));
+          if (low)
+            v = make_float4(__fsub_rn(v.x, __ldg(low + s0)), __fsub_rn(v.y, __ldg(low + s0 + 1)), __fsub_rn(v.z, __ldg(low + s0 + 2)),
+                            __fsub_rn(v.w, __ldg(low + s0 + 3)));
+        }
+        const unsigned word = occupancy_cell(v.w, mn, den) | occupancy_cell(v.z, mn, den) << 8 | occupancy_cell(v.y, mn, den) << 16 |
+                              occupancy_cell(v.x, mn, den) << 24;
+        *reinterpret_cast<unsigned*>(dst + head + 4 * u) = word;
+      } else {  // u - nw = 0..3: head byte u - nw; 4..7: tail byte u - nw - 4
+        const int e = (int)(u - nw);
+        const long long p = e < 4 ? (e < head ? e : -1) : (tail0 + e - 4 < N ? tail0 + e - 4 : -1);
+        if (p < 0) continue;
+        float v = __ldg(src + (N - 1 - p));
+        if (low) v = __fsub_rn(v, __ldg(low + (N - 1 - p)));
+        dst[p] = (unsigned char)occupancy_cell(v, mn, den);
+      }
+    }
+  }
+}
+
 }  // namespace
+
+void launch_map_occupancy(const MapOccupancy& a, int sms, cudaStream_t s) {
+  const long long nblocks = (long long)a.nlayers * a.nmaps;
+  if (nblocks <= 0 || a.cells <= 0) return;
+  const long long by = std::min<long long>(nblocks, 65535);
+  const long long per_block = (a.cells / 4 + 8 + 255) / 256;  // thread blocks that cover one (layer, map) block at one word each
+  const long long bx = std::max<long long>(1, std::min<long long>(per_block, ((long long)sms * 32 + by - 1) / by));
+  k_map_occupancy<<<dim3((unsigned)bx, (unsigned)by), 256, 0, s>>>(a);
+}
 
 void launch_map_at_poses(const MapAtPoses& a, int sms, cudaStream_t s) {
   const long long total = (long long)a.nposes * a.npoints;
