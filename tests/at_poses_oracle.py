@@ -3,30 +3,18 @@ Compiled on first use into a temporary directory (the source tree may be read-on
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "at_poses_oracle.cpp")
-_DEPS = [_SRC, os.path.join(_HERE, "..", "oracle", "te_oracle_footprint.cpp"), os.path.join(_HERE, "..", "oracle", "te_oracle.h")]
+import cpp_oracle
+
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        h = hashlib.sha256(b"".join(open(p, "rb").read() for p in _DEPS)).hexdigest()[:16]
-        out = os.path.join(tempfile.gettempdir(), f"te_at_poses_oracle_{os.getuid()}_{h}.so")
-        if not os.path.exists(out):
-            tmp = f"{out}.{os.getpid()}"
-            subprocess.check_call(["/usr/bin/g++", "-O2", "-std=c++17", "-fPIC", "-fopenmp", "-ffp-contract=off", "-fno-fast-math",
-                                   "-shared", "-o", tmp, _SRC])
-            os.replace(tmp, out)
-        L = C.CDLL(out)
+        L = cpp_oracle.load("at_poses_oracle", cpp_oracle.FOOTPRINT_ORACLE, ["-fopenmp"])
         L.teo_at_poses.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib

@@ -1,6 +1,8 @@
 """Helpers shared by the tests: layer comparison (SURVEY.md §8d tolerances), bit-for-bit comparison, and the maps, paths,
-footprints and requests of the footprint path-check tests."""
+footprints, requests and parameters of the footprint path-check tests.  The te_map helpers are in map_helpers.py."""
 import numpy as np
+
+import synth
 
 RTOL, ATOL = 1e-5, 1e-6  # |a-b| <= RTOL*|b| + ATOL ; NaN positions and exact 0.0/1.0 cells must match exactly
 
@@ -48,16 +50,78 @@ def same_polygons(cnt, xy, ref_cnt, ref_xy, what):
         assert np.array_equal(xy[q, :k].view(np.uint64), ref_xy[q, :k].view(np.uint64)), (what, q)
 
 
+def assert_same_answers(got, want, what=""):
+    """The outputs of two requests: is_safe equal, traversability and area bit for bit (NaN matches NaN), and the untraversable
+    polygons, when the request returns them."""
+    assert np.array_equal(got[0], want[0]), (what, np.nonzero(got[0] != want[0])[0][:10])
+    assert same(got[1], want[1]) and same(got[2], want[2]), what
+    if len(want) > 3:
+        same_polygons(got[3], got[4], want[3], want[4], what)
+
+
+def bits(a):
+    """The uint32 bit patterns of `a` as float32."""
+    return np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
+
+
+def assert_same_bits(a, b, what=""):
+    """float32 bit for bit: every NaN payload too."""
+    assert np.array_equal(bits(a), bits(b)), (what, int((bits(a) != bits(b)).sum()))
+
+
+def same_bits_or_nan(a, b):
+    """float32 bit for bit, except that a NaN matches any NaN (the GPU's NaN payloads differ from x86's)."""
+    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
+    return a.shape == b.shape and bool(np.all((bits(a) == bits(b)) | (np.isnan(a) & np.isnan(b))))
+
+
+def same_bytes(a, b):
+    """Equal shapes and equal bytes, of any dtype."""
+    a, b = np.asarray(a), np.asarray(b)
+    return a.shape == b.shape and np.array_equal(np.ascontiguousarray(a).view(np.uint8), np.ascontiguousarray(b).view(np.uint8))
+
+
+def same_values(a, b):
+    """NaN at the same cells, and equal values at the others."""
+    return np.array_equal(np.isnan(a), np.isnan(b)) and np.array_equal(a[~np.isnan(a)], b[~np.isnan(b)])
+
+
+def close_sweep(a, b):
+    """The tolerance of the prefix-sum footprint sweeps against the oracle: they add the same float32 terms in another order (double
+    accumulation), so a handful of cells whose disk holds default-valued (NaN) cells may differ in the last float32 bit.  NaN and
+    zero (blocked) cells are the same."""
+    if not np.array_equal(np.isnan(a), np.isnan(b)):
+        return False
+    m = ~np.isnan(a)
+    if not np.array_equal(a[m] == 0, b[m] == 0):
+        return False
+    return float((a[m] == b[m]).mean()) > 0.999 and np.allclose(a[m], b[m], rtol=2e-7, atol=0)
+
+
 # ---- maps, paths, footprints and requests of the path-check tests ----------------------------------------------------------
 
 YAML = [(0.45, 0.30, 0.0), (0.45, -0.30, 0.0), (-0.45, -0.30, 0.0), (-0.45, 0.30, 0.0)]   # robot_footprint_parameter.yaml:3
 
 
-def footprint_params(te, oracle, verify):
-    """(library, oracle) FootprintParams: the YAML defaults with verify_roughness set."""
-    ft, fo = te.FootprintParams.yaml_defaults(), oracle.FootprintParams.yaml_defaults()
-    ft.verify_roughness = fo.verify_roughness = verify
-    return ft, fo
+def footprint_params(te, oracle, verify=0, **kw):
+    """(library, oracle) FootprintParams: the YAML defaults with verify_roughness and the fields kw set."""
+    return te_footprint_params(te, verify_roughness=verify, **kw), te_footprint_params(oracle, verify_roughness=verify, **kw)
+
+
+def te_footprint_params(mod, **kw):
+    """The FootprintParams of `mod` (the library or the oracle): the YAML defaults with the fields kw set."""
+    p = mod.FootprintParams.yaml_defaults()
+    for k, v in kw.items():
+        setattr(p, k, v)
+    return p
+
+
+def chain_params(mod, **kw):
+    """The ChainParams of `mod` (the library or the oracle): the YAML defaults with the fields kw set."""
+    p = mod.ChainParams.yaml_defaults(0)
+    for k, v in kw.items():
+        setattr(p, k, v)
+    return p
 
 
 def chain_layers(oracle, og, z, seed):
@@ -198,6 +262,102 @@ def footprint_arrays(R, fps):
             fx.extend(fps[k].tolist())
         fb.append(len(fx))
     return np.asarray(fb, np.int32), np.asarray(fx, np.float32).reshape(-1, 3)
+
+
+def batch_request(rng, og, npaths, nmaps, fps=None, exclude=None, offsets=None, permute=True, **kw):
+    """A mixed_request (keywords kw) on a batch of nmaps maps of geometry og, with its footprints in R["fps"] (drawn first when
+    fps is None) and a path_map R["map"] that interleaves the maps in no order, leaving map `exclude` out.  permute: the first
+    paths visit every map.  offsets: per map, added to the x y of its paths' poses."""
+    if fps is None:
+        fps = request_footprints(rng)
+    R = mixed_request(rng, og, npaths, fps, **kw)
+    R["fps"] = fps
+    maps = [m for m in range(nmaps) if m != exclude]
+    R["map"] = np.asarray(maps, np.int32)[rng.integers(0, len(maps), len(R["kind"]))]
+    if permute:
+        R["map"][:len(maps)] = rng.permutation(maps)
+    if offsets is not None:
+        for q, m in enumerate(R["map"]):
+            R["poses"][R["begin"][q]:R["begin"][q + 1], :2] += offsets[m]
+    return R
+
+
+def subset(R, idx):
+    """The request of the paths `idx` of R, in that order: every per-path array R has, and its footprints."""
+    b, idx = R["begin"], np.asarray(idx, dtype=np.int64)
+    begin = np.concatenate([[0], np.cumsum(b[idx + 1] - b[idx])]).astype(np.int32)
+    poses = np.concatenate([R["poses"][b[q]:b[q + 1]] for q in idx]) if len(idx) else np.zeros((0, 7))
+    S = dict(begin=begin, poses=poses, **{k: R[k][idx] for k in ("radius", "kind", "cons", "cup", "map") if k in R})
+    if "fps" in R:
+        S["fps"] = R["fps"]
+    return S
+
+
+# ---- layers ------------------------------------------------------------------------------------------------------------------
+
+def wrap(a, start):
+    """A default-order (rows, cols) layer in the buffer order of start index `start`: cell (i, j) at ((i + sr) % rows, ...)."""
+    return np.roll(a, (int(start[0]), int(start[1])), axis=(0, 1))
+
+
+def unwrap(a, start):
+    """The default order of a layer stored with start index `start`: the inverse of wrap."""
+    return np.roll(a, (-int(start[0]), -int(start[1])), axis=(0, 1))
+
+
+def noisy(rng, shape, nan, inf, ninf, zero):
+    """A float32 layer with the fractions nan, inf, ninf and zero of NaN, +Inf, -Inf and exact zeros (a fraction of 0 draws
+    nothing), and 1% NaN of other payloads, signalling ones included."""
+    a = (rng.standard_normal(shape) * 3).astype(np.float32)
+    for frac, v in ((nan, np.nan), (inf, np.inf), (ninf, -np.inf), (zero, 0.0)):
+        if frac:
+            a[rng.random(shape) < frac] = v
+    odd = rng.random(shape) < 0.01
+    a.view(np.uint32)[odd] = (rng.integers(0, 2, odd.sum()) << 31 | 0x7f800000 | rng.integers(1, 1 << 23, odd.sum())).astype(np.uint32)
+    return a
+
+
+def walled_terrain(rows, cols, res, kind, seed):
+    """Neighbouring maps of a batch differ sharply: a flat map, a map walled along its first rows and columns, a terrain map, a map
+    walled along its last rows and columns.  A value read across a map boundary would change the cells along that boundary."""
+    if kind == 0:
+        return np.zeros((rows, cols), dtype=np.float32)
+    z = synth.terrain(rows, cols, res, seed, "mixed")
+    if kind == 1:
+        z[:5, :] += np.float32(1.0)
+        z[:, :5] += np.float32(1.0)
+    if kind == 3:
+        z[-5:, :] += np.float32(1.0)
+        z[:, -5:] += np.float32(1.0)
+    return z
+
+
+def walled_batch(oracle, rows, cols, res, n, seed, robot_slope=False):
+    """Chain layers of n walled_terrain maps on the CPU oracle, stacked as (n, cols, rows): map k's layers are the column-major
+    batch[k].T.  robot_slope: also a robot_slope layer per map (its slope with zeros and NaNs)."""
+    og = oracle.Geometry.make(rows, cols, res)
+    names = ("traversability", "slope", "step", "roughness", "elevation") + (("robot_slope",) if robot_slope else ())
+    out = {k: [] for k in names}
+    rng = np.random.default_rng(seed)
+    for k in range(n):
+        z = walled_terrain(rows, cols, res, k % 4, seed + k)
+        ch = oracle.chain(og, oracle.ChainParams.yaml_defaults(0), z)
+        slope, rough = np.array(ch["slope"], dtype=np.float32), np.array(ch["roughness"], dtype=np.float32)
+        for _ in range(3 if k % 4 else 0):
+            # zero patches: checkForRoughness blocks them when verify_roughness is set, checkForSlope with a small max_gap_width
+            a, b = int(rng.integers(0, rows - 10)), int(rng.integers(0, cols - 10))
+            rough[a:a + 9, b:b + 9] = 0.0
+            a, b = int(rng.integers(0, rows - 10)), int(rng.integers(0, cols - 10))
+            slope[a:a + 9, b:b + 9] = 0.0
+        layers = [ch["traversability"], slope, ch["step"], rough, z]
+        if robot_slope:
+            rs = np.array(ch["slope"], dtype=np.float32)
+            rs[rng.random(rs.shape) < 0.002] = 0.0
+            rs[rng.random(rs.shape) < 0.05] = np.nan
+            layers.append(rs)
+        for name, layer in zip(names, layers):
+            out[name].append(np.ascontiguousarray(np.asarray(layer, dtype=np.float32).T))
+    return {k: np.stack(v) for k, v in out.items()}
 
 
 # ---- the hand-derived maps of the untraversable-polygon tests --------------------------------------------------------------

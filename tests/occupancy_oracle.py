@@ -3,29 +3,18 @@ use into a temporary directory (the source tree may be read-only), with the foot
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "occupancy_oracle.cpp")
+import cpp_oracle
+
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        h = hashlib.sha256(open(_SRC, "rb").read()).hexdigest()[:16]
-        out = os.path.join(tempfile.gettempdir(), f"te_occupancy_oracle_{os.getuid()}_{h}.so")
-        if not os.path.exists(out):
-            tmp = f"{out}.{os.getpid()}"
-            subprocess.check_call(["/usr/bin/g++", "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared", "-o",
-                                   tmp, _SRC])
-            os.replace(tmp, out)
-        L = C.CDLL(out)
+        L = cpp_oracle.load("occupancy_oracle")
         L.teo_occupancy_grid.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_void_p]
         L.teo_occupancy_info.argtypes = [C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_void_p,
                                          C.c_void_p, C.c_void_p]

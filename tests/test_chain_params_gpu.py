@@ -12,19 +12,12 @@ import numpy as np
 import pytest
 
 import synth
-from helpers import assert_parity, compare_layer
+from helpers import assert_parity, chain_params, compare_layer
 
 pytestmark = pytest.mark.gpu
 
 LAYERS = ("slope", "step", "roughness", "traversability")
 N = 1024
-
-
-def _params(mod, **kw):
-    p = mod.ChainParams.yaml_defaults(0)
-    for k, v in kw.items():
-        setattr(p, k, v)
-    return p
 
 
 # Open case: with a power-of-two step_critical_cells, CNT * (1/ncrit) * stepMax rounds once in fp32 and may land just below
@@ -55,10 +48,10 @@ def _fused(te, ctx, oracle, z, res=0.02, pos=(0.0, 0.0), what="", step_branch=0,
     """KERNEL_FUSED and oracle.chain on z with the parameters kw; parity asserted; returns (layers, oracle layers, counters)."""
     rows, cols = z.shape
     g, og = te.Geometry.make(rows, cols, res, pos), oracle.Geometry.make(rows, cols, res, pos)
-    ref = oracle.chain(og, _params(oracle, **kw), z)
+    ref = oracle.chain(og, chain_params(oracle, **kw), z)
     ctx.set_kernel(te.KERNEL_FUSED)
     try:
-        got = ctx.chain_host(g, _params(te, **kw), z)
+        got = ctx.chain_host(g, chain_params(te, **kw), z)
         cnt = ctx.flag_counters()
     finally:
         ctx.set_kernel(te.KERNEL_AUTO)
@@ -225,7 +218,7 @@ def _bits_equal(torch, a, b):
 def test_batched_equals_single_maps(te, ctx):
     import torch
     rows, cols, n = 512, 384, 8
-    g, p = te.Geometry.make(rows, cols, 0.02), _params(te, **SET)
+    g, p = te.Geometry.make(rows, cols, 0.02), chain_params(te, **SET)
     maps = np.stack([np.ascontiguousarray(synth.terrain(rows, cols, 0.02, 500 + k, ("gentle", "mixed", "rough")[k % 3]).T)
                      for k in range(n)])
     zd = torch.from_numpy(maps).cuda()
@@ -249,7 +242,7 @@ def test_slabs_equal_the_whole_map(te, ctx):
     import torch
     rows = cols = 2048
     z = _terrain("mixed", 2048, 5)
-    g, p = te.Geometry.make(rows, cols, 0.02), _params(te, **SET)
+    g, p = te.Geometry.make(rows, cols, 0.02), chain_params(te, **SET)
     zd = _dev(torch, z)
     ctx.set_stream(None)
     ctx.set_kernel(te.KERNEL_FUSED)
@@ -272,7 +265,7 @@ def test_slabs_equal_the_whole_map(te, ctx):
 
 def test_map_chain_equals_context_chain(te, ctx):
     z = _terrain("rough", 512, 9)
-    g, p = te.Geometry.make(512, 512, 0.02), _params(te, **SET)
+    g, p = te.Geometry.make(512, 512, 0.02), chain_params(te, **SET)
     ctx.set_kernel(te.KERNEL_FUSED)
     try:
         want = ctx.chain_host(g, p, z)
@@ -303,13 +296,13 @@ def test_parameter_switches_on_one_context(te, ctx):
             c = te.Context(0)
             try:
                 c.set_kernel(te.KERNEL_FUSED)
-                fresh[key] = (c.chain_host(g, _params(te, **kw), z), c.flag_counters())
+                fresh[key] = (c.chain_host(g, chain_params(te, **kw), z), c.flag_counters())
             finally:
                 c.close()
     ctx.set_kernel(te.KERNEL_FUSED)
     try:
         for kw in sets:
-            got = ctx.chain_host(g, _params(te, **kw), z)
+            got = ctx.chain_host(g, chain_params(te, **kw), z)
             want, cnt = fresh[tuple(sorted(kw.items()))]
             for k in LAYERS:
                 assert np.array_equal(got[k].view(np.uint32), want[k].view(np.uint32)), (kw, k)

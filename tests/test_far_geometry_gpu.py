@@ -10,26 +10,12 @@ import pytest
 import far_geometry as fg
 import paths_oracle as po
 import synth
-from helpers import assert_parity, chain_layers
+from helpers import assert_parity, chain_layers, close_sweep, same_values
 
 pytestmark = pytest.mark.gpu
 
 ROWS, COLS = 160, 144
 POS = ["origin", "lv95", "utm"]
-
-
-def _same(a, b):
-    return np.array_equal(np.isnan(a), np.isnan(b)) and np.array_equal(a[~np.isnan(a)], b[~np.isnan(b)])
-
-
-def _close(a, b):
-    """test_footprint_gpu's tolerance of the prefix-sum sweep (another order of the double sums where default-valued cells enter)."""
-    if not np.array_equal(np.isnan(a), np.isnan(b)):
-        return False
-    m = ~np.isnan(a)
-    if not np.array_equal(a[m] == 0, b[m] == 0):
-        return False
-    return float((a[m] == b[m]).mean()) > 0.999 and np.allclose(a[m], b[m], rtol=2e-7, atol=0)
 
 
 def _geoms(te, oracle, res, pos):
@@ -84,7 +70,7 @@ def test_circular_sweep_membership(te, ctx, oracle, pos, res):
         ref2, _, _, _ = oracle.footprint(og, fo, *lay, roughness=lay[1])
         out = np.empty_like(lay[0])
         ctx.footprint(g, ft, *lay, out, te.MEM_HOST, roughness=lay[1])
-        if not _same(out, ref2):
+        if not same_values(out, ref2):
             wrong[(r + o, "roughness")] = int((out != ref2).sum())
     assert not wrong, wrong
 
@@ -99,8 +85,8 @@ def test_circular_sweep_on_chain_layers(te, ctx, oracle, pos, res):
         fo.radius = ft.radius = r
         fo.offset = ft.offset = o
         ref, _, _ = oracle.footprint(og, fo, *lay)
-        assert _same(_footprint(te, ctx, g, ft, lay, True), ref), (r + o, "brute")
-        assert _close(_footprint(te, ctx, g, ft, lay, False), ref), (r + o, "fast")
+        assert same_values(_footprint(te, ctx, g, ft, lay, True), ref), (r + o, "brute")
+        assert close_sweep(_footprint(te, ctx, g, ft, lay, False), ref), (r + o, "fast")
 
 
 def _polygons(res):
@@ -121,7 +107,7 @@ def test_polygon_sweep_membership(te, ctx, oracle, pos, res):
         ox, orot = np.empty_like(lay[0]), np.empty_like(lay[0])
         ctx.footprint_polygon(g, ft, poly, yaw, *lay, ox, orot, te.MEM_HOST)
         for a, b, name in ((ox, rx, "x"), (orot, rrot, "rot")):
-            if not _same(a, b):
+            if not same_values(a, b):
                 wrong[(k, name)] = int((a != b).sum())
     assert not wrong, wrong
 
@@ -138,7 +124,7 @@ def test_polygon_sweep_on_chain_layers(te, ctx, oracle, pos, res):
         ox, orot = np.empty_like(lay[0]), np.empty_like(lay[0])
         ctx.footprint_polygon(g, ft, poly, yaw, *lay, ox, orot, te.MEM_HOST)
         for a, b in ((ox, rx), (orot, rrot)):
-            assert np.array_equal(a == 0, b == 0) and _close(a, b), yaw
+            assert np.array_equal(a == 0, b == 0) and close_sweep(a, b), yaw
 
 
 @pytest.mark.parametrize("pos", POS)
@@ -190,12 +176,12 @@ def test_map_footprint_at_positions(te, ctx, oracle, res):
             m.set_layers_batched(g, 3, *(stack(a) for a in lay), positions=np.asarray(near))
             got = m.footprint(ft)
             for k, ref in enumerate(_oracle_maps(oracle, res, near, lay, fo)):
-                assert _same(got[k], ref), (r + o, "origin", k)
+                assert same_values(got[k], ref), (r + o, "origin", k)
             far = [fg.LV95, fg.UTM]
             m.set_layers_maps(g, [1, 2], *(np.stack([a] * 2) for a in lay), positions=np.asarray(far))
             got = m.footprint_maps(ft, [1, 2])
             for k, ref in enumerate(_oracle_maps(oracle, res, far, lay, fo)):
-                assert _same(got[k], ref), (r + o, far[k], int((got[k] != ref).sum()))
+                assert same_values(got[k], ref), (r + o, far[k], int((got[k] != ref).sum()))
         positions = [fg.ORIGIN, fg.LV95, fg.UTM]
         m.set_layers_batched(g, 3, *(stack(a) for a in lay), positions=np.asarray(positions))
         fo, ft = oracle.FootprintParams.yaml_defaults(), te.FootprintParams.yaml_defaults()
@@ -207,8 +193,8 @@ def test_map_footprint_at_positions(te, ctx, oracle, res):
                 og = oracle.Geometry.make(ROWS, COLS, res, p)
                 refs = np.stack([oracle.footprint_polygon(og, fo, [list(v) for v in pts], y, *lay)[1] for y in yaws])
                 for q in range(len(yaws)):
-                    assert _same(layers[q, k], refs[q]), (p, yaws[q], int((layers[q, k] != refs[q]).sum()))
-                assert _same(worst[k], refs.min(axis=0)) and _same(best[k], refs.max(axis=0)), p
+                    assert same_values(layers[q, k], refs[q]), (p, yaws[q], int((layers[q, k] != refs[q]).sum()))
+                assert same_values(worst[k], refs.min(axis=0)) and same_values(best[k], refs.max(axis=0)), p
                 assert np.array_equal(best_yaw[k], np.argmax(refs, axis=0)), p
     finally:
         m.close()

@@ -3,24 +3,9 @@ import numpy as np
 import pytest
 
 import synth
+from helpers import close_sweep, same_values
 
 pytestmark = pytest.mark.gpu
-
-
-def _same(a, b):
-    return np.array_equal(np.isnan(a), np.isnan(b)) and np.array_equal(a[~np.isnan(a)], b[~np.isnan(b)])
-
-
-def _close(a, b):
-    """The prefix-sum sweep adds the same float32 terms in another order (double accumulation): identical except for the
-    last float32 bit of a handful of cells whose disk holds default-valued (NaN) cells."""
-    if not np.array_equal(np.isnan(a), np.isnan(b)):
-        return False
-    m = ~np.isnan(a)
-    if not np.array_equal(a[m] == 0, b[m] == 0):
-        return False
-    exact = float((a[m] == b[m]).mean())
-    return exact > 0.999 and np.allclose(a[m], b[m], rtol=2e-7, atol=0)
 
 
 def _run(te, ctx, oracle, g, og, layers, fp_t, fp_o):
@@ -38,8 +23,8 @@ def _run(te, ctx, oracle, g, og, layers, fp_t, fp_o):
         tfp = np.empty_like(t)
         ctx.footprint(g, fp_t, t, s, st, e, out, te.MEM_HOST, slope_fp=sfp, step_fp=tfp)
         res.append((out, sfp, tfp))
-    assert _same(res[0][0], ref), "visit-by-visit sweep differs from the oracle"
-    assert _close(res[1][0], ref), ("prefix-sum sweep differs from the oracle", int((res[1][0] != ref).sum()),
+    assert same_values(res[0][0], ref), "visit-by-visit sweep differs from the oracle"
+    assert close_sweep(res[1][0], ref), ("prefix-sum sweep differs from the oracle", int((res[1][0] != ref).sum()),
                                     float(np.nanmax(np.abs(res[1][0] - ref))))
     return (ref, res[1][1], res[1][2]), (ref, rs, rt)
 
@@ -51,7 +36,7 @@ def test_footprint_on_fixture_layers(te, ctx, oracle, fixture_map):
     layers = (d["traversability"], d["traversability_slope"], d["traversability_step"], d["elevation"])
     got, ref = _run(te, ctx, oracle, g, og, layers, te.FootprintParams.yaml_defaults(), oracle.FootprintParams.yaml_defaults())
     for a, b, name in zip(got, ref, ("traversability_footprint", "slope_footprint", "step_footprint")):
-        assert _same(a, b), name
+        assert same_values(a, b), name
     assert (ref[0] == 0).sum() > 100 and (ref[0] > 0).sum() > 100
 
 
@@ -71,7 +56,7 @@ def test_footprint_matches_oracle_on_chain_outputs(te, ctx, oracle, case):
     fo.offset = ft.offset = case["offset"]
     got, ref = _run(te, ctx, oracle, g, og, (ch["traversability"], ch["slope"], ch["step"], z), ft, fo)
     for a, b, name in zip(got, ref, ("traversability_footprint", "slope_footprint", "step_footprint")):
-        assert _same(a, b), (name, int((np.isnan(a) != np.isnan(b)).sum()), float(np.nanmax(np.abs(a - b))))
+        assert same_values(a, b), (name, int((np.isnan(a) != np.isnan(b)).sum()), float(np.nanmax(np.abs(a - b))))
     assert (ref[0] == 0).any() and (ref[0] > 0).any()
     assert np.isfinite(ref[2]).sum() > 0  # step == 0 cells exist, so the gap walk was exercised
 
@@ -119,8 +104,8 @@ def test_footprint_1024_matches_oracle(te, ctx, oracle, offset):
     ref, rs, rt = oracle.footprint(og, fo, t, s, st, e)
     out, sfp, tfp = np.empty_like(t), np.empty_like(t), np.empty_like(t)
     ctx.footprint(g, ft, t, s, st, e, out, te.MEM_HOST, slope_fp=sfp, step_fp=tfp)
-    assert _close(out, ref), (int((out != ref).sum()), float(np.nanmax(np.abs(out - ref))))
-    assert _same(sfp, rs) and _same(tfp, rt)
+    assert close_sweep(out, ref), (int((out != ref).sum()), float(np.nanmax(np.abs(out - ref))))
+    assert same_values(sfp, rs) and same_values(tfp, rt)
     assert (ref == 0).any() and (ref > 0).any()
 
 
@@ -156,8 +141,8 @@ def test_footprint_with_roughness_verification(te, ctx, oracle):
             os.environ.pop("TE_FOOTPRINT_BRUTE", None)
         out, sfp, tfp, rfp = (np.empty_like(t) for _ in range(4))
         ctx.footprint(g, ft, t, s, st, e, out, te.MEM_HOST, slope_fp=sfp, step_fp=tfp, roughness=r, roughness_fp=rfp)
-        assert (_same if brute else _close)(out, ref)
-        assert _same(sfp, rs) and _same(tfp, rt) and _same(rfp, rr)
+        assert (same_values if brute else close_sweep)(out, ref)
+        assert same_values(sfp, rs) and same_values(tfp, rt) and same_values(rfp, rr)
     with pytest.raises(te.TEError) as err:   # the flag without the layer: TE_ERR_MISSING_LAYER, like GridMap::at on a missing layer
         ctx.footprint(g, ft, t, s, st, e, out, te.MEM_HOST)
     assert err.value.code == -2
@@ -220,7 +205,7 @@ def test_polygon_footprint_sweep_matches_oracle(te, ctx, oracle, case):
     for a, b, name in ((ox, rx, "traversability_x"), (orot, rrot, "traversability_rot")):
         assert not np.isnan(a).any() and not np.isnan(b).any(), name
         assert np.array_equal(a == 0, b == 0), (name, int(((a == 0) != (b == 0)).sum()))   # same cells blocked: same polygon membership
-        assert _close(a, b), (name, int((a != b).sum()), float(np.abs(a - b).max()))
+        assert close_sweep(a, b), (name, int((a != b).sum()), float(np.abs(a - b).max()))
     assert (rx == 0).any() and (rx > 0).any() and (rrot > 0).any()
     if case["yaw"] != 0.0:
         assert not np.array_equal(rx, rrot)
@@ -267,7 +252,7 @@ def test_polygon_footprint_with_roughness_check_and_argument_errors(te, ctx, ora
     ox, orot = np.empty_like(lay[0]), np.empty_like(lay[0])
     ctx.footprint_polygon(g, ft, poly, 0.5, *lay, ox, orot, te.MEM_HOST, roughness=rough)
     assert np.array_equal(ox == 0, rx == 0) and np.array_equal(orot == 0, rrot == 0)
-    assert _close(ox, rx) and _close(orot, rrot)
+    assert close_sweep(ox, rx) and close_sweep(orot, rrot)
     fo.verify_roughness = 0
     nx, _ = oracle.footprint_polygon(og, fo, poly, 0.5, *lay)
     assert (rx == 0).sum() >= (nx == 0).sum()                           # the extra predicate can only block more
@@ -301,7 +286,7 @@ def test_footprint_entries_take_circular_buffer_maps(te, ctx, oracle):
     ref, refw = np.empty_like(lay[0]), np.empty_like(lay[0])
     ctx.footprint(g0, fp, *lay, ref, te.MEM_HOST)
     ctx.footprint(gw, fp, *wl, refw, te.MEM_HOST)
-    assert _same(ref, np.roll(refw, (-sr, -sc), axis=(0, 1)))
+    assert same_values(ref, np.roll(refw, (-sr, -sc), axis=(0, 1)))
     px, pr, pxw, prw = (np.empty_like(lay[0]) for _ in range(4))
     ctx.footprint_polygon(g0, fp, poly, 0.7854, *lay, px, pr, te.MEM_HOST)
     ctx.footprint_polygon(gw, fp, poly, 0.7854, *wl, pxw, prw, te.MEM_HOST)

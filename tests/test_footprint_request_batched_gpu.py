@@ -5,8 +5,8 @@ import numpy as np
 import pytest
 
 import paths_oracle as po
-import synth
-from helpers import YAML, footprint_arrays, mixed_request, request_footprints, same, same_polygons
+from helpers import (YAML, assert_same_answers, batch_request, footprint_arrays, request_footprints, subset, te_footprint_params, walled_batch,
+                     walled_terrain)
 
 pytestmark = pytest.mark.gpu
 
@@ -16,77 +16,21 @@ CAP = 64
 LAYERS = ("traversability", "slope", "step", "roughness", "elevation", "robot_slope")
 
 
-def _terrain(rows, cols, res, kind, seed):
-    """Neighbouring maps of a batch differ sharply: a flat map, a map walled along its first rows and columns, a terrain map, a map
-    walled along its last rows and columns.  A value read across a map boundary would change the paths along that boundary."""
-    if kind == 0:
-        return np.zeros((rows, cols), dtype=np.float32)
-    z = synth.terrain(rows, cols, res, seed, "mixed")
-    if kind == 1:
-        z[:5, :] += np.float32(1.0)
-        z[:, :5] += np.float32(1.0)
-    if kind == 3:
-        z[-5:, :] += np.float32(1.0)
-        z[:, -5:] += np.float32(1.0)
-    return z
-
-
-def _batch(oracle, rows, cols, res, n, seed):
-    """Chain layers of n maps on the CPU oracle, stacked as (n, cols, rows): map k's layers are the column-major batch[k].T.  Also a
-    robot_slope layer per map (its slope with zeros and NaNs)."""
-    og = oracle.Geometry.make(rows, cols, res)
-    out = {k: [] for k in LAYERS}
-    rng = np.random.default_rng(seed)
-    for k in range(n):
-        z = _terrain(rows, cols, res, k % 4, seed + k)
-        ch = oracle.chain(og, oracle.ChainParams.yaml_defaults(0), z)
-        slope, rough = np.array(ch["slope"], dtype=np.float32), np.array(ch["roughness"], dtype=np.float32)
-        for _ in range(3 if k % 4 else 0):
-            # zero patches: checkForRoughness blocks them when verify_roughness is set, checkForSlope with a small max_gap_width
-            a, b = int(rng.integers(0, rows - 10)), int(rng.integers(0, cols - 10))
-            rough[a:a + 9, b:b + 9] = 0.0
-            a, b = int(rng.integers(0, rows - 10)), int(rng.integers(0, cols - 10))
-            slope[a:a + 9, b:b + 9] = 0.0
-        rs = np.array(ch["slope"], dtype=np.float32)
-        rs[rng.random(rs.shape) < 0.002] = 0.0
-        rs[rng.random(rs.shape) < 0.05] = np.nan
-        for name, layer in zip(LAYERS, (ch["traversability"], slope, ch["step"], rough, z, rs)):
-            out[name].append(np.ascontiguousarray(np.asarray(layer, dtype=np.float32).T))
-    return {k: np.stack(v) for k, v in out.items()}
-
-
 def _one(B, k):
     """Map k's layers, column-major (rows, cols)."""
     return {x: np.asfortranarray(B[x][k].T) for x in LAYERS}
 
 
-def _subset(R, idx):
-    """The request of the paths `idx` of R, in that order."""
-    b = R["begin"]
-    begin = np.concatenate([[0], np.cumsum(b[idx + 1] - b[idx])]).astype(np.int32)
-    poses = np.concatenate([R["poses"][b[q]:b[q + 1]] for q in idx]) if len(idx) else np.zeros((0, 7))
-    return dict(begin=begin, poses=poses, **{k: R[k][idx] for k in ("radius", "kind", "cons", "cup")})
-
-
 def _request(rng, og, fps, npaths):
     """A mixed request on maps of geometry og, with a path_map that interleaves the maps in no order and leaves map EMPTY out.
     Every sixth path starts at a map corner or edge midpoint, one cell inside: its spirals and hulls reach past the map."""
-    R = mixed_request(rng, og, npaths, fps)
+    R = batch_request(rng, og, npaths, NMAPS, fps, exclude=EMPTY)   # every other map has paths
     lx, ly = og.rows * og.resolution, og.cols * og.resolution
     edges = [(sx * 0.49 * lx, sy * 0.49 * ly) for sx, sy in ((1, 1), (1, -1), (-1, 1), (-1, -1), (1, 0), (-1, 0), (0, 1), (0, -1))]
     for j, q in enumerate(range(2, npaths, 6)):
         if R["begin"][q + 1] > R["begin"][q]:
             R["poses"][R["begin"][q], :2] = edges[j % len(edges)]
-    maps = [m for m in range(NMAPS) if m != EMPTY]
-    R["map"] = np.asarray([maps[int(v)] for v in rng.integers(0, len(maps), len(R["kind"]))], np.int32)
-    R["map"][:len(maps)] = rng.permutation(maps)   # every other map has paths
     return R
-
-
-def _fp(te, verify=0):
-    p = te.FootprintParams.yaml_defaults()
-    p.verify_roughness = verify
-    return p
 
 
 def _batched(ctx, g, ft, B, R, fps, slope, cap, nmaps=NMAPS, memory=0, path_map=None, **kw):
@@ -113,21 +57,15 @@ def _map_by_map(ctx, g, ft, B, R, fps, slope, cap):
     for k in range(NMAPS):
         idx = np.nonzero(R["map"] == k)[0]
         if len(idx):
-            got = _single(ctx, g, ft, _one(B, k), _subset(R, idx), fps, slope, cap)
+            got = _single(ctx, g, ft, _one(B, k), subset(R, idx), fps, slope, cap)
             for o, v in zip(out, got):
                 o[idx] = v
     return tuple(out)
 
 
-def _assert_equal(got, want, what):
-    assert np.array_equal(got[0], want[0]), (what, np.nonzero(got[0] != want[0])[0][:10])
-    assert same(got[1], want[1]) and same(got[2], want[2]), what
-    same_polygons(got[3], got[4], want[3], want[4], what)
-
-
 @pytest.fixture(scope="module")
 def batch(oracle):
-    return _batch(oracle, ROWS, COLS, RES, NMAPS, 500)
+    return walled_batch(oracle, ROWS, COLS, RES, NMAPS, 500, robot_slope=True)
 
 
 @pytest.fixture(scope="module")
@@ -141,10 +79,10 @@ def request_(oracle):
 @pytest.mark.parametrize("slope", [False, True], ids=["no_robot_slope", "robot_slope"])
 def test_batch_equals_map_by_map(te, ctx, batch, request_, verify, slope):
     R, fps = request_
-    g, ft = te.Geometry.make(ROWS, COLS, RES), _fp(te, verify)
+    g, ft = te.Geometry.make(ROWS, COLS, RES), te_footprint_params(te, verify_roughness=verify)
     got = _batched(ctx, g, ft, batch, R, fps, slope, CAP)
     want = _map_by_map(ctx, g, ft, batch, R, fps, slope, CAP)
-    _assert_equal(got, want, (verify, slope))
+    assert_same_answers(got, want, (verify, slope))
     assert (R["kind"] < 0).sum() > 60 and (R["kind"] >= 0).sum() > 60
     assert not (R["map"] == EMPTY).any() and len(set(R["map"].tolist())) == NMAPS - 1
     assert want[0].any() and not want[0].all() and (want[3] > 0).any()
@@ -156,17 +94,17 @@ def test_batch_matches_the_cpu_oracle(te, ctx, oracle, batch, request_):
     R, fps = request_
     g, og = te.Geometry.make(ROWS, COLS, RES), oracle.Geometry.make(ROWS, COLS, RES)
     for verify in (0, 1):
-        ft = _fp(te, verify)
+        ft = te_footprint_params(te, verify_roughness=verify)
         fo = oracle.FootprintParams.yaml_defaults()
         fo.verify_roughness = verify
         got = _batched(ctx, g, ft, batch, R, fps, True, CAP)
         for k in (1, 2):
             idx = np.nonzero(R["map"] == k)[0]
-            S = _subset(R, idx)
+            S = subset(R, idx)
             fb, fx = footprint_arrays(S, fps)
             want = po.check_request(og, fo, _one(batch, k), S["begin"], S["poses"], S["radius"], footprint_begin=fb, footprint_xyz=fx,
                                     conservative=S["cons"], cup=S["cup"], capacity=CAP)
-            _assert_equal(tuple(a[idx] for a in got), want, ("oracle", verify, k))
+            assert_same_answers(tuple(a[idx] for a in got), want, ("oracle", verify, k))
             assert want[0].any() and not want[0].all()
 
 
@@ -195,8 +133,8 @@ def test_each_map_has_its_own_memo(te, ctx):
         got = _batched(ctx, g, ft, B, R, fps, False, CAP, nmaps=2)
         for k in (0, 1):
             idx = np.nonzero(R["map"] == k)[0]
-            want = _single(ctx, g, ft, _one(B, k), _subset(R, idx), fps, False, CAP)
-            _assert_equal(tuple(a[idx] for a in got), want, (order, k))
+            want = _single(ctx, g, ft, _one(B, k), subset(R, idx), fps, False, CAP)
+            assert_same_answers(tuple(a[idx] for a in got), want, (order, k))
             assert (want[0] == (1 if k == 1 else 0)).all(), (order, k, want[0])
 
 
@@ -235,7 +173,7 @@ def test_device_memory_on_a_torch_stream(te, batch, request_):
     """TE_MEM_DEVICE equals TE_MEM_HOST; a path on a map outside the batch gets 0 / NaN / NaN / -1 and changes no other path."""
     import torch
     R, fps = request_
-    g, ft = te.Geometry.make(ROWS, COLS, RES), _fp(te, 1)
+    g, ft = te.Geometry.make(ROWS, COLS, RES), te_footprint_params(te, verify_roughness=1)
     ctx = te.Context(0)
     try:
         want = _batched(ctx, g, ft, batch, R, fps, True, CAP)
@@ -251,23 +189,23 @@ def test_device_memory_on_a_torch_stream(te, batch, request_):
             got = _run_device(ctx, g, ft, Bd, _request_device(R, fps), NMAPS, True)
             marked = _run_device(ctx, g, ft, Bd, _request_device(Rb, fps), NMAPS, True)
         ctx.set_stream(None)
-        _assert_equal(got, want, "device")
+        assert_same_answers(got, want, "device")
         assert (marked[0][bad] == 0).all() and np.isnan(marked[1][bad]).all() and np.isnan(marked[2][bad]).all()
         assert (marked[3][bad] == -1).all()
         ok = np.ones(len(R["kind"]), bool)
         ok[bad] = False
-        _assert_equal(tuple(a[ok] for a in marked), tuple(a[ok] for a in want), "neighbours")
+        assert_same_answers(tuple(a[ok] for a in marked), tuple(a[ok] for a in want), "neighbours")
     finally:
         ctx.close()
 
 
 def test_a_batch_of_one(te, ctx, batch, request_):
     R, fps = request_
-    g, ft = te.Geometry.make(ROWS, COLS, RES), _fp(te, 1)
+    g, ft = te.Geometry.make(ROWS, COLS, RES), te_footprint_params(te, verify_roughness=1)
     R1 = dict(R, map=np.zeros(len(R["kind"]), np.int32))
     got = _batched(ctx, g, ft, {k: v[3:4] for k, v in batch.items()}, R1, fps, True, CAP, nmaps=1)
     want = _single(ctx, g, ft, _one(batch, 3), R, fps, True, CAP)
-    _assert_equal(got, want, "nmaps = 1")
+    assert_same_answers(got, want, "nmaps = 1")
 
 
 def test_batched_chain_then_batched_request(te, ctx, request_):
@@ -276,8 +214,8 @@ def test_batched_chain_then_batched_request(te, ctx, request_):
     import torch
     R, fps = request_
     n = NMAPS
-    g, cp, ft = te.Geometry.make(ROWS, COLS, RES), te.ChainParams.yaml_defaults(0), _fp(te)
-    z = torch.from_numpy(np.stack([np.ascontiguousarray(_terrain(ROWS, COLS, RES, k % 4, 900 + k).T) for k in range(n)])).cuda()
+    g, cp, ft = te.Geometry.make(ROWS, COLS, RES), te.ChainParams.yaml_defaults(0), te_footprint_params(te)
+    z = torch.from_numpy(np.stack([np.ascontiguousarray(walled_terrain(ROWS, COLS, RES, k % 4, 900 + k).T) for k in range(n)])).cuda()
     ctx.set_stream(None)
     slope, step, rough, trav = (torch.empty((n, COLS, ROWS), dtype=torch.float32, device="cuda") for _ in range(4))
     ctx.chain_batched(g, cp, n, z, slope, step, rough, trav, te.MEM_DEVICE)
@@ -291,7 +229,7 @@ def test_batched_chain_then_batched_request(te, ctx, request_):
             continue
         one = [torch.empty((COLS, ROWS), dtype=torch.float32, device="cuda") for _ in range(4)]
         ctx.chain(g, cp, z[k], *one, te.MEM_DEVICE)
-        S = _subset(R, idx)
+        S = subset(R, idx)
         Ld = dict(traversability=one[3], slope=one[0], step=one[1], elevation=z[k], roughness=one[2], robot_slope=None)
         Dk = _request_device(dict(S, map=np.zeros(len(idx), np.int32)), fps)
         m = len(idx)
@@ -306,13 +244,13 @@ def test_batched_chain_then_batched_request(te, ctx, request_):
         torch.cuda.synchronize()
         for o, key in zip(want, ("is_safe", "traversability_out", "area_out", "untraversable_count", "untraversable_xy")):
             o[idx] = out[key].cpu().numpy()
-    _assert_equal(got, tuple(want), "pipeline")
+    assert_same_answers(got, tuple(want), "pipeline")
     assert want[0].any() and not want[0].all()
 
 
 def test_launch_count_does_not_depend_on_the_batch(te, ctx, batch, request_):
     R, fps = request_
-    g, ft = te.Geometry.make(ROWS, COLS, RES), _fp(te)
+    g, ft = te.Geometry.make(ROWS, COLS, RES), te_footprint_params(te)
     counts = []
     for nmaps in (1, NMAPS):
         Rn = dict(R, map=R["map"] % nmaps)
@@ -325,7 +263,7 @@ def test_launch_count_does_not_depend_on_the_batch(te, ctx, batch, request_):
 
 def test_error_codes(te, ctx, batch, request_):
     R, fps = request_
-    g, ft = te.Geometry.make(ROWS, COLS, RES), _fp(te)
+    g, ft = te.Geometry.make(ROWS, COLS, RES), te_footprint_params(te)
 
     def code(path_map=None, **kw):
         fb, fx = footprint_arrays(R, fps)

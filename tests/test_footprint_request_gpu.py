@@ -6,8 +6,8 @@ import pytest
 
 import paths_oracle as po
 import synth
-from helpers import (YAML, chain_layers, footprint_arrays, footprint_params, mixed_request, request_footprints, same,
-                     same_polygons)
+from helpers import (YAML, assert_same_answers, chain_layers, footprint_arrays, footprint_params, mixed_request, request_footprints,
+                     same_polygons, subset)
 
 pytestmark = pytest.mark.gpu
 
@@ -18,14 +18,6 @@ CASES = [
     dict(rows=190, cols=170, res=0.02, seed=43, position=(123.456, -78.9)),
     dict(rows=2048, cols=2048, res=0.02, seed=44),
 ]
-
-
-def _subset(R, idx):
-    """path_begin and poses of the paths `idx` of a request, in that order."""
-    b = R["begin"]
-    begin = np.concatenate([[0], np.cumsum(b[idx + 1] - b[idx])]).astype(np.int32)
-    poses = np.concatenate([R["poses"][b[q]:b[q + 1]] for q in idx]) if len(idx) else np.zeros((0, 7))
-    return begin, poses
 
 
 def _run(ctx, g, ft, L, R, fps, rs, cap, memory=0, **kw):
@@ -45,7 +37,8 @@ def _split(ctx, g, ft, L, R, fps, rs, cap):
     rough = L["roughness"] if ft.verify_roughness else None
     idx = np.nonzero(R["kind"] < 0)[0]
     if len(idx):
-        b, p = _subset(R, idx)
+        S = subset(R, idx)
+        b, p = S["begin"], S["poses"]
         got = ctx.check_footprint_paths_fresh(g, ft, L["traversability"], L["slope"], L["step"], L["elevation"], b, p[:, :2].copy(),
                                               R["radius"][idx], robot_slope=rs, roughness=rough,
                                               compute_untraversable_polygon=R["cup"][idx], untraversable_capacity=cap)
@@ -56,7 +49,8 @@ def _split(ctx, g, ft, L, R, fps, rs, cap):
         idx = np.nonzero(R["kind"] == k)[0]
         if not len(idx):
             continue
-        b, p = _subset(R, idx)
+        S = subset(R, idx)
+        b, p = S["begin"], S["poses"]
         got = ctx.check_footprint_paths_polygon(g, ft, L["traversability"], L["slope"], L["step"], L["elevation"], fxyz, b, p,
                                                 robot_slope=rs, roughness=rough, conservative=R["cons"][idx],
                                                 compute_untraversable_polygon=R["cup"][idx], untraversable_capacity=cap)
@@ -64,13 +58,6 @@ def _split(ctx, g, ft, L, R, fps, rs, cap):
         if cap is not None:
             counts[idx], xy[idx] = got[3], got[4]
     return (safe, trav, area) if cap is None else (safe, trav, area, counts, xy)
-
-
-def _assert_equal(got, want, what):
-    assert np.array_equal(got[0], want[0]), (what, np.nonzero(got[0] != want[0])[0][:10])
-    assert same(got[1], want[1]) and same(got[2], want[2]), what
-    if len(want) > 3:
-        same_polygons(got[3], got[4], want[3], want[4], what)
 
 
 def _to_device(R, fps, L, rs):
@@ -135,9 +122,9 @@ def test_mixed_requests_equal_the_split_calls(te, ctx, oracle, mixed_case):
                 what = (verify, slope_layer is None, cap)
                 want = _split(ctx, g, ft, L, R, fps, slope_layer, cap)
                 got = _run(ctx, g, ft, L, R, fps, slope_layer, cap)
-                _assert_equal(got, want, ("host",) + what)
+                assert_same_answers(got, want, ("host",) + what)
                 assert (got[2][kinds < 0] == 0).all()
-                _assert_equal(_run_device(ctx, g, ft, Ld, slope_dev, D, cap), want, ("device",) + what)
+                assert_same_answers(_run_device(ctx, g, ft, Ld, slope_dev, D, cap), want, ("device",) + what)
                 if cap is not None:
                     assert (got[3] > 0).any() and (got[3][R["cup"] == 0] == 0).all()
     assert want[0].any() and not want[0].all()
@@ -163,7 +150,7 @@ def test_request_matches_the_cpu_oracles(te, ctx, oracle):
                 want = _oracle(og, fo, L, R, fps, rs)
                 for cap in (None, CAP):
                     got = _run(ctx, g, ft, L, R, fps, rs, cap)
-                    _assert_equal(got, want if cap else want[:3], ("oracle", _case_id(case), verify, rs is None, cap))
+                    assert_same_answers(got, want if cap else want[:3], ("oracle", _case_id(case), verify, rs is None, cap))
                 assert want[0].any() and not want[0].all() and (want[3] > 0).any()
 
 
@@ -178,7 +165,7 @@ def test_degenerate_requests(te, ctx, oracle):
     for circular in (1.0, 0.0):   # all circular; all polygonal over one footprint
         R = mixed_request(rng, og, 150, fps[2:3], circular=circular, cap_path=False)
         for cap in (None, CAP):
-            _assert_equal(_run(ctx, g, ft, L, R, fps[2:3], rs, cap), _split(ctx, g, ft, L, R, fps[2:3], rs, cap), (circular, cap))
+            assert_same_answers(_run(ctx, g, ft, L, R, fps[2:3], rs, cap), _split(ctx, g, ft, L, R, fps[2:3], rs, cap), (circular, cap))
     empty = mixed_request(rng, og, 0, fps, cap_path=False)
     got = _run(ctx, g, ft, L, empty, fps, None, CAP)
     assert all(len(a) == 0 for a in got)
@@ -213,7 +200,7 @@ def test_device_mode_on_a_torch_stream(te, oracle):
         assert (got[0][marked] == 0).all() and np.isnan(got[1][marked]).all() and np.isnan(got[2][marked]).all()
         assert (got[3][marked] == -1).all()
         ok = ~marked
-        _assert_equal(tuple(a[ok] for a in got), tuple(a[ok] for a in want), "neighbours")
+        assert_same_answers(tuple(a[ok] for a in got), tuple(a[ok] for a in want), "neighbours")
     finally:
         ctx.close()
 

@@ -6,8 +6,8 @@ import math
 import numpy as np
 import pytest
 
-from test_footprint_batched_gpu import _close, _terrain   # the neighbour-contrast maps of a batch and the prefix-sum tolerance
 import synth
+from helpers import bits, close_sweep, te_footprint_params, walled_terrain
 
 pytestmark = pytest.mark.gpu
 
@@ -16,10 +16,6 @@ PENTAGON = [[0.5, 0.2], [0.1, -0.3], [-0.5, -0.2], [-0.4, 0.26], [0.0, 0.1]]
 # pi/2 and pi make the rectangle's edges axis-parallel again: long lists of uncertain offsets
 YAWS = [0.0, 0.7854, math.pi / 2, -0.3, math.pi, 5.0, 2 * math.pi + 0.1]
 LAYERS = ("traversability", "slope", "step", "elevation")
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, dtype=np.float32).view(np.int32)
 
 
 def _groups(tiles, nyaws, sms):
@@ -42,7 +38,7 @@ def _chain_batch(te, ctx, rows, cols, res, kinds, seed):
     import torch
     n = len(kinds)
     g = te.Geometry.make(rows, cols, res)
-    z = torch.from_numpy(np.stack([np.ascontiguousarray(_terrain(rows, cols, res, k, seed + i).T) for i, k in enumerate(kinds)])).cuda()
+    z = torch.from_numpy(np.stack([np.ascontiguousarray(walled_terrain(rows, cols, res, k, seed + i).T) for i, k in enumerate(kinds)])).cuda()
     slope, step, rough, trav = (torch.empty_like(z) for _ in range(4))
     ctx.set_stream(None)
     ctx.chain_batched(g, te.ChainParams.yaml_defaults(0), n, z, slope, step, rough, trav, te.MEM_DEVICE)
@@ -57,12 +53,6 @@ def _chain_batch(te, ctx, rows, cols, res, kinds, seed):
             a, b = int(rng.integers(0, cols - 10)), int(rng.integers(0, rows - 10))
             B["slope"][m, a:a + 9, b:b + 9] = 0.0
     return g, B
-
-
-def _fp(te, verify_roughness=0):
-    p = te.FootprintParams.yaml_defaults()
-    p.verify_roughness = verify_roughness
-    return p
 
 
 def _single(te, ctx, g, p, B, m, yaw, rough, poly=POLY):
@@ -100,7 +90,7 @@ def test_yaws_match_oracle(te, ctx, oracle, case):
         got = out[k, 0].T
         assert not np.isnan(got).any(), yaw
         assert np.array_equal(got == 0, ref == 0), (yaw, int(((got == 0) != (ref == 0)).sum()))
-        assert _close(got, ref), (yaw, int((got != ref).sum()), float(np.abs(got - ref).max()))
+        assert close_sweep(got, ref), (yaw, int((got != ref).sum()), float(np.abs(got - ref).max()))
     assert (out == 0).any() and (out > 0).any()
     assert not np.array_equal(out[0], out[1])
 
@@ -118,7 +108,7 @@ def test_yaws_equal_single_entry(te, ctx, big, memory, rough):
     layer also its traversability_x.  At this size the launcher splits the seven yaws into groups."""
     import torch
     g, B = big
-    p = _fp(te, 1 if rough else 0)
+    p = te_footprint_params(te, verify_roughness=1 if rough else 0)
     assert _groups(_tiles(512, 384, 1), len(YAWS), _sms()) > 1
     if memory == "host":
         out = _yaws_host(te, ctx, g, p, B, 1, YAWS, rough)
@@ -132,12 +122,12 @@ def test_yaws_equal_single_entry(te, ctx, big, memory, rough):
         out = od.cpu().numpy()
     for k, yaw in enumerate(YAWS):
         x, r = _single(te, ctx, g, p, B, 0, yaw, rough)
-        assert np.array_equal(_bits(out[k, 0]), _bits(r)), (memory, rough, yaw)
+        assert np.array_equal(bits(out[k, 0]), bits(r)), (memory, rough, yaw)
         if yaw == 0.0:
-            assert np.array_equal(_bits(out[k, 0]), _bits(x))
+            assert np.array_equal(bits(out[k, 0]), bits(x))
     assert (out == 0).any() and (out > 0).any()
     if rough:   # the zero-roughness patches block cells that are open without the check
-        plain = _yaws_host(te, ctx, g, _fp(te), B, 1, YAWS[:1], False)
+        plain = _yaws_host(te, ctx, g, te_footprint_params(te), B, 1, YAWS[:1], False)
         assert (out[0] == 0).sum() > (plain[0] == 0).sum()
 
 
@@ -145,14 +135,14 @@ def test_batch_of_maps(te, ctx):
     """nmaps = 5 neighbour-contrast maps, four yaws: layer (k, m) is te_footprint_polygon on map m alone."""
     g, B = _chain_batch(te, ctx, 100, 90, 0.02, [0, 1, 2, 3, 0], 500)
     yaws = [0.7854, 0.0, -2.0, math.pi]
-    p = _fp(te)
+    p = te_footprint_params(te)
     out = _yaws_host(te, ctx, g, p, B, 5, yaws, False)
     for m in range(5):
         for k, yaw in enumerate(yaws):
             x, r = _single(te, ctx, g, p, B, m, yaw, False)
-            assert np.array_equal(_bits(out[k, m]), _bits(r)), (m, yaw)
+            assert np.array_equal(bits(out[k, m]), bits(r)), (m, yaw)
             if yaw == 0.0:
-                assert np.array_equal(_bits(out[k, m]), _bits(x)), m
+                assert np.array_equal(bits(out[k, m]), bits(x)), m
     assert (out[:, 0] > 0).all() and (out[:, 1] == 0).any() and (out[:, 3] == 0).any()
 
 
@@ -164,12 +154,12 @@ def test_yaw_groups(te, ctx, big, nmaps):
     yaws = list(np.linspace(0.0, 2 * math.pi, 24, endpoint=False))
     ngroups = _groups(_tiles(512, 384, nmaps), len(yaws), _sms())
     assert (ngroups > 1) if nmaps == 1 else (ngroups == 1)
-    p = _fp(te)
+    p = te_footprint_params(te)
     out = _yaws_host(te, ctx, g, p, B, nmaps, yaws, False)
     for m in range(nmaps):
         for k in (0, 1, 7, 11, 23) if nmaps == 1 else (0, 5, 23):
             _, r = _single(te, ctx, g, p, B, m, yaws[k], False)
-            assert np.array_equal(_bits(out[k, m]), _bits(r)), (nmaps, m, k)
+            assert np.array_equal(bits(out[k, m]), bits(r)), (nmaps, m, k)
 
 
 def test_launch_count(te, ctx):
@@ -177,7 +167,7 @@ def test_launch_count(te, ctx):
     import torch
     g, B = _chain_batch(te, ctx, 100, 90, 0.02, [1, 2, 3, 0, 2], 700)
     D = {k: torch.from_numpy(v).cuda() for k, v in B.items()}
-    p = _fp(te)
+    p = te_footprint_params(te)
     ctx.set_stream(None)
     counts = {}
     for nmaps in (1, 5):
@@ -200,7 +190,7 @@ def test_argument_errors(te, ctx):
     import ctypes as C
     rows, cols = 40, 30
     g = te.Geometry.make(rows, cols, 0.02)
-    p = _fp(te)
+    p = te_footprint_params(te)
     rng = np.random.default_rng(5)
     lay = [rng.random((1, cols, rows), dtype=np.float32), np.ones((1, cols, rows), np.float32), np.ones((1, cols, rows), np.float32),
            np.zeros((1, cols, rows), np.float32)]
@@ -221,7 +211,7 @@ def test_argument_errors(te, ctx):
     gw = te.Geometry.make(rows, cols, 0.02)
     gw.start_row, gw.start_col = 3, 4
     assert call([0.5], g=gw)[0] == -4                               # a circular-buffer start index, even for one map and one yaw
-    pr = _fp(te, 1)
+    pr = te_footprint_params(te, verify_roughness=1)
     assert call([0.5], p=pr)[0] == -2                               # verify_roughness without the roughness layer
     L = ctx._L
     pts = np.ascontiguousarray(POLY, dtype=np.float64)

@@ -7,7 +7,8 @@ import math
 import numpy as np
 import pytest
 
-from test_footprint_yaws_gpu import (LAYERS, POLY, YAWS, _bits, _chain_batch, _fp, _groups, _sms, _tiles, _yaws_host,  # noqa: F401
+from helpers import bits, te_footprint_params
+from test_footprint_yaws_gpu import (LAYERS, POLY, YAWS, _chain_batch, _groups, _sms, _tiles, _yaws_host,  # noqa: F401
                                      big)
 
 pytestmark = pytest.mark.gpu
@@ -47,7 +48,7 @@ def test_reduce_equals_stack(te, ctx, big, memory, rough):
     """512 x 384 and the seven YAWS (split into yaw groups at this size), verify_roughness off and on, host and device memory."""
     import torch
     g, B = big
-    p = _fp(te, 1 if rough else 0)
+    p = te_footprint_params(te, verify_roughness=1 if rough else 0)
     assert _groups(_tiles(512, 384, 1), len(YAWS), _sms()) > 1
     want = _reduce(_yaws_host(te, ctx, g, p, B, 1, YAWS, rough))
     if memory == "host":
@@ -71,7 +72,7 @@ def test_batch_of_maps(te, ctx):
     """nmaps = 5 neighbour-contrast maps: map m's reductions are those of its stack."""
     g, B = _chain_batch(te, ctx, 100, 90, 0.02, [0, 1, 2, 3, 0], 500)
     yaws = [0.7854, 0.0, -2.0, math.pi]
-    p = _fp(te)
+    p = te_footprint_params(te)
     _same(_reduce_host(te, ctx, g, p, B, 5, yaws, False), _reduce(_yaws_host(te, ctx, g, p, B, 5, yaws, False)))
 
 
@@ -82,7 +83,7 @@ def test_yaw_groups(te, ctx, big, nmaps):
     yaws = list(np.linspace(0.0, 2 * math.pi, 24, endpoint=False))
     ngroups = _groups(_tiles(512, 384, nmaps), len(yaws), _sms())
     assert (ngroups > 1) if nmaps == 1 else (ngroups == 1)
-    p = _fp(te)
+    p = te_footprint_params(te)
     l0 = ctx.stats()[0]
     stack = _yaws_host(te, ctx, g, p, B, nmaps, yaws, False)
     l1 = ctx.stats()[0]
@@ -97,9 +98,9 @@ def test_ties(te, ctx, big):
     worst = best = 0 with best_yaw 0."""
     g, B = big
     yaws = [0.5, 0.0, 0.5, 0.0]
-    p = _fp(te)
+    p = te_footprint_params(te)
     stack = _yaws_host(te, ctx, g, p, B, 1, yaws, False)
-    assert np.array_equal(_bits(stack[0]), _bits(stack[2])) and np.array_equal(_bits(stack[1]), _bits(stack[3]))
+    assert np.array_equal(bits(stack[0]), bits(stack[2])) and np.array_equal(bits(stack[1]), bits(stack[3]))
     got = _reduce_host(te, ctx, g, p, B, 1, yaws, False)
     _same(got, _reduce(stack))
     worst, best, k = got
@@ -111,17 +112,17 @@ def test_ties(te, ctx, big):
 
 def test_one_yaw(te, ctx, big):
     g, B = big
-    p = _fp(te)
+    p = te_footprint_params(te)
     layer = _yaws_host(te, ctx, g, p, B, 1, [0.4], False)[0]
     worst, best, k = _reduce_host(te, ctx, g, p, B, 1, [0.4], False)
-    assert np.array_equal(_bits(worst), _bits(layer)) and np.array_equal(_bits(best), _bits(layer)) and (k == 0).all()
+    assert np.array_equal(bits(worst), bits(layer)) and np.array_equal(bits(best), bits(layer)) and (k == 0).all()
 
 
 @pytest.mark.parametrize("nmaps", [1, 5])
 def test_optional_outputs(te, ctx, big, nmaps):
     """Every non-empty subset of the outputs equals the full call, with and without a yaw-group split."""
     g, B = big
-    p = _fp(te)
+    p = te_footprint_params(te)
     full = _reduce_host(te, ctx, g, p, B, nmaps, YAWS, False)
     for want in [(w, b, k) for w in (True, False) for b in (True, False) for k in (True, False) if w or b or k]:
         got = _reduce_host(te, ctx, g, p, B, nmaps, YAWS, False, want)
@@ -135,7 +136,7 @@ def test_1024_yaws(te, ctx):
     """The cap: 1024 yaws on a small map equal the reduction of the stack built in chunks of te_footprint_polygon_yaws calls."""
     g, B = _chain_batch(te, ctx, 100, 90, 0.02, [2], 900)
     yaws = list(np.linspace(-math.pi, math.pi, 1024, endpoint=False))
-    p = _fp(te)
+    p = te_footprint_params(te)
     stack = np.concatenate([_yaws_host(te, ctx, g, p, B, 1, yaws[a:a + 256], False) for a in range(0, 1024, 256)])
     worst, best, k = _reduce_host(te, ctx, g, p, B, 1, yaws, False)
     _same((worst, best, k), _reduce(stack))
@@ -150,7 +151,7 @@ def test_launch_count(te, ctx):
     assert _groups(_tiles(rows, cols, 1), 64, _sms()) == 1
     g, B = _chain_batch(te, ctx, rows, cols, 0.02, [1, 2, 3, 0, 2], 700)
     D = {k: torch.from_numpy(v).cuda() for k, v in B.items()}
-    p = _fp(te)
+    p = te_footprint_params(te)
     ctx.set_stream(None)
     counts, stacked = {}, set()
     for nmaps in (1, 5):
@@ -173,7 +174,7 @@ def test_launch_count(te, ctx):
 def test_argument_errors(te, ctx):
     rows, cols = 40, 30
     g = te.Geometry.make(rows, cols, 0.02)
-    p = _fp(te)
+    p = te_footprint_params(te)
     rng = np.random.default_rng(5)
     lay = [rng.random((1, cols, rows), dtype=np.float32), np.ones((1, cols, rows), np.float32), np.ones((1, cols, rows), np.float32),
            np.zeros((1, cols, rows), np.float32)]
@@ -194,10 +195,10 @@ def test_argument_errors(te, ctx):
     gw = te.Geometry.make(rows, cols, 0.02)
     gw.start_row, gw.start_col = 3, 4
     assert call([0.5], g=gw) == -4                                  # a circular-buffer start index
-    assert call([0.5], p=_fp(te, 1)) == -2                          # verify_roughness without the roughness layer
+    assert call([0.5], p=te_footprint_params(te, verify_roughness=1)) == -2                          # verify_roughness without the roughness layer
     assert call([0.5], want=(False, False, False)) == -1            # no output
     for bad in (float("nan"), float("inf"), -float("inf")):         # a non-finite traversability_default
-        pd = _fp(te)
+        pd = te_footprint_params(te)
         pd.traversability_default = bad
         assert call([0.5], p=pd) == -1
     L = ctx._L
@@ -221,7 +222,7 @@ def test_map_entries(te, ctx):
     g, B = _chain_batch(te, ctx, rows, cols, 0.02, [2], 1100)
     L = {k: np.asfortranarray(v[0].T) for k, v in B.items()}   # (rows, cols) unwrapped
     yaws = [0.3, math.pi / 2, -1.0, 0.0, 2.5]
-    p = _fp(te, 1)
+    p = te_footprint_params(te, verify_roughness=1)
     stack = _yaws_host(te, ctx, g, p, B, 1, yaws, True)[:, 0]  # (nyaws, cols, rows)
     want = _reduce(stack)
     sr, sc = 3, 4
@@ -235,12 +236,12 @@ def test_map_entries(te, ctx):
     # unwrapped map
     s = m.footprint_polygon_yaws(p, POLY, yaws)
     assert s.shape == (len(yaws), rows, cols)
-    assert np.array_equal(_bits(s), _bits(stack.transpose(0, 2, 1)))
+    assert np.array_equal(bits(s), bits(stack.transpose(0, 2, 1)))
     _same(m.footprint_polygon_yaws_reduce(p, POLY, yaws), tuple(w.T for w in want))
     # start index (3, 4), host memory: every layer re-wrapped
     sw = mw.footprint_polygon_yaws(p, POLY, yaws)
     for k in range(len(yaws)):
-        assert np.array_equal(_bits(sw[k]), _bits(wrap(stack[k].T))), k
+        assert np.array_equal(bits(sw[k]), bits(wrap(stack[k].T))), k
     _same(mw.footprint_polygon_yaws_reduce(p, POLY, yaws), tuple(wrap(w.T) for w in want))
     # the same map in device memory: default order
     ctx.set_stream(None)
@@ -255,7 +256,7 @@ def test_map_entries(te, ctx):
     assert Lb.te_map_footprint_polygon_yaws_reduce(mw._h, C.byref(p), len(pts), pts.ctypes.data, len(ys), ys.ctypes.data,
                                                    *(t.data_ptr() for t in rd), te.MEM_DEVICE) == 0
     ctx.synchronize()
-    assert np.array_equal(_bits(od.cpu().numpy()), _bits(stack))
+    assert np.array_equal(bits(od.cpu().numpy()), bits(stack))
     _same(tuple(t.cpu().numpy() for t in rd), want)
     # the cache is unchanged by all of them
     assert np.array_equal(mw.get_footprint().view(np.uint32), fp0.view(np.uint32))

@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 
 import image_oracle as io
-from helpers import footprint_arrays, mixed_request, request_footprints
+from helpers import bits, mixed_request, request_footprints, same_bits_or_nan, same_bytes
+from map_helpers import ask, close_maps  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -18,31 +19,6 @@ CHAIN = ("traversability", "traversability_slope", "traversability_step", "trave
 # inverted, equal, negative, a difference that rounds in float32, and one that overflows to inf (pixel 0 then gives NaN)
 PAIRS = [(0.0, 1.0), (2.0, -1.5), (0.25, 0.25), (-7.5, -0.3), (-1e7, 0.1), (1.0, 1e-8), (-3e38, 3e38)]
 SHAPES = [(1, 1), (1, 300), (300, 1), (37, 1000), (1000, 37), (513, 511)]
-CAP = 64
-
-
-@pytest.fixture(autouse=True)
-def _close_maps(ctx, monkeypatch):
-    made, real = [], ctx.map
-
-    def tracked():
-        made.append(real())
-        return made[-1]
-
-    monkeypatch.setattr(ctx, "map", tracked)
-    yield
-    for m in made:
-        m.close()
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
-
-
-def _same(a, b):
-    """float32 bit for bit; NaN matches NaN (the GPU's NaN bits differ from x86's)."""
-    a, b = np.asarray(a, np.float32), np.asarray(b, np.float32)
-    return a.shape == b.shape and bool(np.all((_bits(a) == _bits(b)) | (np.isnan(a) & np.isnan(b))))
 
 
 class Images:
@@ -126,7 +102,7 @@ def test_elevation_bits(te, ctx, dtype, shape, nmaps, memory):
     for k, im in enumerate(_layouts(pix)):
         for lo, hi in PAIRS[k::2] + [PAIRS[-1]]:
             assert _chain_image(te, m, g, p, im, lo, hi, memory) == 0, te.load_library().te_last_error()
-            assert _same(_elevation(m), io.elevation(pix, lo, hi)), (k, lo, hi)
+            assert same_bits_or_nan(_elevation(m), io.elevation(pix, lo, hi)), (k, lo, hi)
 
 
 @pytest.mark.parametrize("memory", [0, 1], ids=["host", "device"])
@@ -139,18 +115,12 @@ def test_every_pixel_value(te, ctx, memory):
         m = ctx.map()
         for lo, hi in PAIRS:
             assert _chain_image(te, m, g, p, Images(pix), lo, hi, memory) == 0
-            assert _same(_elevation(m), io.elevation(pix, lo, hi)), (pix.dtype, lo, hi)
+            assert same_bits_or_nan(_elevation(m), io.elevation(pix, lo, hi)), (pix.dtype, lo, hi)
 
 
 def _held(m):
     h = dict(m.get_layers(CHAIN), cache=m.get_footprint())
     return h if m.nmaps > 1 else {k: v[None] for k, v in h.items()}
-
-
-def _ask(m, ft, R, fps):
-    fb, fx = footprint_arrays(R, fps)
-    return m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, max_footprint_vertices=16, conservative=R["cons"],
-                                     compute_untraversable_polygon=R["cup"], untraversable_capacity=CAP)
 
 
 @pytest.mark.parametrize("memory", [0, 1], ids=["host", "device"])
@@ -180,21 +150,21 @@ def test_chain_layers_equal_float_chain(te, ctx, oracle, nmaps, memory):
     for o, k in zip(outs, ("slope", "step", "roughness", "traversability")):
         got = o if isinstance(o, np.ndarray) else o.cpu().numpy()
         want = np.asarray(ref[k]).reshape(nmaps, rows, cols).transpose(0, 2, 1).reshape(-1)  # per map column-major
-        assert _same(got, want), k
+        assert same_bits_or_nan(got, want), k
     ha, hb = _held(a), _held(b)
     for k in hb:
-        assert _same(ha[k], hb[k]), k
+        assert same_bits_or_nan(ha[k], hb[k]), k
     assert np.isnan(ha["cache"]).all()
     with pytest.raises(te.TEError):  # no robot_slope afterwards
         a.get_layers(["robot_slope"])
     if nmaps == 1:
         fps = request_footprints(rng)
-        R = mixed_request(rng, oracle.Geometry.make(rows, cols, res), 60, fps)
+        R = dict(mixed_request(rng, oracle.Geometry.make(rows, cols, res), 60, fps), fps=fps)
         ft = te.FootprintParams.yaml_defaults()
-        ga, gb = _ask(a, ft, R, fps), _ask(b, ft, R, fps)
+        ga, gb = ask(a, ft, R), ask(b, ft, R)
         for x, y in zip(ga, gb):
-            assert np.array_equal(np.asarray(x).view(np.uint8), np.asarray(y).view(np.uint8))
-        assert _same(a.get_footprint(), b.get_footprint())
+            assert same_bytes(x, y)
+        assert same_bits_or_nan(a.get_footprint(), b.get_footprint())
 
 
 @pytest.mark.parametrize("memory", [0, 1], ids=["host", "device"])
@@ -218,14 +188,14 @@ def test_selected_maps_only(te, ctx, memory):
     ref = b.chain_maps(g, p, sel, io.elevation(pix, -0.1, 0.5), outputs=True)
     ha, hb = _held(a), _held(b)
     for k in hb:
-        assert _same(ha[k], hb[k]), k
+        assert same_bits_or_nan(ha[k], hb[k]), k
         for j in range(n):
             if j not in sel:
-                assert _same(ha[k][j], before[k][j]), (k, j)
+                assert same_bits_or_nan(ha[k][j], before[k][j]), (k, j)
     assert np.isnan(ha["cache"][sel]).all()
     if outs is not None:
         for o, k in zip(outs, ("slope", "step", "roughness", "traversability")):
-            assert _same(o, ref[k].transpose(0, 2, 1).reshape(-1)), k
+            assert same_bits_or_nan(o, ref[k].transpose(0, 2, 1).reshape(-1)), k
 
 
 def test_python_views(te, ctx):
@@ -238,13 +208,13 @@ def test_python_views(te, ctx):
     m = ctx.map()
     out = m.chain_image(g, p, view, 0.1, 2.0, outputs=True)
     assert m.nmaps == 3 and out["slope"].shape == (3, 64, 76)
-    assert _same(m.get_layers(["elevation"])["elevation"], io.elevation(np.ascontiguousarray(view), 0.1, 2.0))
+    assert same_bits_or_nan(m.get_layers(["elevation"])["elevation"], io.elevation(np.ascontiguousarray(view), 0.1, 2.0))
     m.chain_image(g, p, view[1].astype(">u2"), 0.1, 2.0)
-    assert m.nmaps == 1 and _same(m.get_layers(["elevation"])["elevation"], io.elevation(np.ascontiguousarray(view[1]), 0.1, 2.0))
+    assert m.nmaps == 1 and same_bits_or_nan(m.get_layers(["elevation"])["elevation"], io.elevation(np.ascontiguousarray(view[1]), 0.1, 2.0))
     m2 = ctx.map()
     m2.chain_image(g, p, np.zeros((3, 64, 76), np.uint16), 0.0, 1.0)
     m2.chain_image_maps(g, p, [2], view[1:2], 0.1, 2.0)
-    assert _same(m2.get_layers(["elevation"])["elevation"][2], io.elevation(np.ascontiguousarray(view[1]), 0.1, 2.0))
+    assert same_bits_or_nan(m2.get_layers(["elevation"])["elevation"][2], io.elevation(np.ascontiguousarray(view[1]), 0.1, 2.0))
 
 
 def test_errors_leave_the_map_unchanged(te, ctx):
@@ -302,7 +272,7 @@ def test_errors_leave_the_map_unchanged(te, ctx):
                                      0.0, 1.0, None, None, None, None, te.MEM_HOST) == BAD_ARG
     after = _held(m)
     for k in before:
-        assert np.array_equal(_bits(after[k]), _bits(before[k])), k
+        assert np.array_equal(bits(after[k]), bits(before[k])), k
 
 
 def test_launches(te, ctx):

@@ -6,7 +6,8 @@ import pytest
 
 import at_poses_oracle as so
 import synth
-from helpers import footprint_arrays, mixed_request, quaternion, request_footprints
+from helpers import assert_same_bits, bits, footprint_arrays, mixed_request, quaternion, request_footprints
+from map_helpers import all_layer_names, close_maps  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -14,28 +15,6 @@ ROWS, COLS, RES, POS = 640, 512, 0.04, (1.3, -0.7)
 POLY = [[0.45, 0.30], [0.45, -0.30], [-0.45, -0.30], [-0.45, 0.30]]   # robot_footprint_parameter.yaml:3
 BAD_ARG, MISSING_LAYER, UNSUPPORTED = -1, -2, -4
 NAN_BITS = 0x7fc00000
-
-
-@pytest.fixture(autouse=True)
-def _close_maps(ctx, monkeypatch):
-    """Every te_map a test opens is destroyed when it ends, failed or not, while the context still exists."""
-    made, real = [], ctx.map
-    monkeypatch.setattr(ctx, "map", lambda: made.append(real()) or made[-1])
-    yield
-    for m in made:
-        m.close()
-
-
-def _bits(a):
-    return np.ascontiguousarray(np.asarray(a, dtype=np.float32)).view(np.uint32)
-
-
-def _same(a, b, what=""):
-    assert np.array_equal(_bits(a), _bits(b)), (what, int((_bits(a) != _bits(b)).sum()))
-
-
-def _all_names(te):
-    return list(te.capi.LAYERS) + list(te.capi.CARRIED_LAYERS) + [te.capi.UNCERTAINTY_RANGE] + list(te.capi.POLYGON_LAYERS)
 
 
 def _carried(rng, rows, cols):
@@ -129,7 +108,7 @@ def test_every_layer_against_the_oracle(te, ctx, oracle):
     torch = pytest.importorskip("torch")
     m = _full_map(te, ctx)
     g = te.Geometry.make(ROWS, COLS, RES, POS)
-    names = _all_names(te)
+    names = all_layer_names(te)
     L = m.get_layers(names)
     cache = L["traversability_footprint"]
     assert np.isfinite(cache).any() and np.isnan(cache).any()          # a cache the request filled in part
@@ -141,27 +120,27 @@ def test_every_layer_against_the_oracle(te, ctx, oracle):
     og = _oracle_geo(oracle, g)
     for n in names:
         want, wv = so.at_poses(og, L[n], poses, pts)
-        _same(got[n], want, n)
+        assert_same_bits(got[n], want, n)
         assert np.array_equal(valid, wv), n
     assert 0.5 < valid.mean() < 0.99
-    assert (_bits(got["traversability"])[valid == 0] == NAN_BITS).all()
+    assert (bits(got["traversability"])[valid == 0] == NAN_BITS).all()
     dev, dvalid = _at_device(torch, m, names, poses, pts)
     for n in names:
-        _same(dev[n], got[n], n)
+        assert_same_bits(dev[n], got[n], n)
     assert np.array_equal(dvalid, valid)
 
 
 # ---- 2. a start index changes nothing --------------------------------------------------------------------------------------
 
 def test_start_index_gives_identical_outputs(te, ctx):
-    names = _all_names(te)
+    names = all_layer_names(te)
     rng = np.random.default_rng(2)
     poses = _poses(rng, 600, POS, (0.5 * ROWS * RES, 0.5 * COLS * RES))
     pts = _pattern()
     a, va = _full_map(te, ctx).at_poses(poses, pts, names)
     b, vb = _full_map(te, ctx, start=(211, 97)).at_poses(poses, pts, names)
     for n in names:
-        _same(b[n], a[n], n)
+        assert_same_bits(b[n], a[n], n)
     assert np.array_equal(va, vb)
 
 
@@ -183,8 +162,8 @@ def test_single_point_is_at_position(te, ctx, oracle):
     L = m.get_layers(["traversability", "elevation"])
     k = valid[:, 0] == 1
     i, j = idx[k, 0].astype(np.int64) % ROWS, idx[k, 0].astype(np.int64) // ROWS
-    _same(got["traversability"][k, 0], L["traversability"][i, j])
-    _same(got["elevation"][k, 0], L["elevation"][i, j])
+    assert_same_bits(got["traversability"][k, 0], L["traversability"][i, j])
+    assert_same_bits(got["elevation"][k, 0], L["elevation"][i, j])
 
 
 # ---- 4. a batch at several positions ---------------------------------------------------------------------------------------
@@ -219,8 +198,8 @@ def test_batch_at_positions(te, ctx):
         assert np.array_equal(valid[sel], wv), k
         assert wv.any() and not wv.all()
         for nm in names:
-            _same(got[nm][sel], want[nm], (k, nm))
-            _same(dev[nm][sel], want[nm], (k, nm))
+            assert_same_bits(got[nm][sel], want[nm], (k, nm))
+            assert_same_bits(dev[nm][sel], want[nm], (k, nm))
 
 
 # ---- 5. uncertainty_range --------------------------------------------------------------------------------------------------
@@ -233,9 +212,9 @@ def test_uncertainty_range_is_numpy_subtraction(te, ctx):
     k = valid == 1
     with np.errstate(invalid="ignore"):                                # Inf - Inf
         want = np.subtract(got["upper_bound"][k], got["lower_bound"][k])
-    _same(got["uncertainty_range"][k], want)
-    assert np.isnan(want).sum() > 100 and len(set(_bits(want)[np.isnan(want)].tolist())) > 3   # NaN payloads of both kinds
-    assert (_bits(got["uncertainty_range"])[~k] == NAN_BITS).all()
+    assert_same_bits(got["uncertainty_range"][k], want)
+    assert np.isnan(want).sum() > 100 and len(set(bits(want)[np.isnan(want)].tolist())) > 3   # NaN payloads of both kinds
+    assert (bits(got["uncertainty_range"])[~k] == NAN_BITS).all()
 
 
 # ---- 6. invalid points -----------------------------------------------------------------------------------------------------
@@ -253,12 +232,12 @@ def test_invalid_points(te, ctx):
     dev, dvalid = _at_device(torch, b, ["traversability", "elevation"], poses, pts, pose_map)
     assert dvalid[:7].sum() == 2 and dvalid[6].all() and dvalid[7].all()    # maps outside the batch, off-map, non-finite
     for n in dev:
-        assert (_bits(dev[n])[dvalid == 0] == NAN_BITS).all() and np.isfinite(dev[n][6]).all()
+        assert (bits(dev[n])[dvalid == 0] == NAN_BITS).all() and np.isfinite(dev[n][6]).all()
     # host memory: the same points on the maps inside the batch
     got, valid = b.at_poses(poses[3:], pts, ["traversability", "elevation"], pose_map=pose_map[3:])
     assert np.array_equal(valid, dvalid[3:])
     for n in got:
-        _same(got[n], dev[n][3:])
+        assert_same_bits(got[n], dev[n][3:])
 
 
 # ---- 7. errors -------------------------------------------------------------------------------------------------------------
@@ -315,7 +294,7 @@ def test_one_launch_per_call(te, ctx):
     m = _full_map(te, ctx)
     rng = np.random.default_rng(8)
     poses, pts = _poses(rng, 500, POS, (0.5 * ROWS * RES, 0.5 * COLS * RES)), _pattern()
-    names = _all_names(te)
+    names = all_layer_names(te)
     N = 64
     z = np.stack([synth.terrain(N, N, RES, 90 + k, "mixed") for k in range(3)]).astype(np.float32)
     b = ctx.map()
@@ -369,10 +348,10 @@ def test_graph_capture(te, oracle):
         replayed, rvalid = out.cpu().numpy().copy(), valid.cpu().numpy().copy()
         c.set_stream(None)
         fresh, fvalid = m.at_poses(new, pts, names)
-        _same(replayed, np.concatenate([fresh[n].reshape(-1) for n in names]))
+        assert_same_bits(replayed, np.concatenate([fresh[n].reshape(-1) for n in names]))
         assert np.array_equal(rvalid, fvalid.reshape(-1))
         want, _ = so.at_poses(_oracle_geo(oracle, g), m.get_layers(["traversability"])["traversability"], new, pts)
-        _same(fresh["traversability"], want)
+        assert_same_bits(fresh["traversability"], want)
         m.close()
     finally:
         c.close()

@@ -6,13 +6,13 @@ import pytest
 
 import paths_oracle as po
 import synth
-from helpers import chain_layers, footprint_arrays, mixed_request, request_footprints, same, same_polygons
+from helpers import batch_request, chain_layers, footprint_arrays, footprint_params, request_footprints, subset
+from map_helpers import assert_batch_matches_singles, assert_same_cache, close_maps  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 ROWS, COLS, RES, NMAPS = 200, 180, 0.02, 5
 EMPTY = 3    # the map without paths
-CAP = 64
 BAD_ARG, UNSUPPORTED = -1, -4
 FILTER = ("traversability", "slope", "step", "elevation")
 
@@ -30,29 +30,8 @@ def maps(te, oracle):
     return og, g, per
 
 
-@pytest.fixture(autouse=True)
-def _close_maps(ctx, monkeypatch):
-    """Every te_map a test opens is destroyed when it ends, failed or not, while the context still exists."""
-    made, real = [], ctx.map
-
-    def tracked():
-        made.append(real())
-        return made[-1]
-
-    monkeypatch.setattr(ctx, "map", tracked)
-    yield
-    for m in made:
-        m.close()
-
-
 def _stack(per, key):
     return np.stack([p[key] for p in per])
-
-
-def _params(te, oracle, verify=0):
-    ft, fo = te.FootprintParams.yaml_defaults(), oracle.FootprintParams.yaml_defaults()
-    ft.verify_roughness = fo.verify_roughness = verify
-    return ft, fo
 
 
 def _load(ctx, g, per, slope, rough=True):
@@ -69,67 +48,9 @@ def _load(ctx, g, per, slope, rough=True):
     return b, singles
 
 
-def _subset(R, idx):
-    """The request of the paths `idx` of R, in that order."""
-    b = R["begin"]
-    begin = np.concatenate([[0], np.cumsum(b[idx + 1] - b[idx])]).astype(np.int32)
-    poses = np.concatenate([R["poses"][b[q]:b[q + 1]] for q in idx]) if len(idx) else np.zeros((0, 7))
-    return dict(begin=begin, poses=poses, **{k: R[k][idx] for k in ("radius", "kind", "cons", "cup", "map")})
-
-
 def _request(rng, og, fps, npaths, planner=False):
     """A mixed request whose paths interleave the maps in no order and leave map EMPTY out."""
-    R = mixed_request(rng, og, npaths, fps, circular=0.6, planner=planner, cap_path=False)
-    maps = [m for m in range(NMAPS) if m != EMPTY]
-    R["map"] = np.asarray([maps[int(v)] for v in rng.integers(0, len(maps), len(R["kind"]))], np.int32)
-    R["map"][:len(maps)] = rng.permutation(maps)
-    return R
-
-
-def _ask(m, ft, R, fps, batched):
-    fb, fx = footprint_arrays(R, fps)
-    kw = dict(max_footprint_vertices=16, conservative=R["cons"], compute_untraversable_polygon=R["cup"], untraversable_capacity=CAP)
-    if batched:
-        return m.check_footprint_request_batched(ft, R["map"], R["begin"], R["poses"], R["radius"], fb, fx, **kw)
-    return m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, **kw)
-
-
-def _same_cache(a, b, what, nan_bits=True):
-    """Caches bit for bit; nan_bits=False lets any NaN match any NaN (the oracle's empty cell is not the library's NaN)."""
-    equal = (a.view(np.uint32) == b.view(np.uint32)) | (not nan_bits and (np.isnan(a) & np.isnan(b)))
-    assert equal.all(), (what, int(np.sum(~equal)))
-
-
-def _both(b, singles, ft, R, fps, oracle_state=None):
-    """One request on the batch and, map by map, its paths on the single maps; asserts the answers and every cache are identical.
-    oracle_state = (og, fo, per-map layers, per-map caches): each map's subsequence is also replayed on the CPU oracle."""
-    got = _ask(b, ft, R, fps, True)
-    n = len(R["kind"])
-    want = [np.zeros(n, np.uint8), np.zeros(n), np.zeros(n), np.zeros(n, np.int32), np.zeros((n, CAP, 2))]
-    for k, s in enumerate(singles):
-        idx = np.nonzero(R["map"] == k)[0]
-        if not len(idx):
-            continue
-        Rk = _subset(R, idx)
-        for o, v in zip(want, _ask(s, ft, Rk, fps, False)):
-            o[idx] = v
-        if oracle_state is not None:
-            og, fo, OL, caches = oracle_state
-            fb, fx = footprint_arrays(Rk, fps)
-            ref = po.check_request(og, fo, OL[k], Rk["begin"], Rk["poses"], Rk["radius"], fb, fx, conservative=Rk["cons"], cup=Rk["cup"],
-                                   cache=caches[k], capacity=CAP)
-            assert np.array_equal(got[0][idx], ref[0]) and same(got[1][idx], ref[1]) and same(got[2][idx], ref[2]), k
-            same_polygons(got[3][idx], got[4][idx], ref[3], ref[4], ("oracle polygons", k))
-    assert np.array_equal(got[0], want[0]), np.nonzero(got[0] != want[0])[0][:10]
-    assert same(got[1], want[1]) and same(got[2], want[2])
-    same_polygons(got[3], got[4], want[3], want[4], "polygons")
-    caches = b.get_footprint()
-    assert caches.shape == (NMAPS, ROWS, COLS)
-    for k, s in enumerate(singles):
-        _same_cache(caches[k], s.get_footprint(), ("cache", k))
-        if oracle_state is not None:
-            _same_cache(caches[k], oracle_state[3][k], ("oracle cache", k), nan_bits=False)
-    return got
+    return batch_request(rng, og, npaths, NMAPS, fps, exclude=EMPTY, circular=0.6, planner=planner, cap_path=False)
 
 
 def _close(*ms):
@@ -177,7 +98,7 @@ def test_chain_batched_layers_equal_stateless_batch(te, ctx, maps):
 @pytest.mark.parametrize("verify,slope,with_oracle", [(0, False, True), (1, True, False), (0, True, False)])
 def test_request_sequences_equal_single_maps(te, ctx, oracle, maps, verify, slope, with_oracle):
     og, g, per = maps
-    ft, fo = _params(te, oracle, verify)
+    ft, fo = footprint_params(te, oracle, verify)
     b, singles = _load(ctx, g, per, slope)
     state = None
     if with_oracle:
@@ -187,9 +108,9 @@ def test_request_sequences_equal_single_maps(te, ctx, oracle, maps, verify, slop
     fps = request_footprints(rng)
     R1 = _request(rng, og, fps, 90)
     R2 = _request(rng, og, fps, 80, planner=True)
-    again = _subset(R1, rng.permutation(len(R1["kind"])))   # revisits: every cell R1 stored, in another order
+    again = subset(R1, rng.permutation(len(R1["kind"])))   # revisits: every cell R1 stored, in another order
     for R in (R1, again, R2):
-        _both(b, singles, ft, R, fps, state)
+        assert_batch_matches_singles(b, singles, ft, R, state)
     cand, keys, stored = b.request_stats()
     assert 0 < stored <= keys <= cand
     assert np.isnan(b.get_footprint()[EMPTY]).all()
@@ -200,7 +121,7 @@ def test_same_cell_first_touched_on_two_maps(te, ctx, oracle, maps):
     """Single-pose circular paths at the same position on two maps whose circles differ: the keys must stay apart, so one map
     stores a traversable value and the other an untraversable one in the same request."""
     og, g, per = maps
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     rng = np.random.default_rng(5)
     n = 400
     cells = rng.choice(ROWS * COLS, n, replace=False)   # one pose per cell, so every check is a first touch
@@ -217,10 +138,10 @@ def test_same_cell_first_touched_on_two_maps(te, ctx, oracle, maps):
     differ = np.nonzero(safe[0] != safe[1])[0][:20]
     assert len(differ) >= 4
     idx = np.repeat(differ, 2)
-    R = _subset(dict(one, map=np.zeros(n, np.int32)), idx)
-    R["map"] = np.tile(np.array([0, 1], np.int32), len(differ))
+    R = subset(dict(one, map=np.zeros(n, np.int32)), idx)
+    R["map"], R["fps"] = np.tile(np.array([0, 1], np.int32), len(differ)), []
     b, singles = _load(ctx, g, per, False)
-    got = _both(b, singles, ft, R, [])
+    got = assert_batch_matches_singles(b, singles, ft, R)
     assert np.array_equal(got[0][0::2], safe[0][differ]) and np.array_equal(got[0][1::2], safe[1][differ])
     cache = b.get_footprint()
     stored = cache[:2, ci[differ], cj[differ]]
@@ -230,18 +151,18 @@ def test_same_cell_first_touched_on_two_maps(te, ctx, oracle, maps):
 
 def test_whole_map_entries_on_a_batch(te, ctx, oracle, maps):
     og, g, per = maps
-    ft, _ = _params(te, oracle, verify=1)
+    ft, _ = footprint_params(te, oracle, verify=1)
     b, singles = _load(ctx, g, per, True)
     rng = np.random.default_rng(41)
     fps = request_footprints(rng)
-    _both(b, singles, ft, _request(rng, og, fps, 60), fps)
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 60))
     before = b.get_footprint()
     swept = b.footprint(ft)
     for k, s in enumerate(singles):   # te_map_footprint keeps each map's cached cells, as on a single map
-        _same_cache(swept[k], s.footprint(ft), ("footprint", k))
+        assert_same_cache(swept[k], s.footprint(ft), ("footprint", k))
     had = np.isfinite(before)
     assert had.any() and np.array_equal(swept[had].view(np.uint32), before[had].view(np.uint32))
-    _same_cache(b.get_footprint(), swept, "cache after the sweep")
+    assert_same_cache(b.get_footprint(), swept, "cache after the sweep")
     # the polygon entries are the stateless batched ones on the resident layers
     pts = np.array([[0.3, 0.2], [-0.3, 0.2], [-0.3, -0.2], [0.3, -0.2]])
     yaws = [0.0, 0.4, 1.3, -2.0]
@@ -261,7 +182,7 @@ def test_whole_map_entries_on_a_batch(te, ctx, oracle, maps):
     ctx.footprint_polygon_batched(g, ft, NMAPS, pts, 0.7, *(lay[k] for k in FILTER), wx, wr, te.MEM_HOST, roughness=lay["roughness"])
     for a, w in zip(b.footprint_polygon(ft, pts, 0.7), (wx, wr)):
         assert np.array_equal(a.view(np.uint32), w.transpose(0, 2, 1).view(np.uint32))
-    _same_cache(b.get_footprint(), swept, "the polygon entries leave the cache alone")
+    assert_same_cache(b.get_footprint(), swept, "the polygon entries leave the cache alone")
     b.clear_footprint()
     assert np.isnan(b.get_footprint()).all()
     _close(b, *singles)
@@ -313,7 +234,7 @@ def test_read_side_on_a_batch(te, ctx, oracle, maps):
 
 def test_error_codes(te, ctx, oracle, maps):
     og, g, per = maps
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     b = ctx.map()
     lay = [_stack(per, k) for k in FILTER]
     with pytest.raises(te.TEError) as e:

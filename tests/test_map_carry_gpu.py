@@ -9,38 +9,16 @@ import pytest
 
 import submap_oracle as so
 import synth
-from helpers import footprint_arrays, mixed_request, request_footprints, same, same_polygons
-from test_submap_gpu import _check_windows, _windows
+from helpers import assert_same_answers, assert_same_bits, bits, mixed_request, noisy, request_footprints, unwrap
+from map_helpers import ask, assert_same_held, check_submaps, close_maps, held, submap_windows  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 ROWS, COLS, RES, POS = 150, 130, 0.02, (0.37, -0.21)
-CAP = 64
 BAD_ARG, MISSING_LAYER, UNSUPPORTED = -1, -2, -4
 MAIN = ("traversability", "traversability_slope", "traversability_step", "traversability_roughness", "elevation")
 FILTER = ("traversability", "slope", "step", "elevation")
-
-
-@pytest.fixture(autouse=True)
-def _close_maps(ctx, monkeypatch):
-    """Every te_map a test opens is destroyed when it ends, failed or not, while the context still exists."""
-    made, real = [], ctx.map
-    monkeypatch.setattr(ctx, "map", lambda: made.append(real()) or made[-1])
-    yield
-    for m in made:
-        m.close()
-
-
-def _bits(a):
-    return np.ascontiguousarray(np.asarray(a, dtype=np.float32)).view(np.uint32)
-
-
-def _same(a, b, what=""):
-    assert np.array_equal(_bits(a), _bits(b)), what
-
-
-def _unwrap(a, start):
-    return np.roll(a, (-start[0], -start[1]), axis=(0, 1))
+NOISE = (0.04, 0.02, 0.02, 0.02)   # fractions of NaN, +Inf, -Inf and zero cells of a noisy layer
 
 
 def _geo(te, start=(0, 0), rows=ROWS, cols=COLS):
@@ -49,23 +27,11 @@ def _geo(te, start=(0, 0), rows=ROWS, cols=COLS):
     return g
 
 
-def _noisy(rng, shape):
-    """float32 layer with NaN (several payloads), +-Inf and exact zeros."""
-    a = (rng.standard_normal(shape) * 3).astype(np.float32)
-    a[rng.random(shape) < 0.04] = np.nan
-    a[rng.random(shape) < 0.02] = np.inf
-    a[rng.random(shape) < 0.02] = -np.inf
-    a[rng.random(shape) < 0.02] = 0.0
-    odd = rng.random(shape) < 0.01   # NaN payloads other than the default one, signalling ones included
-    a.view(np.uint32)[odd] = (rng.integers(0, 2, odd.sum()) << 31 | 0x7f800000 | rng.integers(1, 1 << 23, odd.sum())).astype(np.uint32)
-    return a
-
-
 def _carried(te, seed, n=None):
     """The seven carried layers, (rows, cols) or (n, rows, cols)."""
     rng = np.random.default_rng(seed)
     shape = (ROWS, COLS) if n is None else (n, ROWS, COLS)
-    return {k: _noisy(rng, shape) for k in te.capi.CARRIED_LAYERS}
+    return {k: noisy(rng, shape, *NOISE) for k in te.capi.CARRIED_LAYERS}
 
 
 def _chain(te, ctx, g, seed=5, n=None):
@@ -76,24 +42,6 @@ def _chain(te, ctx, g, seed=5, n=None):
     else:
         m.chain_batched(g, p, n, np.stack([synth.terrain(g.rows, g.cols, RES, seed + k, "mixed") for k in range(n)]))
     return m
-
-
-def _held(te, m):
-    """Every layer the te_map holds, and its cache."""
-    names = []
-    for n in te.capi.LAYERS[:6] + te.capi.CARRIED_LAYERS:
-        try:
-            m.get_layers([n])
-            names.append(n)
-        except te.TEError as e:
-            assert e.code == MISSING_LAYER
-    return dict(m.get_layers(names), cache=m.get_footprint())
-
-
-def _same_held(a, b, what=""):
-    assert set(a) == set(b), (what, sorted(set(a) ^ set(b)))
-    for n in a:
-        _same(a[n], b[n], (what, n))
 
 
 def _device(torch, a):
@@ -124,22 +72,22 @@ def test_round_trip_single_map_with_start_index(te, ctx):
     got = m.get_layers(names)
     for n in names:
         if n == "lower_bound":
-            assert (_bits(got[n]) == 0).all()
+            assert (bits(got[n]) == 0).all()
         else:
-            _same(got[n], C7[n], n)                    # re-wrapped: the buffer order the layers came in
+            assert_same_bits(got[n], C7[n], n)                    # re-wrapped: the buffer order the layers came in
     dev = torch.full((len(names) * ROWS * COLS,), 7.0, dtype=torch.float32, device="cuda")
     gd = m.get_layers(names, out=dev, memory=te.MEM_DEVICE)
     ctx.synchronize()
     for n in names:
-        want = np.zeros((ROWS, COLS), np.float32) if n == "lower_bound" else _unwrap(C7[n], start)
-        _same(gd[n].cpu().numpy(), want, n)            # device memory: default order
+        want = np.zeros((ROWS, COLS), np.float32) if n == "lower_bound" else unwrap(C7[n], start)
+        assert_same_bits(gd[n].cpu().numpy(), want, n)            # device memory: default order
     # device layers are in default order; host reads re-wrap them
     D = _carried(te, 2)
-    m.carry_layers(["upper_bound", "time"], [_device(torch, _unwrap(D["upper_bound"], start)), None], memory=te.MEM_DEVICE)
+    m.carry_layers(["upper_bound", "time"], [_device(torch, unwrap(D["upper_bound"], start)), None], memory=te.MEM_DEVICE)
     ctx.synchronize()
     got = m.get_layers(["upper_bound", "lower_bound", "time"])
-    _same(got["upper_bound"], D["upper_bound"])
-    assert (_bits(got["lower_bound"]) == 0).all() and (_bits(got["time"]) == 0).all()
+    assert_same_bits(got["upper_bound"], D["upper_bound"])
+    assert (bits(got["lower_bound"]) == 0).all() and (bits(got["time"]) == 0).all()
 
 
 @pytest.mark.parametrize("memory", ["host", "device"])
@@ -160,7 +108,7 @@ def test_round_trip_batch(te, ctx, memory):
     got = m.get_layers(names)
     for k in names:
         assert got[k].shape == (n, ROWS, COLS)
-        _same(got[k], C7[k], k)
+        assert_same_bits(got[k], C7[k], k)
     # a selection rewrites only its maps, in map_index order
     S = _carried(te, 5, 2)
     sel = [2, 0]
@@ -171,12 +119,12 @@ def test_round_trip_batch(te, ctx, memory):
         ctx.synchronize()
     got = m.get_layers(names)
     for j, k in enumerate(sel):
-        _same(got["variance"][k], S["variance"][j])
-        assert (_bits(got["upper_bound"][k]) == 0).all()
-    _same(got["variance"][1], C7["variance"][1])
-    _same(got["upper_bound"][1], C7["upper_bound"][1])
+        assert_same_bits(got["variance"][k], S["variance"][j])
+        assert (bits(got["upper_bound"][k]) == 0).all()
+    assert_same_bits(got["variance"][1], C7["variance"][1])
+    assert_same_bits(got["upper_bound"][1], C7["upper_bound"][1])
     for k in ("robot_slope", "horizontal_variance_xy"):
-        _same(got[k], C7[k], k)
+        assert_same_bits(got[k], C7[k], k)
 
 
 # ---- 2. uncertainty_range --------------------------------------------------------------------------------------------------
@@ -187,7 +135,7 @@ def test_uncertainty_range_bits(te, ctx, start):
     g = _geo(te, start)
     m = _chain(te, ctx, g)
     rng = np.random.default_rng(6)
-    up, lo = _noisy(rng, (ROWS, COLS)), _noisy(rng, (ROWS, COLS))
+    up, lo = noisy(rng, (ROWS, COLS), *NOISE), noisy(rng, (ROWS, COLS), *NOISE)
     up[:3, :] = np.inf                                  # Inf - Inf, -Inf - -Inf, Inf - -Inf
     lo[0, :], lo[1, :], lo[2, :] = np.inf, -np.inf, -np.inf
     up[3, :], lo[3, :] = -np.inf, -np.inf
@@ -196,27 +144,27 @@ def test_uncertainty_range_bits(te, ctx, start):
     assert np.isnan(want).sum() > 500 and np.isinf(want).any()
     got = m.get_layers(["traversability", "upper_bound", "lower_bound", "uncertainty_range"])
     assert list(got) == ["traversability", "upper_bound", "lower_bound", "uncertainty_range"]
-    _same(got["uncertainty_range"], want)
-    _same(got["upper_bound"], up)
+    assert_same_bits(got["uncertainty_range"], want)
+    assert_same_bits(got["upper_bound"], up)
     out = torch.full((2 * ROWS * COLS + 1,), 3.0, dtype=torch.float32, device="cuda")
     gd = m.get_layers(["uncertainty_range", "elevation"], out=out[1:], memory=te.MEM_DEVICE)   # 4 bytes off 16-byte alignment
     ctx.synchronize()
-    _same(gd["uncertainty_range"].cpu().numpy(), _unwrap(want, start))
+    assert_same_bits(gd["uncertainty_range"].cpu().numpy(), unwrap(want, start))
     # a batch, in both memory modes
     b = _chain(te, ctx, _geo(te), n=2)
-    U, L = _noisy(rng, (2, ROWS, COLS)), _noisy(rng, (2, ROWS, COLS))
+    U, L = noisy(rng, (2, ROWS, COLS), *NOISE), noisy(rng, (2, ROWS, COLS), *NOISE)
     b.carry_layers(["lower_bound", "upper_bound"], [L, U])
-    _same(b.get_layers(["uncertainty_range"])["uncertainty_range"], _x86_sub(U, L))
+    assert_same_bits(b.get_layers(["uncertainty_range"])["uncertainty_range"], _x86_sub(U, L))
     out = torch.empty(2 * ROWS * COLS, dtype=torch.float32, device="cuda")
     gd = b.get_layers(["uncertainty_range"], out=out, memory=te.MEM_DEVICE)
     ctx.synchronize()
-    _same(gd["uncertainty_range"].cpu().numpy(), _x86_sub(U, L))
+    assert_same_bits(gd["uncertainty_range"].cpu().numpy(), _x86_sub(U, L))
 
 
 def test_uncertainty_range_errors(te, ctx):
     m = _chain(te, ctx, _geo(te))
     rng = np.random.default_rng(7)
-    m.carry_layers(["upper_bound"], [_noisy(rng, (ROWS, COLS))])
+    m.carry_layers(["upper_bound"], [noisy(rng, (ROWS, COLS), *NOISE)])
     with pytest.raises(te.TEError) as e:
         m.get_layers(["uncertainty_range"])
     assert e.value.code == MISSING_LAYER
@@ -238,17 +186,17 @@ def test_submaps_of_carried_layers(te, ctx, oracle):
     C7 = _carried(te, 8)
     m.carry_layers(list(C7), list(C7.values()))
     names = ["traversability", "elevation", "lower_bound", "horizontal_variance_x", "time"]
-    full = {k: _unwrap(v, start) for k, v in m.get_layers(names).items()}   # bit order
+    full = {k: unwrap(v, start) for k, v in m.get_layers(names).items()}   # bit order
     rng = np.random.default_rng(9)
-    pos, length = _windows(rng, 150, _geo(te))
+    pos, length = submap_windows(rng, 150, _geo(te))
     want = so.submap_geometry(oracle.Geometry.make(ROWS, COLS, RES, POS), pos, length)
     assert 0 < want["success"].sum() < len(pos)
-    _check_windows(m.get_submaps(pos, length, names), want, full, names)
+    check_submaps(m.get_submaps(pos, length, names), want, full, names)
     total = len(names) * int((want["rows"] * want["cols"]).sum())
     out = torch.full((total,), -3.0, dtype=torch.float32, device="cuda")
     res = m.get_submaps(pos, length, names, out=out, memory=te.MEM_DEVICE)
     ctx.synchronize()
-    _check_windows([(i, None if d is None else {n: v.cpu().numpy() for n, v in d.items()}) for i, d in res], want, full, names)
+    check_submaps([(i, None if d is None else {n: v.cpu().numpy() for n, v in d.items()}) for i, d in res], want, full, names)
     # a batch: window k on map win_map[k]
     n = 3
     b = _chain(te, ctx, _geo(te), n=n)
@@ -261,7 +209,7 @@ def test_submaps_of_carried_layers(te, ctx, oracle):
     for k in range(n):
         idx = np.nonzero(wm == k)[0]
         wk = {f: v[idx] for f, v in want.items()}
-        _check_windows([res[q] for q in idx], wk, {x: v[k] for x, v in fullb.items()}, bn)
+        check_submaps([res[q] for q in idx], wk, {x: v[k] for x, v in fullb.items()}, bn)
 
 
 # ---- 4. robot_slope through carry ------------------------------------------------------------------------------------------
@@ -274,20 +222,6 @@ def _robot_slope(rng, shape, base):
         a, b = int(rng.integers(0, shape[-2] - 4)), int(rng.integers(0, shape[-1] - 4))
         rs[..., a:a + 3, b:b + 3] = 0.0
     return np.asfortranarray(rs) if rs.ndim == 2 else rs
-
-
-def _ask(m, ft, R, fps, path_map=None):
-    fb, fx = footprint_arrays(R, fps)
-    kw = dict(max_footprint_vertices=16, conservative=R["cons"], compute_untraversable_polygon=R["cup"], untraversable_capacity=CAP)
-    if path_map is not None:
-        return m.check_footprint_request_batched(ft, path_map, R["begin"], R["poses"], R["radius"], fb, fx, **kw)
-    return m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, **kw)
-
-
-def _same_answers(a, b, what):
-    assert np.array_equal(a[0], b[0]), what
-    assert same(a[1], b[1]) and same(a[2], b[2]), what
-    same_polygons(a[3], a[4], b[3], b[4], what)
 
 
 @pytest.mark.parametrize("n", [None, 3])
@@ -309,15 +243,15 @@ def test_robot_slope_through_carry_equals_set_layers(te, ctx, oracle, n):
     else:
         b.set_layers_batched(g, n, *lay, roughness=outs["roughness"], robot_slope=rs)
         nr.set_layers_batched(g, n, *lay, roughness=outs["roughness"])
-    _same_held(_held(te, a), _held(te, b), "layers")
+    assert_same_held(held(te, a), held(te, b), "layers")
     fps = request_footprints(rng)
     gated = False
     for step in range(3):
-        R = mixed_request(rng, og, 120, fps, circular=0.7, cap_path=False)
+        R = dict(mixed_request(rng, og, 120, fps, circular=0.7, cap_path=False), fps=fps)
         pm = None if n is None else rng.integers(0, n, len(R["kind"])).astype(np.int32)
-        ga, gb, gn = _ask(a, ft, R, fps, pm), _ask(b, ft, R, fps, pm), _ask(nr, ft, R, fps, pm)
-        _same_answers(ga, gb, ("answers", step))
-        _same(a.get_footprint(), b.get_footprint(), ("cache", step))
+        ga, gb, gn = ask(a, ft, R, pm), ask(b, ft, R, pm), ask(nr, ft, R, pm)
+        assert_same_answers(ga, gb, ("answers", step))
+        assert_same_bits(a.get_footprint(), b.get_footprint(), ("cache", step))
         assert a.request_stats() == b.request_stats(), step
         gated = gated or not np.array_equal(ga[0], gn[0])
     assert gated   # the request crossed robot_slope zeros: without the layer some answers differ
@@ -334,22 +268,22 @@ def test_carry_leaves_cache_memo_and_answers(te, ctx, oracle):
         m.chain(g, p, z)
     rng = np.random.default_rng(13)
     fps = request_footprints(rng)
-    R = mixed_request(rng, og, 80, fps, circular=0.7, cap_path=False)
-    _same_answers(_ask(a, ft, R, fps), _ask(b, ft, R, fps), "first")
+    R = dict(mixed_request(rng, og, 80, fps, circular=0.7, cap_path=False), fps=fps)
+    assert_same_answers(ask(a, ft, R), ask(b, ft, R), "first")
     cache = a.get_footprint()
     assert np.isfinite(cache).any()
     a.carry_layers(list(te.capi.CARRIED_LAYERS), [None] * 4 + list(_carried(te, 14).values())[4:])
-    _same(a.get_footprint(), cache, "cache after carry")
+    assert_same_bits(a.get_footprint(), cache, "cache after carry")
     for step in range(2):
-        R = mixed_request(rng, og, 80, fps, circular=0.7, cap_path=False)
-        _same_answers(_ask(a, ft, R, fps), _ask(b, ft, R, fps), step)
-        _same(a.get_footprint(), b.get_footprint(), step)
+        R = dict(mixed_request(rng, og, 80, fps, circular=0.7, cap_path=False), fps=fps)
+        assert_same_answers(ask(a, ft, R), ask(b, ft, R), step)
+        assert_same_bits(a.get_footprint(), b.get_footprint(), step)
         assert a.request_stats() == b.request_stats(), step
-    _same(a.footprint(ft), b.footprint(ft), "sweep on the kept cache")
+    assert_same_bits(a.footprint(ft), b.footprint(ft), "sweep on the kept cache")
     # robot_slope only adds the inclination gates of later requests: the cache stays as it was
     cache = a.get_footprint()
     a.carry_layers(["robot_slope"], [np.ones((200, 180), np.float32)])
-    _same(a.get_footprint(), cache, "cache after carrying robot_slope")
+    assert_same_bits(a.get_footprint(), cache, "cache after carrying robot_slope")
 
 
 # ---- 6. lifetime -----------------------------------------------------------------------------------------------------------
@@ -399,30 +333,30 @@ def test_maps_updates_fill_the_selected_maps_carried_layers_with_nan(te, ctx):
 
     for sel, update in (([2, 0], lambda s: b.chain_maps(g, p, s, np.stack([z] * len(s)))), ([1], set_maps),
                         ([3], lambda s: b.chain_image_maps(g, p, s, np.stack([img] * len(s)), 0.0, 1.5))):
-        before = _held(te, b)
+        before = held(te, b)
         n0 = ctx.stats()[0]
         update(sel)
-        after = _held(te, b)
+        after = held(te, b)
         assert set(after) == set(before)
         for k in range(n):
             for name in after:
                 if k in sel and name in names:
                     assert np.isnan(after[name][k]).all(), (sel, k, name)
                 elif k not in sel:
-                    _same(after[name][k], before[name][k], (sel, k, name))
+                    assert_same_bits(after[name][k], before[name][k], (sel, k, name))
         if update is set_maps:
             assert ctx.stats()[0] - n0 == 1   # the NaN fill rides the one k_map_slots launch
     # a selection may not add a layer the batch does not hold; the map is unchanged
-    before = _held(te, b)
+    before = held(te, b)
     for name in ("variance", "robot_slope"):
         with pytest.raises(te.TEError) as e:
             b.carry_layers([name], [None], map_index=[0])
         assert e.value.code == BAD_ARG
-        _same_held(_held(te, b), before, name)
+        assert_same_held(held(te, b), before, name)
     b.carry_layers(["variance"], [None])   # every map: fine
     b.carry_layers(["variance"], [np.ones((1, ROWS, COLS), np.float32)], map_index=[2])
     got = b.get_layers(["variance"])["variance"]
-    assert (got[2] == 1.0).all() and (_bits(got[[0, 1, 3]]) == 0).all()
+    assert (got[2] == 1.0).all() and (bits(got[[0, 1, 3]]) == 0).all()
 
 
 def test_launch_counts(te, ctx):
@@ -448,7 +382,7 @@ def test_error_table_leaves_the_map_unchanged(te, ctx):
     assert fn(None, 0, None, 0x100, ptrs(1), te.MEM_HOST) == BAD_ARG
     b = _chain(te, ctx, _geo(te), n=3)
     b.carry_layers(["upper_bound"], [np.zeros((3, ROWS, COLS), np.float32)])
-    before = _held(te, b)
+    before = held(te, b)
     idx = lambda *v: np.asarray(v, np.int32)  # noqa: E731
     cases = [
         (BAD_ARG, 0, None, 0, 0),                        # empty mask
@@ -472,14 +406,14 @@ def test_error_table_leaves_the_map_unchanged(te, ctx):
     for code, nsel, mi, mask, npt in cases:
         rc = fn(b._h, nsel, None if mi is None else mi.ctypes.data, mask, ptrs(max(npt, 1)), te.MEM_HOST)
         assert rc == code, (nsel, mi, hex(mask), rc, L.te_last_error())
-        _same_held(_held(te, b), before, (nsel, hex(mask)))
+        assert_same_held(held(te, b), before, (nsel, hex(mask)))
     assert fn(b._h, 0, None, 0x100, None, te.MEM_HOST) == BAD_ARG          # a null layers array
     assert fn(b._h, 0, None, 0x100, ptrs(1), 7) == BAD_ARG                 # an unknown memory mode
-    _same_held(_held(te, b), before, "null layers / memory")
+    assert_same_held(held(te, b), before, "null layers / memory")
     # a selection on a map whose layers came with a start index
     w = _chain(te, ctx, _geo(te, (5, 9)))
     w.carry_layers(["upper_bound"], [lay])
-    before = _held(te, w)
+    before = held(te, w)
     sel0 = idx(0)
     assert fn(w._h, 1, sel0.ctypes.data, 0x100, ptrs(1), te.MEM_HOST) == UNSUPPORTED
-    _same_held(_held(te, w), before, "start index")
+    assert_same_held(held(te, w), before, "start index")

@@ -5,11 +5,10 @@ import pytest
 
 import paths_oracle as po
 import synth
-from helpers import chain_layers, footprint_arrays, mixed_request, request_footprints, same, same_polygons
+from helpers import assert_same_answers, chain_layers, footprint_arrays, footprint_params, mixed_request, request_footprints, subset
+from map_helpers import CAP, assert_same_cache
 
 pytestmark = pytest.mark.gpu
-
-CAP = 64
 
 
 def _setup(te, oracle, rows=200, cols=180, res=0.02, seed=61, position=(0.0, 0.0)):
@@ -19,20 +18,6 @@ def _setup(te, oracle, rows=200, cols=180, res=0.02, seed=61, position=(0.0, 0.0
     return og, g, L, rs
 
 
-def _params(te, oracle, verify=0, **kw):
-    ft, fo = te.FootprintParams.yaml_defaults(), oracle.FootprintParams.yaml_defaults()
-    for p in (ft, fo):
-        p.verify_roughness = verify
-        for k, v in kw.items():
-            setattr(p, k, v)
-    return ft, fo
-
-
-def _same_cache(a, b, what):
-    assert np.array_equal(a.view(np.uint32), b.view(np.uint32)) or same(a.astype(np.float64), b.astype(np.float64)), \
-        (what, int(np.sum(~((a == b) | (np.isnan(a) & np.isnan(b))))))
-
-
 def _both(m, og, ft, fo, OL, cache, R, fps):
     """One request on the map and on the oracle; asserts every output and the cache are identical."""
     fb, fx = footprint_arrays(R, fps)
@@ -40,25 +25,15 @@ def _both(m, og, ft, fo, OL, cache, R, fps):
                                     conservative=R["cons"], compute_untraversable_polygon=R["cup"], untraversable_capacity=CAP)
     want = po.check_request(og, fo, OL, R["begin"], R["poses"], R["radius"], fb, fx, conservative=R["cons"], cup=R["cup"],
                             cache=cache, capacity=CAP)
-    assert np.array_equal(got[0], want[0]), np.nonzero(got[0] != want[0])[0][:10]
-    assert same(got[1], want[1]) and same(got[2], want[2])
-    same_polygons(got[3], got[4], want[3], want[4], "polygons")
-    _same_cache(m.get_footprint(), cache, "cache")
+    assert_same_answers(got, want, "polygons")
+    assert_same_cache(m.get_footprint(), cache, nan_bits=False)
     return got
-
-
-def _repeat(R, idx):
-    """A request made of paths `idx` of R (planner batches overlap)."""
-    b = R["begin"]
-    begin = np.concatenate([[0], np.cumsum(b[idx + 1] - b[idx])]).astype(np.int32)
-    poses = np.concatenate([R["poses"][b[q]:b[q + 1]] for q in idx])
-    return dict(begin=begin, poses=poses, radius=R["radius"][idx], kind=R["kind"][idx], cons=R["cons"][idx], cup=R["cup"][idx])
 
 
 @pytest.mark.parametrize("verify,slope", [(0, False), (1, True)])
 def test_request_sequence_matches_oracle(te, ctx, oracle, verify, slope):
     og, g, L, rs = _setup(te, oracle)
-    ft, fo = _params(te, oracle, verify)
+    ft, fo = footprint_params(te, oracle, verify)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"], roughness=L["roughness"],
                  robot_slope=rs if slope else None)
@@ -68,7 +43,7 @@ def test_request_sequence_matches_oracle(te, ctx, oracle, verify, slope):
     fps = request_footprints(rng)
     R1 = mixed_request(rng, og, 60, fps, circular=0.6, cap_path=False)
     R2 = mixed_request(rng, og, 80, fps, circular=0.7, planner=True, cap_path=False)
-    for R in (R1, _repeat(R1, rng.permutation(len(R1["kind"]))), R2, _repeat(R2, np.arange(len(R2["kind"])) // 2)):
+    for R in (R1, subset(R1, rng.permutation(len(R1["kind"]))), R2, subset(R2, np.arange(len(R2["kind"])) // 2)):
         _both(m, og, ft, fo, OL, cache, R, fps)
     cand, keys, stored = m.request_stats()
     assert keys <= cand and stored <= keys
@@ -77,7 +52,7 @@ def test_request_sequence_matches_oracle(te, ctx, oracle, verify, slope):
 
 def test_annulus_blocker_revisit_and_single_poses_in_one_cell(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, seed=62)
-    ft, fo = _params(te, oracle)
+    ft, fo = footprint_params(te, oracle)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"])
     cache = po.empty_cache(og)
@@ -104,7 +79,7 @@ def test_zero_mean_circle_then_fails(te, ctx, oracle):
     og, g = oracle.Geometry.make(rows, cols, 0.05), te.Geometry.make(rows, cols, 0.05)
     ones = np.ones((rows, cols), np.float32, order="F")
     L = dict(traversability=np.zeros((rows, cols), np.float32, order="F"), slope=ones, step=ones, elevation=0 * ones)
-    ft, fo = _params(te, oracle)
+    ft, fo = footprint_params(te, oracle)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"])
     cache = po.empty_cache(og)
@@ -124,7 +99,7 @@ def test_nonfinite_circular_poses(te, ctx, oracle, cup, slope):
     with such an end fails without a polygon after the earlier segments stored their cells.  Asked twice, on the cache the
     first request left."""
     og, g, L, rs = _setup(te, oracle, seed=68)
-    ft, fo = _params(te, oracle)
+    ft, fo = footprint_params(te, oracle)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"], robot_slope=rs if slope else None)
     OL = dict(L, robot_slope=rs if slope else None)
@@ -149,7 +124,7 @@ def test_nonfinite_circular_poses(te, ctx, oracle, cup, slope):
 
 def test_sweep_and_request_share_the_cache(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, rows=160, cols=150, seed=63)
-    ft, fo = _params(te, oracle)
+    ft, fo = footprint_params(te, oracle)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"])
     cache = po.empty_cache(og)
@@ -172,7 +147,7 @@ def test_sweep_and_request_share_the_cache(te, ctx, oracle):
 
 def test_new_layers_clear_cache_and_memo(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, rows=150, cols=140, seed=64)
-    ft, fo = _params(te, oracle)
+    ft, fo = footprint_params(te, oracle)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"])
     rng = np.random.default_rng(13)
@@ -180,7 +155,7 @@ def test_new_layers_clear_cache_and_memo(te, ctx, oracle):
     cache = po.empty_cache(og)
     _both(m, og, ft, fo, L, cache, R, [])
     # a changed max_gap_width rebuilds the memo and keeps the cache
-    ft2, fo2 = _params(te, oracle, max_gap_width=0.1)
+    ft2, fo2 = footprint_params(te, oracle, max_gap_width=0.1)
     _both(m, og, ft2, fo2, L, cache, mixed_request(rng, og, 40, [], circular=1.0, cap_path=False), [])
     # new layers: empty cache, fresh memo
     L2 = dict(L, traversability=np.asfortranarray(L["traversability"] * np.float32(0.5)))
@@ -204,7 +179,7 @@ def test_new_layers_clear_cache_and_memo(te, ctx, oracle):
 
 def test_fresh_map_disjoint_cells_equal_stateless_request(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, seed=65)
-    ft, _ = _params(te, oracle, verify=1)
+    ft, _ = footprint_params(te, oracle, verify=1)
     m = ctx.map()
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"], roughness=L["roughness"], robot_slope=rs)
     rng = np.random.default_rng(15)
@@ -225,8 +200,7 @@ def test_fresh_map_disjoint_cells_equal_stateless_request(te, ctx, oracle):
     want = ctx.check_footprint_request(g, ft, L["traversability"], L["slope"], L["step"], L["elevation"], R["begin"], R["poses"],
                                        R["radius"], fb, fx, robot_slope=rs, roughness=L["roughness"],
                                        compute_untraversable_polygon=R["cup"], untraversable_capacity=CAP)
-    assert np.array_equal(got[0], want[0]) and same(got[1], want[1]) and same(got[2], want[2])
-    same_polygons(got[3], got[4], want[3], want[4], "polygons")
+    assert_same_answers(got, want, "polygons")
     # te_map_footprint_polygon is te_footprint_polygon on the map's layers
     pts = np.array([[0.2, 0.1], [-0.2, 0.1], [-0.2, -0.1], [0.2, -0.1]])
     gx, gr = m.footprint_polygon(ft, pts, 0.3)
@@ -239,7 +213,7 @@ def test_fresh_map_disjoint_cells_equal_stateless_request(te, ctx, oracle):
 
 def test_start_index_layers(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, rows=120, cols=100, seed=66)
-    ft, fo = _params(te, oracle)
+    ft, fo = footprint_params(te, oracle)
     sr, sc = 37, 61
     wrap = lambda a: np.asfortranarray(np.roll(np.roll(a, sr, axis=0), sc, axis=1))  # noqa: E731  map cell (i, j) at (i+sr, j+sc)
     gw = te.Geometry.make(og.rows, og.cols, og.resolution)
@@ -263,7 +237,7 @@ def test_start_index_layers(te, ctx, oracle):
 
 def test_error_codes(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, rows=64, cols=64, seed=67)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     m = ctx.map()
     one = dict(path_begin=np.array([0, 1], np.int32), poses=np.array([[0.0, 0, 0, 0, 0, 0, 1]]), radius=np.array([0.2]),
                footprint_begin=np.zeros(2, np.int32), footprint_xyz=np.zeros((0, 3), np.float32))
@@ -274,7 +248,7 @@ def test_error_codes(te, ctx, oracle):
         m.get_footprint()
     assert e.value.code == -1
     m.set_layers(g, L["traversability"], L["slope"], L["step"], L["elevation"])
-    ftr, _ = _params(te, oracle, verify=1)
+    ftr, _ = footprint_params(te, oracle, verify=1)
     with pytest.raises(te.TEError) as e:
         m.check_footprint_request(ftr, **one)
     assert e.value.code == -2   # verify_roughness without a roughness layer

@@ -7,6 +7,7 @@ import pytest
 import occupancy_oracle as oo
 import synth
 from helpers import footprint_arrays, mixed_request, request_footprints
+from map_helpers import all_layer_names, close_maps  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -14,16 +15,6 @@ RES = 0.04
 YAML = ["traversability", "traversability_slope", "traversability_step", "traversability_roughness"]  # traversability.yaml
 POLY = [[0.45, 0.30], [0.45, -0.30], [-0.45, -0.30], [-0.45, 0.30]]
 BAD_ARG, MISSING_LAYER = -1, -2
-
-
-@pytest.fixture(autouse=True)
-def _close_maps(ctx, monkeypatch):
-    """Every te_map a test opens is destroyed when it ends, failed or not, while the context still exists."""
-    made, real = [], ctx.map
-    monkeypatch.setattr(ctx, "map", lambda: made.append(real()) or made[-1])
-    yield
-    for m in made:
-        m.close()
 
 
 def _same(got, want, what=""):
@@ -129,10 +120,6 @@ def test_value_sweep(te, ctx):
 
 # ---- 3. every layer bit, each with its own range ---------------------------------------------------------------------------
 
-def _all_names(te):
-    return list(te.capi.LAYERS) + list(te.capi.CARRIED_LAYERS) + [te.capi.UNCERTAINTY_RANGE] + list(te.capi.POLYGON_LAYERS)
-
-
 def _full_map(te, ctx, rows, cols, start=(0, 0), seed=5, pos=(1.3, -0.7)):
     """A map holding every layer bit: the chain, robot_slope and the carried layers, a cache a request filled in part, and
     traversability_x / _rot.  start: the same map given with that circular-buffer start index."""
@@ -161,7 +148,7 @@ def _full_map(te, ctx, rows, cols, start=(0, 0), seed=5, pos=(1.3, -0.7)):
 def test_every_layer_bit(te, ctx):
     torch = pytest.importorskip("torch")
     m = _full_map(te, ctx, 320, 256)
-    names = _all_names(te)
+    names = all_layer_names(te)
     rng = np.random.default_rng(3)
     lo = rng.uniform(-1, 1, len(names)).astype(np.float32)
     hi = (lo + rng.choice([-1.0, 1.0, 2.5], len(names))).astype(np.float32)

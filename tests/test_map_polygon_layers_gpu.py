@@ -9,6 +9,8 @@ import numpy as np
 import pytest
 
 import synth
+from helpers import assert_same_bits, bits, close_sweep
+from map_helpers import assert_same_held, close_maps, held  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -17,24 +19,6 @@ POLY = [[0.45, 0.30], [0.45, -0.30], [-0.45, -0.30], [-0.45, 0.30]]   # robot_fo
 XR = ["traversability_x", "traversability_rot"]
 BAD_ARG, MISSING_LAYER, UNSUPPORTED = -1, -2, -4
 SPREAD = np.array([(0.0, 0.0), (13.37, -3.21), (-101.23, 77.7), (1000.01, 0.05), (0.31, 512.39), (-7.77, -3.21)])
-
-
-@pytest.fixture(autouse=True)
-def _close_maps(ctx, monkeypatch):
-    """Every te_map a test opens is destroyed when it ends, failed or not, while the context still exists."""
-    made, real = [], ctx.map
-    monkeypatch.setattr(ctx, "map", lambda: made.append(real()) or made[-1])
-    yield
-    for m in made:
-        m.close()
-
-
-def _bits(a):
-    return np.ascontiguousarray(np.asarray(a, dtype=np.float32)).view(np.uint32)
-
-
-def _same(a, b, what=""):
-    assert np.array_equal(_bits(a), _bits(b)), what
 
 
 def _terrain(n, seed=0, rows=ROWS, cols=COLS):
@@ -53,32 +37,6 @@ def _single(te, ctx, z, pos=(0.0, 0.0)):
     return s
 
 
-def _held(te, m):
-    """Every layer the te_map holds, and its cache."""
-    names = []
-    for n in te.capi.LAYERS[:6] + te.capi.CARRIED_LAYERS + te.capi.POLYGON_LAYERS:
-        try:
-            m.get_layers([n])
-            names.append(n)
-        except te.TEError as e:
-            assert e.code == MISSING_LAYER
-    return dict(m.get_layers(names), cache=m.get_footprint())
-
-
-def _same_held(a, b, what=""):
-    assert set(a) == set(b), (what, sorted(set(a) ^ set(b)))
-    for n in a:
-        _same(a[n], b[n], (what, n))
-
-
-def _close(a, b):
-    """The oracle's rule for the polygon sweep (tests/test_footprint_gpu.py): the prefix sums add the same float32 terms in another
-    order, so a handful of cells may differ in the last float32 bit; the blocked cells are the same."""
-    m = ~np.isnan(a)
-    return (np.array_equal(np.isnan(a), np.isnan(b)) and np.array_equal(a[m] == 0, b[m] == 0)
-            and float((a[m] == b[m]).mean()) > 0.999 and np.allclose(a[m], b[m], rtol=2e-7, atol=0))
-
-
 # ---- 1. single map ---------------------------------------------------------------------------------------------------------
 
 def test_single_map_with_start_index(te, ctx, oracle):
@@ -90,18 +48,18 @@ def test_single_map_with_start_index(te, ctx, oracle):
     m.chain(g, te.ChainParams.yaml_defaults(0), _terrain(1, 3)[0])      # layers in buffer order
     want_x, want_rot = m.footprint_polygon(ft, POLY, yaw)
     got_x, got_rot = m.footprint_polygon_keep(ft, POLY, yaw, outputs=True)
-    _same(got_x, want_x, "x")
-    _same(got_rot, want_rot, "rot")
+    assert_same_bits(got_x, want_x, "x")
+    assert_same_bits(got_rot, want_rot, "rot")
     kept = m.get_layers(XR)                                            # re-wrapped like the map's other outputs
-    _same(kept["traversability_x"], want_x)
-    _same(kept["traversability_rot"], want_rot)
+    assert_same_bits(kept["traversability_x"], want_x)
+    assert_same_bits(kept["traversability_rot"], want_rot)
     # the oracle on the unwrapped layers
     lay = m.get_layers(["traversability", "traversability_slope", "traversability_step", "elevation"])
     unwrap = lambda a: np.asfortranarray(np.roll(a, (-start[0], -start[1]), axis=(0, 1)))  # noqa: E731
     ox, orot = oracle.footprint_polygon(oracle.Geometry.make(ROWS, COLS, RES, pos), oracle.FootprintParams.yaml_defaults(), POLY, yaw,
                                         *(unwrap(lay[k]) for k in ("traversability", "traversability_slope", "traversability_step",
                                                                    "elevation")))
-    assert _close(unwrap(got_x), ox) and _close(unwrap(got_rot), orot)
+    assert close_sweep(unwrap(got_x), ox) and close_sweep(unwrap(got_rot), orot)
     assert (ox > 0).any()
 
 
@@ -117,16 +75,16 @@ def test_whole_batch_a_yaw_per_map(te, ctx):
     for k in range(len(z)):
         sx, srot = _single(te, ctx, z[k]).footprint_polygon(ft, POLY, yaws[k])
         for got in (x[k], kept["traversability_x"][k]):
-            _same(got, sx, k)
+            assert_same_bits(got, sx, k)
         for got in (rot[k], kept["traversability_rot"][k]):
-            _same(got, srot, k)
+            assert_same_bits(got, srot, k)
     # one yaw for every map
     b.footprint_polygon_keep(ft, POLY, -0.4)
     kept = b.get_layers(XR)
     for k in range(len(z)):
         sx, srot = _single(te, ctx, z[k]).footprint_polygon(ft, POLY, -0.4)
-        _same(kept["traversability_x"][k], sx, k)
-        _same(kept["traversability_rot"][k], srot, k)
+        assert_same_bits(kept["traversability_x"][k], sx, k)
+        assert_same_bits(kept["traversability_rot"][k], srot, k)
 
 
 # ---- 3. batch at several positions, scrambled selections -------------------------------------------------------------------
@@ -142,31 +100,31 @@ def test_selection_at_several_positions(te, ctx):
     singles = [_single(te, ctx, z[k], SPREAD[k]) for k in range(n)]
 
     def check(sel, yaws, before):
-        after = _held(te, b)
+        after = held(te, b, polygon=True)
         assert set(after) == set(before) | set(XR), sorted(set(after) ^ set(before))
         for name in after:
             if name not in XR:
-                _same(after[name], before[name], name)                  # the cache and every other layer
+                assert_same_bits(after[name], before[name], name)                  # the cache and every other layer
         for j, k in enumerate(sel):
             sx, srot = singles[k].footprint_polygon(ft, POLY, yaws[j])
-            _same(after["traversability_x"][k], sx, (sel, k))
-            _same(after["traversability_rot"][k], srot, (sel, k))
+            assert_same_bits(after["traversability_x"][k], sx, (sel, k))
+            assert_same_bits(after["traversability_rot"][k], srot, (sel, k))
         for k in set(range(n)) - set(sel):
             for name in XR:
                 if name in before:
-                    _same(after[name][k], before[name][k], (sel, k, name))
+                    assert_same_bits(after[name][k], before[name][k], (sel, k, name))
                 else:
-                    assert (_bits(after[name][k]) == 0xffffffff).all(), (sel, k, name)   # never swept
+                    assert (bits(after[name][k]) == 0xffffffff).all(), (sel, k, name)   # never swept
         assert b.request_stats() == stats
 
-    before = _held(te, b)
+    before = held(te, b, polygon=True)
     sel, yaws = [4, 1], [0.5, -2.0]
     x, rot = b.footprint_polygon_keep(ft, POLY, yaws, map_index=sel, outputs=True)
     check(sel, yaws, before)
-    after = _held(te, b)
+    after = held(te, b, polygon=True)
     for j, k in enumerate(sel):                                         # outputs: the swept maps in map_index order
-        _same(x[j], after["traversability_x"][k])
-        _same(rot[j], after["traversability_rot"][k])
+        assert_same_bits(x[j], after["traversability_x"][k])
+        assert_same_bits(rot[j], after["traversability_rot"][k])
     before = after
     sel, yaws = [3, 0, 5, 1], [1.1, 0.5, 1.1, 0.0]                      # repeated yaws, yaw 0, a map swept again
     b.footprint_polygon_keep(ft, POLY, yaws, map_index=sel)
@@ -213,13 +171,13 @@ def test_get_layers_and_submaps(te, ctx):
     mixed = b.get_layers(["traversability_rot", "elevation", "traversability", "traversability_x", "traversability_slope"])
     assert list(mixed) == ["traversability", "traversability_slope", "elevation"] + XR   # bit order
     for name in XR:
-        _same(mixed[name], kept[name], name)
+        assert_same_bits(mixed[name], kept[name], name)
     out = torch.empty(len(names) * n * ROWS * COLS, dtype=torch.float32, device="cuda")
     dev = b.get_layers(names, out=out, memory=te.MEM_DEVICE)
     ctx.synchronize()
     for name in names:
         got = np.ascontiguousarray(dev[name].cpu().numpy())           # device layers: (n, rows, cols) views in default order
-        _same(got, mixed[name], name)
+        assert_same_bits(got, mixed[name], name)
     # windows inside the map and at its edge, on every map
     half = np.array([0.5 * ROWS * RES, 0.5 * COLS * RES])
     win_map, centres, lengths = [], [], []
@@ -233,11 +191,11 @@ def test_get_layers_and_submaps(te, ctx):
     for (info, lay), k in zip(res, win_map):
         r0, c0, nr, nc = int(info["top_row"]), int(info["top_col"]), int(info["rows"]), int(info["cols"])
         for name in XR:
-            _same(lay[name], kept[name][k][r0:r0 + nr, c0:c0 + nc], (k, name))
+            assert_same_bits(lay[name], kept[name][k][r0:r0 + nr, c0:c0 + nc], (k, name))
     s = _single(te, ctx, z[0])
     s.footprint_polygon_keep(ft, POLY, 0.3)
     (info, lay), = s.get_submaps([(0.1, 0.1)], [(0.6, 0.4)], XR + ["traversability"])
-    _same(lay["traversability_rot"], kept["traversability_rot"][0][int(info["top_row"]):int(info["top_row"]) + int(info["rows"]),
+    assert_same_bits(lay["traversability_rot"], kept["traversability_rot"][0][int(info["top_row"]):int(info["top_row"]) + int(info["rows"]),
                                                                      int(info["top_col"]):int(info["top_col"]) + int(info["cols"])])
 
 
@@ -255,9 +213,9 @@ def test_device_memory_outputs(te, ctx):
         d.footprint_polygon_keep(ft, POLY, yaws, map_index=sel, outputs=(None, dr), memory=te.MEM_DEVICE)
         ctx.synchronize()
         as_host = lambda t: t.cpu().numpy().reshape(ns, COLS, ROWS).transpose(0, 2, 1)  # noqa: E731
-        _same(as_host(dx), hx, sel)
-        _same(as_host(dr), hr, sel)
-        _same_held(_held(te, d), _held(te, h), sel)
+        assert_same_bits(as_host(dx), hx, sel)
+        assert_same_bits(as_host(dr), hr, sel)
+        assert_same_held(held(te, d, polygon=True), held(te, h, polygon=True), sel)
 
 
 # ---- 6. lifetime -----------------------------------------------------------------------------------------------------------
@@ -302,7 +260,7 @@ def test_lifetime(te, ctx):
         ctx.synchronize()
         after = b.get_layers(XR)
         for name in XR:
-            _same(after[name], kept[name], (what, name))
+            assert_same_bits(after[name], kept[name], (what, name))
     # the _maps updates fill the selected maps' layers with 0xffffffff and keep the others
     img = (np.arange(ROWS * COLS).reshape(ROWS, COLS) % 241).astype(np.uint8)
     lay = b.get_layers(["traversability", "traversability_slope", "traversability_step", "traversability_roughness", "elevation"])
@@ -324,9 +282,9 @@ def test_lifetime(te, ctx):
         for k in range(n):
             for name in XR:
                 if k in sel:
-                    assert (_bits(after[name][k]) == 0xffffffff).all(), (what, k, name)
+                    assert (bits(after[name][k]) == 0xffffffff).all(), (what, k, name)
                 else:
-                    _same(after[name][k], before[name][k], (what, k, name))
+                    assert_same_bits(after[name][k], before[name][k], (what, k, name))
     # a _maps_at move, then a sweep of the moved map at its new position
     b.footprint_polygon_keep(ft, POLY, [0.6, 0.6], map_index=[2, 1])
     kept = b.get_layers(XR)
@@ -335,8 +293,8 @@ def test_lifetime(te, ctx):
         s.set_layers(te.Geometry.make(ROWS, COLS, RES, pos), lay["traversability"][k], lay["traversability_slope"][k],
                      lay["traversability_step"][k], lay["elevation"][k], roughness=lay["traversability_roughness"][k])
         sx, srot = s.footprint_polygon(ft, POLY, 0.6)
-        _same(kept["traversability_x"][k], sx, k)
-        _same(kept["traversability_rot"][k], srot, k)
+        assert_same_bits(kept["traversability_x"][k], sx, k)
+        assert_same_bits(kept["traversability_rot"][k], srot, k)
     # whole-map updates drop both layers
     one = _terrain(1, 60)[0]
     for what, update in (("chain_batched", lambda: b.chain_batched(g, p, n, z)),
@@ -366,18 +324,18 @@ def test_maps_update_fills_every_held_layer(te, ctx):
     b = _batch(te, ctx, _terrain(n, 90))
     b.carry_layers(list(te.capi.CARRIED_LAYERS), [None] * len(te.capi.CARRIED_LAYERS))
     b.footprint_polygon_keep(ft, POLY, [0.2, 0.4, 0.6])
-    before = _held(te, b)
+    before = held(te, b, polygon=True)
     lay = {k: before[k][[1]] for k in ("traversability", "traversability_slope", "traversability_step", "traversability_roughness",
                                        "elevation")}
     n0 = ctx.stats()[0]
     b.set_layers_maps(g, [1], lay["traversability"], lay["traversability_slope"], lay["traversability_step"], lay["elevation"],
                       roughness=lay["traversability_roughness"])
     assert ctx.stats()[0] - n0 == 2
-    after = _held(te, b)
+    after = held(te, b, polygon=True)
     for name in te.capi.CARRIED_LAYERS + te.capi.POLYGON_LAYERS:
-        assert (_bits(after[name][1]) == 0xffffffff).all(), name
+        assert (bits(after[name][1]) == 0xffffffff).all(), name
         for k in (0, 2):
-            _same(after[name][k], before[name][k], (k, name))
+            assert_same_bits(after[name][k], before[name][k], (k, name))
 
 
 # ---- 7. errors -------------------------------------------------------------------------------------------------------------
@@ -401,7 +359,7 @@ def test_error_table_leaves_the_map_unchanged(te, ctx):
     b = _batch(te, ctx, _terrain(3, 70))
     b.footprint_polygon_keep(ft, POLY, 0.5, map_index=[1])
     b.footprint(ft)
-    before = _held(te, b)
+    before = held(te, b, polygon=True)
     rough = te.FootprintParams.yaml_defaults()
     rough.verify_roughness = 1
     nan_yaw = dbl([0.1, np.nan, 0.2])
@@ -429,22 +387,22 @@ def test_error_table_leaves_the_map_unchanged(te, ctx):
     for code, kw in cases:
         rc = call(b, **kw)
         assert rc == code, (kw, rc, L.te_last_error())
-        _same_held(_held(te, b), before, kw)
+        assert_same_held(held(te, b, polygon=True), before, kw)
     # verify_roughness without roughness
     nr = ctx.map()
     lay = b.get_layers(["traversability", "traversability_slope", "traversability_step", "elevation"])
     nr.set_layers_batched(te.Geometry.make(ROWS, COLS, RES), 3, *(lay[k] for k in ("traversability", "traversability_slope",
                                                                                      "traversability_step", "elevation")))
-    nr_before = _held(te, nr)
+    nr_before = held(te, nr, polygon=True)
     assert call(nr, p=rough) == MISSING_LAYER
-    _same_held(_held(te, nr), nr_before, "verify_roughness")
+    assert_same_held(held(te, nr, polygon=True), nr_before, "verify_roughness")
     # a selection on a map whose layers came with a start index
     gw = te.Geometry.make(ROWS, COLS, RES)
     gw.start_row, gw.start_col = 5, 9
     w = ctx.map()
     w.chain(gw, te.ChainParams.yaml_defaults(0), _terrain(1, 80)[0])
     assert call(w, nsel=1, mi=idx(0)) == UNSUPPORTED
-    assert "traversability_x" not in _held(te, w)
+    assert "traversability_x" not in held(te, w, polygon=True)
 
 
 def test_distinct_yaw_cap(te, ctx):
@@ -468,5 +426,5 @@ def test_distinct_yaw_cap(te, ctx):
         s = ctx.map()
         s.chain(te.Geometry.make(rows, cols, RES), te.ChainParams.yaml_defaults(0), np.zeros((rows, cols), np.float32))
         sx, srot = s.footprint_polygon(ft, POLY, yaws[k])
-        _same(kept["traversability_x"][k], sx, k)
-        _same(kept["traversability_rot"][k], srot, k)
+        assert_same_bits(kept["traversability_x"][k], sx, k)
+        assert_same_bits(kept["traversability_rot"][k], srot, k)

@@ -11,24 +11,14 @@ import pytest
 
 import paths_oracle as po
 import synth
-from helpers import chain_layers, footprint_arrays, mixed_request, request_footprints, same, same_polygons
+from helpers import assert_same_answers, chain_layers, footprint_arrays, footprint_params, mixed_request, request_footprints, subset
+from map_helpers import CAP, ask, assert_same_cache, close_maps  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-CAP = 64
 BIG = 1 << 22   # max_checks that no request here reaches
 BAD_ARG = -1
 FILTER = ("traversability", "slope", "step", "elevation")
-
-
-@pytest.fixture(autouse=True)
-def _close_maps(ctx, monkeypatch):
-    """Every te_map a test opens is destroyed when it ends, failed or not, while the context still exists."""
-    made, real = [], ctx.map
-    monkeypatch.setattr(ctx, "map", lambda: made.append(real()) or made[-1])
-    yield
-    for m in made:
-        m.close()
 
 
 def _setup(te, oracle, rows=200, cols=180, res=0.02, seed=61):
@@ -36,12 +26,6 @@ def _setup(te, oracle, rows=200, cols=180, res=0.02, seed=61):
     og, g = oracle.Geometry.make(rows, cols, res), te.Geometry.make(rows, cols, res)
     L, rs = chain_layers(oracle, og, z, seed)
     return og, g, L, rs
-
-
-def _params(te, oracle, verify=0):
-    ft, fo = te.FootprintParams.yaml_defaults(), oracle.FootprintParams.yaml_defaults()
-    ft.verify_roughness = fo.verify_roughness = verify
-    return ft, fo
 
 
 def _twins(ctx, g, L, rough=None, robot_slope=None):
@@ -54,24 +38,8 @@ def _twins(ctx, g, L, rough=None, robot_slope=None):
     return out
 
 
-def _subset(R, idx):
-    b = R["begin"]
-    idx = np.asarray(idx, dtype=np.int64)
-    begin = np.concatenate([[0], np.cumsum(b[idx + 1] - b[idx])]).astype(np.int32)
-    poses = np.concatenate([R["poses"][b[q]:b[q + 1]] for q in idx]) if len(idx) else np.zeros((0, 7))
-    S = dict(begin=begin, poses=poses)
-    for k in ("radius", "kind", "cons", "cup", "map"):
-        if k in R:
-            S[k] = R[k][idx]
-    return S
-
-
 def _host(m, ft, R, fps, batched=False):
-    fb, fx = footprint_arrays(R, fps)
-    kw = dict(max_footprint_vertices=16, conservative=R["cons"], compute_untraversable_polygon=R["cup"], untraversable_capacity=CAP)
-    if batched:
-        return m.check_footprint_request_batched(ft, R["map"], R["begin"], R["poses"], R["radius"], fb, fx, **kw)
-    return m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, **kw)
+    return ask(m, ft, dict(R, fps=fps), R["map"] if batched else None)
 
 
 def _prepare(m, ft, R, fps, max_checks=BIG, batched=False, path_map=None, poses=None):
@@ -110,41 +78,26 @@ def _device(m, ft, R, fps, max_checks=BIG, batched=False, path_map=None, poses=N
     return fetch()
 
 
-def _same_out(got, want, what=""):
-    assert np.array_equal(got[0], want[0]), (what, np.nonzero(got[0] != want[0])[0][:10])
-    assert same(got[1], want[1]) and same(got[2], want[2]), what
-    same_polygons(got[3], got[4], want[3], want[4], what)
-
-
-def _same_cache(a, b, what="cache"):
-    equal = a.view(np.uint32) == b.view(np.uint32)
-    assert equal.all(), (what, int(np.sum(~equal)))
-
-
 def _both(H, D, ft, R, fps, batched=False, max_checks=BIG):
     """One request on the host twin and the device twin; asserts outputs, caches and request_stats are identical."""
     want = _host(H, ft, R, fps, batched)
     got = _device(D, ft, R, fps, max_checks, batched)
-    _same_out(got, want)
-    _same_cache(D.get_footprint(), H.get_footprint())
+    assert_same_answers(got, want)
+    assert_same_cache(D.get_footprint(), H.get_footprint())
     assert D.request_stats() == H.request_stats()
     return got
-
-
-def _repeat(R, idx):
-    return _subset(R, idx)
 
 
 @pytest.mark.parametrize("verify,slope", [(0, False), (1, True), (1, False), (0, True)])
 def test_request_sequence_equals_host(te, ctx, oracle, verify, slope):
     og, g, L, rs = _setup(te, oracle)
-    ft, fo = _params(te, oracle, verify)
+    ft, fo = footprint_params(te, oracle, verify)
     H, D = _twins(ctx, g, L, rough=L["roughness"], robot_slope=rs if slope else None)
     rng = np.random.default_rng(7 + verify)
     fps = request_footprints(rng)
     R1 = mixed_request(rng, og, 60, fps, circular=0.6, cap_path=False)
     R2 = mixed_request(rng, og, 80, fps, circular=0.7, planner=True, cap_path=False)
-    seq = (R1, _repeat(R1, rng.permutation(len(R1["kind"]))), R2, _repeat(R2, np.arange(len(R2["kind"])) // 2))
+    seq = (R1, subset(R1, rng.permutation(len(R1["kind"]))), R2, subset(R2, np.arange(len(R2["kind"])) // 2))
     cache = po.empty_cache(og)
     OL = dict(L, robot_slope=rs if slope else None)
     for k, R in enumerate(seq):
@@ -153,16 +106,15 @@ def test_request_sequence_equals_host(te, ctx, oracle, verify, slope):
             fb, fx = footprint_arrays(R, fps)
             want = po.check_request(og, fo, OL, R["begin"], R["poses"], R["radius"], fb, fx, conservative=R["cons"], cup=R["cup"],
                                     cache=cache, capacity=CAP)
-            _same_out(got, want, "oracle")
-            assert np.array_equal(D.get_footprint().view(np.uint32), cache.view(np.uint32)) or \
-                same(D.get_footprint().astype(np.float64), cache.astype(np.float64))
+            assert_same_answers(got, want, "oracle")
+            assert_same_cache(D.get_footprint(), cache, "oracle cache", nan_bits=False)
     cand, keys, stored = D.request_stats()
     assert 0 < keys <= cand and stored <= keys
 
 
 def test_annulus_blocker_revisit_and_single_poses_in_one_cell(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, seed=62)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     H, D = _twins(ctx, g, L)
     rng = np.random.default_rng(9)
     n = 600
@@ -185,7 +137,7 @@ def test_zero_mean_circle_then_fails(te, ctx, oracle):
     g = te.Geometry.make(rows, cols, 0.05)
     ones = np.ones((rows, cols), np.float32, order="F")
     L = dict(traversability=np.zeros((rows, cols), np.float32, order="F"), slope=ones, step=ones, elevation=0 * ones)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     H, D = _twins(ctx, g, L)
     poses = np.array([[0.1, 0.2, 0, 0, 0, 0, 1.0]] * 3)
     R = dict(begin=np.arange(4, dtype=np.int32), poses=poses, radius=np.full(3, 0.2), kind=np.full(3, -1), cons=np.zeros(3, np.uint8),
@@ -205,7 +157,7 @@ def test_back_and_forth_and_failures_across_windows(te, ctx, oracle):
     """A path that goes back and forth along one line (its own centres repeat inside a window), and many straight paths of every
     length through obstacles: failures land on every lane of a window, followed by paths over the failed paths' dropped cells."""
     og, g, L, rs = _setup(te, oracle, seed=64)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     H, D = _twins(ctx, g, L)
     rng = np.random.default_rng(21)
     paths = [np.concatenate([_line_path(og, -1.2, -0.3, 1.2, -0.3, 2), _line_path(og, 1.2, -0.3, -1.2, -0.3, 2),
@@ -221,8 +173,8 @@ def test_back_and_forth_and_failures_across_windows(te, ctx, oracle):
              cons=np.zeros(n, np.uint8), cup=(rng.random(n) < 0.5).astype(np.uint8))
     first = _both(H, D, ft, R, [])
     assert (first[0] == 0).sum() > 10 and (first[0] == 1).sum() > 10
-    _both(H, D, ft, _subset(R, rng.permutation(n)), [])
-    _both(H, D, ft, _subset(R, np.arange(n)[::-1]), [])
+    _both(H, D, ft, subset(R, rng.permutation(n)), [])
+    _both(H, D, ft, subset(R, np.arange(n)[::-1]), [])
 
 
 def test_batch_equals_host_batched(te, ctx, oracle):
@@ -233,7 +185,7 @@ def test_batch_equals_host_batched(te, ctx, oracle):
     H, D = ctx.map(), ctx.map()
     for m in (H, D):
         m.chain_batched(g, cp, nmaps, z)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     og = oracle.Geometry.make(rows, cols, res)
     rng = np.random.default_rng(23)
     fps = request_footprints(rng)
@@ -250,7 +202,7 @@ def test_batch_equals_host_batched(te, ctx, oracle):
 
 def test_unchecked_paths_in_device_memory(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, seed=65)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     rng = np.random.default_rng(25)
     fps = request_footprints(rng)
     R = mixed_request(rng, og, 60, fps, circular=0.8, cap_path=False)
@@ -263,7 +215,7 @@ def test_unchecked_paths_in_device_memory(te, ctx, oracle):
         parts.append(("ok", q))
     # the whole request: every good path, and a bad circular path at each of bad_at
     idx = [q for kind, q in parts if kind == "ok"]
-    good = _subset(R, idx)
+    good = subset(R, idx)
     B = dict(begin=[0], poses=[], radius=[], kind=[], cons=[], cup=[], map=[])
     bads = []
     for kind, q in parts:
@@ -290,16 +242,16 @@ def test_unchecked_paths_in_device_memory(te, ctx, oracle):
     got = _device(D, ft, B, fps, path_map=pm)
     want = _host(H, ft, good, fps)
     keep = np.setdiff1d(np.arange(len(B["kind"])), bads)
-    _same_out(tuple(a[keep] for a in got), want)
+    assert_same_answers(tuple(a[keep] for a in got), want)
     assert (got[0][bads] == 0).all() and np.isnan(got[1][bads]).all() and np.isnan(got[2][bads]).all()
     assert (got[3][bads] == -1).all()
-    _same_cache(D.get_footprint(), H.get_footprint())
+    assert_same_cache(D.get_footprint(), H.get_footprint())
     assert D.request_stats() == H.request_stats()
 
 
 def test_capacity_prefix(te, ctx, oracle):
     og, g, L, rs = _setup(te, oracle, seed=66)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     rng = np.random.default_rng(27)
     fps = request_footprints(rng)
     R = mixed_request(rng, og, 80, fps, circular=0.7, planner=True, cap_path=False)
@@ -320,9 +272,9 @@ def test_capacity_prefix(te, ctx, oracle):
         cut = circ[k:]
         assert (got[0][cut] == 0).all() and np.isnan(got[2][cut]).all() and (got[3][cut][R["cup"][cut] == 1] == -1).all()
         kept = np.sort(np.concatenate([poly, circ[:k]]))
-        want = _host(H, ft, _subset(R, kept), fps)
-        _same_out(tuple(a[kept] for a in got), want)
-        _same_cache(D.get_footprint(), H.get_footprint())
+        want = _host(H, ft, subset(R, kept), fps)
+        assert_same_answers(tuple(a[kept] for a in got), want)
+        assert_same_cache(D.get_footprint(), H.get_footprint())
         assert D.request_stats() == H.request_stats()
     assert seen_cut
 
@@ -347,18 +299,18 @@ def test_launches_fixed(te, ctx, oracle):
     """The same kernels, each launched once, for 1 and 1 000 paths and for 1 and 8 maps: none of the grids' counts depends on the
     request (a grid's size may)."""
     og, g, L, rs = _setup(te, oracle, seed=67)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     rng = np.random.default_rng(29)
     fps = request_footprints(rng)
     _, D = _twins(ctx, g, L)
     R = mixed_request(rng, og, 1000, [], circular=1.0, planner=True, cap_path=False)
-    k1, c1 = _kernels(ctx, D, ft, _subset(R, np.arange(1)), [])
+    k1, c1 = _kernels(ctx, D, ft, subset(R, np.arange(1)), [])
     k1000, c1000 = _kernels(ctx, D, ft, R, [])
     assert k1 == k1000 and c1 == c1000, (k1, k1000)
     assert any("k_req_replay" in k for k in k1) and any("k_map_eval_circles_dev" in k for k in k1)
     Rm = mixed_request(rng, og, 200, fps, circular=0.5, planner=True, cap_path=False)
     Rm["kind"][0], Rm["kind"][1] = -1, 0
-    assert _kernels(ctx, D, ft, _subset(Rm, np.arange(2)), fps) == _kernels(ctx, D, ft, Rm, fps)
+    assert _kernels(ctx, D, ft, subset(Rm, np.arange(2)), fps) == _kernels(ctx, D, ft, Rm, fps)
     B = ctx.map()
     z = np.stack([synth.terrain(64, 64, 0.02, 95 + k, "mixed") for k in range(8)])
     B.chain_batched(te.Geometry.make(64, 64, 0.02), te.ChainParams.yaml_defaults(0), 8, z)
@@ -375,7 +327,7 @@ def test_poses_outside_every_path(te, ctx, oracle):
     """Poses before path_begin[0] (the host entry accepts them) and after path_begin[npaths] (a preallocated pose buffer) belong
     to no path: the request equals the host entry's on the same path_begin."""
     og, g, L, rs = _setup(te, oracle, seed=70)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     rng = np.random.default_rng(33)
     fps = request_footprints(rng)
     H, D = _twins(ctx, g, L, robot_slope=rs)
@@ -386,8 +338,8 @@ def test_poses_outside_every_path(te, ctx, oracle):
         S = dict(R, begin=(R["begin"] + len(lead)).astype(np.int32), poses=np.concatenate([lead, R["poses"]]))
         want = _host(H, ft, S, fps)   # host memory: nposes = path_begin[npaths], the leading poses included
         got = _device(D, ft, S, fps, poses=np.concatenate([S["poses"], trail]))
-        _same_out(got, want)
-        _same_cache(D.get_footprint(), H.get_footprint())
+        assert_same_answers(got, want)
+        assert_same_cache(D.get_footprint(), H.get_footprint())
         assert D.request_stats() == H.request_stats()
 
 
@@ -404,7 +356,7 @@ def test_failure_at_window_lane_then_dropped_cells(te, ctx, oracle, lane):
     g = te.Geometry.make(n, n, res)
     ones = np.ones((n, n), np.float32, order="F")
     L = dict(traversability=np.full((n, n), 0.5, np.float32, order="F"), slope=ones, step=ones, elevation=0 * ones)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     H, D = _twins(ctx, g, L)
     pose = lambda i, j: [_cell(n, res, i), _cell(n, res, j), 0, 0, 0, 0, 1.0]  # noqa: E731
     out = [0.5 * n * res + 1.0, 0.0, 0, 0, 0, 0, 1.0]
@@ -430,7 +382,7 @@ def test_failure_at_window_lane_then_dropped_cells(te, ctx, oracle, lane):
 def test_graph_capture_replays_the_request(te, ctx, oracle):
     import torch
     og, g, L, rs = _setup(te, oracle, seed=68)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     rng = np.random.default_rng(31)
     fps = request_footprints(rng)
     R = mixed_request(rng, og, 60, fps, circular=0.7, cap_path=False)
@@ -466,14 +418,14 @@ def test_graph_capture_replays_the_request(te, ctx, oracle):
     finally:
         ctx.set_stream(None)
     got = tuple(out[k].cpu().numpy() for k in ("is_safe", "traversability_out", "area_out", "untraversable_count", "untraversable_xy"))
-    _same_out(got, want)
-    _same_cache(D.get_footprint(), H.get_footprint())
+    assert_same_answers(got, want)
+    assert_same_cache(D.get_footprint(), H.get_footprint())
 
 
 def test_synchronous_errors(te, ctx, oracle):
     import torch
     og, g, L, rs = _setup(te, oracle, rows=64, cols=64, seed=69)
-    ft, _ = _params(te, oracle)
+    ft, _ = footprint_params(te, oracle)
     L1 = ctx._L
     m = ctx.map()
     dv = lambda a, dt: torch.from_numpy(np.asarray(a, dtype=dt)).cuda()  # noqa: E731

@@ -9,12 +9,12 @@ import pytest
 
 import paths_oracle as po
 import synth
-from helpers import chain_layers, footprint_arrays, mixed_request, request_footprints, same, same_polygons
+from helpers import batch_request, bits, chain_layers, mixed_request, request_footprints, same
+from map_helpers import assert_batch_matches_singles, assert_same_held, close_maps, held  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 ROWS, COLS, RES, NMAPS = 200, 180, 0.02, 5
-CAP = 64
 BAD_ARG, MISSING_LAYER, UNSUPPORTED = -1, -2, -4
 FILTER = ("traversability", "slope", "step", "elevation")
 NAMES = {"traversability": "traversability", "traversability_slope": "slope", "traversability_step": "step",
@@ -34,104 +34,20 @@ def maps(te, oracle):
     return og, g, old, new
 
 
-@pytest.fixture(autouse=True)
-def _close_maps(ctx, monkeypatch):
-    """Every te_map a test opens is destroyed when it ends, failed or not, while the context still exists."""
-    made, real = [], ctx.map
-
-    def tracked():
-        made.append(real())
-        return made[-1]
-
-    monkeypatch.setattr(ctx, "map", tracked)
-    yield
-    for m in made:
-        m.close()
-
-
 def _stack(per, key, idx=None):
     return np.stack([per[k][key] for k in (range(len(per)) if idx is None else idx)])
 
 
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint32)
-
-
-def _held(m):
-    """Every layer the te_map holds, and its caches: (nmaps, rows, cols) arrays on a batch, (rows, cols) on one map."""
-    names = [n for n in NAMES if n not in ("traversability_roughness", "robot_slope")]
-    for opt in ("traversability_roughness", "robot_slope"):
-        try:
-            m.get_layers([opt])
-            names.append(opt)
-        except Exception:
-            pass
-    return dict(m.get_layers(names), cache=m.get_footprint())
-
-
-def _same_state(b, singles, what):
+def _same_state(te, b, singles, what):
     """B's layers and caches equal the single maps', map by map, bit for bit."""
-    hb = {n: v[None] if b.nmaps == 1 else v for n, v in _held(b).items()}
+    hb = {n: v[None] if b.nmaps == 1 else v for n, v in held(te, b).items()}
     for k, s in enumerate(singles):
-        hs = _held(s)
-        assert set(hs) == set(hb), (what, k)
-        for name in hs:
-            assert np.array_equal(_bits(hb[name][k]), _bits(hs[name])), (what, k, name)
+        assert_same_held({n: v[k] for n, v in hb.items()}, held(te, s), (what, k))
 
 
 def _request(rng, og, fps, npaths):
     """A mixed request whose paths visit every map in no order."""
-    R = mixed_request(rng, og, npaths, fps, circular=0.6, cap_path=False)
-    R["map"] = rng.integers(0, NMAPS, len(R["kind"])).astype(np.int32)
-    R["map"][:NMAPS] = rng.permutation(NMAPS)
-    return R
-
-
-def _subset(R, idx):
-    b = R["begin"]
-    begin = np.concatenate([[0], np.cumsum(b[idx + 1] - b[idx])]).astype(np.int32)
-    poses = np.concatenate([R["poses"][b[q]:b[q + 1]] for q in idx]) if len(idx) else np.zeros((0, 7))
-    return dict(begin=begin, poses=poses, **{k: R[k][idx] for k in ("radius", "kind", "cons", "cup", "map")})
-
-
-def _ask(m, ft, R, fps, batched):
-    fb, fx = footprint_arrays(R, fps)
-    kw = dict(max_footprint_vertices=16, conservative=R["cons"], compute_untraversable_polygon=R["cup"], untraversable_capacity=CAP)
-    if batched:
-        return m.check_footprint_request_batched(ft, R["map"], R["begin"], R["poses"], R["radius"], fb, fx, **kw)
-    return m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, **kw)
-
-
-def _both(b, singles, ft, R, fps, oracle_state=None):
-    """One request on the batch and, map by map, its paths on the single maps: answers, polygons and every cache identical.
-    oracle_state = (og, fo, per-map layers, per-map caches): each map's paths are also replayed on the CPU oracle."""
-    got = _ask(b, ft, R, fps, True)
-    n = len(R["kind"])
-    want = [np.zeros(n, np.uint8), np.zeros(n), np.zeros(n), np.zeros(n, np.int32), np.zeros((n, CAP, 2))]
-    for k, s in enumerate(singles):
-        idx = np.nonzero(R["map"] == k)[0]
-        if not len(idx):
-            continue
-        Rk = _subset(R, idx)
-        for o, v in zip(want, _ask(s, ft, Rk, fps, False)):
-            o[idx] = v
-        if oracle_state is not None:
-            og, fo, OL, caches = oracle_state
-            fb, fx = footprint_arrays(Rk, fps)
-            ref = po.check_request(og, fo, OL[k], Rk["begin"], Rk["poses"], Rk["radius"], fb, fx, conservative=Rk["cons"], cup=Rk["cup"],
-                                   cache=caches[k], capacity=CAP)
-            assert np.array_equal(got[0][idx], ref[0]) and same(got[1][idx], ref[1]) and same(got[2][idx], ref[2]), k
-            same_polygons(got[3][idx], got[4][idx], ref[3], ref[4], ("oracle polygons", k))
-    assert np.array_equal(got[0], want[0]), np.nonzero(got[0] != want[0])[0][:10]
-    assert same(got[1], want[1]) and same(got[2], want[2])
-    same_polygons(got[3], got[4], want[3], want[4], "polygons")
-    caches = b.get_footprint()
-    for k, s in enumerate(singles):
-        assert np.array_equal(_bits(caches[k]), _bits(s.get_footprint())), ("cache", k)
-        if oracle_state is not None:
-            oc = oracle_state[3][k]
-            assert ((_bits(caches[k]) == _bits(oc)) | (np.isnan(caches[k]) & np.isnan(oc))).all(), ("oracle cache", k)
-    return got
+    return batch_request(rng, og, npaths, NMAPS, fps, circular=0.6, cap_path=False)
 
 
 def _load_chain(ctx, te, g, elev):
@@ -185,8 +101,8 @@ def test_chain_maps_parity(te, ctx, oracle, maps, memory, outputs):
     b, singles = _load_chain(ctx, te, g, _stack(old, "elevation"))
     rng = np.random.default_rng(7)
     fps = request_footprints(rng)
-    _both(b, singles, ft, _request(rng, og, fps, 60), fps)   # caches and memos of every map in use
-    before = _held(b)
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 60))   # caches and memos of every map in use
+    before = held(te, b)
     sel = [3, 1]
     e = _stack(new, "elevation", sel)
     if memory == "host":
@@ -199,21 +115,21 @@ def test_chain_maps_parity(te, ctx, oracle, maps, memory, outputs):
     want = {k: np.empty((len(sel), COLS, ROWS), np.float32) for k in ("slope", "step", "roughness", "traversability")}
     ctx.chain_batched(g, p, len(sel), np.ascontiguousarray(e.transpose(0, 2, 1)), want["slope"], want["step"], want["roughness"],
                       want["traversability"], te.MEM_HOST)
-    after = _held(b)
+    after = held(te, b)
     for j, k in enumerate(sel):
         for name, key in NAMES.items():
             if key in want:
-                assert np.array_equal(_bits(after[name][k]), _bits(want[key][j].T)), (k, name)
+                assert np.array_equal(bits(after[name][k]), bits(want[key][j].T)), (k, name)
                 if outputs:
-                    assert np.array_equal(_bits(got[key][j]), _bits(want[key][j].T)), (k, key)
-        assert np.array_equal(_bits(after["elevation"][k]), _bits(e[j]))
+                    assert np.array_equal(bits(got[key][j]), bits(want[key][j].T)), (k, key)
+        assert np.array_equal(bits(after["elevation"][k]), bits(e[j]))
         assert np.isnan(after["cache"][k]).all()
     assert got is None or set(got) == set(want)
     for k in set(range(NMAPS)) - set(sel):   # the other maps keep every bit
         for name in before:
-            assert np.array_equal(_bits(after[name][k]), _bits(before[name][k])), (k, name)
-    _same_state(b, singles, "after chain_maps")
-    _both(b, singles, ft, _request(rng, og, fps, 60), fps)   # the kept memos and caches answer as the single maps do
+            assert np.array_equal(bits(after[name][k]), bits(before[name][k])), (k, name)
+    _same_state(te, b, singles, "after chain_maps")
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 60))   # the kept memos and caches answer as the single maps do
 
 
 @pytest.mark.parametrize("kind", ["chain", "slope"])
@@ -236,7 +152,7 @@ def test_interleaved_updates_equal_single_maps(te, ctx, oracle, maps, kind):
         state = (og, fo, OL, [po.empty_cache(og) for _ in singles])
     rng = np.random.default_rng(17 + slope)
     fps = request_footprints(rng)
-    _both(b, singles, ft, _request(rng, og, fps, 70), fps, state)
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 70), state)
 
     sel = [3, 1]
     if slope:
@@ -250,17 +166,17 @@ def test_interleaved_updates_equal_single_maps(te, ctx, oracle, maps, kind):
             singles[k].chain(g, p, new[k]["elevation"])
             state[2][k] = {NAMES[n]: v for n, v in singles[k].get_layers(list(NAMES)[:5]).items()}
             state[3][k] = po.empty_cache(og)
-    _same_state(b, singles, "after the update")
-    _both(b, singles, ft, _request(rng, og, fps, 70), fps, state)
+    _same_state(te, b, singles, "after the update")
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 70), state)
 
     fsel = [0, 3]
     swept = b.footprint_maps(ft, fsel)
     for j, k in enumerate(fsel):
-        assert np.array_equal(_bits(swept[j]), _bits(singles[k].footprint(ft))), ("footprint_maps", k)
+        assert np.array_equal(bits(swept[j]), bits(singles[k].footprint(ft))), ("footprint_maps", k)
         if state is not None:   # the oracle continues from the swept cache (the sweep's last bits are pinned in test_map_gpu)
             state[3][k] = np.asfortranarray(swept[j].copy())
-    _same_state(b, singles, "after footprint_maps")
-    _both(b, singles, ft, _request(rng, og, fps, 70), fps, state)
+    _same_state(te, b, singles, "after footprint_maps")
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 70), state)
 
     lay = {x: new[4][x] for x in FILTER + ("roughness", "robot_slope")}   # map 2 takes map 4's new terrain
     b.set_layers_maps(g, [2], *(lay[x][None] for x in FILTER), roughness=lay["roughness"][None],
@@ -269,15 +185,15 @@ def test_interleaved_updates_equal_single_maps(te, ctx, oracle, maps, kind):
     if state is not None:
         state[2][2] = {x: lay[x] for x in FILTER + ("roughness",)}
         state[3][2] = po.empty_cache(og)
-    _same_state(b, singles, "after set_layers_maps")
-    _both(b, singles, ft, _request(rng, og, fps, 70), fps, state)
+    _same_state(te, b, singles, "after set_layers_maps")
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 70), state)
     # the read side too: submaps and valid_at of every map
     pos, ln = rng.uniform([-1.5, -1.5], [1.5, 1.5], (NMAPS, 2)), np.full((NMAPS, 2), 0.8)
     got = b.get_submaps_batched(np.arange(NMAPS, dtype=np.int32), pos, ln, ["traversability", "elevation"])
     for k, s in enumerate(singles):
         want = s.get_submaps(pos[k:k + 1], ln[k:k + 1], ["traversability", "elevation"])[0]
         for n in ("traversability", "elevation"):
-            assert np.array_equal(_bits(got[k][1][n]), _bits(want[1][n])), (k, n)
+            assert np.array_equal(bits(got[k][1][n]), bits(want[1][n])), (k, n)
     xy = rng.uniform([-2.4, -2.2], [2.4, 2.2], (300, 2))
     pm = rng.integers(0, NMAPS, 300).astype(np.int32)
     want = np.zeros(300, np.uint8)
@@ -298,14 +214,14 @@ def test_stale_memo_would_show(te, ctx, oracle, maps):
     b, singles = _load_set(ctx, g, per, slope=False)
     rng = np.random.default_rng(23)
     R = mixed_request(rng, og, 120, [], circular=1.0, cap_path=False)
-    R["map"] = np.tile(np.array([0, 1], np.int32), 60)
-    first = _both(b, singles, ft, R, [])
+    R["map"], R["fps"] = np.tile(np.array([0, 1], np.int32), 60), []
+    first = assert_batch_matches_singles(b, singles, ft, R)
     kept = b.get_footprint()[0]
     blocked = {x: (new if x in ("slope", "step", "roughness") else per)[1][x] for x in FILTER + ("roughness",)}
     b.set_layers_maps(g, [1], *(blocked[x][None] for x in FILTER), roughness=blocked["roughness"][None])
     singles[1].set_layers(g, *(blocked[x] for x in FILTER), roughness=blocked["roughness"])
-    assert np.array_equal(_bits(b.get_footprint()[0]), _bits(kept)) and np.isnan(b.get_footprint()[1]).all()
-    again = _both(b, singles, ft, R, [])
+    assert np.array_equal(bits(b.get_footprint()[0]), bits(kept)) and np.isnan(b.get_footprint()[1]).all()
+    again = assert_batch_matches_singles(b, singles, ft, R)
     on1 = R["map"] == 1
     assert (again[0][on1] != first[0][on1]).any() or not same(again[1][on1], first[1][on1])
 
@@ -318,19 +234,19 @@ def test_whole_selection_and_one_map(te, ctx, oracle, maps):
     out = b.chain_maps(g, p, perm, _stack(new, "elevation", perm), outputs=True)
     ref = ctx.map()
     ref.chain_batched(g, p, NMAPS, _stack(new, "elevation"))
-    hb, hr = _held(b), _held(ref)
+    hb, hr = held(te, b), held(te, ref)
     for name in hr:
-        assert np.array_equal(_bits(hb[name]), _bits(hr[name])), name
+        assert np.array_equal(bits(hb[name]), bits(hr[name])), name
     for name, key in NAMES.items():
         if key in out:
-            assert np.array_equal(_bits(out[key]), _bits(hr[name][perm])), key
+            assert np.array_equal(bits(out[key]), bits(hr[name][perm])), key
     one, single = ctx.map(), ctx.map()
     one.chain(g, p, old[0]["elevation"])
     one.chain_maps(g, p, [0], new[0]["elevation"][None])
     single.chain(g, p, new[0]["elevation"])
-    _same_state(one, [single], "one map")
+    _same_state(te, one, [single], "one map")
     ft = te.FootprintParams.yaml_defaults()
-    assert np.array_equal(_bits(one.footprint_maps(ft, [0])[0]), _bits(single.footprint(ft)))
+    assert np.array_equal(bits(one.footprint_maps(ft, [0])[0]), bits(single.footprint(ft)))
 
 
 def test_device_memory_entries(te, ctx, oracle, maps):
@@ -344,7 +260,7 @@ def test_device_memory_entries(te, ctx, oracle, maps):
     b, singles = _load_set(ctx, g, old)
     rng = np.random.default_rng(29)
     fps = request_footprints(rng)
-    _both(b, singles, ft, _request(rng, og, fps, 40), fps)
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 40))
     sel = np.array([4, 0], np.int32)
     keys = ("traversability", "slope", "step", "roughness", "elevation", "robot_slope")
     dev = {k: torch.from_numpy(np.ascontiguousarray(_stack(new, k, sel).transpose(0, 2, 1))).cuda() for k in keys}
@@ -357,16 +273,16 @@ def test_device_memory_entries(te, ctx, oracle, maps):
     for k in sel:
         singles[k].set_layers(g, *(new[k][x] for x in FILTER), roughness=new[k]["roughness"], robot_slope=new[k]["robot_slope"])
     ctx.synchronize()
-    _same_state(b, singles, "set_layers_maps in device memory")
-    _both(b, singles, ft, _request(rng, og, fps, 40), fps)
+    _same_state(te, b, singles, "set_layers_maps in device memory")
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 40))
     fsel = np.array([1, 4, 2], np.int32)
     out = torch.full((len(fsel), COLS, ROWS), 7.0, dtype=torch.float32, device="cuda")
     assert L.te_map_footprint_maps(b._h, C.byref(ft), len(fsel), fsel.ctypes.data, out.data_ptr(), te.MEM_DEVICE) == 0
     ctx.synchronize()
     got = out.cpu().numpy()
     for j, k in enumerate(fsel):
-        assert np.array_equal(_bits(got[j].T), _bits(singles[k].footprint(ft))), k
-    _same_state(b, singles, "footprint_maps in device memory")
+        assert np.array_equal(bits(got[j].T), bits(singles[k].footprint(ft))), k
+    _same_state(te, b, singles, "footprint_maps in device memory")
 
 
 def test_page_locked_map_index_reused_at_once(te, ctx, oracle, maps):
@@ -378,7 +294,7 @@ def test_page_locked_map_index_reused_at_once(te, ctx, oracle, maps):
     L = te.load_library()
     b = ctx.map()
     b.chain_batched(g, p, NMAPS, _stack(old, "elevation"))
-    before = _held(b)
+    before = held(te, b)
     idx = torch.empty(2, dtype=torch.int32, pin_memory=True).numpy()
     idx[:] = [3, 1]
     e = torch.from_numpy(np.ascontiguousarray(_stack(new, "elevation", [3, 1]).transpose(0, 2, 1))).cuda()
@@ -389,14 +305,14 @@ def test_page_locked_map_index_reused_at_once(te, ctx, oracle, maps):
                                te.MEM_DEVICE) == 0
     idx[:] = [0, 2]   # the next update's maps
     ctx.synchronize()
-    after = _held(b)
+    after = held(te, b)
     for k in (0, 2, 4):
         for name in before:
             if name != "cache":   # the sweeps above filled every cache
-                assert np.array_equal(_bits(after[name][k]), _bits(before[name][k])), (k, name)
+                assert np.array_equal(bits(after[name][k]), bits(before[name][k])), (k, name)
         assert np.isfinite(after["cache"][k]).any(), k
     for k in (3, 1):
-        assert np.array_equal(_bits(after["elevation"][k]), _bits(new[k]["elevation"])), k
+        assert np.array_equal(bits(after["elevation"][k]), bits(new[k]["elevation"])), k
         assert np.isnan(after["cache"][k]).all(), k
 
 
@@ -417,8 +333,8 @@ def test_odd_cell_count(te, ctx):
                           roughness=lay["traversability_roughness"])
     swept = b.footprint_maps(ft, [1, 2])
     for j, k in enumerate([1, 2]):
-        assert np.array_equal(_bits(swept[j]), _bits(singles[k].footprint(ft))), k
-    _same_state(b, singles, "odd cell count")
+        assert np.array_equal(bits(swept[j]), bits(singles[k].footprint(ft))), k
+    _same_state(te, b, singles, "odd cell count")
 
 
 def test_launch_count_independent_of_nsel(te, ctx, oracle, maps):
@@ -447,18 +363,18 @@ def test_error_codes_leave_the_map_unchanged(te, ctx, oracle, maps):
     b, singles = _load_set(ctx, g, old, slope=False)
     rng = np.random.default_rng(3)
     fps = request_footprints(rng)
-    _both(b, singles, ft, _request(rng, og, fps, 20), fps)   # caches and memos in use
+    assert_batch_matches_singles(b, singles, ft, _request(rng, og, fps, 20))   # caches and memos in use
     e1 = _stack(new, "elevation", [0])
     lay1 = {x: _stack(new, x, [0]) for x in FILTER + ("roughness", "robot_slope")}
-    before = _held(b)
+    before = held(te, b)
 
     def expect(code, call):
         with pytest.raises(te.TEError) as e:
             call()
         assert e.value.code == code, (code, str(e.value))
-        after = _held(b)
+        after = held(te, b)
         for name in before:
-            assert np.array_equal(_bits(after[name]), _bits(before[name])), name
+            assert np.array_equal(bits(after[name]), bits(before[name])), name
 
     for idx in ([1, 1], [-1], [NMAPS], [], [0, 1, 2, 3, 4, 0]):
         n = max(len(idx), 1)
@@ -471,7 +387,7 @@ def test_error_codes_leave_the_map_unchanged(te, ctx, oracle, maps):
     for rc in (L.te_map_chain_maps(b._h, C.byref(g), C.byref(p), 1, None, e1.ctypes.data, None, None, None, None, te.MEM_HOST),
                L.te_map_footprint_maps(b._h, C.byref(ft), 1, None, None, te.MEM_HOST)):
         assert rc == BAD_ARG
-    assert np.array_equal(_bits(_held(b)["cache"]), _bits(before["cache"]))
+    assert np.array_equal(bits(held(te, b)["cache"]), bits(before["cache"]))
     # another geometry
     for gx in (te.Geometry.make(ROWS, COLS, RES, position=(0.5, 0.0)), te.Geometry.make(ROWS, COLS, 0.021)):
         expect(BAD_ARG, lambda: b.chain_maps(gx, p, [0], e1))
@@ -481,12 +397,12 @@ def test_error_codes_leave_the_map_unchanged(te, ctx, oracle, maps):
     expect(BAD_ARG, lambda: b.set_layers_maps(g, [0], *(lay1[x] for x in FILTER), roughness=lay1["roughness"],
                                               robot_slope=lay1["robot_slope"]))
     b = _load_set(ctx, g, old, slope=True)[0]
-    before = _held(b)
+    before = held(te, b)
     expect(UNSUPPORTED, lambda: b.chain_maps(g, p, [0], e1))
     expect(MISSING_LAYER, lambda: b.set_layers_maps(g, [0], *(lay1[x] for x in FILTER), roughness=lay1["roughness"]))
     b = ctx.map()
     b.set_layers_batched(g, NMAPS, *(_stack(old, x) for x in FILTER))
-    before = _held(b)
+    before = held(te, b)
     expect(UNSUPPORTED, lambda: b.chain_maps(g, p, [0], e1))
     # a te_map without layers
     empty = ctx.map()
@@ -501,6 +417,6 @@ def test_error_codes_leave_the_map_unchanged(te, ctx, oracle, maps):
     expect(UNSUPPORTED, lambda: b.chain_maps(gw, p, [0], e1))
     w = ctx.map()
     w.chain(gw, p, old[0]["elevation"])
-    b, before = w, _held(w)
+    b, before = w, held(te, w)
     expect(UNSUPPORTED, lambda: w.chain_maps(gw, p, [0], e1))
     expect(UNSUPPORTED, lambda: w.footprint_maps(ft, [0]))

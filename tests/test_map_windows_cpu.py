@@ -5,6 +5,7 @@ import numpy as np
 
 import submap_oracle as sub
 import windows_oracle as wo
+from helpers import bits
 
 N, RES = 8, 0.5
 SRC = np.asfortranarray(100.0 * np.arange(N)[:, None] + np.arange(N)[None, :], dtype=np.float32)
@@ -13,10 +14,6 @@ NAN = 0x7fc00000
 
 def _geo(oracle):
     return oracle.Geometry.make(N, N, RES)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
 
 
 def _expected(top, rows, cols):
@@ -40,7 +37,7 @@ def test_inside_window_is_getsubmaps(oracle):
     # the window's position is the submap's: top-left corner 1.75 - 0.5 * 2 + 0.25 = 1.0, minus half of 4 cells
     assert pos[0].tolist() == [0.0, 0.0] == [s["position_x"][0], s["position_y"][0]]
     cut = wo.cut(SRC, (0, 0), top[0], 4, 4)
-    assert np.array_equal(_bits(cut), _bits(SRC[2:6, 2:6]))
+    assert np.array_equal(bits(cut), bits(SRC[2:6, 2:6]))
 
 
 def test_top_left_one_cell_above_is_minus_one(oracle):
@@ -50,8 +47,8 @@ def test_top_left_one_cell_above_is_minus_one(oracle):
     assert top[0].tolist() == [-1, 3]
     assert pos[0, 0] == 1.5   # row -1's centre 2.25, its top edge 2.5, minus half of 2 m
     cut = wo.cut(SRC, (0, 0), top[0], 4, 4)
-    assert (_bits(cut[0]) == NAN).all()
-    assert np.array_equal(_bits(cut), _bits(_expected((-1, 3), 4, 4)))
+    assert (bits(cut[0]) == NAN).all()
+    assert np.array_equal(bits(cut), bits(_expected((-1, 3), 4, 4)))
     assert np.array_equal(cut[1:], SRC[0:3, 3:7])
 
 
@@ -61,12 +58,12 @@ def test_half_and_fully_outside_windows(oracle):
     top, _ = wo.window_geometry(g, 4, 4, [(-1.5, 1.6)])
     assert top[0].tolist() == [5, -2]
     cut = wo.cut(SRC, (0, 0), top[0], 4, 4)
-    assert np.array_equal(_bits(cut), _bits(_expected((5, -2), 4, 4)))
-    assert (_bits(cut[3]) == NAN).all() and (_bits(cut[:, :2]) == NAN).all() and np.array_equal(cut[:3, 2:], SRC[5:8, 0:2])
+    assert np.array_equal(bits(cut), bits(_expected((5, -2), 4, 4)))
+    assert (bits(cut[3]) == NAN).all() and (bits(cut[:, :2]) == NAN).all() and np.array_equal(cut[:3, 2:], SRC[5:8, 0:2])
     # far away on both axes, and on one: every cell is unknown
     for p in [(10.0, 10.0), (0.0, -7.0), (-3.25, 0.0)]:
         top, _ = wo.window_geometry(g, 4, 4, [p])
-        assert (_bits(wo.cut(SRC, (0, 0), top[0], 4, 4)) == NAN).all(), p
+        assert (bits(wo.cut(SRC, (0, 0), top[0], 4, 4)) == NAN).all(), p
 
 
 def test_start_index_wraps_rows_and_columns(oracle):
@@ -76,7 +73,7 @@ def test_start_index_wraps_rows_and_columns(oracle):
     # rows 3..6 are stored at 6, 7, 0, 1 and columns 1..5 at 6, 7, 0, 1, 2: both wrap inside the window
     for top in [(3, 1), (-2, 4), (6, -1), (0, 0)]:
         got = wo.cut(stored, start, top, 4, 5)
-        assert np.array_equal(_bits(got), _bits(_expected(top, 4, 5))), top
+        assert np.array_equal(bits(got), bits(_expected(top, 4, 5))), top
 
 
 def test_position_on_a_cell_edge(oracle):

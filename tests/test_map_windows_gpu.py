@@ -11,7 +11,8 @@ import pytest
 import submap_oracle as so
 import synth
 import windows_oracle as wo
-from helpers import footprint_arrays, mixed_request, request_footprints
+from helpers import assert_same_bits, batch_request, noisy, same_bytes
+from map_helpers import ask, assert_same_held, close_maps, held  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -22,35 +23,6 @@ RAW = ("elevation", "variance", "horizontal_variance_x", "horizontal_variance_y"
 BAD_ARG, MISSING_LAYER, UNSUPPORTED = -1, -2, -4
 
 
-@pytest.fixture(autouse=True)
-def _close_maps(ctx, monkeypatch):
-    """Every te_map a test opens is destroyed when it ends, failed or not, while the context still exists."""
-    made, real = [], ctx.map
-    monkeypatch.setattr(ctx, "map", lambda: made.append(real()) or made[-1])
-    yield
-    for m in made:
-        m.close()
-
-
-def _bits(a):
-    return np.ascontiguousarray(np.asarray(a, dtype=np.float32)).view(np.uint32)
-
-
-def _same(a, b, what=""):
-    assert np.array_equal(_bits(a), _bits(b)), what
-
-
-def _noisy(rng, shape):
-    """float32 layer with NaN (several payloads), +-Inf and exact zeros."""
-    a = (rng.standard_normal(shape) * 3).astype(np.float32)
-    a[rng.random(shape) < 0.03] = np.nan
-    a[rng.random(shape) < 0.01] = np.inf
-    a[rng.random(shape) < 0.01] = 0.0
-    odd = rng.random(shape) < 0.01
-    a.view(np.uint32)[odd] = (rng.integers(0, 2, odd.sum()) << 31 | 0x7f800000 | rng.integers(1, 1 << 23, odd.sum())).astype(np.uint32)
-    return a
-
-
 @pytest.fixture(scope="module")
 def source(te, oracle):
     """The elevation map: every layer unwrapped (cell (i, j) at [i, j]) and as its circular buffer stores it."""
@@ -58,7 +30,7 @@ def source(te, oracle):
     z = synth.terrain(SRC_ROWS, SRC_COLS, RES, 31, "mixed").astype(np.float32)
     lay = {"elevation": z}
     for n in FUSED[1:] + RAW[1:]:
-        lay[n] = _noisy(rng, (SRC_ROWS, SRC_COLS))
+        lay[n] = noisy(rng, (SRC_ROWS, SRC_COLS), nan=0.03, inf=0.01, ninf=0, zero=0.01)
     stored = {n: np.asfortranarray(np.roll(a, SRC_START, axis=(0, 1))) for n, a in lay.items()}
     g = te.Geometry.make(SRC_ROWS, SRC_COLS, RES, SRC_POS)
     g.start_row, g.start_col = SRC_START
@@ -77,50 +49,24 @@ def _cut(source, name, top, rows, cols):
 
 
 def _held(te, m):
-    """Every layer the te_map holds, its cache and its positions."""
-    names = []
-    for n in te.capi.LAYERS[:6] + te.capi.CARRIED_LAYERS + te.capi.POLYGON_LAYERS:
-        try:
-            m.get_layers([n])
-            names.append(n)
-        except te.TEError as e:
-            assert e.code == MISSING_LAYER
-    return dict(m.get_layers(names), cache=m.get_footprint(), positions=m.positions())
-
-
-def _same_held(a, b, what=""):
-    assert set(a) == set(b), (what, sorted(set(a) ^ set(b)))
-    for n in a:
-        if n == "positions":
-            assert np.array_equal(a[n], b[n]), what
-        else:
-            _same(a[n], b[n], (what, n))
+    return held(te, m, polygon=True, positions=True)
 
 
 def _request(rng, g, positions, npaths, batched):
-    fps = request_footprints(rng)
-    R = mixed_request(rng, g, npaths, fps, circular=0.6, cap_path=False)
-    R["fps"] = fps
-    n = len(positions)
-    R["map"] = rng.integers(0, n, len(R["kind"])).astype(np.int32)
-    for q, k in enumerate(R["map"]):
-        R["poses"][R["begin"][q]:R["begin"][q + 1], :2] += positions[k] - (g.position_x, g.position_y)
+    """A mixed request whose paths visit the maps at `positions` in no order, each around its own map's position."""
+    R = batch_request(rng, g, npaths, len(positions), offsets=np.asarray(positions) - (g.position_x, g.position_y), permute=False,
+                      circular=0.6, cap_path=False)
     R["batched"] = batched
     return R
 
 
 def _ask(m, te, R):
-    ft = te.FootprintParams.yaml_defaults()
-    fb, fx = footprint_arrays(R, R["fps"])
-    kw = dict(max_footprint_vertices=16, conservative=R["cons"], compute_untraversable_polygon=R["cup"], untraversable_capacity=64)
-    if not R["batched"]:
-        return m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, **kw)
-    return m.check_footprint_request_batched(ft, R["map"], R["begin"], R["poses"], R["radius"], fb, fx, **kw)
+    return ask(m, te.FootprintParams.yaml_defaults(), R, R["map"] if R["batched"] else None)
 
 
 def _same_answers(a, b, what=""):
     for k, (x, y) in enumerate(zip(a, b)):
-        assert np.array_equal(np.asarray(x).view(np.uint8), np.asarray(y).view(np.uint8)), (what, k)
+        assert same_bytes(x, y), (what, k)
 
 
 # ---- 1. a single map: the node's update ----------------------------------------------------------------------------------------
@@ -155,15 +101,15 @@ def test_chain_submap_equals_cut_chain_carry(te, ctx, source, names, memory):
         r = ctx.map()
         r.chain(gs, source["p"], _cut(source, "elevation", top, info.rows, info.cols))
         r.carry_layers(names[1:], [_cut(source, n, top, info.rows, info.cols) for n in names[1:]])
-        _same_held(_held(te, m), _held(te, r), what)
+        assert_same_held(_held(te, m), _held(te, r), what)
         R = _request(rng, gs, np.array([[gs.position_x, gs.position_y]]), 40, False)
         _same_answers(_ask(m, te, R), _ask(r, te, R), what)
-        _same_held(_held(te, m), _held(te, r), (what, "after the request"))
+        assert_same_held(_held(te, m), _held(te, r), (what, "after the request"))
     # a failing getSubmap: info says so, the call refuses and the map is as it was
     before = _held(te, m)
     info = m.chain_submap(source["g"], lay, (500.0, 0.0), (4.0, 4.0), source["p"], memory=memory)
     assert info.success == 0 and info.rows == 0
-    _same_held(_held(te, m), before, "failed getSubmap")
+    assert_same_held(_held(te, m), before, "failed getSubmap")
 
 
 # ---- 2. a batch: a fleet cut out of one map --------------------------------------------------------------------------------------
@@ -220,12 +166,12 @@ def test_chain_windows_batch(te, ctx, source, kernel, memory):
     r.chain_batched(g, source["p"], NB, cuts["elevation"], positions=at)
     r.carry_layers(FUSED[1:], [cuts[n] for n in FUSED[1:]])
     assert np.array_equal(m.positions(), at)
-    _same_held(_held(te, m), _held(te, r), kernel)
+    assert_same_held(_held(te, m), _held(te, r), kernel)
     ft = te.FootprintParams.yaml_defaults()
-    _same(m.footprint(ft), r.footprint(ft), (kernel, "sweep"))
+    assert_same_bits(m.footprint(ft), r.footprint(ft), (kernel, "sweep"))
     R = _request(rng, g, at, 200, True)
     _same_answers(_ask(m, te, R), _ask(r, te, R), kernel)
-    _same_held(_held(te, m), _held(te, r), (kernel, "after the request"))
+    assert_same_held(_held(te, m), _held(te, r), (kernel, "after the request"))
 
 
 def test_windows_agree_with_getsubmap(te, ctx, source):
@@ -253,7 +199,7 @@ def test_windows_agree_with_getsubmap(te, ctx, source):
         assert top[k].tolist() == [ref["top_row"][k], ref["top_col"][k]] == [lib["top_row"][k], lib["top_col"][k]], k
         assert at[k].tolist() == [ref["position_x"][k], ref["position_y"][k]] == got_pos[k].tolist(), k
         block = source["lay"]["elevation"][top[k][0]:top[k][0] + n, top[k][1]:top[k][1] + mcols]
-        _same(elev[k], block, k)
+        assert_same_bits(elev[k], block, k)
     assert matched >= 8, matched
 
 
@@ -273,7 +219,7 @@ def test_chain_windows_selection(te, ctx, source):
     r.chain_batched(g, source["p"], NS, cuts["elevation"], positions=at)
     r.carry_layers(held[1:], [cuts[n] for n in held[1:]])
     ft = te.FootprintParams.yaml_defaults()
-    _same(m.footprint(ft), r.footprint(ft))   # fills the caches, which the unselected maps must keep
+    assert_same_bits(m.footprint(ft), r.footprint(ft))   # fills the caches, which the unselected maps must keep
     R0 = _request(rng, g, at, 60, True)
     _same_answers(_ask(m, te, R0), _ask(r, te, R0))   # and the memo
     for rnd, given in enumerate([("elevation", "upper_bound", "lower_bound"), ("elevation", "lower_bound"), ("elevation",)]):
@@ -285,18 +231,18 @@ def test_chain_windows_selection(te, ctx, source):
         if len(given) > 1:
             r.carry_layers(given[1:], [sc[n] for n in given[1:]], map_index=idx)
         hm, hr = _held(te, m), _held(te, r)
-        _same_held(hm, hr, rnd)
+        assert_same_held(hm, hr, rnd)
         for n in set(held) - set(given):   # held but not given: NaN on the selected maps
             assert np.isnan(hm[n][idx]).all(), (rnd, n)
         R = _request(rng, g, hr["positions"], 60, True)
         _same_answers(_ask(m, te, R), _ask(r, te, R), rnd)
-        _same_held(_held(te, m), _held(te, r), (rnd, "after the request"))
+        assert_same_held(_held(te, m), _held(te, r), (rnd, "after the request"))
     # a carried layer the batch does not hold
     before = _held(te, m)
     with pytest.raises(te.TEError) as e:
         m.chain_windows(g, source["g"], _layers(source, ("elevation", "variance"), 0), pos[:2], source["p"], map_index=[0, 1])
     assert e.value.code == BAD_ARG
-    _same_held(_held(te, m), before, "not held")
+    assert_same_held(_held(te, m), before, "not held")
 
 
 # ---- 4. launches -----------------------------------------------------------------------------------------------------------------
@@ -399,9 +345,9 @@ def test_error_table(te, ctx, source):
     before = _held(te, m)
     for what, call, code in cases:
         assert call() == code, (what, L.te_last_error())
-        _same_held(_held(te, m), before, what)
+        assert_same_held(_held(te, m), before, what)
     # the robot_slope refusal of the _maps entries
     m.carry_layers(["robot_slope"], [np.zeros((NS, NB_ROWS, NB_COLS), np.float32)])
     before = _held(te, m)
     assert win(index=idx) == UNSUPPORTED, L.te_last_error()
-    _same_held(_held(te, m), before, "robot_slope")
+    assert_same_held(_held(te, m), before, "robot_slope")

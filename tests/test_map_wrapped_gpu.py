@@ -9,7 +9,8 @@ import numpy as np
 import pytest
 
 import synth
-from helpers import footprint_arrays, mixed_request, request_footprints
+from helpers import batch_request, bits, same_bytes, subset, unwrap, wrap
+from map_helpers import ask, close_maps, held  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -23,24 +24,6 @@ POLY = [(0.11, 0.07), (-0.1, 0.09), (-0.12, -0.08), (0.1, -0.1)]
 YAWS = [0.0, 0.4, 1.3, 2.9]
 START = np.array([(0, 0), (ROWS - 1, 0), (0, COLS - 1), (37, 53), (64, 1), (5, 100)], np.int32)
 POS = np.array([(0.0, 0.0), (13.37, -3.21), (-101.23, 77.7), (0.31, 0.05), (250.125, 512.39), (-7.77, 0.05)])
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, dtype=np.float32).view(np.uint32)
-
-
-def _same(a, b):
-    a, b = np.asarray(a), np.asarray(b)
-    return a.shape == b.shape and np.array_equal(np.ascontiguousarray(a).view(np.uint8), np.ascontiguousarray(b).view(np.uint8))
-
-
-def _wrap(a, st):
-    """A default-order (rows, cols) layer stored in the buffer order of start index st: cell (i, j) at ((i + sr) % rows, (j + sc) % cols)."""
-    return np.roll(a, (int(st[0]), int(st[1])), axis=(0, 1))
-
-
-def _unwrap(a, st):
-    return np.roll(a, (-int(st[0]), -int(st[1])), axis=(0, 1))
 
 
 def _geo(te, k, start=None):
@@ -60,30 +43,17 @@ def world(te):
     for a, s in ((up, 0), (lo, 1)):
         cells = rng.integers(0, z.size, 200)
         a.reshape(-1)[cells] = payload[(np.arange(200) + s) % 3]
-    wrap = lambda a: np.stack([_wrap(a[k], START[k]) for k in range(NMAPS)])  # noqa: E731
-    return dict(p=te.ChainParams.yaml_defaults(0), g=te.Geometry.make(ROWS, COLS, RES), z=z, up=up, lo=lo, zs=wrap(z), ups=wrap(up),
-                los=wrap(lo))
+    buffered = lambda a: np.stack([wrap(a[k], START[k]) for k in range(NMAPS)])  # noqa: E731
+    return dict(p=te.ChainParams.yaml_defaults(0), g=te.Geometry.make(ROWS, COLS, RES), z=z, up=up, lo=lo, zs=buffered(z),
+                ups=buffered(up), los=buffered(lo))
 
 
-@pytest.fixture
-def maps(ctx):
-    made = []
-
-    def new():
-        made.append(ctx.map())
-        return made[-1]
-
-    yield new
-    for m in made:
-        m.close()
-
-
-def _single(maps, te, world, k, z=None, start=None):
+def _single(ctx, te, world, k, z=None, start=None):
     """The oracle of map k: te_map_chain in host memory at map k's position with its start index in g, then its bounds carried."""
     st = START[k] if start is None else start
-    s = maps()
-    out = s.chain(_geo(te, k, st), world["p"], _wrap(world["z"][k], st) if z is None else _wrap(z, st), outputs=True)
-    s.carry_layers(BOUNDS, [_wrap(world["up"][k], st), _wrap(world["lo"][k], st)])
+    s = ctx.map()
+    out = s.chain(_geo(te, k, st), world["p"], wrap(world["z"][k], st) if z is None else wrap(z, st), outputs=True)
+    s.carry_layers(BOUNDS, [wrap(world["up"][k], st), wrap(world["lo"][k], st)])
     return s, out
 
 
@@ -115,71 +85,45 @@ def _load(b, te, ctx, world, memory, outputs=True):
     return {k: o.cpu().numpy().reshape(NMAPS, COLS, ROWS).transpose(0, 2, 1) for k, o in zip(CHAIN, outs)}
 
 
-def _held(m):
-    return dict(m.get_layers(list(PUBLISHED)), cache=m.get_footprint())
-
-
-def _check_held(b, singles, idx=None, what=""):
-    hb = _held(b)
+def _check_held(te, b, singles, idx=None, what=""):
+    hb = held(te, b, PUBLISHED)
     for k, s in zip(range(NMAPS) if idx is None else idx, singles):
-        hs = _held(s)
+        hs = held(te, s, PUBLISHED)
         for name in hs:
-            assert np.array_equal(_bits(hb[name][k]), _bits(hs[name])), (what, k, name)
+            assert np.array_equal(bits(hb[name][k]), bits(hs[name])), (what, k, name)
 
 
 def _request(rng, world, npaths):
     """A mixed request whose paths visit every map in no order, each around its own map's position."""
-    fps = request_footprints(rng)
-    R = mixed_request(rng, world["g"], npaths, fps, circular=0.6, cap_path=False)
-    R["fps"] = fps
-    R["map"] = rng.integers(0, NMAPS, len(R["kind"])).astype(np.int32)
-    R["map"][:NMAPS] = rng.permutation(NMAPS)
-    for q, m in enumerate(R["map"]):
-        R["poses"][R["begin"][q]:R["begin"][q + 1], :2] += POS[m]
-    return R
-
-
-def _subset(R, idx):
-    b = R["begin"]
-    begin = np.concatenate([[0], np.cumsum(b[idx + 1] - b[idx])]).astype(np.int32)
-    poses = np.concatenate([R["poses"][b[q]:b[q + 1]] for q in idx]) if len(idx) else np.zeros((0, 7))
-    return dict(begin=begin, poses=poses, fps=R["fps"], **{k: R[k][idx] for k in ("radius", "kind", "cons", "cup", "map")})
-
-
-def _ask(m, ft, R, path_map=None):
-    fb, fx = footprint_arrays(R, R["fps"])
-    kw = dict(max_footprint_vertices=16, conservative=R["cons"], compute_untraversable_polygon=R["cup"], untraversable_capacity=64)
-    if path_map is None:
-        return m.check_footprint_request(ft, R["begin"], R["poses"], R["radius"], fb, fx, **kw)
-    return m.check_footprint_request_batched(ft, path_map, R["begin"], R["poses"], R["radius"], fb, fx, **kw)
+    return batch_request(rng, world["g"], npaths, NMAPS, offsets=POS, circular=0.6, cap_path=False)
 
 
 def _check_request(b, singles, ft, R):
-    got = _ask(b, ft, R, R["map"])
+    got = ask(b, ft, R, R["map"])
     for m in range(NMAPS):
         idx = np.nonzero(R["map"] == m)[0]
-        want = _ask(singles[m], ft, _subset(R, idx))
+        want = ask(singles[m], ft, subset(R, idx))
         for a, w, name in zip(got, want, ("is_safe", "traversability", "area", "count")):
-            assert _same(np.asarray(a)[idx], w), (m, name)
+            assert same_bytes(np.asarray(a)[idx], w), (m, name)
         for j, q in enumerate(idx):
             k = max(0, min(int(want[3][j]), 64))
-            assert _same(np.asarray(got[4])[q, :k], want[4][j, :k]), (m, q)
+            assert same_bytes(np.asarray(got[4])[q, :k], want[4][j, :k]), (m, q)
 
 
 @pytest.mark.parametrize("memory", ["host", "device"])
-def test_whole_batch_equals_single_maps(maps, te, ctx, world, memory):
+def test_whole_batch_equals_single_maps(te, ctx, world, memory):
     torch = pytest.importorskip("torch")
     mem = te.MEM_HOST if memory == "host" else te.MEM_DEVICE
     ft = te.FootprintParams.yaml_defaults()
-    b = maps()
+    b = ctx.map()
     got = _load(b, te, ctx, world, mem)
     assert np.array_equal(b.start_indices(), START) and np.array_equal(b.positions(), POS)
-    singles, outs = zip(*(_single(maps, te, world, k) for k in range(NMAPS)))
+    singles, outs = zip(*(_single(ctx, te, world, k) for k in range(NMAPS)))
     for k in range(NMAPS):   # chain outputs: host ones in the map's buffer order, device ones in default order
         for name in CHAIN:
-            want = outs[k][name] if mem == te.MEM_HOST else _unwrap(outs[k][name], START[k])
-            assert np.array_equal(_bits(got[name][k]), _bits(want)), (memory, k, name)
-    _check_held(b, singles, what=memory)
+            want = outs[k][name] if mem == te.MEM_HOST else unwrap(outs[k][name], START[k])
+            assert np.array_equal(bits(got[name][k]), bits(want)), (memory, k, name)
+    _check_held(te, b, singles, what=memory)
     # device reads of the published layers are in default order
     dout = torch.empty(len(PUBLISHED) * NMAPS * ROWS * COLS, dtype=torch.float32, device="cuda")
     dl = b.get_layers(list(PUBLISHED), out=dout, memory=te.MEM_DEVICE)
@@ -187,44 +131,44 @@ def test_whole_batch_equals_single_maps(maps, te, ctx, world, memory):
     for k, s in enumerate(singles):
         hs = s.get_layers(list(PUBLISHED))
         for name in PUBLISHED:
-            assert np.array_equal(_bits(dl[name][k].cpu().numpy()), _bits(_unwrap(hs[name], START[k]))), (memory, k, name)
+            assert np.array_equal(bits(dl[name][k].cpu().numpy()), bits(unwrap(hs[name], START[k]))), (memory, k, name)
     # the circular sweep, then the cache read back in both memories
     cache = b.footprint(ft)
     for k, s in enumerate(singles):
-        assert np.array_equal(_bits(cache[k]), _bits(s.footprint(ft))), k
+        assert np.array_equal(bits(cache[k]), bits(s.footprint(ft))), k
     dc = torch.empty(NMAPS * ROWS * COLS, dtype=torch.float32, device="cuda")
     b._check(b._L.te_map_get_footprint(b._h, dc.data_ptr(), te.MEM_DEVICE))
     ctx.synchronize()
     dc = dc.cpu().numpy().reshape(NMAPS, COLS, ROWS).transpose(0, 2, 1)
     for k, s in enumerate(singles):
-        assert np.array_equal(_bits(dc[k]), _bits(_unwrap(s.get_footprint(), START[k]))), k
+        assert np.array_equal(bits(dc[k]), bits(unwrap(s.get_footprint(), START[k]))), k
     # the polygon sweeps, a list of yaws and its reduction (best_yaw included)
     bx, brot = b.footprint_polygon(ft, POLY, 0.7)
     stack = b.footprint_polygon_yaws(ft, POLY, YAWS)
     worst, best, best_yaw = b.footprint_polygon_yaws_reduce(ft, POLY, YAWS)
     for k, s in enumerate(singles):
         sx, srot = s.footprint_polygon(ft, POLY, 0.7)
-        assert np.array_equal(_bits(bx[k]), _bits(sx)) and np.array_equal(_bits(brot[k]), _bits(srot)), k
+        assert np.array_equal(bits(bx[k]), bits(sx)) and np.array_equal(bits(brot[k]), bits(srot)), k
         sstack = s.footprint_polygon_yaws(ft, POLY, YAWS)
         for y in range(len(YAWS)):
-            assert np.array_equal(_bits(stack[y, k]), _bits(sstack[y])), (k, y)
+            assert np.array_equal(bits(stack[y, k]), bits(sstack[y])), (k, y)
         sw, sb, sy = s.footprint_polygon_yaws_reduce(ft, POLY, YAWS)
-        assert np.array_equal(_bits(worst[k]), _bits(sw)) and np.array_equal(_bits(best[k]), _bits(sb)), k
+        assert np.array_equal(bits(worst[k]), bits(sw)) and np.array_equal(bits(best[k]), bits(sb)), k
         assert np.array_equal(best_yaw[k], sy), k
     # the kept polygon layers, each map at its own yaw
     yk = np.linspace(0.2, 2.7, NMAPS)
     kx, krot = b.footprint_polygon_keep(ft, POLY, yk, outputs=True)
     for k, s in enumerate(singles):
         sx, srot = s.footprint_polygon_keep(ft, POLY, [yk[k]], outputs=True)
-        assert np.array_equal(_bits(kx[k]), _bits(sx)) and np.array_equal(_bits(krot[k]), _bits(srot)), k
+        assert np.array_equal(bits(kx[k]), bits(sx)) and np.array_equal(bits(krot[k]), bits(srot)), k
     kept = b.get_layers(["traversability_x", "traversability_rot"])
     for k, s in enumerate(singles):
         sk = s.get_layers(["traversability_x", "traversability_rot"])
         for name in sk:
-            assert np.array_equal(_bits(kept[name][k]), _bits(sk[name])), (k, name)
+            assert np.array_equal(bits(kept[name][k]), bits(sk[name])), (k, name)
     # a mixed request with untraversable polygons, on caches the sweep filled
     _check_request(b, singles, ft, _request(np.random.default_rng(17), world, 40))
-    _check_held(b, singles, what=f"{memory} after request")
+    _check_held(te, b, singles, what=f"{memory} after request")
     # submaps, valid_at and at_poses depend on positions only
     rng = np.random.default_rng(5)
     n = 36
@@ -245,7 +189,7 @@ def test_whole_batch_equals_single_maps(maps, te, ctx, world, memory):
             assert np.float64(gi[f]).tobytes() == np.float64(ri[f]).tobytes(), (q, f)
         if rl is not None:
             for name in names:
-                assert np.array_equal(_bits(gl[name]), _bits(rl[name])), (q, name)
+                assert np.array_equal(bits(gl[name]), bits(rl[name])), (q, name)
         assert valid[q] == s.valid_at(xy[q:q + 1])[0], q
     poses = np.zeros((n, 7))
     poses[:, :2] = xy
@@ -256,7 +200,7 @@ def test_whole_batch_equals_single_maps(maps, te, ctx, world, memory):
         sl, sok = singles[wmap[q]].at_poses(poses[q:q + 1], points, ["traversability", "uncertainty_range"])
         assert np.array_equal(ok[q], sok[0]), q
         for name in sl:
-            assert np.array_equal(_bits(lay[name][q]), _bits(sl[name][0])), (q, name)
+            assert np.array_equal(bits(lay[name][q]), bits(sl[name][0])), (q, name)
 
 
 def _set_layers_args(out, world, wrapped):
@@ -264,14 +208,14 @@ def _set_layers_args(out, world, wrapped):
     return (out["traversability"], out["slope"], out["step"], z), dict(roughness=out["roughness"])
 
 
-def test_null_or_zero_start_index_is_the_at_entry(maps, te, world):
+def test_null_or_zero_start_index_is_the_at_entry(te, world, ctx):
     """Every _wrapped entry with start_index NULL or all (0, 0) gives the bytes of its _at entry."""
     p, g = world["p"], world["g"]
     ft = te.FootprintParams.yaml_defaults()
     zero = np.zeros((NMAPS, 2), np.int32)
-    held, outs = [], []
+    snaps, outs = [], []
     for mode in ("at", "zero", "null"):
-        m = maps()
+        m = ctx.map()
         if mode == "null":
             e = m._batch_layers(world["z"])
             o = {k: np.empty((NMAPS, COLS, ROWS), np.float32) for k in CHAIN}
@@ -284,17 +228,17 @@ def test_null_or_zero_start_index_is_the_at_entry(maps, te, world):
             o = m.chain_batched(g, p, NMAPS, world["z"], outputs=True, positions=POS, start_index=zero if mode == "zero" else None)
         m.footprint(ft)
         outs.append(o)
-        held.append(_held_core(m))
-    for h, o in zip(held[1:], outs[1:]):
+        snaps.append(_held_core(m))
+    for h, o in zip(snaps[1:], outs[1:]):
         for name in h:
-            assert np.array_equal(_bits(h[name]), _bits(held[0][name])), name
+            assert np.array_equal(bits(h[name]), bits(snaps[0][name])), name
         for name in CHAIN:
-            assert np.array_equal(_bits(o[name]), _bits(outs[0][name])), name
+            assert np.array_equal(bits(o[name]), bits(outs[0][name])), name
     # set_layers_batched and the two selection entries
     ref = outs[0]
-    held = []
+    snaps = []
     for mode in ("at", "zero"):
-        m = maps()
+        m = ctx.map()
         args, kw = _set_layers_args(ref, world, False)
         m.set_layers_batched(g, NMAPS, *args, positions=POS, start_index=zero if mode == "zero" else None, **kw)
         z2 = np.stack([synth.terrain(ROWS, COLS, RES, 950 + k, "rough") for k in range(2)]).astype(np.float32)
@@ -302,61 +246,61 @@ def test_null_or_zero_start_index_is_the_at_entry(maps, te, world):
         m.set_layers_maps(g, [2], *(a[:1] for a in args), roughness=kw["roughness"][:1], positions=POS[5:6],
                           start_index=zero[:1] if mode == "zero" else None)
         m.footprint(ft)
-        held.append(_held_core(m))
-    for name in held[1]:
-        assert np.array_equal(_bits(held[1][name]), _bits(held[0][name])), name
+        snaps.append(_held_core(m))
+    for name in snaps[1]:
+        assert np.array_equal(bits(snaps[1][name]), bits(snaps[0][name])), name
 
 
 def _held_core(m):
     return dict(m.get_layers(list(HELD)), cache=m.get_footprint())
 
 
-def test_selections(maps, te, world):
+def test_selections(te, world, ctx):
     p, g = world["p"], world["g"]
     ft = te.FootprintParams.yaml_defaults()
-    b = maps()
+    b = ctx.map()
     _load(b, te, None, world, te.MEM_HOST, outputs=False)
-    singles = [_single(maps, te, world, k)[0] for k in range(NMAPS)]
+    singles = [_single(ctx, te, world, k)[0] for k in range(NMAPS)]
     b.footprint(ft)
     for s in singles:
         s.footprint(ft)
     rng = np.random.default_rng(23)
     _check_request(b, singles, ft, _request(rng, world, 30))   # fills caches and memos
-    before = _held(b)
+    before = held(te, b, PUBLISHED)
     # reload maps 4 and 1 in new buffer orders at new positions
     idx, new_st = [4, 1], np.array([(11, 97), (ROWS - 1, COLS - 1)], np.int32)
     z2 = np.stack([synth.terrain(ROWS, COLS, RES, 960 + k, "rough") for k in range(2)]).astype(np.float32)
-    got = b.chain_maps(g, p, idx, np.stack([_wrap(z2[j], new_st[j]) for j in range(2)]), outputs=True, positions=POS[[0, 3]],
+    got = b.chain_maps(g, p, idx, np.stack([wrap(z2[j], new_st[j]) for j in range(2)]), outputs=True, positions=POS[[0, 3]],
                        start_index=new_st)
     want_st, want_pos = START.copy(), POS.copy()
     want_st[idx], want_pos[idx] = new_st, POS[[0, 3]]
     assert np.array_equal(b.start_indices(), want_st) and np.array_equal(b.positions(), want_pos)
-    after = _held(b)
+    after = held(te, b, PUBLISHED)
     for k in set(range(NMAPS)) - set(idx):
         for name in after:
-            assert np.array_equal(_bits(after[name][k]), _bits(before[name][k])), (k, name)
+            assert np.array_equal(bits(after[name][k]), bits(before[name][k])), (k, name)
     for j, k in enumerate(idx):
-        s = maps()
+        s = ctx.map()
         gk = te.Geometry.make(ROWS, COLS, RES, position=tuple(want_pos[k]))
         gk.start_row, gk.start_col = (int(v) for v in new_st[j])
-        want = s.chain(gk, p, _wrap(z2[j], new_st[j]), outputs=True)
+        want = s.chain(gk, p, wrap(z2[j], new_st[j]), outputs=True)
         for name in CHAIN:
-            assert np.array_equal(_bits(got[name][j]), _bits(want[name])), (k, name)
+            assert np.array_equal(bits(got[name][j]), bits(want[name])), (k, name)
         singles[k] = s
     # the selection's bounds in their new buffer orders, then a selected sweep, a selected keep, and a request on every map:
     # the maps not reloaded answer from the caches and memos they kept
-    b.carry_layers(BOUNDS, [np.stack([_wrap(world[a][k], new_st[j]) for j, k in enumerate(idx)]) for a in ("up", "lo")], map_index=idx)
+    b.carry_layers(BOUNDS, [np.stack([wrap(world[a][k], new_st[j]) for j, k in enumerate(idx)]) for a in ("up", "lo")], map_index=idx)
     for j, k in enumerate(idx):
-        singles[k].carry_layers(BOUNDS, [_wrap(world["up"][k], new_st[j]), _wrap(world["lo"][k], new_st[j])])
+        singles[k].carry_layers(BOUNDS, [wrap(world["up"][k], new_st[j]), wrap(world["lo"][k], new_st[j])])
     sel = b.footprint_maps(ft, [1, 3, 4])
     for j, k in enumerate([1, 3, 4]):
-        assert np.array_equal(_bits(sel[j]), _bits(singles[k].footprint(ft))), k
+        assert np.array_equal(bits(sel[j]), bits(singles[k].footprint(ft))), k
     kx, krot = b.footprint_polygon_keep(ft, POLY, [0.3, 1.1], map_index=[4, 2], outputs=True)
     for j, (k, y) in enumerate(zip([4, 2], [0.3, 1.1])):
         sx, srot = singles[k].footprint_polygon_keep(ft, POLY, [y], outputs=True)
-        assert np.array_equal(_bits(kx[j]), _bits(sx)) and np.array_equal(_bits(krot[j]), _bits(srot)), k
+        assert np.array_equal(bits(kx[j]), bits(sx)) and np.array_equal(bits(krot[j]), bits(srot)), k
     _check_request(b, singles, ft, _request(rng, world, 30))
-    _check_held(b, singles, what="after the selection")
+    _check_held(te, b, singles, what="after the selection")
     # set_layers_maps_wrapped: map 2 takes map 5's layers in map 5's buffer order, at map 5's position
     s5 = singles[5].get_layers(list(HELD))
     b.set_layers_maps(g, [2], s5["traversability"][None], s5["traversability_slope"][None], s5["traversability_step"][None],
@@ -364,24 +308,24 @@ def test_selections(maps, te, world):
     assert tuple(b.start_indices()[2]) == tuple(START[5])
     b.carry_layers(BOUNDS, [world["ups"][5][None], world["los"][5][None]], map_index=[2])
     singles[5].clear_footprint()
-    assert np.array_equal(_bits(b.footprint_maps(ft, [2])[0]), _bits(singles[5].footprint(ft)))
-    _check_held(b, [singles[5]], [2], "set_layers_maps_wrapped")
+    assert np.array_equal(bits(b.footprint_maps(ft, [2])[0]), bits(singles[5].footprint(ft)))
+    _check_held(te, b, [singles[5]], [2], "set_layers_maps_wrapped")
     # an existing _maps entry gives the maps it loads (0, 0): their host outputs are in default order again
     b.chain_maps(g, p, [3], world["z"][3:4], positions=POS[3:4])
     assert tuple(b.start_indices()[3]) == (0, 0)
-    s3, _ = _single(maps, te, world, 3, start=(0, 0))
+    s3, _ = _single(ctx, te, world, 3, start=(0, 0))
     b.carry_layers(BOUNDS, [world["up"][3][None], world["lo"][3][None]], map_index=[3])
     b.footprint_maps(ft, [3])
     s3.footprint(ft)
-    _check_held(b, [s3], [3], "chain_maps after wrapped")
+    _check_held(te, b, [s3], [3], "chain_maps after wrapped")
 
 
-def test_one_map_from_device_memory(maps, te, ctx, world):
+def test_one_map_from_device_memory(te, ctx, world):
     """nmaps = 1 from a device input with a start index equals te_map_chain in host memory with that start index."""
     torch = pytest.importorskip("torch")
     k = 3
-    s, want = _single(maps, te, world, k)
-    b = maps()
+    s, want = _single(ctx, te, world, k)
+    b = ctx.map()
     e = _dev(torch, world["zs"][k:k + 1])
     outs = [torch.empty(ROWS * COLS, dtype=torch.float32, device="cuda") for _ in CHAIN]
     ctx._order_after_torch(te.MEM_DEVICE)
@@ -392,13 +336,13 @@ def test_one_map_from_device_memory(maps, te, ctx, world):
     b.carry_layers(BOUNDS, [_dev(torch, world["ups"][k:k + 1]), _dev(torch, world["los"][k:k + 1])], memory=te.MEM_DEVICE)
     ctx.synchronize()
     for name, o in zip(CHAIN, outs):
-        assert np.array_equal(_bits(o.cpu().numpy().reshape(COLS, ROWS).T), _bits(_unwrap(want[name], START[k]))), name
-    hb, hs = _held(b), _held(s)
+        assert np.array_equal(bits(o.cpu().numpy().reshape(COLS, ROWS).T), bits(unwrap(want[name], START[k]))), name
+    hb, hs = held(te, b, PUBLISHED), held(te, s, PUBLISHED)
     for name in hs:
-        assert np.array_equal(_bits(hb[name]), _bits(hs[name])), name
+        assert np.array_equal(bits(hb[name]), bits(hs[name])), name
 
 
-def test_launches(maps, te, ctx, world):
+def test_launches(te, ctx, world):
     """A whole-batch _wrapped chain costs its _at entry's launches plus one, whatever nmaps; a host te_map_get_layers of up to
     eight layers costs one."""
     torch = pytest.importorskip("torch")
@@ -414,7 +358,7 @@ def test_launches(maps, te, ctx, world):
     for n in (2, NMAPS):
         e = _dev(torch, world["zs"][:n])
         xy, si = np.ascontiguousarray(POS[:n]), np.ascontiguousarray(START[:n])
-        m = maps()
+        m = ctx.map()
         at = lambda: m._check(m._L.te_map_chain_batched_at(m._h, C.byref(g), C.byref(p), n, e.data_ptr(), None, None, None, None,  # noqa: E731
                                                           te.MEM_DEVICE, xy.ctypes.data))
         wr = lambda: m._check(m._L.te_map_chain_batched_wrapped(m._h, C.byref(g), C.byref(p), n, e.data_ptr(), None, None, None,  # noqa: E731
@@ -431,13 +375,13 @@ def test_launches(maps, te, ctx, world):
         assert launches(lambda: m.get_layers(names)) == 1, n
 
 
-def test_errors_leave_the_map_unchanged(maps, te, world):
+def test_errors_leave_the_map_unchanged(te, world, ctx):
     p, g = world["p"], world["g"]
     ft = te.FootprintParams.yaml_defaults()
-    b = maps()
+    b = ctx.map()
     _load(b, te, None, world, te.MEM_HOST, outputs=False)
     b.footprint(ft)
-    before, pos, st = _held(b), b.positions(), b.start_indices()
+    before, pos, st = held(te, b, PUBLISHED), b.positions(), b.start_indices()
 
     def expect(code, fn):
         with pytest.raises(te.TEError) as e:
@@ -462,6 +406,6 @@ def test_errors_leave_the_map_unchanged(maps, te, world):
     expect(BAD_ARG, lambda: b.chain_maps(g, p, [1, 1], world["zs"][:2], start_index=START[:2]))
     expect(BAD_ARG, lambda: b.chain_maps(g, p, [NMAPS], world["zs"][:1], start_index=START[:1]))
     assert np.array_equal(b.positions(), pos) and np.array_equal(b.start_indices(), st)
-    after = _held(b)
+    after = held(te, b, PUBLISHED)
     for name in after:
-        assert np.array_equal(_bits(after[name]), _bits(before[name])), name
+        assert np.array_equal(bits(after[name]), bits(before[name])), name

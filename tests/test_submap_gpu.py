@@ -6,19 +6,12 @@ import pytest
 
 import submap_oracle as so
 import synth
+from helpers import assert_same_bits, bits, unwrap
+from map_helpers import check_submaps, submap_windows
 
 pytestmark = pytest.mark.gpu
 
 ROWS, COLS, RES, POS = 150, 130, 0.02, (0.37, -0.21)
-
-
-def _bits(a):
-    a = np.ascontiguousarray(np.asarray(a, dtype=np.float32))
-    return a.view(np.uint32)
-
-
-def _same(a, b, what=""):
-    assert np.array_equal(_bits(a), _bits(b)), what
 
 
 def _layers(seed, rows=ROWS, cols=COLS):
@@ -40,11 +33,6 @@ def _geo(te, start=(0, 0), rows=ROWS, cols=COLS):
     return g
 
 
-def _unwrap(a, start):
-    """Default order of a layer stored with a circular-buffer start index: cell (i, j) is stored at ((i + sr) % rows, ...)."""
-    return np.roll(a, (-start[0], -start[1]), axis=(0, 1))
-
-
 def _set(te, ctx, seed=1, start=(0, 0), rough=True, rslope=True):
     t, s, st, r, e, rs = _layers(seed)
     m = ctx.map()
@@ -62,11 +50,11 @@ def test_get_layers_after_set_layers_host_with_start_index(te, ctx):
     m, L = _set(te, ctx, start=start)
     got = m.get_layers(te.capi.LAYERS)
     for k in L:
-        _same(got[k], L[k], k)                   # re-wrapped: the buffer order the layers came in
-    assert np.isnan(got["traversability_footprint"]).all() and _bits(got["traversability_footprint"]).min() == 0xffffffff
+        assert_same_bits(got[k], L[k], k)                   # re-wrapped: the buffer order the layers came in
+    assert np.isnan(got["traversability_footprint"]).all() and bits(got["traversability_footprint"]).min() == 0xffffffff
     sub = m.get_layers(["elevation", "traversability_step"])
     assert list(sub) == ["traversability_step", "elevation"]          # bit order, whatever the order asked for
-    _same(sub["elevation"], L["elevation"])
+    assert_same_bits(sub["elevation"], L["elevation"])
     m.close()
 
 
@@ -79,7 +67,7 @@ def test_get_layers_device_memory_is_unwrapped(te, ctx):
     got = m.get_layers(names, out=out, memory=te.MEM_DEVICE)
     ctx.synchronize()
     for k in names:
-        _same(got[k].cpu().numpy(), _unwrap(L[k], start), k)
+        assert_same_bits(got[k].cpu().numpy(), unwrap(L[k], start), k)
     m.close()
 
 
@@ -91,12 +79,12 @@ def test_get_layers_after_chain_equals_the_chain_outputs(te, ctx):
     got = m.get_layers(["traversability", "traversability_slope", "traversability_step", "traversability_roughness", "elevation"])
     for k, o in (("traversability", "traversability"), ("traversability_slope", "slope"), ("traversability_step", "step"),
                  ("traversability_roughness", "roughness")):
-        _same(got[k], outs[o], k)
-    _same(got["elevation"], np.asarray(z, dtype=np.float32))
+        assert_same_bits(got[k], outs[o], k)
+    assert_same_bits(got["elevation"], np.asarray(z, dtype=np.float32))
     # the cache after a footprint request is what te_map_get_footprint returns
     fp = m.footprint(te.FootprintParams.yaml_defaults())
-    _same(m.get_layers(["traversability_footprint"])["traversability_footprint"], m.get_footprint())
-    _same(fp, m.get_footprint())
+    assert_same_bits(m.get_layers(["traversability_footprint"])["traversability_footprint"], m.get_footprint())
+    assert_same_bits(fp, m.get_footprint())
     with pytest.raises(te.TEError) as e:            # computeTraversability leaves robot_slope to setTraversabilityMap
         m.get_layers(["robot_slope"])
     assert e.value.code == -2
@@ -128,37 +116,8 @@ def test_layer_errors(te, ctx):
     m.close()
 
 
-def _windows(rng, n, g):
-    """Windows of 0 to 1.5 m around centres inside, near the edges (straddling them) and outside the map."""
-    P, Lm = np.array(POS), np.array([g.length_x, g.length_y])
-    kind = rng.integers(0, 3, n)
-    pos = P + rng.uniform(-0.45, 0.45, (n, 2)) * Lm
-    edge = kind == 1
-    pos[edge] = P + rng.choice([-0.5, 0.5], (edge.sum(), 2)) * Lm + rng.uniform(-0.1, 0.1, (edge.sum(), 2))
-    pos[kind == 2] = P + rng.uniform(-1.2, 1.2, ((kind == 2).sum(), 2)) * Lm
-    length = rng.uniform(0.0, 1.5, (n, 2))
-    length[rng.random(n) < 0.1] = 0.0
-    length[rng.random(n) < 0.1] = 2.5 * RES
-    return pos, length
-
-
 def _oracle_geometry(oracle, pos, length):
     return so.submap_geometry(oracle.Geometry.make(ROWS, COLS, RES, POS), pos, length)
-
-
-def _check_windows(res, want, full, names):
-    """Every window: geometry as the oracle's, layers equal to the block of the default-order layers `full`."""
-    assert len(res) == len(want["success"])
-    for k, (info, lay) in enumerate(res):
-        for f in so.FIELDS:
-            assert info[f] == want[f][k] or (np.isnan(info[f]) and np.isnan(want[f][k])), (k, f)
-        if not info["success"]:
-            assert lay is None
-            continue
-        r0, c0, nr, nc = (int(info[f]) for f in ("top_row", "top_col", "rows", "cols"))
-        assert list(lay) == [n for n in full if n in names]
-        for n in lay:
-            _same(np.asarray(lay[n]), full[n][r0:r0 + nr, c0:c0 + nc], (k, n))
 
 
 @pytest.mark.parametrize("names", [None, ["traversability"], ["traversability_step", "elevation", "traversability_footprint"]])
@@ -166,13 +125,13 @@ def test_submaps_host_memory_are_slices_of_the_layers(te, ctx, oracle, names):
     start = (0, 0) if names else (19, 62)
     m, L = _set(te, ctx, seed=4, start=start)
     names = names or list(te.capi.LAYERS)
-    full = {k: _unwrap(v, start) for k, v in m.get_layers(te.capi.LAYERS).items()}
+    full = {k: unwrap(v, start) for k, v in m.get_layers(te.capi.LAYERS).items()}
     rng = np.random.default_rng(8)
-    pos, length = _windows(rng, 120, _geo(te))
+    pos, length = submap_windows(rng, 120, _geo(te))
     res = m.get_submaps(pos, length, names)
     want = _oracle_geometry(oracle, pos, length)
     assert 0 < want["success"].sum() < len(pos)
-    _check_windows(res, want, {k: v for k, v in full.items() if k in names}, names)
+    check_submaps(res, want, {k: v for k, v in full.items() if k in names}, names)
     m.close()
 
 
@@ -181,9 +140,9 @@ def test_submaps_device_memory_and_one_call_equals_single_calls(te, ctx, oracle)
     start = (3, 9)
     m, L = _set(te, ctx, seed=6, start=start)
     names = ["traversability", "traversability_roughness", "robot_slope"]
-    full = {k: _unwrap(v, start) for k, v in m.get_layers(names).items()}
+    full = {k: unwrap(v, start) for k, v in m.get_layers(names).items()}
     rng = np.random.default_rng(12)
-    pos, length = _windows(rng, 300, _geo(te))
+    pos, length = submap_windows(rng, 300, _geo(te))
     want = _oracle_geometry(oracle, pos, length)
     total = len(names) * int((want["rows"] * want["cols"]).sum())
     out = torch.full((total + 5,), -3.0, dtype=torch.float32, device="cuda")
@@ -192,7 +151,7 @@ def test_submaps_device_memory_and_one_call_equals_single_calls(te, ctx, oracle)
     host = out.cpu().numpy()
     assert (host[total:] == -3.0).all()                        # nothing written beyond the windows
     res_np = [(i, None if d is None else {n: v.cpu().numpy() for n, v in d.items()}) for i, d in res]
-    _check_windows(res_np, want, full, names)
+    check_submaps(res_np, want, full, names)
     # 300 windows in one call equal 300 calls of one window each, in host memory
     hres = m.get_submaps(pos, length, names)
     for k in range(len(pos)):
@@ -201,8 +160,8 @@ def test_submaps_device_memory_and_one_call_equals_single_calls(te, ctx, oracle)
         assert bool(i1["success"]) == bool(i0["success"])
         if d0 is not None:
             for n in names:
-                _same(d1[n], d0[n], (k, n))
-                _same(d0[n], res_np[k][1][n], (k, n))
+                assert_same_bits(d1[n], d0[n], (k, n))
+                assert_same_bits(d0[n], res_np[k][1][n], (k, n))
     m.close()
 
 
@@ -228,7 +187,7 @@ def test_capacity_retry_failed_windows_and_launch_count(te, ctx):
     # one gather launch whatever the window count; none when no window has cells
     rng = np.random.default_rng(2)
     for n in (1, 16, 300):
-        p, ln = _windows(rng, n, _geo(te))
+        p, ln = submap_windows(rng, n, _geo(te))
         p[0], ln[0] = POS, (0.3, 0.3)
         before = ctx.stats()[0]
         m.get_submaps(p, ln, ["traversability", "elevation"])
@@ -245,7 +204,7 @@ def test_capacity_retry_failed_windows_and_launch_count(te, ctx):
 @pytest.mark.parametrize("start", [(0, 0), (71, 12)])
 def test_valid_at_matches_oracle(te, ctx, oracle, start):
     m, L = _set(te, ctx, seed=13, start=start)
-    trav = _unwrap(L["traversability"], start)
+    trav = unwrap(L["traversability"], start)
     rng = np.random.default_rng(21)
     g = _geo(te)
     n = 5000

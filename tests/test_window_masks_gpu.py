@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 import window_masks as wm
-from helpers import assert_parity, compare_layer
+from helpers import assert_parity, chain_params, compare_layer
 
 pytestmark = pytest.mark.gpu
 
@@ -28,10 +28,7 @@ def _clock():
 
 
 def _params(mod, shape, **kw):
-    p = mod.ChainParams.yaml_defaults(0)
-    for k, v in {**wm.chain_kwargs(shape), **kw}.items():
-        setattr(p, k, v)
-    return p
+    return chain_params(mod, **{**wm.chain_kwargs(shape), **kw})
 
 
 def _parity(got, ref):
