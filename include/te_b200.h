@@ -177,7 +177,10 @@ int te_chain_batched(te_ctx* ctx, const te_geometry* g, const te_chain_params* p
 /* TraversabilityMap::traversabilityFootprint(const double& radius, const double& offset) —
  * traversability_estimation/src/TraversabilityMap.cpp:307-318 with isTraversable (:654-746),
  * isTraversableForFilters (:774-792), checkForStep (:794-865), checkForSlope (:867-893).
- * out: traversability_footprint; slope_footprint/step_footprint memoisation layers optional. */
+ * out: traversability_footprint; slope_footprint/step_footprint memoisation layers optional.
+ * traversability_default may be NaN or infinite: a cell whose disk visits an invalid traversability cell before its first blocked
+ * one then gets NaN / that infinity (0 when the blocked cell lies within the radius), every other cell what a finite default
+ * gives.  Such a default takes the visit-by-visit sweep, about 50 times slower than the prefix-sum sweep at the YAML footprint. */
 int te_footprint(te_ctx* ctx, const te_geometry* g, const te_slab* slab, const te_footprint_params* p,
                  const float* traversability, const float* slope, const float* step, const float* elevation,
                  float* traversability_footprint, float* slope_footprint_or_null, float* step_footprint_or_null,
@@ -200,6 +203,9 @@ int te_footprint2(te_ctx* ctx, const te_geometry* g, const te_slab* slab, const 
  * isTraversableForFilters, else the mean of the traversability layer over those cells (traversability_default for invalid
  * cells, and when the polygon covers no cell).  Uses p->traversability_default, max_gap_width, critical_step_height,
  * verify_roughness (radius / offset are ignored).  Slab halo: te_footprint's predicate halo + the polygon's reach.
+ * traversability_default may be NaN or infinite: a polygon that holds an invalid cell and no blocked one then gives that default,
+ * as the reference's sum does, every other cell what a finite default gives; the same holds for the batched, list-of-yaws and
+ * te_map polygon sweeps (not for the reductions over yaws, which refuse such a default).
  * TE_ERR_UNSUPPORTED for a polygon that reaches further than 31 cells from its centre. */
 int te_footprint_polygon(te_ctx* ctx, const te_geometry* g, const te_slab* slab, const te_footprint_params* p, int32_t npts,
                          const double* polygon_xy, double footprint_yaw, const float* traversability, const float* slope,

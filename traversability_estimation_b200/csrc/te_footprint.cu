@@ -164,7 +164,8 @@ __global__ void __launch_bounds__(256) k_fp_nearest(FpArgs A, unsigned char* __r
 }
 
 // One warp per input-buffer column: prefix sums of t' = finite(traversability) ? value : default along the row
-// index (double; exact for float32 terms, so the order of summation does not matter) and packed blocked flags.
+// index (double; exact for float32 terms, so the order of summation does not matter) and packed blocked flags.  Only for a finite
+// default (launch_footprint); a default far outside the layer's range, such as 1e6, loses the low bits of the terms after it.
 __global__ void __launch_bounds__(256) k_fp_prepare_p(FpArgs A, Layers L, const unsigned char* __restrict__ blocked, double* __restrict__ P,
                                                     unsigned* __restrict__ bits) {
   const int lane = threadIdx.x & 31;
@@ -473,7 +474,11 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
   const double res = g->resolution, r2 = rmax * rmax, cu = coord_ulp(v.coord_max + rmax);
   const double tol_far = 8.0 * rmax * cu, tol = std::max(1e-9 * r2, tol_far) + 1e-300;
   const int Lmax = lattice_reach(rmax, res, cu);
-  const bool fast = Lmax <= 31 && v.out_ncols <= 65535 && std::getenv("TE_FOOTPRINT_BRUTE") == nullptr;
+  // The prefix sums hold the default of every invalid cell of a column: a NaN or infinite default would make every disk below the
+  // column's first invalid cell non-finite, where the reference adds it only for the invalid cells it visits.  k_sweep adds in
+  // visit order, so it takes that case.
+  const bool fast = Lmax <= 31 && v.out_ncols <= 65535 && std::isfinite(p->traversability_default) &&
+                    std::getenv("TE_FOOTPRINT_BRUTE") == nullptr;
   if (!fast) {
     (a.pos ? k_sweep<true> : k_sweep<false>)<<<std::max(g2, 1), 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
     if (launches) *launches = 3;

@@ -78,9 +78,12 @@ __device__ bool poly_inside_d(const PolyArgs& Q, const Rot2& R, double cx, doubl
 // polygons in registers instead of storing a layer per polygon (PolyArgs::worst / best / best_yaw).  kAt: map z sits at its own
 // position and reads its coordinate tables at A.X + z * A.xs, A.Y + z * A.ys.  kMaps (Q.npoly = 2, the polygons of each map):
 // map z sweeps its own pair of polygons, desc[0] and desc[map_poly[z]], into map slot slot[z] of their layers (slot null: z);
-// device arrays of one entry per map, unused otherwise.  A and Q are taken by value: k_poly_tile then compiles to the code it had
-// as a kernel of its own (by reference it does not).
-template <bool kReduce, bool kAt, bool kMaps>
+// device arrays of one entry per map, unused otherwise.  kInv: the default is NaN or infinite, so it cannot go into the prefix sums
+// (every sum below a column's first invalid cell would be non-finite); invalid cells are staged as 0 and counted in the high byte
+// of the blocked counts (at most NR <= 126 of each per column), and a footprint that holds one gives the default, as the
+// reference's sum does.  A and Q are taken by value: k_poly_tile then compiles to the code it had as a kernel of its own (by
+// reference it does not).
+template <bool kReduce, bool kAt, bool kMaps, bool kInv>
 __device__ __forceinline__ void poly_tile(FpArgs A, PolyArgs Q, const float* __restrict__ trav,
                                           const unsigned char* __restrict__ blocked, const int* __restrict__ map_poly,
                                           const int* __restrict__ slot) {
@@ -116,9 +119,15 @@ __device__ __forceinline__ void poly_tile(FpArgs A, PolyArgs Q, const float* __r
       cb4[m] = 0;
       if (k < NR && col_ok && row >= 0 && row < A.rows) {
         const float t = __ldg(tcol + row);
-        v[m] = finitef(t) ? (double)t : A.tdefault;
-        cb4[m] = bcol[row] != 0 ? 1 : 0;
-        bw |= (unsigned)cb4[m] << (8 * m);
+        if constexpr (kInv) {
+          v[m] = finitef(t) ? (double)t : 0.0;
+          cb4[m] = (bcol[row] != 0 ? 1 : 0) | (finitef(t) ? 0 : 256);
+          bw |= (unsigned)(cb4[m] != 0) << (8 * m);
+        } else {
+          v[m] = finitef(t) ? (double)t : A.tdefault;
+          cb4[m] = bcol[row] != 0 ? 1 : 0;
+          bw |= (unsigned)cb4[m] << (8 * m);
+        }
       }
     }
     anyb |= (int)bw;
@@ -175,6 +184,7 @@ __device__ __forceinline__ void poly_tile(FpArgs A, PolyArgs Q, const float* __r
       const int nruns = D.nruns, nfz = D.nfz;
       double t = 0.0;
       int n = 0, nblk = 0;
+      int ninv = 0;  // kInv: invalid cells in the footprint
       if (interior) {  // no clipping anywhere: the cell count is the table's
         for (int r = 0; r < nruns; ++r) {
           const int w = __ldg(runs + r);
@@ -183,7 +193,13 @@ __device__ __forceinline__ void poly_tile(FpArgs A, PolyArgs Q, const float* __r
           t += pc[hi + 1] - pc[lo];
           if (tile_any) {
             const unsigned short* bc = bbase + dj * PB;
-            nblk += (int)bc[hi + 1] - (int)bc[lo];
+            if constexpr (kInv) {
+              const int d = (int)bc[hi + 1] - (int)bc[lo];
+              nblk += d & 0xff;
+              ninv += d >> 8;
+            } else {
+              nblk += (int)bc[hi + 1] - (int)bc[lo];
+            }
           }
         }
         n = D.ncert;
@@ -200,7 +216,13 @@ __device__ __forceinline__ void poly_tile(FpArgs A, PolyArgs Q, const float* __r
           n += a1 - a0 + 1;
           if (tile_any) {
             const unsigned short* bc = bbase + dj * PB;
-            nblk += (int)bc[hi + 1] - (int)bc[lo];
+            if constexpr (kInv) {
+              const int d = (int)bc[hi + 1] - (int)bc[lo];
+              nblk += d & 0xff;
+              ninv += d >> 8;
+            } else {
+              nblk += (int)bc[hi + 1] - (int)bc[lo];
+            }
           }
         }
       }
@@ -243,13 +265,20 @@ __device__ __forceinline__ void poly_tile(FpArgs A, PolyArgs Q, const float* __r
           n += a1c - a0c + 1;
           if (tile_any) {
             const unsigned short* bc = sB + (size_t)cc * PB + (a0 - rb);
-            nblk += (int)bc[len + 1] - (int)bc[0];
+            if constexpr (kInv) {
+              const int d = (int)bc[len + 1] - (int)bc[0];
+              nblk += d & 0xff;
+              ninv += d >> 8;
+            } else {
+              nblk += (int)bc[len + 1] - (int)bc[0];
+            }
           }
         }
       }
       float result;
       if (nblk > 0) result = 0.0f;                       // :297 / :301
       else if (n == 0) result = (float)A.tdefault;       // :625-628
+      else if (kInv && ninv > 0) result = (float)A.tdefault;  // the sum holds a non-finite default
       else result = (float)(t / (double)n);              // :630
       if constexpr (kReduce) {
         if (result < worst) worst = result;
@@ -271,7 +300,12 @@ __device__ __forceinline__ void poly_tile(FpArgs A, PolyArgs Q, const float* __r
 
 template <bool kReduce>
 __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const float* __restrict__ trav, const unsigned char* __restrict__ blocked) {
-  poly_tile<kReduce, false, false>(A, Q, trav, blocked, nullptr, nullptr);
+  poly_tile<kReduce, false, false, false>(A, Q, trav, blocked, nullptr, nullptr);
+}
+
+// k_poly_tile<false> for a NaN or infinite traversability_default (the reductions refuse one).
+__global__ void __launch_bounds__(256) k_poly_tile_inv(FpArgs A, PolyArgs Q, const float* __restrict__ trav, const unsigned char* __restrict__ blocked) {
+  poly_tile<false, false, false, true>(A, Q, trav, blocked, nullptr, nullptr);
 }
 
 // The polygon layers a te_map keeps (launch_footprint_polygon with PolygonMaps): every map of the launch sweeps the identity and
@@ -279,7 +313,14 @@ __global__ void __launch_bounds__(256) k_poly_tile(FpArgs A, PolyArgs Q, const f
 template <bool kAt>
 __global__ void __launch_bounds__(256) k_poly_tile_maps(FpArgs A, PolyArgs Q, const float* __restrict__ trav, const unsigned char* __restrict__ blocked,
                                                         const int* __restrict__ map_poly, const int* __restrict__ slot) {
-  poly_tile<false, kAt, true>(A, Q, trav, blocked, map_poly, slot);
+  poly_tile<false, kAt, true, false>(A, Q, trav, blocked, map_poly, slot);
+}
+
+template <bool kAt>
+__global__ void __launch_bounds__(256) k_poly_tile_maps_inv(FpArgs A, PolyArgs Q, const float* __restrict__ trav,
+                                                            const unsigned char* __restrict__ blocked, const int* __restrict__ map_poly,
+                                                            const int* __restrict__ slot) {
+  poly_tile<false, kAt, true, true>(A, Q, trav, blocked, map_poly, slot);
 }
 
 // Reduce mode after a yaw-group split: k_poly_tile left group g's partial reduction at g * n cells of each scratch array (sw: worst,
@@ -424,6 +465,7 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
   if (npoly < (maps ? 2 : 1)) { st.why = "no polygon layer to sweep"; return TE_ERR_UNSUPPORTED; }
   if (maps && reduce) { st.why = "per-map polygons have no reduction"; return TE_ERR_UNSUPPORTED; }
   if (reduce && !reduce->worst && !reduce->best && !reduce->best_yaw) { st.why = "no reduction output"; return TE_ERR_UNSUPPORTED; }
+  if (reduce && !std::isfinite(p->traversability_default)) { st.why = "reduction with a non-finite traversability_default"; return TE_ERR_UNSUPPORTED; }
   const int Lp = polygon_reach(g, npts, pts_xy);
   if (Lp > 31) { st.why = "footprint polygon reaches further than 31 cells from its centre"; return TE_ERR_UNSUPPORTED; }
   PolyArgs q{};
@@ -472,7 +514,10 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
     if (cudaFuncSetAttribute(k_poly_tile<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
         cudaFuncSetAttribute(k_poly_tile<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
         cudaFuncSetAttribute(k_poly_tile_maps<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
-        cudaFuncSetAttribute(k_poly_tile_maps<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess) {
+        cudaFuncSetAttribute(k_poly_tile_maps<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
+        cudaFuncSetAttribute(k_poly_tile_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
+        cudaFuncSetAttribute(k_poly_tile_maps_inv<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess ||
+        cudaFuncSetAttribute(k_poly_tile_maps_inv<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smax) != cudaSuccess) {
       st.why = "cudaFuncSetAttribute(max dynamic shared memory) failed"; return TE_ERR_CUDA;
     }
     st.poly_attr = true;
@@ -484,14 +529,16 @@ int launch_footprint_polygon(FootprintState& st, const SlabView& v, const te_geo
   const int nsplit = (q.npoly + q.group - 1) / q.group;  // groups actually launched
   const int nblocks_x = q.row_tiles * nsplit;
   const dim3 grid((unsigned)nblocks_x, (unsigned)col_tiles, (unsigned)nmaps);
+  const bool inv = !std::isfinite(a.tdefault);  // the reductions refuse such a default (footprint_polygon_common)
   if (maps) {
-    (a.pos ? k_poly_tile_maps<true> : k_poly_tile_maps<false>)<<<grid, 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p,
-                                                                                      q.fz + fz.size(), maps->slot);
+    const auto kern = inv ? (a.pos ? k_poly_tile_maps_inv<true> : k_poly_tile_maps_inv<false>)
+                          : (a.pos ? k_poly_tile_maps<true> : k_poly_tile_maps<false>);
+    kern<<<grid, 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p, q.fz + fz.size(), maps->slot);
     if (launches) *launches = 3;
     return 0;
   }
   if (!reduce) {
-    k_poly_tile<false><<<grid, 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p);
+    (inv ? k_poly_tile_inv : k_poly_tile<false>)<<<grid, 256, smem, s>>>(a, q, trav, (const unsigned char*)st.block.p);
     if (launches) *launches = 3;
     return 0;
   }
