@@ -766,9 +766,11 @@ int te_map_footprint_polygon_keep(te_map* map, const te_footprint_params* p, int
  * te_map_check_footprint_request_device, without the circular paths' when the request has none.  Planners whose requests live
  * on the device use te_map_check_footprint_request_device.  Paths run in request order.  A circular path's isTraversable calls
  * (:654-746) read and fill the cache exactly as the reference's do: a centre outside the map gives the default and stores
- * nothing; a cached cell gives its float32 value and is traversable iff it is != 0 (with compute_untraversable_polygon, a cached 0
- * publishes Polygon::fromCircle); any other cell walks the spiral with this check's radius, offset and flag, returns the double
- * mean to the path sum and stores (float) of what the reference stores.  Checks after the first failure of a segment, and the
+ * nothing; a cached cell (a finite value, isValid) gives its float32 value and is traversable iff it is != 0 (with
+ * compute_untraversable_polygon, a cached 0 publishes Polygon::fromCircle); any other cell walks the spiral with this check's
+ * radius, offset and flag, returns the double mean to the path sum and stores (float) of what the reference stores.  A walk can
+ * store a NaN or an infinity (an invalid cell under a non-finite traversability_default, an infinite ring factor at offset 0):
+ * the cell is then not cached, and the next check there walks again with its own radius and flag.  Checks after the first failure of a segment, and the
  * checks of a segment or pose whose checkInclination fails, do not run and store nothing.  Polygonal paths neither read nor
  * change the cache. */
 int te_map_check_footprint_request(te_map* map, const te_footprint_params* p, int32_t npaths, int32_t nposes, const int32_t* path_begin,
@@ -831,8 +833,10 @@ int te_map_get_footprint(te_map* map, float* traversability_footprint, int memor
 int te_map_clear_footprint(te_map* map);
 
 /* Counters of the last te_map_check_footprint_request(_batched): out[0] isTraversable calls its circular paths could make, out[1]
- * distinct circles among them (each is walked once on the device), out[2] cache cells the request stored; totals over every map
- * of a batch.  No reference counterpart. */
+ * distinct circles among them (each is walked once on the device), out[2] cache stores the request made (its walks that ran);
+ * totals over every map of a batch.  While every walk stores a finite value out[2] <= out[1]; a walk that stores a NaN or an
+ * infinity leaves its cell uncached, so a later check there walks and stores again, and out[2] can exceed out[1].  No reference
+ * counterpart. */
 int te_map_request_stats(te_map* map, int64_t out[3]);
 
 /* ---- The read side of a te_map: the layers the reference node publishes and serves ----------------------------------------

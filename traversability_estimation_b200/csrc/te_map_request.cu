@@ -380,16 +380,19 @@ __global__ void __launch_bounds__(256) k_req_dedup(DevReq D) {
 
 // 5. Replay: the service loop of one map, one warp per map, over the map's entries in request order, 32 at a time.  Why this is
 // the sequential loop (one check after the other, as the reference runs it) exactly:
-//   - Which value a check reads depends only on the checks before it in its map: in the sequential loop a cell holds a value this
-//     request stored iff an executed earlier check of the request walked it, and then that walk's float.  The live cache holds
-//     exactly those: a cell the request stored, or one cached when it began, is finite (the walks store finite values); an empty
-//     cell was empty when the request began, so its key's record is a walk.
-//   - Within a window every lane assumes that all lanes before it run.  Among lanes of one cell only the first can find the cell
-//     empty and walk; every later one reads the first one's float (the live value, or the float its record stores).  So under
-//     that assumption each lane's value and verdict are the sequential loop's.
+//   - Which value a check reads depends only on the checks before it in its map: in the sequential loop a cell holds the float of
+//     the last executed earlier check of the request that walked it, or what it held when the request began.  The live cache
+//     holds exactly those.  A check walks iff its cell is not finite (:673, isValid): empty, or holding a NaN or an infinity that
+//     a walk stored (an invalid cell under a non-finite traversability_default, an infinite ring factor at offset 0).  Such a
+//     cell was empty or non-finite when the request began, so every key at it has a walk as its record.
+//   - Within a window every lane assumes that all lanes before it run.  At a cell whose live value is finite every lane reads it.
+//     At any other cell a lane walks (its own record) iff every earlier lane of that cell walked and stored a non-finite float;
+//     otherwise it reads the first finite float stored before it.  So under that assumption each lane's value and verdict are
+//     the sequential loop's.
 //   - The assumption holds up to and including the first failing lane f: no lane before it fails, and entries of one path are
-//     consecutive, so the sequential loop runs lanes 0 .. f in this order.  They commit: first touches store their float, and one
-//     lane folds the values in visit order, so sums, add_segment_d and the verdicts are the sequential loop's bit for bit.
+//     consecutive, so the sequential loop runs lanes 0 .. f in this order.  They commit: a cell keeps the float of its last
+//     committed walk, and one lane folds the values in visit order, so sums, add_segment_d and the verdicts are the sequential
+//     loop's bit for bit.  Every committed walk counts as a store, so under a non-finite value `stored` can exceed the keys.
 //   - The sequential loop then skips the rest of f's path (the `break`s); the next window starts at the first entry of a later
 //     path.  Lanes after f that belong to later paths are evaluated again there: their assumption included dropped lanes, which
 //     store nothing.
@@ -424,7 +427,7 @@ __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* c
     }
     const bool key = have && (E.flags & kEntKey);
     const unsigned long long cell = key ? (unsigned long long)E.cj * A.rows + E.ci : ~0ULL - lane;
-    const int leader = __ffs((int)__match_any_sync(0xffffffffu, cell)) - 1;
+    const unsigned peers = __match_any_sync(0xffffffffu, cell);
     float live = 0.0f, rcache = 0.0f;
     MapRecord R{};
     if (key) {
@@ -432,15 +435,17 @@ __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* c
       R = D.recs[D.kid[E.key]];
       rcache = R.cache;
     }
-    const float lead_cache = __shfl_sync(0xffffffffu, rcache, leader);
-    const bool walk = key && leader == lane && !finitef(live);
+    // the lanes before this one at its cell whose float is finite: the first of them is the first finite store before this lane
+    const unsigned fin = peers & __ballot_sync(0xffffffffu, finitef(rcache)) & ((1u << lane) - 1u);
+    const float first_cache = __shfl_sync(0xffffffffu, rcache, fin ? __ffs((int)fin) - 1 : lane);
+    const bool walk = key && fin == 0 && !finitef(live);
     double t = 0.0;
     bool lok = true;
     int fk = 0;  // the lane's polygon kind if it fails
     if (key) {
       if (walk) { t = R.t; lok = R.state == 0; fk = 2; }  // :679-736
       else {                                              // :673-678
-        const float v = finitef(live) ? live : lead_cache;
+        const float v = finitef(live) ? live : first_cache;
         t = (double)v; lok = v != 0.0f; fk = 1;
       }
     } else if (have && (E.flags & kEntOutside)) {         // :662-667
@@ -453,8 +458,10 @@ __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* c
     const int nhave = __popc(__ballot_sync(0xffffffffu, have));
     const int ncommit = min(f + 1, nhave);
     const bool commit_walk = walk && lane < ncommit;
-    if (commit_walk) mc[cell] = R.cache;
-    stored += __popc(__ballot_sync(0xffffffffu, commit_walk));
+    const unsigned walked = __ballot_sync(0xffffffffu, commit_walk);
+    // the cell keeps the float of its last committed walk
+    if (commit_walk && !(walked & peers & ~((2u << lane) - 1u))) mc[cell] = R.cache;
+    stored += __popc(walked);
     s_t[w][lane] = t;
     s_v[w][lane] = (lok ? 1 : 0) | (fk << 1);
     __syncwarp();
