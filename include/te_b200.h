@@ -1082,6 +1082,53 @@ int te_occupancy_grid_info(const te_geometry* g, int32_t n, const double* positi
 int te_map_get_occupancy(te_map* map, int32_t nsel, const int32_t* map_index_or_null, uint32_t layer_mask, const float* data_min,
                          const float* data_max, int8_t* out, int memory);
 
+/* ---- Point clouds (GridMapRosConverter::toPointCloud), as grid_map_visualization publishes a traversability map -------------
+ * visualization.launch with config/visualization/traversability.yaml publishes traversability_cloud, type point_cloud with layer
+ * elevation: PointCloudVisualization::visualize calls toPointCloud(map, "elevation", cloud), which passes every layer of the map in
+ * message order (SURVEY.md A.8, recalled from grid_map_ros 1.6.x).  The entry below gives the clouds' PointCloud2.data and widths;
+ * the header, stamp and frame id stay the caller's.
+ *
+ * The field layout, one rule: one float32 field per entry of `fields`, 4 bytes each at consecutive offsets, the entry equal to
+ * point_layer replaced by three fields x, y, z; point_step = 4 * the number of fields; height 1, is_dense false, width = the map's
+ * points, row_step = width * point_step.
+ *
+ * toPointCloud for the maps of the call, in a fixed number of launches (te_get_stats counts 3: a count kernel, one cub scan, a
+ * scatter kernel), whatever the maps, fields, start indices and points.
+ *   - Maps: nsel 0 with map_index_or_null NULL is every map of the batch; otherwise the maps map_index[0..nsel), a HOST array of
+ *     distinct indices in 0..nmaps-1 in any order, read before the call returns.  Every te_map takes a selection, one whose start
+ *     index came in g included: each map is read in its own buffer order and at its own position.
+ *   - fields: a HOST array of nfields (1..32) entries in the published map's layer order.  Each is one te_layer bit that
+ *     te_map_get_layers accepts (the carried layers, robot_slope, TE_LAYER_FOOTPRINT (the cache, NaN where empty),
+ *     traversability_x / _rot, TE_LAYER_UNCERTAINTY_RANGE with te_map_get_layers' NaN-payload rule), at most once, or 0: a field
+ *     holding NaN 0x7fc00000 at every point.  0 stands for step_footprint, slope_footprint and roughness_footprint as
+ *     computeTraversability publishes them (TraversabilityMap.cpp:225-228: all NaN); that is exact only for a map published by
+ *     computeTraversability, not after a footprint service call has filled the reference's lazily evaluated layers (:301, :316).
+ *   - point_layer: one te_layer bit the map holds.  It decides which cells are points; it need not be in `fields`, and then the
+ *     records have no x, y, z, as in the reference.
+ *   - basic_mask: the map's basic layers as te_layer bits (0: none, as in the reference's bags).
+ *   - Points: the cells of each map in its buffer order (linear index k: buffer cell (k % rows, k / rows) under the map's start
+ *     index, as GridMapIterator walks it), keeping those where the point layer and, when basic_mask is not 0, every basic layer
+ *     is finite (getPosition3, isValid).  x, y: (float) of getPosition of the cell, on its unwrapped index at its map's position
+ *     (te_grid.cuh's cell_coord), rounded to nearest; z and every other field: the float32 bits as stored, NaN payloads and -0.0
+ *     included.  This order holds in both memory modes.
+ *   - Output: offsets, nsel + 1 (or nmaps + 1) int64 in `memory`: offsets[0] = 0, map k of the call has width offsets[k + 1] -
+ *     offsets[k] and its blob starts at byte point_step * offsets[k] of `data`; the blobs are back to back in call order.
+ *   - Capacity, in points: host memory, when the clouds hold more than capacity_points the call fills offsets, writes nothing to
+ *     data and returns TE_ERR_BAD_ARG (capacity 0 with a NULL data is a sizing query); device memory, offsets are always complete
+ *     and points at or past capacity_points are not written, so the call reads nothing back.
+ *   - Memory: host memory computes the offsets on the device and copies them back once, then writes the records into staging and
+ *     copies back total * point_step bytes; the call returns synchronised.  Device memory is asynchronous on the context stream,
+ *     with no host synchronisation and no allocation once the scratch exists (16 bytes per tile of 1024 cells plus the scan's).
+ *     A whole-batch device call passes its arguments by value (maps at several positions or start indices read a per-map table
+ *     uploaded when it changes), so it can be captured in a CUDA graph; a selection uploads its table as the _maps entries do.
+ *   - Errors, every one found before anything is written: TE_ERR_BAD_ARG for a map without layers, nfields outside 1..32, a null
+ *     fields or offsets, a null data with capacity_points > 0, a negative capacity_points, an entry that is neither 0 nor one known
+ *     bit or that repeats one, a point_layer that is not one known bit, unknown bits in basic_mask, an unknown memory mode and a
+ *     bad selection; TE_ERR_MISSING_LAYER as te_map_get_layers for the field, point and basic layers. */
+int te_map_get_point_cloud(te_map* map, int32_t nsel, const int32_t* map_index_or_null, int32_t nfields, const uint32_t* fields,
+                           uint32_t point_layer, uint32_t basic_mask, void* data, int64_t capacity_points, int64_t* offsets,
+                           int memory);
+
 /* ---- Multi-GPU: one map tiled into column slabs, one process (rank) per GPU (SURVEY.md §8e) -------------------------------
  * The chain and the footprint sweep are stencils of fixed radius, so the only exchange step is a one-shot copy of the
  * neighbours' boundary columns of the INPUT layer(s) into this rank's halo.  The reference has no counterpart (it is a

@@ -222,6 +222,7 @@ SIGNATURES = {
     "te_map_at_poses": (_R, [_P, _P, _I, _P, _I, _P, _U, _P, _P, _I]),
     "te_occupancy_grid_info": (_R, [_G, _I, _P, _P]),
     "te_map_get_occupancy": (_R, [_P, _I, _P, _U, _P, _P, _P, _I]),
+    "te_map_get_point_cloud": (_R, [_P, _I, _P, _I, _P, _U, _U, _P, _L, _P, _I]),
     "te_ipc_export": (_R, [_P, _P]),
     "te_ipc_open": (_R, [_P, _P]),
     "te_ipc_close": (_R, [_P]),
@@ -301,6 +302,22 @@ def occupancy_grid_info(g, positions=None):
     if rc != 0:
         raise TEError(rc, L.te_last_error().decode())
     return info
+
+
+def point_cloud_fields(fields, point_layer="elevation"):
+    """The PointCloud2 layout GridMapRosConverter::toPointCloud gives a cloud of the layers `fields` (names, in message order): one
+    float32 field per entry at consecutive 4-byte offsets, the entry equal to point_layer replaced by x, y, z.  Returns the
+    (name, offset) pairs and point_step (te_b200.h states the same rule for te_map_get_point_cloud)."""
+    names = []
+    for f in fields:
+        names += ["x", "y", "z"] if f == point_layer else [f]
+    return [(n, 4 * k) for k, n in enumerate(names)], 4 * len(names)
+
+
+def point_cloud_dtype(layout, point_step):
+    """The numpy structured dtype of one point of a point_cloud_fields layout: float32 fields at their offsets."""
+    return np.dtype({"names": [n for n, _ in layout], "formats": [np.float32] * len(layout), "offsets": [o for _, o in layout],
+                     "itemsize": point_step})
 
 
 IMAGE_MONO8, IMAGE_MONO16 = 0, 1  # te_image encodings
@@ -1357,3 +1374,46 @@ class Map:
         else:
             v = out.reshape(len(order), n, cols, rows)
         return {name: v[k] for k, name in enumerate(order)}
+
+    def get_point_cloud(self, fields, point_layer="elevation", basic=(), nan_layers=(), maps=None, capacity=None, out=None,
+                        offsets=None, memory=MEM_HOST):
+        """te_map_get_point_cloud (GridMapRosConverter::toPointCloud): the clouds of the maps (maps None: every map; otherwise the
+        maps `maps` in that order) with one float32 field per name of `fields` (message order), the point layer's entry replaced by
+        x, y, z.  A name of `nan_layers` is a field holding NaN 0x7fc00000 (the published map's step_footprint / slope_footprint
+        after computeTraversability); every other name is a LAYER_BITS entry.  basic: the map's basic layers.  Returns (layout,
+        point_step, clouds), layout the (name, offset) pairs of point_cloud_fields.  Host memory: clouds is a list of one numpy
+        structured array per map (point_cloud_dtype), in the reference's point order; capacity None sizes the call first, otherwise
+        a cloud over `capacity` points raises.  Device memory: `out` a uint8 device tensor (capacity None: all of it) and `offsets`
+        an int64 device tensor of n + 1, filled asynchronously on the context stream; clouds is (out, offsets)."""
+        fields, nan_layers = list(fields), set(nan_layers)
+        if len(set(fields)) != len(fields):
+            raise ValueError(f"fields {fields}: each name once")
+        bits = []
+        for f in fields:
+            if f not in nan_layers and f not in LAYER_BITS:
+                raise ValueError(f"field {f!r}: neither a layer ({tuple(LAYER_BITS)}) nor one of nan_layers")
+            bits.append(0 if f in nan_layers else 1 << LAYER_BITS[f])
+        if point_layer not in LAYER_BITS:
+            raise ValueError(f"point_layer {point_layer!r}: not a layer of {tuple(LAYER_BITS)}")
+        fa = np.ascontiguousarray(bits, dtype=np.uint32)
+        layout, step = point_cloud_fields(fields, point_layer)
+        idx = None if maps is None else self._map_index(maps)
+        n = self._n if idx is None else len(idx)
+        fn = self._L.te_map_get_point_cloud
+        args = (self._h, 0 if idx is None else len(idx), _addr(idx), len(fa), _addr(fa), 1 << LAYER_BITS[point_layer],
+                layer_mask(basic) if len(basic) else 0)
+        if memory != MEM_HOST:
+            cap = out.numel() // step if capacity is None else int(capacity)
+            self._ctx._order_after_torch(memory)
+            self._check(fn(*args, _addr(out), cap, _addr(offsets), memory))
+            return layout, step, (out, offsets)
+        offsets = np.full(n + 1, -1, dtype=np.int64)
+        if capacity is None:                      # a sizing call: offsets only
+            rc = fn(*args, None, 0, _addr(offsets), memory)
+            if rc != 0 and offsets[0] != 0:
+                self._check(rc)
+            capacity = int(offsets[-1])
+        data = np.empty(int(capacity) * step, dtype=np.uint8)
+        self._check(fn(*args, _addr(data), int(capacity), _addr(offsets), memory))
+        dt = point_cloud_dtype(layout, step)
+        return layout, step, [data[offsets[k] * step:offsets[k + 1] * step].view(dt) for k in range(n)]

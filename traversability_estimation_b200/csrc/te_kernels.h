@@ -81,6 +81,45 @@ struct MapOccupancy {
 };
 // One k_map_occupancy launch for every layer and map (none when there is no cell).
 void launch_map_occupancy(const MapOccupancy& a, int sms, cudaStream_t s);
+// te_map_get_point_cloud: GridMapRosConverter::toPointCloud of nmaps maps (device pointers), an ordered stream compaction.  Map k of
+// the call is cut into `tiles` tiles of kCloudTile consecutive cells of its buffer order (linear index b: buffer cell (b % rows,
+// b / rows), which is default-order cell ((b % rows - sr) mod rows, (b / rows - sc) mod cols)).  A cell is a point where the point
+// layer and every basic layer are finite; its record is nfields entries of 4 bytes, entry point_e (if any) as x, y, z.  A layer
+// source whose bit is set in its *_range mask is uncertainty_range: that pointer is upper_bound, and `lower` is subtracted.
+constexpr int kCloudMaxFields = 32;
+constexpr int kCloudMaxBasic = 17;  // te_layer bits 0 .. 17 but the unassigned 7
+constexpr int kCloudTile = 1024;    // cells per tile: 4 chunks of one 256-thread block
+struct CloudMap {                   // one map of a call: its slot in the te_map, start index and position
+  int slot, sr, sc, pad;
+  double px, py;
+};
+struct MapCloud {
+  const float* field[kCloudMaxFields];  // entry e's resident layer, every map back to back; null: the NaN 0x7fc00000
+  unsigned field_range;
+  int nfields, point_e;                 // point_e: the entry that expands to x, y, z, or -1
+  const float* point;
+  const float* basic[kCloudMaxBasic];
+  unsigned basic_range;                 // bit b: basic[b]; bit 31: point
+  int nbasic;
+  const float* lower;
+  int rows, cols, nmaps, tiles;         // tiles per map
+  long long cells;                      // rows * cols
+  const CloudMap* maps;                 // device, nmaps; null: map k in slot k at (sr, sc) and (px, py)
+  int sr, sc;
+  double px, py, lenx, leny, res;
+  unsigned long long* count;            // nmaps * tiles + 1 entries (the last 0)
+  unsigned long long* first;            // their exclusive prefix sum: a tile's first point; first[k * tiles] is map k's offset
+  long long* offsets;                   // device memory: gets first[k * tiles] for k = 0 .. nmaps; null in host memory
+  int point_step;                       // bytes: 4 * (nfields + 2 when point_e >= 0)
+  long long capacity;                   // points at or past it are not written
+  unsigned char* out;
+};
+// Bytes of the device scratch the scan of launch_map_cloud_count needs for n tile counts.
+size_t map_cloud_scan_bytes(long long n);
+// k_map_cloud_count, then the exclusive sum of the counts into a.first (cub, in tmp of tmp_bytes): two launches.
+cudaError_t launch_map_cloud_count(const MapCloud& a, void* tmp, size_t tmp_bytes, int sms, cudaStream_t s);
+// k_map_cloud_scatter: every point below a.capacity to its record at a.out + point index * point_step, and a.offsets.  One launch.
+void launch_map_cloud_scatter(const MapCloud& a, int sms, cudaStream_t s);
 struct GridGeo;
 // valid[q] = getIndex(xy[2q], xy[2q+1]) succeeds and traversability is finite there (device pointers; none launched for n = 0).
 // A batch of nmaps maps of geometry g back to back in `trav`: position q is on map pos_map[q] (null: map 0), and a map outside

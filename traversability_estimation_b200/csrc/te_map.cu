@@ -69,6 +69,13 @@ struct te_map {
     size_t mask_off = 0;
     DevBuf buf;
   } tab_all, tab_launch;
+  // te_map_get_point_cloud: the tile counts, their prefix sums and the scan's scratch; and the per-map tables (te::CloudMap) of a
+  // whole batch and of a selection, each uploaded only when it changes, so that a captured whole-batch call keeps reading its own.
+  DevBuf cloud;
+  struct CloudTab {
+    std::vector<te::CloudMap> key;
+    DevBuf buf;
+  } cloud_all, cloud_sel;
 };
 
 namespace {
@@ -400,6 +407,9 @@ int te_map_destroy(te_map* m) {
       for (DevBuf& b : m->sel) b.release();
       m->tab_all.buf.release();
       m->tab_launch.buf.release();
+      m->cloud.release();
+      m->cloud_all.buf.release();
+      m->cloud_sel.buf.release();
       m->fp.release();
     }
   }
@@ -1887,5 +1897,127 @@ int te_map_get_occupancy(te_map* m, int32_t nsel, const int32_t* map_index, uint
   if (st.rc) return st.rc;
   te::launch_map_occupancy(a, c->sms, c->stream);
   if (int rc = launch_check(c, "k_map_occupancy")) return rc;
+  return st.finish();  // host memory: returns synchronised
+}
+
+namespace {
+
+// The device copy of a call's per-map table t, uploaded only when it differs from what the buffer holds; growing it first waits for
+// the launches that may still read it.
+int cloud_table(te_map* m, te_map::CloudTab& t, const std::vector<te::CloudMap>& v, const te::CloudMap** out) {
+  const size_t bytes = sizeof(te::CloudMap) * v.size();
+  if (t.key.size() != v.size() || std::memcmp(t.key.data(), v.data(), bytes) != 0) {
+    if (t.buf.p && t.buf.cap < bytes) TE_CUDA(cudaStreamSynchronize(m->ctx->stream));
+    TE_CUDA(t.buf.reserve(bytes));
+    t.key = v;  // pageable: consumed before cudaMemcpyAsync returns
+    TE_CUDA(cudaMemcpyAsync(t.buf.p, t.key.data(), bytes, cudaMemcpyHostToDevice, m->ctx->stream));
+  }
+  *out = (const te::CloudMap*)t.buf.p;
+  return TE_OK;
+}
+
+}  // namespace
+
+int te_map_get_point_cloud(te_map* m, int32_t nsel, const int32_t* map_index, int32_t nfields, const uint32_t* fields,
+                           uint32_t point_layer, uint32_t basic_mask, void* data, int64_t capacity_points, int64_t* offsets,
+                           int memory) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (nfields < 1 || nfields > te::kCloudMaxFields) return fail(TE_ERR_BAD_ARG, "nfields = %d: need 1..%d", nfields, te::kCloudMaxFields);
+  if (!fields || !offsets) return fail(TE_ERR_BAD_ARG, "fields or offsets is null");
+  if (capacity_points < 0) return fail(TE_ERR_BAD_ARG, "negative capacity_points");
+  if (!data && capacity_points > 0) return fail(TE_ERR_BAD_ARG, "data is null with capacity_points %lld", (long long)capacity_points);
+  const uint32_t known = TE_LAYER_ALL | TE_LAYER_CARRIED | TE_LAYER_UNCERTAINTY_RANGE | TE_LAYER_TRAVERSABILITY_X | TE_LAYER_TRAVERSABILITY_ROT;
+  const auto one_bit = [&](uint32_t b) { return b != 0 && (b & (b - 1)) == 0 && (b & known) != 0; };
+  uint32_t given = 0;
+  for (int e = 0; e < nfields; ++e) {
+    const uint32_t f = fields[e];
+    if (f == 0) continue;
+    if (!one_bit(f)) return fail(TE_ERR_BAD_ARG, "fields[%d] = 0x%x: need 0 (a NaN field) or one te_layer bit", e, f);
+    if (given & f) return fail(TE_ERR_BAD_ARG, "fields[%d] = 0x%x appears twice", e, f);
+    given |= f;
+  }
+  if (!one_bit(point_layer)) return fail(TE_ERR_BAD_ARG, "point_layer 0x%x: need one te_layer bit", point_layer);
+  if (basic_mask & ~known) return fail(TE_ERR_BAD_ARG, "basic_mask 0x%x has bits outside 0x%x", basic_mask, known);
+  if (memory != TE_MEM_HOST && memory != TE_MEM_DEVICE) return fail(TE_ERR_BAD_ARG, "unknown memory mode %d", memory);
+  const bool whole = nsel == 0 && !map_index;
+  if (!whole)
+    if (int rc = check_selection(m, MapSel{nsel, map_index})) return rc;
+  const float* held_src[kLayerBits];
+  int nl = 0;
+  if (int rc = map_layers(m, given | point_layer | basic_mask, true, held_src, &nl)) return rc;  // TE_ERR_MISSING_LAYER
+
+  // uncertainty_range reads upper_bound and subtracts lower_bound
+  const auto src = [&](uint32_t bit) { return bit == TE_LAYER_UNCERTAINTY_RANGE ? lay(m, TE_LAYER_UPPER_BOUND) : lay(m, bit); };
+  te::MapCloud a{};
+  a.point_e = -1;
+  for (int e = 0; e < nfields; ++e) {
+    if (fields[e] == point_layer) a.point_e = e;
+    else if (fields[e]) a.field[e] = src(fields[e]);
+    if (fields[e] == TE_LAYER_UNCERTAINTY_RANGE) a.field_range |= 1u << e;
+  }
+  a.nfields = nfields;
+  a.point = src(point_layer);
+  if (point_layer == TE_LAYER_UNCERTAINTY_RANGE) a.basic_range |= 1u << 31;
+  for (int b = 0; b < kLayerBits; ++b) {
+    if (!((basic_mask >> b) & 1u)) continue;
+    if (b == 15) a.basic_range |= 1u << a.nbasic;
+    a.basic[a.nbasic++] = src(1u << b);
+  }
+  if (((given | point_layer | basic_mask) & TE_LAYER_UNCERTAINTY_RANGE)) a.lower = lay(m, TE_LAYER_LOWER_BOUND);
+  a.point_step = 4 * (nfields + (a.point_e >= 0 ? 2 : 0));
+
+  // each map's slot, start index (a single map's may have come in g) and position
+  const int n = whole ? m->nmaps : nsel;
+  const te_geometry& g = m->geo;
+  std::vector<te::CloudMap> maps(n);
+  for (int k = 0; k < n; ++k) {
+    const int s = whole ? k : map_index[k];
+    const bool in_g = m->geo_in.start_row != 0 || m->geo_in.start_col != 0;
+    const bool at = !m->pos.empty();
+    maps[k] = te::CloudMap{s, in_g ? m->geo_in.start_row : m->start[2 * s], in_g ? m->geo_in.start_col : m->start[2 * s + 1], 0,
+                           at ? m->pos[2 * s] : g.position_x, at ? m->pos[2 * s + 1] : g.position_y};
+  }
+  bool uniform = whole;  // a whole batch with one start index and position takes them by value
+  for (int k = 1; k < n && uniform; ++k)
+    uniform = maps[k].sr == maps[0].sr && maps[k].sc == maps[0].sc && std::memcmp(&maps[k].px, &maps[0].px, 2 * sizeof(double)) == 0;
+  if (uniform) {
+    a.sr = maps[0].sr; a.sc = maps[0].sc; a.px = maps[0].px; a.py = maps[0].py;
+  } else if (int rc = cloud_table(m, whole ? m->cloud_all : m->cloud_sel, maps, &a.maps)) {
+    return rc;
+  }
+  a.rows = g.rows; a.cols = g.cols; a.nmaps = n; a.cells = (long long)map_cells(m);
+  a.lenx = g.length_x; a.leny = g.length_y; a.res = g.resolution;
+  a.tiles = (int)((a.cells + te::kCloudTile - 1) / te::kCloudTile);
+
+  // scratch: the counts, their prefix sums, the scan's temporary storage
+  const long long nt = (long long)n * a.tiles + 1;
+  const size_t cbytes = (sizeof(unsigned long long) * nt + 255) / 256 * 256, tmp_bytes = te::map_cloud_scan_bytes(nt);
+  if (m->cloud.p && m->cloud.cap < 2 * cbytes + tmp_bytes) TE_CUDA(cudaStreamSynchronize(c->stream));
+  TE_CUDA(m->cloud.reserve(2 * cbytes + tmp_bytes));
+  a.count = (unsigned long long*)m->cloud.p;
+  a.first = (unsigned long long*)((char*)m->cloud.p + cbytes);
+  TE_CUDA(te::launch_map_cloud_count(a, (char*)m->cloud.p + 2 * cbytes, tmp_bytes, c->sms, c->stream));
+  if (int rc = launch_check(c, "k_map_cloud_count, DeviceScan", 2)) return rc;
+  // offsets[k] = the first point of map k's first tile; offsets[n] = the total (the entry after the last tile).  Host memory
+  // copies them back before the scatter; in device memory the scatter kernel writes them.
+  const bool host = memory == TE_MEM_HOST;
+  a.capacity = capacity_points;
+  a.out = (unsigned char*)data;
+  a.offsets = host ? nullptr : (long long*)offsets;
+  Staging st(c, host, &g);  // host memory: the records into staging, then one copy of total * point_step bytes
+  if (host) {
+    TE_CUDA(cudaMemcpy2DAsync(offsets, sizeof(int64_t), a.first, sizeof(int64_t) * a.tiles, sizeof(int64_t), n + 1,
+                              cudaMemcpyDeviceToHost, c->stream));
+    TE_CUDA(cudaStreamSynchronize(c->stream));
+    if (offsets[n] > capacity_points)
+      return fail(TE_ERR_BAD_ARG, "the clouds hold %lld points but data has room for %lld: call again with more room",
+                  (long long)offsets[n], (long long)capacity_points);
+    a.capacity = offsets[n];
+    a.out = st.out((uint8_t*)data, (size_t)offsets[n] * a.point_step);
+    if (st.rc) return st.rc;
+  }
+  te::launch_map_cloud_scatter(a, c->sms, c->stream);
+  if (int rc = launch_check(c, "k_map_cloud_scatter")) return rc;
   return st.finish();  // host memory: returns synchronised
 }

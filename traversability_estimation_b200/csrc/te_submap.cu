@@ -1,8 +1,12 @@
 // te_submap.cu — the read side of a te_map: GetGridMap submaps of its resident layers (k_map_gather_submaps),
 // mapHasValidTraversabilityAt for a batch of positions (k_map_valid_at), GridMap::atPosition at points around poses
-// (k_map_at_poses) and GridMapRosConverter::toOccupancyGrid of its layers (k_map_occupancy); and the windows a te_map update cuts out of a larger elevation map (k_map_cut_windows).  Compiled with --fmad=false: k_map_valid_at and k_map_at_poses index positions with te_grid.cuh's getIndex,
-// which the host and the oracle evaluate without contraction, and k_map_at_poses places points as the polygonal paths do.
+// (k_map_at_poses), GridMapRosConverter::toOccupancyGrid of its layers (k_map_occupancy) and toPointCloud (k_map_cloud_count,
+// k_map_cloud_scatter); and the windows a te_map update cuts out of a larger elevation map (k_map_cut_windows).  Compiled with --fmad=false: k_map_valid_at and k_map_at_poses index positions with te_grid.cuh's getIndex,
+// which the host and the oracle evaluate without contraction, k_map_at_poses places points as the polygonal paths do, and
+// k_map_cloud_scatter takes x and y from cell_coord as getPosition computes them.
 #include <algorithm>
+
+#include <cub/device/device_scan.cuh>
 
 #include "te_kernels.h"
 #include "te_grid.cuh"
@@ -239,7 +243,151 @@ __global__ void __launch_bounds__(256) k_map_occupancy(const __grid_constant__ M
   }
 }
 
+// ---- toPointCloud: count the points of every tile, scan the counts, scatter the records --------------------------------------
+
+constexpr int kCloudThreads = 256;  // a tile is kCloudTile / kCloudThreads chunks of one cell per thread
+
+// A layer at absolute cell d (slot * cells + default-order index): the stored bits, or for uncertainty_range (range) upper - lower
+// as te_map_get_layers computes it.
+__device__ __forceinline__ float cloud_read(const float* __restrict__ p, bool range, const float* __restrict__ lower, size_t d) {
+  const float v = __ldg(p + d);
+  return range ? range_sub(v, __ldg(lower + d)) : v;
+}
+
+// Map k of the call: its slot, start index and position.
+__device__ __forceinline__ CloudMap cloud_map(const MapCloud& a, int k) {
+  if (a.maps) return a.maps[k];
+  return CloudMap{k, a.sr, a.sc, 0, a.px, a.py};
+}
+
+// Buffer cell b (< cells) of map M: its default-order row i and column j.
+__device__ __forceinline__ void cloud_cell(const MapCloud& a, const CloudMap& M, unsigned b, int& i, int& j) {
+  const unsigned bj = b / (unsigned)a.rows;
+  i = (int)(b - bj * (unsigned)a.rows) - M.sr;
+  j = (int)bj - M.sc;
+  if (i < 0) i += a.rows;
+  if (j < 0) j += a.cols;
+}
+
+// isValid over the basic layers (when there are any) and getPosition3's check of the point layer at absolute cell d.
+__device__ __forceinline__ bool cloud_valid(const MapCloud& a, size_t d) {
+  if (!isfinite(cloud_read(a.point, a.basic_range >> 31, a.lower, d))) return false;
+  for (int b = 0; b < a.nbasic; ++b)
+    if (!isfinite(cloud_read(a.basic[b], (a.basic_range >> b) & 1u, a.lower, d))) return false;
+  return true;
+}
+
+// One count per tile (grid-stride over the tiles of every map); the entry after the last tile is 0, so that its prefix is the total.
+__global__ void __launch_bounds__(kCloudThreads) k_map_cloud_count(const __grid_constant__ MapCloud a) {
+  const long long ntiles = (long long)a.nmaps * a.tiles;
+  if (blockIdx.x == 0 && threadIdx.x == 0) a.count[ntiles] = 0;
+  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const int k = (int)(t / a.tiles);
+    const CloudMap M = cloud_map(a, k);
+    const long long b0 = (t - (long long)k * a.tiles) * kCloudTile;
+    int n = 0;
+    for (int c = 0; c < kCloudTile / kCloudThreads; ++c) {
+      const long long b = b0 + c * kCloudThreads + threadIdx.x;
+      bool v = false;
+      if (b < a.cells) {
+        int i, j;
+        cloud_cell(a, M, (unsigned)b, i, j);
+        v = cloud_valid(a, (size_t)M.slot * a.cells + (size_t)j * a.rows + i);
+      }
+      n += __syncthreads_count(v);
+    }
+    if (threadIdx.x == 0) a.count[t] = (unsigned long long)n;
+  }
+}
+
+// Every tile again: each chunk of kCloudThreads cells ranks its points with a ballot scan, builds their records in shared memory
+// (point_step bytes each, in point order) and writes them out as consecutive 4-byte words (single bytes when `out` is not 4-byte
+// aligned), so each warp stores one contiguous run.  Points at or past a.capacity are not written.  In device memory it also writes
+// the call's offsets.
+__global__ void __launch_bounds__(kCloudThreads) k_map_cloud_scatter(const __grid_constant__ MapCloud a) {
+  // kCloudThreads records of point_step bytes.  Static, at the largest point_step: dynamic shared memory would make ptxas reserve
+  // shared memory for every kernel of this unit.  48 registers allow 5 blocks per SM, and 6 fit in shared memory.
+  __shared__ unsigned rec[kCloudThreads * (kCloudMaxFields + 2)];
+  __shared__ int wsum[kCloudThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, words = a.point_step >> 2;
+  const long long ntiles = (long long)a.nmaps * a.tiles;
+  const bool aligned = ((uintptr_t)a.out & 3u) == 0;
+  if (a.offsets)
+    for (long long k = (long long)blockIdx.x * kCloudThreads + threadIdx.x; k <= a.nmaps; k += (long long)gridDim.x * kCloudThreads)
+      a.offsets[k] = (long long)a.first[k * a.tiles];
+  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const int k = (int)(t / a.tiles);
+    const CloudMap M = cloud_map(a, k);
+    const long long b0 = (t - (long long)k * a.tiles) * kCloudTile;
+    long long base = (long long)a.first[t];  // the chunk's first point
+    for (int c = 0; c < kCloudTile / kCloudThreads; ++c) {
+      const long long b = b0 + c * kCloudThreads + threadIdx.x;
+      int i = 0, j = 0;
+      size_t d = 0;
+      bool v = false;
+      if (b < a.cells) {
+        cloud_cell(a, M, (unsigned)b, i, j);
+        d = (size_t)M.slot * a.cells + (size_t)j * a.rows + i;
+        v = cloud_valid(a, d);
+      }
+      const unsigned bal = __ballot_sync(0xffffffffu, v);
+      if (lane == 0) wsum[warp] = __popc(bal);
+      __syncthreads();
+      int before = 0, total = 0;
+      for (int w = 0; w < kCloudThreads / 32; ++w) {
+        before += w < warp ? wsum[w] : 0;
+        total += wsum[w];
+      }
+      if (v) {
+        unsigned* r = rec + (size_t)(before + __popc(bal & ((1u << lane) - 1u))) * words;
+        int w = 0;
+        for (int e = 0; e < a.nfields; ++e) {
+          if (e == a.point_e) {
+            r[w++] = __float_as_uint(__double2float_rn(cell_coord(M.px, a.lenx, a.res, i)));
+            r[w++] = __float_as_uint(__double2float_rn(cell_coord(M.py, a.leny, a.res, j)));
+            r[w++] = __float_as_uint(cloud_read(a.point, a.basic_range >> 31, a.lower, d));
+          } else {
+            r[w++] = a.field[e] ? __float_as_uint(cloud_read(a.field[e], (a.field_range >> e) & 1u, a.lower, d)) : 0x7fc00000u;
+          }
+        }
+      }
+      __syncthreads();
+      const long long room = a.capacity - base;
+      const int n = (int)max(0LL, min((long long)total, room));
+      unsigned char* dst = a.out + base * a.point_step;
+      if (aligned) {
+        unsigned* d4 = reinterpret_cast<unsigned*>(dst);
+        for (int w = threadIdx.x; w < n * words; w += kCloudThreads) d4[w] = rec[w];
+      } else {
+        const unsigned char* r1 = reinterpret_cast<const unsigned char*>(rec);
+        for (int w = threadIdx.x; w < n * a.point_step; w += kCloudThreads) dst[w] = r1[w];
+      }
+      base += total;
+      __syncthreads();  // rec and wsum are rewritten by the next chunk
+    }
+  }
+}
+
 }  // namespace
+
+size_t map_cloud_scan_bytes(long long n) {
+  size_t bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)n);
+  return bytes;
+}
+
+cudaError_t launch_map_cloud_count(const MapCloud& a, void* tmp, size_t tmp_bytes, int sms, cudaStream_t s) {
+  const long long ntiles = (long long)a.nmaps * a.tiles;
+  const long long blocks = std::max<long long>(1, std::min<long long>(ntiles, (long long)sms * 16));
+  k_map_cloud_count<<<(unsigned)blocks, kCloudThreads, 0, s>>>(a);
+  return cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, (const unsigned long long*)a.count, a.first, (int)(ntiles + 1), s);
+}
+
+void launch_map_cloud_scatter(const MapCloud& a, int sms, cudaStream_t s) {
+  const long long ntiles = (long long)a.nmaps * a.tiles;
+  const long long blocks = std::max<long long>(1, std::min<long long>(ntiles, (long long)sms * 16));
+  k_map_cloud_scatter<<<(unsigned)blocks, kCloudThreads, 0, s>>>(a);
+}
 
 void launch_map_occupancy(const MapOccupancy& a, int sms, cudaStream_t s) {
   const long long nblocks = (long long)a.nlayers * a.nmaps;
