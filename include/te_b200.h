@@ -826,10 +826,63 @@ int te_map_check_footprint_request_device(te_map* map, const te_footprint_params
                                           uint8_t* is_safe, double* traversability_out, double* area_out, int32_t max_vertices,
                                           int32_t* untraversable_count_or_null, double* untraversable_xy_or_null, int64_t max_checks);
 
+/* Maps with robots of their own (a mixed fleet, simulated environments with randomised robots): the three entries below take the
+ * arguments of the entry they stand for with `params` instead of `p`, a HOST array of nmaps parameter sets indexed by map (not by
+ * path, and for a selection still by map index), read before the call returns.  Map m's paths and sweep read params[m], as a
+ * reference node reads its own robot's traversability_default, max_gap_width, critical_step_height, verify_roughness_footprint,
+ * circular_footprint_offset and radius.
+ *   - Per map: everything a call returns or stores for map m (request outputs and untraversable polygons, the cache, the memo,
+ *     map m's share of te_map_request_stats) is, bit for bit, what the entry it stands for returns or stores on a single-map
+ *     te_map holding map m at its position, given params[m].  With every params[m] equal (the radius aside for the requests,
+ *     which take it per path), each entry is that entry given params[0], launches included.
+ *   - The memo is kept per map: each map's bytes are cleared when its own max_gap_width, critical_step_height or verify_roughness
+ *     differ from those its memo was filled under, and kept otherwise.  The single-parameter entries apply the same rule with p for
+ *     every map.
+ *   - Errors: every rule of the entry applies to each map's params[m] (TE_ERR_BAD_ARG for offset < 0 and, for the sweep, radius
+ *     < 0; for the sweep TE_ERR_UNSUPPORTED for radius + offset over 120 cells; TE_ERR_MISSING_LAYER for verify_roughness without a roughness layer), over every map for a request and over the swept
+ *     maps for the sweep; a null params is TE_ERR_BAD_ARG.  Every error is found on the host, before anything is written: the
+ *     te_map is then unchanged.
+ * Requests: the kernels of the entry they stand for, whatever nmaps and the parameters: a path's circle walks, dedup keys (the map
+ * is part of every key, so two maps never share a walk), replay, polygons and polygonal items read its map's parameters from a
+ * per-map table the te_map keeps on the device (40 bytes per map, uploaded only when its bytes change, so a call with unchanged
+ * parameters makes no host synchronisation and can be captured in a CUDA graph).  When every map's entry is the same there is no
+ * table. */
+int te_map_check_footprint_request_each(te_map* map, const te_footprint_params* params, const int32_t* path_map, int32_t npaths,
+                                        int32_t nposes, const int32_t* path_begin, const double* poses, const double* radius,
+                                        int32_t nvertices, const int32_t* footprint_begin, const float* footprint_xyz,
+                                        int32_t max_footprint_vertices, const uint8_t* conservative_or_null,
+                                        const uint8_t* compute_untraversable_polygon_or_null, uint8_t* is_safe,
+                                        double* traversability_out, double* area_out, int32_t max_vertices,
+                                        int32_t* untraversable_count_or_null, double* untraversable_xy_or_null);
+int te_map_check_footprint_request_device_each(te_map* map, const te_footprint_params* params, const int32_t* path_map_or_null,
+                                               int32_t npaths, int32_t nposes, const int32_t* path_begin, const double* poses,
+                                               const double* radius, int32_t nvertices, const int32_t* footprint_begin,
+                                               const float* footprint_xyz, int32_t max_footprint_vertices,
+                                               const uint8_t* conservative_or_null,
+                                               const uint8_t* compute_untraversable_polygon_or_null, uint8_t* is_safe,
+                                               double* traversability_out, double* area_out, int32_t max_vertices,
+                                               int32_t* untraversable_count_or_null, double* untraversable_xy_or_null,
+                                               int64_t max_checks);
+/* traversabilityFootprint(radius, offset) on the caches of every map (nsel = 0, map_index_or_null NULL: te_map_footprint) or of the
+ * maps map_index[0..nsel) (te_map_footprint_maps, whose rules apply), map m with params[m]; the output holds the swept caches
+ * afterwards as that entry's does.  The swept maps are grouped by bitwise-identical params entries and each group is swept as one
+ * te_map_footprint_maps selection: the sweep's per-radius tables stay kernel parameters.  Launches: those of te_map_footprint_maps
+ * (without output) once per distinct parameter set, plus, with an output and more than one set, the gather of the swept caches
+ * that te_map_get_footprint (a whole batch) or te_map_footprint_maps (a selection) makes for its output.  One set is the entry it
+ * stands for, launches included; a te_map whose start index came in g holds one map, so it always has one set.  Each set
+ * other than the previous sweep's rebuilds the sweep's tables on the host, as
+ * te_map_footprint does when its parameters change.  Unknown memory modes are TE_ERR_BAD_ARG. */
+int te_map_footprint_each(te_map* map, const te_footprint_params* params, int32_t nsel, const int32_t* map_index_or_null,
+                          float* traversability_footprint_or_null, int memory);
+
 /* The cache as publishTraversabilityMap publishes its traversability_footprint layer (in host memory: in the map's buffer
  * order; device memory needs a map without a start index), and resetTraversabilityFootprintLayers (:195-200).  On a batch: every
  * map's cache, back to back. */
 int te_map_get_footprint(te_map* map, float* traversability_footprint, int memory);
+/* The isTraversableForFilters memo the requests keep, one byte per cell of every map (maps back to back, each column-major in
+ * default order, whatever its start index): 0 not evaluated since the memo was last cleared for that map, 1 passes, 2 blocked.
+ * Host memory, returns synchronised.  No reference counterpart: it lets a caller see which maps' memo a call kept. */
+int te_map_get_memo(te_map* map, uint8_t* memo);
 int te_map_clear_footprint(te_map* map);
 
 /* Counters of the last te_map_check_footprint_request(_batched): out[0] isTraversable calls its circular paths could make, out[1]

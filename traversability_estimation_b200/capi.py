@@ -207,7 +207,12 @@ SIGNATURES = {
     "te_map_check_footprint_request": (_R, [_P, _FP, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
     "te_map_check_footprint_request_batched": (_R, [_P, _FP, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
     "te_map_check_footprint_request_device": (_R, [_P, _FP, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P, _L]),
+    "te_map_check_footprint_request_each": (_R, [_P, _FP, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P]),
+    "te_map_check_footprint_request_device_each": (_R, [_P, _FP, _P, _I, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P, _I, _P, _P,
+                                                        _L]),
+    "te_map_footprint_each": (_R, [_P, _FP, _I, _P, _P, _I]),
     "te_map_get_footprint": (_R, [_P, _P, _I]),
+    "te_map_get_memo": (_R, [_P, _P]),
     "te_map_clear_footprint": (_R, [_P]),
     "te_map_request_stats": (_R, [_P, _P]),
     "te_map_carry_layers": (_R, [_P, _I, _P, _U, _P, _I]),
@@ -1062,6 +1067,39 @@ class Map:
         self._check(self._L.te_map_footprint_maps(self._h, C.byref(fp), len(idx), _addr(idx), _addr(buf), MEM_HOST))
         return buf.transpose(0, 2, 1)
 
+    def _params(self, params):
+        """A ctypes array of one FootprintParams per map of the te_map (the _each entries); such an array is passed as it is."""
+        if isinstance(params, C.Array):
+            if len(params) != self._n:
+                raise ValueError(f"{len(params)} parameter sets for a te_map of {self._n} maps: need one per map")
+            return params
+        params = list(params)
+        if len(params) != self._n:
+            raise ValueError(f"{len(params)} parameter sets for a te_map of {self._n} maps: need one per map")
+        return (FootprintParams * len(params))(*params)
+
+    def footprint_each(self, params, map_index=None, memory=MEM_HOST, out=None):
+        """te_map_footprint_each: traversabilityFootprint(radius, offset) on every map's cache (map_index None) or on the maps
+        map_index only, map m with params[m] (one FootprintParams per map).  Host memory returns the swept caches afterwards, as
+        footprint (whole batch) or footprint_maps (a selection) do; device memory fills `out` (a float32 device tensor of the swept
+        maps' cells, or None) asynchronously on the context stream and returns it."""
+        arr = self._params(params)
+        idx = None if map_index is None else self._map_index(map_index)
+        nsel = 0 if idx is None else len(idx)
+        fn = self._L.te_map_footprint_each
+        if memory != MEM_HOST:
+            self._ctx._order_after_torch(memory)
+            self._check(fn(self._h, arr, nsel, _addr(idx), _addr(out), memory))
+            return out
+        if idx is None:
+            buf, res = self._layer_out()
+        else:
+            rows, cols = self._shape()
+            buf = np.empty((nsel, cols, rows), dtype=np.float32)
+            res = buf.transpose(0, 2, 1)
+        self._check(fn(self._h, arr, nsel, _addr(idx), _addr(buf), MEM_HOST))
+        return res
+
     def footprint(self, fp):
         """te_map_footprint (traversabilityFootprint(radius, offset) on the cache); returns the cache afterwards."""
         fn = self._L.te_map_footprint
@@ -1143,12 +1181,23 @@ class Map:
         return self._request(fp, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices, conservative,
                              compute_untraversable_polygon, untraversable_capacity, path_map=path_map)
 
+    def check_footprint_request_each(self, params, path_map, path_begin, poses, radius, footprint_begin, footprint_xyz,
+                                     max_footprint_vertices=None, conservative=None, compute_untraversable_polygon=None,
+                                     untraversable_capacity=None):
+        """te_map_check_footprint_request_each: check_footprint_request_batched with map m's paths checked with params[m] (one
+        FootprintParams per map)."""
+        return self._request(None, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices, conservative,
+                             compute_untraversable_polygon, untraversable_capacity, path_map=path_map, params=params)
+
     def _request(self, fp, path_begin, poses, radius, footprint_begin, footprint_xyz, max_footprint_vertices, conservative,
-                 compute_untraversable_polygon, untraversable_capacity, path_map=None):
-        """The body of check_footprint_request (path_map None) and check_footprint_request_batched: the batched entry takes
-        path_map after the parameters."""
+                 compute_untraversable_polygon, untraversable_capacity, path_map=None, params=None):
+        """The body of check_footprint_request (path_map None), check_footprint_request_batched and check_footprint_request_each
+        (params: one set per map instead of fp): the batched entries take path_map after the parameters."""
         batched = path_map is not None
         fn = self._L.te_map_check_footprint_request_batched if batched else self._L.te_map_check_footprint_request
+        if params is not None:
+            fn = self._L.te_map_check_footprint_request_each
+        par = C.byref(fp) if params is None else self._params(params)
         pm = [np.ascontiguousarray(path_map, dtype=np.int32)] if batched else []
         pb = np.ascontiguousarray(path_begin, dtype=np.int32)
         ps = np.ascontiguousarray(poses, dtype=np.float64).reshape(-1, 7)
@@ -1165,7 +1214,7 @@ class Map:
         counts, uxy = (None, None) if untraversable_capacity is None else _untraversable_outputs(n, maxv)
         if batched and len(pm[0]) != n:
             raise ValueError("path_map needs one entry per path")
-        self._check(fn(self._h, C.byref(fp), *(a.ctypes.data for a in pm), n, len(ps), pb.ctypes.data, ps.ctypes.data,
+        self._check(fn(self._h, par, *(a.ctypes.data for a in pm), n, len(ps), pb.ctypes.data, ps.ctypes.data,
                        rad.ctypes.data, len(fxyz), fb.ctypes.data, fxyz.ctypes.data, int(max_footprint_vertices), _addr(cons),
                        _addr(cup), safe.ctypes.data, trav.ctypes.data, area.ctypes.data, maxv, _addr(counts), _addr(uxy)))
         if untraversable_capacity is None:
@@ -1175,17 +1224,20 @@ class Map:
     def check_footprint_request_device(self, fp, path_begin, poses, radius, footprint_begin, footprint_xyz, is_safe,
                                        traversability_out, area_out, max_checks, path_map=None, max_footprint_vertices=None,
                                        conservative=None, compute_untraversable_polygon=None, untraversable_capacity=None,
-                                       untraversable_count=None, untraversable_xy=None):
+                                       untraversable_count=None, untraversable_xy=None, params=None):
         """te_map_check_footprint_request_device: check_footprint_request(_batched) with every argument a device tensor, as
         Context.check_footprint_request(memory=MEM_DEVICE) takes them (path_map int32 per path, None on a map of one map), results
         in the caller's tensors.  Asynchronous: ordered after torch's current stream, no host synchronisation.  max_checks sizes
-        the work list of circle checks (te_b200.h).  max_footprint_vertices defaults to 16."""
+        the work list of circle checks (te_b200.h).  max_footprint_vertices defaults to 16.  params (a host sequence of one
+        FootprintParams per map, fp then unused): te_map_check_footprint_request_device_each."""
         self._ctx._order_after_torch(MEM_DEVICE)
         n = int(path_begin.numel()) - 1
         mfv = 16 if max_footprint_vertices is None else int(max_footprint_vertices)
         maxv = 0 if untraversable_capacity is None else int(untraversable_capacity)
-        self._check(self._L.te_map_check_footprint_request_device(
-            self._h, C.byref(fp), _addr(path_map), n, int(poses.numel()) // 7, _addr(path_begin), _addr(poses), _addr(radius),
+        fn = self._L.te_map_check_footprint_request_device if params is None else self._L.te_map_check_footprint_request_device_each
+        par = C.byref(fp) if params is None else self._params(params)
+        self._check(fn(
+            self._h, par, _addr(path_map), n, int(poses.numel()) // 7, _addr(path_begin), _addr(poses), _addr(radius),
             int(footprint_xyz.numel()) // 3, _addr(footprint_begin), _addr(footprint_xyz), mfv, _addr(conservative),
             _addr(compute_untraversable_polygon), _addr(is_safe), _addr(traversability_out), _addr(area_out), maxv,
             _addr(untraversable_count), _addr(untraversable_xy), int(max_checks)))
@@ -1201,6 +1253,15 @@ class Map:
         buf, out = self._layer_out()
         self._check(fn(self._h, _addr(buf), MEM_HOST))
         return out
+
+    def get_memo(self):
+        """te_map_get_memo: the isTraversableForFilters memo bytes (0 not evaluated, 1 passes, 2 blocked), uint8 (rows, cols), or
+        (nmaps, rows, cols) on a batch, every map in default order."""
+        rows, cols = self._shape()
+        buf = np.empty((self._n, cols, rows), dtype=np.uint8)
+        self._check(self._L.te_map_get_memo(self._h, buf.ctypes.data))
+        out = buf.transpose(0, 2, 1)
+        return out[0] if self._n == 1 else out
 
     def clear_footprint(self):
         """te_map_clear_footprint (resetTraversabilityFootprintLayers)."""

@@ -1152,7 +1152,7 @@ int te_check_footprint_paths_polygon2(te_ctx* c, const te_geometry* g_in, const 
 int te::host::check_request_host(const te_geometry* g, const te_footprint_params* p, int32_t npaths, int32_t nposes,
                                  const int32_t* path_begin, const double* poses, const double* radius, int32_t nvertices,
                                  const int32_t* footprint_begin, const float* footprint_xyz, int32_t max_footprint_vertices,
-                                 const uint8_t* conservative, int* mp_out) {
+                                 const uint8_t* conservative, int* mp_out, bool per_map, const int32_t* path_map) {
   if (path_begin[0] < 0) return fail(TE_ERR_BAD_ARG, "path_begin[0] must be >= 0");
   if (path_begin[npaths] != nposes) return fail(TE_ERR_BAD_ARG, "path_begin[npaths] = %d != nposes = %d", path_begin[npaths], nposes);
   if (footprint_begin[0] != 0) return fail(TE_ERR_BAD_ARG, "footprint_begin[0] must be 0, got %d", footprint_begin[0]);
@@ -1166,7 +1166,7 @@ int te::host::check_request_host(const te_geometry* g, const te_footprint_params
   for (int32_t q = 0; q < npaths; ++q) {
     const int32_t n = path_begin[q + 1] - path_begin[q], nfp = footprint_begin[q + 1] - footprint_begin[q];
     if (nfp == 0) {  // circular: te_check_footprint_paths_fresh2
-      if (int rc = check_circular_radius(g, p, q, radius[q])) return rc;
+      if (int rc = check_circular_radius(g, per_map ? p + (path_map ? path_map[q] : 0) : p, q, radius[q])) return rc;
       continue;
     }
     // polygonal: te_check_footprint_paths_polygon2

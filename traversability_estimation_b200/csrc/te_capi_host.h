@@ -178,10 +178,12 @@ int check_reduce_outputs(const te::PolygonReduce& r);
 // for max_vertices >= 0 points per path (xy may be null only when max_vertices is 0).
 int check_polygon_outputs(int32_t max_vertices, const int32_t* ucount, const double* uxy);
 // The host-side validation of a te_check_footprint_request request (paths, footprints, radii, conservative caps, finite poses and
-// vertices); sets *mp to the hull input bound of a polygonal item.
+// vertices); sets *mp to the hull input bound of a polygonal item.  per_map: p holds one parameter set per map and path q uses
+// that of its map, p[path_map[q]] (path_map null: p[0]).
 int check_request_host(const te_geometry* g, const te_footprint_params* p, int32_t npaths, int32_t nposes, const int32_t* path_begin,
                        const double* poses, const double* radius, int32_t nvertices, const int32_t* footprint_begin,
-                       const float* footprint_xyz, int32_t max_footprint_vertices, const uint8_t* conservative, int* mp_out);
+                       const float* footprint_xyz, int32_t max_footprint_vertices, const uint8_t* conservative, int* mp_out,
+                       bool per_map = false, const int32_t* path_map = nullptr);
 // Stages the path arrays of `r` and points `r` at the device copies (host memory; null stays null).
 void stage_paths(Staging& st, te::PathChecks& r);
 

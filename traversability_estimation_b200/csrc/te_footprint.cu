@@ -390,6 +390,10 @@ FpArgs geometry_args(const SlabView& v, const te_geometry* g) {
   return a;
 }
 
+bool footprint_reach_ok(double resolution, const te_footprint_params* p) {
+  return !(std::ceil((p->radius + p->offset) / resolution) > 120.0);
+}
+
 int footprint_halo(const te_geometry* g, const te_footprint_params* p) {
   const double res = g->resolution;
   const int spiral = (int)std::ceil((p->radius + p->offset) / res);
@@ -444,7 +448,7 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
                      const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
                      float* step_fp, float* rough_fp, int sms, cudaStream_t s, int* launches) {
   const double rmax = p->radius + p->offset;
-  if (std::ceil(rmax / g->resolution) > 120.0) { st.why = "footprint radius exceeds 120 cells"; return TE_ERR_UNSUPPORTED; }
+  if (!footprint_reach_ok(g->resolution, p)) { st.why = "footprint radius exceeds 120 cells"; return TE_ERR_UNSUPPORTED; }
   if (!st.valid || std::memcmp(&st.key_geo, g, sizeof(*g)) != 0 || std::memcmp(&st.key_par, p, sizeof(*p)) != 0) {
     const std::vector<int> sp = build_spiral(rmax, g->resolution);
     if (st.spiral.reserve(sp.size() * sizeof(int)) != cudaSuccess) { st.why = "allocating the spiral table failed"; return TE_ERR_CUDA; }

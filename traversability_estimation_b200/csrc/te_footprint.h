@@ -42,6 +42,17 @@ struct FootprintState {
 };
 
 int footprint_halo(const te_geometry* g, const te_footprint_params* p);
+// Whether launch_footprint takes p's circle at this resolution: radius + offset within 120 cells (TE_ERR_UNSUPPORTED otherwise).
+bool footprint_reach_ok(double resolution, const te_footprint_params* p);
+
+// The parameters a request reads per map when the maps of a te_map batch have robots of their own (te_map_check_footprint_request
+// _each / _device_each): the circle walk's offset and traversability_default, SpiralIterator's radius flag and the
+// isTraversableForFilters parameters, each as filter_args / path_args take it from a te_footprint_params.  A device table of one
+// entry per map (FpArgs::mp); the radius is a path's own, so it is not here.
+struct FpMapParams {
+  double offset, tdefault, maxgap, crit;
+  int int_norm, verify_rough;
+};
 
 // The sweeps run on `nmaps` (1 .. 65535) maps of the slab's shape stored back to back: map m's layers start m * rows * in_ncols
 // cells into every input, its outputs m * rows * out_ncols cells into every output.  The tables are built once per call.
@@ -128,6 +139,9 @@ struct PathChecks {
   int max_vertices;
   int* ucount;                        // null: no untraversable polygons; else per path a vertex count and max_vertices points in uxy
   double* uxy;
+  // A te_map batch whose maps have parameters of their own: device table of nmaps entries; null: the call's one parameter set
+  // for every map.  Read by launch_map_request_device and by launch_path_checks' polygonal kernels.
+  const FpMapParams* map_params;
 };
 // Asynchronous on `s`.  Launches one kernel for the circular paths (when `r` can have any and `circular` is set; a te_map checks
 // them on its cache instead), then for the polygonal paths an items kernel when there are poses and a combine kernel, whatever the

@@ -63,6 +63,9 @@ struct FpArgs {
   // its position is pos[2m], pos[2m + 1]; xs = ys = 0 and pos null: every map at (posx, posy)
   int xs, ys;
   const double* pos;
+  // maps with parameters of their own (PathChecks::map_params): map m reads mp[m] instead of tdefault, maxgap, crit, int_norm,
+  // verify_rough and the walk's offset (map_params_d, map_walk_offset_d); null: every map reads the fields above
+  const FpMapParams* mp;
 };
 
 constexpr int kPathMaxRings = 127;  // the signed-byte packing of the ring table
@@ -118,6 +121,33 @@ __device__ __forceinline__ FpArgs map_args_d(const FpArgs& A, unsigned m) {
   a.posx = A.pos[2 * (size_t)m];
   a.posy = A.pos[2 * (size_t)m + 1];
   return a;
+}
+
+// Map m's own parameters (A.mp) over those of the call, for a batch whose maps have parameters of their own.
+__device__ __forceinline__ void map_params_d(FpArgs& A, unsigned m) {
+  const FpMapParams q = A.mp[m];
+  A.tdefault = q.tdefault;
+  A.maxgap = q.maxgap;
+  A.crit = q.crit;
+  A.int_norm = q.int_norm;
+  A.verify_rough = q.verify_rough;
+}
+
+// The arguments of path or key map m: its tables and position when the maps sit at their own (AT), its parameters when the maps
+// have their own (EACH: A.mp is set).  Kernels instantiate EACH apart so that the one-parameter-set case keeps its parameters in
+// the constant bank, and its registers.
+template <bool AT, bool EACH>
+__device__ __forceinline__ FpArgs map_view_d(const FpArgs& A0, unsigned m) {
+  FpArgs a = AT ? map_args_d(A0, m) : A0;
+  if constexpr (EACH) map_params_d(a, m);
+  return a;
+}
+
+// radiusMax - radius of map m's circle walks: its own offset when the maps have their own parameters (EACH), else the call's.
+template <bool EACH>
+__device__ __forceinline__ double map_walk_offset_d(const FpArgs& A, double offset, unsigned m) {
+  if constexpr (EACH) return A.mp[m].offset;
+  return offset;
 }
 
 __device__ __forceinline__ bool is_inside_d(const FpArgs& A, double px, double py) {

@@ -47,9 +47,16 @@ struct te_map {
   DevBuf cut;    // the window table of k_map_cut_windows (te_map_chain_submap / _windows, and the moves of `start` below)
   DevBuf wrap;   // maps in their buffer order on the device: host inputs before they are unwrapped, host outputs once re-wrapped
   te::FootprintState fp;  // the map's own scratch; fp.memo is the resident memo
+  // memo_valid: fp.memo holds every map's bytes, each map's evaluated under the parameters of its key (map_memo)
   bool memo_valid = false;
-  double memo_gap = 0.0, memo_crit = 0.0;
-  int memo_rough = 0;
+  struct MemoKey {
+    double gap, crit;
+    int rough;
+  };
+  std::vector<MemoKey> memo_key;
+  // The per-map parameter table of the last request whose maps have parameters of their own (map_param_table), with what it holds
+  std::vector<te::FpMapParams> par_key;
+  DevBuf par_tab;
   te::MapRequestStats last{};
   bool last_device = false;  // the last request ran in device memory: its counters are on the device (fp.req_counters)
   // Where each map sits: pos[2m], pos[2m + 1] (te_map_positions).  geo's position for every map unless an _at entry put maps
@@ -237,18 +244,56 @@ int map_reset(te_map* m, const te_geometry* g_in, const te_geometry* g, int nmap
   return TE_OK;
 }
 
-// The resident isTraversableForFilters memo for these parameters: kept while the layers and max_gap_width, critical_step_height
-// and verify_roughness (all that checkForStep / checkForSlope / checkForRoughness read) stay the same, cleared otherwise.  One byte
-// per cell of every map.
-int map_memo(te_map* m, const te_footprint_params* p) {
-  const int rough = p->verify_roughness != 0;
-  if (m->memo_valid && m->memo_gap == p->max_gap_width && m->memo_crit == p->critical_step_height && m->memo_rough == rough) return TE_OK;
-  TE_CUDA(m->fp.memo.reserve(batch_cells(m)));
-  TE_CUDA(cudaMemsetAsync(m->fp.memo.p, 0, batch_cells(m), m->ctx->stream));
+// The resident isTraversableForFilters memo for these parameters (p[0] for every map, or with `each` p[k] for map k): a map's bytes
+// are kept while the layers and its max_gap_width, critical_step_height and verify_roughness (all that checkForStep /
+// checkForSlope / checkForRoughness read) stay the same, and cleared otherwise, one memset per run of neighbouring maps to clear.
+// One byte per cell of every map.
+int map_memo(te_map* m, const te_footprint_params* p, bool each) {
+  auto key = [&](int k) {
+    const te_footprint_params& q = p[each ? k : 0];
+    return te_map::MemoKey{q.max_gap_width, q.critical_step_height, q.verify_roughness != 0};
+  };
+  auto same = [](const te_map::MemoKey& a, const te_map::MemoKey& b) { return a.gap == b.gap && a.crit == b.crit && a.rough == b.rough; };
+  const size_t cells = map_cells(m);
+  if (!m->memo_valid) {
+    TE_CUDA(m->fp.memo.reserve(batch_cells(m)));
+    m->memo_key.assign(m->nmaps, key(0));
+  }
+  for (int k = 0; k < m->nmaps;) {
+    if (m->memo_valid && same(m->memo_key[k], key(k))) { ++k; continue; }
+    int e = k;
+    for (; e < m->nmaps && !(m->memo_valid && same(m->memo_key[e], key(e))); ++e) m->memo_key[e] = key(e);
+    TE_CUDA(cudaMemsetAsync((unsigned char*)m->fp.memo.p + k * cells, 0, (e - k) * cells, m->ctx->stream));
+    k = e;
+  }
   m->memo_valid = true;
-  m->memo_gap = p->max_gap_width;
-  m->memo_crit = p->critical_step_height;
-  m->memo_rough = rough;
+  return TE_OK;
+}
+
+// The per-map parameter table of a request whose maps have parameters of their own (params: one per map): *out is its device copy,
+// uploaded only when its bytes change (ordered after the kernels that may still read the old table; a table that grows first
+// waits for them), or null when every map's entry is the same, the request then being one of params[0].  The radius is not in
+// the table: a request takes it per path.
+int map_param_table(te_map* m, const te_footprint_params* params, const te::FpMapParams** out) {
+  std::vector<te::FpMapParams> h(m->nmaps);
+  for (int k = 0; k < m->nmaps; ++k) {
+    const te_footprint_params& q = params[k];
+    h[k] = te::FpMapParams{q.offset, q.traversability_default, q.max_gap_width, q.critical_step_height, q.radius_is_integer_norm,
+                           q.verify_roughness != 0 ? 1 : 0};
+  }
+  *out = nullptr;
+  bool uniform = true;
+  for (int k = 1; k < m->nmaps && uniform; ++k) uniform = std::memcmp(&h[k], &h[0], sizeof(h[0])) == 0;
+  if (uniform) return TE_OK;
+  const size_t bytes = sizeof(te::FpMapParams) * h.size();
+  if (m->par_key.size() != h.size() || std::memcmp(m->par_key.data(), h.data(), bytes) != 0) {
+    if (m->par_tab.p && m->par_tab.cap < bytes) TE_CUDA(cudaStreamSynchronize(m->ctx->stream));
+    TE_CUDA(m->par_tab.reserve(bytes));
+    // pageable source: consumed before cudaMemcpyAsync returns, ordered after the kernels queued before on the stream
+    TE_CUDA(cudaMemcpyAsync(m->par_tab.p, h.data(), bytes, cudaMemcpyHostToDevice, m->ctx->stream));
+    m->par_key = std::move(h);
+  }
+  *out = (const te::FpMapParams*)m->par_tab.p;
   return TE_OK;
 }
 
@@ -402,7 +447,7 @@ int te_map_destroy(te_map* m) {
     Guard g(m->ctx);
     if (g.ok) {
       cudaStreamSynchronize(m->ctx->stream);
-      for (DevBuf* b : {&m->fresh, &m->gather, &m->slots, &m->image, &m->cut, &m->wrap}) b->release();
+      for (DevBuf* b : {&m->fresh, &m->gather, &m->slots, &m->image, &m->cut, &m->wrap, &m->par_tab}) b->release();
       for (DevBuf& b : m->layer) b.release();
       for (DevBuf& b : m->sel) b.release();
       m->tab_all.buf.release();
@@ -1197,6 +1242,45 @@ int te_map_footprint_maps(te_map* m, const te_footprint_params* p, int32_t nsel,
   return map_footprint(m, p, &sel, out, memory);
 }
 
+// te_map_footprint(_maps) with map k's parameters params[k]: the swept maps grouped by bitwise-identical parameters, in order of
+// first appearance, each group swept as a te_map_footprint_maps selection (the sweep's per-radius tables stay kernel parameters).
+// One group is the entry it stands for, output included; several gather the swept caches afterwards with map_out.
+int te_map_footprint_each(te_map* m, const te_footprint_params* params, int32_t nsel, const int32_t* map_index, float* out, int memory) {
+  TE_MAP_ENTER(m);
+  const bool whole = nsel == 0 && !map_index;
+  const MapSel sel{nsel, map_index};
+  if (int rc = whole ? map_ready(m) : map_select(m, false, nullptr, sel)) return rc;
+  if (!params) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
+  if (memory != TE_MEM_HOST && memory != TE_MEM_DEVICE) return fail(TE_ERR_BAD_ARG, "unknown memory mode %d", memory);
+  const int n = whole ? m->nmaps : sel.n;
+  std::vector<std::vector<int32_t>> groups;
+  std::map<std::vector<unsigned char>, size_t> group_of;
+  for (int k = 0; k < n; ++k) {
+    const int32_t mi = whole ? k : map_index[k];
+    const te_footprint_params* p = params + mi;
+    if (int rc = map_footprint_params(m, p)) return rc;
+    if (!(p->radius >= 0.0) || !(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint radius/offset of map %d must be >= 0", mi);
+    // the sweep's own limit, found here so that no group is swept before a later one fails
+    if (!te::footprint_reach_ok(m->geo.resolution, p))
+      return fail(TE_ERR_UNSUPPORTED, "footprint radius + offset of map %d spans more than 120 cells", mi);
+    const unsigned char* b = (const unsigned char*)p;
+    const auto it = group_of.emplace(std::vector<unsigned char>(b, b + sizeof(*p)), groups.size());
+    if (it.second) groups.emplace_back();
+    groups[it.first->second].push_back(mi);
+  }
+  if (groups.size() == 1) return map_footprint(m, params + groups[0][0], whole ? nullptr : &sel, out, memory);
+  for (const std::vector<int32_t>& gi : groups) {
+    const MapSel gs{(int32_t)gi.size(), gi.data()};
+    if (int rc = map_footprint(m, params + gi[0], &gs, nullptr, memory)) return rc;
+  }
+  if (!out) return TE_OK;
+  // the caller's selection back in m->slots (and its host staging in m->sel[0]) for map_out's gather
+  if (!whole)
+    if (int rc = map_stage_selection(m, sel, memory == TE_MEM_HOST ? 1u : 0u)) return rc;
+  const float* const from = lay(m, TE_LAYER_FOOTPRINT);
+  return map_out(m, whole ? nullptr : &sel, 1, &from, !whole, &out, memory);
+}
+
 // The te_map polygon entries: footprint_polygon_common on the map's resident layers with the map's own state.  They neither read
 // nor change the traversability_footprint cache or the memo.
 static int map_footprint_polygon(te_map* m, const te_footprint_params* p, int32_t npts, const double* pts_xy, int nouts,
@@ -1389,18 +1473,27 @@ static long long map_request_checks(const te_geometry* g, bool rslope, int32_t n
   return total;
 }
 
-// te_map_check_footprint_request(_batched) in host memory (path_map null: a single map; else checked by the entry) and
-// te_map_check_footprint_request_device.  Host memory validates the paths, sizes max_checks so that no path is cut and stages
-// the arrays; then both run the same launches, and host memory downloads the outputs.
-static int map_request(te_map* m, const te_footprint_params* p, const int32_t* path_map, int32_t npaths, int32_t nposes,
+// te_map_check_footprint_request(_batched, _each) in host memory (path_map null: a single map; else checked by the entry) and
+// te_map_check_footprint_request_device(_each).  Host memory validates the paths, sizes max_checks so that no path is cut and
+// stages the arrays; then both run the same launches, and host memory downloads the outputs.  each: one parameter set per map
+// (the _each entries, p null); otherwise p for every map.
+static int map_request(te_map* m, const te_footprint_params* p, const te_footprint_params* each, const int32_t* path_map,
+                       int32_t npaths, int32_t nposes,
                        const int32_t* path_begin, const double* poses, const double* radius, int32_t nvertices,
                        const int32_t* footprint_begin, const float* footprint_xyz, int32_t max_footprint_vertices,
                        const uint8_t* conservative, const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area,
                        int32_t max_vertices, int32_t* ucount, double* uxy, long long max_checks, int memory) {
   te_ctx* c = m->ctx;
   const bool host = memory == TE_MEM_HOST;
-  if (int rc = map_footprint_params(m, p)) return rc;
-  if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
+  if (each) {
+    for (int k = 0; k < m->nmaps; ++k) {
+      if (int rc = map_footprint_params(m, each + k)) return rc;
+      if (!(each[k].offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset of map %d must be >= 0", k);
+    }
+  } else {
+    if (int rc = map_footprint_params(m, p)) return rc;
+    if (!(p->offset >= 0.0)) return fail(TE_ERR_BAD_ARG, "footprint offset must be >= 0");
+  }
   if (npaths < 0 || nposes < 0 || nvertices < 0 || !path_begin || !poses || !radius || !footprint_begin ||
       (nvertices > 0 && !footprint_xyz) || !is_safe || !traversability || !area)
     return fail(TE_ERR_BAD_ARG, "null argument or negative count");
@@ -1422,8 +1515,8 @@ static int map_request(te_map* m, const te_footprint_params* p, const int32_t* p
   int mp = conservative && max_footprint_vertices > 0 ? 2 * te::kPolyConsCap : 2 * std::max(max_footprint_vertices, 1);
   bool circles = true;  // device memory cannot tell: the circular kernels run and find none
   if (host) {
-    if (int rc = check_request_host(g, p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
-                                    max_footprint_vertices, conservative, &mp))
+    if (int rc = check_request_host(g, each ? each : p, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin,
+                                    footprint_xyz, max_footprint_vertices, conservative, &mp, each != nullptr, path_map))
       return rc;
     max_checks = map_request_checks(g, m->held & TE_LAYER_ROBOT_SLOPE, npaths, path_begin, poses, footprint_begin, &circles, path_map,
                                     spread ? m->pos.data() : nullptr);
@@ -1431,7 +1524,17 @@ static int map_request(te_map* m, const te_footprint_params* p, const int32_t* p
       return fail(TE_ERR_UNSUPPORTED, "the circular paths need %lld circle checks, more than 2^30", max_checks);
   }
   if (int rc = ensure_geometry(c, g)) return rc;
-  if (int rc = map_memo(m, p)) return rc;
+  if (int rc = map_memo(m, each ? each : p, each != nullptr)) return rc;
+  // maps with parameters of their own: the kernels read each map's from a table (none when they are all one set, p = each[0]);
+  // what does not vary per map comes from each[0], and the roughness layer is read when any map verifies roughness
+  const te::FpMapParams* table = nullptr;
+  te_footprint_params base{};
+  if (each) {
+    if (int rc = map_param_table(m, each, &table)) return rc;
+    base = each[0];
+    for (int k = 0; table && k < m->nmaps; ++k) base.verify_roughness |= each[k].verify_roughness != 0;
+    p = &base;
+  }
   PosTables tab{};
   if (spread)
     if (int rc = map_tables_of(m, MapSel{m->nmaps, nullptr}, &tab)) return rc;
@@ -1445,6 +1548,7 @@ static int map_request(te_map* m, const te_footprint_params* p, const int32_t* p
   r.footprint_begin = footprint_begin; r.footprint_xyz = footprint_xyz; r.nvertices = nvertices;
   r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup; r.max_points = mp;
   r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
+  r.map_params = table;
   Staging st(c, host, g);
   stage_paths(st, r);
   if (st.rc) return st.rc;
@@ -1476,7 +1580,7 @@ int te_map_check_footprint_request(te_map* m, const te_footprint_params* p, int3
   TE_MAP_ENTER(m);
   if (int rc = map_ready(m)) return rc;
   if (int rc = map_single(m, "te_map_check_footprint_request_batched")) return rc;
-  return map_request(m, p, nullptr, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+  return map_request(m, p, nullptr, nullptr, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
                      max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy, 0,
                      TE_MEM_HOST);
 }
@@ -1491,7 +1595,7 @@ int te_map_check_footprint_request_batched(te_map* m, const te_footprint_params*
   if (int rc = map_ready(m)) return rc;
   if (!path_map) return fail(TE_ERR_BAD_ARG, "path_map is null");
   if (int rc = check_map_indices(m, path_map, std::max(npaths, 0), "path_map")) return rc;
-  return map_request(m, p, path_map, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+  return map_request(m, p, nullptr, path_map, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
                      max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy, 0,
                      TE_MEM_HOST);
 }
@@ -1505,9 +1609,40 @@ int te_map_check_footprint_request_device(te_map* m, const te_footprint_params* 
   TE_MAP_ENTER(m);
   if (int rc = map_ready(m)) return rc;
   if (!path_map && m->nmaps > 1) return fail(TE_ERR_BAD_ARG, "path_map is null on a te_map of %d maps", m->nmaps);
-  return map_request(m, p, path_map, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
+  return map_request(m, p, nullptr, path_map, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin, footprint_xyz,
                      max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount, uxy,
                      (long long)max_checks, TE_MEM_DEVICE);
+}
+
+int te_map_check_footprint_request_each(te_map* m, const te_footprint_params* params, const int32_t* path_map, int32_t npaths,
+                                        int32_t nposes, const int32_t* path_begin, const double* poses, const double* radius,
+                                        int32_t nvertices, const int32_t* footprint_begin, const float* footprint_xyz,
+                                        int32_t max_footprint_vertices, const uint8_t* conservative, const uint8_t* cup,
+                                        uint8_t* is_safe, double* traversability, double* area, int32_t max_vertices, int32_t* ucount,
+                                        double* uxy) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (!params) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
+  if (!path_map) return fail(TE_ERR_BAD_ARG, "path_map is null");
+  if (int rc = check_map_indices(m, path_map, std::max(npaths, 0), "path_map")) return rc;
+  return map_request(m, nullptr, params, path_map, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin,
+                     footprint_xyz, max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount,
+                     uxy, 0, TE_MEM_HOST);
+}
+
+int te_map_check_footprint_request_device_each(te_map* m, const te_footprint_params* params, const int32_t* path_map,
+                                               int32_t npaths, int32_t nposes, const int32_t* path_begin, const double* poses,
+                                               const double* radius, int32_t nvertices, const int32_t* footprint_begin,
+                                               const float* footprint_xyz, int32_t max_footprint_vertices, const uint8_t* conservative,
+                                               const uint8_t* cup, uint8_t* is_safe, double* traversability, double* area,
+                                               int32_t max_vertices, int32_t* ucount, double* uxy, int64_t max_checks) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (!params) return fail(TE_ERR_BAD_ARG, "footprint parameters are null");
+  if (!path_map && m->nmaps > 1) return fail(TE_ERR_BAD_ARG, "path_map is null on a te_map of %d maps", m->nmaps);
+  return map_request(m, nullptr, params, path_map, npaths, nposes, path_begin, poses, radius, nvertices, footprint_begin,
+                     footprint_xyz, max_footprint_vertices, conservative, cup, is_safe, traversability, area, max_vertices, ucount,
+                     uxy, (long long)max_checks, TE_MEM_DEVICE);
 }
 
 int te_map_get_footprint(te_map* m, float* dst, int memory) {
@@ -1518,6 +1653,19 @@ int te_map_get_footprint(te_map* m, float* dst, int memory) {
     return fail(TE_ERR_UNSUPPORTED, "the map's layers came with a circular-buffer start index: read its cache into host memory");
   const float* const from = lay(m, TE_LAYER_FOOTPRINT);
   return map_out(m, nullptr, 1, &from, false, &dst, memory);
+}
+
+int te_map_get_memo(te_map* m, uint8_t* dst) {
+  TE_MAP_ENTER(m);
+  if (int rc = map_ready(m)) return rc;
+  if (!dst) return fail(TE_ERR_BAD_ARG, "output is null");
+  if (!m->memo_valid) {  // no request since the layers came: nothing evaluated
+    std::memset(dst, 0, batch_cells(m));
+    return TE_OK;
+  }
+  TE_CUDA(cudaMemcpyAsync(dst, m->fp.memo.p, batch_cells(m), cudaMemcpyDeviceToHost, c->stream));
+  TE_CUDA(cudaStreamSynchronize(c->stream));
+  return TE_OK;
 }
 
 int te_map_clear_footprint(te_map* m) {

@@ -34,8 +34,9 @@ struct MapRecord {
 };
 
 // Key k of the request, by the whole warp w of a block of four: its record (k_map_eval_circles_dev).
-// AT: the maps sit at their own positions (FpArgs::pos), and the walk takes the key's map's tables and position.
-template <bool AT>
+// AT: the maps sit at their own positions (FpArgs::pos), and the walk takes the key's map's tables and position.  Maps with
+// parameters of their own (FpArgs::mp): the walk takes the key's map's.
+template <bool AT, bool EACH>
 __device__ __forceinline__ void map_eval_circle_d(const FpArgs& A0, const Layers& L, const PathArgs& P, const MapKey* __restrict__ keys,
                                                   int k, const float* __restrict__ cache, MapRecord* __restrict__ recs) {
   __shared__ Layers s_L[4];
@@ -43,8 +44,8 @@ __device__ __forceinline__ void map_eval_circle_d(const FpArgs& A0, const Layers
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const MapKey K = keys[k];
   FpArgs Am;
-  if constexpr (AT) Am = map_args_d(A0, K.map);
-  const FpArgs& A = AT ? Am : A0;
+  if constexpr (AT || EACH) Am = map_view_d<AT, EACH>(A0, K.map);
+  const FpArgs& A = AT || EACH ? Am : A0;
   MapRecord& R = recs[k];
   // The key's map: its layers, memo and cache start mo cells in.  The walk takes the shifted layer and path arguments from a
   // per-warp copy in shared memory (by reference, as it takes the kernel's own), so no register holds them across the call.
@@ -60,7 +61,7 @@ __device__ __forceinline__ void map_eval_circle_d(const FpArgs& A0, const Layers
     s_P[w].memo += mo;
   }
   __syncwarp();
-  const double rmax = K.rmin + P.offset;
+  const double rmax = K.rmin + map_walk_offset_d<EACH>(A0, P.offset, K.map);
   const int nr = (int)ceil(rmax / A.res);
   const FreshCircle f = fresh_circle_d(A, s_L[w], s_P[w], K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, nr, K.cup != 0);
   if (lane == 0) { R.t = f.t; R.cache = f.cache; R.state = f.ok ? 0 : 1; }
@@ -68,13 +69,13 @@ __device__ __forceinline__ void map_eval_circle_d(const FpArgs& A0, const Layers
 
 // The key count is on the device (*nkeys), so the warps stride over the keys.  The polygons of the failed paths come after the
 // replay (k_req_polygons).
-template <bool AT>
+template <bool AT, bool EACH>
 __global__ void __launch_bounds__(128, 4) k_map_eval_circles_dev(FpArgs A, Layers L, PathArgs P, const MapKey* __restrict__ keys,
                                                               const unsigned long long* __restrict__ nkeys, const float* __restrict__ cache,
                                                               MapRecord* __restrict__ recs) {
   const long long n = (long long)*nkeys;
   for (long long k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; k < n; k += (gridDim.x * blockDim.x) >> 5)  // whole warps
-    map_eval_circle_d<AT>(A, L, P, keys, (int)k, cache, recs);
+    map_eval_circle_d<AT, EACH>(A, L, P, keys, (int)k, cache, recs);
 }
 
 // traversabilityFootprint(radius, offset) on a cache: a cached cell takes the memoised branch and keeps its value, every other cell
@@ -168,7 +169,7 @@ struct DevReq {
   const int* path_map;          // nullptr: one map
   const unsigned char* cup;
   const float* rslope;          // robot_slope of map 0, nullptr: no checkInclination
-  double offset;
+  double offset;                // the call's; FpArgs::mp: each map's own
   unsigned char* is_safe;
   double* trav_out;
   double* area_out;
@@ -217,8 +218,10 @@ __global__ void __launch_bounds__(128) k_req_paths(FpArgs A, DevReq D) {
   if (!req_circular_d(D, q)) { D.status[q] = 0; return; }
   const int b = D.path_begin[q], n = D.path_begin[q + 1] - b;
   const double rmin = D.radius[q];
-  bool ok = rmin >= 0.0 && ceil((rmin + D.offset) / A.res) <= (double)kPathMaxRings && b >= 0 && n >= 0 && b <= D.nposes - n;
-  if (ok && D.path_map) ok = D.path_map[q] >= 0 && D.path_map[q] < D.nmaps;
+  const int m = D.path_map ? D.path_map[q] : 0;
+  bool ok = m >= 0 && m < D.nmaps;
+  const double offset = ok && A.mp ? A.mp[m].offset : D.offset;  // the map's own with FpArgs::mp
+  ok = ok && rmin >= 0.0 && ceil((rmin + offset) / A.res) <= (double)kPathMaxRings && b >= 0 && n >= 0 && b <= D.nposes - n;
   for (int k = 0; k < n && ok; ++k)
     ok = (D.nonfinite_ok || (isfinite(D.poses[7 * (size_t)(b + k)]) && isfinite(D.poses[7 * (size_t)(b + k) + 1]))) &&
          req_path_of_d(D, b + k) == q;
@@ -408,6 +411,7 @@ __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* c
   int e0 = D.lofs[lo];
   const int e1 = D.lofs[hi];
   float* const mc = cache + m * D.map_cells;
+  const double tdefault = A.mp ? A.mp[m].tdefault : A.tdefault;  // the map's own with FpArgs::mp
   // lane 0: the path being folded
   int cur = -1, dead = -1, nLine = 0;
   bool ok = false;
@@ -449,7 +453,7 @@ __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* c
         t = (double)v; lok = v != 0.0f; fk = 1;
       }
     } else if (have && (E.flags & kEntOutside)) {         // :662-667
-      t = A.tdefault; lok = A.tdefault != 0.0; fk = 1;
+      t = tdefault; lok = tdefault != 0.0; fk = 1;
     } else if (have) {                                    // a gate
       lok = false;
     }
@@ -521,7 +525,7 @@ __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* c
 
 // 6. Polygons: one warp per path; a path the replay did not leave a failing circle to publish exits at once.  The pair
 // k_check_paths_fresh_poly calls: fromCircle, or spiral_blockers_d on the failing key and write_cells_polygon_d with its freps.
-template <bool AT>
+template <bool AT, bool EACH>
 __global__ void __launch_bounds__(128, 4) k_req_polygons(FpArgs A0, Layers L, PathArgs P, DevReq D, CircleTable C) {
   __shared__ int s_min[4][kFreshTableRows + 1], s_max[4][kFreshTableRows + 1];
   __shared__ int2 s_stack[4][2 * kFreshTableRows + 4];
@@ -531,7 +535,7 @@ __global__ void __launch_bounds__(128, 4) k_req_polygons(FpArgs A0, Layers L, Pa
   if (q >= D.npaths || D.status[q] != 1) return;  // whole warp
   const ReqFail F = D.fails[q];
   if (F.fkind == 0) return;
-  const double rmax = D.radius[q] + D.offset;
+  const double rmax = D.radius[q] + map_walk_offset_d<EACH>(A0, D.offset, D.path_map ? D.path_map[q] : 0);
   const UntravScratch S{s_min[w], s_max[w], s_stack[w], s_first[w]};
   if (F.fkind == 1) {
     const int n = D.path_begin[q + 1] - D.path_begin[q];
@@ -539,9 +543,9 @@ __global__ void __launch_bounds__(128, 4) k_req_polygons(FpArgs A0, Layers L, Pa
     return;
   }
   const MapKey K = D.keys[F.key];
-  FpArgs Am;  // AT: the key's map's tables and position
-  if constexpr (AT) Am = map_args_d(A0, K.map);
-  const FpArgs& A = AT ? Am : A0;
+  FpArgs Am;  // the key's map's tables and position (AT) and parameters (EACH)
+  if constexpr (AT || EACH) Am = map_view_d<AT, EACH>(A0, K.map);
+  const FpArgs& A = AT || EACH ? Am : A0;
   const long long mo = (long long)K.map * D.map_cells;
   L = shift_layers_d(L, mo);
   P.memo += mo;
@@ -608,13 +612,15 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
     st.why = "clearing the device request workspace failed";
     return TE_ERR_CUDA;
   }
-  const FpArgs a = filter_args(v, g, p, r.rough);
+  FpArgs a = filter_args(v, g, p, r.rough);
+  a.mp = r.map_params;
   const Layers L{r.trav, r.slope, r.step, r.elev, r.rough};
   const PathArgs P = path_args(st, p, r.robot_slope);
   auto blocks = [](long long n, int per) { return (unsigned)std::max((n + per - 1) / per, 1LL); };
   size_t b1 = cub_bytes, b2 = cub_bytes, b3 = cub_bytes;
   k_req_paths<<<blocks(npaths, 128), 128, 0, s>>>(a, D);
   const bool at = a.pos != nullptr;  // maps at their own positions: the instantiations that read each map's tables
+  const bool each = a.mp != nullptr;  // maps with parameters of their own: the instantiations that read each map's
   if (at) k_req_count<true><<<blocks(nposes + 1, 128), 128, 0, s>>>(a, D);
   else k_req_count<false><<<blocks(nposes + 1, 128), 128, 0, s>>>(a, D);
   cudaError_t e = cub::DeviceScan::ExclusiveSum(tmp, b1, (const long long*)D.cnt, D.gofs, (int)np1, s);
@@ -628,13 +634,15 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
   else k_req_list<false><<<blocks(nposes, 128), 128, 0, s>>>(a, D);
   k_req_dedup<<<(unsigned)std::min<long long>(blocks((long long)nc, 256), 8LL * sms), 256, 0, s>>>(D);
   const unsigned ge = (unsigned)std::min<long long>(blocks((long long)nc, 4), 16LL * sms);
-  if (at) k_map_eval_circles_dev<true><<<ge, 128, 0, s>>>(a, L, P, D.keys, D.counters + 1, cache, D.recs);
-  else k_map_eval_circles_dev<false><<<ge, 128, 0, s>>>(a, L, P, D.keys, D.counters + 1, cache, D.recs);
+  const auto eval = at ? (each ? k_map_eval_circles_dev<true, true> : k_map_eval_circles_dev<true, false>)
+                       : (each ? k_map_eval_circles_dev<false, true> : k_map_eval_circles_dev<false, false>);
+  eval<<<ge, 128, 0, s>>>(a, L, P, D.keys, D.counters + 1, cache, D.recs);
   k_req_replay<<<blocks(nmaps, 4), 128, 0, s>>>(a, D, cache);
   *launches = 12;  // nine kernels and three CUB calls, each counted as one launch (a CUB call runs two or more kernels)
   if (r.ucount) {
-    if (at) k_req_polygons<true><<<blocks(npaths, 4), 128, 0, s>>>(a, L, P, D, circle_table());
-    else k_req_polygons<false><<<blocks(npaths, 4), 128, 0, s>>>(a, L, P, D, circle_table());
+    const auto polys = at ? (each ? k_req_polygons<true, true> : k_req_polygons<true, false>)
+                          : (each ? k_req_polygons<false, true> : k_req_polygons<false, false>);
+    polys<<<blocks(npaths, 4), 128, 0, s>>>(a, L, P, D, circle_table());
     ++*launches;
   }
   if (e != cudaSuccess) { st.why = std::string("scan / sort failed: ") + cudaGetErrorString(e); return TE_ERR_CUDA; }

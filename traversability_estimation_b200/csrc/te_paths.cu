@@ -332,8 +332,9 @@ __host__ __device__ inline size_t poly_warp_smem(int mcap, bool poly) {
 // sB (mcap points: a conservative path's earlier polygon2, then the sorted hull input).  POLY: with compute_untraversable_polygon
 // set for the item's path, the walk goes on past blocked cells and collects them (:602-608, :634-638).  With per-path footprints
 // (R.fp_begin) each polygonal path uses its own, and the poses of circular paths are no items.  AT: the maps sit at their own
-// positions (FpArgs::pos), and the item takes its path's map's tables and position.
-template <bool POLY, bool AT>
+// positions (FpArgs::pos), and the item takes its path's map's tables and position.  Maps with parameters of their own
+// (FpArgs::mp): the item takes its path's map's.
+template <bool POLY, bool AT, bool EACH>
 __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L, const PolyPathArgs& P, const PolyUntravArgs& U,
                                                      const RequestArgs& R) {
   extern __shared__ double2 sPoly[];
@@ -366,8 +367,8 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L,
   }
   L = shift_layers_d(L, mo);  // path q's map
   FpArgs Am;
-  if constexpr (AT) Am = map_args_d(A0, R.path_map ? R.path_map[q] : 0);
-  const FpArgs& A = AT ? Am : A0;
+  if constexpr (AT || EACH) Am = map_view_d<AT, EACH>(A0, R.path_map ? R.path_map[q] : 0);
+  const FpArgs& A = AT || EACH ? Am : A0;
   const float* const rslope = P.rslope ? P.rslope + mo : nullptr;
   unsigned char* const memo = P.memo + mo;
   it.q = q;
@@ -531,14 +532,14 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L,
   }
 }
 
-template <bool AT>
+template <bool AT, bool EACH>
 __global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L, PolyPathArgs P, RequestArgs R) {
-  check_polygon_item_d<false, AT>(A, L, P, PolyUntravArgs{}, R);
+  check_polygon_item_d<false, AT, EACH>(A, L, P, PolyUntravArgs{}, R);
 }
 
-template <bool AT>
+template <bool AT, bool EACH>
 __global__ void __launch_bounds__(128) k_check_polygon_items_poly(FpArgs A, Layers L, PolyPathArgs P, PolyUntravArgs U, RequestArgs R) {
-  check_polygon_item_d<true, AT>(A, L, P, U, R);
+  check_polygon_item_d<true, AT, EACH>(A, L, P, U, R);
 }
 
 // One thread per path: the area-weighted combination of the segment results in path order (:522-579).  An unsafe path reports 0;
@@ -733,7 +734,8 @@ int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry*
     if (int rc = ensure_ring_table(st, s)) return rc;
   if (clear_memo)  // one memo for both kinds of path: it depends on the layers only
     if (int rc = reset_filter_memo(st, v, r.nmaps, s)) return rc;
-  const FpArgs a = filter_args(v, g, p, r.rough);
+  FpArgs a = filter_args(v, g, p, r.rough);
+  a.mp = r.map_params;  // a te_map batch whose maps have parameters of their own: read by the polygonal items only
   const Layers L{r.trav, r.slope, r.step, r.elev, r.rough};
   const RequestArgs R{r.footprint_begin, r.footprint_xyz, r.nvertices, r.max_footprint_vertices, r.nposes, r.area_out,
                       r.path_map, r.nmaps, (long long)v.rows * v.cols_total};
@@ -760,19 +762,24 @@ int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry*
   for (int k = 0; r.footprint && k < r.nfp; ++k) {
     P.fx[k] = r.footprint[3 * k]; P.fy[k] = r.footprint[3 * k + 1]; P.fz[k] = r.footprint[3 * k + 2];
   }
-  // maps at their own positions (a te_map): the instantiations that read each path's map's tables
-  const bool at = a.pos != nullptr;
+  // maps at their own positions (a te_map): the instantiations that read each path's map's tables; maps with parameters of their
+  // own: those that read each path's map's
+  const bool at = a.pos != nullptr, each = a.mp != nullptr;
   if (!r.ucount)
-    return launch_polygon_kernels(st, at ? k_check_polygon_items<true> : k_check_polygon_items<false>, k_check_polygon_combine,
-                                  "k_check_polygon_items", false, a, L, P, s, launches, R);
+    return launch_polygon_kernels(st,
+                                  at ? (each ? k_check_polygon_items<true, true> : k_check_polygon_items<true, false>)
+                                     : (each ? k_check_polygon_items<false, true> : k_check_polygon_items<false, false>),
+                                  k_check_polygon_combine, "k_check_polygon_items", false, a, L, P, s, launches, R);
   const size_t cbytes = (sizeof(int) * nitems + 15) / 16 * 16;
   if (st.upoly.reserve(cbytes + sizeof(double2) * nitems * (size_t)std::max(r.max_vertices, 1)) != cudaSuccess) {
     st.why = "allocating the untraversable polygons failed";
     return TE_ERR_CUDA;
   }
   const PolyUntravArgs U{r.cup, (int*)st.upoly.p, (double*)((char*)st.upoly.p + cbytes), UntravOut{r.max_vertices, r.ucount, r.uxy}};
-  return launch_polygon_kernels(st, at ? k_check_polygon_items_poly<true> : k_check_polygon_items_poly<false>, k_check_polygon_combine_poly,
-                                "k_check_polygon_items_poly", true, a, L, P, s, launches, U, R);
+  return launch_polygon_kernels(st,
+                                at ? (each ? k_check_polygon_items_poly<true, true> : k_check_polygon_items_poly<true, false>)
+                                   : (each ? k_check_polygon_items_poly<false, true> : k_check_polygon_items_poly<false, false>),
+                                k_check_polygon_combine_poly, "k_check_polygon_items_poly", true, a, L, P, s, launches, U, R);
 }
 
 }  // namespace te
