@@ -2,6 +2,7 @@
 import numpy as np
 import pytest
 
+import literal_cases
 import synth
 from helpers import assert_parity, compare_layer
 
@@ -157,9 +158,11 @@ def test_streaming_slope_filter_is_bit_identical_to_the_literal_expression(te, c
         ctx.slope(g, crit, d_in, d_out, te.MEM_DEVICE)
         ctx.synchronize()
         got = d_out.cpu()
-        same = (got.view(torch.int32) == ref.view(torch.int32)) | (torch.isnan(got) & torch.isnan(ref))
-        # torch's acos on the CPU and CUDA's libdevice acos may differ in the last bit of the double: allow a handful of cells
-        assert int((~same).sum()) <= 4, (crit, int((~same).sum()), got[~same][:5], ref[~same][:5])
+        # torch's acos on the CPU and CUDA's libdevice acos may differ in the last bits of the double: a cell may differ only
+        # where the exact acos lies within their error of a decision of the expression
+        ok, no = literal_cases.slope_mismatches(nz.numpy(), crit, got.numpy(), ref.numpy())
+        assert not no, (crit, len(no), got[no[:5]], ref[no[:5]])
+        print(f"crit {crit}: {len(ok)} cells explained by acos")
 
 
 @pytest.mark.parametrize("rows,cols,sr,sc", [(192, 160, 37, 101), (128, 96, 0, 5), (128, 96, 127, 0), (2048, 2048, 1000, 77)])
