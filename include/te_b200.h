@@ -883,6 +883,8 @@ int te_map_get_footprint(te_map* map, float* traversability_footprint, int memor
  * default order, whatever its start index): 0 not evaluated since the memo was last cleared for that map, 1 passes, 2 blocked.
  * Host memory, returns synchronised.  No reference counterpart: it lets a caller see which maps' memo a call kept. */
 int te_map_get_memo(te_map* map, uint8_t* memo);
+/* resetTraversabilityFootprintLayers (:195-200): every map's cache empty, slope_footprint and step_footprint NaN (see te_layer);
+ * roughness_footprint and the memo stay. */
 int te_map_clear_footprint(te_map* map);
 
 /* Counters of the last te_map_check_footprint_request(_batched): out[0] isTraversable calls its circular paths could make, out[1]
@@ -920,7 +922,37 @@ typedef enum te_layer {
   TE_LAYER_UNCERTAINTY_RANGE = 1 << 15,
   /* The traversability_footprint service's layers (TraversabilityMap.cpp:239-305): te_map_footprint_polygon_keep gives them. */
   TE_LAYER_TRAVERSABILITY_X = 1 << 16,
-  TE_LAYER_TRAVERSABILITY_ROT = 1 << 17
+  TE_LAYER_TRAVERSABILITY_ROT = 1 << 17,
+  /* 1 << 18 .. 1 << 20 are unassigned.  The layers isTraversableForFilters memoises its checks in (checkForSlope :867-893,
+   * checkForStep :794-865, checkForRoughness :895-921): computeTraversability adds them all NaN (:225-228), and a check writes
+   * 0.0 or 1.0 at a cell it visits whose own input layer (traversability_slope, _step, _roughness) is exactly 0.  The step check
+   * runs only after the slope check passed, the roughness check only after both and with verify_roughness.  A te_map holds, per
+   * map, what a reference node with that map's footprint parameters (its memo key, te_map_get_memo) holds after the same calls:
+   *   - te_map_chain*, te_map_set_layers*, te_map_chain_image*, te_map_chain_submap / _windows and the _maps updates reset the
+   *     selected maps' layers to NaN, as they empty the cache;
+   *   - a request (te_map_check_footprint_request, _batched, _each, _device, _device_each) records every cell at which the
+   *     service loop calls isTraversableForFilters, in order: a circle's walk only where the centre's traversability_footprint is
+   *     not valid when the loop reaches it (:673), its spiral up to and including the first blocked cell (with
+   *     compute_untraversable_polygon on to where the loop ends, :687-729); a polygonal item the path loop reaches, its
+   *     PolygonIterator cells up to the first blocked one, or every one with compute_untraversable_polygon (:600-611).  Cells the
+   *     request's kernels evaluate but the loop never reaches stay NaN;
+   *   - te_map_footprint, _maps and _each (traversabilityFootprint(radius, offset), :307-318) record the spiral prefix of every
+   *     centre whose cache cell is empty; on an empty cache that is every cell, with the values te_footprint2 returns in
+   *     slope_fp / step_fp / rough_fp;
+   *   - a change of a map's memo key (max_gap_width, critical_step_height, verify_roughness) by a request or a sweep resets that
+   *     map's layers to NaN first;
+   *   - te_map_clear_footprint (resetTraversabilityFootprintLayers, :195-200) resets slope_footprint and step_footprint and keeps
+   *     roughness_footprint.
+   * DIFFERENCE: the polygon sweeps (te_map_footprint_polygon, _yaws, _yaws_reduce, _keep) record nothing; the reference's
+   * traversabilityFootprint(yaw) writes these layers at the cells its polygons visit (:601).
+   * Served wherever TE_LAYER_FOOTPRINT is (te_map_get_layers, te_map_get_submaps(_batched), te_map_at_poses,
+   * te_map_get_occupancy, te_map_get_point_cloud fields), NaN as the quiet NaN 0x7fc00000 of the reference's layers.  Every
+   * te_map serves roughness_footprint (NaN where nothing wrote it); the reference's map has that layer only when
+   * verify_roughness_footprint is set. */
+  TE_LAYER_SLOPE_FOOTPRINT = 1 << 21,
+  TE_LAYER_STEP_FOOTPRINT = 1 << 22,
+  TE_LAYER_ROUGHNESS_FOOTPRINT = 1 << 23,
+  TE_LAYER_FOOTPRINT_MEMO = 0xe00000  /* the three bits above */
 } te_layer;
 
 /* mapOut = mapIn for the layers the chain does not make: the carried layers of `layer_mask` (TE_LAYER_CARRIED bits) and
@@ -1152,10 +1184,9 @@ int te_map_get_occupancy(te_map* map, int32_t nsel, const int32_t* map_index_or_
  *     index came in g included: each map is read in its own buffer order and at its own position.
  *   - fields: a HOST array of nfields (1..32) entries in the published map's layer order.  Each is one te_layer bit that
  *     te_map_get_layers accepts (the carried layers, robot_slope, TE_LAYER_FOOTPRINT (the cache, NaN where empty),
- *     traversability_x / _rot, TE_LAYER_UNCERTAINTY_RANGE with te_map_get_layers' NaN-payload rule), at most once, or 0: a field
- *     holding NaN 0x7fc00000 at every point.  0 stands for step_footprint, slope_footprint and roughness_footprint as
- *     computeTraversability publishes them (TraversabilityMap.cpp:225-228: all NaN); that is exact only for a map published by
- *     computeTraversability, not after a footprint service call has filled the reference's lazily evaluated layers (:301, :316).
+ *     traversability_x / _rot, TE_LAYER_UNCERTAINTY_RANGE with te_map_get_layers' NaN-payload rule, TE_LAYER_SLOPE_FOOTPRINT /
+ *     _STEP_FOOTPRINT / _ROUGHNESS_FOOTPRINT as the te_map recorded them), at most once, or 0: a field holding NaN 0x7fc00000 at
+ *     every point, as the reference publishes a layer nothing wrote (computeTraversability's add(), TraversabilityMap.cpp:225-228).
  *   - point_layer: one te_layer bit the map holds.  It decides which cells are points; it need not be in `fields`, and then the
  *     records have no x, y, z, as in the reference.
  *   - basic_mask: the map's basic layers as te_layer bits (0: none, as in the reference's bags).

@@ -30,15 +30,19 @@ UNCERTAINTY_RANGE = "uncertainty_range"
 POLYGON_LAYERS = ("traversability_x", "traversability_rot")
 LAYER_BITS = {**{n: k for k, n in enumerate(LAYERS)}, **{n: 8 + k for k, n in enumerate(CARRIED_LAYERS)}, UNCERTAINTY_RANGE: 15,
               **{n: 16 + k for k, n in enumerate(POLYGON_LAYERS)}}
+# The layers isTraversableForFilters memoises its checks in, recorded by a te_map's requests and sweeps, bits 21 .. 23 (18 .. 20
+# are unassigned).  Every method that takes layer names takes these too.
+FOOTPRINT_MEMO_BITS = {"slope_footprint": 21, "step_footprint": 22, "roughness_footprint": 23}
+_ALL_BITS = {**LAYER_BITS, **FOOTPRINT_MEMO_BITS}
 
 
 def layer_mask(names) -> int:
     """The te_layer mask of layer names (any order; each once)."""
     names = list(names)
-    unknown = [n for n in names if n not in LAYER_BITS]
+    unknown = [n for n in names if n not in _ALL_BITS]
     if unknown or len(set(names)) != len(names):
-        raise ValueError(f"layer names {names}: each once, from {tuple(LAYER_BITS)}")
-    return sum(1 << LAYER_BITS[n] for n in names)
+        raise ValueError(f"layer names {names}: each once, from {tuple(_ALL_BITS)}")
+    return sum(1 << _ALL_BITS[n] for n in names)
 
 
 _layer_mask_of = layer_mask  # for methods whose argument is named layer_mask
@@ -46,7 +50,7 @@ _layer_mask_of = layer_mask  # for methods whose argument is named layer_mask
 
 def layer_order(mask) -> list:
     """The layer names of a te_layer mask in bit order, the order of every output that holds several."""
-    return [n for n, b in sorted(LAYER_BITS.items(), key=lambda x: x[1]) if (mask >> b) & 1]
+    return [n for n, b in sorted(_ALL_BITS.items(), key=lambda x: x[1]) if (mask >> b) & 1]
 
 
 class SubmapInfo(C.Structure):
@@ -1441,7 +1445,8 @@ class Map:
         """te_map_get_point_cloud (GridMapRosConverter::toPointCloud): the clouds of the maps (maps None: every map; otherwise the
         maps `maps` in that order) with one float32 field per name of `fields` (message order), the point layer's entry replaced by
         x, y, z.  A name of `nan_layers` is a field holding NaN 0x7fc00000 (the published map's step_footprint / slope_footprint
-        after computeTraversability); every other name is a LAYER_BITS entry.  basic: the map's basic layers.  Returns (layout,
+        after computeTraversability); every other name is a LAYER_BITS or FOOTPRINT_MEMO_BITS entry (slope_footprint,
+        step_footprint and roughness_footprint as the te_map recorded them).  basic: the map's basic layers.  Returns (layout,
         point_step, clouds), layout the (name, offset) pairs of point_cloud_fields.  Host memory: clouds is a list of one numpy
         structured array per map (point_cloud_dtype), in the reference's point order; capacity None sizes the call first, otherwise
         a cloud over `capacity` points raises.  Device memory: `out` a uint8 device tensor (capacity None: all of it) and `offsets`
@@ -1451,17 +1456,17 @@ class Map:
             raise ValueError(f"fields {fields}: each name once")
         bits = []
         for f in fields:
-            if f not in nan_layers and f not in LAYER_BITS:
-                raise ValueError(f"field {f!r}: neither a layer ({tuple(LAYER_BITS)}) nor one of nan_layers")
-            bits.append(0 if f in nan_layers else 1 << LAYER_BITS[f])
-        if point_layer not in LAYER_BITS:
-            raise ValueError(f"point_layer {point_layer!r}: not a layer of {tuple(LAYER_BITS)}")
+            if f not in nan_layers and f not in _ALL_BITS:
+                raise ValueError(f"field {f!r}: neither a layer ({tuple(_ALL_BITS)}) nor one of nan_layers")
+            bits.append(0 if f in nan_layers else 1 << _ALL_BITS[f])
+        if point_layer not in _ALL_BITS:
+            raise ValueError(f"point_layer {point_layer!r}: not a layer of {tuple(_ALL_BITS)}")
         fa = np.ascontiguousarray(bits, dtype=np.uint32)
         layout, step = point_cloud_fields(fields, point_layer)
         idx = None if maps is None else self._map_index(maps)
         n = self._n if idx is None else len(idx)
         fn = self._L.te_map_get_point_cloud
-        args = (self._h, 0 if idx is None else len(idx), _addr(idx), len(fa), _addr(fa), 1 << LAYER_BITS[point_layer],
+        args = (self._h, 0 if idx is None else len(idx), _addr(idx), len(fa), _addr(fa), 1 << _ALL_BITS[point_layer],
                 layer_mask(basic) if len(basic) else 0)
         if memory != MEM_HOST:
             cap = out.numel() // step if capacity is None else int(capacity)

@@ -28,9 +28,12 @@ namespace {
 // value is exactly 0 (TraversabilityMap.cpp:869, :796, :897) — so k_pred_classify settles those with two or three coalesced
 // loads and collects the others on a work list, which k_pred_heavy walks with one thread per listed cell (the window count,
 // the submap / gap walk): the heavy threads are no longer scattered one or two per warp over the whole map.
-__global__ void __launch_bounds__(256) k_pred_classify(FpArgs A, Layers L, unsigned char* __restrict__ blocked, float* slope_fp,
-                                                       float* step_fp, float* rough_fp, unsigned* __restrict__ list,
-                                                       unsigned* __restrict__ count) {
+// CODES (a te_map sweep, SweepRecord): each cell's recorded-layer code (te_fp_device.cuh) also goes to codes[c], 0 for a cell no
+// check runs on.
+template <bool CODES>
+__device__ __forceinline__ void pred_classify_d(const FpArgs& A, const Layers& L, unsigned char* __restrict__ blocked, float* slope_fp,
+                                                float* step_fp, float* rough_fp, unsigned* __restrict__ list, unsigned* __restrict__ count,
+                                                unsigned char* __restrict__ codes) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int lb = blockIdx.y;
   const bool in = i < A.rows;
@@ -41,6 +44,7 @@ __global__ void __launch_bounds__(256) k_pred_classify(FpArgs A, Layers L, unsig
     heavy = __ldg(L.slope + c) == 0.0f || __ldg(L.step + c) == 0.0f || (A.verify_rough && __ldg(L.rough + c) == 0.0f);
     if (!heavy) {
       blocked[c] = 0;
+      if constexpr (CODES) codes[c] = 0;
       const int oj = lb + A.in_col0 - A.out_col0;
       if (oj >= 0 && oj < A.out_ncols) {
         const size_t oc = ((unsigned)blockIdx.z * A.out_ncols + oj) * (unsigned)A.rows + i;
@@ -60,10 +64,23 @@ __global__ void __launch_bounds__(256) k_pred_classify(FpArgs A, Layers L, unsig
   }
 }
 
+__global__ void __launch_bounds__(256) k_pred_classify(FpArgs A, Layers L, unsigned char* __restrict__ blocked, float* slope_fp,
+                                                       float* step_fp, float* rough_fp, unsigned* __restrict__ list,
+                                                       unsigned* __restrict__ count) {
+  pred_classify_d<false>(A, L, blocked, slope_fp, step_fp, rough_fp, list, count, nullptr);
+}
+
+__global__ void __launch_bounds__(256) k_pred_classify_codes(FpArgs A, Layers L, unsigned char* __restrict__ blocked, float* slope_fp,
+                                                             float* step_fp, float* rough_fp, unsigned* __restrict__ list,
+                                                             unsigned* __restrict__ count, unsigned char* __restrict__ codes) {
+  pred_classify_d<true>(A, L, blocked, slope_fp, step_fp, rough_fp, list, count, codes);
+}
+
 // AT: the maps sit at their own positions (FpArgs::pos); the shared-position instantiation reads A as it always did.
-template <bool AT>
-__global__ void __launch_bounds__(128) k_pred_heavy(FpArgs A, Layers L, unsigned char* __restrict__ blocked, float* slope_fp, float* step_fp,
-                                                    float* rough_fp, const unsigned* __restrict__ list, const unsigned* __restrict__ count) {
+template <bool AT, bool CODES>
+__device__ __forceinline__ void pred_heavy_d(const FpArgs& A, const Layers& L, unsigned char* __restrict__ blocked, float* slope_fp,
+                                             float* step_fp, float* rough_fp, const unsigned* __restrict__ list,
+                                             const unsigned* __restrict__ count, unsigned char* __restrict__ codes) {
   const unsigned n = *count;
   for (unsigned k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
     const unsigned c = list[k];
@@ -77,6 +94,7 @@ __global__ void __launch_bounds__(128) k_pred_heavy(FpArgs A, Layers L, unsigned
     if constexpr (AT) v = filters_d(map_args_d(A, m), Lm, i, j);
     else v = filters_d(A, Lm, i, j);
     blocked[c] = v.ok ? 0 : 1;
+    if constexpr (CODES) codes[c] = (unsigned char)verdict_code_d(v);
     const int oj = j - A.out_col0;
     if (oj >= 0 && oj < A.out_ncols) {
       const size_t oc = ((size_t)m * A.out_ncols + oj) * A.rows + i;
@@ -84,6 +102,51 @@ __global__ void __launch_bounds__(128) k_pred_heavy(FpArgs A, Layers L, unsigned
       if (step_fp) step_fp[oc] = v.tfp;
       if (rough_fp) rough_fp[oc] = v.rfp;
     }
+  }
+}
+
+template <bool AT>
+__global__ void __launch_bounds__(128) k_pred_heavy(FpArgs A, Layers L, unsigned char* __restrict__ blocked, float* slope_fp, float* step_fp,
+                                                    float* rough_fp, const unsigned* __restrict__ list, const unsigned* __restrict__ count) {
+  pred_heavy_d<AT, false>(A, L, blocked, slope_fp, step_fp, rough_fp, list, count, nullptr);
+}
+
+template <bool AT>
+__global__ void __launch_bounds__(128) k_pred_heavy_codes(FpArgs A, Layers L, unsigned char* __restrict__ blocked, float* slope_fp,
+                                                          float* step_fp, float* rough_fp, const unsigned* __restrict__ list,
+                                                          const unsigned* __restrict__ count, unsigned char* __restrict__ codes) {
+  pred_heavy_d<AT, true>(A, L, blocked, slope_fp, step_fp, rough_fp, list, count, codes);
+}
+
+// The recorded layers of a te_map sweep (SweepRecord).  Every empty centre walks its spiral, and the spiral starts at the centre, so
+// k_plane_centres records each empty cell's own code (codes, from the predicates).  A walk reaches only empty cells, whose codes
+// that records, and cached cells.  A cached cell got its value from a walk centred on it, which recorded it, so this is the whole
+// record unless the map's bytes were reset while its cache stayed (a change of the memo key, SweepRecord::walk): only then does
+// k_plane_walks walk every empty centre of the map (one warp each, record_circle_d) to reach the cached cells.
+__global__ void __launch_bounds__(256) k_plane_centres(const unsigned char* __restrict__ codes, const float* __restrict__ cache,
+                                                       const int* __restrict__ slot, unsigned char* plane, size_t cells, int nmaps) {
+  const size_t total = cells * nmaps;
+  for (size_t x = (size_t)blockIdx.x * blockDim.x + threadIdx.x; x < total; x += (size_t)gridDim.x * blockDim.x) {
+    const size_t m = x / cells, r = (slot ? (size_t)slot[m] : m) * cells + (x - m * cells);
+    if (finitef(__ldg(cache + r))) continue;
+    if (const unsigned char code = __ldg(codes + x)) plane[r] |= code;
+  }
+}
+
+template <bool AT>
+__global__ void __launch_bounds__(128) k_plane_walks(FpArgs A0, Layers L, PathArgs P, const float* __restrict__ cache,
+                                                     const int* __restrict__ slot, unsigned char* plane, const int* __restrict__ flags) {
+  const unsigned m = blockIdx.y;  // block row m: map m of the launch
+  if (!flags[m]) return;
+  const size_t cells = (size_t)A0.rows * A0.cols_total, r0 = (slot ? (size_t)slot[m] : m) * cells;
+  FpArgs Am;
+  if constexpr (AT) Am = map_args_d(A0, m);
+  const FpArgs& A = AT ? Am : A0;
+  const Layers Lm = shift_layers_d(L, (long long)(m * cells));
+  for (size_t c = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < cells; c += ((size_t)gridDim.x * blockDim.x) >> 5) {
+    if (finitef(__ldg(cache + r0 + c))) continue;  // whole warp
+    const int i = (int)(c % A.rows), j = (int)(c / A.rows);
+    record_circle_d(A, Lm, P, plane + r0, nullptr, A.X[i], A.Y[j], i, j, A.rmin, A.rmax, (int)ceil(A.rmax / A.res), false);
   }
 }
 
@@ -373,7 +436,7 @@ std::vector<int> build_spiral(double radius, double res) {
 }  // namespace
 
 void FootprintState::release() {
-  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly, &reduce, &rings, &memo, &items, &upoly, &devreq}) b->release();
+  for (DevBuf* b : {&spiral, &block, &tables, &prefix, &list, &poly, &reduce, &rings, &memo, &items, &upoly, &codes, &devreq}) b->release();
   req_counters = nullptr;
   tables_valid = false;
   valid = false;
@@ -417,7 +480,7 @@ FpArgs filter_args(const SlabView& v, const te_geometry* g, const te_footprint_p
 // k_pred_heavy); fills the geometry / parameter part of the kernel arguments.  Shared by the circular and the polygonal sweep.
 int run_predicates(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int nmaps, const float* trav,
                    const float* slope, const float* step, const float* rough, const float* elev, float* slope_fp, float* step_fp,
-                   float* rough_fp, int sms, cudaStream_t s, FpArgs* out_args) {
+                   float* rough_fp, int sms, cudaStream_t s, FpArgs* out_args, unsigned char* codes) {
   const double rmax = p->radius + p->offset;
   if (nmaps < 1 || nmaps > 65535) { st.why = "number of maps outside 1 .. 65535"; return TE_ERR_UNSUPPORTED; }
   const size_t ncell_in = (size_t)v.rows * v.in_ncols * nmaps;
@@ -437,8 +500,15 @@ int run_predicates(FootprintState& st, const SlabView& v, const te_geometry* g, 
     unsigned* lst = cnt + 1;
     cudaMemsetAsync(cnt, 0, sizeof(unsigned), s);
     const dim3 gc((unsigned)((v.rows + 255) / 256), (unsigned)v.in_ncols, (unsigned)nmaps);
-    k_pred_classify<<<gc, 256, 0, s>>>(a, L, (unsigned char*)st.block.p, slope_fp, step_fp, rough_fp, lst, cnt);
-    (a.pos ? k_pred_heavy<true> : k_pred_heavy<false>)<<<std::max(g1, 1), 128, 0, s>>>(a, L, (unsigned char*)st.block.p, slope_fp, step_fp, rough_fp, lst, cnt);
+    unsigned char* const blk = (unsigned char*)st.block.p;
+    if (!codes) {
+      k_pred_classify<<<gc, 256, 0, s>>>(a, L, blk, slope_fp, step_fp, rough_fp, lst, cnt);
+      (a.pos ? k_pred_heavy<true> : k_pred_heavy<false>)<<<std::max(g1, 1), 128, 0, s>>>(a, L, blk, slope_fp, step_fp, rough_fp, lst, cnt);
+    } else {
+      k_pred_classify_codes<<<gc, 256, 0, s>>>(a, L, blk, slope_fp, step_fp, rough_fp, lst, cnt, codes);
+      (a.pos ? k_pred_heavy_codes<true> : k_pred_heavy_codes<false>)<<<std::max(g1, 1), 128, 0, s>>>(a, L, blk, slope_fp, step_fp,
+                                                                                                     rough_fp, lst, cnt, codes);
+    }
   }
   *out_args = a;
   return 0;
@@ -446,7 +516,7 @@ int run_predicates(FootprintState& st, const SlabView& v, const te_geometry* g, 
 
 int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int nmaps, const float* trav,
                      const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
-                     float* step_fp, float* rough_fp, int sms, cudaStream_t s, int* launches) {
+                     float* step_fp, float* rough_fp, int sms, cudaStream_t s, int* launches, const SweepRecord* rec) {
   const double rmax = p->radius + p->offset;
   if (!footprint_reach_ok(g->resolution, p)) { st.why = "footprint radius exceeds 120 cells"; return TE_ERR_UNSUPPORTED; }
   if (!st.valid || std::memcmp(&st.key_geo, g, sizeof(*g)) != 0 || std::memcmp(&st.key_par, p, sizeof(*p)) != 0) {
@@ -461,9 +531,39 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
     st.tables_valid = false;
   }
   FpArgs a{};
-  if (int rc = run_predicates(st, v, g, p, nmaps, trav, slope, step, rough, elev, slope_fp, step_fp, rough_fp, sms, s, &a)) return rc;
-  const size_t ncols_in = (size_t)v.in_ncols * nmaps, ncell_in = (size_t)v.rows * ncols_in;  // input-buffer columns / cells of the batch
+  unsigned char* codes = nullptr;
+  const size_t cells = (size_t)v.rows * v.cols_total;
+  if (rec) {
+    if (v.in_col0 != 0 || v.in_ncols != v.cols_total) { st.why = "a recorded sweep takes whole maps"; return TE_ERR_BAD_ARG; }
+    if (st.codes.reserve(cells * nmaps + sizeof(int) * (size_t)nmaps + 16) != cudaSuccess) {
+      st.why = "allocating the recorded-layer codes failed";
+      return TE_ERR_CUDA;
+    }
+    codes = (unsigned char*)st.codes.p;
+  }
+  if (int rc = run_predicates(st, v, g, p, nmaps, trav, slope, step, rough, elev, slope_fp, step_fp, rough_fp, sms, s, &a, codes)) return rc;
   const Layers L{trav, slope, step, elev, rough};
+  int nrec = 0;  // the recording's launches
+  if (rec) {
+    const long long gp = std::min<long long>(((long long)(cells * nmaps) + 255) / 256, (long long)sms * 8);
+    k_plane_centres<<<(unsigned)std::max(gp, 1LL), 256, 0, s>>>(codes, rec->cache, rec->slot, rec->plane, cells, nmaps);
+    nrec = 1;
+    if (rec->walk) {
+      if (int rc = ensure_ring_table(st, s)) return rc;
+      const std::vector<int> flags(rec->walk, rec->walk + nmaps);
+      int* dflags = (int*)(codes + (cells * nmaps + 15) / 16 * 16);
+      // pageable source: consumed before cudaMemcpyAsync returns, ordered after the kernels queued before on the stream
+      if (cudaMemcpyAsync(dflags, flags.data(), sizeof(int) * (size_t)nmaps, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+        st.why = "uploading the maps to walk failed";
+        return TE_ERR_CUDA;
+      }
+      const PathArgs P = path_args(st, p, nullptr);
+      const dim3 gw((unsigned)std::max(sms * 16 / nmaps, 1), (unsigned)nmaps);
+      (a.pos ? k_plane_walks<true> : k_plane_walks<false>)<<<gw, 128, 0, s>>>(a, L, P, rec->cache, rec->slot, rec->plane, dflags);
+      nrec = 2;
+    }
+  }
+  const size_t ncols_in = (size_t)v.in_ncols * nmaps, ncell_in = (size_t)v.rows * ncols_in;  // input-buffer columns / cells of the batch
   const long long t1 = (long long)ncell_in, t2 = (long long)v.rows * v.out_ncols * nmaps;
   const int g2 = (int)std::min<long long>((t2 + 255) / 256, (long long)sms * 8);
   // The tables classify lattice offsets (k, l) by d2 = (k^2 + l^2) res^2 against r2 = rmax^2; the reference tests the same cell with
@@ -485,7 +585,7 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
                     std::getenv("TE_FOOTPRINT_BRUTE") == nullptr;
   if (!fast) {
     (a.pos ? k_sweep<true> : k_sweep<false>)<<<std::max(g2, 1), 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
-    if (launches) *launches = 3;
+    if (launches) *launches = 3 + nrec;
     return 0;
   }
   // ---- prefix-sum sweep: tables (cached with the spiral) + per-call prefix/bit arrays -----------------
@@ -578,7 +678,7 @@ int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g
   k_fp_nearest<<<std::max(g1b, 1), 256, 0, s>>>(a, (unsigned char*)prefix + pbytes + wbytes);
   const dim3 gs((unsigned)((v.rows + 255) / 256), (unsigned)v.out_ncols, (unsigned)nmaps);
   (a.pos ? k_sweep_fast<true> : k_sweep_fast<false>)<<<gs, 256, 0, s>>>(a, L, (const unsigned char*)st.block.p, out);
-  if (launches) *launches = 5;
+  if (launches) *launches = 5 + nrec;
   return 0;
 }
 

@@ -35,6 +35,7 @@ struct FootprintState {
   DevBuf memo;    // fresh and polygonal path checks: per-cell isTraversableForFilters memo of one call
   DevBuf items;   // polygonal path checks: one result record per pose index
   DevBuf upoly;   // polygonal path checks with untraversable polygons: per pose index a vertex count and max_vertices points
+  DevBuf codes;   // te_map sweeps: the predicates' recorded-layer code of every cell, then one flag per map (SweepRecord)
   DevBuf devreq;  // map requests: the work list, its keys and records, the hash table and the scan / sort scratch
   const unsigned long long* req_counters = nullptr;  // in devreq: candidates, keys, stored of the last map request
   void invalidate() { valid = false; tables_valid = false; }
@@ -56,9 +57,21 @@ struct FpMapParams {
 
 // The sweeps run on `nmaps` (1 .. 65535) maps of the slab's shape stored back to back: map m's layers start m * rows * in_ncols
 // cells into every input, its outputs m * rows * out_ncols cells into every output.  The tables are built once per call.
+// rec (a te_map, null otherwise): the sweep also records in rec->plane the cells at which traversabilityFootprint(radius, offset)
+// calls isTraversableForFilters on the cache rec->cache as the sweep found it: the spiral prefix of every empty centre.  Map k of the
+// launch is map slot[k] (slot: device, nmaps entries; null: k) of the plane and the cache, whole maps of v.rows * v.cols_total cells.
+// The empty centres alone are the record while every cached cell of a map is recorded; walk (HOST, nmaps entries; null: none)
+// marks the maps where that need not hold, whose empty centres then walk their spirals (one launch more, and a host synchronisation
+// the first time a state walks).
+struct SweepRecord {
+  unsigned char* plane;
+  const float* cache;
+  const int* slot;
+  const unsigned char* walk;
+};
 int launch_footprint(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int nmaps, const float* trav,
                      const float* slope, const float* step, const float* rough, const float* elev, float* out, float* slope_fp,
-                     float* step_fp, float* rough_fp, int sms, cudaStream_t s, int* launches);
+                     float* step_fp, float* rough_fp, int sms, cudaStream_t s, int* launches, const SweepRecord* rec = nullptr);
 
 // TraversabilityMap::traversabilityFootprint(double footprintYaw) (TraversabilityMap.cpp:239-305): the footprint polygon placed at
 // every cell centre, rotated by `yaw` (yaw 0: the unrotated traversability_x), into `out` (device; map m's layer starts
@@ -142,6 +155,10 @@ struct PathChecks {
   // A te_map batch whose maps have parameters of their own: device table of nmaps entries; null: the call's one parameter set
   // for every map.  Read by launch_map_request_device and by launch_path_checks' polygonal kernels.
   const FpMapParams* map_params;
+  // A te_map's recorded slope_footprint / step_footprint / roughness_footprint (te_fp_device.cuh: one byte per cell of every map,
+  // like the memo), or null.  Set: the request also records the cells at which the service loop calls isTraversableForFilters
+  // (launch_map_request_device: the walks the replay commits; launch_path_checks: the polygonal items the path loop reaches).
+  unsigned char* plane;
 };
 // Asynchronous on `s`.  Launches one kernel for the circular paths (when `r` can have any and `circular` is set; a te_map checks
 // them on its cache instead), then for the polygonal paths an items kernel when there are poses and a combine kernel, whatever the
@@ -197,5 +214,10 @@ struct MapSlots {
   size_t cells;     // per map
 };
 void launch_map_slots(const MapSlots& a, bool put, int sms, cudaStream_t s);
+
+// A te_map's recorded slope_footprint / step_footprint / roughness_footprint bytes (te_fp_device.cuh), n cells: clear the first two
+// (te_map_clear_footprint), or decode layer `field` (0, 1, 2 in that order) into floats.  One launch each.
+void launch_plane_clear(unsigned char* plane, size_t n, int sms, cudaStream_t s);
+void launch_plane_decode(const unsigned char* plane, int field, float* out, size_t n, int sms, cudaStream_t s);
 
 }  // namespace te

@@ -95,10 +95,11 @@ struct CircleTable {
 // te_footprint.cu: the geometry part of the kernel arguments, and the geometry and isTraversableForFilters parameters.
 FpArgs geometry_args(const SlabView& v, const te_geometry* g);
 FpArgs filter_args(const SlabView& v, const te_geometry* g, const te_footprint_params* p, const float* rough);
-// te_footprint.cu: isTraversableForFilters for every cell of the slab + halo of each of the nmaps maps into st.block.
+// te_footprint.cu: isTraversableForFilters for every cell of the slab + halo of each of the nmaps maps into st.block (and, with
+// `codes`, each cell's recorded-layer code into codes).
 int run_predicates(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p, int nmaps, const float* trav,
                    const float* slope, const float* step, const float* rough, const float* elev, float* slope_fp, float* step_fp,
-                   float* rough_fp, int sms, cudaStream_t s, FpArgs* out_args);
+                   float* rough_fp, int sms, cudaStream_t s, FpArgs* out_args, unsigned char* codes = nullptr);
 // te_paths.cu: SpiralIterator's rings, the ring table of the circle walk, the path arguments and the fromCircle table.
 std::vector<int> spiral_rings(int nRings, std::vector<int>& ring_start);
 int ensure_ring_table(FootprintState& st, cudaStream_t s);
@@ -318,6 +319,33 @@ __device__ __forceinline__ FilterVerdict filters_d(const FpArgs& A, const Layers
   return v;
 }
 
+// ---- the slope_footprint / step_footprint / roughness_footprint layers a te_map records ----------------------------------
+// One byte per cell: two bits per layer (bits 0-1 slope_footprint, 2-3 step_footprint, 4-5 roughness_footprint), each
+// 0 = NaN (not written), 1 = 0.0f, 2 = 1.0f.  A visit of the reference writes a cell's FilterVerdict fields, which depend on the
+// cell, the layers and the isTraversableForFilters parameters only, so a record is the byte OR the verdict's code.
+__device__ __forceinline__ unsigned fp_field_code_d(float v) { return v == 0.0f ? 1u : v == 1.0f ? 2u : 0u; }
+__device__ __forceinline__ unsigned verdict_code_d(const FilterVerdict& v) {
+  return fp_field_code_d(v.sfp) | fp_field_code_d(v.tfp) << 2 | fp_field_code_d(v.rfp) << 4;
+}
+// isTraversableForFilters fails at a cell iff one of its checks wrote 0 (a check fails only on a cell whose own layer is 0).
+__device__ __forceinline__ bool code_blocked_d(unsigned code) { return (code & 0x15u & ~(code >> 1)) != 0; }
+
+// The code map cell (a, b) holds once the reference visits it: what `plane` recorded, or the verdict's.  A plane byte with a
+// slope or step field was written by a visit under the plane's parameters, so it is complete; a byte without one (nothing
+// recorded, or roughness_footprint alone after te_map_clear_footprint) takes the verdict.  A cell the isTraversableForFilters
+// memo (may be null) holds as passing passed every check that ran: each writes 1 where its layer is 0, so the verdict needs no
+// evaluation.  0 for a cell no check runs on.
+__device__ __forceinline__ unsigned visit_code_d(const FpArgs& A, const Layers& L, const unsigned char* plane, const unsigned char* memo,
+                                                 int a, int b) {
+  const size_t c = (size_t)b * A.rows + a;
+  const bool zs = __ldg(L.slope + c) == 0.0f, zt = __ldg(L.step + c) == 0.0f, zr = A.verify_rough && __ldg(L.rough + c) == 0.0f;
+  if (!(zs || zt || zr)) return 0u;
+  const unsigned code = plane[c];
+  if (code & 0x0fu) return code;
+  if (memo && memo[c] == 1) return code | (zs ? 2u : 0u) | (zt ? 8u : 0u) | (zr ? 32u : 0u);
+  return code | verdict_code_d(filters_d(A, L, a, b));
+}
+
 // SpiralIterator::getCurrentRadius (index-space norm of the offset; Eigen's integer norm when int_norm is set) in metres.
 __device__ __forceinline__ double current_radius_d(const FpArgs& A, int di, int dj) {
   const int d2 = di * di + dj * dj;
@@ -431,6 +459,54 @@ __device__ FreshCircle fresh_circle_d(const FpArgs& A, const Layers& L, const Pa
   }
   t /= (double)n;  // :732-734
   return FreshCircle{true, t, (float)t};
+}
+
+// Records in `plane` the cells at which isTraversable(center, rmax, cup, ..., rmin) on an empty cache calls
+// isTraversableForFilters (TraversabilityMap.cpp:687-729), by the whole warp: the spiral with fresh_circle_d's membership, up to and
+// including the first blocked cell.  With cup the loop does not return there (:714): it goes on past blocked cells within rmin and
+// ends after the first blocked cell beyond rmin met while the circle is still traversable (:705-711).  `memo`: visit_code_d's.
+// Warp-uniform.
+__device__ void record_circle_d(const FpArgs& A, const Layers& L, const PathArgs& P, unsigned char* plane, const unsigned char* memo,
+                                double cx, double cy, int ci, int cj, double rmin, double rmax, int nr, bool cup) {
+  const int lane = threadIdx.x & 31;
+  const double r2 = rmax * rmax;
+  const int end = __ldg(P.ring_start + nr + 1), edge0 = __ldg(P.ring_start + max(nr - 1, 1));
+  bool untrav = false;  // cup: a blocked cell within rmin has made the circle untraversable
+  for (int base = 0; base < end; base += 32) {
+    const int k = base + lane;
+    bool member = false, within = true;
+    unsigned code = 0u;
+    int a = 0, b = 0;
+    if (k < end) {
+      const int w = __ldg(P.rings + k);
+      const int di = (int)(signed char)(w & 0xff), dj = (int)(signed char)((w >> 8) & 0xff);
+      a = ci + di;
+      b = cj + dj;
+      if (a >= 0 && b >= 0 && a < A.rows && b < A.cols_total) {
+        member = true;
+        if (k >= edge0) {
+          const double dx = A.X[a] - cx, dy = A.Y[b] - cy;
+          member = dx * dx + dy * dy <= r2;
+        }
+      }
+      if (member) {
+        code = visit_code_d(A, L, plane, memo, a, b);
+        within = rmin == 0.0 || current_radius_d(A, di, dj) <= rmin;
+      }
+    }
+    const bool blk = member && code_blocked_d(code);
+    const unsigned bw = __ballot_sync(0xffffffffu, blk && within), bb = __ballot_sync(0xffffffffu, blk && !within);
+    int last = 32;  // the last lane the walk visits
+    if (!cup) {
+      if (bw | bb) last = __ffs((int)(bw | bb)) - 1;
+    } else if (!untrav && bb) {
+      const int f = __ffs((int)bb) - 1;
+      if (!(bw & ((1u << f) - 1u))) last = f;
+    }
+    if (code && lane <= last) plane[(size_t)b * A.rows + a] = (unsigned char)code;
+    if (last < 32) return;
+    untrav = untrav || bw != 0u;
+  }
 }
 
 __device__ __forceinline__ bool lex_less_d(double2 a, double2 b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }

@@ -17,11 +17,13 @@ using te::cell_coord;
 
 namespace {
 
-constexpr int kLayerBits = 18;  // te_layer bits 0 .. 17 (1 << 7 unassigned)
+constexpr int kLayerBits = 24;  // te_layer bits 0 .. 23 (1 << 7, 1 << 18 .. 1 << 20 unassigned)
 const char* const kLayerNames[kLayerBits] = {"traversability", "traversability_slope", "traversability_step", "traversability_roughness",
                                              "elevation", "robot_slope", "traversability_footprint", nullptr, "upper_bound", "lower_bound",
                                              "variance", "horizontal_variance_x", "horizontal_variance_y", "horizontal_variance_xy",
-                                             "time", "uncertainty_range", "traversability_x", "traversability_rot"};
+                                             "time", "uncertainty_range", "traversability_x", "traversability_rot", nullptr, nullptr,
+                                             nullptr, "slope_footprint", "step_footprint", "roughness_footprint"};
+constexpr int kFootprintMemoBit = 21;  // TE_LAYER_SLOPE_FOOTPRINT: field 0 of the recorded bytes (te_fp_device.cuh)
 // The layers every map holds once it has any (te_map_chain, te_map_set_layers), the cache included.
 constexpr uint32_t kLayersAlways = TE_LAYER_TRAVERSABILITY | TE_LAYER_SLOPE | TE_LAYER_STEP | TE_LAYER_ELEVATION | TE_LAYER_FOOTPRINT;
 
@@ -36,7 +38,9 @@ struct te_map {
   te_geometry geo_in{};  // as the layers came (host memory: with their circular-buffer start index)
   te_geometry geo{};     // the same with the start index cleared: the device layers are in default order
   // The resident layers, indexed by te_layer bit: layer[b] holds bit b's layer of every map while `held` has bit b.  Bit 6,
-  // traversability_footprint, is the cache; uncertainty_range (bit 15) is derived from the bounds and never held.
+  // traversability_footprint, is the cache; uncertainty_range (bit 15) is derived from the bounds and never held.  Bits 21 .. 23
+  // (slope_footprint, step_footprint, roughness_footprint) are never held either: layer[b] receives them decoded from `plane`
+  // when they are read.
   DevBuf layer[kLayerBits];
   uint32_t held = 0;
   DevBuf fresh;  // te_map_footprint(_maps): the sweep before its merge into the cache
@@ -54,6 +58,15 @@ struct te_map {
     int rough;
   };
   std::vector<MemoKey> memo_key;
+  // The recorded slope_footprint / step_footprint / roughness_footprint (te_fp_device.cuh: one byte per cell of every map), valid
+  // while plane_valid, map k's recorded under the parameters plane_key[k] (map_plane); not valid: NaN everywhere.
+  DevBuf plane;
+  bool plane_valid = false;
+  std::vector<MemoKey> plane_key;
+  // plane_covers[k]: every cached cell of map k is recorded (its value came from a walk centred on it, which recorded it).  Only a
+  // reset of the map's bytes on a memo-key change that keeps its cache breaks it, until the cache is emptied (map_footprint then
+  // walks the map's empty centres).
+  std::vector<char> plane_covers;
   // The per-map parameter table of the last request whose maps have parameters of their own (map_param_table), with what it holds
   std::vector<te::FpMapParams> par_key;
   DevBuf par_tab;
@@ -239,6 +252,7 @@ int map_reset(te_map* m, const te_geometry* g_in, const te_geometry* g, int nmap
   m->nmaps = nmaps;
   m->start.assign(2 * (size_t)nmaps, 0);  // a _wrapped entry sets the maps' start indices once their layers are in
   m->memo_valid = false;
+  m->plane_valid = false;
   m->have_layers = false;
   m->held = kLayersAlways;  // a new map replaces the old one wholesale, its elevation map's layers included
   return TE_OK;
@@ -267,6 +281,39 @@ int map_memo(te_map* m, const te_footprint_params* p, bool each) {
     k = e;
   }
   m->memo_valid = true;
+  return TE_OK;
+}
+
+// The recorded layers, reserved for the whole batch and all NaN (under no parameters) when first needed.
+int map_plane_ready(te_map* m) {
+  if (m->plane_valid) return TE_OK;
+  TE_CUDA(m->plane.reserve(batch_cells(m)));
+  TE_CUDA(cudaMemsetAsync(m->plane.p, 0, batch_cells(m), m->ctx->stream));
+  const double none = std::numeric_limits<double>::quiet_NaN();
+  m->plane_key.assign(m->nmaps, te_map::MemoKey{none, none, -1});
+  m->plane_covers.assign(m->nmaps, 1);  // the caches are empty: no request or sweep since the layers came
+  m->plane_valid = true;
+  return TE_OK;
+}
+
+// The recorded layers for a request or a sweep on the maps `sel` (null: every map) under these parameters (p[0] for every map, or
+// with `each` p[k] for map k): a map keeps its bytes while its memo key (map_memo) stays, and is reset to NaN otherwise.
+int map_plane(te_map* m, const te_footprint_params* p, bool each, const MapSel* sel) {
+  auto key = [&](int k) {
+    const te_footprint_params& q = p[each ? k : 0];
+    return te_map::MemoKey{q.max_gap_width, q.critical_step_height, q.verify_roughness != 0};
+  };
+  const size_t cells = map_cells(m);
+  if (int rc = map_plane_ready(m)) return rc;
+  const int n = sel ? sel->n : m->nmaps;
+  for (int j = 0; j < n; ++j) {
+    const int k = sel ? sel->idx[j] : j;
+    const te_map::MemoKey a = m->plane_key[k], b = key(k);
+    if (a.gap == b.gap && a.crit == b.crit && a.rough == b.rough) continue;
+    if (a.rough >= 0) m->plane_covers[k] = 0;  // recorded under other parameters: the cache, which stays, is no longer covered
+    m->plane_key[k] = b;
+    TE_CUDA(cudaMemsetAsync((unsigned char*)m->plane.p + k * cells, 0, cells, m->ctx->stream));
+  }
   return TE_OK;
 }
 
@@ -313,7 +360,7 @@ int map_layers(te_map* m, uint32_t mask, bool with_range, const float* out[kLaye
   if (!with_range && (mask & TE_LAYER_UNCERTAINTY_RANGE))
     return fail(TE_ERR_BAD_ARG, "layer uncertainty_range is published with the map, not held by it: submaps have no such layer");
   const uint32_t known = TE_LAYER_ALL | TE_LAYER_CARRIED | TE_LAYER_TRAVERSABILITY_X | TE_LAYER_TRAVERSABILITY_ROT |
-                         (with_range ? (uint32_t)TE_LAYER_UNCERTAINTY_RANGE : 0u);
+                         TE_LAYER_FOOTPRINT_MEMO | (with_range ? (uint32_t)TE_LAYER_UNCERTAINTY_RANGE : 0u);
   if (mask == 0 || (mask & ~known)) return fail(TE_ERR_BAD_ARG, "layer mask 0x%x: need a non-empty subset of 0x%x", mask, known);
   *n = 0;
   for (int b = 0; b < kLayerBits; ++b) {
@@ -322,6 +369,16 @@ int map_layers(te_map* m, uint32_t mask, bool with_range, const float* out[kLaye
       if ((m->held & (TE_LAYER_UPPER_BOUND | TE_LAYER_LOWER_BOUND)) != (TE_LAYER_UPPER_BOUND | TE_LAYER_LOWER_BOUND))
         return fail(TE_ERR_MISSING_LAYER, "layer uncertainty_range needs upper_bound and lower_bound: the map does not hold both");
       out[(*n)++] = nullptr;
+      continue;
+    }
+    if ((TE_LAYER_FOOTPRINT_MEMO >> b) & 1u) {  // decoded from the recorded bytes into layer[b]
+      const size_t n_cells = batch_cells(m);
+      TE_CUDA(m->layer[b].reserve(sizeof(float) * n_cells));
+      if (int rc = map_plane_ready(m)) return rc;
+      te::launch_plane_decode((const unsigned char*)m->plane.p, b - kFootprintMemoBit, (float*)m->layer[b].p, n_cells, m->ctx->sms,
+                              m->ctx->stream);
+      if (int rc = launch_check(m->ctx, "k_plane_decode")) return rc;
+      out[(*n)++] = (const float*)m->layer[b].p;
       continue;
     }
     const DevBuf* src = map_layer_buf(m, b);
@@ -409,6 +466,10 @@ int map_put_selected(te_map* m, const MapSel& s, uint32_t bits, const float* con
   a.fill_bits = 0xffffffffu;
   a.cache = lay(m, TE_LAYER_FOOTPRINT);
   a.memo = m->memo_valid ? (unsigned char*)m->fp.memo.p : nullptr;  // reserved for the whole batch while valid (map_memo)
+  for (int j = 0; m->plane_valid && j < s.n; ++j) {  // the recorded layers of the new maps: NaN, over an empty cache
+    TE_CUDA(cudaMemsetAsync((unsigned char*)m->plane.p + s.idx[j] * map_cells(m), 0, map_cells(m), c->stream));
+    m->plane_covers[s.idx[j]] = 1;
+  }
   a.slot = (const int*)m->slots.p;
   a.nsel = s.n;
   a.cells = map_cells(m);
@@ -447,7 +508,7 @@ int te_map_destroy(te_map* m) {
     Guard g(m->ctx);
     if (g.ok) {
       cudaStreamSynchronize(m->ctx->stream);
-      for (DevBuf* b : {&m->fresh, &m->gather, &m->slots, &m->image, &m->cut, &m->wrap, &m->par_tab}) b->release();
+      for (DevBuf* b : {&m->fresh, &m->gather, &m->slots, &m->image, &m->cut, &m->wrap, &m->par_tab, &m->plane}) b->release();
       for (DevBuf& b : m->layer) b.release();
       for (DevBuf& b : m->sel) b.release();
       m->tab_all.buf.release();
@@ -1217,9 +1278,17 @@ static int map_footprint(te_map* m, const te_footprint_params* p, const MapSel* 
   const float* in[5];
   if (int rc = map_sweep_inputs(m, p, sel, in)) return rc;
   const int fixed = sel ? 2 : 1;  // k_map_merge, and k_map_slots for a selection
+  // the sweep's own limit, found before the recorded layers change
+  if (!te::footprint_reach_ok(g->resolution, p)) return fail(TE_ERR_UNSUPPORTED, "footprint radius + offset spans more than 120 cells");
+  if (int rc = map_plane(m, p, false, sel)) return rc;
+  std::vector<unsigned char> walk(n);
+  bool any_walk = false;
+  for (int k = 0; k < n; ++k) any_walk |= (walk[k] = m->plane_covers[sel ? sel->idx[k] : k] ? 0 : 1) != 0;
+  const te::SweepRecord rec{(unsigned char*)m->plane.p, lay(m, TE_LAYER_FOOTPRINT), sel ? (const int*)m->slots.p : nullptr,
+                            any_walk ? walk.data() : nullptr};
   int nl = 0;
   int rc = te::launch_footprint(m->fp, view_at(make_view(c, g, s), g, spread ? &tab : nullptr), g, p, n, in[0], in[1], in[2], in[3], in[4],
-                                (float*)m->fresh.p, nullptr, nullptr, nullptr, c->sms, c->stream, &nl);
+                                (float*)m->fresh.p, nullptr, nullptr, nullptr, c->sms, c->stream, &nl, &rec);
   if (rc != 0) return fail(rc, "footprint sweep failed: %s", m->fp.why.c_str());
   // host memory: the whole cache is read back from its resident layer, a selection's from packed scratch (its trav slot)
   float* const dout = !out ? nullptr : memory == TE_MEM_DEVICE ? out : sel ? (float*)m->sel[0].p : nullptr;
@@ -1525,6 +1594,7 @@ static int map_request(te_map* m, const te_footprint_params* p, const te_footpri
   }
   if (int rc = ensure_geometry(c, g)) return rc;
   if (int rc = map_memo(m, each ? each : p, each != nullptr)) return rc;
+  if (int rc = map_plane(m, each ? each : p, each != nullptr, nullptr)) return rc;
   // maps with parameters of their own: the kernels read each map's from a table (none when they are all one set, p = each[0]);
   // what does not vary per map comes from each[0], and the roughness layer is read when any map verifies roughness
   const te::FpMapParams* table = nullptr;
@@ -1549,6 +1619,7 @@ static int map_request(te_map* m, const te_footprint_params* p, const te_footpri
   r.max_footprint_vertices = max_footprint_vertices; r.conservative = conservative; r.cup = cup; r.max_points = mp;
   r.is_safe = is_safe; r.trav_out = traversability; r.area_out = area; r.max_vertices = max_vertices; r.ucount = ucount; r.uxy = uxy;
   r.map_params = table;
+  r.plane = (unsigned char*)m->plane.p;
   Staging st(c, host, g);
   stage_paths(st, r);
   if (st.rc) return st.rc;
@@ -1672,6 +1743,11 @@ int te_map_clear_footprint(te_map* m) {
   TE_MAP_ENTER(m);
   if (int rc = map_ready(m)) return rc;
   TE_CUDA(cudaMemsetAsync(lay(m, TE_LAYER_FOOTPRINT), 0xff, sizeof(float) * batch_cells(m), c->stream));
+  if (m->plane_valid) {
+    m->plane_covers.assign(m->nmaps, 1);  // every cache is empty
+    te::launch_plane_clear((unsigned char*)m->plane.p, batch_cells(m), c->sms, c->stream);
+    return launch_check(c, "k_plane_clear");
+  }
   return TE_OK;
 }
 
@@ -1857,7 +1933,7 @@ static int map_submaps(te_map* m, int32_t nwin, const int32_t* win_map, const do
   if (total == 0) return TE_OK;
   if (!out) return fail(TE_ERR_BAD_ARG, "output is null");
   // the table k_map_gather_submaps reads: the source layers in its first kHead records, then the windows that have cells
-  constexpr int kHead = 4;
+  constexpr int kHead = 6;
   static_assert(sizeof(const float*) * (kLayerBits - 2) <= kHead * sizeof(te::SubmapWindow), "layer table");  // not 1 << 7, range
   std::vector<te::SubmapWindow> table(kHead);
   std::memcpy((void*)table.data(), src, sizeof(const float*) * nl);
@@ -2075,7 +2151,8 @@ int te_map_get_point_cloud(te_map* m, int32_t nsel, const int32_t* map_index, in
   if (!fields || !offsets) return fail(TE_ERR_BAD_ARG, "fields or offsets is null");
   if (capacity_points < 0) return fail(TE_ERR_BAD_ARG, "negative capacity_points");
   if (!data && capacity_points > 0) return fail(TE_ERR_BAD_ARG, "data is null with capacity_points %lld", (long long)capacity_points);
-  const uint32_t known = TE_LAYER_ALL | TE_LAYER_CARRIED | TE_LAYER_UNCERTAINTY_RANGE | TE_LAYER_TRAVERSABILITY_X | TE_LAYER_TRAVERSABILITY_ROT;
+  const uint32_t known = TE_LAYER_ALL | TE_LAYER_CARRIED | TE_LAYER_UNCERTAINTY_RANGE | TE_LAYER_TRAVERSABILITY_X | TE_LAYER_TRAVERSABILITY_ROT |
+                         TE_LAYER_FOOTPRINT_MEMO;
   const auto one_bit = [&](uint32_t b) { return b != 0 && (b & (b - 1)) == 0 && (b & known) != 0; };
   uint32_t given = 0;
   for (int e = 0; e < nfields; ++e) {

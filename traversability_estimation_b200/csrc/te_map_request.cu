@@ -400,7 +400,9 @@ __global__ void __launch_bounds__(256) k_req_dedup(DevReq D) {
 //     path.  Lanes after f that belong to later paths are evaluated again there: their assumption included dropped lanes, which
 //     store nothing.
 //   - Gates fail without a polygon, as the loop's `break`.  Maps share nothing, so their warps run independently.
-__global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* cache) {
+// REC: walked_keys[kid] = 1 for every key whose walk commits (k_req_record).
+template <bool REC>
+__device__ __forceinline__ void req_replay_d(const FpArgs& A, const DevReq& D, float* cache, unsigned char* walked_keys) {
   __shared__ double s_t[4][32];
   __shared__ int s_v[4][32];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -465,6 +467,8 @@ __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* c
     const unsigned walked = __ballot_sync(0xffffffffu, commit_walk);
     // the cell keeps the float of its last committed walk
     if (commit_walk && !(walked & peers & ~((2u << lane) - 1u))) mc[cell] = R.cache;
+    if constexpr (REC)
+      if (commit_walk) walked_keys[D.kid[E.key]] = 1;
     stored += __popc(walked);
     s_t[w][lane] = t;
     s_v[w][lane] = (lok ? 1 : 0) | (fk << 1);
@@ -523,6 +527,32 @@ __global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* c
   if (lane == 0 && stored) atomicAdd(D.counters + 2, stored);
 }
 
+__global__ void __launch_bounds__(128) k_req_replay(FpArgs A, DevReq D, float* cache) { req_replay_d<false>(A, D, cache, nullptr); }
+
+__global__ void __launch_bounds__(128) k_req_replay_rec(FpArgs A, DevReq D, float* cache, unsigned char* walked_keys) {
+  req_replay_d<true>(A, D, cache, walked_keys);
+}
+
+// 7. Recording (a te_map's slope_footprint / step_footprint / roughness_footprint, `plane`): every key whose walk the replay
+// committed walks its spiral again, one warp per key, and records the cells the reference's walk visits (record_circle_d).  A
+// committed walk ran on an empty centre, so its visits are those of a walk on an empty cache.  Maps as k_map_eval_circles_dev.
+template <bool AT, bool EACH>
+__global__ void __launch_bounds__(128) k_req_record(FpArgs A0, Layers L, PathArgs P, const MapKey* __restrict__ keys,
+                                                    const unsigned long long* __restrict__ nkeys,
+                                                    const unsigned char* __restrict__ walked_keys, unsigned char* plane) {
+  const long long n = (long long)*nkeys;
+  for (long long k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; k < n; k += (gridDim.x * blockDim.x) >> 5) {  // whole warps
+    if (!walked_keys[k]) continue;
+    const MapKey K = keys[k];
+    FpArgs Am;
+    if constexpr (AT || EACH) Am = map_view_d<AT, EACH>(A0, K.map);
+    const FpArgs& A = AT || EACH ? Am : A0;
+    const long long mo = (long long)K.map * A.rows * A.cols_total;
+    const double rmax = K.rmin + map_walk_offset_d<EACH>(A0, P.offset, K.map);
+    record_circle_d(A, shift_layers_d(L, mo), P, plane + mo, P.memo + mo, K.cx, K.cy, K.ci, K.cj, K.rmin, rmax, (int)ceil(rmax / A.res), K.cup != 0);
+  }
+}
+
 // 6. Polygons: one warp per path; a path the replay did not leave a failing circle to publish exits at once.  The pair
 // k_check_paths_fresh_poly calls: fromCircle, or spiral_blockers_d on the failing key and write_cells_polygon_d with its freps.
 template <bool AT, bool EACH>
@@ -556,7 +586,33 @@ __global__ void __launch_bounds__(128, 4) k_req_polygons(FpArgs A0, Layers L, Pa
 
 size_t align16(size_t b) { return (b + 15) / 16 * 16; }
 
+// te_map_clear_footprint (resetTraversabilityFootprintLayers, TraversabilityMap.cpp:195-200): slope_footprint and step_footprint
+// become NaN, roughness_footprint stays.
+__global__ void __launch_bounds__(256) k_plane_clear(unsigned char* plane, size_t n) {
+  for (size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x; c < n; c += (size_t)gridDim.x * blockDim.x) plane[c] &= 0x30;
+}
+
+// Layer `field` (0 slope_footprint, 1 step_footprint, 2 roughness_footprint) of the recorded bytes as floats: the quiet NaN
+// 0x7fc00000 the reference's layers hold where nothing wrote them (computeTraversability's add(), the bag's slope_footprint and
+// step_footprint), 0.0f or 1.0f.
+__global__ void __launch_bounds__(256) k_plane_decode(const unsigned char* __restrict__ plane, int field, float* __restrict__ out, size_t n) {
+  for (size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x; c < n; c += (size_t)gridDim.x * blockDim.x) {
+    const unsigned f = (__ldg(plane + c) >> (2 * field)) & 3u;
+    out[c] = f == 0u ? __int_as_float(0x7fc00000) : f == 1u ? 0.0f : 1.0f;
+  }
+}
+
+unsigned plane_blocks(size_t n, int sms) { return (unsigned)std::max<size_t>(std::min<size_t>((n + 255) / 256, (size_t)sms * 8), 1); }
+
 }  // namespace
+
+void launch_plane_clear(unsigned char* plane, size_t n, int sms, cudaStream_t s) {
+  k_plane_clear<<<plane_blocks(n, sms), 256, 0, s>>>(plane, n);
+}
+
+void launch_plane_decode(const unsigned char* plane, int field, float* out, size_t n, int sms, cudaStream_t s) {
+  k_plane_decode<<<plane_blocks(n, sms), 256, 0, s>>>(plane, field, out, n);
+}
 
 int launch_map_request_device(FootprintState& st, const SlabView& v, const te_geometry* g, const te_footprint_params* p,
                               const PathChecks& r, float* cache, long long max_checks, bool nonfinite_ok, int sms, cudaStream_t s,
@@ -589,6 +645,7 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
   const size_t o_lcnt = take(sizeof(int) * np1), o_lofs = take(sizeof(int) * np1);
   const size_t o_entries = take(sizeof(ReqEntry) * nc), o_kid = take(sizeof(int) * nc), o_keys = take(sizeof(MapKey) * nc);
   const size_t o_recs = take(sizeof(MapRecord) * nc), o_table = take(sizeof(int) * (size_t)tslots), o_cub = take(cub_bytes);
+  const size_t o_walked = r.plane ? take(nc) : off;
   if (st.devreq.reserve(off) != cudaSuccess) { st.why = "allocating the device request workspace failed"; return TE_ERR_CUDA; }
   char* base = (char*)st.devreq.p;
   DevReq D{};
@@ -637,8 +694,18 @@ int launch_map_request_device(FootprintState& st, const SlabView& v, const te_ge
   const auto eval = at ? (each ? k_map_eval_circles_dev<true, true> : k_map_eval_circles_dev<true, false>)
                        : (each ? k_map_eval_circles_dev<false, true> : k_map_eval_circles_dev<false, false>);
   eval<<<ge, 128, 0, s>>>(a, L, P, D.keys, D.counters + 1, cache, D.recs);
-  k_req_replay<<<blocks(nmaps, 4), 128, 0, s>>>(a, D, cache);
   *launches = 12;  // nine kernels and three CUB calls, each counted as one launch (a CUB call runs two or more kernels)
+  if (!r.plane) {
+    k_req_replay<<<blocks(nmaps, 4), 128, 0, s>>>(a, D, cache);
+  } else {  // a te_map's recorded layers: which keys' walks commit, then their visits
+    unsigned char* const walked = (unsigned char*)base + o_walked;
+    if (e == cudaSuccess) e = cudaMemsetAsync(walked, 0, nc, s);
+    k_req_replay_rec<<<blocks(nmaps, 4), 128, 0, s>>>(a, D, cache, walked);
+    const auto rec = at ? (each ? k_req_record<true, true> : k_req_record<true, false>)
+                        : (each ? k_req_record<false, true> : k_req_record<false, false>);
+    rec<<<ge, 128, 0, s>>>(a, L, P, D.keys, D.counters + 1, walked, r.plane);
+    *launches += 2;
+  }
   if (r.ucount) {
     const auto polys = at ? (each ? k_req_polygons<true, true> : k_req_polygons<true, false>)
                           : (each ? k_req_polygons<false, true> : k_req_polygons<false, false>);

@@ -334,9 +334,13 @@ __host__ __device__ inline size_t poly_warp_smem(int mcap, bool poly) {
 // (R.fp_begin) each polygonal path uses its own, and the poses of circular paths are no items.  AT: the maps sit at their own
 // positions (FpArgs::pos), and the item takes its path's map's tables and position.  Maps with parameters of their own
 // (FpArgs::mp): the item takes its path's map's.
-template <bool POLY, bool AT, bool EACH>
+// REC (k_check_polygon_items_rec, after the items and combine kernels): no outputs; an item the path loop reaches (every earlier
+// item of its checkable path traversable, its own checkInclination passed) records in `plane` the cells its isTraversable visits:
+// the PolygonIterator prefix up to and including the first blocked cell, or the whole polygon with compute_untraversable_polygon
+// (:601-611).
+template <bool POLY, bool AT, bool EACH, bool REC = false>
 __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L, const PolyPathArgs& P, const PolyUntravArgs& U,
-                                                     const RequestArgs& R) {
+                                                     const RequestArgs& R, unsigned char* plane = nullptr) {
   extern __shared__ double2 sPoly[];
   const int lane = threadIdx.x & 31;
   const int p = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
@@ -362,8 +366,17 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L,
   if (R.fp_begin && R.fp_begin[q + 1] == R.fp_begin[q]) return;  // a pose of a circular path
   const long long mo = map_offset_d(R, q);
   if (!(b >= 0 && b <= p && p < e && e <= P.nposes && (n == 1 || k >= 1)) || mo < 0) {
-    if (lane == 0) P.items[p] = it;
+    if (lane == 0 && !REC) P.items[p] = it;
     return;
+  }
+  if constexpr (REC) {  // the path loop reaches item k: its path is checkable and items k0 .. k-1 are traversable
+    bool reach = true;
+    for (int j = (n == 1 ? 0 : 1) + lane; j < n; j += 32) {
+      const PolyItem o = P.items[b + j];
+      reach = reach && o.q == q && o.flag != 2 && (j >= k || o.flag == 1);
+    }
+    if (!__all_sync(0xffffffffu, reach)) return;
+    plane += mo;
   }
   L = shift_layers_d(L, mo);  // path q's map
   FpArgs Am;
@@ -380,7 +393,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L,
   const float* fxyz = nullptr;  // the path's own footprint
   if (R.fp_begin) {
     if (!__all_sync(0xffffffffu, request_footprint_ok_d(R, q, lane, 32))) {
-      if (lane == 0) P.items[p] = it;  // flag 2
+      if (lane == 0 && !REC) P.items[p] = it;  // flag 2
       return;
     }
     const int fb = R.fp_begin[q];
@@ -393,7 +406,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L,
   for (int s = (cons ? 0 : max(k - 1, 0)) + lane; s <= k; s += 32)
     for (int c = 0; c < 7; ++c) finite = finite && isfinite(P.poses[7 * (size_t)(b + s) + c]);
   if (!__all_sync(0xffffffffu, finite) || m > P.mcap || (cons && nfp * (k + 1) > kPolyConsCap)) {
-    if (lane == 0) P.items[p] = it;  // flag 2
+    if (lane == 0 && !REC) P.items[p] = it;  // flag 2
     return;
   }
   const double* pk = P.poses + 7 * (size_t)(b + k);
@@ -476,6 +489,24 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L,
     // POLY: collect the blocked cells (table row = map row - si) unless the bounding box has more rows than the table
     const bool collect = POLY && cup && nr <= kUntravRows;
     if (POLY && collect) { clear_table_d(S, nr); nr_walk = nr; si_walk = si; }
+    if constexpr (REC) {
+      const bool all = U.cup != nullptr && U.cup[q] != 0;
+      for (long long base = 0; base < total; base += 32) {
+        const long long c = base + lane;
+        unsigned code = 0u;
+        int a = 0, bb = 0;
+        if (c < total) {
+          a = si + (int)(c / nc);
+          bb = sj + (int)(c % nc);
+          if (a >= 0 && bb >= 0 && a < A.rows && bb < A.cols_total && polygon_inside_d(sA, nh, A.X[a], A.Y[bb]))
+            code = visit_code_d(A, L, plane, memo, a, bb);
+        }
+        const unsigned bm = all ? 0u : __ballot_sync(0xffffffffu, code_blocked_d(code));
+        if (code && (!bm || lane < __ffs((int)bm))) plane[(size_t)bb * A.rows + a] = (unsigned char)code;
+        if (bm) break;
+      }
+      return;
+    }
     for (long long base = 0; base < total; base += 32) {  // SubmapIterator order, 32 cells per pass; the sum in visit order
       const long long c = base + lane;
       bool member = false, blk = false;
@@ -515,6 +546,7 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L,
       }
     }
   }
+  if constexpr (REC) return;
   if (lane == 0) {
     it.flag = ok ? 1 : 0;
     it.mean = t;
@@ -535,6 +567,12 @@ __device__ __forceinline__ void check_polygon_item_d(const FpArgs& A0, Layers L,
 template <bool AT, bool EACH>
 __global__ void __launch_bounds__(128) k_check_polygon_items(FpArgs A, Layers L, PolyPathArgs P, RequestArgs R) {
   check_polygon_item_d<false, AT, EACH>(A, L, P, PolyUntravArgs{}, R);
+}
+
+template <bool AT, bool EACH>
+__global__ void __launch_bounds__(128) k_check_polygon_items_rec(FpArgs A, Layers L, PolyPathArgs P, PolyUntravArgs U, RequestArgs R,
+                                                                 unsigned char* plane) {
+  check_polygon_item_d<false, AT, EACH, true>(A, L, P, U, R, plane);
 }
 
 template <bool AT, bool EACH>
@@ -765,21 +803,39 @@ int launch_path_checks(FootprintState& st, const SlabView& v, const te_geometry*
   // maps at their own positions (a te_map): the instantiations that read each path's map's tables; maps with parameters of their
   // own: those that read each path's map's
   const bool at = a.pos != nullptr, each = a.mp != nullptr;
-  if (!r.ucount)
-    return launch_polygon_kernels(st,
-                                  at ? (each ? k_check_polygon_items<true, true> : k_check_polygon_items<true, false>)
-                                     : (each ? k_check_polygon_items<false, true> : k_check_polygon_items<false, false>),
-                                  k_check_polygon_combine, "k_check_polygon_items", false, a, L, P, s, launches, R);
-  const size_t cbytes = (sizeof(int) * nitems + 15) / 16 * 16;
-  if (st.upoly.reserve(cbytes + sizeof(double2) * nitems * (size_t)std::max(r.max_vertices, 1)) != cudaSuccess) {
-    st.why = "allocating the untraversable polygons failed";
-    return TE_ERR_CUDA;
-  }
-  const PolyUntravArgs U{r.cup, (int*)st.upoly.p, (double*)((char*)st.upoly.p + cbytes), UntravOut{r.max_vertices, r.ucount, r.uxy}};
-  return launch_polygon_kernels(st,
+  int rc = 0;
+  if (!r.ucount) {
+    rc = launch_polygon_kernels(st,
+                                at ? (each ? k_check_polygon_items<true, true> : k_check_polygon_items<true, false>)
+                                   : (each ? k_check_polygon_items<false, true> : k_check_polygon_items<false, false>),
+                                k_check_polygon_combine, "k_check_polygon_items", false, a, L, P, s, launches, R);
+  } else {
+    const size_t cbytes = (sizeof(int) * nitems + 15) / 16 * 16;
+    if (st.upoly.reserve(cbytes + sizeof(double2) * nitems * (size_t)std::max(r.max_vertices, 1)) != cudaSuccess) {
+      st.why = "allocating the untraversable polygons failed";
+      return TE_ERR_CUDA;
+    }
+    const PolyUntravArgs U{r.cup, (int*)st.upoly.p, (double*)((char*)st.upoly.p + cbytes), UntravOut{r.max_vertices, r.ucount, r.uxy}};
+    rc = launch_polygon_kernels(st,
                                 at ? (each ? k_check_polygon_items_poly<true, true> : k_check_polygon_items_poly<true, false>)
                                    : (each ? k_check_polygon_items_poly<false, true> : k_check_polygon_items_poly<false, false>),
                                 k_check_polygon_combine_poly, "k_check_polygon_items_poly", true, a, L, P, s, launches, U, R);
+  }
+  if (rc || !r.plane || P.nposes <= 0) return rc;
+  // a te_map's recorded layers: the items the path loop reaches walk their polygons again, reading the items of the first pass
+  const auto rec = at ? (each ? k_check_polygon_items_rec<true, true> : k_check_polygon_items_rec<true, false>)
+                      : (each ? k_check_polygon_items_rec<false, true> : k_check_polygon_items_rec<false, false>);
+  const size_t per_warp = poly_warp_smem(P.mcap, false);
+  const int wpb = per_warp * 4 <= 48 * 1024 ? 4 : 1;
+  if (per_warp * wpb > 48 * 1024 &&
+      cudaFuncSetAttribute(rec, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(per_warp * wpb)) != cudaSuccess) {
+    st.why = "cudaFuncSetAttribute(k_check_polygon_items_rec) failed";
+    return TE_ERR_CUDA;
+  }
+  const PolyUntravArgs U{r.cup, nullptr, nullptr, UntravOut{}};
+  rec<<<(unsigned)(((long long)P.nposes + wpb - 1) / wpb), 32 * wpb, per_warp * wpb, s>>>(a, L, P, U, R, r.plane);
+  ++*launches;
+  return 0;
 }
 
 }  // namespace te
