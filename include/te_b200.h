@@ -136,6 +136,14 @@ int te_get_flag_counters(te_ctx* ctx, uint32_t out[5]);
  * window, 7 null eigenvector, 8 n_z == 0, 9 n_z on a float32 rounding boundary); valid_cells[n] = escalated cells whose
  * normals window held n valid cells.  Diagnostics only; no reference counterpart. */
 int te_get_escalation_stats(te_ctx* ctx, uint32_t reasons[16], uint32_t valid_cells[26]);
+/* The fix-up work list of the last fused launch: tier = 2 the cells the fp32 stencil flagged for the fp64 fix-up, tier = 3 the
+ * cells tier 2 passed on to the literal kernel.  *count receives the number of entries and out[0 .. min(*count, capacity))
+ * the entries themselves, in list order (chunk padding dropped); out may be null when capacity is 0.  An entry is the cell's
+ * index in the launch (map index * rows * out_cols + column * rows + row) | do_n << 30 | do_s << 31, where do_n asks for the
+ * normals part (slope, roughness, normals) and do_s for the step part; tier-3 entries carry do_n only.  Only the LAST launch
+ * is reported: a host-memory te_chain that pipelines column chunks reports its last chunk.  Diagnostics only; no reference
+ * counterpart. */
+int te_get_fixup_cells(te_ctx* ctx, int tier, uint32_t capacity, uint32_t* out, uint32_t* count);
 /* Work decomposition the fused kernel uses for `nmaps` maps of rows x out_ncols output cells on a GPU with `sms`
  * multiprocessors (host arithmetic only, needs no GPU; no reference counterpart — the reference iterates cell by cell).
  * Units are (level, map, column segment, 60-row strip), popped from a queue in that order; a level is a run of columns cut

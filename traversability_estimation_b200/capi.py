@@ -159,6 +159,7 @@ SIGNATURES = {
     "te_get_timing": (_R, [_P, _P, _P, _P]),
     "te_get_flag_counters": (_R, [_P, _P]),
     "te_get_escalation_stats": (_R, [_P, _P, _P]),
+    "te_get_fixup_cells": (_R, [_P, _I, _U, _P, _P]),
     "te_fused_plan": (_R, [_I, _I, _I, _I, _P]),
     "te_slope": (_R, [_P, _G, _D, _P, _P, _I]),
     "te_normals": (_R, [_P, _G, _CP, _P, _P, _P, _P, _I]),
@@ -447,6 +448,17 @@ class Context:
         a, b = (C.c_uint32 * 16)(), (C.c_uint32 * 26)()
         self._check(self._L.te_get_escalation_stats(self._h, a, b))
         return list(a), list(b)
+
+    def fixup_cells(self, tier):
+        """The tier-2 (tier=2) or tier-3 (tier=3) work list of the last fused launch as uint32 entries: cell index of the launch
+        | do_n << 30 | do_s << 31, chunk padding dropped.  Only the last launch: a host-memory chain pipelined in column chunks
+        reports its last chunk."""
+        n = C.c_uint32()
+        self._check(self._L.te_get_fixup_cells(self._h, tier, 0, None, C.byref(n)))
+        out = np.zeros(n.value, dtype=np.uint32)
+        self._check(self._L.te_get_fixup_cells(self._h, tier, n.value, out.ctypes.data if n.value else None, C.byref(n)))
+        assert n.value == len(out), (n.value, len(out))
+        return out
 
     def slope(self, g, critical, nz, out, memory):
         self._order_after_torch(memory)

@@ -599,6 +599,30 @@ int te_get_escalation_stats(te_ctx* c, uint32_t reasons[16], uint32_t valid_cell
   return TE_OK;
 }
 
+int te_get_fixup_cells(te_ctx* c, int tier, uint32_t capacity, uint32_t* out, uint32_t* count) {
+  TE_ENTER(c);
+  if (tier != 2 && tier != 3) return fail(TE_ERR_BAD_ARG, "tier must be 2 or 3, got %d", tier);
+  if (!count || (capacity && !out)) return fail(TE_ERR_BAD_ARG, "null argument");
+  *count = 0;
+  const te::DevBuf& list = tier == 2 ? c->worklist : c->worklist3;
+  if (!c->counter.p || !list.p) return TE_OK;
+  unsigned raw[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  TE_CUDA(cudaStreamSynchronize(c->stream));
+  TE_CUDA(cudaMemcpy(raw, (unsigned*)c->counter.p + 128 * c->counter_phase, sizeof(raw), cudaMemcpyDeviceToHost));
+  // tier 2: raw[0] entries reserved in warp-private chunks (padding included); tier 3: raw[4] entries appended one by one
+  const size_t n = std::min<size_t>(tier == 2 ? raw[0] : raw[4], list.cap / sizeof(unsigned));
+  std::vector<unsigned> h(n);
+  if (n) TE_CUDA(cudaMemcpy(h.data(), list.p, n * sizeof(unsigned), cudaMemcpyDeviceToHost));
+  uint32_t k = 0;
+  for (const unsigned w : h) {
+    if (w == te::LIST_INVALID) continue;
+    if (k < capacity) out[k] = w;
+    ++k;
+  }
+  *count = k;
+  return TE_OK;
+}
+
 int te_slope(te_ctx* c, const te_geometry* g, double crit, const float* nz, float* out, int memory) {
   TE_ENTER(c);
   if (int rc = check_geometry(g)) return rc;
