@@ -887,17 +887,25 @@ class Map:
             raise ValueError(f"positions: need {n} (x, y) pairs, got {xy.size} values")
         return xy
 
-    def chain_batched(self, g, p, nmaps, elevation, outputs=False, positions=None, start_index=None):
+    def chain_batched(self, g, p, nmaps, elevation, outputs=False, positions=None, start_index=None, memory=MEM_HOST):
         """te_map_chain_batched (computeTraversability for every map): elevation (nmaps, rows, cols); empties every cache.
         outputs=True also returns the four layers as a dict of (nmaps, rows, cols) arrays.  positions (nmaps, 2): map m sits at
         positions[m] instead of g's position (te_map_chain_batched_at).  start_index (nmaps, 2): map m's layers (input and
-        output) are in the circular-buffer order of start_index[m] (te_map_chain_batched_wrapped)."""
-        e = self._batch_layers(elevation)
+        output) are in the circular-buffer order of start_index[m] (te_map_chain_batched_wrapped).  memory=MEM_DEVICE: elevation
+        is a float32 device tensor of the nmaps maps back to back, each column-major (a batch too large to stage from the host),
+        read in place; outputs must then be False."""
+        if memory == MEM_HOST:
+            e = self._batch_layers(elevation)
+        elif outputs:
+            raise ValueError("outputs=True copies the layers to host arrays: take them with get_layers in device memory")
+        else:
+            e = elevation
+            self._ctx._order_after_torch(memory)
         out = {k: np.empty((int(nmaps), g.cols, g.rows), dtype=np.float32) for k in ("slope", "step", "roughness", "traversability")} \
             if outputs else {}
         xy = self._positions(positions, int(nmaps))
         args = (self._h, C.byref(g), C.byref(p), int(nmaps), _addr(e),
-                *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")), MEM_HOST)
+                *(_addr(out.get(k)) for k in ("slope", "step", "roughness", "traversability")), memory)
         self._update("te_map_chain_batched", args, xy, start_index, int(nmaps))
         self._g, self._n = g, int(nmaps)
         return {k: v.transpose(0, 2, 1) for k, v in out.items()} if outputs else None
@@ -1116,9 +1124,15 @@ class Map:
         self._check(fn(self._h, arr, nsel, _addr(idx), _addr(buf), MEM_HOST))
         return res
 
-    def footprint(self, fp):
-        """te_map_footprint (traversabilityFootprint(radius, offset) on the cache); returns the cache afterwards."""
+    def footprint(self, fp, out=None, memory=MEM_HOST):
+        """te_map_footprint (traversabilityFootprint(radius, offset) on the cache); returns the cache afterwards.  Device memory:
+        `out` is a float32 device tensor of every map's cells (or None: the cache stays on the device only), filled
+        asynchronously on the context stream and returned."""
         fn = self._L.te_map_footprint
+        if memory != MEM_HOST:
+            self._ctx._order_after_torch(memory)
+            self._check(fn(self._h, C.byref(fp), _addr(out), memory))
+            return out
         if not self._g:
             self._check(fn(self._h, C.byref(fp), None, MEM_HOST))
         buf, out = self._layer_out()
